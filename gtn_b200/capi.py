@@ -91,6 +91,9 @@ SYMBOLS = [
     ("gtnb_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int]),
+    ("gtnb_ngram_ctc_loss", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, C.c_int, _f32p, _vp,
+      C.c_int, _vp, C.c_int]),
 ]
 
 _lib = None
@@ -360,6 +363,48 @@ class Ctx:
         return losses, grads
 
 
+    def ngram_ctc_loss(self, emissions, trans_w, targets, blank=0, want_grad=True, input_lens=None):
+        """Host-buffer entry of gtnb_ngram_ctc_loss: emissions [B,T,C], trans_w [C*C] (row = destination label)
+        -> (losses [B], grads [B,T,C] or None, trans_grad [C*C] or None)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == Cn * Cn
+        cat, lens = _cat_targets(targets)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        losses = np.zeros(B, np.float32)
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        tg = np.zeros(Cn * Cn, np.float32) if want_grad else None
+        self._check(lib().gtnb_ngram_ctc_loss(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), tw.ctypes.data, 0, _p(cat, _i32p), _p(lens, _i32p),
+            int(blank), _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0,
+            None if tg is None else tg.ctypes.data, 0))
+        return losses, grads, tg
+
+    def ngram_ctc_loss_dev(self, emissions, trans_w, targets, blank=0, input_lens=None):
+        """Device-buffer entry: emissions and W uploaded once, gtnb_ngram_ctc_loss on device pointers (gradients
+        in HBM), downloaded afterwards -> (losses, grads, trans_grad)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == Cn * Cn
+        cat, lens = _cat_targets(targets)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        losses = np.zeros(B, np.float32)
+        e_dev, w_dev = self.to_device(e), self.to_device(tw)
+        g_dev, tg_dev = self.alloc(max(e.nbytes, 16)), self.alloc(tw.nbytes)
+        try:
+            self._check(lib().gtnb_ngram_ctc_loss(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), w_dev.ptr, 1, _p(cat, _i32p), _p(lens, _i32p),
+                int(blank), _p(losses, _f32p), g_dev.ptr, 1, tg_dev.ptr, 1))
+            grads = g_dev.download(e.shape)
+            tg = tg_dev.download(tw.shape)
+        finally:
+            for buf in (e_dev, w_dev, g_dev, tg_dev):
+                buf.free()
+        return losses, grads, tg
+
+
 class Lattice:
     def __init__(self, ctx, h, keep=None):
         self.ctx = ctx
@@ -440,3 +485,9 @@ class Lattice:
             self.ctx._check(rc)
         out = dict(arcs=arcs[:B], ilabels=il[:B], olabels=ol[:B], lens=lens[:B], weights=pw[:B])
         return (out, status[:B]) if want_status else out
+
+
+def _cat_targets(targets):
+    lens = np.asarray([len(t) for t in targets], np.int32)
+    cat = np.concatenate([np.asarray(t, np.int32) for t in targets]) if len(targets) else np.zeros(0, np.int32)
+    return np.ascontiguousarray(cat, np.int32), lens

@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <string>
 #include <vector>
 
@@ -721,6 +722,407 @@ extern "C" int gtnb_asg_loss(
   if (ctx) arena_begin(ctx);
   const int rc = asg_loss_run(ctx, B, T, C, emissions, emissions_on_device, trans_w_host, targets, target_lens,
                               losses_host, grads, grads_on_device, trans_grad_host);
+  if (ctx) arena_end(ctx);
+  return rc;
+}
+
+/*
+ * CTC with a learned bigram transition graph G (benchmarks/ctc.cpp:107-134, k_ngram.cu):
+ *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(ctc_b, G), E_b))
+ * G: C nodes, all start and accept, arc j -> i with label i and weight W[i*C + j].
+ */
+namespace {
+
+struct NgramArgs {
+  int B, T, C;
+  const float* emissions;
+  int emissions_on_device;
+  const int32_t* input_lens;
+  const float* trans_w;
+  int trans_on_device;
+  const int32_t* targets;
+  const int32_t* target_lens;
+  int blank;
+  float* losses_host;
+  float* grads;
+  int grads_on_device;
+  float* trans_grad;
+  int trans_grad_on_device;
+};
+
+#define TRY(x)                 \
+  do {                         \
+    if ((rc = (x))) goto done; \
+  } while (0)
+#define TRYCUDA(call)                                      \
+  do {                                                     \
+    cudaError_t e__ = (call);                              \
+    if (e__ != cudaSuccess) {                              \
+      rc = cuda_fail(ctx, e__, #call, __FILE__, __LINE__); \
+      goto done;                                           \
+    }                                                      \
+  } while (0)
+
+/* the gradients' destinations: emission rows zeroed (every row is written), W's gradient copied out */
+int ngram_copy_out(gtnb_ctx* ctx, const NgramArgs& a, const float* tg_dev) {
+  if (a.trans_grad)
+    GTNB_CUDA(ctx, cudaMemcpyAsync(a.trans_grad, tg_dev, sizeof(float) * a.C * a.C,
+                                   a.trans_grad_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                                   ctx->stream));
+  return GTNB_OK;
+}
+
+/*
+ * Materialised lattices, graph by graph as the reference composes them: intersect(E_b, G) and
+ * intersect(P_b, E_b), where P_b = intersect(ctc_b, G) is built on the host WITHOUT the fold (C start states
+ * (0, s), then (l, label(l))).  Reproduces the reference's inf / NaN propagation arc by arc; the path for
+ * non-finite weights.
+ */
+int ngram_ctc_loss_exact(gtnb_ctx* ctx, const NgramArgs& a, const std::vector<int32_t>& Tb) {
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, CC = (long long)C * C;
+  const bool want = a.grads || a.trans_grad;
+  int rc = GTNB_OK;
+  float *e_dev = nullptr, *g_dev = nullptr, *tg_dev = nullptr, *ft_grad = nullptr, *gg_grad = nullptr;
+  int32_t *ft_map_dev = nullptr, *gg_map_dev = nullptr;
+  gtnb_lattice *den = nullptr, *num = nullptr;
+  std::vector<float> W(CC);
+  // G (benchmarks/ctc.cpp transitionsGraph with a label-determined destination): arc j*C + i = j -> i
+  std::vector<uint8_t> gflags(C, 3);
+  std::vector<int32_t> gsrc(CC), gdst(CC), glab(CC), gmap(CC);
+  std::vector<float> gw(CC);
+  struct P {
+    std::vector<uint8_t> flags;
+    std::vector<int32_t> src, dst, lab;
+    std::vector<float> w;
+  };
+  std::vector<P> pg(B);
+  std::vector<gtnb_graph_view> pviews(B);
+  std::vector<int32_t> pmap;
+  gtnb_graph_view gview;
+  std::memset(&gview, 0, sizeof(gview));
+
+  if (a.trans_on_device)
+    GTNB_CUDA(ctx, cudaMemcpy(W.data(), a.trans_w, sizeof(float) * CC, cudaMemcpyDeviceToHost));
+  else
+    std::memcpy(W.data(), a.trans_w, sizeof(float) * CC);
+  for (int j = 0; j < C; j++)
+    for (int i = 0; i < C; i++) {
+      const long long k = (long long)j * C + i;
+      gsrc[k] = j;
+      gdst[k] = i;
+      glab[k] = i;
+      gw[k] = W[(long long)i * C + j];
+      gmap[k] = i * C + j;
+    }
+  gview.num_nodes = C;
+  gview.num_arcs = (int)CC;
+  gview.node_flags = gflags.data();
+  gview.arc_src = gsrc.data();
+  gview.arc_dst = gdst.data();
+  gview.arc_ilabel = gview.arc_olabel = glab.data();
+  gview.weights = gw.data();
+  {
+    long long toff = 0;
+    for (int b = 0; b < B; b++) {
+      const int U = a.target_lens[b], L = 2 * U + 1;
+      const int32_t* y = a.targets + toff;
+      toff += U;
+      auto lab = [&](int l) { return (l & 1) ? y[(l - 1) / 2] : a.blank; };
+      // node of CTC node l: (0, blank) for l = 0, C + l - 1 otherwise; nodes [0, C) are the start states (0, s)
+      auto node = [&](int l) { return l == 0 ? a.blank : C + l - 1; };
+      P& p = pg[b];
+      p.flags.assign(C + L - 1, 0);
+      for (int s = 0; s < C; s++) p.flags[s] = 1 | (L == 1 ? 2 : 0);
+      for (int l = std::max(1, L - 2); l < L; l++) p.flags[node(l)] |= 2;
+      auto arc = [&](int ls, int l) { // every arc of ctc_b (ls -> l) times the matching arcs of G
+        const int i = lab(l);
+        if (ls == 0) {
+          for (int s = 0; s < C; s++) {
+            p.src.push_back(s), p.dst.push_back(node(l)), p.lab.push_back(i);
+            p.w.push_back(W[(long long)i * C + s]), pmap.push_back(i * C + s);
+          }
+        } else {
+          p.src.push_back(node(ls)), p.dst.push_back(node(l)), p.lab.push_back(i);
+          p.w.push_back(W[(long long)i * C + lab(ls)]), pmap.push_back(i * C + lab(ls));
+        }
+      };
+      for (int l = 0; l < L; l++) {
+        arc(l, l);
+        if (l > 0) arc(l - 1, l);
+        if ((l & 1) && l > 1 && lab(l) != lab(l - 2)) arc(l - 2, l);
+      }
+      gtnb_graph_view& v = pviews[b];
+      std::memset(&v, 0, sizeof(v));
+      v.num_nodes = (int)p.flags.size();
+      v.num_arcs = (int)p.src.size();
+      v.node_flags = p.flags.data();
+      v.arc_src = p.src.data();
+      v.arc_dst = p.dst.data();
+      v.arc_ilabel = v.arc_olabel = p.lab.data();
+      v.weights = p.w.data();
+    }
+  }
+  {
+    const long long nP = (long long)pmap.size();
+    if (a.emissions_on_device) {
+      e_dev = const_cast<float*>(a.emissions);
+    } else {
+      TRY(dev_alloc(ctx, &e_dev, per * B));
+      TRYCUDA(cudaMemcpyAsync(e_dev, a.emissions, sizeof(float) * per * B, cudaMemcpyHostToDevice, ctx->stream));
+    }
+    TRY(gtnb_compose_linear(ctx, B, &gview, 1, 1, Tb.data(), C, e_dev, per, &den));
+    TRY(gtnb_compose_linear(ctx, B, pviews.data(), B, 0, Tb.data(), C, e_dev, per, &num));
+    TRY(gtnb_forward(ctx, den, 0, nullptr, nullptr));
+    TRY(gtnb_forward(ctx, num, 0, nullptr, nullptr));
+    if (want) {
+      if (a.grads && a.grads_on_device)
+        g_dev = a.grads;
+      else
+        TRY(dev_alloc(ctx, &g_dev, per * B));
+      TRYCUDA(cudaMemsetAsync(g_dev, 0, sizeof(float) * per * B, ctx->stream));
+      TRY(dev_alloc(ctx, &tg_dev, CC));
+      TRY(dev_alloc(ctx, &gg_grad, CC));
+      TRY(dev_alloc(ctx, &ft_grad, std::max<long long>(nP, 1)));
+      TRY(dev_alloc(ctx, &gg_map_dev, CC));
+      TRY(dev_alloc(ctx, &ft_map_dev, std::max<long long>(nP, 1)));
+      TRYCUDA(cudaMemsetAsync(tg_dev, 0, sizeof(float) * CC, ctx->stream));
+      TRYCUDA(cudaMemsetAsync(gg_grad, 0, sizeof(float) * CC, ctx->stream));
+      TRYCUDA(cudaMemsetAsync(ft_grad, 0, sizeof(float) * std::max<long long>(nP, 1), ctx->stream));
+      std::vector<float> m1(B, -1.0f);
+      TRY(gtnb_backward(ctx, den, 0, nullptr)); // +1 / -1: subtract's gradFunc (functions.cpp:53-58)
+      TRY(gtnb_backward(ctx, num, 0, m1.data()));
+      TRY(gtnb_compose_grad(ctx, den, gg_grad, g_dev, per));
+      TRY(gtnb_compose_grad(ctx, num, ft_grad, g_dev, per));
+      TRY(stage_begin(ctx));
+      TRY(stage_upload(ctx, gg_map_dev, gmap.data(), sizeof(int32_t) * CC));
+      if (nP) TRY(stage_upload(ctx, ft_map_dev, pmap.data(), sizeof(int32_t) * nP));
+      TRY(stage_end(ctx));
+      TRY(launch_scatter_add(ctx, tg_dev, gg_map_dev, gg_grad, CC));
+      TRY(launch_scatter_add(ctx, tg_dev, ft_map_dev, ft_grad, nP));
+      if (a.grads && !a.grads_on_device)
+        TRYCUDA(cudaMemcpyAsync(a.grads, g_dev, sizeof(float) * per * B, cudaMemcpyDeviceToHost, ctx->stream));
+      TRY(ngram_copy_out(ctx, a, tg_dev));
+    }
+    TRY(readback_reserve(ctx, 2 * sizeof(float) * B));
+    float* d = reinterpret_cast<float*>(ctx->readback);
+    float* n = d + B;
+    TRYCUDA(cudaMemcpyAsync(d, den->out_scores, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(n, num->out_scores, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaStreamSynchronize(ctx->stream));
+    for (int b = 0; b < B; b++) a.losses_host[b] = d[b] - n[b];
+  }
+done:
+  if (den) gtnb_lattice_destroy(ctx, den);
+  if (num) gtnb_lattice_destroy(ctx, num);
+  if (!a.emissions_on_device) dev_free(ctx, e_dev);
+  if (!(a.grads && a.grads_on_device)) dev_free(ctx, g_dev);
+  dev_free(ctx, tg_dev);
+  dev_free(ctx, gg_grad);
+  dev_free(ctx, ft_grad);
+  dev_free(ctx, gg_map_dev);
+  dev_free(ctx, ft_map_dev);
+  return rc;
+}
+
+/*
+ * The device path (k_ngram.cu): the folded numerator graphs built on the device from the targets and W, swept by
+ * k_implicit.cu on the second stream; the dense trellis of the denominator on the context's stream.  Both add
+ * their emission gradients into the zero-filled rows with red.add.  *needs_exact: a non-finite weight was met.
+ */
+int ngram_ctc_loss_fast(gtnb_ctx* ctx, const NgramArgs& a, const std::vector<int32_t>& Tb,
+                        const std::vector<SgDims>& dims, const std::vector<int32_t>& off, bool* needs_exact) {
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, CC = (long long)C * C;
+  const bool want = a.grads || a.trans_grad;
+  long long tot_t = 0, tot_A = 0;
+  for (int b = 0; b < B; b++) {
+    tot_t += a.target_lens[b];
+    tot_A += dims[b].A;
+  }
+  int rc = GTNB_OK;
+  float *e_dev = nullptr, *g_dev = nullptr, *w_dev = nullptr, *tg_dev = nullptr, *sigma = nullptr;
+  float *alpha = nullptr, *den = nullptr, *ggrad = nullptr, *minus1 = nullptr;
+  int32_t *small_dev = nullptr, *status = nullptr, *map = nullptr;
+  gtnb_lattice* lat = nullptr;
+  cudaStream_t main_stream = ctx->stream;
+  std::vector<long long> sgn, sga;
+  std::vector<int32_t> small_h((size_t)(tot_t + 3ll * B));
+  std::vector<float> m1(B, -1.0f);
+  if (tot_t) std::memcpy(small_h.data(), a.targets, sizeof(int32_t) * tot_t);
+  std::memcpy(small_h.data() + tot_t, off.data(), sizeof(int32_t) * B);
+  std::memcpy(small_h.data() + tot_t + B, a.target_lens, sizeof(int32_t) * B);
+  std::memcpy(small_h.data() + tot_t + 2ll * B, Tb.data(), sizeof(int32_t) * B);
+
+  TRY(ensure_side_streams(ctx, 0, 0));
+  if (a.emissions_on_device) {
+    e_dev = const_cast<float*>(a.emissions);
+  } else {
+    TRY(dev_alloc(ctx, &e_dev, per * B));
+    TRYCUDA(cudaMemcpyAsync(e_dev, a.emissions, sizeof(float) * per * B, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (a.trans_on_device)
+    w_dev = const_cast<float*>(a.trans_w);
+  else
+    TRY(dev_alloc(ctx, &w_dev, CC));
+  TRY(dev_alloc(ctx, &small_dev, (long long)small_h.size()));
+  TRY(dev_alloc(ctx, &status, 2ll * B));
+  TRY(dev_alloc(ctx, &sigma, C));
+  TRY(dev_alloc(ctx, &alpha, (long long)B * (T + 1) * C));
+  TRY(dev_alloc(ctx, &den, B));
+  TRY(dev_alloc(ctx, &map, tot_A));
+  TRY(composed_alloc(ctx, B, dims.data(), B, 0, Tb.data(), C, e_dev, per, sgn, sga, &lat, true));
+  if (want) {
+    if (a.grads && a.grads_on_device)
+      g_dev = a.grads;
+    else
+      TRY(dev_alloc(ctx, &g_dev, per * B));
+    TRY(dev_alloc(ctx, &tg_dev, CC + C)); // [d/dW | d/dsigma]
+    TRY(dev_alloc(ctx, &ggrad, tot_A));
+    TRY(dev_alloc(ctx, &minus1, B));
+    TRYCUDA(cudaMemsetAsync(g_dev, 0, sizeof(float) * per * B, ctx->stream));
+    TRYCUDA(cudaMemsetAsync(tg_dev, 0, sizeof(float) * (CC + C), ctx->stream));
+    TRYCUDA(cudaMemsetAsync(ggrad, 0, sizeof(float) * tot_A, ctx->stream));
+  }
+  TRYCUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * 2 * B, ctx->stream));
+  // one pinned staging pass: descriptors, [targets | offsets | lens | T], W from the host, the -1 seeds
+  TRY(stage_begin(ctx));
+  TRY(stage_upload(ctx, lat->meta, lat->meta_h.data(), sizeof(GraphMeta) * B));
+  TRY(stage_upload(ctx, small_dev, small_h.data(), sizeof(int32_t) * small_h.size()));
+  if (!a.trans_on_device) TRY(stage_upload(ctx, w_dev, a.trans_w, sizeof(float) * CC));
+  if (want) TRY(stage_upload(ctx, minus1, m1.data(), sizeof(float) * B));
+  TRY(stage_end(ctx));
+
+  TRY(launch_ngram_sigma(ctx, C, w_dev, sigma));
+  TRY(launch_ngram_num_build(ctx, lat, small_dev, small_dev + tot_t, small_dev + tot_t + B, a.blank, w_dev, sigma,
+                             map));
+  // the numerator (2U+2 nodes, <= 3 in-arcs) on the second stream beside the denominator (C^2 per frame)
+  TRYCUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
+  TRYCUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_fork, 0));
+  ctx->stream = ctx->copy_stream;
+  rc = launch_implicit_forward(ctx, lat, status + B);
+  if (!rc && want) rc = launch_implicit_backward(ctx, lat, minus1, g_dev, per, 0, -1, ggrad);
+  ctx->stream = main_stream;
+  if (rc) goto done;
+  TRY(launch_ngram_den_forward(ctx, B, T, C, small_dev + tot_t + 2ll * B, e_dev, per, w_dev, alpha, den, status));
+  if (want)
+    TRY(launch_ngram_den_backward(ctx, B, T, C, small_dev + tot_t + 2ll * B, e_dev, per, w_dev, alpha, den, g_dev,
+                                  per, tg_dev));
+  TRYCUDA(cudaEventRecord(ctx->ev_join, ctx->copy_stream));
+  TRYCUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+  if (want) {
+    TRY(launch_scatter_add(ctx, tg_dev, map, ggrad, tot_A)); // numerator arcs -> W entries and sigma slots
+    TRY(launch_ngram_fold(ctx, C, w_dev, sigma, tg_dev));
+    if (a.grads && !a.grads_on_device)
+      TRYCUDA(cudaMemcpyAsync(a.grads, g_dev, sizeof(float) * per * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRY(ngram_copy_out(ctx, a, tg_dev));
+  }
+  TRY(readback_reserve(ctx, 4 * sizeof(float) * B));
+  {
+    float* d = reinterpret_cast<float*>(ctx->readback);
+    float* n = d + B;
+    int32_t* st = reinterpret_cast<int32_t*>(n + B);
+    TRYCUDA(cudaMemcpyAsync(d, den, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(n, lat->out_scores, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(st, status, sizeof(int32_t) * 2 * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaStreamSynchronize(ctx->stream));
+    for (int b = 0; b < B; b++) a.losses_host[b] = d[b] - n[b];
+    for (int b = 0; b < 2 * B; b++) *needs_exact |= st[b] != 0;
+  }
+done:
+  ctx->stream = main_stream;
+  if (rc) cudaStreamSynchronize(ctx->copy_stream); // nothing may still run on the second stream when the buffers go
+  if (lat) gtnb_lattice_destroy(ctx, lat);
+  if (!a.emissions_on_device) dev_free(ctx, e_dev);
+  if (!(a.grads && a.grads_on_device)) dev_free(ctx, g_dev);
+  if (!a.trans_on_device) dev_free(ctx, w_dev);
+  dev_free(ctx, small_dev);
+  dev_free(ctx, status);
+  dev_free(ctx, sigma);
+  dev_free(ctx, alpha);
+  dev_free(ctx, den);
+  dev_free(ctx, map);
+  dev_free(ctx, tg_dev);
+  dev_free(ctx, ggrad);
+  dev_free(ctx, minus1);
+  return rc;
+}
+
+#undef TRY
+#undef TRYCUDA
+
+int ngram_ctc_loss_run(gtnb_ctx* ctx, const NgramArgs& a) {
+  const int B = a.B, T = a.T, C = a.C;
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !a.emissions || !a.trans_w || !a.target_lens || !a.losses_host)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: bad arguments");
+  if (a.blank < 0 || a.blank >= C)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: blank outside [0, C)");
+  if (C > kNgramMaxLabels)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                "gtnb_ngram_ctc_loss: C = " + std::to_string(C) + " labels; the trellis kernels hold W on chip for C <= " +
+                    std::to_string(kNgramMaxLabels));
+  std::vector<int32_t> Tb(B), off(B);
+  std::vector<SgDims> dims(B);
+  long long tot_t = 0;
+  for (int b = 0; b < B; b++) {
+    const int U = a.target_lens[b];
+    if (U < 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: negative target length");
+    if (U > 0 && !a.targets) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: targets is NULL");
+    const int32_t* y = a.targets + tot_t;
+    int skips = 0;
+    for (int u = 0; u < U; u++) {
+      if (y[u] < 0 || y[u] >= C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: label outside [0, C)");
+      if (u > 0) skips += y[u] != y[u - 1];
+    }
+    off[b] = (int32_t)tot_t;
+    tot_t += U;
+    Tb[b] = a.input_lens ? a.input_lens[b] : T;
+    if (Tb[b] < 0 || Tb[b] > T)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: input_lens outside [0, T]");
+    // folded numerator graph: S + 2U+1 CTC nodes; arcs = self loops + steps + skips + the two S arcs (one if U = 0)
+    const int L = 2 * U + 1;
+    dims[b] = SgDims{L + 1, L + (L - 1) + skips + std::min(L, 2), L >= 2 ? 2 : 1, /*all_valid=*/1, /*uniform=*/1,
+                     /*max_in=*/3, /*max_out=*/3};
+  }
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (B == 0) { // an empty batch: the transition gradient is 0
+    if (a.trans_grad) {
+      if (a.trans_grad_on_device) {
+        GTNB_CUDA(ctx, cudaMemsetAsync(a.trans_grad, 0, sizeof(float) * C * C, ctx->stream));
+        GTNB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      } else {
+        std::memset(a.trans_grad, 0, sizeof(float) * C * C);
+      }
+    }
+    return GTNB_OK;
+  }
+  bool needs_exact = false;
+  int rc = (implicit_dims_supported(dims.data(), B) && ctx->use_implicit)
+               ? ngram_ctc_loss_fast(ctx, a, Tb, dims, off, &needs_exact)
+               : ngram_ctc_loss_exact(ctx, a, Tb);
+  if (rc == GTNB_OK && needs_exact) {
+    // a non-finite weight: the materialised lattices reproduce the reference's inf / NaN propagation
+    arena_end(ctx);
+    arena_begin(ctx);
+    rc = ngram_ctc_loss_exact(ctx, a, Tb);
+  }
+  // T_b = 0: linearGraph(0, C) is one start node that does not accept (creations.cpp:20-33), so both
+  // intersections are empty and the reference's loss is -inf - -inf = NaN (no gradient)
+  for (int b = 0; b < B && rc == GTNB_OK; b++)
+    if (Tb[b] == 0) a.losses_host[b] = std::numeric_limits<float>::quiet_NaN();
+  return rc;
+}
+
+} // namespace
+
+extern "C" int gtnb_ngram_ctc_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const float* trans_w, int trans_on_device, const int32_t* targets, const int32_t* target_lens, int blank,
+    float* losses_host, float* grads, int grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const NgramArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, targets,
+                    target_lens, blank, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+  if (ctx) arena_begin(ctx);
+  const int rc = ngram_ctc_loss_run(ctx, a);
   if (ctx) arena_end(ctx);
   return rc;
 }

@@ -336,6 +336,19 @@ int ensure_side_streams(gtnb_ctx* ctx, int n_streams, int n_events);
 int launch_viterbi_dense(
     gtnb_ctx* ctx, int B, int T_max, int C, const int32_t* T_dev, const float* emis, int64_t stride,
     const float* trans_dev, uint8_t* bp, int32_t* paths, float* scores);
+// kernels (k_ngram.cu): CTC with a learned bigram transition graph
+constexpr int kNgramMaxLabels = 128;
+int launch_ngram_sigma(gtnb_ctx* ctx, int C, const float* W, float* sigma);
+int launch_ngram_num_build(
+    gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
+    const int32_t* tgt_len_dev, int blank, const float* W, const float* sigma, int32_t* map);
+int launch_ngram_den_forward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* W, float* alpha, float* den, int32_t* status);
+int launch_ngram_den_backward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad);
+int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, float* wgrad);
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);

@@ -1,0 +1,410 @@
+/*
+ * k_ngram.cu -- CTC with a learned bigram transition graph (gtnb_ngram_ctc_loss, the timeNgramCtc workload of
+ * benchmarks/ctc.cpp:107-134) without building either lattice.
+ *
+ * G is the label-determined bigram graph: C nodes, every node start and accept, arc j -> i with label i and
+ * weight W[i*C + j] (row = destination, column = source, ASG's layout).  Its state is the previous frame's label.
+ *
+ * Denominator, forwardScore(intersect(E, G)): a dense C-state trellis
+ *     alpha_0 = 0,   alpha_t[i] = e[t-1][i] + logsumexp_j (alpha_{t-1}[j] + W[i][j]),   Z = logsumexp_i alpha_T[i]
+ * (the C start states of G carry 0 at frame 0, so the first frame needs no special case).  One CTA per
+ * utterance, W resident in registers for the whole utterance: the forward kernel holds K entries of one ROW
+ * per thread (lanes_per_row threads per row, a shuffle reduction merges them), the backward kernel K entries
+ * of one COLUMN (beta_{t-1}[j] = logsumexp_i (W[i][j] + e[t-1][i] + beta_t[i])).  The backward kernel also
+ * sums the pair posteriors exp(alpha_{t-1}[j] + W[i][j] + e[t-1][i] + beta_t[i] - Z) over the frames in
+ * registers and flushes them with one atomic per W entry per CTA.  Log semiring, exact per-thread maxima,
+ * exp / log on the SFU (ex2.approx / lg2.approx): every sum has a term equal to 1, so nothing underflows to
+ * zero whatever the spread of W or the emissions.
+ *
+ * Numerator, forwardScore(intersect(intersect(ctc, G), E)): every in-arc of CTC node l >= 1 carries label(l), so
+ * the product is the CTC graph with arc weights W[label(dst)][label(src)], plus the C start states (0, s) of
+ * which only (0, blank) survives frame 0.  Folding those into one start node S gives S -> ctc 0 (weight
+ * sigma_blank) and S -> ctc 1 (sigma_y1), sigma_i = logsumexp_j W[i][j], d sigma_i / d W[i][j] =
+ * softmax_j(W[i][:]).  ngram_num_build_kernel writes that graph (2U+2 nodes, <= 3 in-arcs each) into the
+ * small-graph tables of an implicit lattice, plus an arc -> W-index map (C*C + i for the S arcs, which carry
+ * sigma_i); the sweeps are k_implicit.cu's, and ngram_fold_kernel applies the sigma chain rule.
+ *
+ * Valid only for finite weights: the denominator's forward kernel raises a status bit on any non-finite W
+ * entry or used emission, and the caller repeats the call through the materialised lattices.
+ */
+#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
+#include <algorithm>
+
+#include "gtnb_meta.h"
+#include "simt_emu.h"
+#else
+#include <cuda_runtime.h>
+#include <math_constants.h>
+
+#include <algorithm>
+
+#include "gtnb_internal.h"
+#endif
+
+namespace gtnb {
+
+constexpr int kNgramMaxC = 128; // labels the trellis kernels hold on chip (K * lanes_per_row <= 128)
+#ifndef GTNB_HOST_EMU
+static_assert(kNgramMaxC == kNgramMaxLabels, "gtnb_internal.h states the same limit");
+#endif
+constexpr int kNgramMaxThreads = 512;
+
+/* entries of W per thread and lanes per row (power of two) for an alphabet of C labels */
+inline void ngram_den_shape(int C, int* K, int* lanes, int* threads) {
+  *K = C <= 64 ? 16 : 32;
+  int l = 1;
+  while (l * *K < C) l *= 2;
+  *lanes = l;
+  *threads = (C * l + 31) & ~31;
+}
+
+namespace {
+
+#ifdef GTNB_HOST_EMU
+__device__ __forceinline__ float ng_exp(float x) {
+  return expf(x);
+}
+__device__ __forceinline__ float ng_log(float x) {
+  return logf(x);
+}
+#else
+__device__ __forceinline__ float ng_exp(float x) {
+  return __expf(x); // ex2.approx(x * log2 e)
+}
+__device__ __forceinline__ float ng_log(float x) {
+  return __logf(x); // lg2.approx(x) * ln 2; x >= 1 here
+}
+#endif
+__device__ __forceinline__ float ng_ninf() {
+  return -CUDART_INF_F;
+}
+__device__ __forceinline__ bool ng_finite(float x) {
+  return fabsf(x) < CUDART_INF_F;
+}
+
+/* (m, s) = logsumexp as max + sum of exp(x - max), merged over the `lanes` lanes of a row / column */
+__device__ __forceinline__ void ng_merge(float& m, float& s, int lanes) {
+  for (int o = 1; o < lanes; o <<= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    const float os = __shfl_xor_sync(0xffffffffu, s, o);
+    const float M = fmaxf(m, om);
+    const float Mm = M == ng_ninf() ? 0.0f : M; // all -inf: s stays 0
+    s = s * ng_exp(m - Mm) + os * ng_exp(om - Mm);
+    m = M;
+  }
+}
+
+/* alpha rows of every utterance to alpha[b][(T+1)*C], Z to den[b]; status[b] |= 1 on a non-finite weight */
+template <int K>
+__global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
+    int T, int C, int lanes, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    const float* __restrict__ W, float* __restrict__ alpha, float* __restrict__ den, int32_t* __restrict__ status) {
+  GTNB_STATIC_SMEM_2D(float, A, 2, kNgramMaxC);
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int Tb = lens[b];
+  const int i = tid / lanes, q = tid % lanes;
+  const bool row = i < C;
+  const bool lead = row && q == 0;
+  const float* em = emis + (long long)b * stride;
+  float* al = alpha + (long long)b * (T + 1) * C;
+  bool bad = false;
+  float w[K]; // W[i][q + lanes * k]: interleaved columns, so the lanes of a row read distinct banks
+#pragma unroll
+  for (int k = 0; k < K; k++) {
+    const int j = q + lanes * k;
+    const bool on = row && j < C;
+    w[k] = on ? __ldg(W + i * C + j) : ng_ninf();
+    if (on) bad |= !ng_finite(w[k]);
+  }
+  for (int j = tid; j < kNgramMaxC; j += blockDim.x) A[0][j] = A[1][j] = 0.0f; // alpha_0 = 0; padding stays 0
+  for (int j = tid; j < C; j += blockDim.x) al[j] = 0.0f;
+  __syncthreads();
+  float e_nx = (lead && Tb > 0) ? __ldg(em + i) : 0.0f;
+  for (int t = 1; t <= Tb; t++) {
+    const float e = e_nx;
+    if (lead && t < Tb) e_nx = __ldg(em + (long long)t * C + i);
+    bad |= !ng_finite(e);
+    const float* P = A[(t - 1) & 1];
+    float x[K];
+    float m = ng_ninf();
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      x[k] = P[q + lanes * k] + w[k];
+      m = fmaxf(m, x[k]);
+    }
+    const float mm = m == ng_ninf() ? 0.0f : m;
+    float s = 0.0f;
+#pragma unroll
+    for (int k = 0; k < K; k++) s += ng_exp(x[k] - mm);
+    ng_merge(m, s, lanes);
+    if (lead) {
+      const float v = e + (m + ng_log(s));
+      A[t & 1][i] = v;
+      al[(long long)t * C + i] = v;
+    }
+    __syncthreads();
+  }
+  bad = __syncthreads_or(bad);
+  if (tid < 32) {
+    const float* F = A[Tb & 1];
+    float m = ng_ninf();
+    for (int j = tid; j < C; j += 32) m = fmaxf(m, F[j]);
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float s = 0.0f;
+    for (int j = tid; j < C; j += 32) s += expf(F[j] - m);
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (tid == 0) {
+      den[b] = m + logf(s);
+      if (bad) atomicOr(&status[b], 1);
+    }
+  }
+}
+
+/* d Z / d e added into grad (rows t < T_b), d Z / d W added into wgrad[C*C] (one atomic per entry per CTA) */
+template <int K>
+__global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
+    int T, int C, int lanes, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    const float* __restrict__ W, const float* __restrict__ alpha, const float* __restrict__ den,
+    float* __restrict__ grad, long long grad_stride, float* __restrict__ wgrad) {
+  GTNB_STATIC_SMEM_2D(float, Bt, 2, kNgramMaxC); // beta_t, beta_{t-1}
+  GTNB_STATIC_SMEM(float, G, kNgramMaxC); // e[t-1][i] + beta_t[i]; padding 0
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int Tb = lens[b];
+  const float Z = den[b];
+  if (!ng_finite(Z) || Tb < 1) return; // (non-finite: the caller repeats the call materialised)
+  const int j = tid / lanes, q = tid % lanes;
+  const bool col = j < C;
+  const bool lead = col && q == 0;
+  const float* em = emis + (long long)b * stride;
+  const float* al = alpha + (long long)b * (T + 1) * C;
+  float* gr = grad + (long long)b * grad_stride;
+  float w[K], acc[K]; // W[q + lanes * k][j] and its pair posteriors
+#pragma unroll
+  for (int k = 0; k < K; k++) {
+    const int i = q + lanes * k;
+    w[k] = (col && i < C) ? __ldg(W + i * C + j) : ng_ninf();
+    acc[k] = 0.0f;
+  }
+  for (int i = tid; i < kNgramMaxC; i += blockDim.x) {
+    Bt[Tb & 1][i] = 0.0f; // every node accepts: beta_T = 0
+    G[i] = 0.0f;
+  }
+  // one frame of prefetch: alpha_t and e[t-1] of the rows this thread turns into G, alpha_{t-1} of its column
+  const bool rowt = tid < C;
+  float a_nx = rowt ? al[(long long)Tb * C + tid] : 0.0f;
+  float e_nx = rowt ? __ldg(em + (long long)(Tb - 1) * C + tid) : 0.0f;
+  float aj_nx = col ? al[(long long)(Tb - 1) * C + j] : 0.0f;
+  __syncthreads();
+  for (int t = Tb; t >= 1; t--) {
+    const float a_t = a_nx, e_t = e_nx, aj = aj_nx;
+    if (t > 1) {
+      if (rowt) {
+        a_nx = al[(long long)(t - 1) * C + tid];
+        e_nx = __ldg(em + (long long)(t - 2) * C + tid);
+      }
+      if (col) aj_nx = al[(long long)(t - 2) * C + j];
+    }
+    if (rowt) {
+      const float bt = Bt[t & 1][tid];
+      G[tid] = e_t + bt;
+      atomicAdd(gr + (long long)(t - 1) * C + tid, ng_exp(a_t + bt - Z)); // node posterior
+    }
+    __syncthreads();
+    float x[K];
+    float m = ng_ninf();
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      x[k] = w[k] + G[q + lanes * k];
+      m = fmaxf(m, x[k]);
+    }
+    const float mm = m == ng_ninf() ? 0.0f : m;
+    float s = 0.0f;
+    const float f = ng_exp((mm + aj) - Z); // pair posterior = exp(x - mm) * f
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      const float p = ng_exp(x[k] - mm);
+      s += p;
+      acc[k] = fmaf(p, f, acc[k]);
+    }
+    ng_merge(m, s, lanes);
+    if (lead) Bt[(t - 1) & 1][j] = m + ng_log(s);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < K; k++) {
+    const int i = q + lanes * k;
+    if (col && i < C && acc[k] != 0.0f) atomicAdd(wgrad + i * C + j, acc[k]);
+  }
+}
+
+/* sigma_i = logsumexp_j W[i][j], one warp per row */
+__global__ void __launch_bounds__(256) ngram_sigma_kernel(int C, const float* __restrict__ W, float* __restrict__ sigma) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (i >= C) return; // whole warps
+  float m = ng_ninf();
+  for (int j = lane; j < C; j += 32) m = fmaxf(m, W[i * C + j]);
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  float s = 0.0f;
+  for (int j = lane; j < C; j += 32) s += expf(W[i * C + j] - m);
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) sigma[i] = m + logf(s);
+}
+
+/* wgrad[i][j] += wgrad[C*C + i] * softmax_j(W[i][:]): the S arcs' gradient through sigma_i */
+__global__ void __launch_bounds__(256) ngram_fold_kernel(
+    int C, const float* __restrict__ W, const float* __restrict__ sigma, float* __restrict__ wgrad) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= C * C) return;
+  const int i = a / C;
+  const float g = wgrad[C * C + i];
+  if (g != 0.0f) wgrad[a] += g * expf(W[a] - sigma[i]);
+}
+
+/*
+ * The folded numerator graph of utterance b in the small-graph tables (k_ctc.cu's ctc_build_kernel with
+ * weights): node 0 = S (start), node n >= 1 = CTC node l = n - 1 (benchmarks/ctc.cpp:40-58, accept = last two);
+ * in-arcs of node n in the order skip, step, self, then the S arc for l <= 1.  The in-entry index is the arc
+ * id, and map[grad_graph_off + arc] its W index (C*C + i for an S arc of weight sigma_i).
+ */
+__global__ void __launch_bounds__(256) ngram_num_build_kernel(
+    const GraphMeta* __restrict__ meta, const int32_t* __restrict__ targets, const int32_t* __restrict__ tgt_off,
+    const int32_t* __restrict__ tgt_len, int blank, int C, const float* __restrict__ W,
+    const float* __restrict__ sigma, uint8_t* __restrict__ sg_flags, int32_t* __restrict__ sg_in_ptr,
+    int32_t* __restrict__ sg_in_src, int32_t* __restrict__ sg_in_label, int32_t* __restrict__ sg_in_arc,
+    float* __restrict__ sg_in_w, int32_t* __restrict__ sg_ilabel, int32_t* __restrict__ sg_olabel,
+    int32_t* __restrict__ acc_nodes, int32_t* __restrict__ map) {
+  GTNB_STATIC_SMEM(int, scan, 256);
+  GTNB_STATIC_SMEM(int, carry_box, 1);
+  int& carry = carry_box[0];
+  const int b = blockIdx.x;
+  const GraphMeta m = meta[b];
+  const int tid = threadIdx.x;
+  const int U = tgt_len[b];
+  const int L = 2 * U + 1, N = L + 1;
+  const int32_t* tg = targets + tgt_off[b];
+  uint8_t* fl = sg_flags + m.sg_node_base;
+  int32_t* ip = sg_in_ptr + m.sg_node_base;
+  int32_t* is = sg_in_src + m.sg_arc_base;
+  int32_t* il = sg_in_label + m.sg_arc_base;
+  int32_t* ia = sg_in_arc + m.sg_arc_base;
+  float* iw = sg_in_w + m.sg_arc_base;
+  int32_t* lab_i = sg_ilabel + m.sg_arc_base;
+  int32_t* lab_o = sg_olabel + m.sg_arc_base;
+  int32_t* mp = map + m.grad_graph_off;
+  auto lab = [&](int l) { return (l & 1) ? tg[(l - 1) / 2] : blank; };
+  if (tid == 0) carry = 0;
+  __syncthreads();
+  for (int n0 = 0; n0 < N; n0 += 256) {
+    const int n = n0 + tid, l = n - 1;
+    int label = blank, narcs = 0;
+    bool skip = false;
+    if (n < N && n > 0) {
+      label = lab(l);
+      skip = (l & 1) && l > 1 && label != tg[(l - 1) / 2 - 1];
+      narcs = 1 + (l > 0 ? 1 : 0) + (skip ? 1 : 0) + (l <= 1 ? 1 : 0);
+    }
+    scan[tid] = narcs;
+    __syncthreads();
+    for (int o = 1; o < 256; o <<= 1) {
+      const int v = tid >= o ? scan[tid - o] : 0;
+      __syncthreads();
+      scan[tid] += v;
+      __syncthreads();
+    }
+    const int base = carry + scan[tid] - narcs;
+    if (n < N) {
+      const bool acc = (L >= 2) ? (l == L - 1 || l == L - 2) : (l == 0);
+      fl[n] = (uint8_t)((n == 0 ? 1 : 0) | (acc ? 2 : 0));
+      ip[n] = base;
+      int e = base;
+      auto put = [&](int src, float wt, int widx) {
+        is[e] = src;
+        ia[e] = e;
+        il[e] = label;
+        iw[e] = wt;
+        lab_i[e] = label;
+        lab_o[e] = label;
+        mp[e] = widx;
+        e++;
+      };
+      if (n > 0) {
+        if (skip) put(n - 2, __ldg(W + label * C + lab(l - 2)), label * C + lab(l - 2));
+        if (l > 0) put(n - 1, __ldg(W + label * C + lab(l - 1)), label * C + lab(l - 1));
+        put(n, __ldg(W + label * C + label), label * C + label);
+        if (l <= 1) put(0, sigma[label], C * C + label);
+      }
+    }
+    __syncthreads();
+    if (tid == 255) carry += scan[255];
+    __syncthreads();
+  }
+  if (tid == 0) {
+    ip[N] = carry;
+    int32_t* acc = acc_nodes + m.acc_base;
+    if (L >= 2) {
+      acc[0] = L - 1; // device nodes of CTC nodes L - 2, L - 1
+      acc[1] = L;
+    } else {
+      acc[0] = 1;
+    }
+  }
+}
+
+} // namespace
+
+#ifndef GTNB_HOST_EMU
+
+int launch_ngram_sigma(gtnb_ctx* ctx, int C, const float* W, float* sigma) {
+  GTNB_LAUNCH(ctx, "ngram_sigma", ngram_sigma_kernel<<<(C * 32 + 255) / 256, 256, 0, ctx->stream>>>(C, W, sigma));
+  return GTNB_OK;
+}
+
+int launch_ngram_num_build(
+    gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
+    const int32_t* tgt_len_dev, int blank, const float* W, const float* sigma, int32_t* map) {
+  if (lat->B == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "ngram_num_build", ngram_num_build_kernel<<<lat->B, 256, 0, ctx->stream>>>(
+      lat->meta, targets_dev, tgt_off_dev, tgt_len_dev, blank, lat->C, W, sigma, lat->sg_flags, lat->sg_in_ptr,
+      lat->sg_in_src, lat->sg_in_label, lat->sg_in_arc, lat->sg_in_w, lat->sg_ilabel, lat->sg_olabel,
+      lat->acc_nodes, map));
+  return GTNB_OK;
+}
+
+int launch_ngram_den_forward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* W, float* alpha, float* den, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  int K, lanes, threads;
+  ngram_den_shape(C, &K, &lanes, &threads);
+  if (K == 16)
+    GTNB_LAUNCH(ctx, "ngram_den_forward", ngram_den_forward_kernel<16><<<B, threads, 0, ctx->stream>>>(
+        T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
+  else
+    GTNB_LAUNCH(ctx, "ngram_den_forward", ngram_den_forward_kernel<32><<<B, threads, 0, ctx->stream>>>(
+        T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
+  return GTNB_OK;
+}
+
+int launch_ngram_den_backward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  int K, lanes, threads;
+  ngram_den_shape(C, &K, &lanes, &threads);
+  if (K == 16)
+    GTNB_LAUNCH(ctx, "ngram_den_backward", ngram_den_backward_kernel<16><<<B, threads, 0, ctx->stream>>>(
+        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
+  else
+    GTNB_LAUNCH(ctx, "ngram_den_backward", ngram_den_backward_kernel<32><<<B, threads, 0, ctx->stream>>>(
+        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
+  return GTNB_OK;
+}
+
+int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, float* wgrad) {
+  GTNB_LAUNCH(ctx, "ngram_fold", ngram_fold_kernel<<<(C * C + 255) / 256, 256, 0, ctx->stream>>>(C, W, sigma, wgrad));
+  return GTNB_OK;
+}
+
+#endif // GTNB_HOST_EMU
+
+} // namespace gtnb

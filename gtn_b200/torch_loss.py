@@ -121,3 +121,70 @@ class ASGLossFunction(torch.autograd.Function):
 
 def asg_loss(emissions, transitions, targets, reduction="mean", allreduce=True):
     return ASGLossFunction.apply(emissions, transitions, targets, reduction, allreduce)
+
+
+class NgramCTCLossFunction(torch.autograd.Function):
+    """CTC with a learned bigram transition graph G (benchmarks/ctc.cpp:107-134, timeNgramCtc):
+        loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(ctc_b, G), E_b))
+    G: C nodes, all start and accept, arc j -> i with label i and weight transitions[i, j] (row = destination
+    label, column = source label), shared by the minibatch and, with torch.distributed initialised, by all ranks
+    (the transition gradient is all-reduced over NCCL, as asg_loss does).
+
+    emissions: float32 CUDA tensor [B, T, C]; transitions: float32 CUDA tensor of C*C elements ([C, C] or flat) on
+    the same device; targets: list of 1-D int sequences; input_lengths: None, a list or an int tensor (any
+    device).  Everything runs on the current stream of the emissions' device, device pointers in and out: only
+    the B losses (and input_lengths, when given on the GPU) are copied to the host.
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True):
+        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        e = emissions.contiguous()
+        B, T, Cn = e.shape
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == Cn * Cn
+        w = transitions.detach().contiguous()
+        stream = torch.cuda.current_stream(e.device).cuda_stream
+        g = _ctx_for(e.device, stream)
+        lens = np.asarray([len(t) for t in targets], np.int32)
+        cat = np.ascontiguousarray(
+            np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
+        il = None
+        if input_lengths is not None:
+            il = np.ascontiguousarray(
+                input_lengths.detach().cpu().numpy() if torch.is_tensor(input_lengths) else input_lengths, np.int32)
+            assert il.shape == (B,)
+        losses = np.zeros(B, np.float32)
+        grad = torch.empty_like(e)  # every row is written by the call
+        tg = torch.empty(Cn * Cn, dtype=torch.float32, device=e.device)
+        g._check(capi.lib().gtnb_ngram_ctc_loss(
+            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), w.data_ptr(), 1,
+            cat.ctypes.data_as(capi._i32p), lens.ctypes.data_as(capi._i32p), int(blank),
+            losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, tg.data_ptr(), 1))
+        tg = tg.view_as(transitions)
+        ctx.world = 1
+        if allreduce and torch.distributed.is_available() and torch.distributed.is_initialized():
+            torch.distributed.all_reduce(tg, op=torch.distributed.ReduceOp.SUM)
+            ctx.world = torch.distributed.get_world_size()
+        out = torch.from_numpy(losses).to(e.device)
+        ctx.save_for_backward(grad, tg)
+        ctx.reduction = reduction
+        ctx.B = B
+        return out.mean() if reduction == "mean" else out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        grad, tg = ctx.saved_tensors
+        if ctx.reduction == "mean":
+            # the mean over the GLOBAL batch when the transition gradient was summed over the ranks
+            scale = grad_output / ctx.B
+            return grad * scale, tg * (scale / ctx.world), None, None, None, None, None
+        # reduction "none": as asg_loss, the transition gradient was summed over the batch inside the call, which
+        # is the chain rule's answer only for a uniform upstream gradient
+        assert bool((grad_output == grad_output.flatten()[0]).all()), \
+            "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
+        return grad * grad_output.view(-1, 1, 1), tg * grad_output.flatten()[0], None, None, None, None, None
+
+
+def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True):
+    return NgramCTCLossFunction.apply(emissions, transitions, targets, input_lengths, blank, reduction, allreduce)

@@ -366,6 +366,39 @@ int gtnb_asg_loss(
     float* trans_grad_host);
 
 /*
+ * CTC with a learned bigram transition graph for a whole minibatch (benchmarks/ctc.cpp:107-134, timeNgramCtc):
+ *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(ctc_b, G), E_b))
+ * E_b: linearGraph(T_b, C) on the first T_b = input_lens[b] (or T) rows of emissions_b; ctc_b: the CTC graph of
+ * target_b with `blank` (as gtnb_ctc_loss); G: C nodes, every node start and accept, arc j -> i with label i and
+ * weight trans_w[i*C + j] (row = destination label, column = source label, ASG's layout), so G's state is the
+ * previous frame's label, blank included.
+ * trans_w [C*C] and trans_grad (nullable, [C*C]: the batch sum of d loss_b / d trans_w, as Graph::addGrad
+ * accumulates it) live on the device when *_on_device, else on the host; likewise emissions and grads
+ * (nullable, [B][T][C]: d loss_b / d e_b).  Unlike gtnb_ctc_loss, EVERY row of grads is written: rows t >= T_b
+ * are set to 0, so the caller needs no memset.  An infeasible target (T_b too short) gives +inf and the
+ * denominator's gradient alone.  Needs C <= 128 (GTNB_ERR_UNSUPPORTED above: W is held on chip); labels outside
+ * [0, C), negative lengths or T_b > T are GTNB_ERR_INVALID_ARGUMENT.
+ */
+int gtnb_ngram_ctc_loss(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* nullable */
+    const float* trans_w,
+    int trans_on_device,
+    const int32_t* targets,
+    const int32_t* target_lens,
+    int blank,
+    float* losses_host,
+    float* grads, /* nullable */
+    int grads_on_device,
+    float* trans_grad, /* nullable */
+    int trans_grad_on_device);
+
+/*
  * viterbiPath + viterbiScore of compose(linearGraph(T, C; e_b), transitions) for a whole
  * minibatch (test/criterion_test.cpp:308-345, BASELINE.json configs[3]) WITHOUT
  * materialising the T*C*C lattice (32.75 M arcs per utterance at T=2000, C=128).
