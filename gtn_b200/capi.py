@@ -94,6 +94,9 @@ SYMBOLS = [
     ("gtnb_ngram_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int, _vp, C.c_int]),
+    ("gtnb_asg_loss_ex", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, _f32p, _vp, C.c_int, _vp,
+      C.c_int]),
 ]
 
 _lib = None
@@ -397,6 +400,48 @@ class Ctx:
             self._check(lib().gtnb_ngram_ctc_loss(
                 self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), w_dev.ptr, 1, _p(cat, _i32p), _p(lens, _i32p),
                 int(blank), _p(losses, _f32p), g_dev.ptr, 1, tg_dev.ptr, 1))
+            grads = g_dev.download(e.shape)
+            tg = tg_dev.download(tw.shape)
+        finally:
+            for buf in (e_dev, w_dev, g_dev, tg_dev):
+                buf.free()
+        return losses, grads, tg
+
+    def asg_loss_ex(self, emissions, trans_w, targets, want_grad=True, input_lens=None):
+        """Host-buffer entry of gtnb_asg_loss_ex: emissions [B,T,C], trans_w [C + C*C] (start weights, then the
+        C x C matrix, row = destination label), input_lens [B] or None
+        -> (losses [B], grads [B,T,C] or None, trans_grad [C + C*C] or None)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == Cn + Cn * Cn
+        cat, lens = _cat_targets(targets)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        losses = np.zeros(B, np.float32)
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        tg = np.zeros(Cn + Cn * Cn, np.float32) if want_grad else None
+        self._check(lib().gtnb_asg_loss_ex(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), tw.ctypes.data, 0, _p(cat, _i32p), _p(lens, _i32p),
+            _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0, None if tg is None else tg.ctypes.data,
+            0))
+        return losses, grads, tg
+
+    def asg_loss_ex_dev(self, emissions, trans_w, targets, input_lens=None):
+        """Device-buffer entry: emissions and trans_w uploaded once, gtnb_asg_loss_ex on device pointers (gradients
+        in HBM), downloaded afterwards -> (losses, grads, trans_grad)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == Cn + Cn * Cn
+        cat, lens = _cat_targets(targets)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        losses = np.zeros(B, np.float32)
+        e_dev, w_dev = self.to_device(e), self.to_device(tw)
+        g_dev, tg_dev = self.alloc(max(e.nbytes, 16)), self.alloc(tw.nbytes)
+        try:
+            self._check(lib().gtnb_asg_loss_ex(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), w_dev.ptr, 1, _p(cat, _i32p), _p(lens, _i32p),
+                _p(losses, _f32p), g_dev.ptr, 1, tg_dev.ptr, 1))
             grads = g_dev.download(e.shape)
             tg = tg_dev.download(tw.shape)
         finally:

@@ -478,10 +478,17 @@ extern "C" int gtnb_viterbi_dense(
  * (accumulated over the batch, graph.cpp:96-100) the transitions.  The denominator lattice
  * is materialised on the device (C + (T-1) C^2 arcs per utterance); compose(fal_b,
  * transitions) is a 2U-arc chain built on the host from the target (pure construction).
+ * input_lens (nullable: T for every utterance): e_b is linearGraph(T_b, C) on the first T_b rows; the rows of
+ * grads beyond T_b are zeroed.
  */
+static int asg_loss_call(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
+    const int32_t* input_lens, const float* trans_w_host, const int32_t* targets, const int32_t* target_lens,
+    float* losses_host, float* grads, int grads_on_device, float* trans_grad_host);
+
 static int asg_loss_run(
     gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
-    const float* trans_w_host, const int32_t* targets, const int32_t* target_lens,
+    const int32_t* input_lens, const float* trans_w_host, const int32_t* targets, const int32_t* target_lens,
     float* losses_host, float* grads, int grads_on_device, float* trans_grad_host) {
   if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions || !trans_w_host || !target_lens || !losses_host)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss: bad arguments");
@@ -535,6 +542,7 @@ static int asg_loss_run(
   std::vector<gtnb_graph_view> fviews(B);
   std::vector<int32_t> ft_map;
   std::vector<int32_t> Tb(B, T);
+  if (input_lens) std::copy(input_lens, input_lens + B, Tb.begin());
   long long toff = 0;
   for (int b = 0; b < B; b++) {
     const int U = target_lens[b];
@@ -706,7 +714,7 @@ done:
     // a non-finite weight: repeat through the materialised lattices, which reproduce the
     // reference's inf / NaN propagation arc by arc
     ctx->use_implicit = false;
-    rc = gtnb_asg_loss(ctx, B, T, C, emissions, emissions_on_device, trans_w_host, targets, target_lens,
+    rc = asg_loss_call(ctx, B, T, C, emissions, emissions_on_device, input_lens, trans_w_host, targets, target_lens,
                        losses_host, grads, grads_on_device, trans_grad_host);
     ctx->use_implicit = true;
   }
@@ -715,15 +723,23 @@ done:
 #undef TRYCUDA
 }
 
+static int asg_loss_call(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
+    const int32_t* input_lens, const float* trans_w_host, const int32_t* targets, const int32_t* target_lens,
+    float* losses_host, float* grads, int grads_on_device, float* trans_grad_host) {
+  if (ctx) arena_begin(ctx);
+  const int rc = asg_loss_run(ctx, B, T, C, emissions, emissions_on_device, input_lens, trans_w_host, targets,
+                              target_lens, losses_host, grads, grads_on_device, trans_grad_host);
+  if (ctx) arena_end(ctx);
+  return rc;
+}
+
 extern "C" int gtnb_asg_loss(
     gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
     const float* trans_w_host, const int32_t* targets, const int32_t* target_lens,
     float* losses_host, float* grads, int grads_on_device, float* trans_grad_host) {
-  if (ctx) arena_begin(ctx);
-  const int rc = asg_loss_run(ctx, B, T, C, emissions, emissions_on_device, trans_w_host, targets, target_lens,
-                              losses_host, grads, grads_on_device, trans_grad_host);
-  if (ctx) arena_end(ctx);
-  return rc;
+  return asg_loss_call(ctx, B, T, C, emissions, emissions_on_device, nullptr, trans_w_host, targets, target_lens,
+                       losses_host, grads, grads_on_device, trans_grad_host);
 }
 
 /*
@@ -1123,6 +1139,262 @@ extern "C" int gtnb_ngram_ctc_loss(
                     target_lens, blank, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
   if (ctx) arena_begin(ctx);
   const int rc = ngram_ctc_loss_run(ctx, a);
+  if (ctx) arena_end(ctx);
+  return rc;
+}
+
+/*
+ * ASG with per-utterance frame counts and device-resident transitions (gtnb_asg_loss_ex):
+ *   loss_b = forwardScore(compose(E_b, transitions)) - forwardScore(compose(compose(fal_b, transitions), E_b))
+ * with E_b = linearGraph(T_b, C) on the first T_b rows.  For C <= 128 the denominator is k_ngram.cu's dense trellis
+ * in its start mode and the numerator graphs are built on the device; otherwise (and for non-finite weights) the
+ * call goes through asg_loss_run with the same T_b.
+ */
+namespace {
+
+struct AsgArgs {
+  int B, T, C;
+  const float* emissions;
+  int emissions_on_device;
+  const int32_t* input_lens;
+  const float* trans_w;
+  int trans_on_device;
+  const int32_t* targets;
+  const int32_t* target_lens;
+  float* losses_host;
+  float* grads;
+  int grads_on_device;
+  float* trans_grad;
+  int trans_grad_on_device;
+};
+
+#define TRY(x)                 \
+  do {                         \
+    if ((rc = (x))) goto done; \
+  } while (0)
+#define TRYCUDA(call)                                      \
+  do {                                                     \
+    cudaError_t e__ = (call);                              \
+    if (e__ != cudaSuccess) {                              \
+      rc = cuda_fail(ctx, e__, #call, __FILE__, __LINE__); \
+      goto done;                                           \
+    }                                                      \
+  } while (0)
+
+/*
+ * The device path: the numerator graphs (U+1 nodes, two in-arcs each) built on the device from the targets and
+ * trans_w and swept by k_implicit.cu on the second stream; the denominator's dense trellis in start mode on the
+ * context's stream.  Both add their emission gradients into the zero-filled rows with red.add; the numerator's
+ * arc gradients are scattered into trans_grad after the streams join.  *needs_exact: a non-finite weight.
+ */
+int asg_loss_ex_fast(gtnb_ctx* ctx, const AsgArgs& a, const std::vector<int32_t>& Tb, const std::vector<SgDims>& dims,
+                     const std::vector<int32_t>& off, bool* needs_exact) {
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, nTrans = C + (long long)C * C;
+  const bool want = a.grads || a.trans_grad;
+  long long tot_t = 0, tot_A = 0;
+  for (int b = 0; b < B; b++) {
+    tot_t += a.target_lens[b];
+    tot_A += dims[b].A;
+  }
+  int rc = GTNB_OK;
+  float *e_dev = nullptr, *g_dev = nullptr, *w_dev = nullptr, *tg_dev = nullptr;
+  float *alpha = nullptr, *den = nullptr, *ggrad = nullptr, *minus1 = nullptr;
+  int32_t *small_dev = nullptr, *status = nullptr, *map = nullptr;
+  gtnb_lattice* lat = nullptr;
+  cudaStream_t main_stream = ctx->stream;
+  std::vector<long long> sgn, sga;
+  std::vector<int32_t> small_h((size_t)(tot_t + 3ll * B));
+  std::vector<float> m1(B, -1.0f);
+  if (tot_t) std::memcpy(small_h.data(), a.targets, sizeof(int32_t) * tot_t);
+  std::memcpy(small_h.data() + tot_t, off.data(), sizeof(int32_t) * B);
+  std::memcpy(small_h.data() + tot_t + B, a.target_lens, sizeof(int32_t) * B);
+  std::memcpy(small_h.data() + tot_t + 2ll * B, Tb.data(), sizeof(int32_t) * B);
+
+  TRY(ensure_side_streams(ctx, 0, 0));
+  if (a.emissions_on_device) {
+    e_dev = const_cast<float*>(a.emissions);
+  } else {
+    TRY(dev_alloc(ctx, &e_dev, per * B));
+    TRYCUDA(cudaMemcpyAsync(e_dev, a.emissions, sizeof(float) * per * B, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  if (a.trans_on_device)
+    w_dev = const_cast<float*>(a.trans_w);
+  else
+    TRY(dev_alloc(ctx, &w_dev, nTrans));
+  TRY(dev_alloc(ctx, &small_dev, (long long)small_h.size()));
+  TRY(dev_alloc(ctx, &status, 2ll * B));
+  TRY(dev_alloc(ctx, &alpha, asg_alpha_floats(B, T, C))); // rows and per-frame offsets
+  TRY(dev_alloc(ctx, &den, B));
+  TRY(dev_alloc(ctx, &map, tot_A));
+  TRY(composed_alloc(ctx, B, dims.data(), B, 0, Tb.data(), C, e_dev, per, sgn, sga, &lat, true));
+  if (want) {
+    if (a.grads && a.grads_on_device)
+      g_dev = a.grads;
+    else
+      TRY(dev_alloc(ctx, &g_dev, per * B));
+    if (a.trans_grad && a.trans_grad_on_device)
+      tg_dev = a.trans_grad;
+    else
+      TRY(dev_alloc(ctx, &tg_dev, nTrans));
+    TRY(dev_alloc(ctx, &ggrad, tot_A));
+    TRY(dev_alloc(ctx, &minus1, B));
+    TRYCUDA(cudaMemsetAsync(g_dev, 0, sizeof(float) * per * B, ctx->stream));
+    TRYCUDA(cudaMemsetAsync(tg_dev, 0, sizeof(float) * nTrans, ctx->stream));
+    if (tot_A) TRYCUDA(cudaMemsetAsync(ggrad, 0, sizeof(float) * tot_A, ctx->stream));
+  }
+  TRYCUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * 2 * B, ctx->stream));
+  // one pinned staging pass: descriptors, [targets | offsets | lens | T], trans_w from the host, the -1 seeds
+  TRY(stage_begin(ctx));
+  TRY(stage_upload(ctx, lat->meta, lat->meta_h.data(), sizeof(GraphMeta) * B));
+  TRY(stage_upload(ctx, small_dev, small_h.data(), sizeof(int32_t) * small_h.size()));
+  if (!a.trans_on_device) TRY(stage_upload(ctx, w_dev, a.trans_w, sizeof(float) * nTrans));
+  if (want) TRY(stage_upload(ctx, minus1, m1.data(), sizeof(float) * B));
+  TRY(stage_end(ctx));
+
+  TRY(launch_asg_num_build(ctx, lat, small_dev, small_dev + tot_t, small_dev + tot_t + B, w_dev, map));
+  // the numerator (U+1 nodes, <= 2 in-arcs) on the second stream beside the denominator (C^2 per frame)
+  TRYCUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
+  TRYCUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_fork, 0));
+  ctx->stream = ctx->copy_stream;
+  rc = launch_implicit_forward(ctx, lat, status + B);
+  if (!rc && want) rc = launch_implicit_backward(ctx, lat, minus1, g_dev, per, 0, -1, ggrad);
+  ctx->stream = main_stream;
+  if (rc) goto done;
+  TRY(launch_asg_den_forward(ctx, B, T, C, small_dev + tot_t + 2ll * B, e_dev, per, w_dev, alpha, den, status));
+  if (want)
+    TRY(launch_asg_den_backward(ctx, B, T, C, small_dev + tot_t + 2ll * B, e_dev, per, w_dev, alpha, den, g_dev, per,
+                                tg_dev));
+  TRYCUDA(cudaEventRecord(ctx->ev_join, ctx->copy_stream));
+  TRYCUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+  if (want) {
+    TRY(launch_scatter_add(ctx, tg_dev, map, ggrad, tot_A)); // numerator arcs -> start weights and matrix entries
+    if (a.grads && !a.grads_on_device)
+      TRYCUDA(cudaMemcpyAsync(a.grads, g_dev, sizeof(float) * per * B, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a.trans_grad && !a.trans_grad_on_device)
+      TRYCUDA(cudaMemcpyAsync(a.trans_grad, tg_dev, sizeof(float) * nTrans, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  TRY(readback_reserve(ctx, 4 * sizeof(float) * B));
+  {
+    float* d = reinterpret_cast<float*>(ctx->readback);
+    float* n = d + B;
+    int32_t* st = reinterpret_cast<int32_t*>(n + B);
+    TRYCUDA(cudaMemcpyAsync(d, den, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(n, lat->out_scores, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(st, status, sizeof(int32_t) * 2 * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaStreamSynchronize(ctx->stream));
+    for (int b = 0; b < B; b++) a.losses_host[b] = d[b] - n[b];
+    for (int b = 0; b < 2 * B; b++) *needs_exact |= st[b] != 0;
+  }
+done:
+  ctx->stream = main_stream;
+  if (rc) cudaStreamSynchronize(ctx->copy_stream); // nothing may still run on the second stream when the buffers go
+  if (lat) gtnb_lattice_destroy(ctx, lat);
+  if (!a.emissions_on_device) dev_free(ctx, e_dev);
+  if (!(a.grads && a.grads_on_device)) dev_free(ctx, g_dev);
+  if (!a.trans_on_device) dev_free(ctx, w_dev);
+  if (!(a.trans_grad && a.trans_grad_on_device)) dev_free(ctx, tg_dev);
+  dev_free(ctx, small_dev);
+  dev_free(ctx, status);
+  dev_free(ctx, alpha);
+  dev_free(ctx, den);
+  dev_free(ctx, map);
+  dev_free(ctx, ggrad);
+  dev_free(ctx, minus1);
+  return rc;
+}
+
+/*
+ * Every other case -- C > 128, a non-finite weight or used emission, or the implicit path switched off -- through
+ * asg_loss_run with the same T_b (the implicit sweeps, else the materialised lattices).  Device-resident
+ * transitions and their gradient go through host copies on this route only.
+ */
+int asg_loss_ex_generic(gtnb_ctx* ctx, const AsgArgs& a, const std::vector<int32_t>& Tb) {
+  const long long nTrans = a.C + (long long)a.C * a.C;
+  std::vector<float> tw, tg;
+  const float* tw_host = a.trans_w;
+  if (a.trans_on_device) {
+    tw.resize(nTrans);
+    GTNB_CUDA(ctx, cudaMemcpy(tw.data(), a.trans_w, sizeof(float) * nTrans, cudaMemcpyDeviceToHost));
+    tw_host = tw.data();
+  }
+  float* tg_host = a.trans_grad;
+  if (a.trans_grad && a.trans_grad_on_device) {
+    tg.resize(nTrans);
+    tg_host = tg.data();
+  }
+  const int rc = asg_loss_run(ctx, a.B, a.T, a.C, a.emissions, a.emissions_on_device, Tb.data(), tw_host, a.targets,
+                              a.target_lens, a.losses_host, a.grads, a.grads_on_device, tg_host);
+  if (rc == GTNB_OK && a.trans_grad && a.trans_grad_on_device)
+    GTNB_CUDA(ctx, cudaMemcpy(a.trans_grad, tg.data(), sizeof(float) * nTrans, cudaMemcpyHostToDevice));
+  return rc;
+}
+
+#undef TRY
+#undef TRYCUDA
+
+int asg_loss_ex_run(gtnb_ctx* ctx, const AsgArgs& a) {
+  const int B = a.B, T = a.T, C = a.C;
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !a.emissions || !a.trans_w || !a.target_lens || !a.losses_host)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: bad arguments");
+  const long long nTrans = C + (long long)C * C;
+  std::vector<int32_t> Tb(B), off(B);
+  std::vector<SgDims> dims(B);
+  long long tot_t = 0;
+  for (int b = 0; b < B; b++) {
+    const int U = a.target_lens[b];
+    if (U < 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: negative target length");
+    if (U > 0 && !a.targets) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: targets is NULL");
+    const int32_t* y = a.targets + tot_t;
+    for (int u = 0; u < U; u++)
+      if (y[u] < 0 || y[u] >= C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: label outside [0, C)");
+    off[b] = (int32_t)tot_t;
+    tot_t += U;
+    Tb[b] = a.input_lens ? a.input_lens[b] : T;
+    if (Tb[b] < 0 || Tb[b] > T)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: input_lens outside [0, T]");
+    // compose(fal_b, transitions): U+1 nodes, 2U arcs (none when U = 0), node U accepts
+    dims[b] = SgDims{U + 1, 2 * U, U > 0 ? 1 : 0, /*all_valid=*/1, /*uniform=*/1, /*max_in=*/2, /*max_out=*/2};
+  }
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (B == 0) { // an empty batch: the transition gradient is 0
+    if (a.trans_grad) {
+      if (a.trans_grad_on_device) {
+        GTNB_CUDA(ctx, cudaMemsetAsync(a.trans_grad, 0, sizeof(float) * nTrans, ctx->stream));
+        GTNB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      } else {
+        std::memset(a.trans_grad, 0, sizeof(float) * nTrans);
+      }
+    }
+    return GTNB_OK;
+  }
+  bool needs_exact = false;
+  const bool fast = C <= kNgramMaxLabels && ctx->use_implicit && implicit_dims_supported(dims.data(), B);
+  int rc = fast ? asg_loss_ex_fast(ctx, a, Tb, dims, off, &needs_exact) : asg_loss_ex_generic(ctx, a, Tb);
+  if (rc == GTNB_OK && needs_exact) {
+    // a non-finite weight: asg_loss_run's sweeps raise the same status bit and end in the materialised lattices,
+    // which reproduce the reference's inf / NaN propagation
+    arena_end(ctx);
+    arena_begin(ctx);
+    rc = asg_loss_ex_generic(ctx, a, Tb);
+  }
+  // T_b = 0: linearGraph(0, C) is one start node that does not accept (creations.cpp:20-33), so both
+  // compositions are empty and the reference's loss is -inf - -inf = NaN (no gradient)
+  for (int b = 0; b < B && rc == GTNB_OK; b++)
+    if (Tb[b] == 0) a.losses_host[b] = std::numeric_limits<float>::quiet_NaN();
+  return rc;
+}
+
+} // namespace
+
+extern "C" int gtnb_asg_loss_ex(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const float* trans_w, int trans_on_device, const int32_t* targets, const int32_t* target_lens,
+    float* losses_host, float* grads, int grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const AsgArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, targets,
+                  target_lens, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+  if (ctx) arena_begin(ctx);
+  const int rc = asg_loss_ex_run(ctx, a);
   if (ctx) arena_end(ctx);
   return rc;
 }

@@ -349,6 +349,19 @@ int launch_ngram_den_backward(
     gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
     const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad);
 int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, float* wgrad);
+// the same trellis in ASG's start mode (trans_w, trans_grad: [C + C*C], start weights first) and ASG's
+// forced-alignment numerator graphs built on the device
+long long asg_alpha_floats(int B, int T, int C); // floats of the alpha buffer of launch_asg_den_*
+int launch_asg_den_forward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* trans_w, float* alpha, float* den, int32_t* status);
+int launch_asg_den_backward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* trans_w, const float* alpha, const float* den, float* grad, long long grad_stride,
+    float* trans_grad);
+int launch_asg_num_build(
+    gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
+    const int32_t* tgt_len_dev, const float* trans_w, int32_t* map);
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);

@@ -26,6 +26,11 @@
  *
  * Valid only for finite weights: the denominator's forward kernel raises a status bit on any non-finite W
  * entry or used emission, and the caller repeats the call through the materialised lattices.
+ *
+ * ASG (gtnb_asg_loss_ex) runs the same trellis in its START mode: the first frame starts from ASG's start weights,
+ * alpha_1 = e[0] + s, and the rows are kept relative to per-frame offsets accumulated in double (see the forward
+ * kernel).  Its numerator, compose(fal_b, transitions), is a U+1-node chain that asg_num_build_kernel writes into the
+ * same small-graph tables for k_implicit.cu's sweeps; it needs no fold.
  */
 #ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
@@ -56,6 +61,14 @@ inline void ngram_den_shape(int C, int* K, int* lanes, int* threads) {
   while (l * *K < C) l *= 2;
   *lanes = l;
   *threads = (C * l + 31) & ~31;
+}
+
+/*
+ * The start mode's alpha buffer (asg_den_* launchers): the alpha rows [B][(T+1)*C], then, 8-byte aligned, the
+ * per-frame offsets [B][T+1] as doubles (slot 0: Z).
+ */
+long long asg_alpha_floats(int B, int T, int C) {
+  return ((long long)B * (T + 1) * C + 1) / 2 * 2 + 2ll * B * (T + 1);
 }
 
 namespace {
@@ -94,8 +107,20 @@ __device__ __forceinline__ void ng_merge(float& m, float& s, int lanes) {
   }
 }
 
-/* alpha rows of every utterance to alpha[b][(T+1)*C], Z to den[b]; status[b] |= 1 on a non-finite weight */
-template <int K>
+__device__ __forceinline__ double* asg_offsets(float* alpha, int B, int T, int C, int b) {
+  return reinterpret_cast<double*>(alpha + ((long long)B * (T + 1) * C + 1) / 2 * 2) + (long long)b * (T + 1);
+}
+
+/*
+ * alpha rows of every utterance to alpha[b][(T+1)*C], Z to den[b]; status[b] |= 1 on a non-finite weight.
+ * START (ASG's denominator, forwardScore(compose(E, transitions))): W is ASG's [C + C*C] -- the start weights s,
+ * then the C x C matrix -- and the first frame starts from them, alpha_1[i] = e[0][i] + s[i]; the recursion
+ * through the matrix begins at t = 2.  Without START, alpha_0 = 0 and W is the C x C matrix alone.
+ * START also keeps every row relative to an offset, alpha_t = row_t + c_t with c_t = c_{t-1} + row_{t-1}[0]
+ * accumulated in double (asg_offsets; c_1 = 0): the stored rows stay within a frame's spread of scores, so the
+ * backward kernel's posteriors exp(alpha + beta - Z) do not cancel fp32 scores that grow with t.
+ */
+template <int K, bool START = false>
 __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
     int T, int C, int lanes, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
     const float* __restrict__ W, float* __restrict__ alpha, float* __restrict__ den, int32_t* __restrict__ status) {
@@ -106,21 +131,41 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   const bool row = i < C;
   const bool lead = row && q == 0;
   const float* em = emis + (long long)b * stride;
+  const float* Wm = START ? W + C : W;
   float* al = alpha + (long long)b * (T + 1) * C;
+  double* cs = START ? asg_offsets(alpha, gridDim.x, T, C, b) : nullptr;
+  double c = 0.0; // START: the offset of the row in A[(t - 1) & 1]
   bool bad = false;
   float w[K]; // W[i][q + lanes * k]: interleaved columns, so the lanes of a row read distinct banks
 #pragma unroll
   for (int k = 0; k < K; k++) {
     const int j = q + lanes * k;
     const bool on = row && j < C;
-    w[k] = on ? __ldg(W + i * C + j) : ng_ninf();
+    w[k] = on ? __ldg(Wm + i * C + j) : ng_ninf();
     if (on) bad |= !ng_finite(w[k]);
+  }
+  float s_i = 0.0f;
+  if (START && lead) {
+    s_i = __ldg(W + i);
+    bad |= !ng_finite(s_i);
   }
   for (int j = tid; j < kNgramMaxC; j += blockDim.x) A[0][j] = A[1][j] = 0.0f; // alpha_0 = 0; padding stays 0
   for (int j = tid; j < C; j += blockDim.x) al[j] = 0.0f;
   __syncthreads();
   float e_nx = (lead && Tb > 0) ? __ldg(em + i) : 0.0f;
-  for (int t = 1; t <= Tb; t++) {
+  if (START && Tb > 0) { // alpha_1 = e[0] + s
+    const float e = e_nx;
+    if (lead && Tb > 1) e_nx = __ldg(em + C + i);
+    bad |= !ng_finite(e);
+    if (lead) {
+      const float v = e + s_i;
+      A[1][i] = v;
+      al[C + i] = v;
+    }
+    if (tid == 0) cs[1] = 0.0;
+    __syncthreads();
+  }
+  for (int t = START ? 2 : 1; t <= Tb; t++) {
     const float e = e_nx;
     if (lead && t < Tb) e_nx = __ldg(em + (long long)t * C + i);
     bad |= !ng_finite(e);
@@ -138,9 +183,14 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
     for (int k = 0; k < K; k++) s += ng_exp(x[k] - mm);
     ng_merge(m, s, lanes);
     if (lead) {
-      const float v = e + (m + ng_log(s));
+      float v = e + (m + ng_log(s));
+      if (START) v -= P[0];
       A[t & 1][i] = v;
       al[(long long)t * C + i] = v;
+    }
+    if (START) {
+      c += (double)P[0];
+      if (tid == 0) cs[t] = c;
     }
     __syncthreads();
   }
@@ -154,14 +204,26 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
     for (int j = tid; j < C; j += 32) s += expf(F[j] - m);
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (tid == 0) {
-      den[b] = m + logf(s);
+      if (START) {
+        const double Z = c + (double)(m + logf(s));
+        cs[0] = Z;
+        den[b] = (float)Z;
+      } else {
+        den[b] = m + logf(s);
+      }
       if (bad) atomicOr(&status[b], 1);
     }
   }
 }
 
-/* d Z / d e added into grad (rows t < T_b), d Z / d W added into wgrad[C*C] (one atomic per entry per CTA) */
-template <int K>
+/*
+ * d Z / d e added into grad (rows t < T_b), d Z / d W added into wgrad[C*C] (one atomic per entry per CTA).
+ * START: W and wgrad are ASG's [C + C*C]; the pair posteriors on the matrix run over t >= 2 only, and the
+ * frame-1 node posteriors exp(alpha_1[i] + beta_1[i] - Z) are the start weights' gradient.  As in the forward
+ * kernel, beta_t = row_t + d_t with d_{t-1} = d_t + G[0] in double (d_T = 0), and a posterior's exponent is
+ * row + row' + (float)(c + d - Z).
+ */
+template <int K, bool START = false>
 __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
     int T, int C, int lanes, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
     const float* __restrict__ W, const float* __restrict__ alpha, const float* __restrict__ den,
@@ -178,11 +240,15 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
   const float* em = emis + (long long)b * stride;
   const float* al = alpha + (long long)b * (T + 1) * C;
   float* gr = grad + (long long)b * grad_stride;
+  const float* Wm = START ? W + C : W;
+  const double* cs = START ? asg_offsets(const_cast<float*>(alpha), gridDim.x, T, C, b) : nullptr;
+  const double Zd = START ? cs[0] : 0.0;
+  double d = 0.0, c_t = START ? cs[Tb] : 0.0, c_nx = (START && Tb > 1) ? cs[Tb - 1] : 0.0;
   float w[K], acc[K]; // W[q + lanes * k][j] and its pair posteriors
 #pragma unroll
   for (int k = 0; k < K; k++) {
     const int i = q + lanes * k;
-    w[k] = (col && i < C) ? __ldg(W + i * C + j) : ng_ninf();
+    w[k] = (col && i < C) ? __ldg(Wm + i * C + j) : ng_ninf();
     acc[k] = 0.0f;
   }
   for (int i = tid; i < kNgramMaxC; i += blockDim.x) {
@@ -197,18 +263,23 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
   __syncthreads();
   for (int t = Tb; t >= 1; t--) {
     const float a_t = a_nx, e_t = e_nx, aj = aj_nx;
+    const double c_prev = c_nx; // START: c_{t-1}
     if (t > 1) {
       if (rowt) {
         a_nx = al[(long long)(t - 1) * C + tid];
         e_nx = __ldg(em + (long long)(t - 2) * C + tid);
       }
       if (col) aj_nx = al[(long long)(t - 2) * C + j];
+      if (START && t > 2) c_nx = cs[t - 2];
     }
     if (rowt) {
       const float bt = Bt[t & 1][tid];
       G[tid] = e_t + bt;
-      atomicAdd(gr + (long long)(t - 1) * C + tid, ng_exp(a_t + bt - Z)); // node posterior
+      const float p = ng_exp(START ? (a_t + bt) + (float)(c_t + d - Zd) : a_t + bt - Z); // node posterior
+      atomicAdd(gr + (long long)(t - 1) * C + tid, p);
+      if (START && t == 1) atomicAdd(wgrad + tid, p); // d Z / d s
     }
+    if (START && t == 1) break; // (uniform) frame 1 has no transition through the matrix
     __syncthreads();
     float x[K];
     float m = ng_ninf();
@@ -219,7 +290,7 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
     }
     const float mm = m == ng_ninf() ? 0.0f : m;
     float s = 0.0f;
-    const float f = ng_exp((mm + aj) - Z); // pair posterior = exp(x - mm) * f
+    const float f = ng_exp(START ? (mm + aj) + (float)(c_prev + d - Zd) : (mm + aj) - Z); // pair = exp(x - mm) * f
 #pragma unroll
     for (int k = 0; k < K; k++) {
       const float p = ng_exp(x[k] - mm);
@@ -227,13 +298,20 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
       acc[k] = fmaf(p, f, acc[k]);
     }
     ng_merge(m, s, lanes);
-    if (lead) Bt[(t - 1) & 1][j] = m + ng_log(s);
+    if (START) {
+      const float g0 = G[0];
+      if (lead) Bt[(t - 1) & 1][j] = (m + ng_log(s)) - g0;
+      d += (double)g0;
+      c_t = c_prev;
+    } else if (lead) {
+      Bt[(t - 1) & 1][j] = m + ng_log(s);
+    }
     __syncthreads();
   }
 #pragma unroll
   for (int k = 0; k < K; k++) {
     const int i = q + lanes * k;
-    if (col && i < C && acc[k] != 0.0f) atomicAdd(wgrad + i * C + j, acc[k]);
+    if (col && i < C && acc[k] != 0.0f) atomicAdd(wgrad + (START ? C : 0) + i * C + j, acc[k]);
   }
 }
 
@@ -350,6 +428,56 @@ __global__ void __launch_bounds__(256) ngram_num_build_kernel(
   }
 }
 
+/*
+ * compose(fal_b, transitions) of ASG's numerator (test/criterion_test.cpp:244-305) in the small-graph tables:
+ * U+1 nodes, node l = "l labels consumed", start 0, accept U (none when U = 0).  Arcs in the reference's creation
+ * order: 0 -> 1 (weight s[y0]), then per node l >= 1 a self loop (W[y_{l-1}][y_{l-1}]) and the step l -> l+1
+ * (W[y_l][y_{l-1}]).  So node n >= 1 has exactly two in-arcs, both labelled y_{n-1}: arc 2n-2 from n-1, arc
+ * 2n-1 its self loop; the in-entry index is the arc id, and map[grad_graph_off + arc] its index in trans_w.
+ */
+__global__ void __launch_bounds__(256) asg_num_build_kernel(
+    const GraphMeta* __restrict__ meta, const int32_t* __restrict__ targets, const int32_t* __restrict__ tgt_off,
+    const int32_t* __restrict__ tgt_len, int C, const float* __restrict__ trans_w, uint8_t* __restrict__ sg_flags,
+    int32_t* __restrict__ sg_in_ptr, int32_t* __restrict__ sg_in_src, int32_t* __restrict__ sg_in_label,
+    int32_t* __restrict__ sg_in_arc, float* __restrict__ sg_in_w, int32_t* __restrict__ sg_ilabel,
+    int32_t* __restrict__ sg_olabel, int32_t* __restrict__ acc_nodes, int32_t* __restrict__ map) {
+  const int b = blockIdx.x;
+  const GraphMeta m = meta[b];
+  const int U = tgt_len[b], N = U + 1;
+  const int32_t* y = targets + tgt_off[b];
+  uint8_t* fl = sg_flags + m.sg_node_base;
+  int32_t* ip = sg_in_ptr + m.sg_node_base;
+  int32_t* is = sg_in_src + m.sg_arc_base;
+  int32_t* il = sg_in_label + m.sg_arc_base;
+  int32_t* ia = sg_in_arc + m.sg_arc_base;
+  float* iw = sg_in_w + m.sg_arc_base;
+  int32_t* lab_i = sg_ilabel + m.sg_arc_base;
+  int32_t* lab_o = sg_olabel + m.sg_arc_base;
+  int32_t* mp = map + m.grad_graph_off;
+  for (int n = threadIdx.x; n <= N; n += blockDim.x) {
+    if (n == N) {
+      ip[N] = 2 * U;
+      continue;
+    }
+    fl[n] = (uint8_t)((n == 0 ? 1 : 0) | (U > 0 && n == U ? 2 : 0));
+    ip[n] = n == 0 ? 0 : 2 * (n - 1);
+    if (n == 0) continue;
+    const int label = y[n - 1], e = 2 * (n - 1);
+    const int widx[2] = {n == 1 ? label : C + label * C + y[n - 2], C + label * C + label};
+#pragma unroll
+    for (int k = 0; k < 2; k++) {
+      is[e + k] = n - 1 + k;
+      ia[e + k] = e + k;
+      il[e + k] = label;
+      iw[e + k] = __ldg(trans_w + widx[k]);
+      lab_i[e + k] = label;
+      lab_o[e + k] = label;
+      mp[e + k] = widx[k];
+    }
+  }
+  if (threadIdx.x == 0 && U > 0) acc_nodes[m.acc_base] = U;
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
@@ -370,33 +498,76 @@ int launch_ngram_num_build(
   return GTNB_OK;
 }
 
-int launch_ngram_den_forward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* W, float* alpha, float* den, int32_t* status) {
+namespace {
+
+template <bool START>
+int den_forward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int32_t* lens_dev, const float* emis,
+                long long stride, const float* W, float* alpha, float* den, int32_t* status) {
   if (B == 0) return GTNB_OK;
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
   if (K == 16)
-    GTNB_LAUNCH(ctx, "ngram_den_forward", ngram_den_forward_kernel<16><<<B, threads, 0, ctx->stream>>>(
+    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<16, START><<<B, threads, 0, ctx->stream>>>(
         T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
   else
-    GTNB_LAUNCH(ctx, "ngram_den_forward", ngram_den_forward_kernel<32><<<B, threads, 0, ctx->stream>>>(
+    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<32, START><<<B, threads, 0, ctx->stream>>>(
         T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
   return GTNB_OK;
+}
+
+template <bool START>
+int den_backward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int32_t* lens_dev, const float* emis,
+                 long long stride, const float* W, const float* alpha, const float* den, float* grad,
+                 long long grad_stride, float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  int K, lanes, threads;
+  ngram_den_shape(C, &K, &lanes, &threads);
+  if (K == 16)
+    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<16, START><<<B, threads, 0, ctx->stream>>>(
+        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
+  else
+    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<32, START><<<B, threads, 0, ctx->stream>>>(
+        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
+  return GTNB_OK;
+}
+
+} // namespace
+
+int launch_ngram_den_forward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* W, float* alpha, float* den, int32_t* status) {
+  return den_forward<false>(ctx, "ngram_den_forward", B, T, C, lens_dev, emis, stride, W, alpha, den, status);
 }
 
 int launch_ngram_den_backward(
     gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
     const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad) {
-  if (B == 0) return GTNB_OK;
-  int K, lanes, threads;
-  ngram_den_shape(C, &K, &lanes, &threads);
-  if (K == 16)
-    GTNB_LAUNCH(ctx, "ngram_den_backward", ngram_den_backward_kernel<16><<<B, threads, 0, ctx->stream>>>(
-        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
-  else
-    GTNB_LAUNCH(ctx, "ngram_den_backward", ngram_den_backward_kernel<32><<<B, threads, 0, ctx->stream>>>(
-        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
+  return den_backward<false>(ctx, "ngram_den_backward", B, T, C, lens_dev, emis, stride, W, alpha, den, grad,
+                             grad_stride, wgrad);
+}
+
+int launch_asg_den_forward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* trans_w, float* alpha, float* den, int32_t* status) {
+  return den_forward<true>(ctx, "asg_den_forward", B, T, C, lens_dev, emis, stride, trans_w, alpha, den, status);
+}
+
+int launch_asg_den_backward(
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    const float* trans_w, const float* alpha, const float* den, float* grad, long long grad_stride,
+    float* trans_grad) {
+  return den_backward<true>(ctx, "asg_den_backward", B, T, C, lens_dev, emis, stride, trans_w, alpha, den, grad,
+                            grad_stride, trans_grad);
+}
+
+int launch_asg_num_build(
+    gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
+    const int32_t* tgt_len_dev, const float* trans_w, int32_t* map) {
+  if (lat->B == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "asg_num_build", asg_num_build_kernel<<<lat->B, 256, 0, ctx->stream>>>(
+      lat->meta, targets_dev, tgt_off_dev, tgt_len_dev, lat->C, trans_w, lat->sg_flags, lat->sg_in_ptr,
+      lat->sg_in_src, lat->sg_in_label, lat->sg_in_arc, lat->sg_in_w, lat->sg_ilabel, lat->sg_olabel,
+      lat->acc_nodes, map));
   return GTNB_OK;
 }
 

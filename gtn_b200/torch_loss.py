@@ -15,6 +15,16 @@ from . import capi
 _ctx_cache = {}
 
 
+def _lengths(input_lengths, B):
+    """None, or input_lengths (a list or an int tensor on any device) as a contiguous int32 [B] host array"""
+    if input_lengths is None:
+        return None
+    il = np.ascontiguousarray(
+        input_lengths.detach().cpu().numpy() if torch.is_tensor(input_lengths) else input_lengths, np.int32)
+    assert il.shape == (B,)
+    return il
+
+
 def _ctx_for(device, stream):
     key = (device.index, stream)
     if key not in _ctx_cache:
@@ -26,11 +36,13 @@ class CTCLossFunction(torch.autograd.Function):
     """loss_b = forwardScore(e_b) - forwardScore(intersect(ctcGraph(target_b), e_b))  (benchmarks/ctc.cpp:150-158).
 
     emissions: float32 CUDA tensor [B, T, C] (unnormalised scores are fine: the normaliser is part of the loss);
-    targets: list of 1-D int sequences; returns the mean loss over the batch (reduction="mean") or the [B] vector.
+    targets: list of 1-D int sequences; input_lengths: None (T frames each), a list or an int tensor (any device):
+    e_b is then the first input_lengths[b] frames, and the gradient of the padding frames is 0.  Returns the mean
+    loss over the batch (reduction="mean") or the [B] vector.
     """
 
     @staticmethod
-    def forward(ctx, emissions, targets, blank=0, reduction="mean"):
+    def forward(ctx, emissions, targets, blank=0, reduction="mean", input_lengths=None):
         assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
         e = emissions.contiguous()
         B, T, Cn = e.shape
@@ -39,10 +51,12 @@ class CTCLossFunction(torch.autograd.Function):
         lens = np.asarray([len(t) for t in targets], np.int32)
         cat = np.ascontiguousarray(
             np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
+        il = _lengths(input_lengths, B)
         losses = np.zeros(B, np.float32)
-        grad = torch.empty_like(e)
+        grad = torch.empty_like(e)  # (with input_lengths the call zeroes the padding rows)
         g._check(capi.lib().gtnb_ctc_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, None, cat.ctypes.data_as(capi._i32p),
+            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p),
+            cat.ctypes.data_as(capi._i32p),
             lens.ctypes.data_as(capi._i32p), int(blank), losses.ctypes.data_as(capi._f32p),
             grad.data_ptr(), 1))
         out = torch.from_numpy(losses).to(e.device)
@@ -56,12 +70,12 @@ class CTCLossFunction(torch.autograd.Function):
         (grad,) = ctx.saved_tensors
         if ctx.reduction == "mean":
             scale = grad_output / ctx.B
-            return grad * scale, None, None, None
-        return grad * grad_output.view(-1, 1, 1), None, None, None
+            return grad * scale, None, None, None, None
+        return grad * grad_output.view(-1, 1, 1), None, None, None, None
 
 
-def ctc_loss(emissions, targets, blank=0, reduction="mean"):
-    return CTCLossFunction.apply(emissions, targets, blank, reduction)
+def ctc_loss(emissions, targets, blank=0, reduction="mean", input_lengths=None):
+    return CTCLossFunction.apply(emissions, targets, blank, reduction, input_lengths)
 
 
 class ASGLossFunction(torch.autograd.Function):
@@ -72,28 +86,45 @@ class ASGLossFunction(torch.autograd.Function):
 
     emissions: float32 CUDA tensor [B, T, C]; transitions: float32 tensor [C + C*C] (start weights, then the
     C x C matrix, row = destination label) on any device; targets: list of 1-D int sequences.
+
+    input_lengths: None (T frames each), a list or an int tensor (any device).  When given, e_b is the first
+    input_lengths[b] frames (the gradient of the padding frames is 0) and the call goes through gtnb_asg_loss_ex
+    on device pointers: transitions must then be a float32 CUDA tensor on the emissions' device, and the
+    transition gradient stays on the device.
     """
 
     @staticmethod
-    def forward(ctx, emissions, transitions, targets, reduction="mean", allreduce=True):
+    def forward(ctx, emissions, transitions, targets, reduction="mean", allreduce=True, input_lengths=None):
         assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
         e = emissions.contiguous()
         B, T, Cn = e.shape
         assert transitions.numel() == Cn + Cn * Cn
         stream = torch.cuda.current_stream(e.device).cuda_stream
         g = _ctx_for(e.device, stream)
-        tw = np.ascontiguousarray(transitions.detach().to("cpu", torch.float32).numpy())
         lens = np.asarray([len(t) for t in targets], np.int32)
         cat = np.ascontiguousarray(
             np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
         losses = np.zeros(B, np.float32)
-        tgrad = np.zeros(Cn + Cn * Cn, np.float32)
-        grad = torch.empty_like(e)
-        g._check(capi.lib().gtnb_asg_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, tw.ctypes.data_as(capi._f32p), cat.ctypes.data_as(capi._i32p),
-            lens.ctypes.data_as(capi._i32p), losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
-            tgrad.ctypes.data_as(capi._f32p)))
-        tg = torch.from_numpy(tgrad).to(e.device)
+        if input_lengths is not None:
+            assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+            il = _lengths(input_lengths, B)
+            w = transitions.detach().contiguous()
+            grad = torch.empty_like(e)  # every row is written by the call
+            tg = torch.empty(Cn + Cn * Cn, dtype=torch.float32, device=e.device)
+            g._check(capi.lib().gtnb_asg_loss_ex(
+                g.h, B, T, Cn, e.data_ptr(), 1, il.ctypes.data_as(capi._i32p), w.data_ptr(), 1,
+                cat.ctypes.data_as(capi._i32p), lens.ctypes.data_as(capi._i32p), losses.ctypes.data_as(capi._f32p),
+                grad.data_ptr(), 1, tg.data_ptr(), 1))
+            tg = tg.view_as(transitions)
+        else:
+            tw = np.ascontiguousarray(transitions.detach().to("cpu", torch.float32).numpy())
+            tgrad = np.zeros(Cn + Cn * Cn, np.float32)
+            grad = torch.empty_like(e)
+            g._check(capi.lib().gtnb_asg_loss(
+                g.h, B, T, Cn, e.data_ptr(), 1, tw.ctypes.data_as(capi._f32p), cat.ctypes.data_as(capi._i32p),
+                lens.ctypes.data_as(capi._i32p), losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
+                tgrad.ctypes.data_as(capi._f32p)))
+            tg = torch.from_numpy(tgrad).to(e.device)
         ctx.world = 1
         if allreduce and torch.distributed.is_available() and torch.distributed.is_initialized():
             torch.distributed.all_reduce(tg, op=torch.distributed.ReduceOp.SUM)
@@ -111,16 +142,16 @@ class ASGLossFunction(torch.autograd.Function):
         if ctx.reduction == "mean":
             # the mean over the GLOBAL batch when the transition gradient was summed over the ranks
             scale = grad_output / ctx.B
-            return grad * scale, (tg * (scale / ctx.world)).to(ctx.tdev), None, None, None
+            return grad * scale, (tg * (scale / ctx.world)).to(ctx.tdev), None, None, None, None
         # reduction "none": the incoming gradient is per utterance; the transition gradient was already summed
         # over the batch inside the kernel, which is only the chain rule's answer for a uniform grad_output
         assert bool((grad_output == grad_output.flatten()[0]).all()), \
             "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
-        return grad * grad_output.view(-1, 1, 1), (tg * grad_output.flatten()[0]).to(ctx.tdev), None, None, None
+        return grad * grad_output.view(-1, 1, 1), (tg * grad_output.flatten()[0]).to(ctx.tdev), None, None, None, None
 
 
-def asg_loss(emissions, transitions, targets, reduction="mean", allreduce=True):
-    return ASGLossFunction.apply(emissions, transitions, targets, reduction, allreduce)
+def asg_loss(emissions, transitions, targets, reduction="mean", allreduce=True, input_lengths=None):
+    return ASGLossFunction.apply(emissions, transitions, targets, reduction, allreduce, input_lengths)
 
 
 class NgramCTCLossFunction(torch.autograd.Function):

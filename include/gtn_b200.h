@@ -366,6 +366,38 @@ int gtnb_asg_loss(
     float* trans_grad_host);
 
 /*
+ * ASG on a padded minibatch with the transitions anywhere (the loss of gtnb_asg_loss):
+ *   loss_b = forwardScore(compose(E_b, transitions)) - forwardScore(compose(compose(fal_b, transitions), E_b))
+ * E_b: linearGraph(T_b, C) on the first T_b = input_lens[b] (or T) rows of emissions_b.
+ * trans_w [C + C*C] in gtnb_asg_loss's layout (the C start weights, then the C x C matrix, row = destination
+ * label) and trans_grad (nullable, [C + C*C]: the batch sum of d loss_b / d trans_w) live on the device when
+ * *_on_device, else on the host; likewise emissions and grads (nullable, [B][T][C]: d loss_b / d e_b).  EVERY
+ * row of grads is written: rows t >= T_b are set to 0.  T_b = 0 gives NaN (linearGraph(0, C) accepts nothing);
+ * an infeasible target (T_b < U) or U = 0 gives +inf and the denominator's gradient alone.  B = 0 zeroes
+ * trans_grad.  Labels outside [0, C), negative lengths or T_b > T are GTNB_ERR_INVALID_ARGUMENT.
+ * For C <= 128 the transitions never leave the device: the denominator is a dense on-chip trellis and the
+ * numerator graphs are built on the device.  Larger alphabets and non-finite weights take the route of
+ * gtnb_asg_loss (with T_b), which reads the transitions on the host.
+ */
+int gtnb_asg_loss_ex(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* nullable */
+    const float* trans_w,
+    int trans_on_device,
+    const int32_t* targets,
+    const int32_t* target_lens,
+    float* losses_host,
+    float* grads, /* nullable */
+    int grads_on_device,
+    float* trans_grad, /* nullable */
+    int trans_grad_on_device);
+
+/*
  * CTC with a learned bigram transition graph for a whole minibatch (benchmarks/ctc.cpp:107-134, timeNgramCtc):
  *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(ctc_b, G), E_b))
  * E_b: linearGraph(T_b, C) on the first T_b = input_lens[b] (or T) rows of emissions_b; ctc_b: the CTC graph of

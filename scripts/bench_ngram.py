@@ -1,8 +1,11 @@
 """CTC with a learned bigram transition graph (gtnb_ngram_ctc_loss, benchmarks/ctc.cpp:107-134) at BASELINE.json
-configs[2]'s shape, B=128 T=500 C=64 U=50, next to the ASG criterion (gtnb_asg_loss) at the same shape, on the
-same emissions and the same C x C transition matrix, in one run.  One JSON record on stdout, nothing written:
+configs[2]'s shape, B=128 T=500 C=64 U=50, next to the ASG criterion (gtnb_asg_loss, and gtnb_asg_loss_ex with the
+transitions on the device) at the same shape, on the same emissions and the same C x C transition matrix, in one
+run.  One JSON record on stdout, nothing written:
 
   ngram.value / asg.value   device-resident buffers, utterances / s (CUDA events, L2 flushed between steps)
+  asg_ex.full / .ragged     gtnb_asg_loss_ex, every buffer on the device, with input_lens = T and with input_lens
+                            drawn uniformly from [U, T] (seed 5)
   ngram.e2e                 every buffer on the host (pinned emissions and gradients)
   *.kernels_ms_per_step     per-kernel CUDA-event times
   ngram.trellis             the dense-trellis kernels against the bound they hit: 2 B T C^2 MUFU ex2 per step
@@ -58,6 +61,9 @@ def main():
     i32p, f32p = capi._i32p, capi._f32p
     e_dev, g_dev = ctx.to_device(e), ctx.alloc(e.nbytes)
     w_dev, wg_dev = ctx.to_device(W), ctx.alloc(W.nbytes)
+    tw_dev, twg_dev = ctx.to_device(tw), ctx.alloc(tw.nbytes)
+    full_lens = np.full(B, T, np.int32)
+    ragged_lens = np.random.default_rng(5).integers(U, T + 1, B).astype(np.int32)
     hp_e, hp_g = Ct.c_void_p(), Ct.c_void_p()
     ctx._check(L.gtnb_host_alloc(ctx.h, e.nbytes, Ct.byref(hp_e)))
     ctx._check(L.gtnb_host_alloc(ctx.h, e.nbytes, Ct.byref(hp_g)))
@@ -77,6 +83,12 @@ def main():
         ctx._check(L.gtnb_asg_loss(ctx.h, B, T, C, e_dev.ptr, 1, tw.ctypes.data_as(f32p), cat.ctypes.data_as(i32p),
                                    lens.ctypes.data_as(i32p), losses.ctypes.data_as(f32p), g_dev.ptr, 1,
                                    tgrad.ctypes.data_as(f32p)))
+
+    def asg_ex(in_lens):
+        # the transitions and their gradient in HBM (the torch path with input_lengths)
+        ctx._check(L.gtnb_asg_loss_ex(ctx.h, B, T, C, e_dev.ptr, 1, in_lens.ctypes.data_as(i32p), tw_dev.ptr, 1,
+                                      cat.ctypes.data_as(i32p), lens.ctypes.data_as(i32p), losses.ctypes.data_as(f32p),
+                                      g_dev.ptr, 1, twg_dev.ptr, 1))
 
     def region(step, profile):
         for _ in range(args.warmup):
@@ -102,6 +114,10 @@ def main():
     gpu_losses, gpu_grads = losses.copy(), g_dev.download((B, T, C))
     ems, _, _ = region(lambda: ngram(False), False)
     ams, amed, akern = region(asg, True)
+    asg_losses = losses.copy()
+    xms, xmed, xkern = region(lambda: asg_ex(full_lens), True)
+    ex_losses = losses.copy()
+    rms, rmed, rkern = region(lambda: asg_ex(ragged_lens), True)
 
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
                         "-i", "0"], capture_output=True, text=True).stdout.strip()
@@ -124,7 +140,15 @@ def main():
         "asg": {"value": B / (ams * 1e-3), "unit": "utt/s", "ms_per_step": ams, "ms_per_step_median": amed,
                 "kernels_ms_per_step": akern,
                 "note": "implicit_* are k_implicit.cu's wide-path kernels on the dense C x C denominator plus the "
-                        "forced-alignment numerator's sweeps"}}
+                        "forced-alignment numerator's sweeps"},
+        "asg_ex": {"full": {"value": B / (xms * 1e-3), "unit": "utt/s", "ms_per_step": xms, "ms_per_step_median": xmed,
+                            "kernels_ms_per_step": xkern, "input_lens": "T for every utterance",
+                            "max_rel_loss_vs_asg": float(np.max(np.abs(ex_losses - asg_losses) / np.abs(asg_losses)))},
+                   "ragged": {"value": B / (rms * 1e-3), "unit": "utt/s", "ms_per_step": rms,
+                              "ms_per_step_median": rmed, "kernels_ms_per_step": rkern,
+                              "input_lens": "uniform in [U, T], seed 5, mean %.1f" % float(ragged_lens.mean())},
+                   "note": "asg_den_* are k_ngram.cu's trellis kernels in start mode, implicit_* the numerator's "
+                           "sweeps on the second stream"}}
     from oracle import pyoracle as po
     if args.cpu_sample > 0 and po.have_ref():
         from tests import ngram_oracle as no
@@ -137,7 +161,7 @@ def main():
         out["ngram"]["cpu_baseline"] = {"value": n / sec, "unit": "utt/s", "seconds": sec,
                                         "kind": "reference, %d utterances one after the other on one thread" % n}
     print(json.dumps(out))
-    for buf in (e_dev, g_dev, w_dev, wg_dev):
+    for buf in (e_dev, g_dev, w_dev, wg_dev, tw_dev, twg_dev):
         buf.free()
     ctx._check(L.gtnb_host_free(ctx.h, hp_e.value))
     ctx._check(L.gtnb_host_free(ctx.h, hp_g.value))
