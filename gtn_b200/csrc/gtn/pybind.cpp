@@ -295,6 +295,12 @@ PYBIND11_MODULE(_gtn, m) {
     d["out_arcs"] = arr(vs.outArcs);
     d["start"] = arr(vs.start);
     d["accept"] = arr(vs.accept);
+    d["flags"] = py::array_t<uint8_t>((py::ssize_t)vs.flags.size(), vs.flags.data());
+    d["src"] = arr(vs.src);
+    d["dst"] = arr(vs.dst);
+    d["ilabel"] = arr(vs.il);
+    d["olabel"] = arr(vs.ol);
+    d["weights"] = py::array_t<float>((py::ssize_t)vs.w.size(), vs.w.data());
     return d;
   }, "g"_a);
   m.def("device_launch_count", []() {

@@ -370,7 +370,9 @@ struct Adj {
   std::vector<int32_t> in_ptr, in_arcs, out_ptr, out_arcs, start, accept;
 };
 
-int validate_view(gtnb_ctx* ctx, const gtnb_graph_view& v) {
+} // namespace
+
+int gtnb::validate_view(gtnb_ctx* ctx, const gtnb_graph_view& v) {
   if (v.num_nodes < 0 || v.num_arcs < 0)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "graph view: negative size");
   if (v.num_nodes > 0 && !v.node_flags)
@@ -384,6 +386,8 @@ int validate_view(gtnb_ctx* ctx, const gtnb_graph_view& v) {
   }
   return GTNB_OK;
 }
+
+namespace {
 
 void build_adj(const gtnb_graph_view& v, Adj& adj) {
   int N = v.num_nodes, A = v.num_arcs;
@@ -632,13 +636,16 @@ int composed_alloc(
     std::vector<long long>& sga, gtnb_lattice** out, bool implicit_only) {
   *out = nullptr;
   int maxN = 0, maxA = 0, maxIn = 0, maxOut = 0;
+  bool arc = false;
   for (int g = 0; g < n_graphs; g++) {
     maxN = std::max(maxN, dims[g].N);
     maxA = std::max(maxA, dims[g].A);
     maxIn = std::max(maxIn, dims[g].max_in);
     maxOut = std::max(maxOut, dims[g].max_out);
+    arc |= !dims[g].uniform;
   }
   gtnb_lattice* lat = new gtnb_lattice();
+  lat->arc_labels = implicit_only && arc;
   lat->max_in_deg = maxIn;
   lat->max_out_deg = maxOut;
   lat->B = B;
@@ -1231,7 +1238,7 @@ int gtnb_compose_linear(
 int gtnb::compose_linear_impl(
     gtnb_ctx* ctx, int B, const gtnb_graph_view* graphs, int n_graphs, int linear_first,
     const int32_t* T, int C, const float* emissions_dev, int64_t emissions_stride, bool implicit_only,
-    gtnb_lattice** out) {
+    gtnb_lattice** out, bool arc_labels, const float* arc_weights_dev) {
   if (!ctx || !out || B < 0 || !graphs || !T || C <= 0 || (n_graphs != B && n_graphs != 1))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_compose_linear: bad arguments");
   *out = nullptr;
@@ -1279,6 +1286,7 @@ int gtnb::compose_linear_impl(
         int lab = linear_first ? v.arc_ilabel[a] : v.arc_olabel[a];
         if (lab == GTNB_EPSILON)
           return GTNB_ERR_UNSUPPORTED;
+        if (arc_labels && !(lab >= 0 && lab < C)) continue; // never matches: no entry, gradient 0
         s.in_src.push_back(v.arc_src[a]);
         s.in_label.push_back((lab >= 0 && lab < C) ? lab : -1);
         s.in_arc.push_back(a);
@@ -1286,6 +1294,13 @@ int gtnb::compose_linear_impl(
         if (exact_ties) s.in_out_pos.push_back(out_pos[a]);
       }
       s.in_ptr[d + 1] = (int)s.in_src.size();
+    }
+    if (arc_labels) {
+      // the tables hold the entries kept; the by-arc-id label copies (read for Viterbi paths only, which
+      // the loss never asks for) are cut to the same slab size
+      s.A = (int)s.in_src.size();
+      s.il.resize(s.A);
+      s.ol.resize(s.A);
     }
     if (exact_ties) {
       s.start_rank.assign(s.N, -1);
@@ -1332,13 +1347,20 @@ int gtnb::compose_linear_impl(
     for (int n = 0; n < s.N; n++) max_out = std::max(max_out, outdeg[n]);
     dims[g] = SgDims{s.N, s.A, (int)s.acc.size(), all_valid, uniform, max_in, max_out};
   }
-  if (implicit_only && !implicit_dims_supported(dims.data(), n_graphs))
+  if (implicit_only && !implicit_dims_supported(dims.data(), n_graphs, arc_labels ? C : 0))
     return fail(ctx, GTNB_ERR_UNSUPPORTED, "graph operand does not qualify for the implicit sweeps");
   std::vector<long long> sgn, sga;
   gtnb_lattice* lat = nullptr;
   int rc = composed_alloc(ctx, B, dims.data(), n_graphs, linear_first, T, C, emissions_dev,
                           emissions_stride, sgn, sga, &lat, implicit_only);
   if (rc) return rc;
+  if (arc_labels && n_graphs != 1) { // arc-gradient slabs in Graph arc numbering, whatever was left out
+    long long off = 0;
+    for (int b = 0; b < B; b++) {
+      lat->meta_h[b].grad_graph_off = off;
+      off += graphs[b].num_arcs;
+    }
+  }
   const long long tc = lat->tot_acc;
 #define TRY(x)              \
   do {                      \
@@ -1361,6 +1383,21 @@ int gtnb::compose_linear_impl(
     TRY(upload_slabs(ctx, lat->sg_in_arc, sga, pi));
     for (int g = 0; g < n_graphs; g++) pf[g] = &sg[g].in_w;
     TRY(upload_slabs(ctx, lat->sg_in_w, sga, pf));
+    if (arc_weights_dev) {
+      // entry k of graph g reads arc_weights_dev[first arc of g + in_arc[k]]; padding keeps its 0
+      std::vector<int32_t> widx((size_t)lat->tot_sgA, -1);
+      long long first = 0;
+      for (int g = 0; g < n_graphs; g++) {
+        for (size_t k = 0; k < sg[g].in_arc.size(); k++) widx[sga[g] + k] = (int32_t)(first + sg[g].in_arc[k]);
+        first += graphs[g].num_arcs;
+      }
+      int32_t* widx_dev = nullptr;
+      TRY(dev_alloc(ctx, &widx_dev, lat->tot_sgA));
+      rc = upload(ctx, widx_dev, widx.data(), lat->tot_sgA);
+      if (!rc) rc = launch_gather(ctx, lat->sg_in_w, widx_dev, arc_weights_dev, lat->tot_sgA);
+      dev_free(ctx, widx_dev);
+      if (rc) goto bad;
+    }
     for (int g = 0; g < n_graphs; g++) pi[g] = &sg[g].il;
     TRY(upload_slabs(ctx, lat->sg_ilabel, sga, pi));
     for (int g = 0; g < n_graphs; g++) pi[g] = &sg[g].ol;

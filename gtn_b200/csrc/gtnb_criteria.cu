@@ -1398,3 +1398,230 @@ extern "C" int gtnb_asg_loss_ex(
   if (ctx) arena_end(ctx);
   return rc;
 }
+
+/*
+ * Loss over user-supplied target graphs (the criterion of the reference's pytorch_loss.py and of its word
+ * decomposition examples):
+ *   loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b))
+ * E_b: linearGraph(T_b, C) on the first T_b rows of emissions_b; A_b: graph b, matched on its olabels.
+ * The implicit sweeps of k_implicit.cu run intersect(A_b, E_b) without building it (the arc-label instantiations
+ * when some graph is not label-uniform), with forwardScore(E_b) (k_linear.cu) beside the forward sweep.  Graphs that
+ * do not fit the implicit layout, C above the arc-label limit, the implicit flag off, or a non-finite value met by
+ * a sweep take the materialised lattices (gtnb_compose_linear, forward, backward, compose_grad), the normaliser's
+ * included.
+ */
+namespace {
+
+struct GraphLossArgs {
+  int B, T, C;
+  const float* emissions;
+  int emissions_on_device;
+  const int32_t* input_lens;
+  const gtnb_graph_view* graphs;
+  const float* arc_weights;
+  int arc_weights_on_device;
+  float* losses_host;
+  float* grads;
+  int grads_on_device;
+  float* arc_grads;
+  int arc_grads_on_device;
+};
+
+#define TRY(x)                 \
+  do {                         \
+    if ((rc = (x))) goto done; \
+  } while (0)
+#define TRYCUDA(call)                                      \
+  do {                                                     \
+    cudaError_t e__ = (call);                              \
+    if (e__ != cudaSuccess) {                              \
+      rc = cuda_fail(ctx, e__, #call, __FILE__, __LINE__); \
+      goto done;                                           \
+    }                                                      \
+  } while (0)
+
+/* one attempt; implicit: try the sweeps first (the materialised lattices when the graphs do not qualify).
+ * *needs_exact: a sweep met a non-finite weight or emission, the outputs are not to be used. */
+int graph_loss_once(gtnb_ctx* ctx, const GraphLossArgs& a, const std::vector<gtnb_graph_view>& views,
+                    const std::vector<int32_t>& Tb, long long tot_arcs, bool implicit, bool* needs_exact) {
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C;
+  const bool want = a.grads || a.arc_grads;
+  int maxT = 0;
+  for (int b = 0; b < B; b++) maxT = std::max(maxT, Tb[b]);
+  int rc = GTNB_OK;
+  float *e_dev = nullptr, *g_dev = nullptr, *ag_dev = nullptr, *den = nullptr, *minus1 = nullptr;
+  int32_t *T_dev = nullptr, *status = nullptr;
+  gtnb_lattice *lat = nullptr, *dlat = nullptr;
+  cudaStream_t main_stream = ctx->stream;
+  const float* aw_dev = a.arc_weights_on_device ? a.arc_weights : nullptr;
+  const float* den_scores = nullptr;
+  std::vector<float> m1(B, -1.0f); // subtract's gradFunc, functions.cpp:53-58
+  // materialised route: forwardScore(E_b) as the reference computes it, non-finite emissions included (its sweep
+  // turns a node whose in-scores are all NaN into -inf), from the lattice of one start-and-accept node with a
+  // self-loop per label: compose(free, E_b) is E_b arc for arc
+  std::vector<uint8_t> free_flags(1, 3);
+  std::vector<int32_t> free_src(C, 0), free_lab(C);
+  for (int c = 0; c < C; c++) free_lab[c] = c;
+  gtnb_graph_view free_view;
+  std::memset(&free_view, 0, sizeof(free_view));
+  free_view.num_nodes = 1;
+  free_view.num_arcs = C;
+  free_view.node_flags = free_flags.data();
+  free_view.arc_src = free_view.arc_dst = free_src.data();
+  free_view.arc_ilabel = free_view.arc_olabel = free_lab.data();
+
+  TRY(ensure_side_streams(ctx, 0, 0));
+  if (a.emissions_on_device) {
+    e_dev = const_cast<float*>(a.emissions);
+  } else {
+    TRY(dev_alloc(ctx, &e_dev, per * B));
+    TRYCUDA(cudaMemcpyAsync(e_dev, a.emissions, sizeof(float) * per * B, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  TRY(dev_alloc(ctx, &den, B));
+  TRY(dev_alloc(ctx, &T_dev, B));
+  TRY(dev_alloc(ctx, &status, B));
+  TRY(dev_alloc(ctx, &minus1, B));
+  if (want) {
+    if (a.grads && a.grads_on_device)
+      g_dev = a.grads;
+    else
+      TRY(dev_alloc(ctx, &g_dev, per * B)); // also the scratch of a call that only wants the arc gradients
+    TRYCUDA(cudaMemsetAsync(g_dev, 0, sizeof(float) * per * B, ctx->stream));
+    if (a.arc_grads) {
+      if (a.arc_grads_on_device)
+        ag_dev = a.arc_grads;
+      else
+        TRY(dev_alloc(ctx, &ag_dev, tot_arcs));
+      if (tot_arcs) TRYCUDA(cudaMemsetAsync(ag_dev, 0, sizeof(float) * tot_arcs, ctx->stream));
+    }
+  }
+  TRYCUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * B, ctx->stream));
+  TRY(stage_begin(ctx));
+  TRY(stage_upload(ctx, T_dev, Tb.data(), sizeof(int32_t) * B));
+  TRY(stage_upload(ctx, minus1, m1.data(), sizeof(float) * B));
+  TRY(stage_end(ctx));
+
+  if (implicit) {
+    rc = compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, e_dev, per, true, &lat, true, aw_dev);
+    if (rc == GTNB_ERR_UNSUPPORTED) { // does not fit the implicit layout: materialise
+      implicit = false;
+      rc = GTNB_OK;
+    } else if (rc) {
+      goto done;
+    }
+  }
+  if (implicit) {
+    // forwardScore(E_b) and its +1 gradient on the second stream, beside the forward sweep
+    TRYCUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
+    TRYCUDA(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_fork, 0));
+    ctx->stream = ctx->copy_stream;
+    rc = launch_linear_forward(ctx, B, T_dev, maxT, C, e_dev, per, 0, den, want ? g_dev : nullptr, per, nullptr,
+                               1.0f, 0);
+    ctx->stream = main_stream;
+    if (rc) goto done;
+    TRYCUDA(cudaEventRecord(ctx->ev_join, ctx->copy_stream));
+    TRY(launch_implicit_forward(ctx, lat, status));
+    TRYCUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+    if (want) TRY(launch_implicit_backward(ctx, lat, minus1, g_dev, per, 0, -1, ag_dev));
+    den_scores = den;
+  } else {
+    TRY(compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, e_dev, per, false, &lat, false, aw_dev));
+    TRY(compose_linear_impl(ctx, B, &free_view, 1, 0, Tb.data(), C, e_dev, per, false, &dlat));
+    TRY(gtnb_forward(ctx, dlat, 0, nullptr, nullptr));
+    TRY(gtnb_forward(ctx, lat, 0, nullptr, nullptr));
+    if (want) {
+      TRY(gtnb_backward(ctx, dlat, 0, nullptr)); // +1
+      TRY(gtnb_compose_grad(ctx, dlat, nullptr, g_dev, per));
+      TRY(gtnb_backward(ctx, lat, 0, m1.data()));
+      TRY(gtnb_compose_grad(ctx, lat, ag_dev, g_dev, per));
+    }
+    den_scores = dlat->out_scores;
+  }
+  if (a.grads && !a.grads_on_device)
+    TRYCUDA(cudaMemcpyAsync(a.grads, g_dev, sizeof(float) * per * B, cudaMemcpyDeviceToHost, ctx->stream));
+  if (a.arc_grads && !a.arc_grads_on_device && tot_arcs)
+    TRYCUDA(cudaMemcpyAsync(a.arc_grads, ag_dev, sizeof(float) * tot_arcs, cudaMemcpyDeviceToHost, ctx->stream));
+  TRY(readback_reserve(ctx, 3 * sizeof(float) * B));
+  {
+    float* d = reinterpret_cast<float*>(ctx->readback);
+    float* n = d + B;
+    int32_t* st = reinterpret_cast<int32_t*>(n + B);
+    TRYCUDA(cudaMemcpyAsync(d, den_scores, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(n, lat->out_scores, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaMemcpyAsync(st, status, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    TRYCUDA(cudaStreamSynchronize(ctx->stream));
+    for (int b = 0; b < B; b++) a.losses_host[b] = d[b] - n[b];
+    if (implicit)
+      for (int b = 0; b < B; b++) *needs_exact |= st[b] != 0;
+  }
+done:
+  ctx->stream = main_stream;
+  if (rc) cudaStreamSynchronize(ctx->copy_stream); // nothing may still run on the second stream when the buffers go
+  if (lat) gtnb_lattice_destroy(ctx, lat);
+  if (dlat) gtnb_lattice_destroy(ctx, dlat);
+  if (!a.emissions_on_device) dev_free(ctx, e_dev);
+  if (!(a.grads && a.grads_on_device)) dev_free(ctx, g_dev);
+  if (!(a.arc_grads && a.arc_grads_on_device)) dev_free(ctx, ag_dev);
+  dev_free(ctx, den);
+  dev_free(ctx, T_dev);
+  dev_free(ctx, status);
+  dev_free(ctx, minus1);
+  return rc;
+}
+
+#undef TRY
+#undef TRYCUDA
+
+int graph_loss_run(gtnb_ctx* ctx, const GraphLossArgs& a) {
+  const int B = a.B, T = a.T, C = a.C;
+  if (!ctx || B < 0 || T < 0 || C <= 0 || (B > 0 && (!a.emissions || !a.graphs || !a.losses_host)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_graph_loss: bad arguments");
+  std::vector<int32_t> Tb(B);
+  std::vector<gtnb_graph_view> views(a.graphs, a.graphs + B);
+  long long tot_arcs = 0;
+  for (int b = 0; b < B; b++) {
+    Tb[b] = a.input_lens ? a.input_lens[b] : T;
+    if (Tb[b] < 0 || Tb[b] > T) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_graph_loss: input_lens outside [0, T]");
+    if (validate_view(ctx, views[b])) return GTNB_ERR_INVALID_ARGUMENT;
+    for (int k = 0; k < views[b].num_arcs; k++)
+      if (views[b].arc_olabel[k] == GTNB_EPSILON)
+        return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                    "gtnb_graph_loss: graph " + std::to_string(b) +
+                        " has epsilon arcs; remove them first (remove(g, epsilon))");
+    if (a.arc_weights && !a.arc_weights_on_device) views[b].weights = a.arc_weights + tot_arcs;
+    tot_arcs += views[b].num_arcs;
+  }
+  if (tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_graph_loss: more than 2^31 arcs");
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (B == 0) return GTNB_OK;
+  // (graphs that are not label-uniform need C <= k_implicit.cu's kArcMaxLabels: compose_linear_impl checks)
+  const bool implicit = ctx->use_implicit;
+  bool needs_exact = false;
+  int rc = graph_loss_once(ctx, a, views, Tb, tot_arcs, implicit, &needs_exact);
+  if (rc == GTNB_OK && needs_exact) {
+    // a non-finite weight or emission: the materialised lattices reproduce the reference's inf / NaN
+    // propagation arc by arc
+    arena_end(ctx);
+    arena_begin(ctx);
+    rc = graph_loss_once(ctx, a, views, Tb, tot_arcs, false, &needs_exact);
+  }
+  // T_b = 0: linearGraph(0, C) accepts nothing, so both scores are -inf and the loss is NaN (no gradient)
+  for (int b = 0; b < B && rc == GTNB_OK; b++)
+    if (Tb[b] == 0) a.losses_host[b] = std::numeric_limits<float>::quiet_NaN();
+  return rc;
+}
+
+} // namespace
+
+extern "C" int gtnb_graph_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, float* losses_host,
+    float* grads, int grads_on_device, float* arc_grads, int arc_grads_on_device) {
+  const GraphLossArgs a{B, T, C, emissions, emissions_on_device, input_lens, graphs, arc_weights,
+                        arc_weights_on_device, losses_host, grads, grads_on_device, arc_grads, arc_grads_on_device};
+  if (ctx) arena_begin(ctx);
+  const int rc = graph_loss_run(ctx, a);
+  if (ctx) arena_end(ctx);
+  return rc;
+}

@@ -98,6 +98,7 @@ struct gtnb_lattice {
   int C = 0;
   int max_lvl_nodes = 0, max_lvl_arcs = 0; // upper bounds over the batch
   int max_in_deg = 0, max_out_deg = 0; // of the graph operands (composed lattices)
+  bool arc_labels = false; // some graph operand is not label-uniform: k_implicit.cu's arc-label kernels
   int max_T = 0;
   long long tot_N = 0, tot_A = 0, tot_L = 0, tot_acc = 0, tot_bl = 0, tot_bn = 0;
   long long tot_sgN = 0, tot_sgA = 0;
@@ -173,6 +174,7 @@ int launch_ctc_build(
     const int32_t* tgt_len_dev, int blank);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
+int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_sub(gtnb_ctx* ctx, const float* a, const float* b, float* out, int n);
 
 int fail(gtnb_ctx* ctx, int code, const std::string& msg);
@@ -305,7 +307,7 @@ int launch_backward_fused(
     gtnb_ctx* ctx, gtnb_lattice* lat, const float* deltas_dev, float* grad_emis, int64_t grad_stride);
 // kernels (k_dense.cu): factored dense-trellis Viterbi
 bool implicit_supported(const gtnb_lattice* lat);
-bool implicit_dims_supported(const SgDims* dims, int n_graphs);
+bool implicit_dims_supported(const SgDims* dims, int n_graphs, int arc_C = 0);
 int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0 = 0, int nb = -1);
 /* k_bidir.cu: the CTC criterion in one launch (two-CTA clusters meeting in the middle), normaliser included */
 bool bidir_supported(const gtnb_lattice* lat, const float* emissions, int64_t stride, const float* grad, int64_t grad_stride);
@@ -329,9 +331,14 @@ int launch_banded_backward(
 int launch_implicit_backward(
     gtnb_ctx* ctx, gtnb_lattice* lat, const float* deltas_dev, float* grad_emis, int64_t grad_stride,
     int b0 = 0, int nb = -1, float* grad_graph = nullptr);
+/* arc_labels (gtnb_graph_loss): arcs whose label is outside [0, C) are left out of the tables, graphs that are not
+ * label-uniform may take the implicit sweeps, and graph b's arc-gradient slab starts at the sum of the earlier
+ * graphs' num_arcs.  arc_weights_dev (nullable): [sum num_arcs] device weights that replace the views' weights. */
 int compose_linear_impl(
     gtnb_ctx* ctx, int B, const gtnb_graph_view* graphs, int n_graphs, int linear_first, const int32_t* T,
-    int C, const float* emissions_dev, int64_t emissions_stride, bool implicit_only, gtnb_lattice** out);
+    int C, const float* emissions_dev, int64_t emissions_stride, bool implicit_only, gtnb_lattice** out,
+    bool arc_labels = false, const float* arc_weights_dev = nullptr);
+int validate_view(gtnb_ctx* ctx, const gtnb_graph_view& v);
 int ensure_side_streams(gtnb_ctx* ctx, int n_streams, int n_events);
 int launch_viterbi_dense(
     gtnb_ctx* ctx, int B, int T_max, int C, const int32_t* T_dev, const float* emis, int64_t stride,

@@ -153,6 +153,12 @@ __global__ void scatter_add_kernel(float* __restrict__ dst, const int32_t* __res
        i += (long long)gridDim.x * blockDim.x)
     atomicAdd(&dst[idx[i]], src[i]);
 }
+__global__ void gather_kernel(float* __restrict__ dst, const int32_t* __restrict__ idx,
+                              const float* __restrict__ src, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x)
+    if (idx[i] >= 0) dst[i] = src[idx[i]];
+}
 __global__ void sub_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = a[i] - b[i];
@@ -165,6 +171,14 @@ int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const floa
   if (n <= 0) return GTNB_OK;
   int blocks = (int)std::min<long long>((n + 255) / 256, 1024);
   GTNB_LAUNCH(ctx, "scatter_add", scatter_add_kernel<<<blocks, 256, 0, ctx->stream>>>(dst, idx, src, n));
+  return GTNB_OK;
+}
+
+/* dst[i] = src[idx[i]] where idx[i] >= 0: device-resident arc weights into a graph operand's in-arc table */
+int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n) {
+  if (n <= 0) return GTNB_OK;
+  int blocks = (int)std::min<long long>((n + 255) / 256, 1024);
+  GTNB_LAUNCH(ctx, "gather", gather_kernel<<<blocks, 256, 0, ctx->stream>>>(dst, idx, src, n));
   return GTNB_OK;
 }
 

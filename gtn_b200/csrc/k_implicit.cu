@@ -31,6 +31,13 @@
  * the caller re-runs the batch through the materialised path, which reproduces the
  * reference's NaN / inf propagation arc by arc.  Requires: no epsilon labels, all labels in
  * [0, C), all in-arcs of a graph node carry the same label (CTC, forced alignment, ASG).
+ *
+ * Arc-label mode (template flag ARC, gtnb_graph_loss on graphs where some node's in-arcs carry
+ * different labels: a wildcard state, hand-built graphs): every in-arc reads its own emission
+ * e[t-1][label(a)] from the frame's emission row staged in shared memory (any C up to
+ * kArcMaxLabels), and the backward sums the arc posteriors of a frame per label in a C-float
+ * shared row that is flushed to global memory once per frame.  Only the several-nodes-per-thread
+ * path and the wide kernels have this mode; with ARC = false they compile to what they were.
  */
 #ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
@@ -68,9 +75,15 @@ struct ImpLayout {
   int off_outptr, off_outent, off_cursor, off_cur, off_ng, off_accg; // backward only
   int off_sw, off_act, off_erow, off_rows3; // wide kernels
   int total;
+  int off_alab, off_earc, off_ge; // arc-label mode: per-entry labels, [2][C] emission rows, [C] emission gradients
 };
 
-ImpLayout make_imp_layout(int maxN, int maxA, bool backward, bool wide = false, int C = 0) {
+// arc-label mode: the emission row of a frame is staged by every thread in steps of kImpThreads,
+// kArcRows values per thread (held in registers while the frame before is swept)
+constexpr int kArcRows = 4;
+constexpr int kArcMaxLabels = kArcRows * kImpThreads;
+
+ImpLayout make_imp_layout(int maxN, int maxA, bool backward, bool wide = false, int C = 0, bool arc = false) {
   ImpLayout o;
   o.pitch = (maxN + 3) & ~3;
   o.tabN = maxN + 1;
@@ -103,6 +116,12 @@ ImpLayout make_imp_layout(int maxN, int maxA, bool backward, bool wide = false, 
     o.off_act = take(4 * 2 * o.tabN);
     o.off_erow = take(4 * 2 * std::max(C, 4));
     o.off_rows3 = take(4 * 3 * o.pitch);
+  }
+  o.off_alab = o.off_earc = o.off_ge = 0;
+  if (arc) {
+    o.off_alab = take(4 * o.tabA);
+    o.off_earc = wide ? o.off_erow : take(4 * 2 * std::max(C, 4));
+    if (backward) o.off_ge = take(4 * std::max(C, 4));
   }
   o.total = off;
   return o;
@@ -280,10 +299,53 @@ __device__ __noinline__ float imp_fwd_node_any(
   return mx + ilog1p(sum);
 }
 
+/* arc-label mode: the same two passes, every in-arc with its own label's emission */
+__device__ __noinline__ float imp_fwd_node_arc(
+    int e0, int e1, const float* erow, const int* t_alab, const int* t_src, const float* t_w, const float* prev) {
+  float mx = ninf();
+#pragma unroll 1
+  for (int a = e0; a < e1; a++) mx = fmaxf(mx, prev[t_src[a]] + (t_w[a] + erow[t_alab[a]]));
+  if (mx == CUDART_INF_F || mx == -CUDART_INF_F) return mx;
+  float sum = -1.0f;
+#pragma unroll 1
+  for (int a = e0; a < e1; a++) sum += iexp((prev[t_src[a]] + (t_w[a] + erow[t_alab[a]])) - mx);
+  return mx + ilog1p(sum);
+}
+
+/* arc-label mode: the per-entry matched labels of the graph operand -> shared memory */
+__device__ __forceinline__ void load_arc_labels(const GraphMeta& m, const int32_t* __restrict__ sg_in_label,
+                                                int* t_alab) {
+  const int32_t* il = sg_in_label + m.sg_arc_base;
+  for (int e = threadIdx.x; e < m.sg_A; e += kImpThreads) t_alab[e] = il[e];
+  __syncthreads();
+}
+
+/* arc-label mode: emission row `row` (C floats) -> shared memory; returns "some value is not finite" */
+__device__ __forceinline__ bool stage_erow(const float* row, float* dst, int C) {
+  bool bad = false;
+  for (int c = threadIdx.x; c < C; c += kImpThreads) {
+    const float v = __ldg(row + c);
+    dst[c] = v;
+    bad |= !finite_f(v);
+  }
+  return bad;
+}
+
+/* arc-label mode: one frame's per-label sums of the arc posteriors -> the emission gradient, and the
+ * row zeroed for the next frame (each thread flushes and zeroes the same labels) */
+__device__ __forceinline__ void flush_erow_grad(float* GE, float* gr, int C, float delta) {
+  for (int c = threadIdx.x; c < C; c += kImpThreads) {
+    const float v = GE[c];
+    GE[c] = 0.0f;
+    if (v != 0.0f) atomicAdd(gr + c, v * delta);
+  }
+}
+
 /* ------------------------------------------------------------------ */
 /* forward                                                             */
 /* ------------------------------------------------------------------ */
 
+template <bool ARC = false>
 __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -312,12 +374,15 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
 
   bool bad = load_tables(m, sg_flags, sg_in_ptr, sg_in_src, sg_in_label, sg_in_w, t_inptr, t_src, t_w,
                          t_lab, t_flags);
+  int* t_alab = reinterpret_cast<int*>(smem + lay.off_alab); // ARC only
+  float* E_s = reinterpret_cast<float*>(smem + lay.off_earc); // ARC only: [2][C], frame t-1 at (t-1) & 1
+  if (ARC) load_arc_labels(m, sg_in_label, t_alab);
   float* sc = scores + m.node_base;
   const float* em = emissions + m.emis_off;
   // fast path: one node per thread, every node with at most three in-arcs (block-uniform)
   int my_deg = 0;
   if (tid < N1) my_deg = t_inptr[tid + 1] - t_inptr[tid];
-  const bool fast = (N1 <= kImpThreads) && !__syncthreads_or(my_deg > 3);
+  const bool fast = !ARC && (N1 <= kImpThreads) && !__syncthreads_or(my_deg > 3);
   float* S0 = S;
   float* S1 = S + (fast ? kFastRow : lay.pitch);
   // frame 0: start nodes carry the implicit 0 (shortest.cpp:129-135), nothing else exists
@@ -332,6 +397,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
       S0[i] = v;
       sc[i] = v;
     }
+    if (ARC && T > 0) bad |= stage_erow(em, E_s, C);
   }
   __syncthreads();
 
@@ -424,16 +490,28 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     for (int t = 1; t <= T; t++) {
       const float* er = em + (long long)(t - 1) * C;
       float* srow = sc + (long long)t * pitch;
-      for (int i = tid; i < N1; i += kImpThreads) {
-        const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
-        float sv = ninf();
-        if (e1 > e0) {
-          const float e = __ldg(er + t_lab[i]);
-          bad |= !finite_f(e);
-          sv = imp_fwd_node_any(e0, e1, e, t_src, t_w, prev);
+      if (ARC) {
+        // frame t-1's row was staged before the last barrier; frame t's goes to the other half
+        const float* Ecur = E_s + ((t - 1) & 1) * C;
+        for (int i = tid; i < N1; i += kImpThreads) {
+          const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
+          const float sv = (e1 > e0) ? imp_fwd_node_arc(e0, e1, Ecur, t_alab, t_src, t_w, prev) : ninf();
+          cur[i] = sv;
+          srow[i] = sv;
         }
-        cur[i] = sv;
-        srow[i] = sv;
+        if (t < T) bad |= stage_erow(er + C, E_s + (t & 1) * C, C);
+      } else {
+        for (int i = tid; i < N1; i += kImpThreads) {
+          const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
+          float sv = ninf();
+          if (e1 > e0) {
+            const float e = __ldg(er + t_lab[i]);
+            bad |= !finite_f(e);
+            sv = imp_fwd_node_any(e0, e1, e, t_src, t_w, prev);
+          }
+          cur[i] = sv;
+          srow[i] = sv;
+        }
       }
       float* tmp = prev;
       prev = cur;
@@ -495,7 +573,7 @@ __device__ __forceinline__ void build_out_lists(
 /* backward                                                            */
 /* ------------------------------------------------------------------ */
 
-template <bool GRAPH_GRAD>
+template <bool GRAPH_GRAD, bool ARC = false>
 __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -535,6 +613,10 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
   float* ggr = GRAPH_GRAD ? grad_graph + m.grad_graph_off : nullptr;
 
   load_tables(m, sg_flags, sg_in_ptr, sg_in_src, sg_in_label, sg_in_w, t_inptr, t_src, t_w, t_lab, t_flags);
+  int* t_alab = reinterpret_cast<int*>(smem + lay.off_alab); // ARC only
+  float* E_s = reinterpret_cast<float*>(smem + lay.off_earc); // ARC only: frame t-1's emission row
+  float* GE = reinterpret_cast<float*>(smem + lay.off_ge); // ARC only: frame t-1's emission gradient per label
+  if (ARC) load_arc_labels(m, sg_in_label, t_alab);
 
   build_out_lists(N1, A1, t_src, t_outptr, t_outent, t_cursor);
 
@@ -556,7 +638,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     my_deg = t_inptr[tid + 1] - t_inptr[tid];
     my_od = t_outptr[tid + 1] - t_outptr[tid];
   }
-  const bool fast = (N1 <= kImpThreads) && !__syncthreads_or(my_deg > 3 || my_od > 3);
+  const bool fast = !ARC && (N1 <= kImpThreads) && !__syncthreads_or(my_deg > 3 || my_od > 3);
   float* Sa = S;
   float* Sb = S + (fast ? kFastRow : lay.pitch);
   float* CURa = CUR;
@@ -710,6 +792,8 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     // ---- general path: several nodes per thread, two barriers per level
     if (GRAPH_GRAD)
       for (int a = tid; a < A1; a += kImpThreads) ACCG[a] = 0.0f;
+    if (ARC)
+      for (int c = tid; c < C; c += kImpThreads) GE[c] = 0.0f;
     for (int i = tid; i < N1; i += kImpThreads) {
       const float sT = sc[(long long)T * pitch + i];
       Sa[i] = sT;
@@ -721,24 +805,43 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
       const float* er = em + (long long)(t - 1) * C;
       float* gr = gem + (long long)(t - 1) * C;
       for (int i = tid; i < N1; i += kImpThreads) Sprev[i] = sc[(long long)(t - 1) * pitch + i];
+      if (ARC) stage_erow(er, E_s, C);
       __syncthreads();
-      for (int i = tid; i < N1; i += kImpThreads) {
-        const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
-        if (e1 == e0) continue;
-        const float gi = NG[i], sn = Sown[i];
-        const bool ex = sn > -CUDART_INF_F;
-        const float e = __ldg(er + t_lab[i]);
-        float acc = 0.0f;
+      if (ARC) {
+        for (int i = tid; i < N1; i += kImpThreads) {
+          const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
+          if (e1 == e0) continue;
+          const float gi = NG[i], sn = Sown[i];
+          const bool ex = sn > -CUDART_INF_F;
 #pragma unroll 1
-        for (int a = e0; a < e1; a++) {
-          const float c = ex ? gi * iexp(Sprev[t_src[a]] + (t_w[a] + e) - sn) : 0.0f;
-          CURa[a] = c;
-          acc += c;
-          if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this thread only
+          for (int a = e0; a < e1; a++) {
+            const int lab = t_alab[a];
+            const float c = ex ? gi * iexp(Sprev[t_src[a]] + (t_w[a] + E_s[lab]) - sn) : 0.0f;
+            CURa[a] = c;
+            if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this thread only
+            if (c != 0.0f) atomicAdd(&GE[lab], c); // shared: one global add per label and frame below
+          }
         }
-        if (acc != 0.0f) atomicAdd(gr + t_lab[i], acc * delta);
+      } else {
+        for (int i = tid; i < N1; i += kImpThreads) {
+          const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
+          if (e1 == e0) continue;
+          const float gi = NG[i], sn = Sown[i];
+          const bool ex = sn > -CUDART_INF_F;
+          const float e = __ldg(er + t_lab[i]);
+          float acc = 0.0f;
+#pragma unroll 1
+          for (int a = e0; a < e1; a++) {
+            const float c = ex ? gi * iexp(Sprev[t_src[a]] + (t_w[a] + e) - sn) : 0.0f;
+            CURa[a] = c;
+            acc += c;
+            if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this thread only
+          }
+          if (acc != 0.0f) atomicAdd(gr + t_lab[i], acc * delta);
+        }
       }
       __syncthreads();
+      if (ARC) flush_erow_grad(GE, gr, C, delta);
       for (int u = tid; u < N1; u += kImpThreads) {
         float gn = 0.0f;
 #pragma unroll 1
@@ -793,7 +896,7 @@ __device__ __forceinline__ unsigned group_mask() {
   return (G >= 32) ? 0xffffffffu : (((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1)));
 }
 
-template <int G>
+template <int G, bool ARC = false>
 __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -825,6 +928,8 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
 
   bool bad = load_tables(m, sg_flags, sg_in_ptr, sg_in_src, sg_in_label, sg_in_w, t_inptr, t_src, t_w,
                          t_lab, t_flags);
+  int* t_alab = reinterpret_cast<int*>(smem + lay.off_alab); // ARC only
+  if (ARC) load_arc_labels(m, sg_in_label, t_alab);
   build_wide_tables(N1, A1, t_inptr, t_src, t_w, nullptr, t_sw, t_act, nullptr);
   float* sc = scores + m.node_base;
   const float* em = emissions + m.emis_off;
@@ -835,7 +940,9 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
     prev[i] = v;
     sc[i] = v;
   }
-  if (T > 0 && tid < C) {
+  if (ARC) {
+    if (T > 0) bad |= stage_erow(em, E_s, C);
+  } else if (T > 0 && tid < C) {
     const float e0v = __ldg(em + tid);
     E_s[tid] = e0v;
     bad |= !finite_f(e0v);
@@ -852,14 +959,22 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
     float* Enext = E_s + (t & 1) * C;
     const bool ld = (t < T) && tid < C; // next frame's emissions: in flight during this level
     float enext = 0.0f;
-    if (ld) enext = __ldg(em + (long long)t * C + tid);
+    if (!ARC && ld) enext = __ldg(em + (long long)t * C + tid);
+    float en[kArcRows]; // ARC: the next frame's row, kArcRows values per thread
+    if (ARC) {
+#pragma unroll
+      for (int k = 0; k < kArcRows; k++) {
+        const int c = tid + k * kImpThreads;
+        en[k] = (t < T && c < C) ? __ldg(em + (long long)t * C + c) : 0.0f;
+      }
+    }
     float* srow = sc + (long long)t * pitch;
     for (int r = 0; r < rounds; r++) {
       const int slot = r * kSlots + slot0;
       const bool on = slot < n_act;
       const int u = on ? t_act[slot] : 0;
       const int e0 = on ? t_inptr[u] : 0, e1 = on ? t_inptr[u + 1] : 0;
-      const float e = on ? Ecur[t_lab[u]] : 0.0f;
+      const float e = (!ARC && on) ? Ecur[t_lab[u]] : 0.0f;
       float v[kWideCap];
       float mx = ninf();
 #pragma unroll
@@ -868,7 +983,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
         v[k] = ninf();
         if (a < e1) {
           const int2 sw = t_sw[a];
-          v[k] = prev[sw.x] + (__int_as_float(sw.y) + e);
+          v[k] = prev[sw.x] + (__int_as_float(sw.y) + (ARC ? Ecur[t_alab[a]] : e));
         }
         mx = fmaxf(mx, v[k]);
       }
@@ -892,9 +1007,19 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
         cur[i] = ninf();
         srow[i] = ninf();
       }
-    if (ld) {
+    if (!ARC && ld) {
       Enext[tid] = enext;
       bad |= !finite_f(enext);
+    }
+    if (ARC) {
+#pragma unroll
+      for (int k = 0; k < kArcRows; k++) {
+        const int c = tid + k * kImpThreads;
+        if (t < T && c < C) {
+          Enext[c] = en[k];
+          bad |= !finite_f(en[k]);
+        }
+      }
     }
     float* tmp = prev;
     prev = cur;
@@ -920,7 +1045,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
   if (bad) atomicOr(&status[blockIdx.x], 1);
 }
 
-template <int G, bool GRAPH_GRAD>
+template <int G, bool GRAPH_GRAD, bool ARC = false>
 __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -964,6 +1089,9 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
   float* ggr = GRAPH_GRAD ? grad_graph + m.grad_graph_off : nullptr;
 
   load_tables(m, sg_flags, sg_in_ptr, sg_in_src, sg_in_label, sg_in_w, t_inptr, t_src, t_w, t_lab, t_flags);
+  int* t_alab = reinterpret_cast<int*>(smem + lay.off_alab); // ARC only
+  float* GE = reinterpret_cast<float*>(smem + lay.off_ge); // ARC only: frame t-1's emission gradient per label
+  if (ARC) load_arc_labels(m, sg_in_label, t_alab);
   build_out_lists(N1, A1, t_src, t_outptr, t_outent, t_cursor);
   build_wide_tables(N1, A1, t_inptr, t_src, t_w, t_outptr, t_sw, t_act, t_acto);
 
@@ -991,7 +1119,12 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
   }
   if (GRAPH_GRAD)
     for (int a = tid; a < A1; a += kImpThreads) ACCG[a] = 0.0f;
-  if (tid < C) E_s[((T - 1) & 1) * C + tid] = __ldg(em + (long long)(T - 1) * C + tid);
+  if (ARC) {
+    stage_erow(em + (long long)(T - 1) * C, E_s + ((T - 1) & 1) * C, C);
+    for (int c = tid; c < C; c += kImpThreads) GE[c] = 0.0f;
+  } else if (tid < C) {
+    E_s[((T - 1) & 1) * C + tid] = __ldg(em + (long long)(T - 1) * C + tid);
+  }
   __syncthreads();
 
   constexpr int kSlots = kImpThreads / G;
@@ -1005,16 +1138,24 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
     const bool more = t >= 2;
     float snext = ninf(), enext = 0.0f; // in flight during this level
     if (more && tid < N1) snext = __ldg(sc + (long long)(t - 2) * pitch + tid);
-    if (more && tid < C) enext = __ldg(em + (long long)(t - 2) * C + tid);
+    if (!ARC && more && tid < C) enext = __ldg(em + (long long)(t - 2) * C + tid);
+    float en[kArcRows]; // ARC: frame t-2's row, kArcRows values per thread
+    if (ARC) {
+#pragma unroll
+      for (int k = 0; k < kArcRows; k++) {
+        const int c = tid + k * kImpThreads;
+        en[k] = (more && c < C) ? __ldg(em + (long long)(t - 2) * C + c) : 0.0f;
+      }
+    }
     float* gr = gem + (long long)(t - 1) * C;
-    // phase 1: arc gradients of level t (shortest.cpp:62-80), emission gradient per node
+    // phase 1: arc gradients of level t (shortest.cpp:62-80), emission gradient per node (ARC: per label)
     for (int r = 0; r < rounds; r++) {
       const int slot = r * kSlots + slot0;
       const bool on = slot < n_act;
       const int u = on ? t_act[slot] : 0;
       const int e0 = on ? t_inptr[u] : 0, e1 = on ? t_inptr[u + 1] : 0;
       const int lab = on ? t_lab[u] : 0;
-      const float e = on ? Ecur[lab] : 0.0f;
+      const float e = (!ARC && on) ? Ecur[lab] : 0.0f;
       const float g = NG[u], sn = own[u];
       const float se = (sn == -CUDART_INF_F) ? CUDART_INF_F : sn; // missing node: factors exp(-inf)
       float acc = 0.0f;
@@ -1023,17 +1164,22 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
         const int a = e0 + sub + k * G;
         if (a < e1) {
           const int2 sw = t_sw[a];
-          const float c = g * iexp(prv[sw.x] + (__int_as_float(sw.y) + e) - se);
+          const int alab = ARC ? t_alab[a] : 0;
+          const float c = g * iexp(prv[sw.x] + (__int_as_float(sw.y) + (ARC ? Ecur[alab] : e)) - se);
           CUR[a] = c;
           acc += c;
           if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this lane only
+          if (ARC && c != 0.0f) atomicAdd(&GE[alab], c); // shared: one global add per label and frame below
         }
       }
+      if (!ARC) {
 #pragma unroll
-      for (int o = G / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(gmask, acc, o);
-      if (on && sub == 0 && acc != 0.0f) atomicAdd(gr + lab, acc * delta);
+        for (int o = G / 2; o > 0; o >>= 1) acc += __shfl_xor_sync(gmask, acc, o);
+        if (on && sub == 0 && acc != 0.0f) atomicAdd(gr + lab, acc * delta);
+      }
     }
     __syncthreads();
+    if (ARC) flush_erow_grad(GE, gr, C, delta);
     // phase 2: node gradients of frame t-1, gathered over the out-arcs
     for (int r = 0; r < rounds_o; r++) {
       const int slot = r * kSlots + slot0;
@@ -1053,7 +1199,14 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
     for (int i = tid; i < N1; i += kImpThreads)
       if (t_outptr[i + 1] == t_outptr[i]) NG[i] = 0.0f;
     if (tid < N1) nxt[tid] = snext;
-    if (more && tid < C) Enext[tid] = enext;
+    if (!ARC && more && tid < C) Enext[tid] = enext;
+    if (ARC) {
+#pragma unroll
+      for (int k = 0; k < kArcRows; k++) {
+        const int c = tid + k * kImpThreads;
+        if (more && c < C) Enext[c] = en[k];
+      }
+    }
     float* tmp = own;
     own = prv;
     prv = nxt;
@@ -1070,10 +1223,10 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
 namespace {
 
 /* 0: one node per thread / several nodes per thread (implicit_*_kernel decides per CTA);
- * otherwise the lanes per node of the wide kernels */
-int wide_lanes(int max_in, int max_out, int maxN, int C, bool backward) {
+ * otherwise the lanes per node of the wide kernels (arc-label mode: C up to kArcMaxLabels) */
+int wide_lanes(int max_in, int max_out, int maxN, int C, bool backward, bool arc = false) {
   const int deg = backward ? std::max(max_in, max_out) : max_in;
-  if (deg <= 3 || maxN > kImpThreads || C > kImpThreads) return 0;
+  if (deg <= 3 || maxN > kImpThreads || C > (arc ? kArcMaxLabels : kImpThreads)) return 0;
   int G = 1;
   while (G < 32 && (deg + G - 1) / G > kWideCap) G *= 2;
   if ((deg + G - 1) / G > kWideCap) return 0;
@@ -1084,14 +1237,22 @@ int wide_lanes(int max_in, int max_out, int maxN, int C, bool backward) {
 
 #ifndef GTNB_HOST_EMU
 
-bool implicit_dims_supported(const SgDims* dims, int n_graphs) {
+/* arc_C > 0 (gtnb_graph_loss, labels in [0, arc_C)): graphs that are not label-uniform are accepted
+ * and take the arc-label kernels, which need C <= kArcMaxLabels and the larger layout */
+bool implicit_dims_supported(const SgDims* dims, int n_graphs, int arc_C) {
   int maxN = 0, maxA = 0;
+  bool arc = false;
   for (int g = 0; g < n_graphs; g++) {
-    if (!dims[g].uniform || !dims[g].all_valid) return false;
+    if (!dims[g].all_valid) return false;
+    if (!dims[g].uniform) {
+      if (arc_C <= 0) return false;
+      arc = true;
+    }
     maxN = std::max(maxN, dims[g].N);
     maxA = std::max(maxA, dims[g].A);
   }
-  return make_imp_layout(maxN, maxA, true, true, kImpThreads).total <= 200 * 1024;
+  if (arc && arc_C > kArcMaxLabels) return false;
+  return make_imp_layout(maxN, maxA, true, true, arc ? arc_C : kImpThreads, arc).total <= 200 * 1024;
 }
 
 /* true when every graph of the batch can take the implicit path */
@@ -1112,63 +1273,63 @@ bool implicit_supported(const gtnb_lattice* lat) {
       deltas_dev ? deltas_dev + b0 : nullptr, grad_emis + (long long)b0 * grad_stride,           \
       (long long)grad_stride, lat->C, lay
 
-/* utterances [b0, b0 + nb) of the batch (nb < 0: all): one CTA each, on ctx->stream */
-int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0, int nb) {
-  if (nb < 0) nb = lat->B - b0;
-  if (nb <= 0) return GTNB_OK;
-  const int G = wide_lanes(lat->max_in_deg, lat->max_out_deg, lat->max_lvl_nodes, lat->C, false);
-  const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, false, G > 0, lat->C);
+namespace {
+
+/* the launch of one mode; the arc-label instantiations carry their own names in the profile log */
+template <bool ARC>
+int implicit_forward_mode(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0, int nb) {
+  const int G = wide_lanes(lat->max_in_deg, lat->max_out_deg, lat->max_lvl_nodes, lat->C, false, ARC);
+  const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, false, G > 0, lat->C, ARC);
+  const char* name = ARC ? "implicit_forward_arc" : "implicit_forward";
 #define GTNB_LAUNCH_FWD(K)                                                                \
   do {                                                                                    \
     if (lay.total > 48 * 1024) {                                                          \
       int rc = ensure_max_smem(ctx, (const void*)K);                                      \
       if (rc) return rc;                                                                  \
     }                                                                                     \
-    GTNB_LAUNCH(ctx, "implicit_forward", K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_FWD_ARGS)); \
+    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_FWD_ARGS)); \
   } while (0)
   switch (G) {
-    case 0: GTNB_LAUNCH_FWD(implicit_forward_kernel); break;
-    case 1: GTNB_LAUNCH_FWD(implicit_forward_wide_kernel<1>); break;
-    case 2: GTNB_LAUNCH_FWD(implicit_forward_wide_kernel<2>); break;
-    case 4: GTNB_LAUNCH_FWD(implicit_forward_wide_kernel<4>); break;
-    case 8: GTNB_LAUNCH_FWD(implicit_forward_wide_kernel<8>); break;
-    case 16: GTNB_LAUNCH_FWD(implicit_forward_wide_kernel<16>); break;
-    default: GTNB_LAUNCH_FWD(implicit_forward_wide_kernel<32>); break;
+    case 0: GTNB_LAUNCH_FWD(implicit_forward_kernel<ARC>); break;
+    case 1: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<1, ARC>)); break;
+    case 2: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<2, ARC>)); break;
+    case 4: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<4, ARC>)); break;
+    case 8: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<8, ARC>)); break;
+    case 16: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<16, ARC>)); break;
+    default: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<32, ARC>)); break;
   }
 #undef GTNB_LAUNCH_FWD
   return GTNB_OK;
 }
 
-/* grad_graph (may be NULL): gradients w.r.t. the graph operands' arc weights, slab of graph b at
- * meta[b].grad_graph_off (0 for a graph shared by the batch), accumulated with atomics */
-int launch_implicit_backward(
+template <bool ARC>
+int implicit_backward_mode(
     gtnb_ctx* ctx, gtnb_lattice* lat, const float* deltas_dev, float* grad_emis, int64_t grad_stride,
     int b0, int nb, float* grad_graph) {
-  if (nb < 0) nb = lat->B - b0;
-  if (nb <= 0) return GTNB_OK;
-  const int G = wide_lanes(lat->max_in_deg, lat->max_out_deg, lat->max_lvl_nodes, lat->C, true);
-  const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, true, G > 0, lat->C);
+  const int G = wide_lanes(lat->max_in_deg, lat->max_out_deg, lat->max_lvl_nodes, lat->C, true, ARC);
+  const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, true, G > 0, lat->C, ARC);
+  const char* name = ARC ? "implicit_backward_arc" : "implicit_backward";
 #define GTNB_LAUNCH_BWD(K)                                                                \
   do {                                                                                    \
     if (lay.total > 48 * 1024) {                                                          \
       int rc = ensure_max_smem(ctx, (const void*)K);                                      \
       if (rc) return rc;                                                                  \
     }                                                                                     \
-    GTNB_LAUNCH(ctx, "implicit_backward", K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_BWD_ARGS)); \
+    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_BWD_ARGS)); \
   } while (0)
 #define GTNB_LAUNCH_BWD_G(GG)                                               \
   do {                                                                      \
     if (grad_graph)                                                         \
-      GTNB_LAUNCH_BWD((implicit_backward_wide_kernel<GG, true>));           \
+      GTNB_LAUNCH_BWD((implicit_backward_wide_kernel<GG, true, ARC>));      \
     else                                                                    \
-      GTNB_LAUNCH_BWD((implicit_backward_wide_kernel<GG, false>));          \
+      GTNB_LAUNCH_BWD((implicit_backward_wide_kernel<GG, false, ARC>));     \
   } while (0)
   switch (G) {
     case 0:
       if (grad_graph)
-        GTNB_LAUNCH_BWD(implicit_backward_kernel<true>);
+        GTNB_LAUNCH_BWD((implicit_backward_kernel<true, ARC>));
       else
-        GTNB_LAUNCH_BWD(implicit_backward_kernel<false>);
+        GTNB_LAUNCH_BWD((implicit_backward_kernel<false, ARC>));
       break;
     case 1: GTNB_LAUNCH_BWD_G(1); break;
     case 2: GTNB_LAUNCH_BWD_G(2); break;
@@ -1180,6 +1341,28 @@ int launch_implicit_backward(
 #undef GTNB_LAUNCH_BWD_G
 #undef GTNB_LAUNCH_BWD
   return GTNB_OK;
+}
+
+} // namespace
+
+/* utterances [b0, b0 + nb) of the batch (nb < 0: all): one CTA each, on ctx->stream */
+int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0, int nb) {
+  if (nb < 0) nb = lat->B - b0;
+  if (nb <= 0) return GTNB_OK;
+  return lat->arc_labels ? implicit_forward_mode<true>(ctx, lat, status_dev, b0, nb)
+                         : implicit_forward_mode<false>(ctx, lat, status_dev, b0, nb);
+}
+
+/* grad_graph (may be NULL): gradients w.r.t. the graph operands' arc weights, slab of graph b at
+ * meta[b].grad_graph_off (0 for a graph shared by the batch), accumulated with atomics */
+int launch_implicit_backward(
+    gtnb_ctx* ctx, gtnb_lattice* lat, const float* deltas_dev, float* grad_emis, int64_t grad_stride,
+    int b0, int nb, float* grad_graph) {
+  if (nb < 0) nb = lat->B - b0;
+  if (nb <= 0) return GTNB_OK;
+  return lat->arc_labels
+             ? implicit_backward_mode<true>(ctx, lat, deltas_dev, grad_emis, grad_stride, b0, nb, grad_graph)
+             : implicit_backward_mode<false>(ctx, lat, deltas_dev, grad_emis, grad_stride, b0, nb, grad_graph);
 }
 
 #endif // GTNB_HOST_EMU

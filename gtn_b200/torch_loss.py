@@ -219,3 +219,75 @@ class NgramCTCLossFunction(torch.autograd.Function):
 
 def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True):
     return NgramCTCLossFunction.apply(emissions, transitions, targets, input_lengths, blank, reduction, allreduce)
+
+
+def _graph_view(g):
+    """capi view of a gtn_b200.gtn.Graph built on the host, in its own arc-list order"""
+    from . import _gtn
+    d = _gtn.arc_lists(g)
+    return capi.make_view(d["flags"], d["src"], d["dst"], d["ilabel"], d["olabel"], d["weights"], d["in_ptr"],
+                          d["in_arcs"], d["out_ptr"], d["out_arcs"], d["start"], d["accept"])
+
+
+class GraphLossFunction(torch.autograd.Function):
+    """loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b)) with one target graph A_b per utterance
+    (bindings/python/examples/pytorch_loss.py, the word-decomposition examples), through gtnb_graph_loss.
+
+    emissions: float32 CUDA tensor [B, T, C]; graphs: B gtn_b200.gtn.Graph built on the host, matched on their
+    olabels (epsilon arcs must be removed first); input_lengths: None, a list or an int tensor (any device).
+    weights: None (the graphs' own weights, no gradient) or a float32 CUDA tensor of sum_b A_b elements, the arc
+    weights of all graphs in batch order and Graph arc numbering, which replace the graphs' weights and receive their
+    gradient (gather it from a parameter to learn, e.g., decomposition weights).  Everything runs on the current
+    stream of the emissions' device; the emission and weight gradients stay on the device, only the B losses are
+    copied to the host.
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, weights, graphs, input_lengths=None, reduction="mean"):
+        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        e = emissions.contiguous()
+        B, T, Cn = e.shape
+        assert len(graphs) == B
+        views = [_graph_view(g) for g in graphs]
+        counts = [v.num_arcs for v, _ in views]
+        n_arcs = sum(counts)
+        arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
+        w = ag = None
+        if weights is not None:
+            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
+            assert weights.numel() == n_arcs
+            w = weights.detach().contiguous()
+            ag = torch.empty(max(n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
+        stream = torch.cuda.current_stream(e.device).cuda_stream
+        g = _ctx_for(e.device, stream)
+        il = _lengths(input_lengths, B)
+        losses = np.zeros(B, np.float32)
+        grad = torch.empty_like(e)  # every row is written by the call
+        g._check(capi.lib().gtnb_graph_loss(
+            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
+            None if w is None else w.data_ptr(), 1, losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
+            None if ag is None else ag.data_ptr(), 1))
+        out = torch.from_numpy(losses).to(e.device)
+        if ag is not None:
+            ag = ag[:n_arcs].view_as(weights)
+            # utterance of every arc, for a per-utterance upstream gradient (reduction "none")
+            ctx.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(e.device)
+        ctx.save_for_backward(grad, ag)
+        ctx.reduction = reduction
+        ctx.B = B
+        return out.mean() if reduction == "mean" else out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        grad, ag = ctx.saved_tensors
+        if ctx.reduction == "mean":
+            scale = grad_output / ctx.B
+            return grad * scale, None if ag is None else ag * scale, None, None, None
+        # reduction "none": every graph belongs to one utterance, so its arcs take that utterance's upstream gradient
+        go = grad_output.reshape(-1)
+        wg = None if ag is None else ag * go[ctx.owner].view_as(ag)
+        return grad * go.view(-1, 1, 1), wg, None, None, None
+
+
+def graph_loss(emissions, graphs, input_lengths=None, weights=None, reduction="mean"):
+    return GraphLossFunction.apply(emissions, weights, graphs, input_lengths, reduction)

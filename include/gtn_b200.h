@@ -431,6 +431,40 @@ int gtnb_ngram_ctc_loss(
     int trans_grad_on_device);
 
 /*
+ * Loss over one user-supplied target graph per utterance (the criterion of the reference's pytorch_loss.py and of
+ * its word-decomposition examples):
+ *   loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b))
+ * E_b: linearGraph(T_b, C) on the first T_b = input_lens[b] (or T) rows of emissions_b ([B][T][C]); A_b =
+ * graphs[b], a host view as gtnb_pack takes it, matched on its olabels (= ilabels for an acceptor).  Arcs labelled
+ * outside [0, C) never match (gradient 0); an epsilon arc is GTNB_ERR_UNSUPPORTED (remove(g, epsilon) first).
+ * arc_weights (nullable, [sum_b A_b] in batch order, on the device when arc_weights_on_device) replace the views'
+ * weights.  grads (nullable, d loss_b / d e_b, [B][T][C]): EVERY row is written, 0 beyond T_b.  arc_grads
+ * (nullable, [sum_b A_b]: d loss_b / d A_b's arc weights, Graph arc numbering) is written, not accumulated.
+ * T_b = 0 gives NaN (linearGraph(0, C) accepts nothing); a graph with no accepting path of T_b arcs, or an empty
+ * graph, gives +inf and the denominator's gradient alone.  T_b > T, negative lengths or a malformed view are
+ * GTNB_ERR_INVALID_ARGUMENT.  B = 0 is a no-op.
+ * The frames are swept without building intersect(A_b, E_b) when the graphs fit k_implicit.cu's layout (graphs
+ * whose nodes have in-arcs of different labels: C <= 1024); otherwise, with the "implicit" flag off, or when a
+ * non-finite weight or emission is met, the lattices are materialised.
+ */
+int gtnb_graph_loss(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    float* losses_host,
+    float* grads, /* nullable */
+    int grads_on_device,
+    float* arc_grads, /* nullable */
+    int arc_grads_on_device);
+
+/*
  * viterbiPath + viterbiScore of compose(linearGraph(T, C; e_b), transitions) for a whole
  * minibatch (test/criterion_test.cpp:308-345, BASELINE.json configs[3]) WITHOUT
  * materialising the T*C*C lattice (32.75 M arcs per utterance at T=2000, C=128).
