@@ -306,9 +306,7 @@ class Ctx:
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         tw = np.ascontiguousarray(trans_w, dtype=np.float32)
-        lens = np.asarray([len(t) for t in targets], np.int32)
-        cat = np.ascontiguousarray(
-            np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
+        cat, lens = _cat_targets(targets)
         losses = np.zeros(B, np.float32)
         grads = np.zeros_like(e) if want_grad else None
         tg = np.zeros(Cn + Cn * Cn, np.float32) if want_grad else None
@@ -335,10 +333,7 @@ class Ctx:
         """Host-buffer entry point: emissions [B,T,C] float32 numpy -> (losses, grads)."""
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        lens = np.asarray([len(t) for t in targets], np.int32)
-        cat = (np.concatenate([np.asarray(t, np.int32) for t in targets])
-               if B else np.zeros(0, np.int32))
-        cat = np.ascontiguousarray(cat, np.int32)
+        cat, lens = _cat_targets(targets)
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         losses = np.zeros(B, np.float32)
         grads = np.zeros_like(e) if want_grad else None
@@ -352,8 +347,7 @@ class Ctx:
         in HBM in, gradients in HBM out), downloads the gradients afterwards -> (losses, grads)."""
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        lens = np.asarray([len(t) for t in targets], np.int32)
-        cat = np.ascontiguousarray(np.concatenate([np.asarray(t, np.int32) for t in targets]), np.int32)
+        cat, lens = _cat_targets(targets)
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         losses = np.zeros(B, np.float32)
         e_dev = self.to_device(e)

@@ -32,6 +32,29 @@ def _ctx_for(device, stream):
     return _ctx_cache[key]
 
 
+def _allreduce_transitions(ctx, tg, allreduce):
+    """Sum the transition gradient tg over the ranks when torch.distributed is initialised (the multi-GPU form of
+    Graph::addGrad under grad_lock, graph.cpp:96-100); ctx.world is the number of ranks summed over."""
+    ctx.world = 1
+    if allreduce and torch.distributed.is_available() and torch.distributed.is_initialized():
+        torch.distributed.all_reduce(tg, op=torch.distributed.ReduceOp.SUM)
+        ctx.world = torch.distributed.get_world_size()
+
+
+def _transition_backward(ctx, grad_output):
+    """(emission gradient, transition gradient) of asg_loss / ngram_ctc_loss times the upstream gradient"""
+    grad, tg = ctx.saved_tensors
+    if ctx.reduction == "mean":
+        # the mean over the GLOBAL batch when the transition gradient was summed over the ranks
+        scale = grad_output / ctx.B
+        return grad * scale, tg * (scale / ctx.world)
+    # reduction "none": the incoming gradient is per utterance; the transition gradient was already summed
+    # over the batch inside the kernel, which is only the chain rule's answer for a uniform grad_output
+    assert bool((grad_output == grad_output.flatten()[0]).all()), \
+        "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
+    return grad * grad_output.view(-1, 1, 1), tg * grad_output.flatten()[0]
+
+
 class CTCLossFunction(torch.autograd.Function):
     """loss_b = forwardScore(e_b) - forwardScore(intersect(ctcGraph(target_b), e_b))  (benchmarks/ctc.cpp:150-158).
 
@@ -48,9 +71,7 @@ class CTCLossFunction(torch.autograd.Function):
         B, T, Cn = e.shape
         stream = torch.cuda.current_stream(e.device).cuda_stream
         g = _ctx_for(e.device, stream)
-        lens = np.asarray([len(t) for t in targets], np.int32)
-        cat = np.ascontiguousarray(
-            np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
+        cat, lens = capi._cat_targets(targets)
         il = _lengths(input_lengths, B)
         losses = np.zeros(B, np.float32)
         grad = torch.empty_like(e)  # (with input_lengths the call zeroes the padding rows)
@@ -101,9 +122,7 @@ class ASGLossFunction(torch.autograd.Function):
         assert transitions.numel() == Cn + Cn * Cn
         stream = torch.cuda.current_stream(e.device).cuda_stream
         g = _ctx_for(e.device, stream)
-        lens = np.asarray([len(t) for t in targets], np.int32)
-        cat = np.ascontiguousarray(
-            np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
+        cat, lens = capi._cat_targets(targets)
         losses = np.zeros(B, np.float32)
         if input_lengths is not None:
             assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
@@ -125,10 +144,7 @@ class ASGLossFunction(torch.autograd.Function):
                 lens.ctypes.data_as(capi._i32p), losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
                 tgrad.ctypes.data_as(capi._f32p)))
             tg = torch.from_numpy(tgrad).to(e.device)
-        ctx.world = 1
-        if allreduce and torch.distributed.is_available() and torch.distributed.is_initialized():
-            torch.distributed.all_reduce(tg, op=torch.distributed.ReduceOp.SUM)
-            ctx.world = torch.distributed.get_world_size()
+        _allreduce_transitions(ctx, tg, allreduce)
         out = torch.from_numpy(losses).to(e.device)
         ctx.save_for_backward(grad, tg)
         ctx.reduction = reduction
@@ -138,16 +154,8 @@ class ASGLossFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_output):
-        grad, tg = ctx.saved_tensors
-        if ctx.reduction == "mean":
-            # the mean over the GLOBAL batch when the transition gradient was summed over the ranks
-            scale = grad_output / ctx.B
-            return grad * scale, (tg * (scale / ctx.world)).to(ctx.tdev), None, None, None, None
-        # reduction "none": the incoming gradient is per utterance; the transition gradient was already summed
-        # over the batch inside the kernel, which is only the chain rule's answer for a uniform grad_output
-        assert bool((grad_output == grad_output.flatten()[0]).all()), \
-            "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
-        return grad * grad_output.view(-1, 1, 1), (tg * grad_output.flatten()[0]).to(ctx.tdev), None, None, None, None
+        grad, tg = _transition_backward(ctx, grad_output)
+        return grad, tg.to(ctx.tdev), None, None, None, None
 
 
 def asg_loss(emissions, transitions, targets, reduction="mean", allreduce=True, input_lengths=None):
@@ -177,14 +185,8 @@ class NgramCTCLossFunction(torch.autograd.Function):
         w = transitions.detach().contiguous()
         stream = torch.cuda.current_stream(e.device).cuda_stream
         g = _ctx_for(e.device, stream)
-        lens = np.asarray([len(t) for t in targets], np.int32)
-        cat = np.ascontiguousarray(
-            np.concatenate([np.asarray(t, np.int32) for t in targets]) if B else np.zeros(0, np.int32), np.int32)
-        il = None
-        if input_lengths is not None:
-            il = np.ascontiguousarray(
-                input_lengths.detach().cpu().numpy() if torch.is_tensor(input_lengths) else input_lengths, np.int32)
-            assert il.shape == (B,)
+        cat, lens = capi._cat_targets(targets)
+        il = _lengths(input_lengths, B)
         losses = np.zeros(B, np.float32)
         grad = torch.empty_like(e)  # every row is written by the call
         tg = torch.empty(Cn * Cn, dtype=torch.float32, device=e.device)
@@ -193,10 +195,7 @@ class NgramCTCLossFunction(torch.autograd.Function):
             cat.ctypes.data_as(capi._i32p), lens.ctypes.data_as(capi._i32p), int(blank),
             losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, tg.data_ptr(), 1))
         tg = tg.view_as(transitions)
-        ctx.world = 1
-        if allreduce and torch.distributed.is_available() and torch.distributed.is_initialized():
-            torch.distributed.all_reduce(tg, op=torch.distributed.ReduceOp.SUM)
-            ctx.world = torch.distributed.get_world_size()
+        _allreduce_transitions(ctx, tg, allreduce)
         out = torch.from_numpy(losses).to(e.device)
         ctx.save_for_backward(grad, tg)
         ctx.reduction = reduction
@@ -205,16 +204,8 @@ class NgramCTCLossFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_output):
-        grad, tg = ctx.saved_tensors
-        if ctx.reduction == "mean":
-            # the mean over the GLOBAL batch when the transition gradient was summed over the ranks
-            scale = grad_output / ctx.B
-            return grad * scale, tg * (scale / ctx.world), None, None, None, None, None
-        # reduction "none": as asg_loss, the transition gradient was summed over the batch inside the call, which
-        # is the chain rule's answer only for a uniform upstream gradient
-        assert bool((grad_output == grad_output.flatten()[0]).all()), \
-            "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
-        return grad * grad_output.view(-1, 1, 1), tg * grad_output.flatten()[0], None, None, None, None, None
+        grad, tg = _transition_backward(ctx, grad_output)
+        return grad, tg, None, None, None, None, None
 
 
 def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True):

@@ -1,5 +1,5 @@
 /*
- * tests/emu/asg_emu.cpp -- TEST INFRASTRUCTURE: the device side of gtnb_asg_loss_ex as asg_loss_ex_fast runs it,
+ * tests/emu/asg_emu.cpp -- TEST INFRASTRUCTURE: the device side of gtnb_asg_loss_ex as trellis_loss_fast runs it,
  * from the SOURCE of gtn_b200/csrc/k_ngram.cu (ASG's numerator graphs, the dense trellis in its start mode) and
  * k_implicit.cu (the numerator's sweeps), on the CPU through tests/emu/simt_emu.h.  Only the launch geometry, the
  * table slabs and the scatter of the numerator's arc gradients (launch_scatter_add: dst[map[a]] += src[a]) are

@@ -1,6 +1,6 @@
 /*
  * tests/emu/ngram_emu.cpp -- TEST INFRASTRUCTURE: the device side of gtnb_ngram_ctc_loss as
- * ngram_ctc_loss_fast runs it, from the SOURCE of gtn_b200/csrc/k_ngram.cu (sigma, the folded numerator
+ * trellis_loss_fast runs it, from the SOURCE of gtn_b200/csrc/k_ngram.cu (sigma, the folded numerator
  * graphs, the dense-trellis forward / backward, the sigma fold) and k_implicit.cu (the numerator's sweeps), on
  * the CPU through tests/emu/simt_emu.h.  Only the launch geometry, the table slabs and the scatter of the
  * numerator's arc gradients (launch_scatter_add: dst[map[a]] += src[a]) are restated here.
