@@ -18,6 +18,8 @@ ERR_LOGIC = 3
 ERR_RUNTIME = 4
 ERR_UNSUPPORTED = 5
 EPSILON = -1
+DENSE_ASG = 0  # gtnb_viterbi_dense_ex graph kinds
+DENSE_BIGRAM = 1
 
 _f32p = C.POINTER(C.c_float)
 _i32p = C.POINTER(C.c_int32)
@@ -88,6 +90,8 @@ SYMBOLS = [
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _f32p, _i32p, _i32p, _f32p, _vp, C.c_int, _f32p]),
     ("gtnb_viterbi_dense", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _f32p, _i32p, _f32p]),
+    ("gtnb_viterbi_dense_ex", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int]),
     ("gtnb_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int]),
@@ -328,6 +332,42 @@ class Ctx:
             self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), _p(tw, _f32p), _p(paths, _i32p),
             _p(scores, _f32p)))
         return paths[:, :T], scores[:B]
+
+    def viterbi_dense_ex(self, emissions, trans_w, kind=DENSE_ASG, input_lens=None):
+        """Host-buffer entry of gtnb_viterbi_dense_ex: emissions [B,T,C], trans_w [C + C*C] (DENSE_ASG) or [C*C]
+        (DENSE_BIGRAM) -> (paths [B,T] int32, -1 beyond T_b; scores [B])."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == (Cn * Cn if kind == DENSE_BIGRAM else Cn + Cn * Cn)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        paths = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
+        scores = np.full(max(B, 1), np.nan, np.float32)
+        self._check(lib().gtnb_viterbi_dense_ex(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), int(kind), tw.ctypes.data, 0, paths.ctypes.data,
+            scores.ctypes.data, 0))
+        return paths[:B, :T], scores[:B]
+
+    def viterbi_dense_ex_dev(self, emissions, trans_w, kind=DENSE_ASG, input_lens=None):
+        """Device-buffer entry: emissions and trans_w uploaded once, gtnb_viterbi_dense_ex on device pointers
+        (paths and scores in HBM), downloaded afterwards -> (paths, scores)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == (Cn * Cn if kind == DENSE_BIGRAM else Cn + Cn * Cn)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        e_dev, w_dev = self.to_device(e), self.to_device(tw)
+        p_dev = self.to_device(np.full((max(B, 1), max(T, 1)), -7, np.int32))  # every entry is written
+        s_dev = self.to_device(np.full(max(B, 1), np.nan, np.float32))
+        try:
+            self._check(lib().gtnb_viterbi_dense_ex(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), int(kind), w_dev.ptr, 1, p_dev.ptr, s_dev.ptr, 1))
+            paths = p_dev.download((max(B, 1), max(T, 1)), np.int32)
+            scores = s_dev.download((max(B, 1),))
+        finally:
+            for buf in (e_dev, w_dev, p_dev, s_dev):
+                buf.free()
+        return paths.ravel()[:B * T].reshape(B, T), scores[:B]
 
     def ctc_loss(self, emissions, targets, blank=0, want_grad=True, input_lens=None):
         """Host-buffer entry point: emissions [B,T,C] float32 numpy -> (losses, grads)."""

@@ -569,46 +569,77 @@ extern "C" int gtnb_ctc_loss(
   });
 }
 
+namespace {
+
 /*
- * viterbiPath(compose(linearGraph(T, C; e_b), transitions)) for a whole minibatch, with the
- * dense transitions graph of test/criterion_test.cpp:244-254 / :316-326, through the
- * factored kernel (k_dense.cu): the T*C*C lattice is never materialised.
+ * The body of gtnb_viterbi_dense and gtnb_viterbi_dense_ex: viterbiPath / viterbiScore of the lattice of every
+ * utterance through the factored kernel (k_dense.cu); the T*C*C lattice is never materialised.  Host transitions
+ * and input_lens go up in one staged copy; device transitions are read where they are.  Outputs on the device are
+ * written in place and the call returns once the work is enqueued; host outputs are copied back and waited for.
+ * empty_score: the score of an utterance with T_b = 0.
  * (the device scratch of a call comes from the context's call-scoped arena, as in gtnb_ctc_loss: no stream-ordered
  * allocations on the path after the first call of a shape)
  */
-extern "C" int gtnb_viterbi_dense(
-    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
-    const int32_t* input_lens, const float* trans_w_host, int32_t* paths_host, float* scores_host) {
-  if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions || !trans_w_host)
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_viterbi_dense: bad arguments");
+int viterbi_dense_run(gtnb_ctx* ctx, const char* fn, int B, int T, int C, const float* emissions,
+                      int emissions_on_device, const int32_t* input_lens, bool bigram, const float* trans_w,
+                      int trans_on_device, int32_t* paths, float* scores, int outputs_on_device, float empty_score) {
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions || !trans_w)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
   if (B == 0) return GTNB_OK;
   GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
   if (input_lens)
     for (int b = 0; b < B; b++)
       if (input_lens[b] < 0 || input_lens[b] > T)
-        return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_viterbi_dense: input_lens out of range");
+        return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": input_lens out of range");
   const long long per = (long long)T * C;
+  const long long n_trans = (bigram ? 0 : (long long)C) + (long long)C * C;
   CallScope scope(ctx);
   float *e_dev = nullptr, *tr_dev = nullptr, *sc_dev = nullptr;
   int32_t *T_dev = nullptr, *paths_dev = nullptr;
   uint8_t* bp = nullptr;
   GTNB_TRY(scope.input(emissions, emissions_on_device, per * B, &e_dev));
-  GTNB_TRY(scope.alloc(&tr_dev, (long long)C + (long long)C * C));
-  GTNB_TRY(scope.alloc(&sc_dev, B));
-  GTNB_TRY(scope.alloc(&paths_dev, (long long)B * std::max(T, 1)));
-  GTNB_TRY(scope.alloc(&bp, (long long)B * std::max(T, 1) * C));
+  GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, n_trans, &tr_dev));
+  GTNB_TRY(scope.borrow(scores, scores && outputs_on_device, B, &sc_dev));
+  GTNB_TRY(scope.borrow(paths, paths && outputs_on_device, (long long)B * std::max(T, 1), &paths_dev));
+  GTNB_TRY(scope.alloc(&bp, (long long)B * std::max(T, 1) * dense_bp_pitch(C)));
   if (input_lens) GTNB_TRY(scope.alloc(&T_dev, B));
   GTNB_TRY(stage_begin(ctx));
-  GTNB_TRY(stage_upload(ctx, tr_dev, trans_w_host, sizeof(float) * ((size_t)C + (size_t)C * C)));
+  if (!trans_on_device) GTNB_TRY(stage_upload(ctx, tr_dev, trans_w, sizeof(float) * n_trans));
   if (input_lens) GTNB_TRY(stage_upload(ctx, T_dev, input_lens, sizeof(int32_t) * B));
   GTNB_TRY(stage_end(ctx));
-  GTNB_TRY(launch_viterbi_dense(ctx, B, T, C, T_dev, e_dev, per, tr_dev, bp, paths_dev, sc_dev));
-  if (paths_host && T > 0)
-    GTNB_CUDA(ctx, cudaMemcpyAsync(paths_host, paths_dev, sizeof(int32_t) * (size_t)B * T, cudaMemcpyDeviceToHost,
+  GTNB_TRY(launch_viterbi_dense(ctx, B, T, C, bigram, T_dev, e_dev, per, tr_dev, empty_score, bp, paths_dev, sc_dev));
+  if (outputs_on_device) return GTNB_OK;
+  if (paths && T > 0)
+    GTNB_CUDA(ctx, cudaMemcpyAsync(paths, paths_dev, sizeof(int32_t) * (size_t)B * T, cudaMemcpyDeviceToHost,
                                    ctx->stream));
-  if (scores_host)
-    GTNB_CUDA(ctx, cudaMemcpyAsync(scores_host, sc_dev, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+  if (scores)
+    GTNB_CUDA(ctx, cudaMemcpyAsync(scores, sc_dev, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
   return scope.sync();
+}
+
+} // namespace
+
+/*
+ * viterbiPath(compose(linearGraph(T, C; e_b), transitions)) for a whole minibatch, with the
+ * dense transitions graph of test/criterion_test.cpp:244-254 / :316-326: the ASG kind of
+ * gtnb_viterbi_dense_ex with host transitions and host outputs, except that T_b = 0 scores 0.
+ */
+extern "C" int gtnb_viterbi_dense(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
+    const int32_t* input_lens, const float* trans_w_host, int32_t* paths_host, float* scores_host) {
+  return viterbi_dense_run(ctx, "gtnb_viterbi_dense", B, T, C, emissions, emissions_on_device, input_lens, false,
+                           trans_w_host, 0, paths_host, scores_host, 0, 0.0f);
+}
+
+extern "C" int gtnb_viterbi_dense_ex(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    int kind, const float* trans_w, int trans_on_device, int32_t* paths, float* scores, int outputs_on_device) {
+  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_viterbi_dense_ex: unknown graph kind");
+  // T_b = 0: linearGraph(0, C) is one start node that does not accept (creations.cpp:20-33): no path, score -inf
+  return viterbi_dense_run(ctx, "gtnb_viterbi_dense_ex", B, T, C, emissions, emissions_on_device, input_lens,
+                           kind == GTNB_DENSE_BIGRAM, trans_w, trans_on_device, paths, scores, outputs_on_device,
+                           -std::numeric_limits<float>::infinity());
 }
 
 namespace {

@@ -340,9 +340,12 @@ int compose_linear_impl(
     bool arc_labels = false, const float* arc_weights_dev = nullptr);
 int validate_view(gtnb_ctx* ctx, const gtnb_graph_view& v);
 int ensure_side_streams(gtnb_ctx* ctx, int n_streams, int n_events);
+// kernel (k_dense.cu): factored dense-trellis Viterbi.  bigram: trans_dev is n-gram CTC's [C*C] W (every state
+// starts), else ASG's [C + C*C]; bp holds [B][T_max][dense_bp_pitch(C)] bytes; 1 <= C <= 224
+int dense_bp_pitch(int C);
 int launch_viterbi_dense(
-    gtnb_ctx* ctx, int B, int T_max, int C, const int32_t* T_dev, const float* emis, int64_t stride,
-    const float* trans_dev, uint8_t* bp, int32_t* paths, float* scores);
+    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const float* emis, int64_t stride,
+    const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores);
 // kernels (k_ngram.cu): CTC with a learned bigram transition graph
 constexpr int kNgramMaxLabels = 128;
 int launch_ngram_sigma(gtnb_ctx* ctx, int C, const float* W, float* sigma);

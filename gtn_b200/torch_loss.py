@@ -212,6 +212,70 @@ def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0,
     return NgramCTCLossFunction.apply(emissions, transitions, targets, input_lengths, blank, reduction, allreduce)
 
 
+@torch.no_grad()
+def _viterbi_dense(emissions, transitions, input_lengths, kind):
+    assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+    assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+    w = transitions.detach().contiguous()
+    current = torch.cuda.current_stream(e.device)
+    g = _ctx_for(e.device, current.cuda_stream)
+    il = _lengths(input_lengths, B)
+    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)  # every entry is written by the call
+    scores = torch.empty(B, dtype=torch.float32, device=e.device)
+    # the call returns once its work is enqueued on the context's stream, which is the current stream unless that
+    # is the legacy default stream (the context then has a stream of its own): order the two both ways
+    ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(g.h), device=e.device)
+    ctx_stream.wait_stream(current)
+    g._check(capi.lib().gtnb_viterbi_dense_ex(
+        g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), kind, w.data_ptr(), 1,
+        paths.data_ptr(), scores.data_ptr(), 1))
+    current.wait_stream(ctx_stream)
+    return paths, scores
+
+
+def asg_viterbi(emissions, transitions, input_lengths=None):
+    """Best path of compose(E_b, transitions) for every utterance, with the transitions asg_loss trains
+    (examples/asg.cpp's decoding, test/criterion_test.cpp:328-344), through gtnb_viterbi_dense_ex.
+
+    emissions: float32 CUDA tensor [B, T, C]; transitions: float32 CUDA tensor of C + C*C elements (start weights,
+    then the C x C matrix, row = destination label) on the same device; input_lengths: None, a list or an int tensor
+    (any device).  Returns (paths [B, T] int32, the label of every frame, -1 beyond T_b; scores [B], viterbiScore,
+    -inf for T_b = 0), both CUDA tensors written on the current stream; only input_lengths visits the host.
+    """
+    return _viterbi_dense(emissions, transitions, input_lengths, capi.DENSE_ASG)
+
+
+def ngram_ctc_viterbi(emissions, transitions, input_lengths=None):
+    """Best path of intersect(E_b, G) for every utterance, G the bigram transition graph ngram_ctc_loss trains,
+    through gtnb_viterbi_dense_ex.  transitions: float32 CUDA tensor of C*C elements ([C, C] or flat, row =
+    destination label).  The arguments and results are those of asg_viterbi; collapse(paths, blank) gives the
+    transcript.
+    """
+    return _viterbi_dense(emissions, transitions, input_lengths, capi.DENSE_BIGRAM)
+
+
+@torch.no_grad()
+def collapse(paths, blank=None):
+    """Transcripts of frame-level paths: repeats merged, then `blank` dropped when one is given (CTC's rule; with
+    blank=None, ASG's).  paths: int tensor [B, T], -1 padding.  Returns (labels [B, T] int32, each row's transcript
+    followed by -1, lengths [B] int64), on the paths' device, without a host synchronisation."""
+    p = paths.int()
+    B, T = p.shape
+    keep = p >= 0
+    keep[:, 1:] &= p[:, 1:] != p[:, :-1]
+    if blank is not None:
+        keep &= p != blank
+    lengths = keep.sum(dim=1)
+    # the kept labels of a row go to the front: slot = number of kept labels before them
+    slot = torch.where(keep, keep.cumsum(dim=1) - 1, T)
+    out = torch.full((B, T + 1), -1, dtype=torch.int32, device=p.device)
+    out.scatter_(1, slot, torch.where(keep, p, -1))
+    return out[:, :T].contiguous(), lengths
+
+
 def _graph_view(g):
     """capi view of a gtn_b200.gtn.Graph built on the host, in its own arc-list order"""
     from . import _gtn

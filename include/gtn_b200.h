@@ -472,7 +472,10 @@ int gtnb_graph_loss(
  * accept, arcs 0 -> i+1 (label i, weight trans_w[i]) and j+1 -> i+1 (label i, weight
  * trans_w[C + i*C + j]).  paths_host [B][T]: the best path's labels (-1 where there is no
  * accepting path / beyond input_lens[b]); scores_host [B]: viterbiScore.  Paths are
- * bit-identical to the reference's, ties included.  Needs C <= 256, C % 4 == 0.
+ * bit-identical to the reference's, ties included.  Needs C <= 224 (GTNB_ERR_UNSUPPORTED
+ * above: the C x C weights are held in shared memory).  The ASG kind of gtnb_viterbi_dense_ex
+ * with host transitions and host outputs, with one known deviation from the reference kept
+ * for compatibility: an utterance with input_lens[b] = 0 scores 0 here, -inf there.
  */
 int gtnb_viterbi_dense(
     gtnb_ctx* ctx,
@@ -485,6 +488,44 @@ int gtnb_viterbi_dense(
     const float* trans_w_host,
     int32_t* paths_host,
     float* scores_host);
+
+/* graph kinds of gtnb_viterbi_dense_ex */
+#define GTNB_DENSE_ASG 0 /* trans_w [C + C*C]: start weights, then W; gtnb_asg_loss_ex's layout */
+#define GTNB_DENSE_BIGRAM 1 /* trans_w [C*C]: W alone, every state starts; gtnb_ngram_ctc_loss's layout */
+
+/*
+ * Batched Viterbi decoding with the learned transitions of gtnb_asg_loss_ex (kind GTNB_DENSE_ASG) or
+ * gtnb_ngram_ctc_loss (kind GTNB_DENSE_BIGRAM), without materialising the T*C*C lattice:
+ *   ASG:    viterbiPath / viterbiScore of compose(E_b, transitions), transitions as at gtnb_viterbi_dense;
+ *   BIGRAM: viterbiPath / viterbiScore of intersect(E_b, G), G as at gtnb_ngram_ctc_loss (C nodes, every node
+ *           start and accept, arc j -> i with label i and weight trans_w[i*C + j]).
+ * E_b: linearGraph(T_b, C) on the first T_b = input_lens[b] (or T) rows of emissions_b ([B][T][C]); rows t >= T_b
+ * are never read.  trans_w lives on the device when trans_on_device (read in place on the context's stream, never
+ * copied to the host), else on the host; likewise emissions.  paths ([B][T], nullable): the labels of the best
+ * path, -1 beyond T_b and where there is no accepting path; EVERY entry is written.  scores ([B], nullable):
+ * viterbiScore, -inf without an accepting path.  Both live on the device when outputs_on_device: the call then
+ * returns once the work is enqueued on the context's stream; host outputs are complete when it returns.
+ * Ties go to the reference's choice (the smallest predecessor state, then the first best final state), so paths
+ * and scores equal the reference's for finite emissions and finite or -inf weights (-inf forbids a transition).
+ * NaN is never chosen as a maximum, so a NaN acts like -inf; the reference propagates it instead.
+ * T_b = 0 gives score -inf and an all -1 path (linearGraph(0, C) accepts nothing).  Needs 1 <= C <= 224
+ * (GTNB_ERR_UNSUPPORTED above); an unknown kind, input_lens outside [0, T] or a NULL ctx, emissions or trans_w is
+ * GTNB_ERR_INVALID_ARGUMENT.  B = 0 is a no-op.
+ */
+int gtnb_viterbi_dense_ex(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    int kind,
+    const float* trans_w,
+    int trans_on_device,
+    int32_t* paths, /* nullable */
+    float* scores, /* nullable */
+    int outputs_on_device);
 
 #ifdef __cplusplus
 }
