@@ -28,19 +28,9 @@
  * Not applicable (status bit 2 -> the caller repeats the call through the other kernels): an
  * in-arc from outside the band, two in-arcs from the same source, in-degree > 3.
  */
-#ifdef GTNB_HOST_EMU // the kernels below compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include <algorithm>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -49,75 +39,9 @@ namespace {
 constexpr int kBandPf = 8; // frames per register prefetch block (see k_implicit.cu)
 constexpr int kBandMaxThreads = 512; // 16 warps: leaves 128 registers per thread
 
-__device__ __forceinline__ float b_ninf() {
-  return -CUDART_INF_F;
-}
-__device__ __forceinline__ bool b_finite(float x) {
-  return fabsf(x) < CUDART_INF_F;
-}
-#ifdef GTNB_HOST_EMU
-__device__ __forceinline__ float b_iexp(float x) {
-  return exp2f(x * 1.4426950408889634f);
-}
-__device__ __forceinline__ float b_lg2(float x) {
-  return log2f(x);
-}
-__device__ __forceinline__ void b_ldg_if(bool p, float& dst, const float* src) {
-  if (p) dst = *src;
-}
-__device__ __forceinline__ void b_ldg_keep(float& dst, const float* src) {
-  dst = *src;
-}
-__device__ __forceinline__ void b_red_if(bool p, float* dst, float v) {
-  if (p) atomicAdd(dst, v);
-}
-#else
-__device__ __forceinline__ float b_iexp(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x * 1.4426950408889634f));
-  return y;
-}
-__device__ __forceinline__ float b_lg2(float x) {
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void b_ldg_if(bool p, float& dst, const float* src) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "setp.ne.s32 q, %2, 0;\n"
-      "@q ld.global.nc.f32 %0, [%1];\n"
-      "}\n"
-      : "+f"(dst)
-      : "l"(src), "r"((int)p));
-}
-__device__ __forceinline__ void b_ldg_keep(float& dst, const float* src) {
-  asm volatile("ld.relaxed.cta.global.f32 %0, [%1];" : "=f"(dst) : "l"(src) : "memory");
-}
-__device__ __forceinline__ void b_red_if(bool p, float* dst, float v) {
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "setp.ne.s32 q, %2, 0;\n"
-      "@q red.global.add.f32 [%0], %1;\n"
-      "}\n" ::"l"(dst),
-      "f"(v), "r"((int)p)
-      : "memory");
-}
-#endif
-/* as lse3 of k_implicit.cu */
-__device__ __forceinline__ float b_lse3(float v0, float v1, float v2) {
-  const float mx = fmaxf(fmaxf(v0, v1), v2);
-  const float sum = (b_iexp(v0 - mx) + b_iexp(v1 - mx)) + b_iexp(v2 - mx);
-  const float r = fmaf(b_lg2(sum), 0.6931471805599453f, mx);
-  return (fabsf(mx) == CUDART_INF_F) ? mx : r;
-}
-
 /* CTA-wide max / sum for any number of warps <= 32; `red` holds 32 floats */
 __device__ __forceinline__ float b_block_max(float v, float* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  v = warp_max(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
@@ -126,8 +50,7 @@ __device__ __forceinline__ float b_block_max(float v, float* red) {
   return r;
 }
 __device__ __forceinline__ float b_block_sum(float v, float* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  v = warp_sum(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
@@ -150,7 +73,7 @@ __device__ __forceinline__ BandNode load_band_node(
     const int32_t* __restrict__ sg_in_label, const float* __restrict__ sg_in_w, bool& bad,
     bool& unsupported) {
   BandNode b;
-  b.w0 = b.w1 = b.w2 = b_ninf();
+  b.w0 = b.w1 = b.w2 = neg_inf();
   b.label = 0;
   b.has = false;
   b.flags = 0;
@@ -164,7 +87,7 @@ __device__ __forceinline__ BandNode load_band_node(
   for (int a = e0; a < e1; a++) {
     const int d = n - sg_in_src[m.sg_arc_base + a];
     const float w = sg_in_w[m.sg_arc_base + a];
-    bad |= !b_finite(w);
+    bad |= !is_finite(w);
     if (d < 0 || d > 2 || ((seen >> d) & 1u)) {
       unsupported = true;
       continue;
@@ -217,7 +140,7 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_forward_kernel(
   const float* eml = emissions + m.emis_off + bn.label;
 
   // frame 0: start nodes carry the implicit 0 (shortest.cpp:129-135)
-  float s = (ok && (bn.flags & 1)) ? 0.0f : b_ninf();
+  float s = (ok && (bn.flags & 1)) ? 0.0f : neg_inf();
   if (own) {
     sc[n] = s;
     row0[n] = s;
@@ -241,7 +164,7 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_forward_kernel(
     const float e = has ? pf[idx] : 0.0f;                                             \
     const float s1 = __shfl_up_sync(0xffffffffu, s, 1);                               \
     const float s2 = __shfl_up_sync(0xffffffffu, s, 2);                               \
-    s = b_lse3(s + (w0 + e), s1 + (w1 + e), s2 + (w2 + e));                           \
+    s = lse3(s + (w0 + e), s1 + (w1 + e), s2 + (w2 + e));                           \
     chk = fmaf(e, 0.0f, chk);                                                         \
     if (own) *grow = s;                                                               \
     grow += pitch;                                                                    \
@@ -251,9 +174,9 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_forward_kernel(
     _Pragma("unroll") for (int j = 0; j < kBandPf; j++) pf[j] = nx[j];                \
     _Pragma("unroll") for (int j = 0; j < kBandPf; j++) {                             \
       if (GUARDED)                                                                    \
-        b_ldg_if(has && f0 + 2 * kBandPf + j < T, nx[j], epf + (long long)j * C);     \
+        ldg_if(has && f0 + 2 * kBandPf + j < T, nx[j], epf + (long long)j * C);     \
       else                                                                            \
-        b_ldg_keep(nx[j], epf + (long long)j * C);                                    \
+        ldg_keep(nx[j], epf + (long long)j * C);                                    \
     }                                                                                 \
     epf += (long long)kBandPf * C;                                                    \
   }
@@ -263,7 +186,7 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_forward_kernel(
   for (; f0 + 3 * kBandPf <= T; f0 += kBandPf) {
 #pragma unroll
     for (int kb = 0; kb < kBandPf / K; kb++) {
-      if (lane < H) s = ok ? rd[n] : b_ninf(); // the halo re-reads the neighbour warp's nodes
+      if (lane < H) s = ok ? rd[n] : neg_inf(); // the halo re-reads the neighbour warp's nodes
 #pragma unroll
       for (int j = 0; j < K; j++) GTNB_BAND_FWD_FRAME(kb * K + j)
       if (own) wr[n] = s;
@@ -279,7 +202,7 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_forward_kernel(
 #pragma unroll
     for (int kb = 0; kb < kBandPf / K; kb++) {
       if (f0 + kb * K >= T) break; // uniform over the CTA
-      if (lane < H) s = ok ? rd[n] : b_ninf();
+      if (lane < H) s = ok ? rd[n] : neg_inf();
 #pragma unroll
       for (int j = 0; j < K; j++) {
         if (f0 + kb * K + j < T) GTNB_BAND_FWD_FRAME(kb * K + j)
@@ -299,7 +222,7 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_forward_kernel(
 
   // accept nodes of the last frame (shortest.cpp:147-159); every node is owned by one lane
   const bool acc = own && (bn.flags & 2);
-  const float sT = acc ? fin[n] : b_ninf();
+  const float sT = acc ? fin[n] : neg_inf();
   const float mx = b_block_max(sT, red);
   float out = mx;
   if (mx != CUDART_INF_F && mx != -CUDART_INF_F) {
@@ -351,16 +274,16 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_backward_kernel(
   const bool has = bn.has;
 
   const float out = out_scores[blockIdx.x];
-  if (!b_finite(out) || T < 1) return; // no accepting path: no gradient (uniform over the CTA)
+  if (!is_finite(out) || T < 1) return; // no accepting path: no gradient (uniform over the CTA)
   const float delta = deltas ? deltas[blockIdx.x] : 1.0f;
   const float* scu = scores + m.node_base + (ok ? n : 0);
   const float* eml = emissions + m.emis_off + bn.label;
   float* gl = grad_emis + (long long)blockIdx.x * grad_stride + (long long)(T - 1) * C + bn.label;
 
   // seeds: nodeGrad[accept] = exp(score - maxA) / exp(out - maxA) (shortest.cpp:49-60)
-  float s_t = ok ? __ldg(scu + (long long)T * pitch) : b_ninf(); // S_T[n]
+  float s_t = ok ? __ldg(scu + (long long)T * pitch) : neg_inf(); // S_T[n]
   const bool acc = ok && (bn.flags & 2);
-  const float mxa = b_block_max((own && acc) ? s_t : b_ninf(), red);
+  const float mxa = b_block_max((own && acc) ? s_t : neg_inf(), red);
   const float denom = expf(out - mxa);
   float G = acc ? expf(s_t - mxa) / denom : 0.0f; // every lane seeds its own node, halo included
 
@@ -369,7 +292,7 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_backward_kernel(
 #pragma unroll
   for (int j = 0; j < kBandPf; j++) {
     const int f = T - 1 - j;
-    nxs[j] = (ok && f >= 0) ? __ldg(scu + (long long)f * pitch) : b_ninf();
+    nxs[j] = (ok && f >= 0) ? __ldg(scu + (long long)f * pitch) : neg_inf();
     nxe[j] = (has && f >= 0) ? __ldg(eml + (long long)f * C) : 0.0f;
   }
   const float* spf = scu + (long long)(T - 1 - kBandPf) * pitch; // only dereferenced while >= row 0
@@ -384,12 +307,12 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_backward_kernel(
     const float sp2 = __shfl_up_sync(0xffffffffu, s_p, 2);                            \
     /* a node that does not exist (score -inf) gets exp(-inf) = 0 on all its arcs */  \
     const float se = (s_t == -CUDART_INF_F) ? CUDART_INF_F : s_t;                     \
-    const float c0 = G * b_iexp(s_p + (w0 + e) - se);                                 \
-    const float c1 = G * b_iexp(sp1 + (w1 + e) - se);                                 \
-    const float c2 = G * b_iexp(sp2 + (w2 + e) - se);                                 \
+    const float c0 = G * fexp(s_p + (w0 + e) - se);                                 \
+    const float c1 = G * fexp(sp1 + (w1 + e) - se);                                 \
+    const float c2 = G * fexp(sp2 + (w2 + e) - se);                                 \
     const float acc_e = (c0 + c1) + c2;                                               \
     G = (c0 + __shfl_down_sync(0xffffffffu, c1, 1)) + __shfl_down_sync(0xffffffffu, c2, 2); \
-    b_red_if(own && acc_e != 0.0f, gl, acc_e * delta);                                \
+    red_if(own && acc_e != 0.0f, gl, acc_e * delta);                                \
     gl -= C;                                                                          \
     s_t = s_p;                                                                        \
   }
@@ -402,11 +325,11 @@ __global__ void __launch_bounds__(kBandMaxThreads, 1) banded_backward_kernel(
     _Pragma("unroll") for (int j = 0; j < kBandPf; j++) {                             \
       if (GUARDED) {                                                                  \
         const bool inb = T - 1 - (i0 + kBandPf + j) >= 0;                             \
-        b_ldg_if(ok && inb, nxs[j], spf - (long long)j * pitch);                      \
-        b_ldg_if(has && inb, nxe[j], epf - (long long)j * C);                         \
+        ldg_if(ok && inb, nxs[j], spf - (long long)j * pitch);                      \
+        ldg_if(has && inb, nxe[j], epf - (long long)j * C);                         \
       } else {                                                                        \
-        b_ldg_keep(nxs[j], spf - (long long)j * pitch);                               \
-        b_ldg_keep(nxe[j], epf - (long long)j * C);                                   \
+        ldg_keep(nxs[j], spf - (long long)j * pitch);                               \
+        ldg_keep(nxe[j], epf - (long long)j * C);                                   \
       }                                                                               \
     }                                                                                 \
     spf -= (long long)kBandPf * pitch;                                                \

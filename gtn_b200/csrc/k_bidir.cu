@@ -66,20 +66,9 @@
  * arc.  Requires: <= 224 graph nodes, in- and out-degree <= 3, one label per node (CTC, forced alignment),
  * C a multiple of 4 and <= 128, 16-byte aligned emissions.  Anything else takes k_implicit.cu.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtn_b200.h"
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include <algorithm>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -104,8 +93,6 @@ constexpr int kSlots = 4; // posterior slots per label in a row of the helpers' 
 constexpr int kMaxHeavy = 4; // labels carried by more than kSlots nodes that get the cooperative sum
 constexpr float kNeg = -1.0e30f; // "this node does not exist" (finite: absorbs every later add)
 constexpr float kHuge = 1.0e29f; // inputs at or above this magnitude take the exact (materialised) path
-constexpr float kLog2e = 1.4426950408889634f;
-constexpr float kLn2 = 0.6931471805599453f;
 constexpr int kIntMin = -2147483647 - 1;
 // FX kernels (C == 64 or 128): the saved-score rows in HBM, the rows of their shared-memory stages and the
 // overflow area of a posterior row all have this many floats, whatever the utterance's node count -- which makes
@@ -174,267 +161,6 @@ struct Params {
   Layout lay;
 };
 
-/* ------------------------------------------------------------------ */
-/* PTX helpers (restated for the host emulation of tests/emu)          */
-/* ------------------------------------------------------------------ */
-#ifdef GTNB_HOST_EMU
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return emu::shared_window(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
-  emu::mbar_init(bar, count);
-}
-__device__ __forceinline__ void mbar_init_fence() {}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  emu::mbar_expect_tx(bar, bytes);
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  emu::mbar_arrive(bar);
-}
-__device__ __forceinline__ void mbar_arrive_n(uint32_t bar, int n) {
-  emu::mbar_arrive_n(bar, n);
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  emu::mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-  emu::mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  emu::bulk_g2s(dst, src, bytes, bar);
-}
-__device__ __forceinline__ void bar_named(int id, int nthreads) {
-  emu::named_barrier(id, nthreads);
-}
-__device__ __forceinline__ float lds(uint32_t addr) {
-  return *emu::shared_ptr<float>(addr);
-}
-__device__ __forceinline__ void sts(uint32_t addr, float v) {
-  *emu::shared_ptr<float>(addr) = v;
-}
-__device__ __forceinline__ uint32_t lds_u(uint32_t addr) {
-  return *emu::shared_ptr<uint32_t>(addr);
-}
-__device__ __forceinline__ void sts_u(uint32_t addr, uint32_t v) {
-  *emu::shared_ptr<uint32_t>(addr) = v;
-}
-__device__ __forceinline__ float4 lds_v4(uint32_t addr) {
-  return *emu::shared_ptr<float4>(addr);
-}
-struct f2 {
-  float x, y;
-};
-__device__ __forceinline__ f2 lds_v2(uint32_t addr) {
-  f2 v;
-  v.x = *emu::shared_ptr<float>(addr);
-  v.y = *emu::shared_ptr<float>(addr + 4);
-  return v;
-}
-__device__ __forceinline__ void sts_v2(uint32_t addr, float a, float b) {
-  *emu::shared_ptr<float>(addr) = a;
-  *emu::shared_ptr<float>(addr + 4) = b;
-}
-__device__ __forceinline__ void stg_v2(float* p, float a, float b) {
-  p[0] = a;
-  p[1] = b;
-}
-__device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {
-  return *emu::shared_ptr<uint16_t>(addr);
-}
-__device__ __forceinline__ void sts_u16(uint32_t addr, uint32_t v) {
-  *emu::shared_ptr<uint16_t>(addr) = (uint16_t)v;
-}
-__device__ __forceinline__ int lds_s8(uint32_t addr) {
-  return *emu::shared_ptr<int8_t>(addr);
-}
-__device__ __forceinline__ void sts_s8(uint32_t addr, int v) {
-  *emu::shared_ptr<int8_t>(addr) = (int8_t)v;
-}
-__device__ __forceinline__ void smem_max_s32(uint32_t addr, int v) {
-  std::atomic_ref<int32_t> a(*emu::shared_ptr<int32_t>(addr));
-  int32_t cur = a.load();
-  while (cur < v && !a.compare_exchange_weak(cur, v)) {
-  }
-}
-__device__ __forceinline__ void stg_v4(float* p, float4 v) {
-  *reinterpret_cast<float4*>(p) = v;
-}
-__device__ __forceinline__ float ex2(float x) {
-  return exp2f(x);
-}
-__device__ __forceinline__ float lg2(float x) {
-  return log2f(x);
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  emu::cluster_sync();
-}
-__device__ __forceinline__ void cluster_arrive_only() {
-  emu::cluster_arrive();
-}
-__device__ __forceinline__ void cluster_wait_only() {
-  emu::cluster_wait();
-}
-__device__ __forceinline__ unsigned cluster_rank() {
-  return emu::cluster_ctarank();
-}
-__device__ __forceinline__ void fence_proxy_async() {}
-__device__ __forceinline__ void stg(float* p, float v) {
-  *p = v;
-}
-#else
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_init_fence() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-/* n arrivals at once (a node warp arriving on behalf of the helper warps in the phases they sit out) */
-__device__ __forceinline__ void mbar_arrive_n(uint32_t bar, int n) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-/* for the warps that wait a whole block ahead of the math: the try_wait suspends the thread in hardware for up
- * to the hinted time (ns) and wakes it when the phase completes -- no issue slots spent polling (as a nanosleep
- * loop would) */
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  do {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(bar), "r"(parity), "r"(20000u)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void bar_named(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ float lds(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts(uint32_t addr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t lds_u(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts_u(uint32_t addr, uint32_t v) {
-  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ float4 lds_v4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-struct f2 {
-  float x, y;
-};
-__device__ __forceinline__ f2 lds_v2(uint32_t addr) {
-  f2 v;
-  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts_v2(uint32_t addr, float a, float b) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ void stg_v2(float* p, float a, float b) {
-  asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ uint32_t lds_u16(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts_u16(uint32_t addr, uint32_t v) {
-  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ int lds_s8(uint32_t addr) {
-  int v;
-  asm volatile("ld.shared.s8 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts_s8(uint32_t addr, int v) {
-  asm volatile("st.shared.u8 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void smem_max_s32(uint32_t addr, int v) { // native ATOMS.MAX.S32
-  asm volatile("red.shared.max.s32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
-__device__ __forceinline__ void stg_v4(float* p, float4 v) {
-  asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float lg2(float x) {
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-/* barrier.cluster: arrive has release, wait has acquire semantics at cluster scope -- the saved scores
- * a CTA stored before it are visible to its partner after it */
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-/* the split form for the producer warp, which has nothing to publish and nothing to acquire: it arrives
- * before its copy loop (so that the others' barrier never waits for it) and waits after it */
-__device__ __forceinline__ void cluster_arrive_only() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void cluster_wait_only() {
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ unsigned cluster_rank() {
-  unsigned r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-/* orders generic-proxy accesses (the partner's stores to global memory, this CTA's reads / writes of a
- * shared-memory stage) before the async-proxy copies issued next */
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async;" ::: "memory");
-}
-__device__ __forceinline__ void stg(float* p, float v) {
-  asm volatile("st.global.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
-}
-#endif
-
 __device__ __forceinline__ bool finite_ok(float x) {
   return fabsf(x) < kHuge;
 }
@@ -443,14 +169,14 @@ __device__ __forceinline__ bool finite_ok(float x) {
  * kNeg + lg2(3) = kNeg (absorbed).  max + lg2(1 + 2^(x1 - max) + 2^(x2 - max)) over the two scores that are not
  * the maximum: 3 MUFU instead of 4 -- the SFU was the busiest pipe of these kernels when profiled on an earlier GPU
  * target (not re-measured on the H100), the ALU that sorts the three was not */
-__device__ __forceinline__ float lse3(float a, float b, float c) {
+__device__ __forceinline__ float lse3_log2(float a, float b, float c) {
   const float lo = fminf(a, b), hi = fmaxf(a, b);
   const float m = fmaxf(hi, c), x1 = fminf(hi, c);
   return m + lg2(1.0f + (ex2(x1 - m) + ex2(lo - m)));
 }
 
 /* logsumexp of two scores */
-__device__ __forceinline__ float lse2(float a, float b) { // max + lg2(1 + 2^-|a - b|): 2 MUFU
+__device__ __forceinline__ float lse2_log2(float a, float b) { // max + lg2(1 + 2^-|a - b|): 2 MUFU
   return fmaxf(a, b) + lg2(1.0f + ex2(-fabsf(a - b)));
 }
 
@@ -496,12 +222,12 @@ __device__ __forceinline__ void publish_block_max(S& st, float stored) {
   // two words, used alternately: the one the NEXT block will publish into is reset here (every thread
   // has read it at the start of this block, many barriers ago)
   if ((threadIdx.x & 31) == 0) smem_max_s32(st.redi, wm);
-  if (threadIdx.x == 0) sts_u(st.redi ^ 4u, (uint32_t)kIntMin);
+  if (threadIdx.x == 0) sts_u32(st.redi ^ 4u, (uint32_t)kIntMin);
 }
 /* at the start of the next block: the adjustment every node thread applies (same value in all of them) */
 template <class S>
 __device__ __forceinline__ void fetch_block_adjust(S& st) {
-  const int mx = (int)lds_u(st.redi);
+  const int mx = (int)lds_u32(st.redi);
   st.redi ^= 4u;
   // nothing alive (or nothing published yet): no adjustment
   const float off = (mx <= -2000000000) ? 0.0f : (float)mx;
@@ -528,22 +254,24 @@ template <int DIR, int PH, bool ZW, int NQ, bool FX>
 __device__ __forceinline__ void node_step(NodeState& st, const NodeUni& un, int r, bool last) {
   using SD = Strd<NQ, FX>;
   const int rr = DIR ? -r : r;
-  const float x = lds(st.ea + (uint32_t)(rr * SD::c4(un)));
+  const float x = lds_f32(st.ea + (uint32_t)(rr * SD::c4(un)));
   // ZW: every arc weight of the graph is 0 (CTC, forced alignment): no adds
-  const float v = ZW ? lse3(lds(st.pc + st.so0), lds(st.pc + st.so1), lds(st.pc + st.so2))
-                     : lse3(lds(st.pc + st.so0) + st.w0, lds(st.pc + st.so1) + st.w1, lds(st.pc + st.so2) + st.w2);
+  const float v = ZW ? lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2))
+                     : lse3_log2(lds_f32(st.pc + st.so0) + st.w0, lds_f32(st.pc + st.so1) + st.w1,
+                                 lds_f32(st.pc + st.so2) + st.w2);
   // A: alpha_s = v + e[s-1][label(u)].  B: beta_s = v; what the predecessors read is beta_s + e[s-1][label(u)]
   const float val = DIR == 0 ? v + fmaf(x, kLog2e, -st.adj) : v - st.adj;
   const float stored = DIR == 0 ? val : fmaf(x, kLog2e, val);
   st.adj = 0.0f;
-  sts(st.qc + st.u4, stored);
+  sts_f32(st.qc + st.u4, stored);
   if (PH == 2) {
     // the posterior, written into the node's slot of the helpers' block
-    sts(st.ga + (uint32_t)(rr * SD::g4(un)), ex2(((val - st.Zh) + lds(st.oa + (uint32_t)(rr * SD::p4(un)))) - st.zsub));
+    sts_f32(st.ga + (uint32_t)(rr * SD::g4(un)),
+            ex2(((val - st.Zh) + lds_f32(st.oa + (uint32_t)(rr * SD::p4(un)))) - st.zsub));
   }
   if (last) publish_block_max(st, stored);
   bar_named(1, un.nact);
-  if (PH == 1) stg(st.gs + rr * SD::pitch(un), val); // after the barrier: nothing waits for it
+  if (PH == 1) stg_f32(st.gs + rr * SD::pitch(un), val); // after the barrier: nothing waits for it
   const uint32_t t = st.pc;
   st.pc = st.qc;
   st.qc = t;
@@ -565,22 +293,20 @@ __device__ __forceinline__ void node_rows(NodeState& st, const NodeUni& un, int 
 
 /* reduction over the node threads of the CTA (named barrier 1): max, then sum */
 __device__ __forceinline__ float node_reduce_max(float v, uint32_t red, int warp, int nwarps, int nact) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if ((threadIdx.x & 31) == 0) sts(red + 4u * warp, v);
+  v = warp_max(v);
+  if ((threadIdx.x & 31) == 0) sts_f32(red + 4u * warp, v);
   bar_named(1, nact);
-  float r = lds(red);
-  for (int w = 1; w < nwarps; w++) r = fmaxf(r, lds(red + 4u * w));
+  float r = lds_f32(red);
+  for (int w = 1; w < nwarps; w++) r = fmaxf(r, lds_f32(red + 4u * w));
   bar_named(1, nact);
   return r;
 }
 __device__ __forceinline__ float node_reduce_sum(float v, uint32_t red, int warp, int nwarps, int nact) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) sts(red + 4u * warp, v);
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) sts_f32(red + 4u * warp, v);
   bar_named(1, nact);
-  float r = lds(red);
-  for (int w = 1; w < nwarps; w++) r += lds(red + 4u * w);
+  float r = lds_f32(red);
+  for (int w = 1; w < nwarps; w++) r += lds_f32(red + 4u * w);
   bar_named(1, nact);
   return r;
 }
@@ -598,15 +324,16 @@ __device__ __forceinline__ void node_first_phase2(
     NodeState& st, const NodeUni& un, bool act, uint32_t red, int warp, int nwarps, float doth, bool last,
     float* z_out, uint32_t feas_a, uint32_t spare) {
   using SD = Strd<NQ, FX>;
-  const float x = lds(st.ea);
+  const float x = lds_f32(st.ea);
   st.ea += DIR ? -SD::c4(un) : SD::c4(un);
-  const float v = ZW ? lse3(lds(st.pc + st.so0), lds(st.pc + st.so1), lds(st.pc + st.so2))
-                     : lse3(lds(st.pc + st.so0) + st.w0, lds(st.pc + st.so1) + st.w1, lds(st.pc + st.so2) + st.w2);
+  const float v = ZW ? lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2))
+                     : lse3_log2(lds_f32(st.pc + st.so0) + st.w0, lds_f32(st.pc + st.so1) + st.w1,
+                                 lds_f32(st.pc + st.so2) + st.w2);
   const float val = DIR == 0 ? v + fmaf(x, kLog2e, -st.adj) : v - st.adj;
   const float stored = DIR == 0 ? val : fmaf(x, kLog2e, val);
   st.adj = 0.0f;
-  sts(st.qc + st.u4, stored);
-  const float o = lds(st.oa);
+  sts_f32(st.qc + st.u4, stored);
+  const float o = lds_f32(st.oa);
   // TwoSum (Knuth): hi + lo == val + o exactly
   const float hi = val + o;
   const float bb = hi - val;
@@ -622,10 +349,10 @@ __device__ __forceinline__ void node_first_phase2(
   st.zsub = st.Zl;
   // the posterior mass of a level (1, or 0 without an accepting path): the helper warps take the mass on the
   // label with the most nodes as this minus the other labels' (visible to them through g_full)
-  if (threadIdx.x == 0) sts(feas_a, feasible ? 1.0f : 0.0f);
+  if (threadIdx.x == 0) sts_f32(feas_a, feasible ? 1.0f : 0.0f);
   if (z_out && threadIdx.x == 0)
     *z_out = feasible ? (float)(((double)st.Dc + ((double)m + (double)st.Zl)) * 0.6931471805599453) : -CUDART_INF_F;
-  sts(st.ga, ex2(((val - st.Zh) + o) - st.zsub));
+  sts_f32(st.ga, ex2(((val - st.Zh) + o) - st.zsub));
   st.oa += DIR ? -SD::p4(un) : SD::p4(un);
   if (st.ga != spare) st.ga += DIR ? -SD::g4(un) : SD::g4(un); // (loss only: the one posterior goes to the spare word)
   if (last) publish_block_max(st, stored);
@@ -694,7 +421,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
   int v = 0; // blocks visited
   if (DIR == 0) {
     // level 0: start nodes carry the implicit 0 (shortest.cpp:129-135)
-    if (cx.fl[nid] & 1) sts(st.pc + st.u4, 0.0f);
+    if (cx.fl[nid] & 1) sts_f32(st.pc + st.u4, 0.0f);
     bar_named(1, nact);
     st.gs = cx.saved + nid;
     for (; v < cx.n_ph1; v++) {
@@ -702,7 +429,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
       st.ea = e_row0 + (uint32_t)(s * cx.e_stage_bytes);
       if (v > 0) fetch_block_adjust(st);
-      if (tid == 0) stg(cx.boff_own + 4 * v, st.D);
+      if (tid == 0) stg_f32(cx.boff_own + 4 * v, st.D);
       node_rows<0, 1, ZW, NQ, FX>(st, un, kBlk); // A's phase-1 blocks are always full
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -712,16 +439,16 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
     const int j0 = cx.nblk - 1, n0 = min(kBlk, cx.T - kBlk * j0);
     mbar_wait(bar_e_full(cx.bars, 0), 0);
     st.ea = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4) + cx.lab4;
-    if (tid == 0) stg(cx.boff_own + 4 * j0, 0.0f);
+    if (tid == 0) stg_f32(cx.boff_own + 4 * j0, 0.0f);
     {
-      const float e2 = lds(st.ea) * kLog2e;
+      const float e2 = lds_f32(st.ea) * kLog2e;
       st.ea -= un.c4;
       const float val = (cx.fl[nid] & 2) ? 0.0f : kNeg;
-      sts(st.pc + st.u4, val + e2); // written to the row the first step READS
+      sts_f32(st.pc + st.u4, val + e2); // written to the row the first step READS
       st.gs = cx.saved + (long long)(cx.T - 1) * cx.pitch + nid;
       if (n0 == 1) publish_block_max(st, val + e2);
       bar_named(1, nact);
-      stg(st.gs, val);
+      stg_f32(st.gs, val);
       st.gs -= un.pitch;
     }
     node_rows<1, 1, ZW, NQ, FX>(st, un, n0 - 1);
@@ -732,7 +459,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
       st.ea = e_row0 + (uint32_t)(s * cx.e_stage_bytes);
       fetch_block_adjust(st);
-      if (tid == 0) stg(cx.boff_own + 4 * (cx.nblk - 1 - v), st.D);
+      if (tid == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), st.D);
       node_rows<1, 1, ZW, NQ, FX>(st, un, kBlk);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -763,7 +490,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
     st.oa = o_row0 + (uint32_t)(so * cx.o_stage_bytes);
     st.ga = g_row0 + (uint32_t)(sg * g_stride);
     if (v > 0) fetch_block_adjust(st);
-    const float doth = lds(cx.od_base + 16u * so);
+    const float doth = lds_f32(cx.od_base + 16u * so);
     if (v2 == 0) {
       node_first_phase2<DIR, ZW, NQ, FX>(st, un, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
                                          DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.spare);
@@ -827,17 +554,17 @@ template <int DIR, int PH, int NQ>
 __device__ __forceinline__ void pair_step(PairState& ps, const NodeUni& un, int r, bool last) {
   using SD = Strd<NQ, true>;
   const int rr = DIR ? -r : r;
-  const float xl = lds(ps.ea_l + (uint32_t)(rr * SD::c4(un)));
-  const float xb = lds(ps.ea_b + (uint32_t)(rr * SD::c4(un)));
+  const float xl = lds_f32(ps.ea_l + (uint32_t)(rr * SD::c4(un)));
+  const float xb = lds_f32(ps.ea_b + (uint32_t)(rr * SD::c4(un)));
   float vl, vb;
   if (DIR == 0) {
-    const f2 pv = lds_v2(ps.pc + ps.t8); // pair t-1: (label 2t-3, blank 2t-2)
-    vb = lse2(ps.ab, ps.al);
-    vl = lse3(ps.al, pv.y, ps.skip ? pv.x : kNeg);
+    const f32x2 pv = lds_v2_f32(ps.pc + ps.t8); // pair t-1: (label 2t-3, blank 2t-2)
+    vb = lse2_log2(ps.ab, ps.al);
+    vl = lse3_log2(ps.al, pv.y, ps.skip ? pv.x : kNeg);
   } else {
-    const float nl = lds(ps.pc + ps.t8 + 16u); // label 2t+1
-    vb = lse2(ps.ab, nl);
-    vl = lse3(ps.al, ps.ab, ps.skip ? nl : kNeg);
+    const float nl = lds_f32(ps.pc + ps.t8 + 16u); // label 2t+1
+    vb = lse2_log2(ps.ab, nl);
+    vl = lse3_log2(ps.al, ps.ab, ps.skip ? nl : kNeg);
   }
   const float val_l = DIR == 0 ? vl + fmaf(xl, kLog2e, -ps.adj) : vl - ps.adj;
   const float val_b = DIR == 0 ? vb + fmaf(xb, kLog2e, -ps.adj) : vb - ps.adj;
@@ -845,15 +572,15 @@ __device__ __forceinline__ void pair_step(PairState& ps, const NodeUni& un, int 
   ps.ab = DIR == 0 ? val_b : fmaf(xb, kLog2e, val_b);
   ps.adj = 0.0f;
   if (DIR == 0)
-    sts_v2(ps.qc + ps.t8 + 8u, ps.al, ps.ab);
+    sts_v2_f32(ps.qc + ps.t8 + 8u, ps.al, ps.ab);
   else
-    sts(ps.qc + ps.t8 + 8u, ps.al); // only the label is read by a neighbour
+    sts_f32(ps.qc + ps.t8 + 8u, ps.al); // only the label is read by a neighbour
   if (PH == 2)
-    sts(ps.ga + (uint32_t)(rr * SD::g4(un)),
-        ex2(((val_l - ps.Zh) + lds(ps.oa + (uint32_t)(rr * SD::p4(un)))) - ps.zsub));
+    sts_f32(ps.ga + (uint32_t)(rr * SD::g4(un)),
+        ex2(((val_l - ps.Zh) + lds_f32(ps.oa + (uint32_t)(rr * SD::p4(un)))) - ps.zsub));
   if (last) publish_block_max(ps, fmaxf(ps.al, ps.ab));
   bar_named(1, un.nact);
-  if (PH == 1) stg_v2(ps.gs + rr * SD::pitch(un), val_l, val_b);
+  if (PH == 1) stg_v2_f32(ps.gs + rr * SD::pitch(un), val_l, val_b);
   const uint32_t t = ps.pc;
   ps.pc = ps.qc;
   ps.qc = t;
@@ -877,18 +604,18 @@ __device__ __forceinline__ void pair_first_phase2(
     PairState& ps, const NodeUni& un, bool act_l, bool act_b, uint32_t red, int warp, int nwarps, float doth, bool last,
     float* z_out, uint32_t feas_a, bool want_g) {
   using SD = Strd<NQ, true>;
-  const float xl = lds(ps.ea_l), xb = lds(ps.ea_b);
+  const float xl = lds_f32(ps.ea_l), xb = lds_f32(ps.ea_b);
   ps.ea_l += DIR ? -SD::c4(un) : SD::c4(un);
   ps.ea_b += DIR ? -SD::c4(un) : SD::c4(un);
   float vl, vb;
   if (DIR == 0) {
-    const f2 pv = lds_v2(ps.pc + ps.t8);
-    vb = lse2(ps.ab, ps.al);
-    vl = lse3(ps.al, pv.y, ps.skip ? pv.x : kNeg);
+    const f32x2 pv = lds_v2_f32(ps.pc + ps.t8);
+    vb = lse2_log2(ps.ab, ps.al);
+    vl = lse3_log2(ps.al, pv.y, ps.skip ? pv.x : kNeg);
   } else {
-    const float nl = lds(ps.pc + ps.t8 + 16u);
-    vb = lse2(ps.ab, nl);
-    vl = lse3(ps.al, ps.ab, ps.skip ? nl : kNeg);
+    const float nl = lds_f32(ps.pc + ps.t8 + 16u);
+    vb = lse2_log2(ps.ab, nl);
+    vl = lse3_log2(ps.al, ps.ab, ps.skip ? nl : kNeg);
   }
   const float val_l = DIR == 0 ? vl + fmaf(xl, kLog2e, -ps.adj) : vl - ps.adj;
   const float val_b = DIR == 0 ? vb + fmaf(xb, kLog2e, -ps.adj) : vb - ps.adj;
@@ -896,10 +623,10 @@ __device__ __forceinline__ void pair_first_phase2(
   ps.ab = DIR == 0 ? val_b : fmaf(xb, kLog2e, val_b);
   ps.adj = 0.0f;
   if (DIR == 0)
-    sts_v2(ps.qc + ps.t8 + 8u, ps.al, ps.ab);
+    sts_v2_f32(ps.qc + ps.t8 + 8u, ps.al, ps.ab);
   else
-    sts(ps.qc + ps.t8 + 8u, ps.al);
-  const f2 o = lds_v2(ps.oa); // the partner's scores of (label, blank)
+    sts_f32(ps.qc + ps.t8 + 8u, ps.al);
+  const f32x2 o = lds_v2_f32(ps.oa); // the partner's scores of (label, blank)
   // TwoSum (Knuth) of both: hi + lo == val + o exactly
   const float hl = val_l + o.x, bl = hl - val_l, ll = (val_l - (hl - bl)) + (o.x - bl);
   const float hb = val_b + o.y, bb = hb - val_b, lb = (val_b - (hb - bb)) + (o.y - bb);
@@ -912,11 +639,11 @@ __device__ __forceinline__ void pair_first_phase2(
   ps.Zl = feasible ? lg2(S) : 0.0f;
   ps.Dc = ps.D + doth;
   ps.zsub = ps.Zl;
-  if (threadIdx.x == 0) sts(feas_a, feasible ? 1.0f : 0.0f);
+  if (threadIdx.x == 0) sts_f32(feas_a, feasible ? 1.0f : 0.0f);
   if (z_out && threadIdx.x == 0)
     *z_out = feasible ? (float)(((double)ps.Dc + ((double)m + (double)ps.Zl)) * 0.6931471805599453) : -CUDART_INF_F;
   if (want_g) {
-    sts(ps.ga, ex2(((val_l - ps.Zh) + o.x) - ps.zsub));
+    sts_f32(ps.ga, ex2(((val_l - ps.Zh) + o.x) - ps.zsub));
     ps.ga += DIR ? -SD::g4(un) : SD::g4(un);
   }
   ps.oa += DIR ? -SD::p4(un) : SD::p4(un);
@@ -949,7 +676,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     // level 0: start nodes carry the implicit 0 (shortest.cpp:129-135)
     ps.al = (has_label && (ctc_flags(2 * tp - 1, cx.N1) & 1)) ? 0.0f : kNeg;
     ps.ab = (ctc_flags(2 * tp, cx.N1) & 1) ? 0.0f : kNeg;
-    sts_v2(ps.pc + ps.t8 + 8u, ps.al, ps.ab);
+    sts_v2_f32(ps.pc + ps.t8 + 8u, ps.al, ps.ab);
     bar_named(1, nact);
     ps.gs = cx.saved + 2 * tp;
     for (; v < cx.n_ph1; v++) {
@@ -958,7 +685,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       ps.ea_l = e_row0_l + (uint32_t)(s * cx.e_stage_bytes);
       ps.ea_b = e_row0_b + (uint32_t)(s * cx.e_stage_bytes);
       if (v > 0) fetch_block_adjust(ps);
-      if (tid == 0) stg(cx.boff_own + 4 * v, ps.D);
+      if (tid == 0) stg_f32(cx.boff_own + 4 * v, ps.D);
       pair_rows<0, 1, NQ>(ps, un, kBlk);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -969,20 +696,20 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     mbar_wait(bar_e_full(cx.bars, 0), 0);
     ps.ea_l = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4) + cx.lab4;
     ps.ea_b = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4) + cx.blank4;
-    if (tid == 0) stg(cx.boff_own + 4 * j0, 0.0f);
+    if (tid == 0) stg_f32(cx.boff_own + 4 * j0, 0.0f);
     {
-      const float el = lds(ps.ea_l) * kLog2e, eb = lds(ps.ea_b) * kLog2e;
+      const float el = lds_f32(ps.ea_l) * kLog2e, eb = lds_f32(ps.ea_b) * kLog2e;
       ps.ea_l -= un.c4;
       ps.ea_b -= un.c4;
       const float val_l = (has_label && (ctc_flags(2 * tp - 1, cx.N1) & 2)) ? 0.0f : kNeg;
       const float val_b = (ctc_flags(2 * tp, cx.N1) & 2) ? 0.0f : kNeg;
       ps.al = val_l + el;
       ps.ab = val_b + eb;
-      sts(ps.pc + ps.t8 + 8u, ps.al); // written to the row the first step READS
+      sts_f32(ps.pc + ps.t8 + 8u, ps.al); // written to the row the first step READS
       ps.gs = cx.saved + (long long)(cx.T - 1) * cx.pitch + 2 * tp;
       if (n0 == 1) publish_block_max(ps, fmaxf(ps.al, ps.ab));
       bar_named(1, nact);
-      stg_v2(ps.gs, val_l, val_b);
+      stg_v2_f32(ps.gs, val_l, val_b);
       ps.gs -= un.pitch;
     }
     pair_rows<1, 1, NQ>(ps, un, n0 - 1);
@@ -994,7 +721,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       ps.ea_l = e_row0_l + (uint32_t)(s * cx.e_stage_bytes);
       ps.ea_b = e_row0_b + (uint32_t)(s * cx.e_stage_bytes);
       fetch_block_adjust(ps);
-      if (tid == 0) stg(cx.boff_own + 4 * (cx.nblk - 1 - v), ps.D);
+      if (tid == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), ps.D);
       pair_rows<1, 1, NQ>(ps, un, kBlk);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -1024,7 +751,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     ps.oa = o_row0 + (uint32_t)(so * cx.o_stage_bytes);
     ps.ga = g_row0 + (uint32_t)(sg * g_stride);
     if (v > 0) fetch_block_adjust(ps);
-    const float doth = lds(cx.od_base + 16u * so);
+    const float doth = lds_f32(cx.od_base + 16u * so);
     if (v2 == 0) {
       pair_first_phase2<DIR, NQ>(ps, un, act_l, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
                                  DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.want_g);
@@ -1071,17 +798,6 @@ struct QuadState {
   bool rows; // lane < 28: the thread's slots exist in a row
 };
 
-__device__ __forceinline__ float warp_max_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 /* the recursion of one level for the thread's four pairs; val_*: the scores proper (alpha / beta) */
 template <int DIR>
 __device__ __forceinline__ void quad_values(QuadState& q, const float* xl, float xb, float* val_l, float* val_b) {
@@ -1098,8 +814,8 @@ __device__ __forceinline__ void quad_values(QuadState& q, const float* xl, float
 #pragma unroll
     for (int i = 0; i < kQuad; i++) {
       const float ql = i ? q.al[i - 1] : pl, qb = i ? q.ab[i - 1] : pb;
-      nb[i] = lse2(q.ab[i], q.al[i]) + fmaf(xb, kLog2e, -q.adj);
-      nl[i] = lse3(q.al[i], qb, (q.skip >> i) & 1u ? ql : kNeg) + fmaf(xl[i], kLog2e, -q.adj);
+      nb[i] = lse2_log2(q.ab[i], q.al[i]) + fmaf(xb, kLog2e, -q.adj);
+      nl[i] = lse3_log2(q.al[i], qb, (q.skip >> i) & 1u ? ql : kNeg) + fmaf(xl[i], kLog2e, -q.adj);
     }
 #pragma unroll
     for (int i = 0; i < kQuad; i++) {
@@ -1112,8 +828,8 @@ __device__ __forceinline__ void quad_values(QuadState& q, const float* xl, float
 #pragma unroll
     for (int i = 0; i < kQuad; i++) {
       const float ql = i + 1 < kQuad ? q.al[i + 1] : nx;
-      val_b[i] = lse2(q.ab[i], ql) - q.adj;
-      val_l[i] = lse3(q.al[i], q.ab[i], (q.skip >> i) & 1u ? ql : kNeg) - q.adj;
+      val_b[i] = lse2_log2(q.ab[i], ql) - q.adj;
+      val_l[i] = lse3_log2(q.al[i], q.ab[i], (q.skip >> i) & 1u ? ql : kNeg) - q.adj;
     }
 #pragma unroll
     for (int i = 0; i < kQuad; i++) {
@@ -1140,22 +856,22 @@ __device__ __forceinline__ void quad_step(QuadState& q, const NodeUni& un, int r
   const uint32_t er = q.ea + (uint32_t)(rr * SD::c4(un));
   float xl[kQuad];
 #pragma unroll
-  for (int i = 0; i < kQuad; i++) xl[i] = lds(er + q.el[i]);
-  const float xb = lds(er + q.eb);
+  for (int i = 0; i < kQuad; i++) xl[i] = lds_f32(er + q.el[i]);
+  const float xb = lds_f32(er + q.eb);
   float val_l[kQuad], val_b[kQuad];
   quad_values<DIR>(q, xl, xb, val_l, val_b);
   if (PH == 2) {
     const uint32_t orow = q.oa + (uint32_t)(rr * SD::p4(un));
-    const float4 o0 = lds_v4(orow), o1 = lds_v4(orow + 16u); // (label, blank) x 4
+    const float4 o0 = lds_v4_f32(orow), o1 = lds_v4_f32(orow + 16u); // (label, blank) x 4
     const float ol[kQuad] = {o0.x, o0.z, o1.x, o1.z};
     const uint32_t grow = q.ga + (uint32_t)(rr * SD::g4(un));
 #pragma unroll
-    for (int i = 0; i < kQuad; i++) sts(grow + q.gl[i], ex2(((val_l[i] - q.Zh) + ol[i]) - q.zsub));
+    for (int i = 0; i < kQuad; i++) sts_f32(grow + q.gl[i], ex2(((val_l[i] - q.Zh) + ol[i]) - q.zsub));
   }
   if (PH == 1 && q.rows) {
     float* g = q.gs + rr * SD::pitch(un);
-    stg_v4(g, make_float4(val_l[0], val_b[0], val_l[1], val_b[1]));
-    stg_v4(g + 4, make_float4(val_l[2], val_b[2], val_l[3], val_b[3]));
+    stg_v4_f32(g, make_float4(val_l[0], val_b[0], val_l[1], val_b[1]));
+    stg_v4_f32(g + 4, make_float4(val_l[2], val_b[2], val_l[3], val_b[3]));
   }
   if (last) next_adj = quad_block_max(q);
 }
@@ -1180,12 +896,12 @@ __device__ __forceinline__ void quad_first_phase2(
   using SD = Strd<NQ, true>;
   float xl[kQuad];
 #pragma unroll
-  for (int i = 0; i < kQuad; i++) xl[i] = lds(q.ea + q.el[i]);
-  const float xb = lds(q.ea + q.eb);
+  for (int i = 0; i < kQuad; i++) xl[i] = lds_f32(q.ea + q.el[i]);
+  const float xb = lds_f32(q.ea + q.eb);
   q.ea += DIR ? -SD::c4(un) : SD::c4(un);
   float val_l[kQuad], val_b[kQuad];
   quad_values<DIR>(q, xl, xb, val_l, val_b);
-  const float4 o0 = lds_v4(q.oa), o1 = lds_v4(q.oa + 16u);
+  const float4 o0 = lds_v4_f32(q.oa), o1 = lds_v4_f32(q.oa + 16u);
   const float ol[kQuad] = {o0.x, o0.z, o1.x, o1.z}, ob[kQuad] = {o0.y, o0.w, o1.y, o1.w};
   float hl[kQuad], ll[kQuad], hb[kQuad], lb[kQuad];
   float m = 2.0f * kNeg;
@@ -1201,7 +917,7 @@ __device__ __forceinline__ void quad_first_phase2(
     if ((act_l >> i) & 1u) m = fmaxf(m, hl[i]);
     if ((act_b >> i) & 1u) m = fmaxf(m, hb[i]);
   }
-  m = warp_max_f(m);
+  m = warp_max(m);
   const bool live = m > 1.5f * kNeg;
   float term = 0.0f;
 #pragma unroll
@@ -1209,18 +925,18 @@ __device__ __forceinline__ void quad_first_phase2(
     if (live && ((act_l >> i) & 1u)) term += ex2((hl[i] - m) + ll[i]);
     if (live && ((act_b >> i) & 1u)) term += ex2((hb[i] - m) + lb[i]);
   }
-  const float S = warp_sum_f(term);
+  const float S = warp_sum(term);
   const bool feasible = m > kNeg * 0.5f && S > 0.0f;
   q.Zh = feasible ? m : 1.0e30f;
   q.Zl = feasible ? lg2(S) : 0.0f;
   q.Dc = q.D + doth;
   q.zsub = q.Zl;
-  if ((threadIdx.x & 31) == 0) sts(feas_a, feasible ? 1.0f : 0.0f);
+  if ((threadIdx.x & 31) == 0) sts_f32(feas_a, feasible ? 1.0f : 0.0f);
   if (z_out && (threadIdx.x & 31) == 0)
     *z_out = feasible ? (float)(((double)q.Dc + ((double)m + (double)q.Zl)) * 0.6931471805599453) : -CUDART_INF_F;
   if (want_g) {
 #pragma unroll
-    for (int i = 0; i < kQuad; i++) sts(q.ga + q.gl[i], ex2(((val_l[i] - q.Zh) + ol[i]) - q.zsub));
+    for (int i = 0; i < kQuad; i++) sts_f32(q.ga + q.gl[i], ex2(((val_l[i] - q.Zh) + ol[i]) - q.zsub));
     q.ga += DIR ? -SD::g4(un) : SD::g4(un);
   }
   q.oa += DIR ? -SD::p4(un) : SD::p4(un);
@@ -1266,7 +982,7 @@ __device__ __forceinline__ void quad_role(QuadState& q, const NodeCtx& cx, int n
         q.adj = next_adj;
         q.D += next_adj;
       }
-      if (lane == 0) stg(cx.boff_own + 4 * v, q.D);
+      if (lane == 0) stg_f32(cx.boff_own + 4 * v, q.D);
       quad_rows<0, 1, NQ>(q, un, kBlk, next_adj);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -1276,24 +992,24 @@ __device__ __forceinline__ void quad_role(QuadState& q, const NodeCtx& cx, int n
     const int j0 = cx.nblk - 1, n0 = min(kBlk, cx.T - kBlk * j0);
     mbar_wait(bar_e_full(cx.bars, 0), 0);
     q.ea = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4);
-    if (lane == 0) stg(cx.boff_own + 4 * j0, 0.0f);
+    if (lane == 0) stg_f32(cx.boff_own + 4 * j0, 0.0f);
     {
       float val_l[kQuad], val_b[kQuad];
-      const float eb = lds(q.ea + q.eb) * kLog2e;
+      const float eb = lds_f32(q.ea + q.eb) * kLog2e;
 #pragma unroll
       for (int i = 0; i < kQuad; i++) {
         const int k = kQuad * lane + i;
         val_l[i] = (((act_l >> i) & 1u) && (ctc_flags(2 * k - 1, cx.N1) & 2)) ? 0.0f : kNeg;
         val_b[i] = (((act_b >> i) & 1u) && (ctc_flags(2 * k, cx.N1) & 2)) ? 0.0f : kNeg;
-        q.al[i] = val_l[i] + lds(q.ea + q.el[i]) * kLog2e;
+        q.al[i] = val_l[i] + lds_f32(q.ea + q.el[i]) * kLog2e;
         q.ab[i] = val_b[i] + eb;
       }
       q.ea -= un.c4;
       q.gs = cx.saved + (long long)(cx.T - 1) * cx.pitch + 8 * lane;
       if (n0 == 1) next_adj = quad_block_max(q);
       if (q.rows) {
-        stg_v4(q.gs, make_float4(val_l[0], val_b[0], val_l[1], val_b[1]));
-        stg_v4(q.gs + 4, make_float4(val_l[2], val_b[2], val_l[3], val_b[3]));
+        stg_v4_f32(q.gs, make_float4(val_l[0], val_b[0], val_l[1], val_b[1]));
+        stg_v4_f32(q.gs + 4, make_float4(val_l[2], val_b[2], val_l[3], val_b[3]));
       }
       q.gs -= un.pitch;
     }
@@ -1306,7 +1022,7 @@ __device__ __forceinline__ void quad_role(QuadState& q, const NodeCtx& cx, int n
       q.ea = cx.e_base + dir_off + (uint32_t)(s * cx.e_stage_bytes);
       q.adj = next_adj;
       q.D += next_adj;
-      if (lane == 0) stg(cx.boff_own + 4 * (cx.nblk - 1 - v), q.D);
+      if (lane == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), q.D);
       quad_rows<1, 1, NQ>(q, un, kBlk, next_adj);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -1343,7 +1059,7 @@ __device__ __forceinline__ void quad_role(QuadState& q, const NodeCtx& cx, int n
       q.adj = next_adj;
       q.D += next_adj;
     }
-    const float doth = lds(cx.od_base + 16u * so);
+    const float doth = lds_f32(cx.od_base + 16u * so);
     if (v2 == 0) {
       quad_first_phase2<DIR, NQ>(q, un, act_l, act_b, doth, nfr == 1, DIR == 0 ? cx.out_score : nullptr, cx.feas_a,
                                  cx.want_g, next_adj);
@@ -1421,7 +1137,7 @@ __device__ __forceinline__ void helper_block(
 #pragma unroll
   for (int i = 0; i < NQ; i++) {
     const bool ok = row_on && k.eoff[i] != 0xffffffffu;
-    x[i] = ok ? lds_v4(estage + k.eoff[i]) : make_float4(-3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f);
+    x[i] = ok ? lds_v4_f32(estage + k.eoff[i]) : make_float4(-3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f);
     const float hi = fmaxf(fmaxf(x[i].x, x[i].y), fmaxf(x[i].z, x[i].w));
     const float lo = fminf(fminf(x[i].x, x[i].y), fminf(x[i].z, x[i].w));
     const float nan_probe = (x[i].x + x[i].y) + (x[i].z + x[i].w); // fmaxf / fminf drop NaNs, a sum keeps them
@@ -1455,10 +1171,10 @@ __device__ __forceinline__ void helper_block(
           const uint32_t a = gblock + k.hoff[h];
           int q = hs.l16;
           for (; q + 16 < k.hlen[h]; q += 32) {
-            a0 += lds(a + 4u * q);
-            a1 += lds(a + 4u * (q + 16));
+            a0 += lds_f32(a + 4u * q);
+            a1 += lds_f32(a + 4u * (q + 16));
           }
-          if (q < k.hlen[h]) a0 += lds(a + 4u * q);
+          if (q < k.hlen[h]) a0 += lds_f32(a + 4u * q);
         }
         hsum[h] = half_sum(a0 + a1);
       }
@@ -1471,7 +1187,7 @@ __device__ __forceinline__ void helper_block(
       for (int j = 0; j < 4; j++) o[4 * i + j] = 0.0f;
       if (row_on && k.eoff[i] != 0xffffffffu) {
         const uint32_t a = gblock + k.goff[i];
-        const float4 g0 = lds_v4(a), g1 = lds_v4(a + 16), g2 = lds_v4(a + 32), g3 = lds_v4(a + 48);
+        const float4 g0 = lds_v4_f32(a), g1 = lds_v4_f32(a + 16), g2 = lds_v4_f32(a + 32), g3 = lds_v4_f32(a + 48);
         o[4 * i + 0] = (g0.x + g0.y) + (g0.z + g0.w);
         o[4 * i + 1] = (g1.x + g1.y) + (g1.z + g1.w);
         o[4 * i + 2] = (g2.x + g2.y) + (g2.z + g2.w);
@@ -1481,11 +1197,11 @@ __device__ __forceinline__ void helper_block(
           for (int j = 0; j < 4; j++) {
             const int s1 = (k.hsel[i] >> (4 * j)) & 15;
             if (s1 == 15) { // beyond the cooperative slots: this lane sums the label's positions itself
-              const uint32_t w = lds_u(hs.seg + 4u * (uint32_t)((k.eoff[i] >> 2) - hs.r * hs.C + j));
+              const uint32_t w = lds_u32(hs.seg + 4u * (uint32_t)((k.eoff[i] >> 2) - hs.r * hs.C + j));
               const int len = (w >> 10) & 1023;
               const uint32_t p = gblock + k.ovf + (w & 1023u) * 4u;
               float acc = 0.0f;
-              for (int q = 0; q < len; q++) acc += lds(p + 4u * q);
+              for (int q = 0; q < len; q++) acc += lds_f32(p + 4u * q);
               o[4 * i + j] = acc;
             } else if (s1 == 14) { // the complement label: nothing was stored for it
               o[4 * i + j] = 0.0f;
@@ -1500,7 +1216,7 @@ __device__ __forceinline__ void helper_block(
       }
     }
     if (has_comp) { // mass on the label with the most nodes = the level's mass - everybody else's
-      const float cm = lds(feas_a) - half_sum(part);
+      const float cm = lds_f32(feas_a) - half_sum(part);
 #pragma unroll
       for (int i = 0; i < NQ; i++)
 #pragma unroll
@@ -1511,7 +1227,7 @@ __device__ __forceinline__ void helper_block(
     for (int i = 0; i < NQ; i++) {
       if (row_on && k.eoff[i] != 0xffffffffu) {
         // d(forwardScore(e) - forwardScore(lattice)) / d e[f][c] = softmax - posterior mass on label c
-        stg_v4(gout + (k.eoff[i] >> 2), make_float4(fmaf(x[i].x, inv, -o[4 * i + 0]), fmaf(x[i].y, inv, -o[4 * i + 1]),
+        stg_v4_f32(gout + (k.eoff[i] >> 2), make_float4(fmaf(x[i].x, inv, -o[4 * i + 0]), fmaf(x[i].y, inv, -o[4 * i + 1]),
                                                     fmaf(x[i].z, inv, -o[4 * i + 2]), fmaf(x[i].w, inv, -o[4 * i + 3])));
       }
     }
@@ -1533,7 +1249,7 @@ __device__ __forceinline__ void helper_block_fast(
     bool has_comp, int comp_rel, uint32_t feas_a, uint32_t g_empty_bar, float* gout) {
   float4 x[NQ];
 #pragma unroll
-  for (int i = 0; i < NQ; i++) x[i] = lds_v4(ea + 256u * i); // chunk i: labels 64 i + 4 l16 .. + 3
+  for (int i = 0; i < NQ; i++) x[i] = lds_v4_f32(ea + 256u * i); // chunk i: labels 64 i + 4 l16 .. + 3
   __syncwarp();
   if (hs.lane == 0) mbar_arrive(e_empty_bar); // the emission rows are in registers
   float mx = fmaxf(fmaxf(x[0].x, x[0].y), fmaxf(x[0].z, x[0].w));
@@ -1558,17 +1274,12 @@ __device__ __forceinline__ void helper_block_fast(
   // a NaN or +inf emission makes the sum NaN, a -inf / huge one trips the range checks
   hs.bad |= !(lo > -kHuge && mx < kHuge && sm < 3.0e38f);
   if (hs.l16 == 0) hs.zacc += mx + lg2(sm) * kLn2; // logsumexp of the row
-  float inv;
-#ifdef GTNB_HOST_EMU
-  inv = 1.0f / sm;
-#else
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(sm));
-#endif
+  const float inv = rcp_approx(sm);
   float o[4 * NQ];
 #pragma unroll
   for (int i = 0; i < NQ; i++) {
     const uint32_t a = ga + 1024u * i; // 64 labels * kSlots floats further on
-    const float4 g0 = lds_v4(a), g1 = lds_v4(a + 16), g2 = lds_v4(a + 32), g3 = lds_v4(a + 48);
+    const float4 g0 = lds_v4_f32(a), g1 = lds_v4_f32(a + 16), g2 = lds_v4_f32(a + 32), g3 = lds_v4_f32(a + 48);
     o[4 * i + 0] = (g0.x + g0.y) + (g0.z + g0.w);
     o[4 * i + 1] = (g1.x + g1.y) + (g1.z + g1.w);
     o[4 * i + 2] = (g2.x + g2.y) + (g2.z + g2.w);
@@ -1578,12 +1289,12 @@ __device__ __forceinline__ void helper_block_fast(
   // (htab: label | first overflow position << 8 | nodes << 18)
 #pragma unroll 1
   for (int h = 0; h < nheavy; h++) {
-    const uint32_t w = lds_u(htab + 4u * h);
+    const uint32_t w = lds_u32(htab + 4u * h);
     const int hlen = (int)(w >> 18);
     const uint32_t hq = ovf_row + 4u * ((w >> 8) & 1023u) + 4u * hs.l16;
-    float a0 = hs.l16 < hlen ? lds(hq) : 0.0f;
+    float a0 = hs.l16 < hlen ? lds_f32(hq) : 0.0f;
     for (int q0 = 16; q0 < hlen; q0 += 16) // (rare: a label on more than 16 nodes that is not the complement label)
-      if (q0 + hs.l16 < hlen) a0 += lds(hq + 4u * q0);
+      if (q0 + hs.l16 < hlen) a0 += lds_f32(hq + 4u * q0);
     const float hsum = half_sum(a0);
     const int rel = (int)(w & 255u) - 4 * hs.l16; // which of this lane's labels (64 i + 4 l16 + j  ->  64 i + j), if any
 #pragma unroll
@@ -1598,7 +1309,7 @@ __device__ __forceinline__ void helper_block_fast(
     float part = 0.0f;
 #pragma unroll
     for (int i = 0; i < NQ; i++) part += (o[4 * i + 0] + o[4 * i + 1]) + (o[4 * i + 2] + o[4 * i + 3]);
-    const float cm = lds(feas_a) - half_sum(part);
+    const float cm = lds_f32(feas_a) - half_sum(part);
 #pragma unroll
     for (int i = 0; i < NQ; i++) {
 #pragma unroll
@@ -1610,7 +1321,7 @@ __device__ __forceinline__ void helper_block_fast(
   for (int i = 0; i < NQ; i++) {
     const float4 gr = make_float4(fmaf(x[i].x, inv, -o[4 * i + 0]), fmaf(x[i].y, inv, -o[4 * i + 1]),
                                   fmaf(x[i].z, inv, -o[4 * i + 2]), fmaf(x[i].w, inv, -o[4 * i + 3]));
-    stg_v4(gout + 64 * i, gr);
+    stg_v4_f32(gout + 64 * i, gr);
   }
   __syncwarp();
   if (hs.lane == 0) mbar_arrive(g_empty_bar); // this warp is done with the posterior block
@@ -1693,8 +1404,8 @@ __global__ void __launch_bounds__(
   for (int i = tid; i < 2 * kRowF; i += blockDim.x) ring[i] = kNeg;
   // posterior blocks: all zero -- the slots no node writes to must read as 0 for good
   if (want_g)
-    for (int i = tid; i < kSG * (L.g_block_bytes >> 2); i += blockDim.x) sts(g_base + 4u * i, 0.0f);
-  if (tid < 2) sts_u(redi_a + 4u * tid, (uint32_t)kIntMin);
+    for (int i = tid; i < kSG * (L.g_block_bytes >> 2); i += blockDim.x) sts_f32(g_base + 4u * i, 0.0f);
+  if (tid < 2) sts_u32(redi_a + 4u * tid, (uint32_t)kIntMin);
 
   const uint8_t* fl = P.sg_flags + m.sg_node_base;
   const int32_t* ip = P.sg_in_ptr + m.sg_node_base;
@@ -1981,7 +1692,7 @@ __global__ void __launch_bounds__(
     for (int v = 0; v < n_visit; v++) {
       const int s = v % kSE, j = block_of(v);
       if (lane == 0) {
-        if (v >= kSE) mbar_wait_relaxed(e_empty(s), ((v / kSE) - 1) & 1);
+        if (v >= kSE) mbar_wait_suspend(e_empty(s), ((v / kSE) - 1) & 1);
         const uint32_t bytes = (uint32_t)(rows_of(j) * C * 4);
         mbar_expect_tx(e_full(s), bytes);
         bulk_g2s(e_base + (uint32_t)(s * L.e_stage_bytes), em + (long long)j * kBlk * C, bytes, e_full(s));
@@ -1997,7 +1708,7 @@ __global__ void __launch_bounds__(
           waited = true;
         }
         if (lane == 0) {
-          if (v2 >= kSO) mbar_wait_relaxed(o_empty(so), ((v2 / kSO) - 1) & 1);
+          if (v2 >= kSO) mbar_wait_suspend(o_empty(so), ((v2 / kSO) - 1) & 1);
           const uint32_t bytes = (uint32_t)(rows_of(j) * pitch * 4);
           mbar_expect_tx(o_full(so), bytes + 16u);
           bulk_g2s(o_base + (uint32_t)(so * L.o_stage_bytes), saved + (long long)j * kBlk * pitch, bytes, o_full(so));
@@ -2029,46 +1740,46 @@ __global__ void __launch_bounds__(
     for (int c = ht; c < C; c += 32 * kHelpers) {
       int n = 0;
       for (int u = 0; u < N1; u++) n += lds_s8(nlab_a + (uint32_t)u) == c;
-      sts_u(seg_a + 4u * c, (uint32_t)n);
+      sts_u32(seg_a + 4u * c, (uint32_t)n);
     }
     bar_named(2, 32 * kHelpers);
     if (ht == 0) {
       // the label with the most nodes, when it has more than kSlots (CTC: blank): the complement label
       int comp = -1, cn = kSlots;
       for (int c = 0; c < C; c++) {
-        const int n = (int)lds_u(seg_a + 4u * c);
+        const int n = (int)lds_u32(seg_a + 4u * c);
         if (n > cn) {
           cn = n;
           comp = c;
         }
       }
       if (MODE != 0) comp = P.ctc_blank; // the pair / quad threads never form a blank posterior, whatever U is
-      sts_u(hlist_a + 100u, (uint32_t)comp);
+      sts_u32(hlist_a + 100u, (uint32_t)comp);
       int nh = 0, at = 0;
       for (int c = 0; c < C; c++) {
-        const int n = (int)lds_u(seg_a + 4u * c);
+        const int n = (int)lds_u32(seg_a + 4u * c);
         if (c == comp) {
-          sts_u(seg_a + 4u * c, seg_pack(0, n, 14));
+          sts_u32(seg_a + 4u * c, seg_pack(0, n, 14));
         } else if (n > kSlots) {
           int slot1 = 15;
           if (nh < kMaxHeavy) {
-            sts_u(hlist_a + 4u * nh, (uint32_t)c);
+            sts_u32(hlist_a + 4u * nh, (uint32_t)c);
             slot1 = ++nh;
           }
-          sts_u(seg_a + 4u * c, seg_pack(at, n, slot1));
+          sts_u32(seg_a + 4u * c, seg_pack(at, n, slot1));
           at += n;
         } else {
-          sts_u(seg_a + 4u * c, seg_pack(0, n, 0));
+          sts_u32(seg_a + 4u * c, seg_pack(0, n, 0));
         }
       }
-      sts_u(hlist_a + 4u * kMaxHeavy, (uint32_t)nh);
+      sts_u32(hlist_a + 4u * kMaxHeavy, (uint32_t)nh);
       for (int u = 0; u < N1; u++)
         if (lds_s8(nlab_a + (uint32_t)u) < 0) sts_u16(perm_a + 2u * u, 4u * (uint32_t)(kSlots * C + at++));
     }
     bar_named(2, 32 * kHelpers);
-    nheavy = (int)lds_u(hlist_a + 4u * kMaxHeavy);
+    nheavy = (int)lds_u32(hlist_a + 4u * kMaxHeavy);
     for (int c = ht; c < C; c += 32 * kHelpers) {
-      const uint32_t w = lds_u(seg_a + 4u * c);
+      const uint32_t w = lds_u32(seg_a + 4u * c);
       const uint32_t s1 = w >> 20;
       // the complement label's nodes all store into the row's last word, which nobody reads (with >= 5 of them
       // out of the overflow area it is never an overflow position)
@@ -2088,7 +1799,7 @@ __global__ void __launch_bounds__(
     hk.goff[i] = (uint32_t)(hs.r * L.pg + kSlots * c) * 4u;
     hk.hsel[i] = 0;
     if (want_g && c < C)
-      for (int j = 0; j < 4; j++) hk.hsel[i] |= ((lds_u(seg_a + 4u * (c + j)) >> 20) & 15u) << (4 * j);
+      for (int j = 0; j < 4; j++) hk.hsel[i] |= ((lds_u32(seg_a + 4u * (c + j)) >> 20) & 15u) << (4 * j);
   }
   hk.ovf = (uint32_t)(hs.r * L.pg + kSlots * C) * 4u;
 #pragma unroll
@@ -2096,7 +1807,7 @@ __global__ void __launch_bounds__(
     hk.hoff[h] = 0;
     hk.hlen[h] = 0;
     if (want_g && h < nheavy) {
-      const uint32_t w = lds_u(seg_a + 4u * lds_u(hlist_a + 4u * h));
+      const uint32_t w = lds_u32(seg_a + 4u * lds_u32(hlist_a + 4u * h));
       hk.hoff[h] = hk.ovf + (w & 1023u) * 4u;
       hk.hlen[h] = (int)((w >> 10) & 1023u);
     }
@@ -2105,7 +1816,7 @@ __global__ void __launch_bounds__(
   if (!want_g) {
     for (; v < n_ph1; v++) {
       const int s = v % kSE;
-      mbar_wait_relaxed(e_full(s), (v / kSE) & 1);
+      mbar_wait_suspend(e_full(s), (v / kSE) & 1);
       helper_block<NQ, false>(hs, hk, rows_of(block_of(v)), e_base + (uint32_t)(s * L.e_stage_bytes), e_empty(s), 0, 0,
                               0, false, 0, nullptr);
     }
@@ -2115,16 +1826,16 @@ __global__ void __launch_bounds__(
     v = n_ph1;
     // the common shape takes helper_block_fast (warp-uniform, in fact CTA-uniform, decision)
     int n15 = 0;
-    for (int c = 0; c < C; c++) n15 += ((lds_u(seg_a + 4u * c) >> 20) & 15u) == 15u;
+    for (int c = 0; c < C; c++) n15 += ((lds_u32(seg_a + 4u * c) >> 20) & 15u) == 15u;
     const bool fast = C == 64 * NQ && n15 == 0;
     // label | overflow start << 8 | nodes << 18 of the cooperative labels, for helper_block_fast
     const uint32_t htab = hlist_a + 4u * (kMaxHeavy + 1);
     if (lane < nheavy) { // (every helper warp writes the same values)
-      const uint32_t hc = lds_u(hlist_a + 4u * lane), w = lds_u(seg_a + 4u * hc);
-      sts_u(htab + 4u * lane, hc | ((w & 1023u) << 8) | (((w >> 10) & 1023u) << 18));
+      const uint32_t hc = lds_u32(hlist_a + 4u * lane), w = lds_u32(seg_a + 4u * hc);
+      sts_u32(htab + 4u * lane, hc | ((w & 1023u) << 8) | (((w >> 10) & 1023u) << 18));
     }
     __syncwarp();
-    const int comp = (int)lds_u(hlist_a + 100u);
+    const int comp = (int)lds_u32(hlist_a + 100u);
     const bool has_comp = comp >= 0;
     const int comp_rel = has_comp ? comp - 4 * hs.l16 : -1000;
     const uint32_t feas_a = hlist_a + 96u;
@@ -2134,7 +1845,7 @@ __global__ void __launch_bounds__(
       const int s = v % kSE, sg = v2 % kSG, j = block_of(v);
       // the node warps arrive on g_full after they are through the block: its emission stage was
       // complete long before that (they waited for it), so one wait covers both
-      mbar_wait_relaxed(g_full(sg), (v2 / kSG) & 1);
+      mbar_wait_suspend(g_full(sg), (v2 / kSG) & 1);
       if (fast && rows_of(j) == kBlk) {
         const uint32_t gb = g_base + (uint32_t)(sg * L.g_block_bytes);
         helper_block_fast<NQ>(hs, e_base + (uint32_t)(s * L.e_stage_bytes) + f_e, e_empty(s), gb + f_g, gb + hk.ovf, htab,

@@ -23,16 +23,9 @@
  *
  *   compose_grad_kernel = compose's gradFunc (compose.cpp:496-518).
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -40,16 +33,6 @@ namespace {
 
 constexpr int kWarpsPerBlock = 8;
 constexpr int kMaxWords = 256; // graphs of up to 8192 nodes
-
-__device__ __forceinline__ unsigned lanemask_lt() {
-#ifdef GTNB_HOST_EMU
-  return (1u << (threadIdx.x & 31)) - 1u;
-#else
-  unsigned m;
-  asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
-  return m;
-#endif
-}
 
 /* ---- k1: per-frame alive sets ------------------------------------- */
 

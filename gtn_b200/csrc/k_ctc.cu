@@ -9,18 +9,9 @@
  * (in-arc lists ordered by (source, position in the source's out list), arc ids
  * in the reference's creation order), so no per-utterance host work is left.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-
-#include <algorithm>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 

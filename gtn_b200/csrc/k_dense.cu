@@ -34,14 +34,7 @@
  * Back-pointer rows are dense_bp_pitch(C) bytes apart (C rounded up to a multiple of 4), so the
  * traceback reads every row as whole 32-bit words for any C.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 

@@ -30,14 +30,6 @@
  * list with the same label, in list order" -- which is what all three produce (the sorted ones find the run
  * by binary search, :282-374).
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
-#include <algorithm>
-
-#include "gtnb_gcompose.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -45,8 +37,7 @@
 #include <vector>
 
 #include "gtnb_gcompose.h"
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -59,16 +50,6 @@ constexpr int kThreads = 1024; // one CTA per pair: every warp it can get to hid
 #endif
 constexpr int kEps = -1; // gtn::epsilon (graph.h:21)
 constexpr int kCache = 4; // destinations of a light state kept in registers between the passes of the ordered search
-
-__device__ __forceinline__ long long now_ns() {
-#ifdef GTNB_HOST_EMU
-  return 0;
-#else
-  long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-#endif
-}
 
 /* reach[] and ids[] are updated with atomics (performed in L2): every read goes to L2 as well (ld.global.cg),
  * a line cached in L1 before the update would be stale */
@@ -442,7 +423,7 @@ __global__ void __launch_bounds__(kThreads) gcompose_search_kernel(const PairDev
   const int tid = threadIdx.x;
   int32_t* queue = P.queue;
 
-  const long long t_start = now_ns();
+  const long long t_start = globaltimer();
   const int lane = tid & 31, warp = tid >> 5;
   // ---- 1. co-reachability (compose.cpp:64-104), unless gcompose_reach_kernel has been there
   if (tid == 0) *q_tail = 0;
@@ -485,7 +466,7 @@ __global__ void __launch_bounds__(kThreads) gcompose_search_kernel(const PairDev
   }
   } // !reach_done
 
-  const long long t_reach = now_ns();
+  const long long t_reach = globaltimer();
   // ---- 2. forward construction in the reference's order (compose.cpp:389-489)
   // start pairs, in (g1.start() x g2.start()) order: serial, the lists are short
   if (tid == 0) {
@@ -658,7 +639,7 @@ __global__ void __launch_bounds__(kThreads) gcompose_search_kernel(const PairDev
     P.counts[0] = next_id;
     P.counts[1] = arc_base;
     P.counts[2] = (int32_t)((t_reach - t_start) / 1000); // microseconds of the two phases (GTNB_GC_TIMES=1 prints them)
-    P.counts[3] = (int32_t)((now_ns() - t_reach) / 1000);
+    P.counts[3] = (int32_t)((globaltimer() - t_reach) / 1000);
   }
 }
 

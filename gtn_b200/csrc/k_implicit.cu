@@ -39,19 +39,9 @@
  * shared row that is flushed to global memory once per frame.  Only the several-nodes-per-thread
  * path and the wide kernels have this mode; with ARC = false they compile to what they were.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include <algorithm>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -59,6 +49,9 @@ namespace {
 
 constexpr int kImpThreads = 256;
 constexpr int kPf = 8; // frames of register prefetch (emissions, saved scores)
+/* (Alternatives that were slower at B=256 on an earlier GPU target, not re-measured on the H100: a 2-deep
+ * register ring behind prefetch.global.L1 issued 8 frames ahead; prefetching the three source scores
+ * of every arc into registers instead of staging the row in shared memory.) */
 // Fast path (graph operand with <= kImpThreads nodes, in/out degree <= 3): one node per thread,
 // branch-free.  Score rows and arc-gradient buffers have compile-time strides so that the two
 // halves of each double buffer differ by an immediate offset; absent arcs point at a dummy
@@ -127,44 +120,8 @@ ImpLayout make_imp_layout(int maxN, int maxA, bool backward, bool wide = false, 
   return o;
 }
 
-__device__ __forceinline__ float ninf() {
-  return -CUDART_INF_F;
-}
-__device__ __forceinline__ bool finite_f(float x) {
-  return fabsf(x) < CUDART_INF_F;
-}
-/* the two SFU primitives (the host emulation of tests/emu substitutes exp2f / log2f) */
-#ifdef GTNB_HOST_EMU
-__device__ __forceinline__ float sfu_ex2(float x) {
-  return exp2f(x);
-}
-__device__ __forceinline__ float sfu_lg2(float x) {
-  return log2f(x);
-}
-#else
-__device__ __forceinline__ float sfu_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float sfu_lg2(float x) {
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-#endif
-/* exp / log1p on the SFU, as in k_staged.cu */
-__device__ __forceinline__ float iexp(float x) {
-  return sfu_ex2(x * 1.4426950408889634f);
-}
-__device__ __forceinline__ float ilog1p(float x) {
-  const float y = sfu_lg2(1.0f + x);
-  return (x < 1e-3f) ? x * (1.0f - 0.5f * x) : y * 0.6931471805599453f;
-}
-
 __device__ __forceinline__ float block_max(float v, float* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  v = warp_max(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
@@ -174,8 +131,7 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return r;
 }
 __device__ __forceinline__ float block_sum(float v, float* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  v = warp_sum(v);
   __syncthreads();
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
@@ -203,7 +159,7 @@ __device__ __forceinline__ bool load_tables(
     t_src[e] = is[e];
     const float w = iw[e];
     t_w[e] = w;
-    bad |= !finite_f(w);
+    bad |= !is_finite(w);
   }
   __syncthreads();
   for (int i = tid; i < N1; i += kImpThreads) {
@@ -214,102 +170,30 @@ __device__ __forceinline__ bool load_tables(
   return bad;
 }
 
-/* Predicated read-only load straight into its destination register.  With a plain
- * `if (p) x = __ldg(q)` in the unrolled frame loop ptxas gathers the eight prefetches of a
- * block at its end, into temporaries, and copies them to the loop-carried registers at the
- * back edge -- a full-latency stall every kPf frames. */
-__device__ __forceinline__ void ldg_if(bool p, float& dst, const float* src) {
-#ifdef GTNB_HOST_EMU
-  if (p) dst = *src;
-  return;
-#else
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "setp.ne.s32 q, %2, 0;\n"
-      "@q ld.global.nc.f32 %0, [%1];\n"
-      "}\n"
-      : "+f"(dst)
-      : "l"(src), "r"((int)p));
-#endif
-}
-/* (Alternatives that were slower at B=256 on an earlier GPU target, not re-measured on the H100: a 2-deep
- * register ring behind prefetch.global.L1 issued 8 frames ahead; prefetching the three source scores
- * of every arc into registers instead of staging the row in shared memory.) */
-/* Unpredicated variant for the steady part of the frame loop (address always valid): a strong
- * (relaxed, CTA scope) load, which ptxas must keep on its side of the bar.sync it was written
- * on, writing the loop-carried ring register directly. */
-__device__ __forceinline__ void ldg_keep(float& dst, const float* src) {
-#ifdef GTNB_HOST_EMU
-  dst = *src;
-#else
-  asm volatile("ld.relaxed.cta.global.f32 %0, [%1];" : "=f"(dst) : "l"(src) : "memory");
-#endif
-}
-/* predicated red.global.add.f32 (no branch, no reconvergence point in the frame loop) */
-__device__ __forceinline__ void red_if(bool p, float* dst, float v) {
-#ifdef GTNB_HOST_EMU
-  if (p) atomicAdd(dst, v);
-  return;
-#else
-  asm volatile(
-      "{\n"
-      ".reg .pred q;\n"
-      "setp.ne.s32 q, %2, 0;\n"
-      "@q red.global.add.f32 [%0], %1;\n"
-      "}\n" ::"l"(dst),
-      "f"(v), "r"((int)p)
-      : "memory");
-#endif
-}
-
-/* Barrier over the first `nthreads` threads of the CTA only (a multiple of 32): warps that hold no
- * graph node leave the frame loop altogether instead of issuing its instruction stream for
- * nothing (CTC at U=100: 201 nodes = 7 of the 8 warps; the 8th cost 1/8 of the issue slots).
- * Named barrier 1; __syncthreads() (barrier 0) keeps synchronising the whole CTA elsewhere. */
-__device__ __forceinline__ void bar_nodes(int nthreads) {
-#ifdef GTNB_HOST_EMU
-  emu::named_barrier(1, nthreads);
-#else
-  asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory");
-#endif
-}
-
-/* three in-arcs, branch-free: absent arcs carry -inf and add exp(-inf) = 0 in arc order
- * (shortest.cpp:102-114); an all--inf (or +inf) maximum is returned as is.  The sum is >= 1
- * (the maximum contributes exp(0)), where lg2.approx has an absolute error <= 2^-22: far
- * below one ulp of any score this recursion produces after a few frames. */
-__device__ __forceinline__ float lse3(float v0, float v1, float v2) {
-  const float mx = fmaxf(fmaxf(v0, v1), v2);
-  const float sum = (iexp(v0 - mx) + iexp(v1 - mx)) + iexp(v2 - mx);
-  const float r = fmaf(sfu_lg2(sum), 0.6931471805599453f, mx);
-  return (fabsf(mx) == CUDART_INF_F) ? mx : r;
-}
-
 /* one node, any in-degree: the reference's two passes (shortest.cpp:121-136, :102-114) */
 __device__ __noinline__ float imp_fwd_node_any(
     int e0, int e1, float e, const int* t_src, const float* t_w, const float* prev) {
-  float mx = ninf();
+  float mx = neg_inf();
 #pragma unroll 1
   for (int a = e0; a < e1; a++) mx = fmaxf(mx, prev[t_src[a]] + (t_w[a] + e));
   if (mx == CUDART_INF_F || mx == -CUDART_INF_F) return mx;
   float sum = -1.0f;
 #pragma unroll 1
-  for (int a = e0; a < e1; a++) sum += iexp((prev[t_src[a]] + (t_w[a] + e)) - mx);
-  return mx + ilog1p(sum);
+  for (int a = e0; a < e1; a++) sum += fexp((prev[t_src[a]] + (t_w[a] + e)) - mx);
+  return mx + flog1p(sum);
 }
 
 /* arc-label mode: the same two passes, every in-arc with its own label's emission */
 __device__ __noinline__ float imp_fwd_node_arc(
     int e0, int e1, const float* erow, const int* t_alab, const int* t_src, const float* t_w, const float* prev) {
-  float mx = ninf();
+  float mx = neg_inf();
 #pragma unroll 1
   for (int a = e0; a < e1; a++) mx = fmaxf(mx, prev[t_src[a]] + (t_w[a] + erow[t_alab[a]]));
   if (mx == CUDART_INF_F || mx == -CUDART_INF_F) return mx;
   float sum = -1.0f;
 #pragma unroll 1
-  for (int a = e0; a < e1; a++) sum += iexp((prev[t_src[a]] + (t_w[a] + erow[t_alab[a]])) - mx);
-  return mx + ilog1p(sum);
+  for (int a = e0; a < e1; a++) sum += fexp((prev[t_src[a]] + (t_w[a] + erow[t_alab[a]])) - mx);
+  return mx + flog1p(sum);
 }
 
 /* arc-label mode: the per-entry matched labels of the graph operand -> shared memory */
@@ -326,7 +210,7 @@ __device__ __forceinline__ bool stage_erow(const float* row, float* dst, int C) 
   for (int c = threadIdx.x; c < C; c += kImpThreads) {
     const float v = __ldg(row + c);
     dst[c] = v;
-    bad |= !finite_f(v);
+    bad |= !is_finite(v);
   }
   return bad;
 }
@@ -387,13 +271,13 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
   float* S1 = S + (fast ? kFastRow : lay.pitch);
   // frame 0: start nodes carry the implicit 0 (shortest.cpp:129-135), nothing else exists
   if (fast) {
-    const float v = (tid < N1 && (t_flags[tid] & 1)) ? 0.0f : ninf();
+    const float v = (tid < N1 && (t_flags[tid] & 1)) ? 0.0f : neg_inf();
     S0[tid] = v;
     if (tid < N1) sc[tid] = v;
-    if (tid == 0) S0[kRowDummy] = S1[kRowDummy] = ninf();
+    if (tid == 0) S0[kRowDummy] = S1[kRowDummy] = neg_inf();
   } else {
     for (int i = tid; i < N1; i += kImpThreads) {
-      const float v = (t_flags[i] & 1) ? 0.0f : ninf();
+      const float v = (t_flags[i] & 1) ? 0.0f : neg_inf();
       S0[i] = v;
       sc[i] = v;
     }
@@ -448,7 +332,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     const float sv = lse3(P[i0] + (w0 + e), P[i1] + (w1 + e), P[i2] + (w2 + e)); \
     chk = fmaf(e, 0.0f, chk);                                            \
     Q[tid] = sv;                                                         \
-    bar_nodes(nact);                                                     \
+    bar_named<1>(nact);                                                     \
     if (act) *grow = sv; /* after the barrier: nothing waits for it */   \
     grow += pitch;                                                       \
   }
@@ -463,7 +347,10 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     }                                                                    \
     epf += (long long)kPf * C;                                           \
   }
-    const int nact = (N1 + 31) & ~31; // threads of the warps that hold nodes
+    // threads of the warps that hold nodes: the frame loop synchronises them alone on named barrier 1, so that
+    // warps without a graph node leave it instead of issuing its instruction stream for nothing (CTC at
+    // U=100: 201 nodes = 7 of the 8 warps)
+    const int nact = (N1 + 31) & ~31;
     if (tid < nact) {
       for (; f0 + 3 * kPf <= T; f0 += kPf) {
 #pragma unroll
@@ -495,7 +382,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
         const float* Ecur = E_s + ((t - 1) & 1) * C;
         for (int i = tid; i < N1; i += kImpThreads) {
           const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
-          const float sv = (e1 > e0) ? imp_fwd_node_arc(e0, e1, Ecur, t_alab, t_src, t_w, prev) : ninf();
+          const float sv = (e1 > e0) ? imp_fwd_node_arc(e0, e1, Ecur, t_alab, t_src, t_w, prev) : neg_inf();
           cur[i] = sv;
           srow[i] = sv;
         }
@@ -503,10 +390,10 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
       } else {
         for (int i = tid; i < N1; i += kImpThreads) {
           const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
-          float sv = ninf();
+          float sv = neg_inf();
           if (e1 > e0) {
             const float e = __ldg(er + t_lab[i]);
-            bad |= !finite_f(e);
+            bad |= !is_finite(e);
             sv = imp_fwd_node_any(e0, e1, e, t_src, t_w, prev);
           }
           cur[i] = sv;
@@ -522,7 +409,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
 
   // accept nodes of the last frame (shortest.cpp:147-159)
   const float* Sf = (T & 1) ? S1 : S0;
-  float mx = ninf();
+  float mx = neg_inf();
   for (int i = tid; i < N1; i += kImpThreads)
     if (t_flags[i] & 2) mx = fmaxf(mx, Sf[i]);
   mx = block_max(mx, red);
@@ -621,13 +508,13 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
   build_out_lists(N1, A1, t_src, t_outptr, t_outent, t_cursor);
 
   const float out = out_scores[blockIdx.x];
-  if (!finite_f(out) || T < 1) return; // no accepting path (empty lattice): no gradient
+  if (!is_finite(out) || T < 1) return; // no accepting path (empty lattice): no gradient
   const float delta = deltas ? deltas[blockIdx.x] : 1.0f;
   const float* sc = scores + m.node_base;
   const float* em = emissions + m.emis_off;
   float* gem = grad_emis + (long long)blockIdx.x * grad_stride;
   // seeds: nodeGrad[accept] = exp(score - maxA) / exp(out - maxA) (shortest.cpp:49-60)
-  float mxa = ninf();
+  float mxa = neg_inf();
   for (int i = tid; i < N1; i += kImpThreads)
     if (t_flags[i] & 2) mxa = fmaxf(mxa, sc[(long long)T * pitch + i]);
   mxa = block_max(mxa, red);
@@ -682,18 +569,18 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
 #pragma unroll
     for (int j = 0; j < kPf; j++) {
       const int f = T - 2 - j;
-      nxs[j] = (act && f >= 0) ? __ldg(scu + (long long)f * pitch) : ninf();
+      nxs[j] = (act && f >= 0) ? __ldg(scu + (long long)f * pitch) : neg_inf();
       nxe[j] = (has && f >= 0) ? __ldg(eml + (long long)f * C) : 0.0f;
     }
     // first frame of the next refill; only dereferenced while >= row 0
     const float* spf = scu + (long long)(T - 2 - kPf) * pitch;
     const float* epf = eml + (long long)(T - 2 - kPf) * C;
     // prologue: the arc factors of level T need row T-1 in shared memory
-    float s_own = act ? __ldg(scu + (long long)T * pitch) : ninf(); // S_T[u]
-    float s_nxt = act ? __ldg(scu + (long long)(T - 1) * pitch) : ninf(); // S_{T-1}[u]
+    float s_own = act ? __ldg(scu + (long long)T * pitch) : neg_inf(); // S_T[u]
+    float s_nxt = act ? __ldg(scu + (long long)(T - 1) * pitch) : neg_inf(); // S_{T-1}[u]
     Sb[tid] = s_nxt;
     if (tid == 0) {
-      Sa[kRowDummy] = Sb[kRowDummy] = ninf();
+      Sa[kRowDummy] = Sb[kRowDummy] = neg_inf();
       CURa[kCurDummy] = CURb[kCurDummy] = 0.0f;
     }
     float g = (act && (t_flags[tid] & 2)) ? expf(s_own - mxa) / denom : 0.0f;
@@ -702,9 +589,9 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     {
       const float e = has ? __ldg(eml + (long long)(T - 1) * C) : 0.0f;
       const float se = (s_own == -CUDART_INF_F) ? CUDART_INF_F : s_own;
-      E0 = iexp(Sb[i0] + (w0 + e) - se);
-      E1 = iexp(Sb[i1] + (w1 + e) - se);
-      E2 = iexp(Sb[i2] + (w2 + e) - se);
+      E0 = fexp(Sb[i0] + (w0 + e) - se);
+      E1 = fexp(Sb[i1] + (w1 + e) - se);
+      E2 = fexp(Sb[i2] + (w2 + e) - se);
     }
     float* gl = gem + (long long)(T - 1) * C + (has ? t_lab[tid] : 0); // emission gradient of level t
     float ga0 = 0.0f, ga1 = 0.0f, ga2 = 0.0f; // gradients of the node's in-arcs of the graph operand
@@ -728,7 +615,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     const float s_f = ps[j]; /* S_{t-2}[u] */                                         \
     const float e_f = has ? pe[j] : 0.0f; /* e[t-2][label] */                         \
     Sw[tid] = s_f;                                                                    \
-    bar_nodes(nact);                                                                  \
+    bar_named<1>(nact);                                                                  \
     g = (Cw[q0] + Cw[q1]) + Cw[q2]; /* node gradient of level t-1: the serial chain */ \
     /* the emission gradient of level t leaves after the barrier, in the shadow of the gather \
        (ptxas turns the predicated red into a branch: before the barrier it delayed every   \
@@ -739,9 +626,9 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     s_nxt = s_f;                                                                      \
     { /* arc factors of level t-1; a node that does not exist (score -inf) gets exp(-inf) */ \
       const float se = (s_own == -CUDART_INF_F) ? CUDART_INF_F : s_own;               \
-      E0 = iexp(Sw[i0] + (w0 + e_f) - se);                                            \
-      E1 = iexp(Sw[i1] + (w1 + e_f) - se);                                            \
-      E2 = iexp(Sw[i2] + (w2 + e_f) - se);                                            \
+      E0 = fexp(Sw[i0] + (w0 + e_f) - se);                                            \
+      E1 = fexp(Sw[i1] + (w1 + e_f) - se);                                            \
+      E2 = fexp(Sw[i2] + (w2 + e_f) - se);                                            \
     }                                                                                 \
   }
 #define GTNB_BWD_REFILL(GUARDED)                                                      \
@@ -763,7 +650,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     spf -= (long long)kPf * pitch;                                                    \
     epf -= (long long)kPf * C;                                                        \
   }
-    const int nact = (N1 + 31) & ~31; // threads of the warps that hold nodes (see bar_nodes)
+    const int nact = (N1 + 31) & ~31; // threads of the warps that hold nodes (see the forward kernel)
     if (tid < nact) {
       for (; i0_ + 2 * kPf + 1 <= T; i0_ += kPf) {
         GTNB_BWD_REFILL(false)
@@ -816,7 +703,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
 #pragma unroll 1
           for (int a = e0; a < e1; a++) {
             const int lab = t_alab[a];
-            const float c = ex ? gi * iexp(Sprev[t_src[a]] + (t_w[a] + E_s[lab]) - sn) : 0.0f;
+            const float c = ex ? gi * fexp(Sprev[t_src[a]] + (t_w[a] + E_s[lab]) - sn) : 0.0f;
             CURa[a] = c;
             if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this thread only
             if (c != 0.0f) atomicAdd(&GE[lab], c); // shared: one global add per label and frame below
@@ -832,7 +719,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
           float acc = 0.0f;
 #pragma unroll 1
           for (int a = e0; a < e1; a++) {
-            const float c = ex ? gi * iexp(Sprev[t_src[a]] + (t_w[a] + e) - sn) : 0.0f;
+            const float c = ex ? gi * fexp(Sprev[t_src[a]] + (t_w[a] + e) - sn) : 0.0f;
             CURa[a] = c;
             acc += c;
             if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this thread only
@@ -936,7 +823,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
   float* prev = S;
   float* cur = S + lay.pitch;
   for (int i = tid; i < N1; i += kImpThreads) {
-    const float v = (t_flags[i] & 1) ? 0.0f : ninf();
+    const float v = (t_flags[i] & 1) ? 0.0f : neg_inf();
     prev[i] = v;
     sc[i] = v;
   }
@@ -945,7 +832,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
   } else if (T > 0 && tid < C) {
     const float e0v = __ldg(em + tid);
     E_s[tid] = e0v;
-    bad |= !finite_f(e0v);
+    bad |= !is_finite(e0v);
   }
   __syncthreads();
 
@@ -976,11 +863,11 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
       const int e0 = on ? t_inptr[u] : 0, e1 = on ? t_inptr[u + 1] : 0;
       const float e = (!ARC && on) ? Ecur[t_lab[u]] : 0.0f;
       float v[kWideCap];
-      float mx = ninf();
+      float mx = neg_inf();
 #pragma unroll
       for (int k = 0; k < kWideCap; k++) {
         const int a = e0 + sub + k * G;
-        v[k] = ninf();
+        v[k] = neg_inf();
         if (a < e1) {
           const int2 sw = t_sw[a];
           v[k] = prev[sw.x] + (__int_as_float(sw.y) + (ARC ? Ecur[t_alab[a]] : e));
@@ -991,10 +878,10 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
       for (int o = G / 2; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(gmask, mx, o));
       float sum = 0.0f;
 #pragma unroll
-      for (int k = 0; k < kWideCap; k++) sum += iexp(v[k] - mx);
+      for (int k = 0; k < kWideCap; k++) sum += fexp(v[k] - mx);
 #pragma unroll
       for (int o = G / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(gmask, sum, o);
-      const float lg = sfu_lg2(sum);
+      const float lg = lg2(sum);
       const float sv = (fabsf(mx) == CUDART_INF_F) ? mx : fmaf(lg, 0.6931471805599453f, mx);
       if (on && sub == 0) {
         cur[u] = sv;
@@ -1004,12 +891,12 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
     // a node without in-arcs does not exist past frame 0
     for (int i = tid; i < N1; i += kImpThreads)
       if (t_inptr[i + 1] == t_inptr[i]) {
-        cur[i] = ninf();
-        srow[i] = ninf();
+        cur[i] = neg_inf();
+        srow[i] = neg_inf();
       }
     if (!ARC && ld) {
       Enext[tid] = enext;
-      bad |= !finite_f(enext);
+      bad |= !is_finite(enext);
     }
     if (ARC) {
 #pragma unroll
@@ -1017,7 +904,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
         const int c = tid + k * kImpThreads;
         if (t < T && c < C) {
           Enext[c] = en[k];
-          bad |= !finite_f(en[k]);
+          bad |= !is_finite(en[k]);
         }
       }
     }
@@ -1029,7 +916,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
 
   // accept nodes of the last frame (shortest.cpp:147-159); `prev` is the last row written
   const float* Sf = prev;
-  float mx = ninf();
+  float mx = neg_inf();
   for (int i = tid; i < N1; i += kImpThreads)
     if (t_flags[i] & 2) mx = fmaxf(mx, Sf[i]);
   mx = block_max(mx, red);
@@ -1096,13 +983,13 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
   build_wide_tables(N1, A1, t_inptr, t_src, t_w, t_outptr, t_sw, t_act, t_acto);
 
   const float out = out_scores[blockIdx.x];
-  if (!finite_f(out) || T < 1) return; // no accepting path (empty lattice): no gradient
+  if (!is_finite(out) || T < 1) return; // no accepting path (empty lattice): no gradient
   const float delta = deltas ? deltas[blockIdx.x] : 1.0f;
   const float* sc = scores + m.node_base;
   const float* em = emissions + m.emis_off;
   float* gem = grad_emis + (long long)blockIdx.x * grad_stride;
 
-  float mxa = ninf();
+  float mxa = neg_inf();
   for (int i = tid; i < N1; i += kImpThreads)
     if (t_flags[i] & 2) mxa = fmaxf(mxa, sc[(long long)T * pitch + i]);
   mxa = block_max(mxa, red);
@@ -1136,7 +1023,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
     const float* Ecur = E_s + ((t - 1) & 1) * C; // frame t-1
     float* Enext = E_s + (t & 1) * C; // frame t-2 (same parity as t)
     const bool more = t >= 2;
-    float snext = ninf(), enext = 0.0f; // in flight during this level
+    float snext = neg_inf(), enext = 0.0f; // in flight during this level
     if (more && tid < N1) snext = __ldg(sc + (long long)(t - 2) * pitch + tid);
     if (!ARC && more && tid < C) enext = __ldg(em + (long long)(t - 2) * C + tid);
     float en[kArcRows]; // ARC: frame t-2's row, kArcRows values per thread
@@ -1165,7 +1052,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
         if (a < e1) {
           const int2 sw = t_sw[a];
           const int alab = ARC ? t_alab[a] : 0;
-          const float c = g * iexp(prv[sw.x] + (__int_as_float(sw.y) + (ARC ? Ecur[alab] : e)) - se);
+          const float c = g * fexp(prv[sw.x] + (__int_as_float(sw.y) + (ARC ? Ecur[alab] : e)) - se);
           CUR[a] = c;
           acc += c;
           if (GRAPH_GRAD) ACCG[a] += c; // entry a belongs to this lane only

@@ -8,18 +8,9 @@
  * argmax indicator.  Rows are independent, so this is one warp per frame row,
  * fully coalesced, followed by a fixed-order per-utterance reduction.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <cstdint>
 
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include <cstdint>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 

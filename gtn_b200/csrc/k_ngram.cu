@@ -32,19 +32,9 @@
  * kernel).  Its numerator, compose(fal_b, transitions), is a U+1-node chain that asg_num_build_kernel writes into the
  * same small-graph tables for k_implicit.cu's sweeps; it needs no fold.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include <algorithm>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -73,36 +63,14 @@ long long asg_alpha_floats(int B, int T, int C) {
 
 namespace {
 
-#ifdef GTNB_HOST_EMU
-__device__ __forceinline__ float ng_exp(float x) {
-  return expf(x);
-}
-__device__ __forceinline__ float ng_log(float x) {
-  return logf(x);
-}
-#else
-__device__ __forceinline__ float ng_exp(float x) {
-  return __expf(x); // ex2.approx(x * log2 e)
-}
-__device__ __forceinline__ float ng_log(float x) {
-  return __logf(x); // lg2.approx(x) * ln 2; x >= 1 here
-}
-#endif
-__device__ __forceinline__ float ng_ninf() {
-  return -CUDART_INF_F;
-}
-__device__ __forceinline__ bool ng_finite(float x) {
-  return fabsf(x) < CUDART_INF_F;
-}
-
 /* (m, s) = logsumexp as max + sum of exp(x - max), merged over the `lanes` lanes of a row / column */
 __device__ __forceinline__ void ng_merge(float& m, float& s, int lanes) {
   for (int o = 1; o < lanes; o <<= 1) {
     const float om = __shfl_xor_sync(0xffffffffu, m, o);
     const float os = __shfl_xor_sync(0xffffffffu, s, o);
     const float M = fmaxf(m, om);
-    const float Mm = M == ng_ninf() ? 0.0f : M; // all -inf: s stays 0
-    s = s * ng_exp(m - Mm) + os * ng_exp(om - Mm);
+    const float Mm = M == neg_inf() ? 0.0f : M; // all -inf: s stays 0
+    s = s * exp_fast(m - Mm) + os * exp_fast(om - Mm);
     m = M;
   }
 }
@@ -141,13 +109,13 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   for (int k = 0; k < K; k++) {
     const int j = q + lanes * k;
     const bool on = row && j < C;
-    w[k] = on ? __ldg(Wm + i * C + j) : ng_ninf();
-    if (on) bad |= !ng_finite(w[k]);
+    w[k] = on ? __ldg(Wm + i * C + j) : neg_inf();
+    if (on) bad |= !is_finite(w[k]);
   }
   float s_i = 0.0f;
   if (START && lead) {
     s_i = __ldg(W + i);
-    bad |= !ng_finite(s_i);
+    bad |= !is_finite(s_i);
   }
   for (int j = tid; j < kNgramMaxC; j += blockDim.x) A[0][j] = A[1][j] = 0.0f; // alpha_0 = 0; padding stays 0
   for (int j = tid; j < C; j += blockDim.x) al[j] = 0.0f;
@@ -156,7 +124,7 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   if (START && Tb > 0) { // alpha_1 = e[0] + s
     const float e = e_nx;
     if (lead && Tb > 1) e_nx = __ldg(em + C + i);
-    bad |= !ng_finite(e);
+    bad |= !is_finite(e);
     if (lead) {
       const float v = e + s_i;
       A[1][i] = v;
@@ -168,22 +136,22 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   for (int t = START ? 2 : 1; t <= Tb; t++) {
     const float e = e_nx;
     if (lead && t < Tb) e_nx = __ldg(em + (long long)t * C + i);
-    bad |= !ng_finite(e);
+    bad |= !is_finite(e);
     const float* P = A[(t - 1) & 1];
     float x[K];
-    float m = ng_ninf();
+    float m = neg_inf();
 #pragma unroll
     for (int k = 0; k < K; k++) {
       x[k] = P[q + lanes * k] + w[k];
       m = fmaxf(m, x[k]);
     }
-    const float mm = m == ng_ninf() ? 0.0f : m;
+    const float mm = m == neg_inf() ? 0.0f : m;
     float s = 0.0f;
 #pragma unroll
-    for (int k = 0; k < K; k++) s += ng_exp(x[k] - mm);
+    for (int k = 0; k < K; k++) s += exp_fast(x[k] - mm);
     ng_merge(m, s, lanes);
     if (lead) {
-      float v = e + (m + ng_log(s));
+      float v = e + (m + log_fast(s));
       if (START) v -= P[0];
       A[t & 1][i] = v;
       al[(long long)t * C + i] = v;
@@ -197,12 +165,12 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   bad = __syncthreads_or(bad);
   if (tid < 32) {
     const float* F = A[Tb & 1];
-    float m = ng_ninf();
+    float m = neg_inf();
     for (int j = tid; j < C; j += 32) m = fmaxf(m, F[j]);
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    m = warp_max(m);
     float s = 0.0f;
     for (int j = tid; j < C; j += 32) s += expf(F[j] - m);
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    s = warp_sum(s);
     if (tid == 0) {
       if (START) {
         const double Z = c + (double)(m + logf(s));
@@ -233,7 +201,7 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
   const int b = blockIdx.x, tid = threadIdx.x;
   const int Tb = lens[b];
   const float Z = den[b];
-  if (!ng_finite(Z) || Tb < 1) return; // (non-finite: the caller repeats the call materialised)
+  if (!is_finite(Z) || Tb < 1) return; // (non-finite: the caller repeats the call materialised)
   const int j = tid / lanes, q = tid % lanes;
   const bool col = j < C;
   const bool lead = col && q == 0;
@@ -248,7 +216,7 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
 #pragma unroll
   for (int k = 0; k < K; k++) {
     const int i = q + lanes * k;
-    w[k] = (col && i < C) ? __ldg(Wm + i * C + j) : ng_ninf();
+    w[k] = (col && i < C) ? __ldg(Wm + i * C + j) : neg_inf();
     acc[k] = 0.0f;
   }
   for (int i = tid; i < kNgramMaxC; i += blockDim.x) {
@@ -275,36 +243,36 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
     if (rowt) {
       const float bt = Bt[t & 1][tid];
       G[tid] = e_t + bt;
-      const float p = ng_exp(START ? (a_t + bt) + (float)(c_t + d - Zd) : a_t + bt - Z); // node posterior
+      const float p = exp_fast(START ? (a_t + bt) + (float)(c_t + d - Zd) : a_t + bt - Z); // node posterior
       atomicAdd(gr + (long long)(t - 1) * C + tid, p);
       if (START && t == 1) atomicAdd(wgrad + tid, p); // d Z / d s
     }
     if (START && t == 1) break; // (uniform) frame 1 has no transition through the matrix
     __syncthreads();
     float x[K];
-    float m = ng_ninf();
+    float m = neg_inf();
 #pragma unroll
     for (int k = 0; k < K; k++) {
       x[k] = w[k] + G[q + lanes * k];
       m = fmaxf(m, x[k]);
     }
-    const float mm = m == ng_ninf() ? 0.0f : m;
+    const float mm = m == neg_inf() ? 0.0f : m;
     float s = 0.0f;
-    const float f = ng_exp(START ? (mm + aj) + (float)(c_prev + d - Zd) : (mm + aj) - Z); // pair = exp(x - mm) * f
+    const float f = exp_fast(START ? (mm + aj) + (float)(c_prev + d - Zd) : (mm + aj) - Z); // pair = exp(x - mm) * f
 #pragma unroll
     for (int k = 0; k < K; k++) {
-      const float p = ng_exp(x[k] - mm);
+      const float p = exp_fast(x[k] - mm);
       s += p;
       acc[k] = fmaf(p, f, acc[k]);
     }
     ng_merge(m, s, lanes);
     if (START) {
       const float g0 = G[0];
-      if (lead) Bt[(t - 1) & 1][j] = (m + ng_log(s)) - g0;
+      if (lead) Bt[(t - 1) & 1][j] = (m + log_fast(s)) - g0;
       d += (double)g0;
       c_t = c_prev;
     } else if (lead) {
-      Bt[(t - 1) & 1][j] = m + ng_log(s);
+      Bt[(t - 1) & 1][j] = m + log_fast(s);
     }
     __syncthreads();
   }
@@ -319,12 +287,12 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
 __global__ void __launch_bounds__(256) ngram_sigma_kernel(int C, const float* __restrict__ W, float* __restrict__ sigma) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
   if (i >= C) return; // whole warps
-  float m = ng_ninf();
+  float m = neg_inf();
   for (int j = lane; j < C; j += 32) m = fmaxf(m, W[i * C + j]);
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_max(m);
   float s = 0.0f;
   for (int j = lane; j < C; j += 32) s += expf(W[i * C + j] - m);
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  s = warp_sum(s);
   if (lane == 0) sigma[i] = m + logf(s);
 }
 

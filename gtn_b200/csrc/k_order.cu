@@ -30,19 +30,9 @@
  * One CTA per utterance walks the frames; the ranks of a frame come from a presence bitmap of its keys
  * (distinct integers below N * K) and a prefix sum of the popcounts.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtn_b200.h"
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-
-#include <algorithm>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 

@@ -20,30 +20,15 @@
  * the running sum started at -1 (shortest.cpp:102-114).  score + weight is a
  * single fp32 add (no FMA can be contracted into it: there is no multiply).
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <cstdlib>
 
-#include "gtn_b200.h"
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include <cstdlib>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
 namespace {
 
 constexpr int kThreads = 256;
-
-__device__ __forceinline__ float neg_inf() {
-  return -CUDART_INF_F;
-}
 
 /* getScore (shortest.cpp:102-114) given max and sum already reduced */
 __device__ __forceinline__ float finish_score(int count, float mx, float sum_m1, bool tropical) {

@@ -30,18 +30,9 @@
  * the 8-byte arc records; per-graph slabs start on 4-element boundaries and
  * every array has 16 elements of slack, so the extra elements are always mapped.
  */
-#ifdef GTNB_HOST_EMU // this file compiled by g++ against tests/emu/simt_emu.h (CPU test suite)
 #include <algorithm>
 
-#include "gtn_b200.h"
-#include "gtnb_meta.h"
-#include "simt_emu.h"
-#else
-#include <cuda_runtime.h>
-#include <math_constants.h>
-
-#include "gtnb_internal.h"
-#endif
+#include "gtnb_ptx.h"
 
 namespace gtnb {
 
@@ -55,159 +46,6 @@ constexpr int consumer_warps(int /*G*/) {
 }
 constexpr int kMaxLevelsInSmem = 6144;
 constexpr int kMaxStages = 8;
-
-__device__ __forceinline__ float neg_inf() {
-  return -CUDART_INF_F;
-}
-#ifdef GTNB_HOST_EMU
-/* the PTX below, restated for the host emulation (tests/emu/simt_emu.h): shared-window addresses are
- * offsets into the CTA's emulated shared memory, mbarriers and the bulk copy are emu:: objects */
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return emu::shared_window(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
-  emu::mbar_init(bar, count);
-}
-__device__ __forceinline__ void mbar_init_fence() {}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  emu::mbar_expect_tx(bar, bytes);
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  emu::mbar_arrive(bar);
-}
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-  emu::mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  emu::mbar_wait(bar, parity);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  emu::bulk_g2s(dst, src, bytes, bar);
-}
-template <int NC>
-__device__ __forceinline__ void consumer_bar() {
-  emu::named_barrier(1, NC);
-}
-__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
-  return *emu::shared_ptr<uint32_t>(addr);
-}
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-  return *emu::shared_ptr<float>(addr);
-}
-__device__ __forceinline__ int2 lds_v2(uint32_t addr) {
-  return *emu::shared_ptr<int2>(addr);
-}
-__device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
-  *emu::shared_ptr<float>(addr) = v;
-}
-__device__ __forceinline__ void red_shared_add(uint32_t addr, float v) {
-  atomicAdd(emu::shared_ptr<float>(addr), v);
-}
-__device__ __forceinline__ float fexp(float x) {
-  return exp2f(x * 1.4426950408889634f);
-}
-__device__ __forceinline__ float flog1p(float x) {
-  const float y = log2f(1.0f + x);
-  return (x < 1e-3f) ? x * (1.0f - 0.5f * x) : y * 0.6931471805599453f;
-}
-#else
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-/* makes the mbarrier.init of the elected thread visible to the async proxy */
-__device__ __forceinline__ void mbar_init_fence() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-/* producer-side wait: the slot frees up a whole level later, so sleep between polls instead
- * of burning the consumers' issue slots */
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0;
-  for (;;) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (done) break;
-    __nanosleep(64);
-  }
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-/* TMA 1-D bulk copy global -> shared, completion on an mbarrier */
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar)
-      : "memory");
-}
-template <int NC>
-__device__ __forceinline__ void consumer_bar() {
-  asm volatile("bar.sync 1, %0;" ::"n"(NC) : "memory");
-}
-
-/* shared-memory accesses through 32-bit shared-window addresses: keeps the per-level
- * address arithmetic in 32-bit integer ops instead of 64-bit generic pointers */
-__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ int2 lds_v2(uint32_t addr) {
-  int2 v;
-  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-__device__ __forceinline__ void red_shared_add(uint32_t addr, float v) {
-  asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-
-/* exp / log1p on the SFU: one MUFU each (ex2.approx.ftz / lg2.approx.ftz) */
-__device__ __forceinline__ float fexp(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x * 1.4426950408889634f));
-  return y;
-}
-__device__ __forceinline__ float flog1p(float x) {
-  // x = sum(exp(s - max)) - 1 >= 0; series near 0 keeps the relative accuracy log1p is used for
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(1.0f + x));
-  return (x < 1e-3f) ? x * (1.0f - 0.5f * x) : y * 0.6931471805599453f;
-}
-
-#endif // GTNB_HOST_EMU
 
 /* Shared-memory carve-up, computed on the host and passed by value. */
 struct Layout {
@@ -254,7 +92,7 @@ Layout make_layout(int max_lvl_nodes, int max_lvl_arcs, int L, int log2_stages, 
 template <int MODE>
 __device__ __noinline__ float fwd_node_any(uint32_t r0raw, int r0, int r1, const int2* st_arc, const float* prev) {
   const bool is_start = (r0raw & kStartBit) != 0;
-  float mx = neg_inf();
+  float mx = -CUDART_INF_F;
 #pragma unroll 1
   for (int a = r0; a < r1; a++) {
     const int2 rec = st_arc[a];
@@ -285,17 +123,17 @@ __device__ __forceinline__ float fwd_node(
   const int deg = (int)(r1raw & kRowMask) - r0;
   if (deg > 3 || (r0raw & kStartBit)) return fwd_node_any<MODE>(r0raw, r0, r0 + deg, st_arc, prev);
   const uint32_t a = A + 8u * r0;
-  float v0 = neg_inf(), v1 = neg_inf(), v2 = neg_inf();
+  float v0 = -CUDART_INF_F, v1 = -CUDART_INF_F, v2 = -CUDART_INF_F;
   if (deg > 0) {
-    const int2 rec = lds_v2(a);
+    const int2 rec = lds_v2_u32(a);
     v0 = lds_f32(P + 4u * rec.x) + __int_as_float(rec.y);
   }
   if (deg > 1) {
-    const int2 rec = lds_v2(a + 8u);
+    const int2 rec = lds_v2_u32(a + 8u);
     v1 = lds_f32(P + 4u * rec.x) + __int_as_float(rec.y);
   }
   if (deg > 2) {
-    const int2 rec = lds_v2(a + 16u);
+    const int2 rec = lds_v2_u32(a + 16u);
     v2 = lds_f32(P + 4u * rec.x) + __int_as_float(rec.y);
   }
   const float mx = fmaxf(fmaxf(v0, v1), v2);
@@ -358,7 +196,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
       uint32_t par = 0; // wraps & 1: the slot's previous use is empty-phase (wraps - 1)
 #pragma unroll 1
       for (int l = 0; l < L; l++) {
-        if (l >= S) mbar_wait_relaxed(sbase + 8 * (kMaxStages + s), par ^ 1);
+        if (l >= S) mbar_wait_sleep(sbase + 8 * (kMaxStages + s), par ^ 1);
         const uint32_t st = sbase + lay.off_stage + s * lay.stage_bytes;
         const uint32_t fb = sbase + 8 * s;
         const int lo = s_lvln[l], hi = s_lvln[l + 1];
@@ -427,7 +265,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
       const int deg = r1 - r0;
       if (MODE == MODE_PATH) {
         // strictly-greater relaxations in arc order; a start node begins at 0 (shortest.cpp:202-218)
-        float best = neg_inf();
+        float best = -CUDART_INF_F;
         int barc = 0x7fffffff;
         for (int a = r0 + sub; a < r1; a += G) {
           const int2 rec = st_arc[a];
@@ -458,7 +296,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
           bp[lo + i] = (barc == 0x7fffffff) ? -1 : barc;
         }
       } else {
-        float mx = neg_inf();
+        float mx = -CUDART_INF_F;
 #pragma unroll 1
         for (int a = r0 + sub; a < r1; a += G) {
           const int2 rec = st_arc[a];
@@ -490,7 +328,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
         }
       }
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     if (tid == 0) mbar_arrive(sbase + 8 * (kMaxStages + s));
     if (++s == S) {
       s = 0;
@@ -503,7 +341,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
   // accept nodes (all in the last level): shortest.cpp:147-159 / :226-237
   if (tid == 0) {
     const int32_t* acc = acc_nodes + m.acc_base;
-    float mx = neg_inf();
+    float mx = -CUDART_INF_F;
     int best = -1;
     for (int k = 0; k < m.n_accept; k++) {
       const float v = __ldcg(&sc[acc[k]]);
@@ -515,7 +353,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
     float out;
     if (MODE == MODE_LOG) {
       if (m.n_accept == 0) {
-        out = neg_inf();
+        out = -CUDART_INF_F;
       } else if (mx == CUDART_INF_F || mx == -CUDART_INF_F) {
         out = mx;
       } else {
@@ -524,7 +362,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
         out = mx + log1pf(sum);
       }
     } else {
-      out = (m.n_accept == 0) ? neg_inf() : mx;
+      out = (m.n_accept == 0) ? -CUDART_INF_F : mx;
     }
     out_scores[blockIdx.x] = out;
     best_accept[blockIdx.x] = best;
@@ -540,7 +378,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_forward_staged
 __device__ __noinline__ void bwd_node_any(
     uint32_t r0raw, int r0, int r1, float g, float sn, float delta, const int2* st_arc,
     const float* st_psc, float* ng_prev, float* ag) {
-  float mx = neg_inf();
+  float mx = -CUDART_INF_F;
 #pragma unroll 1
   for (int a = r0; a < r1; a++) {
     const int2 rec = st_arc[a];
@@ -578,7 +416,7 @@ __device__ __forceinline__ void bwd_node(
 #pragma unroll
   for (int j = 0; j < 3; j++) {
     if (j < deg) {
-      const int2 rec = lds_v2(a + 8u * j);
+      const int2 rec = lds_v2_u32(a + 8u * j);
       const float cur = g * fexp(lds_f32(P + 4u * rec.x) + __int_as_float(rec.y) - sn);
       red_shared_add(NGp + 4u * rec.x, cur);
       ag[r0 + j] = cur * delta;
@@ -648,7 +486,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_backward_stage
 #pragma unroll 1
       for (int k = 0; k < iters; k++) {
         const int l = L - 1 - k;
-        if (k >= S) mbar_wait_relaxed(sbase + 8 * (kMaxStages + s), par ^ 1);
+        if (k >= S) mbar_wait_sleep(sbase + 8 * (kMaxStages + s), par ^ 1);
         const uint32_t st = sbase + lay.off_stage + s * lay.stage_bytes;
         const uint32_t fb = sbase + 8 * s;
         const int plo = s_lvln[l - 1], lo = s_lvln[l], hi = s_lvln[l + 1];
@@ -684,20 +522,20 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_backward_stage
     const int lo = L > 0 ? s_lvln[L - 1] : 0, hi = L > 0 ? s_lvln[L] : 0;
     for (int i = tid; i < hi - lo; i += kConsumers) s_top[i] = gsc[lo + i];
     for (int i = tid; i < 3 * lay.win_nodes; i += kConsumers) s_ng[i] = 0.0f;
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     if (tid == 0 && L > 0) {
       const int32_t* acc = acc_nodes + m.acc_base;
       if (TROPICAL) {
         const int best = best_accept[blockIdx.x];
         if (best >= 0) s_ng[best - lo] += 1.0f;
       } else {
-        float mx = neg_inf();
+        float mx = -CUDART_INF_F;
         for (int k = 0; k < m.n_accept; k++) mx = fmaxf(mx, s_top[acc[k] - lo]);
         const float denom = expf(out_scores[blockIdx.x] - mx);
         for (int k = 0; k < m.n_accept; k++) s_ng[acc[k] - lo] += expf(s_top[acc[k] - lo] - mx) / denom;
       }
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
   }
 
   int s = 0;
@@ -746,7 +584,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_backward_stage
       }
       if (TROPICAL) {
         // the arc the forward pass cached as its first maximum (shortest.cpp:124-127,131-134)
-        float mx = neg_inf();
+        float mx = -CUDART_INF_F;
         int arg = 0x7fffffff;
         for (int a = r0 + sub; a < r1; a += G) {
           const int2 rec = st_arc[a];
@@ -777,7 +615,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_backward_stage
         const bool exact = !(fabsf(sn) < CUDART_INF_F); // +-inf / NaN score: reference formula verbatim
         float mx = 0.0f;
         if (exact) {
-          mx = neg_inf();
+          mx = -CUDART_INF_F;
 #pragma unroll 1
           for (int a = r0; a < r1; a++) {
             const int2 rec = st_arc[a];
@@ -798,7 +636,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(G) + 32) sd_backward_stage
       }
     }
     for (int i = tid; i < lay.win_nodes; i += kConsumers) ng_zero[i] = 0.0f;
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     // the previous iteration's stage held this level's own scores: free it now,
     // and keep this iteration's score window (level l-1) as the next "own"
     if (tid == 0 && k > 0) mbar_arrive(sbase + 8 * (kMaxStages + (s == 0 ? S - 1 : s - 1)));
@@ -823,16 +661,16 @@ __device__ __noinline__ float fused_row_any(float g, float sn, int e0, int e1, u
   const bool exact = !(fabsf(sn) < CUDART_INF_F);
   float mx = 0.0f, acc = 0.0f;
   if (exact) {
-    mx = neg_inf();
+    mx = -CUDART_INF_F;
 #pragma unroll 1
     for (int e = e0; e < e1; e++) {
-      const int2 rec = lds_v2(Ae + 8u * e);
+      const int2 rec = lds_v2_u32(Ae + 8u * e);
       mx = fmaxf(mx, lds_f32(P + 4u * rec.x) + __int_as_float(rec.y));
     }
   }
 #pragma unroll 1
   for (int e = e0; e < e1; e++) {
-    const int2 rec = lds_v2(Ae + 8u * e);
+    const int2 rec = lds_v2_u32(Ae + 8u * e);
     const float cur = arc_grad_log(g, lds_f32(P + 4u * rec.x) + __int_as_float(rec.y), sn, mx, exact);
     sts_f32(CUR + 4u * e, cur);
     acc += cur;
@@ -857,18 +695,18 @@ __device__ __noinline__ void fused_level_slow(
       const float acc = fused_row_any(lds_f32(NGc + 4u * i), lds_f32(OWN + 4u * i), e0, e1, Ae, P, CUR);
       if (e1 > e0) atomicAdd(&gem_l[t_label[i]], acc * delta);
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     for (int u = tid; u < N1; u += kConsumers) {
       float sum = 0.0f;
 #pragma unroll 1
       for (int q = t_outptr[u]; q < t_outptr[u + 1]; q++) sum += lds_f32(CUR + 4u * t_outent[q]);
       sts_f32(NGp0 + 4u * u, sum);
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     return;
   }
   for (int i = tid; i < win_nodes; i += kConsumers) sts_f32(NGp0 + 4u * i, 0.0f);
-  consumer_bar<kConsumers>();
+  bar_named<1, kConsumers>();
   for (int i = tid; i < cnt; i += kConsumers) {
     const uint32_t r0raw = lds_u32(R + 4u * i);
     const int r0 = (int)(r0raw & kRowMask);
@@ -878,24 +716,24 @@ __device__ __noinline__ void fused_level_slow(
     const bool exact = !(fabsf(sn) < CUDART_INF_F) || (r0raw & kStartBit);
     float mx = 0.0f;
     if (exact) {
-      mx = neg_inf();
+      mx = -CUDART_INF_F;
 #pragma unroll 1
       for (int a = r0; a < r1; a++) {
-        const int2 rec = lds_v2(A + 8u * a);
+        const int2 rec = lds_v2_u32(A + 8u * a);
         mx = fmaxf(mx, lds_f32(P + 4u * rec.x) + __int_as_float(rec.y));
       }
       if (r0raw & kStartBit) mx = fmaxf(mx, 0.0f);
     }
 #pragma unroll 1
     for (int a = r0; a < r1; a++) {
-      const int2 rec = lds_v2(A + 8u * a);
+      const int2 rec = lds_v2_u32(A + 8u * a);
       const float v = lds_f32(P + 4u * rec.x) + __int_as_float(rec.y);
       const float cur = arc_grad_log(g, v, sn, mx, exact);
       red_shared_add(NGp + 4u * rec.x, cur);
       atomicAdd(&gem[ggi[a].y], cur * delta);
     }
   }
-  consumer_bar<kConsumers>();
+  bar_named<1, kConsumers>();
 }
 
 /*
@@ -976,7 +814,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
 #pragma unroll 1
       for (int k = 0; k < iters; k++) {
         const int l = L - 1 - k;
-        if (k >= S) mbar_wait_relaxed(sbase + 8 * (kMaxStages + s), par ^ 1);
+        if (k >= S) mbar_wait_sleep(sbase + 8 * (kMaxStages + s), par ^ 1);
         const uint32_t st = sbase + lay.off_stage + s * lay.stage_bytes;
         const uint32_t fb = sbase + 8 * s;
         const int plo = s_lvln[l - 1], lo = s_lvln[l], hi = s_lvln[l + 1];
@@ -1014,25 +852,25 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
     int* t_src = reinterpret_cast<int*>(s_cur); // borrowed until the tables are built
     for (int i = tid; i <= N1; i += kConsumers) t_inptr[i] = ip[i];
     for (int e = tid; e < A1; e += kConsumers) t_src[e] = is[e];
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     for (int u = tid; u < N1; u += kConsumers) {
       t_label[u] = (t_inptr[u] < t_inptr[u + 1]) ? il[t_inptr[u]] : 0;
       int c = 0;
       for (int e = 0; e < A1; e++) c += (t_src[e] == u);
       t_outptr[u + 1] = c;
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     if (tid == 0) {
       t_outptr[0] = 0;
       for (int u = 0; u < N1; u++) t_outptr[u + 1] += t_outptr[u];
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     for (int u = tid; u < N1; u += kConsumers) {
       int pos = t_outptr[u];
       for (int e = 0; e < A1; e++)
         if (t_src[e] == u) t_outent[pos++] = e;
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
   }
 
   // top level: its own scores, and the accept seeds (shortest.cpp:49-60)
@@ -1040,15 +878,15 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
     const int lo = L > 0 ? s_lvln[L - 1] : 0, hi = L > 0 ? s_lvln[L] : 0;
     for (int i = tid; i < hi - lo; i += kConsumers) s_top[i] = gsc[lo + i];
     for (int i = tid; i < 2 * lay.win_nodes; i += kConsumers) s_ng[i] = 0.0f;
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
     if (tid == 0 && L > 0) {
       const int32_t* acc = acc_nodes + m.acc_base;
-      float mx = neg_inf();
+      float mx = -CUDART_INF_F;
       for (int k = 0; k < m.n_accept; k++) mx = fmaxf(mx, s_top[acc[k] - lo]);
       const float denom = expf(out_scores[blockIdx.x] - mx);
       for (int k = 0; k < m.n_accept; k++) s_ng[acc[k] - lo] += expf(s_top[acc[k] - lo] - mx) / denom;
     }
-    consumer_bar<kConsumers>();
+    bar_named<1, kConsumers>();
   }
 
   // per-thread constants of "my" graph node (thread u <-> node u while N1 <= kConsumers)
@@ -1113,19 +951,19 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
         } else {
           const uint32_t ae = Ae + 8u * my_e0, ce = CUR + 4u * my_e0;
           if (deg > 0) {
-            const int2 rec = lds_v2(ae);
+            const int2 rec = lds_v2_u32(ae);
             const float cur = g * fexp(lds_f32(P + 4u * rec.x) + __int_as_float(rec.y) - sn);
             sts_f32(ce, cur);
             acc += cur;
           }
           if (deg > 1) {
-            const int2 rec = lds_v2(ae + 8u);
+            const int2 rec = lds_v2_u32(ae + 8u);
             const float cur = g * fexp(lds_f32(P + 4u * rec.x) + __int_as_float(rec.y) - sn);
             sts_f32(ce + 4u, cur);
             acc += cur;
           }
           if (deg > 2) {
-            const int2 rec = lds_v2(ae + 16u);
+            const int2 rec = lds_v2_u32(ae + 16u);
             const float cur = g * fexp(lds_f32(P + 4u * rec.x) + __int_as_float(rec.y) - sn);
             sts_f32(ce + 8u, cur);
             acc += cur;
@@ -1133,7 +971,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
         }
         if (deg > 0) atomicAdd(&gem_l[my_lab], acc * delta);
       }
-      consumer_bar<kConsumers>();
+      bar_named<1, kConsumers>();
       if (tid < N1) {
         // phase 2: source node `tid` gathers its out-arcs (no atomics, fixed order)
         float sum = 0.0f;
@@ -1147,7 +985,7 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
         g_in_reg = true;
         if (!next_steady) sts_f32(NGp0 + 4u * tid, sum);
       }
-      if (!next_steady) consumer_bar<kConsumers>();
+      if (!next_steady) bar_named<1, kConsumers>();
     } else {
       g_in_reg = false;
       fused_level_slow(

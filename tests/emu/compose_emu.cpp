@@ -9,10 +9,7 @@
 #include "../../gtn_b200/csrc/k_compose.cu"
 #include "../../gtn_b200/csrc/k_shortest.cu"
 #include "../../gtn_b200/csrc/k_order.cu"
-// k_shortest.cu and k_staged.cu each keep a file-local neg_inf(): one translation unit here
-#define neg_inf staged_neg_inf
 #include "../../gtn_b200/csrc/k_staged.cu"
-#undef neg_inf
 
 #include <vector>
 

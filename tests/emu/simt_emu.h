@@ -6,8 +6,8 @@
  * barrier.  It checks index arithmetic, barrier placement (a misplaced barrier deadlocks or trips the
  * result), shuffle semantics and tails; it does not model the memory system or timing.
  *
- * A kernel file opts in with `#ifdef GTNB_HOST_EMU` around its CUDA includes, its inline PTX
- * helpers and its launchers (gtn_b200/csrc/k_banded.cu).
+ * A kernel file opts in by including gtn_b200/csrc/gtnb_ptx.h, which holds the emulated form of every
+ * inline-PTX helper next to its PTX, and by `#ifndef GTNB_HOST_EMU` around its launchers.
  */
 #pragma once
 

@@ -13,8 +13,9 @@ def build(name, kernels):
     """tests/emu/<name>_emu.cpp + the kernel sources it includes -> tests/emu/lib<name>_emu.so (path).
     Skips the calling test when the toolchain cannot build it (no C++20 <barrier>)."""
     so = os.path.join(EMU, "lib%s_emu.so" % name)
+    # every kernel file includes gtnb_ptx.h, which includes gtnb_meta.h
     src = [os.path.join(EMU, "%s_emu.cpp" % name), os.path.join(EMU, "simt_emu.h")] + \
-          [os.path.join(CSRC, k) for k in kernels]
+          [os.path.join(CSRC, k) for k in kernels + ["gtnb_ptx.h", "gtnb_meta.h"]]
     if os.path.exists(so) and all(os.path.getmtime(s) <= os.path.getmtime(so) for s in src):
         return so
     cmd = ["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-Wno-unknown-pragmas", "-I", EMU, "-I", CSRC,

@@ -53,3 +53,14 @@ def test_product_library_contains_no_emulation_code():
     so = os.path.join(ROOT, "gtn_b200", "lib", "libgtn_b200.so")
     syms = subprocess.run(["nm", "-DC", "--defined-only", so], capture_output=True, text=True).stdout
     assert "emu::" not in syms and "simt" not in syms.lower()
+
+
+def test_kernel_files_contain_no_inline_ptx():
+    """Inline PTX lives in gtnb_ptx.h only, next to the emulated form tests/emu runs instead of it, so that one
+    file shows every place where the emulated kernel sources differ from the compiled ones."""
+    import glob
+    import re
+    files = sorted(glob.glob(os.path.join(ROOT, "gtn_b200", "csrc", "k_*.cu")))
+    assert files
+    offenders = [os.path.basename(f) for f in files if re.search(r"\basm\b", open(f).read())]
+    assert offenders == []
