@@ -104,6 +104,9 @@ SYMBOLS = [
     ("gtnb_graph_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _f32p, _vp, C.c_int,
       _vp, C.c_int]),
+    ("gtnb_graph_transitions_loss", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.c_int, _vp, C.c_int,
+      _f32p, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int]),
 ]
 
 _lib = None
@@ -534,6 +537,64 @@ class Ctx:
             for buf in bufs:
                 buf.free()
         return losses, grads, ag
+
+    def graph_transitions_loss(self, emissions, views, trans_w, kind=DENSE_ASG, want_grad=True, input_lens=None,
+                               arc_weights=None):
+        """Host-buffer entry of gtnb_graph_transitions_loss: emissions [B,T,C], views: B (view, keepalive) pairs from
+        make_view, trans_w [C + C*C] (DENSE_ASG) or [C*C] (DENSE_BIGRAM), arc_weights [sum A_b] or None
+        -> (losses [B], grads [B,T,C] or None, arc_grads [sum A_b] or None, trans_grad or None)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
+        assert aw is None or aw.size == n_arcs
+        losses = np.zeros(B, np.float32)
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
+        tg = np.full(tw.size, np.nan, np.float32) if want_grad else None
+        self._check(lib().gtnb_graph_transitions_loss(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0, kind,
+            tw.ctypes.data, 0, _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0,
+            None if ag is None else ag.ctypes.data, 0, None if tg is None else tg.ctypes.data, 0))
+        return losses, grads, None if ag is None else ag[:n_arcs], tg
+
+    def graph_transitions_loss_dev(self, emissions, views, trans_w, kind=DENSE_ASG, input_lens=None,
+                                   arc_weights=None):
+        """Device-buffer entry: emissions, trans_w (and arc_weights, when given) uploaded once,
+        gtnb_graph_transitions_loss on device pointers (gradients in HBM), downloaded afterwards
+        -> (losses, grads, arc_grads, trans_grad)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        losses = np.zeros(B, np.float32)
+        bufs = [self.to_device(e), self.alloc(max(e.nbytes, 16)), self.alloc(4 * max(n_arcs, 4)), self.to_device(tw),
+                self.alloc(tw.nbytes)]
+        e_dev, g_dev, ag_dev, w_dev, tg_dev = bufs
+        aw_dev = None
+        if arc_weights is not None:
+            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
+            assert aw.size == n_arcs
+            aw_dev = self.to_device(aw)
+            bufs.append(aw_dev)
+        try:
+            self._check(lib().gtnb_graph_transitions_loss(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if aw_dev is None else aw_dev.ptr, 1, kind,
+                w_dev.ptr, 1, _p(losses, _f32p), g_dev.ptr, 1, ag_dev.ptr, 1, tg_dev.ptr, 1))
+            grads = g_dev.download(e.shape)
+            ag = ag_dev.download((max(n_arcs, 1),))[:n_arcs]
+            tg = tg_dev.download(tw.shape)
+        finally:
+            for buf in bufs:
+                buf.free()
+        return losses, grads, ag, tg
 
 
 class Lattice:

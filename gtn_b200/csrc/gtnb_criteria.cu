@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "gtnb_internal.h"
+#include "gtnb_product.h"
 
 using namespace gtnb;
 
@@ -706,27 +707,54 @@ struct AsgGraphs {
   std::vector<int32_t> map; // transitions arc of every chain arc
 };
 
-void build_asg_graphs(int C, const float* trans_w_host, const Targets& t, AsgGraphs* g) {
-  const int nTrans = C + C * C;
-  HostGraph& tr = g->trans;
-  tr.flags.assign(C + 1, 2);
-  tr.flags[0] = 1;
-  tr.src.resize(nTrans);
-  tr.dst.resize(nTrans);
-  tr.label.resize(nTrans);
-  tr.w.assign(trans_w_host, trans_w_host + nTrans);
+/*
+ * The dense transition graph G of the trellis criteria from host weights, and the trans_w slot of every arc (map,
+ * nullable).  ASG (criterion_test.cpp:244-254, w = [s | W]): node 0 starts, nodes 1..C accept, arc i = 0 -> i+1 of
+ * weight s[i], arc C + i*C + j = j+1 -> i+1 of weight W[i][j] (arc k reads w[k]).  BIGRAM (benchmarks/ctc.cpp
+ * transitionsGraph with a label-determined destination, w = W): C nodes, all start and accept, arc j*C + i = j -> i
+ * of weight W[i][j].  The arc into state i carries label i.
+ */
+void dense_graph(bool bigram, int C, const float* w, HostGraph* G, std::vector<int32_t>* map) {
+  const long long CC = (long long)C * C, n = bigram ? CC : C + CC;
+  G->src.resize(n);
+  G->dst.resize(n);
+  G->label.resize(n);
+  G->w.resize(n);
+  if (map) map->resize(n);
+  if (bigram) {
+    G->flags.assign(C, 3);
+    for (int j = 0; j < C; j++)
+      for (int i = 0; i < C; i++) {
+        const long long k = (long long)j * C + i;
+        G->src[k] = j;
+        G->dst[k] = i;
+        G->label[k] = i;
+        G->w[k] = w[(long long)i * C + j];
+        if (map) (*map)[k] = i * C + j;
+      }
+    return;
+  }
+  G->flags.assign(C + 1, 2);
+  G->flags[0] = 1;
+  G->w.assign(w, w + n);
   for (int i = 0; i < C; i++) {
-    tr.src[i] = 0;
-    tr.dst[i] = i + 1;
-    tr.label[i] = i;
+    G->src[i] = 0;
+    G->dst[i] = i + 1;
+    G->label[i] = i;
   }
   for (int i = 0; i < C; i++)
     for (int j = 0; j < C; j++) {
       const int a = C + i * C + j;
-      tr.src[a] = j + 1;
-      tr.dst[a] = i + 1;
-      tr.label[a] = i;
+      G->src[a] = j + 1;
+      G->dst[a] = i + 1;
+      G->label[a] = i;
     }
+  if (map)
+    for (long long k = 0; k < n; k++) (*map)[k] = (int32_t)k;
+}
+
+void build_asg_graphs(int C, const float* trans_w_host, const Targets& t, AsgGraphs* g) {
+  dense_graph(false, C, trans_w_host, &g->trans, nullptr);
   // compose(fal_b, transitions): node l = "l labels consumed"; arcs: 0->1, then per node a
   // self loop and the step to the next label, in the reference's creation order
   g->chains.resize(t.B);
@@ -887,38 +915,75 @@ struct TrellisCriterion {
   // n-gram: the numerator's start arcs carry sigma_i = logsumexp_j W[i][j] (launch_ngram_sigma), whose gradient C
   // extra slots after W's collect and launch_ngram_fold folds into W's; the gradient is then never built in place
   bool fold;
-  decltype(&launch_ngram_num_build) num_build;
   decltype(&launch_ngram_den_forward) den_forward;
   decltype(&launch_ngram_den_backward) den_backward;
 };
 
-int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const TransitionArgs& a, const Targets& t,
-                      const std::vector<SgDims>& dims, bool* needs_exact) {
+/*
+ * The numerator of gtnb_ngram_ctc_loss / gtnb_asg_loss_ex: graphs built on the device from the targets
+ * (launch_ngram_num_build / launch_asg_num_build) straight into the small-graph tables of an implicit lattice.
+ * The interface of trellis_loss_fast's numerators: alloc (scratch and, where it can, the lattice), stage (uploads in
+ * the call's one staging pass), build (on the call's stream once the transitions and sigma are there), T_dev (the
+ * frame counts), map (the transition slot of every numerator arc, tot_A of them), scatter (the arc gradient's
+ * other destinations).
+ */
+struct TargetsNumerator {
+  using Build = int (*)(gtnb_ctx*, gtnb_lattice*, const int32_t*, const int32_t*, const int32_t*, int, const float*,
+                        const float*, int32_t*);
+  const Targets& t;
+  const std::vector<SgDims>& dims;
+  int C;
+  Build build_kernel;
+  int blank;
+  long long tot_A = 0;
+  std::vector<int32_t> small_h;
+  int32_t *small_dev = nullptr, *map = nullptr;
+
+  bool wants_arc_grads() const { return false; }
+  int alloc(CallScope& scope, const float* e_dev, long long per, gtnb_lattice** lat) {
+    std::vector<long long> sgn, sga;
+    tot_A = 0;
+    for (int b = 0; b < t.B; b++) tot_A += dims[b].A;
+    small_h = t.packed();
+    GTNB_TRY(scope.alloc(&small_dev, (long long)small_h.size()));
+    GTNB_TRY(scope.alloc(&map, tot_A));
+    return composed_alloc(scope.ctx(), t.B, dims.data(), t.B, 0, t.T(), C, e_dev, per, sgn, sga, lat, true);
+  }
+  int stage(CallScope& scope, gtnb_lattice* lat) {
+    GTNB_TRY(stage_upload(scope.ctx(), lat->meta, lat->meta_h.data(), sizeof(GraphMeta) * t.B));
+    return stage_upload(scope.ctx(), small_dev, small_h.data(), sizeof(int32_t) * small_h.size());
+  }
+  const int32_t* T_dev() const { return small_dev + t.tot_t + 2ll * t.B; }
+  int build(CallScope& scope, gtnb_lattice*& lat, const float* w_dev, const float* sigma) {
+    return build_kernel(scope.ctx(), lat, small_dev, small_dev + t.tot_t, small_dev + t.tot_t + t.B, blank, w_dev,
+                        sigma, map);
+  }
+  int scatter(CallScope&, const float*) { return GTNB_OK; }
+};
+
+template <class Numerator>
+int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const TransitionArgs& a, Numerator& num,
+                      bool* needs_exact) {
   gtnb_ctx* ctx = scope.ctx();
   const int B = a.B, T = a.T, C = a.C;
-  const long long per = (long long)T * C, tot_t = t.tot_t;
-  const bool want = a.grads || a.trans_grad;
-  long long tot_A = 0;
-  for (int b = 0; b < B; b++) tot_A += dims[b].A;
+  const long long per = (long long)T * C;
+  const bool want = a.grads || a.trans_grad || num.wants_arc_grads();
   float *e_dev = nullptr, *w_dev = nullptr, *sigma = nullptr, *alpha = nullptr, *den = nullptr;
   float *ggrad = nullptr, *minus1 = nullptr;
-  int32_t *small_dev = nullptr, *status = nullptr, *map = nullptr;
+  int32_t* status = nullptr;
   OutBuf g, tg;
-  std::vector<long long> sgn, sga;
   std::vector<float> m1(B, -1.0f);
   gtnb_lattice*& lat = scope.lattice();
 
   GTNB_TRY(ensure_side_streams(ctx, 0, 0));
   GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
   GTNB_TRY(scope.borrow(a.trans_w, a.trans_on_device != 0, k.n_trans, &w_dev)); // (host: staged below)
-  const std::vector<int32_t> small_h = t.packed();
-  GTNB_TRY(scope.alloc(&small_dev, (long long)small_h.size()));
   GTNB_TRY(scope.alloc(&status, 2ll * B));
   if (k.fold) GTNB_TRY(scope.alloc(&sigma, C));
   GTNB_TRY(scope.alloc(&alpha, k.alpha_floats));
   GTNB_TRY(scope.alloc(&den, B));
-  GTNB_TRY(scope.alloc(&map, tot_A));
-  GTNB_TRY(composed_alloc(ctx, B, dims.data(), B, 0, t.T(), C, e_dev, per, sgn, sga, &lat, true));
+  GTNB_TRY(num.alloc(scope, e_dev, per, &lat));
+  const long long tot_A = num.tot_A;
   if (want) {
     const long long n_grad = k.n_trans + (k.fold ? C : 0); // [d/dtrans | d/dsigma]
     GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
@@ -930,16 +995,16 @@ int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const Transit
     if (tot_A) GTNB_CUDA(ctx, cudaMemsetAsync(ggrad, 0, sizeof(float) * tot_A, ctx->stream));
   }
   GTNB_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(int32_t) * 2 * B, ctx->stream));
-  // one pinned staging pass: descriptors, [targets | offsets | lens | T], the transitions from the host, the -1 seeds
+  // one pinned staging pass: the numerator's (descriptors, [targets | offsets | lens | T] or the product maps), the
+  // transitions from the host, the -1 seeds
   GTNB_TRY(stage_begin(ctx));
-  GTNB_TRY(stage_upload(ctx, lat->meta, lat->meta_h.data(), sizeof(GraphMeta) * B));
-  GTNB_TRY(stage_upload(ctx, small_dev, small_h.data(), sizeof(int32_t) * small_h.size()));
+  GTNB_TRY(num.stage(scope, lat));
   if (!a.trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, a.trans_w, sizeof(float) * k.n_trans));
   if (want) GTNB_TRY(stage_upload(ctx, minus1, m1.data(), sizeof(float) * B));
   GTNB_TRY(stage_end(ctx));
 
   if (k.fold) GTNB_TRY(launch_ngram_sigma(ctx, C, w_dev, sigma));
-  GTNB_TRY(k.num_build(ctx, lat, small_dev, small_dev + tot_t, small_dev + tot_t + B, a.blank, w_dev, sigma, map));
+  GTNB_TRY(num.build(scope, lat, w_dev, sigma));
   // the numerator (a few in-arcs per node) on the second stream beside the denominator (C^2 per frame)
   GTNB_TRY(fork_to(ctx, ctx->copy_stream));
   {
@@ -947,13 +1012,14 @@ int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const Transit
     GTNB_TRY(launch_implicit_forward(ctx, lat, status + B));
     if (want) GTNB_TRY(launch_implicit_backward(ctx, lat, minus1, g.dev, per, 0, -1, ggrad));
   }
-  const int32_t* T_dev = small_dev + tot_t + 2ll * B;
+  const int32_t* T_dev = num.T_dev();
   GTNB_TRY(k.den_forward(ctx, B, T, C, T_dev, e_dev, per, w_dev, alpha, den, status));
   if (want) GTNB_TRY(k.den_backward(ctx, B, T, C, T_dev, e_dev, per, w_dev, alpha, den, g.dev, per, tg.dev));
   GTNB_TRY(join_from(ctx, ctx->copy_stream));
   if (want) {
-    GTNB_TRY(launch_scatter_add(ctx, tg.dev, map, ggrad, tot_A)); // numerator arcs -> transition (and sigma) slots
+    GTNB_TRY(launch_scatter_add(ctx, tg.dev, num.map, ggrad, tot_A)); // numerator arcs -> transition (and sigma) slots
     if (k.fold) GTNB_TRY(launch_ngram_fold(ctx, C, w_dev, sigma, tg.dev));
+    GTNB_TRY(num.scatter(scope, ggrad));
     GTNB_TRY(g.copy_out(ctx, per * B));
     GTNB_TRY(tg.copy_out(ctx, k.n_trans));
   }
@@ -961,36 +1027,78 @@ int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const Transit
 }
 
 /*
- * n-gram CTC through materialised lattices, graph by graph as the reference composes them: intersect(E_b, G) and
- * intersect(P_b, E_b), where P_b = intersect(ctc_b, G) is built on the host WITHOUT the fold (C start states
- * (0, s), then (l, label(l))).  Reproduces the reference's inf / NaN propagation arc by arc; the path for
- * non-finite weights.
+ * The materialised route of the trellis criteria, graph by graph as the reference composes them: the denominator
+ * compose(E_b, G) (G from dense_graph, one for the batch, gmap its arcs' transition slots) and the numerator
+ * compose(P_b, E_b) with the host-built products P_b (pmap: the transition slot of every arc, in batch order).
+ * arc_of (nullable): the slot of arc_grads (tot_arcs floats) of every numerator arc.  Reproduces the reference's
+ * inf / NaN propagation arc by arc; the path for non-finite weights.
+ */
+int transitions_loss_materialised(CallScope& scope, const TransitionArgs& a, const int32_t* Tb, const HostGraph& G,
+                                  const std::vector<int32_t>& gmap, long long n_trans,
+                                  const std::vector<gtnb_graph_view>& pviews, const std::vector<int32_t>& pmap,
+                                  const std::vector<int32_t>* arc_of, const OutBuf* arc_grads, long long tot_arcs) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, nG = (long long)gmap.size(), nP = (long long)pmap.size();
+  const bool want = a.grads || a.trans_grad || arc_grads;
+  const gtnb_graph_view gview = G.view();
+  float *e_dev = nullptr, *ft_grad = nullptr, *gg_grad = nullptr;
+  int32_t *ft_map_dev = nullptr, *gg_map_dev = nullptr, *arc_of_dev = nullptr;
+  OutBuf g, tg;
+  gtnb_lattice*& den = scope.lattice();
+  gtnb_lattice*& num = scope.lattice();
+  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
+  GTNB_TRY(gtnb_compose_linear(ctx, B, &gview, 1, 1, Tb, C, e_dev, per, &den));
+  GTNB_TRY(gtnb_compose_linear(ctx, B, pviews.data(), B, 0, Tb, C, e_dev, per, &num));
+  GTNB_TRY(gtnb_forward(ctx, den, 0, nullptr, nullptr));
+  GTNB_TRY(gtnb_forward(ctx, num, 0, nullptr, nullptr));
+  if (want) {
+    GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
+    GTNB_CUDA(ctx, cudaMemsetAsync(g.dev, 0, sizeof(float) * per * B, ctx->stream));
+    GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, n_trans, &tg, /*alias=*/false));
+    GTNB_TRY(scope.alloc(&gg_grad, nG));
+    GTNB_TRY(scope.alloc(&ft_grad, std::max<long long>(nP, 1)));
+    GTNB_TRY(scope.alloc(&gg_map_dev, nG));
+    GTNB_TRY(scope.alloc(&ft_map_dev, std::max<long long>(nP, 1)));
+    if (arc_of) GTNB_TRY(scope.alloc(&arc_of_dev, std::max<long long>(nP, 1)));
+    GTNB_CUDA(ctx, cudaMemsetAsync(tg.dev, 0, sizeof(float) * n_trans, ctx->stream));
+    GTNB_CUDA(ctx, cudaMemsetAsync(gg_grad, 0, sizeof(float) * nG, ctx->stream));
+    GTNB_CUDA(ctx, cudaMemsetAsync(ft_grad, 0, sizeof(float) * std::max<long long>(nP, 1), ctx->stream));
+    if (arc_grads && tot_arcs) GTNB_CUDA(ctx, cudaMemsetAsync(arc_grads->dev, 0, sizeof(float) * tot_arcs, ctx->stream));
+    std::vector<float> m1(B, -1.0f);
+    GTNB_TRY(gtnb_backward(ctx, den, 0, nullptr)); // +1 / -1: subtract's gradFunc (functions.cpp:53-58)
+    GTNB_TRY(gtnb_backward(ctx, num, 0, m1.data()));
+    GTNB_TRY(gtnb_compose_grad(ctx, den, gg_grad, g.dev, per));
+    GTNB_TRY(gtnb_compose_grad(ctx, num, ft_grad, g.dev, per));
+    GTNB_TRY(stage_begin(ctx));
+    GTNB_TRY(stage_upload(ctx, gg_map_dev, gmap.data(), sizeof(int32_t) * nG));
+    if (nP) GTNB_TRY(stage_upload(ctx, ft_map_dev, pmap.data(), sizeof(int32_t) * nP));
+    if (arc_of && nP) GTNB_TRY(stage_upload(ctx, arc_of_dev, arc_of->data(), sizeof(int32_t) * nP));
+    GTNB_TRY(stage_end(ctx));
+    GTNB_TRY(launch_scatter_add(ctx, tg.dev, gg_map_dev, gg_grad, nG));
+    GTNB_TRY(launch_scatter_add(ctx, tg.dev, ft_map_dev, ft_grad, nP));
+    if (arc_grads && arc_of) GTNB_TRY(launch_scatter_add(ctx, arc_grads->dev, arc_of_dev, ft_grad, nP));
+    GTNB_TRY(g.copy_out(ctx, per * B));
+    GTNB_TRY(tg.copy_out(ctx, n_trans));
+    if (arc_grads) GTNB_TRY(arc_grads->copy_out(ctx, tot_arcs));
+  }
+  bool unused = false;
+  return read_losses(scope, B, den->out_scores, num->out_scores, nullptr, 0, a.losses_host, &unused);
+}
+
+/*
+ * n-gram CTC through materialised lattices: intersect(E_b, G) and intersect(P_b, E_b), where P_b = intersect(ctc_b,
+ * G) is built on the host WITHOUT the fold (C start states (0, s), then (l, label(l))).
  */
 int ngram_ctc_loss_exact(CallScope& scope, const TransitionArgs& a, const Targets& t) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, T = a.T, C = a.C;
-  const long long per = (long long)T * C, CC = (long long)C * C;
-  const bool want = a.grads || a.trans_grad;
+  const int B = a.B, C = a.C;
+  const long long CC = (long long)C * C;
   std::vector<float> W(CC);
   GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, CC));
-  // G (benchmarks/ctc.cpp transitionsGraph with a label-determined destination): arc j*C + i = j -> i
   HostGraph G;
-  G.flags.assign(C, 3);
-  G.src.resize(CC);
-  G.dst.resize(CC);
-  G.label.resize(CC);
-  G.w.resize(CC);
-  std::vector<int32_t> gmap(CC);
-  for (int j = 0; j < C; j++)
-    for (int i = 0; i < C; i++) {
-      const long long k = (long long)j * C + i;
-      G.src[k] = j;
-      G.dst[k] = i;
-      G.label[k] = i;
-      G.w[k] = W[(long long)i * C + j];
-      gmap[k] = i * C + j;
-    }
-  const gtnb_graph_view gview = G.view();
+  std::vector<int32_t> gmap;
+  dense_graph(true, C, W.data(), &G, &gmap);
   std::vector<HostGraph> pg(B);
   std::vector<gtnb_graph_view> pviews(B);
   std::vector<int32_t> pmap;
@@ -1023,44 +1131,7 @@ int ngram_ctc_loss_exact(CallScope& scope, const TransitionArgs& a, const Target
     }
     pviews[b] = p.view();
   }
-  const long long nP = (long long)pmap.size();
-  float *e_dev = nullptr, *ft_grad = nullptr, *gg_grad = nullptr;
-  int32_t *ft_map_dev = nullptr, *gg_map_dev = nullptr;
-  OutBuf g, tg;
-  gtnb_lattice*& den = scope.lattice();
-  gtnb_lattice*& num = scope.lattice();
-  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
-  GTNB_TRY(gtnb_compose_linear(ctx, B, &gview, 1, 1, t.T(), C, e_dev, per, &den));
-  GTNB_TRY(gtnb_compose_linear(ctx, B, pviews.data(), B, 0, t.T(), C, e_dev, per, &num));
-  GTNB_TRY(gtnb_forward(ctx, den, 0, nullptr, nullptr));
-  GTNB_TRY(gtnb_forward(ctx, num, 0, nullptr, nullptr));
-  if (want) {
-    GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
-    GTNB_CUDA(ctx, cudaMemsetAsync(g.dev, 0, sizeof(float) * per * B, ctx->stream));
-    GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, CC, &tg, /*alias=*/false));
-    GTNB_TRY(scope.alloc(&gg_grad, CC));
-    GTNB_TRY(scope.alloc(&ft_grad, std::max<long long>(nP, 1)));
-    GTNB_TRY(scope.alloc(&gg_map_dev, CC));
-    GTNB_TRY(scope.alloc(&ft_map_dev, std::max<long long>(nP, 1)));
-    GTNB_CUDA(ctx, cudaMemsetAsync(tg.dev, 0, sizeof(float) * CC, ctx->stream));
-    GTNB_CUDA(ctx, cudaMemsetAsync(gg_grad, 0, sizeof(float) * CC, ctx->stream));
-    GTNB_CUDA(ctx, cudaMemsetAsync(ft_grad, 0, sizeof(float) * std::max<long long>(nP, 1), ctx->stream));
-    std::vector<float> m1(B, -1.0f);
-    GTNB_TRY(gtnb_backward(ctx, den, 0, nullptr)); // +1 / -1: subtract's gradFunc (functions.cpp:53-58)
-    GTNB_TRY(gtnb_backward(ctx, num, 0, m1.data()));
-    GTNB_TRY(gtnb_compose_grad(ctx, den, gg_grad, g.dev, per));
-    GTNB_TRY(gtnb_compose_grad(ctx, num, ft_grad, g.dev, per));
-    GTNB_TRY(stage_begin(ctx));
-    GTNB_TRY(stage_upload(ctx, gg_map_dev, gmap.data(), sizeof(int32_t) * CC));
-    if (nP) GTNB_TRY(stage_upload(ctx, ft_map_dev, pmap.data(), sizeof(int32_t) * nP));
-    GTNB_TRY(stage_end(ctx));
-    GTNB_TRY(launch_scatter_add(ctx, tg.dev, gg_map_dev, gg_grad, CC));
-    GTNB_TRY(launch_scatter_add(ctx, tg.dev, ft_map_dev, ft_grad, nP));
-    GTNB_TRY(g.copy_out(ctx, per * B));
-    GTNB_TRY(tg.copy_out(ctx, CC));
-  }
-  bool unused = false;
-  return read_losses(scope, B, den->out_scores, num->out_scores, nullptr, 0, a.losses_host, &unused);
+  return transitions_loss_materialised(scope, a, t.T(), G, gmap, CC, pviews, pmap, nullptr, nullptr, 0);
 }
 
 /*
@@ -1124,13 +1195,14 @@ extern "C" int gtnb_ngram_ctc_loss(
     dims[b] = SgDims{L + 1, L + (L - 1) + t.skips[b] + std::min(L, 2), L >= 2 ? 2 : 1, /*all_valid=*/1,
                      /*uniform=*/1, /*max_in=*/3, /*max_out=*/3};
   }
-  const TrellisCriterion ngram{(long long)C * C, (long long)B * (T + 1) * C, /*fold=*/true, launch_ngram_num_build,
-                               launch_ngram_den_forward, launch_ngram_den_backward};
+  const TrellisCriterion ngram{(long long)C * C, (long long)B * (T + 1) * C, /*fold=*/true, launch_ngram_den_forward,
+                               launch_ngram_den_backward};
   const bool fast = implicit_dims_supported(dims.data(), B) && ctx->use_implicit;
   return run_criterion(ctx, B, t.T(), losses_host, trans_grad, trans_grad_on_device, (long long)C * C, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
-                         return f ? trellis_loss_fast(scope, ngram, a, t, dims, needs_exact)
-                                  : ngram_ctc_loss_exact(scope, a, t);
+                         if (!f) return ngram_ctc_loss_exact(scope, a, t);
+                         TargetsNumerator num{t, dims, C, launch_ngram_num_build, blank};
+                         return trellis_loss_fast(scope, ngram, a, num, needs_exact);
                        });
 }
 
@@ -1167,14 +1239,15 @@ extern "C" int gtnb_asg_loss_ex(
     const int U = target_lens[b];
     dims[b] = SgDims{U + 1, 2 * U, U > 0 ? 1 : 0, /*all_valid=*/1, /*uniform=*/1, /*max_in=*/2, /*max_out=*/2};
   }
-  const TrellisCriterion asg{nTrans, asg_alpha_floats(B, T, C), /*fold=*/false, asg_num_build, launch_asg_den_forward,
+  const TrellisCriterion asg{nTrans, asg_alpha_floats(B, T, C), /*fold=*/false, launch_asg_den_forward,
                              launch_asg_den_backward};
   // (a non-finite weight: gtnb_asg_loss's sweeps raise the same status bit and end in the materialised lattices)
   const bool fast = C <= kNgramMaxLabels && ctx->use_implicit && implicit_dims_supported(dims.data(), B);
   return run_criterion(ctx, B, t.T(), losses_host, trans_grad, trans_grad_on_device, nTrans, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
-                         return f ? trellis_loss_fast(scope, asg, a, t, dims, needs_exact)
-                                  : asg_loss_generic(scope, a, t);
+                         if (!f) return asg_loss_generic(scope, a, t);
+                         TargetsNumerator num{t, dims, C, asg_num_build, -1};
+                         return trellis_loss_fast(scope, asg, a, num, needs_exact);
                        });
 }
 
@@ -1322,5 +1395,204 @@ extern "C" int gtnb_graph_loss(
   return run_criterion(ctx, B, Tb.data(), losses_host, nullptr, 0, 0, ctx->use_implicit,
                        [&](CallScope& scope, bool implicit, bool* needs_exact) {
                          return graph_loss_once(scope, a, views, Tb, tot_arcs, implicit, needs_exact);
+                       });
+}
+
+/*
+ * Loss over user-supplied target graphs with a learned dense transition graph G (the ASG and CTC alignment graphs of
+ * the reference's examples/learned_decompositions.cpp and examples/priors.cpp, completed with "the standard emissions
+ * and transitions graph"):
+ *   ASG:    loss_b = forwardScore(compose(E_b, G)) - forwardScore(compose(compose(A_b, G), E_b))
+ *   BIGRAM: loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b))
+ * G and trans_w as in gtnb_asg_loss_ex / gtnb_ngram_ctc_loss; E_b, A_b and the arc weights as in gtnb_graph_loss.
+ * The numerators are the products of gtnb_product.h, built on the host once per call; their weights are folded on
+ * the device from the transitions where they lie (launch_product_fold).  The device route sweeps them with
+ * k_implicit.cu beside k_ngram.cu's dense trellis (trellis_loss_fast); a non-finite value, the implicit flag off or
+ * a product that does not fit the implicit layout take the materialised lattices.
+ */
+namespace {
+
+/* trellis_loss_fast's numerator for the user graphs: the (folded) products, weighted by launch_product_fold */
+struct GraphNumerator {
+  const std::vector<ProductGraph>& prods;
+  const std::vector<gtnb_graph_view>& views; // A_b, host weights (or none) in place
+  const std::vector<int32_t>& Tb;
+  int C;
+  bool bigram;
+  const float* arc_weights_dev; // nullable: the views' weights
+  float* arc_grads;
+  int arc_grads_on_device;
+  long long tot_arcs;
+  long long tot_A = 0;
+  std::vector<gtnb_graph_view> pviews;
+  std::vector<int32_t> tidx_h, arc_of_h;
+  std::vector<float> w_A_h;
+  int32_t *map = nullptr, *arc_of = nullptr, *Tb_dev = nullptr;
+  float *w_A = nullptr, *fw = nullptr;
+  const float* e_dev = nullptr;
+  long long per = 0;
+  OutBuf ag;
+
+  bool wants_arc_grads() const { return arc_grads != nullptr; }
+  int alloc(CallScope& scope, const float* e, long long stride, gtnb_lattice**) {
+    const int B = (int)views.size();
+    e_dev = e;
+    per = stride;
+    pviews.resize(B);
+    long long off = 0;
+    for (int b = 0; b < B; b++) {
+      pviews[b] = prods[b].view();
+      tidx_h.insert(tidx_h.end(), prods[b].tidx.begin(), prods[b].tidx.end());
+      for (int32_t k : prods[b].arc_of) arc_of_h.push_back((int32_t)(off + k));
+      off += views[b].num_arcs;
+    }
+    tot_A = (long long)tidx_h.size();
+    GTNB_TRY(scope.alloc(&Tb_dev, B));
+    GTNB_TRY(scope.alloc(&map, tot_A));
+    GTNB_TRY(scope.alloc(&arc_of, tot_A));
+    GTNB_TRY(scope.alloc(&fw, tot_A));
+    if (!arc_weights_dev) {
+      w_A_h.assign(tot_arcs, 0.0f);
+      off = 0;
+      for (int b = 0; b < B; b++) {
+        if (views[b].weights) std::copy(views[b].weights, views[b].weights + views[b].num_arcs, w_A_h.begin() + off);
+        off += views[b].num_arcs;
+      }
+      GTNB_TRY(scope.alloc(&w_A, tot_arcs));
+    }
+    if (arc_grads) {
+      GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, tot_arcs, &ag));
+      if (tot_arcs) GTNB_CUDA(scope.ctx(), cudaMemsetAsync(ag.dev, 0, sizeof(float) * tot_arcs, scope.ctx()->stream));
+    }
+    return GTNB_OK;
+  }
+  int stage(CallScope& scope, gtnb_lattice*) {
+    gtnb_ctx* ctx = scope.ctx();
+    GTNB_TRY(stage_upload(ctx, Tb_dev, Tb.data(), sizeof(int32_t) * Tb.size()));
+    if (tot_A) {
+      GTNB_TRY(stage_upload(ctx, map, tidx_h.data(), sizeof(int32_t) * tot_A));
+      GTNB_TRY(stage_upload(ctx, arc_of, arc_of_h.data(), sizeof(int32_t) * tot_A));
+    }
+    if (!arc_weights_dev && tot_arcs) GTNB_TRY(stage_upload(ctx, w_A, w_A_h.data(), sizeof(float) * tot_arcs));
+    return GTNB_OK;
+  }
+  const int32_t* T_dev() const { return Tb_dev; }
+  int build(CallScope& scope, gtnb_lattice*& lat, const float* w_dev, const float* sigma) {
+    gtnb_ctx* ctx = scope.ctx();
+    const int nW = bigram ? C * C : C + C * C;
+    GTNB_TRY(launch_product_fold(ctx, tot_A, arc_weights_dev ? arc_weights_dev : w_A, arc_of, w_dev, nW, sigma, map,
+                                 fw));
+    // the products are label-uniform: the plain instantiations, with the folded weights gathered into the tables
+    return compose_linear_impl(ctx, (int)pviews.size(), pviews.data(), (int)pviews.size(), 0, Tb.data(), C, e_dev,
+                               per, true, &lat, false, fw);
+  }
+  int scatter(CallScope& scope, const float* ggrad) {
+    if (!arc_grads) return GTNB_OK;
+    GTNB_TRY(launch_scatter_add(scope.ctx(), ag.dev, arc_of, ggrad, tot_A));
+    return ag.copy_out(scope.ctx(), tot_arcs);
+  }
+};
+
+/* the materialised route: the unfolded products weighted on the host, the dense lattice of G.  built: the device
+ * route's products, which for ASG (where folding changes nothing) are the unfolded ones; BIGRAM builds its own. */
+int graph_transitions_exact(CallScope& scope, const TransitionArgs& a, bool bigram,
+                            const std::vector<ProductGraph>& built,
+                            const std::vector<gtnb_graph_view>& views, const std::vector<int32_t>& Tb,
+                            const float* arc_weights, int arc_weights_on_device, float* arc_grads,
+                            int arc_grads_on_device, long long tot_arcs) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, C = a.C;
+  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
+  std::vector<float> W(n_trans), w_A;
+  GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, n_trans));
+  if (arc_weights && arc_weights_on_device) {
+    w_A.resize(tot_arcs);
+    GTNB_TRY(read_to_host(ctx, w_A.data(), arc_weights, 1, tot_arcs));
+  }
+  HostGraph G;
+  std::vector<int32_t> gmap;
+  dense_graph(bigram, C, W.data(), &G, &gmap);
+  std::vector<ProductGraph> unfolded(bigram ? B : 0);
+  const std::vector<ProductGraph>& prods = bigram ? unfolded : built;
+  std::vector<std::vector<float>> pw(B);
+  std::vector<gtnb_graph_view> pviews(B);
+  std::vector<int32_t> pmap, arc_of;
+  long long off = 0;
+  for (int b = 0; b < B; b++) {
+    if (bigram) build_product(views[b], C, bigram, /*fold=*/false, &unfolded[b]);
+    product_weights(prods[b], w_A.empty() ? views[b].weights : w_A.data() + off, W.data(), &pw[b]);
+    pviews[b] = prods[b].view();
+    pviews[b].weights = pw[b].data();
+    pmap.insert(pmap.end(), prods[b].tidx.begin(), prods[b].tidx.end());
+    for (int32_t k : prods[b].arc_of) arc_of.push_back((int32_t)(off + k));
+    off += views[b].num_arcs;
+  }
+  OutBuf ag;
+  if (arc_grads) GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, tot_arcs, &ag));
+  return transitions_loss_materialised(scope, a, Tb.data(), G, gmap, n_trans, pviews, pmap, &arc_of,
+                                       arc_grads ? &ag : nullptr, tot_arcs);
+}
+
+} // namespace
+
+extern "C" int gtnb_graph_transitions_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, int kind,
+    const float* trans_w, int trans_on_device, float* losses_host, float* grads, int grads_on_device,
+    float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const char* fn = "gtnb_graph_transitions_loss";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !trans_w || (B > 0 && (!emissions || !graphs || !losses_host)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown graph kind");
+  if (C > kNgramMaxLabels)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                std::string(fn) + ": C = " + std::to_string(C) +
+                    " labels; the trellis kernels hold the transitions on chip for C <= " +
+                    std::to_string(kNgramMaxLabels));
+  const bool bigram = kind == GTNB_DENSE_BIGRAM;
+  std::vector<int32_t> Tb(B);
+  std::vector<gtnb_graph_view> views(graphs, graphs + B);
+  long long tot_arcs = 0;
+  for (int b = 0; b < B; b++) {
+    Tb[b] = input_lens ? input_lens[b] : T;
+    if (Tb[b] < 0 || Tb[b] > T) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": input_lens outside [0, T]");
+    if (validate_view(ctx, views[b])) return GTNB_ERR_INVALID_ARGUMENT;
+    for (int k = 0; k < views[b].num_arcs; k++)
+      if (views[b].arc_olabel[k] == GTNB_EPSILON)
+        return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                    std::string(fn) + ": graph " + std::to_string(b) +
+                        " has epsilon arcs; remove them first (remove(g, epsilon))");
+    if (arc_weights && !arc_weights_on_device) views[b].weights = arc_weights + tot_arcs;
+    tot_arcs += views[b].num_arcs;
+  }
+  if (tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": more than 2^31 arcs");
+  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
+                         nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
+  // the device route's numerators (BIGRAM: folded), whose shapes decide whether it can be taken
+  std::vector<ProductGraph> prods(B);
+  std::vector<SgDims> dims(B);
+  for (int b = 0; b < B; b++) {
+    build_product(views[b], C, bigram, /*fold=*/true, &prods[b]);
+    const ProductGraph& p = prods[b];
+    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, /*uniform=*/1, p.max_in,
+                     p.max_out};
+  }
+  const TrellisCriterion k = bigram ? TrellisCriterion{n_trans, (long long)B * (T + 1) * C, /*fold=*/true,
+                                                       launch_ngram_den_forward, launch_ngram_den_backward}
+                                    : TrellisCriterion{n_trans, asg_alpha_floats(B, T, C), /*fold=*/false,
+                                                       launch_asg_den_forward, launch_asg_den_backward};
+  const bool fast = ctx->use_implicit && implicit_dims_supported(dims.data(), B);
+  return run_criterion(ctx, B, Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans, fast,
+                       [&](CallScope& scope, bool f, bool* needs_exact) {
+                         if (!f)
+                           return graph_transitions_exact(scope, a, bigram, prods, views, Tb, arc_weights,
+                                                          arc_weights_on_device, arc_grads, arc_grads_on_device,
+                                                          tot_arcs);
+                         GraphNumerator num{prods, views, Tb, C, bigram,
+                                            arc_weights && arc_weights_on_device ? arc_weights : nullptr,
+                                            arc_grads, arc_grads_on_device, tot_arcs};
+                         return trellis_loss_fast(scope, k, a, num, needs_exact);
                        });
 }

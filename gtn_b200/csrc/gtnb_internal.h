@@ -359,6 +359,9 @@ int launch_ngram_den_backward(
     gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
     const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad);
 int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, float* wgrad);
+// out[k] = w_A[arc_of[k]] + Wx[tidx[k]], Wx = [W (nW floats) | sigma]: the weights of gtnb_product.h's products
+int launch_product_fold(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W, int nW,
+                        const float* sigma, const int32_t* tidx, float* out);
 // the same trellis in ASG's start mode (trans_w, trans_grad: [C + C*C], start weights first) and ASG's
 // forced-alignment numerator graphs built on the device
 long long asg_alpha_floats(int B, int T, int C); // floats of the alpha buffer of launch_asg_den_*

@@ -307,6 +307,21 @@ __global__ void __launch_bounds__(256) ngram_fold_kernel(
 }
 
 /*
+ * The arc weights of the numerator products of gtnb_graph_transitions_loss (gtnb_product.h):
+ * out[k] = w_A[arc_of[k]] + Wx[tidx[k]], Wx = [W (nW floats) | sigma]; sigma is read for tidx >= nW only (BIGRAM's
+ * folded start arcs).  One thread per product arc.
+ */
+__global__ void __launch_bounds__(256) product_fold_kernel(
+    long long n, const float* __restrict__ w_A, const int32_t* __restrict__ arc_of, const float* __restrict__ W,
+    int nW, const float* __restrict__ sigma, const int32_t* __restrict__ tidx, float* __restrict__ out) {
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int t = __ldg(tidx + k);
+  const float wx = t < nW ? __ldg(W + t) : __ldg(sigma + (t - nW));
+  out[k] = __ldg(w_A + __ldg(arc_of + k)) + wx;
+}
+
+/*
  * The folded numerator graph of utterance b in the small-graph tables (k_ctc.cu's ctc_build_kernel with
  * weights): node 0 = S (start), node n >= 1 = CTC node l = n - 1 (benchmarks/ctc.cpp:40-58, accept = last two);
  * in-arcs of node n in the order skip, step, self, then the S arc for l <= 1.  The in-entry index is the arc
@@ -541,6 +556,14 @@ int launch_asg_num_build(
 
 int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, float* wgrad) {
   GTNB_LAUNCH(ctx, "ngram_fold", ngram_fold_kernel<<<(C * C + 255) / 256, 256, 0, ctx->stream>>>(C, W, sigma, wgrad));
+  return GTNB_OK;
+}
+
+int launch_product_fold(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W, int nW,
+                        const float* sigma, const int32_t* tidx, float* out) {
+  if (n == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "product_fold", product_fold_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
+      n, w_A, arc_of, W, nW, sigma, tidx, out));
   return GTNB_OK;
 }
 

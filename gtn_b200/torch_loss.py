@@ -346,3 +346,78 @@ class GraphLossFunction(torch.autograd.Function):
 
 def graph_loss(emissions, graphs, input_lengths=None, weights=None, reduction="mean"):
     return GraphLossFunction.apply(emissions, weights, graphs, input_lengths, reduction)
+
+
+class GraphTransitionsLossFunction(torch.autograd.Function):
+    """graph_loss's user target graphs with asg_loss's or ngram_ctc_loss's learned transitions, through
+    gtnb_graph_transitions_loss:
+        kind "asg":    loss_b = forwardScore(compose(E_b, G)) - forwardScore(compose(compose(A_b, G), E_b))
+        kind "bigram": loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b))
+    G: asg_loss's transitions graph (transitions [C + C*C]: start weights, then the C x C matrix, row = destination
+    label) or ngram_ctc_loss's bigram graph (transitions [C*C], every state starts and accepts).  The graphs, weights
+    and input_lengths are graph_loss's.  transitions: float32 CUDA tensor on the emissions' device.  The emission,
+    transition and weight gradients stay on the device; only the B losses are copied to the host.  The transition
+    gradient is summed over the ranks as asg_loss does (allreduce).
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, transitions, weights, graphs, kind="asg", input_lengths=None, reduction="mean",
+                allreduce=True):
+        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        assert kind in ("asg", "bigram")
+        e = emissions.contiguous()
+        B, T, Cn = e.shape
+        assert len(graphs) == B
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        kid = capi.DENSE_BIGRAM if kind == "bigram" else capi.DENSE_ASG
+        assert transitions.numel() == (Cn * Cn if kid == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+        tw = transitions.detach().contiguous()
+        views = [_graph_view(g) for g in graphs]
+        counts = [v.num_arcs for v, _ in views]
+        n_arcs = sum(counts)
+        arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
+        w = ag = None
+        if weights is not None:
+            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
+            assert weights.numel() == n_arcs
+            w = weights.detach().contiguous()
+            ag = torch.empty(max(n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
+        stream = torch.cuda.current_stream(e.device).cuda_stream
+        g = _ctx_for(e.device, stream)
+        il = _lengths(input_lengths, B)
+        losses = np.zeros(B, np.float32)
+        grad = torch.empty_like(e)  # every row is written by the call
+        tg = torch.empty(transitions.numel(), dtype=torch.float32, device=e.device)
+        g._check(capi.lib().gtnb_graph_transitions_loss(
+            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
+            None if w is None else w.data_ptr(), 1, kid, tw.data_ptr(), 1, losses.ctypes.data_as(capi._f32p),
+            grad.data_ptr(), 1, None if ag is None else ag.data_ptr(), 1, tg.data_ptr(), 1))
+        tg = tg.view_as(transitions)
+        _allreduce_transitions(ctx, tg, allreduce)
+        out = torch.from_numpy(losses).to(e.device)
+        if ag is not None:
+            ag = ag[:n_arcs].view_as(weights)
+            ctx.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(e.device)
+        ctx.save_for_backward(grad, tg)
+        ctx.ag = ag  # (computed here, neither an input nor an output: held on ctx)
+        ctx.reduction = reduction
+        ctx.B = B
+        return out.mean() if reduction == "mean" else out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        egrad, tgrad = _transition_backward(ctx, grad_output)
+        ag = ctx.ag
+        if ag is None:
+            wg = None
+        elif ctx.reduction == "mean":
+            wg = ag * (grad_output / ctx.B)
+        else:  # every graph belongs to one utterance: its arcs take that utterance's upstream gradient
+            wg = ag * grad_output.reshape(-1)[ctx.owner].view_as(ag)
+        return egrad, tgrad, wg, None, None, None, None, None
+
+
+def graph_transitions_loss(emissions, transitions, graphs, kind="asg", input_lengths=None, weights=None,
+                           reduction="mean", allreduce=True):
+    return GraphTransitionsLossFunction.apply(emissions, transitions, weights, graphs, kind, input_lengths, reduction,
+                                              allreduce)

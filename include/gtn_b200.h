@@ -527,6 +527,49 @@ int gtnb_viterbi_dense_ex(
     float* scores, /* nullable */
     int outputs_on_device);
 
+/*
+ * Loss over one user-supplied target graph per utterance with a learned dense transition graph G (the word
+ * decomposition and prior graphs of the reference's examples/learned_decompositions.cpp and examples/priors.cpp,
+ * completed with the standard emissions and transitions graph):
+ *   GTNB_DENSE_ASG:    loss_b = forwardScore(compose(E_b, G)) - forwardScore(compose(compose(A_b, G), E_b)),
+ *                      G and trans_w ([C + C*C]) as at gtnb_asg_loss_ex / gtnb_viterbi_dense;
+ *   GTNB_DENSE_BIGRAM: loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b)),
+ *                      G and trans_w ([C*C]) as at gtnb_ngram_ctc_loss.
+ * E_b, graphs, arc_weights and the epsilon rule are those of gtnb_graph_loss: A_b is matched on its olabels, arcs
+ * labelled outside [0, C) never match (gradient 0), an epsilon arc is GTNB_ERR_UNSUPPORTED.  Outputs: losses_host
+ * [B]; grads (nullable, [B][T][C], d loss_b / d e_b), EVERY row written, 0 beyond T_b; arc_grads (nullable,
+ * [sum_b A_b], d loss_b / d A_b's arc weights in Graph arc numbering) and trans_grad (nullable, the batch sum of
+ * d loss_b / d trans_w), written, not accumulated.  Every buffer lives on the device or the host according to its
+ * own *_on_device flag.  T_b = 0 gives NaN; a graph with no accepting path of T_b arcs, no start node or no arcs
+ * gives +inf and the denominator's gradient alone.  B = 0 zeroes trans_grad.  T_b > T, negative lengths, an
+ * unknown kind or a malformed view are GTNB_ERR_INVALID_ARGUMENT; C > 128 is GTNB_ERR_UNSUPPORTED.
+ * The numerator compose(A_b, G) is built on the host from the graph's structure only; its weights are folded on
+ * the device from the transitions where they lie, which on this route never visit the host.  It is swept without
+ * building the lattice beside the dense trellis of the denominator.  Non-finite values, the "implicit" flag off, or
+ * products too wide for the implicit layout (e.g. wildcard states at large C) take the materialised lattices.
+ */
+int gtnb_graph_transitions_loss(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    int kind,
+    const float* trans_w,
+    int trans_on_device,
+    float* losses_host,
+    float* grads, /* nullable */
+    int grads_on_device,
+    float* arc_grads, /* nullable */
+    int arc_grads_on_device,
+    float* trans_grad, /* nullable */
+    int trans_grad_on_device);
+
 #ifdef __cplusplus
 }
 #endif
