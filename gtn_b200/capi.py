@@ -107,6 +107,9 @@ SYMBOLS = [
     ("gtnb_graph_transitions_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.c_int, _vp, C.c_int,
       _f32p, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int]),
+    ("gtnb_graph_viterbi", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _vp, _vp, _vp,
+      C.c_int]),
 ]
 
 _lib = None
@@ -537,6 +540,56 @@ class Ctx:
             for buf in bufs:
                 buf.free()
         return losses, grads, ag
+
+    def graph_viterbi(self, emissions, views, input_lens=None, arc_weights=None):
+        """Host-buffer entry of gtnb_graph_viterbi: emissions [B,T,C], views: B (view, keepalive) pairs from make_view,
+        arc_weights [sum A_b] or None -> (paths [B,T] int32, scores [B], arcs [B,T] int32)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
+        assert aw is None or aw.size == n_arcs
+        paths = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
+        arcs = np.full((max(B, 1), max(T, 1)), -7, np.int32)
+        scores = np.full(max(B, 1), np.nan, np.float32)
+        self._check(lib().gtnb_graph_viterbi(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0,
+            paths.ctypes.data, arcs.ctypes.data, scores.ctypes.data, 0))
+        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
+
+    def graph_viterbi_dev(self, emissions, views, input_lens=None, arc_weights=None):
+        """Device-buffer entry: emissions (and arc_weights, when given) uploaded once, gtnb_graph_viterbi on device
+        pointers (outputs in HBM), downloaded afterwards -> (paths, scores, arcs)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        fill = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
+        bufs = [self.to_device(e), self.to_device(fill), self.to_device(fill),
+                self.to_device(np.full(max(B, 1), np.nan, np.float32))]
+        e_dev, p_dev, a_dev, s_dev = bufs
+        w_dev = None
+        if arc_weights is not None:
+            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
+            assert aw.size == n_arcs
+            w_dev = self.to_device(aw)
+            bufs.append(w_dev)
+        try:
+            self._check(lib().gtnb_graph_viterbi(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if w_dev is None else w_dev.ptr, 1,
+                p_dev.ptr, a_dev.ptr, s_dev.ptr, 1))
+            paths = p_dev.download(fill.shape, np.int32)
+            arcs = a_dev.download(fill.shape, np.int32)
+            scores = s_dev.download((max(B, 1),))
+        finally:
+            for buf in bufs:
+                buf.free()
+        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
 
     def graph_transitions_loss(self, emissions, views, trans_w, kind=DENSE_ASG, want_grad=True, input_lens=None,
                                arc_weights=None):

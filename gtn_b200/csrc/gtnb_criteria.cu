@@ -1264,6 +1264,35 @@ extern "C" int gtnb_asg_loss_ex(
  */
 namespace {
 
+/*
+ * The checks gtnb_graph_loss, gtnb_graph_transitions_loss and gtnb_graph_viterbi make of their graphs: T_b =
+ * input_lens[b] (or T) in [0, T], well-formed views, no epsilon arc, fewer than 2^31 arcs in all.  Host arc weights
+ * are spliced into the copied views; *tot_arcs = sum_b A_b.
+ */
+int parse_graphs(gtnb_ctx* ctx, const char* fn, int B, int T, const int32_t* input_lens, const gtnb_graph_view* graphs,
+                 const float* arc_weights, int arc_weights_on_device, std::vector<int32_t>* Tb,
+                 std::vector<gtnb_graph_view>* views, long long* tot_arcs) {
+  Tb->resize(B);
+  views->assign(graphs, graphs + B);
+  *tot_arcs = 0;
+  for (int b = 0; b < B; b++) {
+    gtnb_graph_view& v = (*views)[b];
+    (*Tb)[b] = input_lens ? input_lens[b] : T;
+    if ((*Tb)[b] < 0 || (*Tb)[b] > T)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": input_lens outside [0, T]");
+    if (validate_view(ctx, v)) return GTNB_ERR_INVALID_ARGUMENT;
+    for (int k = 0; k < v.num_arcs; k++)
+      if (v.arc_olabel[k] == GTNB_EPSILON)
+        return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                    std::string(fn) + ": graph " + std::to_string(b) +
+                        " has epsilon arcs; remove them first (remove(g, epsilon))");
+    if (arc_weights && !arc_weights_on_device) v.weights = arc_weights + *tot_arcs;
+    *tot_arcs += v.num_arcs;
+  }
+  if (*tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": more than 2^31 arcs");
+  return GTNB_OK;
+}
+
 struct GraphLossArgs {
   int B, T, C;
   const float* emissions;
@@ -1375,22 +1404,11 @@ extern "C" int gtnb_graph_loss(
                         losses_host, grads, grads_on_device, arc_grads, arc_grads_on_device};
   if (!ctx || B < 0 || T < 0 || C <= 0 || (B > 0 && (!emissions || !graphs || !losses_host)))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_graph_loss: bad arguments");
-  std::vector<int32_t> Tb(B);
-  std::vector<gtnb_graph_view> views(graphs, graphs + B);
+  std::vector<int32_t> Tb;
+  std::vector<gtnb_graph_view> views;
   long long tot_arcs = 0;
-  for (int b = 0; b < B; b++) {
-    Tb[b] = input_lens ? input_lens[b] : T;
-    if (Tb[b] < 0 || Tb[b] > T) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_graph_loss: input_lens outside [0, T]");
-    if (validate_view(ctx, views[b])) return GTNB_ERR_INVALID_ARGUMENT;
-    for (int k = 0; k < views[b].num_arcs; k++)
-      if (views[b].arc_olabel[k] == GTNB_EPSILON)
-        return fail(ctx, GTNB_ERR_UNSUPPORTED,
-                    "gtnb_graph_loss: graph " + std::to_string(b) +
-                        " has epsilon arcs; remove them first (remove(g, epsilon))");
-    if (arc_weights && !arc_weights_on_device) views[b].weights = arc_weights + tot_arcs;
-    tot_arcs += views[b].num_arcs;
-  }
-  if (tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_graph_loss: more than 2^31 arcs");
+  GTNB_TRY(parse_graphs(ctx, "gtnb_graph_loss", B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb,
+                        &views, &tot_arcs));
   // (graphs that are not label-uniform need C <= k_implicit.cu's kArcMaxLabels: compose_linear_impl checks)
   return run_criterion(ctx, B, Tb.data(), losses_host, nullptr, 0, 0, ctx->use_implicit,
                        [&](CallScope& scope, bool implicit, bool* needs_exact) {
@@ -1551,22 +1569,11 @@ extern "C" int gtnb_graph_transitions_loss(
                     " labels; the trellis kernels hold the transitions on chip for C <= " +
                     std::to_string(kNgramMaxLabels));
   const bool bigram = kind == GTNB_DENSE_BIGRAM;
-  std::vector<int32_t> Tb(B);
-  std::vector<gtnb_graph_view> views(graphs, graphs + B);
+  std::vector<int32_t> Tb;
+  std::vector<gtnb_graph_view> views;
   long long tot_arcs = 0;
-  for (int b = 0; b < B; b++) {
-    Tb[b] = input_lens ? input_lens[b] : T;
-    if (Tb[b] < 0 || Tb[b] > T) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": input_lens outside [0, T]");
-    if (validate_view(ctx, views[b])) return GTNB_ERR_INVALID_ARGUMENT;
-    for (int k = 0; k < views[b].num_arcs; k++)
-      if (views[b].arc_olabel[k] == GTNB_EPSILON)
-        return fail(ctx, GTNB_ERR_UNSUPPORTED,
-                    std::string(fn) + ": graph " + std::to_string(b) +
-                        " has epsilon arcs; remove them first (remove(g, epsilon))");
-    if (arc_weights && !arc_weights_on_device) views[b].weights = arc_weights + tot_arcs;
-    tot_arcs += views[b].num_arcs;
-  }
-  if (tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": more than 2^31 arcs");
+  GTNB_TRY(parse_graphs(ctx, fn, B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
+                        &tot_arcs));
   const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
                          nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
   const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
@@ -1595,4 +1602,183 @@ extern "C" int gtnb_graph_transitions_loss(
                                             arc_grads, arc_grads_on_device, tot_arcs};
                          return trellis_loss_fast(scope, k, a, num, needs_exact);
                        });
+}
+
+/*
+ * Viterbi alignment over user-supplied target graphs: viterbiPath / viterbiScore of compose(A_b, E_b), with E_b, A_b,
+ * the arc weights, the olabel matching and the epsilon rule of gtnb_graph_loss.  The device route sweeps
+ * intersect(A_b, E_b) in the tropical semiring without building it and traces the path back from the saved score
+ * rows (k_implicit.cu).  An utterance whose trace met a tie (with exact_ties on) or whose sweep met a non-finite
+ * value is re-run alone on the materialised route, which breaks ties as the reference does; the whole batch takes
+ * that route when the graphs do not fit the implicit layout or the implicit flag is off.
+ */
+namespace {
+
+struct GraphViterbiArgs {
+  int B, T, C;
+  const float* emissions;
+  int emissions_on_device;
+  const float* arc_weights;
+  int arc_weights_on_device;
+  int32_t* paths;
+  int32_t* arcs;
+  float* scores;
+  int outputs_on_device;
+};
+
+/*
+ * The materialised route for the utterances `which`: gtnb_compose_linear (the lattice is put in the reference's
+ * relaxation order while exact_ties is on, k_order.cu), gtnb_forward(tropical) for the score and gtnb_viterbi_path.
+ * A_b is matched on its olabels, so its ilabels play no part in the composition: they are replaced by the arc ids,
+ * which the path's ilabels then carry back.  The rows are written into the device outputs p_dev / a_dev (nullable)
+ * and s_dev.
+ */
+int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::vector<gtnb_graph_view>& views,
+                        const std::vector<int32_t>& Tb, long long tot_arcs, const float* e_dev,
+                        const std::vector<int>& which, int32_t* p_dev, int32_t* a_dev, float* s_dev) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int T = a.T, C = a.C, ml = std::max(T, 1);
+  const long long per = (long long)T * C;
+  std::vector<float> host_w;
+  if (a.arc_weights && a.arc_weights_on_device) {
+    host_w.resize((size_t)std::max(tot_arcs, 1ll));
+    GTNB_TRY(read_to_host(ctx, host_w.data(), a.arc_weights, 1, tot_arcs));
+  }
+  std::vector<long long> first_arc(a.B, 0);
+  int max_arcs = 0;
+  for (int b = 0; b < a.B; b++) {
+    if (b > 0) first_arc[b] = first_arc[b - 1] + views[b - 1].num_arcs;
+    max_arcs = std::max(max_arcs, views[b].num_arcs);
+  }
+  std::vector<int32_t> iota(std::max(max_arcs, 1));
+  for (int k = 0; k < max_arcs; k++) iota[k] = k;
+  // the utterances with frames (T_b = 0 accepts nothing) and their emission rows, contiguous
+  std::vector<int> sub;
+  for (int b : which)
+    if (Tb[b] > 0) sub.push_back(b);
+  const int n = (int)sub.size();
+  std::vector<float> sc(std::max(n, 1), -std::numeric_limits<float>::infinity());
+  std::vector<int32_t> parc((size_t)std::max(n, 1) * ml, -1), plab(parc.size(), -1), plen(std::max(n, 1), -1);
+  if (n > 0) {
+    std::vector<gtnb_graph_view> sv(n);
+    std::vector<int32_t> sT(n);
+    const float* e_sub = e_dev;
+    if (n < a.B) {
+      float* e_copy = nullptr;
+      GTNB_TRY(scope.alloc(&e_copy, per * n));
+      for (int k = 0; k < n; k++)
+        GTNB_CUDA(ctx, cudaMemcpyAsync(e_copy + per * k, e_dev + per * sub[k], sizeof(float) * per,
+                                       cudaMemcpyDeviceToDevice, ctx->stream));
+      e_sub = e_copy;
+    }
+    for (int k = 0; k < n; k++) {
+      sv[k] = views[sub[k]];
+      sv[k].arc_ilabel = iota.data();
+      sT[k] = Tb[sub[k]];
+      if (!host_w.empty()) sv[k].weights = host_w.data() + first_arc[sub[k]];
+    }
+    gtnb_lattice*& lat = scope.lattice();
+    GTNB_TRY(gtnb_compose_linear(ctx, n, sv.data(), n, 0, sT.data(), C, e_sub, per, &lat));
+    GTNB_TRY(gtnb_forward(ctx, lat, 1, sc.data(), nullptr));
+    GTNB_TRY(gtnb_viterbi_path(ctx, lat, ml, nullptr, parc.data(), plab.data(), nullptr, plen.data(), nullptr));
+  }
+  // the rows of every utterance in `which` (T_b = 0: score -inf, no path), staged on the host and copied from
+  // pageable memory (each copy has left the host buffer when it returns)
+  const size_t nw = which.size();
+  std::vector<int32_t> prow(nw * ml), arow(nw * ml);
+  std::vector<float> srow(nw);
+  size_t k = 0;
+  for (size_t j = 0; j < nw; j++) {
+    const int b = which[j];
+    const bool run = k < sub.size() && sub[k] == b;
+    const int len = run ? plen[k] : -1;
+    for (int t = 0; t < T; t++) {
+      prow[j * ml + t] = t < len ? plab[k * ml + t] : -1;
+      arow[j * ml + t] = t < len ? parc[k * ml + t] : -1;
+    }
+    srow[j] = run ? sc[k] : -std::numeric_limits<float>::infinity();
+    if (p_dev && T > 0)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(p_dev + (long long)b * T, &prow[j * ml], sizeof(int32_t) * T,
+                                     cudaMemcpyHostToDevice, ctx->stream));
+    if (a_dev && T > 0)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a_dev + (long long)b * T, &arow[j * ml], sizeof(int32_t) * T,
+                                     cudaMemcpyHostToDevice, ctx->stream));
+    GTNB_CUDA(ctx, cudaMemcpyAsync(s_dev + b, &srow[j], sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    k += run;
+  }
+  return scope.sync();
+}
+
+int graph_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const std::vector<gtnb_graph_view>& views,
+                      const std::vector<int32_t>& Tb, long long tot_arcs) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, nrow = (long long)B * T;
+  const bool dev_out = a.outputs_on_device != 0;
+  float *e_dev = nullptr, *s_dev = nullptr;
+  int32_t *p_dev = nullptr, *a_dev = nullptr, *status = nullptr;
+  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
+  GTNB_TRY(scope.borrow(a.scores, a.scores && dev_out, B, &s_dev));
+  if (a.paths) GTNB_TRY(scope.borrow(a.paths, dev_out, nrow, &p_dev));
+  if (a.arcs) GTNB_TRY(scope.borrow(a.arcs, dev_out, nrow, &a_dev));
+  GTNB_TRY(scope.alloc(&status, B));
+  GTNB_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(int32_t) * B, ctx->stream));
+
+  std::vector<int> exact;
+  bool implicit = ctx->use_implicit;
+  gtnb_lattice*& lat = scope.lattice();
+  if (implicit) {
+    const int rc = compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, e_dev, per, true, &lat, true,
+                                       a.arc_weights_on_device ? a.arc_weights : nullptr);
+    if (rc == GTNB_ERR_UNSUPPORTED) // does not fit the implicit layout: materialise
+      implicit = false;
+    else
+      GTNB_TRY(rc);
+    implicit = implicit && implicit_trace_supported(lat);
+  }
+  if (implicit) {
+    GTNB_TRY(launch_implicit_forward(ctx, lat, status, 0, -1, /*tropical=*/true));
+    GTNB_TRY(launch_implicit_trace(ctx, lat, status, p_dev, a_dev, s_dev, T));
+    // one status word per utterance decides the route: bit 1 a non-finite value, bit 2 a tie on the traced path
+    GTNB_TRY(readback_reserve(ctx, sizeof(int32_t) * B));
+    int32_t* st = reinterpret_cast<int32_t*>(ctx->readback);
+    GTNB_CUDA(ctx, cudaMemcpyAsync(st, status, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    GTNB_TRY(scope.sync());
+    for (int b = 0; b < B; b++)
+      if (Tb[b] > 0 && ((st[b] & 1) || ((st[b] & 2) && ctx->exact_ties))) exact.push_back(b);
+  } else {
+    for (int b = 0; b < B; b++) exact.push_back(b);
+  }
+  if (!exact.empty()) GTNB_TRY(graph_viterbi_exact(scope, a, views, Tb, tot_arcs, e_dev, exact, p_dev, a_dev, s_dev));
+  if (!dev_out) {
+    if (a.scores)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a.scores, s_dev, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a.paths && nrow)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a.paths, p_dev, sizeof(int32_t) * nrow, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a.arcs && nrow)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a.arcs, a_dev, sizeof(int32_t) * nrow, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  return scope.sync();
+}
+
+} // namespace
+
+extern "C" int gtnb_graph_viterbi(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, int32_t* paths, int32_t* arcs,
+    float* scores, int outputs_on_device) {
+  const char* fn = "gtnb_graph_viterbi";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || (B > 0 && (!emissions || !graphs)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  std::vector<int32_t> Tb;
+  std::vector<gtnb_graph_view> views;
+  long long tot_arcs = 0;
+  GTNB_TRY(parse_graphs(ctx, fn, B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
+                        &tot_arcs));
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  const GraphViterbiArgs a{B, T, C, emissions, emissions_on_device, arc_weights, arc_weights_on_device,
+                           paths, arcs, scores, outputs_on_device};
+  return graph_viterbi_run(scope, a, views, Tb, tot_arcs);
 }

@@ -308,7 +308,15 @@ int launch_backward_fused(
 // kernels (k_dense.cu): factored dense-trellis Viterbi
 bool implicit_supported(const gtnb_lattice* lat);
 bool implicit_dims_supported(const SgDims* dims, int n_graphs, int arc_C = 0);
-int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0 = 0, int nb = -1);
+/* tropical: max instead of logadd (viterbiScore); the saved score rows then feed launch_implicit_trace */
+int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0 = 0, int nb = -1,
+                            bool tropical = false);
+/* viterbiPath from a tropical launch_implicit_forward's score rows: paths / arcs (nullable, [B][T_out]) get the matched
+ * label and the graph arc of every frame, -1 beyond T_b and without an accepting path; scores_out [B]; status bit 2
+ * marks a tie on the traced path, bit 1 a score of +inf / NaN */
+bool implicit_trace_supported(const gtnb_lattice* lat);
+int launch_implicit_trace(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int32_t* paths, int32_t* arcs,
+                          float* scores_out, int T_out);
 /* k_bidir.cu: the CTC criterion in one launch (two-CTA clusters meeting in the middle), normaliser included */
 bool bidir_supported(const gtnb_lattice* lat, const float* emissions, int64_t stride, const float* grad, int64_t grad_stride);
 int bidir_blocks(int max_T);

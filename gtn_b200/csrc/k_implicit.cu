@@ -38,6 +38,10 @@
  * kArcMaxLabels), and the backward sums the arc posteriors of a frame per label in a C-float
  * shared row that is flushed to global memory once per frame.  Only the several-nodes-per-thread
  * path and the wide kernels have this mode; with ARC = false they compile to what they were.
+ *
+ * Tropical mode (template flag TROP, gtnb_graph_viterbi): the forward kernels take the max instead of the logadd,
+ * and implicit_trace_kernel walks the best path back from the saved score rows (with TROP = false the forward
+ * kernels compile to what they were).
  */
 #include <algorithm>
 
@@ -196,6 +200,28 @@ __device__ __noinline__ float imp_fwd_node_arc(
   return mx + flog1p(sum);
 }
 
+/* tropical (max) semiring: the first pass alone -- the best in-arc value fl(S[src] + fl(w + e)) */
+__device__ __noinline__ float imp_fwd_node_max(
+    int e0, int e1, float e, const int* t_src, const float* t_w, const float* prev) {
+  float mx = neg_inf();
+#pragma unroll 1
+  for (int a = e0; a < e1; a++) mx = fmaxf(mx, prev[t_src[a]] + (t_w[a] + e));
+  return mx;
+}
+__device__ __noinline__ float imp_fwd_node_arc_max(
+    int e0, int e1, const float* erow, const int* t_alab, const int* t_src, const float* t_w, const float* prev) {
+  float mx = neg_inf();
+#pragma unroll 1
+  for (int a = e0; a < e1; a++) mx = fmaxf(mx, prev[t_src[a]] + (t_w[a] + erow[t_alab[a]]));
+  return mx;
+}
+
+/* the fast path's combine of three in-arc values: logadd, or max in the tropical semiring */
+template <bool TROP>
+__device__ __forceinline__ float combine3(float v0, float v1, float v2) {
+  return TROP ? fmaxf(fmaxf(v0, v1), v2) : lse3(v0, v1, v2);
+}
+
 /* arc-label mode: the per-entry matched labels of the graph operand -> shared memory */
 __device__ __forceinline__ void load_arc_labels(const GraphMeta& m, const int32_t* __restrict__ sg_in_label,
                                                 int* t_alab) {
@@ -229,7 +255,9 @@ __device__ __forceinline__ void flush_erow_grad(float* GE, float* gr, int C, flo
 /* forward                                                             */
 /* ------------------------------------------------------------------ */
 
-template <bool ARC = false>
+/* TROP: the tropical semiring (viterbiScore, gtnb_graph_viterbi): every logadd becomes a max, the score rows are
+ * saved as before for implicit_trace_kernel */
+template <bool ARC = false, bool TROP = false>
 __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -329,7 +357,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     const float e = has ? pf[j] : 0.0f; /* idle threads load node 0's */ \
     const float* P = ((j)&1) ? S1 : S0;                                  \
     float* Q = ((j)&1) ? S0 : S1;                                        \
-    const float sv = lse3(P[i0] + (w0 + e), P[i1] + (w1 + e), P[i2] + (w2 + e)); \
+    const float sv = combine3<TROP>(P[i0] + (w0 + e), P[i1] + (w1 + e), P[i2] + (w2 + e)); \
     chk = fmaf(e, 0.0f, chk);                                            \
     Q[tid] = sv;                                                         \
     bar_named<1>(nact);                                                     \
@@ -382,7 +410,10 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
         const float* Ecur = E_s + ((t - 1) & 1) * C;
         for (int i = tid; i < N1; i += kImpThreads) {
           const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
-          const float sv = (e1 > e0) ? imp_fwd_node_arc(e0, e1, Ecur, t_alab, t_src, t_w, prev) : neg_inf();
+          float sv = neg_inf();
+          if (e1 > e0)
+            sv = TROP ? imp_fwd_node_arc_max(e0, e1, Ecur, t_alab, t_src, t_w, prev)
+                      : imp_fwd_node_arc(e0, e1, Ecur, t_alab, t_src, t_w, prev);
           cur[i] = sv;
           srow[i] = sv;
         }
@@ -394,7 +425,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
           if (e1 > e0) {
             const float e = __ldg(er + t_lab[i]);
             bad |= !is_finite(e);
-            sv = imp_fwd_node_any(e0, e1, e, t_src, t_w, prev);
+            sv = TROP ? imp_fwd_node_max(e0, e1, e, t_src, t_w, prev) : imp_fwd_node_any(e0, e1, e, t_src, t_w, prev);
           }
           cur[i] = sv;
           srow[i] = sv;
@@ -414,7 +445,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     if (t_flags[i] & 2) mx = fmaxf(mx, Sf[i]);
   mx = block_max(mx, red);
   float out = mx;
-  if (mx != CUDART_INF_F && mx != -CUDART_INF_F) {
+  if (!TROP && mx != CUDART_INF_F && mx != -CUDART_INF_F) {
     float sum = 0.0f;
     for (int i = tid; i < N1; i += kImpThreads)
       if (t_flags[i] & 2) sum += expf(Sf[i] - mx);
@@ -783,7 +814,7 @@ __device__ __forceinline__ unsigned group_mask() {
   return (G >= 32) ? 0xffffffffu : (((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1)));
 }
 
-template <int G, bool ARC = false>
+template <int G, bool ARC = false, bool TROP = false>
 __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -876,13 +907,16 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
       }
 #pragma unroll
       for (int o = G / 2; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(gmask, mx, o));
-      float sum = 0.0f;
+      float sv = mx;
+      if (!TROP) {
+        float sum = 0.0f;
 #pragma unroll
-      for (int k = 0; k < kWideCap; k++) sum += fexp(v[k] - mx);
+        for (int k = 0; k < kWideCap; k++) sum += fexp(v[k] - mx);
 #pragma unroll
-      for (int o = G / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(gmask, sum, o);
-      const float lg = lg2(sum);
-      const float sv = (fabsf(mx) == CUDART_INF_F) ? mx : fmaf(lg, 0.6931471805599453f, mx);
+        for (int o = G / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(gmask, sum, o);
+        const float lg = lg2(sum);
+        sv = (fabsf(mx) == CUDART_INF_F) ? mx : fmaf(lg, 0.6931471805599453f, mx);
+      }
       if (on && sub == 0) {
         cur[u] = sv;
         srow[u] = sv;
@@ -921,7 +955,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_wide_kernel(
     if (t_flags[i] & 2) mx = fmaxf(mx, Sf[i]);
   mx = block_max(mx, red);
   float out = mx;
-  if (mx != CUDART_INF_F && mx != -CUDART_INF_F) {
+  if (!TROP && mx != CUDART_INF_F && mx != -CUDART_INF_F) {
     float sum = 0.0f;
     for (int i = tid; i < N1; i += kImpThreads)
       if (t_flags[i] & 2) sum += expf(Sf[i] - mx);
@@ -1105,6 +1139,208 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_wide_kernel(
       if (ACCG[a] != 0.0f) atomicAdd(&ggr[in_arc[a]], ACCG[a] * delta);
 }
 
+/* ------------------------------------------------------------------ */
+/* Viterbi traceback of a tropical forward sweep (any variant above)   */
+/* ------------------------------------------------------------------ */
+
+constexpr int kTrMaxFrames = 16; // frames of score and emission rows per staged block
+constexpr int kTrSmemTarget = 96 * 1024; // the block shrinks until the CTA fits two per SM
+constexpr int kTrTie = 2; // status bit beside the non-finite bit 1: a tie on the traced path
+constexpr int kTrLoads = 8; // staging loads in flight per thread
+
+struct TraceLayout {
+  int K; // frames per staged block
+  int pitch; // floats per staged score row (max over the batch, multiple of 4)
+  int off_inptr, off_src, off_w, off_lab, off_arc, off_red, off_buf;
+  int total;
+};
+
+TraceLayout make_trace_layout(int maxN, int maxA, int C, int K) {
+  TraceLayout o;
+  o.K = K;
+  o.pitch = (maxN + 3) & ~3;
+  const int A = std::max(maxA, 1);
+  int off = 0;
+  auto take = [&](long long bytes) {
+    int at = off;
+    off += (int)((bytes + 15) & ~15ll);
+    return at;
+  };
+  o.off_inptr = take(4ll * (maxN + 2));
+  o.off_src = take(4ll * A);
+  o.off_w = take(4ll * A);
+  o.off_lab = take(4ll * A);
+  o.off_arc = take(4ll * A);
+  o.off_red = take(4 * 16);
+  o.off_buf = take(4ll * 2 * K * (o.pitch + C)); // two blocks: K score rows, then K emission rows
+  o.total = off;
+  return o;
+}
+
+/*
+ * viterbiPath of intersect(A_b, E_b) from the score rows a TROP forward saved, without back-pointers: at node v of
+ * frame t every in-arc's candidate fl(S_{t-1}[src] + fl(w + e[t-1][label])) is recomputed exactly as the forward
+ * computed it, and the in-arc whose candidate == S_t[v] is taken.  One CTA per utterance; warp 0 walks a block of
+ * K frames held in shared memory while the other warps stage the next block with independent loads, so the
+ * dependent chain of T_b steps pays shared-memory latency, not a global load per frame.
+ * Outputs: paths / arcs (nullable, [B][T_out]): the matched label and the graph arc of the in-arc taken at every
+ * frame, -1 beyond T_b and everywhere without an accepting path; out_scores [B]: viterbiScore (-inf for T_b = 0:
+ * linearGraph(0, C) accepts nothing).  Status: kTrTie when two accept nodes share the best score at frame T_b or two
+ * candidates reach the maximum at a node of the path (the reference breaks such ties by its own arc order, which the
+ * caller reproduces on the materialised route); bit 1 for a score of +inf / NaN.  Only nodes of the traced path are
+ * visited, and every predecessor of one lies on an accepting path, so nodes the reference prunes play no part.
+ */
+__global__ void __launch_bounds__(kImpThreads) implicit_trace_kernel(
+    const GraphMeta* __restrict__ meta,
+    const uint8_t* __restrict__ sg_flags,
+    const int32_t* __restrict__ sg_in_ptr,
+    const int32_t* __restrict__ sg_in_src,
+    const int32_t* __restrict__ sg_in_label,
+    const float* __restrict__ sg_in_w,
+    const int32_t* __restrict__ sg_in_arc,
+    const float* __restrict__ emissions,
+    const float* __restrict__ scores,
+    int32_t* __restrict__ status,
+    int32_t* __restrict__ paths,
+    int32_t* __restrict__ arcs,
+    float* __restrict__ out_scores,
+    int T_out,
+    int C,
+    const TraceLayout lay) {
+  GTNB_DYNAMIC_SMEM(unsigned char, smem);
+  const GraphMeta m = meta[blockIdx.x];
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int N1 = m.sg_N, A1 = m.sg_A, T = m.T, K = lay.K;
+  const int pitch = (N1 + 3) & ~3;
+  int* t_inptr = reinterpret_cast<int*>(smem + lay.off_inptr);
+  int* t_src = reinterpret_cast<int*>(smem + lay.off_src);
+  float* t_w = reinterpret_cast<float*>(smem + lay.off_w);
+  int* t_lab = reinterpret_cast<int*>(smem + lay.off_lab);
+  int* t_arc = reinterpret_cast<int*>(smem + lay.off_arc);
+  float* red = reinterpret_cast<float*>(smem + lay.off_red);
+  float* buf = reinterpret_cast<float*>(smem + lay.off_buf);
+  const int bstride = K * (lay.pitch + C);
+  const float* sc = scores + m.node_base;
+  const float* em = emissions + m.emis_off;
+  int32_t* po = paths ? paths + (long long)blockIdx.x * T_out : nullptr;
+  int32_t* ao = arcs ? arcs + (long long)blockIdx.x * T_out : nullptr;
+
+  for (int i = tid; i <= N1; i += kImpThreads) t_inptr[i] = sg_in_ptr[m.sg_node_base + i];
+  for (int a = tid; a < A1; a += kImpThreads) {
+    t_src[a] = sg_in_src[m.sg_arc_base + a];
+    t_w[a] = sg_in_w[m.sg_arc_base + a];
+    t_lab[a] = sg_in_label[m.sg_arc_base + a];
+    t_arc[a] = sg_in_arc[m.sg_arc_base + a];
+  }
+  // the best accept node of frame T_b (shortest.cpp:147-159), the first of them, and how many share its score
+  const float* sT = sc + (long long)T * pitch;
+  const uint8_t* fl = sg_flags + m.sg_node_base;
+  float mx = neg_inf();
+  for (int i = tid; i < N1; i += kImpThreads)
+    if (fl[i] & 2) mx = fmaxf(mx, sT[i]);
+  mx = block_max(mx, red); // (its barriers also order the table writes above)
+  float first = neg_inf(), n_best = 0.0f; // -(node id), exact in a float
+  for (int i = tid; i < N1; i += kImpThreads)
+    if ((fl[i] & 2) && sT[i] == mx) {
+      first = fmaxf(first, -(float)i);
+      n_best += 1.0f;
+    }
+  first = block_max(first, red);
+  n_best = block_sum(n_best, red);
+  const bool found = T > 0 && is_finite(mx);
+  if (tid == 0) {
+    out_scores[blockIdx.x] = T > 0 ? mx : neg_inf();
+    const int st = ((T > 0 && mx != -CUDART_INF_F && !found) ? 1 : 0) | ((found && n_best > 1.0f) ? kTrTie : 0);
+    if (st) atomicOr(&status[blockIdx.x], st);
+  }
+  for (int t = (found ? T : 0) + tid; t < T_out; t += kImpThreads) {
+    if (po) po[t] = -1;
+    if (ao) ao[t] = -1;
+  }
+  if (!found) return;
+
+  // n rows of `width` floats (the first `valid` read, the rest 0) -> shared memory, kTrLoads independent loads in
+  // flight per thread: one load at a time would make the staging warps, not the walk, set the pace
+  auto copy_rows = [&](float* dst, int dpitch, const float* src, int spitch, int width, int valid, int n, int first,
+                       int nthr) {
+    const int total = n * width;
+    for (int base = tid - first; base < total; base += kTrLoads * nthr) {
+      float v[kTrLoads];
+#pragma unroll
+      for (int u = 0; u < kTrLoads; u++) {
+        const int idx = base + u * nthr, k = idx / width, i = idx - k * width;
+        v[u] = (idx < total && i < valid) ? __ldg(src + (long long)k * spitch + i) : 0.0f;
+      }
+#pragma unroll
+      for (int u = 0; u < kTrLoads; u++) {
+        const int idx = base + u * nthr, k = idx / width, i = idx - k * width;
+        if (idx < total) dst[k * dpitch + i] = v[u];
+      }
+    }
+  };
+  // block j holds frames [max(0, T - (j+1)K), T - jK) in buffer j & 1
+  auto stage = [&](int j, int first, int nthr) {
+    const int fhi = T - j * K, flo = max(0, fhi - K), n = fhi - flo;
+    float* ds = buf + (j & 1) * bstride;
+    copy_rows(ds, lay.pitch, sc + (long long)flo * pitch, pitch, pitch, N1, n, first, nthr);
+    copy_rows(ds + K * lay.pitch, C, em + (long long)flo * C, C, C, C, n, first, nthr);
+  };
+  const int nblk = (T + K - 1) / K;
+  stage(0, 0, kImpThreads);
+  __syncthreads();
+  const int v = (int)-first;
+  float s = mx;
+  int e0 = t_inptr[v], e1 = t_inptr[v + 1]; // the in-entries of v, fetched one step ahead by the lane that picks v
+  bool tie = false, lost = false;
+  for (int j = 0; j < nblk; j++) {
+    if (tid < 32) {
+      const int fhi = T - j * K, flo = max(0, fhi - K);
+      const float* blk = buf + (j & 1) * bstride;
+      for (int f = fhi - 1; f >= flo; f--) {
+        const float* Srow = blk + (f - flo) * lay.pitch;
+        const float* Erow = blk + K * lay.pitch + (f - flo) * C;
+        int pick = -1, hits = 0, n0 = e0, n1 = e0;
+        float ns = s;
+        for (int base = e0; base < e1; base += 32) {
+          const int a = base + lane;
+          int p0 = 0, p1 = 0;
+          float sp = neg_inf();
+          bool hit = false;
+          if (a < e1) {
+            const int src = t_src[a];
+            sp = Srow[src];
+            p0 = t_inptr[src];
+            p1 = t_inptr[src + 1];
+            hit = sp + (t_w[a] + Erow[t_lab[a]]) == s; // the forward's association, bit for bit
+          }
+          const unsigned mk = __ballot_sync(0xffffffffu, hit);
+          hits += __popc(mk);
+          if (pick < 0 && mk) {
+            const int l = __popc((mk & (0u - mk)) - 1u); // the lowest hit lane
+            pick = base + l;
+            ns = __shfl_sync(0xffffffffu, sp, l);
+            n0 = __shfl_sync(0xffffffffu, p0, l);
+            n1 = __shfl_sync(0xffffffffu, p1, l);
+          }
+        }
+        tie |= hits > 1;
+        lost |= hits == 0; // (cannot happen with finite values; the caller re-runs the utterance if it does)
+        if (lane == 0) {
+          if (po) po[f] = pick < 0 ? -1 : t_lab[pick];
+          if (ao) ao[f] = pick < 0 ? -1 : t_arc[pick];
+        }
+        s = ns;
+        e0 = n0;
+        e1 = n1;
+      }
+    } else if (j + 1 < nblk) {
+      stage(j + 1, 32, kImpThreads - 32);
+    }
+    __syncthreads();
+  }
+  if (tid == 0 && (tie || lost)) atomicOr(&status[blockIdx.x], (tie ? kTrTie : 0) | (lost ? 1 : 0));
+}
+
 } // namespace
 
 namespace {
@@ -1163,11 +1399,12 @@ bool implicit_supported(const gtnb_lattice* lat) {
 namespace {
 
 /* the launch of one mode; the arc-label instantiations carry their own names in the profile log */
-template <bool ARC>
+template <bool ARC, bool TROP>
 int implicit_forward_mode(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0, int nb) {
   const int G = wide_lanes(lat->max_in_deg, lat->max_out_deg, lat->max_lvl_nodes, lat->C, false, ARC);
   const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, false, G > 0, lat->C, ARC);
-  const char* name = ARC ? "implicit_forward_arc" : "implicit_forward";
+  const char* name = ARC ? (TROP ? "implicit_forward_arc_max" : "implicit_forward_arc")
+                         : (TROP ? "implicit_forward_max" : "implicit_forward");
 #define GTNB_LAUNCH_FWD(K)                                                                \
   do {                                                                                    \
     if (lay.total > 48 * 1024) {                                                          \
@@ -1177,13 +1414,13 @@ int implicit_forward_mode(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev,
     GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_FWD_ARGS)); \
   } while (0)
   switch (G) {
-    case 0: GTNB_LAUNCH_FWD(implicit_forward_kernel<ARC>); break;
-    case 1: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<1, ARC>)); break;
-    case 2: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<2, ARC>)); break;
-    case 4: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<4, ARC>)); break;
-    case 8: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<8, ARC>)); break;
-    case 16: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<16, ARC>)); break;
-    default: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<32, ARC>)); break;
+    case 0: GTNB_LAUNCH_FWD((implicit_forward_kernel<ARC, TROP>)); break;
+    case 1: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<1, ARC, TROP>)); break;
+    case 2: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<2, ARC, TROP>)); break;
+    case 4: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<4, ARC, TROP>)); break;
+    case 8: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<8, ARC, TROP>)); break;
+    case 16: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<16, ARC, TROP>)); break;
+    default: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<32, ARC, TROP>)); break;
   }
 #undef GTNB_LAUNCH_FWD
   return GTNB_OK;
@@ -1233,11 +1470,45 @@ int implicit_backward_mode(
 } // namespace
 
 /* utterances [b0, b0 + nb) of the batch (nb < 0: all): one CTA each, on ctx->stream */
-int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0, int nb) {
+int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0, int nb, bool tropical) {
   if (nb < 0) nb = lat->B - b0;
   if (nb <= 0) return GTNB_OK;
-  return lat->arc_labels ? implicit_forward_mode<true>(ctx, lat, status_dev, b0, nb)
-                         : implicit_forward_mode<false>(ctx, lat, status_dev, b0, nb);
+  if (tropical)
+    return lat->arc_labels ? implicit_forward_mode<true, true>(ctx, lat, status_dev, b0, nb)
+                           : implicit_forward_mode<false, true>(ctx, lat, status_dev, b0, nb);
+  return lat->arc_labels ? implicit_forward_mode<true, false>(ctx, lat, status_dev, b0, nb)
+                         : implicit_forward_mode<false, false>(ctx, lat, status_dev, b0, nb);
+}
+
+namespace {
+/* the staged block of the traceback: kTrMaxFrames frames, halved until the CTA fits two per SM */
+TraceLayout trace_layout(const gtnb_lattice* lat) {
+  TraceLayout lay = make_trace_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, lat->C, kTrMaxFrames);
+  while (lay.K > 1 && lay.total > kTrSmemTarget)
+    lay = make_trace_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, lat->C, lay.K / 2);
+  return lay;
+}
+} // namespace
+
+bool implicit_trace_supported(const gtnb_lattice* lat) {
+  return trace_layout(lat).total <= kMaxDynamicSmem;
+}
+
+int launch_implicit_trace(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int32_t* paths, int32_t* arcs,
+                          float* scores_out, int T_out) {
+  if (lat->B <= 0) return GTNB_OK;
+  const TraceLayout lay = trace_layout(lat);
+  if (lay.total > kMaxDynamicSmem) return fail(ctx, GTNB_ERR_UNSUPPORTED, "implicit_trace: graphs too large");
+  if (lay.total > 48 * 1024) {
+    int rc = ensure_max_smem(ctx, (const void*)implicit_trace_kernel);
+    if (rc) return rc;
+  }
+  GTNB_LAUNCH(ctx, "implicit_trace",
+              implicit_trace_kernel<<<lat->B, kImpThreads, lay.total, ctx->stream>>>(
+                  lat->meta, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w,
+                  lat->sg_in_arc, lat->emissions, lat->scores, status_dev, paths, arcs, scores_out, T_out, lat->C,
+                  lay));
+  return GTNB_OK;
 }
 
 /* grad_graph (may be NULL): gradients w.r.t. the graph operands' arc weights, slab of graph b at

@@ -421,3 +421,44 @@ def graph_transitions_loss(emissions, transitions, graphs, kind="asg", input_len
                            reduction="mean", allreduce=True):
     return GraphTransitionsLossFunction.apply(emissions, transitions, weights, graphs, kind, input_lengths, reduction,
                                               allreduce)
+
+
+@torch.no_grad()
+def graph_viterbi(emissions, graphs, input_lengths=None, weights=None):
+    """Best path of compose(A_b, E_b) for every utterance, A_b = graphs[b] (viterbiPath / viterbiScore of the lattice
+    graph_loss sums over), through gtnb_graph_viterbi: the alignment the model picks within its own target graph, e.g.
+    a forced alignment with CTC, word-piece decomposition or hand-built graphs.
+
+    emissions: float32 CUDA tensor [B, T, C]; graphs, input_lengths and weights as in graph_loss (weights: None, or
+    a float32 CUDA tensor of sum_b A_b arc weights that replace the graphs' own).  Returns (paths [B, T] int32, the
+    matched label of the arc taken at every frame; scores [B] float32, viterbiScore; arcs [B, T] int32, that arc's id
+    in graphs[b]), all -1 beyond T_b and where there is no accepting path (score -inf), as CUDA tensors on the
+    emissions' device, written on the current stream.  Ties are broken as the reference breaks them.
+    collapse(paths, blank) turns the paths into transcripts.
+    """
+    assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    assert len(graphs) == B
+    views = [_graph_view(g) for g in graphs]
+    n_arcs = sum(v.num_arcs for v, _ in views)
+    arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
+    w = None
+    if weights is not None:
+        assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
+        assert weights.numel() == n_arcs
+        w = weights.detach().contiguous()
+    current = torch.cuda.current_stream(e.device)
+    g = _ctx_for(e.device, current.cuda_stream)
+    il = _lengths(input_lengths, B)
+    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)  # every entry is written by the call
+    arcs = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    scores = torch.empty(B, dtype=torch.float32, device=e.device)
+    # the context's stream is the current stream unless that is the legacy default stream: order the two both ways
+    ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(g.h), device=e.device)
+    ctx_stream.wait_stream(current)
+    g._check(capi.lib().gtnb_graph_viterbi(
+        g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
+        None if w is None else w.data_ptr(), 1, paths.data_ptr(), arcs.data_ptr(), scores.data_ptr(), 1))
+    current.wait_stream(ctx_stream)
+    return paths, scores, arcs

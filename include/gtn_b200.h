@@ -570,6 +570,42 @@ int gtnb_graph_transitions_loss(
     float* trans_grad, /* nullable */
     int trans_grad_on_device);
 
+/*
+ * Batched Viterbi alignment over one user-supplied target graph per utterance: viterbiPath and viterbiScore of
+ * compose(A_b, E_b), the best path through the user's own graph (a forced alignment with any topology; CTC graphs
+ * give CTC forced alignment).  E_b, graphs, arc_weights, the olabel matching, labels outside [0, C) and the epsilon
+ * rule are exactly those of gtnb_graph_loss.  The lattice is frame synchronous, so a path has exactly T_b arcs, one
+ * per frame: paths ([B][T], nullable) gets the matched label of the arc taken at frame t, arcs ([B][T], nullable)
+ * that arc's id in A_b (Graph arc numbering), both -1 beyond T_b and in every slot when there is no accepting path;
+ * EVERY entry is written.  scores ([B], nullable): viterbiScore, -inf without an accepting path (T_b = 0 included:
+ * linearGraph(0, C) accepts nothing; so do infeasible and empty graphs).  Outputs live on the device when
+ * outputs_on_device, else on the host; emissions and arc_weights each where their own flag says.
+ * Paths and scores equal the reference's, ties included: the frames are swept in the tropical semiring without
+ * building the lattice and the path is traced back from the saved scores; an utterance whose traced path meets a
+ * tie, or whose sweep meets a non-finite value, is re-run alone on the materialised lattice (gtnb_compose_linear,
+ * gtnb_forward, gtnb_viterbi_path), as is the whole batch when the graphs do not fit the sweep's layout or the
+ * "implicit" flag is off.  With "exact_ties" off a tie keeps the device route's path, which is then one of the
+ * optimal paths.  The call reads back one status word per utterance to decide the route, so unlike
+ * gtnb_viterbi_dense_ex it returns only once every output is complete, on the device ones too.
+ * Malformed views, input_lens outside [0, T] or negative are GTNB_ERR_INVALID_ARGUMENT; an epsilon arc is
+ * GTNB_ERR_UNSUPPORTED.  B = 0 is a no-op.
+ */
+int gtnb_graph_viterbi(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    int32_t* paths, /* [B][T] nullable: matched label of the arc taken at frame t */
+    int32_t* arcs, /* [B][T] nullable: that arc's id in A_b (Graph arc numbering) */
+    float* scores, /* [B] nullable: viterbiScore */
+    int outputs_on_device);
+
 #ifdef __cplusplus
 }
 #endif
