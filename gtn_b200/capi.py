@@ -110,6 +110,9 @@ SYMBOLS = [
     ("gtnb_graph_viterbi", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _vp, _vp, _vp,
       C.c_int]),
+    ("gtnb_graph_transitions_viterbi", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.c_int, _vp, C.c_int,
+      _vp, _vp, _vp, C.c_int]),
 ]
 
 _lib = None
@@ -648,6 +651,65 @@ class Ctx:
             for buf in bufs:
                 buf.free()
         return losses, grads, ag, tg
+
+    def graph_transitions_viterbi(self, emissions, views, trans_w, kind=DENSE_ASG, input_lens=None, arc_weights=None):
+        """Host-buffer entry of gtnb_graph_transitions_viterbi: emissions [B,T,C], views: B (view, keepalive) pairs
+        from make_view, trans_w [C + C*C] (DENSE_ASG) or [C*C] (DENSE_BIGRAM), arc_weights [sum A_b] or None
+        -> (paths [B,T] int32, scores [B], arcs [B,T] int32)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
+        assert aw is None or aw.size == n_arcs
+        paths = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
+        arcs = np.full((max(B, 1), max(T, 1)), -7, np.int32)
+        scores = np.full(max(B, 1), np.nan, np.float32)
+        self._check(lib().gtnb_graph_transitions_viterbi(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0, kind,
+            tw.ctypes.data, 0, paths.ctypes.data, arcs.ctypes.data, scores.ctypes.data, 0))
+        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
+
+    def graph_transitions_viterbi_dev(self, emissions, views, trans_w, kind=DENSE_ASG, input_lens=None,
+                                      arc_weights=None, trans_on_device=True):
+        """Device-buffer entry: emissions (and arc_weights, when given; trans_w unless trans_on_device is False)
+        uploaded once, gtnb_graph_transitions_viterbi on device pointers (outputs in HBM), downloaded afterwards
+        -> (paths, scores, arcs)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        fill = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
+        bufs = [self.to_device(e), self.to_device(fill), self.to_device(fill),
+                self.to_device(np.full(max(B, 1), np.nan, np.float32))]
+        e_dev, p_dev, a_dev, s_dev = bufs
+        w_dev = aw_dev = None
+        if trans_on_device:
+            w_dev = self.to_device(tw)
+            bufs.append(w_dev)
+        if arc_weights is not None:
+            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
+            assert aw.size == n_arcs
+            aw_dev = self.to_device(aw)
+            bufs.append(aw_dev)
+        try:
+            self._check(lib().gtnb_graph_transitions_viterbi(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if aw_dev is None else aw_dev.ptr, 1, kind,
+                tw.ctypes.data if w_dev is None else w_dev.ptr, int(w_dev is not None), p_dev.ptr, a_dev.ptr,
+                s_dev.ptr, 1))
+            paths = p_dev.download(fill.shape, np.int32)
+            arcs = a_dev.download(fill.shape, np.int32)
+            scores = s_dev.download((max(B, 1),))
+        finally:
+            for buf in bufs:
+                buf.free()
+        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
 
 
 class Lattice:

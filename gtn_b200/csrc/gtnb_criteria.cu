@@ -1626,16 +1626,31 @@ struct GraphViterbiArgs {
   int outputs_on_device;
 };
 
+/* every view's first arc in the batch's numbering, and iota = 0, 1, ... as long as the largest view's arc list */
+void arc_numbering(const std::vector<gtnb_graph_view>& views, std::vector<long long>* first_arc,
+                   std::vector<int32_t>* iota) {
+  first_arc->assign(views.size(), 0);
+  int max_arcs = 0;
+  for (size_t b = 0; b < views.size(); b++) {
+    if (b > 0) (*first_arc)[b] = (*first_arc)[b - 1] + views[b - 1].num_arcs;
+    max_arcs = std::max(max_arcs, views[b].num_arcs);
+  }
+  iota->resize(std::max(max_arcs, 1));
+  for (int k = 0; k < max_arcs; k++) (*iota)[k] = k;
+}
+
 /*
  * The materialised route for the utterances `which`: gtnb_compose_linear (the lattice is put in the reference's
  * relaxation order while exact_ties is on, k_order.cu), gtnb_forward(tropical) for the score and gtnb_viterbi_path.
  * A_b is matched on its olabels, so its ilabels play no part in the composition: they are replaced by the arc ids,
  * which the path's ilabels then carry back.  The rows are written into the device outputs p_dev / a_dev (nullable)
- * and s_dev.
+ * and s_dev.  arc_map (nullable): per utterance, the arc the caller reports for each arc of views[b]
+ * (gtnb_graph_transitions_viterbi: views[b] is compose(A_b, G), the map its gradInfo into A_b).
  */
 int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::vector<gtnb_graph_view>& views,
                         const std::vector<int32_t>& Tb, long long tot_arcs, const float* e_dev,
-                        const std::vector<int>& which, int32_t* p_dev, int32_t* a_dev, float* s_dev) {
+                        const std::vector<int>& which, int32_t* p_dev, int32_t* a_dev, float* s_dev,
+                        const std::vector<std::vector<int32_t>>* arc_map = nullptr) {
   gtnb_ctx* ctx = scope.ctx();
   const int T = a.T, C = a.C, ml = std::max(T, 1);
   const long long per = (long long)T * C;
@@ -1644,14 +1659,9 @@ int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::
     host_w.resize((size_t)std::max(tot_arcs, 1ll));
     GTNB_TRY(read_to_host(ctx, host_w.data(), a.arc_weights, 1, tot_arcs));
   }
-  std::vector<long long> first_arc(a.B, 0);
-  int max_arcs = 0;
-  for (int b = 0; b < a.B; b++) {
-    if (b > 0) first_arc[b] = first_arc[b - 1] + views[b - 1].num_arcs;
-    max_arcs = std::max(max_arcs, views[b].num_arcs);
-  }
-  std::vector<int32_t> iota(std::max(max_arcs, 1));
-  for (int k = 0; k < max_arcs; k++) iota[k] = k;
+  std::vector<long long> first_arc;
+  std::vector<int32_t> iota;
+  arc_numbering(views, &first_arc, &iota);
   // the utterances with frames (T_b = 0 accepts nothing) and their emission rows, contiguous
   std::vector<int> sub;
   for (int b : which)
@@ -1694,7 +1704,7 @@ int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::
     const int len = run ? plen[k] : -1;
     for (int t = 0; t < T; t++) {
       prow[j * ml + t] = t < len ? plab[k * ml + t] : -1;
-      arow[j * ml + t] = t < len ? parc[k * ml + t] : -1;
+      arow[j * ml + t] = t >= len ? -1 : arc_map ? (*arc_map)[b][parc[k * ml + t]] : parc[k * ml + t];
     }
     srow[j] = run ? sc[k] : -std::numeric_limits<float>::infinity();
     if (p_dev && T > 0)
@@ -1709,26 +1719,72 @@ int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::
   return scope.sync();
 }
 
+/* the device buffers of a graph Viterbi call: the emissions, the outputs (the user's own when they are on the
+ * device) and one zeroed status word per utterance */
+struct ViterbiBufs {
+  float *e_dev = nullptr, *s_dev = nullptr;
+  int32_t *p_dev = nullptr, *a_dev = nullptr, *status = nullptr;
+};
+
+int viterbi_open(CallScope& scope, const GraphViterbiArgs& a, ViterbiBufs* v) {
+  gtnb_ctx* ctx = scope.ctx();
+  const long long nrow = (long long)a.B * a.T;
+  const bool dev_out = a.outputs_on_device != 0;
+  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, (long long)a.T * a.C * a.B, &v->e_dev));
+  GTNB_TRY(scope.borrow(a.scores, a.scores && dev_out, a.B, &v->s_dev));
+  if (a.paths) GTNB_TRY(scope.borrow(a.paths, dev_out, nrow, &v->p_dev));
+  if (a.arcs) GTNB_TRY(scope.borrow(a.arcs, dev_out, nrow, &v->a_dev));
+  GTNB_TRY(scope.alloc(&v->status, a.B));
+  GTNB_CUDA(ctx, cudaMemsetAsync(v->status, 0, sizeof(int32_t) * a.B, ctx->stream));
+  return GTNB_OK;
+}
+
+/*
+ * The tail both graph Viterbi calls share.  implicit: the device route has written every row, and one status word
+ * per utterance decides which re-run alone on the exact route: bit 1 a non-finite value, bit 2 a tie on the traced
+ * path while exact_ties is on.  Otherwise every utterance takes the exact route.  exact(which) writes the rows of
+ * `which`; then host outputs are copied out.
+ */
+template <typename Exact>
+int viterbi_finish(CallScope& scope, const GraphViterbiArgs& a, const std::vector<int32_t>& Tb, bool implicit,
+                   const ViterbiBufs& v, Exact&& exact) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B;
+  const long long nrow = (long long)B * a.T;
+  std::vector<int> which;
+  if (implicit) {
+    GTNB_TRY(readback_reserve(ctx, sizeof(int32_t) * B));
+    int32_t* st = reinterpret_cast<int32_t*>(ctx->readback);
+    GTNB_CUDA(ctx, cudaMemcpyAsync(st, v.status, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    GTNB_TRY(scope.sync());
+    for (int b = 0; b < B; b++)
+      if (Tb[b] > 0 && ((st[b] & 1) || ((st[b] & 2) && ctx->exact_ties))) which.push_back(b);
+  } else {
+    for (int b = 0; b < B; b++) which.push_back(b);
+  }
+  if (!which.empty()) GTNB_TRY(exact(which));
+  if (!a.outputs_on_device) {
+    if (a.scores)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a.scores, v.s_dev, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a.paths && nrow)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a.paths, v.p_dev, sizeof(int32_t) * nrow, cudaMemcpyDeviceToHost, ctx->stream));
+    if (a.arcs && nrow)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(a.arcs, v.a_dev, sizeof(int32_t) * nrow, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  return scope.sync();
+}
+
 int graph_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const std::vector<gtnb_graph_view>& views,
                       const std::vector<int32_t>& Tb, long long tot_arcs) {
   gtnb_ctx* ctx = scope.ctx();
   const int B = a.B, T = a.T, C = a.C;
-  const long long per = (long long)T * C, nrow = (long long)B * T;
-  const bool dev_out = a.outputs_on_device != 0;
-  float *e_dev = nullptr, *s_dev = nullptr;
-  int32_t *p_dev = nullptr, *a_dev = nullptr, *status = nullptr;
-  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
-  GTNB_TRY(scope.borrow(a.scores, a.scores && dev_out, B, &s_dev));
-  if (a.paths) GTNB_TRY(scope.borrow(a.paths, dev_out, nrow, &p_dev));
-  if (a.arcs) GTNB_TRY(scope.borrow(a.arcs, dev_out, nrow, &a_dev));
-  GTNB_TRY(scope.alloc(&status, B));
-  GTNB_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(int32_t) * B, ctx->stream));
-
-  std::vector<int> exact;
+  const long long per = (long long)T * C;
+  ViterbiBufs v;
+  GTNB_TRY(viterbi_open(scope, a, &v));
   bool implicit = ctx->use_implicit;
   gtnb_lattice*& lat = scope.lattice();
   if (implicit) {
-    const int rc = compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, e_dev, per, true, &lat, true,
+    const int rc = compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, v.e_dev, per, true, &lat, true,
                                        a.arc_weights_on_device ? a.arc_weights : nullptr);
     if (rc == GTNB_ERR_UNSUPPORTED) // does not fit the implicit layout: materialise
       implicit = false;
@@ -1737,28 +1793,12 @@ int graph_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const std::ve
     implicit = implicit && implicit_trace_supported(lat);
   }
   if (implicit) {
-    GTNB_TRY(launch_implicit_forward(ctx, lat, status, 0, -1, /*tropical=*/true));
-    GTNB_TRY(launch_implicit_trace(ctx, lat, status, p_dev, a_dev, s_dev, T));
-    // one status word per utterance decides the route: bit 1 a non-finite value, bit 2 a tie on the traced path
-    GTNB_TRY(readback_reserve(ctx, sizeof(int32_t) * B));
-    int32_t* st = reinterpret_cast<int32_t*>(ctx->readback);
-    GTNB_CUDA(ctx, cudaMemcpyAsync(st, status, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ctx->stream));
-    GTNB_TRY(scope.sync());
-    for (int b = 0; b < B; b++)
-      if (Tb[b] > 0 && ((st[b] & 1) || ((st[b] & 2) && ctx->exact_ties))) exact.push_back(b);
-  } else {
-    for (int b = 0; b < B; b++) exact.push_back(b);
+    GTNB_TRY(launch_implicit_forward(ctx, lat, v.status, 0, -1, /*tropical=*/true));
+    GTNB_TRY(launch_implicit_trace(ctx, lat, v.status, v.p_dev, v.a_dev, v.s_dev, T));
   }
-  if (!exact.empty()) GTNB_TRY(graph_viterbi_exact(scope, a, views, Tb, tot_arcs, e_dev, exact, p_dev, a_dev, s_dev));
-  if (!dev_out) {
-    if (a.scores)
-      GTNB_CUDA(ctx, cudaMemcpyAsync(a.scores, s_dev, sizeof(float) * B, cudaMemcpyDeviceToHost, ctx->stream));
-    if (a.paths && nrow)
-      GTNB_CUDA(ctx, cudaMemcpyAsync(a.paths, p_dev, sizeof(int32_t) * nrow, cudaMemcpyDeviceToHost, ctx->stream));
-    if (a.arcs && nrow)
-      GTNB_CUDA(ctx, cudaMemcpyAsync(a.arcs, a_dev, sizeof(int32_t) * nrow, cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  return scope.sync();
+  return viterbi_finish(scope, a, Tb, implicit, v, [&](const std::vector<int>& which) {
+    return graph_viterbi_exact(scope, a, views, Tb, tot_arcs, v.e_dev, which, v.p_dev, v.a_dev, v.s_dev);
+  });
 }
 
 } // namespace
@@ -1781,4 +1821,184 @@ extern "C" int gtnb_graph_viterbi(
   const GraphViterbiArgs a{B, T, C, emissions, emissions_on_device, arc_weights, arc_weights_on_device,
                            paths, arcs, scores, outputs_on_device};
   return graph_viterbi_run(scope, a, views, Tb, tot_arcs);
+}
+
+/*
+ * Viterbi alignment over user-supplied target graphs with learned transitions: viterbiPath / viterbiScore of the
+ * numerators of gtnb_graph_transitions_loss, compose(compose(A_b, G), E_b) for ASG and
+ * intersect(intersect(A_b, G), E_b) for BIGRAM.  The device route sweeps the loss's products (gtnb_product.h, BIGRAM
+ * folded) in the tropical semiring, with weights folded on the device from the transitions where they lie; BIGRAM's
+ * folded start arcs read tau_l = max_j W[l][j] there instead of sigma_l.  The trace reports product arcs, which
+ * launch_product_arc_map takes back to A_b's.  The exact route composes A_b with G in the reference's own numbering
+ * (gtnb_compose_graphs) and runs graph_viterbi_exact on the result, so ties break as the reference breaks them.
+ */
+namespace {
+
+int graph_transitions_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, bool bigram, const float* trans_w,
+                                    int trans_on_device, const std::vector<gtnb_graph_view>& views,
+                                    const std::vector<int32_t>& Tb, long long tot_arcs, const float* e_dev,
+                                    const std::vector<int>& which, int32_t* p_dev, int32_t* a_dev, float* s_dev) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, C = a.C;
+  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
+  std::vector<float> W(n_trans), w_A;
+  GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
+  if (a.arc_weights && a.arc_weights_on_device) {
+    w_A.resize((size_t)std::max(tot_arcs, 1ll));
+    GTNB_TRY(read_to_host(ctx, w_A.data(), a.arc_weights, 1, tot_arcs));
+  }
+  HostGraph G;
+  dense_graph(bigram, C, W.data(), &G, nullptr);
+  const gtnb_graph_view gv = G.view();
+  // A'_b: A_b with its ilabels replaced by the arc ids (A_b is matched on its olabels, so the composition is the
+  // same); the pairs that can accept anything
+  std::vector<long long> first_arc;
+  std::vector<int32_t> iota;
+  arc_numbering(views, &first_arc, &iota);
+  std::vector<int> pairs;
+  std::vector<gtnb_graph_view> first;
+  for (int b : which) {
+    if (Tb[b] == 0 || views[b].num_nodes == 0) continue;
+    gtnb_graph_view v = views[b];
+    v.arc_ilabel = iota.data();
+    if (!w_A.empty()) v.weights = w_A.data() + first_arc[b];
+    pairs.push_back(b);
+    first.push_back(v);
+  }
+  const int n = (int)pairs.size();
+  // the composed graphs on the host, in the reference's numbering; arc_map[b]: the A_b arc of each of their arcs
+  struct Composed {
+    std::vector<uint8_t> flags;
+    std::vector<int32_t> src, dst, il, ol;
+    std::vector<float> w;
+  };
+  std::vector<Composed> cg(n);
+  std::vector<std::vector<int32_t>> arc_map(B);
+  std::vector<gtnb_graph_view> cviews(B);
+  for (auto& v : cviews) std::memset(&v, 0, sizeof(v)); // (utterances without a pair: the empty graph)
+  if (n > 0) {
+    std::vector<int32_t> kind(n, 0); // the reference's unsorted matcher
+    gtnb_composed* res = nullptr;
+    GTNB_TRY(gtnb_compose_graphs(ctx, n, first.data(), n, &gv, 1, kind.data(), &res));
+    int rc = GTNB_OK;
+    for (int k = 0; k < n && rc == GTNB_OK; k++) {
+      int32_t N = 0, A = 0;
+      rc = gtnb_composed_sizes(res, k, &N, &A);
+      if (rc != GTNB_OK) {
+        rc = fail(ctx, rc, "gtnb_graph_transitions_viterbi: sizes of a composed graph");
+        break;
+      }
+      Composed& c = cg[k];
+      c.flags.resize(std::max(N, 1));
+      for (auto* x : {&c.src, &c.dst, &c.il, &c.ol}) x->resize(std::max(A, 1));
+      c.w.resize(std::max(A, 1));
+      std::vector<int32_t>& m = arc_map[pairs[k]];
+      m.resize(std::max(A, 1));
+      rc = gtnb_composed_download(ctx, res, k, c.flags.data(), c.src.data(), c.dst.data(), c.il.data(), c.ol.data(),
+                                  c.w.data(), m.data(), nullptr);
+      gtnb_graph_view& v = cviews[pairs[k]];
+      v.num_nodes = N;
+      v.num_arcs = A;
+      v.node_flags = c.flags.data();
+      v.arc_src = c.src.data();
+      v.arc_dst = c.dst.data();
+      v.arc_ilabel = c.il.data();
+      v.arc_olabel = c.ol.data();
+      v.weights = c.w.data();
+    }
+    gtnb_composed_destroy(ctx, res);
+    GTNB_TRY(rc);
+  }
+  GraphViterbiArgs ca = a;
+  ca.arc_weights = nullptr; // the composed graphs carry their weights
+  return graph_viterbi_exact(scope, ca, cviews, Tb, 0, e_dev, which, p_dev, a_dev, s_dev, &arc_map);
+}
+
+int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, bool bigram, const float* trans_w,
+                                  int trans_on_device, const std::vector<gtnb_graph_view>& views,
+                                  const std::vector<int32_t>& Tb, long long tot_arcs) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C;
+  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
+  ViterbiBufs v;
+  GTNB_TRY(viterbi_open(scope, a, &v));
+
+  // the loss's numerators (BIGRAM folded), whose shapes decide whether the device route can be taken
+  std::vector<ProductGraph> prods(B);
+  std::vector<SgDims> dims(B);
+  for (int b = 0; b < B; b++) {
+    build_product(views[b], C, bigram, /*fold=*/true, &prods[b]);
+    const ProductGraph& p = prods[b];
+    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, /*uniform=*/1, p.max_in,
+                     p.max_out};
+  }
+  bool implicit = ctx->use_implicit && implicit_dims_supported(dims.data(), B);
+  GraphNumerator num{prods, views, Tb, C, bigram, a.arc_weights && a.arc_weights_on_device ? a.arc_weights : nullptr,
+                     nullptr, 0, tot_arcs};
+  gtnb_lattice*& lat = scope.lattice();
+  if (implicit) {
+    GTNB_TRY(num.alloc(scope, v.e_dev, per, nullptr));
+    float *w_dev = nullptr, *tau = nullptr;
+    long long* off = nullptr;
+    GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, n_trans, &w_dev));
+    if (bigram) GTNB_TRY(scope.alloc(&tau, C));
+    // off: every utterance's first product arc, then its first A arc (launch_product_arc_map)
+    std::vector<long long> off_h(2 * (size_t)B, 0);
+    for (int b = 1; b < B; b++) {
+      off_h[b] = off_h[b - 1] + (long long)prods[b - 1].src.size();
+      off_h[B + b] = off_h[B + b - 1] + views[b - 1].num_arcs;
+    }
+    if (v.a_dev) GTNB_TRY(scope.alloc(&off, 2ll * B));
+    GTNB_TRY(stage_begin(ctx));
+    GTNB_TRY(num.stage(scope, nullptr));
+    if (!trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
+    if (off) GTNB_TRY(stage_upload(ctx, off, off_h.data(), sizeof(long long) * 2 * B));
+    GTNB_TRY(stage_end(ctx));
+    if (bigram) GTNB_TRY(launch_ngram_tau(ctx, C, w_dev, tau));
+    const int rc = num.build(scope, lat, w_dev, tau);
+    if (rc == GTNB_ERR_UNSUPPORTED) // does not fit the implicit layout: materialise
+      implicit = false;
+    else
+      GTNB_TRY(rc);
+    implicit = implicit && implicit_trace_supported(lat);
+    if (implicit) {
+      GTNB_TRY(launch_implicit_forward(ctx, lat, v.status, 0, -1, /*tropical=*/true));
+      GTNB_TRY(launch_implicit_trace(ctx, lat, v.status, v.p_dev, v.a_dev, v.s_dev, T));
+      if (v.a_dev) GTNB_TRY(launch_product_arc_map(ctx, B, T, off, num.arc_of, v.a_dev));
+    }
+  }
+  return viterbi_finish(scope, a, Tb, implicit, v, [&](const std::vector<int>& which) {
+    return graph_transitions_viterbi_exact(scope, a, bigram, trans_w, trans_on_device, views, Tb, tot_arcs, v.e_dev,
+                                           which, v.p_dev, v.a_dev, v.s_dev);
+  });
+}
+
+} // namespace
+
+extern "C" int gtnb_graph_transitions_viterbi(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, int kind,
+    const float* trans_w, int trans_on_device, int32_t* paths, int32_t* arcs, float* scores, int outputs_on_device) {
+  const char* fn = "gtnb_graph_transitions_viterbi";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !trans_w || (B > 0 && (!emissions || !graphs)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown graph kind");
+  if (C > kNgramMaxLabels)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                std::string(fn) + ": C = " + std::to_string(C) + " labels; the product builder takes C <= " +
+                    std::to_string(kNgramMaxLabels));
+  std::vector<int32_t> Tb;
+  std::vector<gtnb_graph_view> views;
+  long long tot_arcs = 0;
+  GTNB_TRY(parse_graphs(ctx, fn, B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
+                        &tot_arcs));
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  const GraphViterbiArgs a{B, T, C, emissions, emissions_on_device, arc_weights, arc_weights_on_device,
+                           paths, arcs, scores, outputs_on_device};
+  return graph_transitions_viterbi_run(scope, a, kind == GTNB_DENSE_BIGRAM, trans_w, trans_on_device, views, Tb,
+                                       tot_arcs);
 }

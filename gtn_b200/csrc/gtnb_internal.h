@@ -370,6 +370,11 @@ int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, 
 // out[k] = w_A[arc_of[k]] + Wx[tidx[k]], Wx = [W (nW floats) | sigma]: the weights of gtnb_product.h's products
 int launch_product_fold(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W, int nW,
                         const float* sigma, const int32_t* tidx, float* out);
+// tau_i = max_j W[i][j] (NaN-propagating): the tropical sigma of BIGRAM's folded start arcs
+int launch_ngram_tau(gtnb_ctx* ctx, int C, const float* W, float* tau);
+// arcs [B][T_out], product arc ids (-1 none) -> A arc ids: arc_of[off[b] + a] - off[B + b]
+int launch_product_arc_map(gtnb_ctx* ctx, int B, int T_out, const long long* off, const int32_t* arc_of,
+                           int32_t* arcs);
 // the same trellis in ASG's start mode (trans_w, trans_grad: [C + C*C], start weights first) and ASG's
 // forced-alignment numerator graphs built on the device
 long long asg_alpha_floats(int B, int T, int C); // floats of the alpha buffer of launch_asg_den_*

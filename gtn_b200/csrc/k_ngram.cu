@@ -296,6 +296,42 @@ __global__ void __launch_bounds__(256) ngram_sigma_kernel(int C, const float* __
   if (lane == 0) sigma[i] = m + logf(s);
 }
 
+/* the max of two floats that keeps a NaN of either (fmaxf drops it) */
+__device__ __forceinline__ float max_nan(float a, float b) {
+  return (b > a || b != b) ? b : a;
+}
+
+/*
+ * tau_i = max_j W[i][j], one warp per row: the tropical sigma, the weight of BIGRAM's folded start arcs on
+ * gtnb_graph_transitions_viterbi's device route.  A NaN anywhere in the row gives tau_i = NaN, so the weights the
+ * sweep loads carry it and flag the utterance for the exact route.
+ */
+__global__ void __launch_bounds__(256) ngram_tau_kernel(int C, const float* __restrict__ W, float* __restrict__ tau) {
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (i >= C) return; // whole warps
+  float m = neg_inf();
+  for (int j = lane; j < C; j += 32) m = max_nan(m, __ldg(W + i * C + j));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) tau[i] = m;
+}
+
+/*
+ * The traced arcs of gtnb_graph_transitions_viterbi from product arc ids to A_b's arc ids, in place: row b of
+ * arcs ([B][T_out]) holds product arcs of utterance b (-1: no arc), arc_of its A arcs in the batch's numbering;
+ * off[b] = b's first product arc, off[B + b] = b's first A arc.  One thread per entry.
+ */
+__global__ void __launch_bounds__(256) product_arc_map_kernel(
+    long long n, int T_out, const long long* __restrict__ off, const int32_t* __restrict__ arc_of,
+    int32_t* __restrict__ arcs) {
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int a = arcs[k];
+  if (a < 0) return;
+  const int b = (int)(k / T_out);
+  arcs[k] = __ldg(arc_of + __ldg(off + b) + a) - (int32_t)__ldg(off + (n / T_out) + b);
+}
+
 /* wgrad[i][j] += wgrad[C*C + i] * softmax_j(W[i][:]): the S arcs' gradient through sigma_i */
 __global__ void __launch_bounds__(256) ngram_fold_kernel(
     int C, const float* __restrict__ W, const float* __restrict__ sigma, float* __restrict__ wgrad) {
@@ -564,6 +600,20 @@ int launch_product_fold(gtnb_ctx* ctx, long long n, const float* w_A, const int3
   if (n == 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "product_fold", product_fold_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
       n, w_A, arc_of, W, nW, sigma, tidx, out));
+  return GTNB_OK;
+}
+
+int launch_ngram_tau(gtnb_ctx* ctx, int C, const float* W, float* tau) {
+  GTNB_LAUNCH(ctx, "ngram_tau", ngram_tau_kernel<<<(C * 32 + 255) / 256, 256, 0, ctx->stream>>>(C, W, tau));
+  return GTNB_OK;
+}
+
+int launch_product_arc_map(gtnb_ctx* ctx, int B, int T_out, const long long* off, const int32_t* arc_of,
+                           int32_t* arcs) {
+  const long long n = (long long)B * T_out;
+  if (n == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "product_arc_map", product_arc_map_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
+      n, T_out, off, arc_of, arcs));
   return GTNB_OK;
 }
 

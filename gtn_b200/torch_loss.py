@@ -462,3 +462,49 @@ def graph_viterbi(emissions, graphs, input_lengths=None, weights=None):
         None if w is None else w.data_ptr(), 1, paths.data_ptr(), arcs.data_ptr(), scores.data_ptr(), 1))
     current.wait_stream(ctx_stream)
     return paths, scores, arcs
+
+
+@torch.no_grad()
+def graph_transitions_viterbi(emissions, transitions, graphs, kind="asg", input_lengths=None, weights=None):
+    """Best path of graph_transitions_loss's numerator for every utterance, through gtnb_graph_transitions_viterbi:
+        kind "asg":    viterbiPath / viterbiScore of compose(compose(A_b, G), E_b)
+        kind "bigram": viterbiPath / viterbiScore of intersect(intersect(A_b, G), E_b)
+    the decomposition and frame-level alignment a model trained with graph_transitions_loss picks within its own
+    target graph.  emissions, transitions, graphs, kind, input_lengths and weights as in graph_transitions_loss.
+    Returns (paths [B, T] int32, the label of the arc taken at every frame; scores [B] float32, viterbiScore; arcs
+    [B, T] int32, that arc's id in graphs[b]), all -1 beyond T_b and where there is no accepting path (score -inf), as
+    CUDA tensors on the emissions' device, written on the current stream.  Ties are broken as the reference breaks
+    them.  collapse(paths, blank) turns the paths into transcripts.
+    """
+    assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+    assert kind in ("asg", "bigram")
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    assert len(graphs) == B
+    assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+    kid = capi.DENSE_BIGRAM if kind == "bigram" else capi.DENSE_ASG
+    assert transitions.numel() == (Cn * Cn if kid == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+    tw = transitions.detach().contiguous()
+    views = [_graph_view(g) for g in graphs]
+    n_arcs = sum(v.num_arcs for v, _ in views)
+    arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
+    w = None
+    if weights is not None:
+        assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
+        assert weights.numel() == n_arcs
+        w = weights.detach().contiguous()
+    current = torch.cuda.current_stream(e.device)
+    g = _ctx_for(e.device, current.cuda_stream)
+    il = _lengths(input_lengths, B)
+    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)  # every entry is written by the call
+    arcs = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    scores = torch.empty(B, dtype=torch.float32, device=e.device)
+    # the context's stream is the current stream unless that is the legacy default stream: order the two both ways
+    ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(g.h), device=e.device)
+    ctx_stream.wait_stream(current)
+    g._check(capi.lib().gtnb_graph_transitions_viterbi(
+        g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
+        None if w is None else w.data_ptr(), 1, kid, tw.data_ptr(), 1, paths.data_ptr(), arcs.data_ptr(),
+        scores.data_ptr(), 1))
+    current.wait_stream(ctx_stream)
+    return paths, scores, arcs

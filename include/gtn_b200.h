@@ -606,6 +606,49 @@ int gtnb_graph_viterbi(
     float* scores, /* [B] nullable: viterbiScore */
     int outputs_on_device);
 
+/*
+ * Batched Viterbi alignment over one user-supplied target graph per utterance with a learned dense transition graph
+ * G: viterbiPath and viterbiScore of the numerators of gtnb_graph_transitions_loss,
+ *   GTNB_DENSE_ASG:    compose(compose(A_b, G), E_b),
+ *   GTNB_DENSE_BIGRAM: intersect(intersect(A_b, G), E_b),
+ * the decomposition and frame-level alignment a model trained with that loss picks.  G, trans_w's layouts, E_b,
+ * graphs, arc_weights, the olabel matching, labels outside [0, C) and the epsilon rule are exactly those of
+ * gtnb_graph_transitions_loss.  Outputs are those of gtnb_graph_viterbi: paths ([B][T], nullable) gets the label of
+ * the arc taken at frame t, arcs ([B][T], nullable) that arc's id in A_b (Graph arc numbering), both -1 beyond T_b
+ * and in every slot when there is no accepting path; EVERY entry is written.  scores ([B], nullable): viterbiScore,
+ * -inf without an accepting path (T_b = 0, an empty graph, a graph with no start node and an infeasible graph
+ * included).  Outputs live on the device when outputs_on_device, else on the host; emissions, arc_weights and
+ * trans_w each where their own flag says.
+ * Paths, arcs and scores equal the reference's, ties included.  The device route sweeps the loss's products in the
+ * tropical semiring (BIGRAM's folded start arcs weigh tau_l = max_j W[l][j]) with the transitions on the device and
+ * traces the path back; an utterance whose traced path meets a tie (with "exact_ties" on), or whose sweep meets a
+ * non-finite value, is re-run alone on compose(A_b, G) built in the reference's numbering (gtnb_compose_graphs,
+ * then gtnb_compose_linear, gtnb_forward, gtnb_viterbi_path), as is the whole batch when the products do not fit
+ * the sweep's layout or the "implicit" flag is off; only that route reads the transitions to the host.  The call
+ * reads back one status word per utterance, so it returns only once every output is complete, device ones too.
+ * C > 128 and an epsilon arc are GTNB_ERR_UNSUPPORTED, as is a pair too large for gtnb_compose_graphs on the exact
+ * route; an unknown kind, T_b > T, negative lengths or a malformed view are GTNB_ERR_INVALID_ARGUMENT.  B = 0 is a
+ * no-op.
+ */
+int gtnb_graph_transitions_viterbi(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    int kind, /* GTNB_DENSE_ASG | GTNB_DENSE_BIGRAM */
+    const float* trans_w,
+    int trans_on_device,
+    int32_t* paths, /* [B][T] nullable: label of the arc taken at frame t */
+    int32_t* arcs, /* [B][T] nullable: that frame's arc id in A_b (Graph arc numbering) */
+    float* scores, /* [B] nullable: viterbiScore */
+    int outputs_on_device);
+
 #ifdef __cplusplus
 }
 #endif

@@ -61,6 +61,44 @@ def as_dict(g):
     return go.make(d["flags"], d["src"], d["dst"], d["ilabel"], d["olabel"], d["weights"])
 
 
+def transitions(C, kind):
+    """the workloads' seeded transitions: [C + C*C] for ASG, [C*C] for BIGRAM"""
+    n = (C + C * C) if kind == capi.DENSE_ASG else C * C
+    return np.random.default_rng(5).uniform(-1, 1, n).astype(np.float32)
+
+
+def decomp_graphs(rng, B, n_labels):
+    """B word-piece decomposition graphs of seeded transcripts of ~60 letters over go.inventory(26, n_labels) ->
+    (graphs, C = pieces + 1)"""
+    pieces = go.inventory(26, n_labels, seed=7)
+    gs = []
+    for b in range(B):
+        letters = [int(x) for x in rng.integers(0, 26, int(rng.integers(55, 66)))]
+        g = as_dict(go.decomposition_graph(GTN_OPS, letters, pieces))
+        g["w"] = rng.uniform(-0.5, 0.5, len(g["src"])).astype(np.float32)
+        gs.append(g)
+    return gs, len(pieces) + 1
+
+
+def workloads():
+    """the four workloads of the module docstring, built in turn -> (name, emissions, graphs, kind, input lengths or
+    None, targets or None)"""
+    B, T = 128, 500
+    rng = np.random.default_rng(11)
+    dec, C = decomp_graphs(rng, B, 128)
+    e = np.random.default_rng(12).uniform(-5, 5, (B, T, C)).astype(np.float32)
+    yield "decomp_asg", e, dec, capi.DENSE_ASG, None, None
+    B, T, C, U = 128, 500, 64, 50
+    e, targets = util.bench_inputs(B, T, C, U)
+    lens = np.full(B, T, np.int32)
+    yield "ctc_bigram", e, [go.ctc_graph(t, blank=0) for t in targets], capi.DENSE_BIGRAM, lens, targets
+    yield "fal_asg", e, [gt.fal_graph(t) for t in targets], capi.DENSE_ASG, lens, targets
+    B, T = 128, 500
+    dec, C = decomp_graphs(rng, B, 64)
+    e = np.random.default_rng(13).uniform(-5, 5, (B, T, C)).astype(np.float32)
+    yield "wildcard_asg", e, [go.with_wildcards(g, C, w_loop=-1.0) for g in dec], capi.DENSE_ASG, None, None
+
+
 class Lib:
     """a build of libgtn_b200.so and a context of it (path None: this build, on ctx)"""
 
@@ -154,7 +192,7 @@ def main():
         views = [capi.make_view(g["flags"], g["src"], g["dst"], g["ilabel"], g["olabel"], g["w"]) for g in graphs]
         arr = (capi.GraphView * B)(*[v for v, _ in views])
         n_arcs = sum(len(g["src"]) for g in graphs)
-        tw = np.random.default_rng(5).uniform(-1, 1, (C + C * C) if kind == capi.DENSE_ASG else C * C).astype(np.float32)
+        tw = transitions(C, kind)
         il = None if lens is None else np.ascontiguousarray(lens, np.int32)
         bufs = dict(e=ctx.to_device(e), g=ctx.alloc(e.nbytes), ag=ctx.alloc(4 * max(n_arcs, 4)), tw=ctx.to_device(tw),
                     tg=ctx.alloc(tw.nbytes))
@@ -265,49 +303,14 @@ def main():
            "l2": "flushed before every timed call",
            "buffers": "emissions, transitions and every gradient on the device; graphs as host views"}
 
-    # 1. word-piece decompositions, ASG transitions, C = 128
-    B, T = 128, 500
-    rng = np.random.default_rng(11)
-
-    def decomps(n_labels):
-        pieces = go.inventory(26, n_labels, seed=7)
-        gs = []
-        for b in range(B):
-            letters = [int(x) for x in rng.integers(0, 26, int(rng.integers(55, 66)))]
-            g = as_dict(go.decomposition_graph(GTN_OPS, letters, pieces))
-            g["w"] = rng.uniform(-0.5, 0.5, len(g["src"])).astype(np.float32)
-            gs.append(g)
-        return gs, len(pieces) + 1
-
-    dec, C = decomps(128)
-    e = np.random.default_rng(12).uniform(-5, 5, (B, T, C)).astype(np.float32)
-    out["decomp_asg"], bufs, _, _ = workload(e, dec, capi.DENSE_ASG)
-    for b in bufs.values():
-        b.free()
-
-    # 2. CTC graphs + bigram transitions, 3. force-align chains + ASG transitions, at the n-gram shape
-    B, T, C, U = 128, 500, 64, 50
-    e, targets = util.bench_inputs(B, T, C, U)
-    lens = np.full(B, T, np.int32)
-    rec, bufs, tw, gl = workload(e, [go.ctc_graph(t, blank=0) for t in targets], capi.DENSE_BIGRAM, lens)
-    target_criterion("gtnb_ngram_ctc_loss", bufs, tw, targets, lens, gl, rec)
-    out["ctc_bigram"] = rec
-    for b in bufs.values():
-        b.free()
-    rec, bufs, tw, gl = workload(e, [gt.fal_graph(t) for t in targets], capi.DENSE_ASG, lens)
-    target_criterion("gtnb_asg_loss_ex", bufs, tw, targets, lens, gl, rec)
-    out["fal_asg"] = rec
-    for b in bufs.values():
-        b.free()
-
-    # 4. wildcard graphs, C = 64
-    B, T = 128, 500
-    dec, C = decomps(64)
-    e = np.random.default_rng(13).uniform(-5, 5, (B, T, C)).astype(np.float32)
-    out["wildcard_asg"], bufs, _, _ = workload(e, [go.with_wildcards(g, C, w_loop=-1.0) for g in dec],
-                                               capi.DENSE_ASG)
-    for b in bufs.values():
-        b.free()
+    criteria = {"ctc_bigram": "gtnb_ngram_ctc_loss", "fal_asg": "gtnb_asg_loss_ex"}
+    for name, e, graphs, kind, lens, targets in workloads():
+        rec, bufs, tw, gl = workload(e, graphs, kind, lens)
+        if name in criteria:  # the same inputs through the built-in target graphs' criterion
+            target_criterion(criteria[name], bufs, tw, targets, lens, gl, rec)
+        out[name] = rec
+        for b in bufs.values():
+            b.free()
 
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", "0"],
                        capture_output=True, text=True).stdout.strip()
