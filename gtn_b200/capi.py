@@ -107,6 +107,9 @@ SYMBOLS = [
     ("gtnb_graph_transitions_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.c_int, _vp, C.c_int,
       _f32p, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int]),
+    ("gtnb_sparse_transitions_loss", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.POINTER(GraphView),
+      _vp, C.c_int, _f32p, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int]),
     ("gtnb_graph_viterbi", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _vp, _vp, _vp,
       C.c_int]),
@@ -647,6 +650,69 @@ class Ctx:
             grads = g_dev.download(e.shape)
             ag = ag_dev.download((max(n_arcs, 1),))[:n_arcs]
             tg = tg_dev.download(tw.shape)
+        finally:
+            for buf in bufs:
+                buf.free()
+        return losses, grads, ag, tg
+
+    def sparse_transitions_loss(self, emissions, views, transitions, trans_w, want_grad=True, input_lens=None,
+                                arc_weights=None):
+        """Host-buffer entry of gtnb_sparse_transitions_loss: emissions [B,T,C], views: B (view, keepalive) pairs from
+        make_view, transitions: G's (view, keepalive) pair (an acceptor; its weights are ignored), trans_w
+        [G.num_arcs], arc_weights [sum A_b] or None
+        -> (losses [B], grads [B,T,C] or None, arc_grads [sum A_b] or None, trans_grad [G.num_arcs] or None)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        gv = transitions[0]
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == gv.num_arcs
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
+        assert aw is None or aw.size == n_arcs
+        losses = np.zeros(B, np.float32)
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
+        tg = np.full(max(tw.size, 1), np.nan, np.float32) if want_grad else None
+        self._check(lib().gtnb_sparse_transitions_loss(
+            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0,
+            C.byref(gv), tw.ctypes.data if tw.size else None, 0, _p(losses, _f32p),
+            None if grads is None else grads.ctypes.data, 0, None if ag is None else ag.ctypes.data, 0,
+            None if tg is None else tg.ctypes.data, 0))
+        return (losses, grads, None if ag is None else ag[:n_arcs], None if tg is None else tg[:tw.size])
+
+    def sparse_transitions_loss_dev(self, emissions, views, transitions, trans_w, input_lens=None, arc_weights=None):
+        """Device-buffer entry: emissions, trans_w (and arc_weights, when given) uploaded once,
+        gtnb_sparse_transitions_loss on device pointers (gradients in HBM), downloaded afterwards
+        -> (losses, grads, arc_grads, trans_grad)."""
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        assert len(views) == B
+        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+        n_arcs = sum(v.num_arcs for v, _ in views)
+        gv = transitions[0]
+        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+        assert tw.size == gv.num_arcs
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        losses = np.zeros(B, np.float32)
+        bufs = [self.to_device(e), self.alloc(max(e.nbytes, 16)), self.alloc(4 * max(n_arcs, 4)),
+                self.to_device(tw if tw.size else np.zeros(1, np.float32)), self.alloc(max(tw.nbytes, 16))]
+        e_dev, g_dev, ag_dev, w_dev, tg_dev = bufs
+        aw_dev = None
+        if arc_weights is not None:
+            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
+            assert aw.size == n_arcs
+            aw_dev = self.to_device(aw)
+            bufs.append(aw_dev)
+        try:
+            self._check(lib().gtnb_sparse_transitions_loss(
+                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if aw_dev is None else aw_dev.ptr, 1,
+                C.byref(gv), w_dev.ptr, 1, _p(losses, _f32p), g_dev.ptr, 1, ag_dev.ptr, 1, tg_dev.ptr, 1))
+            grads = g_dev.download(e.shape)
+            ag = ag_dev.download((max(n_arcs, 1),))[:n_arcs]
+            tg = tg_dev.download((max(tw.size, 1),))[:tw.size]
         finally:
             for buf in bufs:
                 buf.free()

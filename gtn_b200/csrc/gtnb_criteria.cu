@@ -917,6 +917,29 @@ struct TrellisCriterion {
   bool fold;
   decltype(&launch_ngram_den_forward) den_forward;
   decltype(&launch_ngram_den_backward) den_backward;
+  float* alpha = nullptr;
+
+  /*
+   * The interface of trellis_loss_fast's denominators: n_sigma (the folded start weights, 0 without a fold), alloc
+   * (scratch), stage (uploads in the call's one staging pass), sigma (the folded start weights from the transitions
+   * on the device), forward / backward (the sweeps; the backward adds into the zero-filled emission rows and the
+   * transition gradient), fold (the sigma slots of the gradient into the transitions').
+   */
+  long long n_sigma(int C) const { return fold ? C : 0; }
+  int alloc(CallScope& scope, int /*B*/, int /*T*/) { return scope.alloc(&alpha, alpha_floats); }
+  int stage(CallScope&) { return GTNB_OK; }
+  int sigma(gtnb_ctx* ctx, int C, const float* w, float* sig) { return launch_ngram_sigma(ctx, C, w, sig); }
+  int forward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
+              float* den, int32_t* status) {
+    return den_forward(ctx, B, T, C, lens, e, per, w, alpha, den, status);
+  }
+  int backward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
+               const float* den, float* grad, float* wgrad) {
+    return den_backward(ctx, B, T, C, lens, e, per, w, alpha, den, grad, per, wgrad);
+  }
+  int fold_grad(gtnb_ctx* ctx, int C, const float* w, const float* sig, float* wgrad) {
+    return launch_ngram_fold(ctx, C, w, sig, wgrad);
+  }
 };
 
 /*
@@ -961,14 +984,14 @@ struct TargetsNumerator {
   int scatter(CallScope&, const float*) { return GTNB_OK; }
 };
 
-template <class Numerator>
-int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const TransitionArgs& a, Numerator& num,
-                      bool* needs_exact) {
+template <class Numerator, class Denominator>
+int trellis_loss_fast(CallScope& scope, Denominator& k, const TransitionArgs& a, Numerator& num, bool* needs_exact) {
   gtnb_ctx* ctx = scope.ctx();
   const int B = a.B, T = a.T, C = a.C;
   const long long per = (long long)T * C;
+  const long long n_sigma = k.n_sigma(C);
   const bool want = a.grads || a.trans_grad || num.wants_arc_grads();
-  float *e_dev = nullptr, *w_dev = nullptr, *sigma = nullptr, *alpha = nullptr, *den = nullptr;
+  float *e_dev = nullptr, *w_dev = nullptr, *sigma = nullptr, *den = nullptr;
   float *ggrad = nullptr, *minus1 = nullptr;
   int32_t* status = nullptr;
   OutBuf g, tg;
@@ -979,15 +1002,15 @@ int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const Transit
   GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
   GTNB_TRY(scope.borrow(a.trans_w, a.trans_on_device != 0, k.n_trans, &w_dev)); // (host: staged below)
   GTNB_TRY(scope.alloc(&status, 2ll * B));
-  if (k.fold) GTNB_TRY(scope.alloc(&sigma, C));
-  GTNB_TRY(scope.alloc(&alpha, k.alpha_floats));
+  if (n_sigma) GTNB_TRY(scope.alloc(&sigma, n_sigma));
+  GTNB_TRY(k.alloc(scope, B, T));
   GTNB_TRY(scope.alloc(&den, B));
   GTNB_TRY(num.alloc(scope, e_dev, per, &lat));
   const long long tot_A = num.tot_A;
   if (want) {
-    const long long n_grad = k.n_trans + (k.fold ? C : 0); // [d/dtrans | d/dsigma]
+    const long long n_grad = k.n_trans + n_sigma; // [d/dtrans | d/dsigma]
     GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
-    GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, n_grad, &tg, /*alias=*/!k.fold));
+    GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, n_grad, &tg, /*alias=*/!n_sigma));
     GTNB_TRY(scope.alloc(&ggrad, tot_A));
     GTNB_TRY(scope.alloc(&minus1, B));
     GTNB_CUDA(ctx, cudaMemsetAsync(g.dev, 0, sizeof(float) * per * B, ctx->stream));
@@ -999,11 +1022,12 @@ int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const Transit
   // transitions from the host, the -1 seeds
   GTNB_TRY(stage_begin(ctx));
   GTNB_TRY(num.stage(scope, lat));
+  GTNB_TRY(k.stage(scope));
   if (!a.trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, a.trans_w, sizeof(float) * k.n_trans));
   if (want) GTNB_TRY(stage_upload(ctx, minus1, m1.data(), sizeof(float) * B));
   GTNB_TRY(stage_end(ctx));
 
-  if (k.fold) GTNB_TRY(launch_ngram_sigma(ctx, C, w_dev, sigma));
+  if (n_sigma) GTNB_TRY(k.sigma(ctx, C, w_dev, sigma));
   GTNB_TRY(num.build(scope, lat, w_dev, sigma));
   // the numerator (a few in-arcs per node) on the second stream beside the denominator (C^2 per frame)
   GTNB_TRY(fork_to(ctx, ctx->copy_stream));
@@ -1013,12 +1037,12 @@ int trellis_loss_fast(CallScope& scope, const TrellisCriterion& k, const Transit
     if (want) GTNB_TRY(launch_implicit_backward(ctx, lat, minus1, g.dev, per, 0, -1, ggrad));
   }
   const int32_t* T_dev = num.T_dev();
-  GTNB_TRY(k.den_forward(ctx, B, T, C, T_dev, e_dev, per, w_dev, alpha, den, status));
-  if (want) GTNB_TRY(k.den_backward(ctx, B, T, C, T_dev, e_dev, per, w_dev, alpha, den, g.dev, per, tg.dev));
+  GTNB_TRY(k.forward(ctx, B, T, C, T_dev, e_dev, per, w_dev, den, status));
+  if (want) GTNB_TRY(k.backward(ctx, B, T, C, T_dev, e_dev, per, w_dev, den, g.dev, tg.dev));
   GTNB_TRY(join_from(ctx, ctx->copy_stream));
   if (want) {
     GTNB_TRY(launch_scatter_add(ctx, tg.dev, num.map, ggrad, tot_A)); // numerator arcs -> transition (and sigma) slots
-    if (k.fold) GTNB_TRY(launch_ngram_fold(ctx, C, w_dev, sigma, tg.dev));
+    if (n_sigma) GTNB_TRY(k.fold_grad(ctx, C, w_dev, sigma, tg.dev));
     GTNB_TRY(num.scatter(scope, ggrad));
     GTNB_TRY(g.copy_out(ctx, per * B));
     GTNB_TRY(tg.copy_out(ctx, k.n_trans));
@@ -1195,7 +1219,7 @@ extern "C" int gtnb_ngram_ctc_loss(
     dims[b] = SgDims{L + 1, L + (L - 1) + t.skips[b] + std::min(L, 2), L >= 2 ? 2 : 1, /*all_valid=*/1,
                      /*uniform=*/1, /*max_in=*/3, /*max_out=*/3};
   }
-  const TrellisCriterion ngram{(long long)C * C, (long long)B * (T + 1) * C, /*fold=*/true, launch_ngram_den_forward,
+  TrellisCriterion ngram{(long long)C * C, (long long)B * (T + 1) * C, /*fold=*/true, launch_ngram_den_forward,
                                launch_ngram_den_backward};
   const bool fast = implicit_dims_supported(dims.data(), B) && ctx->use_implicit;
   return run_criterion(ctx, B, t.T(), losses_host, trans_grad, trans_grad_on_device, (long long)C * C, fast,
@@ -1239,7 +1263,7 @@ extern "C" int gtnb_asg_loss_ex(
     const int U = target_lens[b];
     dims[b] = SgDims{U + 1, 2 * U, U > 0 ? 1 : 0, /*all_valid=*/1, /*uniform=*/1, /*max_in=*/2, /*max_out=*/2};
   }
-  const TrellisCriterion asg{nTrans, asg_alpha_floats(B, T, C), /*fold=*/false, launch_asg_den_forward,
+  TrellisCriterion asg{nTrans, asg_alpha_floats(B, T, C), /*fold=*/false, launch_asg_den_forward,
                              launch_asg_den_backward};
   // (a non-finite weight: gtnb_asg_loss's sweeps raise the same status bit and end in the materialised lattices)
   const bool fast = C <= kNgramMaxLabels && ctx->use_implicit && implicit_dims_supported(dims.data(), B);
@@ -1441,6 +1465,8 @@ struct GraphNumerator {
   float* arc_grads;
   int arc_grads_on_device;
   long long tot_arcs;
+  int nW = -1; // slots of Wx before sigma; -1: the dense kind's (gtnb_sparse_transitions_loss: G's arc count)
+  bool arc_labels = false; // some product is not label-uniform: k_implicit.cu's arc-label instantiations
   long long tot_A = 0;
   std::vector<gtnb_graph_view> pviews;
   std::vector<int32_t> tidx_h, arc_of_h;
@@ -1497,12 +1523,13 @@ struct GraphNumerator {
   const int32_t* T_dev() const { return Tb_dev; }
   int build(CallScope& scope, gtnb_lattice*& lat, const float* w_dev, const float* sigma) {
     gtnb_ctx* ctx = scope.ctx();
-    const int nW = bigram ? C * C : C + C * C;
-    GTNB_TRY(launch_product_fold(ctx, tot_A, arc_weights_dev ? arc_weights_dev : w_A, arc_of, w_dev, nW, sigma, map,
+    const int n_w = nW >= 0 ? nW : bigram ? C * C : C + C * C;
+    GTNB_TRY(launch_product_fold(ctx, tot_A, arc_weights_dev ? arc_weights_dev : w_A, arc_of, w_dev, n_w, sigma, map,
                                  fw));
-    // the products are label-uniform: the plain instantiations, with the folded weights gathered into the tables
+    // the dense kinds' products are label-uniform: the plain instantiations, with the folded weights gathered into
+    // the tables
     return compose_linear_impl(ctx, (int)pviews.size(), pviews.data(), (int)pviews.size(), 0, Tb.data(), C, e_dev,
-                               per, true, &lat, false, fw);
+                               per, true, &lat, arc_labels, fw);
   }
   int scatter(CallScope& scope, const float* ggrad) {
     if (!arc_grads) return GTNB_OK;
@@ -1586,7 +1613,7 @@ extern "C" int gtnb_graph_transitions_loss(
     dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, /*uniform=*/1, p.max_in,
                      p.max_out};
   }
-  const TrellisCriterion k = bigram ? TrellisCriterion{n_trans, (long long)B * (T + 1) * C, /*fold=*/true,
+  TrellisCriterion k = bigram ? TrellisCriterion{n_trans, (long long)B * (T + 1) * C, /*fold=*/true,
                                                        launch_ngram_den_forward, launch_ngram_den_backward}
                                     : TrellisCriterion{n_trans, asg_alpha_floats(B, T, C), /*fold=*/false,
                                                        launch_asg_den_forward, launch_asg_den_backward};
@@ -1601,6 +1628,166 @@ extern "C" int gtnb_graph_transitions_loss(
                                             arc_weights && arc_weights_on_device ? arc_weights : nullptr,
                                             arc_grads, arc_grads_on_device, tot_arcs};
                          return trellis_loss_fast(scope, k, a, num, needs_exact);
+                       });
+}
+
+/*
+ * Loss over user-supplied target graphs with a learned transition graph G of any shape (an epsilon-free acceptor:
+ * n-gram graphs of any order, pruned token LMs, HMM topologies; the intersect(emissions, transitions) pattern of the
+ * reference's benchmarks/ctc.cpp and examples):
+ *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b))
+ * with E_b, A_b and the arc weights of gtnb_graph_transitions_loss and G's weights in trans_w by arc id.  The device
+ * route sweeps the denominator with k_sparse.cu over G's tables and the folded products of gtnb_product.h with
+ * k_implicit.cu (trellis_loss_fast); a non-finite value, the implicit flag off, or a G or product outside the
+ * kernels' layout take the materialised lattices with the unfolded products.
+ */
+namespace {
+
+/* trellis_loss_fast's denominator for a G of any shape: G's tables and start groups in one device buffer */
+struct SparseDenominator {
+  const SparseTables& t;
+  long long n_trans; // G's arcs, labels outside [0, C) included
+  std::vector<int32_t> packed;
+  int32_t* tab = nullptr;
+  float* alpha = nullptr;
+  double* offs = nullptr;
+  SparseDev dev{};
+  const int32_t *grp_ptr = nullptr, *grp_arc = nullptr;
+
+  int groups() const { return (int)t.grp_ptr.size() - 1; }
+  long long n_sigma(int) const { return groups(); }
+  int alloc(CallScope& scope, int B, int T) {
+    packed.assign(t.flags.begin(), t.flags.end());
+    std::vector<size_t> at;
+    for (const std::vector<int32_t>* v : {&t.in_ptr, &t.in_src, &t.in_lab, &t.in_arc, &t.out_ptr, &t.out_dst,
+                                          &t.out_lab, &t.out_arc, &t.grp_ptr, &t.grp_arc}) {
+      at.push_back(packed.size());
+      packed.insert(packed.end(), v->begin(), v->end());
+    }
+    GTNB_TRY(scope.alloc(&tab, (long long)packed.size()));
+    dev = SparseDev{t.S, t.A, sparse_den_lanes(t.S, t.A), tab, tab + at[0], tab + at[1], tab + at[2], tab + at[3],
+                    tab + at[4], tab + at[5], tab + at[6], tab + at[7]};
+    grp_ptr = tab + at[8];
+    grp_arc = tab + at[9];
+    GTNB_TRY(scope.alloc(&alpha, (long long)B * (T + 1) * t.S));
+    return scope.alloc(&offs, (long long)B * (T + 1));
+  }
+  int stage(CallScope& scope) { return stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()); }
+  int sigma(gtnb_ctx* ctx, int, const float* w, float* sig) {
+    return launch_sparse_sigma(ctx, groups(), grp_ptr, grp_arc, w, sig);
+  }
+  int forward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
+              float* den, int32_t* status) {
+    return launch_sparse_den_forward(ctx, dev, B, T, C, lens, e, per, w, alpha, offs, den, status);
+  }
+  int backward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
+               const float*, float* grad, float* wgrad) {
+    return launch_sparse_den_backward(ctx, dev, B, T, C, lens, e, per, w, alpha, offs, grad, per, wgrad);
+  }
+  int fold_grad(gtnb_ctx* ctx, int, const float* w, const float* sig, float* wgrad) {
+    return launch_sparse_fold(ctx, groups(), grp_ptr, grp_arc, (int)n_trans, w, sig, wgrad);
+  }
+};
+
+/* the materialised route: G (its arcs with a label in [0, C)) weighted on the host, the unfolded products */
+int sparse_transitions_exact(CallScope& scope, const TransitionArgs& a, const gtnb_graph_view& Gv,
+                             const SparseTables& t, const std::vector<gtnb_graph_view>& views,
+                             const std::vector<int32_t>& Tb, const float* arc_weights, int arc_weights_on_device,
+                             float* arc_grads, int arc_grads_on_device, long long tot_arcs) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, C = a.C;
+  const long long n_trans = Gv.num_arcs;
+  std::vector<float> W(std::max<long long>(n_trans, 1)), w_A;
+  if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, n_trans));
+  if (arc_weights && arc_weights_on_device && tot_arcs) {
+    w_A.resize(tot_arcs);
+    GTNB_TRY(read_to_host(ctx, w_A.data(), arc_weights, 1, tot_arcs));
+  }
+  HostGraph G;
+  G.flags = t.flags;
+  std::vector<int32_t> gmap;
+  for (int g = 0; g < Gv.num_arcs; g++)
+    if (Gv.arc_olabel[g] >= 0 && Gv.arc_olabel[g] < C) {
+      G.arc(Gv.arc_src[g], Gv.arc_dst[g], Gv.arc_olabel[g], W[g]);
+      gmap.push_back(g);
+    }
+  std::vector<ProductGraph> prods(B);
+  std::vector<std::vector<float>> pw(B);
+  std::vector<gtnb_graph_view> pviews(B);
+  std::vector<int32_t> pmap, arc_of;
+  long long off = 0;
+  for (int b = 0; b < B; b++) {
+    build_sparse_product(views[b], Gv, t, C, /*fold=*/false, &prods[b]);
+    product_weights(prods[b], w_A.empty() ? views[b].weights : w_A.data() + off, W.data(), &pw[b]);
+    pviews[b] = prods[b].view();
+    pviews[b].weights = pw[b].data();
+    pmap.insert(pmap.end(), prods[b].tidx.begin(), prods[b].tidx.end());
+    for (int32_t k : prods[b].arc_of) arc_of.push_back((int32_t)(off + k));
+    off += views[b].num_arcs;
+  }
+  OutBuf ag;
+  if (arc_grads) GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, tot_arcs, &ag));
+  return transitions_loss_materialised(scope, a, Tb.data(), G, gmap, n_trans, pviews, pmap, &arc_of,
+                                       arc_grads ? &ag : nullptr, tot_arcs);
+}
+
+} // namespace
+
+extern "C" int gtnb_sparse_transitions_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
+    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, float* losses_host, float* grads,
+    int grads_on_device, float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const std::string fn = "gtnb_sparse_transitions_loss";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !transitions ||
+      (B > 0 && (!emissions || !graphs || !losses_host || !trans_w)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  const gtnb_graph_view& Gv = *transitions;
+  if (validate_view(ctx, Gv)) return GTNB_ERR_INVALID_ARGUMENT;
+  if (Gv.num_nodes < 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the transition graph has no nodes");
+  for (int g = 0; g < Gv.num_arcs; g++) {
+    if (Gv.arc_ilabel[g] == GTNB_EPSILON || Gv.arc_olabel[g] == GTNB_EPSILON)
+      return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                  fn + ": the transition graph has epsilon arcs; remove them first (remove(g, epsilon))");
+    if (Gv.arc_ilabel[g] != Gv.arc_olabel[g])
+      return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                  fn + ": the transition graph is a transducer; make it an acceptor first (projectInput / "
+                       "projectOutput)");
+  }
+  std::vector<int32_t> Tb;
+  std::vector<gtnb_graph_view> views;
+  long long tot_arcs = 0;
+  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
+                        &tot_arcs));
+  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
+                         nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+  const long long n_trans = Gv.num_arcs;
+  SparseTables t;
+  sparse_tables(Gv, C, &t);
+  // the device route's numerators (folded), whose shapes decide, with G's, whether it can be taken
+  const bool den_fits = ctx->use_implicit && sparse_den_supported(t.S, t.A, C);
+  std::vector<ProductGraph> prods(den_fits ? B : 0);
+  std::vector<SgDims> dims(prods.size());
+  bool uniform = true;
+  for (size_t b = 0; b < prods.size(); b++) {
+    build_sparse_product(views[b], Gv, t, C, /*fold=*/true, &prods[b]);
+    const ProductGraph& p = prods[b];
+    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, p.uniform ? 1 : 0, p.max_in,
+                     p.max_out};
+    uniform &= p.uniform;
+  }
+  const bool fast = den_fits && implicit_dims_supported(dims.data(), B, C);
+  return run_criterion(ctx, B, Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans, fast,
+                       [&](CallScope& scope, bool f, bool* needs_exact) {
+                         if (!f)
+                           return sparse_transitions_exact(scope, a, Gv, t, views, Tb, arc_weights,
+                                                           arc_weights_on_device, arc_grads, arc_grads_on_device,
+                                                           tot_arcs);
+                         SparseDenominator den{t, n_trans};
+                         GraphNumerator num{prods, views, Tb, C, false,
+                                            arc_weights && arc_weights_on_device ? arc_weights : nullptr,
+                                            arc_grads, arc_grads_on_device, tot_arcs, (int)n_trans, !uniform};
+                         return trellis_loss_fast(scope, den, a, num, needs_exact);
                        });
 }
 

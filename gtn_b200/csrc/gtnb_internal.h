@@ -388,6 +388,21 @@ int launch_asg_den_backward(
 int launch_asg_num_build(
     gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
     const int32_t* tgt_len_dev, const float* trans_w, int32_t* map);
+// kernels (k_sparse.cu): the denominator of gtnb_sparse_transitions_loss over a G of any shape (SparseDev, gtnb_meta.h).
+// The envelope, one predicate: 1 <= S <= kSparseMaxStates nodes, A <= kSparseMaxArcs arcs with a label in [0, C),
+// 1 <= C <= kSparseMaxLabels.  alpha: [B][(T+1)*S] floats; offs: [B][T+1] doubles (slot 0: Z).
+bool sparse_den_supported(int S, int A, int C);
+int launch_sparse_den_forward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
+                              const float* emis, long long stride, const float* w, float* alpha, double* offs,
+                              float* den, int32_t* status);
+int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
+                               const float* emis, long long stride, const float* w, const float* alpha,
+                               const double* offs, float* grad, long long grad_stride, float* wgrad);
+// sigma_k = logsumexp of start group k's weights, and its gradient (wgrad[nG + k]) folded back by softmax
+int launch_sparse_sigma(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
+                        float* sigma);
+int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, int nG, const float* w,
+                       const float* sigma, float* wgrad);
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);

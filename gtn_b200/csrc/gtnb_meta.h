@@ -14,6 +14,28 @@ constexpr uint32_t kStartBit = 0x40000000u; // node is a start node
 constexpr uint32_t kAcceptBit = 0x80000000u; // node is an accept node
 constexpr int kAlign = 4; // elements; keeps every per-graph slab 16-byte aligned
 
+/*
+ * G's tables as k_sparse.cu's denominator sweeps read them (gtnb_product.h's SparseTables on the device): S nodes,
+ * A arcs with a label in [0, C); in-arcs by destination, out-arcs by source; *_arc is G's arc id, which indexes the
+ * transition weights and their gradient.  lanes: threads per node (a power of two <= 32).
+ */
+struct SparseDev {
+  int S, A, lanes;
+  const int32_t* flags; // bit 0 start, bit 1 accept
+  const int32_t *in_ptr, *in_src, *in_lab, *in_arc;
+  const int32_t *out_ptr, *out_dst, *out_lab, *out_arc;
+};
+/* the envelope of k_sparse.cu's kernels: rows and arc gradients of G held in shared memory (sparse_den_supported) */
+constexpr int kSparseMaxStates = 4096;
+constexpr int kSparseMaxArcs = 32768;
+constexpr int kSparseMaxLabels = 1024;
+/* SparseDev::lanes: a power of two <= 32 with about four arcs per thread at G's mean degree */
+inline int sparse_den_lanes(int S, int A) {
+  int lanes = 1;
+  while (lanes < 32 && 4ll * lanes * (S > 1 ? S : 1) < (long long)A) lanes *= 2;
+  return lanes;
+}
+
 /* semiring / output of the shortest-distance kernels */
 enum { MODE_LOG = 0, MODE_TROPICAL = 1, MODE_PATH = 2 };
 

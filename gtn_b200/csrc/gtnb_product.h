@@ -22,6 +22,7 @@
 
 #include <algorithm>
 #include <cstdint>
+#include <unordered_map>
 #include <vector>
 
 #include "gtn_b200.h"
@@ -34,6 +35,7 @@ struct ProductGraph {
   std::vector<int32_t> arc_of; // A arc of every product arc
   std::vector<int32_t> tidx; // slot of Wx of every product arc
   int n_acc = 0, max_in = 0, max_out = 0;
+  bool uniform = true; // every node's in-arcs carry one label (build_sparse_product: not always)
 
   gtnb_graph_view view() const {
     gtnb_graph_view v{};
@@ -126,6 +128,231 @@ inline void build_product(const gtnb_graph_view& A, int C, bool bigram, bool fol
   for (size_t k = 0; k < p->src.size(); k++) {
     indeg[p->dst[k]]++;
     outdeg[p->src[k]]++;
+  }
+  p->max_in = *std::max_element(indeg.begin(), indeg.end());
+  p->max_out = *std::max_element(outdeg.begin(), outdeg.end());
+  p->n_acc = (int)std::count_if(p->flags.begin(), p->flags.end(), [](uint8_t f) { return (f & 2) != 0; });
+}
+
+/*
+ * G of gtnb_sparse_transitions_loss: an epsilon-free acceptor of any shape, weights in trans_w by G's arc id.  Arcs
+ * labelled outside [0, C) never match and are left out of every table.
+ *  - in_* (by destination) and out_* (by source, ascending label within a source): the denominator's sweeps
+ *    (k_sparse.cu) and the product builder;
+ *  - the start groups of the fold: the arcs out of start nodes, grouped by (destination, label).  Group k has the
+ *    arcs grp_arc[grp_ptr[k] .. grp_ptr[k + 1]); sigma_k = logsumexp of their weights is the weight of the folded
+ *    start arcs into that destination with that label.
+ */
+struct SparseTables {
+  int S = 0, A = 0, max_in = 0, max_out = 0;
+  std::vector<uint8_t> flags;
+  std::vector<int32_t> in_ptr, in_src, in_lab, in_arc;
+  std::vector<int32_t> out_ptr, out_dst, out_lab, out_arc;
+  std::vector<int32_t> grp_ptr, grp_arc, grp_dst, grp_lab;
+};
+
+inline void sparse_tables(const gtnb_graph_view& G, int C, SparseTables* t) {
+  const int S = G.num_nodes;
+  t->S = S;
+  t->flags.assign(G.node_flags, G.node_flags + S);
+  std::vector<int32_t> kept;
+  for (int g = 0; g < G.num_arcs; g++)
+    if (G.arc_olabel[g] >= 0 && G.arc_olabel[g] < C) kept.push_back(g);
+  t->A = (int)kept.size();
+  auto csr = [&](const int32_t* key, std::vector<int32_t>& order, std::vector<int32_t>& ptr) {
+    ptr.assign(S + 1, 0);
+    for (int g : kept) ptr[key[g] + 1]++;
+    for (int v = 0; v < S; v++) ptr[v + 1] += ptr[v];
+    order = kept; // stable: arc id order within a node
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return key[x] < key[y]; });
+  };
+  std::vector<int32_t> in_order, out_order;
+  csr(G.arc_dst, in_order, t->in_ptr);
+  csr(G.arc_src, out_order, t->out_ptr);
+  for (int u = 0; u < S; u++) // out lists by ascending label (equal_range in build_sparse_product)
+    std::stable_sort(out_order.begin() + t->out_ptr[u], out_order.begin() + t->out_ptr[u + 1],
+                     [&](int x, int y) { return G.arc_olabel[x] < G.arc_olabel[y]; });
+  t->in_src.resize(t->A);
+  t->in_lab.resize(t->A);
+  t->in_arc = in_order;
+  t->out_dst.resize(t->A);
+  t->out_lab.resize(t->A);
+  t->out_arc = out_order;
+  for (int k = 0; k < t->A; k++) {
+    t->in_src[k] = G.arc_src[in_order[k]];
+    t->in_lab[k] = G.arc_olabel[in_order[k]];
+    t->out_dst[k] = G.arc_dst[out_order[k]];
+    t->out_lab[k] = G.arc_olabel[out_order[k]];
+  }
+  t->max_in = t->max_out = 0;
+  for (int v = 0; v < S; v++) {
+    t->max_in = std::max(t->max_in, t->in_ptr[v + 1] - t->in_ptr[v]);
+    t->max_out = std::max(t->max_out, t->out_ptr[v + 1] - t->out_ptr[v]);
+  }
+  std::unordered_map<long long, int> group;
+  std::vector<std::vector<int32_t>> members;
+  for (int g : kept) {
+    if (!(G.node_flags[G.arc_src[g]] & 1)) continue;
+    const long long key = (long long)G.arc_dst[g] * C + G.arc_olabel[g];
+    auto it = group.find(key);
+    if (it == group.end()) {
+      it = group.emplace(key, (int)members.size()).first;
+      members.emplace_back();
+      t->grp_dst.push_back(G.arc_dst[g]);
+      t->grp_lab.push_back(G.arc_olabel[g]);
+    }
+    members[it->second].push_back(g);
+  }
+  t->grp_ptr.assign(1, 0);
+  t->grp_arc.clear();
+  for (const auto& m : members) {
+    t->grp_arc.insert(t->grp_arc.end(), m.begin(), m.end());
+    t->grp_ptr.push_back((int32_t)t->grp_arc.size());
+  }
+}
+
+/*
+ * The numerator of gtnb_sparse_transitions_loss, intersect(A, G), from structure only: the (A node, G node) pairs
+ * reachable from the start pairs, trimmed to those that reach an accept pair (A and G both accept).  An A arc u -> v
+ * and a G arc p -> q with the same label in [0, C) give the arc (u, p) -> (v, q); arc_of is the A arc, tidx the G arc.
+ * Unfolded (the exact route): every (A start, G start) pair is a start state.  Folded (the device route): those start
+ * copies collapse into one start node S (node 0), with one arc S -> (v, q) per out-arc a: u -> v of an A start node u
+ * and per start group k of G with a's label and destination q; its tidx is nG + k (nG = G's arc count), so Wx =
+ * [trans_w | sigma] and its weight is w_a + sigma_k.  The pairs with both nodes start are then ordinary states,
+ * reached through in-arcs only.  An empty product keeps one node that neither starts nor accepts.
+ */
+inline void build_sparse_product(const gtnb_graph_view& A, const gtnb_graph_view& G, const SparseTables& t, int C,
+                                 bool fold, ProductGraph* p) {
+  const int N = A.num_nodes, nA = A.num_arcs, nG = G.num_arcs;
+  const long long S = t.S;
+  std::vector<int32_t> a_ptr(N + 1, 0), a_out;
+  for (int a = 0; a < nA; a++)
+    if (A.arc_olabel[a] >= 0 && A.arc_olabel[a] < C) a_ptr[A.arc_src[a] + 1]++;
+  for (int u = 0; u < N; u++) a_ptr[u + 1] += a_ptr[u];
+  a_out.resize(a_ptr[N]);
+  {
+    std::vector<int32_t> fill(a_ptr.begin(), a_ptr.end() - 1);
+    for (int a = 0; a < nA; a++)
+      if (A.arc_olabel[a] >= 0 && A.arc_olabel[a] < C) a_out[fill[A.arc_src[a]]++] = a;
+  }
+  std::unordered_map<long long, int32_t> id;
+  std::vector<long long> state; // u * S + p of every state; the folded S is -1
+  std::vector<int32_t> src, dst, lab, arc_of, tidx;
+  auto node = [&](int u, int q) {
+    const long long key = (long long)u * S + q;
+    auto it = id.find(key);
+    if (it != id.end()) return it->second;
+    const int32_t n = (int32_t)state.size();
+    id.emplace(key, n);
+    state.push_back(key);
+    return n;
+  };
+  auto put = [&](int s, int d, int l, int a, int g) {
+    src.push_back(s);
+    dst.push_back(d);
+    lab.push_back(l);
+    arc_of.push_back(a);
+    tidx.push_back(g);
+  };
+  const bool a_start_acc = [&] {
+    for (int u = 0; u < N; u++)
+      if ((A.node_flags[u] & 3) == 3) return true;
+    return false;
+  }();
+  bool g_start_acc = false;
+  for (int q = 0; q < t.S; q++) g_start_acc |= (t.flags[q] & 3) == 3;
+  if (fold) {
+    state.push_back(-1); // S
+    std::vector<std::vector<int32_t>> by_label(C);
+    for (size_t k = 0; k + 1 < t.grp_ptr.size(); k++) by_label[t.grp_lab[k]].push_back((int32_t)k);
+    for (int u = 0; u < N; u++) {
+      if (!(A.node_flags[u] & 1)) continue;
+      for (int e = a_ptr[u]; e < a_ptr[u + 1]; e++) {
+        const int a = a_out[e], l = A.arc_olabel[a];
+        for (int32_t k : by_label[l]) put(0, node(A.arc_dst[a], t.grp_dst[k]), l, a, nG + k);
+      }
+    }
+  } else {
+    for (int u = 0; u < N; u++)
+      if (A.node_flags[u] & 1)
+        for (int q = 0; q < t.S; q++)
+          if (t.flags[q] & 1) node(u, q);
+  }
+  // breadth-first over the states found so far; every new state is appended, so one pass reaches them all
+  for (size_t n = fold ? 1 : 0; n < state.size(); n++) {
+    const int u = (int)(state[n] / S), q = (int)(state[n] % S);
+    const int32_t* ol = t.out_lab.data();
+    for (int e = a_ptr[u]; e < a_ptr[u + 1]; e++) {
+      const int a = a_out[e], l = A.arc_olabel[a];
+      const int32_t* lo = std::lower_bound(ol + t.out_ptr[q], ol + t.out_ptr[q + 1], l);
+      for (const int32_t* it = lo; it != ol + t.out_ptr[q + 1] && *it == l; it++) {
+        const int k = (int)(it - ol);
+        put((int)n, node(A.arc_dst[a], t.out_dst[k]), l, a, t.out_arc[k]);
+      }
+    }
+  }
+  const int M = (int)state.size();
+  auto accepts = [&](int n) {
+    if (state[n] < 0) return a_start_acc && g_start_acc;
+    return (A.node_flags[state[n] / S] & 2) && (t.flags[state[n] % S] & 2);
+  };
+  auto starts = [&](int n) {
+    if (fold) return n == 0;
+    return (A.node_flags[state[n] / S] & 1) && (t.flags[state[n] % S] & 1);
+  };
+  // trim: keep the states from which an accept state is reachable
+  std::vector<int32_t> in_ptr(M + 1, 0), in_src(src.size());
+  for (int32_t d : dst) in_ptr[d + 1]++;
+  for (int n = 0; n < M; n++) in_ptr[n + 1] += in_ptr[n];
+  {
+    std::vector<int32_t> fill(in_ptr.begin(), in_ptr.end() - 1);
+    for (size_t k = 0; k < src.size(); k++) in_src[fill[dst[k]]++] = src[k];
+  }
+  std::vector<char> live(M, 0);
+  std::vector<int32_t> stack;
+  for (int n = 0; n < M; n++)
+    if (accepts(n)) {
+      live[n] = 1;
+      stack.push_back(n);
+    }
+  while (!stack.empty()) {
+    const int n = stack.back();
+    stack.pop_back();
+    for (int k = in_ptr[n]; k < in_ptr[n + 1]; k++)
+      if (!live[in_src[k]]) {
+        live[in_src[k]] = 1;
+        stack.push_back(in_src[k]);
+      }
+  }
+  std::vector<int32_t> renum(M, -1);
+  int kept = 0;
+  for (int n = 0; n < M; n++)
+    if (live[n]) renum[n] = kept++;
+  p->flags.assign(std::max(kept, 1), 0);
+  for (int n = 0; n < M; n++)
+    if (live[n]) p->flags[renum[n]] = (uint8_t)((starts(n) ? 1 : 0) | (accepts(n) ? 2 : 0));
+  p->src.clear();
+  p->dst.clear();
+  p->label.clear();
+  p->arc_of.clear();
+  p->tidx.clear();
+  for (size_t k = 0; k < src.size(); k++) {
+    if (!live[src[k]] || !live[dst[k]]) continue;
+    p->src.push_back(renum[src[k]]);
+    p->dst.push_back(renum[dst[k]]);
+    p->label.push_back(lab[k]);
+    p->arc_of.push_back(arc_of[k]);
+    p->tidx.push_back(tidx[k]);
+  }
+  const size_t P = p->flags.size();
+  std::vector<int32_t> indeg(P, 0), outdeg(P, 0), in_label(P, -1);
+  p->uniform = true;
+  for (size_t k = 0; k < p->src.size(); k++) {
+    indeg[p->dst[k]]++;
+    outdeg[p->src[k]]++;
+    int32_t& il = in_label[p->dst[k]];
+    if (il >= 0 && il != p->label[k]) p->uniform = false;
+    il = p->label[k];
   }
   p->max_in = *std::max_element(indeg.begin(), indeg.end());
   p->max_out = *std::max_element(outdeg.begin(), outdeg.end());

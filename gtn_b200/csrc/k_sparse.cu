@@ -1,0 +1,347 @@
+/*
+ * k_sparse.cu -- the denominator of gtnb_sparse_transitions_loss, forwardScore(intersect(E_b, G)) and its gradients,
+ * for a transition graph G of any shape (an epsilon-free acceptor: n-gram graphs of any order, pruned token LMs,
+ * HMM topologies), without building the T_b * |G| lattice.
+ *
+ * The product state at frame t is a G node, so the sweeps are
+ *     alpha_0[v] = 0 on G's start nodes (-inf elsewhere),
+ *     alpha_t[v] = logsumexp over in-arcs a: u -> v of (alpha_{t-1}[u] + w_a + e[t-1][label_a]),
+ *     Z = logsumexp of alpha_{T_b} over G's accept nodes,
+ *     beta_{T_b}[u] = 0 on accept nodes, beta_t[u] = logsumexp over out-arcs a: u -> v of (w_a + e[t][label_a] +
+ *     beta_{t+1}[v]),
+ * and the posterior of arc a at frame t, exp(alpha_t[u] + w_a + e[t][label_a] + beta_{t+1}[v] - Z), is added into the
+ * emission gradient (row t, column label_a) and into the arc's weight gradient (summed over frames and utterances).
+ *
+ * Layout: one CTA per utterance.  The two score rows of the sweep ([2][S] floats), the emission row of the frame
+ * ([2][C], double-buffered so that the next row loads during the sweep) and, in the backward kernel, the per-CTA
+ * accumulators of the arc gradient ([A] floats) and of the frame's emission gradient ([2][C]) live in shared memory.
+ * G's tables (CSR by destination for the forward, by source for the backward) are read through the read-only path
+ * from L2, where one copy serves every CTA: at the envelope (S = 4096, A = 32768) they are 400 KB, too large to sit
+ * in shared memory beside the rows, and the frames read them in the same order, so the L1 keeps the hot part.  A node
+ * is handled by `lanes` threads (a power of two, chosen from G's mean degree) that stride over its arcs with an online
+ * logsumexp and merge with shuffles; the loop over nodes has the same trip count in every warp.  Each thread owns the
+ * same arcs at every frame, so the arc accumulators take plain adds and go to global memory once per CTA.
+ *
+ * Scores are kept relative to per-frame offsets accumulated in double (DESIGN.md, "ASG on padded batches"): row t is
+ * stored as alpha_t - c_t with c_t = c_{t-1} + max(row_{t-1}) (the maximum of every warp is left in shared memory and
+ * merged after the frame's barrier), and likewise beta_t - d_t.  A posterior's exponent is row + row' + (float)(c_t +
+ * d_{t+1} - Z), so fp32 scores that grow with t never cancel.  exp / log on the SFU (ex2.approx / lg2.approx).
+ *
+ * Valid only for finite weights: the forward kernel raises status bit 1 on any non-finite weight or used emission,
+ * and the caller repeats the call on the materialised route.
+ */
+#include <algorithm>
+
+#include "gtnb_ptx.h"
+
+namespace gtnb {
+
+constexpr int kSparseThreads = 512;
+constexpr int kSparseWarps = kSparseThreads / 32;
+
+/* floats of dynamic shared memory of the two sweeps */
+inline int sparse_fwd_smem_floats(int S, int C) {
+  return 2 * S + 2 * C + 2 * kSparseWarps;
+}
+inline int sparse_bwd_smem_floats(int S, int A, int C) {
+  return 2 * S + 4 * C + A + 2 * kSparseWarps;
+}
+
+namespace {
+
+/* the per-lane (m, s) of an online logsumexp: s = sum of exp(x - m) over the terms seen; -inf and NaN terms skipped */
+__device__ __forceinline__ void lse_add(float& m, float& s, float x) {
+  if (x > m) {
+    s = s * exp_fast(m - x) + 1.0f;
+    m = x;
+  } else if (x > neg_inf()) {
+    s += exp_fast(x - m);
+  }
+}
+
+/* (m, s) merged over the `lanes` consecutive lanes of a node; every lane of the group gets the result */
+__device__ __forceinline__ void lse_merge(float& m, float& s, int lanes) {
+  for (int o = 1; o < lanes; o <<= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    const float os = __shfl_xor_sync(0xffffffffu, s, o);
+    const float M = fmaxf(m, om);
+    const float Mm = M == neg_inf() ? 0.0f : M; // all -inf: s stays 0
+    s = s * exp_fast(m - Mm) + os * exp_fast(om - Mm);
+    m = M;
+  }
+}
+
+/* the maximum of the previous frame's row from the per-warp maxima; 0 when the row is all -inf */
+__device__ __forceinline__ float row_offset(const float* red) {
+  float M = neg_inf();
+#pragma unroll
+  for (int i = 0; i < kSparseWarps; i++) M = fmaxf(M, red[i]);
+  return M == neg_inf() ? 0.0f : M;
+}
+
+/*
+ * alpha rows of utterance b to alpha[b][(T+1)*S] (relative to the offsets), the offsets c_t to offs[b][t] for t >= 1
+ * and Z to offs[b][0] (double) and den[b] (float); status[b] |= 1 on a non-finite weight or used emission.
+ */
+__global__ void __launch_bounds__(kSparseThreads) sparse_den_forward_kernel(
+    SparseDev g, int T, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    const float* __restrict__ w, float* __restrict__ alpha, double* __restrict__ offs, float* __restrict__ den,
+    int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int S = g.S, lanes = g.lanes;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  float* red = E + 2 * C; // [2][kSparseWarps]
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  float* al = alpha + (long long)b * (T + 1) * S;
+  double* of = offs + (long long)b * (T + 1);
+  bool bad = false;
+  float mx = neg_inf();
+  for (int v = tid; v < S; v += nt) {
+    const float a0 = (__ldg(g.flags + v) & 1) ? 0.0f : neg_inf();
+    rows[v] = a0;
+    al[v] = a0;
+    mx = fmaxf(mx, a0);
+  }
+  mx = warp_max(mx);
+  if (tid % 32 == 0) red[tid / 32] = mx;
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  __syncthreads();
+  double c_off = 0.0;
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    const float Mp = row_offset(red + ((t - 1) & 1) * kSparseWarps);
+    mx = neg_inf();
+    for (int v0 = 0; v0 < S; v0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int v = v0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (v < S) {
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int k = __ldg(g.in_ptr + v) + q; k < k1; k += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + k));
+          const float ek = Er[__ldg(g.in_lab + k)];
+          bad |= !(is_finite(wk) && is_finite(ek));
+          lse_add(m, s, P[__ldg(g.in_src + k)] + (wk + ek));
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (v < S) {
+        const float val = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mp;
+        if (q == 0) {
+          Q[v] = val;
+          al[(long long)t * S + v] = val;
+        }
+        mx = fmaxf(mx, val);
+      }
+    }
+    mx = warp_max(mx);
+    if (tid % 32 == 0) red[(t & 1) * kSparseWarps + tid / 32] = mx;
+    c_off += (double)Mp;
+    if (tid == 0) of[t] = c_off;
+    __syncthreads();
+  }
+  bad = __syncthreads_or(bad);
+  if (tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    for (int v = tid; v < S; v += 32)
+      if (__ldg(g.flags + v) & 2) m = fmaxf(m, F[v]);
+    m = warp_max(m);
+    float s = 0.0f;
+    if (m != neg_inf())
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) s += expf(F[v] - m);
+    s = warp_sum(s);
+    if (tid == 0) {
+      const double Z = m == neg_inf() ? (double)neg_inf() : c_off + (double)(m + logf(s));
+      of[0] = Z;
+      den[b] = (float)Z;
+      if (bad) atomicOr(&status[b], 1);
+    }
+  }
+}
+
+/*
+ * d Z / d e added into grad (rows t < T_b; one red.add per label and frame per CTA) and d Z / d w added into
+ * wgrad[G's arc id] (one per arc per CTA).  Nothing when Z is not finite (no accepting path: the reference's gradient
+ * of a -inf score is 0 on the paths that do not exist) or T_b = 0.
+ */
+__global__ void __launch_bounds__(kSparseThreads) sparse_den_backward_kernel(
+    SparseDev g, int T, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    const float* __restrict__ w, const float* __restrict__ alpha, const double* __restrict__ offs,
+    float* __restrict__ grad, long long grad_stride, float* __restrict__ wgrad) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int S = g.S, A = g.A, lanes = g.lanes;
+  float* rows = sm; // [2][S] beta rows
+  float* E = sm + 2 * S; // [2][C] emission rows
+  float* Eg = E + 2 * C; // [2][C] the frame's emission gradient
+  float* acc = Eg + 2 * C; // [A] arc gradient, by out-table position
+  float* red = acc + A; // [2][kSparseWarps]
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const double* of = offs + (long long)b * (T + 1);
+  const double Z = of[0];
+  if (Tb < 1 || !(fabs(Z) < (double)CUDART_INF_F)) return;
+  const float* em = emis + (long long)b * stride;
+  const float* al = alpha + (long long)b * (T + 1) * S;
+  float* gr = grad + (long long)b * grad_stride;
+  float mx = neg_inf();
+  for (int v = tid; v < S; v += nt) {
+    const float b0 = (__ldg(g.flags + v) & 2) ? 0.0f : neg_inf();
+    rows[(Tb & 1) * S + v] = b0;
+    mx = fmaxf(mx, b0);
+  }
+  mx = warp_max(mx);
+  if (tid % 32 == 0) red[(Tb & 1) * kSparseWarps + tid / 32] = mx;
+  for (int k = tid; k < A; k += nt) acc[k] = 0.0f;
+  for (int c = tid; c < 2 * C; c += nt) Eg[c] = 0.0f;
+  for (int c = tid; c < C; c += nt) E[((Tb - 1) & 1) * C + c] = __ldg(em + (long long)(Tb - 1) * C + c);
+  __syncthreads();
+  double d = 0.0; // d_{t+1}
+  for (int t = Tb - 1; t >= 0; t--) {
+    const float* Nx = rows + ((t + 1) & 1) * S;
+    float* Cur = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    float* Eg_t = Eg + (t & 1) * C;
+    float* Eg_prev = Eg + ((t + 1) & 1) * C; // frame t + 1's, complete since the barrier
+    for (int c = tid; c < C; c += nt) {
+      if (t > 0) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)(t - 1) * C + c);
+      if (t + 1 < Tb) {
+        const float v = Eg_prev[c];
+        if (v != 0.0f) atomicAdd(gr + (long long)(t + 1) * C + c, v);
+        Eg_prev[c] = 0.0f;
+      }
+    }
+    const float Mb = row_offset(red + ((t + 1) & 1) * kSparseWarps);
+    const double c_t = t > 0 ? of[t] : 0.0;
+    const float fo = (float)(c_t + d - Z);
+    mx = neg_inf();
+    for (int u0 = 0; u0 < S; u0 += groups) {
+      const int u = u0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (u < S) {
+        const float au = al[(long long)t * S + u] + fo; // alpha_t[u] + c_t + d_{t+1} - Z, in the exponent's terms
+        const int k1 = __ldg(g.out_ptr + u + 1);
+        for (int k = __ldg(g.out_ptr + u) + q; k < k1; k += lanes) {
+          const int lab = __ldg(g.out_lab + k);
+          const float x = Nx[__ldg(g.out_dst + k)] + (__ldg(w + __ldg(g.out_arc + k)) + Er[lab]);
+          lse_add(m, s, x);
+          const float p = exp_fast(au + x);
+          if (p != 0.0f) {
+            acc[k] += p;
+            atomicAdd(Eg_t + lab, p);
+          }
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (u < S) {
+        const float val = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mb;
+        if (q == 0) Cur[u] = val;
+        mx = fmaxf(mx, val);
+      }
+    }
+    mx = warp_max(mx);
+    if (tid % 32 == 0) red[(t & 1) * kSparseWarps + tid / 32] = mx;
+    d += (double)Mb;
+    __syncthreads();
+  }
+  for (int c = tid; c < C; c += nt) { // frame 0's emission gradient
+    const float v = Eg[c];
+    if (v != 0.0f) atomicAdd(gr + c, v);
+  }
+  for (int k = tid; k < A; k += nt)
+    if (acc[k] != 0.0f) atomicAdd(wgrad + __ldg(g.out_arc + k), acc[k]);
+}
+
+/* sigma_k = logsumexp of the weights of start group k (gtnb_product.h), one warp per group */
+__global__ void __launch_bounds__(256) sparse_sigma_kernel(int K, const int32_t* __restrict__ grp_ptr,
+                                                           const int32_t* __restrict__ grp_arc,
+                                                           const float* __restrict__ w, float* __restrict__ sigma) {
+  const int k = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (k >= K) return; // whole warps
+  const int a0 = __ldg(grp_ptr + k), a1 = __ldg(grp_ptr + k + 1);
+  float m = neg_inf();
+  for (int j = a0 + lane; j < a1; j += 32) m = fmaxf(m, __ldg(w + __ldg(grp_arc + j)));
+  m = warp_max(m);
+  float s = 0.0f;
+  if (m != neg_inf())
+    for (int j = a0 + lane; j < a1; j += 32) s += expf(__ldg(w + __ldg(grp_arc + j)) - m);
+  s = warp_sum(s);
+  if (lane == 0) sigma[k] = m == neg_inf() ? m : m + logf(s);
+}
+
+/* wgrad[a] += wgrad[nG + k] * exp(w_a - sigma_k) for every arc a of start group k: the folded start arcs' gradient
+ * through sigma (every arc is in one group at most: no race), one thread per group */
+__global__ void __launch_bounds__(256) sparse_fold_kernel(int K, const int32_t* __restrict__ grp_ptr,
+                                                          const int32_t* __restrict__ grp_arc, int nG,
+                                                          const float* __restrict__ w,
+                                                          const float* __restrict__ sigma, float* __restrict__ wgrad) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const float gk = wgrad[nG + k];
+  if (gk == 0.0f) return;
+  const float sk = sigma[k];
+  for (int j = __ldg(grp_ptr + k); j < __ldg(grp_ptr + k + 1); j++) {
+    const int a = __ldg(grp_arc + j);
+    wgrad[a] += gk * expf(__ldg(w + a) - sk);
+  }
+}
+
+} // namespace
+
+#ifndef GTNB_HOST_EMU
+
+bool sparse_den_supported(int S, int A, int C) {
+  return S >= 1 && S <= kSparseMaxStates && A <= kSparseMaxArcs && C >= 1 && C <= kSparseMaxLabels;
+}
+
+int launch_sparse_den_forward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
+                              const float* emis, long long stride, const float* w, float* alpha, double* offs,
+                              float* den, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_den_forward_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_fwd_smem_floats(g.S, C);
+  GTNB_LAUNCH(ctx, "sparse_den_forward", sparse_den_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      g, T, C, lens, emis, stride, w, alpha, offs, den, status));
+  return GTNB_OK;
+}
+
+int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
+                               const float* emis, long long stride, const float* w, const float* alpha,
+                               const double* offs, float* grad, long long grad_stride, float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_den_backward_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_bwd_smem_floats(g.S, g.A, C);
+  GTNB_LAUNCH(ctx, "sparse_den_backward", sparse_den_backward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      g, T, C, lens, emis, stride, w, alpha, offs, grad, grad_stride, wgrad));
+  return GTNB_OK;
+}
+
+int launch_sparse_sigma(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
+                        float* sigma) {
+  if (K == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "sparse_sigma", sparse_sigma_kernel<<<(unsigned)(((long long)K * 32 + 255) / 256), 256, 0,
+                                                         ctx->stream>>>(K, grp_ptr, grp_arc, w, sigma));
+  return GTNB_OK;
+}
+
+int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, int nG, const float* w,
+                       const float* sigma, float* wgrad) {
+  if (K == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "sparse_fold", sparse_fold_kernel<<<(unsigned)((K + 255) / 256), 256, 0, ctx->stream>>>(
+      K, grp_ptr, grp_arc, nG, w, sigma, wgrad));
+  return GTNB_OK;
+}
+
+#endif // GTNB_HOST_EMU
+
+} // namespace gtnb

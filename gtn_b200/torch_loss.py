@@ -423,6 +423,66 @@ def graph_transitions_loss(emissions, transitions, graphs, kind="asg", input_len
                                               allreduce)
 
 
+class SparseTransitionsLossFunction(GraphTransitionsLossFunction):
+    """graph_loss's user target graphs with a learned transition graph G of any shape (an n-gram graph of any order,
+    a pruned token LM, an HMM topology), through gtnb_sparse_transitions_loss:
+        loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b))
+    transitions_graph: G, a gtn_b200.gtn.Graph acceptor without epsilon arcs, whose own weights are ignored;
+    transitions: float32 CUDA tensor of G.num_arcs() weights in G's arc numbering, on the emissions' device.  The
+    graphs, weights, input_lengths, reduction and allreduce are graph_transitions_loss's; so is the backward.
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, transitions, weights, graphs, transitions_graph, input_lengths=None, reduction="mean",
+                allreduce=True):
+        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        e = emissions.contiguous()
+        B, T, Cn = e.shape
+        assert len(graphs) == B
+        gv = _graph_view(transitions_graph)
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == gv[0].num_arcs
+        tw = transitions.detach().contiguous()
+        views = [_graph_view(g) for g in graphs]
+        counts = [v.num_arcs for v, _ in views]
+        n_arcs = sum(counts)
+        arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
+        w = ag = None
+        if weights is not None:
+            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
+            assert weights.numel() == n_arcs
+            w = weights.detach().contiguous()
+            ag = torch.empty(max(n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
+        stream = torch.cuda.current_stream(e.device).cuda_stream
+        g = _ctx_for(e.device, stream)
+        il = _lengths(input_lengths, B)
+        losses = np.zeros(B, np.float32)
+        grad = torch.empty_like(e)  # every row is written by the call
+        tg = torch.empty(max(transitions.numel(), 1), dtype=torch.float32, device=e.device)
+        g._check(capi.lib().gtnb_sparse_transitions_loss(
+            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
+            None if w is None else w.data_ptr(), 1, C.byref(gv[0]), tw.data_ptr(), 1,
+            losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if ag is None else ag.data_ptr(), 1,
+            tg.data_ptr(), 1))
+        tg = tg[:transitions.numel()].view_as(transitions)
+        _allreduce_transitions(ctx, tg, allreduce)
+        out = torch.from_numpy(losses).to(e.device)
+        if ag is not None:
+            ag = ag[:n_arcs].view_as(weights)
+            ctx.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(e.device)
+        ctx.save_for_backward(grad, tg)
+        ctx.ag = ag  # (computed here, neither an input nor an output: held on ctx)
+        ctx.reduction = reduction
+        ctx.B = B
+        return out.mean() if reduction == "mean" else out
+
+
+def sparse_transitions_loss(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
+                            reduction="mean", allreduce=True):
+    return SparseTransitionsLossFunction.apply(emissions, transitions, weights, graphs, transitions_graph,
+                                               input_lengths, reduction, allreduce)
+
+
 @torch.no_grad()
 def graph_viterbi(emissions, graphs, input_lengths=None, weights=None):
     """Best path of compose(A_b, E_b) for every utterance, A_b = graphs[b] (viterbiPath / viterbiScore of the lattice

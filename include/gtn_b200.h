@@ -571,6 +571,47 @@ int gtnb_graph_transitions_loss(
     int trans_grad_on_device);
 
 /*
+ * Loss over one user-supplied target graph per utterance with a learned transition graph G of any shape (n-gram
+ * graphs of any order, pruned or sparse token LMs, HMM topologies):
+ *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b)).
+ * transitions: G's structure, an epsilon-free acceptor (ilabel == olabel on every arc) with any start and accept
+ * sets, cycles and node count; its own weights are ignored.  trans_w: [G.num_arcs] weights in G's arc numbering.
+ * E_b, graphs, arc_weights, the outputs and their *_on_device flags are those of gtnb_graph_transitions_loss;
+ * trans_grad is [G.num_arcs], the batch sum, written, not accumulated.  An arc of A_b or G labelled outside [0, C)
+ * never matches (gradient 0).  T_b = 0 gives NaN; no accepting path of T_b arcs through A_b and G gives +inf and the
+ * denominator's gradient alone; a G that accepts nothing in T_b frames gives NaN.  B = 0 zeroes trans_grad.
+ * Epsilon arcs in A_b or G, or a G that is a transducer, are GTNB_ERR_UNSUPPORTED (remove(g, epsilon), projectInput
+ * / projectOutput first); malformed views, a G without nodes, bad lengths or a NULL trans_w with B > 0 are
+ * GTNB_ERR_INVALID_ARGUMENT.
+ * Device route (the transitions never visit the host): the denominator is swept over G's tables without building
+ * the lattice (k_sparse.cu) when G fits the kernels' envelope -- at most 4096 nodes, 32768 arcs labelled in [0, C),
+ * C <= 1024 -- and the numerators are the products of gtnb_product.h, built on the host from structure only, with
+ * G's start copies folded into one start node, weighted on the device and swept by the implicit kernels.  A G or a
+ * product outside that layout, a non-finite value, or the "implicit" flag off take the materialised lattices.
+ */
+int gtnb_sparse_transitions_loss(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    const gtnb_graph_view* transitions,
+    const float* trans_w,
+    int trans_on_device,
+    float* losses_host,
+    float* grads, /* nullable */
+    int grads_on_device,
+    float* arc_grads, /* nullable */
+    int arc_grads_on_device,
+    float* trans_grad, /* nullable */
+    int trans_grad_on_device);
+
+/*
  * Batched Viterbi alignment over one user-supplied target graph per utterance: viterbiPath and viterbiScore of
  * compose(A_b, E_b), the best path through the user's own graph (a forced alignment with any topology; CTC graphs
  * give CTC forced alignment).  E_b, graphs, arc_weights, the olabel matching, labels outside [0, C) and the epsilon
