@@ -348,6 +348,14 @@ class Ctx:
     def viterbi_dense_ex(self, emissions, trans_w, kind=DENSE_ASG, input_lens=None):
         """Host-buffer entry of gtnb_viterbi_dense_ex: emissions [B,T,C], trans_w [C + C*C] (DENSE_ASG) or [C*C]
         (DENSE_BIGRAM) -> (paths [B,T] int32, -1 beyond T_b; scores [B])."""
+        return self._viterbi_dense_ex(False, emissions, trans_w, kind, input_lens)
+
+    def viterbi_dense_ex_dev(self, emissions, trans_w, kind=DENSE_ASG, input_lens=None):
+        """Device-buffer entry: emissions and trans_w uploaded once, gtnb_viterbi_dense_ex on device pointers
+        (paths and scores in HBM), downloaded afterwards -> (paths, scores)."""
+        return self._viterbi_dense_ex(True, emissions, trans_w, kind, input_lens)
+
+    def _viterbi_dense_ex(self, dev, emissions, trans_w, kind, input_lens):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
@@ -355,69 +363,46 @@ class Ctx:
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         paths = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
         scores = np.full(max(B, 1), np.nan, np.float32)
-        self._check(lib().gtnb_viterbi_dense_ex(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), int(kind), tw.ctypes.data, 0, paths.ctypes.data,
-            scores.ctypes.data, 0))
-        return paths[:B, :T], scores[:B]
-
-    def viterbi_dense_ex_dev(self, emissions, trans_w, kind=DENSE_ASG, input_lens=None):
-        """Device-buffer entry: emissions and trans_w uploaded once, gtnb_viterbi_dense_ex on device pointers
-        (paths and scores in HBM), downloaded afterwards -> (paths, scores)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
-        assert tw.size == (Cn * Cn if kind == DENSE_BIGRAM else Cn + Cn * Cn)
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        e_dev, w_dev = self.to_device(e), self.to_device(tw)
-        p_dev = self.to_device(np.full((max(B, 1), max(T, 1)), -7, np.int32))  # every entry is written
-        s_dev = self.to_device(np.full(max(B, 1), np.nan, np.float32))
-        try:
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_viterbi_dense_ex(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), int(kind), w_dev.ptr, 1, p_dev.ptr, s_dev.ptr, 1))
-            paths = p_dev.download((max(B, 1), max(T, 1)), np.int32)
-            scores = s_dev.download((max(B, 1),))
-        finally:
-            for buf in (e_dev, w_dev, p_dev, s_dev):
-                buf.free()
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), int(kind), p.inp(tw), p.flag, p.out(paths),
+                p.out(scores), p.flag))
         return paths.ravel()[:B * T].reshape(B, T), scores[:B]
 
     def ctc_loss(self, emissions, targets, blank=0, want_grad=True, input_lens=None):
         """Host-buffer entry point: emissions [B,T,C] float32 numpy -> (losses, grads)."""
+        return self._ctc_loss(False, emissions, targets, blank, want_grad, input_lens)
+
+    def ctc_loss_dev(self, emissions, targets, blank=0, input_lens=None):
+        """Device-buffer entry point: uploads once, runs gtnb_ctc_loss on device pointers (emissions
+        in HBM in, gradients in HBM out), downloads the gradients afterwards -> (losses, grads)."""
+        return self._ctc_loss(True, emissions, targets, blank, True, input_lens)
+
+    def _ctc_loss(self, dev, emissions, targets, blank, want_grad, input_lens):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         cat, lens = _cat_targets(targets)
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         losses = np.zeros(B, np.float32)
         grads = np.zeros_like(e) if want_grad else None
-        self._check(lib().gtnb_ctc_loss(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), _p(cat, _i32p), _p(lens, _i32p),
-            blank, _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0))
-        return losses, grads
-
-    def ctc_loss_dev(self, emissions, targets, blank=0, input_lens=None):
-        """Device-buffer entry point: uploads once, runs gtnb_ctc_loss on device pointers (emissions
-        in HBM in, gradients in HBM out), downloads the gradients afterwards -> (losses, grads)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        cat, lens = _cat_targets(targets)
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        losses = np.zeros(B, np.float32)
-        e_dev = self.to_device(e)
-        g_dev = self.alloc(e.nbytes)
-        try:
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_ctc_loss(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), _p(cat, _i32p), _p(lens, _i32p),
-                blank, _p(losses, _f32p), g_dev.ptr, 1))
-            grads = g_dev.download(e.shape)
-        finally:
-            e_dev.free()
-            g_dev.free()
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), _p(cat, _i32p), _p(lens, _i32p),
+                blank, _p(losses, _f32p), p.out(grads), p.flag))
         return losses, grads
 
 
     def ngram_ctc_loss(self, emissions, trans_w, targets, blank=0, want_grad=True, input_lens=None):
         """Host-buffer entry of gtnb_ngram_ctc_loss: emissions [B,T,C], trans_w [C*C] (row = destination label)
         -> (losses [B], grads [B,T,C] or None, trans_grad [C*C] or None)."""
+        return self._ngram_ctc_loss(False, emissions, trans_w, targets, blank, want_grad, input_lens)
+
+    def ngram_ctc_loss_dev(self, emissions, trans_w, targets, blank=0, input_lens=None):
+        """Device-buffer entry: emissions and W uploaded once, gtnb_ngram_ctc_loss on device pointers (gradients
+        in HBM), downloaded afterwards -> (losses, grads, trans_grad)."""
+        return self._ngram_ctc_loss(True, emissions, trans_w, targets, blank, True, input_lens)
+
+    def _ngram_ctc_loss(self, dev, emissions, trans_w, targets, blank, want_grad, input_lens):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
@@ -427,39 +412,24 @@ class Ctx:
         losses = np.zeros(B, np.float32)
         grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
         tg = np.zeros(Cn * Cn, np.float32) if want_grad else None
-        self._check(lib().gtnb_ngram_ctc_loss(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), tw.ctypes.data, 0, _p(cat, _i32p), _p(lens, _i32p),
-            int(blank), _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0,
-            None if tg is None else tg.ctypes.data, 0))
-        return losses, grads, tg
-
-    def ngram_ctc_loss_dev(self, emissions, trans_w, targets, blank=0, input_lens=None):
-        """Device-buffer entry: emissions and W uploaded once, gtnb_ngram_ctc_loss on device pointers (gradients
-        in HBM), downloaded afterwards -> (losses, grads, trans_grad)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
-        assert tw.size == Cn * Cn
-        cat, lens = _cat_targets(targets)
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        losses = np.zeros(B, np.float32)
-        e_dev, w_dev = self.to_device(e), self.to_device(tw)
-        g_dev, tg_dev = self.alloc(max(e.nbytes, 16)), self.alloc(tw.nbytes)
-        try:
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_ngram_ctc_loss(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), w_dev.ptr, 1, _p(cat, _i32p), _p(lens, _i32p),
-                int(blank), _p(losses, _f32p), g_dev.ptr, 1, tg_dev.ptr, 1))
-            grads = g_dev.download(e.shape)
-            tg = tg_dev.download(tw.shape)
-        finally:
-            for buf in (e_dev, w_dev, g_dev, tg_dev):
-                buf.free()
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), p.inp(tw), p.flag, _p(cat, _i32p),
+                _p(lens, _i32p), int(blank), _p(losses, _f32p), p.out(grads), p.flag, p.out(tg), p.flag))
         return losses, grads, tg
 
     def asg_loss_ex(self, emissions, trans_w, targets, want_grad=True, input_lens=None):
         """Host-buffer entry of gtnb_asg_loss_ex: emissions [B,T,C], trans_w [C + C*C] (start weights, then the
         C x C matrix, row = destination label), input_lens [B] or None
         -> (losses [B], grads [B,T,C] or None, trans_grad [C + C*C] or None)."""
+        return self._asg_loss_ex(False, emissions, trans_w, targets, want_grad, input_lens)
+
+    def asg_loss_ex_dev(self, emissions, trans_w, targets, input_lens=None):
+        """Device-buffer entry: emissions and trans_w uploaded once, gtnb_asg_loss_ex on device pointers (gradients
+        in HBM), downloaded afterwards -> (losses, grads, trans_grad)."""
+        return self._asg_loss_ex(True, emissions, trans_w, targets, True, input_lens)
+
+    def _asg_loss_ex(self, dev, emissions, trans_w, targets, want_grad, input_lens):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
@@ -469,191 +439,87 @@ class Ctx:
         losses = np.zeros(B, np.float32)
         grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
         tg = np.zeros(Cn + Cn * Cn, np.float32) if want_grad else None
-        self._check(lib().gtnb_asg_loss_ex(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), tw.ctypes.data, 0, _p(cat, _i32p), _p(lens, _i32p),
-            _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0, None if tg is None else tg.ctypes.data,
-            0))
-        return losses, grads, tg
-
-    def asg_loss_ex_dev(self, emissions, trans_w, targets, input_lens=None):
-        """Device-buffer entry: emissions and trans_w uploaded once, gtnb_asg_loss_ex on device pointers (gradients
-        in HBM), downloaded afterwards -> (losses, grads, trans_grad)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
-        assert tw.size == Cn + Cn * Cn
-        cat, lens = _cat_targets(targets)
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        losses = np.zeros(B, np.float32)
-        e_dev, w_dev = self.to_device(e), self.to_device(tw)
-        g_dev, tg_dev = self.alloc(max(e.nbytes, 16)), self.alloc(tw.nbytes)
-        try:
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_asg_loss_ex(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), w_dev.ptr, 1, _p(cat, _i32p), _p(lens, _i32p),
-                _p(losses, _f32p), g_dev.ptr, 1, tg_dev.ptr, 1))
-            grads = g_dev.download(e.shape)
-            tg = tg_dev.download(tw.shape)
-        finally:
-            for buf in (e_dev, w_dev, g_dev, tg_dev):
-                buf.free()
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), p.inp(tw), p.flag, _p(cat, _i32p),
+                _p(lens, _i32p), _p(losses, _f32p), p.out(grads), p.flag, p.out(tg), p.flag))
         return losses, grads, tg
 
     def graph_loss(self, emissions, views, want_grad=True, input_lens=None, arc_weights=None):
         """Host-buffer entry of gtnb_graph_loss: emissions [B,T,C], views: B (view, keepalive) pairs from make_view,
         arc_weights [sum A_b] or None -> (losses [B], grads [B,T,C] or None, arc_grads [sum A_b] or None)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
-        assert aw is None or aw.size == n_arcs
-        losses = np.zeros(B, np.float32)
-        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
-        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
-        self._check(lib().gtnb_graph_loss(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0,
-            _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0, None if ag is None else ag.ctypes.data,
-            0))
-        return losses, grads, None if ag is None else ag[:n_arcs]
+        return self._graph_loss(False, emissions, views, want_grad, input_lens, arc_weights)
 
     def graph_loss_dev(self, emissions, views, input_lens=None, arc_weights=None):
         """Device-buffer entry: emissions (and arc_weights, when given) uploaded once, gtnb_graph_loss on device
         pointers (gradients in HBM), downloaded afterwards -> (losses, grads, arc_grads)."""
+        return self._graph_loss(True, emissions, views, True, input_lens, arc_weights)
+
+    def _graph_loss(self, dev, emissions, views, want_grad, input_lens, arc_weights):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
+        arr, n_arcs, aw = _graph_batch(views, B, arc_weights)
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         losses = np.zeros(B, np.float32)
-        bufs = [self.to_device(e), self.alloc(max(e.nbytes, 16)), self.alloc(4 * max(n_arcs, 4))]
-        e_dev, g_dev, ag_dev = bufs
-        w_dev = None
-        if arc_weights is not None:
-            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
-            assert aw.size == n_arcs
-            w_dev = self.to_device(aw)
-            bufs.append(w_dev)
-        try:
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_graph_loss(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if w_dev is None else w_dev.ptr, 1,
-                _p(losses, _f32p), g_dev.ptr, 1, ag_dev.ptr, 1))
-            grads = g_dev.download(e.shape)
-            ag = ag_dev.download((max(n_arcs, 1),))[:n_arcs]
-        finally:
-            for buf in bufs:
-                buf.free()
-        return losses, grads, ag
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, _p(losses, _f32p),
+                p.out(grads), p.flag, p.out(ag), p.flag))
+        return losses, grads, None if ag is None else ag[:n_arcs]
 
     def graph_viterbi(self, emissions, views, input_lens=None, arc_weights=None):
         """Host-buffer entry of gtnb_graph_viterbi: emissions [B,T,C], views: B (view, keepalive) pairs from make_view,
         arc_weights [sum A_b] or None -> (paths [B,T] int32, scores [B], arcs [B,T] int32)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
-        assert aw is None or aw.size == n_arcs
-        paths = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
-        arcs = np.full((max(B, 1), max(T, 1)), -7, np.int32)
-        scores = np.full(max(B, 1), np.nan, np.float32)
-        self._check(lib().gtnb_graph_viterbi(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0,
-            paths.ctypes.data, arcs.ctypes.data, scores.ctypes.data, 0))
-        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
+        return self._graph_viterbi(False, emissions, views, input_lens, arc_weights)
 
     def graph_viterbi_dev(self, emissions, views, input_lens=None, arc_weights=None):
         """Device-buffer entry: emissions (and arc_weights, when given) uploaded once, gtnb_graph_viterbi on device
         pointers (outputs in HBM), downloaded afterwards -> (paths, scores, arcs)."""
+        return self._graph_viterbi(True, emissions, views, input_lens, arc_weights)
+
+    def _graph_viterbi(self, dev, emissions, views, input_lens, arc_weights):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
+        arr, _, aw = _graph_batch(views, B, arc_weights)
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        fill = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
-        bufs = [self.to_device(e), self.to_device(fill), self.to_device(fill),
-                self.to_device(np.full(max(B, 1), np.nan, np.float32))]
-        e_dev, p_dev, a_dev, s_dev = bufs
-        w_dev = None
-        if arc_weights is not None:
-            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
-            assert aw.size == n_arcs
-            w_dev = self.to_device(aw)
-            bufs.append(w_dev)
-        try:
+        out = _viterbi_outputs(B, T)
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_graph_viterbi(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if w_dev is None else w_dev.ptr, 1,
-                p_dev.ptr, a_dev.ptr, s_dev.ptr, 1))
-            paths = p_dev.download(fill.shape, np.int32)
-            arcs = a_dev.download(fill.shape, np.int32)
-            scores = s_dev.download((max(B, 1),))
-        finally:
-            for buf in bufs:
-                buf.free()
-        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, *map(p.out, out),
+                p.flag))
+        return _viterbi_results(out, B, T)
 
     def graph_transitions_loss(self, emissions, views, trans_w, kind=DENSE_ASG, want_grad=True, input_lens=None,
                                arc_weights=None):
         """Host-buffer entry of gtnb_graph_transitions_loss: emissions [B,T,C], views: B (view, keepalive) pairs from
         make_view, trans_w [C + C*C] (DENSE_ASG) or [C*C] (DENSE_BIGRAM), arc_weights [sum A_b] or None
         -> (losses [B], grads [B,T,C] or None, arc_grads [sum A_b] or None, trans_grad or None)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
-        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
-        assert aw is None or aw.size == n_arcs
-        losses = np.zeros(B, np.float32)
-        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
-        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
-        tg = np.full(tw.size, np.nan, np.float32) if want_grad else None
-        self._check(lib().gtnb_graph_transitions_loss(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0, kind,
-            tw.ctypes.data, 0, _p(losses, _f32p), None if grads is None else grads.ctypes.data, 0,
-            None if ag is None else ag.ctypes.data, 0, None if tg is None else tg.ctypes.data, 0))
-        return losses, grads, None if ag is None else ag[:n_arcs], tg
+        return self._graph_transitions_loss(False, emissions, views, trans_w, kind, want_grad, input_lens, arc_weights)
 
     def graph_transitions_loss_dev(self, emissions, views, trans_w, kind=DENSE_ASG, input_lens=None,
                                    arc_weights=None):
         """Device-buffer entry: emissions, trans_w (and arc_weights, when given) uploaded once,
         gtnb_graph_transitions_loss on device pointers (gradients in HBM), downloaded afterwards
         -> (losses, grads, arc_grads, trans_grad)."""
+        return self._graph_transitions_loss(True, emissions, views, trans_w, kind, True, input_lens, arc_weights)
+
+    def _graph_transitions_loss(self, dev, emissions, views, trans_w, kind, want_grad, input_lens, arc_weights):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
+        arr, n_arcs, aw = _graph_batch(views, B, arc_weights)
         tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         losses = np.zeros(B, np.float32)
-        bufs = [self.to_device(e), self.alloc(max(e.nbytes, 16)), self.alloc(4 * max(n_arcs, 4)), self.to_device(tw),
-                self.alloc(tw.nbytes)]
-        e_dev, g_dev, ag_dev, w_dev, tg_dev = bufs
-        aw_dev = None
-        if arc_weights is not None:
-            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
-            assert aw.size == n_arcs
-            aw_dev = self.to_device(aw)
-            bufs.append(aw_dev)
-        try:
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
+        tg = np.full(tw.size, np.nan, np.float32) if want_grad else None
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_graph_transitions_loss(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if aw_dev is None else aw_dev.ptr, 1, kind,
-                w_dev.ptr, 1, _p(losses, _f32p), g_dev.ptr, 1, ag_dev.ptr, 1, tg_dev.ptr, 1))
-            grads = g_dev.download(e.shape)
-            ag = ag_dev.download((max(n_arcs, 1),))[:n_arcs]
-            tg = tg_dev.download(tw.shape)
-        finally:
-            for buf in bufs:
-                buf.free()
-        return losses, grads, ag, tg
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, kind, p.inp(tw), p.flag,
+                _p(losses, _f32p), p.out(grads), p.flag, p.out(ag), p.flag, p.out(tg), p.flag))
+        return losses, grads, None if ag is None else ag[:n_arcs], tg
 
     def sparse_transitions_loss(self, emissions, views, transitions, trans_w, want_grad=True, input_lens=None,
                                 arc_weights=None):
@@ -661,121 +527,64 @@ class Ctx:
         make_view, transitions: G's (view, keepalive) pair (an acceptor; its weights are ignored), trans_w
         [G.num_arcs], arc_weights [sum A_b] or None
         -> (losses [B], grads [B,T,C] or None, arc_grads [sum A_b] or None, trans_grad [G.num_arcs] or None)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
-        gv = transitions[0]
-        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
-        assert tw.size == gv.num_arcs
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
-        assert aw is None or aw.size == n_arcs
-        losses = np.zeros(B, np.float32)
-        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
-        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
-        tg = np.full(max(tw.size, 1), np.nan, np.float32) if want_grad else None
-        self._check(lib().gtnb_sparse_transitions_loss(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0,
-            C.byref(gv), tw.ctypes.data if tw.size else None, 0, _p(losses, _f32p),
-            None if grads is None else grads.ctypes.data, 0, None if ag is None else ag.ctypes.data, 0,
-            None if tg is None else tg.ctypes.data, 0))
-        return (losses, grads, None if ag is None else ag[:n_arcs], None if tg is None else tg[:tw.size])
+        return self._sparse_transitions_loss(False, emissions, views, transitions, trans_w, want_grad, input_lens,
+                                             arc_weights)
 
     def sparse_transitions_loss_dev(self, emissions, views, transitions, trans_w, input_lens=None, arc_weights=None):
         """Device-buffer entry: emissions, trans_w (and arc_weights, when given) uploaded once,
         gtnb_sparse_transitions_loss on device pointers (gradients in HBM), downloaded afterwards
         -> (losses, grads, arc_grads, trans_grad)."""
+        return self._sparse_transitions_loss(True, emissions, views, transitions, trans_w, True, input_lens,
+                                             arc_weights)
+
+    def _sparse_transitions_loss(self, dev, emissions, views, transitions, trans_w, want_grad, input_lens,
+                                 arc_weights):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
+        arr, n_arcs, aw = _graph_batch(views, B, arc_weights)
         gv = transitions[0]
         tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
         assert tw.size == gv.num_arcs
+        # an empty G: no host pointer at all, or a device buffer that is never read
+        tw_arg = tw if tw.size else np.zeros(1, np.float32) if dev else None
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         losses = np.zeros(B, np.float32)
-        bufs = [self.to_device(e), self.alloc(max(e.nbytes, 16)), self.alloc(4 * max(n_arcs, 4)),
-                self.to_device(tw if tw.size else np.zeros(1, np.float32)), self.alloc(max(tw.nbytes, 16))]
-        e_dev, g_dev, ag_dev, w_dev, tg_dev = bufs
-        aw_dev = None
-        if arc_weights is not None:
-            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
-            assert aw.size == n_arcs
-            aw_dev = self.to_device(aw)
-            bufs.append(aw_dev)
-        try:
+        grads = np.full_like(e, np.nan) if want_grad else None  # every row is written
+        ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
+        tg = np.full(max(tw.size, 1), np.nan, np.float32) if want_grad else None
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_sparse_transitions_loss(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if aw_dev is None else aw_dev.ptr, 1,
-                C.byref(gv), w_dev.ptr, 1, _p(losses, _f32p), g_dev.ptr, 1, ag_dev.ptr, 1, tg_dev.ptr, 1))
-            grads = g_dev.download(e.shape)
-            ag = ag_dev.download((max(n_arcs, 1),))[:n_arcs]
-            tg = tg_dev.download((max(tw.size, 1),))[:tw.size]
-        finally:
-            for buf in bufs:
-                buf.free()
-        return losses, grads, ag, tg
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, C.byref(gv), p.inp(tw_arg),
+                p.flag, _p(losses, _f32p), p.out(grads), p.flag, p.out(ag), p.flag, p.out(tg), p.flag))
+        return (losses, grads, None if ag is None else ag[:n_arcs], None if tg is None else tg[:tw.size])
 
     def graph_transitions_viterbi(self, emissions, views, trans_w, kind=DENSE_ASG, input_lens=None, arc_weights=None):
         """Host-buffer entry of gtnb_graph_transitions_viterbi: emissions [B,T,C], views: B (view, keepalive) pairs
         from make_view, trans_w [C + C*C] (DENSE_ASG) or [C*C] (DENSE_BIGRAM), arc_weights [sum A_b] or None
         -> (paths [B,T] int32, scores [B], arcs [B,T] int32)."""
-        e = np.ascontiguousarray(emissions, dtype=np.float32)
-        B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
-        tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
-        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
-        assert aw is None or aw.size == n_arcs
-        paths = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
-        arcs = np.full((max(B, 1), max(T, 1)), -7, np.int32)
-        scores = np.full(max(B, 1), np.nan, np.float32)
-        self._check(lib().gtnb_graph_transitions_viterbi(
-            self.h, B, T, Cn, e.ctypes.data, 0, _p(il, _i32p), arr, None if aw is None else aw.ctypes.data, 0, kind,
-            tw.ctypes.data, 0, paths.ctypes.data, arcs.ctypes.data, scores.ctypes.data, 0))
-        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
+        return self._graph_transitions_viterbi(False, emissions, views, trans_w, kind, input_lens, arc_weights, False)
 
     def graph_transitions_viterbi_dev(self, emissions, views, trans_w, kind=DENSE_ASG, input_lens=None,
                                       arc_weights=None, trans_on_device=True):
         """Device-buffer entry: emissions (and arc_weights, when given; trans_w unless trans_on_device is False)
         uploaded once, gtnb_graph_transitions_viterbi on device pointers (outputs in HBM), downloaded afterwards
         -> (paths, scores, arcs)."""
+        return self._graph_transitions_viterbi(True, emissions, views, trans_w, kind, input_lens, arc_weights,
+                                               bool(trans_on_device))
+
+    def _graph_transitions_viterbi(self, dev, emissions, views, trans_w, kind, input_lens, arc_weights,
+                                   trans_on_device):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
-        assert len(views) == B
-        arr = (GraphView * max(B, 1))(*[v for v, _ in views])
-        n_arcs = sum(v.num_arcs for v, _ in views)
+        arr, _, aw = _graph_batch(views, B, arc_weights)
         tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
-        fill = np.full((max(B, 1), max(T, 1)), -7, np.int32)  # every entry is written
-        bufs = [self.to_device(e), self.to_device(fill), self.to_device(fill),
-                self.to_device(np.full(max(B, 1), np.nan, np.float32))]
-        e_dev, p_dev, a_dev, s_dev = bufs
-        w_dev = aw_dev = None
-        if trans_on_device:
-            w_dev = self.to_device(tw)
-            bufs.append(w_dev)
-        if arc_weights is not None:
-            aw = np.ascontiguousarray(arc_weights, np.float32).ravel()
-            assert aw.size == n_arcs
-            aw_dev = self.to_device(aw)
-            bufs.append(aw_dev)
-        try:
+        out = _viterbi_outputs(B, T)
+        with _Placed(self, dev) as p:
             self._check(lib().gtnb_graph_transitions_viterbi(
-                self.h, B, T, Cn, e_dev.ptr, 1, _p(il, _i32p), arr, None if aw_dev is None else aw_dev.ptr, 1, kind,
-                tw.ctypes.data if w_dev is None else w_dev.ptr, int(w_dev is not None), p_dev.ptr, a_dev.ptr,
-                s_dev.ptr, 1))
-            paths = p_dev.download(fill.shape, np.int32)
-            arcs = a_dev.download(fill.shape, np.int32)
-            scores = s_dev.download((max(B, 1),))
-        finally:
-            for buf in bufs:
-                buf.free()
-        return (paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T))
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, kind,
+                p.inp(tw, trans_on_device), int(trans_on_device), *map(p.out, out), p.flag))
+        return _viterbi_results(out, B, T)
 
 
 class Lattice:
@@ -858,6 +667,67 @@ class Lattice:
             self.ctx._check(rc)
         out = dict(arcs=arcs[:B], ilabels=il[:B], olabels=ol[:B], lens=lens[:B], weights=pw[:B])
         return (out, status[:B]) if want_status else out
+
+
+class _Placed:
+    """Where the buffers of one call live.  On the host a buffer is passed as a pointer into its numpy array.  On the
+    device (dev) it is uploaded and passed as a device pointer; an output is downloaded back into its array when the
+    `with` block ends without an error.  Every device buffer is freed when the block ends, on every path."""
+
+    def __init__(self, ctx, dev):
+        self.ctx, self.dev, self.flag = ctx, bool(dev), int(bool(dev))
+        self._bufs, self._outs = [], []
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        try:
+            if exc_type is None:
+                for buf, a in self._outs:
+                    a[...] = buf.download(a.shape, a.dtype)
+        finally:
+            for buf in self._bufs:
+                buf.free()
+
+    def inp(self, a, dev=None):
+        """pointer to a (None: None); dev overrides where this one buffer lives"""
+        if a is None:
+            return None
+        if not (self.dev if dev is None else dev):
+            return a.ctypes.data
+        buf = self.ctx.to_device(a)
+        self._bufs.append(buf)
+        return buf.ptr
+
+    def out(self, a):
+        """pointer to the output a, which holds its fill (the value of every entry the call fails to write)"""
+        ptr = self.inp(a)
+        if a is not None and self.dev:
+            self._outs.append((self._bufs[-1], a))
+        return ptr
+
+
+def _graph_batch(views, B, arc_weights):
+    """-> (GraphView array of the B (view, keepalive) pairs, their arc count, arc_weights as float32 or None)"""
+    assert len(views) == B
+    arr = (GraphView * max(B, 1))(*[v for v, _ in views])
+    n_arcs = sum(v.num_arcs for v, _ in views)
+    aw = None if arc_weights is None else np.ascontiguousarray(arc_weights, np.float32).ravel()
+    assert aw is None or aw.size == n_arcs
+    return arr, n_arcs, aw
+
+
+def _viterbi_outputs(B, T):
+    """paths, arcs and scores of a graph Viterbi call, filled so that an entry left unwritten shows"""
+    fill = np.full((max(B, 1), max(T, 1)), -7, np.int32)
+    return fill, fill.copy(), np.full(max(B, 1), np.nan, np.float32)
+
+
+def _viterbi_results(out, B, T):
+    """-> (paths [B,T], scores [B], arcs [B,T])"""
+    paths, arcs, scores = out
+    return paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T)
 
 
 def _cat_targets(targets):

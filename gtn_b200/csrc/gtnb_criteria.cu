@@ -572,6 +572,9 @@ extern "C" int gtnb_ctc_loss(
 
 namespace {
 
+/* the transition weights of a dense kind: ASG [s | W] (C + C*C), BIGRAM W (C*C) */
+long long dense_trans_count(bool bigram, int C) { return (bigram ? 0 : (long long)C) + (long long)C * C; }
+
 /*
  * The body of gtnb_viterbi_dense and gtnb_viterbi_dense_ex: viterbiPath / viterbiScore of the lattice of every
  * utterance through the factored kernel (k_dense.cu); the T*C*C lattice is never materialised.  Host transitions
@@ -593,7 +596,7 @@ int viterbi_dense_run(gtnb_ctx* ctx, const char* fn, int B, int T, int C, const 
       if (input_lens[b] < 0 || input_lens[b] > T)
         return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": input_lens out of range");
   const long long per = (long long)T * C;
-  const long long n_trans = (bigram ? 0 : (long long)C) + (long long)C * C;
+  const long long n_trans = dense_trans_count(bigram, C);
   CallScope scope(ctx);
   float *e_dev = nullptr, *tr_dev = nullptr, *sc_dev = nullptr;
   int32_t *T_dev = nullptr, *paths_dev = nullptr;
@@ -715,7 +718,7 @@ struct AsgGraphs {
  * of weight W[i][j].  The arc into state i carries label i.
  */
 void dense_graph(bool bigram, int C, const float* w, HostGraph* G, std::vector<int32_t>* map) {
-  const long long CC = (long long)C * C, n = bigram ? CC : C + CC;
+  const long long n = dense_trans_count(bigram, C);
   G->src.resize(n);
   G->dst.resize(n);
   G->label.resize(n);
@@ -1289,20 +1292,50 @@ extern "C" int gtnb_asg_loss_ex(
 namespace {
 
 /*
- * The checks gtnb_graph_loss, gtnb_graph_transitions_loss and gtnb_graph_viterbi make of their graphs: T_b =
- * input_lens[b] (or T) in [0, T], well-formed views, no epsilon arc, fewer than 2^31 arcs in all.  Host arc weights
- * are spliced into the copied views; *tot_arcs = sum_b A_b.
+ * The batch of user target graphs every graph entry point takes, as parse_graphs checks it.  The arcs are numbered
+ * through the batch, graph after graph (first_arc).  Host arc weights are spliced into the copied views; device arc
+ * weights (arc_weights_dev) are used where they lie, and the views keep the caller's weights pointer.
  */
-int parse_graphs(gtnb_ctx* ctx, const char* fn, int B, int T, const int32_t* input_lens, const gtnb_graph_view* graphs,
-                 const float* arc_weights, int arc_weights_on_device, std::vector<int32_t>* Tb,
-                 std::vector<gtnb_graph_view>* views, long long* tot_arcs) {
-  Tb->resize(B);
-  views->assign(graphs, graphs + B);
-  *tot_arcs = 0;
+struct GraphBatch {
+  int B = 0, T = 0, C = 0;
+  std::vector<int32_t> Tb;
+  std::vector<gtnb_graph_view> views;
+  std::vector<long long> first_arc; // every view's first arc in the batch's numbering
+  long long tot_arcs = 0;
+  const float* arc_weights_dev = nullptr;
+
+  /* the views with host weights, for the routes that run on the host: device weights are read back into *host_w */
+  int host_views(gtnb_ctx* ctx, std::vector<float>* host_w, std::vector<gtnb_graph_view>* out) const {
+    *out = views;
+    if (!arc_weights_dev) return GTNB_OK;
+    host_w->resize((size_t)std::max(tot_arcs, 1ll));
+    if (tot_arcs) GTNB_TRY(read_to_host(ctx, host_w->data(), arc_weights_dev, 1, tot_arcs));
+    for (int b = 0; b < B; b++) (*out)[b].weights = host_w->data() + first_arc[b];
+    return GTNB_OK;
+  }
+};
+
+/*
+ * The argument check the graph entry points share, then own_checks() (the entry point's own), then the graphs: T_b =
+ * input_lens[b] (or T) in [0, T], well-formed views, no epsilon arc, fewer than 2^31 arcs in all.  args_ok: the
+ * entry point's own pointer arguments are present.
+ */
+template <class Checks>
+int parse_graphs(gtnb_ctx* ctx, const char* fn, int B, int T, int C, const float* emissions,
+                 const gtnb_graph_view* graphs, bool args_ok, const int32_t* input_lens, const float* arc_weights,
+                 int arc_weights_on_device, GraphBatch* gb, Checks&& own_checks) {
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !args_ok || (B > 0 && (!emissions || !graphs)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  GTNB_TRY(own_checks());
+  gb->B = B, gb->T = T, gb->C = C;
+  gb->Tb.resize(B);
+  gb->views.assign(graphs, graphs + B);
+  gb->first_arc.resize(B);
+  gb->arc_weights_dev = arc_weights_on_device ? arc_weights : nullptr;
   for (int b = 0; b < B; b++) {
-    gtnb_graph_view& v = (*views)[b];
-    (*Tb)[b] = input_lens ? input_lens[b] : T;
-    if ((*Tb)[b] < 0 || (*Tb)[b] > T)
+    gtnb_graph_view& v = gb->views[b];
+    gb->Tb[b] = input_lens ? input_lens[b] : T;
+    if (gb->Tb[b] < 0 || gb->Tb[b] > T)
       return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": input_lens outside [0, T]");
     if (validate_view(ctx, v)) return GTNB_ERR_INVALID_ARGUMENT;
     for (int k = 0; k < v.num_arcs; k++)
@@ -1310,20 +1343,27 @@ int parse_graphs(gtnb_ctx* ctx, const char* fn, int B, int T, const int32_t* inp
         return fail(ctx, GTNB_ERR_UNSUPPORTED,
                     std::string(fn) + ": graph " + std::to_string(b) +
                         " has epsilon arcs; remove them first (remove(g, epsilon))");
-    if (arc_weights && !arc_weights_on_device) v.weights = arc_weights + *tot_arcs;
-    *tot_arcs += v.num_arcs;
+    gb->first_arc[b] = gb->tot_arcs;
+    if (arc_weights && !arc_weights_on_device) v.weights = arc_weights + gb->tot_arcs;
+    gb->tot_arcs += v.num_arcs;
   }
-  if (*tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": more than 2^31 arcs");
+  if (gb->tot_arcs >= (1ll << 31)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": more than 2^31 arcs");
+  return GTNB_OK;
+}
+
+int no_own_checks() { return GTNB_OK; }
+
+/* rc of building the implicit sweeps: GTNB_ERR_UNSUPPORTED (the graphs do not fit the implicit layout) turns
+ * *implicit off, so that the caller materialises */
+int implicit_or_materialise(int rc, bool* implicit) {
+  if (rc != GTNB_ERR_UNSUPPORTED) return rc;
+  *implicit = false;
   return GTNB_OK;
 }
 
 struct GraphLossArgs {
-  int B, T, C;
   const float* emissions;
   int emissions_on_device;
-  const gtnb_graph_view* graphs;
-  const float* arc_weights;
-  int arc_weights_on_device;
   float* losses_host;
   float* grads;
   int grads_on_device;
@@ -1333,11 +1373,12 @@ struct GraphLossArgs {
 
 /* one attempt; implicit: try the sweeps first (the materialised lattices when the graphs do not qualify).
  * *needs_exact: a sweep met a non-finite weight or emission, the outputs are not to be used. */
-int graph_loss_once(CallScope& scope, const GraphLossArgs& a, const std::vector<gtnb_graph_view>& views,
-                    const std::vector<int32_t>& Tb, long long tot_arcs, bool implicit, bool* needs_exact) {
+int graph_loss_once(CallScope& scope, const GraphLossArgs& a, const GraphBatch& gb, bool implicit,
+                    bool* needs_exact) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, T = a.T, C = a.C;
-  const long long per = (long long)T * C;
+  const int B = gb.B, T = gb.T, C = gb.C;
+  const std::vector<int32_t>& Tb = gb.Tb;
+  const long long per = (long long)T * C, tot_arcs = gb.tot_arcs;
   const bool want = a.grads || a.arc_grads;
   const int maxT = *std::max_element(Tb.begin(), Tb.end());
   float *e_dev = nullptr, *den = nullptr, *minus1 = nullptr;
@@ -1345,7 +1386,6 @@ int graph_loss_once(CallScope& scope, const GraphLossArgs& a, const std::vector<
   OutBuf g, ag;
   gtnb_lattice*& lat = scope.lattice();
   gtnb_lattice*& dlat = scope.lattice();
-  const float* aw_dev = a.arc_weights_on_device ? a.arc_weights : nullptr;
   const float* den_scores = nullptr;
   std::vector<float> m1(B, -1.0f); // subtract's gradFunc, functions.cpp:53-58
   // materialised route: forwardScore(E_b) as the reference computes it, non-finite emissions included (its sweep
@@ -1380,13 +1420,10 @@ int graph_loss_once(CallScope& scope, const GraphLossArgs& a, const std::vector<
   GTNB_TRY(stage_upload(ctx, minus1, m1.data(), sizeof(float) * B));
   GTNB_TRY(stage_end(ctx));
 
-  if (implicit) {
-    const int rc = compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, e_dev, per, true, &lat, true, aw_dev);
-    if (rc == GTNB_ERR_UNSUPPORTED) // does not fit the implicit layout: materialise
-      implicit = false;
-    else
-      GTNB_TRY(rc);
-  }
+  if (implicit)
+    GTNB_TRY(implicit_or_materialise(compose_linear_impl(ctx, B, gb.views.data(), B, 0, Tb.data(), C, e_dev, per,
+                                                         true, &lat, true, gb.arc_weights_dev),
+                                     &implicit));
   if (implicit) {
     // forwardScore(E_b) and its +1 gradient on the second stream, beside the forward sweep
     GTNB_TRY(fork_to(ctx, ctx->copy_stream));
@@ -1400,7 +1437,8 @@ int graph_loss_once(CallScope& scope, const GraphLossArgs& a, const std::vector<
     if (want) GTNB_TRY(launch_implicit_backward(ctx, lat, minus1, g.dev, per, 0, -1, ag.dev));
     den_scores = den;
   } else {
-    GTNB_TRY(compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, e_dev, per, false, &lat, false, aw_dev));
+    GTNB_TRY(compose_linear_impl(ctx, B, gb.views.data(), B, 0, Tb.data(), C, e_dev, per, false, &lat, false,
+                                 gb.arc_weights_dev));
     GTNB_TRY(compose_linear_impl(ctx, B, &free_view, 1, 0, Tb.data(), C, e_dev, per, false, &dlat));
     GTNB_TRY(gtnb_forward(ctx, dlat, 0, nullptr, nullptr));
     GTNB_TRY(gtnb_forward(ctx, lat, 0, nullptr, nullptr));
@@ -1424,19 +1462,15 @@ extern "C" int gtnb_graph_loss(
     gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
     const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, float* losses_host,
     float* grads, int grads_on_device, float* arc_grads, int arc_grads_on_device) {
-  const GraphLossArgs a{B, T, C, emissions, emissions_on_device, graphs, arc_weights, arc_weights_on_device,
-                        losses_host, grads, grads_on_device, arc_grads, arc_grads_on_device};
-  if (!ctx || B < 0 || T < 0 || C <= 0 || (B > 0 && (!emissions || !graphs || !losses_host)))
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_graph_loss: bad arguments");
-  std::vector<int32_t> Tb;
-  std::vector<gtnb_graph_view> views;
-  long long tot_arcs = 0;
-  GTNB_TRY(parse_graphs(ctx, "gtnb_graph_loss", B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb,
-                        &views, &tot_arcs));
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, "gtnb_graph_loss", B, T, C, emissions, graphs, B == 0 || losses_host, input_lens,
+                        arc_weights, arc_weights_on_device, &gb, no_own_checks));
+  const GraphLossArgs a{emissions, emissions_on_device, losses_host, grads, grads_on_device, arc_grads,
+                        arc_grads_on_device};
   // (graphs that are not label-uniform need C <= k_implicit.cu's kArcMaxLabels: compose_linear_impl checks)
-  return run_criterion(ctx, B, Tb.data(), losses_host, nullptr, 0, 0, ctx->use_implicit,
+  return run_criterion(ctx, B, gb.Tb.data(), losses_host, nullptr, 0, 0, ctx->use_implicit,
                        [&](CallScope& scope, bool implicit, bool* needs_exact) {
-                         return graph_loss_once(scope, a, views, Tb, tot_arcs, implicit, needs_exact);
+                         return graph_loss_once(scope, a, gb, implicit, needs_exact);
                        });
 }
 
@@ -1454,18 +1488,40 @@ extern "C" int gtnb_graph_loss(
  */
 namespace {
 
+/* the checks of the entry points that take a dense transition graph kind */
+int check_dense_kind(gtnb_ctx* ctx, const char* fn, int kind, int C) {
+  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown graph kind");
+  if (C > kNgramMaxLabels)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                std::string(fn) + ": C = " + std::to_string(C) +
+                    " labels; the product builder and the trellis kernels take C <= " +
+                    std::to_string(kNgramMaxLabels));
+  return GTNB_OK;
+}
+
+/* the device route's numerators, build(view, &p) for every graph of the batch, and whether the implicit sweeps take
+ * them all (the dense kinds' products are label-uniform, so C bears only on gtnb_sparse_transitions_loss's) */
+template <class Build>
+bool device_products(const GraphBatch& gb, Build&& build, std::vector<ProductGraph>* prods) {
+  prods->resize(gb.B);
+  std::vector<SgDims> dims(gb.B);
+  for (int b = 0; b < gb.B; b++) {
+    ProductGraph& p = (*prods)[b];
+    build(gb.views[b], &p);
+    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, p.uniform ? 1 : 0, p.max_in,
+                     p.max_out};
+  }
+  return implicit_dims_supported(dims.data(), gb.B, gb.C);
+}
+
 /* trellis_loss_fast's numerator for the user graphs: the (folded) products, weighted by launch_product_fold */
 struct GraphNumerator {
+  const GraphBatch& gb;
   const std::vector<ProductGraph>& prods;
-  const std::vector<gtnb_graph_view>& views; // A_b, host weights (or none) in place
-  const std::vector<int32_t>& Tb;
-  int C;
-  bool bigram;
-  const float* arc_weights_dev; // nullable: the views' weights
+  int n_w; // slots of Wx before sigma: the transition count
   float* arc_grads;
   int arc_grads_on_device;
-  long long tot_arcs;
-  int nW = -1; // slots of Wx before sigma; -1: the dense kind's (gtnb_sparse_transitions_loss: G's arc count)
   bool arc_labels = false; // some product is not label-uniform: k_implicit.cu's arc-label instantiations
   long long tot_A = 0;
   std::vector<gtnb_graph_view> pviews;
@@ -1479,28 +1535,27 @@ struct GraphNumerator {
 
   bool wants_arc_grads() const { return arc_grads != nullptr; }
   int alloc(CallScope& scope, const float* e, long long stride, gtnb_lattice**) {
-    const int B = (int)views.size();
+    const int B = gb.B;
+    const long long tot_arcs = gb.tot_arcs;
     e_dev = e;
     per = stride;
     pviews.resize(B);
-    long long off = 0;
     for (int b = 0; b < B; b++) {
       pviews[b] = prods[b].view();
       tidx_h.insert(tidx_h.end(), prods[b].tidx.begin(), prods[b].tidx.end());
-      for (int32_t k : prods[b].arc_of) arc_of_h.push_back((int32_t)(off + k));
-      off += views[b].num_arcs;
+      for (int32_t k : prods[b].arc_of) arc_of_h.push_back((int32_t)(gb.first_arc[b] + k));
+      arc_labels |= !prods[b].uniform;
     }
     tot_A = (long long)tidx_h.size();
     GTNB_TRY(scope.alloc(&Tb_dev, B));
     GTNB_TRY(scope.alloc(&map, tot_A));
     GTNB_TRY(scope.alloc(&arc_of, tot_A));
     GTNB_TRY(scope.alloc(&fw, tot_A));
-    if (!arc_weights_dev) {
+    if (!gb.arc_weights_dev) {
       w_A_h.assign(tot_arcs, 0.0f);
-      off = 0;
       for (int b = 0; b < B; b++) {
-        if (views[b].weights) std::copy(views[b].weights, views[b].weights + views[b].num_arcs, w_A_h.begin() + off);
-        off += views[b].num_arcs;
+        const gtnb_graph_view& v = gb.views[b];
+        if (v.weights) std::copy(v.weights, v.weights + v.num_arcs, w_A_h.begin() + gb.first_arc[b]);
       }
       GTNB_TRY(scope.alloc(&w_A, tot_arcs));
     }
@@ -1512,70 +1567,68 @@ struct GraphNumerator {
   }
   int stage(CallScope& scope, gtnb_lattice*) {
     gtnb_ctx* ctx = scope.ctx();
-    GTNB_TRY(stage_upload(ctx, Tb_dev, Tb.data(), sizeof(int32_t) * Tb.size()));
+    GTNB_TRY(stage_upload(ctx, Tb_dev, gb.Tb.data(), sizeof(int32_t) * gb.Tb.size()));
     if (tot_A) {
       GTNB_TRY(stage_upload(ctx, map, tidx_h.data(), sizeof(int32_t) * tot_A));
       GTNB_TRY(stage_upload(ctx, arc_of, arc_of_h.data(), sizeof(int32_t) * tot_A));
     }
-    if (!arc_weights_dev && tot_arcs) GTNB_TRY(stage_upload(ctx, w_A, w_A_h.data(), sizeof(float) * tot_arcs));
+    if (!gb.arc_weights_dev && gb.tot_arcs)
+      GTNB_TRY(stage_upload(ctx, w_A, w_A_h.data(), sizeof(float) * gb.tot_arcs));
     return GTNB_OK;
   }
   const int32_t* T_dev() const { return Tb_dev; }
   int build(CallScope& scope, gtnb_lattice*& lat, const float* w_dev, const float* sigma) {
     gtnb_ctx* ctx = scope.ctx();
-    const int n_w = nW >= 0 ? nW : bigram ? C * C : C + C * C;
-    GTNB_TRY(launch_product_fold(ctx, tot_A, arc_weights_dev ? arc_weights_dev : w_A, arc_of, w_dev, n_w, sigma, map,
-                                 fw));
+    GTNB_TRY(launch_product_fold(ctx, tot_A, gb.arc_weights_dev ? gb.arc_weights_dev : w_A, arc_of, w_dev, n_w, sigma,
+                                 map, fw));
     // the dense kinds' products are label-uniform: the plain instantiations, with the folded weights gathered into
     // the tables
-    return compose_linear_impl(ctx, (int)pviews.size(), pviews.data(), (int)pviews.size(), 0, Tb.data(), C, e_dev,
-                               per, true, &lat, arc_labels, fw);
+    return compose_linear_impl(ctx, (int)pviews.size(), pviews.data(), (int)pviews.size(), 0, gb.Tb.data(), gb.C,
+                               e_dev, per, true, &lat, arc_labels, fw);
   }
   int scatter(CallScope& scope, const float* ggrad) {
     if (!arc_grads) return GTNB_OK;
     GTNB_TRY(launch_scatter_add(scope.ctx(), ag.dev, arc_of, ggrad, tot_A));
-    return ag.copy_out(scope.ctx(), tot_arcs);
+    return ag.copy_out(scope.ctx(), gb.tot_arcs);
   }
 };
 
-/* the materialised route: the unfolded products weighted on the host, the dense lattice of G.  built: the device
- * route's products, which for ASG (where folding changes nothing) are the unfolded ones; BIGRAM builds its own. */
-int graph_transitions_exact(CallScope& scope, const TransitionArgs& a, bool bigram,
-                            const std::vector<ProductGraph>& built,
-                            const std::vector<gtnb_graph_view>& views, const std::vector<int32_t>& Tb,
-                            const float* arc_weights, int arc_weights_on_device, float* arc_grads,
-                            int arc_grads_on_device, long long tot_arcs) {
+/*
+ * The materialised route of gtnb_graph_transitions_loss and gtnb_sparse_transitions_loss: make_G(W, &G, &gmap)
+ * builds G from the n_trans host weights W, gmap holding the trans_w slot of each of G's arcs; unfold(view, &p)
+ * builds the unfolded products, which are weighted on the host.  built (nullable): the device route's products,
+ * taken as they are where folding changes nothing (ASG).
+ */
+template <class MakeG, class Unfold>
+int transitions_exact(CallScope& scope, const TransitionArgs& a, const GraphBatch& gb, long long n_trans,
+                      MakeG&& make_G, Unfold&& unfold, const std::vector<ProductGraph>* built, float* arc_grads,
+                      int arc_grads_on_device) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, C = a.C;
-  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
-  std::vector<float> W(n_trans), w_A;
-  GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, n_trans));
-  if (arc_weights && arc_weights_on_device) {
-    w_A.resize(tot_arcs);
-    GTNB_TRY(read_to_host(ctx, w_A.data(), arc_weights, 1, tot_arcs));
-  }
+  const int B = gb.B;
+  std::vector<float> W(std::max(n_trans, 1ll)), host_w;
+  if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, n_trans));
+  std::vector<gtnb_graph_view> views;
+  GTNB_TRY(gb.host_views(ctx, &host_w, &views));
   HostGraph G;
   std::vector<int32_t> gmap;
-  dense_graph(bigram, C, W.data(), &G, &gmap);
-  std::vector<ProductGraph> unfolded(bigram ? B : 0);
-  const std::vector<ProductGraph>& prods = bigram ? unfolded : built;
+  make_G(W.data(), &G, &gmap);
+  std::vector<ProductGraph> unfolded(built ? 0 : B);
+  const std::vector<ProductGraph>& prods = built ? *built : unfolded;
   std::vector<std::vector<float>> pw(B);
   std::vector<gtnb_graph_view> pviews(B);
   std::vector<int32_t> pmap, arc_of;
-  long long off = 0;
   for (int b = 0; b < B; b++) {
-    if (bigram) build_product(views[b], C, bigram, /*fold=*/false, &unfolded[b]);
-    product_weights(prods[b], w_A.empty() ? views[b].weights : w_A.data() + off, W.data(), &pw[b]);
+    if (!built) unfold(views[b], &unfolded[b]);
+    product_weights(prods[b], views[b].weights, W.data(), &pw[b]);
     pviews[b] = prods[b].view();
     pviews[b].weights = pw[b].data();
     pmap.insert(pmap.end(), prods[b].tidx.begin(), prods[b].tidx.end());
-    for (int32_t k : prods[b].arc_of) arc_of.push_back((int32_t)(off + k));
-    off += views[b].num_arcs;
+    for (int32_t k : prods[b].arc_of) arc_of.push_back((int32_t)(gb.first_arc[b] + k));
   }
   OutBuf ag;
-  if (arc_grads) GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, tot_arcs, &ag));
-  return transitions_loss_materialised(scope, a, Tb.data(), G, gmap, n_trans, pviews, pmap, &arc_of,
-                                       arc_grads ? &ag : nullptr, tot_arcs);
+  if (arc_grads) GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, gb.tot_arcs, &ag));
+  return transitions_loss_materialised(scope, a, gb.Tb.data(), G, gmap, n_trans, pviews, pmap, &arc_of,
+                                       arc_grads ? &ag : nullptr, gb.tot_arcs);
 }
 
 } // namespace
@@ -1586,47 +1639,34 @@ extern "C" int gtnb_graph_transitions_loss(
     const float* trans_w, int trans_on_device, float* losses_host, float* grads, int grads_on_device,
     float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
   const char* fn = "gtnb_graph_transitions_loss";
-  if (!ctx || B < 0 || T < 0 || C <= 0 || !trans_w || (B > 0 && (!emissions || !graphs || !losses_host)))
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
-  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown graph kind");
-  if (C > kNgramMaxLabels)
-    return fail(ctx, GTNB_ERR_UNSUPPORTED,
-                std::string(fn) + ": C = " + std::to_string(C) +
-                    " labels; the trellis kernels hold the transitions on chip for C <= " +
-                    std::to_string(kNgramMaxLabels));
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, fn, B, T, C, emissions, graphs, trans_w && (B == 0 || losses_host), input_lens,
+                        arc_weights, arc_weights_on_device, &gb, [&] { return check_dense_kind(ctx, fn, kind, C); }));
   const bool bigram = kind == GTNB_DENSE_BIGRAM;
-  std::vector<int32_t> Tb;
-  std::vector<gtnb_graph_view> views;
-  long long tot_arcs = 0;
-  GTNB_TRY(parse_graphs(ctx, fn, B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
-                        &tot_arcs));
   const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
                          nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
-  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
+  const long long n_trans = dense_trans_count(bigram, C);
   // the device route's numerators (BIGRAM: folded), whose shapes decide whether it can be taken
-  std::vector<ProductGraph> prods(B);
-  std::vector<SgDims> dims(B);
-  for (int b = 0; b < B; b++) {
-    build_product(views[b], C, bigram, /*fold=*/true, &prods[b]);
-    const ProductGraph& p = prods[b];
-    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, /*uniform=*/1, p.max_in,
-                     p.max_out};
-  }
+  std::vector<ProductGraph> prods;
+  const bool fits = device_products(
+      gb, [&](const gtnb_graph_view& v, ProductGraph* p) { build_product(v, C, bigram, /*fold=*/true, p); }, &prods);
   TrellisCriterion k = bigram ? TrellisCriterion{n_trans, (long long)B * (T + 1) * C, /*fold=*/true,
                                                        launch_ngram_den_forward, launch_ngram_den_backward}
                                     : TrellisCriterion{n_trans, asg_alpha_floats(B, T, C), /*fold=*/false,
                                                        launch_asg_den_forward, launch_asg_den_backward};
-  const bool fast = ctx->use_implicit && implicit_dims_supported(dims.data(), B);
-  return run_criterion(ctx, B, Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans, fast,
-                       [&](CallScope& scope, bool f, bool* needs_exact) {
+  return run_criterion(ctx, B, gb.Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans,
+                       ctx->use_implicit && fits, [&](CallScope& scope, bool f, bool* needs_exact) {
                          if (!f)
-                           return graph_transitions_exact(scope, a, bigram, prods, views, Tb, arc_weights,
-                                                          arc_weights_on_device, arc_grads, arc_grads_on_device,
-                                                          tot_arcs);
-                         GraphNumerator num{prods, views, Tb, C, bigram,
-                                            arc_weights && arc_weights_on_device ? arc_weights : nullptr,
-                                            arc_grads, arc_grads_on_device, tot_arcs};
+                           return transitions_exact(
+                               scope, a, gb, n_trans,
+                               [&](const float* W, HostGraph* G, std::vector<int32_t>* gmap) {
+                                 dense_graph(bigram, C, W, G, gmap);
+                               },
+                               [&](const gtnb_graph_view& v, ProductGraph* p) {
+                                 build_product(v, C, bigram, /*fold=*/false, p);
+                               },
+                               bigram ? nullptr : &prods, arc_grads, arc_grads_on_device);
+                         GraphNumerator num{gb, prods, (int)n_trans, arc_grads, arc_grads_on_device};
                          return trellis_loss_fast(scope, k, a, num, needs_exact);
                        });
 }
@@ -1689,60 +1729,8 @@ struct SparseDenominator {
   }
 };
 
-/* the materialised route: G (its arcs with a label in [0, C)) weighted on the host, the unfolded products */
-int sparse_transitions_exact(CallScope& scope, const TransitionArgs& a, const gtnb_graph_view& Gv,
-                             const SparseTables& t, const std::vector<gtnb_graph_view>& views,
-                             const std::vector<int32_t>& Tb, const float* arc_weights, int arc_weights_on_device,
-                             float* arc_grads, int arc_grads_on_device, long long tot_arcs) {
-  gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, C = a.C;
-  const long long n_trans = Gv.num_arcs;
-  std::vector<float> W(std::max<long long>(n_trans, 1)), w_A;
-  if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, n_trans));
-  if (arc_weights && arc_weights_on_device && tot_arcs) {
-    w_A.resize(tot_arcs);
-    GTNB_TRY(read_to_host(ctx, w_A.data(), arc_weights, 1, tot_arcs));
-  }
-  HostGraph G;
-  G.flags = t.flags;
-  std::vector<int32_t> gmap;
-  for (int g = 0; g < Gv.num_arcs; g++)
-    if (Gv.arc_olabel[g] >= 0 && Gv.arc_olabel[g] < C) {
-      G.arc(Gv.arc_src[g], Gv.arc_dst[g], Gv.arc_olabel[g], W[g]);
-      gmap.push_back(g);
-    }
-  std::vector<ProductGraph> prods(B);
-  std::vector<std::vector<float>> pw(B);
-  std::vector<gtnb_graph_view> pviews(B);
-  std::vector<int32_t> pmap, arc_of;
-  long long off = 0;
-  for (int b = 0; b < B; b++) {
-    build_sparse_product(views[b], Gv, t, C, /*fold=*/false, &prods[b]);
-    product_weights(prods[b], w_A.empty() ? views[b].weights : w_A.data() + off, W.data(), &pw[b]);
-    pviews[b] = prods[b].view();
-    pviews[b].weights = pw[b].data();
-    pmap.insert(pmap.end(), prods[b].tidx.begin(), prods[b].tidx.end());
-    for (int32_t k : prods[b].arc_of) arc_of.push_back((int32_t)(off + k));
-    off += views[b].num_arcs;
-  }
-  OutBuf ag;
-  if (arc_grads) GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, tot_arcs, &ag));
-  return transitions_loss_materialised(scope, a, Tb.data(), G, gmap, n_trans, pviews, pmap, &arc_of,
-                                       arc_grads ? &ag : nullptr, tot_arcs);
-}
-
-} // namespace
-
-extern "C" int gtnb_sparse_transitions_loss(
-    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
-    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
-    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, float* losses_host, float* grads,
-    int grads_on_device, float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
-  const std::string fn = "gtnb_sparse_transitions_loss";
-  if (!ctx || B < 0 || T < 0 || C <= 0 || !transitions ||
-      (B > 0 && (!emissions || !graphs || !losses_host || !trans_w)))
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
-  const gtnb_graph_view& Gv = *transitions;
+/* the checks of gtnb_sparse_transitions_loss's transition graph */
+int check_transition_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& Gv) {
   if (validate_view(ctx, Gv)) return GTNB_ERR_INVALID_ARGUMENT;
   if (Gv.num_nodes < 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the transition graph has no nodes");
   for (int g = 0; g < Gv.num_arcs; g++) {
@@ -1754,39 +1742,56 @@ extern "C" int gtnb_sparse_transitions_loss(
                   fn + ": the transition graph is a transducer; make it an acceptor first (projectInput / "
                        "projectOutput)");
   }
-  std::vector<int32_t> Tb;
-  std::vector<gtnb_graph_view> views;
-  long long tot_arcs = 0;
-  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
-                        &tot_arcs));
+  return GTNB_OK;
+}
+
+} // namespace
+
+extern "C" int gtnb_sparse_transitions_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
+    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, float* losses_host, float* grads,
+    int grads_on_device, float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const std::string fn = "gtnb_sparse_transitions_loss";
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, C, emissions, graphs,
+                        transitions && (B == 0 || (losses_host && trans_w)), input_lens, arc_weights,
+                        arc_weights_on_device, &gb, [&] { return check_transition_graph(ctx, fn, *transitions); }));
+  const gtnb_graph_view& Gv = *transitions;
   const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
                          nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
   const long long n_trans = Gv.num_arcs;
   SparseTables t;
   sparse_tables(Gv, C, &t);
   // the device route's numerators (folded), whose shapes decide, with G's, whether it can be taken
-  const bool den_fits = ctx->use_implicit && sparse_den_supported(t.S, t.A, C);
-  std::vector<ProductGraph> prods(den_fits ? B : 0);
-  std::vector<SgDims> dims(prods.size());
-  bool uniform = true;
-  for (size_t b = 0; b < prods.size(); b++) {
-    build_sparse_product(views[b], Gv, t, C, /*fold=*/true, &prods[b]);
-    const ProductGraph& p = prods[b];
-    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, p.uniform ? 1 : 0, p.max_in,
-                     p.max_out};
-    uniform &= p.uniform;
-  }
-  const bool fast = den_fits && implicit_dims_supported(dims.data(), B, C);
-  return run_criterion(ctx, B, Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans, fast,
+  std::vector<ProductGraph> prods;
+  const bool fast = ctx->use_implicit && sparse_den_supported(t.S, t.A, C) &&
+                    device_products(
+                        gb,
+                        [&](const gtnb_graph_view& v, ProductGraph* p) {
+                          build_sparse_product(v, Gv, t, C, /*fold=*/true, p);
+                        },
+                        &prods);
+  return run_criterion(ctx, B, gb.Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
                          if (!f)
-                           return sparse_transitions_exact(scope, a, Gv, t, views, Tb, arc_weights,
-                                                           arc_weights_on_device, arc_grads, arc_grads_on_device,
-                                                           tot_arcs);
+                           return transitions_exact(
+                               scope, a, gb, n_trans,
+                               [&](const float* W, HostGraph* G, std::vector<int32_t>* gmap) {
+                                 // G's arcs with a label in [0, C)
+                                 G->flags = t.flags;
+                                 for (int g = 0; g < Gv.num_arcs; g++)
+                                   if (Gv.arc_olabel[g] >= 0 && Gv.arc_olabel[g] < C) {
+                                     G->arc(Gv.arc_src[g], Gv.arc_dst[g], Gv.arc_olabel[g], W[g]);
+                                     gmap->push_back(g);
+                                   }
+                               },
+                               [&](const gtnb_graph_view& v, ProductGraph* p) {
+                                 build_sparse_product(v, Gv, t, C, /*fold=*/false, p);
+                               },
+                               nullptr, arc_grads, arc_grads_on_device);
                          SparseDenominator den{t, n_trans};
-                         GraphNumerator num{prods, views, Tb, C, false,
-                                            arc_weights && arc_weights_on_device ? arc_weights : nullptr,
-                                            arc_grads, arc_grads_on_device, tot_arcs, (int)n_trans, !uniform};
+                         GraphNumerator num{gb, prods, (int)n_trans, arc_grads, arc_grads_on_device};
                          return trellis_loss_fast(scope, den, a, num, needs_exact);
                        });
 }
@@ -1802,77 +1807,69 @@ extern "C" int gtnb_sparse_transitions_loss(
 namespace {
 
 struct GraphViterbiArgs {
-  int B, T, C;
   const float* emissions;
   int emissions_on_device;
-  const float* arc_weights;
-  int arc_weights_on_device;
   int32_t* paths;
   int32_t* arcs;
   float* scores;
   int outputs_on_device;
 };
 
-/* every view's first arc in the batch's numbering, and iota = 0, 1, ... as long as the largest view's arc list */
-void arc_numbering(const std::vector<gtnb_graph_view>& views, std::vector<long long>* first_arc,
-                   std::vector<int32_t>* iota) {
-  first_arc->assign(views.size(), 0);
+/* the device buffers of a graph Viterbi call: the emissions, the outputs (the user's own when they are on the
+ * device) and one zeroed status word per utterance */
+struct ViterbiBufs {
+  float *e_dev = nullptr, *s_dev = nullptr;
+  int32_t *p_dev = nullptr, *a_dev = nullptr, *status = nullptr;
+};
+
+/* 0, 1, ... as long as the largest view's arc list: the arc ids a view's ilabels are replaced with */
+std::vector<int32_t> arc_ids(const std::vector<gtnb_graph_view>& views) {
   int max_arcs = 0;
-  for (size_t b = 0; b < views.size(); b++) {
-    if (b > 0) (*first_arc)[b] = (*first_arc)[b - 1] + views[b - 1].num_arcs;
-    max_arcs = std::max(max_arcs, views[b].num_arcs);
-  }
-  iota->resize(std::max(max_arcs, 1));
-  for (int k = 0; k < max_arcs; k++) (*iota)[k] = k;
+  for (const gtnb_graph_view& v : views) max_arcs = std::max(max_arcs, v.num_arcs);
+  std::vector<int32_t> ids(std::max(max_arcs, 1));
+  for (int k = 0; k < max_arcs; k++) ids[k] = k;
+  return ids;
 }
 
 /*
  * The materialised route for the utterances `which`: gtnb_compose_linear (the lattice is put in the reference's
  * relaxation order while exact_ties is on, k_order.cu), gtnb_forward(tropical) for the score and gtnb_viterbi_path.
- * A_b is matched on its olabels, so its ilabels play no part in the composition: they are replaced by the arc ids,
- * which the path's ilabels then carry back.  The rows are written into the device outputs p_dev / a_dev (nullable)
- * and s_dev.  arc_map (nullable): per utterance, the arc the caller reports for each arc of views[b]
- * (gtnb_graph_transitions_viterbi: views[b] is compose(A_b, G), the map its gradInfo into A_b).
+ * views: one per utterance, with host weights.  A_b is matched on its olabels, so its ilabels play no part in the
+ * composition: they are replaced by the arc ids, which the path's ilabels then carry back.  The rows are written into
+ * the device outputs v.p_dev / v.a_dev (nullable) and v.s_dev.  arc_map (nullable): per utterance, the arc the caller
+ * reports for each arc of views[b] (gtnb_graph_transitions_viterbi: views[b] is compose(A_b, G), the map its gradInfo
+ * into A_b).
  */
-int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::vector<gtnb_graph_view>& views,
-                        const std::vector<int32_t>& Tb, long long tot_arcs, const float* e_dev,
-                        const std::vector<int>& which, int32_t* p_dev, int32_t* a_dev, float* s_dev,
+int graph_viterbi_exact(CallScope& scope, const GraphBatch& gb, const std::vector<gtnb_graph_view>& views,
+                        const ViterbiBufs& v, const std::vector<int>& which,
                         const std::vector<std::vector<int32_t>>* arc_map = nullptr) {
   gtnb_ctx* ctx = scope.ctx();
-  const int T = a.T, C = a.C, ml = std::max(T, 1);
+  const int T = gb.T, C = gb.C, ml = std::max(T, 1);
   const long long per = (long long)T * C;
-  std::vector<float> host_w;
-  if (a.arc_weights && a.arc_weights_on_device) {
-    host_w.resize((size_t)std::max(tot_arcs, 1ll));
-    GTNB_TRY(read_to_host(ctx, host_w.data(), a.arc_weights, 1, tot_arcs));
-  }
-  std::vector<long long> first_arc;
-  std::vector<int32_t> iota;
-  arc_numbering(views, &first_arc, &iota);
+  const std::vector<int32_t> ids = arc_ids(views);
   // the utterances with frames (T_b = 0 accepts nothing) and their emission rows, contiguous
   std::vector<int> sub;
   for (int b : which)
-    if (Tb[b] > 0) sub.push_back(b);
+    if (gb.Tb[b] > 0) sub.push_back(b);
   const int n = (int)sub.size();
   std::vector<float> sc(std::max(n, 1), -std::numeric_limits<float>::infinity());
   std::vector<int32_t> parc((size_t)std::max(n, 1) * ml, -1), plab(parc.size(), -1), plen(std::max(n, 1), -1);
   if (n > 0) {
     std::vector<gtnb_graph_view> sv(n);
     std::vector<int32_t> sT(n);
-    const float* e_sub = e_dev;
-    if (n < a.B) {
+    const float* e_sub = v.e_dev;
+    if (n < gb.B) {
       float* e_copy = nullptr;
       GTNB_TRY(scope.alloc(&e_copy, per * n));
       for (int k = 0; k < n; k++)
-        GTNB_CUDA(ctx, cudaMemcpyAsync(e_copy + per * k, e_dev + per * sub[k], sizeof(float) * per,
+        GTNB_CUDA(ctx, cudaMemcpyAsync(e_copy + per * k, v.e_dev + per * sub[k], sizeof(float) * per,
                                        cudaMemcpyDeviceToDevice, ctx->stream));
       e_sub = e_copy;
     }
     for (int k = 0; k < n; k++) {
       sv[k] = views[sub[k]];
-      sv[k].arc_ilabel = iota.data();
-      sT[k] = Tb[sub[k]];
-      if (!host_w.empty()) sv[k].weights = host_w.data() + first_arc[sub[k]];
+      sv[k].arc_ilabel = ids.data();
+      sT[k] = gb.Tb[sub[k]];
     }
     gtnb_lattice*& lat = scope.lattice();
     GTNB_TRY(gtnb_compose_linear(ctx, n, sv.data(), n, 0, sT.data(), C, e_sub, per, &lat));
@@ -1894,35 +1891,28 @@ int graph_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, const std::
       arow[j * ml + t] = t >= len ? -1 : arc_map ? (*arc_map)[b][parc[k * ml + t]] : parc[k * ml + t];
     }
     srow[j] = run ? sc[k] : -std::numeric_limits<float>::infinity();
-    if (p_dev && T > 0)
-      GTNB_CUDA(ctx, cudaMemcpyAsync(p_dev + (long long)b * T, &prow[j * ml], sizeof(int32_t) * T,
+    if (v.p_dev && T > 0)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(v.p_dev + (long long)b * T, &prow[j * ml], sizeof(int32_t) * T,
                                      cudaMemcpyHostToDevice, ctx->stream));
-    if (a_dev && T > 0)
-      GTNB_CUDA(ctx, cudaMemcpyAsync(a_dev + (long long)b * T, &arow[j * ml], sizeof(int32_t) * T,
+    if (v.a_dev && T > 0)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(v.a_dev + (long long)b * T, &arow[j * ml], sizeof(int32_t) * T,
                                      cudaMemcpyHostToDevice, ctx->stream));
-    GTNB_CUDA(ctx, cudaMemcpyAsync(s_dev + b, &srow[j], sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    GTNB_CUDA(ctx, cudaMemcpyAsync(v.s_dev + b, &srow[j], sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     k += run;
   }
   return scope.sync();
 }
 
-/* the device buffers of a graph Viterbi call: the emissions, the outputs (the user's own when they are on the
- * device) and one zeroed status word per utterance */
-struct ViterbiBufs {
-  float *e_dev = nullptr, *s_dev = nullptr;
-  int32_t *p_dev = nullptr, *a_dev = nullptr, *status = nullptr;
-};
-
-int viterbi_open(CallScope& scope, const GraphViterbiArgs& a, ViterbiBufs* v) {
+int viterbi_open(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, ViterbiBufs* v) {
   gtnb_ctx* ctx = scope.ctx();
-  const long long nrow = (long long)a.B * a.T;
+  const long long nrow = (long long)gb.B * gb.T;
   const bool dev_out = a.outputs_on_device != 0;
-  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, (long long)a.T * a.C * a.B, &v->e_dev));
-  GTNB_TRY(scope.borrow(a.scores, a.scores && dev_out, a.B, &v->s_dev));
+  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, (long long)gb.T * gb.C * gb.B, &v->e_dev));
+  GTNB_TRY(scope.borrow(a.scores, a.scores && dev_out, gb.B, &v->s_dev));
   if (a.paths) GTNB_TRY(scope.borrow(a.paths, dev_out, nrow, &v->p_dev));
   if (a.arcs) GTNB_TRY(scope.borrow(a.arcs, dev_out, nrow, &v->a_dev));
-  GTNB_TRY(scope.alloc(&v->status, a.B));
-  GTNB_CUDA(ctx, cudaMemsetAsync(v->status, 0, sizeof(int32_t) * a.B, ctx->stream));
+  GTNB_TRY(scope.alloc(&v->status, gb.B));
+  GTNB_CUDA(ctx, cudaMemsetAsync(v->status, 0, sizeof(int32_t) * gb.B, ctx->stream));
   return GTNB_OK;
 }
 
@@ -1933,11 +1923,11 @@ int viterbi_open(CallScope& scope, const GraphViterbiArgs& a, ViterbiBufs* v) {
  * `which`; then host outputs are copied out.
  */
 template <typename Exact>
-int viterbi_finish(CallScope& scope, const GraphViterbiArgs& a, const std::vector<int32_t>& Tb, bool implicit,
+int viterbi_finish(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, bool implicit,
                    const ViterbiBufs& v, Exact&& exact) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B;
-  const long long nrow = (long long)B * a.T;
+  const int B = gb.B;
+  const long long nrow = (long long)B * gb.T;
   std::vector<int> which;
   if (implicit) {
     GTNB_TRY(readback_reserve(ctx, sizeof(int32_t) * B));
@@ -1945,7 +1935,7 @@ int viterbi_finish(CallScope& scope, const GraphViterbiArgs& a, const std::vecto
     GTNB_CUDA(ctx, cudaMemcpyAsync(st, v.status, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ctx->stream));
     GTNB_TRY(scope.sync());
     for (int b = 0; b < B; b++)
-      if (Tb[b] > 0 && ((st[b] & 1) || ((st[b] & 2) && ctx->exact_ties))) which.push_back(b);
+      if (gb.Tb[b] > 0 && ((st[b] & 1) || ((st[b] & 2) && ctx->exact_ties))) which.push_back(b);
   } else {
     for (int b = 0; b < B; b++) which.push_back(b);
   }
@@ -1961,30 +1951,28 @@ int viterbi_finish(CallScope& scope, const GraphViterbiArgs& a, const std::vecto
   return scope.sync();
 }
 
-int graph_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const std::vector<gtnb_graph_view>& views,
-                      const std::vector<int32_t>& Tb, long long tot_arcs) {
+int graph_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, T = a.T, C = a.C;
-  const long long per = (long long)T * C;
   ViterbiBufs v;
-  GTNB_TRY(viterbi_open(scope, a, &v));
+  GTNB_TRY(viterbi_open(scope, a, gb, &v));
   bool implicit = ctx->use_implicit;
   gtnb_lattice*& lat = scope.lattice();
   if (implicit) {
-    const int rc = compose_linear_impl(ctx, B, views.data(), B, 0, Tb.data(), C, v.e_dev, per, true, &lat, true,
-                                       a.arc_weights_on_device ? a.arc_weights : nullptr);
-    if (rc == GTNB_ERR_UNSUPPORTED) // does not fit the implicit layout: materialise
-      implicit = false;
-    else
-      GTNB_TRY(rc);
+    GTNB_TRY(implicit_or_materialise(compose_linear_impl(ctx, gb.B, gb.views.data(), gb.B, 0, gb.Tb.data(), gb.C,
+                                                         v.e_dev, (long long)gb.T * gb.C, true, &lat, true,
+                                                         gb.arc_weights_dev),
+                                     &implicit));
     implicit = implicit && implicit_trace_supported(lat);
   }
   if (implicit) {
     GTNB_TRY(launch_implicit_forward(ctx, lat, v.status, 0, -1, /*tropical=*/true));
-    GTNB_TRY(launch_implicit_trace(ctx, lat, v.status, v.p_dev, v.a_dev, v.s_dev, T));
+    GTNB_TRY(launch_implicit_trace(ctx, lat, v.status, v.p_dev, v.a_dev, v.s_dev, gb.T));
   }
-  return viterbi_finish(scope, a, Tb, implicit, v, [&](const std::vector<int>& which) {
-    return graph_viterbi_exact(scope, a, views, Tb, tot_arcs, v.e_dev, which, v.p_dev, v.a_dev, v.s_dev);
+  return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
+    std::vector<float> host_w;
+    std::vector<gtnb_graph_view> views;
+    GTNB_TRY(gb.host_views(ctx, &host_w, &views));
+    return graph_viterbi_exact(scope, gb, views, v, which);
   });
 }
 
@@ -1994,20 +1982,15 @@ extern "C" int gtnb_graph_viterbi(
     gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
     const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, int32_t* paths, int32_t* arcs,
     float* scores, int outputs_on_device) {
-  const char* fn = "gtnb_graph_viterbi";
-  if (!ctx || B < 0 || T < 0 || C <= 0 || (B > 0 && (!emissions || !graphs)))
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
-  std::vector<int32_t> Tb;
-  std::vector<gtnb_graph_view> views;
-  long long tot_arcs = 0;
-  GTNB_TRY(parse_graphs(ctx, fn, B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
-                        &tot_arcs));
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, "gtnb_graph_viterbi", B, T, C, emissions, graphs, true, input_lens, arc_weights,
+                        arc_weights_on_device, &gb, no_own_checks));
   if (B == 0) return GTNB_OK;
   GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
   CallScope scope(ctx);
-  const GraphViterbiArgs a{B, T, C, emissions, emissions_on_device, arc_weights, arc_weights_on_device,
-                           paths, arcs, scores, outputs_on_device};
-  return graph_viterbi_run(scope, a, views, Tb, tot_arcs);
+  return graph_viterbi_run(scope, GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,
+                                                   outputs_on_device},
+                           gb);
 }
 
 /*
@@ -2021,34 +2004,27 @@ extern "C" int gtnb_graph_viterbi(
  */
 namespace {
 
-int graph_transitions_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a, bool bigram, const float* trans_w,
-                                    int trans_on_device, const std::vector<gtnb_graph_view>& views,
-                                    const std::vector<int32_t>& Tb, long long tot_arcs, const float* e_dev,
-                                    const std::vector<int>& which, int32_t* p_dev, int32_t* a_dev, float* s_dev) {
+int graph_transitions_viterbi_exact(CallScope& scope, const GraphBatch& gb, bool bigram, const float* trans_w,
+                                    int trans_on_device, const ViterbiBufs& vb, const std::vector<int>& which) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, C = a.C;
-  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
-  std::vector<float> W(n_trans), w_A;
+  const int B = gb.B, C = gb.C;
+  const long long n_trans = dense_trans_count(bigram, C);
+  std::vector<float> W(n_trans), host_w;
   GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
-  if (a.arc_weights && a.arc_weights_on_device) {
-    w_A.resize((size_t)std::max(tot_arcs, 1ll));
-    GTNB_TRY(read_to_host(ctx, w_A.data(), a.arc_weights, 1, tot_arcs));
-  }
+  std::vector<gtnb_graph_view> views;
+  GTNB_TRY(gb.host_views(ctx, &host_w, &views));
   HostGraph G;
   dense_graph(bigram, C, W.data(), &G, nullptr);
   const gtnb_graph_view gv = G.view();
   // A'_b: A_b with its ilabels replaced by the arc ids (A_b is matched on its olabels, so the composition is the
   // same); the pairs that can accept anything
-  std::vector<long long> first_arc;
-  std::vector<int32_t> iota;
-  arc_numbering(views, &first_arc, &iota);
+  const std::vector<int32_t> ids = arc_ids(views);
   std::vector<int> pairs;
   std::vector<gtnb_graph_view> first;
   for (int b : which) {
-    if (Tb[b] == 0 || views[b].num_nodes == 0) continue;
+    if (gb.Tb[b] == 0 || views[b].num_nodes == 0) continue;
     gtnb_graph_view v = views[b];
-    v.arc_ilabel = iota.data();
-    if (!w_A.empty()) v.weights = w_A.data() + first_arc[b];
+    v.arc_ilabel = ids.data();
     pairs.push_back(b);
     first.push_back(v);
   }
@@ -2096,45 +2072,36 @@ int graph_transitions_viterbi_exact(CallScope& scope, const GraphViterbiArgs& a,
     gtnb_composed_destroy(ctx, res);
     GTNB_TRY(rc);
   }
-  GraphViterbiArgs ca = a;
-  ca.arc_weights = nullptr; // the composed graphs carry their weights
-  return graph_viterbi_exact(scope, ca, cviews, Tb, 0, e_dev, which, p_dev, a_dev, s_dev, &arc_map);
+  return graph_viterbi_exact(scope, gb, cviews, vb, which, &arc_map);
 }
 
-int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, bool bigram, const float* trans_w,
-                                  int trans_on_device, const std::vector<gtnb_graph_view>& views,
-                                  const std::vector<int32_t>& Tb, long long tot_arcs) {
+int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, bool bigram,
+                                  const float* trans_w, int trans_on_device) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = a.B, T = a.T, C = a.C;
-  const long long per = (long long)T * C;
-  const long long n_trans = (bigram ? 0 : C) + (long long)C * C;
+  const int B = gb.B, T = gb.T, C = gb.C;
+  const long long n_trans = dense_trans_count(bigram, C);
   ViterbiBufs v;
-  GTNB_TRY(viterbi_open(scope, a, &v));
+  GTNB_TRY(viterbi_open(scope, a, gb, &v));
 
   // the loss's numerators (BIGRAM folded), whose shapes decide whether the device route can be taken
-  std::vector<ProductGraph> prods(B);
-  std::vector<SgDims> dims(B);
-  for (int b = 0; b < B; b++) {
-    build_product(views[b], C, bigram, /*fold=*/true, &prods[b]);
-    const ProductGraph& p = prods[b];
-    dims[b] = SgDims{(int)p.flags.size(), (int)p.src.size(), p.n_acc, /*all_valid=*/1, /*uniform=*/1, p.max_in,
-                     p.max_out};
-  }
-  bool implicit = ctx->use_implicit && implicit_dims_supported(dims.data(), B);
-  GraphNumerator num{prods, views, Tb, C, bigram, a.arc_weights && a.arc_weights_on_device ? a.arc_weights : nullptr,
-                     nullptr, 0, tot_arcs};
+  std::vector<ProductGraph> prods;
+  const bool fits = device_products(
+      gb, [&](const gtnb_graph_view& view, ProductGraph* p) { build_product(view, C, bigram, /*fold=*/true, p); },
+      &prods);
+  bool implicit = ctx->use_implicit && fits;
+  GraphNumerator num{gb, prods, (int)n_trans, nullptr, 0};
   gtnb_lattice*& lat = scope.lattice();
   if (implicit) {
-    GTNB_TRY(num.alloc(scope, v.e_dev, per, nullptr));
+    GTNB_TRY(num.alloc(scope, v.e_dev, (long long)T * C, nullptr));
     float *w_dev = nullptr, *tau = nullptr;
     long long* off = nullptr;
     GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, n_trans, &w_dev));
     if (bigram) GTNB_TRY(scope.alloc(&tau, C));
     // off: every utterance's first product arc, then its first A arc (launch_product_arc_map)
     std::vector<long long> off_h(2 * (size_t)B, 0);
-    for (int b = 1; b < B; b++) {
-      off_h[b] = off_h[b - 1] + (long long)prods[b - 1].src.size();
-      off_h[B + b] = off_h[B + b - 1] + views[b - 1].num_arcs;
+    for (int b = 0; b < B; b++) {
+      if (b > 0) off_h[b] = off_h[b - 1] + (long long)prods[b - 1].src.size();
+      off_h[B + b] = gb.first_arc[b];
     }
     if (v.a_dev) GTNB_TRY(scope.alloc(&off, 2ll * B));
     GTNB_TRY(stage_begin(ctx));
@@ -2143,11 +2110,7 @@ int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, b
     if (off) GTNB_TRY(stage_upload(ctx, off, off_h.data(), sizeof(long long) * 2 * B));
     GTNB_TRY(stage_end(ctx));
     if (bigram) GTNB_TRY(launch_ngram_tau(ctx, C, w_dev, tau));
-    const int rc = num.build(scope, lat, w_dev, tau);
-    if (rc == GTNB_ERR_UNSUPPORTED) // does not fit the implicit layout: materialise
-      implicit = false;
-    else
-      GTNB_TRY(rc);
+    GTNB_TRY(implicit_or_materialise(num.build(scope, lat, w_dev, tau), &implicit));
     implicit = implicit && implicit_trace_supported(lat);
     if (implicit) {
       GTNB_TRY(launch_implicit_forward(ctx, lat, v.status, 0, -1, /*tropical=*/true));
@@ -2155,9 +2118,8 @@ int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, b
       if (v.a_dev) GTNB_TRY(launch_product_arc_map(ctx, B, T, off, num.arc_of, v.a_dev));
     }
   }
-  return viterbi_finish(scope, a, Tb, implicit, v, [&](const std::vector<int>& which) {
-    return graph_transitions_viterbi_exact(scope, a, bigram, trans_w, trans_on_device, views, Tb, tot_arcs, v.e_dev,
-                                           which, v.p_dev, v.a_dev, v.s_dev);
+  return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
+    return graph_transitions_viterbi_exact(scope, gb, bigram, trans_w, trans_on_device, v, which);
   });
 }
 
@@ -2168,24 +2130,14 @@ extern "C" int gtnb_graph_transitions_viterbi(
     const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device, int kind,
     const float* trans_w, int trans_on_device, int32_t* paths, int32_t* arcs, float* scores, int outputs_on_device) {
   const char* fn = "gtnb_graph_transitions_viterbi";
-  if (!ctx || B < 0 || T < 0 || C <= 0 || !trans_w || (B > 0 && (!emissions || !graphs)))
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
-  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
-    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown graph kind");
-  if (C > kNgramMaxLabels)
-    return fail(ctx, GTNB_ERR_UNSUPPORTED,
-                std::string(fn) + ": C = " + std::to_string(C) + " labels; the product builder takes C <= " +
-                    std::to_string(kNgramMaxLabels));
-  std::vector<int32_t> Tb;
-  std::vector<gtnb_graph_view> views;
-  long long tot_arcs = 0;
-  GTNB_TRY(parse_graphs(ctx, fn, B, T, input_lens, graphs, arc_weights, arc_weights_on_device, &Tb, &views,
-                        &tot_arcs));
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, fn, B, T, C, emissions, graphs, trans_w != nullptr, input_lens, arc_weights,
+                        arc_weights_on_device, &gb, [&] { return check_dense_kind(ctx, fn, kind, C); }));
   if (B == 0) return GTNB_OK;
   GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
   CallScope scope(ctx);
-  const GraphViterbiArgs a{B, T, C, emissions, emissions_on_device, arc_weights, arc_weights_on_device,
-                           paths, arcs, scores, outputs_on_device};
-  return graph_transitions_viterbi_run(scope, a, kind == GTNB_DENSE_BIGRAM, trans_w, trans_on_device, views, Tb,
-                                       tot_arcs);
+  return graph_transitions_viterbi_run(scope,
+                                       GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,
+                                                        outputs_on_device},
+                                       gb, kind == GTNB_DENSE_BIGRAM, trans_w, trans_on_device);
 }

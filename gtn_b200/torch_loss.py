@@ -284,6 +284,73 @@ def _graph_view(g):
                           d["in_arcs"], d["out_ptr"], d["out_arcs"], d["start"], d["accept"])
 
 
+class _GraphCall:
+    """One batch of user graphs as the graph criteria and decoders hand it to the C ABI: the emissions (e, B, T, C),
+    the context of the current stream (g), input_lengths (il: a pointer or None), the graphs' views (kept alive here)
+    and their GraphView array (arr), the arc weights (w: a device pointer or None) and, with arc_grads and weights,
+    the buffer the call writes the weights' gradient into (ag) and the utterance of every arc (owner)."""
+
+    def __init__(self, emissions, graphs, weights, input_lengths, arc_grads):
+        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        self.e = e = emissions.contiguous()
+        B, T, Cn = e.shape
+        self.B, self.T, self.C = B, T, Cn
+        assert len(graphs) == B
+        self.views = [_graph_view(g) for g in graphs]
+        counts = [v.num_arcs for v, _ in self.views]
+        self.n_arcs = sum(counts)
+        self.arr = (capi.GraphView * max(B, 1))(*[v for v, _ in self.views])
+        self.weights = self.ag = self.owner = None
+        if weights is not None:
+            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
+            assert weights.numel() == self.n_arcs
+            self.weights = weights.detach().contiguous()
+            if arc_grads:
+                self.ag = torch.empty(max(self.n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
+                # utterance of every arc, for a per-utterance upstream gradient (reduction "none")
+                self.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(
+                    e.device)
+        self.w = None if self.weights is None else self.weights.data_ptr()
+        self.current = torch.cuda.current_stream(e.device)
+        self.g = _ctx_for(e.device, self.current.cuda_stream)
+        self.lengths = _lengths(input_lengths, B)
+        self.il = None if self.lengths is None else self.lengths.ctypes.data_as(capi._i32p)
+
+    def loss_output(self, ctx, losses, reduction, weights):
+        """the criterion's output from the B host losses; ctx keeps what _weight_backward needs"""
+        # (the arc gradient is computed here, neither an input nor an output: held on ctx)
+        ctx.ag = None if self.ag is None else self.ag[:self.n_arcs].view_as(weights)
+        ctx.owner = self.owner
+        ctx.reduction = reduction
+        ctx.B = self.B
+        out = torch.from_numpy(losses).to(self.e.device)
+        return out.mean() if reduction == "mean" else out
+
+    def viterbi(self, call):
+        """(paths, scores, arcs) of call(paths, arcs, scores), a graph Viterbi C call on device pointers"""
+        B, T, device = self.B, self.T, self.e.device
+        paths = torch.empty((B, T), dtype=torch.int32, device=device)  # every entry is written by the call
+        arcs = torch.empty((B, T), dtype=torch.int32, device=device)
+        scores = torch.empty(B, dtype=torch.float32, device=device)
+        # the context's stream is the current stream unless that is the legacy default stream: order the two both ways
+        ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(self.g.h), device=device)
+        ctx_stream.wait_stream(self.current)
+        self.g._check(call(paths.data_ptr(), arcs.data_ptr(), scores.data_ptr()))
+        self.current.wait_stream(ctx_stream)
+        return paths, scores, arcs
+
+
+def _weight_backward(ctx, grad_output):
+    """the arc-weight gradient of the graph criteria times the upstream gradient (None without weights)"""
+    ag = ctx.ag
+    if ag is None:
+        return None
+    if ctx.reduction == "mean":
+        return ag * (grad_output / ctx.B)
+    # reduction "none": every graph belongs to one utterance, so its arcs take that utterance's upstream gradient
+    return ag * grad_output.reshape(-1)[ctx.owner].view_as(ag)
+
+
 class GraphLossFunction(torch.autograd.Function):
     """loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b)) with one target graph A_b per utterance
     (bindings/python/examples/pytorch_loss.py, the word-decomposition examples), through gtnb_graph_loss.
@@ -299,53 +366,44 @@ class GraphLossFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, emissions, weights, graphs, input_lengths=None, reduction="mean"):
-        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
-        e = emissions.contiguous()
-        B, T, Cn = e.shape
-        assert len(graphs) == B
-        views = [_graph_view(g) for g in graphs]
-        counts = [v.num_arcs for v, _ in views]
-        n_arcs = sum(counts)
-        arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
-        w = ag = None
-        if weights is not None:
-            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
-            assert weights.numel() == n_arcs
-            w = weights.detach().contiguous()
-            ag = torch.empty(max(n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
-        stream = torch.cuda.current_stream(e.device).cuda_stream
-        g = _ctx_for(e.device, stream)
-        il = _lengths(input_lengths, B)
-        losses = np.zeros(B, np.float32)
-        grad = torch.empty_like(e)  # every row is written by the call
-        g._check(capi.lib().gtnb_graph_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
-            None if w is None else w.data_ptr(), 1, losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
-            None if ag is None else ag.data_ptr(), 1))
-        out = torch.from_numpy(losses).to(e.device)
-        if ag is not None:
-            ag = ag[:n_arcs].view_as(weights)
-            # utterance of every arc, for a per-utterance upstream gradient (reduction "none")
-            ctx.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(e.device)
-        ctx.save_for_backward(grad, ag)
-        ctx.reduction = reduction
-        ctx.B = B
-        return out.mean() if reduction == "mean" else out
+        c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=True)
+        losses = np.zeros(c.B, np.float32)
+        grad = torch.empty_like(c.e)  # every row is written by the call
+        c.g._check(capi.lib().gtnb_graph_loss(
+            c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, losses.ctypes.data_as(capi._f32p),
+            grad.data_ptr(), 1, None if c.ag is None else c.ag.data_ptr(), 1))
+        ctx.save_for_backward(grad)
+        return c.loss_output(ctx, losses, reduction, weights)
 
     @staticmethod
     def backward(ctx, grad_output):
-        grad, ag = ctx.saved_tensors
+        (grad,) = ctx.saved_tensors
         if ctx.reduction == "mean":
-            scale = grad_output / ctx.B
-            return grad * scale, None if ag is None else ag * scale, None, None, None
-        # reduction "none": every graph belongs to one utterance, so its arcs take that utterance's upstream gradient
-        go = grad_output.reshape(-1)
-        wg = None if ag is None else ag * go[ctx.owner].view_as(ag)
-        return grad * go.view(-1, 1, 1), wg, None, None, None
+            egrad = grad * (grad_output / ctx.B)
+        else:
+            egrad = grad * grad_output.reshape(-1).view(-1, 1, 1)
+        return egrad, _weight_backward(ctx, grad_output), None, None, None
 
 
 def graph_loss(emissions, graphs, input_lengths=None, weights=None, reduction="mean"):
     return GraphLossFunction.apply(emissions, weights, graphs, input_lengths, reduction)
+
+
+def _transitions_forward(ctx, emissions, transitions, weights, graphs, input_lengths, reduction, allreduce, n_tg,
+                         call):
+    """the forward of graph_transitions_loss and sparse_transitions_loss: call(c, tw, losses, grad, tg) makes the C
+    call, with a transition gradient buffer of n_tg floats"""
+    c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=True)
+    assert transitions.is_cuda and transitions.device == c.e.device and transitions.dtype == torch.float32
+    tw = transitions.detach().contiguous()
+    losses = np.zeros(c.B, np.float32)
+    grad = torch.empty_like(c.e)  # every row is written by the call
+    tg = torch.empty(n_tg, dtype=torch.float32, device=c.e.device)
+    c.g._check(call(c, tw, losses, grad, tg))
+    tg = tg[:transitions.numel()].view_as(transitions)
+    _allreduce_transitions(ctx, tg, allreduce)
+    ctx.save_for_backward(grad, tg)
+    return c.loss_output(ctx, losses, reduction, weights)
 
 
 class GraphTransitionsLossFunction(torch.autograd.Function):
@@ -363,58 +421,21 @@ class GraphTransitionsLossFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, emissions, transitions, weights, graphs, kind="asg", input_lengths=None, reduction="mean",
                 allreduce=True):
-        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
         assert kind in ("asg", "bigram")
-        e = emissions.contiguous()
-        B, T, Cn = e.shape
-        assert len(graphs) == B
-        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
         kid = capi.DENSE_BIGRAM if kind == "bigram" else capi.DENSE_ASG
+        Cn = emissions.shape[-1]
         assert transitions.numel() == (Cn * Cn if kid == capi.DENSE_BIGRAM else Cn + Cn * Cn)
-        tw = transitions.detach().contiguous()
-        views = [_graph_view(g) for g in graphs]
-        counts = [v.num_arcs for v, _ in views]
-        n_arcs = sum(counts)
-        arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
-        w = ag = None
-        if weights is not None:
-            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
-            assert weights.numel() == n_arcs
-            w = weights.detach().contiguous()
-            ag = torch.empty(max(n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
-        stream = torch.cuda.current_stream(e.device).cuda_stream
-        g = _ctx_for(e.device, stream)
-        il = _lengths(input_lengths, B)
-        losses = np.zeros(B, np.float32)
-        grad = torch.empty_like(e)  # every row is written by the call
-        tg = torch.empty(transitions.numel(), dtype=torch.float32, device=e.device)
-        g._check(capi.lib().gtnb_graph_transitions_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
-            None if w is None else w.data_ptr(), 1, kid, tw.data_ptr(), 1, losses.ctypes.data_as(capi._f32p),
-            grad.data_ptr(), 1, None if ag is None else ag.data_ptr(), 1, tg.data_ptr(), 1))
-        tg = tg.view_as(transitions)
-        _allreduce_transitions(ctx, tg, allreduce)
-        out = torch.from_numpy(losses).to(e.device)
-        if ag is not None:
-            ag = ag[:n_arcs].view_as(weights)
-            ctx.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(e.device)
-        ctx.save_for_backward(grad, tg)
-        ctx.ag = ag  # (computed here, neither an input nor an output: held on ctx)
-        ctx.reduction = reduction
-        ctx.B = B
-        return out.mean() if reduction == "mean" else out
+        return _transitions_forward(
+            ctx, emissions, transitions, weights, graphs, input_lengths, reduction, allreduce, transitions.numel(),
+            lambda c, tw, losses, grad, tg: capi.lib().gtnb_graph_transitions_loss(
+                c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, kid, tw.data_ptr(), 1,
+                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if c.ag is None else c.ag.data_ptr(), 1,
+                tg.data_ptr(), 1))
 
     @staticmethod
     def backward(ctx, grad_output):
         egrad, tgrad = _transition_backward(ctx, grad_output)
-        ag = ctx.ag
-        if ag is None:
-            wg = None
-        elif ctx.reduction == "mean":
-            wg = ag * (grad_output / ctx.B)
-        else:  # every graph belongs to one utterance: its arcs take that utterance's upstream gradient
-            wg = ag * grad_output.reshape(-1)[ctx.owner].view_as(ag)
-        return egrad, tgrad, wg, None, None, None, None, None
+        return egrad, tgrad, _weight_backward(ctx, grad_output), None, None, None, None, None
 
 
 def graph_transitions_loss(emissions, transitions, graphs, kind="asg", input_lengths=None, weights=None,
@@ -435,46 +456,15 @@ class SparseTransitionsLossFunction(GraphTransitionsLossFunction):
     @staticmethod
     def forward(ctx, emissions, transitions, weights, graphs, transitions_graph, input_lengths=None, reduction="mean",
                 allreduce=True):
-        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
-        e = emissions.contiguous()
-        B, T, Cn = e.shape
-        assert len(graphs) == B
         gv = _graph_view(transitions_graph)
-        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
         assert transitions.numel() == gv[0].num_arcs
-        tw = transitions.detach().contiguous()
-        views = [_graph_view(g) for g in graphs]
-        counts = [v.num_arcs for v, _ in views]
-        n_arcs = sum(counts)
-        arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
-        w = ag = None
-        if weights is not None:
-            assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
-            assert weights.numel() == n_arcs
-            w = weights.detach().contiguous()
-            ag = torch.empty(max(n_arcs, 1), dtype=torch.float32, device=e.device)  # written by the call
-        stream = torch.cuda.current_stream(e.device).cuda_stream
-        g = _ctx_for(e.device, stream)
-        il = _lengths(input_lengths, B)
-        losses = np.zeros(B, np.float32)
-        grad = torch.empty_like(e)  # every row is written by the call
-        tg = torch.empty(max(transitions.numel(), 1), dtype=torch.float32, device=e.device)
-        g._check(capi.lib().gtnb_sparse_transitions_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
-            None if w is None else w.data_ptr(), 1, C.byref(gv[0]), tw.data_ptr(), 1,
-            losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if ag is None else ag.data_ptr(), 1,
-            tg.data_ptr(), 1))
-        tg = tg[:transitions.numel()].view_as(transitions)
-        _allreduce_transitions(ctx, tg, allreduce)
-        out = torch.from_numpy(losses).to(e.device)
-        if ag is not None:
-            ag = ag[:n_arcs].view_as(weights)
-            ctx.owner = torch.repeat_interleave(torch.arange(B), torch.tensor(counts, dtype=torch.long)).to(e.device)
-        ctx.save_for_backward(grad, tg)
-        ctx.ag = ag  # (computed here, neither an input nor an output: held on ctx)
-        ctx.reduction = reduction
-        ctx.B = B
-        return out.mean() if reduction == "mean" else out
+        return _transitions_forward(
+            ctx, emissions, transitions, weights, graphs, input_lengths, reduction, allreduce,
+            max(transitions.numel(), 1),
+            lambda c, tw, losses, grad, tg: capi.lib().gtnb_sparse_transitions_loss(
+                c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1,
+                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if c.ag is None else c.ag.data_ptr(), 1,
+                tg.data_ptr(), 1))
 
 
 def sparse_transitions_loss(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
@@ -496,32 +486,9 @@ def graph_viterbi(emissions, graphs, input_lengths=None, weights=None):
     emissions' device, written on the current stream.  Ties are broken as the reference breaks them.
     collapse(paths, blank) turns the paths into transcripts.
     """
-    assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
-    e = emissions.contiguous()
-    B, T, Cn = e.shape
-    assert len(graphs) == B
-    views = [_graph_view(g) for g in graphs]
-    n_arcs = sum(v.num_arcs for v, _ in views)
-    arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
-    w = None
-    if weights is not None:
-        assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
-        assert weights.numel() == n_arcs
-        w = weights.detach().contiguous()
-    current = torch.cuda.current_stream(e.device)
-    g = _ctx_for(e.device, current.cuda_stream)
-    il = _lengths(input_lengths, B)
-    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)  # every entry is written by the call
-    arcs = torch.empty((B, T), dtype=torch.int32, device=e.device)
-    scores = torch.empty(B, dtype=torch.float32, device=e.device)
-    # the context's stream is the current stream unless that is the legacy default stream: order the two both ways
-    ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(g.h), device=e.device)
-    ctx_stream.wait_stream(current)
-    g._check(capi.lib().gtnb_graph_viterbi(
-        g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
-        None if w is None else w.data_ptr(), 1, paths.data_ptr(), arcs.data_ptr(), scores.data_ptr(), 1))
-    current.wait_stream(ctx_stream)
-    return paths, scores, arcs
+    c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=False)
+    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_graph_viterbi(
+        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, paths, arcs, scores, 1))
 
 
 @torch.no_grad()
@@ -536,35 +503,11 @@ def graph_transitions_viterbi(emissions, transitions, graphs, kind="asg", input_
     CUDA tensors on the emissions' device, written on the current stream.  Ties are broken as the reference breaks
     them.  collapse(paths, blank) turns the paths into transcripts.
     """
-    assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
     assert kind in ("asg", "bigram")
-    e = emissions.contiguous()
-    B, T, Cn = e.shape
-    assert len(graphs) == B
-    assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+    c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=False)
+    assert transitions.is_cuda and transitions.device == c.e.device and transitions.dtype == torch.float32
     kid = capi.DENSE_BIGRAM if kind == "bigram" else capi.DENSE_ASG
-    assert transitions.numel() == (Cn * Cn if kid == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+    assert transitions.numel() == (c.C * c.C if kid == capi.DENSE_BIGRAM else c.C + c.C * c.C)
     tw = transitions.detach().contiguous()
-    views = [_graph_view(g) for g in graphs]
-    n_arcs = sum(v.num_arcs for v, _ in views)
-    arr = (capi.GraphView * max(B, 1))(*[v for v, _ in views])
-    w = None
-    if weights is not None:
-        assert weights.is_cuda and weights.device == e.device and weights.dtype == torch.float32
-        assert weights.numel() == n_arcs
-        w = weights.detach().contiguous()
-    current = torch.cuda.current_stream(e.device)
-    g = _ctx_for(e.device, current.cuda_stream)
-    il = _lengths(input_lengths, B)
-    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)  # every entry is written by the call
-    arcs = torch.empty((B, T), dtype=torch.int32, device=e.device)
-    scores = torch.empty(B, dtype=torch.float32, device=e.device)
-    # the context's stream is the current stream unless that is the legacy default stream: order the two both ways
-    ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(g.h), device=e.device)
-    ctx_stream.wait_stream(current)
-    g._check(capi.lib().gtnb_graph_transitions_viterbi(
-        g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), arr,
-        None if w is None else w.data_ptr(), 1, kid, tw.data_ptr(), 1, paths.data_ptr(), arcs.data_ptr(),
-        scores.data_ptr(), 1))
-    current.wait_stream(ctx_stream)
-    return paths, scores, arcs
+    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_graph_transitions_viterbi(
+        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, kid, tw.data_ptr(), 1, paths, arcs, scores, 1))
