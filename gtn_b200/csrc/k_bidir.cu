@@ -28,7 +28,8 @@
  *                 - PAIR (gtnb_ctc_loss with a gradient, C = 64 / 128): the graphs are CTC target graphs, taken from
  *                   the targets themselves (no ctc_build launch); thread t owns label 2t-1 AND blank 2t, keeps
  *                   their scores in registers, reads its neighbour pair with one LDS.64 (A) / one LDS (B), writes
- *                   one STS.64 / STG.64; the blank's two-term logsumexp costs 2 MUFU, the label's 3 (max + lg2(1 +
+ *                   one STS.64 (A) / STS (B) and saves the label's score alone (one STG); the blank's two-term
+ *                   logsumexp costs 2 MUFU, the label's 3 (max + lg2(1 +
  *                   two terms)), the blank's posterior is never formed (complement label).  <= 4 warps, 26 / 31
  *                   SASS instructions per PAIR and level (the one-node-per-thread kernels: 2 x 19 / 2 x 24).
  *                 - QUAD (loss-only calls): one node warp, four pairs per thread, neighbours by shuffle, no barrier
@@ -51,9 +52,14 @@
  *                 nothing: its mass is the level's mass minus everybody else's; no floating-point atomics
  *                 anywhere -- and the finished gradient row leaves as one 16-byte store per lane.
  *
- * What bounds it (scripts/ubench/chain*.cu measure the pieces): not HBM and not one pipe, but the dependent chain of a
- * level, several CTAs deep on an SM: 512 CTAs at B = 256 do not divide evenly over the 132 SMs of an H100, and the
- * SMs that hold the most CTAs finish last.
+ * What bounds it: at the benchmark's shape (B = 256, T = 1000, C = 64, U = 100) the three node-warp variants, whose
+ * chains differ widely (7 warps and a barrier, 4 warps and a barrier, 1 warp and none), all took about the same
+ * time; what they share is the saved-score traffic, 229 MB written in phase 1 and read back in phase 2 at the fixed
+ * pitch, about two thirds of everything the kernel moves (counted from the shapes).  Saving the PAIR kernels' label
+ * scores alone (the blank's are read only at the meeting level) halved that traffic and cut the kernel from 0.376 to
+ * 0.315 ms (medians, H100 80GB HBM3 at a 400 W limit, DESIGN.md).  How the rest of a level's time splits has not
+ * been measured; the dependent chain of a level, several CTAs deep on an SM, is the likeliest bound
+ * (scripts/ubench/chain*.cu time its pieces).
  *
  * Numerics: gamma's exponent is evaluated as ((x - Zh) + y) - zsub with x the larger of alpha/beta: both
  * subtractions are exact or nearly so (Sterbenz), so the posterior carries only the rounding error the
@@ -98,6 +104,8 @@ constexpr int kIntMin = -2147483647 - 1;
 // overflow area of a posterior row all have this many floats, whatever the utterance's node count -- which makes
 // every per-level address of the node warps base + compile-time constant (no pointer arithmetic on the chain)
 constexpr int kFixedPitch = 32 * kMaxNodeWarps;
+// PAIR kernels: floats per saved LABEL row (one per pair, <= 112 pairs); see pair_role for the block layout
+constexpr int kHalfPitch = kFixedPitch / 2;
 
 struct Layout {
   int off_ring, off_e, off_o, off_g, off_od, off_seg, off_perm, off_nlab, off_hlist, off_red, off_redi,
@@ -145,6 +153,7 @@ struct Params {
   const float* sg_in_w;
   const float* emissions;
   float* saved; // [node_base + f * pitch + u]: alpha_{f+1} for f < M (written by A), beta_{f+1} for f >= M (by B)
+                // (PAIR kernels: label scores only, see pair_role)
   float* boff; // [utterance][2][nblk_cap][4]: the score offset in effect for the rows of each block, per CTA
   float* out_scores; // [B] forwardScore of the lattice (natural log)
   float* zparts; // [2B * kHelpers] forwardScore(emissions): the part each helper warp of the pair of CTAs summed
@@ -519,13 +528,17 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
  * arc from label 2t-3 unless the label repeats).  The PAIR kernels give thread t BOTH nodes (2t-1, 2t):
  *   - half the node warps (4 instead of 7 at U = 100) and half the barrier arrivals per level;
  *   - the thread's own scores stay in registers; what it needs from its neighbour is ONE LDS.64 (A: the pair
- *     t-1) or one LDS (B: the label of pair t+1) instead of six loads, and its two results leave as one
- *     STS.64 / STG.64;
+ *     t-1) or one LDS (B: the label of pair t+1) instead of six loads, its two results go to the chain row as
+ *     one STS.64 (B: one STS, the label's), and only the label's is saved (one STG);
  *   - the blank's logsumexp has two terms: max + lg2(1 + 2^-|a-b|), 2 MUFU instead of 4;
  *   - the blank's posterior is never formed: blank is the complement label of the helper warps.
  * 28 / 34 SASS instructions per PAIR and level instead of 2 x 19 / 2 x 24, 6 / 7 MUFU instead of 8 / 10.
- * Row layouts: slot(node n) = n + 1 in the saved-score rows (pair t = floats 2t, 2t+1: 8-byte aligned), n + 3 in
- * the chain rows (pair t-1 of thread 0 and the label beyond the last pair read the row's kNeg).
+ * Row layouts: slot(node n) = n + 3 in the chain rows (pair t-1 of thread 0 and the label beyond the last pair read
+ * the row's kNeg).  Saved scores: the partner reads a blank score only at the meeting level (Z); every other level
+ * it reads the label's alone (blank is the complement label), so the saved rows hold LABEL scores only, kHalfPitch
+ * floats per row, pair t at float t: block j of n rows starts at float j * kBlk * kFixedPitch as it always did, its
+ * label rows take the first n * kHalfPitch floats, and -- in the block of the meeting level only -- the meeting
+ * row's blank scores follow them.  Half the saved-score traffic of full rows, in HBM both ways.
  */
 /* start / accept flags of node n of a CTC target graph with N1 = 2U + 1 nodes (benchmarks/ctc.cpp:43-44): the PAIR /
  * QUAD kernels take the graph from the target itself and never read ctc_build_kernel's tables */
@@ -544,7 +557,8 @@ struct PairState {
   uint32_t ea_l, ea_b; // emissions of the label / of blank in the current stage, first row of the block
   uint32_t oa; // the partner's score of this thread's label node, first row of the block
   uint32_t ga; // where the label's posterior goes
-  float* gs; // where the pair's scores are saved (phase 1)
+  float* gs; // where the label's score is saved (phase 1), first row of the block
+  float lastb; // phase 1: the saved blank score of the block's last level (stored only at the meeting level)
   float adj, D, Zh, zsub, Zl, Dc;
   uint32_t redi;
   bool skip; // A: label 2t-1 has the skip in-arc; B: label 2t+1 has it (= this thread's label has the skip out-arc)
@@ -577,10 +591,13 @@ __device__ __forceinline__ void pair_step(PairState& ps, const NodeUni& un, int 
     sts_f32(ps.qc + ps.t8 + 8u, ps.al); // only the label is read by a neighbour
   if (PH == 2)
     sts_f32(ps.ga + (uint32_t)(rr * SD::g4(un)),
-        ex2(((val_l - ps.Zh) + lds_f32(ps.oa + (uint32_t)(rr * SD::p4(un)))) - ps.zsub));
+        ex2(((val_l - ps.Zh) + lds_f32(ps.oa + (uint32_t)(rr * 4 * kHalfPitch))) - ps.zsub));
   if (last) publish_block_max(ps, fmaxf(ps.al, ps.ab));
   bar_named(1, un.nact);
-  if (PH == 1) stg_v2_f32(ps.gs + rr * SD::pitch(un), val_l, val_b);
+  if (PH == 1) {
+    stg_f32(ps.gs + rr * kHalfPitch, val_l);
+    if (last) ps.lastb = val_b;
+  }
   const uint32_t t = ps.pc;
   ps.pc = ps.qc;
   ps.qc = t;
@@ -595,14 +612,14 @@ __device__ __forceinline__ void pair_rows(PairState& ps, const NodeUni& un, int 
 #pragma unroll 1
     for (int r = 0; r < n; r++) pair_step<DIR, PH, NQ>(ps, un, r, r == n - 1);
   }
-  if (PH == 1) ps.gs += (DIR ? -n : n) * Strd<NQ, true>::pitch(un);
 }
 
-/* the first level of phase 2 (see node_first_phase2): Z over BOTH nodes of every pair */
+/* the first level of phase 2 (see node_first_phase2): Z over BOTH nodes of every pair; ob: the partner's blank
+ * score of this pair at this level */
 template <int DIR, int NQ>
 __device__ __forceinline__ void pair_first_phase2(
     PairState& ps, const NodeUni& un, bool act_l, bool act_b, uint32_t red, int warp, int nwarps, float doth, bool last,
-    float* z_out, uint32_t feas_a, bool want_g) {
+    float* z_out, uint32_t feas_a, bool want_g, uint32_t ob) {
   using SD = Strd<NQ, true>;
   const float xl = lds_f32(ps.ea_l), xb = lds_f32(ps.ea_b);
   ps.ea_l += DIR ? -SD::c4(un) : SD::c4(un);
@@ -626,7 +643,7 @@ __device__ __forceinline__ void pair_first_phase2(
     sts_v2_f32(ps.qc + ps.t8 + 8u, ps.al, ps.ab);
   else
     sts_f32(ps.qc + ps.t8 + 8u, ps.al);
-  const f32x2 o = lds_v2_f32(ps.oa); // the partner's scores of (label, blank)
+  const f32x2 o = {lds_f32(ps.oa), lds_f32(ob)}; // the partner's scores of (label, blank)
   // TwoSum (Knuth) of both: hi + lo == val + o exactly
   const float hl = val_l + o.x, bl = hl - val_l, ll = (val_l - (hl - bl)) + (o.x - bl);
   const float hb = val_b + o.y, bb = hb - val_b, lb = (val_b - (hb - bb)) + (o.y - bb);
@@ -646,7 +663,7 @@ __device__ __forceinline__ void pair_first_phase2(
     sts_f32(ps.ga, ex2(((val_l - ps.Zh) + o.x) - ps.zsub));
     ps.ga += DIR ? -SD::g4(un) : SD::g4(un);
   }
-  ps.oa += DIR ? -SD::p4(un) : SD::p4(un);
+  ps.oa += DIR ? -4 * kHalfPitch : 4 * kHalfPitch;
   if (last) publish_block_max(ps, fmaxf(ps.al, ps.ab));
   bar_named(1, un.nact);
   const uint32_t t = ps.pc;
@@ -671,6 +688,10 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
   const uint32_t e_row0_l = cx.e_base + cx.lab4 + dir_off; // cx.lab4: this thread's label
   const uint32_t e_row0_b = cx.e_base + cx.blank4 + dir_off;
   const bool act_l = act && has_label;
+  // saved scores (see the layout above): this pair's label in row 0 of block j.  The meeting level is the last one of
+  // the CTA's last phase-1 block (A: the last row of a full block; B: row 0); its blank scores go behind that block's
+  // n label rows
+  auto label_at = [&](int j) { return cx.saved + (long long)j * (kBlk * kFixedPitch) + tp; };
   int v = 0;
   if (DIR == 0) {
     // level 0: start nodes carry the implicit 0 (shortest.cpp:129-135)
@@ -678,15 +699,16 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     ps.ab = (ctc_flags(2 * tp, cx.N1) & 1) ? 0.0f : kNeg;
     sts_v2_f32(ps.pc + ps.t8 + 8u, ps.al, ps.ab);
     bar_named(1, nact);
-    ps.gs = cx.saved + 2 * tp;
     for (; v < cx.n_ph1; v++) {
       const int s = v & (kSE - 1);
       mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
       ps.ea_l = e_row0_l + (uint32_t)(s * cx.e_stage_bytes);
       ps.ea_b = e_row0_b + (uint32_t)(s * cx.e_stage_bytes);
+      ps.gs = label_at(v);
       if (v > 0) fetch_block_adjust(ps);
       if (tid == 0) stg_f32(cx.boff_own + 4 * v, ps.D);
       pair_rows<0, 1, NQ>(ps, un, kBlk);
+      if (v == cx.n_ph1 - 1) stg_f32(label_at(v) + kBlk * kHalfPitch, ps.lastb);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
     }
@@ -706,13 +728,15 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       ps.al = val_l + el;
       ps.ab = val_b + eb;
       sts_f32(ps.pc + ps.t8 + 8u, ps.al); // written to the row the first step READS
-      ps.gs = cx.saved + (long long)(cx.T - 1) * cx.pitch + 2 * tp;
+      ps.gs = label_at(j0) + (n0 - 1) * kHalfPitch;
+      ps.lastb = val_b;
       if (n0 == 1) publish_block_max(ps, fmaxf(ps.al, ps.ab));
       bar_named(1, nact);
-      stg_v2_f32(ps.gs, val_l, val_b);
-      ps.gs -= un.pitch;
+      stg_f32(ps.gs, val_l);
+      ps.gs -= kHalfPitch;
     }
     pair_rows<1, 1, NQ>(ps, un, n0 - 1);
+    if (cx.n_ph1 == 1) stg_f32(label_at(j0) + n0 * kHalfPitch, ps.lastb);
     __syncwarp();
     if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, 0), arr1);
     for (v = 1; v < cx.n_ph1; v++) {
@@ -720,9 +744,11 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
       ps.ea_l = e_row0_l + (uint32_t)(s * cx.e_stage_bytes);
       ps.ea_b = e_row0_b + (uint32_t)(s * cx.e_stage_bytes);
+      ps.gs = label_at(cx.nblk - 1 - v) + (kBlk - 1) * kHalfPitch;
       fetch_block_adjust(ps);
       if (tid == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), ps.D);
       pair_rows<1, 1, NQ>(ps, un, kBlk);
+      if (v == cx.n_ph1 - 1) stg_f32(label_at(cx.nblk - 1 - v) + kBlk * kHalfPitch, ps.lastb);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
     }
@@ -730,7 +756,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
   cluster_sync_all();
   // ---- phase 2
   if (cx.n_ph2 <= 0) return;
-  const uint32_t o_row0 = cx.o_base + ps.t8 + (DIR ? (uint32_t)((kBlk - 1) * cx.pitch * 4) : 0u);
+  const uint32_t o_row0 = cx.o_base + 4u * (uint32_t)tp + (DIR ? (uint32_t)((kBlk - 1) * kHalfPitch * 4) : 0u);
   uint32_t g_row0 = 0;
   int g_stride = 0;
   if (cx.want_g) {
@@ -753,8 +779,10 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     if (v > 0) fetch_block_adjust(ps);
     const float doth = lds_f32(cx.od_base + 16u * so);
     if (v2 == 0) {
+      // the meeting row's blank scores follow the block's nfr label rows (B reads row kBlk - 1, A row 0)
+      const uint32_t ob = ps.oa + (uint32_t)((DIR ? 1 : nfr) * kHalfPitch * 4);
       pair_first_phase2<DIR, NQ>(ps, un, act_l, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
-                                 DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.want_g);
+                                 DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.want_g, ob);
       if (cx.want_g) pair_rows<DIR, 2, NQ>(ps, un, nfr - 1);
     } else {
       ps.zsub = ps.Zl - ((ps.D + doth) - ps.Dc);
@@ -1709,7 +1737,8 @@ __global__ void __launch_bounds__(
         }
         if (lane == 0) {
           if (v2 >= kSO) mbar_wait_suspend(o_empty(so), ((v2 / kSO) - 1) & 1);
-          const uint32_t bytes = (uint32_t)(rows_of(j) * pitch * 4);
+          // PAIR: the label rows, plus the meeting row's blank scores behind them in the first block
+          const uint32_t bytes = PAIR ? (uint32_t)((rows_of(j) + (v2 == 0)) * kHalfPitch * 4) : (uint32_t)(rows_of(j) * pitch * 4);
           mbar_expect_tx(o_full(so), bytes + 16u);
           bulk_g2s(o_base + (uint32_t)(so * L.o_stage_bytes), saved + (long long)j * kBlk * pitch, bytes, o_full(so));
           bulk_g2s(od_base + 16u * so, boff_oth + 4 * j, 16u, o_full(so));
