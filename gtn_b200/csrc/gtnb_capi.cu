@@ -301,12 +301,8 @@ int gtnb_ctx_set_flag(gtnb_ctx* ctx, const char* name, int value) {
     return GTNB_OK;
   }
   if (ctx && name && std::string(name) == "bidir_mode") {
-    if (value < -1 || value > 2) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctx_set_flag: bidir_mode is -1 (auto), 0, 1 or 2");
+    if (value < -1 || value > 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctx_set_flag: bidir_mode is -1 (default), 0 or 1");
     ctx->bidir_mode = value;
-    return GTNB_OK;
-  }
-  if (ctx && name && std::string(name) == "banded") {
-    ctx->use_banded = value;
     return GTNB_OK;
   }
   return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctx_set_flag: unknown flag");

@@ -369,13 +369,12 @@ int ctc_loss_run(
   GTNB_TRY(composed_alloc(ctx, B, dims.data(), B, 0, t.T(), C, e_dev, per, sgn, sga, &lat, implicit));
   pc.mark("alloc+meta");
   // the whole criterion in one launch per sub-batch (k_bidir.cu) when the batch qualifies
-  const bool bidir =
-      implicit && ctx->use_bidir && ctx->use_banded == 0 && bidir_supported(lat, e_dev, per, g.dev, per);
-  // PAIR / QUAD kernels (graphs from the targets, one launch): everything small goes through MAPPED pinned memory --
+  const bool bidir = implicit && ctx->use_bidir && bidir_supported(lat, e_dev, per, g.dev, per);
+  // PAIR kernels (graphs from the targets, one launch): everything small goes through MAPPED pinned memory --
   // the kernel reads the descriptors and targets in place and writes its results straight into the read-back
   // block; no upload, no memset, no download on the path (those enqueues were a large share of the host work)
-  const bool direct = implicit && ctx->use_bidir && ctx->use_banded == 0 && ctx->bidir_mode != 0 &&
-                      bidir_supported(lat, e_dev, per, g.dev, per) && bidir_takes_targets(lat, 1, blank);
+  const bool direct = implicit && ctx->use_bidir && ctx->bidir_mode != 0 &&
+                      bidir_supported(lat, e_dev, per, g.dev, per) && bidir_takes_targets(lat, blank);
   if (bidir && direct) {
     const long long zpb = 2ll * B * bidir_zparts();
     GTNB_TRY(readback_reserve(ctx, (zpb + 2ll * B) * sizeof(float)));
@@ -438,30 +437,19 @@ int ctc_loss_run(
   }
 
   // ctcGraph -> intersect(ctc, emissions) -> forwardScore -> backward(-1) -> compose gradFunc
-  // (k_bidir.cu's PAIR / QUAD kernels take the CTC target graphs from the targets themselves: no tables to build)
+  // (k_bidir.cu's PAIR kernels take the CTC target graphs from the targets themselves: no tables to build)
   if (!(bidir && direct))
     GTNB_TRY(launch_ctc_build(ctx, lat, small_dev, small_dev + tot_t, small_dev + tot_t + B, blank));
   const int32_t* bidir_targets = direct ? small_mapped : small_dev;
   if (implicit) {
-    // the sweeps: k_implicit.cu, or (experimental flag) the temporally blocked ones of k_banded.cu
-    const bool banded = ctx->use_banded != 0 && banded_supported(ctx, lat);
-    auto sweep_forward = [&](int b0, int nb) {
-      return banded ? launch_banded_forward(ctx, lat, status_dev, b0, nb)
-                    : launch_implicit_forward(ctx, lat, status_dev, b0, nb);
-    };
-    auto sweep_backward = [&](int b0, int nb) {
-      return banded ? launch_banded_backward(ctx, lat, deltas_dev, g.dev, per, b0, nb)
-                    : launch_implicit_backward(ctx, lat, deltas_dev, g.dev, per, b0, nb);
-    };
     // everything below only needs what is already enqueued on the main stream (graphs, staging,
     // the memset of the gradients) plus its own slice of the emissions
     cudaEvent_t ev_setup = ctx->side_events[K], ev_lin = ctx->side_events[K + 1];
     const int32_t* T_dev = small_dev + tot_t + 2ll * B;
     GTNB_CUDA(ctx, cudaEventRecord(ev_setup, ctx->stream));
     if (bidir && K == 1 && !h2d_event && !(grads && !grads_on_device)) {
-      GTNB_TRY(launch_bidir_ctc(ctx, lat, status_dev, zparts_dev, boff_dev, g.dev, per, 0, -1, /*zero_w=*/1,
-                                bidir_scores_dev, blank, bidir_targets, bidir_targets + tot_t,
-                                direct ? meta_mapped : nullptr));
+      GTNB_TRY(launch_bidir_ctc(ctx, lat, status_dev, zparts_dev, boff_dev, g.dev, per, 0, -1, bidir_scores_dev,
+                                blank, bidir_targets, bidir_targets + tot_t, direct ? meta_mapped : nullptr));
     } else if (!bidir && K == 1 && !h2d_event && !(grads && !grads_on_device)) {
       // forwardScore(emissions) and its +1 gradient beside the forward sweep
       GTNB_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ev_setup, 0));
@@ -471,9 +459,9 @@ int ctc_loss_run(
                                        input_lens ? 0 : 1, row_scratch));
       }
       GTNB_CUDA(ctx, cudaEventRecord(ev_lin, ctx->copy_stream));
-      GTNB_TRY(sweep_forward(0, -1));
+      GTNB_TRY(launch_implicit_forward(ctx, lat, status_dev));
       GTNB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_lin, 0));
-      if (grads) GTNB_TRY(sweep_backward(0, -1));
+      if (grads) GTNB_TRY(launch_implicit_backward(ctx, lat, deltas_dev, g.dev, per));
     } else {
       for (int k = 0; k < K; k++) {
         const int b0 = chunk_lo[k], nb = chunk_lo[k + 1] - chunk_lo[k];
@@ -483,16 +471,15 @@ int ctc_loss_run(
         {
           OnStream side(ctx, cs);
           if (bidir) {
-            GTNB_TRY(launch_bidir_ctc(ctx, lat, status_dev, zparts_dev, boff_dev, g.dev, per, b0, nb, /*zero_w=*/1,
-                                      bidir_scores_dev, blank, bidir_targets, bidir_targets + tot_t,
-                                      direct ? meta_mapped : nullptr));
+            GTNB_TRY(launch_bidir_ctc(ctx, lat, status_dev, zparts_dev, boff_dev, g.dev, per, b0, nb, bidir_scores_dev,
+                                      blank, bidir_targets, bidir_targets + tot_t, direct ? meta_mapped : nullptr));
           } else {
             GTNB_TRY(launch_linear_forward(ctx, nb, T_dev + b0, maxT, C, e_dev + (long long)b0 * per, per, 0,
                                            z_dev + b0, g.dev ? g.dev + (long long)b0 * per : nullptr, per, nullptr,
                                            1.0f, input_lens ? 0 : 1,
                                            row_scratch + (long long)b0 * std::max(maxT, 1)));
-            GTNB_TRY(sweep_forward(b0, nb));
-            if (grads) GTNB_TRY(sweep_backward(b0, nb));
+            GTNB_TRY(launch_implicit_forward(ctx, lat, status_dev, b0, nb));
+            if (grads) GTNB_TRY(launch_implicit_backward(ctx, lat, deltas_dev, g.dev, per, b0, nb));
           }
         }
         if (grads && !grads_on_device)

@@ -64,10 +64,9 @@ struct gtnb_ctx {
   };
   bool use_staged = true; // gtnb_ctx_set_flag("staged", 0) forces the generic kernels
   bool use_implicit = true; // gtnb_ctx_set_flag("implicit", 0): criteria materialise the lattice
-  int bidir_mode = -1; // k_bidir.cu on CTC graphs ("bidir_mode" flag): 1 PAIR kernels, 2 QUAD, 0 one node per thread; -1 (default) = PAIR with a gradient (within 2 % of QUAD on an H100, profiles/h100_variants.json), QUAD for loss-only calls (0.154 vs 0.168 ms)
+  int bidir_mode = -1; // k_bidir.cu on CTC graphs ("bidir_mode" flag): 0 one node per thread; 1 and -1 (default) the PAIR kernels, ahead of every other node-warp variant measured on an H100 with and without a gradient (profiles/h100_bidir_pair_saves.json)
   bool use_bidir = kBidirDefault; // gtnb_ctx_set_flag("bidir", 0): the CTC criterion takes the two sweeps of k_implicit.cu instead of the bidirectional kernel (k_bidir.cu)
   bool exact_ties = true; // gtnb_ctx_set_flag("exact_ties", 0) turns it off: composed lattices are put in the reference's relaxation order so that viterbiPath breaks exact ties like shortest.cpp:212-218 (k_order.cu)
-  int use_banded = 0; // gtnb_ctx_set_flag("banded", K): EXPERIMENTAL temporally blocked CTC sweeps (k_banded.cu), K frames per barrier
   // Call-scoped device arena (the criteria): while arena_on, dev_alloc bumps a pointer inside one cached
   // allocation instead of ~25 stream-ordered allocations per call (each a microsecond or two of host time
   // ahead of the first launch); everything allocated in the scope is released together when it ends.
@@ -323,19 +322,13 @@ int bidir_blocks(int max_T);
 int bidir_zparts(); // partial sums of forwardScore(emissions) per CTA
 int launch_bidir_ctc(
     gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, float* grad_emis,
-    int64_t grad_stride, int b0 = 0, int nb = -1, int zero_w = 0, float* out_scores_dev = nullptr,
+    int64_t grad_stride, int b0 = 0, int nb = -1, float* out_scores_dev = nullptr,
     int ctc_blank = -1, const int32_t* targets_dev = nullptr, const int32_t* tgt_off_dev = nullptr,
     const GraphMeta* meta_src = nullptr); // meta_src: the descriptors somewhere else than lat->meta (mapped host memory)
-// ctc_blank >= 0 + the targets: CTC target graphs, taken from the targets themselves (PAIR / QUAD kernels)
-bool bidir_takes_targets(const gtnb_lattice* lat, int zero_w, int ctc_blank);
+// ctc_blank >= 0 + the targets: CTC target graphs, taken from the targets themselves (PAIR kernels)
+bool bidir_takes_targets(const gtnb_lattice* lat, int ctc_blank);
 /* k_order.cu (experimental): a composed lattice's rows and accept list in the order the reference's shortestPath relaxes / creates them */
 int launch_relax_order(gtnb_ctx* ctx, gtnb_lattice* lat);
-/* k_banded.cu (experimental): same contract as the implicit sweeps, for band-shaped graph operands */
-bool banded_supported(const gtnb_ctx* ctx, const gtnb_lattice* lat);
-int launch_banded_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int b0 = 0, int nb = -1);
-int launch_banded_backward(
-    gtnb_ctx* ctx, gtnb_lattice* lat, const float* deltas_dev, float* grad_emis, int64_t grad_stride,
-    int b0 = 0, int nb = -1);
 int launch_implicit_backward(
     gtnb_ctx* ctx, gtnb_lattice* lat, const float* deltas_dev, float* grad_emis, int64_t grad_stride,
     int b0 = 0, int nb = -1, float* grad_graph = nullptr);

@@ -79,7 +79,7 @@ struct GraphMeta {
   int cap_N; // slab capacities
   int cap_A;
   int cap_L;
-  int tgt_off; // gtnb_ctc_loss: first label of this utterance in the concatenated targets (k_bidir.cu PAIR / QUAD)
+  int tgt_off; // gtnb_ctc_loss: first label of this utterance in the concatenated targets (k_bidir.cu PAIR)
   int pad_;
 };
 

@@ -24,16 +24,14 @@
  * 2T, and HBM traffic does not grow: each half of the saved scores is written once and read once.
  *
  * Inside a CTA (warp-specialised):
- *   node warps    the recursion.  Three variants (launch_bidir_ctc picks):
- *                 - PAIR (gtnb_ctc_loss with a gradient, C = 64 / 128): the graphs are CTC target graphs, taken from
+ *   node warps    the recursion.  Two variants (launch_bidir_ctc picks):
+ *                 - PAIR (gtnb_ctc_loss at C = 64 / 128): the graphs are CTC target graphs, taken from
  *                   the targets themselves (no ctc_build launch); thread t owns label 2t-1 AND blank 2t, keeps
  *                   their scores in registers, reads its neighbour pair with one LDS.64 (A) / one LDS (B), writes
  *                   one STS.64 (A) / STS (B) and saves the label's score alone (one STG); the blank's two-term
  *                   logsumexp costs 2 MUFU, the label's 3 (max + lg2(1 +
  *                   two terms)), the blank's posterior is never formed (complement label).  <= 4 warps, 26 / 31
  *                   SASS instructions per PAIR and level (the one-node-per-thread kernels: 2 x 19 / 2 x 24).
- *                 - QUAD (loss-only calls): one node warp, four pairs per thread, neighbours by shuffle, no barrier
- *                   on the chain at all.
  *                 - one node per thread (any graph in the envelope; <= 7 warps): per level 3 LDS of the neighbours'
  *                   scores (absent arcs read a slot that holds a large negative finite number, so there is no
  *                   -inf / NaN special casing on the chain), one STS, one named barrier.
@@ -52,12 +50,12 @@
  *                 nothing: its mass is the level's mass minus everybody else's; no floating-point atomics
  *                 anywhere -- and the finished gradient row leaves as one 16-byte store per lane.
  *
- * What bounds it: at the benchmark's shape (B = 256, T = 1000, C = 64, U = 100) the three node-warp variants, whose
- * chains differ widely (7 warps and a barrier, 4 warps and a barrier, 1 warp and none), all took about the same
- * time; what they share is the saved-score traffic, 229 MB written in phase 1 and read back in phase 2 at the fixed
- * pitch, about two thirds of everything the kernel moves (counted from the shapes).  Saving the PAIR kernels' label
- * scores alone (the blank's are read only at the meeting level) halved that traffic and cut the kernel from 0.376 to
- * 0.315 ms (medians, H100 80GB HBM3 at a 400 W limit, DESIGN.md).  How the rest of a level's time splits has not
+ * What bounds it: at the benchmark's shape (B = 256, T = 1000, C = 64, U = 100) node-warp variants whose chains
+ * differ widely (7 warps and a barrier, 4 warps and a barrier, and a since-removed one of 1 warp and no barrier,
+ * DESIGN.md) all took about the same time; what they share is the saved-score traffic, 229 MB written in phase 1
+ * and read back in phase 2 at the fixed pitch, about two thirds of everything the kernel moves (counted from the
+ * shapes).  Saving the PAIR kernels' label scores alone (the blank's are read only at the meeting level) halved that
+ * traffic and cut the kernel from 0.376 to 0.315 ms (medians, H100 80GB HBM3 at a 400 W limit, DESIGN.md).  How the rest of a level's time splits has not
  * been measured; the dependent chain of a level, several CTAs deep on an SM, is the likeliest bound
  * (scripts/ubench/chain*.cu time its pieces).
  *
@@ -69,8 +67,9 @@
  *
  * Valid when every weight is finite (|x| < 1e29): otherwise a status bit is raised and the caller repeats
  * the batch through the materialised path, which reproduces the reference's inf / NaN propagation arc by
- * arc.  Requires: <= 224 graph nodes, in- and out-degree <= 3, one label per node (CTC, forced alignment),
- * C a multiple of 4 and <= 128, 16-byte aligned emissions.  Anything else takes k_implicit.cu.
+ * arc.  Requires: <= 224 graph nodes, in- and out-degree <= 3, one label per node, every arc weight 0 (the CTC
+ * target graphs of gtnb_ctc_loss, its only caller), C a multiple of 4 and <= 128, 16-byte aligned emissions.
+ * Anything else takes k_implicit.cu.
  */
 #include <algorithm>
 
@@ -83,8 +82,6 @@ namespace bidir {
 constexpr int kMaxNodes = 256; // table capacity
 constexpr int kMaxNodeWarps = 7; // graph nodes per utterance: at most 224, one per thread (4 CTAs of 12 warps per SM at 40 registers)
 constexpr int kMaxPairWarps = 4; // PAIR kernels: two nodes per thread, (U + 1) <= 112 pairs
-constexpr int kQuadSpare = 1; // QUAD kernels: idle warps that make the CTA 7 warps, so that the node warps of the four
-                              // CTAs of an SM land on four different schedulers (warp slot mod 4: 0, 3, 2, 1)
 constexpr int kRowF = 264; // floats per chain row in shared memory
 constexpr int kDummy = 256; // slot of every chain row that holds kNeg (absent arcs point here)
 constexpr int kBlk = 8; // frames per block (one TMA copy, one helper pass, one renormalisation)
@@ -163,8 +160,7 @@ struct Params {
   int C;
   int nwn; // node warps in the launch (ceil(max nodes / 32))
   int nblk_cap;
-  int zero_w; // every arc weight of every graph is 0 (host knowledge: CTC / forced alignment targets)
-  int ctc_blank; // PAIR / QUAD kernels: the graphs are CTC target graphs with this blank label ...
+  int ctc_blank; // PAIR kernels: the graphs are CTC target graphs with this blank label ...
   const int32_t* targets; // ... taken from the targets themselves: concatenated labels,
   // at GraphMeta::tgt_off of utterance b (the kernel never reads ctc_build_kernel's tables)
   Layout lay;
@@ -191,7 +187,6 @@ __device__ __forceinline__ float lse2_log2(float a, float b) { // max + lg2(1 + 
 
 struct NodeState {
   uint32_t so0, so1, so2; // byte offsets of the three neighbours in a chain row
-  float w0, w1, w2; // arc weights, log2 units
   uint32_t u4; // this node's byte offset in a row
   uint32_t pc, qc; // chain rows: read / write (swapped every level)
   uint32_t ea; // this node's emission in the current stage row
@@ -259,15 +254,13 @@ struct Strd {
  * r: the level's row within the block, counted in the CTA's own direction from the row st.ea / st.oa / st.ga /
  * st.gs point at (a constant after unrolling: with FX every address is register + immediate).
  * last: the block's last level (publishes the maximum for the renormalisation) */
-template <int DIR, int PH, bool ZW, int NQ, bool FX>
+template <int DIR, int PH, int NQ, bool FX>
 __device__ __forceinline__ void node_step(NodeState& st, const NodeUni& un, int r, bool last) {
   using SD = Strd<NQ, FX>;
   const int rr = DIR ? -r : r;
   const float x = lds_f32(st.ea + (uint32_t)(rr * SD::c4(un)));
-  // ZW: every arc weight of the graph is 0 (CTC, forced alignment): no adds
-  const float v = ZW ? lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2))
-                     : lse3_log2(lds_f32(st.pc + st.so0) + st.w0, lds_f32(st.pc + st.so1) + st.w1,
-                                 lds_f32(st.pc + st.so2) + st.w2);
+  // every arc weight of the graph is 0 (ctc_build_kernel's CTC graphs): no adds
+  const float v = lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2));
   // A: alpha_s = v + e[s-1][label(u)].  B: beta_s = v; what the predecessors read is beta_s + e[s-1][label(u)]
   const float val = DIR == 0 ? v + fmaf(x, kLog2e, -st.adj) : v - st.adj;
   const float stored = DIR == 0 ? val : fmaf(x, kLog2e, val);
@@ -287,15 +280,15 @@ __device__ __forceinline__ void node_step(NodeState& st, const NodeUni& un, int 
 }
 
 /* n levels from the rows st.ea / st.oa / st.ga / st.gs point at; st.gs moves on, the others are set per block */
-template <int DIR, int PH, bool ZW, int NQ, bool FX>
+template <int DIR, int PH, int NQ, bool FX>
 __device__ __forceinline__ void node_rows(NodeState& st, const NodeUni& un, int n) {
   // (a rolled loop with the last level peeled was slower on an earlier GPU target; not re-measured on the H100)
   if (n == kBlk) {
 #pragma unroll
-    for (int r = 0; r < kBlk; r++) node_step<DIR, PH, ZW, NQ, FX>(st, un, r, r == kBlk - 1);
+    for (int r = 0; r < kBlk; r++) node_step<DIR, PH, NQ, FX>(st, un, r, r == kBlk - 1);
   } else {
 #pragma unroll 1
-    for (int r = 0; r < n; r++) node_step<DIR, PH, ZW, NQ, FX>(st, un, r, r == n - 1);
+    for (int r = 0; r < n; r++) node_step<DIR, PH, NQ, FX>(st, un, r, r == n - 1);
   }
   if (PH == 1) st.gs += (DIR ? -n : n) * Strd<NQ, FX>::pitch(un);
 }
@@ -328,16 +321,14 @@ __device__ __forceinline__ float node_reduce_sum(float v, uint32_t red, int warp
  * level's posterior follows.  An utterance without any accepting path (Z = kNeg-like) gets Zh = +1e30,
  * which makes every posterior ex2(-huge) = 0.  `doth`: the partner's offset for this block.
  */
-template <int DIR, bool ZW, int NQ, bool FX>
+template <int DIR, int NQ, bool FX>
 __device__ __forceinline__ void node_first_phase2(
     NodeState& st, const NodeUni& un, bool act, uint32_t red, int warp, int nwarps, float doth, bool last,
     float* z_out, uint32_t feas_a, uint32_t spare) {
   using SD = Strd<NQ, FX>;
   const float x = lds_f32(st.ea);
   st.ea += DIR ? -SD::c4(un) : SD::c4(un);
-  const float v = ZW ? lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2))
-                     : lse3_log2(lds_f32(st.pc + st.so0) + st.w0, lds_f32(st.pc + st.so1) + st.w1,
-                                 lds_f32(st.pc + st.so2) + st.w2);
+  const float v = lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2));
   const float val = DIR == 0 ? v + fmaf(x, kLog2e, -st.adj) : v - st.adj;
   const float stored = DIR == 0 ? val : fmaf(x, kLog2e, val);
   st.adj = 0.0f;
@@ -411,7 +402,7 @@ __device__ __forceinline__ uint32_t bar_tbl_ready(uint32_t bars) {
  * direction is folded into per-thread base addresses up front, so that a block costs its levels plus a
  * few dozen instructions.
  */
-template <int DIR, bool ZW, int NQ, bool FX>
+template <int DIR, int NQ, bool FX>
 __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool act, int nid) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   NodeUni un;
@@ -439,7 +430,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       st.ea = e_row0 + (uint32_t)(s * cx.e_stage_bytes);
       if (v > 0) fetch_block_adjust(st);
       if (tid == 0) stg_f32(cx.boff_own + 4 * v, st.D);
-      node_rows<0, 1, ZW, NQ, FX>(st, un, kBlk); // A's phase-1 blocks are always full
+      node_rows<0, 1, NQ, FX>(st, un, kBlk); // A's phase-1 blocks are always full
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
     }
@@ -460,7 +451,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       stg_f32(st.gs, val);
       st.gs -= un.pitch;
     }
-    node_rows<1, 1, ZW, NQ, FX>(st, un, n0 - 1);
+    node_rows<1, 1, NQ, FX>(st, un, n0 - 1);
     __syncwarp();
     if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, 0), arr1);
     for (v = 1; v < cx.n_ph1; v++) {
@@ -469,7 +460,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       st.ea = e_row0 + (uint32_t)(s * cx.e_stage_bytes);
       fetch_block_adjust(st);
       if (tid == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), st.D);
-      node_rows<1, 1, ZW, NQ, FX>(st, un, kBlk);
+      node_rows<1, 1, NQ, FX>(st, un, kBlk);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
     }
@@ -501,13 +492,13 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
     if (v > 0) fetch_block_adjust(st);
     const float doth = lds_f32(cx.od_base + 16u * so);
     if (v2 == 0) {
-      node_first_phase2<DIR, ZW, NQ, FX>(st, un, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
+      node_first_phase2<DIR, NQ, FX>(st, un, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
                                          DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.spare);
-      if (cx.want_g) node_rows<DIR, 2, ZW, NQ, FX>(st, un, nfr - 1);
+      if (cx.want_g) node_rows<DIR, 2, NQ, FX>(st, un, nfr - 1);
     } else {
       // offsets moved since the meeting level: all integers, the differences are exact
       st.zsub = st.Zl - ((st.D + doth) - st.Dc);
-      node_rows<DIR, 2, ZW, NQ, FX>(st, un, nfr);
+      node_rows<DIR, 2, NQ, FX>(st, un, nfr);
     }
     __syncwarp();
     if (lane == 0) {
@@ -540,8 +531,8 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
  * label rows take the first n * kHalfPitch floats, and -- in the block of the meeting level only -- the meeting
  * row's blank scores follow them.  Half the saved-score traffic of full rows, in HBM both ways.
  */
-/* start / accept flags of node n of a CTC target graph with N1 = 2U + 1 nodes (benchmarks/ctc.cpp:43-44): the PAIR /
- * QUAD kernels take the graph from the target itself and never read ctc_build_kernel's tables */
+/* start / accept flags of node n of a CTC target graph with N1 = 2U + 1 nodes (benchmarks/ctc.cpp:43-44): the PAIR
+ * kernels take the graph from the target itself and never read ctc_build_kernel's tables */
 /* does label node n (odd) have the skip in-arc from label n - 2: not for the first label, not for a repeat (:51-54) */
 __device__ __forceinline__ bool ctc_skip(const int32_t* tg, int n, int N1) {
   return n >= 3 && n < N1 && tg[(n - 1) / 2] != tg[(n - 3) / 2];
@@ -787,314 +778,6 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     } else {
       ps.zsub = ps.Zl - ((ps.D + doth) - ps.Dc);
       pair_rows<DIR, 2, NQ>(ps, un, nfr);
-    }
-    __syncwarp();
-    if (lane == 0) {
-      mbar_arrive_n(bar_e_empty(cx.bars, s), arr2);
-      mbar_arrive(bar_o_empty(cx.bars, so));
-      mbar_arrive(bar_g_full(cx.bars, sg));
-    }
-  }
-}
-
-/* ------------------------------------------------------------------ */
-/* node warp, CTC quad mode: ONE warp per CTA, four pairs per thread    */
-/* ------------------------------------------------------------------ */
-
-/*
- * The pair kernels still pay one named barrier and one shared-memory round trip per level, and four warps whose
- * chains the scheduler has to interleave.  Here thread t owns the pairs 4t .. 4t+3 (nodes 8t-1 .. 8t+6): three of
- * its four neighbour pairs are its own registers, the fourth comes by ONE shuffle pair (A: pair 4t-1 from lane t-1)
- * or one shuffle (B: the label of pair 4t+4 from lane t+1).  No chain rows, no barrier on the chain, eight
- * independent logsumexps per thread and level to hide each other's latency; the renormalisation maximum is one
- * REDUX.  Saved scores leave as two STG.128, the partner's arrive as two LDS.128 (slots 8t .. 8t+7 of a row).
- * Pairs beyond the graph (k > U) are phantoms: in B nothing ever feeds them (they stay at kNeg), in A they only
- * read lower pairs and nothing real reads them; they are kept out of Z, their posteriors go to the trash word, and
- * lanes >= 28 (slots beyond the 224-float row) neither load nor store rows.
- */
-constexpr int kQuad = 4; // pairs per thread
-
-struct QuadState {
-  float al[kQuad], ab[kQuad]; // what the neighbours read of the label / blank nodes (A: alpha, B: beta + emission)
-  uint32_t el[kQuad]; // byte offset of each label's emission inside a row
-  uint32_t gl[kQuad]; // byte offset of each label's posterior slot inside a row of the helpers' block
-  uint32_t skip; // bit i: A: label of pair 4t+i has the skip in-arc; B: label of pair 4t+i+1 has it
-  uint32_t eb; // byte offset of blank's emission
-  uint32_t ea, oa, ga; // first row of the block: emission stage, partner's scores (this thread's 8 slots), posteriors
-  float* gs; // where the thread's 8 scores are saved (phase 1)
-  float adj, D, Zh, zsub, Zl, Dc;
-  bool rows; // lane < 28: the thread's slots exist in a row
-};
-
-/* the recursion of one level for the thread's four pairs; val_*: the scores proper (alpha / beta) */
-template <int DIR>
-__device__ __forceinline__ void quad_values(QuadState& q, const float* xl, float xb, float* val_l, float* val_b) {
-  const int lane = threadIdx.x & 31;
-  if (DIR == 0) {
-    // pair 4t-1 from the lane below (lane 0: nothing there)
-    float pl = __shfl_up_sync(0xffffffffu, q.al[kQuad - 1], 1);
-    float pb = __shfl_up_sync(0xffffffffu, q.ab[kQuad - 1], 1);
-    if (lane == 0) {
-      pl = kNeg;
-      pb = kNeg;
-    }
-    float nl[kQuad], nb[kQuad];
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      const float ql = i ? q.al[i - 1] : pl, qb = i ? q.ab[i - 1] : pb;
-      nb[i] = lse2_log2(q.ab[i], q.al[i]) + fmaf(xb, kLog2e, -q.adj);
-      nl[i] = lse3_log2(q.al[i], qb, (q.skip >> i) & 1u ? ql : kNeg) + fmaf(xl[i], kLog2e, -q.adj);
-    }
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      val_l[i] = q.al[i] = nl[i];
-      val_b[i] = q.ab[i] = nb[i];
-    }
-  } else {
-    float nx = __shfl_down_sync(0xffffffffu, q.al[0], 1); // the label of pair 4t+4
-    if (lane == 31) nx = kNeg;
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      const float ql = i + 1 < kQuad ? q.al[i + 1] : nx;
-      val_b[i] = lse2_log2(q.ab[i], ql) - q.adj;
-      val_l[i] = lse3_log2(q.al[i], q.ab[i], (q.skip >> i) & 1u ? ql : kNeg) - q.adj;
-    }
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      q.al[i] = fmaf(xl[i], kLog2e, val_l[i]);
-      q.ab[i] = fmaf(xb, kLog2e, val_b[i]);
-    }
-  }
-  q.adj = 0.0f;
-}
-
-/* the largest kept score of the warp as an integer (what the next block subtracts) */
-__device__ __forceinline__ float quad_block_max(const QuadState& q) {
-  float m = fmaxf(q.al[0], q.ab[0]);
-#pragma unroll
-  for (int i = 1; i < kQuad; i++) m = fmaxf(m, fmaxf(q.al[i], q.ab[i]));
-  const int iv = __reduce_max_sync(0xffffffffu, __float2int_rn(fmaxf(m, -2.0e9f)));
-  return iv <= -2000000000 ? 0.0f : (float)iv;
-}
-
-template <int DIR, int PH, int NQ>
-__device__ __forceinline__ void quad_step(QuadState& q, const NodeUni& un, int r, bool last, float& next_adj) {
-  using SD = Strd<NQ, true>;
-  const int rr = DIR ? -r : r;
-  const uint32_t er = q.ea + (uint32_t)(rr * SD::c4(un));
-  float xl[kQuad];
-#pragma unroll
-  for (int i = 0; i < kQuad; i++) xl[i] = lds_f32(er + q.el[i]);
-  const float xb = lds_f32(er + q.eb);
-  float val_l[kQuad], val_b[kQuad];
-  quad_values<DIR>(q, xl, xb, val_l, val_b);
-  if (PH == 2) {
-    const uint32_t orow = q.oa + (uint32_t)(rr * SD::p4(un));
-    const float4 o0 = lds_v4_f32(orow), o1 = lds_v4_f32(orow + 16u); // (label, blank) x 4
-    const float ol[kQuad] = {o0.x, o0.z, o1.x, o1.z};
-    const uint32_t grow = q.ga + (uint32_t)(rr * SD::g4(un));
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) sts_f32(grow + q.gl[i], ex2(((val_l[i] - q.Zh) + ol[i]) - q.zsub));
-  }
-  if (PH == 1 && q.rows) {
-    float* g = q.gs + rr * SD::pitch(un);
-    stg_v4_f32(g, make_float4(val_l[0], val_b[0], val_l[1], val_b[1]));
-    stg_v4_f32(g + 4, make_float4(val_l[2], val_b[2], val_l[3], val_b[3]));
-  }
-  if (last) next_adj = quad_block_max(q);
-}
-
-template <int DIR, int PH, int NQ>
-__device__ __forceinline__ void quad_rows(QuadState& q, const NodeUni& un, int n, float& next_adj) {
-  if (n == kBlk) {
-#pragma unroll
-    for (int r = 0; r < kBlk; r++) quad_step<DIR, PH, NQ>(q, un, r, r == kBlk - 1, next_adj);
-  } else {
-#pragma unroll 1
-    for (int r = 0; r < n; r++) quad_step<DIR, PH, NQ>(q, un, r, r == n - 1, next_adj);
-  }
-  if (PH == 1) q.gs += (DIR ? -n : n) * Strd<NQ, true>::pitch(un);
-}
-
-/* the first level of phase 2: Z over every real node (see node_first_phase2) */
-template <int DIR, int NQ>
-__device__ __forceinline__ void quad_first_phase2(
-    QuadState& q, const NodeUni& un, uint32_t act_l, uint32_t act_b, float doth, bool last, float* z_out, uint32_t feas_a,
-    bool want_g, float& next_adj) {
-  using SD = Strd<NQ, true>;
-  float xl[kQuad];
-#pragma unroll
-  for (int i = 0; i < kQuad; i++) xl[i] = lds_f32(q.ea + q.el[i]);
-  const float xb = lds_f32(q.ea + q.eb);
-  q.ea += DIR ? -SD::c4(un) : SD::c4(un);
-  float val_l[kQuad], val_b[kQuad];
-  quad_values<DIR>(q, xl, xb, val_l, val_b);
-  const float4 o0 = lds_v4_f32(q.oa), o1 = lds_v4_f32(q.oa + 16u);
-  const float ol[kQuad] = {o0.x, o0.z, o1.x, o1.z}, ob[kQuad] = {o0.y, o0.w, o1.y, o1.w};
-  float hl[kQuad], ll[kQuad], hb[kQuad], lb[kQuad];
-  float m = 2.0f * kNeg;
-#pragma unroll
-  for (int i = 0; i < kQuad; i++) {
-    // TwoSum (Knuth): hi + lo == val + o exactly
-    hl[i] = val_l[i] + ol[i];
-    const float bl = hl[i] - val_l[i];
-    ll[i] = (val_l[i] - (hl[i] - bl)) + (ol[i] - bl);
-    hb[i] = val_b[i] + ob[i];
-    const float bb = hb[i] - val_b[i];
-    lb[i] = (val_b[i] - (hb[i] - bb)) + (ob[i] - bb);
-    if ((act_l >> i) & 1u) m = fmaxf(m, hl[i]);
-    if ((act_b >> i) & 1u) m = fmaxf(m, hb[i]);
-  }
-  m = warp_max(m);
-  const bool live = m > 1.5f * kNeg;
-  float term = 0.0f;
-#pragma unroll
-  for (int i = 0; i < kQuad; i++) {
-    if (live && ((act_l >> i) & 1u)) term += ex2((hl[i] - m) + ll[i]);
-    if (live && ((act_b >> i) & 1u)) term += ex2((hb[i] - m) + lb[i]);
-  }
-  const float S = warp_sum(term);
-  const bool feasible = m > kNeg * 0.5f && S > 0.0f;
-  q.Zh = feasible ? m : 1.0e30f;
-  q.Zl = feasible ? lg2(S) : 0.0f;
-  q.Dc = q.D + doth;
-  q.zsub = q.Zl;
-  if ((threadIdx.x & 31) == 0) sts_f32(feas_a, feasible ? 1.0f : 0.0f);
-  if (z_out && (threadIdx.x & 31) == 0)
-    *z_out = feasible ? (float)(((double)q.Dc + ((double)m + (double)q.Zl)) * 0.6931471805599453) : -CUDART_INF_F;
-  if (want_g) {
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) sts_f32(q.ga + q.gl[i], ex2(((val_l[i] - q.Zh) + ol[i]) - q.zsub));
-    q.ga += DIR ? -SD::g4(un) : SD::g4(un);
-  }
-  q.oa += DIR ? -SD::p4(un) : SD::p4(un);
-  if (last) next_adj = quad_block_max(q);
-}
-
-/* the node warp of one CTA, both phases (node_role's protocol; nw_act == 1) */
-template <int DIR, int NQ>
-__device__ __forceinline__ void quad_role(QuadState& q, const NodeCtx& cx, int n_pairs) {
-  const int lane = threadIdx.x & 31;
-  NodeUni un;
-  un.c4 = 4 * cx.C;
-  un.p4 = 4 * cx.pitch;
-  un.g4 = 4 * cx.pg;
-  un.pitch = cx.pitch;
-  un.nact = 32;
-  const int arr1 = cx.want_g ? 1 + kHelpers : 1;
-  const int arr2 = !cx.want_g ? 1 + kHelpers : 1;
-  const uint32_t dir_off = DIR ? (uint32_t)((kBlk - 1) * cx.C * 4) : 0u;
-  uint32_t act_l = 0, act_b = 0; // which of the thread's nodes exist
-#pragma unroll
-  for (int i = 0; i < kQuad; i++) {
-    const int k = kQuad * lane + i;
-    if (k < n_pairs) act_b |= 1u << i;
-    if (k >= 1 && k < n_pairs) act_l |= 1u << i;
-  }
-  float next_adj = 0.0f;
-  int v = 0;
-  if (DIR == 0) {
-    // level 0: start nodes carry the implicit 0 (shortest.cpp:129-135)
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      const int k = kQuad * lane + i;
-      q.al[i] = (((act_l >> i) & 1u) && (ctc_flags(2 * k - 1, cx.N1) & 1)) ? 0.0f : kNeg;
-      q.ab[i] = (((act_b >> i) & 1u) && (ctc_flags(2 * k, cx.N1) & 1)) ? 0.0f : kNeg;
-    }
-    q.gs = cx.saved + 8 * lane;
-    for (; v < cx.n_ph1; v++) {
-      const int s = v & (kSE - 1);
-      mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
-      q.ea = cx.e_base + dir_off + (uint32_t)(s * cx.e_stage_bytes);
-      if (v > 0) {
-        q.adj = next_adj;
-        q.D += next_adj;
-      }
-      if (lane == 0) stg_f32(cx.boff_own + 4 * v, q.D);
-      quad_rows<0, 1, NQ>(q, un, kBlk, next_adj);
-      __syncwarp();
-      if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
-    }
-  } else if (cx.T > 0) {
-    // level T: accept nodes carry 0; what the predecessors read is beta_T + e[T-1][label]
-    const int j0 = cx.nblk - 1, n0 = min(kBlk, cx.T - kBlk * j0);
-    mbar_wait(bar_e_full(cx.bars, 0), 0);
-    q.ea = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4);
-    if (lane == 0) stg_f32(cx.boff_own + 4 * j0, 0.0f);
-    {
-      float val_l[kQuad], val_b[kQuad];
-      const float eb = lds_f32(q.ea + q.eb) * kLog2e;
-#pragma unroll
-      for (int i = 0; i < kQuad; i++) {
-        const int k = kQuad * lane + i;
-        val_l[i] = (((act_l >> i) & 1u) && (ctc_flags(2 * k - 1, cx.N1) & 2)) ? 0.0f : kNeg;
-        val_b[i] = (((act_b >> i) & 1u) && (ctc_flags(2 * k, cx.N1) & 2)) ? 0.0f : kNeg;
-        q.al[i] = val_l[i] + lds_f32(q.ea + q.el[i]) * kLog2e;
-        q.ab[i] = val_b[i] + eb;
-      }
-      q.ea -= un.c4;
-      q.gs = cx.saved + (long long)(cx.T - 1) * cx.pitch + 8 * lane;
-      if (n0 == 1) next_adj = quad_block_max(q);
-      if (q.rows) {
-        stg_v4_f32(q.gs, make_float4(val_l[0], val_b[0], val_l[1], val_b[1]));
-        stg_v4_f32(q.gs + 4, make_float4(val_l[2], val_b[2], val_l[3], val_b[3]));
-      }
-      q.gs -= un.pitch;
-    }
-    quad_rows<1, 1, NQ>(q, un, n0 - 1, next_adj);
-    __syncwarp();
-    if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, 0), arr1);
-    for (v = 1; v < cx.n_ph1; v++) {
-      const int s = v & (kSE - 1);
-      mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
-      q.ea = cx.e_base + dir_off + (uint32_t)(s * cx.e_stage_bytes);
-      q.adj = next_adj;
-      q.D += next_adj;
-      if (lane == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), q.D);
-      quad_rows<1, 1, NQ>(q, un, kBlk, next_adj);
-      __syncwarp();
-      if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
-    }
-  }
-  cluster_sync_all();
-  // ---- phase 2
-  if (cx.n_ph2 <= 0) return;
-  // lanes >= 28 read (harmless) words of the stage / block that belong to other rows: keep them in bounds
-  const uint32_t o_row0 = cx.o_base + (q.rows ? 32u * (uint32_t)lane : 0u) + (DIR ? (uint32_t)((kBlk - 1) * cx.pitch * 4) : 0u);
-  uint32_t g_row0 = 0;
-  int g_stride = 0;
-  if (cx.want_g) {
-    mbar_wait(bar_tbl_ready(cx.bars), 0); // the helper warps' tables
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      const int k = kQuad * lane + i;
-      // a label that does not exist stores into the row's last word, which nobody reads
-      q.gl[i] = ((act_l >> i) & 1u) ? lds_u16(cx.perm_a + 2u * (uint32_t)(2 * k - 1)) : 4u * (uint32_t)(cx.pg - 1);
-    }
-    g_row0 = cx.g_base + (DIR ? (uint32_t)((kBlk - 1) * cx.pg * 4) : 0u);
-    g_stride = cx.g_block_bytes;
-  }
-  for (int v2 = 0; v2 < cx.n_ph2; v2++, v++) {
-    const int s = v & (kSE - 1), so = v2 & (kSO - 1), sg = v2 & (kSG - 1);
-    const int nfr = DIR ? kBlk : min(kBlk, cx.T - kBlk * v);
-    mbar_wait(bar_e_full(cx.bars, s), (v / kSE) & 1);
-    mbar_wait(bar_o_full(cx.bars, so), (v2 / kSO) & 1);
-    if (v2 >= kSG) mbar_wait(bar_g_empty(cx.bars, sg), ((v2 / kSG) - 1) & 1);
-    q.ea = cx.e_base + dir_off + (uint32_t)(s * cx.e_stage_bytes);
-    q.oa = o_row0 + (uint32_t)(so * cx.o_stage_bytes);
-    q.ga = g_row0 + (uint32_t)(sg * g_stride);
-    if (v > 0) {
-      q.adj = next_adj;
-      q.D += next_adj;
-    }
-    const float doth = lds_f32(cx.od_base + 16u * so);
-    if (v2 == 0) {
-      quad_first_phase2<DIR, NQ>(q, un, act_l, act_b, doth, nfr == 1, DIR == 0 ? cx.out_score : nullptr, cx.feas_a,
-                                 cx.want_g, next_adj);
-      if (cx.want_g) quad_rows<DIR, 2, NQ>(q, un, nfr - 1, next_adj);
-    } else {
-      q.zsub = q.Zl - ((q.D + doth) - q.Dc);
-      quad_rows<DIR, 2, NQ>(q, un, nfr, next_adj);
     }
     __syncwarp();
     if (lane == 0) {
@@ -1359,14 +1042,11 @@ __device__ __forceinline__ void helper_block_fast(
 /* the kernel                                                          */
 /* ------------------------------------------------------------------ */
 
-/* MODE 0: one node per thread (any graph in the envelope); 1: PAIR (CTC graphs, two nodes per thread); 2: QUAD (CTC
- * graphs, one node warp with four pairs per thread, plus kQuadSpare idle warps: see launch_bidir_ctc) */
-template <int NQ, bool ZW, bool FX, int MODE>
-__global__ void __launch_bounds__(
-    32 * ((MODE == 2 ? 1 + kQuadSpare : MODE == 1 ? kMaxPairWarps : kMaxNodeWarps) + 1 + kHelpers), 4)
+/* MODE 0: one node per thread (any graph in the envelope); 1: PAIR (CTC graphs, two nodes per thread) */
+template <int NQ, bool FX, int MODE>
+__global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWarps) + 1 + kHelpers), 4)
     bidir_ctc_kernel(const Params P) {
   constexpr bool PAIR = MODE == 1;
-  constexpr bool QUAD = MODE == 2;
   GTNB_DYNAMIC_SMEM_128(unsigned char, smem);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.x >> 1;
@@ -1393,7 +1073,7 @@ __global__ void __launch_bounds__(
   const uint32_t g_base = smem_u32(smem + L.off_g);
 
   const int n_pairs = (N1 + 1) >> 1; // PAIR: U + 1
-  const int nw_act = QUAD ? 1 : PAIR ? (n_pairs + 31) >> 5 : (N1 + 31) >> 5; // node warps of THIS utterance
+  const int nw_act = PAIR ? (n_pairs + 31) >> 5 : (N1 + 31) >> 5; // node warps of THIS utterance
   const int nact = 32 * nw_act;
   const int nblk = (T + kBlk - 1) / kBlk;
   // levels 1..M: alpha saved, posterior by B; M+1..T: beta saved, posterior by A.  T/2 rounded UP to a block: CTA B
@@ -1474,68 +1154,6 @@ __global__ void __launch_bounds__(
   }
   __syncthreads();
 
-  if (QUAD && warp < P.nwn) {
-    /* ============================ the node warp, four pairs per thread ============================ */
-    QuadState q;
-    q.skip = 0;
-    q.eb = 4u * (uint32_t)P.ctc_blank;
-#pragma unroll
-    for (int i = 0; i < kQuad; i++) {
-      const int k = kQuad * lane + i; // pair
-      const int lnode = 2 * k - 1;
-      const bool has = k >= 1 && k < n_pairs;
-      q.el[i] = 4u * (uint32_t)(has ? tg[k - 1] : P.ctc_blank);
-      q.gl[i] = 4u * (uint32_t)(L.pg - 1);
-      const int sk_node = dir == 0 ? lnode : lnode + 2;
-      if (ctc_skip(tg, sk_node, N1)) q.skip |= 1u << i;
-      q.al[i] = q.ab[i] = kNeg;
-    }
-    q.rows = 8 * lane + 7 < pitch;
-    q.gs = nullptr;
-    q.Zh = q.zsub = q.Zl = q.Dc = 0.0f;
-    q.adj = q.D = 0.0f;
-    q.ea = q.oa = q.ga = 0;
-    __syncthreads(); // (S1) all roles
-    NodeCtx cx;
-    cx.fl = fl;
-    cx.saved = saved;
-    cx.boff_own = boff_own;
-    cx.out_score = P.out_scores + b;
-    cx.bars = bars;
-    cx.e_base = e_base;
-    cx.o_base = o_base;
-    cx.g_base = g_base;
-    cx.od_base = od_base;
-    cx.perm_a = perm_a;
-    cx.red_a = red_a;
-    cx.spare = 0;
-    cx.lab4 = 0;
-    cx.blank4 = q.eb;
-    cx.feas_a = hlist_a + 96u;
-    cx.e_stage_bytes = L.e_stage_bytes;
-    cx.o_stage_bytes = L.o_stage_bytes;
-    cx.g_block_bytes = L.g_block_bytes;
-    cx.pg = L.pg;
-    cx.C = C;
-    cx.T = T;
-    cx.N1 = N1;
-    cx.pitch = pitch;
-    cx.nblk = nblk;
-    cx.n_ph1 = n_ph1;
-    cx.n_ph2 = n_ph2;
-    cx.nw_act = 1;
-    cx.want_g = want_g;
-    if (dir == 0)
-      quad_role<0, NQ>(q, cx, n_pairs);
-    else
-      quad_role<1, NQ>(q, cx, n_pairs);
-    if (T == 0 && dir == 0 && tid == 0) {
-      int n = 0;
-      for (int i = 0; i < N1; i++) n += (ctc_flags(i, N1) & 3) == 3;
-      P.out_scores[b] = n ? logf((float)n) : -CUDART_INF_F;
-    }
-    return;
-  }
   if (PAIR && warp < P.nwn) {
     /* ============================ node warps, two nodes per thread ============================ */
     const bool act = tid < n_pairs;
@@ -1640,9 +1258,6 @@ __global__ void __launch_bounds__(
     st.so0 = 4u * (uint32_t)nb_[0];
     st.so1 = 4u * (uint32_t)nb_[1];
     st.so2 = 4u * (uint32_t)nb_[2];
-    st.w0 = wb_[0] * kLog2e;
-    st.w1 = wb_[1] * kLog2e;
-    st.w2 = wb_[2] * kLog2e;
     // the scratch is about to be overwritten by the score stages: everybody is done reading it
     __syncthreads(); // (S1) all roles
     if (warp >= nw_act) { // node warp without a node of this utterance
@@ -1690,9 +1305,9 @@ __global__ void __launch_bounds__(
     cx.nw_act = nw_act;
     cx.want_g = want_g;
     if (dir == 0)
-      node_role<0, ZW, NQ, FX>(st, cx, act, nid);
+      node_role<0, NQ, FX>(st, cx, act, nid);
     else
-      node_role<1, ZW, NQ, FX>(st, cx, act, nid);
+      node_role<1, NQ, FX>(st, cx, act, nid);
     if (bad) *(volatile int32_t*)&P.status[b] = 1; // (every writer stores the same 1: no atomic needed)
     if (T == 0 && dir == 0 && tid == 0) {
       // no frames: the lattice is the graph's start-and-accept nodes, each with score 0
@@ -1705,7 +1320,7 @@ __global__ void __launch_bounds__(
 
   __syncthreads(); // (S1)
 
-  if (warp > P.nwn + kHelpers) { // QUAD: the idle warps
+  if (warp > P.nwn + kHelpers) { // (no launch has warps beyond the helpers; without this test ptxas schedules every kernel differently)
     cluster_sync_all();
     return;
   }
@@ -1782,7 +1397,7 @@ __global__ void __launch_bounds__(
           comp = c;
         }
       }
-      if (MODE != 0) comp = P.ctc_blank; // the pair / quad threads never form a blank posterior, whatever U is
+      if (MODE != 0) comp = P.ctc_blank; // the pair threads never form a blank posterior, whatever U is
       sts_u32(hlist_a + 100u, (uint32_t)comp);
       int nh = 0, at = 0;
       for (int c = 0; c < C; c++) {
@@ -1912,11 +1527,11 @@ bool bidir_supported(const gtnb_lattice* lat, const float* emissions, int64_t st
   return true;
 }
 
-/* true when launch_bidir_ctc would run its PAIR / QUAD kernels, which read the CTC target graphs from the targets
+/* true when launch_bidir_ctc would run its PAIR kernels, which read the CTC target graphs from the targets
  * themselves: the caller (gtnb_ctc_loss) then skips ctc_build_kernel altogether */
-bool bidir_takes_targets(const gtnb_lattice* lat, int zero_w, int ctc_blank) {
+bool bidir_takes_targets(const gtnb_lattice* lat, int ctc_blank) {
   const bool fx = (lat->C == 64 || lat->C == 128) && lat->score_pitch == bidir::kFixedPitch;
-  return fx && zero_w && ctc_blank >= 0 && ctc_blank < lat->C && lat->max_lvl_nodes <= 2 * 32 * bidir::kMaxPairWarps - 1;
+  return fx && ctc_blank >= 0 && ctc_blank < lat->C && lat->max_lvl_nodes <= 2 * 32 * bidir::kMaxPairWarps - 1;
 }
 
 /* blocks of 8 frames per utterance: boff_dev holds B * 2 * bidir_blocks(max T) * 4 floats */
@@ -1930,7 +1545,7 @@ int bidir_zparts() {
 }
 int launch_bidir_ctc(
     gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, float* grad_emis,
-    int64_t grad_stride, int b0, int nb, int zero_w, float* out_scores_dev, int ctc_blank, const int32_t* targets_dev,
+    int64_t grad_stride, int b0, int nb, float* out_scores_dev, int ctc_blank, const int32_t* targets_dev,
     const int32_t* tgt_off_dev, const GraphMeta* meta_src) {
   if (nb < 0) nb = lat->B - b0;
   if (nb <= 0) return GTNB_OK;
@@ -1958,37 +1573,32 @@ int launch_bidir_ctc(
   const int max_pitch = fx ? bidir::kFixedPitch : ((lat->max_lvl_nodes + 3) & ~3);
   P.lay = bidir::make_layout(lat->C, max_pitch);
   // NQ: float4 chunks of an emission row per helper lane
-  // the graphs are ctc_build_kernel's (gtnb_ctc_loss): PAIR (two nodes per thread; the default) or QUAD (one node
-  // warp, four pairs per thread) kernels; gtnb_ctx_set_flag("bidir_mode", 0 | 1 | 2) picks one for comparison
+  // the graphs are ctc_build_kernel's (gtnb_ctc_loss): the PAIR kernels (two nodes per thread) unless
+  // gtnb_ctx_set_flag("bidir_mode", 0) asks for one node per thread
   (void)tgt_off_dev; // (the offsets travel in the descriptors: GraphMeta::tgt_off)
-  const bool ctc_ok = bidir_takes_targets(lat, zero_w, ctc_blank) && targets_dev;
+  const bool ctc_ok = bidir_takes_targets(lat, ctc_blank) && targets_dev;
   P.targets = targets_dev;
-  const int mode = !ctc_ok ? 0 : ctx->bidir_mode >= 0 ? ctx->bidir_mode : (grad_emis ? 1 : 2);
+  const int mode = !ctc_ok || ctx->bidir_mode == 0 ? 0 : 1;
   void (*kern)(const bidir::Params);
-  if (mode == 2)
-    kern = lat->C == 64 ? bidir::bidir_ctc_kernel<1, true, true, 2> : bidir::bidir_ctc_kernel<2, true, true, 2>;
-  else if (mode == 1)
-    kern = lat->C == 64 ? bidir::bidir_ctc_kernel<1, true, true, 1> : bidir::bidir_ctc_kernel<2, true, true, 1>;
+  if (mode == 1)
+    kern = lat->C == 64 ? bidir::bidir_ctc_kernel<1, true, 1> : bidir::bidir_ctc_kernel<2, true, 1>;
   else if (fx && lat->C == 64)
-    kern = zero_w ? bidir::bidir_ctc_kernel<1, true, true, 0> : bidir::bidir_ctc_kernel<1, false, true, 0>;
+    kern = bidir::bidir_ctc_kernel<1, true, 0>;
   else if (fx)
-    kern = zero_w ? bidir::bidir_ctc_kernel<2, true, true, 0> : bidir::bidir_ctc_kernel<2, false, true, 0>;
+    kern = bidir::bidir_ctc_kernel<2, true, 0>;
   else if (lat->C <= 64)
-    kern = zero_w ? bidir::bidir_ctc_kernel<1, true, false, 0> : bidir::bidir_ctc_kernel<1, false, false, 0>;
+    kern = bidir::bidir_ctc_kernel<1, false, 0>;
   else
-    kern = zero_w ? bidir::bidir_ctc_kernel<2, true, false, 0> : bidir::bidir_ctc_kernel<2, false, false, 0>;
+    kern = bidir::bidir_ctc_kernel<2, false, 0>;
   if (mode == 1) P.nwn = std::max(1, ((lat->max_lvl_nodes + 1) / 2 + 31) / 32);
-  if (mode == 2) P.nwn = 1;
-  const int spare_warps = mode == 2 ? bidir::kQuadSpare : 0;
   P.ctc_blank = ctc_blank;
-  P.zero_w = zero_w;
   if (P.lay.total > 48 * 1024) {
     int rc = ensure_max_smem(ctx, (const void*)kern);
     if (rc) return rc;
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(2 * nb, 1, 1);
-  cfg.blockDim = dim3(32 * (P.nwn + 1 + bidir::kHelpers + spare_warps), 1, 1);
+  cfg.blockDim = dim3(32 * (P.nwn + 1 + bidir::kHelpers), 1, 1);
   cfg.dynamicSmemBytes = P.lay.total;
   cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];

@@ -105,9 +105,9 @@ int64_t gtnb_ctx_launch_count(const gtnb_ctx* ctx);
  * which is how the tests cross-check the two families.  "implicit" (default 1): the
  * criteria (gtnb_ctc_loss) sweep the frames of intersect(target graph, emissions) without
  * materialising the lattice; 0 makes them build it and run the lattice kernels.
- * "banded" (default 0, EXPERIMENTAL): value K in {1, 2, 4, 8}: gtnb_ctc_loss's implicit sweeps run
- * K frames per barrier with warp-shuffle neighbour exchange (k_banded.cu) when the target graphs
- * are band shaped.  "exact_ties" (default 0, EXPERIMENTAL; set before gtnb_compose_linear): gtnb_viterbi_path
+ * "bidir_mode" (default -1): the node warps of gtnb_ctc_loss's one-launch kernel (k_bidir.cu) at
+ * C = 64 / 128: -1 or 1 the PAIR kernels (a label and a blank node per thread), 0 one node per
+ * thread; any other value is rejected.  "exact_ties" (default 0, EXPERIMENTAL; set before gtnb_compose_linear): gtnb_viterbi_path
  * on a composed lattice breaks exact score ties like the reference's shortestPath (k_order.cu).
  */
 int gtnb_ctx_set_flag(gtnb_ctx* ctx, const char* name, int value);

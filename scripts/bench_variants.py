@@ -4,8 +4,8 @@ the first variant.
 
     python scripts/bench_variants.py [B T C U] > variants.json
 
-The bidir_* variants with an explicit bidir_mode are what the default (bidir_mode -1: PAIR with a gradient,
-QUAD loss-only, gtnb_internal.h) was chosen from.
+The bidir_* variants with an explicit bidir_mode are what the default (bidir_mode -1: the PAIR kernels,
+gtnb_internal.h) was chosen from.
 """
 import json
 import sys
@@ -36,7 +36,7 @@ def step(want_grad=True):
 VARIANTS = [("two_sweeps", {"bidir": 0}, True), ("bidir", {"bidir": 1, "bidir_mode": -1}, True),
             ("bidir_loss_only", {"bidir": 1, "bidir_mode": -1}, False), ("two_sweeps_loss_only", {"bidir": 0}, False)]
 VARIANTS += [("bidir_%s%s" % (m, "" if wg else "_loss_only"), {"bidir": 1, "bidir_mode": k}, wg)
-             for wg in (True, False) for k, m in ((0, "node"), (1, "pair"), (2, "quad"))]
+             for wg in (True, False) for k, m in ((0, "node"), (1, "pair"))]
 out = {"shape": [B, T, C, U]}
 ref = None
 for name, flags, wg in VARIANTS:

@@ -18,10 +18,11 @@ extern "C" {
  * targets concatenated, target_lens[B]; emissions [B][T][C]; input_lens[B] or NULL.
  * out_scores[B] = forwardScore(intersect(ctc_b, e_b)); znorm[B] = forwardScore(e_b);
  * grad [B][T][C] (NULL: loss only) = d(znorm - out) / d e; status[B].
+ * bidir_mode: as gtnb_ctx_set_flag's -- 0 the one-node-per-thread kernel, otherwise launch_bidir_ctc's choice.
  */
 int emu_bidir_ctc(
     int B, int T, int C, const float* emissions, const int32_t* input_lens, const int32_t* targets,
-    const int32_t* target_lens, int blank, int zero_w, float* out_scores, float* znorm, float* grad, int32_t* status) {
+    const int32_t* target_lens, int blank, int bidir_mode, float* out_scores, float* znorm, float* grad, int32_t* status) {
   using namespace gtnb;
   std::vector<GraphMeta> meta(B);
   std::vector<int32_t> tgt_off(B);
@@ -81,32 +82,25 @@ int emu_bidir_ctc(
   P.grad = grad;
   P.grad_stride = (long long)T * C;
   P.C = C;
-  P.zero_w = zero_w;
-  // launch_bidir_ctc's rule: the PAIR kernels (two nodes per thread) for gtnb_ctc_loss's own graphs; zero_w = 2
-  // asks for the general FX kernel on the same graphs
-  const bool ctc_ok = fx && (zero_w == 1 || zero_w == 3) && maxN <= 2 * 32 * bidir::kMaxPairWarps - 1;
-  const bool pair = ctc_ok && zero_w == 1, quad = ctc_ok && zero_w == 3; // 1: gtnb_ctc_loss's default, 3: "bidir_mode" 2
+  // launch_bidir_ctc's rule: the PAIR kernels (two nodes per thread) for gtnb_ctc_loss's own graphs
+  const bool pair = fx && bidir_mode != 0 && maxN <= 2 * 32 * bidir::kMaxPairWarps - 1;
   P.ctc_blank = blank;
   P.targets = targets;
   for (int b = 0; b < B; b++) meta[b].tgt_off = tgt_off[b];
-  P.nwn = quad ? 1 : pair ? std::max(1, ((maxN + 1) / 2 + 31) / 32) : std::max(1, (maxN + 31) / 32);
+  P.nwn = pair ? std::max(1, ((maxN + 1) / 2 + 31) / 32) : std::max(1, (maxN + 31) / 32);
   P.lay = bidir::make_layout(C, fx ? bidir::kFixedPitch : ((maxN + 3) & ~3));
-  const unsigned block = 32 * (P.nwn + 1 + bidir::kHelpers + (quad ? bidir::kQuadSpare : 0));
+  const unsigned block = 32 * (P.nwn + 1 + bidir::kHelpers);
   emu::launch_clusters(2 * B, 2, block, P.lay.total, [&] {
-    // ctc_build_kernel writes weight 0 on every arc: the zero-weight variant, as gtnb_ctc_loss launches it;
-    // zero_w = 0 exercises the general one on the same graphs
-    if (quad)
-      C == 64 ? bidir::bidir_ctc_kernel<1, true, true, 2>(P) : bidir::bidir_ctc_kernel<2, true, true, 2>(P);
-    else if (pair)
-      C == 64 ? bidir::bidir_ctc_kernel<1, true, true, 1>(P) : bidir::bidir_ctc_kernel<2, true, true, 1>(P);
+    if (pair)
+      C == 64 ? bidir::bidir_ctc_kernel<1, true, 1>(P) : bidir::bidir_ctc_kernel<2, true, 1>(P);
     else if (fx && C == 64)
-      zero_w ? bidir::bidir_ctc_kernel<1, true, true, 0>(P) : bidir::bidir_ctc_kernel<1, false, true, 0>(P);
+      bidir::bidir_ctc_kernel<1, true, 0>(P);
     else if (fx)
-      zero_w ? bidir::bidir_ctc_kernel<2, true, true, 0>(P) : bidir::bidir_ctc_kernel<2, false, true, 0>(P);
+      bidir::bidir_ctc_kernel<2, true, 0>(P);
     else if (C <= 64)
-      zero_w ? bidir::bidir_ctc_kernel<1, true, false, 0>(P) : bidir::bidir_ctc_kernel<1, false, false, 0>(P);
+      bidir::bidir_ctc_kernel<1, false, 0>(P);
     else
-      zero_w ? bidir::bidir_ctc_kernel<2, true, false, 0>(P) : bidir::bidir_ctc_kernel<2, false, false, 0>(P);
+      bidir::bidir_ctc_kernel<2, false, 0>(P);
   });
   if (emu::g_launch_failed.exchange(false)) return emu::kEmuNoThreads;
   for (int b = 0; b < B; b++) {

@@ -25,7 +25,7 @@ def emu():
     return lib
 
 
-def run(lib, e, targets, lens=None, blank=0, want_grad=True, zero_w=1):
+def run(lib, e, targets, lens=None, blank=0, want_grad=True, bidir_mode=-1):
     B, T, Cn = e.shape
     e = np.ascontiguousarray(e, np.float32)
     tl = np.asarray([len(t) for t in targets], np.int32)
@@ -36,7 +36,7 @@ def run(lib, e, targets, lens=None, blank=0, want_grad=True, zero_w=1):
     grad = np.zeros((B, T, Cn), np.float32) if want_grad else None
     status = np.zeros(B, np.int32)
     rc = lib.emu_bidir_ctc(B, T, Cn, e.ctypes.data_as(f32p), None if il is None else il.ctypes.data_as(i32p),
-                           cat.ctypes.data_as(i32p), tl.ctypes.data_as(i32p), blank, zero_w, out.ctypes.data_as(f32p),
+                           cat.ctypes.data_as(i32p), tl.ctypes.data_as(i32p), blank, bidir_mode, out.ctypes.data_as(f32p),
                            zn.ctypes.data_as(f32p), None if grad is None else grad.ctypes.data_as(f32p),
                            status.ctypes.data_as(i32p))
     emu_build.check(rc)
@@ -53,24 +53,23 @@ def run(lib, e, targets, lens=None, blank=0, want_grad=True, zero_w=1):
     (2, 1, 8, 0),      # T = 1, empty targets
     (2, 33, 8, 16),    # T = 2U + 1: a single feasible alignment per utterance
     (2, 8, 8, 2),      # T = 8: one block, everything in CTA B's first phase
-    (2, 12, 64, 0),    # PAIR / QUAD kernels on an empty target (one pair: the blank alone)
+    (2, 12, 64, 0),    # PAIR kernels on an empty target (one pair: the blank alone)
     (2, 20, 64, 1),    # ... and on a single label
-    (1, 232, 64, 111), # ... and on the longest target they take (223 nodes: 112 pairs, 28 lanes of the QUAD warp)
+    (1, 232, 64, 111), # ... and on the longest target they take (223 nodes: 112 pairs)
     (1, 24, 8, 3),     # T = 24: M = 16, the halves differ by a block
 ])
 def test_bidir_kernel_source_matches_oracle(emu, oracle, shape):
     from oracle import f64
     B, T, Cn, U = shape
     e, targets = util.bench_inputs(B, T, Cn, U, seed=77 + T)
-    # zero_w: 0 the general weighted kernel, 1 gtnb_ctc_loss's choice (C = 64 / 128: the PAIR kernels, two nodes per
-    # thread), 2 the general zero-weight kernel on the same graphs, 3 the QUAD kernels (one node warp, four pairs per
-    # thread; "bidir_mode" 2)
-    for zero_w in ((T % 2,) if Cn not in (64, 128) else (0, 1, 2, 3)):
-        check_one(emu, oracle, f64, e, targets, B, T, zero_w)
+    # bidir_mode: -1 gtnb_ctc_loss's choice (C = 64 / 128: the PAIR kernels, two nodes per thread), 0 the
+    # one-node-per-thread kernel on the same graphs
+    for bidir_mode in ((-1,) if Cn not in (64, 128) else (-1, 0)):
+        check_one(emu, oracle, f64, e, targets, B, T, bidir_mode)
 
 
-def check_one(emu, oracle, f64, e, targets, B, T, zero_w):
-    loss, grad, status = run(emu, e, targets, zero_w=zero_w)
+def check_one(emu, oracle, f64, e, targets, B, T, bidir_mode):
+    loss, grad, status = run(emu, e, targets, bidir_mode=bidir_mode)
     assert not status.any()
     for b in range(B):
         lo, go = oracle.ctc_loss(e[b], targets[b], 0, True)
@@ -108,17 +107,19 @@ def test_bidir_ragged_lengths_repeats_and_infeasible(emu, oracle, Cn):
 
 
 def test_bidir_loss_only_and_non_finite(emu, oracle):
-    B, T, Cn, U = 3, 50, 8, 6
-    e, targets = util.bench_inputs(B, T, Cn, U, seed=9)
-    loss, grad, status = run(emu, e, targets, want_grad=False)
-    assert grad is None and not status.any()
-    for b in range(B):
-        lo, _ = oracle.ctc_loss(e[b], targets[b], 0, False)
-        assert util.close(loss[b], lo)
-    e[1, 20, 3] = -np.inf
-    e[2, 40, 0] = np.nan
-    _, _, status = run(emu, e, targets)
-    assert status[0] == 0 and status[1] == 1 and status[2] == 1
+    # C = 8: the one-node-per-thread kernel; C = 64 / 128: the PAIR kernels, which loss-only calls take too
+    for Cn in (8, 64, 128):
+        B, T, U = 3, 50, 6
+        e, targets = util.bench_inputs(B, T, Cn, U, seed=9)
+        loss, grad, status = run(emu, e, targets, want_grad=False)
+        assert grad is None and not status.any()
+        for b in range(B):
+            lo, _ = oracle.ctc_loss(e[b], targets[b], 0, False)
+            assert util.close(loss[b], lo), (Cn, b, loss[b], lo)
+        e[1, 20, 3] = -np.inf
+        e[2, 40, 0] = np.nan
+        _, _, status = run(emu, e, targets)
+        assert status[0] == 0 and status[1] == 1 and status[2] == 1, Cn
 
 
 def test_bidir_benchmark_graph(emu, oracle):

@@ -18,7 +18,7 @@ def test_pair_meeting_row_in_b_only_block(emu, oracle, shape):
     from oracle import f64
     B, T, Cn, U = shape
     e, targets = util.bench_inputs(B, T, Cn, U, seed=131 + T)
-    check_one(emu, oracle, f64, e, targets, B, T, 1)
+    check_one(emu, oracle, f64, e, targets, B, T, -1)
 
 
 @pytest.mark.parametrize("T", [5, 40, 61])
@@ -26,7 +26,7 @@ def test_pair_loss_only(emu, oracle, T):
     """PAIR without a gradient: Z from the meeting row (labels and blanks of both CTAs) alone."""
     B, Cn, U = 2, 64, 6
     e, targets = util.bench_inputs(B, T, Cn, U, seed=17 + T)
-    loss, grad, status = run(emu, e, targets, want_grad=False, zero_w=1)
+    loss, grad, status = run(emu, e, targets, want_grad=False)
     assert grad is None and not status.any()
     for b in range(B):
         lo, _ = oracle.ctc_loss(e[b], targets[b], 0, False)

@@ -73,19 +73,11 @@ def run(lib, e, tables, lens):
 
 
 def float64_gradient(x, target):
-    """d loss / d emissions of the same lattice evaluated in float64 (scripts/banded_model.py): the
-    referee when two fp32 evaluations differ by more than the tolerance -- the oracle's own fp32
-    gradient is 5e-4 off it at T=270, C=8 (tests/golden/README.md has the T=1000 figures)."""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("banded_model", os.path.join(HERE, "..", "scripts", "banded_model.py"))
-    bm = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(bm)
-    w, lab, start, accept = bm.ctc_band(target)
-    S = bm.forward_plain(x, w, lab, start)
-    _, g = bm.backward_plain(x, w, lab, accept, S, delta=-1.0)
-    mx = x.max(1, keepdims=True)
-    lse = mx[:, 0] + np.log(np.exp(x - mx).sum(1))
-    return np.exp(x - lse[:, None]) + g
+    """d loss / d emissions of the same lattice evaluated in float64 (oracle/f64.py): the referee when two
+    fp32 evaluations differ by more than the tolerance -- the oracle's own fp32 gradient is 5e-4 off it at
+    T=270, C=8 (tests/golden/README.md has the T=1000 figures)."""
+    from oracle import f64
+    return f64.ctc_f64(x, target)[1]
 
 
 def check_against_oracle(oracle, e, targets, lens, out, grad, T):
@@ -168,9 +160,8 @@ def test_ctc_build_kernel_then_sweeps(emu, oracle, shape):
 
 def test_kernel_sources_at_the_benchmark_shape_against_the_reference_golden(emu):
     """One utterance of BASELINE config 2 (T=1000, C=64, U=100: 201 graph nodes, 7 node warps) through the
-    source of k_ctc.cu + k_implicit.cu, and through k_banded.cu at K=4, against the golden vector generated
-    from the real reference (tests/golden/make_golden.py) and its float64 evaluation."""
-    import ctypes
+    source of k_ctc.cu + k_implicit.cu against the golden vector generated from the real reference
+    (tests/golden/make_golden.py) and its float64 evaluation."""
     gold = np.load(os.path.join(HERE, "golden", "reference_golden.npz"))
     e, tg = util.bench_inputs(1, 1000, 64, 100)
     T, Cn = 1000, 64
@@ -179,21 +170,6 @@ def test_kernel_sources_at_the_benchmark_shape_against_the_reference_golden(emu)
     lse = mx[:, 0] + np.log(np.exp(x - mx).sum(1))
     soft = np.exp(x - lse[:, None])
 
-    def check(out, grad, what):
-        loss = float(lse.sum() - np.float64(out[0]))
-        assert util.close(loss, gold["c2_loss"][0]), (what, loss, gold["c2_loss"][0])
-        assert abs(loss - float(gold["c2_loss_f64"])) < 1e-3 * abs(loss)
-        g = soft + grad[0]
-        # two fp32 evaluations of this lattice differ by ~1e-3 (tests/golden/README.md): the float64
-        # gradient is the referee, and the kernel must be no further from it than the reference is
-        g64 = gold["c2_grad_f64"]  # [T][C]
-        assert g64.shape == g.shape
-        err_kernel = np.abs(g - g64).max()
-        err_reference = np.abs(gold["c2_grad"][0] - g64).max()
-        assert util.grad_close(g, gold["c2_grad"][0], 5.0 * T) or err_kernel <= err_reference, (what, err_kernel)
-        assert np.allclose(-grad[0].sum(1), 1.0, atol=2e-3)
-
-    # k_ctc.cu + k_implicit.cu
     cat = np.ascontiguousarray(tg[0], np.int32)
     tl = np.array([len(tg[0])], np.int32)
     lens = np.array([T], np.int32)
@@ -206,20 +182,18 @@ def test_kernel_sources_at_the_benchmark_shape_against_the_reference_golden(emu)
                               status.ctypes.data_as(i32p), None, None, None)
     emu_build.check(rc)
     assert not status.any()
-    check(out, grad, "implicit")
-
-    # k_banded.cu, K = 4
-    lib = ctypes.CDLL(emu_build.build("banded", ["k_banded.cu"]))
-    lib.emu_banded_ctc.argtypes = [C.c_int, C.c_int, C.c_int, f32p, i32p, i32p, i32p, C.c_int, C.c_int, f32p, f32p, i32p]
-    out2 = np.zeros(1, np.float32)
-    grad2 = np.zeros((1, T, Cn), np.float32)
-    status2 = np.zeros(1, np.int32)
-    rc = lib.emu_banded_ctc(1, T, Cn, ee.ctypes.data_as(f32p), lens.ctypes.data_as(i32p), cat.ctypes.data_as(i32p),
-                            tl.ctypes.data_as(i32p), 0, 4, out2.ctypes.data_as(f32p), grad2.ctypes.data_as(f32p),
-                            status2.ctypes.data_as(i32p))
-    emu_build.check(rc)
-    assert not status2.any()
-    check(out2, grad2, "banded")
+    loss = float(lse.sum() - np.float64(out[0]))
+    assert util.close(loss, gold["c2_loss"][0]), (loss, gold["c2_loss"][0])
+    assert abs(loss - float(gold["c2_loss_f64"])) < 1e-3 * abs(loss)
+    g = soft + grad[0]
+    # two fp32 evaluations of this lattice differ by ~1e-3 (tests/golden/README.md): the float64
+    # gradient is the referee, and the kernel must be no further from it than the reference is
+    g64 = gold["c2_grad_f64"]  # [T][C]
+    assert g64.shape == g.shape
+    err_kernel = np.abs(g - g64).max()
+    err_reference = np.abs(gold["c2_grad"][0] - g64).max()
+    assert util.grad_close(g, gold["c2_grad"][0], 5.0 * T) or err_kernel <= err_reference, err_kernel
+    assert np.allclose(-grad[0].sum(1), 1.0, atol=2e-3)
 
 
 def general_tables(og, Cn):
