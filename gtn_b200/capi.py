@@ -116,6 +116,12 @@ SYMBOLS = [
     ("gtnb_graph_transitions_viterbi", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.c_int, _vp, C.c_int,
       _vp, _vp, _vp, C.c_int]),
+    ("gtnb_viterbi_sparse", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _vp, _vp, _vp,
+      C.c_int]),
+    ("gtnb_sparse_transitions_viterbi", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.POINTER(GraphView),
+      _vp, C.c_int, _vp, _vp, _vp, C.c_int]),
 ]
 
 _lib = None
@@ -586,6 +592,60 @@ class Ctx:
                 p.inp(tw, trans_on_device), int(trans_on_device), *map(p.out, out), p.flag))
         return _viterbi_results(out, B, T)
 
+    def viterbi_sparse(self, emissions, transitions, trans_w, input_lens=None):
+        """Host-buffer entry of gtnb_viterbi_sparse: emissions [B,T,C], transitions: G's (view, keepalive) pair (an
+        acceptor; its weights are ignored), trans_w [G.num_arcs] -> (paths [B,T] int32, scores [B], arcs [B,T] int32:
+        G's arc per frame)."""
+        return self._viterbi_sparse(False, emissions, transitions, trans_w, input_lens, False)
+
+    def viterbi_sparse_dev(self, emissions, transitions, trans_w, input_lens=None, trans_on_device=True):
+        """Device-buffer entry: emissions (and trans_w unless trans_on_device is False) uploaded once,
+        gtnb_viterbi_sparse on device pointers (outputs in HBM), downloaded afterwards -> (paths, scores, arcs)."""
+        return self._viterbi_sparse(True, emissions, transitions, trans_w, input_lens, bool(trans_on_device))
+
+    def _viterbi_sparse(self, dev, emissions, transitions, trans_w, input_lens, trans_on_device):
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        gv = transitions[0]
+        tw = _sparse_trans_w(gv, trans_w)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        out = _viterbi_outputs(B, T)
+        with _Placed(self, dev) as p:
+            self._check(lib().gtnb_viterbi_sparse(
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), C.byref(gv), p.inp(tw, trans_on_device),
+                int(trans_on_device), *map(p.out, out), p.flag))
+        return _viterbi_results(out, B, T)
+
+    def sparse_transitions_viterbi(self, emissions, views, transitions, trans_w, input_lens=None, arc_weights=None):
+        """Host-buffer entry of gtnb_sparse_transitions_viterbi: emissions [B,T,C], views: B (view, keepalive) pairs
+        from make_view, transitions: G's (view, keepalive) pair, trans_w [G.num_arcs], arc_weights [sum A_b] or None
+        -> (paths [B,T] int32, scores [B], arcs [B,T] int32: A_b's arc per frame)."""
+        return self._sparse_transitions_viterbi(False, emissions, views, transitions, trans_w, input_lens, arc_weights,
+                                                False)
+
+    def sparse_transitions_viterbi_dev(self, emissions, views, transitions, trans_w, input_lens=None,
+                                       arc_weights=None, trans_on_device=True):
+        """Device-buffer entry: emissions (and arc_weights, when given; trans_w unless trans_on_device is False)
+        uploaded once, gtnb_sparse_transitions_viterbi on device pointers (outputs in HBM), downloaded afterwards
+        -> (paths, scores, arcs)."""
+        return self._sparse_transitions_viterbi(True, emissions, views, transitions, trans_w, input_lens, arc_weights,
+                                                bool(trans_on_device))
+
+    def _sparse_transitions_viterbi(self, dev, emissions, views, transitions, trans_w, input_lens, arc_weights,
+                                    trans_on_device):
+        e = np.ascontiguousarray(emissions, dtype=np.float32)
+        B, T, Cn = e.shape
+        arr, _, aw = _graph_batch(views, B, arc_weights)
+        gv = transitions[0]
+        tw = _sparse_trans_w(gv, trans_w)
+        il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
+        out = _viterbi_outputs(B, T)
+        with _Placed(self, dev) as p:
+            self._check(lib().gtnb_sparse_transitions_viterbi(
+                self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, C.byref(gv),
+                p.inp(tw, trans_on_device), int(trans_on_device), *map(p.out, out), p.flag))
+        return _viterbi_results(out, B, T)
+
 
 class Lattice:
     def __init__(self, ctx, h, keep=None):
@@ -728,6 +788,16 @@ def _viterbi_results(out, B, T):
     """-> (paths [B,T], scores [B], arcs [B,T])"""
     paths, arcs, scores = out
     return paths.ravel()[:B * T].reshape(B, T), scores[:B], arcs.ravel()[:B * T].reshape(B, T)
+
+
+def _sparse_trans_w(gv, trans_w):
+    """trans_w as float32 for a G of gv.num_arcs arcs (None stays None, for the argument checks); an empty G gets a
+    one-element buffer that is never read"""
+    if trans_w is None:
+        return None
+    tw = np.ascontiguousarray(trans_w, dtype=np.float32).ravel()
+    assert tw.size == gv.num_arcs
+    return tw if tw.size else np.zeros(1, np.float32)
 
 
 def _cat_targets(targets):

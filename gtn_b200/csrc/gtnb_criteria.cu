@@ -1670,20 +1670,14 @@ extern "C" int gtnb_graph_transitions_loss(
  */
 namespace {
 
-/* trellis_loss_fast's denominator for a G of any shape: G's tables and start groups in one device buffer */
-struct SparseDenominator {
-  const SparseTables& t;
-  long long n_trans; // G's arcs, labels outside [0, C) included
+/* G's tables and start groups (gtnb_product.h) in one device buffer, filled by stage() */
+struct SparseDevTables {
   std::vector<int32_t> packed;
   int32_t* tab = nullptr;
-  float* alpha = nullptr;
-  double* offs = nullptr;
   SparseDev dev{};
   const int32_t *grp_ptr = nullptr, *grp_arc = nullptr;
 
-  int groups() const { return (int)t.grp_ptr.size() - 1; }
-  long long n_sigma(int) const { return groups(); }
-  int alloc(CallScope& scope, int B, int T) {
+  int alloc(CallScope& scope, const SparseTables& t) {
     packed.assign(t.flags.begin(), t.flags.end());
     std::vector<size_t> at;
     for (const std::vector<int32_t>* v : {&t.in_ptr, &t.in_src, &t.in_lab, &t.in_arc, &t.out_ptr, &t.out_dst,
@@ -1696,23 +1690,51 @@ struct SparseDenominator {
                     tab + at[4], tab + at[5], tab + at[6], tab + at[7]};
     grp_ptr = tab + at[8];
     grp_arc = tab + at[9];
+    return GTNB_OK;
+  }
+  int stage(CallScope& scope) { return stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()); }
+};
+
+/* G's arcs with a label in [0, C), weighted from the host weights W; gmap (nullable) gets each one's arc id */
+void sparse_host_graph(const gtnb_graph_view& Gv, const SparseTables& t, int C, const float* W, HostGraph* G,
+                       std::vector<int32_t>* gmap) {
+  G->flags = t.flags;
+  for (int g = 0; g < Gv.num_arcs; g++)
+    if (Gv.arc_olabel[g] >= 0 && Gv.arc_olabel[g] < C) {
+      G->arc(Gv.arc_src[g], Gv.arc_dst[g], Gv.arc_olabel[g], W[g]);
+      if (gmap) gmap->push_back(g);
+    }
+}
+
+/* trellis_loss_fast's denominator for a G of any shape: G's tables and start groups in one device buffer */
+struct SparseDenominator {
+  const SparseTables& t;
+  long long n_trans; // G's arcs, labels outside [0, C) included
+  SparseDevTables tabs;
+  float* alpha = nullptr;
+  double* offs = nullptr;
+
+  int groups() const { return (int)t.grp_ptr.size() - 1; }
+  long long n_sigma(int) const { return groups(); }
+  int alloc(CallScope& scope, int B, int T) {
+    GTNB_TRY(tabs.alloc(scope, t));
     GTNB_TRY(scope.alloc(&alpha, (long long)B * (T + 1) * t.S));
     return scope.alloc(&offs, (long long)B * (T + 1));
   }
-  int stage(CallScope& scope) { return stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()); }
+  int stage(CallScope& scope) { return tabs.stage(scope); }
   int sigma(gtnb_ctx* ctx, int, const float* w, float* sig) {
-    return launch_sparse_sigma(ctx, groups(), grp_ptr, grp_arc, w, sig);
+    return launch_sparse_sigma(ctx, groups(), tabs.grp_ptr, tabs.grp_arc, w, sig);
   }
   int forward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
               float* den, int32_t* status) {
-    return launch_sparse_den_forward(ctx, dev, B, T, C, lens, e, per, w, alpha, offs, den, status);
+    return launch_sparse_den_forward(ctx, tabs.dev, B, T, C, lens, e, per, w, alpha, offs, den, status);
   }
   int backward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
                const float*, float* grad, float* wgrad) {
-    return launch_sparse_den_backward(ctx, dev, B, T, C, lens, e, per, w, alpha, offs, grad, per, wgrad);
+    return launch_sparse_den_backward(ctx, tabs.dev, B, T, C, lens, e, per, w, alpha, offs, grad, per, wgrad);
   }
   int fold_grad(gtnb_ctx* ctx, int, const float* w, const float* sig, float* wgrad) {
-    return launch_sparse_fold(ctx, groups(), grp_ptr, grp_arc, (int)n_trans, w, sig, wgrad);
+    return launch_sparse_fold(ctx, groups(), tabs.grp_ptr, tabs.grp_arc, (int)n_trans, w, sig, wgrad);
   }
 };
 
@@ -1765,13 +1787,7 @@ extern "C" int gtnb_sparse_transitions_loss(
                            return transitions_exact(
                                scope, a, gb, n_trans,
                                [&](const float* W, HostGraph* G, std::vector<int32_t>* gmap) {
-                                 // G's arcs with a label in [0, C)
-                                 G->flags = t.flags;
-                                 for (int g = 0; g < Gv.num_arcs; g++)
-                                   if (Gv.arc_olabel[g] >= 0 && Gv.arc_olabel[g] < C) {
-                                     G->arc(Gv.arc_src[g], Gv.arc_dst[g], Gv.arc_olabel[g], W[g]);
-                                     gmap->push_back(g);
-                                   }
+                                 sparse_host_graph(Gv, t, C, W, G, gmap);
                                },
                                [&](const gtnb_graph_view& v, ProductGraph* p) {
                                  build_sparse_product(v, Gv, t, C, /*fold=*/false, p);
@@ -1822,14 +1838,18 @@ std::vector<int32_t> arc_ids(const std::vector<gtnb_graph_view>& views) {
  * The materialised route for the utterances `which`: gtnb_compose_linear (the lattice is put in the reference's
  * relaxation order while exact_ties is on, k_order.cu), gtnb_forward(tropical) for the score and gtnb_viterbi_path.
  * views: one per utterance, with host weights.  A_b is matched on its olabels, so its ilabels play no part in the
- * composition: they are replaced by the arc ids, which the path's ilabels then carry back.  The rows are written into
- * the device outputs v.p_dev / v.a_dev (nullable) and v.s_dev.  arc_map (nullable): per utterance, the arc the caller
- * reports for each arc of views[b] (gtnb_graph_transitions_viterbi: views[b] is compose(A_b, G), the map its gradInfo
- * into A_b).
+ * composition: they are replaced by the arc ids, which the path's ilabels then carry back.  linear_first
+ * (gtnb_viterbi_sparse): views holds one graph G shared by the batch, matched on its ilabels, and the lattice is
+ * compose(E_b, G) -- the reference's intersect(E_b, G) -- with G's olabels replaced by the arc ids instead.  The rows
+ * are written into the device outputs v.p_dev / v.a_dev (nullable) and v.s_dev.  arc_map (nullable): per utterance,
+ * the arc the caller reports for each arc of views[b] (gtnb_graph_transitions_viterbi: views[b] is compose(A_b, G),
+ * the map its gradInfo into A_b).  The utterances run in groups whose lattices fit the device memory together (a
+ * tie-heavy batch does not materialise every lattice at once); one that does not fit alone is
+ * GTNB_ERR_UNSUPPORTED, from gtnb_compose_linear.
  */
 int graph_viterbi_exact(CallScope& scope, const GraphBatch& gb, const std::vector<gtnb_graph_view>& views,
                         const ViterbiBufs& v, const std::vector<int>& which,
-                        const std::vector<std::vector<int32_t>>* arc_map = nullptr) {
+                        const std::vector<std::vector<int32_t>>* arc_map = nullptr, bool linear_first = false) {
   gtnb_ctx* ctx = scope.ctx();
   const int T = gb.T, C = gb.C, ml = std::max(T, 1);
   const long long per = (long long)T * C;
@@ -1841,27 +1861,58 @@ int graph_viterbi_exact(CallScope& scope, const GraphBatch& gb, const std::vecto
   const int n = (int)sub.size();
   std::vector<float> sc(std::max(n, 1), -std::numeric_limits<float>::infinity());
   std::vector<int32_t> parc((size_t)std::max(n, 1) * ml, -1), plab(parc.size(), -1), plen(std::max(n, 1), -1);
-  if (n > 0) {
-    std::vector<gtnb_graph_view> sv(n);
-    std::vector<int32_t> sT(n);
-    const float* e_sub = v.e_dev;
-    if (n < gb.B) {
-      float* e_copy = nullptr;
-      GTNB_TRY(scope.alloc(&e_copy, per * n));
-      for (int k = 0; k < n; k++)
-        GTNB_CUDA(ctx, cudaMemcpyAsync(e_copy + per * k, v.e_dev + per * sub[k], sizeof(float) * per,
-                                       cudaMemcpyDeviceToDevice, ctx->stream));
-      e_sub = e_copy;
+  const float* e_sub = v.e_dev;
+  if (n > 0 && n < gb.B) {
+    float* e_copy = nullptr;
+    GTNB_TRY(scope.alloc(&e_copy, per * n));
+    for (int k = 0; k < n; k++)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(e_copy + per * k, v.e_dev + per * sub[k], sizeof(float) * per,
+                                     cudaMemcpyDeviceToDevice, ctx->stream));
+    e_sub = e_copy;
+  }
+  // the groups' budget: half of the device memory still free (this call's own buffers, e.g. the decode's
+  // back-pointers, already count as used), the rest left to gtnb_forward and gtnb_viterbi_path
+  size_t free_b = 0, total_b = 0;
+  GTNB_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+  const unsigned long long budget = std::min<unsigned long long>(free_b, ctx->total_mem ? ctx->total_mem : free_b) / 2;
+  for (int k0 = 0, k1 = 0; k0 < n; k0 = k1) {
+    // the group [k0, k1): the bytes gtnb_compose_linear asks for its lattice (gtnb_capi.cu: every graph's node, arc
+    // and level slabs, then one alive bit per frame and node of the largest graph), within the budget
+    unsigned long long slabs = 0;
+    long long maxN = 0, maxT = 0;
+    for (; k1 < n; k1++) {
+      const gtnb_graph_view& g = views[linear_first ? 0 : sub[k1]];
+      const long long Tb = gb.Tb[sub[k1]], N = g.num_nodes;
+      const unsigned long long s = 8ull * align_up((Tb + 1) * N + 1, kAlign) +
+                                   20ull * align_up(std::max(Tb * g.num_arcs, 1ll), kAlign) +
+                                   8ull * align_up(Tb + 2, kAlign);
+      const long long mN = std::max(maxN, N), mT = std::max(maxT, Tb);
+      const unsigned long long need = slabs + s + 4ull * (k1 - k0 + 1) * (mT + 1) * ((mN + 31) / 32);
+      if (k1 > k0 && need > budget) break;
+      slabs += s;
+      maxN = mN;
+      maxT = mT;
     }
-    for (int k = 0; k < n; k++) {
-      sv[k] = views[sub[k]];
-      sv[k].arc_ilabel = ids.data();
-      sT[k] = gb.Tb[sub[k]];
+    const int m = k1 - k0;
+    std::vector<gtnb_graph_view> sv(linear_first ? 1 : m);
+    std::vector<int32_t> sT(m);
+    for (int k = 0; k < m; k++) {
+      if (k < (int)sv.size()) {
+        sv[k] = views[linear_first ? 0 : sub[k0 + k]];
+        (linear_first ? sv[k].arc_olabel : sv[k].arc_ilabel) = ids.data();
+      }
+      sT[k] = gb.Tb[sub[k0 + k]];
     }
     gtnb_lattice*& lat = scope.lattice();
-    GTNB_TRY(gtnb_compose_linear(ctx, n, sv.data(), n, 0, sT.data(), C, e_sub, per, &lat));
-    GTNB_TRY(gtnb_forward(ctx, lat, 1, sc.data(), nullptr));
-    GTNB_TRY(gtnb_viterbi_path(ctx, lat, ml, nullptr, parc.data(), plab.data(), nullptr, plen.data(), nullptr));
+    GTNB_TRY(gtnb_compose_linear(ctx, m, sv.data(), (int)sv.size(), linear_first ? 1 : 0, sT.data(), C,
+                                 e_sub + per * k0, per, &lat));
+    GTNB_TRY(gtnb_forward(ctx, lat, 1, sc.data() + k0, nullptr));
+    // the arc ids are the path's ilabels (A_b) or olabels (G, linear_first)
+    int32_t* ia = (linear_first ? plab : parc).data() + (size_t)k0 * ml;
+    int32_t* oa = (linear_first ? parc : plab).data() + (size_t)k0 * ml;
+    GTNB_TRY(gtnb_viterbi_path(ctx, lat, ml, nullptr, ia, oa, nullptr, plen.data() + k0, nullptr));
+    gtnb_lattice_destroy(ctx, lat); // (gtnb_viterbi_path has synchronised)
+    lat = nullptr;
   }
   // the rows of every utterance in `which` (T_b = 0: score -inf, no path), staged on the host and copied from
   // pageable memory (each copy has left the host buffer when it returns)
@@ -1991,18 +2042,15 @@ extern "C" int gtnb_graph_viterbi(
  */
 namespace {
 
-int graph_transitions_viterbi_exact(CallScope& scope, const GraphBatch& gb, bool bigram, const float* trans_w,
-                                    int trans_on_device, const ViterbiBufs& vb, const std::vector<int>& which) {
+/* the exact route for the utterances `which`: compose(A'_b, G) on the device in the reference's numbering, G (gv,
+ * host weights) the second operand, then graph_viterbi_exact through the composed graphs' gradInfo into A_b */
+int graph_transitions_viterbi_exact(CallScope& scope, const char* fn, const GraphBatch& gb, const gtnb_graph_view& gv,
+                                    const ViterbiBufs& vb, const std::vector<int>& which) {
   gtnb_ctx* ctx = scope.ctx();
-  const int B = gb.B, C = gb.C;
-  const long long n_trans = dense_trans_count(bigram, C);
-  std::vector<float> W(n_trans), host_w;
-  GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
+  const int B = gb.B;
+  std::vector<float> host_w;
   std::vector<gtnb_graph_view> views;
   GTNB_TRY(gb.host_views(ctx, &host_w, &views));
-  HostGraph G;
-  dense_graph(bigram, C, W.data(), &G, nullptr);
-  const gtnb_graph_view gv = G.view();
   // A'_b: A_b with its ilabels replaced by the arc ids (A_b is matched on its olabels, so the composition is the
   // same); the pairs that can accept anything
   const std::vector<int32_t> ids = arc_ids(views);
@@ -2035,7 +2083,7 @@ int graph_transitions_viterbi_exact(CallScope& scope, const GraphBatch& gb, bool
       int32_t N = 0, A = 0;
       rc = gtnb_composed_sizes(res, k, &N, &A);
       if (rc != GTNB_OK) {
-        rc = fail(ctx, rc, "gtnb_graph_transitions_viterbi: sizes of a composed graph");
+        rc = fail(ctx, rc, std::string(fn) + ": sizes of a composed graph");
         break;
       }
       Composed& c = cg[k];
@@ -2062,28 +2110,57 @@ int graph_transitions_viterbi_exact(CallScope& scope, const GraphBatch& gb, bool
   return graph_viterbi_exact(scope, gb, cviews, vb, which, &arc_map);
 }
 
-int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, bool bigram,
-                                  const float* trans_w, int trans_on_device) {
+/* the weights of the folded start arcs of a dense kind's products: BIGRAM's tau_l = max_j W[l][j], none for ASG */
+struct DenseTau {
+  bool bigram;
+  int C;
+  float* tau = nullptr;
+  int alloc(CallScope& scope) { return bigram ? scope.alloc(&tau, C) : GTNB_OK; }
+  int stage(CallScope&) { return GTNB_OK; }
+  int launch(gtnb_ctx* ctx, const float* w) { return bigram ? launch_ngram_tau(ctx, C, w, tau) : GTNB_OK; }
+};
+
+/* ... and of a G of any shape: tau_k = max over G's start group k (gtnb_product.h) */
+struct SparseTau {
+  const SparseTables& t;
+  std::vector<int32_t> packed;
+  int32_t* tab = nullptr;
+  float* tau = nullptr;
+  int groups() const { return (int)t.grp_ptr.size() - 1; }
+  int alloc(CallScope& scope) {
+    packed = t.grp_ptr;
+    packed.insert(packed.end(), t.grp_arc.begin(), t.grp_arc.end());
+    GTNB_TRY(scope.alloc(&tab, (long long)packed.size()));
+    return scope.alloc(&tau, std::max(groups(), 1));
+  }
+  int stage(CallScope& scope) { return stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()); }
+  int launch(gtnb_ctx* ctx, const float* w) {
+    return launch_sparse_tau(ctx, groups(), tab, tab + t.grp_ptr.size(), w, tau);
+  }
+};
+
+/*
+ * The Viterbi alignment of the transitions losses' numerators.  prods: the device route's (folded) products, taken
+ * when `fast`; tau: the weights of their folded start arcs, slots n_trans... of Wx; make_G(W, &G): G from the
+ * n_trans host weights, for the exact route.
+ */
+template <class Tau, class MakeG>
+int transitions_viterbi_run(CallScope& scope, const char* fn, const GraphViterbiArgs& a, const GraphBatch& gb,
+                            const std::vector<ProductGraph>& prods, bool fast, long long n_trans, const float* trans_w,
+                            int trans_on_device, Tau& tau, MakeG&& make_G) {
   gtnb_ctx* ctx = scope.ctx();
   const int B = gb.B, T = gb.T, C = gb.C;
-  const long long n_trans = dense_trans_count(bigram, C);
   ViterbiBufs v;
   GTNB_TRY(viterbi_open(scope, a, gb, &v));
-
-  // the loss's numerators (BIGRAM folded), whose shapes decide whether the device route can be taken
-  std::vector<ProductGraph> prods;
-  const bool fits = device_products(
-      gb, [&](const gtnb_graph_view& view, ProductGraph* p) { build_product(view, C, bigram, /*fold=*/true, p); },
-      &prods);
-  bool implicit = ctx->use_implicit && fits;
+  bool implicit = ctx->use_implicit && fast;
   GraphNumerator num{gb, prods, (int)n_trans, nullptr, 0};
   gtnb_lattice*& lat = scope.lattice();
   if (implicit) {
     GTNB_TRY(num.alloc(scope, v.e_dev, (long long)T * C, nullptr));
-    float *w_dev = nullptr, *tau = nullptr;
+    float* w_dev = nullptr;
     long long* off = nullptr;
-    GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, n_trans, &w_dev));
-    if (bigram) GTNB_TRY(scope.alloc(&tau, C));
+    GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, std::max(n_trans, 1ll), &w_dev));
+    GTNB_TRY(tau.alloc(scope));
     // off: every utterance's first product arc, then its first A arc (launch_product_arc_map)
     std::vector<long long> off_h(2 * (size_t)B, 0);
     for (int b = 0; b < B; b++) {
@@ -2093,11 +2170,12 @@ int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, c
     if (v.a_dev) GTNB_TRY(scope.alloc(&off, 2ll * B));
     GTNB_TRY(stage_begin(ctx));
     GTNB_TRY(num.stage(scope, nullptr));
+    GTNB_TRY(tau.stage(scope));
     if (!trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
     if (off) GTNB_TRY(stage_upload(ctx, off, off_h.data(), sizeof(long long) * 2 * B));
     GTNB_TRY(stage_end(ctx));
-    if (bigram) GTNB_TRY(launch_ngram_tau(ctx, C, w_dev, tau));
-    GTNB_TRY(implicit_or_materialise(num.build(scope, lat, w_dev, tau), &implicit));
+    GTNB_TRY(tau.launch(ctx, w_dev));
+    GTNB_TRY(implicit_or_materialise(num.build(scope, lat, w_dev, tau.tau), &implicit));
     implicit = implicit && implicit_trace_supported(lat);
     if (implicit) {
       GTNB_TRY(launch_implicit_forward(ctx, lat, v.status, 0, -1, /*tropical=*/true));
@@ -2106,8 +2184,26 @@ int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, c
     }
   }
   return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
-    return graph_transitions_viterbi_exact(scope, gb, bigram, trans_w, trans_on_device, v, which);
+    std::vector<float> W(std::max(n_trans, 1ll));
+    if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
+    HostGraph G;
+    make_G(W.data(), &G);
+    return graph_transitions_viterbi_exact(scope, fn, gb, G.view(), v, which);
   });
+}
+
+int graph_transitions_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, bool bigram,
+                                  const float* trans_w, int trans_on_device) {
+  const int C = gb.C;
+  // the loss's numerators (BIGRAM folded), whose shapes decide whether the device route can be taken
+  std::vector<ProductGraph> prods;
+  const bool fits = device_products(
+      gb, [&](const gtnb_graph_view& view, ProductGraph* p) { build_product(view, C, bigram, /*fold=*/true, p); },
+      &prods);
+  DenseTau tau{bigram, C};
+  return transitions_viterbi_run(scope, "gtnb_graph_transitions_viterbi", a, gb, prods, fits,
+                                 dense_trans_count(bigram, C), trans_w, trans_on_device, tau,
+                                 [&](const float* W, HostGraph* G) { dense_graph(bigram, C, W, G, nullptr); });
 }
 
 } // namespace
@@ -2127,4 +2223,111 @@ extern "C" int gtnb_graph_transitions_viterbi(
                                        GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,
                                                         outputs_on_device},
                                        gb, kind == GTNB_DENSE_BIGRAM, trans_w, trans_on_device);
+}
+
+/*
+ * Viterbi decoding and alignment with a learned transition graph G of any shape (gtnb_sparse_transitions_loss's G):
+ *   gtnb_viterbi_sparse:              viterbiPath / viterbiScore of intersect(E_b, G), the decode;
+ *   gtnb_sparse_transitions_viterbi:  ... of intersect(intersect(A_b, G), E_b), the loss's numerator.
+ * The decode's device route sweeps G's tables in the tropical semiring (k_sparse.cu) and traces the path back from
+ * 16-bit back-pointers; its exact route composes E_b with G, G's olabels replaced by its arc ids, so that the path's
+ * olabels carry the arcs back.  The alignment is graph_transitions_viterbi's sequence with the loss's folded sparse
+ * products, whose folded start arcs weigh tau_k = max over G's start group k.  Both take their exact route per
+ * utterance on a non-finite value or a tie (exact_ties on), and for the whole batch outside the kernels' layout or
+ * with the implicit flag off; only the exact routes read trans_w to the host.
+ */
+namespace {
+
+int viterbi_sparse_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
+                       const float* trans_w, int trans_on_device) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = gb.B, T = gb.T, C = gb.C;
+  const long long n_trans = Gv.num_arcs;
+  ViterbiBufs v;
+  GTNB_TRY(viterbi_open(scope, a, gb, &v));
+  SparseTables t;
+  sparse_tables(Gv, C, &t);
+  const bool implicit = ctx->use_implicit && sparse_den_supported(t.S, t.A, C);
+  if (implicit) {
+    SparseDevTables tabs;
+    GTNB_TRY(tabs.alloc(scope, t));
+    float* w_dev = nullptr;
+    int32_t *T_dev = nullptr, *head = nullptr;
+    uint16_t* bp = nullptr;
+    GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, std::max(n_trans, 1ll), &w_dev));
+    GTNB_TRY(scope.alloc(&T_dev, B));
+    GTNB_TRY(scope.alloc(&head, B));
+    GTNB_TRY(scope.alloc(&bp, std::max((long long)B * T * t.S, 1ll)));
+    GTNB_TRY(stage_begin(ctx));
+    GTNB_TRY(tabs.stage(scope));
+    GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
+    if (!trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
+    GTNB_TRY(stage_end(ctx));
+    GTNB_TRY(launch_sparse_viterbi(ctx, tabs.dev, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head, v.s_dev,
+                                   v.p_dev, v.a_dev, v.status));
+  }
+  return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
+    std::vector<float> W(std::max(n_trans, 1ll));
+    if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
+    gtnb_graph_view g = Gv;
+    g.weights = W.data();
+    return graph_viterbi_exact(scope, gb, {g}, v, which, nullptr, /*linear_first=*/true);
+  });
+}
+
+} // namespace
+
+extern "C" int gtnb_viterbi_sparse(gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device,
+                                   const int32_t* input_lens, const gtnb_graph_view* transitions, const float* trans_w,
+                                   int trans_on_device, int32_t* paths, int32_t* arcs, float* scores,
+                                   int outputs_on_device) {
+  const std::string fn = "gtnb_viterbi_sparse";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !transitions || (B > 0 && (!emissions || !trans_w)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  GTNB_TRY(check_transition_graph(ctx, fn, *transitions));
+  GraphBatch gb; // the batch without target graphs: its lengths
+  gb.B = B, gb.T = T, gb.C = C;
+  gb.Tb.resize(B);
+  for (int b = 0; b < B; b++) {
+    gb.Tb[b] = input_lens ? input_lens[b] : T;
+    if (gb.Tb[b] < 0 || gb.Tb[b] > T) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": input_lens outside [0, T]");
+  }
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  return viterbi_sparse_run(scope, GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,
+                                                    outputs_on_device},
+                            gb, *transitions, trans_w, trans_on_device);
+}
+
+extern "C" int gtnb_sparse_transitions_viterbi(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
+    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, int32_t* paths, int32_t* arcs,
+    float* scores, int outputs_on_device) {
+  const std::string fn = "gtnb_sparse_transitions_viterbi";
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, C, emissions, graphs, transitions && (B == 0 || trans_w), input_lens,
+                        arc_weights, arc_weights_on_device, &gb,
+                        [&] { return check_transition_graph(ctx, fn, *transitions); }));
+  if (B == 0) return GTNB_OK;
+  const gtnb_graph_view& Gv = *transitions;
+  SparseTables t;
+  sparse_tables(Gv, C, &t);
+  // the loss's numerators (folded), whose shapes decide, with G's, whether the device route can be taken
+  std::vector<ProductGraph> prods;
+  const bool fast = ctx->use_implicit && sparse_den_supported(t.S, t.A, C) &&
+                    device_products(
+                        gb,
+                        [&](const gtnb_graph_view& v, ProductGraph* p) {
+                          build_sparse_product(v, Gv, t, C, /*fold=*/true, p);
+                        },
+                        &prods);
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  SparseTau tau{t};
+  return transitions_viterbi_run(
+      scope, fn.c_str(), GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores, outputs_on_device}, gb, prods, fast,
+      Gv.num_arcs, trans_w, trans_on_device, tau,
+      [&](const float* W, HostGraph* G) { sparse_host_graph(Gv, t, C, W, G, nullptr); });
 }

@@ -392,6 +392,14 @@ int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, 
                                const float* emis, long long stride, const float* w, const float* alpha,
                                const double* offs, float* grad, long long grad_stride, float* wgrad);
 // sigma_k = logsumexp of start group k's weights, and its gradient (wgrad[nG + k]) folded back by softmax
+// gtnb_viterbi_sparse over the same tables: the tropical sweep (bp: [B][T][S] back-pointers, head: [B] best accept
+// nodes, score: [B]) and the traceback into paths / arcs ([B][T], nullable); status bit 1 non-finite, bit 2 a tie
+int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
+                          const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
+                          float* score, int32_t* paths, int32_t* arcs, int32_t* status);
+// tau_k = max (NaN kept) over start group k: the folded start arcs of gtnb_sparse_transitions_viterbi
+int launch_sparse_tau(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
+                      float* tau);
 int launch_sparse_sigma(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
                         float* sigma);
 int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, int nG, const float* w,

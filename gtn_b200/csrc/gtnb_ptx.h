@@ -31,6 +31,10 @@ __device__ __forceinline__ float neg_inf() {
 __device__ __forceinline__ bool is_finite(float x) {
   return fabsf(x) < CUDART_INF_F;
 }
+/* the max of two floats that keeps a NaN of either (fmaxf drops it) */
+__device__ __forceinline__ float max_nan(float a, float b) {
+  return (b > a || b != b) ? b : a;
+}
 
 /* the two floats of a 64-bit shared-memory load (the emulator has no CUDA vector types beyond int2 / float4) */
 struct f32x2 {

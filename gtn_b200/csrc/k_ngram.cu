@@ -296,11 +296,6 @@ __global__ void __launch_bounds__(256) ngram_sigma_kernel(int C, const float* __
   if (lane == 0) sigma[i] = m + logf(s);
 }
 
-/* the max of two floats that keeps a NaN of either (fmaxf drops it) */
-__device__ __forceinline__ float max_nan(float a, float b) {
-  return (b > a || b != b) ? b : a;
-}
-
 /*
  * tau_i = max_j W[i][j], one warp per row: the tropical sigma, the weight of BIGRAM's folded start arcs on
  * gtnb_graph_transitions_viterbi's device route.  A NaN anywhere in the row gives tau_i = NaN, so the weights the

@@ -29,6 +29,12 @@
  *
  * Valid only for finite weights: the forward kernel raises status bit 1 on any non-finite weight or used emission,
  * and the caller repeats the call on the materialised route.
+ *
+ * The decoder gtnb_viterbi_sparse sweeps the same tables in the tropical semiring (sparse_viterbi_forward_kernel):
+ * S_t[v] = max over in-arcs a: u -> v of fl(S_{t-1}[u] + fl(w_a + e[t-1][label_a])), the reference's association
+ * (compose.cpp:435, then shortest.cpp:213), with absolute scores so that the score is bit-exact.  Per (frame, node) it
+ * keeps a 16-bit back-pointer in HBM, the winning in-arc's position in the node's in-list plus a tie flag, and
+ * sparse_viterbi_trace_kernel walks them back from the best accept node.
  */
 #include <algorithm>
 
@@ -46,6 +52,12 @@ inline int sparse_fwd_smem_floats(int S, int C) {
 inline int sparse_bwd_smem_floats(int S, int A, int C) {
   return 2 * S + 4 * C + A + 2 * kSparseWarps;
 }
+inline int sparse_vit_smem_floats(int S, int C) {
+  return 2 * S + 2 * C;
+}
+/* a back-pointer: the in-list position (in-degree <= kSparseMaxArcs) and the tie flag; kBpNone on a -inf node */
+constexpr int kBpTie = 0x8000;
+constexpr uint16_t kBpNone = 0xFFFF;
 
 namespace {
 
@@ -296,6 +308,158 @@ __global__ void __launch_bounds__(256) sparse_fold_kernel(int K, const int32_t* 
   }
 }
 
+/* a max and its argmax merged over the `lanes` consecutive lanes of a group: the lowest index among equal maxima,
+ * tie = 1 when more than one candidate reaches a finite max; every lane of the group gets the result */
+__device__ __forceinline__ void argmax_merge(float& m, int& k, int& tie, int lanes) {
+  for (int o = 1; o < lanes; o <<= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    const int ok = __shfl_xor_sync(0xffffffffu, k, o);
+    const int ot = __shfl_xor_sync(0xffffffffu, tie, o);
+    if (om > m) {
+      m = om;
+      k = ok;
+      tie = ot;
+    } else if (om == m && m != neg_inf()) {
+      k = min(k, ok);
+      tie = 1;
+    }
+  }
+}
+
+/* one candidate of a lane's running (m, k, tie): strict >, so the first of equal candidates stays; -inf and NaN
+ * candidates never win */
+__device__ __forceinline__ void argmax_add(float& m, int& k, int& tie, float x, int j) {
+  if (x > m) {
+    m = x;
+    k = j;
+    tie = 0;
+  } else if (x == m && x != neg_inf()) {
+    tie = 1;
+  }
+}
+
+/*
+ * The tropical sweep of gtnb_viterbi_sparse over intersect(E_b, G) for utterance b = blockIdx.x, in the layout of
+ * sparse_den_forward_kernel (rows and emission rows in shared memory, G's tables from L2, `lanes` threads per node).
+ * bp[b][t-1][v] (t = 1 .. T_b): the in-list position of the in-arc that reaches S_t[v], | kBpTie when another in-arc
+ * reaches it too; kBpNone where S_t[v] = -inf (on no path).  Then the best accept node of frame T_b, the first in
+ * node order, to head[b] (-1 when no accept node is finite, T_b = 0 included) and its score to score[b].
+ * status[b] |= 1 on a NaN or +inf weight or used emission (-inf only forbids the arc), |= 2 when two accept nodes
+ * reach the best score.
+ */
+__global__ void __launch_bounds__(kSparseThreads) sparse_viterbi_forward_kernel(
+    SparseDev g, int T, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    const float* __restrict__ w, uint16_t* __restrict__ bp, int32_t* __restrict__ head, float* __restrict__ score,
+    int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int S = g.S, lanes = g.lanes;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  uint16_t* bpb = bp + (long long)b * T * S;
+  bool bad = false;
+  for (int v = tid; v < S; v += nt) rows[v] = (__ldg(g.flags + v) & 1) ? 0.0f : neg_inf();
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  __syncthreads();
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    uint16_t* bpt = bpb + (long long)(t - 1) * S;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    for (int v0 = 0; v0 < S; v0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int v = v0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, k0 = 0;
+      if (v < S) {
+        k0 = __ldg(g.in_ptr + v);
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + j));
+          const float ek = Er[__ldg(g.in_lab + j)];
+          bad |= !(wk < CUDART_INF_F && ek < CUDART_INF_F);
+          argmax_add(m, k, tie, P[__ldg(g.in_src + j)] + (wk + ek), j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (v < S && q == 0) {
+        Q[v] = m;
+        bpt[v] = m == neg_inf() ? kBpNone : (uint16_t)((k - k0) | (tie ? kBpTie : 0));
+      }
+    }
+    __syncthreads();
+  }
+  bad = __syncthreads_or(bad);
+  if (tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    int k = 0x7fffffff, tie = 0;
+    if (Tb > 0)
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) argmax_add(m, k, tie, F[v], v);
+    argmax_merge(m, k, tie, 32);
+    if (tid == 0) {
+      head[b] = m == neg_inf() ? -1 : k;
+      score[b] = m;
+      const int st = (bad ? 1 : 0) | (tie ? 2 : 0);
+      if (st) atomicOr(&status[b], st);
+    }
+  }
+}
+
+/*
+ * The traceback of gtnb_viterbi_sparse, one warp per utterance: paths[b][t] = the label and arcs[b][t] = G's arc id
+ * of the arc the best path takes at frame t (both nullable), walked back from head[b] through bp; -1 beyond T_b and
+ * in the whole row without a path.  status[b] |= 2 when a node of the path carries the tie flag.
+ */
+__global__ void __launch_bounds__(256) sparse_viterbi_trace_kernel(
+    SparseDev g, int B, int T, const int32_t* __restrict__ lens, const uint16_t* __restrict__ bp,
+    const int32_t* __restrict__ head, int32_t* __restrict__ paths, int32_t* __restrict__ arcs,
+    int32_t* __restrict__ status) {
+  const int b = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (b >= B) return; // whole warps
+  const int h = head[b];
+  const int n = h < 0 ? 0 : lens[b]; // the path's frames
+  int32_t* pr = paths ? paths + (long long)b * T : nullptr;
+  int32_t* ar = arcs ? arcs + (long long)b * T : nullptr;
+  for (int t = n + lane; t < T; t += 32) {
+    if (pr) pr[t] = -1;
+    if (ar) ar[t] = -1;
+  }
+  if (lane != 0 || n == 0) return;
+  const uint16_t* bpb = bp + (long long)b * T * g.S;
+  int v = h, tie = 0;
+  for (int t = n; t >= 1; t--) {
+    const int e = __ldg(bpb + (long long)(t - 1) * g.S + v);
+    const int k = __ldg(g.in_ptr + v) + (e & (kBpTie - 1));
+    tie |= e & kBpTie;
+    if (pr) pr[t - 1] = __ldg(g.in_lab + k);
+    if (ar) ar[t - 1] = __ldg(g.in_arc + k);
+    v = __ldg(g.in_src + k);
+  }
+  if (tie) atomicOr(&status[b], 2);
+}
+
+/* tau_k = the max of the weights of start group k (gtnb_product.h), NaN kept: the tropical counterpart of sigma, the
+ * weight of gtnb_sparse_transitions_viterbi's folded start arcs; one warp per group */
+__global__ void __launch_bounds__(256) sparse_tau_kernel(int K, const int32_t* __restrict__ grp_ptr,
+                                                         const int32_t* __restrict__ grp_arc,
+                                                         const float* __restrict__ w, float* __restrict__ tau) {
+  const int k = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (k >= K) return; // whole warps
+  const int a0 = __ldg(grp_ptr + k), a1 = __ldg(grp_ptr + k + 1);
+  float m = neg_inf();
+  for (int j = a0 + lane; j < a1; j += 32) m = max_nan(m, __ldg(w + __ldg(grp_arc + j)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) tau[k] = m;
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
@@ -339,6 +503,28 @@ int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32
   if (K == 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "sparse_fold", sparse_fold_kernel<<<(unsigned)((K + 255) / 256), 256, 0, ctx->stream>>>(
       K, grp_ptr, grp_arc, nG, w, sigma, wgrad));
+  return GTNB_OK;
+}
+
+int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
+                          const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
+                          float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_viterbi_forward_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_vit_smem_floats(g.S, C);
+  GTNB_LAUNCH(ctx, "sparse_viterbi_forward", sparse_viterbi_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      g, T, C, lens, emis, stride, w, bp, head, score, status));
+  GTNB_LAUNCH(ctx, "sparse_viterbi_trace", sparse_viterbi_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256),
+                                                                         256, 0, ctx->stream>>>(
+      g, B, T, lens, bp, head, paths, arcs, status));
+  return GTNB_OK;
+}
+
+int launch_sparse_tau(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
+                      float* tau) {
+  if (K == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "sparse_tau", sparse_tau_kernel<<<(unsigned)(((long long)K * 32 + 255) / 256), 256, 0,
+                                                     ctx->stream>>>(K, grp_ptr, grp_arc, w, tau));
   return GTNB_OK;
 }
 

@@ -295,7 +295,10 @@ class _GraphCall:
         self.e = e = emissions.contiguous()
         B, T, Cn = e.shape
         self.B, self.T, self.C = B, T, Cn
-        assert len(graphs) == B
+        if graphs is None:  # a decoder without target graphs
+            graphs = []
+        else:
+            assert len(graphs) == B
         self.views = [_graph_view(g) for g in graphs]
         counts = [v.num_arcs for v, _ in self.views]
         self.n_arcs = sum(counts)
@@ -511,3 +514,46 @@ def graph_transitions_viterbi(emissions, transitions, graphs, kind="asg", input_
     tw = transitions.detach().contiguous()
     return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_graph_transitions_viterbi(
         c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, kid, tw.data_ptr(), 1, paths, arcs, scores, 1))
+
+
+def _sparse_transitions(c, transitions, transitions_graph):
+    """(G's view pair, trans_w on the device) of the sparse Viterbi calls"""
+    assert transitions.is_cuda and transitions.device == c.e.device and transitions.dtype == torch.float32
+    gv = _graph_view(transitions_graph)
+    assert transitions.numel() == gv[0].num_arcs
+    # (an empty G: a one-element buffer that is never read)
+    tw = transitions.detach().contiguous() if transitions.numel() else torch.zeros(1, device=c.e.device)
+    return gv, tw
+
+
+@torch.no_grad()
+def sparse_viterbi(emissions, transitions, transitions_graph, input_lengths=None):
+    """Best path of intersect(E_b, G) for every utterance, G the learned transition graph of sparse_transitions_loss
+    (an n-gram graph of any order, a pruned token LM, an HMM topology), through gtnb_viterbi_sparse: the decode of a
+    model trained with that loss.  emissions, transitions, transitions_graph and input_lengths as in
+    sparse_transitions_loss.  Returns (paths [B, T] int32, the label of every frame; scores [B] float32, viterbiScore;
+    arcs [B, T] int32, the G arc taken at every frame, i.e. the state sequence), all -1 beyond T_b and where there is
+    no accepting path (score -inf), as CUDA tensors on the emissions' device, written on the current stream; only
+    input_lengths and one status word per utterance visit the host.  Ties are broken as the reference breaks them.
+    collapse(paths, blank) turns the paths into transcripts.
+    """
+    c = _GraphCall(emissions, None, None, input_lengths, arc_grads=False)
+    gv, tw = _sparse_transitions(c, transitions, transitions_graph)
+    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_viterbi_sparse(
+        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1))
+
+
+@torch.no_grad()
+def sparse_transitions_viterbi(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None):
+    """Best path of sparse_transitions_loss's numerator, intersect(intersect(A_b, G), E_b), for every utterance,
+    through gtnb_sparse_transitions_viterbi: the decomposition and frame-level alignment a model trained with
+    sparse_transitions_loss picks within its own target graph.  The arguments are sparse_transitions_loss's.  Returns
+    (paths [B, T] int32, the label of the arc taken at every frame; scores [B] float32, viterbiScore; arcs [B, T]
+    int32, that arc's id in graphs[b]), all -1 beyond T_b and where there is no accepting path (score -inf), as CUDA
+    tensors on the emissions' device, written on the current stream.  Ties are broken as the reference breaks them.
+    """
+    c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=False)
+    gv, tw = _sparse_transitions(c, transitions, transitions_graph)
+    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_sparse_transitions_viterbi(
+        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs,
+        scores, 1))

@@ -690,6 +690,81 @@ int gtnb_graph_transitions_viterbi(
     float* scores, /* [B] nullable: viterbiScore */
     int outputs_on_device);
 
+/*
+ * Batched Viterbi decoding with a learned transition graph G of any shape: viterbiPath and viterbiScore of
+ * intersect(E_b, G), E_b = linearGraph(T_b, C) on the first T_b rows of utterance b -- the best label sequence under
+ * the G a model trained with gtnb_sparse_transitions_loss learned (an n-gram graph of any order, a pruned token LM,
+ * an HMM topology).  transitions and trans_w are exactly those of gtnb_sparse_transitions_loss: G's structure, an
+ * epsilon-free acceptor whose own weights are ignored, and [G.num_arcs] weights in G's arc numbering; a G arc
+ * labelled outside [0, C) never matches.  paths ([B][T], nullable) gets the label of frame t, arcs ([B][T], nullable)
+ * the G arc taken at frame t (Graph arc numbering: the state sequence of an HMM topology), both -1 beyond T_b and in
+ * every slot when there is no accepting path; EVERY entry is written.  scores ([B], nullable): viterbiScore, -inf
+ * without an accepting path (T_b = 0 included: linearGraph(0, C) accepts nothing).  Outputs live on the device when
+ * outputs_on_device, else on the host; emissions and trans_w each where their own flag says.  collapse the paths for
+ * transcripts.
+ * Paths, arcs and scores equal the reference's, ties included.  The device route sweeps G's tables frame by frame in
+ * the tropical semiring without building the T_b * |G| lattice (k_sparse.cu) when G fits the kernels' envelope -- at
+ * most 4096 nodes, 32768 arcs labelled in [0, C), C <= 1024 -- keeping a 16-bit back-pointer per frame and node
+ * (2 * B * T * S bytes of scratch), and traces the path back.  An utterance whose traced path meets a tie (with
+ * "exact_ties" on), or whose sweep meets a NaN or +inf (-inf only forbids an arc), is re-run on the materialised
+ * lattice (gtnb_compose_linear with E_b first, gtnb_forward, gtnb_viterbi_path), as is the whole batch outside the
+ * envelope or with the "implicit" flag off; only that route reads trans_w to the host, and it runs the utterances in
+ * groups that fit the device memory.  With "exact_ties" off a tie keeps the device route's path, one of the optimal
+ * paths.  The call reads back one status word per utterance, so it returns only once every output is complete,
+ * device ones too.
+ * Epsilon arcs or a transducer G, and a lattice too large to materialise for one utterance on the exact route, are
+ * GTNB_ERR_UNSUPPORTED; a malformed view, a G without nodes, a NULL trans_w with B > 0 and input_lens outside [0, T]
+ * are GTNB_ERR_INVALID_ARGUMENT.  B = 0 is a no-op.
+ */
+int gtnb_viterbi_sparse(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    const gtnb_graph_view* transitions, /* G: structure only, its own weights ignored */
+    const float* trans_w, /* [G.num_arcs], G's arc numbering */
+    int trans_on_device,
+    int32_t* paths, /* [B][T] nullable: label of frame t */
+    int32_t* arcs, /* [B][T] nullable: the G arc taken at frame t (Graph arc numbering) */
+    float* scores, /* [B] nullable: viterbiScore */
+    int outputs_on_device);
+
+/*
+ * Batched Viterbi alignment over one user-supplied target graph per utterance with a learned transition graph G of
+ * any shape: viterbiPath and viterbiScore of intersect(intersect(A_b, G), E_b), the numerator of
+ * gtnb_sparse_transitions_loss -- the decomposition and frame-level alignment a model trained with that loss picks.
+ * E_b, graphs, arc_weights, transitions, trans_w, labels outside [0, C) and the epsilon rule are those of
+ * gtnb_sparse_transitions_loss; the outputs, the routing and their rules are those of gtnb_graph_transitions_viterbi
+ * (arcs: A_b's arc ids).  The device route sweeps the loss's folded products in the tropical semiring, G's start
+ * copies folded into one start node whose arcs weigh tau_k = max over a group of G's start arcs, with trans_w on the
+ * device; the exact route composes A_b with G in the reference's numbering (gtnb_compose_graphs).  The device route
+ * is taken when G fits gtnb_viterbi_sparse's envelope and every product the implicit sweeps' layout.
+ * Epsilon arcs in A_b or G, a transducer G and a pair too large for the exact route are GTNB_ERR_UNSUPPORTED;
+ * malformed views, a G without nodes, a NULL trans_w with B > 0 and bad lengths are GTNB_ERR_INVALID_ARGUMENT.
+ * B = 0 is a no-op.
+ */
+int gtnb_sparse_transitions_viterbi(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    const gtnb_graph_view* transitions, /* G: structure only, its own weights ignored */
+    const float* trans_w, /* [G.num_arcs], G's arc numbering */
+    int trans_on_device,
+    int32_t* paths, /* [B][T] nullable: label of the arc taken at frame t */
+    int32_t* arcs, /* [B][T] nullable: that frame's arc id in A_b (Graph arc numbering) */
+    float* scores, /* [B] nullable: viterbiScore */
+    int outputs_on_device);
+
 #ifdef __cplusplus
 }
 #endif
