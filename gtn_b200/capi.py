@@ -122,6 +122,12 @@ SYMBOLS = [
     ("gtnb_sparse_transitions_viterbi", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.POINTER(GraphView),
       _vp, C.c_int, _vp, _vp, _vp, C.c_int]),
+    ("gtnb_backoff_transitions_loss", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.POINTER(GraphView),
+      _vp, C.c_int, _f32p, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int]),
+    ("gtnb_viterbi_backoff", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _vp, _vp, _vp,
+      C.c_int]),
 ]
 
 _lib = None
@@ -543,8 +549,21 @@ class Ctx:
         return self._sparse_transitions_loss(True, emissions, views, transitions, trans_w, True, input_lens,
                                              arc_weights)
 
+    def backoff_transitions_loss(self, emissions, views, transitions, trans_w, want_grad=True, input_lens=None,
+                                 arc_weights=None):
+        """Host-buffer entry of gtnb_backoff_transitions_loss: sparse_transitions_loss's arguments and results, with
+        epsilon arcs (backoff arcs) allowed in the transition graph."""
+        return self._sparse_transitions_loss(False, emissions, views, transitions, trans_w, want_grad, input_lens,
+                                             arc_weights, "gtnb_backoff_transitions_loss")
+
+    def backoff_transitions_loss_dev(self, emissions, views, transitions, trans_w, input_lens=None, arc_weights=None):
+        """Device-buffer entry of gtnb_backoff_transitions_loss, as sparse_transitions_loss_dev
+        -> (losses, grads, arc_grads, trans_grad)."""
+        return self._sparse_transitions_loss(True, emissions, views, transitions, trans_w, True, input_lens,
+                                             arc_weights, "gtnb_backoff_transitions_loss")
+
     def _sparse_transitions_loss(self, dev, emissions, views, transitions, trans_w, want_grad, input_lens,
-                                 arc_weights):
+                                 arc_weights, fn="gtnb_sparse_transitions_loss"):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         arr, n_arcs, aw = _graph_batch(views, B, arc_weights)
@@ -559,7 +578,7 @@ class Ctx:
         ag = np.full(max(n_arcs, 1), np.nan, np.float32) if want_grad else None  # written, not accumulated
         tg = np.full(max(tw.size, 1), np.nan, np.float32) if want_grad else None
         with _Placed(self, dev) as p:
-            self._check(lib().gtnb_sparse_transitions_loss(
+            self._check(getattr(lib(), fn)(
                 self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, C.byref(gv), p.inp(tw_arg),
                 p.flag, _p(losses, _f32p), p.out(grads), p.flag, p.out(ag), p.flag, p.out(tg), p.flag))
         return (losses, grads, None if ag is None else ag[:n_arcs], None if tg is None else tg[:tw.size])
@@ -603,7 +622,18 @@ class Ctx:
         gtnb_viterbi_sparse on device pointers (outputs in HBM), downloaded afterwards -> (paths, scores, arcs)."""
         return self._viterbi_sparse(True, emissions, transitions, trans_w, input_lens, bool(trans_on_device))
 
-    def _viterbi_sparse(self, dev, emissions, transitions, trans_w, input_lens, trans_on_device):
+    def viterbi_backoff(self, emissions, transitions, trans_w, input_lens=None):
+        """Host-buffer entry of gtnb_viterbi_backoff: viterbi_sparse's arguments and results, with epsilon arcs
+        (backoff arcs) allowed in the transition graph; arcs holds the emitting G arc of every frame."""
+        return self._viterbi_sparse(False, emissions, transitions, trans_w, input_lens, False, "gtnb_viterbi_backoff")
+
+    def viterbi_backoff_dev(self, emissions, transitions, trans_w, input_lens=None, trans_on_device=True):
+        """Device-buffer entry of gtnb_viterbi_backoff, as viterbi_sparse_dev -> (paths, scores, arcs)."""
+        return self._viterbi_sparse(True, emissions, transitions, trans_w, input_lens, bool(trans_on_device),
+                                    "gtnb_viterbi_backoff")
+
+    def _viterbi_sparse(self, dev, emissions, transitions, trans_w, input_lens, trans_on_device,
+                        fn="gtnb_viterbi_sparse"):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         gv = transitions[0]
@@ -611,7 +641,7 @@ class Ctx:
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         out = _viterbi_outputs(B, T)
         with _Placed(self, dev) as p:
-            self._check(lib().gtnb_viterbi_sparse(
+            self._check(getattr(lib(), fn)(
                 self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), C.byref(gv), p.inp(tw, trans_on_device),
                 int(trans_on_device), *map(p.out, out), p.flag))
         return _viterbi_results(out, B, T)

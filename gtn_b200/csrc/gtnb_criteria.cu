@@ -1738,12 +1738,13 @@ struct SparseDenominator {
   }
 };
 
-/* the checks of gtnb_sparse_transitions_loss's transition graph */
-int check_transition_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& Gv) {
+/* the checks of gtnb_sparse_transitions_loss's transition graph; epsilon (the backoff entry points): epsilon arcs,
+ * GTNB_EPSILON on both sides, are G's own */
+int check_transition_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& Gv, bool epsilon = false) {
   if (validate_view(ctx, Gv)) return GTNB_ERR_INVALID_ARGUMENT;
   if (Gv.num_nodes < 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the transition graph has no nodes");
   for (int g = 0; g < Gv.num_arcs; g++) {
-    if (Gv.arc_ilabel[g] == GTNB_EPSILON || Gv.arc_olabel[g] == GTNB_EPSILON)
+    if (!epsilon && (Gv.arc_ilabel[g] == GTNB_EPSILON || Gv.arc_olabel[g] == GTNB_EPSILON))
       return fail(ctx, GTNB_ERR_UNSUPPORTED,
                   fn + ": the transition graph has epsilon arcs; remove them first (remove(g, epsilon))");
     if (Gv.arc_ilabel[g] != Gv.arc_olabel[g])
@@ -1754,24 +1755,12 @@ int check_transition_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_grap
   return GTNB_OK;
 }
 
-} // namespace
-
-extern "C" int gtnb_sparse_transitions_loss(
-    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
-    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
-    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, float* losses_host, float* grads,
-    int grads_on_device, float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
-  const std::string fn = "gtnb_sparse_transitions_loss";
-  GraphBatch gb;
-  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, C, emissions, graphs,
-                        transitions && (B == 0 || (losses_host && trans_w)), input_lens, arc_weights,
-                        arc_weights_on_device, &gb, [&] { return check_transition_graph(ctx, fn, *transitions); }));
-  const gtnb_graph_view& Gv = *transitions;
-  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
-                         nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+/* gtnb_sparse_transitions_loss after its checks, t = sparse_tables(Gv); also gtnb_backoff_transitions_loss's route for
+ * an epsilon-free G */
+int sparse_transitions_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
+                                const SparseTables& t, float* arc_grads, int arc_grads_on_device) {
+  const int B = a.B, C = a.C;
   const long long n_trans = Gv.num_arcs;
-  SparseTables t;
-  sparse_tables(Gv, C, &t);
   // the device route's numerators (folded), whose shapes decide, with G's, whether it can be taken
   std::vector<ProductGraph> prods;
   const bool fast = ctx->use_implicit && sparse_den_supported(t.S, t.A, C) &&
@@ -1781,7 +1770,7 @@ extern "C" int gtnb_sparse_transitions_loss(
                           build_sparse_product(v, Gv, t, C, /*fold=*/true, p);
                         },
                         &prods);
-  return run_criterion(ctx, B, gb.Tb.data(), losses_host, trans_grad, trans_grad_on_device, n_trans, fast,
+  return run_criterion(ctx, B, gb.Tb.data(), a.losses_host, a.trans_grad, a.trans_grad_on_device, n_trans, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
                          if (!f)
                            return transitions_exact(
@@ -1797,6 +1786,25 @@ extern "C" int gtnb_sparse_transitions_loss(
                          GraphNumerator num{gb, prods, (int)n_trans, arc_grads, arc_grads_on_device};
                          return trellis_loss_fast(scope, den, a, num, needs_exact);
                        });
+}
+
+} // namespace
+
+extern "C" int gtnb_sparse_transitions_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
+    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, float* losses_host, float* grads,
+    int grads_on_device, float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const std::string fn = "gtnb_sparse_transitions_loss";
+  GraphBatch gb;
+  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, C, emissions, graphs,
+                        transitions && (B == 0 || (losses_host && trans_w)), input_lens, arc_weights,
+                        arc_weights_on_device, &gb, [&] { return check_transition_graph(ctx, fn, *transitions); }));
+  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
+                         nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+  SparseTables t;
+  sparse_tables(*transitions, C, &t);
+  return sparse_transitions_loss_run(ctx, a, gb, *transitions, t, arc_grads, arc_grads_on_device);
 }
 
 /*
@@ -2330,4 +2338,505 @@ extern "C" int gtnb_sparse_transitions_viterbi(
       scope, fn.c_str(), GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores, outputs_on_device}, gb, prods, fast,
       Gv.num_arcs, trans_w, trans_on_device, tau,
       [&](const float* W, HostGraph* G) { sparse_host_graph(Gv, t, C, W, G, nullptr); });
+}
+
+/*
+ * Loss and Viterbi decoding with a backoff transition graph G: the formulas of gtnb_sparse_transitions_loss and
+ * gtnb_viterbi_sparse with epsilon arcs in G (ilabel == olabel == GTNB_EPSILON), the backoff arcs of a pruned n-gram
+ * LM.  An epsilon arc moves G without consuming a frame, at any frame 0 .. T_b, and weighs its trans_w alone
+ * (compose.cpp:139-205).  An epsilon-free G takes the sparse entry points' own routes.  Otherwise the device route
+ * sweeps the denominator over G's tables and the numerators P_b = A_b o G (gtnb_product.h, unfolded, with G's
+ * epsilon arcs) over their own tables, one CTA each, with k_sparse.cu's sparse_eps_* kernels, and the decode sweeps G
+ * in the tropical semiring.  The exact route composes E_b with G, and P_b with E_b, in the reference's numbering
+ * (gtnb_compose_graphs, which composes epsilon arcs), then runs gtnb_forward / gtnb_backward / gtnb_viterbi_path, one
+ * utterance at a time.
+ */
+namespace {
+
+/* acceptors with epsilon arcs (SparseTables with its epsilon tables) in one device buffer for the sparse_eps_*
+ * kernels: add() every graph, its arc ids shifted by arc_base and its score rows at `rows`, then alloc(), stage() */
+struct EpsDevTables {
+  std::vector<int32_t> packed;
+  std::vector<std::vector<size_t>> at; // per graph: where each of its tables starts in packed
+  std::vector<SparseEpsDev> desc;
+  int32_t* tab = nullptr;
+  SparseEpsDev* dev = nullptr;
+  int max_S = 1, max_AE = 0;
+
+  void add(const SparseTables& t, int32_t arc_base, long long rows) {
+    std::vector<size_t> o{packed.size()};
+    packed.insert(packed.end(), t.flags.begin(), t.flags.end());
+    auto put = [&](const std::vector<int32_t>& v, int32_t shift) {
+      o.push_back(packed.size());
+      for (int32_t x : v) packed.push_back(x + shift);
+    };
+    for (auto* v : {&t.in_ptr, &t.in_src, &t.in_lab}) put(*v, 0);
+    put(t.in_arc, arc_base);
+    for (auto* v : {&t.out_ptr, &t.out_dst, &t.out_lab}) put(*v, 0);
+    put(t.out_arc, arc_base);
+    put(t.eps_in_ptr, 0);
+    put(t.eps_in_src, 0);
+    put(t.eps_in_arc, arc_base);
+    put(t.eps_out_ptr, 0);
+    put(t.eps_out_dst, 0);
+    put(t.eps_out_arc, arc_base);
+    for (auto* v : {&t.fwd_ptr, &t.fwd_node, &t.bwd_ptr, &t.bwd_node, &t.lanes}) put(*v, 0);
+    at.push_back(o);
+    SparseEpsDev d{};
+    d.g.S = t.S;
+    d.g.A = t.A;
+    d.g.lanes = sparse_den_lanes(t.S, t.A);
+    d.E = t.E;
+    d.L = t.L;
+    d.rows = rows;
+    desc.push_back(d);
+    max_S = std::max(max_S, t.S);
+    max_AE = std::max(max_AE, t.A + t.E);
+  }
+  int alloc(CallScope& scope) {
+    GTNB_TRY(scope.alloc(&tab, (long long)packed.size()));
+    GTNB_TRY(scope.alloc(&dev, (long long)desc.size()));
+    for (size_t i = 0; i < desc.size(); i++) {
+      const int32_t* p[20];
+      for (int j = 0; j < 20; j++) p[j] = tab + at[i][j];
+      SparseEpsDev& d = desc[i];
+      d.g.flags = p[0];
+      d.g.in_ptr = p[1], d.g.in_src = p[2], d.g.in_lab = p[3], d.g.in_arc = p[4];
+      d.g.out_ptr = p[5], d.g.out_dst = p[6], d.g.out_lab = p[7], d.g.out_arc = p[8];
+      d.eps_in_ptr = p[9], d.eps_in_src = p[10], d.eps_in_arc = p[11];
+      d.eps_out_ptr = p[12], d.eps_out_dst = p[13], d.eps_out_arc = p[14];
+      d.fwd_ptr = p[15], d.fwd_node = p[16], d.bwd_ptr = p[17], d.bwd_node = p[18], d.lanes = p[19];
+    }
+    return GTNB_OK;
+  }
+  int stage(CallScope& scope) {
+    GTNB_TRY(stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()));
+    return stage_upload(scope.ctx(), dev, desc.data(), sizeof(SparseEpsDev) * desc.size());
+  }
+};
+
+bool eps_fits(const SparseTables& t, int C) { return sparse_eps_supported(t.S, t.A, t.E, t.L, t.max_in_all, C); }
+
+/* the checks of the backoff entry points' G, and its tables (with the epsilon tables) into t: a cycle of epsilon arcs
+ * has no finite closure (the reference's forwardScore and viterbi throw "Graph has a cycle", shortest.cpp:150, 230) */
+int check_backoff_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& Gv, int C, SparseTables* t) {
+  GTNB_TRY(check_transition_graph(ctx, fn, Gv, /*epsilon=*/true));
+  sparse_tables(Gv, C, t);
+  sparse_eps_tables(Gv, t);
+  if (t->cycle.empty()) return GTNB_OK;
+  std::string path;
+  for (int32_t v : t->cycle) path += std::to_string(v) + " -> ";
+  return fail(ctx, GTNB_ERR_INVALID_ARGUMENT,
+              fn + ": the transition graph has a cycle of epsilon arcs: " + path + std::to_string(t->cycle[0]));
+}
+
+/* the device route of gtnb_backoff_transitions_loss: ptabs[b] the tables of prods[b] (P_b = A_b o G, unfolded) */
+int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatch& gb, long long n_trans,
+                      const SparseTables& t, const std::vector<ProductGraph>& prods,
+                      const std::vector<SparseTables>& ptabs, float* arc_grads, int arc_grads_on_device,
+                      bool* needs_exact) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, tot_arcs = gb.tot_arcs;
+  const bool want = a.grads || a.trans_grad || arc_grads;
+  EpsDevTables den_t, num_t;
+  den_t.add(t, 0, 0);
+  std::vector<int32_t> arc_of_h, tidx_h;
+  long long rows = 0;
+  for (int b = 0; b < B; b++) {
+    num_t.add(ptabs[b], (int32_t)tidx_h.size(), rows);
+    rows += (long long)(gb.Tb[b] + 1) * ptabs[b].S;
+    for (int32_t k : prods[b].arc_of) arc_of_h.push_back(k < 0 ? -1 : (int32_t)(gb.first_arc[b] + k));
+    tidx_h.insert(tidx_h.end(), prods[b].tidx.begin(), prods[b].tidx.end());
+  }
+  const long long tot_P = (long long)tidx_h.size();
+  std::vector<float> w_A_h;
+  float *e_dev = nullptr, *w_dev = nullptr, *den = nullptr, *num = nullptr, *alpha_d = nullptr, *alpha_n = nullptr;
+  float *fw = nullptr, *w_A = nullptr, *pgrad = nullptr;
+  double *offs_d = nullptr, *offs_n = nullptr;
+  int32_t *status = nullptr, *T_dev = nullptr, *arc_of = nullptr, *tidx = nullptr;
+  OutBuf g, tg, ag;
+  GTNB_TRY(ensure_side_streams(ctx, 0, 0));
+  GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
+  GTNB_TRY(scope.borrow(a.trans_w, a.trans_on_device != 0, n_trans, &w_dev)); // (host: staged below)
+  GTNB_TRY(scope.alloc(&status, 2ll * B));
+  GTNB_TRY(scope.alloc(&den, B));
+  GTNB_TRY(scope.alloc(&num, B));
+  GTNB_TRY(scope.alloc(&T_dev, B));
+  GTNB_TRY(scope.alloc(&offs_d, (long long)B * (T + 1)));
+  GTNB_TRY(scope.alloc(&offs_n, (long long)B * (T + 1)));
+  GTNB_TRY(scope.alloc(&alpha_d, (long long)B * (T + 1) * t.S));
+  GTNB_TRY(scope.alloc(&alpha_n, rows));
+  GTNB_TRY(scope.alloc(&fw, tot_P));
+  GTNB_TRY(scope.alloc(&arc_of, tot_P));
+  GTNB_TRY(scope.alloc(&tidx, tot_P));
+  GTNB_TRY(den_t.alloc(scope));
+  GTNB_TRY(num_t.alloc(scope));
+  if (!gb.arc_weights_dev) {
+    w_A_h.assign((size_t)std::max(tot_arcs, 1ll), 0.0f);
+    for (int b = 0; b < B; b++) {
+      const gtnb_graph_view& v = gb.views[b];
+      if (v.weights) std::copy(v.weights, v.weights + v.num_arcs, w_A_h.begin() + gb.first_arc[b]);
+    }
+    GTNB_TRY(scope.alloc(&w_A, (long long)w_A_h.size()));
+  }
+  if (want) {
+    GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
+    GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, n_trans, &tg));
+    GTNB_TRY(scope.output(arc_grads, arc_grads_on_device, tot_arcs, &ag));
+    GTNB_TRY(scope.alloc(&pgrad, tot_P));
+    GTNB_CUDA(ctx, cudaMemsetAsync(g.dev, 0, sizeof(float) * per * B, ctx->stream));
+    if (n_trans) GTNB_CUDA(ctx, cudaMemsetAsync(tg.dev, 0, sizeof(float) * n_trans, ctx->stream));
+    if (tot_arcs) GTNB_CUDA(ctx, cudaMemsetAsync(ag.dev, 0, sizeof(float) * tot_arcs, ctx->stream));
+    if (tot_P) GTNB_CUDA(ctx, cudaMemsetAsync(pgrad, 0, sizeof(float) * tot_P, ctx->stream));
+  }
+  GTNB_CUDA(ctx, cudaMemsetAsync(status, 0, sizeof(int32_t) * 2 * B, ctx->stream));
+  GTNB_TRY(stage_begin(ctx));
+  GTNB_TRY(den_t.stage(scope));
+  GTNB_TRY(num_t.stage(scope));
+  GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
+  if (tot_P) {
+    GTNB_TRY(stage_upload(ctx, arc_of, arc_of_h.data(), sizeof(int32_t) * tot_P));
+    GTNB_TRY(stage_upload(ctx, tidx, tidx_h.data(), sizeof(int32_t) * tot_P));
+  }
+  if (!a.trans_on_device && n_trans) GTNB_TRY(stage_upload(ctx, w_dev, a.trans_w, sizeof(float) * n_trans));
+  if (w_A) GTNB_TRY(stage_upload(ctx, w_A, w_A_h.data(), sizeof(float) * w_A_h.size()));
+  GTNB_TRY(stage_end(ctx));
+  GTNB_TRY(launch_sparse_eps_gather(ctx, tot_P, gb.arc_weights_dev ? gb.arc_weights_dev : w_A, arc_of, w_dev, tidx, fw));
+  // the numerators (small, one graph per CTA) on the second stream beside the denominator (G for every CTA); both
+  // add into the zero-filled emission rows with red.add
+  GTNB_TRY(fork_to(ctx, ctx->copy_stream));
+  {
+    OnStream side(ctx, ctx->copy_stream);
+    GTNB_TRY(launch_sparse_eps_forward(ctx, num_t.dev, 1, num_t.max_S, B, T, C, T_dev, e_dev, per, fw, alpha_n, offs_n,
+                                       num, status + B));
+    if (want)
+      GTNB_TRY(launch_sparse_eps_backward(ctx, num_t.dev, 1, num_t.max_S, num_t.max_AE, B, T, C, T_dev, e_dev, per, fw,
+                                          alpha_n, offs_n, -1.0f, g.dev, per, pgrad));
+  }
+  GTNB_TRY(launch_sparse_eps_forward(ctx, den_t.dev, 0, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d, offs_d, den,
+                                     status));
+  if (want)
+    GTNB_TRY(launch_sparse_eps_backward(ctx, den_t.dev, 0, t.S, t.A + t.E, B, T, C, T_dev, e_dev, per, w_dev, alpha_d,
+                                        offs_d, 1.0f, g.dev, per, tg.dev));
+  GTNB_TRY(join_from(ctx, ctx->copy_stream));
+  if (want) {
+    GTNB_TRY(launch_sparse_eps_scatter(ctx, tot_P, pgrad, arc_of, tidx, tg.dev, arc_grads ? ag.dev : nullptr));
+    GTNB_TRY(g.copy_out(ctx, per * B));
+    GTNB_TRY(tg.copy_out(ctx, n_trans));
+    GTNB_TRY(ag.copy_out(ctx, tot_arcs));
+  }
+  return read_losses(scope, B, den, num, status, 2ll * B, a.losses_host, needs_exact);
+}
+
+/* the composed graph of one pair, downloaded: gi1 / gi2 the arcs of the two operands behind each arc (-1: none) */
+struct ComposedHost {
+  std::vector<uint8_t> flags;
+  std::vector<int32_t> src, dst, il, ol, gi1, gi2;
+  std::vector<float> w;
+  int N = 0, A = 0;
+  gtnb_graph_view view() const {
+    gtnb_graph_view v;
+    std::memset(&v, 0, sizeof(v));
+    v.num_nodes = N;
+    v.num_arcs = A;
+    v.node_flags = flags.data();
+    v.arc_src = src.data();
+    v.arc_dst = dst.data();
+    v.arc_ilabel = il.data();
+    v.arc_olabel = ol.data();
+    v.weights = w.data();
+    return v;
+  }
+};
+
+/* compose(first, second) in the reference's numbering; kind: the matcher (gtnb_compose_graphs) */
+int compose_host(gtnb_ctx* ctx, const gtnb_graph_view& first, const gtnb_graph_view& second, int32_t kind,
+                 ComposedHost* c) {
+  gtnb_composed* res = nullptr;
+  GTNB_TRY(gtnb_compose_graphs(ctx, 1, &first, 1, &second, 1, &kind, &res));
+  int rc = gtnb_composed_sizes(res, 0, &c->N, &c->A);
+  if (rc == GTNB_OK) {
+    c->flags.resize(std::max(c->N, 1));
+    for (auto* v : {&c->src, &c->dst, &c->il, &c->ol, &c->gi1, &c->gi2}) v->resize(std::max(c->A, 1));
+    c->w.resize(std::max(c->A, 1));
+    rc = gtnb_composed_download(ctx, res, 0, c->flags.data(), c->src.data(), c->dst.data(), c->il.data(), c->ol.data(),
+                                c->w.data(), c->gi1.data(), c->gi2.data());
+  }
+  gtnb_composed_destroy(ctx, res);
+  return rc;
+}
+
+/* E_b = linearGraph(T_b, C) on host rows e ([T_b][C]): arc t * C + c goes t -> t + 1 with label c.  The reference's
+ * linearGraph is marked arc-sorted (creations.cpp:30-31), so it composes with the sorted matcher on its side. */
+void linear_host(int Tb, int C, const float* e, HostGraph* E) {
+  E->flags.assign(Tb + 1, 0);
+  E->flags[0] |= 1;
+  E->flags[Tb] |= 2;
+  for (int t = 0; t < Tb; t++)
+    for (int c = 0; c < C; c++) E->arc(t, t + 1, c, e[(long long)t * C + c]);
+}
+
+/* n floats from the host into a user buffer on the device or the host */
+int write_user(gtnb_ctx* ctx, float* user, int on_device, const float* host, long long n) {
+  if (!user || n <= 0) return GTNB_OK;
+  if (!on_device) {
+    std::memcpy(user, host, sizeof(float) * n);
+    return GTNB_OK;
+  }
+  GTNB_CUDA(ctx, cudaMemcpyAsync(user, host, sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
+  GTNB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return GTNB_OK;
+}
+
+/*
+ * The exact route of gtnb_backoff_transitions_loss, one utterance at a time: the denominator compose(E_b, G) and the
+ * numerator compose(P_b, E_b) (P_b unfolded, weighted on the host) in the reference's numbering, packed into one
+ * lattice, gtnb_forward and gtnb_backward with +1 / -1, and the arc gradients taken back through the compositions'
+ * gradInfo.  Reproduces the reference's inf / NaN propagation arc by arc.
+ */
+int backoff_loss_exact(CallScope& scope, const TransitionArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
+                       const SparseTables& t, float* arc_grads, int arc_grads_on_device) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = a.B, T = a.T, C = a.C;
+  const long long per = (long long)T * C, n_trans = Gv.num_arcs, tot_arcs = gb.tot_arcs;
+  const bool want = a.grads || a.trans_grad || arc_grads;
+  std::vector<float> W(std::max(n_trans, 1ll)), host_w, e((size_t)std::max(per * B, 1ll));
+  if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), a.trans_w, a.trans_on_device, n_trans));
+  if (per * B) GTNB_TRY(read_to_host(ctx, e.data(), a.emissions, a.emissions_on_device, per * B));
+  std::vector<gtnb_graph_view> views;
+  GTNB_TRY(gb.host_views(ctx, &host_w, &views));
+  gtnb_graph_view G = Gv;
+  G.weights = W.data();
+  std::vector<float> gh(want ? (size_t)std::max(per * B, 1ll) : 0, 0.0f), agh((size_t)std::max(tot_arcs, 1ll), 0.0f);
+  std::vector<double> tgd((size_t)std::max(n_trans, 1ll), 0.0);
+  for (int b = 0; b < B; b++) {
+    const int Tb = gb.Tb[b];
+    if (Tb == 0) continue; // (NaN, no gradient: run_criterion)
+    HostGraph E;
+    linear_host(Tb, C, e.data() + per * b, &E);
+    const gtnb_graph_view Ev = E.view();
+    ProductGraph p;
+    build_sparse_product(views[b], Gv, t, C, /*fold=*/false, &p);
+    std::vector<float> pw;
+    product_weights(p, views[b].weights, W.data(), &pw);
+    gtnb_graph_view pv = p.view();
+    pv.weights = pw.data();
+    ComposedHost cg[2];
+    GTNB_TRY(compose_host(ctx, Ev, G, /*first sorted=*/1, &cg[0]));
+    GTNB_TRY(compose_host(ctx, pv, Ev, /*second sorted=*/2, &cg[1]));
+    // an empty composition (nothing reachable) scores -inf and has no gradient
+    float sc[2] = {-std::numeric_limits<float>::infinity(), -std::numeric_limits<float>::infinity()};
+    std::vector<gtnb_graph_view> lv;
+    std::vector<int> which;
+    for (int k = 0; k < 2; k++)
+      if (cg[k].N > 0) {
+        lv.push_back(cg[k].view());
+        which.push_back(k);
+      }
+    if (!lv.empty()) {
+      gtnb_lattice*& lat = scope.lattice();
+      GTNB_TRY(gtnb_pack(ctx, (int)lv.size(), lv.data(), &lat));
+      float s[2];
+      GTNB_TRY(gtnb_forward(ctx, lat, 0, s, nullptr));
+      for (size_t i = 0; i < which.size(); i++) sc[which[i]] = s[i];
+      if (want) {
+        float deltas[2];
+        for (size_t i = 0; i < which.size(); i++) deltas[i] = which[i] == 0 ? 1.0f : -1.0f; // subtract's gradFunc
+        GTNB_TRY(gtnb_backward(ctx, lat, 0, deltas));
+        for (size_t i = 0; i < which.size(); i++) {
+          const ComposedHost& c = cg[which[i]];
+          std::vector<float> ga((size_t)std::max(c.A, 1));
+          GTNB_TRY(gtnb_lattice_arc_grads(ctx, lat, (int)i, ga.data()));
+          for (int k = 0; k < c.A; k++) {
+            const float v = ga[k];
+            // E_b is the first operand of the denominator and the second of the numerator
+            const int ea = which[i] == 0 ? c.gi1[k] : c.gi2[k], oa = which[i] == 0 ? c.gi2[k] : c.gi1[k];
+            if (ea >= 0) gh[per * b + ea] += v;
+            if (oa < 0) continue;
+            if (which[i] == 0) {
+              tgd[oa] += v;
+            } else {
+              tgd[p.tidx[oa]] += v;
+              if (p.arc_of[oa] >= 0) agh[gb.first_arc[b] + p.arc_of[oa]] += v;
+            }
+          }
+        }
+      }
+      gtnb_lattice_destroy(ctx, lat);
+      lat = nullptr;
+    }
+    a.losses_host[b] = sc[0] - sc[1];
+  }
+  if (!want) return GTNB_OK;
+  std::vector<float> tgh(tgd.begin(), tgd.end());
+  GTNB_TRY(write_user(ctx, a.grads, a.grads_on_device, gh.data(), per * B));
+  GTNB_TRY(write_user(ctx, a.trans_grad, a.trans_grad_on_device, tgh.data(), n_trans));
+  return write_user(ctx, arc_grads, arc_grads_on_device, agh.data(), tot_arcs);
+}
+
+int backoff_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
+                     const SparseTables& t, float* arc_grads, int arc_grads_on_device) {
+  const int B = a.B, C = a.C;
+  const long long n_trans = Gv.num_arcs;
+  // the device route's numerators and their tables, whose shapes decide, with G's, whether it can be taken
+  std::vector<ProductGraph> prods;
+  std::vector<SparseTables> ptabs;
+  bool fast = ctx->use_implicit && eps_fits(t, C);
+  if (fast) {
+    prods.resize(B);
+    ptabs.resize(B);
+    for (int b = 0; b < B && fast; b++) {
+      build_sparse_product(gb.views[b], Gv, t, C, /*fold=*/false, &prods[b]);
+      const gtnb_graph_view pv = prods[b].view();
+      sparse_tables(pv, C, &ptabs[b]);
+      sparse_eps_tables(pv, &ptabs[b]);
+      fast = eps_fits(ptabs[b], C);
+    }
+  }
+  return run_criterion(ctx, B, gb.Tb.data(), a.losses_host, a.trans_grad, a.trans_grad_on_device, n_trans, fast,
+                       [&](CallScope& scope, bool f, bool* needs_exact) {
+                         if (!f) return backoff_loss_exact(scope, a, gb, Gv, t, arc_grads, arc_grads_on_device);
+                         return backoff_loss_fast(scope, a, gb, n_trans, t, prods, ptabs, arc_grads,
+                                                  arc_grads_on_device, needs_exact);
+                       });
+}
+
+/*
+ * The exact route of gtnb_viterbi_backoff for the utterances `which`: compose(E_b, G') in the reference's numbering,
+ * G' = G with its arc ids as olabels, then gtnb_forward(tropical) and gtnb_viterbi_path.  The path's arcs with an
+ * epsilon ilabel are G's epsilon arcs, which use no frame and are not reported.
+ */
+int backoff_viterbi_exact(CallScope& scope, const GraphBatch& gb, const gtnb_graph_view& Gv, const float* W,
+                          const ViterbiBufs& v, const std::vector<int>& which) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int T = gb.T, C = gb.C;
+  const long long per = (long long)T * C;
+  std::vector<int32_t> ids(std::max(Gv.num_arcs, 1));
+  for (int k = 0; k < Gv.num_arcs; k++) ids[k] = k;
+  gtnb_graph_view G = Gv;
+  G.arc_olabel = ids.data();
+  G.weights = W;
+  std::vector<float> e((size_t)std::max(per, 1ll));
+  std::vector<int32_t> prow(std::max(T, 1)), arow(std::max(T, 1));
+  for (int b : which) {
+    const int Tb = gb.Tb[b];
+    std::fill(prow.begin(), prow.end(), -1);
+    std::fill(arow.begin(), arow.end(), -1);
+    float score = -std::numeric_limits<float>::infinity();
+    if (Tb > 0) {
+      GTNB_TRY(read_to_host(ctx, e.data(), v.e_dev + per * b, 1, (long long)Tb * C));
+      HostGraph E;
+      linear_host(Tb, C, e.data(), &E);
+      ComposedHost c;
+      GTNB_TRY(compose_host(ctx, E.view(), G, /*first sorted=*/1, &c));
+      if (c.N > 0) {
+        const gtnb_graph_view cv = c.view();
+        gtnb_lattice*& lat = scope.lattice();
+        GTNB_TRY(gtnb_pack(ctx, 1, &cv, &lat));
+        float s = 0.0f;
+        GTNB_TRY(gtnb_forward(ctx, lat, 1, &s, nullptr));
+        const int ml = std::max(c.N, 1);
+        std::vector<int32_t> pa(ml), il(ml), ol(ml);
+        int32_t len = -1;
+        GTNB_TRY(gtnb_viterbi_path(ctx, lat, ml, pa.data(), il.data(), ol.data(), nullptr, &len, nullptr));
+        gtnb_lattice_destroy(ctx, lat);
+        lat = nullptr;
+        if (len >= 0) {
+          score = s;
+          for (int k = 0, f = 0; k < len; k++)
+            if (il[k] != GTNB_EPSILON && f < T) {
+              prow[f] = il[k];
+              arow[f++] = ol[k];
+            }
+        }
+      }
+    }
+    if (v.p_dev && T > 0)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(v.p_dev + (long long)b * T, prow.data(), sizeof(int32_t) * T,
+                                     cudaMemcpyHostToDevice, ctx->stream));
+    if (v.a_dev && T > 0)
+      GTNB_CUDA(ctx, cudaMemcpyAsync(v.a_dev + (long long)b * T, arow.data(), sizeof(int32_t) * T,
+                                     cudaMemcpyHostToDevice, ctx->stream));
+    GTNB_CUDA(ctx, cudaMemcpyAsync(v.s_dev + b, &score, sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    GTNB_TRY(scope.sync()); // (the rows are reused by the next utterance)
+  }
+  return GTNB_OK;
+}
+
+int backoff_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
+                        const SparseTables& t, const float* trans_w, int trans_on_device) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = gb.B, T = gb.T, C = gb.C;
+  const long long n_trans = Gv.num_arcs;
+  ViterbiBufs v;
+  GTNB_TRY(viterbi_open(scope, a, gb, &v));
+  const bool implicit = ctx->use_implicit && eps_fits(t, C);
+  if (implicit) {
+    EpsDevTables tabs;
+    tabs.add(t, 0, 0);
+    GTNB_TRY(tabs.alloc(scope));
+    float* w_dev = nullptr;
+    int32_t *T_dev = nullptr, *head = nullptr;
+    uint16_t* bp = nullptr;
+    GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, std::max(n_trans, 1ll), &w_dev));
+    GTNB_TRY(scope.alloc(&T_dev, B));
+    GTNB_TRY(scope.alloc(&head, B));
+    GTNB_TRY(scope.alloc(&bp, (long long)B * (T + 1) * t.S));
+    GTNB_TRY(stage_begin(ctx));
+    GTNB_TRY(tabs.stage(scope));
+    GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
+    if (!trans_on_device && n_trans) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
+    GTNB_TRY(stage_end(ctx));
+    GTNB_TRY(launch_sparse_eps_viterbi(ctx, tabs.dev, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head,
+                                       v.s_dev, v.p_dev, v.a_dev, v.status));
+  }
+  return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
+    std::vector<float> W(std::max(n_trans, 1ll));
+    if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
+    return backoff_viterbi_exact(scope, gb, Gv, W.data(), v, which);
+  });
+}
+
+} // namespace
+
+extern "C" int gtnb_backoff_transitions_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
+    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, float* losses_host, float* grads,
+    int grads_on_device, float* arc_grads, int arc_grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  const std::string fn = "gtnb_backoff_transitions_loss";
+  GraphBatch gb;
+  SparseTables t;
+  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, C, emissions, graphs,
+                        transitions && (B == 0 || (losses_host && trans_w)), input_lens, arc_weights,
+                        arc_weights_on_device, &gb, [&] { return check_backoff_graph(ctx, fn, *transitions, C, &t); }));
+  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, nullptr,
+                         nullptr, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
+  if (t.E == 0) return sparse_transitions_loss_run(ctx, a, gb, *transitions, t, arc_grads, arc_grads_on_device);
+  return backoff_loss_run(ctx, a, gb, *transitions, t, arc_grads, arc_grads_on_device);
+}
+
+extern "C" int gtnb_viterbi_backoff(gtnb_ctx* ctx, int B, int T, int C, const float* emissions,
+                                    int emissions_on_device, const int32_t* input_lens,
+                                    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device,
+                                    int32_t* paths, int32_t* arcs, float* scores, int outputs_on_device) {
+  const std::string fn = "gtnb_viterbi_backoff";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !transitions || (B > 0 && (!emissions || !trans_w)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  SparseTables t;
+  GTNB_TRY(check_backoff_graph(ctx, fn, *transitions, C, &t));
+  GraphBatch gb; // the batch without target graphs: its lengths
+  gb.B = B, gb.T = T, gb.C = C;
+  gb.Tb.resize(B);
+  for (int b = 0; b < B; b++) {
+    gb.Tb[b] = input_lens ? input_lens[b] : T;
+    if (gb.Tb[b] < 0 || gb.Tb[b] > T) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": input_lens outside [0, T]");
+  }
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  const GraphViterbiArgs a{emissions, emissions_on_device, paths, arcs, scores, outputs_on_device};
+  if (t.E == 0) return viterbi_sparse_run(scope, a, gb, *transitions, trans_w, trans_on_device);
+  return backoff_viterbi_run(scope, a, gb, *transitions, t, trans_w, trans_on_device);
 }

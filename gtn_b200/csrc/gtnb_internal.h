@@ -404,6 +404,26 @@ int launch_sparse_sigma(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int3
                         float* sigma);
 int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, int nG, const float* w,
                        const float* sigma, float* wgrad);
+// The backoff sweeps over acceptors with epsilon arcs (SparseEpsDev, gtnb_meta.h): gs[0] for every CTA, or gs[b] for
+// CTA b when per_cta (then alpha rows at gs[b].rows, and max_S / max_AE the largest S / A + E of the batch).  The
+// envelope: S <= kSparseMaxStates, A + E <= kSparseMaxArcs, L <= kSparseMaxLevels, in-degree below kBpStart, C <=
+// kSparseMaxLabels (sparse_eps_supported).  The backward adds sgn times the gradients.  The decode's bp: [B][T + 1][S].
+int launch_sparse_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int B, int T, int C,
+                              const int32_t* lens, const float* emis, long long stride, const float* w, float* alpha,
+                              double* offs, float* den, int32_t* status);
+int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int max_AE, int B,
+                               int T, int C, const int32_t* lens, const float* emis, long long stride, const float* w,
+                               const float* alpha, const double* offs, float sgn, float* grad, long long grad_stride,
+                               float* wgrad);
+int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, int S, int B, int T, int C, const int32_t* lens,
+                              const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
+                              float* score, int32_t* paths, int32_t* arcs, int32_t* status);
+// out[k] = w_A[arc_of[k]] + W[tidx[k]], W[tidx[k]] alone where arc_of[k] < 0 (G's epsilon arcs in the numerators)
+int launch_sparse_eps_gather(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W,
+                             const int32_t* tidx, float* out);
+// tgrad[tidx[k]] += pg[k], and agrad[arc_of[k]] += pg[k] where arc_of[k] >= 0 (agrad nullable)
+int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const int32_t* arc_of, const int32_t* tidx,
+                              float* tgrad, float* agrad);
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);

@@ -36,6 +36,34 @@ inline int sparse_den_lanes(int S, int A) {
   return lanes;
 }
 
+/*
+ * An acceptor with epsilon arcs as k_sparse.cu's backoff sweeps read it (gtnb_product.h's SparseTables with its
+ * epsilon tables): g holds the emitting arcs, then come the E epsilon arcs (by destination and by source; *_arc
+ * indexes the weights and their gradient like g's) in L topological levels.  Forward level l is the nodes
+ * fwd_node[fwd_ptr[l] .. fwd_ptr[l + 1]), whose epsilon in-arcs leave nodes of earlier levels only; backward level l
+ * (bwd_*) likewise over the epsilon out-arcs.  lanes[l] / lanes[L + l]: threads per node of forward / backward level
+ * l.  rows: the first float of this graph's score rows when every CTA reads its own graph (the numerators).
+ */
+struct SparseEpsDev {
+  SparseDev g;
+  int E, L;
+  const int32_t *eps_in_ptr, *eps_in_src, *eps_in_arc;
+  const int32_t *eps_out_ptr, *eps_out_dst, *eps_out_arc;
+  const int32_t *fwd_ptr, *fwd_node, *bwd_ptr, *bwd_node, *lanes;
+  long long rows;
+};
+/* the envelope's level bound: each level costs one CTA barrier per frame (a backoff n-gram of order n has n - 1) */
+constexpr int kSparseMaxLevels = 32;
+/* the backoff decode's back-pointer of a start node at frame 0; a node's in-list (emitting then epsilon in-arcs) is
+ * below it, so both fit the 15 position bits */
+constexpr int kBpStart = 0x7FFE;
+/* the envelope of the backoff sweeps, for G and for every numerator: S nodes, A emitting and E epsilon arcs, L levels,
+ * max_in the largest in-degree counting both kinds of arc */
+inline bool sparse_eps_supported(int S, int A, int E, int L, int max_in, int C) {
+  return S >= 1 && S <= kSparseMaxStates && (long long)A + E <= kSparseMaxArcs && L <= kSparseMaxLevels &&
+         max_in < kBpStart && C >= 1 && C <= kSparseMaxLabels;
+}
+
 /* semiring / output of the shortest-distance kernels */
 enum { MODE_LOG = 0, MODE_TROPICAL = 1, MODE_PATH = 2 };
 

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "gtn_b200.h"
+#include "gtnb_meta.h"
 
 namespace gtnb {
 
@@ -149,6 +150,14 @@ struct SparseTables {
   std::vector<int32_t> in_ptr, in_src, in_lab, in_arc;
   std::vector<int32_t> out_ptr, out_dst, out_lab, out_arc;
   std::vector<int32_t> grp_ptr, grp_arc, grp_dst, grp_lab;
+  // G's epsilon arcs (sparse_eps_tables; empty for an epsilon-free G), kept apart from the emitting lists above
+  int E = 0, L = 0; // epsilon arcs, topological levels
+  std::vector<int32_t> eps_in_ptr, eps_in_src, eps_in_arc; // by destination ([S + 1] pointers)
+  std::vector<int32_t> eps_out_ptr, eps_out_dst, eps_out_arc; // by source
+  std::vector<int32_t> fwd_ptr, fwd_node, bwd_ptr, bwd_node; // [L + 1] pointers: the levels' nodes
+  std::vector<int32_t> lanes; // [2L]: threads per node of every forward, then every backward level
+  int max_in_all = 0; // the largest in-degree counting both kinds of arc
+  std::vector<int32_t> cycle; // the nodes of an epsilon cycle, in arc order, when G has one (then no levels)
 };
 
 inline void sparse_tables(const gtnb_graph_view& G, int C, SparseTables* t) {
@@ -212,6 +221,98 @@ inline void sparse_tables(const gtnb_graph_view& G, int C, SparseTables* t) {
 }
 
 /*
+ * The epsilon arcs of G (olabel GTNB_EPSILON; the backoff entry points: ilabel too) into t, after sparse_tables.  An
+ * epsilon arc moves G without consuming a frame, so a frame's scores are closed over them in topological order.
+ * Kahn's algorithm gives every node a forward level, 0 without epsilon in-arcs, else 1 + the largest level of their
+ * sources; levels 1 .. L are t->fwd_* (level l at index l - 1), and a level only reads nodes finished in earlier
+ * ones.  The backward levels mirror them over the epsilon out-arcs (0 without any, else 1 + the largest level of
+ * their destinations), so that a node's departures are complete before it reads them.  Both number L, the longest
+ * epsilon path: a backoff n-gram of order n has n - 1.  A cycle of epsilon arcs leaves t->cycle set (its nodes in
+ * arc order) and no levels.
+ */
+inline void sparse_eps_tables(const gtnb_graph_view& G, SparseTables* t) {
+  const int S = t->S;
+  std::vector<int32_t> eps;
+  for (int g = 0; g < G.num_arcs; g++)
+    if (G.arc_olabel[g] == GTNB_EPSILON) eps.push_back(g);
+  t->E = (int)eps.size();
+  auto csr = [&](const int32_t* key, const int32_t* other, std::vector<int32_t>& ptr, std::vector<int32_t>& nb,
+                 std::vector<int32_t>& arc) {
+    ptr.assign(S + 1, 0);
+    for (int g : eps) ptr[key[g] + 1]++;
+    for (int v = 0; v < S; v++) ptr[v + 1] += ptr[v];
+    arc = eps;
+    std::stable_sort(arc.begin(), arc.end(), [&](int x, int y) { return key[x] < key[y]; });
+    nb.resize(arc.size());
+    for (size_t k = 0; k < arc.size(); k++) nb[k] = other[arc[k]];
+  };
+  csr(G.arc_dst, G.arc_src, t->eps_in_ptr, t->eps_in_src, t->eps_in_arc);
+  csr(G.arc_src, G.arc_dst, t->eps_out_ptr, t->eps_out_dst, t->eps_out_arc);
+  t->max_in_all = 0;
+  for (int v = 0; v < S; v++)
+    t->max_in_all = std::max(t->max_in_all, t->in_ptr[v + 1] - t->in_ptr[v] + t->eps_in_ptr[v + 1] - t->eps_in_ptr[v]);
+  // Kahn over the epsilon subgraph: order holds the nodes in a topological order, lf their forward levels
+  std::vector<int32_t> indeg(S), lf(S, 0), order;
+  for (int v = 0; v < S; v++) {
+    indeg[v] = t->eps_in_ptr[v + 1] - t->eps_in_ptr[v];
+    if (!indeg[v]) order.push_back(v);
+  }
+  for (size_t i = 0; i < order.size(); i++) {
+    const int u = order[i];
+    for (int k = t->eps_out_ptr[u]; k < t->eps_out_ptr[u + 1]; k++) {
+      const int v = t->eps_out_dst[k];
+      lf[v] = std::max(lf[v], lf[u] + 1);
+      if (--indeg[v] == 0) order.push_back(v);
+    }
+  }
+  t->cycle.clear();
+  if ((int)order.size() < S) {
+    // every node left has an epsilon in-arc from another node left: walk them back until a node repeats
+    int v = 0;
+    while (!indeg[v]) v++;
+    std::vector<int32_t> seen(S, -1), walk;
+    while (seen[v] < 0) {
+      seen[v] = (int32_t)walk.size();
+      walk.push_back(v);
+      for (int k = t->eps_in_ptr[v]; k < t->eps_in_ptr[v + 1]; k++)
+        if (indeg[t->eps_in_src[k]]) {
+          v = t->eps_in_src[k];
+          break;
+        }
+    }
+    t->cycle.assign(walk.begin() + seen[v], walk.end());
+    std::reverse(t->cycle.begin(), t->cycle.end());
+    t->L = 0;
+    return;
+  }
+  std::vector<int32_t> lb(S, 0);
+  for (int i = S - 1; i >= 0; i--) {
+    const int u = order[i];
+    for (int k = t->eps_out_ptr[u]; k < t->eps_out_ptr[u + 1]; k++) lb[u] = std::max(lb[u], lb[t->eps_out_dst[k]] + 1);
+  }
+  t->L = S ? std::max(*std::max_element(lf.begin(), lf.end()), 0) : 0;
+  auto levels = [&](const std::vector<int32_t>& lev, const std::vector<int32_t>& ptr_of, std::vector<int32_t>& ptr,
+                    std::vector<int32_t>& node) {
+    ptr.assign(t->L + 1, 0);
+    for (int v = 0; v < S; v++)
+      if (lev[v]) ptr[lev[v]]++;
+    for (int l = 0; l < t->L; l++) ptr[l + 1] += ptr[l];
+    node.assign(ptr[t->L], 0);
+    std::vector<int32_t> fill(ptr.begin(), ptr.end() - 1);
+    for (int v = 0; v < S; v++)
+      if (lev[v]) node[fill[lev[v] - 1]++] = v;
+    for (int l = 0; l < t->L; l++) { // about four arcs per thread at the level's mean degree
+      long long arcs = 0;
+      for (int i = ptr[l]; i < ptr[l + 1]; i++) arcs += ptr_of[node[i] + 1] - ptr_of[node[i]];
+      t->lanes.push_back(sparse_den_lanes(ptr[l + 1] - ptr[l], (int)arcs));
+    }
+  };
+  t->lanes.clear();
+  levels(lf, t->eps_in_ptr, t->fwd_ptr, t->fwd_node);
+  levels(lb, t->eps_out_ptr, t->bwd_ptr, t->bwd_node);
+}
+
+/*
  * The numerator of gtnb_sparse_transitions_loss, intersect(A, G), from structure only: the (A node, G node) pairs
  * reachable from the start pairs, trimmed to those that reach an accept pair (A and G both accept).  An A arc u -> v
  * and a G arc p -> q with the same label in [0, C) give the arc (u, p) -> (v, q); arc_of is the A arc, tidx the G arc.
@@ -220,6 +321,8 @@ inline void sparse_tables(const gtnb_graph_view& G, int C, SparseTables* t) {
  * and per start group k of G with a's label and destination q; its tidx is nG + k (nG = G's arc count), so Wx =
  * [trans_w | sigma] and its weight is w_a + sigma_k.  The pairs with both nodes start are then ordinary states,
  * reached through in-arcs only.  An empty product keeps one node that neither starts nor accepts.
+ * When t has epsilon tables (sparse_eps_tables; the backoff entry points, unfolded only), G's epsilon arc p -> q
+ * gives (u, p) -> (u, q) for every A node u, labelled GTNB_EPSILON, with arc_of -1 and tidx the G arc.
  */
 inline void build_sparse_product(const gtnb_graph_view& A, const gtnb_graph_view& G, const SparseTables& t, int C,
                                  bool fold, ProductGraph* p) {
@@ -290,6 +393,10 @@ inline void build_sparse_product(const gtnb_graph_view& A, const gtnb_graph_view
         put((int)n, node(A.arc_dst[a], t.out_dst[k]), l, a, t.out_arc[k]);
       }
     }
+    // G's epsilon arcs (sparse_eps_tables): A stays, G moves, (u, q) -> (u, q'); no A arc, so arc_of is -1
+    if (!t.eps_out_ptr.empty())
+      for (int k = t.eps_out_ptr[q]; k < t.eps_out_ptr[q + 1]; k++)
+        put((int)n, node(u, t.eps_out_dst[k]), GTNB_EPSILON, -1, t.eps_out_arc[k]);
   }
   const int M = (int)state.size();
   auto accepts = [&](int n) {
@@ -350,6 +457,7 @@ inline void build_sparse_product(const gtnb_graph_view& A, const gtnb_graph_view
   for (size_t k = 0; k < p->src.size(); k++) {
     indeg[p->dst[k]]++;
     outdeg[p->src[k]]++;
+    if (p->label[k] == GTNB_EPSILON) continue;
     int32_t& il = in_label[p->dst[k]];
     if (il >= 0 && il != p->label[k]) p->uniform = false;
     il = p->label[k];
@@ -359,10 +467,12 @@ inline void build_sparse_product(const gtnb_graph_view& A, const gtnb_graph_view
   p->n_acc = (int)std::count_if(p->flags.begin(), p->flags.end(), [](uint8_t f) { return (f & 2) != 0; });
 }
 
-/* the product's arc weights: w[k] = w_A[arc_of[k]] + Wx[tidx[k]] (w_A NULL: every A weight 0) */
+/* the product's arc weights: w[k] = w_A[arc_of[k]] + Wx[tidx[k]] (w_A NULL: every A weight 0); Wx[tidx[k]] alone
+ * for an epsilon arc of G (arc_of -1), compose's weight for an arc of one side (compose.cpp:201-205) */
 inline void product_weights(const ProductGraph& p, const float* w_A, const float* Wx, std::vector<float>* w) {
   w->resize(p.src.size());
-  for (size_t k = 0; k < p.src.size(); k++) (*w)[k] = (w_A ? w_A[p.arc_of[k]] : 0.0f) + Wx[p.tidx[k]];
+  for (size_t k = 0; k < p.src.size(); k++)
+    (*w)[k] = p.arc_of[k] < 0 ? Wx[p.tidx[k]] : (w_A ? w_A[p.arc_of[k]] : 0.0f) + Wx[p.tidx[k]];
 }
 
 } // namespace gtnb

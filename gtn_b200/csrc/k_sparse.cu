@@ -35,6 +35,11 @@
  * (compose.cpp:435, then shortest.cpp:213), with absolute scores so that the score is bit-exact.  Per (frame, node) it
  * keeps a 16-bit back-pointer in HBM, the winning in-arc's position in the node's in-list plus a tie flag, and
  * sparse_viterbi_trace_kernel walks them back from the best accept node.
+ *
+ * The backoff entry points (gtnb_backoff_transitions_loss, gtnb_viterbi_backoff) take a G with epsilon arcs, and
+ * their numerators A_b o G have them too.  The sparse_eps_* kernels are the kernels above with an epsilon closure
+ * after every frame's emitting update (one CTA barrier per topological level of the epsilon subgraph) and per-CTA
+ * tables, so that one launch sweeps B different numerators; an epsilon-free G keeps the kernels above.
  */
 #include <algorithm>
 
@@ -460,6 +465,452 @@ __global__ void __launch_bounds__(256) sparse_tau_kernel(int K, const int32_t* _
   if (lane == 0) tau[k] = m;
 }
 
+/*
+ * The backoff sweeps: the kernels above over an acceptor with epsilon arcs (SparseEpsDev, gtnb_meta.h), one CTA per
+ * utterance.  An epsilon arc consumes no frame, so every frame's row, frame 0's and frame T_b's included, is closed
+ * over the epsilon arcs after its emitting update, one topological level at a time with one CTA barrier per level.
+ * The CTA's graph is gs[b] when per_cta (the numerators: every utterance its own product A_b o G, its score rows at
+ * gs[b].rows) and gs[0] otherwise (the denominator, G for the whole batch).
+ */
+
+/* the closure of row R over the forward levels, R[v] = logadd(R[v], logsumexp over v's epsilon in-arcs u -> v of
+ * R[u] + w): rows relative to one offset stay so.  bad |= a non-finite epsilon weight.  Ends on a barrier. */
+__device__ __forceinline__ void eps_close_fwd(const SparseEpsDev& x, const float* __restrict__ w, float* R, bool& bad) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    const int n0 = __ldg(x.fwd_ptr + l), n1 = __ldg(x.fwd_ptr + l + 1);
+    for (int i0 = n0; i0 < n1; i0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int i = i0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      int v = 0;
+      if (i < n1) {
+        v = __ldg(x.fwd_node + i);
+        const int k1 = __ldg(x.eps_in_ptr + v + 1);
+        for (int k = __ldg(x.eps_in_ptr + v) + q; k < k1; k += lanes) {
+          const float wk = __ldg(w + __ldg(x.eps_in_arc + k));
+          bad |= !is_finite(wk);
+          lse_add(m, s, R[__ldg(x.eps_in_src + k)] + wk);
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (i < n1 && q == 0 && m != neg_inf()) {
+        lse_add(m, s, R[v]);
+        R[v] = m + log_fast(s);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+/* the closure of a beta row R over the backward levels, R[u] = logadd(R[u], logsumexp over u's epsilon out-arcs
+ * u -> v of w + R[v]), and the posterior exp(al[u] + fo + w + R[v]) of each epsilon arc added into acc[k] (k: its
+ * position in the epsilon out-table; fo = c_t + d_t - Z, R relative to d_t).  Ends on a barrier. */
+__device__ __forceinline__ void eps_close_bwd(const SparseEpsDev& x, const float* __restrict__ w, float* R,
+                                              const float* __restrict__ al, float fo, float* acc) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + x.L + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    const int n0 = __ldg(x.bwd_ptr + l), n1 = __ldg(x.bwd_ptr + l + 1);
+    for (int i0 = n0; i0 < n1; i0 += groups) {
+      const int i = i0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      int u = 0;
+      if (i < n1) {
+        u = __ldg(x.bwd_node + i);
+        const float au = al[u] + fo;
+        const int k1 = __ldg(x.eps_out_ptr + u + 1);
+        for (int k = __ldg(x.eps_out_ptr + u) + q; k < k1; k += lanes) {
+          const float xk = __ldg(w + __ldg(x.eps_out_arc + k)) + R[__ldg(x.eps_out_dst + k)];
+          lse_add(m, s, xk);
+          const float p = exp_fast(au + xk);
+          if (p != 0.0f) acc[k] += p;
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (i < n1 && q == 0 && m != neg_inf()) {
+        lse_add(m, s, R[u]);
+        R[u] = m + log_fast(s);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+/* the maximum of row R over the CTA into red[kSparseWarps] (merged by row_offset after the next barrier); the row
+ * also to out (nullable) */
+__device__ __forceinline__ void row_max(const float* R, int S, float* out, float* red) {
+  float mx = neg_inf();
+  for (int v = threadIdx.x; v < S; v += blockDim.x) {
+    const float r = R[v];
+    if (out) out[v] = r;
+    mx = fmaxf(mx, r);
+  }
+  mx = warp_max(mx);
+  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = mx;
+}
+
+/*
+ * sparse_den_forward_kernel with the epsilon closure: alpha rows (after the closure) to alpha + the CTA's row base,
+ * c_t to offs[b][t], Z to offs[b][0] and den[b]; status[b] |= 1 on a non-finite weight or used emission.
+ */
+__global__ void __launch_bounds__(kSparseThreads) sparse_eps_forward_kernel(
+    const SparseEpsDev* __restrict__ gs, int per_cta, int T, int C, const int32_t* __restrict__ lens,
+    const float* __restrict__ emis, long long stride, const float* __restrict__ w, float* __restrict__ alpha,
+    double* __restrict__ offs, float* __restrict__ den, int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const SparseEpsDev x = gs[per_cta ? b : 0];
+  const SparseDev& g = x.g;
+  const int S = g.S, lanes = g.lanes;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  float* red = E + 2 * C; // [2][kSparseWarps]
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  float* al = alpha + (per_cta ? x.rows : (long long)b * (T + 1) * S);
+  double* of = offs + (long long)b * (T + 1);
+  bool bad = false;
+  for (int v = tid; v < S; v += nt) rows[v] = (__ldg(g.flags + v) & 1) ? 0.0f : neg_inf();
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  __syncthreads();
+  eps_close_fwd(x, w, rows, bad);
+  row_max(rows, S, al, red);
+  __syncthreads();
+  double c_off = 0.0;
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    const float Mp = row_offset(red + ((t - 1) & 1) * kSparseWarps);
+    for (int v0 = 0; v0 < S; v0 += groups) {
+      const int v = v0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (v < S) {
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int k = __ldg(g.in_ptr + v) + q; k < k1; k += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + k));
+          const float ek = Er[__ldg(g.in_lab + k)];
+          bad |= !(is_finite(wk) && is_finite(ek));
+          lse_add(m, s, P[__ldg(g.in_src + k)] + (wk + ek));
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (v < S && q == 0) Q[v] = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mp;
+    }
+    __syncthreads();
+    eps_close_fwd(x, w, Q, bad);
+    row_max(Q, S, al + (long long)t * S, red + (t & 1) * kSparseWarps);
+    c_off += (double)Mp;
+    if (tid == 0) of[t] = c_off;
+    __syncthreads();
+  }
+  bad = __syncthreads_or(bad);
+  if (tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    for (int v = tid; v < S; v += 32)
+      if (__ldg(g.flags + v) & 2) m = fmaxf(m, F[v]);
+    m = warp_max(m);
+    float s = 0.0f;
+    if (m != neg_inf())
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) s += expf(F[v] - m);
+    s = warp_sum(s);
+    if (tid == 0) {
+      const double Z = m == neg_inf() ? (double)neg_inf() : c_off + (double)(m + logf(s));
+      of[0] = Z;
+      den[b] = (float)Z;
+      if (bad) atomicOr(&status[b], 1);
+    }
+  }
+}
+
+/*
+ * sparse_den_backward_kernel with the epsilon closure: sgn * d Z / d e added into grad and sgn * d Z / d w into
+ * wgrad (the numerators: sgn = -1), an epsilon arc's posterior exp(alpha_t[u] + w + beta_t[v] - Z) into wgrad alone.
+ */
+__global__ void __launch_bounds__(kSparseThreads) sparse_eps_backward_kernel(
+    const SparseEpsDev* __restrict__ gs, int per_cta, int T, int C, const int32_t* __restrict__ lens,
+    const float* __restrict__ emis, long long stride, const float* __restrict__ w, const float* __restrict__ alpha,
+    const double* __restrict__ offs, float sgn, float* __restrict__ grad, long long grad_stride,
+    float* __restrict__ wgrad) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const SparseEpsDev x = gs[per_cta ? b : 0];
+  const SparseDev& g = x.g;
+  const int S = g.S, A = g.A, lanes = g.lanes;
+  float* rows = sm; // [2][S] beta rows
+  float* E = sm + 2 * S; // [2][C] emission rows
+  float* Eg = E + 2 * C; // [2][C] the frame's emission gradient
+  float* acc = Eg + 2 * C; // [A + E] arc gradient, by out-table position, then by epsilon out-table position
+  float* red = acc + A + x.E; // [2][kSparseWarps]
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const double* of = offs + (long long)b * (T + 1);
+  const double Z = of[0];
+  if (Tb < 1 || !(fabs(Z) < (double)CUDART_INF_F)) return;
+  const float* em = emis + (long long)b * stride;
+  const float* al = alpha + (per_cta ? x.rows : (long long)b * (T + 1) * S);
+  float* gr = grad + (long long)b * grad_stride;
+  for (int v = tid; v < S; v += nt) rows[(Tb & 1) * S + v] = (__ldg(g.flags + v) & 2) ? 0.0f : neg_inf();
+  for (int k = tid; k < A + x.E; k += nt) acc[k] = 0.0f;
+  for (int c = tid; c < 2 * C; c += nt) Eg[c] = 0.0f;
+  for (int c = tid; c < C; c += nt) E[((Tb - 1) & 1) * C + c] = __ldg(em + (long long)(Tb - 1) * C + c);
+  __syncthreads();
+  eps_close_bwd(x, w, rows + (Tb & 1) * S, al + (long long)Tb * S, (float)(of[Tb] - Z), acc + A);
+  row_max(rows + (Tb & 1) * S, S, nullptr, red + (Tb & 1) * kSparseWarps);
+  __syncthreads();
+  double d = 0.0; // d_{t+1}
+  for (int t = Tb - 1; t >= 0; t--) {
+    const float* Nx = rows + ((t + 1) & 1) * S;
+    float* Cur = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    float* Eg_t = Eg + (t & 1) * C;
+    float* Eg_prev = Eg + ((t + 1) & 1) * C; // frame t + 1's, complete since the barrier
+    for (int c = tid; c < C; c += nt) {
+      if (t > 0) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)(t - 1) * C + c);
+      if (t + 1 < Tb) {
+        const float v = Eg_prev[c];
+        if (v != 0.0f) atomicAdd(gr + (long long)(t + 1) * C + c, sgn * v);
+        Eg_prev[c] = 0.0f;
+      }
+    }
+    const float Mb = row_offset(red + ((t + 1) & 1) * kSparseWarps);
+    const double c_t = t > 0 ? of[t] : 0.0;
+    const float fo = (float)(c_t + d - Z);
+    for (int u0 = 0; u0 < S; u0 += groups) {
+      const int u = u0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (u < S) {
+        const float au = al[(long long)t * S + u] + fo;
+        const int k1 = __ldg(g.out_ptr + u + 1);
+        for (int k = __ldg(g.out_ptr + u) + q; k < k1; k += lanes) {
+          const int lab = __ldg(g.out_lab + k);
+          const float xk = Nx[__ldg(g.out_dst + k)] + (__ldg(w + __ldg(g.out_arc + k)) + Er[lab]);
+          lse_add(m, s, xk);
+          const float p = exp_fast(au + xk);
+          if (p != 0.0f) {
+            acc[k] += p;
+            atomicAdd(Eg_t + lab, p);
+          }
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (u < S && q == 0) Cur[u] = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mb;
+    }
+    __syncthreads();
+    eps_close_bwd(x, w, Cur, al + (long long)t * S, (float)(c_t + (d + (double)Mb) - Z), acc + A);
+    row_max(Cur, S, nullptr, red + (t & 1) * kSparseWarps);
+    d += (double)Mb;
+    __syncthreads();
+  }
+  for (int c = tid; c < C; c += nt) { // frame 0's emission gradient
+    const float v = Eg[c];
+    if (v != 0.0f) atomicAdd(gr + c, sgn * v);
+  }
+  for (int k = tid; k < A; k += nt)
+    if (acc[k] != 0.0f) atomicAdd(wgrad + __ldg(g.out_arc + k), sgn * acc[k]);
+  for (int k = tid; k < x.E; k += nt)
+    if (acc[A + k] != 0.0f) atomicAdd(wgrad + __ldg(x.eps_out_arc + k), sgn * acc[A + k]);
+}
+
+/* the tropical closure of row R over the forward levels: an epsilon arc u -> v wins over v's score when fl(R[u] + w)
+ * is larger; bp[v] then gets its position in v's combined in-list (the ne emitting in-arcs first), and the tie flag
+ * when another candidate, of either kind, reaches the same finite maximum.  bad |= a NaN or +inf epsilon weight. */
+__device__ __forceinline__ void eps_close_trop(const SparseEpsDev& x, const float* __restrict__ w, float* R,
+                                               uint16_t* bp, bool& bad) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    const int n0 = __ldg(x.fwd_ptr + l), n1 = __ldg(x.fwd_ptr + l + 1);
+    for (int i0 = n0; i0 < n1; i0 += groups) {
+      const int i = i0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, v = 0, k0 = 0;
+      if (i < n1) {
+        v = __ldg(x.fwd_node + i);
+        k0 = __ldg(x.eps_in_ptr + v);
+        const int k1 = __ldg(x.eps_in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(x.eps_in_arc + j));
+          bad |= !(wk < CUDART_INF_F);
+          argmax_add(m, k, tie, R[__ldg(x.eps_in_src + j)] + wk, j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (i < n1 && q == 0) {
+        const float cur = R[v];
+        if (m > cur) {
+          const int ne = __ldg(x.g.in_ptr + v + 1) - __ldg(x.g.in_ptr + v);
+          R[v] = m;
+          bp[v] = (uint16_t)((ne + k - k0) | (tie ? kBpTie : 0));
+        } else if (m == cur && m != neg_inf()) {
+          bp[v] |= kBpTie;
+        }
+      }
+    }
+    __syncthreads();
+  }
+}
+
+/*
+ * sparse_viterbi_forward_kernel with the epsilon closure, G = gs[0] for every utterance.  bp[b][t][v] (t = 0 .. T_b,
+ * T + 1 rows per utterance): the position of the arc that reaches S_t[v] in v's combined in-list (its emitting
+ * in-arcs from frame t - 1, then its epsilon in-arcs from frame t), kBpStart for a start node at frame 0 that no
+ * epsilon arc improves, | kBpTie on a tie; kBpNone where S_t[v] = -inf.
+ */
+__global__ void __launch_bounds__(kSparseThreads) sparse_eps_viterbi_kernel(
+    const SparseEpsDev* __restrict__ gs, int T, int C, const int32_t* __restrict__ lens,
+    const float* __restrict__ emis, long long stride, const float* __restrict__ w, uint16_t* __restrict__ bp,
+    int32_t* __restrict__ head, float* __restrict__ score, int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
+  const SparseEpsDev x = gs[0];
+  const SparseDev& g = x.g;
+  const int S = g.S, lanes = g.lanes;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  uint16_t* bpb = bp + (long long)b * (T + 1) * S;
+  bool bad = false;
+  for (int v = tid; v < S; v += nt) {
+    const bool st = __ldg(g.flags + v) & 1;
+    rows[v] = st ? 0.0f : neg_inf();
+    bpb[v] = st ? (uint16_t)kBpStart : kBpNone;
+  }
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  __syncthreads();
+  eps_close_trop(x, w, rows, bpb, bad);
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    uint16_t* bpt = bpb + (long long)t * S;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    for (int v0 = 0; v0 < S; v0 += groups) {
+      const int v = v0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, k0 = 0;
+      if (v < S) {
+        k0 = __ldg(g.in_ptr + v);
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + j));
+          const float ek = Er[__ldg(g.in_lab + j)];
+          bad |= !(wk < CUDART_INF_F && ek < CUDART_INF_F);
+          argmax_add(m, k, tie, P[__ldg(g.in_src + j)] + (wk + ek), j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (v < S && q == 0) {
+        Q[v] = m;
+        bpt[v] = m == neg_inf() ? kBpNone : (uint16_t)((k - k0) | (tie ? kBpTie : 0));
+      }
+    }
+    __syncthreads();
+    eps_close_trop(x, w, Q, bpt, bad); // (its last barrier ends the frame)
+  }
+  bad = __syncthreads_or(bad);
+  if (tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    int k = 0x7fffffff, tie = 0;
+    if (Tb > 0)
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) argmax_add(m, k, tie, F[v], v);
+    argmax_merge(m, k, tie, 32);
+    if (tid == 0) {
+      head[b] = m == neg_inf() ? -1 : k;
+      score[b] = m;
+      const int st = (bad ? 1 : 0) | (tie ? 2 : 0);
+      if (st) atomicOr(&status[b], st);
+    }
+  }
+}
+
+/*
+ * The traceback of sparse_eps_viterbi_kernel, one warp per utterance: inside a frame it follows epsilon
+ * back-pointers (they use no frame and are not reported), and an emitting one writes paths[b][t - 1] / arcs[b][t - 1]
+ * and steps to frame t - 1; it ends at frame 0 on kBpStart.  -1 beyond T_b and in the whole row without a path.
+ * status[b] |= 2 when a node of the path carries the tie flag.
+ */
+__global__ void __launch_bounds__(256) sparse_eps_trace_kernel(
+    const SparseEpsDev* __restrict__ gs, int B, int T, const int32_t* __restrict__ lens,
+    const uint16_t* __restrict__ bp, const int32_t* __restrict__ head, int32_t* __restrict__ paths,
+    int32_t* __restrict__ arcs, int32_t* __restrict__ status) {
+  const int b = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (b >= B) return; // whole warps
+  const SparseEpsDev x = gs[0];
+  const int h = head[b];
+  const int n = h < 0 ? 0 : lens[b];
+  int32_t* pr = paths ? paths + (long long)b * T : nullptr;
+  int32_t* ar = arcs ? arcs + (long long)b * T : nullptr;
+  for (int t = n + lane; t < T; t += 32) {
+    if (pr) pr[t] = -1;
+    if (ar) ar[t] = -1;
+  }
+  if (lane != 0 || n == 0) return;
+  const int S = x.g.S;
+  const uint16_t* bpb = bp + (long long)b * (T + 1) * S;
+  int v = h, tie = 0, t = n;
+  for (;;) {
+    const int e = __ldg(bpb + (long long)t * S + v);
+    if (e == kBpNone) break; // (not on a path from a finite head)
+    const int pos = e & (kBpTie - 1);
+    tie |= e & kBpTie;
+    if (t == 0 && pos == kBpStart) break;
+    const int k0 = __ldg(x.g.in_ptr + v), ne = __ldg(x.g.in_ptr + v + 1) - k0;
+    if (pos >= ne) { // an epsilon arc inside frame t
+      v = __ldg(x.eps_in_src + __ldg(x.eps_in_ptr + v) + pos - ne);
+      continue;
+    }
+    const int k = k0 + pos;
+    if (pr) pr[t - 1] = __ldg(x.g.in_lab + k);
+    if (ar) ar[t - 1] = __ldg(x.g.in_arc + k);
+    v = __ldg(x.g.in_src + k);
+    t--;
+  }
+  if (tie) atomicOr(&status[b], 2);
+}
+
+/* the numerators' weights, gathered: w[k] = fl(w_A[arc_of[k]] + W[tidx[k]]), W[tidx[k]] alone for an epsilon arc
+ * (arc_of -1); w_A NULL: every A weight 0 */
+__global__ void __launch_bounds__(256) sparse_eps_gather_kernel(long long n, const float* __restrict__ w_A,
+                                                                const int32_t* __restrict__ arc_of,
+                                                                const float* __restrict__ W,
+                                                                const int32_t* __restrict__ tidx,
+                                                                float* __restrict__ out) {
+  const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int a = __ldg(arc_of + k);
+  const float wg = __ldg(W + __ldg(tidx + k));
+  out[k] = a < 0 ? wg : (w_A ? __ldg(w_A + a) : 0.0f) + wg;
+}
+
+/* the numerators' arc gradients (already signed) into the transition gradient (tidx) and, where an A arc is behind
+ * the product arc, into the arc gradient (arc_of >= 0; nullable) */
+__global__ void __launch_bounds__(256) sparse_eps_scatter_kernel(long long n, const float* __restrict__ pg,
+                                                                 const int32_t* __restrict__ arc_of,
+                                                                 const int32_t* __restrict__ tidx,
+                                                                 float* __restrict__ tgrad, float* __restrict__ agrad) {
+  const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const float v = pg[k];
+  if (v == 0.0f) return;
+  atomicAdd(tgrad + __ldg(tidx + k), v);
+  const int a = __ldg(arc_of + k);
+  if (agrad && a >= 0) atomicAdd(agrad + a, v);
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
@@ -525,6 +976,59 @@ int launch_sparse_tau(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_
   if (K == 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "sparse_tau", sparse_tau_kernel<<<(unsigned)(((long long)K * 32 + 255) / 256), 256, 0,
                                                      ctx->stream>>>(K, grp_ptr, grp_arc, w, tau));
+  return GTNB_OK;
+}
+
+int launch_sparse_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int B, int T, int C,
+                              const int32_t* lens, const float* emis, long long stride, const float* w, float* alpha,
+                              double* offs, float* den, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_forward_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_fwd_smem_floats(max_S, C);
+  GTNB_LAUNCH(ctx, "sparse_eps_forward", sparse_eps_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      gs, per_cta, T, C, lens, emis, stride, w, alpha, offs, den, status));
+  return GTNB_OK;
+}
+
+int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int max_AE, int B,
+                               int T, int C, const int32_t* lens, const float* emis, long long stride, const float* w,
+                               const float* alpha, const double* offs, float sgn, float* grad, long long grad_stride,
+                               float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_backward_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_bwd_smem_floats(max_S, max_AE, C);
+  GTNB_LAUNCH(ctx, "sparse_eps_backward", sparse_eps_backward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      gs, per_cta, T, C, lens, emis, stride, w, alpha, offs, sgn, grad, grad_stride, wgrad));
+  return GTNB_OK;
+}
+
+int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, int S, int B, int T, int C, const int32_t* lens,
+                              const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
+                              float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_viterbi_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_vit_smem_floats(S, C);
+  GTNB_LAUNCH(ctx, "sparse_eps_viterbi", sparse_eps_viterbi_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      gs, T, C, lens, emis, stride, w, bp, head, score, status));
+  GTNB_LAUNCH(ctx, "sparse_eps_trace", sparse_eps_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0,
+                                                                 ctx->stream>>>(gs, B, T, lens, bp, head, paths, arcs,
+                                                                                status));
+  return GTNB_OK;
+}
+
+int launch_sparse_eps_gather(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W,
+                             const int32_t* tidx, float* out) {
+  if (n == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "sparse_eps_gather", sparse_eps_gather_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
+      n, w_A, arc_of, W, tidx, out));
+  return GTNB_OK;
+}
+
+int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const int32_t* arc_of, const int32_t* tidx,
+                              float* tgrad, float* agrad) {
+  if (n == 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "sparse_eps_scatter", sparse_eps_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0,
+                                                                     ctx->stream>>>(n, pg, arc_of, tidx, tgrad, agrad));
   return GTNB_OK;
 }
 

@@ -476,6 +476,33 @@ def sparse_transitions_loss(emissions, transitions, transitions_graph, graphs, i
                                                input_lengths, reduction, allreduce)
 
 
+class BackoffTransitionsLossFunction(GraphTransitionsLossFunction):
+    """sparse_transitions_loss with a backoff transition graph, through gtnb_backoff_transitions_loss: G may have
+    epsilon arcs (ilabel == olabel == gtn.epsilon), the backoff arcs of a pruned n-gram token LM, which move G without
+    consuming a frame and weigh their own transitions entry; the score sums over every path, the backoff paths
+    included.  The arguments and the backward are sparse_transitions_loss's; an epsilon-free G gives its results.
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, transitions, weights, graphs, transitions_graph, input_lengths=None, reduction="mean",
+                allreduce=True):
+        gv = _graph_view(transitions_graph)
+        assert transitions.numel() == gv[0].num_arcs
+        return _transitions_forward(
+            ctx, emissions, transitions, weights, graphs, input_lengths, reduction, allreduce,
+            max(transitions.numel(), 1),
+            lambda c, tw, losses, grad, tg: capi.lib().gtnb_backoff_transitions_loss(
+                c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1,
+                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if c.ag is None else c.ag.data_ptr(), 1,
+                tg.data_ptr(), 1))
+
+
+def backoff_transitions_loss(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
+                             reduction="mean", allreduce=True):
+    return BackoffTransitionsLossFunction.apply(emissions, transitions, weights, graphs, transitions_graph,
+                                                input_lengths, reduction, allreduce)
+
+
 @torch.no_grad()
 def graph_viterbi(emissions, graphs, input_lengths=None, weights=None):
     """Best path of compose(A_b, E_b) for every utterance, A_b = graphs[b] (viterbiPath / viterbiScore of the lattice
@@ -540,6 +567,19 @@ def sparse_viterbi(emissions, transitions, transitions_graph, input_lengths=None
     c = _GraphCall(emissions, None, None, input_lengths, arc_grads=False)
     gv, tw = _sparse_transitions(c, transitions, transitions_graph)
     return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_viterbi_sparse(
+        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1))
+
+
+@torch.no_grad()
+def backoff_viterbi(emissions, transitions, transitions_graph, input_lengths=None):
+    """Best path of intersect(E_b, G) for every utterance, G the backoff transition graph of backoff_transitions_loss
+    (epsilon arcs allowed), through gtnb_viterbi_backoff: the decode of a model trained with that loss.  The arguments
+    and outputs are sparse_viterbi's.  arcs[b, t] is the emitting G arc taken at frame t: an epsilon arc uses no frame
+    and is not reported.  Ties are broken as the reference breaks them.
+    """
+    c = _GraphCall(emissions, None, None, input_lengths, arc_grads=False)
+    gv, tw = _sparse_transitions(c, transitions, transitions_graph)
+    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_viterbi_backoff(
         c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1))
 
 

@@ -765,6 +765,78 @@ int gtnb_sparse_transitions_viterbi(
     float* scores, /* [B] nullable: viterbiScore */
     int outputs_on_device);
 
+/*
+ * Loss with a backoff transition graph G: gtnb_sparse_transitions_loss with epsilon arcs allowed in G, the backoff
+ * arcs of a pruned n-gram token LM (each history state has arcs for the labels seen after it and one epsilon arc to
+ * its shorter history), composed natively instead of removed:
+ *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(A_b, G), E_b)).
+ * An epsilon arc of G has ilabel == olabel == GTNB_EPSILON.  It moves G without consuming a frame, at any frame
+ * 0 .. T_b (leaving a start node at frame 0 and reaching an accept node at frame T_b included), weighs trans_w[arc]
+ * alone, and gets its gradient in trans_grad (none in the emission gradient).  The score sums over every path, the
+ * backoff paths included, as the reference's does.  Arguments, outputs and every other rule are those of
+ * gtnb_sparse_transitions_loss, and an epsilon-free G gives exactly its results.  A cycle of epsilon arcs in G is
+ * GTNB_ERR_INVALID_ARGUMENT (the message names it); epsilon arcs in A_b, an arc with epsilon on one side only and a
+ * transducer G are GTNB_ERR_UNSUPPORTED.
+ * Device route (k_sparse.cu's backoff sweeps): G's epsilon arcs are put in topological levels, and every frame's
+ * scores are closed over them one level per CTA barrier.  The denominator sweeps G's tables; the numerators
+ * A_b o G (built on the host from structure only, with G's epsilon arcs) sweep their own tables, one CTA each, with
+ * weights gathered on the device.  The envelope, for G and for every numerator: at most 4096 nodes, 32768 emitting
+ * plus epsilon arcs, 32 levels (the longest chain of epsilon arcs; a backoff n-gram of order n has n - 1), C <= 1024.
+ * Outside it, with a non-finite value or with the "implicit" flag off, the exact route composes E_b with G and the
+ * numerators with E_b (gtnb_compose_graphs) and runs the materialised lattices utterance by utterance.
+ */
+int gtnb_backoff_transitions_loss(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    const gtnb_graph_view* transitions, /* G: structure only, epsilon arcs allowed; its own weights ignored */
+    const float* trans_w, /* [G.num_arcs], G's arc numbering */
+    int trans_on_device,
+    float* losses_host,
+    float* grads, /* nullable */
+    int grads_on_device,
+    float* arc_grads, /* nullable */
+    int arc_grads_on_device,
+    float* trans_grad, /* nullable */
+    int trans_grad_on_device);
+
+/*
+ * Batched Viterbi decoding with a backoff transition graph G: gtnb_viterbi_sparse with epsilon arcs allowed in G
+ * (gtnb_backoff_transitions_loss's G and epsilon rule), viterbiPath / viterbiScore of intersect(E_b, G).  An epsilon
+ * arc uses no frame and is not reported: paths[b][t] / arcs[b][t] are the label and the emitting G arc taken at
+ * frame t.  Scores are bit-exact, and paths, arcs and scores equal the reference's, ties included.  Outputs, routing
+ * and their rules are gtnb_viterbi_sparse's, and an epsilon-free G gives exactly its results.  The device route
+ * sweeps G's tables in the tropical semiring with the epsilon closure after every frame and keeps a 16-bit
+ * back-pointer per frame and node (2 * B * (T + 1) * S bytes of scratch), which indexes the node's emitting in-arcs
+ * from the frame before, then its epsilon in-arcs from the same frame; the trace follows epsilon back-pointers
+ * inside a frame.  Its envelope is gtnb_backoff_transitions_loss's.  An utterance with a tie on its traced path
+ * ("exact_ties" on) or a NaN or +inf is re-run on compose(E_b, G) (gtnb_compose_graphs, gtnb_forward,
+ * gtnb_viterbi_path), as is the whole batch outside the envelope or with the "implicit" flag off.
+ * Error rules are gtnb_backoff_transitions_loss's for G and gtnb_viterbi_sparse's otherwise.
+ */
+int gtnb_viterbi_backoff(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    const gtnb_graph_view* transitions, /* G: structure only, epsilon arcs allowed; its own weights ignored */
+    const float* trans_w, /* [G.num_arcs], G's arc numbering */
+    int trans_on_device,
+    int32_t* paths, /* [B][T] nullable: label of frame t */
+    int32_t* arcs, /* [B][T] nullable: the emitting G arc taken at frame t (Graph arc numbering) */
+    float* scores, /* [B] nullable: viterbiScore */
+    int outputs_on_device);
+
 #ifdef __cplusplus
 }
 #endif
