@@ -128,6 +128,9 @@ SYMBOLS = [
     ("gtnb_viterbi_backoff", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _vp, _vp, _vp,
       C.c_int]),
+    ("gtnb_backoff_transitions_viterbi", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.POINTER(GraphView),
+      _vp, C.c_int, _vp, _vp, _vp, C.c_int]),
 ]
 
 _lib = None
@@ -661,8 +664,22 @@ class Ctx:
         return self._sparse_transitions_viterbi(True, emissions, views, transitions, trans_w, input_lens, arc_weights,
                                                 bool(trans_on_device))
 
+    def backoff_transitions_viterbi(self, emissions, views, transitions, trans_w, input_lens=None, arc_weights=None):
+        """Host-buffer entry of gtnb_backoff_transitions_viterbi: sparse_transitions_viterbi's arguments and results,
+        with epsilon arcs (backoff arcs) allowed in the transition graph; arcs holds A_b's emitting arc of every
+        frame."""
+        return self._sparse_transitions_viterbi(False, emissions, views, transitions, trans_w, input_lens, arc_weights,
+                                                False, "gtnb_backoff_transitions_viterbi")
+
+    def backoff_transitions_viterbi_dev(self, emissions, views, transitions, trans_w, input_lens=None,
+                                        arc_weights=None, trans_on_device=True):
+        """Device-buffer entry of gtnb_backoff_transitions_viterbi, as sparse_transitions_viterbi_dev
+        -> (paths, scores, arcs)."""
+        return self._sparse_transitions_viterbi(True, emissions, views, transitions, trans_w, input_lens, arc_weights,
+                                                bool(trans_on_device), "gtnb_backoff_transitions_viterbi")
+
     def _sparse_transitions_viterbi(self, dev, emissions, views, transitions, trans_w, input_lens, arc_weights,
-                                    trans_on_device):
+                                    trans_on_device, fn="gtnb_sparse_transitions_viterbi"):
         e = np.ascontiguousarray(emissions, dtype=np.float32)
         B, T, Cn = e.shape
         arr, _, aw = _graph_batch(views, B, arc_weights)
@@ -671,7 +688,7 @@ class Ctx:
         il = None if input_lens is None else np.ascontiguousarray(input_lens, np.int32)
         out = _viterbi_outputs(B, T)
         with _Placed(self, dev) as p:
-            self._check(lib().gtnb_sparse_transitions_viterbi(
+            self._check(getattr(lib(), fn)(
                 self.h, B, T, Cn, p.inp(e), p.flag, _p(il, _i32p), arr, p.inp(aw), p.flag, C.byref(gv),
                 p.inp(tw, trans_on_device), int(trans_on_device), *map(p.out, out), p.flag))
         return _viterbi_results(out, B, T)

@@ -2430,6 +2430,50 @@ int check_backoff_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_v
               fn + ": the transition graph has a cycle of epsilon arcs: " + path + std::to_string(t->cycle[0]));
 }
 
+/* the device route's numerators P_b = A_b o G (unfolded, with G's epsilon arcs) into prods and their tables into
+ * ptabs, for the whole batch; false, at the first that does not fit the backoff envelope */
+bool backoff_products(const GraphBatch& gb, const gtnb_graph_view& Gv, const SparseTables& t, int C,
+                      std::vector<ProductGraph>* prods, std::vector<SparseTables>* ptabs) {
+  prods->resize(gb.B);
+  ptabs->resize(gb.B);
+  for (int b = 0; b < gb.B; b++) {
+    build_sparse_product(gb.views[b], Gv, t, C, /*fold=*/false, &(*prods)[b]);
+    const gtnb_graph_view pv = (*prods)[b].view();
+    sparse_tables(pv, C, &(*ptabs)[b]);
+    sparse_eps_tables(pv, &(*ptabs)[b]);
+    if (!eps_fits((*ptabs)[b], C)) return false;
+  }
+  return true;
+}
+
+/* the numerators' device tables, one graph per CTA with its rows ((T_b + 1) * S_b entries) after the previous
+ * utterance's, and the product arcs' A arc (arc_of, -1 for G's epsilon arcs) and G arc (tidx) in the batch's
+ * numbering; -> the rows of the batch */
+long long backoff_numerators(const GraphBatch& gb, const std::vector<ProductGraph>& prods,
+                             const std::vector<SparseTables>& ptabs, EpsDevTables* num_t,
+                             std::vector<int32_t>* arc_of, std::vector<int32_t>* tidx) {
+  long long rows = 0;
+  for (int b = 0; b < gb.B; b++) {
+    num_t->add(ptabs[b], (int32_t)tidx->size(), rows);
+    rows += (long long)(gb.Tb[b] + 1) * ptabs[b].S;
+    for (int32_t k : prods[b].arc_of) arc_of->push_back(k < 0 ? -1 : (int32_t)(gb.first_arc[b] + k));
+    tidx->insert(tidx->end(), prods[b].tidx.begin(), prods[b].tidx.end());
+  }
+  return rows;
+}
+
+/* the batch's host arc weights in its numbering into w_A (an arc without weights: 0) when they are not on the device;
+ * -> whether there are any to upload */
+bool host_arc_weights(const GraphBatch& gb, std::vector<float>* w_A) {
+  if (gb.arc_weights_dev) return false;
+  w_A->assign((size_t)std::max(gb.tot_arcs, 1ll), 0.0f);
+  for (int b = 0; b < gb.B; b++) {
+    const gtnb_graph_view& v = gb.views[b];
+    if (v.weights) std::copy(v.weights, v.weights + v.num_arcs, w_A->begin() + gb.first_arc[b]);
+  }
+  return true;
+}
+
 /* the device route of gtnb_backoff_transitions_loss: ptabs[b] the tables of prods[b] (P_b = A_b o G, unfolded) */
 int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatch& gb, long long n_trans,
                       const SparseTables& t, const std::vector<ProductGraph>& prods,
@@ -2442,13 +2486,7 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
   EpsDevTables den_t, num_t;
   den_t.add(t, 0, 0);
   std::vector<int32_t> arc_of_h, tidx_h;
-  long long rows = 0;
-  for (int b = 0; b < B; b++) {
-    num_t.add(ptabs[b], (int32_t)tidx_h.size(), rows);
-    rows += (long long)(gb.Tb[b] + 1) * ptabs[b].S;
-    for (int32_t k : prods[b].arc_of) arc_of_h.push_back(k < 0 ? -1 : (int32_t)(gb.first_arc[b] + k));
-    tidx_h.insert(tidx_h.end(), prods[b].tidx.begin(), prods[b].tidx.end());
-  }
+  const long long rows = backoff_numerators(gb, prods, ptabs, &num_t, &arc_of_h, &tidx_h);
   const long long tot_P = (long long)tidx_h.size();
   std::vector<float> w_A_h;
   float *e_dev = nullptr, *w_dev = nullptr, *den = nullptr, *num = nullptr, *alpha_d = nullptr, *alpha_n = nullptr;
@@ -2472,14 +2510,7 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
   GTNB_TRY(scope.alloc(&tidx, tot_P));
   GTNB_TRY(den_t.alloc(scope));
   GTNB_TRY(num_t.alloc(scope));
-  if (!gb.arc_weights_dev) {
-    w_A_h.assign((size_t)std::max(tot_arcs, 1ll), 0.0f);
-    for (int b = 0; b < B; b++) {
-      const gtnb_graph_view& v = gb.views[b];
-      if (v.weights) std::copy(v.weights, v.weights + v.num_arcs, w_A_h.begin() + gb.first_arc[b]);
-    }
-    GTNB_TRY(scope.alloc(&w_A, (long long)w_A_h.size()));
-  }
+  if (host_arc_weights(gb, &w_A_h)) GTNB_TRY(scope.alloc(&w_A, (long long)w_A_h.size()));
   if (want) {
     GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
     GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, n_trans, &tg));
@@ -2682,18 +2713,7 @@ int backoff_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const GraphBatch& g
   // the device route's numerators and their tables, whose shapes decide, with G's, whether it can be taken
   std::vector<ProductGraph> prods;
   std::vector<SparseTables> ptabs;
-  bool fast = ctx->use_implicit && eps_fits(t, C);
-  if (fast) {
-    prods.resize(B);
-    ptabs.resize(B);
-    for (int b = 0; b < B && fast; b++) {
-      build_sparse_product(gb.views[b], Gv, t, C, /*fold=*/false, &prods[b]);
-      const gtnb_graph_view pv = prods[b].view();
-      sparse_tables(pv, C, &ptabs[b]);
-      sparse_eps_tables(pv, &ptabs[b]);
-      fast = eps_fits(ptabs[b], C);
-    }
-  }
+  const bool fast = ctx->use_implicit && eps_fits(t, C) && backoff_products(gb, Gv, t, C, &prods, &ptabs);
   return run_criterion(ctx, B, gb.Tb.data(), a.losses_host, a.trans_grad, a.trans_grad_on_device, n_trans, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
                          if (!f) return backoff_loss_exact(scope, a, gb, Gv, t, arc_grads, arc_grads_on_device);
@@ -2703,20 +2723,18 @@ int backoff_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const GraphBatch& g
 }
 
 /*
- * The exact route of gtnb_viterbi_backoff for the utterances `which`: compose(E_b, G') in the reference's numbering,
- * G' = G with its arc ids as olabels, then gtnb_forward(tropical) and gtnb_viterbi_path.  The path's arcs with an
- * epsilon ilabel are G's epsilon arcs, which use no frame and are not reported.
+ * The exact Viterbi route of the backoff entry points for the utterances `which`, one at a time: compose(b, E_b, &c)
+ * composes utterance b's lattice c (E_b = linearGraph(T_b, C) on its rows) in the reference's numbering, then
+ * gtnb_forward(tropical) and gtnb_viterbi_path run on it.  The path's arcs with an epsilon ilabel are G's epsilon
+ * arcs, which use no frame and are not reported; of the others, the ilabel is the label and the olabel the reported
+ * arc, or the other way round when arc_in.
  */
-int backoff_viterbi_exact(CallScope& scope, const GraphBatch& gb, const gtnb_graph_view& Gv, const float* W,
-                          const ViterbiBufs& v, const std::vector<int>& which) {
+template <class Compose>
+int eps_viterbi_exact(CallScope& scope, const GraphBatch& gb, const ViterbiBufs& v, const std::vector<int>& which,
+                      bool arc_in, Compose&& compose) {
   gtnb_ctx* ctx = scope.ctx();
   const int T = gb.T, C = gb.C;
   const long long per = (long long)T * C;
-  std::vector<int32_t> ids(std::max(Gv.num_arcs, 1));
-  for (int k = 0; k < Gv.num_arcs; k++) ids[k] = k;
-  gtnb_graph_view G = Gv;
-  G.arc_olabel = ids.data();
-  G.weights = W;
   std::vector<float> e((size_t)std::max(per, 1ll));
   std::vector<int32_t> prow(std::max(T, 1)), arow(std::max(T, 1));
   for (int b : which) {
@@ -2729,7 +2747,7 @@ int backoff_viterbi_exact(CallScope& scope, const GraphBatch& gb, const gtnb_gra
       HostGraph E;
       linear_host(Tb, C, e.data(), &E);
       ComposedHost c;
-      GTNB_TRY(compose_host(ctx, E.view(), G, /*first sorted=*/1, &c));
+      GTNB_TRY(compose(b, E.view(), &c));
       if (c.N > 0) {
         const gtnb_graph_view cv = c.view();
         gtnb_lattice*& lat = scope.lattice();
@@ -2746,8 +2764,8 @@ int backoff_viterbi_exact(CallScope& scope, const GraphBatch& gb, const gtnb_gra
           score = s;
           for (int k = 0, f = 0; k < len; k++)
             if (il[k] != GTNB_EPSILON && f < T) {
-              prow[f] = il[k];
-              arow[f++] = ol[k];
+              prow[f] = arc_in ? ol[k] : il[k];
+              arow[f++] = arc_in ? il[k] : ol[k];
             }
         }
       }
@@ -2762,6 +2780,20 @@ int backoff_viterbi_exact(CallScope& scope, const GraphBatch& gb, const gtnb_gra
     GTNB_TRY(scope.sync()); // (the rows are reused by the next utterance)
   }
   return GTNB_OK;
+}
+
+/* the exact route of gtnb_viterbi_backoff: compose(E_b, G'), G' = G with its arc ids as olabels (host weights W) */
+int backoff_viterbi_exact(CallScope& scope, const GraphBatch& gb, const gtnb_graph_view& Gv, const float* W,
+                          const ViterbiBufs& v, const std::vector<int>& which) {
+  std::vector<int32_t> ids(std::max(Gv.num_arcs, 1));
+  for (int k = 0; k < Gv.num_arcs; k++) ids[k] = k;
+  gtnb_graph_view G = Gv;
+  G.arc_olabel = ids.data();
+  G.weights = W;
+  return eps_viterbi_exact(scope, gb, v, which, /*arc_in=*/false,
+                           [&](int, const gtnb_graph_view& E, ComposedHost* c) {
+                             return compose_host(scope.ctx(), E, G, /*first sorted=*/1, c);
+                           });
 }
 
 int backoff_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
@@ -2795,6 +2827,92 @@ int backoff_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const Graph
     std::vector<float> W(std::max(n_trans, 1ll));
     if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
     return backoff_viterbi_exact(scope, gb, Gv, W.data(), v, which);
+  });
+}
+
+/*
+ * The exact route of gtnb_backoff_transitions_viterbi: compose(compose(A'_b, G), E_b), A'_b = A_b with its arc ids
+ * as ilabels (its olabels are matched, so the composition is the same) and G with its epsilon arcs and host weights
+ * W, in the reference's numbering: the unsorted matcher for the first (graph_transitions_viterbi_exact's), E_b's side
+ * sorted for the second (backoff_loss_exact's).  The path's ilabels are A_b's arcs and its olabels the labels.
+ */
+int backoff_align_exact(CallScope& scope, const GraphBatch& gb, const gtnb_graph_view& Gv, const float* W,
+                        const ViterbiBufs& v, const std::vector<int>& which) {
+  gtnb_ctx* ctx = scope.ctx();
+  std::vector<float> host_w;
+  std::vector<gtnb_graph_view> views;
+  GTNB_TRY(gb.host_views(ctx, &host_w, &views));
+  const std::vector<int32_t> ids = arc_ids(views);
+  gtnb_graph_view G = Gv;
+  G.weights = W;
+  return eps_viterbi_exact(scope, gb, v, which, /*arc_in=*/true,
+                           [&](int b, const gtnb_graph_view& E, ComposedHost* c) {
+                             if (views[b].num_nodes == 0) return GTNB_OK; // (c->N = 0: no path)
+                             gtnb_graph_view a = views[b];
+                             a.arc_ilabel = ids.data();
+                             ComposedHost num;
+                             GTNB_TRY(compose_host(ctx, a, G, /*unsorted=*/0, &num));
+                             if (num.N == 0) return GTNB_OK;
+                             return compose_host(ctx, num.view(), E, /*second sorted=*/2, c);
+                           });
+}
+
+/*
+ * gtnb_backoff_transitions_viterbi for a G with epsilon arcs (t its tables).  The device route reuses the loss's
+ * numerators and their tables (backoff_products, backoff_numerators): their weights are gathered on the device, and
+ * sparse_eps_align_* sweep them one CTA each and trace the paths back to A_b's arcs.  viterbi_finish re-runs an
+ * utterance on backoff_align_exact on a non-finite value or a tie (exact_ties on); the whole batch takes that route
+ * outside the envelope or with the implicit flag off.  Only that route reads trans_w to the host.
+ */
+int backoff_align_run(CallScope& scope, const GraphViterbiArgs& a, const GraphBatch& gb, const gtnb_graph_view& Gv,
+                      const SparseTables& t, const std::vector<ProductGraph>& prods,
+                      const std::vector<SparseTables>& ptabs, bool fast, const float* trans_w, int trans_on_device) {
+  gtnb_ctx* ctx = scope.ctx();
+  const int B = gb.B, T = gb.T, C = gb.C;
+  const long long n_trans = Gv.num_arcs;
+  ViterbiBufs v;
+  GTNB_TRY(viterbi_open(scope, a, gb, &v));
+  const bool implicit = ctx->use_implicit && fast;
+  if (implicit) {
+    EpsDevTables num_t;
+    std::vector<int32_t> arc_of_h, tidx_h, a_first_h(B);
+    const long long rows = backoff_numerators(gb, prods, ptabs, &num_t, &arc_of_h, &tidx_h);
+    const long long tot_P = (long long)tidx_h.size();
+    for (int b = 0; b < B; b++) a_first_h[b] = (int32_t)gb.first_arc[b];
+    std::vector<float> w_A_h;
+    float *w_dev = nullptr, *fw = nullptr, *w_A = nullptr;
+    int32_t *T_dev = nullptr, *head = nullptr, *arc_of = nullptr, *tidx = nullptr, *a_first = nullptr;
+    uint16_t* bp = nullptr;
+    GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, std::max(n_trans, 1ll), &w_dev));
+    GTNB_TRY(scope.alloc(&T_dev, B));
+    GTNB_TRY(scope.alloc(&head, B));
+    GTNB_TRY(scope.alloc(&a_first, B));
+    GTNB_TRY(scope.alloc(&bp, std::max(rows, 1ll)));
+    GTNB_TRY(scope.alloc(&fw, std::max(tot_P, 1ll)));
+    GTNB_TRY(scope.alloc(&arc_of, std::max(tot_P, 1ll)));
+    GTNB_TRY(scope.alloc(&tidx, std::max(tot_P, 1ll)));
+    GTNB_TRY(num_t.alloc(scope));
+    if (host_arc_weights(gb, &w_A_h)) GTNB_TRY(scope.alloc(&w_A, (long long)w_A_h.size()));
+    GTNB_TRY(stage_begin(ctx));
+    GTNB_TRY(num_t.stage(scope));
+    GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
+    GTNB_TRY(stage_upload(ctx, a_first, a_first_h.data(), sizeof(int32_t) * B));
+    if (tot_P) {
+      GTNB_TRY(stage_upload(ctx, arc_of, arc_of_h.data(), sizeof(int32_t) * tot_P));
+      GTNB_TRY(stage_upload(ctx, tidx, tidx_h.data(), sizeof(int32_t) * tot_P));
+    }
+    if (!trans_on_device && n_trans) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
+    if (w_A) GTNB_TRY(stage_upload(ctx, w_A, w_A_h.data(), sizeof(float) * w_A_h.size()));
+    GTNB_TRY(stage_end(ctx));
+    GTNB_TRY(launch_sparse_eps_gather(ctx, tot_P, gb.arc_weights_dev ? gb.arc_weights_dev : w_A, arc_of, w_dev, tidx,
+                                      fw));
+    GTNB_TRY(launch_sparse_eps_align(ctx, num_t.dev, num_t.max_S, B, T, C, T_dev, v.e_dev, (long long)T * C, fw, bp,
+                                     head, v.s_dev, arc_of, a_first, v.p_dev, v.a_dev, v.status));
+  }
+  return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
+    std::vector<float> W(std::max(n_trans, 1ll));
+    if (n_trans) GTNB_TRY(read_to_host(ctx, W.data(), trans_w, trans_on_device, n_trans));
+    return backoff_align_exact(scope, gb, Gv, W.data(), v, which);
   });
 }
 
@@ -2839,4 +2957,31 @@ extern "C" int gtnb_viterbi_backoff(gtnb_ctx* ctx, int B, int T, int C, const fl
   const GraphViterbiArgs a{emissions, emissions_on_device, paths, arcs, scores, outputs_on_device};
   if (t.E == 0) return viterbi_sparse_run(scope, a, gb, *transitions, trans_w, trans_on_device);
   return backoff_viterbi_run(scope, a, gb, *transitions, t, trans_w, trans_on_device);
+}
+
+extern "C" int gtnb_backoff_transitions_viterbi(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const gtnb_graph_view* graphs, const float* arc_weights, int arc_weights_on_device,
+    const gtnb_graph_view* transitions, const float* trans_w, int trans_on_device, int32_t* paths, int32_t* arcs,
+    float* scores, int outputs_on_device) {
+  const std::string fn = "gtnb_backoff_transitions_viterbi";
+  GraphBatch gb;
+  SparseTables t;
+  GTNB_TRY(parse_graphs(ctx, fn.c_str(), B, T, C, emissions, graphs, transitions && (B == 0 || trans_w), input_lens,
+                        arc_weights, arc_weights_on_device, &gb,
+                        [&] { return check_backoff_graph(ctx, fn, *transitions, C, &t); }));
+  if (B == 0) return GTNB_OK;
+  if (t.E == 0)
+    return gtnb_sparse_transitions_viterbi(ctx, B, T, C, emissions, emissions_on_device, input_lens, graphs,
+                                           arc_weights, arc_weights_on_device, transitions, trans_w, trans_on_device,
+                                           paths, arcs, scores, outputs_on_device);
+  // the loss's numerators, whose shapes decide, with G's, whether the device route can be taken
+  std::vector<ProductGraph> prods;
+  std::vector<SparseTables> ptabs;
+  const bool fast = ctx->use_implicit && eps_fits(t, C) && backoff_products(gb, *transitions, t, C, &prods, &ptabs);
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  return backoff_align_run(scope, GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,
+                                                   outputs_on_device},
+                           gb, *transitions, t, prods, ptabs, fast, trans_w, trans_on_device);
 }

@@ -418,6 +418,13 @@ int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_ct
 int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, int S, int B, int T, int C, const int32_t* lens,
                               const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
                               float* score, int32_t* paths, int32_t* arcs, int32_t* status);
+// gtnb_backoff_transitions_viterbi over the numerators gs[b] (per CTA, max_S their largest S): the decode's sweep with
+// bp at gs[b].rows ((T_b + 1) * S_b per utterance), then the trace, which reports arcs[b][t] = arc_of[product arc] -
+// a_first[b] (A_b's own arc ids; a_first: [B] each utterance's first A arc in arc_of's numbering)
+int launch_sparse_eps_align(gtnb_ctx* ctx, const SparseEpsDev* gs, int max_S, int B, int T, int C,
+                            const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
+                            int32_t* head, float* score, const int32_t* arc_of, const int32_t* a_first,
+                            int32_t* paths, int32_t* arcs, int32_t* status);
 // out[k] = w_A[arc_of[k]] + W[tidx[k]], W[tidx[k]] alone where arc_of[k] < 0 (G's epsilon arcs in the numerators)
 int launch_sparse_eps_gather(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W,
                              const int32_t* tidx, float* out);

@@ -39,7 +39,9 @@
  * The backoff entry points (gtnb_backoff_transitions_loss, gtnb_viterbi_backoff) take a G with epsilon arcs, and
  * their numerators A_b o G have them too.  The sparse_eps_* kernels are the kernels above with an epsilon closure
  * after every frame's emitting update (one CTA barrier per topological level of the epsilon subgraph) and per-CTA
- * tables, so that one launch sweeps B different numerators; an epsilon-free G keeps the kernels above.
+ * tables, so that one launch sweeps B different numerators; an epsilon-free G keeps the kernels above.  The
+ * alignment gtnb_backoff_transitions_viterbi runs the decode's tropical sweep and trace over those per-CTA
+ * numerators (sparse_eps_align_*), reporting A_b's arcs.
  */
 #include <algorithm>
 
@@ -759,18 +761,21 @@ __device__ __forceinline__ void eps_close_trop(const SparseEpsDev& x, const floa
 }
 
 /*
- * sparse_viterbi_forward_kernel with the epsilon closure, G = gs[0] for every utterance.  bp[b][t][v] (t = 0 .. T_b,
- * T + 1 rows per utterance): the position of the arc that reaches S_t[v] in v's combined in-list (its emitting
- * in-arcs from frame t - 1, then its epsilon in-arcs from frame t), kBpStart for a start node at frame 0 that no
- * epsilon arc improves, | kBpTie on a tie; kBpNone where S_t[v] = -inf.
+ * sparse_viterbi_forward_kernel with the epsilon closure over graph x = gs[gi] for utterance b = blockIdx.x.  bpb[t][v]
+ * (t = 0 .. T_b; bpb = bp + rows_at(b, x), the utterance's back-pointers): the position of the arc that reaches S_t[v] in v's combined in-list
+ * (its emitting in-arcs from frame t - 1, then its epsilon in-arcs from frame t), kBpStart for a start node at frame 0
+ * that no epsilon arc improves, | kBpTie on a tie; kBpNone where S_t[v] = -inf.
  */
-__global__ void __launch_bounds__(kSparseThreads) sparse_eps_viterbi_kernel(
-    const SparseEpsDev* __restrict__ gs, int T, int C, const int32_t* __restrict__ lens,
-    const float* __restrict__ emis, long long stride, const float* __restrict__ w, uint16_t* __restrict__ bp,
-    int32_t* __restrict__ head, float* __restrict__ score, int32_t* __restrict__ status) {
+template <class Rows>
+__device__ __forceinline__ void eps_viterbi_sweep(const SparseEpsDev* __restrict__ gs, int gi, int C,
+                                                  const int32_t* __restrict__ lens,
+                                                  const float* __restrict__ emis, long long stride,
+                                                  const float* __restrict__ w, uint16_t* __restrict__ bp,
+                                                  Rows rows_at, int32_t* __restrict__ head,
+                                                  float* __restrict__ score, int32_t* __restrict__ status) {
   GTNB_DYNAMIC_SMEM(float, sm);
   const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
-  const SparseEpsDev x = gs[0];
+  const SparseEpsDev x = gs[gi];
   const SparseDev& g = x.g;
   const int S = g.S, lanes = g.lanes;
   float* rows = sm; // [2][S]
@@ -778,7 +783,7 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_viterbi_kernel(
   const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
   const int Tb = lens[b];
   const float* em = emis + (long long)b * stride;
-  uint16_t* bpb = bp + (long long)b * (T + 1) * S;
+  uint16_t* bpb = bp + rows_at(b, x);
   bool bad = false;
   for (int v = tid; v < S; v += nt) {
     const bool st = __ldg(g.flags + v) & 1;
@@ -837,19 +842,39 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_viterbi_kernel(
   }
 }
 
+/* the decode's sweep, G = gs[0] for every utterance; bp: [B][T + 1][S] */
+__global__ void __launch_bounds__(kSparseThreads) sparse_eps_viterbi_kernel(
+    const SparseEpsDev* __restrict__ gs, int T, int C, const int32_t* __restrict__ lens,
+    const float* __restrict__ emis, long long stride, const float* __restrict__ w, uint16_t* __restrict__ bp,
+    int32_t* __restrict__ head, float* __restrict__ score, int32_t* __restrict__ status) {
+  eps_viterbi_sweep(gs, 0, C, lens, emis, stride, w, bp,
+                    [&](int b, const SparseEpsDev& x) { return (long long)b * (T + 1) * x.g.S; }, head, score,
+                    status);
+}
+
+/* the alignment's sweep (gtnb_backoff_transitions_viterbi), every CTA its own numerator gs[b] = P_b: its
+ * back-pointers at bp + gs[b].rows, (T_b + 1) * S_b of them, the layout of the loss's score rows */
+__global__ void __launch_bounds__(kSparseThreads) sparse_eps_align_kernel(
+    const SparseEpsDev* __restrict__ gs, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis,
+    long long stride, const float* __restrict__ w, uint16_t* __restrict__ bp, int32_t* __restrict__ head,
+    float* __restrict__ score, int32_t* __restrict__ status) {
+  eps_viterbi_sweep(gs, blockIdx.x, C, lens, emis, stride, w, bp, [](int, const SparseEpsDev& x) { return x.rows; },
+                    head, score, status);
+}
+
 /*
- * The traceback of sparse_eps_viterbi_kernel, one warp per utterance: inside a frame it follows epsilon
- * back-pointers (they use no frame and are not reported), and an emitting one writes paths[b][t - 1] / arcs[b][t - 1]
- * and steps to frame t - 1; it ends at frame 0 on kBpStart.  -1 beyond T_b and in the whole row without a path.
- * status[b] |= 2 when a node of the path carries the tie flag.
+ * The traceback of eps_viterbi_sweep for utterance b over graph x, its back-pointers at bp + rows_at(S), by lane 0 of
+ * its warp (the other lanes only write the row's tail): inside a frame it follows epsilon back-pointers (they use no frame and are not reported), and an emitting
+ * one writes paths[b][t - 1] = its label / arcs[b][t - 1] = arc(its arc id) and steps to frame t - 1; it ends at
+ * frame 0 on kBpStart.  -1 beyond T_b and in the whole row without a path.  status[b] |= 2 when a node of the path
+ * carries the tie flag.
  */
-__global__ void __launch_bounds__(256) sparse_eps_trace_kernel(
-    const SparseEpsDev* __restrict__ gs, int B, int T, const int32_t* __restrict__ lens,
-    const uint16_t* __restrict__ bp, const int32_t* __restrict__ head, int32_t* __restrict__ paths,
-    int32_t* __restrict__ arcs, int32_t* __restrict__ status) {
-  const int b = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
-  if (b >= B) return; // whole warps
-  const SparseEpsDev x = gs[0];
+template <class Rows, class Arc>
+__device__ __forceinline__ void eps_trace(const SparseEpsDev& x, int b, int T, const int32_t* __restrict__ lens,
+                                          const uint16_t* __restrict__ bp, Rows rows_at,
+                                          const int32_t* __restrict__ head, int32_t* __restrict__ paths,
+                                          int32_t* __restrict__ arcs, int32_t* __restrict__ status, Arc arc) {
+  const int lane = threadIdx.x % 32;
   const int h = head[b];
   const int n = h < 0 ? 0 : lens[b];
   int32_t* pr = paths ? paths + (long long)b * T : nullptr;
@@ -860,7 +885,7 @@ __global__ void __launch_bounds__(256) sparse_eps_trace_kernel(
   }
   if (lane != 0 || n == 0) return;
   const int S = x.g.S;
-  const uint16_t* bpb = bp + (long long)b * (T + 1) * S;
+  const uint16_t* bpb = bp + rows_at(S);
   int v = h, tie = 0, t = n;
   for (;;) {
     const int e = __ldg(bpb + (long long)t * S + v);
@@ -875,11 +900,37 @@ __global__ void __launch_bounds__(256) sparse_eps_trace_kernel(
     }
     const int k = k0 + pos;
     if (pr) pr[t - 1] = __ldg(x.g.in_lab + k);
-    if (ar) ar[t - 1] = __ldg(x.g.in_arc + k);
+    if (ar) ar[t - 1] = arc(__ldg(x.g.in_arc + k));
     v = __ldg(x.g.in_src + k);
     t--;
   }
   if (tie) atomicOr(&status[b], 2);
+}
+
+/* the decode's traceback, one warp per utterance: G's arc ids */
+__global__ void __launch_bounds__(256) sparse_eps_trace_kernel(
+    const SparseEpsDev* __restrict__ gs, int B, int T, const int32_t* __restrict__ lens,
+    const uint16_t* __restrict__ bp, const int32_t* __restrict__ head, int32_t* __restrict__ paths,
+    int32_t* __restrict__ arcs, int32_t* __restrict__ status) {
+  const int b = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
+  if (b >= B) return; // whole warps
+  const SparseEpsDev x = gs[0];
+  eps_trace(x, b, T, lens, bp, [&](int S) { return (long long)b * (T + 1) * S; }, head, paths, arcs, status,
+            [](int a) { return a; });
+}
+
+/* the alignment's traceback, one warp per utterance over its numerator gs[b]: the product arc's A arc, arc_of (the
+ * loss's table, the batch's numbering) less a_first[b], utterance b's first A arc, so A_b's own numbering */
+__global__ void __launch_bounds__(256) sparse_eps_align_trace_kernel(
+    const SparseEpsDev* __restrict__ gs, int B, int T, const int32_t* __restrict__ lens,
+    const uint16_t* __restrict__ bp, const int32_t* __restrict__ head, const int32_t* __restrict__ arc_of,
+    const int32_t* __restrict__ a_first, int32_t* __restrict__ paths, int32_t* __restrict__ arcs,
+    int32_t* __restrict__ status) {
+  const int b = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
+  if (b >= B) return; // whole warps
+  const SparseEpsDev x = gs[b];
+  eps_trace(x, b, T, lens, bp, [&](int) { return x.rows; }, head, paths, arcs, status,
+            [&](int a) { return __ldg(arc_of + a) - __ldg(a_first + b); });
 }
 
 /* the numerators' weights, gathered: w[k] = fl(w_A[arc_of[k]] + W[tidx[k]]), W[tidx[k]] alone for an epsilon arc
@@ -1013,6 +1064,21 @@ int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, int S, int 
   GTNB_LAUNCH(ctx, "sparse_eps_trace", sparse_eps_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0,
                                                                  ctx->stream>>>(gs, B, T, lens, bp, head, paths, arcs,
                                                                                 status));
+  return GTNB_OK;
+}
+
+int launch_sparse_eps_align(gtnb_ctx* ctx, const SparseEpsDev* gs, int max_S, int B, int T, int C,
+                            const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
+                            int32_t* head, float* score, const int32_t* arc_of, const int32_t* a_first,
+                            int32_t* paths, int32_t* arcs, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_align_kernel)) return rc;
+  const size_t smem = sizeof(float) * sparse_vit_smem_floats(max_S, C);
+  GTNB_LAUNCH(ctx, "sparse_eps_align", sparse_eps_align_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
+      gs, C, lens, emis, stride, w, bp, head, score, status));
+  GTNB_LAUNCH(ctx, "sparse_eps_align_trace",
+              sparse_eps_align_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0, ctx->stream>>>(
+                  gs, B, T, lens, bp, head, arc_of, a_first, paths, arcs, status));
   return GTNB_OK;
 }
 

@@ -597,3 +597,19 @@ def sparse_transitions_viterbi(emissions, transitions, transitions_graph, graphs
     return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_sparse_transitions_viterbi(
         c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs,
         scores, 1))
+
+
+@torch.no_grad()
+def backoff_transitions_viterbi(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None):
+    """Best path of backoff_transitions_loss's numerator, intersect(intersect(A_b, G), E_b), for every utterance,
+    through gtnb_backoff_transitions_viterbi: the decomposition and frame-level alignment a model trained with
+    backoff_transitions_loss picks within its own target graph, under the backoff LM it was trained with.  The
+    arguments are backoff_transitions_loss's and the outputs sparse_transitions_viterbi's: arcs[b, t] is the arc of
+    graphs[b] taken at frame t, and an epsilon arc of G uses no frame and is not reported.  Ties are broken as the
+    reference breaks them.
+    """
+    c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=False)
+    gv, tw = _sparse_transitions(c, transitions, transitions_graph)
+    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_backoff_transitions_viterbi(
+        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs,
+        scores, 1))

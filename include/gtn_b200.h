@@ -837,6 +837,42 @@ int gtnb_viterbi_backoff(
     float* scores, /* [B] nullable: viterbiScore */
     int outputs_on_device);
 
+/*
+ * Batched Viterbi alignment over one user-supplied target graph per utterance with a backoff transition graph G:
+ * viterbiPath and viterbiScore of intersect(intersect(A_b, G), E_b), the numerator of gtnb_backoff_transitions_loss --
+ * the decomposition and frame-level alignment a model trained with that loss picks, under the LM it was trained with.
+ * paths[b][t] is the label of the emitting arc taken at frame t and arcs[b][t] that arc's id in A_b; an epsilon arc of
+ * G uses no frame and is not reported, at frame 0 and after frame T_b included.  Every other output rule is
+ * gtnb_sparse_transitions_viterbi's (-1 beyond T_b and for an utterance without an accepting path, score -inf, every
+ * entry written), and an epsilon-free G gives exactly its results.  Error rules for G are
+ * gtnb_backoff_transitions_loss's, all others gtnb_sparse_transitions_viterbi's.
+ * Device route: the loss's numerators A_b o G (built on the host from structure only, with G's epsilon arcs) are
+ * swept in the tropical semiring one CTA each, with the epsilon closure after every frame and bit-exact scores, and
+ * keep a 16-bit back-pointer per frame and node (2 * sum over b of (T_b + 1) * S_b bytes of scratch, S_b the
+ * numerator's nodes); the trace reports A_b's arcs.  Its envelope is gtnb_backoff_transitions_loss's, for every
+ * numerator.  An utterance with a tie on its traced path ("exact_ties" on) or a NaN or +inf is re-run on
+ * compose(compose(A_b, G), E_b) (gtnb_compose_graphs, gtnb_forward, gtnb_viterbi_path), as is the whole batch outside
+ * the envelope or with the "implicit" flag off; only that route reads trans_w to the host.
+ */
+int gtnb_backoff_transitions_viterbi(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const float* emissions,
+    int emissions_on_device,
+    const int32_t* input_lens, /* host, nullable */
+    const gtnb_graph_view* graphs,
+    const float* arc_weights, /* nullable */
+    int arc_weights_on_device,
+    const gtnb_graph_view* transitions, /* G: structure only, epsilon arcs allowed; its own weights ignored */
+    const float* trans_w, /* [G.num_arcs], G's arc numbering */
+    int trans_on_device,
+    int32_t* paths, /* [B][T] nullable: label of the emitting arc taken at frame t */
+    int32_t* arcs, /* [B][T] nullable: that frame's arc id in A_b (Graph arc numbering) */
+    float* scores, /* [B] nullable: viterbiScore */
+    int outputs_on_device);
+
 #ifdef __cplusplus
 }
 #endif
