@@ -305,6 +305,12 @@ int gtnb_ctx_set_flag(gtnb_ctx* ctx, const char* name, int value) {
     ctx->bidir_mode = value;
     return GTNB_OK;
   }
+  if (ctx && name && std::string(name) == "sparse_cluster") {
+    if (value != 0 && value != 1 && value != 2 && value != 4 && value != 8)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctx_set_flag: sparse_cluster is 0 (default), 1, 2, 4 or 8");
+    ctx->sparse_cluster = value;
+    return GTNB_OK;
+  }
   return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctx_set_flag: unknown flag");
 }
 

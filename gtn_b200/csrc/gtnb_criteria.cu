@@ -1695,6 +1695,20 @@ struct SparseDevTables {
   int stage(CallScope& scope) { return stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()); }
 };
 
+/*
+ * Which of k_sparse.cu's kernels sweep an epsilon-free G = t: true when some do, with sp->N = 1 for the one-CTA
+ * kernels and sp = the plan of a thread-block cluster otherwise.  The "sparse_cluster" flag decides: 0 the one-CTA
+ * kernels or nothing; 1 the cluster kernels for a G outside the one-CTA envelope; 2, 4, 8 a cluster of that size
+ * wherever it fits, the rule of 1 elsewhere.
+ */
+bool sparse_route(const gtnb_ctx* ctx, const SparseTables& t, int C, SparseSplit* sp) {
+  const int flag = ctx->sparse_cluster;
+  if (flag > 1 && sparse_cluster_plan(t, C, flag, sp)) return true;
+  sp->N = 1;
+  if (sparse_den_supported(t.S, t.A, C)) return true;
+  return flag != 0 && sparse_cluster_plan(t, C, 0, sp) != 0;
+}
+
 /* G's arcs with a label in [0, C), weighted from the host weights W; gmap (nullable) gets each one's arc id */
 void sparse_host_graph(const gtnb_graph_view& Gv, const SparseTables& t, int C, const float* W, HostGraph* G,
                        std::vector<int32_t>* gmap) {
@@ -1710,6 +1724,7 @@ void sparse_host_graph(const gtnb_graph_view& Gv, const SparseTables& t, int C, 
 struct SparseDenominator {
   const SparseTables& t;
   long long n_trans; // G's arcs, labels outside [0, C) included
+  SparseSplit split; // sparse_route's: N = 1 the one-CTA sweeps, else a cluster's
   SparseDevTables tabs;
   float* alpha = nullptr;
   double* offs = nullptr;
@@ -1727,10 +1742,15 @@ struct SparseDenominator {
   }
   int forward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
               float* den, int32_t* status) {
+    if (split.N > 1)
+      return launch_sparse_cl_den_forward(ctx, tabs.dev, split, B, T, C, lens, e, per, w, alpha, offs, den, status);
     return launch_sparse_den_forward(ctx, tabs.dev, B, T, C, lens, e, per, w, alpha, offs, den, status);
   }
   int backward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
                const float*, float* grad, float* wgrad) {
+    if (split.N > 1)
+      return launch_sparse_cl_den_backward(ctx, tabs.dev, split, B, T, C, lens, e, per, w, alpha, offs, grad, per,
+                                           wgrad);
     return launch_sparse_den_backward(ctx, tabs.dev, B, T, C, lens, e, per, w, alpha, offs, grad, per, wgrad);
   }
   int fold_grad(gtnb_ctx* ctx, int, const float* w, const float* sig, float* wgrad) {
@@ -1763,7 +1783,8 @@ int sparse_transitions_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const Gr
   const long long n_trans = Gv.num_arcs;
   // the device route's numerators (folded), whose shapes decide, with G's, whether it can be taken
   std::vector<ProductGraph> prods;
-  const bool fast = ctx->use_implicit && sparse_den_supported(t.S, t.A, C) &&
+  SparseSplit split{};
+  const bool fast = ctx->use_implicit && sparse_route(ctx, t, C, &split) &&
                     device_products(
                         gb,
                         [&](const gtnb_graph_view& v, ProductGraph* p) {
@@ -1782,7 +1803,7 @@ int sparse_transitions_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const Gr
                                  build_sparse_product(v, Gv, t, C, /*fold=*/false, p);
                                },
                                nullptr, arc_grads, arc_grads_on_device);
-                         SparseDenominator den{t, n_trans};
+                         SparseDenominator den{t, n_trans, split};
                          GraphNumerator num{gb, prods, (int)n_trans, arc_grads, arc_grads_on_device};
                          return trellis_loss_fast(scope, den, a, num, needs_exact);
                        });
@@ -2255,7 +2276,8 @@ int viterbi_sparse_run(CallScope& scope, const GraphViterbiArgs& a, const GraphB
   GTNB_TRY(viterbi_open(scope, a, gb, &v));
   SparseTables t;
   sparse_tables(Gv, C, &t);
-  const bool implicit = ctx->use_implicit && sparse_den_supported(t.S, t.A, C);
+  SparseSplit split{};
+  const bool implicit = ctx->use_implicit && sparse_route(ctx, t, C, &split);
   if (implicit) {
     SparseDevTables tabs;
     GTNB_TRY(tabs.alloc(scope, t));
@@ -2271,8 +2293,12 @@ int viterbi_sparse_run(CallScope& scope, const GraphViterbiArgs& a, const GraphB
     GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
     if (!trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
     GTNB_TRY(stage_end(ctx));
-    GTNB_TRY(launch_sparse_viterbi(ctx, tabs.dev, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head, v.s_dev,
-                                   v.p_dev, v.a_dev, v.status));
+    if (split.N > 1)
+      GTNB_TRY(launch_sparse_cl_viterbi(ctx, tabs.dev, split, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp,
+                                        head, v.s_dev, v.p_dev, v.a_dev, v.status));
+    else
+      GTNB_TRY(launch_sparse_viterbi(ctx, tabs.dev, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head,
+                                     v.s_dev, v.p_dev, v.a_dev, v.status));
   }
   return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
     std::vector<float> W(std::max(n_trans, 1ll));
@@ -2324,7 +2350,8 @@ extern "C" int gtnb_sparse_transitions_viterbi(
   sparse_tables(Gv, C, &t);
   // the loss's numerators (folded), whose shapes decide, with G's, whether the device route can be taken
   std::vector<ProductGraph> prods;
-  const bool fast = ctx->use_implicit && sparse_den_supported(t.S, t.A, C) &&
+  SparseSplit split{}; // (the alignment sweeps the products alone: only whether G has a device route matters)
+  const bool fast = ctx->use_implicit && sparse_route(ctx, t, C, &split) &&
                     device_products(
                         gb,
                         [&](const gtnb_graph_view& v, ProductGraph* p) {

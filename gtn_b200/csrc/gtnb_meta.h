@@ -36,6 +36,39 @@ inline int sparse_den_lanes(int S, int A) {
   return lanes;
 }
 
+/* the CTA of k_sparse.cu's sweeps */
+constexpr int kSparseThreads = 512;
+constexpr int kSparseWarps = kSparseThreads / 32;
+
+/*
+ * A G too large for one CTA is swept by a thread-block cluster of N CTAs per utterance (k_sparse.cu's sparse_cl_*
+ * kernels): rank r computes the nodes [in[r], in[r + 1]) of the forward and the tropical sweep and the nodes
+ * [out[r], out[r + 1]) of the backward sweep (sparse_cluster_splits, gtnb_product.h: contiguous ranges with balanced
+ * arc counts).  Every CTA keeps the whole [2][S] score rows; the backward's arc-gradient accumulator holds the rank's
+ * own out-arcs only, which is what lifts the arc limit.
+ */
+constexpr int kSparseClusterMax = 8; // CTAs per cluster: the portable maximum
+struct SparseSplit {
+  int N; // 2, 4 or 8
+  int own_out; // the most out-arcs a rank owns: the backward's accumulators
+  int32_t in[kSparseClusterMax + 1], out[kSparseClusterMax + 1];
+};
+/* the cluster kernels' bounds on G; inside them sparse_cluster_plan (gtnb_product.h) decides from the shared memory
+ * the actual splits need (the full trigram at C = 64, 4096 nodes / 262 144 arcs, takes N = 8: 162 KB) */
+constexpr int kSparseClusterMaxStates = 16384;
+constexpr int kSparseClusterMaxArcs = 262144;
+constexpr long long kSparseClusterSmemBytes = 227 * 1024; // a CTA's opt-in dynamic shared memory on sm_90
+/* kBpNone = 0xFFFF must not be a position | tie flag: the last position of an in-list is at most 0x7FFD */
+constexpr int kSparseClusterMaxInDegree = 32766;
+/* floats of dynamic shared memory of the cluster sweeps: rows [2][S], emission rows [2][C], the per-warp row maxima
+ * of every rank [2][N * kSparseWarps]; the backward adds the emission gradient [2][C] and own_arcs accumulators */
+inline long long sparse_cl_fwd_smem_floats(int S, int C, int N) {
+  return 2ll * S + 2ll * C + 2ll * N * kSparseWarps;
+}
+inline long long sparse_cl_bwd_smem_floats(int S, int C, int N, int own_arcs) {
+  return 2ll * S + 4ll * C + own_arcs + 2ll * N * kSparseWarps;
+}
+
 /*
  * An acceptor with epsilon arcs as k_sparse.cu's backoff sweeps read it (gtnb_product.h's SparseTables with its
  * epsilon tables): g holds the emitting arcs, then come the E epsilon arcs (by destination and by source; *_arc

@@ -220,6 +220,44 @@ inline void sparse_tables(const gtnb_graph_view& G, int C, SparseTables* t) {
   }
 }
 
+/* N contiguous node ranges with balanced arc counts from a CSR pointer array ptr[S + 1]: rank r gets the nodes
+ * [split[r], split[r + 1]), split[r] the first node at or after arc r * A / N, so that no rank holds more than
+ * A / N + the largest degree arcs.  A rank may own no node (a hub's list spans several shares). */
+inline void sparse_cluster_splits(const std::vector<int32_t>& ptr, int N, int32_t* split) {
+  const int S = (int)ptr.size() - 1;
+  const long long A = ptr[S];
+  split[0] = 0;
+  for (int r = 1; r < N; r++)
+    split[r] = (int32_t)(std::lower_bound(ptr.begin(), ptr.begin() + S, (int32_t)((A * r + N - 1) / N)) - ptr.begin());
+  split[N] = S;
+}
+
+/*
+ * The cluster size of k_sparse.cu's sparse_cl_* kernels for G = t: the smallest N in {2, 4, 8} (or `force` alone when
+ * it is not 0) whose forward and backward sweeps fit the 227 KB of shared memory a CTA can opt in to, with the splits
+ * that N gets; 0 when none does or G is outside the kernels' bounds (gtnb_meta.h: S <= 16384 nodes, A <= 262 144
+ * arcs, in-degree <= 32 766, C <= 1024).  With C = 64 that is e.g. S = 4096 up to the whole 262 144 arcs (N = 8), or
+ * S = 16 384 with 131 072 arcs (N = 8, 194 KB).  *sp gets N and the splits.
+ */
+inline int sparse_cluster_plan(const SparseTables& t, int C, int force, SparseSplit* sp) {
+  if (t.S < 1 || t.S > kSparseClusterMaxStates || t.A > kSparseClusterMaxArcs || C < 1 || C > kSparseMaxLabels ||
+      t.max_in > kSparseClusterMaxInDegree)
+    return 0;
+  for (int N = 2; N <= kSparseClusterMax; N *= 2) {
+    if (force && N != force) continue;
+    sp->N = N;
+    sparse_cluster_splits(t.in_ptr, N, sp->in);
+    sparse_cluster_splits(t.out_ptr, N, sp->out);
+    sp->own_out = 0;
+    for (int r = 0; r < N; r++)
+      sp->own_out = std::max(sp->own_out, t.out_ptr[sp->out[r + 1]] - t.out_ptr[sp->out[r]]);
+    const long long floats =
+        std::max(sparse_cl_fwd_smem_floats(t.S, C, N), sparse_cl_bwd_smem_floats(t.S, C, N, sp->own_out));
+    if (floats * (long long)sizeof(float) <= kSparseClusterSmemBytes) return N;
+  }
+  return 0;
+}
+
 /*
  * The epsilon arcs of G (olabel GTNB_EPSILON; the backoff entry points: ilabel too) into t, after sparse_tables.  An
  * epsilon arc moves G without consuming a frame, so a frame's scores are closed over them in topological order.

@@ -5,7 +5,8 @@
  * `#ifdef GTNB_HOST_EMU`: this header is the one place where the emulated build swaps code.
  *
  * It also does the include switch of the kernel files: under GTNB_HOST_EMU (g++, CPU test suite) the SIMT
- * emulator tests/emu/simt_emu.h and the plain-data headers, otherwise the CUDA runtime and gtnb_internal.h.
+ * emulator tests/emu/simt_emu.h (with simt_emu_dsmem.h, its distributed shared memory) and the plain-data headers,
+ * otherwise the CUDA runtime and gtnb_internal.h.
  */
 #pragma once
 
@@ -13,6 +14,7 @@
 #include "gtn_b200.h"
 #include "gtnb_meta.h"
 #include "simt_emu.h"
+#include "simt_emu_dsmem.h"
 #else
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -188,6 +190,9 @@ __device__ __forceinline__ void cluster_wait_only() {
 }
 __device__ __forceinline__ unsigned cluster_rank() {
   return emu::cluster_ctarank();
+}
+__device__ __forceinline__ void sts_cluster_f32(uint32_t addr, unsigned rank, float v) {
+  *emu::cluster_shared_ptr<float>(addr, rank) = v;
 }
 
 __device__ __forceinline__ unsigned lanemask_lt() {
@@ -446,6 +451,19 @@ __device__ __forceinline__ unsigned cluster_rank() {
   unsigned r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
+}
+/* a store into the distributed shared memory of the cluster: addr is a shared-window address of this CTA, and the
+ * float goes to the same offset in the CTA of rank `rank` (this CTA's own rank included).  Ordered before the
+ * peer's reads by the next barrier.cluster arrive.release / wait.acquire pair. */
+__device__ __forceinline__ void sts_cluster_f32(uint32_t addr, unsigned rank, float v) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 ra;\n"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n"
+      "st.shared::cluster.f32 [ra], %2;\n"
+      "}\n" ::"r"(addr),
+      "r"(rank), "f"(v)
+      : "memory");
 }
 
 /* ---- special registers ---- */

@@ -30,6 +30,10 @@
  * Valid only for finite weights: the forward kernel raises status bit 1 on any non-finite weight or used emission,
  * and the caller repeats the call on the materialised route.
  *
+ * A G beyond that CTA's shared memory (S > 4096 or A > 32768) is swept by one thread-block cluster per utterance
+ * (the sparse_cl_* kernels below, behind the "sparse_cluster" context flag): the rows whole in every CTA, the nodes
+ * and the arc accumulators split over the ranks, results exchanged through distributed shared memory.
+ *
  * The decoder gtnb_viterbi_sparse sweeps the same tables in the tropical semiring (sparse_viterbi_forward_kernel):
  * S_t[v] = max over in-arcs a: u -> v of fl(S_{t-1}[u] + fl(w_a + e[t-1][label_a])), the reference's association
  * (compose.cpp:435, then shortest.cpp:213), with absolute scores so that the score is bit-exact.  Per (frame, node) it
@@ -48,9 +52,6 @@
 #include "gtnb_ptx.h"
 
 namespace gtnb {
-
-constexpr int kSparseThreads = 512;
-constexpr int kSparseWarps = kSparseThreads / 32;
 
 /* floats of dynamic shared memory of the two sweeps */
 inline int sparse_fwd_smem_floats(int S, int C) {
@@ -465,6 +466,285 @@ __global__ void __launch_bounds__(256) sparse_tau_kernel(int K, const int32_t* _
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
   if (lane == 0) tau[k] = m;
+}
+
+/*
+ * The cluster sweeps: the three sweeps above for a G that one CTA's shared memory cannot hold, one thread-block
+ * cluster of N = sp.N CTAs per utterance (b = blockIdx.x / N).  Every CTA keeps the whole [2][S] rows; rank r
+ * computes the new row for its own nodes only (sp.in for the forward and the tropical sweep, sp.out for the backward),
+ * with the `lanes` threads, arc order and merges of the one-CTA kernels, and stores each result into the row of every
+ * CTA of the cluster through distributed shared memory.  The per-warp row maxima go the same way ([2][N *
+ * kSparseWarps]; a maximum does not depend on how the row is cut), so rows, offsets, Z, scores and back-pointers are
+ * bit-identical to the one-CTA kernels'.  One barrier.cluster per frame replaces the CTA barrier: after it the frame's
+ * row is complete in every CTA and nobody reads the row before it any more, which is the row the next frame
+ * overwrites.  The backward keeps accumulators for its own out-arcs only (about A / N) and its own emission-gradient
+ * rows, so only the order of the adds into grad and wgrad differs.  Global outputs are written by a node's owner, the
+ * per-utterance ones by rank 0.
+ */
+
+/* v into the float at p of every CTA of the cluster, this one included */
+__device__ __forceinline__ void cluster_store(float* p, int N, float v) {
+  const uint32_t a = smem_u32(p);
+  for (int r = 0; r < N; r++) sts_cluster_f32(a, r, v);
+}
+
+/* row_offset over the n per-warp maxima of every rank, by whole warps */
+__device__ __forceinline__ float cluster_row_offset(const float* red, int n) {
+  float M = neg_inf();
+  for (int i = threadIdx.x % 32; i < n; i += 32) M = fmaxf(M, red[i]);
+  M = warp_max(M);
+  return M == neg_inf() ? 0.0f : M;
+}
+
+/* a sweep's first row, R[v] = 0 where flags[v] has `bit` and -inf elsewhere: the same in every CTA, so each fills
+ * its own copy (also to out, nullable) and leaves the row's maximum in red[par] ([2][n], the rest -inf) */
+__device__ __forceinline__ void cluster_first_row(const SparseDev& g, int bit, float* R, float* out, float* red, int n,
+                                                  int par) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  float mx = neg_inf();
+  for (int v = tid; v < g.S; v += nt) {
+    const float a0 = (__ldg(g.flags + v) & bit) ? 0.0f : neg_inf();
+    R[v] = a0;
+    if (out) out[v] = a0;
+    mx = fmaxf(mx, a0);
+  }
+  for (int i = tid; i < 2 * n; i += nt) red[i] = neg_inf();
+  __syncthreads();
+  mx = warp_max(mx);
+  if (tid % 32 == 0) red[par * n + tid / 32] = mx;
+}
+
+/* sparse_den_forward_kernel by a cluster: the same outputs */
+__global__ void __launch_bounds__(kSparseThreads) sparse_cl_den_forward_kernel(
+    SparseDev g, SparseSplit sp, int T, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis,
+    long long stride, const float* __restrict__ w, float* __restrict__ alpha, double* __restrict__ offs,
+    float* __restrict__ den, int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int S = g.S, lanes = g.lanes, N = sp.N, nred = N * kSparseWarps;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  float* red = E + 2 * C; // [2][nred]
+  const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
+  const int n0 = sp.in[rank], n1 = sp.in[rank + 1]; // this CTA's nodes
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  float* al = alpha + (long long)b * (T + 1) * S;
+  double* of = offs + (long long)b * (T + 1);
+  bool bad = false;
+  cluster_first_row(g, 1, rows, rank == 0 ? al : nullptr, red, nred, 0);
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  cluster_sync_all(); // every CTA's first row is in place before a peer stores into its shared memory
+  double c_off = 0.0;
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    const float Mp = cluster_row_offset(red + ((t - 1) & 1) * nred, nred);
+    float mx = neg_inf();
+    for (int v0 = n0; v0 < n1; v0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int v = v0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (v < n1) {
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int k = __ldg(g.in_ptr + v) + q; k < k1; k += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + k));
+          const float ek = Er[__ldg(g.in_lab + k)];
+          bad |= !(is_finite(wk) && is_finite(ek));
+          lse_add(m, s, P[__ldg(g.in_src + k)] + (wk + ek));
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (v < n1) {
+        const float val = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mp;
+        if (q == 0) {
+          cluster_store(Q + v, N, val);
+          al[(long long)t * S + v] = val;
+        }
+        mx = fmaxf(mx, val);
+      }
+    }
+    mx = warp_max(mx);
+    if (tid % 32 == 0) cluster_store(red + (t & 1) * nred + rank * kSparseWarps + tid / 32, N, mx);
+    cluster_arrive_only();
+    c_off += (double)Mp;
+    if (rank == 0 && tid == 0) of[t] = c_off;
+    cluster_wait_only();
+  }
+  bad = __syncthreads_or(bad);
+  if (bad && tid == 0) atomicOr(&status[b], 1);
+  if (rank == 0 && tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    for (int v = tid; v < S; v += 32)
+      if (__ldg(g.flags + v) & 2) m = fmaxf(m, F[v]);
+    m = warp_max(m);
+    float s = 0.0f;
+    if (m != neg_inf())
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) s += expf(F[v] - m);
+    s = warp_sum(s);
+    if (tid == 0) {
+      const double Z = m == neg_inf() ? (double)neg_inf() : c_off + (double)(m + logf(s));
+      of[0] = Z;
+      den[b] = (float)Z;
+    }
+  }
+}
+
+/* sparse_den_backward_kernel by a cluster: rank r adds the posteriors of its own nodes' out-arcs */
+__global__ void __launch_bounds__(kSparseThreads) sparse_cl_den_backward_kernel(
+    SparseDev g, SparseSplit sp, int T, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis,
+    long long stride, const float* __restrict__ w, const float* __restrict__ alpha, const double* __restrict__ offs,
+    float* __restrict__ grad, long long grad_stride, float* __restrict__ wgrad) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int S = g.S, lanes = g.lanes, N = sp.N, nred = N * kSparseWarps;
+  float* rows = sm; // [2][S] beta rows
+  float* E = sm + 2 * S; // [2][C] emission rows
+  float* Eg = E + 2 * C; // [2][C] the frame's emission gradient, this CTA's share
+  float* red = Eg + 2 * C; // [2][nred]
+  float* acc = red + 2 * nred; // [own out-arcs] arc gradient, by out-table position - ka
+  const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
+  const int n0 = sp.out[rank], n1 = sp.out[rank + 1]; // this CTA's nodes
+  const int ka = __ldg(g.out_ptr + n0), kn = __ldg(g.out_ptr + n1) - ka; // and their out-arcs
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const double* of = offs + (long long)b * (T + 1);
+  const double Z = of[0];
+  if (Tb < 1 || !(fabs(Z) < (double)CUDART_INF_F)) return; // (the whole cluster)
+  const float* em = emis + (long long)b * stride;
+  const float* al = alpha + (long long)b * (T + 1) * S;
+  float* gr = grad + (long long)b * grad_stride;
+  cluster_first_row(g, 2, rows + (Tb & 1) * S, nullptr, red, nred, Tb & 1);
+  for (int k = tid; k < kn; k += nt) acc[k] = 0.0f;
+  for (int c = tid; c < 2 * C; c += nt) Eg[c] = 0.0f;
+  for (int c = tid; c < C; c += nt) E[((Tb - 1) & 1) * C + c] = __ldg(em + (long long)(Tb - 1) * C + c);
+  cluster_sync_all();
+  double d = 0.0; // d_{t+1}
+  for (int t = Tb - 1; t >= 0; t--) {
+    const float* Nx = rows + ((t + 1) & 1) * S;
+    float* Cur = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    float* Eg_t = Eg + (t & 1) * C;
+    float* Eg_prev = Eg + ((t + 1) & 1) * C; // frame t + 1's, complete since the barrier
+    for (int c = tid; c < C; c += nt) {
+      if (t > 0) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)(t - 1) * C + c);
+      if (t + 1 < Tb) {
+        const float v = Eg_prev[c];
+        if (v != 0.0f) atomicAdd(gr + (long long)(t + 1) * C + c, v);
+        Eg_prev[c] = 0.0f;
+      }
+    }
+    const float Mb = cluster_row_offset(red + ((t + 1) & 1) * nred, nred);
+    const double c_t = t > 0 ? of[t] : 0.0;
+    const float fo = (float)(c_t + d - Z);
+    float mx = neg_inf();
+    for (int u0 = n0; u0 < n1; u0 += groups) {
+      const int u = u0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (u < n1) {
+        const float au = al[(long long)t * S + u] + fo; // alpha_t[u] + c_t + d_{t+1} - Z, in the exponent's terms
+        const int k1 = __ldg(g.out_ptr + u + 1);
+        for (int k = __ldg(g.out_ptr + u) + q; k < k1; k += lanes) {
+          const int lab = __ldg(g.out_lab + k);
+          const float x = Nx[__ldg(g.out_dst + k)] + (__ldg(w + __ldg(g.out_arc + k)) + Er[lab]);
+          lse_add(m, s, x);
+          const float p = exp_fast(au + x);
+          if (p != 0.0f) {
+            acc[k - ka] += p;
+            atomicAdd(Eg_t + lab, p);
+          }
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (u < n1) {
+        const float val = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mb;
+        if (q == 0) cluster_store(Cur + u, N, val);
+        mx = fmaxf(mx, val);
+      }
+    }
+    mx = warp_max(mx);
+    if (tid % 32 == 0) cluster_store(red + (t & 1) * nred + rank * kSparseWarps + tid / 32, N, mx);
+    cluster_arrive_only();
+    d += (double)Mb;
+    cluster_wait_only();
+  }
+  for (int c = tid; c < C; c += nt) { // frame 0's emission gradient
+    const float v = Eg[c];
+    if (v != 0.0f) atomicAdd(gr + c, v);
+  }
+  for (int k = tid; k < kn; k += nt)
+    if (acc[k] != 0.0f) atomicAdd(wgrad + __ldg(g.out_arc + ka + k), acc[k]);
+}
+
+/* sparse_viterbi_forward_kernel by a cluster: the same back-pointers, head, score and status */
+__global__ void __launch_bounds__(kSparseThreads) sparse_cl_viterbi_forward_kernel(
+    SparseDev g, SparseSplit sp, int T, int C, const int32_t* __restrict__ lens, const float* __restrict__ emis,
+    long long stride, const float* __restrict__ w, uint16_t* __restrict__ bp, int32_t* __restrict__ head,
+    float* __restrict__ score, int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const int S = g.S, lanes = g.lanes, N = sp.N;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
+  const int n0 = sp.in[rank], n1 = sp.in[rank + 1]; // this CTA's nodes
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  uint16_t* bpb = bp + (long long)b * T * S;
+  bool bad = false;
+  for (int v = tid; v < S; v += nt) rows[v] = (__ldg(g.flags + v) & 1) ? 0.0f : neg_inf();
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  cluster_sync_all();
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    uint16_t* bpt = bpb + (long long)(t - 1) * S;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    for (int v0 = n0; v0 < n1; v0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int v = v0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, k0 = 0;
+      if (v < n1) {
+        k0 = __ldg(g.in_ptr + v);
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + j));
+          const float ek = Er[__ldg(g.in_lab + j)];
+          bad |= !(wk < CUDART_INF_F && ek < CUDART_INF_F);
+          argmax_add(m, k, tie, P[__ldg(g.in_src + j)] + (wk + ek), j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (v < n1 && q == 0) {
+        cluster_store(Q + v, N, m);
+        bpt[v] = m == neg_inf() ? kBpNone : (uint16_t)((k - k0) | (tie ? kBpTie : 0));
+      }
+    }
+    cluster_sync_all();
+  }
+  bad = __syncthreads_or(bad);
+  if (bad && tid == 0) atomicOr(&status[b], 1);
+  if (rank == 0 && tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    int k = 0x7fffffff, tie = 0;
+    if (Tb > 0)
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) argmax_add(m, k, tie, F[v], v);
+    argmax_merge(m, k, tie, 32);
+    if (tid == 0) {
+      head[b] = m == neg_inf() ? -1 : k;
+      score[b] = m;
+      if (tie) atomicOr(&status[b], 2);
+    }
+  }
 }
 
 /*
@@ -1016,6 +1296,71 @@ int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C
   const size_t smem = sizeof(float) * sparse_vit_smem_floats(g.S, C);
   GTNB_LAUNCH(ctx, "sparse_viterbi_forward", sparse_viterbi_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
       g, T, C, lens, emis, stride, w, bp, head, score, status));
+  GTNB_LAUNCH(ctx, "sparse_viterbi_trace", sparse_viterbi_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256),
+                                                                         256, 0, ctx->stream>>>(
+      g, B, T, lens, bp, head, paths, arcs, status));
+  return GTNB_OK;
+}
+
+namespace {
+
+/* B clusters of N CTAs of kSparseThreads threads; attr: the caller's, alive until the launch */
+cudaLaunchConfig_t cluster_config(gtnb_ctx* ctx, int B, int N, size_t smem, cudaLaunchAttribute* attr) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(B * N), 1, 1);
+  cfg.blockDim = dim3(kSparseThreads, 1, 1);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = ctx->stream;
+  attr->id = cudaLaunchAttributeClusterDimension;
+  attr->val.clusterDim.x = (unsigned)N;
+  attr->val.clusterDim.y = 1;
+  attr->val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+} // namespace
+
+int launch_sparse_cl_den_forward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                                 const int32_t* lens, const float* emis, long long stride, const float* w,
+                                 float* alpha, double* offs, float* den, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_den_forward_kernel)) return rc;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg =
+      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_fwd_smem_floats(g.S, C, sp.N), &attr);
+  GTNB_LAUNCH(ctx, "sparse_cl_den_forward",
+              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_den_forward_kernel, g, sp, T, C, lens, emis, stride, w,
+                                                alpha, offs, den, status)));
+  return GTNB_OK;
+}
+
+int launch_sparse_cl_den_backward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                                  const int32_t* lens, const float* emis, long long stride, const float* w,
+                                  const float* alpha, const double* offs, float* grad, long long grad_stride,
+                                  float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_den_backward_kernel)) return rc;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg =
+      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_bwd_smem_floats(g.S, C, sp.N, sp.own_out), &attr);
+  GTNB_LAUNCH(ctx, "sparse_cl_den_backward",
+              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_den_backward_kernel, g, sp, T, C, lens, emis, stride,
+                                                w, alpha, (const double*)offs, grad, grad_stride, wgrad)));
+  return GTNB_OK;
+}
+
+int launch_sparse_cl_viterbi(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                             const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
+                             int32_t* head, float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_viterbi_forward_kernel)) return rc;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = cluster_config(ctx, B, sp.N, sizeof(float) * sparse_vit_smem_floats(g.S, C), &attr);
+  GTNB_LAUNCH(ctx, "sparse_cl_viterbi_forward",
+              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_viterbi_forward_kernel, g, sp, T, C, lens, emis,
+                                                stride, w, bp, head, score, status)));
   GTNB_LAUNCH(ctx, "sparse_viterbi_trace", sparse_viterbi_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256),
                                                                          256, 0, ctx->stream>>>(
       g, B, T, lens, bp, head, paths, arcs, status));

@@ -32,6 +32,19 @@ def _ctx_for(device, stream):
     return _ctx_cache[key]
 
 
+def _clustered(g, large_transitions, call):
+    """call() with the "sparse_cluster" flag of the cached context g at 1 when large_transitions: a transition graph
+    beyond one CTA's shared memory (over 4096 states or 32 768 arcs) then takes the thread-block-cluster kernels of
+    k_sparse.cu instead of the materialised route; the flag is restored after the call"""
+    if not large_transitions:
+        return call()
+    g.set_flag("sparse_cluster", 1)
+    try:
+        return call()
+    finally:
+        g.set_flag("sparse_cluster", 0)
+
+
 def _allreduce_transitions(ctx, tg, allreduce):
     """Sum the transition gradient tg over the ranks when torch.distributed is initialised (the multi-GPU form of
     Graph::addGrad under grad_lock, graph.cpp:96-100); ctx.world is the number of ranks summed over."""
@@ -454,26 +467,33 @@ class SparseTransitionsLossFunction(GraphTransitionsLossFunction):
     transitions_graph: G, a gtn_b200.gtn.Graph acceptor without epsilon arcs, whose own weights are ignored;
     transitions: float32 CUDA tensor of G.num_arcs() weights in G's arc numbering, on the emissions' device.  The
     graphs, weights, input_lengths, reduction and allreduce are graph_transitions_loss's; so is the backward.
+    large_transitions=True: a G of up to 16 384 states and 262 144 arcs (a full trigram at C = 64) keeps the device
+    route, swept by one thread-block cluster per utterance (_clustered); a smaller G is not affected.
     """
 
     @staticmethod
     def forward(ctx, emissions, transitions, weights, graphs, transitions_graph, input_lengths=None, reduction="mean",
-                allreduce=True):
+                allreduce=True, large_transitions=False):
         gv = _graph_view(transitions_graph)
         assert transitions.numel() == gv[0].num_arcs
         return _transitions_forward(
             ctx, emissions, transitions, weights, graphs, input_lengths, reduction, allreduce,
             max(transitions.numel(), 1),
-            lambda c, tw, losses, grad, tg: capi.lib().gtnb_sparse_transitions_loss(
-                c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1,
-                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if c.ag is None else c.ag.data_ptr(), 1,
-                tg.data_ptr(), 1))
+            lambda c, tw, losses, grad, tg: _clustered(
+                c.g, large_transitions, lambda: capi.lib().gtnb_sparse_transitions_loss(
+                    c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1,
+                    losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
+                    None if c.ag is None else c.ag.data_ptr(), 1, tg.data_ptr(), 1)))
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return GraphTransitionsLossFunction.backward(ctx, grad_output) + (None,)
 
 
 def sparse_transitions_loss(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
-                            reduction="mean", allreduce=True):
+                            reduction="mean", allreduce=True, large_transitions=False):
     return SparseTransitionsLossFunction.apply(emissions, transitions, weights, graphs, transitions_graph,
-                                               input_lengths, reduction, allreduce)
+                                               input_lengths, reduction, allreduce, large_transitions)
 
 
 class BackoffTransitionsLossFunction(GraphTransitionsLossFunction):
@@ -554,7 +574,7 @@ def _sparse_transitions(c, transitions, transitions_graph):
 
 
 @torch.no_grad()
-def sparse_viterbi(emissions, transitions, transitions_graph, input_lengths=None):
+def sparse_viterbi(emissions, transitions, transitions_graph, input_lengths=None, large_transitions=False):
     """Best path of intersect(E_b, G) for every utterance, G the learned transition graph of sparse_transitions_loss
     (an n-gram graph of any order, a pruned token LM, an HMM topology), through gtnb_viterbi_sparse: the decode of a
     model trained with that loss.  emissions, transitions, transitions_graph and input_lengths as in
@@ -562,12 +582,13 @@ def sparse_viterbi(emissions, transitions, transitions_graph, input_lengths=None
     arcs [B, T] int32, the G arc taken at every frame, i.e. the state sequence), all -1 beyond T_b and where there is
     no accepting path (score -inf), as CUDA tensors on the emissions' device, written on the current stream; only
     input_lengths and one status word per utterance visit the host.  Ties are broken as the reference breaks them.
-    collapse(paths, blank) turns the paths into transcripts.
+    collapse(paths, blank) turns the paths into transcripts.  large_transitions as in sparse_transitions_loss.
     """
     c = _GraphCall(emissions, None, None, input_lengths, arc_grads=False)
     gv, tw = _sparse_transitions(c, transitions, transitions_graph)
-    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_viterbi_sparse(
-        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1))
+    return c.viterbi(lambda paths, arcs, scores: _clustered(
+        c.g, large_transitions, lambda: capi.lib().gtnb_viterbi_sparse(
+            c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1)))
 
 
 @torch.no_grad()
@@ -584,19 +605,22 @@ def backoff_viterbi(emissions, transitions, transitions_graph, input_lengths=Non
 
 
 @torch.no_grad()
-def sparse_transitions_viterbi(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None):
+def sparse_transitions_viterbi(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
+                               large_transitions=False):
     """Best path of sparse_transitions_loss's numerator, intersect(intersect(A_b, G), E_b), for every utterance,
     through gtnb_sparse_transitions_viterbi: the decomposition and frame-level alignment a model trained with
     sparse_transitions_loss picks within its own target graph.  The arguments are sparse_transitions_loss's.  Returns
     (paths [B, T] int32, the label of the arc taken at every frame; scores [B] float32, viterbiScore; arcs [B, T]
     int32, that arc's id in graphs[b]), all -1 beyond T_b and where there is no accepting path (score -inf), as CUDA
     tensors on the emissions' device, written on the current stream.  Ties are broken as the reference breaks them.
+    large_transitions as in sparse_transitions_loss.
     """
     c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=False)
     gv, tw = _sparse_transitions(c, transitions, transitions_graph)
-    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_sparse_transitions_viterbi(
-        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs,
-        scores, 1))
+    return c.viterbi(lambda paths, arcs, scores: _clustered(
+        c.g, large_transitions, lambda: capi.lib().gtnb_sparse_transitions_viterbi(
+            c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths,
+            arcs, scores, 1)))
 
 
 @torch.no_grad()

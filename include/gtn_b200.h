@@ -109,6 +109,14 @@ int64_t gtnb_ctx_launch_count(const gtnb_ctx* ctx);
  * C = 64 / 128: -1 or 1 the PAIR kernels (a label and a blank node per thread), 0 one node per
  * thread; any other value is rejected.  "exact_ties" (default 0, EXPERIMENTAL; set before gtnb_compose_linear): gtnb_viterbi_path
  * on a composed lattice breaks exact score ties like the reference's shortestPath (k_order.cu).
+ * "sparse_cluster" (default 0): the route of gtnb_sparse_transitions_loss, gtnb_viterbi_sparse and
+ * gtnb_sparse_transitions_viterbi for a transition graph G beyond one CTA's shared memory (over 4096 nodes or 32768
+ * arcs).  0: the materialised route.  1: G is swept by one thread-block cluster of 2, 4 or 8 CTAs per utterance
+ * (k_sparse.cu's sparse_cl_* kernels) when it has at most 16384 nodes, 262144 arcs labelled in [0, C), in-degree
+ * 32766, C <= 1024, and the cluster's shared memory holds it (the score rows in every CTA, an arc-gradient
+ * accumulator split over the CTAs: e.g. 4096 nodes with 262144 arcs, or 16384 nodes with 131072 arcs); a smaller G
+ * keeps the one-CTA kernels.  2, 4, 8 (testing and measurement): additionally every G that fits a cluster of that
+ * size takes it; results are bit-identical apart from the order of the gradient sums.  Other values are rejected.
  */
 int gtnb_ctx_set_flag(gtnb_ctx* ctx, const char* name, int value);
 
@@ -588,6 +596,10 @@ int gtnb_graph_transitions_loss(
  * C <= 1024 -- and the numerators are the products of gtnb_product.h, built on the host from structure only, with
  * G's start copies folded into one start node, weighted on the device and swept by the implicit kernels.  A G or a
  * product outside that layout, a non-finite value, or the "implicit" flag off take the materialised lattices.
+ * With the "sparse_cluster" flag at 1 a larger G (gtnb_ctx_set_flag: up to 16384 nodes / 262144 arcs, the full trigram
+ * at C = 64) stays on the device route, swept by a thread-block cluster per utterance; its scratch grows with G's
+ * node count S: 4 * B * (T + 1) * S bytes of score rows (1 GB at B = 128, T = 500, S = 4096), and a failed
+ * allocation is GTNB_ERR_RUNTIME as on every route.
  */
 int gtnb_sparse_transitions_loss(
     gtnb_ctx* ctx,
@@ -711,7 +723,9 @@ int gtnb_graph_transitions_viterbi(
  * envelope or with the "implicit" flag off; only that route reads trans_w to the host, and it runs the utterances in
  * groups that fit the device memory.  With "exact_ties" off a tie keeps the device route's path, one of the optimal
  * paths.  The call reads back one status word per utterance, so it returns only once every output is complete,
- * device ones too.
+ * device ones too.  With the "sparse_cluster" flag at 1 a larger G (gtnb_ctx_set_flag: up to 16384 nodes / 262144
+ * arcs) keeps the device route, swept by a thread-block cluster per utterance with the same back-pointers (0.5 GB of
+ * them at B = 128, T = 500, S = 4096) and the same retry rules.
  * Epsilon arcs or a transducer G, and a lattice too large to materialise for one utterance on the exact route, are
  * GTNB_ERR_UNSUPPORTED; a malformed view, a G without nodes, a NULL trans_w with B > 0 and input_lens outside [0, T]
  * are GTNB_ERR_INVALID_ARGUMENT.  B = 0 is a no-op.
@@ -741,7 +755,8 @@ int gtnb_viterbi_sparse(
  * (arcs: A_b's arc ids).  The device route sweeps the loss's folded products in the tropical semiring, G's start
  * copies folded into one start node whose arcs weigh tau_k = max over a group of G's start arcs, with trans_w on the
  * device; the exact route composes A_b with G in the reference's numbering (gtnb_compose_graphs).  The device route
- * is taken when G fits gtnb_viterbi_sparse's envelope and every product the implicit sweeps' layout.
+ * is taken when G fits gtnb_viterbi_sparse's envelope ("sparse_cluster" at 1: its cluster envelope) and every product
+ * the implicit sweeps' layout.
  * Epsilon arcs in A_b or G, a transducer G and a pair too large for the exact route are GTNB_ERR_UNSUPPORTED;
  * malformed views, a G without nodes, a NULL trans_w with B > 0 and bad lengths are GTNB_ERR_INVALID_ARGUMENT.
  * B = 0 is a no-op.
