@@ -2444,6 +2444,21 @@ struct EpsDevTables {
 
 bool eps_fits(const SparseTables& t, int C) { return sparse_eps_supported(t.S, t.A, t.E, t.L, t.max_in_all, C); }
 
+/*
+ * sparse_route for a G with epsilon arcs (t with its epsilon tables): true when k_sparse.cu has kernels for its
+ * denominator, with sp->N = 1 for the one-CTA sparse_eps_* kernels and sp = the plan of a thread-block cluster (the
+ * sparse_cl_eps_* kernels) otherwise.  The "sparse_cluster" flag decides as there: 0 the one-CTA kernels or nothing;
+ * 1 a cluster for a G outside the one-CTA envelope; 2, 4, 8 a cluster of that size wherever it fits, the rule of 1
+ * elsewhere.  The numerators keep the one-CTA kernels and their envelope (backoff_products).
+ */
+bool backoff_route(const gtnb_ctx* ctx, const SparseTables& t, int C, SparseSplit* sp) {
+  const int flag = ctx->sparse_cluster;
+  if (flag > 1 && sparse_cluster_plan(t, C, flag, sp)) return true;
+  sp->N = 1;
+  if (eps_fits(t, C)) return true;
+  return flag != 0 && sparse_cluster_plan(t, C, 0, sp) != 0;
+}
+
 /* the checks of the backoff entry points' G, and its tables (with the epsilon tables) into t: a cycle of epsilon arcs
  * has no finite closure (the reference's forwardScore and viterbi throw "Graph has a cycle", shortest.cpp:150, 230) */
 int check_backoff_graph(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& Gv, int C, SparseTables* t) {
@@ -2501,9 +2516,10 @@ bool host_arc_weights(const GraphBatch& gb, std::vector<float>* w_A) {
   return true;
 }
 
-/* the device route of gtnb_backoff_transitions_loss: ptabs[b] the tables of prods[b] (P_b = A_b o G, unfolded) */
+/* the device route of gtnb_backoff_transitions_loss: ptabs[b] the tables of prods[b] (P_b = A_b o G, unfolded);
+ * split: backoff_route's, a cluster's plan for the denominator when split.N > 1 */
 int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatch& gb, long long n_trans,
-                      const SparseTables& t, const std::vector<ProductGraph>& prods,
+                      const SparseTables& t, const SparseSplit& split, const std::vector<ProductGraph>& prods,
                       const std::vector<SparseTables>& ptabs, float* arc_grads, int arc_grads_on_device,
                       bool* needs_exact) {
   gtnb_ctx* ctx = scope.ctx();
@@ -2516,10 +2532,12 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
   const long long rows = backoff_numerators(gb, prods, ptabs, &num_t, &arc_of_h, &tidx_h);
   const long long tot_P = (long long)tidx_h.size();
   std::vector<float> w_A_h;
+  std::vector<int32_t> cut_h;
+  if (split.N > 1) sparse_eps_cluster_cuts(t, split, &cut_h);
   float *e_dev = nullptr, *w_dev = nullptr, *den = nullptr, *num = nullptr, *alpha_d = nullptr, *alpha_n = nullptr;
   float *fw = nullptr, *w_A = nullptr, *pgrad = nullptr;
   double *offs_d = nullptr, *offs_n = nullptr;
-  int32_t *status = nullptr, *T_dev = nullptr, *arc_of = nullptr, *tidx = nullptr;
+  int32_t *status = nullptr, *T_dev = nullptr, *arc_of = nullptr, *tidx = nullptr, *cut = nullptr;
   OutBuf g, tg, ag;
   GTNB_TRY(ensure_side_streams(ctx, 0, 0));
   GTNB_TRY(scope.input(a.emissions, a.emissions_on_device, per * B, &e_dev));
@@ -2537,6 +2555,7 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
   GTNB_TRY(scope.alloc(&tidx, tot_P));
   GTNB_TRY(den_t.alloc(scope));
   GTNB_TRY(num_t.alloc(scope));
+  if (!cut_h.empty()) GTNB_TRY(scope.alloc(&cut, (long long)cut_h.size()));
   if (host_arc_weights(gb, &w_A_h)) GTNB_TRY(scope.alloc(&w_A, (long long)w_A_h.size()));
   if (want) {
     GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
@@ -2552,6 +2571,7 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
   GTNB_TRY(stage_begin(ctx));
   GTNB_TRY(den_t.stage(scope));
   GTNB_TRY(num_t.stage(scope));
+  if (cut) GTNB_TRY(stage_upload(ctx, cut, cut_h.data(), sizeof(int32_t) * cut_h.size()));
   GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
   if (tot_P) {
     GTNB_TRY(stage_upload(ctx, arc_of, arc_of_h.data(), sizeof(int32_t) * tot_P));
@@ -2572,11 +2592,19 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
       GTNB_TRY(launch_sparse_eps_backward(ctx, num_t.dev, 1, num_t.max_S, num_t.max_AE, B, T, C, T_dev, e_dev, per, fw,
                                           alpha_n, offs_n, -1.0f, g.dev, per, pgrad));
   }
-  GTNB_TRY(launch_sparse_eps_forward(ctx, den_t.dev, 0, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d, offs_d, den,
-                                     status));
-  if (want)
-    GTNB_TRY(launch_sparse_eps_backward(ctx, den_t.dev, 0, t.S, t.A + t.E, B, T, C, T_dev, e_dev, per, w_dev, alpha_d,
-                                        offs_d, 1.0f, g.dev, per, tg.dev));
+  if (split.N > 1) {
+    GTNB_TRY(launch_sparse_cl_eps_forward(ctx, den_t.dev, split, cut, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d,
+                                          offs_d, den, status));
+    if (want)
+      GTNB_TRY(launch_sparse_cl_eps_backward(ctx, den_t.dev, split, cut, t.S, B, T, C, T_dev, e_dev, per, w_dev,
+                                             alpha_d, offs_d, g.dev, per, tg.dev));
+  } else {
+    GTNB_TRY(launch_sparse_eps_forward(ctx, den_t.dev, 0, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d, offs_d, den,
+                                       status));
+    if (want)
+      GTNB_TRY(launch_sparse_eps_backward(ctx, den_t.dev, 0, t.S, t.A + t.E, B, T, C, T_dev, e_dev, per, w_dev,
+                                          alpha_d, offs_d, 1.0f, g.dev, per, tg.dev));
+  }
   GTNB_TRY(join_from(ctx, ctx->copy_stream));
   if (want) {
     GTNB_TRY(launch_sparse_eps_scatter(ctx, tot_P, pgrad, arc_of, tidx, tg.dev, arc_grads ? ag.dev : nullptr));
@@ -2740,11 +2768,13 @@ int backoff_loss_run(gtnb_ctx* ctx, const TransitionArgs& a, const GraphBatch& g
   // the device route's numerators and their tables, whose shapes decide, with G's, whether it can be taken
   std::vector<ProductGraph> prods;
   std::vector<SparseTables> ptabs;
-  const bool fast = ctx->use_implicit && eps_fits(t, C) && backoff_products(gb, Gv, t, C, &prods, &ptabs);
+  SparseSplit split{};
+  const bool fast =
+      ctx->use_implicit && backoff_route(ctx, t, C, &split) && backoff_products(gb, Gv, t, C, &prods, &ptabs);
   return run_criterion(ctx, B, gb.Tb.data(), a.losses_host, a.trans_grad, a.trans_grad_on_device, n_trans, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
                          if (!f) return backoff_loss_exact(scope, a, gb, Gv, t, arc_grads, arc_grads_on_device);
-                         return backoff_loss_fast(scope, a, gb, n_trans, t, prods, ptabs, arc_grads,
+                         return backoff_loss_fast(scope, a, gb, n_trans, t, split, prods, ptabs, arc_grads,
                                                   arc_grads_on_device, needs_exact);
                        });
 }
@@ -2830,25 +2860,34 @@ int backoff_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const Graph
   const long long n_trans = Gv.num_arcs;
   ViterbiBufs v;
   GTNB_TRY(viterbi_open(scope, a, gb, &v));
-  const bool implicit = ctx->use_implicit && eps_fits(t, C);
+  SparseSplit split{};
+  const bool implicit = ctx->use_implicit && backoff_route(ctx, t, C, &split);
   if (implicit) {
     EpsDevTables tabs;
     tabs.add(t, 0, 0);
     GTNB_TRY(tabs.alloc(scope));
+    std::vector<int32_t> cut_h;
+    if (split.N > 1) sparse_eps_cluster_cuts(t, split, &cut_h);
     float* w_dev = nullptr;
-    int32_t *T_dev = nullptr, *head = nullptr;
+    int32_t *T_dev = nullptr, *head = nullptr, *cut = nullptr;
     uint16_t* bp = nullptr;
     GTNB_TRY(scope.borrow(trans_w, trans_on_device != 0, std::max(n_trans, 1ll), &w_dev));
     GTNB_TRY(scope.alloc(&T_dev, B));
     GTNB_TRY(scope.alloc(&head, B));
     GTNB_TRY(scope.alloc(&bp, (long long)B * (T + 1) * t.S));
+    if (!cut_h.empty()) GTNB_TRY(scope.alloc(&cut, (long long)cut_h.size()));
     GTNB_TRY(stage_begin(ctx));
     GTNB_TRY(tabs.stage(scope));
+    if (cut) GTNB_TRY(stage_upload(ctx, cut, cut_h.data(), sizeof(int32_t) * cut_h.size()));
     GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
     if (!trans_on_device && n_trans) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
     GTNB_TRY(stage_end(ctx));
-    GTNB_TRY(launch_sparse_eps_viterbi(ctx, tabs.dev, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head,
-                                       v.s_dev, v.p_dev, v.a_dev, v.status));
+    if (split.N > 1)
+      GTNB_TRY(launch_sparse_cl_eps_viterbi(ctx, tabs.dev, split, cut, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C,
+                                            w_dev, bp, head, v.s_dev, v.p_dev, v.a_dev, v.status));
+    else
+      GTNB_TRY(launch_sparse_eps_viterbi(ctx, tabs.dev, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp,
+                                         head, v.s_dev, v.p_dev, v.a_dev, v.status));
   }
   return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
     std::vector<float> W(std::max(n_trans, 1ll));
@@ -3005,7 +3044,9 @@ extern "C" int gtnb_backoff_transitions_viterbi(
   // the loss's numerators, whose shapes decide, with G's, whether the device route can be taken
   std::vector<ProductGraph> prods;
   std::vector<SparseTables> ptabs;
-  const bool fast = ctx->use_implicit && eps_fits(t, C) && backoff_products(gb, *transitions, t, C, &prods, &ptabs);
+  SparseSplit split{}; // (the alignment sweeps the numerators alone: only whether G has a device route matters)
+  const bool fast = ctx->use_implicit && backoff_route(ctx, t, C, &split) &&
+                    backoff_products(gb, *transitions, t, C, &prods, &ptabs);
   GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
   CallScope scope(ctx);
   return backoff_align_run(scope, GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,

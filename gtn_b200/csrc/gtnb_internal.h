@@ -67,7 +67,7 @@ struct gtnb_ctx {
   int bidir_mode = -1; // k_bidir.cu on CTC graphs ("bidir_mode" flag): 0 one node per thread; 1 and -1 (default) the PAIR kernels, ahead of every other node-warp variant measured on an H100 with and without a gradient (profiles/h100_bidir_pair_saves.json)
   bool use_bidir = kBidirDefault; // gtnb_ctx_set_flag("bidir", 0): the CTC criterion takes the two sweeps of k_implicit.cu instead of the bidirectional kernel (k_bidir.cu)
   bool exact_ties = true; // gtnb_ctx_set_flag("exact_ties", 0) turns it off: composed lattices are put in the reference's relaxation order so that viterbiPath breaks exact ties like shortest.cpp:212-218 (k_order.cu)
-  int sparse_cluster = 0; // gtnb_ctx_set_flag("sparse_cluster", v): 0 a G outside the one-CTA envelope of k_sparse.cu takes the materialised route; 1 it takes the cluster kernels where sparse_cluster_plan has a plan; 2, 4, 8 additionally every G that fits a cluster of that size takes it (testing and measurement)
+  int sparse_cluster = 0; // gtnb_ctx_set_flag("sparse_cluster", v): 0 a G outside the one-CTA envelope of k_sparse.cu takes the materialised route; 1 it takes the cluster kernels where sparse_cluster_plan has a plan; 2, 4, 8 additionally every G that fits a cluster of that size takes it (testing and measurement); the backoff entry points read it the same way for a G with epsilon arcs (backoff_route, sparse_cl_eps_* kernels)
   // Call-scoped device arena (the criteria): while arena_on, dev_alloc bumps a pointer inside one cached
   // allocation instead of ~25 stream-ordered allocations per call (each a microsecond or two of host time
   // ahead of the first launch); everything allocated in the scope is released together when it ends.
@@ -446,6 +446,23 @@ int launch_sparse_eps_gather(gtnb_ctx* ctx, long long n, const float* w_A, const
 // tgrad[tidx[k]] += pg[k], and agrad[arc_of[k]] += pg[k] where arc_of[k] >= 0 (agrad nullable)
 int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const int32_t* arc_of, const int32_t* tidx,
                               float* tgrad, float* agrad);
+// The denominator's three backoff sweeps (gs[0] = G, S its nodes) by a thread-block cluster of sp.N CTAs per
+// utterance, for a G outside sparse_eps_supported and inside sparse_cluster_plan (gtnb_product.h: S <= 16384,
+// A + E <= 262144, L <= kSparseMaxLevels, in-degree below kBpStart, C <= 1024, and the shared memory of the plan's
+// splits within 227 KB); cut: sparse_eps_cluster_cuts, on the device.  Same buffers and outputs as the one-CTA
+// launchers with per_cta off (the backward with sgn = 1); rows / offsets / scores / back-pointers bit-identical.  The
+// scratch grows with S: alpha 4 * B * (T + 1) * S bytes, the decode's bp 2 * B * (T + 1) * S bytes.
+int launch_sparse_cl_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                                 const float* w, float* alpha, double* offs, float* den, int32_t* status);
+int launch_sparse_cl_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                                  int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                                  const float* w, const float* alpha, const double* offs, float* grad,
+                                  long long grad_stride, float* wgrad);
+int launch_sparse_cl_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                                 const float* w, uint16_t* bp, int32_t* head, float* score, int32_t* paths,
+                                 int32_t* arcs, int32_t* status);
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);

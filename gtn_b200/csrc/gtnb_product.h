@@ -220,15 +220,23 @@ inline void sparse_tables(const gtnb_graph_view& G, int C, SparseTables* t) {
   }
 }
 
-/* N contiguous node ranges with balanced arc counts from a CSR pointer array ptr[S + 1]: rank r gets the nodes
- * [split[r], split[r + 1]), split[r] the first node at or after arc r * A / N, so that no rank holds more than
- * A / N + the largest degree arcs.  A rank may own no node (a hub's list spans several shares). */
-inline void sparse_cluster_splits(const std::vector<int32_t>& ptr, int N, int32_t* split) {
-  const int S = (int)ptr.size() - 1;
-  const long long A = ptr[S];
+/* N contiguous node ranges with balanced arc counts from a CSR pointer array ptr[S + 1] (plus a second one, eps,
+ * when not null: a node's emitting and epsilon arcs counted together): rank r gets the nodes [split[r], split[r + 1]),
+ * split[r] the first node at or after arc r * A / N, so that no rank holds more than A / N + the largest degree arcs.
+ * A rank may own no node (a hub's list spans several shares). */
+inline void sparse_cluster_splits(const std::vector<int32_t>& ptr, int N, int32_t* split,
+                                  const std::vector<int32_t>* eps = nullptr) {
+  std::vector<int32_t> sum;
+  if (eps) {
+    sum.resize(ptr.size());
+    for (size_t v = 0; v < ptr.size(); v++) sum[v] = ptr[v] + (*eps)[v];
+  }
+  const std::vector<int32_t>& p = eps ? sum : ptr;
+  const int S = (int)p.size() - 1;
+  const long long A = p[S];
   split[0] = 0;
   for (int r = 1; r < N; r++)
-    split[r] = (int32_t)(std::lower_bound(ptr.begin(), ptr.begin() + S, (int32_t)((A * r + N - 1) / N)) - ptr.begin());
+    split[r] = (int32_t)(std::lower_bound(p.begin(), p.begin() + S, (int32_t)((A * r + N - 1) / N)) - p.begin());
   split[N] = S;
 }
 
@@ -238,19 +246,26 @@ inline void sparse_cluster_splits(const std::vector<int32_t>& ptr, int N, int32_
  * that N gets; 0 when none does or G is outside the kernels' bounds (gtnb_meta.h: S <= 16384 nodes, A <= 262 144
  * arcs, in-degree <= 32 766, C <= 1024).  With C = 64 that is e.g. S = 4096 up to the whole 262 144 arcs (N = 8), or
  * S = 16 384 with 131 072 arcs (N = 8, 194 KB).  *sp gets N and the splits.
+ * A G with epsilon arcs (t.E > 0, sparse_eps_tables; the sparse_cl_eps_* kernels) counts them beside the emitting
+ * ones: A + E <= 262 144, the splits balance both kinds, own_out holds a rank's emitting and epsilon out-arcs (the
+ * backward's accumulators), and L <= kSparseMaxLevels, the combined in-degree below kBpStart.  The backoff 4-gram of
+ * 8563 states / 57 231 + 8562 arcs at C = 64 takes N = 2 (about 200 KB).
  */
 inline int sparse_cluster_plan(const SparseTables& t, int C, int force, SparseSplit* sp) {
-  if (t.S < 1 || t.S > kSparseClusterMaxStates || t.A > kSparseClusterMaxArcs || C < 1 || C > kSparseMaxLabels ||
-      t.max_in > kSparseClusterMaxInDegree)
+  const bool eps = t.E > 0;
+  if (t.S < 1 || t.S > kSparseClusterMaxStates || (long long)t.A + t.E > kSparseClusterMaxArcs || C < 1 ||
+      C > kSparseMaxLabels ||
+      (eps ? t.L > kSparseMaxLevels || t.max_in_all >= kBpStart : t.max_in > kSparseClusterMaxInDegree))
     return 0;
   for (int N = 2; N <= kSparseClusterMax; N *= 2) {
     if (force && N != force) continue;
     sp->N = N;
-    sparse_cluster_splits(t.in_ptr, N, sp->in);
-    sparse_cluster_splits(t.out_ptr, N, sp->out);
+    sparse_cluster_splits(t.in_ptr, N, sp->in, eps ? &t.eps_in_ptr : nullptr);
+    sparse_cluster_splits(t.out_ptr, N, sp->out, eps ? &t.eps_out_ptr : nullptr);
     sp->own_out = 0;
     for (int r = 0; r < N; r++)
-      sp->own_out = std::max(sp->own_out, t.out_ptr[sp->out[r + 1]] - t.out_ptr[sp->out[r]]);
+      sp->own_out = std::max(sp->own_out, t.out_ptr[sp->out[r + 1]] - t.out_ptr[sp->out[r]] +
+                                              (eps ? t.eps_out_ptr[sp->out[r + 1]] - t.eps_out_ptr[sp->out[r]] : 0));
     const long long floats =
         std::max(sparse_cl_fwd_smem_floats(t.S, C, N), sparse_cl_bwd_smem_floats(t.S, C, N, sp->own_out));
     if (floats * (long long)sizeof(float) <= kSparseClusterSmemBytes) return N;
@@ -348,6 +363,26 @@ inline void sparse_eps_tables(const gtnb_graph_view& G, SparseTables* t) {
   t->lanes.clear();
   levels(lf, t->eps_in_ptr, t->fwd_ptr, t->fwd_node);
   levels(lb, t->eps_out_ptr, t->bwd_ptr, t->bwd_node);
+}
+
+/*
+ * Each rank's share of each epsilon level under the cluster plan sp (sparse_cluster_plan) of G = t: the nodes of a
+ * level that the rank owns in the emitting update, sp.in forward and sp.out backward, so that a node keeps one owner
+ * through the frame.  A level lists its nodes in ascending id, so the share is one contiguous run of it:
+ * cut[(d * L + l) * (N + 1) + r] .. [... + r + 1] into fwd_node (d = 0) or bwd_node (d = 1), found with lower_bound.
+ */
+inline void sparse_eps_cluster_cuts(const SparseTables& t, const SparseSplit& sp, std::vector<int32_t>* cut) {
+  const int N = sp.N;
+  cut->assign((size_t)2 * t.L * (N + 1), 0);
+  for (int d = 0; d < 2; d++) {
+    const std::vector<int32_t>& ptr = d ? t.bwd_ptr : t.fwd_ptr;
+    const std::vector<int32_t>& node = d ? t.bwd_node : t.fwd_node;
+    const int32_t* split = d ? sp.out : sp.in;
+    for (int l = 0; l < t.L; l++)
+      for (int r = 0; r <= N; r++)
+        (*cut)[(size_t)(d * t.L + l) * (N + 1) + r] =
+            (int32_t)(std::lower_bound(node.begin() + ptr[l], node.begin() + ptr[l + 1], split[r]) - node.begin());
+  }
 }
 
 /*

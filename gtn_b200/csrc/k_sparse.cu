@@ -45,7 +45,8 @@
  * after every frame's emitting update (one CTA barrier per topological level of the epsilon subgraph) and per-CTA
  * tables, so that one launch sweeps B different numerators; an epsilon-free G keeps the kernels above.  The
  * alignment gtnb_backoff_transitions_viterbi runs the decode's tropical sweep and trace over those per-CTA
- * numerators (sparse_eps_align_*), reporting A_b's arcs.
+ * numerators (sparse_eps_align_*), reporting A_b's arcs.  A backoff G beyond one CTA has its denominator swept by a
+ * thread-block cluster (sparse_cl_eps_*), the closure's levels cut over the ranks.
  */
 #include <algorithm>
 
@@ -1213,6 +1214,384 @@ __global__ void __launch_bounds__(256) sparse_eps_align_trace_kernel(
             [&](int a) { return __ldg(arc_of + a) - __ldg(a_first + b); });
 }
 
+/*
+ * The backoff cluster sweeps: the denominator's sparse_eps_* sweeps (G = gs[0] for every utterance) for a G that one
+ * CTA's shared memory cannot hold, one thread-block cluster of N = sp.N CTAs per utterance, the layout of the
+ * sparse_cl_* kernels with the closure of the sparse_eps_* ones.  A rank closes the nodes of each level that it owns
+ * in the emitting update (sp.in in the forward and the tropical sweep, sp.out in the backward): a level lists its
+ * nodes in ascending id, so they are one contiguous run of it, cut[(d * L + l) * (N + 1) + rank] .. [... + rank + 1]
+ * (d = 0 forward, 1 backward; sparse_eps_cluster_cuts, gtnb_product.h), and one barrier.cluster per level replaces
+ * the CTA barrier.  A level reads only nodes of earlier levels and its own node, so no store lands in an entry a peer
+ * reads before the barrier.  A node keeps its owner through the frame, so its alpha entry, its back-pointer and its
+ * later tie flag are written by one CTA.  After the last level every CTA holds the whole closed row and takes its
+ * maximum itself (a maximum does not depend on the order) behind a CTA barrier.  Per frame: 1 + L cluster barriers
+ * and one CTA barrier, against the one-CTA kernels' 2 + L CTA barriers; rows, offsets, Z, back-pointers, head, score
+ * and status are theirs bit for bit.  The backward's accumulators hold the rank's own emitting and epsilon out-arcs,
+ * flushed with red.add, so only the order of the adds into grad and wgrad differs.  The launch bounds ask for two
+ * CTAs per SM: ptxas then allots 64 registers and spills nothing (without the minimum it chose 40 / 64 and spilled).
+ */
+
+/* eps_close_fwd by a cluster: this rank's share of every forward level, each result into every CTA */
+__device__ __forceinline__ void cl_eps_close_fwd(const SparseEpsDev& x, const int32_t* __restrict__ cut, int N,
+                                                 int rank, const float* __restrict__ w, float* R, bool& bad) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    const int n0 = __ldg(cut + l * (N + 1) + rank), n1 = __ldg(cut + l * (N + 1) + rank + 1);
+    for (int i0 = n0; i0 < n1; i0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int i = i0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      int v = 0;
+      if (i < n1) {
+        v = __ldg(x.fwd_node + i);
+        const int k1 = __ldg(x.eps_in_ptr + v + 1);
+        for (int k = __ldg(x.eps_in_ptr + v) + q; k < k1; k += lanes) {
+          const float wk = __ldg(w + __ldg(x.eps_in_arc + k));
+          bad |= !is_finite(wk);
+          lse_add(m, s, R[__ldg(x.eps_in_src + k)] + wk);
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (i < n1 && q == 0 && m != neg_inf()) {
+        lse_add(m, s, R[v]);
+        cluster_store(R + v, N, m + log_fast(s));
+      }
+    }
+    cluster_sync_all();
+  }
+}
+
+/* eps_close_bwd by a cluster: this rank's share of every backward level; acc: its own epsilon out-arcs, by epsilon
+ * out-table position - ea */
+__device__ __forceinline__ void cl_eps_close_bwd(const SparseEpsDev& x, const int32_t* __restrict__ cut, int N,
+                                                 int rank, const float* __restrict__ w, float* R,
+                                                 const float* __restrict__ al, float fo, float* acc, int ea) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  const int32_t* bcut = cut + x.L * (N + 1);
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + x.L + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    const int n0 = __ldg(bcut + l * (N + 1) + rank), n1 = __ldg(bcut + l * (N + 1) + rank + 1);
+    for (int i0 = n0; i0 < n1; i0 += groups) {
+      const int i = i0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      int u = 0;
+      if (i < n1) {
+        u = __ldg(x.bwd_node + i);
+        const float au = al[u] + fo;
+        const int k1 = __ldg(x.eps_out_ptr + u + 1);
+        for (int k = __ldg(x.eps_out_ptr + u) + q; k < k1; k += lanes) {
+          const float xk = __ldg(w + __ldg(x.eps_out_arc + k)) + R[__ldg(x.eps_out_dst + k)];
+          lse_add(m, s, xk);
+          const float p = exp_fast(au + xk);
+          if (p != 0.0f) acc[k - ea] += p;
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (i < n1 && q == 0 && m != neg_inf()) {
+        lse_add(m, s, R[u]);
+        cluster_store(R + u, N, m + log_fast(s));
+      }
+    }
+    cluster_sync_all();
+  }
+}
+
+/* eps_close_trop by a cluster: this rank's share of every forward level; the back-pointers of its own nodes */
+__device__ __forceinline__ void cl_eps_close_trop(const SparseEpsDev& x, const int32_t* __restrict__ cut, int N,
+                                                  int rank, const float* __restrict__ w, float* R, uint16_t* bp,
+                                                  bool& bad) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    const int n0 = __ldg(cut + l * (N + 1) + rank), n1 = __ldg(cut + l * (N + 1) + rank + 1);
+    for (int i0 = n0; i0 < n1; i0 += groups) {
+      const int i = i0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, v = 0, k0 = 0;
+      if (i < n1) {
+        v = __ldg(x.fwd_node + i);
+        k0 = __ldg(x.eps_in_ptr + v);
+        const int k1 = __ldg(x.eps_in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(x.eps_in_arc + j));
+          bad |= !(wk < CUDART_INF_F);
+          argmax_add(m, k, tie, R[__ldg(x.eps_in_src + j)] + wk, j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (i < n1 && q == 0) {
+        const float cur = R[v];
+        if (m > cur) {
+          const int ne = __ldg(x.g.in_ptr + v + 1) - __ldg(x.g.in_ptr + v);
+          cluster_store(R + v, N, m);
+          bp[v] = (uint16_t)((ne + k - k0) | (tie ? kBpTie : 0));
+        } else if (m == cur && m != neg_inf()) {
+          bp[v] |= kBpTie;
+        }
+      }
+    }
+    cluster_sync_all();
+  }
+}
+
+/* the maximum of a closed row R, whole in every CTA, into red[nt / 32] (merged by cluster_row_offset after the CTA
+ * barrier that follows); R[v] to out[v] (nullable) for this rank's nodes [n0, n1) */
+__device__ __forceinline__ void cl_row_max(const float* R, int S, int n0, int n1, float* out, float* red) {
+  float mx = neg_inf();
+  for (int v = threadIdx.x; v < S; v += blockDim.x) {
+    const float r = R[v];
+    if (out && v >= n0 && v < n1) out[v] = r;
+    mx = fmaxf(mx, r);
+  }
+  mx = warp_max(mx);
+  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = mx;
+}
+
+/* sparse_eps_forward_kernel (per_cta off) by a cluster: the same alpha rows, offsets, Z, den and status */
+__global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_forward_kernel(
+    const SparseEpsDev* __restrict__ gs, SparseSplit sp, const int32_t* __restrict__ cut, int T, int C,
+    const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride, const float* __restrict__ w,
+    float* __restrict__ alpha, double* __restrict__ offs, float* __restrict__ den, int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const SparseEpsDev x = gs[0];
+  const SparseDev& g = x.g;
+  const int S = g.S, lanes = g.lanes, N = sp.N;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  float* red = E + 2 * C; // [2][kSparseWarps]: this CTA's per-warp maxima of the closed rows
+  const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
+  const int n0 = sp.in[rank], n1 = sp.in[rank + 1]; // this CTA's nodes
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  float* al = alpha + (long long)b * (T + 1) * S;
+  double* of = offs + (long long)b * (T + 1);
+  bool bad = false;
+  for (int v = tid; v < S; v += nt) rows[v] = (__ldg(g.flags + v) & 1) ? 0.0f : neg_inf();
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  cluster_sync_all(); // every CTA's first row is in place before a peer stores into its shared memory
+  cl_eps_close_fwd(x, cut, N, rank, w, rows, bad);
+  cl_row_max(rows, S, n0, n1, al, red);
+  __syncthreads();
+  double c_off = 0.0;
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    const float Mp = cluster_row_offset(red + ((t - 1) & 1) * kSparseWarps, nt / 32);
+    for (int v0 = n0; v0 < n1; v0 += groups) { // (the same trip count in every warp: the merge shuffles)
+      const int v = v0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (v < n1) {
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int k = __ldg(g.in_ptr + v) + q; k < k1; k += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + k));
+          const float ek = Er[__ldg(g.in_lab + k)];
+          bad |= !(is_finite(wk) && is_finite(ek));
+          lse_add(m, s, P[__ldg(g.in_src + k)] + (wk + ek));
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (v < n1 && q == 0) cluster_store(Q + v, N, m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mp);
+    }
+    cluster_sync_all();
+    cl_eps_close_fwd(x, cut, N, rank, w, Q, bad); // (its last barrier: the closed row is whole in every CTA)
+    cl_row_max(Q, S, n0, n1, al + (long long)t * S, red + (t & 1) * kSparseWarps);
+    c_off += (double)Mp;
+    if (rank == 0 && tid == 0) of[t] = c_off;
+    __syncthreads();
+  }
+  bad = __syncthreads_or(bad);
+  if (bad && tid == 0) atomicOr(&status[b], 1);
+  if (rank == 0 && tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    for (int v = tid; v < S; v += 32)
+      if (__ldg(g.flags + v) & 2) m = fmaxf(m, F[v]);
+    m = warp_max(m);
+    float s = 0.0f;
+    if (m != neg_inf())
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) s += expf(F[v] - m);
+    s = warp_sum(s);
+    if (tid == 0) {
+      const double Z = m == neg_inf() ? (double)neg_inf() : c_off + (double)(m + logf(s));
+      of[0] = Z;
+      den[b] = (float)Z;
+    }
+  }
+}
+
+/* sparse_eps_backward_kernel (per_cta off, sgn = 1) by a cluster: rank r adds the posteriors of its own nodes'
+ * emitting and epsilon out-arcs */
+__global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_backward_kernel(
+    const SparseEpsDev* __restrict__ gs, SparseSplit sp, const int32_t* __restrict__ cut, int T, int C,
+    const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride, const float* __restrict__ w,
+    const float* __restrict__ alpha, const double* __restrict__ offs, float* __restrict__ grad, long long grad_stride,
+    float* __restrict__ wgrad) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const SparseEpsDev x = gs[0];
+  const SparseDev& g = x.g;
+  const int S = g.S, lanes = g.lanes, N = sp.N;
+  float* rows = sm; // [2][S] beta rows
+  float* E = sm + 2 * S; // [2][C] emission rows
+  float* Eg = E + 2 * C; // [2][C] the frame's emission gradient, this CTA's share
+  float* red = Eg + 2 * C; // [2][kSparseWarps]
+  float* acc = red + 2 * kSparseWarps; // own emitting out-arcs (by out-table position - ka), then own epsilon ones
+  const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
+  const int n0 = sp.out[rank], n1 = sp.out[rank + 1]; // this CTA's nodes
+  const int ka = __ldg(g.out_ptr + n0), kn = __ldg(g.out_ptr + n1) - ka; // their emitting out-arcs
+  const int ea = __ldg(x.eps_out_ptr + n0), en = __ldg(x.eps_out_ptr + n1) - ea; // and epsilon out-arcs
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const double* of = offs + (long long)b * (T + 1);
+  const double Z = of[0];
+  if (Tb < 1 || !(fabs(Z) < (double)CUDART_INF_F)) return; // (the whole cluster: its ranks share b)
+  const float* em = emis + (long long)b * stride;
+  const float* al = alpha + (long long)b * (T + 1) * S;
+  float* gr = grad + (long long)b * grad_stride;
+  for (int v = tid; v < S; v += nt) rows[(Tb & 1) * S + v] = (__ldg(g.flags + v) & 2) ? 0.0f : neg_inf();
+  for (int k = tid; k < kn + en; k += nt) acc[k] = 0.0f;
+  for (int c = tid; c < 2 * C; c += nt) Eg[c] = 0.0f;
+  for (int c = tid; c < C; c += nt) E[((Tb - 1) & 1) * C + c] = __ldg(em + (long long)(Tb - 1) * C + c);
+  cluster_sync_all();
+  cl_eps_close_bwd(x, cut, N, rank, w, rows + (Tb & 1) * S, al + (long long)Tb * S, (float)(of[Tb] - Z), acc + kn,
+                   ea);
+  cl_row_max(rows + (Tb & 1) * S, S, 0, 0, nullptr, red + (Tb & 1) * kSparseWarps);
+  __syncthreads();
+  double d = 0.0; // d_{t+1}
+  for (int t = Tb - 1; t >= 0; t--) {
+    const float* Nx = rows + ((t + 1) & 1) * S;
+    float* Cur = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    float* Eg_t = Eg + (t & 1) * C;
+    float* Eg_prev = Eg + ((t + 1) & 1) * C; // frame t + 1's, complete since the barrier
+    for (int c = tid; c < C; c += nt) {
+      if (t > 0) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)(t - 1) * C + c);
+      if (t + 1 < Tb) {
+        const float v = Eg_prev[c];
+        if (v != 0.0f) atomicAdd(gr + (long long)(t + 1) * C + c, v);
+        Eg_prev[c] = 0.0f;
+      }
+    }
+    const float Mb = cluster_row_offset(red + ((t + 1) & 1) * kSparseWarps, nt / 32);
+    const double c_t = t > 0 ? of[t] : 0.0;
+    const float fo = (float)(c_t + d - Z);
+    for (int u0 = n0; u0 < n1; u0 += groups) {
+      const int u = u0 + grp;
+      float m = neg_inf(), s = 0.0f;
+      if (u < n1) {
+        const float au = al[(long long)t * S + u] + fo;
+        const int k1 = __ldg(g.out_ptr + u + 1);
+        for (int k = __ldg(g.out_ptr + u) + q; k < k1; k += lanes) {
+          const int lab = __ldg(g.out_lab + k);
+          const float xk = Nx[__ldg(g.out_dst + k)] + (__ldg(w + __ldg(g.out_arc + k)) + Er[lab]);
+          lse_add(m, s, xk);
+          const float p = exp_fast(au + xk);
+          if (p != 0.0f) {
+            acc[k - ka] += p;
+            atomicAdd(Eg_t + lab, p);
+          }
+        }
+      }
+      lse_merge(m, s, lanes);
+      if (u < n1 && q == 0) cluster_store(Cur + u, N, m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mb);
+    }
+    cluster_sync_all();
+    cl_eps_close_bwd(x, cut, N, rank, w, Cur, al + (long long)t * S, (float)(c_t + (d + (double)Mb) - Z), acc + kn,
+                     ea);
+    cl_row_max(Cur, S, 0, 0, nullptr, red + (t & 1) * kSparseWarps);
+    d += (double)Mb;
+    __syncthreads();
+  }
+  for (int c = tid; c < C; c += nt) { // frame 0's emission gradient
+    const float v = Eg[c];
+    if (v != 0.0f) atomicAdd(gr + c, v);
+  }
+  for (int k = tid; k < kn; k += nt)
+    if (acc[k] != 0.0f) atomicAdd(wgrad + __ldg(g.out_arc + ka + k), acc[k]);
+  for (int k = tid; k < en; k += nt)
+    if (acc[kn + k] != 0.0f) atomicAdd(wgrad + __ldg(x.eps_out_arc + ea + k), acc[kn + k]);
+}
+
+/* sparse_eps_viterbi_kernel by a cluster: the same back-pointers ([B][T + 1][S]), head, score and status */
+__global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_viterbi_kernel(
+    const SparseEpsDev* __restrict__ gs, SparseSplit sp, const int32_t* __restrict__ cut, int T, int C,
+    const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride, const float* __restrict__ w,
+    uint16_t* __restrict__ bp, int32_t* __restrict__ head, float* __restrict__ score, int32_t* __restrict__ status) {
+  GTNB_DYNAMIC_SMEM(float, sm);
+  const SparseEpsDev x = gs[0];
+  const SparseDev& g = x.g;
+  const int S = g.S, lanes = g.lanes, N = sp.N;
+  float* rows = sm; // [2][S]
+  float* E = sm + 2 * S; // [2][C]
+  const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
+  const int n0 = sp.in[rank], n1 = sp.in[rank + 1]; // this CTA's nodes
+  const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+  const int Tb = lens[b];
+  const float* em = emis + (long long)b * stride;
+  uint16_t* bpb = bp + (long long)b * (T + 1) * S;
+  bool bad = false;
+  for (int v = tid; v < S; v += nt) {
+    const bool st = __ldg(g.flags + v) & 1;
+    rows[v] = st ? 0.0f : neg_inf();
+    if (v >= n0 && v < n1) bpb[v] = st ? (uint16_t)kBpStart : kBpNone;
+  }
+  if (Tb > 0)
+    for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
+  cluster_sync_all();
+  cl_eps_close_trop(x, cut, N, rank, w, rows, bpb, bad);
+  for (int t = 1; t <= Tb; t++) {
+    const float* P = rows + ((t - 1) & 1) * S;
+    float* Q = rows + (t & 1) * S;
+    const float* Er = E + (t & 1) * C;
+    uint16_t* bpt = bpb + (long long)t * S;
+    if (t < Tb)
+      for (int c = tid; c < C; c += nt) E[((t + 1) & 1) * C + c] = __ldg(em + (long long)t * C + c);
+    for (int v0 = n0; v0 < n1; v0 += groups) {
+      const int v = v0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, k0 = 0;
+      if (v < n1) {
+        k0 = __ldg(g.in_ptr + v);
+        const int k1 = __ldg(g.in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(g.in_arc + j));
+          const float ek = Er[__ldg(g.in_lab + j)];
+          bad |= !(wk < CUDART_INF_F && ek < CUDART_INF_F);
+          argmax_add(m, k, tie, P[__ldg(g.in_src + j)] + (wk + ek), j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (v < n1 && q == 0) {
+        cluster_store(Q + v, N, m);
+        bpt[v] = m == neg_inf() ? kBpNone : (uint16_t)((k - k0) | (tie ? kBpTie : 0));
+      }
+    }
+    cluster_sync_all();
+    cl_eps_close_trop(x, cut, N, rank, w, Q, bpt, bad); // (its last barrier ends the frame)
+  }
+  bad = __syncthreads_or(bad);
+  if (bad && tid == 0) atomicOr(&status[b], 1);
+  if (rank == 0 && tid < 32) {
+    const float* F = rows + (Tb & 1) * S;
+    float m = neg_inf();
+    int k = 0x7fffffff, tie = 0;
+    if (Tb > 0)
+      for (int v = tid; v < S; v += 32)
+        if (__ldg(g.flags + v) & 2) argmax_add(m, k, tie, F[v], v);
+    argmax_merge(m, k, tie, 32);
+    if (tid == 0) {
+      head[b] = m == neg_inf() ? -1 : k;
+      score[b] = m;
+      if (tie) atomicOr(&status[b], 2);
+    }
+  }
+}
+
 /* the numerators' weights, gathered: w[k] = fl(w_A[arc_of[k]] + W[tidx[k]]), W[tidx[k]] alone for an epsilon arc
  * (arc_of -1); w_A NULL: every A weight 0 */
 __global__ void __launch_bounds__(256) sparse_eps_gather_kernel(long long n, const float* __restrict__ w_A,
@@ -1440,6 +1819,52 @@ int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const
   if (n == 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "sparse_eps_scatter", sparse_eps_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0,
                                                                      ctx->stream>>>(n, pg, arc_of, tidx, tgrad, agrad));
+  return GTNB_OK;
+}
+
+int launch_sparse_cl_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                                 const float* w, float* alpha, double* offs, float* den, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_eps_forward_kernel)) return rc;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg =
+      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_fwd_smem_floats(S, C, sp.N), &attr);
+  GTNB_LAUNCH(ctx, "sparse_cl_eps_forward",
+              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_eps_forward_kernel, gs, sp, cut, T, C, lens, emis,
+                                                stride, w, alpha, offs, den, status)));
+  return GTNB_OK;
+}
+
+int launch_sparse_cl_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                                  int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                                  const float* w, const float* alpha, const double* offs, float* grad,
+                                  long long grad_stride, float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_eps_backward_kernel)) return rc;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg =
+      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_bwd_smem_floats(S, C, sp.N, sp.own_out), &attr);
+  GTNB_LAUNCH(ctx, "sparse_cl_eps_backward",
+              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_eps_backward_kernel, gs, sp, cut, T, C, lens, emis,
+                                                stride, w, alpha, offs, grad, grad_stride, wgrad)));
+  return GTNB_OK;
+}
+
+int launch_sparse_cl_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                                 const float* w, uint16_t* bp, int32_t* head, float* score, int32_t* paths,
+                                 int32_t* arcs, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_eps_viterbi_kernel)) return rc;
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = cluster_config(ctx, B, sp.N, sizeof(float) * sparse_vit_smem_floats(S, C), &attr);
+  GTNB_LAUNCH(ctx, "sparse_cl_eps_viterbi",
+              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_eps_viterbi_kernel, gs, sp, cut, T, C, lens, emis,
+                                                stride, w, bp, head, score, status)));
+  GTNB_LAUNCH(ctx, "sparse_eps_trace", sparse_eps_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0,
+                                                                 ctx->stream>>>(gs, B, T, lens, bp, head, paths, arcs,
+                                                                                status));
   return GTNB_OK;
 }
 

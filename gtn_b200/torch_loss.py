@@ -501,26 +501,34 @@ class BackoffTransitionsLossFunction(GraphTransitionsLossFunction):
     epsilon arcs (ilabel == olabel == gtn.epsilon), the backoff arcs of a pruned n-gram token LM, which move G without
     consuming a frame and weigh their own transitions entry; the score sums over every path, the backoff paths
     included.  The arguments and the backward are sparse_transitions_loss's; an epsilon-free G gives its results.
+    large_transitions=True: a backoff G beyond one CTA (over 4096 states or 32 768 emitting plus epsilon arcs), up to
+    16 384 states and 262 144 arcs, keeps the device route, its denominator swept by one thread-block cluster per
+    utterance (_clustered); a smaller G is not affected.
     """
 
     @staticmethod
     def forward(ctx, emissions, transitions, weights, graphs, transitions_graph, input_lengths=None, reduction="mean",
-                allreduce=True):
+                allreduce=True, large_transitions=False):
         gv = _graph_view(transitions_graph)
         assert transitions.numel() == gv[0].num_arcs
         return _transitions_forward(
             ctx, emissions, transitions, weights, graphs, input_lengths, reduction, allreduce,
             max(transitions.numel(), 1),
-            lambda c, tw, losses, grad, tg: capi.lib().gtnb_backoff_transitions_loss(
-                c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1,
-                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, None if c.ag is None else c.ag.data_ptr(), 1,
-                tg.data_ptr(), 1))
+            lambda c, tw, losses, grad, tg: _clustered(
+                c.g, large_transitions, lambda: capi.lib().gtnb_backoff_transitions_loss(
+                    c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1,
+                    losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1,
+                    None if c.ag is None else c.ag.data_ptr(), 1, tg.data_ptr(), 1)))
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return GraphTransitionsLossFunction.backward(ctx, grad_output) + (None,)
 
 
 def backoff_transitions_loss(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
-                             reduction="mean", allreduce=True):
+                             reduction="mean", allreduce=True, large_transitions=False):
     return BackoffTransitionsLossFunction.apply(emissions, transitions, weights, graphs, transitions_graph,
-                                                input_lengths, reduction, allreduce)
+                                                input_lengths, reduction, allreduce, large_transitions)
 
 
 @torch.no_grad()
@@ -592,16 +600,18 @@ def sparse_viterbi(emissions, transitions, transitions_graph, input_lengths=None
 
 
 @torch.no_grad()
-def backoff_viterbi(emissions, transitions, transitions_graph, input_lengths=None):
+def backoff_viterbi(emissions, transitions, transitions_graph, input_lengths=None, large_transitions=False):
     """Best path of intersect(E_b, G) for every utterance, G the backoff transition graph of backoff_transitions_loss
     (epsilon arcs allowed), through gtnb_viterbi_backoff: the decode of a model trained with that loss.  The arguments
     and outputs are sparse_viterbi's.  arcs[b, t] is the emitting G arc taken at frame t: an epsilon arc uses no frame
-    and is not reported.  Ties are broken as the reference breaks them.
+    and is not reported.  Ties are broken as the reference breaks them.  large_transitions as in
+    backoff_transitions_loss.
     """
     c = _GraphCall(emissions, None, None, input_lengths, arc_grads=False)
     gv, tw = _sparse_transitions(c, transitions, transitions_graph)
-    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_viterbi_backoff(
-        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1))
+    return c.viterbi(lambda paths, arcs, scores: _clustered(
+        c.g, large_transitions, lambda: capi.lib().gtnb_viterbi_backoff(
+            c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs, scores, 1)))
 
 
 @torch.no_grad()
@@ -624,16 +634,18 @@ def sparse_transitions_viterbi(emissions, transitions, transitions_graph, graphs
 
 
 @torch.no_grad()
-def backoff_transitions_viterbi(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None):
+def backoff_transitions_viterbi(emissions, transitions, transitions_graph, graphs, input_lengths=None, weights=None,
+                                large_transitions=False):
     """Best path of backoff_transitions_loss's numerator, intersect(intersect(A_b, G), E_b), for every utterance,
     through gtnb_backoff_transitions_viterbi: the decomposition and frame-level alignment a model trained with
     backoff_transitions_loss picks within its own target graph, under the backoff LM it was trained with.  The
     arguments are backoff_transitions_loss's and the outputs sparse_transitions_viterbi's: arcs[b, t] is the arc of
     graphs[b] taken at frame t, and an epsilon arc of G uses no frame and is not reported.  Ties are broken as the
-    reference breaks them.
+    reference breaks them.  large_transitions as in backoff_transitions_loss.
     """
     c = _GraphCall(emissions, graphs, weights, input_lengths, arc_grads=False)
     gv, tw = _sparse_transitions(c, transitions, transitions_graph)
-    return c.viterbi(lambda paths, arcs, scores: capi.lib().gtnb_backoff_transitions_viterbi(
-        c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths, arcs,
-        scores, 1))
+    return c.viterbi(lambda paths, arcs, scores: _clustered(
+        c.g, large_transitions, lambda: capi.lib().gtnb_backoff_transitions_viterbi(
+            c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths,
+            arcs, scores, 1)))

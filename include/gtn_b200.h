@@ -117,6 +117,11 @@ int64_t gtnb_ctx_launch_count(const gtnb_ctx* ctx);
  * accumulator split over the CTAs: e.g. 4096 nodes with 262144 arcs, or 16384 nodes with 131072 arcs); a smaller G
  * keeps the one-CTA kernels.  2, 4, 8 (testing and measurement): additionally every G that fits a cluster of that
  * size takes it; results are bit-identical apart from the order of the gradient sums.  Other values are rejected.
+ * The flag governs gtnb_backoff_transitions_loss, gtnb_viterbi_backoff and gtnb_backoff_transitions_viterbi the same
+ * way for a backoff G (with epsilon arcs) beyond their one-CTA envelope: at 1 its denominator is swept by a cluster
+ * (k_sparse.cu's sparse_cl_eps_* kernels) when it has at most 16384 nodes, 262144 emitting plus epsilon arcs, 32
+ * levels, a combined in-degree below 32766, C <= 1024, and the cluster's shared memory holds it (e.g. a backoff
+ * 4-gram of 8563 states / 65 793 arcs at C = 64 takes 2 CTAs); the numerators keep their one-CTA envelope.
  */
 int gtnb_ctx_set_flag(gtnb_ctx* ctx, const char* name, int value);
 
@@ -799,6 +804,9 @@ int gtnb_sparse_transitions_viterbi(
  * plus epsilon arcs, 32 levels (the longest chain of epsilon arcs; a backoff n-gram of order n has n - 1), C <= 1024.
  * Outside it, with a non-finite value or with the "implicit" flag off, the exact route composes E_b with G and the
  * numerators with E_b (gtnb_compose_graphs) and runs the materialised lattices utterance by utterance.
+ * With the "sparse_cluster" flag at 1 a larger G (gtnb_ctx_set_flag: up to 16384 nodes / 262144 emitting plus epsilon
+ * arcs) keeps the device route, its denominator swept by a thread-block cluster per utterance; the scratch grows with
+ * G's nodes S: alpha is 4 * B * (T + 1) * S bytes (2.2 GB for a backoff 4-gram of 8563 states at B = 128, T = 500).
  */
 int gtnb_backoff_transitions_loss(
     gtnb_ctx* ctx,
@@ -834,6 +842,9 @@ int gtnb_backoff_transitions_loss(
  * inside a frame.  Its envelope is gtnb_backoff_transitions_loss's.  An utterance with a tie on its traced path
  * ("exact_ties" on) or a NaN or +inf is re-run on compose(E_b, G) (gtnb_compose_graphs, gtnb_forward,
  * gtnb_viterbi_path), as is the whole batch outside the envelope or with the "implicit" flag off.
+ * With the "sparse_cluster" flag at 1 a larger G (up to 16384 nodes / 262144 emitting plus epsilon arcs) keeps the
+ * device route, swept by a thread-block cluster per utterance with the same back-pointers (1.1 GB for a backoff 4-gram
+ * of 8563 states at B = 128, T = 500).
  * Error rules are gtnb_backoff_transitions_loss's for G and gtnb_viterbi_sparse's otherwise.
  */
 int gtnb_viterbi_backoff(
@@ -867,7 +878,9 @@ int gtnb_viterbi_backoff(
  * numerator's nodes); the trace reports A_b's arcs.  Its envelope is gtnb_backoff_transitions_loss's, for every
  * numerator.  An utterance with a tie on its traced path ("exact_ties" on) or a NaN or +inf is re-run on
  * compose(compose(A_b, G), E_b) (gtnb_compose_graphs, gtnb_forward, gtnb_viterbi_path), as is the whole batch outside
- * the envelope or with the "implicit" flag off; only that route reads trans_w to the host.
+ * the envelope or with the "implicit" flag off; only that route reads trans_w to the host.  With the "sparse_cluster"
+ * flag at 1 a G beyond the one-CTA envelope (up to gtnb_viterbi_backoff's cluster envelope) keeps the device route:
+ * the alignment sweeps the numerators alone, so only the gate changes.
  */
 int gtnb_backoff_transitions_viterbi(
     gtnb_ctx* ctx,
