@@ -1742,16 +1742,11 @@ struct SparseDenominator {
   }
   int forward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
               float* den, int32_t* status) {
-    if (split.N > 1)
-      return launch_sparse_cl_den_forward(ctx, tabs.dev, split, B, T, C, lens, e, per, w, alpha, offs, den, status);
-    return launch_sparse_den_forward(ctx, tabs.dev, B, T, C, lens, e, per, w, alpha, offs, den, status);
+    return launch_sparse_den_forward(ctx, tabs.dev, split, B, T, C, lens, e, per, w, alpha, offs, den, status);
   }
   int backward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
                const float*, float* grad, float* wgrad) {
-    if (split.N > 1)
-      return launch_sparse_cl_den_backward(ctx, tabs.dev, split, B, T, C, lens, e, per, w, alpha, offs, grad, per,
-                                           wgrad);
-    return launch_sparse_den_backward(ctx, tabs.dev, B, T, C, lens, e, per, w, alpha, offs, grad, per, wgrad);
+    return launch_sparse_den_backward(ctx, tabs.dev, split, B, T, C, lens, e, per, w, alpha, offs, grad, per, wgrad);
   }
   int fold_grad(gtnb_ctx* ctx, int, const float* w, const float* sig, float* wgrad) {
     return launch_sparse_fold(ctx, groups(), tabs.grp_ptr, tabs.grp_arc, (int)n_trans, w, sig, wgrad);
@@ -2293,12 +2288,8 @@ int viterbi_sparse_run(CallScope& scope, const GraphViterbiArgs& a, const GraphB
     GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
     if (!trans_on_device) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
     GTNB_TRY(stage_end(ctx));
-    if (split.N > 1)
-      GTNB_TRY(launch_sparse_cl_viterbi(ctx, tabs.dev, split, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp,
-                                        head, v.s_dev, v.p_dev, v.a_dev, v.status));
-    else
-      GTNB_TRY(launch_sparse_viterbi(ctx, tabs.dev, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head,
-                                     v.s_dev, v.p_dev, v.a_dev, v.status));
+    GTNB_TRY(launch_sparse_viterbi(ctx, tabs.dev, split, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp, head,
+                                   v.s_dev, v.p_dev, v.a_dev, v.status));
   }
   return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
     std::vector<float> W(std::max(n_trans, 1ll));
@@ -2586,25 +2577,18 @@ int backoff_loss_fast(CallScope& scope, const TransitionArgs& a, const GraphBatc
   GTNB_TRY(fork_to(ctx, ctx->copy_stream));
   {
     OnStream side(ctx, ctx->copy_stream);
-    GTNB_TRY(launch_sparse_eps_forward(ctx, num_t.dev, 1, num_t.max_S, B, T, C, T_dev, e_dev, per, fw, alpha_n, offs_n,
-                                       num, status + B));
+    const SparseSplit one{1}; // the numerators: one CTA each
+    GTNB_TRY(launch_sparse_eps_forward(ctx, num_t.dev, one, nullptr, 1, num_t.max_S, B, T, C, T_dev, e_dev, per, fw,
+                                       alpha_n, offs_n, num, status + B));
     if (want)
-      GTNB_TRY(launch_sparse_eps_backward(ctx, num_t.dev, 1, num_t.max_S, num_t.max_AE, B, T, C, T_dev, e_dev, per, fw,
-                                          alpha_n, offs_n, -1.0f, g.dev, per, pgrad));
+      GTNB_TRY(launch_sparse_eps_backward(ctx, num_t.dev, one, nullptr, 1, num_t.max_S, num_t.max_AE, B, T, C, T_dev,
+                                          e_dev, per, fw, alpha_n, offs_n, -1.0f, g.dev, per, pgrad));
   }
-  if (split.N > 1) {
-    GTNB_TRY(launch_sparse_cl_eps_forward(ctx, den_t.dev, split, cut, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d,
-                                          offs_d, den, status));
-    if (want)
-      GTNB_TRY(launch_sparse_cl_eps_backward(ctx, den_t.dev, split, cut, t.S, B, T, C, T_dev, e_dev, per, w_dev,
-                                             alpha_d, offs_d, g.dev, per, tg.dev));
-  } else {
-    GTNB_TRY(launch_sparse_eps_forward(ctx, den_t.dev, 0, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d, offs_d, den,
-                                       status));
-    if (want)
-      GTNB_TRY(launch_sparse_eps_backward(ctx, den_t.dev, 0, t.S, t.A + t.E, B, T, C, T_dev, e_dev, per, w_dev,
-                                          alpha_d, offs_d, 1.0f, g.dev, per, tg.dev));
-  }
+  GTNB_TRY(launch_sparse_eps_forward(ctx, den_t.dev, split, cut, 0, t.S, B, T, C, T_dev, e_dev, per, w_dev, alpha_d,
+                                     offs_d, den, status));
+  if (want)
+    GTNB_TRY(launch_sparse_eps_backward(ctx, den_t.dev, split, cut, 0, t.S, t.A + t.E, B, T, C, T_dev, e_dev, per, w_dev,
+                                        alpha_d, offs_d, 1.0f, g.dev, per, tg.dev));
   GTNB_TRY(join_from(ctx, ctx->copy_stream));
   if (want) {
     GTNB_TRY(launch_sparse_eps_scatter(ctx, tot_P, pgrad, arc_of, tidx, tg.dev, arc_grads ? ag.dev : nullptr));
@@ -2882,12 +2866,8 @@ int backoff_viterbi_run(CallScope& scope, const GraphViterbiArgs& a, const Graph
     GTNB_TRY(stage_upload(ctx, T_dev, gb.Tb.data(), sizeof(int32_t) * B));
     if (!trans_on_device && n_trans) GTNB_TRY(stage_upload(ctx, w_dev, trans_w, sizeof(float) * n_trans));
     GTNB_TRY(stage_end(ctx));
-    if (split.N > 1)
-      GTNB_TRY(launch_sparse_cl_eps_viterbi(ctx, tabs.dev, split, cut, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C,
-                                            w_dev, bp, head, v.s_dev, v.p_dev, v.a_dev, v.status));
-    else
-      GTNB_TRY(launch_sparse_eps_viterbi(ctx, tabs.dev, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev, bp,
-                                         head, v.s_dev, v.p_dev, v.a_dev, v.status));
+    GTNB_TRY(launch_sparse_eps_viterbi(ctx, tabs.dev, split, cut, t.S, B, T, C, T_dev, v.e_dev, (long long)T * C, w_dev,
+                                       bp, head, v.s_dev, v.p_dev, v.a_dev, v.status));
   }
   return viterbi_finish(scope, a, gb, implicit, v, [&](const std::vector<int>& which) {
     std::vector<float> W(std::max(n_trans, 1ll));

@@ -386,35 +386,27 @@ int launch_asg_num_build(
 // The envelope, one predicate: 1 <= S <= kSparseMaxStates nodes, A <= kSparseMaxArcs arcs with a label in [0, C),
 // 1 <= C <= kSparseMaxLabels.  alpha: [B][(T+1)*S] floats; offs: [B][T+1] doubles (slot 0: Z).
 bool sparse_den_supported(int S, int A, int C);
-int launch_sparse_den_forward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
-                              const float* emis, long long stride, const float* w, float* alpha, double* offs,
-                              float* den, int32_t* status);
-int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
-                               const float* emis, long long stride, const float* w, const float* alpha,
-                               const double* offs, float* grad, long long grad_stride, float* wgrad);
-// sigma_k = logsumexp of start group k's weights, and its gradient (wgrad[nG + k]) folded back by softmax
+// sp: sparse_route's split.  sp.N = 1 sweeps each utterance with one CTA (G inside sparse_den_supported); otherwise a
+// thread-block cluster of sp.N CTAs per utterance does, for a G inside sparse_cluster_plan (gtnb_product.h: S <= 16384,
+// A <= 262144, in-degree <= 32766, C <= 1024, and the shared memory of the plan's splits within 227 KB).  Same buffers
+// and outputs either way: rows / offsets / scores / back-pointers bit-identical.  The scratch grows with S: alpha
+// 4 * B * (T + 1) * S bytes, bp 2 * B * T * S bytes.
+int launch_sparse_den_forward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                              const int32_t* lens, const float* emis, long long stride, const float* w, float* alpha,
+                              double* offs, float* den, int32_t* status);
+int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                               const int32_t* lens, const float* emis, long long stride, const float* w,
+                               const float* alpha, const double* offs, float* grad, long long grad_stride,
+                               float* wgrad);
 // gtnb_viterbi_sparse over the same tables: the tropical sweep (bp: [B][T][S] back-pointers, head: [B] best accept
 // nodes, score: [B]) and the traceback into paths / arcs ([B][T], nullable); status bit 1 non-finite, bit 2 a tie
-int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
-                          const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
-                          float* score, int32_t* paths, int32_t* arcs, int32_t* status);
-// The same three sweeps by a thread-block cluster of sp.N CTAs per utterance, for a G outside sparse_den_supported and
-// inside sparse_cluster_plan (gtnb_product.h: S <= 16384, A <= 262144, in-degree <= 32766, C <= 1024, and the shared
-// memory of the plan's splits within 227 KB); same buffers, same outputs, rows / offsets / scores / back-pointers
-// bit-identical.  The scratch grows with S: alpha 4 * B * (T + 1) * S bytes, bp 2 * B * T * S bytes.
-int launch_sparse_cl_den_forward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
-                                 const int32_t* lens, const float* emis, long long stride, const float* w,
-                                 float* alpha, double* offs, float* den, int32_t* status);
-int launch_sparse_cl_den_backward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
-                                  const int32_t* lens, const float* emis, long long stride, const float* w,
-                                  const float* alpha, const double* offs, float* grad, long long grad_stride,
-                                  float* wgrad);
-int launch_sparse_cl_viterbi(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
-                             const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
-                             int32_t* head, float* score, int32_t* paths, int32_t* arcs, int32_t* status);
+int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                          const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
+                          int32_t* head, float* score, int32_t* paths, int32_t* arcs, int32_t* status);
 // tau_k = max (NaN kept) over start group k: the folded start arcs of gtnb_sparse_transitions_viterbi
 int launch_sparse_tau(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
                       float* tau);
+// sigma_k = logsumexp of start group k's weights, and its gradient (wgrad[nG + k]) folded back by softmax
 int launch_sparse_sigma(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
                         float* sigma);
 int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, int nG, const float* w,
@@ -423,16 +415,23 @@ int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32
 // CTA b when per_cta (then alpha rows at gs[b].rows, and max_S / max_AE the largest S / A + E of the batch).  The
 // envelope: S <= kSparseMaxStates, A + E <= kSparseMaxArcs, L <= kSparseMaxLevels, in-degree below kBpStart, C <=
 // kSparseMaxLabels (sparse_eps_supported).  The backward adds sgn times the gradients.  The decode's bp: [B][T + 1][S].
-int launch_sparse_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int B, int T, int C,
-                              const int32_t* lens, const float* emis, long long stride, const float* w, float* alpha,
-                              double* offs, float* den, int32_t* status);
-int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int max_AE, int B,
-                               int T, int C, const int32_t* lens, const float* emis, long long stride, const float* w,
-                               const float* alpha, const double* offs, float sgn, float* grad, long long grad_stride,
-                               float* wgrad);
-int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, int S, int B, int T, int C, const int32_t* lens,
-                              const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
-                              float* score, int32_t* paths, int32_t* arcs, int32_t* status);
+// sp: backoff_route's split; the numerators pass sp.N = 1.  sp.N > 1 sweeps the denominator (gs[0] = G, max_S its
+// S, per_cta off, sgn = 1) by a thread-block cluster of sp.N CTAs per utterance, for a G outside sparse_eps_supported
+// and inside sparse_cluster_plan (S <= 16384, A + E <= 262144, L <= kSparseMaxLevels, in-degree below kBpStart,
+// C <= 1024, and the shared memory of the plan's splits within 227 KB); cut: sparse_eps_cluster_cuts on the device
+// (unused when sp.N = 1).  Same outputs either way, bit-identical but for the order of the gradient adds.
+int launch_sparse_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                              int per_cta, int max_S, int B, int T, int C, const int32_t* lens, const float* emis,
+                              long long stride, const float* w, float* alpha, double* offs, float* den,
+                              int32_t* status);
+int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                               int per_cta, int max_S, int max_AE, int B, int T, int C, const int32_t* lens,
+                               const float* emis, long long stride, const float* w, const float* alpha,
+                               const double* offs, float sgn, float* grad, long long grad_stride, float* wgrad);
+int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut, int S,
+                              int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                              const float* w, uint16_t* bp, int32_t* head, float* score, int32_t* paths, int32_t* arcs,
+                              int32_t* status);
 // gtnb_backoff_transitions_viterbi over the numerators gs[b] (per CTA, max_S their largest S): the decode's sweep with
 // bp at gs[b].rows ((T_b + 1) * S_b per utterance), then the trace, which reports arcs[b][t] = arc_of[product arc] -
 // a_first[b] (A_b's own arc ids; a_first: [B] each utterance's first A arc in arc_of's numbering)
@@ -446,23 +445,6 @@ int launch_sparse_eps_gather(gtnb_ctx* ctx, long long n, const float* w_A, const
 // tgrad[tidx[k]] += pg[k], and agrad[arc_of[k]] += pg[k] where arc_of[k] >= 0 (agrad nullable)
 int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const int32_t* arc_of, const int32_t* tidx,
                               float* tgrad, float* agrad);
-// The denominator's three backoff sweeps (gs[0] = G, S its nodes) by a thread-block cluster of sp.N CTAs per
-// utterance, for a G outside sparse_eps_supported and inside sparse_cluster_plan (gtnb_product.h: S <= 16384,
-// A + E <= 262144, L <= kSparseMaxLevels, in-degree below kBpStart, C <= 1024, and the shared memory of the plan's
-// splits within 227 KB); cut: sparse_eps_cluster_cuts, on the device.  Same buffers and outputs as the one-CTA
-// launchers with per_cta off (the backward with sgn = 1); rows / offsets / scores / back-pointers bit-identical.  The
-// scratch grows with S: alpha 4 * B * (T + 1) * S bytes, the decode's bp 2 * B * (T + 1) * S bytes.
-int launch_sparse_cl_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
-                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
-                                 const float* w, float* alpha, double* offs, float* den, int32_t* status);
-int launch_sparse_cl_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
-                                  int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
-                                  const float* w, const float* alpha, const double* offs, float* grad,
-                                  long long grad_stride, float* wgrad);
-int launch_sparse_cl_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
-                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
-                                 const float* w, uint16_t* bp, int32_t* head, float* score, int32_t* paths,
-                                 int32_t* arcs, int32_t* status);
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);

@@ -49,6 +49,7 @@
  * thread-block cluster (sparse_cl_eps_*), the closure's levels cut over the ranks.
  */
 #include <algorithm>
+#include <utility>
 
 #include "gtnb_ptx.h"
 
@@ -756,13 +757,49 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_cl_viterbi_forward_kern
  * gs[b].rows) and gs[0] otherwise (the denominator, G for the whole batch).
  */
 
+/*
+ * The team that closes a row over the epsilon levels.  OneCta: the CTA closes every node of a level, and a CTA barrier
+ * ends the level.  Cluster: rank `rank` of a cluster of N CTAs (the sparse_cl_eps_* kernels below) closes its run of
+ * each level, cut[(d * L + l) * (N + 1) + rank .. + 1] (d = 0 forward, 1 backward), stores each result into every
+ * CTA through distributed shared memory, and a barrier.cluster ends the level.  The closure helpers are written once
+ * over the team, so a node is closed by the same threads over the same arcs in the same order either way.
+ */
+struct OneCta {
+  /* the level table of each direction, and this CTA's nodes [n0, n1) of level l in it */
+  __device__ __forceinline__ const int32_t* fwd_levels(const SparseEpsDev& x) const { return x.fwd_ptr; }
+  __device__ __forceinline__ const int32_t* bwd_levels(const SparseEpsDev& x) const { return x.bwd_ptr; }
+  __device__ __forceinline__ void level(const int32_t* lv, int l, int& n0, int& n1) const {
+    n0 = __ldg(lv + l), n1 = __ldg(lv + l + 1);
+  }
+  __device__ __forceinline__ bool owns(int, int, int) const { return true; } // node v of this CTA's [n0, n1)
+  __device__ __forceinline__ void put(float* p, float v) const { *p = v; }
+  __device__ __forceinline__ void sync() const { __syncthreads(); }
+};
+
+struct Cluster {
+  const int32_t* cut; // [2][L][N + 1] (sparse_eps_cluster_cuts, gtnb_product.h)
+  int N, rank;
+  __device__ __forceinline__ const int32_t* fwd_levels(const SparseEpsDev&) const { return cut; }
+  __device__ __forceinline__ const int32_t* bwd_levels(const SparseEpsDev& x) const { return cut + x.L * (N + 1); }
+  __device__ __forceinline__ void level(const int32_t* lv, int l, int& n0, int& n1) const {
+    n0 = __ldg(lv + l * (N + 1) + rank), n1 = __ldg(lv + l * (N + 1) + rank + 1);
+  }
+  __device__ __forceinline__ bool owns(int v, int n0, int n1) const { return v >= n0 && v < n1; }
+  __device__ __forceinline__ void put(float* p, float v) const { cluster_store(p, N, v); }
+  __device__ __forceinline__ void sync() const { cluster_sync_all(); }
+};
+
 /* the closure of row R over the forward levels, R[v] = logadd(R[v], logsumexp over v's epsilon in-arcs u -> v of
- * R[u] + w): rows relative to one offset stay so.  bad |= a non-finite epsilon weight.  Ends on a barrier. */
-__device__ __forceinline__ void eps_close_fwd(const SparseEpsDev& x, const float* __restrict__ w, float* R, bool& bad) {
+ * R[u] + w): rows relative to one offset stay so.  bad |= a non-finite epsilon weight.  Ends on the team's barrier. */
+template <class Team>
+__device__ __forceinline__ void eps_close_fwd(Team team, const SparseEpsDev& x, const float* __restrict__ w, float* R,
+                                              bool& bad) {
   const int tid = threadIdx.x, nt = blockDim.x;
+  const int32_t* lv = team.fwd_levels(x);
   for (int l = 0; l < x.L; l++) {
     const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
-    const int n0 = __ldg(x.fwd_ptr + l), n1 = __ldg(x.fwd_ptr + l + 1);
+    int n0, n1;
+    team.level(lv, l, n0, n1);
     for (int i0 = n0; i0 < n1; i0 += groups) { // (the same trip count in every warp: the merge shuffles)
       const int i = i0 + grp;
       float m = neg_inf(), s = 0.0f;
@@ -779,22 +816,26 @@ __device__ __forceinline__ void eps_close_fwd(const SparseEpsDev& x, const float
       lse_merge(m, s, lanes);
       if (i < n1 && q == 0 && m != neg_inf()) {
         lse_add(m, s, R[v]);
-        R[v] = m + log_fast(s);
+        team.put(R + v, m + log_fast(s));
       }
     }
-    __syncthreads();
+    team.sync();
   }
 }
 
 /* the closure of a beta row R over the backward levels, R[u] = logadd(R[u], logsumexp over u's epsilon out-arcs
- * u -> v of w + R[v]), and the posterior exp(al[u] + fo + w + R[v]) of each epsilon arc added into acc[k] (k: its
- * position in the epsilon out-table; fo = c_t + d_t - Z, R relative to d_t).  Ends on a barrier. */
-__device__ __forceinline__ void eps_close_bwd(const SparseEpsDev& x, const float* __restrict__ w, float* R,
-                                              const float* __restrict__ al, float fo, float* acc) {
+ * u -> v of w + R[v]), and the posterior exp(al[u] + fo + w + R[v]) of each epsilon arc added into acc[k - ea] (k: its
+ * position in the epsilon out-table; ea: the team's first; fo = c_t + d_t - Z, R relative to d_t).  Ends on the
+ * team's barrier. */
+template <class Team>
+__device__ __forceinline__ void eps_close_bwd(Team team, const SparseEpsDev& x, const float* __restrict__ w, float* R,
+                                              const float* __restrict__ al, float fo, float* acc, int ea) {
   const int tid = threadIdx.x, nt = blockDim.x;
+  const int32_t* lv = team.bwd_levels(x);
   for (int l = 0; l < x.L; l++) {
     const int lanes = __ldg(x.lanes + x.L + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
-    const int n0 = __ldg(x.bwd_ptr + l), n1 = __ldg(x.bwd_ptr + l + 1);
+    int n0, n1;
+    team.level(lv, l, n0, n1);
     for (int i0 = n0; i0 < n1; i0 += groups) {
       const int i = i0 + grp;
       float m = neg_inf(), s = 0.0f;
@@ -807,26 +848,70 @@ __device__ __forceinline__ void eps_close_bwd(const SparseEpsDev& x, const float
           const float xk = __ldg(w + __ldg(x.eps_out_arc + k)) + R[__ldg(x.eps_out_dst + k)];
           lse_add(m, s, xk);
           const float p = exp_fast(au + xk);
-          if (p != 0.0f) acc[k] += p;
+          if (p != 0.0f) acc[k - ea] += p;
         }
       }
       lse_merge(m, s, lanes);
       if (i < n1 && q == 0 && m != neg_inf()) {
         lse_add(m, s, R[u]);
-        R[u] = m + log_fast(s);
+        team.put(R + u, m + log_fast(s));
       }
     }
-    __syncthreads();
+    team.sync();
   }
 }
 
-/* the maximum of row R over the CTA into red[kSparseWarps] (merged by row_offset after the next barrier); the row
- * also to out (nullable) */
-__device__ __forceinline__ void row_max(const float* R, int S, float* out, float* red) {
+/* the tropical closure of row R over the forward levels: an epsilon arc u -> v wins over v's score when fl(R[u] + w)
+ * is larger; bp[v] then gets its position in v's combined in-list (the ne emitting in-arcs first), and the tie flag
+ * when another candidate, of either kind, reaches the same finite maximum.  bad |= a NaN or +inf epsilon weight. */
+template <class Team>
+__device__ __forceinline__ void eps_close_trop(Team team, const SparseEpsDev& x, const float* __restrict__ w, float* R,
+                                               uint16_t* bp, bool& bad) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  const int32_t* lv = team.fwd_levels(x);
+  for (int l = 0; l < x.L; l++) {
+    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
+    int n0, n1;
+    team.level(lv, l, n0, n1);
+    for (int i0 = n0; i0 < n1; i0 += groups) {
+      const int i = i0 + grp;
+      float m = neg_inf();
+      int k = 0x7fffffff, tie = 0, v = 0, k0 = 0;
+      if (i < n1) {
+        v = __ldg(x.fwd_node + i);
+        k0 = __ldg(x.eps_in_ptr + v);
+        const int k1 = __ldg(x.eps_in_ptr + v + 1);
+        for (int j = k0 + q; j < k1; j += lanes) {
+          const float wk = __ldg(w + __ldg(x.eps_in_arc + j));
+          bad |= !(wk < CUDART_INF_F);
+          argmax_add(m, k, tie, R[__ldg(x.eps_in_src + j)] + wk, j);
+        }
+      }
+      argmax_merge(m, k, tie, lanes);
+      if (i < n1 && q == 0) {
+        const float cur = R[v];
+        if (m > cur) {
+          const int ne = __ldg(x.g.in_ptr + v + 1) - __ldg(x.g.in_ptr + v);
+          team.put(R + v, m);
+          bp[v] = (uint16_t)((ne + k - k0) | (tie ? kBpTie : 0));
+        } else if (m == cur && m != neg_inf()) {
+          bp[v] |= kBpTie;
+        }
+      }
+    }
+    team.sync();
+  }
+}
+
+/* the maximum of a closed row R, whole in every CTA of the team, into red[nt / 32] (merged after the CTA barrier that
+ * follows, by row_offset in one CTA and cluster_row_offset in a cluster); R[v] to out[v] (nullable) for this CTA's
+ * nodes [n0, n1) */
+template <class Team>
+__device__ __forceinline__ void row_max(Team team, const float* R, int S, int n0, int n1, float* out, float* red) {
   float mx = neg_inf();
   for (int v = threadIdx.x; v < S; v += blockDim.x) {
     const float r = R[v];
-    if (out) out[v] = r;
+    if (out && team.owns(v, n0, n1)) out[v] = r;
     mx = fmaxf(mx, r);
   }
   mx = warp_max(mx);
@@ -859,8 +944,8 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_forward_kernel(
   if (Tb > 0)
     for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
   __syncthreads();
-  eps_close_fwd(x, w, rows, bad);
-  row_max(rows, S, al, red);
+  eps_close_fwd(OneCta(), x, w, rows, bad);
+  row_max(OneCta(), rows, S, 0, S, al, red);
   __syncthreads();
   double c_off = 0.0;
   for (int t = 1; t <= Tb; t++) {
@@ -886,8 +971,8 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_forward_kernel(
       if (v < S && q == 0) Q[v] = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mp;
     }
     __syncthreads();
-    eps_close_fwd(x, w, Q, bad);
-    row_max(Q, S, al + (long long)t * S, red + (t & 1) * kSparseWarps);
+    eps_close_fwd(OneCta(), x, w, Q, bad);
+    row_max(OneCta(), Q, S, 0, S, al + (long long)t * S, red + (t & 1) * kSparseWarps);
     c_off += (double)Mp;
     if (tid == 0) of[t] = c_off;
     __syncthreads();
@@ -945,8 +1030,8 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_backward_kernel(
   for (int c = tid; c < 2 * C; c += nt) Eg[c] = 0.0f;
   for (int c = tid; c < C; c += nt) E[((Tb - 1) & 1) * C + c] = __ldg(em + (long long)(Tb - 1) * C + c);
   __syncthreads();
-  eps_close_bwd(x, w, rows + (Tb & 1) * S, al + (long long)Tb * S, (float)(of[Tb] - Z), acc + A);
-  row_max(rows + (Tb & 1) * S, S, nullptr, red + (Tb & 1) * kSparseWarps);
+  eps_close_bwd(OneCta(), x, w, rows + (Tb & 1) * S, al + (long long)Tb * S, (float)(of[Tb] - Z), acc + A, 0);
+  row_max(OneCta(), rows + (Tb & 1) * S, S, 0, S, nullptr, red + (Tb & 1) * kSparseWarps);
   __syncthreads();
   double d = 0.0; // d_{t+1}
   for (int t = Tb - 1; t >= 0; t--) {
@@ -987,8 +1072,8 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_backward_kernel(
       if (u < S && q == 0) Cur[u] = m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mb;
     }
     __syncthreads();
-    eps_close_bwd(x, w, Cur, al + (long long)t * S, (float)(c_t + (d + (double)Mb) - Z), acc + A);
-    row_max(Cur, S, nullptr, red + (t & 1) * kSparseWarps);
+    eps_close_bwd(OneCta(), x, w, Cur, al + (long long)t * S, (float)(c_t + (d + (double)Mb) - Z), acc + A, 0);
+    row_max(OneCta(), Cur, S, 0, S, nullptr, red + (t & 1) * kSparseWarps);
     d += (double)Mb;
     __syncthreads();
   }
@@ -1000,45 +1085,6 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_eps_backward_kernel(
     if (acc[k] != 0.0f) atomicAdd(wgrad + __ldg(g.out_arc + k), sgn * acc[k]);
   for (int k = tid; k < x.E; k += nt)
     if (acc[A + k] != 0.0f) atomicAdd(wgrad + __ldg(x.eps_out_arc + k), sgn * acc[A + k]);
-}
-
-/* the tropical closure of row R over the forward levels: an epsilon arc u -> v wins over v's score when fl(R[u] + w)
- * is larger; bp[v] then gets its position in v's combined in-list (the ne emitting in-arcs first), and the tie flag
- * when another candidate, of either kind, reaches the same finite maximum.  bad |= a NaN or +inf epsilon weight. */
-__device__ __forceinline__ void eps_close_trop(const SparseEpsDev& x, const float* __restrict__ w, float* R,
-                                               uint16_t* bp, bool& bad) {
-  const int tid = threadIdx.x, nt = blockDim.x;
-  for (int l = 0; l < x.L; l++) {
-    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
-    const int n0 = __ldg(x.fwd_ptr + l), n1 = __ldg(x.fwd_ptr + l + 1);
-    for (int i0 = n0; i0 < n1; i0 += groups) {
-      const int i = i0 + grp;
-      float m = neg_inf();
-      int k = 0x7fffffff, tie = 0, v = 0, k0 = 0;
-      if (i < n1) {
-        v = __ldg(x.fwd_node + i);
-        k0 = __ldg(x.eps_in_ptr + v);
-        const int k1 = __ldg(x.eps_in_ptr + v + 1);
-        for (int j = k0 + q; j < k1; j += lanes) {
-          const float wk = __ldg(w + __ldg(x.eps_in_arc + j));
-          bad |= !(wk < CUDART_INF_F);
-          argmax_add(m, k, tie, R[__ldg(x.eps_in_src + j)] + wk, j);
-        }
-      }
-      argmax_merge(m, k, tie, lanes);
-      if (i < n1 && q == 0) {
-        const float cur = R[v];
-        if (m > cur) {
-          const int ne = __ldg(x.g.in_ptr + v + 1) - __ldg(x.g.in_ptr + v);
-          R[v] = m;
-          bp[v] = (uint16_t)((ne + k - k0) | (tie ? kBpTie : 0));
-        } else if (m == cur && m != neg_inf()) {
-          bp[v] |= kBpTie;
-        }
-      }
-    }
-    __syncthreads();
-  }
 }
 
 /*
@@ -1074,7 +1120,7 @@ __device__ __forceinline__ void eps_viterbi_sweep(const SparseEpsDev* __restrict
   if (Tb > 0)
     for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
   __syncthreads();
-  eps_close_trop(x, w, rows, bpb, bad);
+  eps_close_trop(OneCta(), x, w, rows, bpb, bad);
   for (int t = 1; t <= Tb; t++) {
     const float* P = rows + ((t - 1) & 1) * S;
     float* Q = rows + (t & 1) * S;
@@ -1103,7 +1149,7 @@ __device__ __forceinline__ void eps_viterbi_sweep(const SparseEpsDev* __restrict
       }
     }
     __syncthreads();
-    eps_close_trop(x, w, Q, bpt, bad); // (its last barrier ends the frame)
+    eps_close_trop(OneCta(), x, w, Q, bpt, bad); // (its last barrier ends the frame)
   }
   bad = __syncthreads_or(bad);
   if (tid < 32) {
@@ -1228,124 +1274,9 @@ __global__ void __launch_bounds__(256) sparse_eps_align_trace_kernel(
  * and one CTA barrier, against the one-CTA kernels' 2 + L CTA barriers; rows, offsets, Z, back-pointers, head, score
  * and status are theirs bit for bit.  The backward's accumulators hold the rank's own emitting and epsilon out-arcs,
  * flushed with red.add, so only the order of the adds into grad and wgrad differs.  The launch bounds ask for two
- * CTAs per SM: ptxas then allots 64 registers and spills nothing (without the minimum it chose 40 / 64 and spilled).
+ * CTAs per SM: ptxas then allots 64 registers (63 in the backward) and spills nothing (without the minimum it chose
+ * 40 / 64 and spilled).
  */
-
-/* eps_close_fwd by a cluster: this rank's share of every forward level, each result into every CTA */
-__device__ __forceinline__ void cl_eps_close_fwd(const SparseEpsDev& x, const int32_t* __restrict__ cut, int N,
-                                                 int rank, const float* __restrict__ w, float* R, bool& bad) {
-  const int tid = threadIdx.x, nt = blockDim.x;
-  for (int l = 0; l < x.L; l++) {
-    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
-    const int n0 = __ldg(cut + l * (N + 1) + rank), n1 = __ldg(cut + l * (N + 1) + rank + 1);
-    for (int i0 = n0; i0 < n1; i0 += groups) { // (the same trip count in every warp: the merge shuffles)
-      const int i = i0 + grp;
-      float m = neg_inf(), s = 0.0f;
-      int v = 0;
-      if (i < n1) {
-        v = __ldg(x.fwd_node + i);
-        const int k1 = __ldg(x.eps_in_ptr + v + 1);
-        for (int k = __ldg(x.eps_in_ptr + v) + q; k < k1; k += lanes) {
-          const float wk = __ldg(w + __ldg(x.eps_in_arc + k));
-          bad |= !is_finite(wk);
-          lse_add(m, s, R[__ldg(x.eps_in_src + k)] + wk);
-        }
-      }
-      lse_merge(m, s, lanes);
-      if (i < n1 && q == 0 && m != neg_inf()) {
-        lse_add(m, s, R[v]);
-        cluster_store(R + v, N, m + log_fast(s));
-      }
-    }
-    cluster_sync_all();
-  }
-}
-
-/* eps_close_bwd by a cluster: this rank's share of every backward level; acc: its own epsilon out-arcs, by epsilon
- * out-table position - ea */
-__device__ __forceinline__ void cl_eps_close_bwd(const SparseEpsDev& x, const int32_t* __restrict__ cut, int N,
-                                                 int rank, const float* __restrict__ w, float* R,
-                                                 const float* __restrict__ al, float fo, float* acc, int ea) {
-  const int tid = threadIdx.x, nt = blockDim.x;
-  const int32_t* bcut = cut + x.L * (N + 1);
-  for (int l = 0; l < x.L; l++) {
-    const int lanes = __ldg(x.lanes + x.L + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
-    const int n0 = __ldg(bcut + l * (N + 1) + rank), n1 = __ldg(bcut + l * (N + 1) + rank + 1);
-    for (int i0 = n0; i0 < n1; i0 += groups) {
-      const int i = i0 + grp;
-      float m = neg_inf(), s = 0.0f;
-      int u = 0;
-      if (i < n1) {
-        u = __ldg(x.bwd_node + i);
-        const float au = al[u] + fo;
-        const int k1 = __ldg(x.eps_out_ptr + u + 1);
-        for (int k = __ldg(x.eps_out_ptr + u) + q; k < k1; k += lanes) {
-          const float xk = __ldg(w + __ldg(x.eps_out_arc + k)) + R[__ldg(x.eps_out_dst + k)];
-          lse_add(m, s, xk);
-          const float p = exp_fast(au + xk);
-          if (p != 0.0f) acc[k - ea] += p;
-        }
-      }
-      lse_merge(m, s, lanes);
-      if (i < n1 && q == 0 && m != neg_inf()) {
-        lse_add(m, s, R[u]);
-        cluster_store(R + u, N, m + log_fast(s));
-      }
-    }
-    cluster_sync_all();
-  }
-}
-
-/* eps_close_trop by a cluster: this rank's share of every forward level; the back-pointers of its own nodes */
-__device__ __forceinline__ void cl_eps_close_trop(const SparseEpsDev& x, const int32_t* __restrict__ cut, int N,
-                                                  int rank, const float* __restrict__ w, float* R, uint16_t* bp,
-                                                  bool& bad) {
-  const int tid = threadIdx.x, nt = blockDim.x;
-  for (int l = 0; l < x.L; l++) {
-    const int lanes = __ldg(x.lanes + l), groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
-    const int n0 = __ldg(cut + l * (N + 1) + rank), n1 = __ldg(cut + l * (N + 1) + rank + 1);
-    for (int i0 = n0; i0 < n1; i0 += groups) {
-      const int i = i0 + grp;
-      float m = neg_inf();
-      int k = 0x7fffffff, tie = 0, v = 0, k0 = 0;
-      if (i < n1) {
-        v = __ldg(x.fwd_node + i);
-        k0 = __ldg(x.eps_in_ptr + v);
-        const int k1 = __ldg(x.eps_in_ptr + v + 1);
-        for (int j = k0 + q; j < k1; j += lanes) {
-          const float wk = __ldg(w + __ldg(x.eps_in_arc + j));
-          bad |= !(wk < CUDART_INF_F);
-          argmax_add(m, k, tie, R[__ldg(x.eps_in_src + j)] + wk, j);
-        }
-      }
-      argmax_merge(m, k, tie, lanes);
-      if (i < n1 && q == 0) {
-        const float cur = R[v];
-        if (m > cur) {
-          const int ne = __ldg(x.g.in_ptr + v + 1) - __ldg(x.g.in_ptr + v);
-          cluster_store(R + v, N, m);
-          bp[v] = (uint16_t)((ne + k - k0) | (tie ? kBpTie : 0));
-        } else if (m == cur && m != neg_inf()) {
-          bp[v] |= kBpTie;
-        }
-      }
-    }
-    cluster_sync_all();
-  }
-}
-
-/* the maximum of a closed row R, whole in every CTA, into red[nt / 32] (merged by cluster_row_offset after the CTA
- * barrier that follows); R[v] to out[v] (nullable) for this rank's nodes [n0, n1) */
-__device__ __forceinline__ void cl_row_max(const float* R, int S, int n0, int n1, float* out, float* red) {
-  float mx = neg_inf();
-  for (int v = threadIdx.x; v < S; v += blockDim.x) {
-    const float r = R[v];
-    if (out && v >= n0 && v < n1) out[v] = r;
-    mx = fmaxf(mx, r);
-  }
-  mx = warp_max(mx);
-  if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = mx;
-}
 
 /* sparse_eps_forward_kernel (per_cta off) by a cluster: the same alpha rows, offsets, Z, den and status */
 __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_forward_kernel(
@@ -1361,6 +1292,7 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_forward_kerne
   float* red = E + 2 * C; // [2][kSparseWarps]: this CTA's per-warp maxima of the closed rows
   const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
   const int n0 = sp.in[rank], n1 = sp.in[rank + 1]; // this CTA's nodes
+  const Cluster team{cut, N, rank}; // the closure's
   const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
   const int Tb = lens[b];
   const float* em = emis + (long long)b * stride;
@@ -1371,8 +1303,8 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_forward_kerne
   if (Tb > 0)
     for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
   cluster_sync_all(); // every CTA's first row is in place before a peer stores into its shared memory
-  cl_eps_close_fwd(x, cut, N, rank, w, rows, bad);
-  cl_row_max(rows, S, n0, n1, al, red);
+  eps_close_fwd(team, x, w, rows, bad);
+  row_max(team, rows, S, n0, n1, al, red);
   __syncthreads();
   double c_off = 0.0;
   for (int t = 1; t <= Tb; t++) {
@@ -1398,8 +1330,8 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_forward_kerne
       if (v < n1 && q == 0) cluster_store(Q + v, N, m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mp);
     }
     cluster_sync_all();
-    cl_eps_close_fwd(x, cut, N, rank, w, Q, bad); // (its last barrier: the closed row is whole in every CTA)
-    cl_row_max(Q, S, n0, n1, al + (long long)t * S, red + (t & 1) * kSparseWarps);
+    eps_close_fwd(team, x, w, Q, bad); // (its last barrier: the closed row is whole in every CTA)
+    row_max(team, Q, S, n0, n1, al + (long long)t * S, red + (t & 1) * kSparseWarps);
     c_off += (double)Mp;
     if (rank == 0 && tid == 0) of[t] = c_off;
     __syncthreads();
@@ -1445,6 +1377,7 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_backward_kern
   const int n0 = sp.out[rank], n1 = sp.out[rank + 1]; // this CTA's nodes
   const int ka = __ldg(g.out_ptr + n0), kn = __ldg(g.out_ptr + n1) - ka; // their emitting out-arcs
   const int ea = __ldg(x.eps_out_ptr + n0), en = __ldg(x.eps_out_ptr + n1) - ea; // and epsilon out-arcs
+  const Cluster team{cut, N, rank}; // the closure's
   const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
   const int Tb = lens[b];
   const double* of = offs + (long long)b * (T + 1);
@@ -1458,9 +1391,8 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_backward_kern
   for (int c = tid; c < 2 * C; c += nt) Eg[c] = 0.0f;
   for (int c = tid; c < C; c += nt) E[((Tb - 1) & 1) * C + c] = __ldg(em + (long long)(Tb - 1) * C + c);
   cluster_sync_all();
-  cl_eps_close_bwd(x, cut, N, rank, w, rows + (Tb & 1) * S, al + (long long)Tb * S, (float)(of[Tb] - Z), acc + kn,
-                   ea);
-  cl_row_max(rows + (Tb & 1) * S, S, 0, 0, nullptr, red + (Tb & 1) * kSparseWarps);
+  eps_close_bwd(team, x, w, rows + (Tb & 1) * S, al + (long long)Tb * S, (float)(of[Tb] - Z), acc + kn, ea);
+  row_max(team, rows + (Tb & 1) * S, S, 0, 0, nullptr, red + (Tb & 1) * kSparseWarps);
   __syncthreads();
   double d = 0.0; // d_{t+1}
   for (int t = Tb - 1; t >= 0; t--) {
@@ -1501,9 +1433,8 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_backward_kern
       if (u < n1 && q == 0) cluster_store(Cur + u, N, m == neg_inf() ? neg_inf() : (m + log_fast(s)) - Mb);
     }
     cluster_sync_all();
-    cl_eps_close_bwd(x, cut, N, rank, w, Cur, al + (long long)t * S, (float)(c_t + (d + (double)Mb) - Z), acc + kn,
-                     ea);
-    cl_row_max(Cur, S, 0, 0, nullptr, red + (t & 1) * kSparseWarps);
+    eps_close_bwd(team, x, w, Cur, al + (long long)t * S, (float)(c_t + (d + (double)Mb) - Z), acc + kn, ea);
+    row_max(team, Cur, S, 0, 0, nullptr, red + (t & 1) * kSparseWarps);
     d += (double)Mb;
     __syncthreads();
   }
@@ -1530,6 +1461,7 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_viterbi_kerne
   float* E = sm + 2 * S; // [2][C]
   const int rank = (int)cluster_rank(), b = blockIdx.x / N, tid = threadIdx.x, nt = blockDim.x;
   const int n0 = sp.in[rank], n1 = sp.in[rank + 1]; // this CTA's nodes
+  const Cluster team{cut, N, rank}; // the closure's
   const int groups = nt / lanes, grp = tid / lanes, q = tid % lanes;
   const int Tb = lens[b];
   const float* em = emis + (long long)b * stride;
@@ -1543,7 +1475,7 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_viterbi_kerne
   if (Tb > 0)
     for (int c = tid; c < C; c += nt) E[C + c] = __ldg(em + c); // row 0 in E[1]: frame t reads E[t & 1]
   cluster_sync_all();
-  cl_eps_close_trop(x, cut, N, rank, w, rows, bpb, bad);
+  eps_close_trop(team, x, w, rows, bpb, bad);
   for (int t = 1; t <= Tb; t++) {
     const float* P = rows + ((t - 1) & 1) * S;
     float* Q = rows + (t & 1) * S;
@@ -1572,7 +1504,7 @@ __global__ void __launch_bounds__(kSparseThreads, 2) sparse_cl_eps_viterbi_kerne
       }
     }
     cluster_sync_all();
-    cl_eps_close_trop(x, cut, N, rank, w, Q, bpt, bad); // (its last barrier ends the frame)
+    eps_close_trop(team, x, w, Q, bpt, bad); // (its last barrier ends the frame)
   }
   bad = __syncthreads_or(bad);
   if (bad && tid == 0) atomicOr(&status[b], 1);
@@ -1629,26 +1561,69 @@ bool sparse_den_supported(int S, int A, int C) {
   return S >= 1 && S <= kSparseMaxStates && A <= kSparseMaxArcs && C >= 1 && C <= kSparseMaxLabels;
 }
 
-int launch_sparse_den_forward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
-                              const float* emis, long long stride, const float* w, float* alpha, double* offs,
-                              float* den, int32_t* status) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_den_forward_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_fwd_smem_floats(g.S, C);
-  GTNB_LAUNCH(ctx, "sparse_den_forward", sparse_den_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      g, T, C, lens, emis, stride, w, alpha, offs, den, status));
+namespace {
+
+/* kernel on B CTAs of kSparseThreads threads with `floats` floats of dynamic shared memory */
+template <class... P, class... A>
+int launch_ctas(gtnb_ctx* ctx, const char* name, void (*kernel)(P...), int B, long long floats, A&&... args) {
+  if (const int rc = ensure_max_smem(ctx, (const void*)kernel)) return rc;
+  GTNB_LAUNCH(ctx, name,
+              kernel<<<B, kSparseThreads, sizeof(float) * floats, ctx->stream>>>(std::forward<A>(args)...));
   return GTNB_OK;
 }
 
-int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
-                               const float* emis, long long stride, const float* w, const float* alpha,
-                               const double* offs, float* grad, long long grad_stride, float* wgrad) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_den_backward_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_bwd_smem_floats(g.S, g.A, C);
-  GTNB_LAUNCH(ctx, "sparse_den_backward", sparse_den_backward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      g, T, C, lens, emis, stride, w, alpha, offs, grad, grad_stride, wgrad));
+/* kernel on B clusters of N such CTAs */
+template <class... P, class... A>
+int launch_clusters(gtnb_ctx* ctx, const char* name, void (*kernel)(P...), int B, int N, long long floats,
+                    A&&... args) {
+  if (const int rc = ensure_max_smem(ctx, (const void*)kernel)) return rc;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(B * N), 1, 1);
+  cfg.blockDim = dim3(kSparseThreads, 1, 1);
+  cfg.dynamicSmemBytes = sizeof(float) * floats;
+  cfg.stream = ctx->stream;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = (unsigned)N;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  GTNB_LAUNCH(ctx, name, GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...)));
   return GTNB_OK;
+}
+
+/* one warp per utterance */
+unsigned trace_blocks(int B) {
+  return (unsigned)(((long long)B * 32 + 255) / 256);
+}
+
+} // namespace
+
+int launch_sparse_den_forward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                              const int32_t* lens, const float* emis, long long stride, const float* w, float* alpha,
+                              double* offs, float* den, int32_t* status) {
+  if (B == 0) return GTNB_OK;
+  if (sp.N == 1)
+    return launch_ctas(ctx, "sparse_den_forward", sparse_den_forward_kernel, B, sparse_fwd_smem_floats(g.S, C), g, T,
+                       C, lens, emis, stride, w, alpha, offs, den, status);
+  return launch_clusters(ctx, "sparse_cl_den_forward", sparse_cl_den_forward_kernel, B, sp.N,
+                         sparse_cl_fwd_smem_floats(g.S, C, sp.N), g, sp, T, C, lens, emis, stride, w, alpha, offs,
+                         den, status);
+}
+
+int launch_sparse_den_backward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                               const int32_t* lens, const float* emis, long long stride, const float* w,
+                               const float* alpha, const double* offs, float* grad, long long grad_stride,
+                               float* wgrad) {
+  if (B == 0) return GTNB_OK;
+  if (sp.N == 1)
+    return launch_ctas(ctx, "sparse_den_backward", sparse_den_backward_kernel, B,
+                       sparse_bwd_smem_floats(g.S, g.A, C), g, T, C, lens, emis, stride, w, alpha, offs, grad,
+                       grad_stride, wgrad);
+  return launch_clusters(ctx, "sparse_cl_den_backward", sparse_cl_den_backward_kernel, B, sp.N,
+                         sparse_cl_bwd_smem_floats(g.S, C, sp.N, sp.own_out), g, sp, T, C, lens, emis, stride, w,
+                         alpha, offs, grad, grad_stride, wgrad);
 }
 
 int launch_sparse_sigma(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_t* grp_arc, const float* w,
@@ -1667,81 +1642,18 @@ int launch_sparse_fold(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32
   return GTNB_OK;
 }
 
-int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, int B, int T, int C, const int32_t* lens,
-                          const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
-                          float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
+int launch_sparse_viterbi(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
+                          const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
+                          int32_t* head, float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
   if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_viterbi_forward_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_vit_smem_floats(g.S, C);
-  GTNB_LAUNCH(ctx, "sparse_viterbi_forward", sparse_viterbi_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      g, T, C, lens, emis, stride, w, bp, head, score, status));
-  GTNB_LAUNCH(ctx, "sparse_viterbi_trace", sparse_viterbi_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256),
-                                                                         256, 0, ctx->stream>>>(
-      g, B, T, lens, bp, head, paths, arcs, status));
-  return GTNB_OK;
-}
-
-namespace {
-
-/* B clusters of N CTAs of kSparseThreads threads; attr: the caller's, alive until the launch */
-cudaLaunchConfig_t cluster_config(gtnb_ctx* ctx, int B, int N, size_t smem, cudaLaunchAttribute* attr) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(B * N), 1, 1);
-  cfg.blockDim = dim3(kSparseThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = ctx->stream;
-  attr->id = cudaLaunchAttributeClusterDimension;
-  attr->val.clusterDim.x = (unsigned)N;
-  attr->val.clusterDim.y = 1;
-  attr->val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cfg;
-}
-
-} // namespace
-
-int launch_sparse_cl_den_forward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
-                                 const int32_t* lens, const float* emis, long long stride, const float* w,
-                                 float* alpha, double* offs, float* den, int32_t* status) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_den_forward_kernel)) return rc;
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg =
-      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_fwd_smem_floats(g.S, C, sp.N), &attr);
-  GTNB_LAUNCH(ctx, "sparse_cl_den_forward",
-              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_den_forward_kernel, g, sp, T, C, lens, emis, stride, w,
-                                                alpha, offs, den, status)));
-  return GTNB_OK;
-}
-
-int launch_sparse_cl_den_backward(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
-                                  const int32_t* lens, const float* emis, long long stride, const float* w,
-                                  const float* alpha, const double* offs, float* grad, long long grad_stride,
-                                  float* wgrad) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_den_backward_kernel)) return rc;
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg =
-      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_bwd_smem_floats(g.S, C, sp.N, sp.own_out), &attr);
-  GTNB_LAUNCH(ctx, "sparse_cl_den_backward",
-              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_den_backward_kernel, g, sp, T, C, lens, emis, stride,
-                                                w, alpha, (const double*)offs, grad, grad_stride, wgrad)));
-  return GTNB_OK;
-}
-
-int launch_sparse_cl_viterbi(gtnb_ctx* ctx, const SparseDev& g, const SparseSplit& sp, int B, int T, int C,
-                             const int32_t* lens, const float* emis, long long stride, const float* w, uint16_t* bp,
-                             int32_t* head, float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_viterbi_forward_kernel)) return rc;
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg = cluster_config(ctx, B, sp.N, sizeof(float) * sparse_vit_smem_floats(g.S, C), &attr);
-  GTNB_LAUNCH(ctx, "sparse_cl_viterbi_forward",
-              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_viterbi_forward_kernel, g, sp, T, C, lens, emis,
-                                                stride, w, bp, head, score, status)));
-  GTNB_LAUNCH(ctx, "sparse_viterbi_trace", sparse_viterbi_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256),
-                                                                         256, 0, ctx->stream>>>(
+  const long long floats = sparse_vit_smem_floats(g.S, C);
+  if (const int rc = sp.N == 1 ? launch_ctas(ctx, "sparse_viterbi_forward", sparse_viterbi_forward_kernel, B, floats, g,
+                                             T, C, lens, emis, stride, w, bp, head, score, status)
+                               : launch_clusters(ctx, "sparse_cl_viterbi_forward", sparse_cl_viterbi_forward_kernel, B,
+                                                 sp.N, floats, g, sp, T, C, lens, emis, stride, w, bp, head, score,
+                                                 status))
+    return rc;
+  GTNB_LAUNCH(ctx, "sparse_viterbi_trace", sparse_viterbi_trace_kernel<<<trace_blocks(B), 256, 0, ctx->stream>>>(
       g, B, T, lens, bp, head, paths, arcs, status));
   return GTNB_OK;
 }
@@ -1754,40 +1666,52 @@ int launch_sparse_tau(gtnb_ctx* ctx, int K, const int32_t* grp_ptr, const int32_
   return GTNB_OK;
 }
 
-int launch_sparse_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int B, int T, int C,
-                              const int32_t* lens, const float* emis, long long stride, const float* w, float* alpha,
-                              double* offs, float* den, int32_t* status) {
+int launch_sparse_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                              int per_cta, int max_S, int B, int T, int C, const int32_t* lens, const float* emis,
+                              long long stride, const float* w, float* alpha, double* offs, float* den,
+                              int32_t* status) {
   if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_forward_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_fwd_smem_floats(max_S, C);
-  GTNB_LAUNCH(ctx, "sparse_eps_forward", sparse_eps_forward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      gs, per_cta, T, C, lens, emis, stride, w, alpha, offs, den, status));
-  return GTNB_OK;
+  if (sp.N > 1 && per_cta)
+    return fail(ctx, GTNB_ERR_LOGIC, "launch_sparse_eps_forward: a cluster sweeps the denominator alone (per_cta 0)");
+  if (sp.N == 1)
+    return launch_ctas(ctx, "sparse_eps_forward", sparse_eps_forward_kernel, B, sparse_fwd_smem_floats(max_S, C), gs,
+                       per_cta, T, C, lens, emis, stride, w, alpha, offs, den, status);
+  return launch_clusters(ctx, "sparse_cl_eps_forward", sparse_cl_eps_forward_kernel, B, sp.N,
+                         sparse_cl_fwd_smem_floats(max_S, C, sp.N), gs, sp, cut, T, C, lens, emis, stride, w, alpha,
+                         offs, den, status);
 }
 
-int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, int per_cta, int max_S, int max_AE, int B,
-                               int T, int C, const int32_t* lens, const float* emis, long long stride, const float* w,
-                               const float* alpha, const double* offs, float sgn, float* grad, long long grad_stride,
-                               float* wgrad) {
+int launch_sparse_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
+                               int per_cta, int max_S, int max_AE, int B, int T, int C, const int32_t* lens,
+                               const float* emis, long long stride, const float* w, const float* alpha,
+                               const double* offs, float sgn, float* grad, long long grad_stride, float* wgrad) {
   if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_backward_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_bwd_smem_floats(max_S, max_AE, C);
-  GTNB_LAUNCH(ctx, "sparse_eps_backward", sparse_eps_backward_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      gs, per_cta, T, C, lens, emis, stride, w, alpha, offs, sgn, grad, grad_stride, wgrad));
-  return GTNB_OK;
+  if (sp.N > 1 && (per_cta || sgn != 1.0f))
+    return fail(ctx, GTNB_ERR_LOGIC,
+                "launch_sparse_eps_backward: a cluster sweeps the denominator alone (per_cta 0, sgn 1)");
+  if (sp.N == 1)
+    return launch_ctas(ctx, "sparse_eps_backward", sparse_eps_backward_kernel, B,
+                       sparse_bwd_smem_floats(max_S, max_AE, C), gs, per_cta, T, C, lens, emis, stride, w, alpha,
+                       offs, sgn, grad, grad_stride, wgrad);
+  return launch_clusters(ctx, "sparse_cl_eps_backward", sparse_cl_eps_backward_kernel, B, sp.N,
+                         sparse_cl_bwd_smem_floats(max_S, C, sp.N, sp.own_out), gs, sp, cut, T, C, lens, emis, stride,
+                         w, alpha, offs, grad, grad_stride, wgrad);
 }
 
-int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, int S, int B, int T, int C, const int32_t* lens,
-                              const float* emis, long long stride, const float* w, uint16_t* bp, int32_t* head,
-                              float* score, int32_t* paths, int32_t* arcs, int32_t* status) {
+int launch_sparse_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut, int S,
+                              int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
+                              const float* w, uint16_t* bp, int32_t* head, float* score, int32_t* paths, int32_t* arcs,
+                              int32_t* status) {
   if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_viterbi_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_vit_smem_floats(S, C);
-  GTNB_LAUNCH(ctx, "sparse_eps_viterbi", sparse_eps_viterbi_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      gs, T, C, lens, emis, stride, w, bp, head, score, status));
-  GTNB_LAUNCH(ctx, "sparse_eps_trace", sparse_eps_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0,
-                                                                 ctx->stream>>>(gs, B, T, lens, bp, head, paths, arcs,
-                                                                                status));
+  const long long floats = sparse_vit_smem_floats(S, C);
+  if (const int rc = sp.N == 1 ? launch_ctas(ctx, "sparse_eps_viterbi", sparse_eps_viterbi_kernel, B, floats, gs, T, C,
+                                             lens, emis, stride, w, bp, head, score, status)
+                               : launch_clusters(ctx, "sparse_cl_eps_viterbi", sparse_cl_eps_viterbi_kernel, B, sp.N,
+                                                 floats, gs, sp, cut, T, C, lens, emis, stride, w, bp, head, score,
+                                                 status))
+    return rc;
+  GTNB_LAUNCH(ctx, "sparse_eps_trace", sparse_eps_trace_kernel<<<trace_blocks(B), 256, 0, ctx->stream>>>(
+      gs, B, T, lens, bp, head, paths, arcs, status));
   return GTNB_OK;
 }
 
@@ -1796,13 +1720,11 @@ int launch_sparse_eps_align(gtnb_ctx* ctx, const SparseEpsDev* gs, int max_S, in
                             int32_t* head, float* score, const int32_t* arc_of, const int32_t* a_first,
                             int32_t* paths, int32_t* arcs, int32_t* status) {
   if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_eps_align_kernel)) return rc;
-  const size_t smem = sizeof(float) * sparse_vit_smem_floats(max_S, C);
-  GTNB_LAUNCH(ctx, "sparse_eps_align", sparse_eps_align_kernel<<<B, kSparseThreads, smem, ctx->stream>>>(
-      gs, C, lens, emis, stride, w, bp, head, score, status));
-  GTNB_LAUNCH(ctx, "sparse_eps_align_trace",
-              sparse_eps_align_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0, ctx->stream>>>(
-                  gs, B, T, lens, bp, head, arc_of, a_first, paths, arcs, status));
+  if (const int rc = launch_ctas(ctx, "sparse_eps_align", sparse_eps_align_kernel, B, sparse_vit_smem_floats(max_S, C),
+                                 gs, C, lens, emis, stride, w, bp, head, score, status))
+    return rc;
+  GTNB_LAUNCH(ctx, "sparse_eps_align_trace", sparse_eps_align_trace_kernel<<<trace_blocks(B), 256, 0, ctx->stream>>>(
+      gs, B, T, lens, bp, head, arc_of, a_first, paths, arcs, status));
   return GTNB_OK;
 }
 
@@ -1819,52 +1741,6 @@ int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const
   if (n == 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "sparse_eps_scatter", sparse_eps_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0,
                                                                      ctx->stream>>>(n, pg, arc_of, tidx, tgrad, agrad));
-  return GTNB_OK;
-}
-
-int launch_sparse_cl_eps_forward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
-                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
-                                 const float* w, float* alpha, double* offs, float* den, int32_t* status) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_eps_forward_kernel)) return rc;
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg =
-      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_fwd_smem_floats(S, C, sp.N), &attr);
-  GTNB_LAUNCH(ctx, "sparse_cl_eps_forward",
-              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_eps_forward_kernel, gs, sp, cut, T, C, lens, emis,
-                                                stride, w, alpha, offs, den, status)));
-  return GTNB_OK;
-}
-
-int launch_sparse_cl_eps_backward(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
-                                  int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
-                                  const float* w, const float* alpha, const double* offs, float* grad,
-                                  long long grad_stride, float* wgrad) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_eps_backward_kernel)) return rc;
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg =
-      cluster_config(ctx, B, sp.N, sizeof(float) * sparse_cl_bwd_smem_floats(S, C, sp.N, sp.own_out), &attr);
-  GTNB_LAUNCH(ctx, "sparse_cl_eps_backward",
-              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_eps_backward_kernel, gs, sp, cut, T, C, lens, emis,
-                                                stride, w, alpha, offs, grad, grad_stride, wgrad)));
-  return GTNB_OK;
-}
-
-int launch_sparse_cl_eps_viterbi(gtnb_ctx* ctx, const SparseEpsDev* gs, const SparseSplit& sp, const int32_t* cut,
-                                 int S, int B, int T, int C, const int32_t* lens, const float* emis, long long stride,
-                                 const float* w, uint16_t* bp, int32_t* head, float* score, int32_t* paths,
-                                 int32_t* arcs, int32_t* status) {
-  if (B == 0) return GTNB_OK;
-  if (const int rc = ensure_max_smem(ctx, (const void*)sparse_cl_eps_viterbi_kernel)) return rc;
-  cudaLaunchAttribute attr;
-  const cudaLaunchConfig_t cfg = cluster_config(ctx, B, sp.N, sizeof(float) * sparse_vit_smem_floats(S, C), &attr);
-  GTNB_LAUNCH(ctx, "sparse_cl_eps_viterbi",
-              GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, sparse_cl_eps_viterbi_kernel, gs, sp, cut, T, C, lens, emis,
-                                                stride, w, bp, head, score, status)));
-  GTNB_LAUNCH(ctx, "sparse_eps_trace", sparse_eps_trace_kernel<<<(unsigned)(((long long)B * 32 + 255) / 256), 256, 0,
-                                                                 ctx->stream>>>(gs, B, T, lens, bp, head, paths, arcs,
-                                                                                status));
   return GTNB_OK;
 }
 
