@@ -20,6 +20,9 @@ ERR_UNSUPPORTED = 5
 EPSILON = -1
 DENSE_ASG = 0  # gtnb_viterbi_dense_ex graph kinds
 DENSE_BIGRAM = 1
+F32 = 0  # gtnb_ctc_loss_ex element types
+BF16 = 1
+F16 = 2
 
 _f32p = C.POINTER(C.c_float)
 _i32p = C.POINTER(C.c_int32)
@@ -95,6 +98,8 @@ SYMBOLS = [
     ("gtnb_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int]),
+    ("gtnb_ctc_loss_ex", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _i32p, _i32p, C.c_int, _f32p, _vp]),
     ("gtnb_ngram_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int, _vp, C.c_int]),

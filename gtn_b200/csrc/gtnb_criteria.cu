@@ -308,12 +308,20 @@ struct HostGraph {
  * One attempt.  allow_implicit: sweep the frames without building the lattice (k_implicit.cu)
  * when the target graphs qualify; *needs_exact is set when that sweep met a non-finite weight,
  * in which case the outputs are not to be used and the caller repeats the call materialised.
+ * dtype: the element type of emissions and grads (GTNB_BF16 / GTNB_F16: both on the device).  16-bit buffers go to
+ * k_bidir.cu as they are when the batch takes it; otherwise the emissions are widened into float32 scratch, the
+ * float32 route runs on that, and its gradient is rounded into grads.
  */
 int ctc_loss_run(
-    CallScope& scope, int B, int T, int C, const float* emissions, int emissions_on_device,
+    CallScope& scope, int B, int T, int C, const void* emissions_in, int emissions_on_device,
     const int32_t* input_lens, const int32_t* targets, const int32_t* target_lens, int blank,
-    float* losses_host, float* grads, int grads_on_device, bool allow_implicit, bool* needs_exact) {
+    float* losses_host, void* grads_in, int grads_on_device, bool allow_implicit, bool* needs_exact,
+    int dtype = GTNB_F32) {
   gtnb_ctx* ctx = scope.ctx();
+  const bool half = dtype != GTNB_F32;
+  // float32: the caller's buffers; 16-bit: none yet (the route decides below)
+  const float* emissions = half ? nullptr : static_cast<const float*>(emissions_in);
+  float* grads = half ? nullptr : static_cast<float*>(grads_in);
   *needs_exact = false;
   PhaseClock pc;
   const long long per = (long long)T * C;
@@ -355,7 +363,7 @@ int ctc_loss_run(
   OutBuf g;
   // host emissions: the copy runs on a second stream while this one builds the target graphs and the
   // lattice structure (k_ctc.cu, compose alive / count / scan need no emissions)
-  GTNB_TRY(scope.borrow(emissions, emissions_on_device != 0, per * B, &e_dev));
+  if (!half) GTNB_TRY(scope.borrow(emissions, emissions_on_device != 0, per * B, &e_dev));
   if (grads) {
     GTNB_TRY(scope.output(grads, grads_on_device, per * B, &g));
     // with full-length utterances the normaliser's gradient overwrites every element
@@ -367,8 +375,29 @@ int ctc_loss_run(
   std::vector<long long> sgn, sga;
   gtnb_lattice*& lat = scope.lattice();
   GTNB_TRY(composed_alloc(ctx, B, dims.data(), B, 0, t.T(), C, e_dev, per, sgn, sga, &lat, implicit));
+  bool native = false; // 16-bit buffers read and written by k_bidir.cu in place
+  if (half) {
+    native = implicit && ctx->use_bidir && bidir_supported(lat, emissions_in, per, grads_in, per, dtype);
+    if (native) {
+      // the kernel reads elements of dtype through lat->emissions (only k_bidir.cu runs on this route; e_dev stays
+      // NULL, nothing reads float32 emissions)
+      lat->emissions = static_cast<const float*>(emissions_in);
+      if (grads_in && input_lens) GTNB_CUDA(ctx, cudaMemsetAsync(grads_in, 0, 2ull * per * B, ctx->stream));
+    } else {
+      float* wide = nullptr;
+      GTNB_TRY(scope.alloc(&wide, per * B));
+      GTNB_TRY(launch_widen(ctx, emissions_in, dtype, wide, per * B));
+      lat->emissions = e_dev = wide;
+      if (grads_in) {
+        GTNB_TRY(scope.alloc(&g.dev, per * B));
+        if (input_lens) GTNB_CUDA(ctx, cudaMemsetAsync(g.dev, 0, sizeof(float) * per * B, ctx->stream));
+        grads = g.dev;
+      }
+    }
+  }
   pc.mark("alloc+meta");
   // the whole criterion in one launch per sub-batch (k_bidir.cu) when the batch qualifies
+  // (native: true, the 16-bit envelope lies inside the float32 one and the buffers' alignment was checked above)
   const bool bidir = implicit && ctx->use_bidir && bidir_supported(lat, e_dev, per, g.dev, per);
   // PAIR kernels (graphs from the targets, one launch): everything small goes through MAPPED pinned memory --
   // the kernel reads the descriptors and targets in place and writes its results straight into the read-back
@@ -447,7 +476,10 @@ int ctc_loss_run(
     cudaEvent_t ev_setup = ctx->side_events[K], ev_lin = ctx->side_events[K + 1];
     const int32_t* T_dev = small_dev + tot_t + 2ll * B;
     GTNB_CUDA(ctx, cudaEventRecord(ev_setup, ctx->stream));
-    if (bidir && K == 1 && !h2d_event && !(grads && !grads_on_device)) {
+    if (native) {
+      GTNB_TRY(launch_bidir_ctc(ctx, lat, status_dev, zparts_dev, boff_dev, grads_in, per, 0, -1, bidir_scores_dev,
+                                blank, bidir_targets, bidir_targets + tot_t, direct ? meta_mapped : nullptr, dtype));
+    } else if (bidir && K == 1 && !h2d_event && !(grads && !grads_on_device)) {
       GTNB_TRY(launch_bidir_ctc(ctx, lat, status_dev, zparts_dev, boff_dev, g.dev, per, 0, -1, bidir_scores_dev,
                                 blank, bidir_targets, bidir_targets + tot_t, direct ? meta_mapped : nullptr));
     } else if (!bidir && K == 1 && !h2d_event && !(grads && !grads_on_device)) {
@@ -510,6 +542,8 @@ int ctc_loss_run(
     }
     GTNB_TRY(g.copy_out(ctx, per * B));
   }
+  // 16-bit, widened: the float32 gradient rounded into the caller's buffer
+  if (half && !native && grads_in) GTNB_TRY(launch_narrow(ctx, g.dev, grads_in, dtype, per * B));
   pc.mark("launches");
   const int zp = bidir ? 2 * bidir_zparts() : 1; // partial sums of forwardScore(emissions) per utterance
   GTNB_TRY(readback_reserve(ctx, (zp + 2) * sizeof(float) * B));
@@ -554,6 +588,25 @@ extern "C" int gtnb_ctc_loss(
   return with_exact_retry(scope, ctx->use_implicit, [&](bool implicit, bool* needs_exact) {
     return ctc_loss_run(scope, B, T, C, emissions, emissions_on_device, input_lens, targets, target_lens, blank,
                         losses_host, grads, grads_on_device, implicit, needs_exact);
+  });
+}
+
+extern "C" int gtnb_ctc_loss_ex(
+    gtnb_ctx* ctx, int B, int T, int C, const void* emissions_dev, int dtype, const int32_t* input_lens,
+    const int32_t* targets, const int32_t* target_lens, int blank, float* losses_host, void* grads_dev) {
+  if (dtype != GTNB_F32 && dtype != GTNB_BF16 && dtype != GTNB_F16)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctc_loss_ex: unknown dtype");
+  if (dtype == GTNB_F32)
+    return gtnb_ctc_loss(ctx, B, T, C, static_cast<const float*>(emissions_dev), 1, input_lens, targets, target_lens,
+                         blank, losses_host, static_cast<float*>(grads_dev), 1);
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions_dev || !target_lens || !losses_host)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctc_loss_ex: bad arguments");
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  CallScope scope(ctx);
+  return with_exact_retry(scope, ctx->use_implicit, [&](bool implicit, bool* needs_exact) {
+    return ctc_loss_run(scope, B, T, C, emissions_dev, 1, input_lens, targets, target_lens, blank, losses_host,
+                        grads_dev, 1, implicit, needs_exact, dtype);
   });
 }
 

@@ -318,14 +318,18 @@ bool implicit_trace_supported(const gtnb_lattice* lat);
 int launch_implicit_trace(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int32_t* paths, int32_t* arcs,
                           float* scores_out, int T_out);
 /* k_bidir.cu: the CTC criterion in one launch (two-CTA clusters meeting in the middle), normaliser included */
-bool bidir_supported(const gtnb_lattice* lat, const float* emissions, int64_t stride, const float* grad, int64_t grad_stride);
+/* dtype (GTNB_F32 / GTNB_BF16 / GTNB_F16): the element type of the emissions and the gradient, which launch_bidir_ctc
+ * reads and writes as they are (lat->emissions then points at elements of that type); 16-bit types need C % 8 == 0 */
+bool bidir_supported(const gtnb_lattice* lat, const void* emissions, int64_t stride, const void* grad, int64_t grad_stride,
+                     int dtype = GTNB_F32);
 int bidir_blocks(int max_T);
 int bidir_zparts(); // partial sums of forwardScore(emissions) per CTA
 int launch_bidir_ctc(
-    gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, float* grad_emis,
+    gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, void* grad_emis,
     int64_t grad_stride, int b0 = 0, int nb = -1, float* out_scores_dev = nullptr,
     int ctc_blank = -1, const int32_t* targets_dev = nullptr, const int32_t* tgt_off_dev = nullptr,
-    const GraphMeta* meta_src = nullptr); // meta_src: the descriptors somewhere else than lat->meta (mapped host memory)
+    const GraphMeta* meta_src = nullptr, // meta_src: the descriptors somewhere else than lat->meta (mapped host memory)
+    int dtype = GTNB_F32);
 // ctc_blank >= 0 + the targets: CTC target graphs, taken from the targets themselves (PAIR kernels)
 bool bidir_takes_targets(const gtnb_lattice* lat, int ctc_blank);
 /* k_order.cu (experimental): a composed lattice's rows and accept list in the order the reference's shortestPath relaxes / creates them */
@@ -448,6 +452,9 @@ int launch_sparse_eps_scatter(gtnb_ctx* ctx, long long n, const float* pg, const
 // kernels (k_compose.cu)
 int launch_compose(gtnb_ctx* ctx, gtnb_lattice* lat, cudaEvent_t emissions_ready = nullptr);
 int launch_compose_grad(gtnb_ctx* ctx, gtnb_lattice* lat, float* grad_graph, float* grad_emis, int64_t grad_stride);
+// kernels (k_cast.cu): n elements between 16-bit storage (GTNB_BF16 / GTNB_F16) and float32, rounding to nearest even
+int launch_widen(gtnb_ctx* ctx, const void* src, int dtype, float* dst, long long n);
+int launch_narrow(gtnb_ctx* ctx, const float* src, void* dst, int dtype, long long n);
 // kernels (k_linear.cu)
 int launch_linear_forward(
     gtnb_ctx* ctx, int B, const int32_t* T_dev, int maxT, int C, const float* emis, int64_t stride,

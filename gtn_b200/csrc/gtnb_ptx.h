@@ -10,6 +10,9 @@
  */
 #pragma once
 
+#include <cmath>
+#include <type_traits>
+
 #ifdef GTNB_HOST_EMU
 #include "gtn_b200.h"
 #include "gtnb_meta.h"
@@ -42,6 +45,20 @@ __device__ __forceinline__ float max_nan(float a, float b) {
 struct f32x2 {
   float x, y;
 };
+
+/* 16-bit emission elements (gtnb_ctc_loss_ex): storage only -- every kernel widens them to float32 on load
+ * (exactly) and rounds float32 results to them on store (to nearest, ties to even) */
+struct bf16_t {
+  uint16_t bits;
+};
+struct f16_t {
+  uint16_t bits;
+};
+
+/* bfloat16 is the upper half of a float32: widening is a shift */
+__device__ __forceinline__ float bf16_bits_f32(uint32_t h) {
+  return __int_as_float((int)(h << 16));
+}
 
 /* full-warp butterfly reductions: every lane gets the result */
 __device__ __forceinline__ float warp_max(float v) {
@@ -193,6 +210,51 @@ __device__ __forceinline__ unsigned cluster_rank() {
 }
 __device__ __forceinline__ void sts_cluster_f32(uint32_t addr, unsigned rank, float v) {
   *emu::cluster_shared_ptr<float>(addr, rank) = v;
+}
+
+/* 16-bit conversions: the float32 -> 16-bit ones round to nearest, ties to even, with overflow to inf, subnormal
+ * results and a quiet NaN (sign and leading payload bits kept), as cvt.rn does */
+__device__ __forceinline__ float f16_bits_f32(uint32_t h) {
+  const uint32_t s = (h & 0x8000u) << 16, e = (h >> 10) & 31u, m = h & 0x3ffu;
+  if (e == 0) return s ? -std::ldexp((float)m, -24) : std::ldexp((float)m, -24); // zero / subnormal
+  if (e == 31) return __int_as_float((int)(s | 0x7f800000u | (m << 13))); // inf / NaN
+  return __int_as_float((int)(s | ((e + 112u) << 23) | (m << 13)));
+}
+__device__ __forceinline__ uint32_t f32_bf16_bits(float v) {
+  const uint32_t x = (uint32_t)__float_as_int(v);
+  if ((x & 0x7fffffffu) > 0x7f800000u) return (x >> 16) | 0x40u; // NaN: quiet
+  return (x + 0x7fffu + ((x >> 16) & 1u)) >> 16;
+}
+__device__ __forceinline__ uint32_t f32_f16_bits(float v) {
+  const uint32_t x = (uint32_t)__float_as_int(v), s = (x >> 16) & 0x8000u, ax = x & 0x7fffffffu;
+  if (ax > 0x7f800000u) return s | 0x7e00u | ((ax >> 13) & 0x3ffu); // NaN: quiet
+  if (ax >= 0x477ff000u) return s | 0x7c00u; // |v| >= 65520 (the tie above 65504 goes to the even inf)
+  if (ax < 0x38800000u) { // below 2^-14: a subnormal result in units of 2^-24
+    if (ax <= 0x33000000u) return s; // <= 2^-25: 0 (2^-25 itself is the tie, to the even 0)
+    const uint32_t sh = 126u - (ax >> 23), m = (ax & 0x7fffffu) | 0x800000u;
+    uint32_t r = m >> sh;
+    const uint32_t rem = m & ((1u << sh) - 1u), half = 1u << (sh - 1u);
+    if (rem > half || (rem == half && (r & 1u))) r++;
+    return s | r;
+  }
+  const uint32_t r = ax - 0x38000000u; // exponent rebiased 127 -> 15
+  return s | ((r + 0xfffu + ((r >> 13) & 1u)) >> 13);
+}
+/* two fp16 of a 32-bit word, low half first */
+__device__ __forceinline__ f32x2 f16x2_bits_f32x2(uint32_t w) {
+  return f32x2{f16_bits_f32(w & 0xffffu), f16_bits_f32(w >> 16)};
+}
+/* 8 bytes to global memory: four 16-bit elements packed two per word, the first in the low half */
+__device__ __forceinline__ void stg_v2_b32(void* p, uint32_t a, uint32_t b) {
+  uint32_t* q = static_cast<uint32_t*>(p);
+  q[0] = a;
+  q[1] = b;
+}
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  return f32_bf16_bits(lo) | (f32_bf16_bits(hi) << 16);
+}
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+  return f32_f16_bits(lo) | (f32_f16_bits(hi) << 16);
 }
 
 __device__ __forceinline__ unsigned lanemask_lt() {
@@ -466,6 +528,47 @@ __device__ __forceinline__ void sts_cluster_f32(uint32_t addr, unsigned rank, fl
       : "memory");
 }
 
+/* ---- 16-bit conversions (round to nearest, ties to even) ---- */
+
+__device__ __forceinline__ float f16_bits_f32(uint32_t h) {
+  float y;
+  asm("{\n.reg .b16 t;\ncvt.u16.u32 t, %1;\ncvt.f32.f16 %0, t;\n}" : "=f"(y) : "r"(h));
+  return y;
+}
+__device__ __forceinline__ uint32_t f32_bf16_bits(float v) {
+  uint32_t r;
+  asm("{\n.reg .b16 t;\ncvt.rn.bf16.f32 t, %1;\ncvt.u32.u16 %0, t;\n}" : "=r"(r) : "f"(v));
+  return r;
+}
+__device__ __forceinline__ uint32_t f32_f16_bits(float v) {
+  uint32_t r;
+  asm("{\n.reg .b16 t;\ncvt.rn.f16.f32 t, %1;\ncvt.u32.u16 %0, t;\n}" : "=r"(r) : "f"(v));
+  return r;
+}
+/* two fp16 of a 32-bit word, low half first */
+__device__ __forceinline__ f32x2 f16x2_bits_f32x2(uint32_t w) {
+  f32x2 v;
+  asm("{\n.reg .b16 lo, hi;\nmov.b32 {lo, hi}, %2;\ncvt.f32.f16 %0, lo;\ncvt.f32.f16 %1, hi;\n}"
+      : "=f"(v.x), "=f"(v.y)
+      : "r"(w));
+  return v;
+}
+/* 8 bytes to global memory: four 16-bit elements packed two per word, the first in the low half */
+__device__ __forceinline__ void stg_v2_b32(void* p, uint32_t a, uint32_t b) {
+  asm volatile("st.global.v2.b32 [%0], {%1, %2};" ::"l"(p), "r"(a), "r"(b) : "memory");
+}
+/* one cvt for two floats: the first operand of cvt.rn.*x2 goes to the upper half */
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
 /* ---- special registers ---- */
 
 __device__ __forceinline__ unsigned lanemask_lt() {
@@ -480,6 +583,65 @@ __device__ __forceinline__ long long globaltimer() {
 }
 
 #endif // GTNB_HOST_EMU
+
+/* ---- elements of type E (float, bf16_t or f16_t) as float32: widened exactly on load, rounded to nearest even
+ * on store.  With E = float each is the float32 primitive itself. ---- */
+
+/* one element of a shared-memory stage */
+template <class E>
+__device__ __forceinline__ float lds_elem(uint32_t addr) {
+  if constexpr (std::is_same_v<E, bf16_t>)
+    return bf16_bits_f32(lds_u16(addr));
+  else if constexpr (std::is_same_v<E, f16_t>)
+    return f16_bits_f32(lds_u16(addr));
+  else
+    return lds_f32(addr);
+}
+/* four consecutive elements of a shared-memory stage: 16 bytes of float32, 8 bytes of a 16-bit type */
+template <class E>
+__device__ __forceinline__ float4 lds_elem4(uint32_t addr) {
+  if constexpr (std::is_same_v<E, float>) {
+    return lds_v4_f32(addr);
+  } else {
+    const int2 w = lds_v2_u32(addr);
+    if constexpr (std::is_same_v<E, bf16_t>) {
+      return make_float4(bf16_bits_f32((uint32_t)w.x & 0xffffu), __int_as_float(w.x & (int)0xffff0000u),
+                         bf16_bits_f32((uint32_t)w.y & 0xffffu), __int_as_float(w.y & (int)0xffff0000u));
+    } else {
+      const f32x2 a = f16x2_bits_f32x2((uint32_t)w.x), b = f16x2_bits_f32x2((uint32_t)w.y);
+      return make_float4(a.x, a.y, b.x, b.y);
+    }
+  }
+}
+/* four floats to global memory as E (16 or 8 bytes, aligned to that) */
+template <class E>
+__device__ __forceinline__ void stg_elem4(E* p, float4 v) {
+  if constexpr (std::is_same_v<E, bf16_t>)
+    stg_v2_b32(p, pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
+  else if constexpr (std::is_same_v<E, f16_t>)
+    stg_v2_b32(p, pack_f16x2(v.x, v.y), pack_f16x2(v.z, v.w));
+  else
+    stg_v4_f32(p, v);
+}
+/* one element in global memory, either way */
+template <class E>
+__device__ __forceinline__ float ldg_elem(const E* p) {
+  if constexpr (std::is_same_v<E, bf16_t>)
+    return bf16_bits_f32(p->bits);
+  else if constexpr (std::is_same_v<E, f16_t>)
+    return f16_bits_f32(p->bits);
+  else
+    return *p;
+}
+template <class E>
+__device__ __forceinline__ void stg_elem(E* p, float v) {
+  if constexpr (std::is_same_v<E, bf16_t>)
+    p->bits = (uint16_t)f32_bf16_bits(v);
+  else if constexpr (std::is_same_v<E, f16_t>)
+    p->bits = (uint16_t)f32_f16_bits(v);
+  else
+    *p = v;
+}
 
 /* natural-log exp / log1p on the SFU */
 __device__ __forceinline__ float fexp(float x) {

@@ -70,6 +70,12 @@
  * arc.  Requires: <= 224 graph nodes, in- and out-degree <= 3, one label per node, every arc weight 0 (the CTC
  * target graphs of gtnb_ctc_loss, its only caller), C a multiple of 4 and <= 128, 16-byte aligned emissions.
  * Anything else takes k_implicit.cu.
+ *
+ * Element type E (gtnb_ctc_loss_ex): the emissions and the gradient are float32, bfloat16 or fp16; only the edges
+ * change -- the TMA copies move kBlk * C * sizeof(E) bytes, the node warps widen their emission with one LDS.U16
+ * (bf16: a shift, fp16: a conversion), the helper warps load four labels as 8 bytes and store four rounded gradients
+ * as 8 bytes.  Scores, renormalisation, logsumexps, Z and posteriors stay float32, so a 16-bit call returns exactly
+ * the float32 kernel's result on the widened emissions, its gradient rounded to E.  16-bit needs C % 8 == 0.
  */
 #include <algorithm>
 
@@ -112,7 +118,7 @@ struct Layout {
   int total;
 };
 
-inline Layout make_layout(int C, int max_pitch) {
+inline Layout make_layout(int C, int max_pitch, int esize = 4) { // esize: bytes per emission element
   Layout L;
   int off = 0;
   auto take = [&](int bytes) {
@@ -121,7 +127,7 @@ inline Layout make_layout(int C, int max_pitch) {
     return at;
   };
   L.off_ring = take(2 * kRowF * 4);
-  L.e_stage_bytes = kBlk * C * 4;
+  L.e_stage_bytes = kBlk * C * esize;
   L.off_e = take(kSE * L.e_stage_bytes);
   L.o_stage_bytes = kBlk * max_pitch * 4;
   // the out-arc scratch of CTA B's set-up (cnt[256] + dst[768] + w[768]) aliases the score stages
@@ -148,14 +154,14 @@ struct Params {
   const int32_t* sg_in_src;
   const int32_t* sg_in_label;
   const float* sg_in_w;
-  const float* emissions;
+  const void* emissions; // [B][T][C] of the kernel's element type E
   float* saved; // [node_base + f * pitch + u]: alpha_{f+1} for f < M (written by A), beta_{f+1} for f >= M (by B)
                 // (PAIR kernels: label scores only, see pair_role)
   float* boff; // [utterance][2][nblk_cap][4]: the score offset in effect for the rows of each block, per CTA
   float* out_scores; // [B] forwardScore of the lattice (natural log)
   float* zparts; // [2B * kHelpers] forwardScore(emissions): the part each helper warp of the pair of CTAs summed
   int32_t* status; // [B] bit 0: a weight was not finite
-  float* grad; // [B][grad_stride] or NULL (loss only)
+  void* grad; // [B][grad_stride] of E, or NULL (loss only)
   long long grad_stride;
   int C;
   int nwn; // node warps in the launch (ceil(max nodes / 32))
@@ -240,9 +246,9 @@ __device__ __forceinline__ void fetch_block_adjust(S& st) {
 }
 
 /* strides of the per-level accesses: compile-time constants in the FX kernels */
-template <int NQ, bool FX>
+template <int NQ, bool FX, class E>
 struct Strd {
-  __device__ __forceinline__ static int c4(const NodeUni& un) { return FX ? 256 * NQ : un.c4; }
+  __device__ __forceinline__ static int c4(const NodeUni& un) { return FX ? 64 * (int)sizeof(E) * NQ : un.c4; }
   __device__ __forceinline__ static int p4(const NodeUni& un) { return FX ? 4 * kFixedPitch : un.p4; }
   __device__ __forceinline__ static int g4(const NodeUni& un) {
     return FX ? 4 * (kSlots * 64 * NQ + kFixedPitch) : un.g4;
@@ -254,11 +260,11 @@ struct Strd {
  * r: the level's row within the block, counted in the CTA's own direction from the row st.ea / st.oa / st.ga /
  * st.gs point at (a constant after unrolling: with FX every address is register + immediate).
  * last: the block's last level (publishes the maximum for the renormalisation) */
-template <int DIR, int PH, int NQ, bool FX>
+template <int DIR, int PH, int NQ, bool FX, class E>
 __device__ __forceinline__ void node_step(NodeState& st, const NodeUni& un, int r, bool last) {
-  using SD = Strd<NQ, FX>;
+  using SD = Strd<NQ, FX, E>;
   const int rr = DIR ? -r : r;
-  const float x = lds_f32(st.ea + (uint32_t)(rr * SD::c4(un)));
+  const float x = lds_elem<E>(st.ea + (uint32_t)(rr * SD::c4(un)));
   // every arc weight of the graph is 0 (ctc_build_kernel's CTC graphs): no adds
   const float v = lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2));
   // A: alpha_s = v + e[s-1][label(u)].  B: beta_s = v; what the predecessors read is beta_s + e[s-1][label(u)]
@@ -280,17 +286,17 @@ __device__ __forceinline__ void node_step(NodeState& st, const NodeUni& un, int 
 }
 
 /* n levels from the rows st.ea / st.oa / st.ga / st.gs point at; st.gs moves on, the others are set per block */
-template <int DIR, int PH, int NQ, bool FX>
+template <int DIR, int PH, int NQ, bool FX, class E>
 __device__ __forceinline__ void node_rows(NodeState& st, const NodeUni& un, int n) {
   // (a rolled loop with the last level peeled was slower on an earlier GPU target; not re-measured on the H100)
   if (n == kBlk) {
 #pragma unroll
-    for (int r = 0; r < kBlk; r++) node_step<DIR, PH, NQ, FX>(st, un, r, r == kBlk - 1);
+    for (int r = 0; r < kBlk; r++) node_step<DIR, PH, NQ, FX, E>(st, un, r, r == kBlk - 1);
   } else {
 #pragma unroll 1
-    for (int r = 0; r < n; r++) node_step<DIR, PH, NQ, FX>(st, un, r, r == n - 1);
+    for (int r = 0; r < n; r++) node_step<DIR, PH, NQ, FX, E>(st, un, r, r == n - 1);
   }
-  if (PH == 1) st.gs += (DIR ? -n : n) * Strd<NQ, FX>::pitch(un);
+  if (PH == 1) st.gs += (DIR ? -n : n) * Strd<NQ, FX, E>::pitch(un);
 }
 
 /* reduction over the node threads of the CTA (named barrier 1): max, then sum */
@@ -321,12 +327,12 @@ __device__ __forceinline__ float node_reduce_sum(float v, uint32_t red, int warp
  * level's posterior follows.  An utterance without any accepting path (Z = kNeg-like) gets Zh = +1e30,
  * which makes every posterior ex2(-huge) = 0.  `doth`: the partner's offset for this block.
  */
-template <int DIR, int NQ, bool FX>
+template <int DIR, int NQ, bool FX, class E>
 __device__ __forceinline__ void node_first_phase2(
     NodeState& st, const NodeUni& un, bool act, uint32_t red, int warp, int nwarps, float doth, bool last,
     float* z_out, uint32_t feas_a, uint32_t spare) {
-  using SD = Strd<NQ, FX>;
-  const float x = lds_f32(st.ea);
+  using SD = Strd<NQ, FX, E>;
+  const float x = lds_elem<E>(st.ea);
   st.ea += DIR ? -SD::c4(un) : SD::c4(un);
   const float v = lse3_log2(lds_f32(st.pc + st.so0), lds_f32(st.pc + st.so1), lds_f32(st.pc + st.so2));
   const float val = DIR == 0 ? v + fmaf(x, kLog2e, -st.adj) : v - st.adj;
@@ -402,11 +408,11 @@ __device__ __forceinline__ uint32_t bar_tbl_ready(uint32_t bars) {
  * direction is folded into per-thread base addresses up front, so that a block costs its levels plus a
  * few dozen instructions.
  */
-template <int DIR, int NQ, bool FX>
+template <int DIR, int NQ, bool FX, class E>
 __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool act, int nid) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   NodeUni un;
-  un.c4 = 4 * cx.C;
+  un.c4 = (int)sizeof(E) * cx.C;
   un.p4 = 4 * cx.pitch;
   un.g4 = 4 * cx.pg;
   un.pitch = cx.pitch;
@@ -417,7 +423,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
   const int arr1 = (warp == 0 && cx.want_g) ? 1 + kHelpers : 1;
   const int arr2 = (warp == 0 && !cx.want_g) ? 1 + kHelpers : 1;
   // first row of a FULL block in this direction
-  const uint32_t e_row0 = cx.e_base + cx.lab4 + (DIR ? (uint32_t)((kBlk - 1) * cx.C * 4) : 0u);
+  const uint32_t e_row0 = cx.e_base + cx.lab4 + (DIR ? (uint32_t)((kBlk - 1) * cx.C * (int)sizeof(E)) : 0u);
   int v = 0; // blocks visited
   if (DIR == 0) {
     // level 0: start nodes carry the implicit 0 (shortest.cpp:129-135)
@@ -430,7 +436,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       st.ea = e_row0 + (uint32_t)(s * cx.e_stage_bytes);
       if (v > 0) fetch_block_adjust(st);
       if (tid == 0) stg_f32(cx.boff_own + 4 * v, st.D);
-      node_rows<0, 1, NQ, FX>(st, un, kBlk); // A's phase-1 blocks are always full
+      node_rows<0, 1, NQ, FX, E>(st, un, kBlk); // A's phase-1 blocks are always full
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
     }
@@ -438,10 +444,10 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
     // level T: accept nodes carry 0; what the predecessors read is beta_T + e[T-1][label]
     const int j0 = cx.nblk - 1, n0 = min(kBlk, cx.T - kBlk * j0);
     mbar_wait(bar_e_full(cx.bars, 0), 0);
-    st.ea = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4) + cx.lab4;
+    st.ea = cx.e_base + (uint32_t)((n0 - 1) * cx.C * (int)sizeof(E)) + cx.lab4;
     if (tid == 0) stg_f32(cx.boff_own + 4 * j0, 0.0f);
     {
-      const float e2 = lds_f32(st.ea) * kLog2e;
+      const float e2 = lds_elem<E>(st.ea) * kLog2e;
       st.ea -= un.c4;
       const float val = (cx.fl[nid] & 2) ? 0.0f : kNeg;
       sts_f32(st.pc + st.u4, val + e2); // written to the row the first step READS
@@ -451,7 +457,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       stg_f32(st.gs, val);
       st.gs -= un.pitch;
     }
-    node_rows<1, 1, NQ, FX>(st, un, n0 - 1);
+    node_rows<1, 1, NQ, FX, E>(st, un, n0 - 1);
     __syncwarp();
     if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, 0), arr1);
     for (v = 1; v < cx.n_ph1; v++) {
@@ -460,7 +466,7 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
       st.ea = e_row0 + (uint32_t)(s * cx.e_stage_bytes);
       fetch_block_adjust(st);
       if (tid == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), st.D);
-      node_rows<1, 1, NQ, FX>(st, un, kBlk);
+      node_rows<1, 1, NQ, FX, E>(st, un, kBlk);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
     }
@@ -492,13 +498,13 @@ __device__ __forceinline__ void node_role(NodeState& st, const NodeCtx& cx, bool
     if (v > 0) fetch_block_adjust(st);
     const float doth = lds_f32(cx.od_base + 16u * so);
     if (v2 == 0) {
-      node_first_phase2<DIR, NQ, FX>(st, un, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
+      node_first_phase2<DIR, NQ, FX, E>(st, un, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
                                          DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.spare);
-      if (cx.want_g) node_rows<DIR, 2, NQ, FX>(st, un, nfr - 1);
+      if (cx.want_g) node_rows<DIR, 2, NQ, FX, E>(st, un, nfr - 1);
     } else {
       // offsets moved since the meeting level: all integers, the differences are exact
       st.zsub = st.Zl - ((st.D + doth) - st.Dc);
-      node_rows<DIR, 2, NQ, FX>(st, un, nfr);
+      node_rows<DIR, 2, NQ, FX, E>(st, un, nfr);
     }
     __syncwarp();
     if (lane == 0) {
@@ -555,12 +561,12 @@ struct PairState {
   bool skip; // A: label 2t-1 has the skip in-arc; B: label 2t+1 has it (= this thread's label has the skip out-arc)
 };
 
-template <int DIR, int PH, int NQ>
+template <int DIR, int PH, int NQ, class E>
 __device__ __forceinline__ void pair_step(PairState& ps, const NodeUni& un, int r, bool last) {
-  using SD = Strd<NQ, true>;
+  using SD = Strd<NQ, true, E>;
   const int rr = DIR ? -r : r;
-  const float xl = lds_f32(ps.ea_l + (uint32_t)(rr * SD::c4(un)));
-  const float xb = lds_f32(ps.ea_b + (uint32_t)(rr * SD::c4(un)));
+  const float xl = lds_elem<E>(ps.ea_l + (uint32_t)(rr * SD::c4(un)));
+  const float xb = lds_elem<E>(ps.ea_b + (uint32_t)(rr * SD::c4(un)));
   float vl, vb;
   if (DIR == 0) {
     const f32x2 pv = lds_v2_f32(ps.pc + ps.t8); // pair t-1: (label 2t-3, blank 2t-2)
@@ -594,25 +600,25 @@ __device__ __forceinline__ void pair_step(PairState& ps, const NodeUni& un, int 
   ps.qc = t;
 }
 
-template <int DIR, int PH, int NQ>
+template <int DIR, int PH, int NQ, class E>
 __device__ __forceinline__ void pair_rows(PairState& ps, const NodeUni& un, int n) {
   if (n == kBlk) {
 #pragma unroll
-    for (int r = 0; r < kBlk; r++) pair_step<DIR, PH, NQ>(ps, un, r, r == kBlk - 1);
+    for (int r = 0; r < kBlk; r++) pair_step<DIR, PH, NQ, E>(ps, un, r, r == kBlk - 1);
   } else {
 #pragma unroll 1
-    for (int r = 0; r < n; r++) pair_step<DIR, PH, NQ>(ps, un, r, r == n - 1);
+    for (int r = 0; r < n; r++) pair_step<DIR, PH, NQ, E>(ps, un, r, r == n - 1);
   }
 }
 
 /* the first level of phase 2 (see node_first_phase2): Z over BOTH nodes of every pair; ob: the partner's blank
  * score of this pair at this level */
-template <int DIR, int NQ>
+template <int DIR, int NQ, class E>
 __device__ __forceinline__ void pair_first_phase2(
     PairState& ps, const NodeUni& un, bool act_l, bool act_b, uint32_t red, int warp, int nwarps, float doth, bool last,
     float* z_out, uint32_t feas_a, bool want_g, uint32_t ob) {
-  using SD = Strd<NQ, true>;
-  const float xl = lds_f32(ps.ea_l), xb = lds_f32(ps.ea_b);
+  using SD = Strd<NQ, true, E>;
+  const float xl = lds_elem<E>(ps.ea_l), xb = lds_elem<E>(ps.ea_b);
   ps.ea_l += DIR ? -SD::c4(un) : SD::c4(un);
   ps.ea_b += DIR ? -SD::c4(un) : SD::c4(un);
   float vl, vb;
@@ -663,11 +669,11 @@ __device__ __forceinline__ void pair_first_phase2(
 }
 
 /* the pair warps of one CTA, both phases: node_role's protocol (stages, barriers, offsets) on pairs */
-template <int DIR, int NQ>
+template <int DIR, int NQ, class E>
 __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int tp, bool act, bool has_label) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   NodeUni un;
-  un.c4 = 4 * cx.C;
+  un.c4 = (int)sizeof(E) * cx.C;
   un.p4 = 4 * cx.pitch;
   un.g4 = 4 * cx.pg;
   un.pitch = cx.pitch;
@@ -675,7 +681,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
   const int nact = un.nact;
   const int arr1 = (warp == 0 && cx.want_g) ? 1 + kHelpers : 1;
   const int arr2 = (warp == 0 && !cx.want_g) ? 1 + kHelpers : 1;
-  const uint32_t dir_off = DIR ? (uint32_t)((kBlk - 1) * cx.C * 4) : 0u;
+  const uint32_t dir_off = DIR ? (uint32_t)((kBlk - 1) * cx.C * (int)sizeof(E)) : 0u;
   const uint32_t e_row0_l = cx.e_base + cx.lab4 + dir_off; // cx.lab4: this thread's label
   const uint32_t e_row0_b = cx.e_base + cx.blank4 + dir_off;
   const bool act_l = act && has_label;
@@ -698,7 +704,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       ps.gs = label_at(v);
       if (v > 0) fetch_block_adjust(ps);
       if (tid == 0) stg_f32(cx.boff_own + 4 * v, ps.D);
-      pair_rows<0, 1, NQ>(ps, un, kBlk);
+      pair_rows<0, 1, NQ, E>(ps, un, kBlk);
       if (v == cx.n_ph1 - 1) stg_f32(label_at(v) + kBlk * kHalfPitch, ps.lastb);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -707,11 +713,11 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     // level T: accept nodes carry 0; what the predecessors read is beta_T + e[T-1][label]
     const int j0 = cx.nblk - 1, n0 = min(kBlk, cx.T - kBlk * j0);
     mbar_wait(bar_e_full(cx.bars, 0), 0);
-    ps.ea_l = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4) + cx.lab4;
-    ps.ea_b = cx.e_base + (uint32_t)((n0 - 1) * cx.C * 4) + cx.blank4;
+    ps.ea_l = cx.e_base + (uint32_t)((n0 - 1) * cx.C * (int)sizeof(E)) + cx.lab4;
+    ps.ea_b = cx.e_base + (uint32_t)((n0 - 1) * cx.C * (int)sizeof(E)) + cx.blank4;
     if (tid == 0) stg_f32(cx.boff_own + 4 * j0, 0.0f);
     {
-      const float el = lds_f32(ps.ea_l) * kLog2e, eb = lds_f32(ps.ea_b) * kLog2e;
+      const float el = lds_elem<E>(ps.ea_l) * kLog2e, eb = lds_elem<E>(ps.ea_b) * kLog2e;
       ps.ea_l -= un.c4;
       ps.ea_b -= un.c4;
       const float val_l = (has_label && (ctc_flags(2 * tp - 1, cx.N1) & 2)) ? 0.0f : kNeg;
@@ -726,7 +732,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       stg_f32(ps.gs, val_l);
       ps.gs -= kHalfPitch;
     }
-    pair_rows<1, 1, NQ>(ps, un, n0 - 1);
+    pair_rows<1, 1, NQ, E>(ps, un, n0 - 1);
     if (cx.n_ph1 == 1) stg_f32(label_at(j0) + n0 * kHalfPitch, ps.lastb);
     __syncwarp();
     if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, 0), arr1);
@@ -738,7 +744,7 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
       ps.gs = label_at(cx.nblk - 1 - v) + (kBlk - 1) * kHalfPitch;
       fetch_block_adjust(ps);
       if (tid == 0) stg_f32(cx.boff_own + 4 * (cx.nblk - 1 - v), ps.D);
-      pair_rows<1, 1, NQ>(ps, un, kBlk);
+      pair_rows<1, 1, NQ, E>(ps, un, kBlk);
       if (v == cx.n_ph1 - 1) stg_f32(label_at(cx.nblk - 1 - v) + kBlk * kHalfPitch, ps.lastb);
       __syncwarp();
       if (lane == 0) mbar_arrive_n(bar_e_empty(cx.bars, s), arr1);
@@ -772,12 +778,12 @@ __device__ __forceinline__ void pair_role(PairState& ps, const NodeCtx& cx, int 
     if (v2 == 0) {
       // the meeting row's blank scores follow the block's nfr label rows (B reads row kBlk - 1, A row 0)
       const uint32_t ob = ps.oa + (uint32_t)((DIR ? 1 : nfr) * kHalfPitch * 4);
-      pair_first_phase2<DIR, NQ>(ps, un, act_l, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
+      pair_first_phase2<DIR, NQ, E>(ps, un, act_l, act, cx.red_a, warp, cx.nw_act, doth, nfr == 1,
                                  DIR == 0 ? cx.out_score : nullptr, cx.feas_a, cx.want_g, ob);
-      if (cx.want_g) pair_rows<DIR, 2, NQ>(ps, un, nfr - 1);
+      if (cx.want_g) pair_rows<DIR, 2, NQ, E>(ps, un, nfr - 1);
     } else {
       ps.zsub = ps.Zl - ((ps.D + doth) - ps.Dc);
-      pair_rows<DIR, 2, NQ>(ps, un, nfr);
+      pair_rows<DIR, 2, NQ, E>(ps, un, nfr);
     }
     __syncwarp();
     if (lane == 0) {
@@ -838,17 +844,17 @@ struct HelperConst {
   uint32_t ovf; // byte offset of the row's overflow area
 };
 
-template <int NQ, bool WANT_G>
+template <int NQ, bool WANT_G, class E>
 __device__ __forceinline__ void helper_block(
     HelperState& hs, const HelperConst<NQ>& k, int nfr, uint32_t estage, uint32_t e_empty_bar, uint32_t gblock,
-    uint32_t g_empty_bar, int nheavy, bool has_comp, uint32_t feas_a, float* gout) {
+    uint32_t g_empty_bar, int nheavy, bool has_comp, uint32_t feas_a, E* gout) {
   const bool row_on = hs.r < nfr;
   float4 x[NQ];
   float mx = -3.0e38f;
 #pragma unroll
   for (int i = 0; i < NQ; i++) {
     const bool ok = row_on && k.eoff[i] != 0xffffffffu;
-    x[i] = ok ? lds_v4_f32(estage + k.eoff[i]) : make_float4(-3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f);
+    x[i] = ok ? lds_elem4<E>(estage + k.eoff[i]) : make_float4(-3.0e38f, -3.0e38f, -3.0e38f, -3.0e38f);
     const float hi = fmaxf(fmaxf(x[i].x, x[i].y), fmaxf(x[i].z, x[i].w));
     const float lo = fminf(fminf(x[i].x, x[i].y), fminf(x[i].z, x[i].w));
     const float nan_probe = (x[i].x + x[i].y) + (x[i].z + x[i].w); // fmaxf / fminf drop NaNs, a sum keeps them
@@ -908,7 +914,7 @@ __device__ __forceinline__ void helper_block(
           for (int j = 0; j < 4; j++) {
             const int s1 = (k.hsel[i] >> (4 * j)) & 15;
             if (s1 == 15) { // beyond the cooperative slots: this lane sums the label's positions itself
-              const uint32_t w = lds_u32(hs.seg + 4u * (uint32_t)((k.eoff[i] >> 2) - hs.r * hs.C + j));
+              const uint32_t w = lds_u32(hs.seg + 4u * (uint32_t)(k.eoff[i] / (uint32_t)sizeof(E) - hs.r * hs.C + j));
               const int len = (w >> 10) & 1023;
               const uint32_t p = gblock + k.ovf + (w & 1023u) * 4u;
               float acc = 0.0f;
@@ -938,8 +944,9 @@ __device__ __forceinline__ void helper_block(
     for (int i = 0; i < NQ; i++) {
       if (row_on && k.eoff[i] != 0xffffffffu) {
         // d(forwardScore(e) - forwardScore(lattice)) / d e[f][c] = softmax - posterior mass on label c
-        stg_v4_f32(gout + (k.eoff[i] >> 2), make_float4(fmaf(x[i].x, inv, -o[4 * i + 0]), fmaf(x[i].y, inv, -o[4 * i + 1]),
-                                                    fmaf(x[i].z, inv, -o[4 * i + 2]), fmaf(x[i].w, inv, -o[4 * i + 3])));
+        stg_elem4(gout + k.eoff[i] / (uint32_t)sizeof(E),
+                  make_float4(fmaf(x[i].x, inv, -o[4 * i + 0]), fmaf(x[i].y, inv, -o[4 * i + 1]),
+                              fmaf(x[i].z, inv, -o[4 * i + 2]), fmaf(x[i].w, inv, -o[4 * i + 3])));
       }
     }
     __syncwarp();
@@ -954,13 +961,13 @@ __device__ __forceinline__ void helper_block(
  * cooperative label {label, overflow start in floats, nodes} in shared memory.  About a third of the generic
  * version's instructions.
  */
-template <int NQ>
+template <int NQ, class E>
 __device__ __forceinline__ void helper_block_fast(
     HelperState& hs, uint32_t ea, uint32_t e_empty_bar, uint32_t ga, uint32_t ovf_row, uint32_t htab, int nheavy,
-    bool has_comp, int comp_rel, uint32_t feas_a, uint32_t g_empty_bar, float* gout) {
+    bool has_comp, int comp_rel, uint32_t feas_a, uint32_t g_empty_bar, E* gout) {
   float4 x[NQ];
 #pragma unroll
-  for (int i = 0; i < NQ; i++) x[i] = lds_v4_f32(ea + 256u * i); // chunk i: labels 64 i + 4 l16 .. + 3
+  for (int i = 0; i < NQ; i++) x[i] = lds_elem4<E>(ea + 64u * (uint32_t)sizeof(E) * i); // chunk i: labels 64 i + 4 l16 .. + 3
   __syncwarp();
   if (hs.lane == 0) mbar_arrive(e_empty_bar); // the emission rows are in registers
   float mx = fmaxf(fmaxf(x[0].x, x[0].y), fmaxf(x[0].z, x[0].w));
@@ -1032,7 +1039,7 @@ __device__ __forceinline__ void helper_block_fast(
   for (int i = 0; i < NQ; i++) {
     const float4 gr = make_float4(fmaf(x[i].x, inv, -o[4 * i + 0]), fmaf(x[i].y, inv, -o[4 * i + 1]),
                                   fmaf(x[i].z, inv, -o[4 * i + 2]), fmaf(x[i].w, inv, -o[4 * i + 3]));
-    stg_v4_f32(gout + 64 * i, gr);
+    stg_elem4(gout + 64 * i, gr);
   }
   __syncwarp();
   if (hs.lane == 0) mbar_arrive(g_empty_bar); // this warp is done with the posterior block
@@ -1043,7 +1050,8 @@ __device__ __forceinline__ void helper_block_fast(
 /* ------------------------------------------------------------------ */
 
 /* MODE 0: one node per thread (any graph in the envelope); 1: PAIR (CTC graphs, two nodes per thread) */
-template <int NQ, bool FX, int MODE>
+/* E: the element type of the emissions and of the gradient (float, bf16_t or f16_t); everything in between is float32 */
+template <int NQ, bool FX, int MODE, class E = float>
 __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWarps) + 1 + kHelpers), 4)
     bidir_ctc_kernel(const Params P) {
   constexpr bool PAIR = MODE == 1;
@@ -1120,7 +1128,7 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
   const int32_t* is = P.sg_in_src + m.sg_arc_base;
   const int32_t* il = P.sg_in_label + m.sg_arc_base;
   const float* iw = P.sg_in_w + m.sg_arc_base;
-  const float* em = P.emissions + m.emis_off;
+  const E* em = static_cast<const E*>(P.emissions) + m.emis_off;
   float* saved = P.saved + m.node_base;
 
   // B: the out-arcs of every node, gathered from the in-arc tables (scratch aliases the score stages)
@@ -1192,8 +1200,8 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
     cx.perm_a = perm_a;
     cx.red_a = red_a;
     cx.spare = 0;
-    cx.lab4 = 4u * (uint32_t)labn;
-    cx.blank4 = 4u * (uint32_t)P.ctc_blank;
+    cx.lab4 = (uint32_t)sizeof(E) * (uint32_t)labn;
+    cx.blank4 = (uint32_t)sizeof(E) * (uint32_t)P.ctc_blank;
     cx.feas_a = hlist_a + 96u;
     cx.e_stage_bytes = L.e_stage_bytes;
     cx.o_stage_bytes = L.o_stage_bytes;
@@ -1209,9 +1217,9 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
     cx.nw_act = nw_act;
     cx.want_g = want_g;
     if (dir == 0)
-      pair_role<0, NQ>(ps, cx, tp, act, has_label);
+      pair_role<0, NQ, E>(ps, cx, tp, act, has_label);
     else
-      pair_role<1, NQ>(ps, cx, tp, act, has_label);
+      pair_role<1, NQ, E>(ps, cx, tp, act, has_label);
     if (T == 0 && dir == 0 && tid == 0) {
       int n = 0;
       for (int i = 0; i < N1; i++) n += (ctc_flags(i, N1) & 3) == 3;
@@ -1273,7 +1281,7 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
     st.ea = st.oa = 0;
     st.ga = spare;
     st.redi = redi_a;
-    const uint32_t lab4 = 4u * (uint32_t)labn;
+    const uint32_t lab4 = (uint32_t)sizeof(E) * (uint32_t)labn;
 
     NodeCtx cx;
     cx.fl = fl;
@@ -1305,9 +1313,9 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
     cx.nw_act = nw_act;
     cx.want_g = want_g;
     if (dir == 0)
-      node_role<0, NQ, FX>(st, cx, act, nid);
+      node_role<0, NQ, FX, E>(st, cx, act, nid);
     else
-      node_role<1, NQ, FX>(st, cx, act, nid);
+      node_role<1, NQ, FX, E>(st, cx, act, nid);
     if (bad) *(volatile int32_t*)&P.status[b] = 1; // (every writer stores the same 1: no atomic needed)
     if (T == 0 && dir == 0 && tid == 0) {
       // no frames: the lattice is the graph's start-and-accept nodes, each with score 0
@@ -1336,7 +1344,7 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
       const int s = v % kSE, j = block_of(v);
       if (lane == 0) {
         if (v >= kSE) mbar_wait_suspend(e_empty(s), ((v / kSE) - 1) & 1);
-        const uint32_t bytes = (uint32_t)(rows_of(j) * C * 4);
+        const uint32_t bytes = (uint32_t)(rows_of(j) * C * (int)sizeof(E));
         mbar_expect_tx(e_full(s), bytes);
         bulk_g2s(e_base + (uint32_t)(s * L.e_stage_bytes), em + (long long)j * kBlk * C, bytes, e_full(s));
       }
@@ -1439,7 +1447,7 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
 #pragma unroll
   for (int i = 0; i < NQ; i++) {
     const int c = 4 * (hs.l16 + 16 * i);
-    hk.eoff[i] = c < C ? (uint32_t)(hs.r * C + c) * 4u : 0xffffffffu;
+    hk.eoff[i] = c < C ? (uint32_t)(hs.r * C + c) * (uint32_t)sizeof(E) : 0xffffffffu;
     hk.goff[i] = (uint32_t)(hs.r * L.pg + kSlots * c) * 4u;
     hk.hsel[i] = 0;
     if (want_g && c < C)
@@ -1461,7 +1469,7 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
     for (; v < n_ph1; v++) {
       const int s = v % kSE;
       mbar_wait_suspend(e_full(s), (v / kSE) & 1);
-      helper_block<NQ, false>(hs, hk, rows_of(block_of(v)), e_base + (uint32_t)(s * L.e_stage_bytes), e_empty(s), 0, 0,
+      helper_block<NQ, false, E>(hs, hk, rows_of(block_of(v)), e_base + (uint32_t)(s * L.e_stage_bytes), e_empty(s), 0, 0,
                               0, false, 0, nullptr);
     }
   }
@@ -1483,8 +1491,9 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
     const bool has_comp = comp >= 0;
     const int comp_rel = has_comp ? comp - 4 * hs.l16 : -1000;
     const uint32_t feas_a = hlist_a + 96u;
-    const uint32_t f_e = (uint32_t)(hs.r * C + 4 * hs.l16) * 4u, f_g = (uint32_t)(hs.r * L.pg + kSlots * 4 * hs.l16) * 4u;
-    float* const f_out = P.grad + (long long)b * P.grad_stride + hs.r * C + 4 * hs.l16;
+    const uint32_t f_e = (uint32_t)(hs.r * C + 4 * hs.l16) * (uint32_t)sizeof(E), f_g = (uint32_t)(hs.r * L.pg + kSlots * 4 * hs.l16) * 4u;
+    E* const grad = static_cast<E*>(P.grad);
+    E* const f_out = grad + (long long)b * P.grad_stride + hs.r * C + 4 * hs.l16;
     for (int v2 = 0; v2 < n_ph2; v2++, v++) {
       const int s = v % kSE, sg = v2 % kSG, j = block_of(v);
       // the node warps arrive on g_full after they are through the block: its emission stage was
@@ -1492,13 +1501,13 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
       mbar_wait_suspend(g_full(sg), (v2 / kSG) & 1);
       if (fast && rows_of(j) == kBlk) {
         const uint32_t gb = g_base + (uint32_t)(sg * L.g_block_bytes);
-        helper_block_fast<NQ>(hs, e_base + (uint32_t)(s * L.e_stage_bytes) + f_e, e_empty(s), gb + f_g, gb + hk.ovf, htab,
+        helper_block_fast<NQ, E>(hs, e_base + (uint32_t)(s * L.e_stage_bytes) + f_e, e_empty(s), gb + f_g, gb + hk.ovf, htab,
                               nheavy, has_comp, comp_rel, feas_a, g_empty(sg), f_out + (long long)j * kBlk * C);
         continue;
       }
-      helper_block<NQ, true>(hs, hk, rows_of(j), e_base + (uint32_t)(s * L.e_stage_bytes), e_empty(s),
+      helper_block<NQ, true, E>(hs, hk, rows_of(j), e_base + (uint32_t)(s * L.e_stage_bytes), e_empty(s),
                              g_base + (uint32_t)(sg * L.g_block_bytes), g_empty(sg), nheavy, has_comp, feas_a,
-                             P.grad + (long long)b * P.grad_stride + (long long)j * kBlk * C);
+                             grad + (long long)b * P.grad_stride + (long long)j * kBlk * C);
     }
   }
   // forwardScore(emissions): the rows this warp summed
@@ -1514,9 +1523,13 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
 
 static_assert(bidir::kFixedPitch == kImplicitFixedPitch, "gtnb_compose_linear allocates the rows");
 
-/* true when every utterance of the batch qualifies for the bidirectional kernel */
-bool bidir_supported(const gtnb_lattice* lat, const float* emissions, int64_t stride, const float* grad, int64_t grad_stride) {
+/* true when every utterance of the batch qualifies for the bidirectional kernel with emissions and gradients of
+ * type dtype (GTNB_F32 / GTNB_BF16 / GTNB_F16).  16-bit elements need C % 8 == 0: every TMA row copy and every 8-byte
+ * access of the helper warps then stays a multiple of 16 / 8 bytes */
+bool bidir_supported(const gtnb_lattice* lat, const void* emissions, int64_t stride, const void* grad, int64_t grad_stride,
+                     int dtype) {
   if (!lat->composed || lat->C % 4 != 0 || lat->C > 128 || lat->C < 4) return false;
+  if (dtype != GTNB_F32 && lat->C % 8 != 0) return false;
   if (lat->max_lvl_nodes > 32 * bidir::kMaxNodeWarps || lat->max_in_deg > 3 || lat->max_out_deg > 3) return false;
   if (((uintptr_t)emissions & 15) || (stride & 3)) return false;
   if (grad && (((uintptr_t)grad & 15) || (grad_stride & 3))) return false;
@@ -1543,10 +1556,23 @@ int bidir_blocks(int max_T) {
 int bidir_zparts() {
   return bidir::kHelpers;
 }
+namespace {
+/* the instantiation launch_bidir_ctc runs for element type E */
+template <class E>
+void (*bidir_kernel_for(int mode, bool fx, int C))(const bidir::Params) {
+  if (mode == 1) return C == 64 ? bidir::bidir_ctc_kernel<1, true, 1, E> : bidir::bidir_ctc_kernel<2, true, 1, E>;
+  if (fx && C == 64) return bidir::bidir_ctc_kernel<1, true, 0, E>;
+  if (fx) return bidir::bidir_ctc_kernel<2, true, 0, E>;
+  if (C <= 64) return bidir::bidir_ctc_kernel<1, false, 0, E>;
+  return bidir::bidir_ctc_kernel<2, false, 0, E>;
+}
+} // namespace
+
 int launch_bidir_ctc(
-    gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, float* grad_emis,
+    gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, void* grad_emis,
     int64_t grad_stride, int b0, int nb, float* out_scores_dev, int ctc_blank, const int32_t* targets_dev,
-    const int32_t* tgt_off_dev, const GraphMeta* meta_src) {
+    const int32_t* tgt_off_dev, const GraphMeta* meta_src, int dtype) {
+  const int esize = dtype == GTNB_F32 ? 4 : 2;
   if (nb < 0) nb = lat->B - b0;
   if (nb <= 0) return GTNB_OK;
   bidir::Params P;
@@ -1563,7 +1589,7 @@ int launch_bidir_ctc(
   P.out_scores = (out_scores_dev ? out_scores_dev : lat->out_scores) + b0;
   P.zparts = zparts_dev + 2ll * b0 * bidir::kHelpers;
   P.status = status_dev + b0;
-  P.grad = grad_emis ? grad_emis + (long long)b0 * grad_stride : nullptr;
+  P.grad = grad_emis ? static_cast<char*>(grad_emis) + (long long)b0 * grad_stride * esize : nullptr;
   P.grad_stride = grad_stride;
   P.C = lat->C;
   P.nwn = std::max(1, (lat->max_lvl_nodes + 31) / 32);
@@ -1571,7 +1597,7 @@ int launch_bidir_ctc(
   // fixed pitch (gtnb_compose_linear, implicit lattices): compile-time strides in the node warps
   const bool fx = (lat->C == 64 || lat->C == 128) && lat->score_pitch == bidir::kFixedPitch;
   const int max_pitch = fx ? bidir::kFixedPitch : ((lat->max_lvl_nodes + 3) & ~3);
-  P.lay = bidir::make_layout(lat->C, max_pitch);
+  P.lay = bidir::make_layout(lat->C, max_pitch, esize);
   // NQ: float4 chunks of an emission row per helper lane
   // the graphs are ctc_build_kernel's (gtnb_ctc_loss): the PAIR kernels (two nodes per thread) unless
   // gtnb_ctx_set_flag("bidir_mode", 0) asks for one node per thread
@@ -1579,17 +1605,9 @@ int launch_bidir_ctc(
   const bool ctc_ok = bidir_takes_targets(lat, ctc_blank) && targets_dev;
   P.targets = targets_dev;
   const int mode = !ctc_ok || ctx->bidir_mode == 0 ? 0 : 1;
-  void (*kern)(const bidir::Params);
-  if (mode == 1)
-    kern = lat->C == 64 ? bidir::bidir_ctc_kernel<1, true, 1> : bidir::bidir_ctc_kernel<2, true, 1>;
-  else if (fx && lat->C == 64)
-    kern = bidir::bidir_ctc_kernel<1, true, 0>;
-  else if (fx)
-    kern = bidir::bidir_ctc_kernel<2, true, 0>;
-  else if (lat->C <= 64)
-    kern = bidir::bidir_ctc_kernel<1, false, 0>;
-  else
-    kern = bidir::bidir_ctc_kernel<2, false, 0>;
+  void (*kern)(const bidir::Params) = dtype == GTNB_BF16  ? bidir_kernel_for<bf16_t>(mode, fx, lat->C)
+                                      : dtype == GTNB_F16 ? bidir_kernel_for<f16_t>(mode, fx, lat->C)
+                                                          : bidir_kernel_for<float>(mode, fx, lat->C);
   if (mode == 1) P.nwn = std::max(1, ((lat->max_lvl_nodes + 1) / 2 + 31) / 32);
   P.ctc_blank = ctc_blank;
   if (P.lay.total > 48 * 1024) {

@@ -68,18 +68,29 @@ def _transition_backward(ctx, grad_output):
     return grad * grad_output.view(-1, 1, 1), tg * grad_output.flatten()[0]
 
 
+# the element types of ctc_loss's emissions, as gtnb_ctc_loss_ex names them
+_CTC_DTYPES = {torch.float32: capi.F32, torch.bfloat16: capi.BF16, torch.float16: capi.F16}
+
+
 class CTCLossFunction(torch.autograd.Function):
     """loss_b = forwardScore(e_b) - forwardScore(intersect(ctcGraph(target_b), e_b))  (benchmarks/ctc.cpp:150-158).
 
-    emissions: float32 CUDA tensor [B, T, C] (unnormalised scores are fine: the normaliser is part of the loss);
-    targets: list of 1-D int sequences; input_lengths: None (T frames each), a list or an int tensor (any device):
-    e_b is then the first input_lengths[b] frames, and the gradient of the padding frames is 0.  Returns the mean
-    loss over the batch (reduction="mean") or the [B] vector.
+    emissions: float32, bfloat16 or float16 CUDA tensor [B, T, C] (unnormalised scores are fine: the normaliser is
+    part of the loss); targets: list of 1-D int sequences; input_lengths: None (T frames each), a list or an int
+    tensor (any device): e_b is then the first input_lengths[b] frames, and the gradient of the padding frames is 0.
+    Returns the mean loss over the batch (reduction="mean") or the [B] vector, as float32 whatever the emissions'
+    dtype (under autocast torch's own ctc_loss runs in float32 too).
+
+    Half-precision emissions (bf16 / fp16 logits of a model under torch.autocast) go in as they are, through
+    gtnb_ctc_loss_ex: the losses are those of the float32 call on emissions.float(), bit for bit, and the gradient,
+    kept for backward and returned in the emissions' dtype, is that call's float32 gradient rounded to the dtype.
+    Nothing is upcast outside the call.
     """
 
     @staticmethod
     def forward(ctx, emissions, targets, blank=0, reduction="mean", input_lengths=None):
-        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        assert emissions.is_cuda and emissions.dim() == 3
+        assert emissions.dtype in _CTC_DTYPES, "ctc_loss: emissions must be float32, bfloat16 or float16"
         e = emissions.contiguous()
         B, T, Cn = e.shape
         stream = torch.cuda.current_stream(e.device).cuda_stream
@@ -88,11 +99,17 @@ class CTCLossFunction(torch.autograd.Function):
         il = _lengths(input_lengths, B)
         losses = np.zeros(B, np.float32)
         grad = torch.empty_like(e)  # (with input_lengths the call zeroes the padding rows)
-        g._check(capi.lib().gtnb_ctc_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p),
-            cat.ctypes.data_as(capi._i32p),
-            lens.ctypes.data_as(capi._i32p), int(blank), losses.ctypes.data_as(capi._f32p),
-            grad.data_ptr(), 1))
+        il_p = None if il is None else il.ctypes.data_as(capi._i32p)
+        if e.dtype == torch.float32:
+            g._check(capi.lib().gtnb_ctc_loss(
+                g.h, B, T, Cn, e.data_ptr(), 1, il_p,
+                cat.ctypes.data_as(capi._i32p),
+                lens.ctypes.data_as(capi._i32p), int(blank), losses.ctypes.data_as(capi._f32p),
+                grad.data_ptr(), 1))
+        else:
+            g._check(capi.lib().gtnb_ctc_loss_ex(
+                g.h, B, T, Cn, e.data_ptr(), _CTC_DTYPES[e.dtype], il_p, cat.ctypes.data_as(capi._i32p),
+                lens.ctypes.data_as(capi._i32p), int(blank), losses.ctypes.data_as(capi._f32p), grad.data_ptr()))
         out = torch.from_numpy(losses).to(e.device)
         ctx.save_for_backward(grad)
         ctx.reduction = reduction
@@ -105,7 +122,8 @@ class CTCLossFunction(torch.autograd.Function):
         if ctx.reduction == "mean":
             scale = grad_output / ctx.B
             return grad * scale, None, None, None, None
-        return grad * grad_output.view(-1, 1, 1), None, None, None, None
+        # (a 16-bit grad times the float32 [B] upstream gradient promotes to float32: back to the emissions' dtype)
+        return (grad * grad_output.view(-1, 1, 1)).to(grad.dtype), None, None, None, None
 
 
 def ctc_loss(emissions, targets, blank=0, reduction="mean", input_lengths=None):

@@ -353,6 +353,35 @@ int gtnb_ctc_loss(
     float* grads,
     int grads_on_device);
 
+#define GTNB_F32 0 /* float32 elements */
+#define GTNB_BF16 1 /* bfloat16 elements */
+#define GTNB_F16 2 /* IEEE half-precision elements */
+
+/*
+ * gtnb_ctc_loss on device buffers of a chosen element type: emissions_dev and grads_dev (nullable) are [B][T][C] of
+ * dtype (GTNB_F32, GTNB_BF16 or GTNB_F16), both on the device; losses_host [B] stays float32.  Targets, lengths,
+ * blank, infeasible targets, non-finite values and the zeroed rows t >= input_lens[b] follow gtnb_ctc_loss.
+ * The result is gtnb_ctc_loss's on the emissions widened to float32 (exact): the same losses, bit for bit, and its
+ * float32 gradient rounded to dtype (to nearest, ties to even).  Internally the arithmetic is float32 throughout:
+ * the one-launch kernel (k_bidir.cu) reads and writes the 16-bit buffers in place when the batch takes it, C % 8 == 0
+ * and both buffers are 16-byte aligned; any other batch is widened into float32 scratch once, run as gtnb_ctc_loss
+ * runs it, and its gradient rounded into grads_dev.  GTNB_F32 is gtnb_ctc_loss with both buffers on the device.
+ * An unknown dtype is GTNB_ERR_INVALID_ARGUMENT.
+ */
+int gtnb_ctc_loss_ex(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev,
+    int dtype,
+    const int32_t* input_lens, /* host, nullable */
+    const int32_t* targets,
+    const int32_t* target_lens,
+    int blank,
+    float* losses_host,
+    void* grads_dev); /* nullable */
+
 /*
  * ASG criterion for a whole minibatch (test/criterion_test.cpp:244-305, examples/asg.cpp:59-81,
  * BASELINE.json configs[2]):
