@@ -20,7 +20,7 @@ ERR_UNSUPPORTED = 5
 EPSILON = -1
 DENSE_ASG = 0  # gtnb_viterbi_dense_ex graph kinds
 DENSE_BIGRAM = 1
-F32 = 0  # gtnb_ctc_loss_ex element types
+F32 = 0  # element types of gtnb_ctc_loss_ex and the *_typed entry points
 BF16 = 1
 F16 = 2
 
@@ -106,6 +106,12 @@ SYMBOLS = [
     ("gtnb_asg_loss_ex", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, _f32p, _vp, C.c_int, _vp,
       C.c_int]),
+    ("gtnb_ngram_ctc_loss_typed", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, _i32p, _i32p, C.c_int, _f32p, _vp, _vp]),
+    ("gtnb_asg_loss_typed", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, _i32p, _i32p, _f32p, _vp, _vp]),
+    ("gtnb_viterbi_dense_typed", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.c_int, _vp, _vp, _vp]),
     ("gtnb_graph_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, _f32p, _vp, C.c_int,
       _vp, C.c_int]),

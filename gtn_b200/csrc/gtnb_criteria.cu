@@ -620,13 +620,15 @@ long long dense_trans_count(bool bigram, int C) { return (bigram ? 0 : (long lon
  * utterance through the factored kernel (k_dense.cu); the T*C*C lattice is never materialised.  Host transitions
  * and input_lens go up in one staged copy; device transitions are read where they are.  Outputs on the device are
  * written in place and the call returns once the work is enqueued; host outputs are copied back and waited for.
- * empty_score: the score of an utterance with T_b = 0.
+ * empty_score: the score of an utterance with T_b = 0.  dtype: the element type behind emissions (GTNB_BF16 / GTNB_F16:
+ * a device buffer of that type, which the kernel reads in place).
  * (the device scratch of a call comes from the context's call-scoped arena, as in gtnb_ctc_loss: no stream-ordered
  * allocations on the path after the first call of a shape)
  */
 int viterbi_dense_run(gtnb_ctx* ctx, const char* fn, int B, int T, int C, const float* emissions,
                       int emissions_on_device, const int32_t* input_lens, bool bigram, const float* trans_w,
-                      int trans_on_device, int32_t* paths, float* scores, int outputs_on_device, float empty_score) {
+                      int trans_on_device, int32_t* paths, float* scores, int outputs_on_device, float empty_score,
+                      int dtype = GTNB_F32) {
   if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions || !trans_w)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
   if (B == 0) return GTNB_OK;
@@ -651,7 +653,8 @@ int viterbi_dense_run(gtnb_ctx* ctx, const char* fn, int B, int T, int C, const 
   if (!trans_on_device) GTNB_TRY(stage_upload(ctx, tr_dev, trans_w, sizeof(float) * n_trans));
   if (input_lens) GTNB_TRY(stage_upload(ctx, T_dev, input_lens, sizeof(int32_t) * B));
   GTNB_TRY(stage_end(ctx));
-  GTNB_TRY(launch_viterbi_dense(ctx, B, T, C, bigram, T_dev, e_dev, per, tr_dev, empty_score, bp, paths_dev, sc_dev));
+  GTNB_TRY(launch_viterbi_dense(ctx, B, T, C, bigram, T_dev, e_dev, per, tr_dev, empty_score, bp, paths_dev, sc_dev,
+                                dtype));
   if (outputs_on_device) return GTNB_OK;
   if (paths && T > 0)
     GTNB_CUDA(ctx, cudaMemcpyAsync(paths, paths_dev, sizeof(int32_t) * (size_t)B * T, cudaMemcpyDeviceToHost,
@@ -686,6 +689,19 @@ extern "C" int gtnb_viterbi_dense_ex(
                            -std::numeric_limits<float>::infinity());
 }
 
+extern "C" int gtnb_viterbi_dense_typed(
+    gtnb_ctx* ctx, int B, int T, int C, const void* emissions_dev, int dtype, const int32_t* input_lens, int kind,
+    const float* trans_w_dev, int32_t* paths_dev, float* scores_dev) {
+  if (dtype != GTNB_F32 && dtype != GTNB_BF16 && dtype != GTNB_F16)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_viterbi_dense_typed: unknown dtype");
+  if (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_viterbi_dense_typed: unknown graph kind");
+  // (16-bit emissions travel in the float pointer; the kernel reads them as dtype)
+  return viterbi_dense_run(ctx, "gtnb_viterbi_dense_typed", B, T, C, static_cast<const float*>(emissions_dev), 1,
+                           input_lens, kind == GTNB_DENSE_BIGRAM, trans_w_dev, 1, paths_dev, scores_dev, 1,
+                           -std::numeric_limits<float>::infinity(), dtype);
+}
+
 namespace {
 
 /* the arguments of gtnb_ngram_ctc_loss, gtnb_asg_loss_ex and (host buffers, blank unused) gtnb_asg_loss */
@@ -704,7 +720,50 @@ struct TransitionArgs {
   int grads_on_device;
   float* trans_grad;
   int trans_grad_on_device;
+  // the element type behind emissions and grads: GTNB_F32, or (the _typed entry points) GTNB_BF16 / GTNB_F16 for
+  // device buffers of that type carried in these pointers, which only trellis_loss_fast and widened read
+  int dtype = GTNB_F32;
 };
+
+/* n floats on the call's stream, outside its arena: they outlive the scope's reopen() of an exact retry inside a
+ * route (asg_loss's), which hands the arena out afresh */
+struct StreamFloats {
+  gtnb_ctx* ctx;
+  float* p = nullptr;
+  int alloc(long long n) {
+    GTNB_CUDA(ctx, cudaMallocAsync((void**)&p, sizeof(float) * (size_t)std::max(n, 1ll), ctx->stream));
+    return GTNB_OK;
+  }
+  ~StreamFloats() {
+    if (p) cudaFreeAsync(p, ctx->stream);
+  }
+};
+
+/*
+ * A route that reads float32 emissions, run for a (a.dtype 16-bit: the emissions widened once into float32 by
+ * launch_widen, the route run on them with its gradient in float32, which launch_narrow then rounds into a.grads and
+ * the call waits for).  A float32 a goes to the route as it is.
+ */
+template <class Route>
+int widened(CallScope& scope, const TransitionArgs& a, Route&& route) {
+  if (a.dtype == GTNB_F32) return route(a);
+  gtnb_ctx* ctx = scope.ctx();
+  const long long n = (long long)a.B * a.T * a.C;
+  TransitionArgs w = a;
+  StreamFloats e{ctx}, g{ctx};
+  GTNB_TRY(e.alloc(n));
+  GTNB_TRY(launch_widen(ctx, a.emissions, a.dtype, e.p, n));
+  w.emissions = e.p;
+  w.dtype = GTNB_F32;
+  if (a.grads) {
+    GTNB_TRY(g.alloc(n));
+    w.grads = g.p;
+  }
+  GTNB_TRY(route(w));
+  if (!a.grads) return GTNB_OK;
+  GTNB_TRY(launch_narrow(ctx, w.grads, a.grads, a.dtype, n));
+  return scope.sync();
+}
 
 /*
  * gtnb_ngram_ctc_loss, gtnb_asg_loss_ex and gtnb_graph_loss after their argument checks: attempt(scope, fast,
@@ -961,6 +1020,7 @@ struct TrellisCriterion {
   decltype(&launch_ngram_den_forward) den_forward;
   decltype(&launch_ngram_den_backward) den_backward;
   float* alpha = nullptr;
+  int dtype = GTNB_F32; // the element type of the emissions the sweeps read (GTNB_F32 / GTNB_BF16 / GTNB_F16)
 
   /*
    * The interface of trellis_loss_fast's denominators: n_sigma (the folded start weights, 0 without a fold), alloc
@@ -974,11 +1034,11 @@ struct TrellisCriterion {
   int sigma(gtnb_ctx* ctx, int C, const float* w, float* sig) { return launch_ngram_sigma(ctx, C, w, sig); }
   int forward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
               float* den, int32_t* status) {
-    return den_forward(ctx, B, T, C, lens, e, per, w, alpha, den, status);
+    return den_forward(ctx, B, T, C, lens, e, per, w, alpha, den, status, dtype);
   }
   int backward(gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens, const float* e, long long per, const float* w,
                const float* den, float* grad, float* wgrad) {
-    return den_backward(ctx, B, T, C, lens, e, per, w, alpha, den, grad, per, wgrad);
+    return den_backward(ctx, B, T, C, lens, e, per, w, alpha, den, grad, per, wgrad, dtype);
   }
   int fold_grad(gtnb_ctx* ctx, int C, const float* w, const float* sig, float* wgrad) {
     return launch_ngram_fold(ctx, C, w, sig, wgrad);
@@ -1027,6 +1087,11 @@ struct TargetsNumerator {
   int scatter(CallScope&, const float*) { return GTNB_OK; }
 };
 
+/*
+ * 16-bit a (a.dtype, the native route; the denominator k reads the same type): both sweeps read the caller's emissions
+ * in place, add their gradients into float32 scratch as for float32, and narrow_kernel rounds that into a.grads once
+ * the streams have joined.
+ */
 template <class Numerator, class Denominator>
 int trellis_loss_fast(CallScope& scope, Denominator& k, const TransitionArgs& a, Numerator& num, bool* needs_exact) {
   gtnb_ctx* ctx = scope.ctx();
@@ -1034,6 +1099,7 @@ int trellis_loss_fast(CallScope& scope, Denominator& k, const TransitionArgs& a,
   const long long per = (long long)T * C;
   const long long n_sigma = k.n_sigma(C);
   const bool want = a.grads || a.trans_grad || num.wants_arc_grads();
+  const bool half = a.dtype != GTNB_F32;
   float *e_dev = nullptr, *w_dev = nullptr, *sigma = nullptr, *den = nullptr;
   float *ggrad = nullptr, *minus1 = nullptr;
   int32_t* status = nullptr;
@@ -1049,10 +1115,11 @@ int trellis_loss_fast(CallScope& scope, Denominator& k, const TransitionArgs& a,
   GTNB_TRY(k.alloc(scope, B, T));
   GTNB_TRY(scope.alloc(&den, B));
   GTNB_TRY(num.alloc(scope, e_dev, per, &lat));
+  if (half) lat->dtype = a.dtype; // (16-bit: the targets' numerators only, whose alloc makes the lattice)
   const long long tot_A = num.tot_A;
   if (want) {
     const long long n_grad = k.n_trans + n_sigma; // [d/dtrans | d/dsigma]
-    GTNB_TRY(scope.output(a.grads, a.grads_on_device, per * B, &g));
+    GTNB_TRY(scope.output(half ? nullptr : a.grads, a.grads_on_device, per * B, &g));
     GTNB_TRY(scope.output(a.trans_grad, a.trans_grad_on_device, n_grad, &tg, /*alias=*/!n_sigma));
     GTNB_TRY(scope.alloc(&ggrad, tot_A));
     GTNB_TRY(scope.alloc(&minus1, B));
@@ -1088,6 +1155,7 @@ int trellis_loss_fast(CallScope& scope, Denominator& k, const TransitionArgs& a,
     if (n_sigma) GTNB_TRY(k.fold_grad(ctx, C, w_dev, sigma, tg.dev));
     GTNB_TRY(num.scatter(scope, ggrad));
     GTNB_TRY(g.copy_out(ctx, per * B));
+    if (half && a.grads) GTNB_TRY(launch_narrow(ctx, g.dev, a.grads, a.dtype, per * B));
     GTNB_TRY(tg.copy_out(ctx, k.n_trans));
   }
   return read_losses(scope, B, den, lat->out_scores, status, 2ll * B, a.losses_host, needs_exact);
@@ -1238,39 +1306,70 @@ int asg_loss_generic(CallScope& scope, const TransitionArgs& a, const Targets& t
  *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(ctc_b, G), E_b))
  * G: C nodes, all start and accept, arc j -> i with label i and weight W[i*C + j].
  */
-extern "C" int gtnb_ngram_ctc_loss(
-    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
-    const float* trans_w, int trans_on_device, const int32_t* targets, const int32_t* target_lens, int blank,
-    float* losses_host, float* grads, int grads_on_device, float* trans_grad, int trans_grad_on_device) {
-  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, targets,
-                         target_lens, blank, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
-  if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions || !trans_w || !target_lens || !losses_host)
+namespace {
+
+/* gtnb_ngram_ctc_loss and gtnb_ngram_ctc_loss_typed: a.dtype's emissions on the native route, or widened */
+int ngram_ctc_loss_call(gtnb_ctx* ctx, const TransitionArgs& a) {
+  const int B = a.B, T = a.T, C = a.C;
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !a.emissions || !a.trans_w || !a.target_lens || !a.losses_host)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: bad arguments");
-  if (blank < 0 || blank >= C)
+  if (a.blank < 0 || a.blank >= C)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: blank outside [0, C)");
   if (C > kNgramMaxLabels)
     return fail(ctx, GTNB_ERR_UNSUPPORTED,
                 "gtnb_ngram_ctc_loss: C = " + std::to_string(C) + " labels; the trellis kernels hold W on chip for C <= " +
                     std::to_string(kNgramMaxLabels));
   Targets t;
-  GTNB_TRY(parse_targets(ctx, "gtnb_ngram_ctc_loss", B, T, C, input_lens, targets, target_lens, &t));
+  GTNB_TRY(parse_targets(ctx, "gtnb_ngram_ctc_loss", B, T, C, a.input_lens, a.targets, a.target_lens, &t));
   std::vector<SgDims> dims(B);
   for (int b = 0; b < B; b++) {
     if (!t.in_range[b]) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: label outside [0, C)");
     // folded numerator graph: S + 2U+1 CTC nodes; arcs = self loops + steps + skips + the two S arcs (one if U = 0)
-    const int L = 2 * target_lens[b] + 1;
+    const int L = 2 * a.target_lens[b] + 1;
     dims[b] = SgDims{L + 1, L + (L - 1) + t.skips[b] + std::min(L, 2), L >= 2 ? 2 : 1, /*all_valid=*/1,
                      /*uniform=*/1, /*max_in=*/3, /*max_out=*/3};
   }
   TrellisCriterion ngram{(long long)C * C, (long long)B * (T + 1) * C, /*fold=*/true, launch_ngram_den_forward,
                                launch_ngram_den_backward};
+  ngram.dtype = a.dtype;
   const bool fast = implicit_dims_supported(dims.data(), B) && ctx->use_implicit;
-  return run_criterion(ctx, B, t.T(), losses_host, trans_grad, trans_grad_on_device, (long long)C * C, fast,
+  return run_criterion(ctx, B, t.T(), a.losses_host, a.trans_grad, a.trans_grad_on_device, (long long)C * C, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
-                         if (!f) return ngram_ctc_loss_exact(scope, a, t);
-                         TargetsNumerator num{t, dims, C, launch_ngram_num_build, blank};
+                         if (!f)
+                           return widened(scope, a, [&](const TransitionArgs& w) {
+                             return ngram_ctc_loss_exact(scope, w, t);
+                           });
+                         TargetsNumerator num{t, dims, C, launch_ngram_num_build, a.blank};
                          return trellis_loss_fast(scope, ngram, a, num, needs_exact);
                        });
+}
+
+bool known_dtype(int dtype) { return dtype == GTNB_F32 || dtype == GTNB_BF16 || dtype == GTNB_F16; }
+
+} // namespace
+
+/*
+ * CTC with a learned bigram transition graph G (benchmarks/ctc.cpp:107-134, k_ngram.cu):
+ *   loss_b = forwardScore(intersect(E_b, G)) - forwardScore(intersect(intersect(ctc_b, G), E_b))
+ * G: C nodes, all start and accept, arc j -> i with label i and weight W[i*C + j].
+ */
+extern "C" int gtnb_ngram_ctc_loss(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const float* trans_w, int trans_on_device, const int32_t* targets, const int32_t* target_lens, int blank,
+    float* losses_host, float* grads, int grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  return ngram_ctc_loss_call(ctx, TransitionArgs{B, T, C, emissions, emissions_on_device, input_lens, trans_w,
+                                                 trans_on_device, targets, target_lens, blank, losses_host, grads,
+                                                 grads_on_device, trans_grad, trans_grad_on_device});
+}
+
+extern "C" int gtnb_ngram_ctc_loss_typed(
+    gtnb_ctx* ctx, int B, int T, int C, const void* emissions_dev, int dtype, const int32_t* input_lens,
+    const float* trans_w_dev, const int32_t* targets, const int32_t* target_lens, int blank, float* losses_host,
+    void* grads_dev, float* trans_grad_dev) {
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss_typed: unknown dtype");
+  return ngram_ctc_loss_call(ctx, TransitionArgs{B, T, C, static_cast<const float*>(emissions_dev), 1, input_lens,
+                                                 trans_w_dev, 1, targets, target_lens, blank, losses_host,
+                                                 static_cast<float*>(grads_dev), 1, trans_grad_dev, 1, dtype});
 }
 
 namespace {
@@ -1288,34 +1387,65 @@ int asg_num_build(gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, 
  * in its start mode and the numerator graphs are built on the device; otherwise (and for non-finite weights) the
  * call goes through gtnb_asg_loss's machinery with the same T_b.
  */
-extern "C" int gtnb_asg_loss_ex(
-    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
-    const float* trans_w, int trans_on_device, const int32_t* targets, const int32_t* target_lens,
-    float* losses_host, float* grads, int grads_on_device, float* trans_grad, int trans_grad_on_device) {
-  const TransitionArgs a{B, T, C, emissions, emissions_on_device, input_lens, trans_w, trans_on_device, targets,
-                         target_lens, -1, losses_host, grads, grads_on_device, trans_grad, trans_grad_on_device};
-  if (!ctx || B < 0 || T < 0 || C <= 0 || !emissions || !trans_w || !target_lens || !losses_host)
+namespace {
+
+/* gtnb_asg_loss_ex and gtnb_asg_loss_typed: a.dtype's emissions on the native route, or widened */
+int asg_loss_ex_call(gtnb_ctx* ctx, const TransitionArgs& a) {
+  const int B = a.B, T = a.T, C = a.C;
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !a.emissions || !a.trans_w || !a.target_lens || !a.losses_host)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: bad arguments");
   const long long nTrans = C + (long long)C * C;
   Targets t;
-  GTNB_TRY(parse_targets(ctx, "gtnb_asg_loss_ex", B, T, C, input_lens, targets, target_lens, &t));
+  GTNB_TRY(parse_targets(ctx, "gtnb_asg_loss_ex", B, T, C, a.input_lens, a.targets, a.target_lens, &t));
   std::vector<SgDims> dims(B);
   for (int b = 0; b < B; b++) {
     if (!t.in_range[b]) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: label outside [0, C)");
     // compose(fal_b, transitions): U+1 nodes, 2U arcs (none when U = 0), node U accepts
-    const int U = target_lens[b];
+    const int U = a.target_lens[b];
     dims[b] = SgDims{U + 1, 2 * U, U > 0 ? 1 : 0, /*all_valid=*/1, /*uniform=*/1, /*max_in=*/2, /*max_out=*/2};
   }
   TrellisCriterion asg{nTrans, asg_alpha_floats(B, T, C), /*fold=*/false, launch_asg_den_forward,
                              launch_asg_den_backward};
+  asg.dtype = a.dtype;
   // (a non-finite weight: gtnb_asg_loss's sweeps raise the same status bit and end in the materialised lattices)
   const bool fast = C <= kNgramMaxLabels && ctx->use_implicit && implicit_dims_supported(dims.data(), B);
-  return run_criterion(ctx, B, t.T(), losses_host, trans_grad, trans_grad_on_device, nTrans, fast,
+  return run_criterion(ctx, B, t.T(), a.losses_host, a.trans_grad, a.trans_grad_on_device, nTrans, fast,
                        [&](CallScope& scope, bool f, bool* needs_exact) {
-                         if (!f) return asg_loss_generic(scope, a, t);
+                         if (!f)
+                           return widened(scope, a, [&](const TransitionArgs& w) {
+                             return asg_loss_generic(scope, w, t);
+                           });
                          TargetsNumerator num{t, dims, C, asg_num_build, -1};
                          return trellis_loss_fast(scope, asg, a, num, needs_exact);
                        });
+}
+
+} // namespace
+
+/*
+ * ASG with per-utterance frame counts and device-resident transitions (gtnb_asg_loss_ex):
+ *   loss_b = forwardScore(compose(E_b, transitions)) - forwardScore(compose(compose(fal_b, transitions), E_b))
+ * with E_b = linearGraph(T_b, C) on the first T_b rows.  For C <= 128 the denominator is k_ngram.cu's dense trellis
+ * in its start mode and the numerator graphs are built on the device; otherwise (and for non-finite weights) the
+ * call goes through gtnb_asg_loss's machinery with the same T_b.
+ */
+extern "C" int gtnb_asg_loss_ex(
+    gtnb_ctx* ctx, int B, int T, int C, const float* emissions, int emissions_on_device, const int32_t* input_lens,
+    const float* trans_w, int trans_on_device, const int32_t* targets, const int32_t* target_lens,
+    float* losses_host, float* grads, int grads_on_device, float* trans_grad, int trans_grad_on_device) {
+  return asg_loss_ex_call(ctx, TransitionArgs{B, T, C, emissions, emissions_on_device, input_lens, trans_w,
+                                              trans_on_device, targets, target_lens, -1, losses_host, grads,
+                                              grads_on_device, trans_grad, trans_grad_on_device});
+}
+
+extern "C" int gtnb_asg_loss_typed(
+    gtnb_ctx* ctx, int B, int T, int C, const void* emissions_dev, int dtype, const int32_t* input_lens,
+    const float* trans_w_dev, const int32_t* targets, const int32_t* target_lens, float* losses_host,
+    void* grads_dev, float* trans_grad_dev) {
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_typed: unknown dtype");
+  return asg_loss_ex_call(ctx, TransitionArgs{B, T, C, static_cast<const float*>(emissions_dev), 1, input_lens,
+                                              trans_w_dev, 1, targets, target_lens, -1, losses_host,
+                                              static_cast<float*>(grads_dev), 1, trans_grad_dev, 1, dtype});
 }
 
 /*

@@ -130,6 +130,9 @@ struct gtnb_lattice {
   // compose operands kept on the device
   const float* emissions = nullptr;
   int64_t emissions_stride = 0;
+  // the element type behind `emissions` (GTNB_F32 / GTNB_BF16 / GTNB_F16).  A 16-bit lattice is read only by
+  // k_implicit.cu's one-node / several-nodes-per-thread log-semiring sweeps; every other mode refuses it
+  int dtype = GTNB_F32;
   uint8_t* sg_flags = nullptr; // per small-graph node
   int32_t* sg_in_ptr = nullptr; // [sgN + 1] per graph
   int32_t* sg_in_src = nullptr; // per in-entry (sgA)
@@ -349,21 +352,25 @@ int ensure_side_streams(gtnb_ctx* ctx, int n_streams, int n_events);
 // kernel (k_dense.cu): factored dense-trellis Viterbi.  bigram: trans_dev is n-gram CTC's [C*C] W (every state
 // starts), else ASG's [C + C*C]; bp holds [B][T_max][dense_bp_pitch(C)] bytes; 1 <= C <= 224
 int dense_bp_pitch(int C);
+// emis: elements of dtype (GTNB_F32 / GTNB_BF16 / GTNB_F16), read as they are
 int launch_viterbi_dense(
-    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const float* emis, int64_t stride,
-    const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores);
+    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const void* emis, int64_t stride,
+    const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores, int dtype = GTNB_F32);
 // kernels (k_ngram.cu): CTC with a learned bigram transition graph
 constexpr int kNgramMaxLabels = 128;
 int launch_ngram_sigma(gtnb_ctx* ctx, int C, const float* W, float* sigma);
 int launch_ngram_num_build(
     gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
     const int32_t* tgt_len_dev, int blank, const float* W, const float* sigma, int32_t* map);
+// the dense trellis (launch_*_den_*): emis holds elements of dtype (GTNB_F32 / GTNB_BF16 / GTNB_F16), read as they
+// are; grad stays float32
 int launch_ngram_den_forward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* W, float* alpha, float* den, int32_t* status);
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
+    const float* W, float* alpha, float* den, int32_t* status, int dtype = GTNB_F32);
 int launch_ngram_den_backward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad);
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
+    const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad,
+    int dtype = GTNB_F32);
 int launch_ngram_fold(gtnb_ctx* ctx, int C, const float* W, const float* sigma, float* wgrad);
 // out[k] = w_A[arc_of[k]] + Wx[tidx[k]], Wx = [W (nW floats) | sigma]: the weights of gtnb_product.h's products
 int launch_product_fold(gtnb_ctx* ctx, long long n, const float* w_A, const int32_t* arc_of, const float* W, int nW,
@@ -377,12 +384,12 @@ int launch_product_arc_map(gtnb_ctx* ctx, int B, int T_out, const long long* off
 // forced-alignment numerator graphs built on the device
 long long asg_alpha_floats(int B, int T, int C); // floats of the alpha buffer of launch_asg_den_*
 int launch_asg_den_forward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* trans_w, float* alpha, float* den, int32_t* status);
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
+    const float* trans_w, float* alpha, float* den, int32_t* status, int dtype = GTNB_F32);
 int launch_asg_den_backward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
     const float* trans_w, const float* alpha, const float* den, float* grad, long long grad_stride,
-    float* trans_grad);
+    float* trans_grad, int dtype = GTNB_F32);
 int launch_asg_num_build(
     gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
     const int32_t* tgt_len_dev, const float* trans_w, int32_t* map);

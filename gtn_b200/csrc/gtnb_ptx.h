@@ -98,6 +98,12 @@ __device__ __forceinline__ void ldg_if(bool p, float& dst, const float* src) {
 __device__ __forceinline__ void ldg_keep(float& dst, const float* src) {
   dst = *src;
 }
+__device__ __forceinline__ void ldg_if_u16(bool p, uint32_t& dst, const uint16_t* src) {
+  if (p) dst = *src;
+}
+__device__ __forceinline__ void ldg_keep_u16(uint32_t& dst, const uint16_t* src) {
+  dst = *src;
+}
 __device__ __forceinline__ void red_if(bool p, float* dst, float v) {
   if (p) atomicAdd(dst, v);
 }
@@ -220,6 +226,9 @@ __device__ __forceinline__ float f16_bits_f32(uint32_t h) {
   if (e == 31) return __int_as_float((int)(s | 0x7f800000u | (m << 13))); // inf / NaN
   return __int_as_float((int)(s | ((e + 112u) << 23) | (m << 13)));
 }
+__device__ __forceinline__ float ldg_f16_f32(const uint16_t* p) {
+  return f16_bits_f32(*p);
+}
 __device__ __forceinline__ uint32_t f32_bf16_bits(float v) {
   const uint32_t x = (uint32_t)__float_as_int(v);
   if ((x & 0x7fffffffu) > 0x7f800000u) return (x >> 16) | 0x40u; // NaN: quiet
@@ -314,6 +323,26 @@ __device__ __forceinline__ void ldg_if(bool p, float& dst, const float* src) {
  * on, writing the loop-carried ring register directly. */
 __device__ __forceinline__ void ldg_keep(float& dst, const float* src) {
   asm volatile("ld.relaxed.cta.global.f32 %0, [%1];" : "=f"(dst) : "l"(src) : "memory");
+}
+/* the same two loads of one 16-bit element, zero-extended into a 32-bit register */
+__device__ __forceinline__ void ldg_if_u16(bool p, uint32_t& dst, const uint16_t* src) {
+  asm volatile(
+      "{\n"
+      ".reg .pred q;\n"
+      "setp.ne.s32 q, %2, 0;\n"
+      "@q ld.global.nc.u16 %0, [%1];\n"
+      "}\n"
+      : "+r"(dst)
+      : "l"(src), "r"((int)p));
+}
+__device__ __forceinline__ void ldg_keep_u16(uint32_t& dst, const uint16_t* src) {
+  asm volatile("ld.relaxed.cta.global.u16 %0, [%1];" : "=r"(dst) : "l"(src) : "memory");
+}
+/* one IEEE half element of global memory, widened (exact) */
+__device__ __forceinline__ float ldg_f16_f32(const uint16_t* p) {
+  float y;
+  asm("{\n.reg .b16 h;\nld.global.nc.b16 h, [%1];\ncvt.f32.f16 %0, h;\n}" : "=f"(y) : "l"(p));
+  return y;
 }
 /* predicated red.global.add.f32 (no branch, no reconvergence point in the frame loop) */
 __device__ __forceinline__ void red_if(bool p, float* dst, float v) {
@@ -623,15 +652,54 @@ __device__ __forceinline__ void stg_elem4(E* p, float4 v) {
   else
     stg_v4_f32(p, v);
 }
-/* one element in global memory, either way */
+/* one element in global memory, either way (a float32 element through __ldg, as the float32 kernels load it) */
 template <class E>
 __device__ __forceinline__ float ldg_elem(const E* p) {
   if constexpr (std::is_same_v<E, bf16_t>)
     return bf16_bits_f32(p->bits);
   else if constexpr (std::is_same_v<E, f16_t>)
-    return f16_bits_f32(p->bits);
+    return ldg_f16_f32(&p->bits);
   else
+    return __ldg(p);
+}
+/* the same through a plain load, for the float32 loads that never went through __ldg */
+template <class E>
+__device__ __forceinline__ float ld_elem(const E* p) {
+  if constexpr (std::is_same_v<E, float>)
     return *p;
+  else
+    return ldg_elem(p);
+}
+/*
+ * A slot of a register ring of prefetched elements (k_implicit.cu's frame loops): the float itself, or the 16 bits in
+ * a 32-bit register, widened by ring_f32 where the value is used -- so a 16-bit load is not waited for where it is
+ * issued.  ldg_ring / ldg_if / ldg_keep fill a slot; with E = float they are the float32 loads themselves.
+ */
+template <class E>
+using ring_t = std::conditional_t<std::is_same_v<E, float>, float, uint32_t>;
+template <class E>
+__device__ __forceinline__ float ring_f32(ring_t<E> r) {
+  if constexpr (std::is_same_v<E, bf16_t>)
+    return bf16_bits_f32(r);
+  else if constexpr (std::is_same_v<E, f16_t>)
+    return f16_bits_f32(r);
+  else
+    return r;
+}
+template <class E>
+__device__ __forceinline__ ring_t<E> ldg_ring(const E* p) {
+  if constexpr (std::is_same_v<E, float>)
+    return __ldg(p);
+  else
+    return __ldg(&p->bits);
+}
+template <class E, std::enable_if_t<!std::is_same_v<E, float>, int> = 0>
+__device__ __forceinline__ void ldg_if(bool p, uint32_t& dst, const E* src) {
+  ldg_if_u16(p, dst, &src->bits);
+}
+template <class E, std::enable_if_t<!std::is_same_v<E, float>, int> = 0>
+__device__ __forceinline__ void ldg_keep(uint32_t& dst, const E* src) {
+  ldg_keep_u16(dst, &src->bits);
 }
 template <class E>
 __device__ __forceinline__ void stg_elem(E* p, float v) {

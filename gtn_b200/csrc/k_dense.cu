@@ -33,6 +33,8 @@
  * warp shuffles; the traceback runs on one warp with 8 back-pointer rows in flight.
  * Back-pointer rows are dense_bp_pitch(C) bytes apart (C rounded up to a multiple of 4), so the
  * traceback reads every row as whole 32-bit words for any C.
+ * The emissions may be float32, bfloat16 or fp16 (template parameter E, gtnb_viterbi_dense_typed): every element is
+ * widened to float32 on load, so the 16-bit kernels relax exactly the float32 kernels' candidates.
  */
 #include "gtnb_ptx.h"
 
@@ -47,12 +49,12 @@ namespace {
 
 constexpr int kDenseThreads = 256;
 
-template <int G, bool BIGRAM = false>
+template <int G, bool BIGRAM = false, class E = float> // E: the element type of the emissions (float, bf16_t, f16_t)
 __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
     int T_max,
     int C,
     const int32_t* __restrict__ T_arr, // nullable
-    const float* __restrict__ emis,
+    const E* __restrict__ emis,
     long long stride,
     const float* __restrict__ trans, // ASG: [C] start arcs, then [C][C]; BIGRAM: [C][C]; w(j -> i) at [i*C + j]
     uint8_t* __restrict__ bp, // [B][T_max][pitch]
@@ -70,7 +72,7 @@ __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
   const int lane = tid & 31, warp = tid >> 5;
   constexpr int SPW = 32 / G; // states per warp
   const int sub = lane / SPW; // which slice of the predecessors
-  const float* e = emis + (long long)b * stride;
+  const E* e = emis + (long long)b * stride;
   uint8_t* mybp = bp + (long long)b * T_max * pitch;
   const float* W = BIGRAM ? trans : trans + C;
 
@@ -83,7 +85,7 @@ __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
       s_sc[C + i] = 0.0f; // the start states of G, read as frame -1 by the loop below
     } else if (T > 0) {
       // frame 0: single predecessor, the start node (score 0): fl(0 + fl(e + w_start))
-      s_sc[i] = __fadd_rn(0.0f, __fadd_rn(e[i], trans[i]));
+      s_sc[i] = __fadd_rn(0.0f, __fadd_rn(ld_elem(e + i), trans[i]));
       mybp[i] = 0;
     }
   }
@@ -97,7 +99,7 @@ __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
     for (int p = 0; p < n_pass; p++) {
       const int i = p * (kDenseThreads / G) + warp * SPW + (lane % SPW);
       const bool live = i < C;
-      const float et = live ? __ldg(&e[(long long)t * C + i]) : 0.0f;
+      const float et = live ? ldg_elem(e + (long long)t * C + i) : 0.0f;
       float best = -CUDART_INF_F;
       int bj = 0x7fffffff;
       if (live) {
@@ -226,12 +228,12 @@ __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
 
 #ifndef GTNB_HOST_EMU
 
-int launch_viterbi_dense(
-    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const float* emis, int64_t stride,
+namespace {
+
+template <class E>
+int viterbi_dense_typed(
+    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const E* emis, int64_t stride,
     const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores) {
-  if (B == 0) return GTNB_OK;
-  if (C < 1 || C > 256)
-    return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_viterbi_dense: needs 1 <= C <= 256");
   int G = 1;
   while (G < 32 && C * (G * 2) <= kDenseThreads) G *= 2;
   const size_t smem = sizeof(float) * ((size_t)C * (C + 32 / G) + 2 * (size_t)C);
@@ -240,10 +242,10 @@ int launch_viterbi_dense(
                 "gtnb_viterbi_dense: the transitions tile does not fit shared memory (C <= 224)");
 #define LAUNCH_DENSE(G_, K_)                                                                        \
   do {                                                                                              \
-    int rc__ = ensure_max_smem(ctx, (const void*)viterbi_dense_kernel<G_, K_>);                     \
+    int rc__ = ensure_max_smem(ctx, (const void*)viterbi_dense_kernel<G_, K_, E>);                  \
     if (rc__) return rc__;                                                                          \
     GTNB_LAUNCH(ctx, K_ ? "viterbi_dense_bigram" : "viterbi_dense",                                 \
-                viterbi_dense_kernel<G_, K_><<<B, kDenseThreads, smem, ctx->stream>>>(              \
+                viterbi_dense_kernel<G_, K_, E><<<B, kDenseThreads, smem, ctx->stream>>>(           \
                     T_max, C, T_dev, emis, (long long)stride, trans_dev, bp, paths, scores, empty_score)); \
   } while (0)
 #define LAUNCH_KIND(G_)            \
@@ -264,6 +266,28 @@ int launch_viterbi_dense(
 #undef LAUNCH_KIND
 #undef LAUNCH_DENSE
   return GTNB_OK;
+}
+
+} // namespace
+
+int launch_viterbi_dense(
+    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const void* emis, int64_t stride,
+    const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores, int dtype) {
+  if (B == 0) return GTNB_OK;
+  if (C < 1 || C > 256)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_viterbi_dense: needs 1 <= C <= 256");
+  switch (dtype) {
+    case GTNB_F32:
+      return viterbi_dense_typed(ctx, B, T_max, C, bigram, T_dev, static_cast<const float*>(emis), stride, trans_dev,
+                                 empty_score, bp, paths, scores);
+    case GTNB_BF16:
+      return viterbi_dense_typed(ctx, B, T_max, C, bigram, T_dev, static_cast<const bf16_t*>(emis), stride, trans_dev,
+                                 empty_score, bp, paths, scores);
+    case GTNB_F16:
+      return viterbi_dense_typed(ctx, B, T_max, C, bigram, T_dev, static_cast<const f16_t*>(emis), stride, trans_dev,
+                                 empty_score, bp, paths, scores);
+    default: return fail(ctx, GTNB_ERR_LOGIC, "launch_viterbi_dense: unknown element type");
+  }
 }
 
 #endif // GTNB_HOST_EMU

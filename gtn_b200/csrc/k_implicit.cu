@@ -42,6 +42,11 @@
  * Tropical mode (template flag TROP, gtnb_graph_viterbi): the forward kernels take the max instead of the logadd,
  * and implicit_trace_kernel walks the best path back from the saved score rows (with TROP = false the forward
  * kernels compile to what they were).
+ *
+ * Element type (template parameter E, lat->dtype): the one-node / several-nodes-per-thread log-semiring kernels of
+ * label-uniform graphs -- the mode the trellis criteria's numerators take -- also read bfloat16 / fp16 emissions,
+ * widened to float32 where a frame uses them (the prefetch rings hold the 16 bits); the emission gradient stays
+ * float32.  Every other mode has float32 instantiations only and refuses a 16-bit lattice (implicit_elem_mode).
  */
 #include <algorithm>
 
@@ -230,11 +235,12 @@ __device__ __forceinline__ void load_arc_labels(const GraphMeta& m, const int32_
   __syncthreads();
 }
 
-/* arc-label mode: emission row `row` (C floats) -> shared memory; returns "some value is not finite" */
-__device__ __forceinline__ bool stage_erow(const float* row, float* dst, int C) {
+/* arc-label mode: emission row `row` (C elements) -> shared memory; returns "some value is not finite" */
+template <class E>
+__device__ __forceinline__ bool stage_erow(const E* row, float* dst, int C) {
   bool bad = false;
   for (int c = threadIdx.x; c < C; c += kImpThreads) {
-    const float v = __ldg(row + c);
+    const float v = ldg_elem(row + c);
     dst[c] = v;
     bad |= !is_finite(v);
   }
@@ -256,8 +262,9 @@ __device__ __forceinline__ void flush_erow_grad(float* GE, float* gr, int C, flo
 /* ------------------------------------------------------------------ */
 
 /* TROP: the tropical semiring (viterbiScore, gtnb_graph_viterbi): every logadd becomes a max, the score rows are
- * saved as before for implicit_trace_kernel */
-template <bool ARC = false, bool TROP = false>
+ * saved as before for implicit_trace_kernel.  E: the element type of the emissions (float, or bf16_t / f16_t, widened
+ * on load; only <false, false> is built for those) */
+template <bool ARC = false, bool TROP = false, class E = float>
 __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -265,7 +272,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     const int32_t* __restrict__ sg_in_src,
     const int32_t* __restrict__ sg_in_label,
     const float* __restrict__ sg_in_w,
-    const float* __restrict__ emissions,
+    const E* __restrict__ emissions,
     float* __restrict__ scores,
     float* __restrict__ out_scores,
     int32_t* __restrict__ status,
@@ -290,7 +297,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
   float* E_s = reinterpret_cast<float*>(smem + lay.off_earc); // ARC only: [2][C], frame t-1 at (t-1) & 1
   if (ARC) load_arc_labels(m, sg_in_label, t_alab);
   float* sc = scores + m.node_base;
-  const float* em = emissions + m.emis_off;
+  const E* em = emissions + m.emis_off;
   // fast path: one node per thread, every node with at most three in-arcs (block-uniform)
   int my_deg = 0;
   if (tid < N1) my_deg = t_inptr[tid + 1] - t_inptr[tid];
@@ -332,7 +339,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
         w2 = t_w[e0 + 2];
       }
     }
-    const float* eml = em + (has ? t_lab[tid] : 0);
+    const E* eml = em + (has ? t_lab[tid] : 0);
     // Emissions of the node's label reach the thread through two register blocks: pf[] holds
     // frames f0 .. f0+kPf-1 (complete), nx[] frames f0+kPf .. f0+2kPf-1, in flight since the
     // previous block boundary.  At a block boundary nx[] is copied to pf[] and the kPf loads of
@@ -343,18 +350,20 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     // (Where the refill sits matters to ptxas: at the END of the block here -- all loads on one
     // scoreboard, waited 7 frames later; at the top it spreads them over the scoreboards the
     // LDS / MUFU results use.  The backward sweep needs it at the top.  Checked in SASS.)
-    float pf[kPf], nx[kPf];
+    // (16-bit elements travel through the ring as their bits and are widened where a step uses them)
+    ring_t<E> pf[kPf], nx[kPf];
 #pragma unroll
-    for (int j = 0; j < kPf; j++) pf[j] = (has && j < T) ? __ldg(eml + (long long)j * C) : 0.0f;
+    for (int j = 0; j < kPf; j++) pf[j] = (has && j < T) ? ldg_ring(eml + (long long)j * C) : ring_t<E>(0);
 #pragma unroll
-    for (int j = 0; j < kPf; j++) nx[j] = (has && kPf + j < T) ? __ldg(eml + (long long)(kPf + j) * C) : 0.0f;
-    const float* epf = eml + (long long)(2 * kPf) * C; // first frame of the next refill
+    for (int j = 0; j < kPf; j++)
+      nx[j] = (has && kPf + j < T) ? ldg_ring(eml + (long long)(kPf + j) * C) : ring_t<E>(0);
+    const E* epf = eml + (long long)(2 * kPf) * C; // first frame of the next refill
     float* grow = sc + pitch + tid; // this node's score in frame f + 1
     float chk = 0.0f; // becomes NaN when a used emission is not finite
     int f0 = 0;
 #define GTNB_FWD_STEP(j)                                                 \
   {                                                                      \
-    const float e = has ? pf[j] : 0.0f; /* idle threads load node 0's */ \
+    const float e = has ? ring_f32<E>(pf[j]) : 0.0f; /* idle threads load node 0's */ \
     const float* P = ((j)&1) ? S1 : S0;                                  \
     float* Q = ((j)&1) ? S0 : S1;                                        \
     const float sv = combine3<TROP>(P[i0] + (w0 + e), P[i1] + (w1 + e), P[i2] + (w2 + e)); \
@@ -403,7 +412,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
     float* prev = S0;
     float* cur = S1;
     for (int t = 1; t <= T; t++) {
-      const float* er = em + (long long)(t - 1) * C;
+      const E* er = em + (long long)(t - 1) * C;
       float* srow = sc + (long long)t * pitch;
       if (ARC) {
         // frame t-1's row was staged before the last barrier; frame t's goes to the other half
@@ -423,7 +432,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_forward_kernel(
           const int e0 = t_inptr[i], e1 = t_inptr[i + 1];
           float sv = neg_inf();
           if (e1 > e0) {
-            const float e = __ldg(er + t_lab[i]);
+            const float e = ldg_elem(er + t_lab[i]);
             bad |= !is_finite(e);
             sv = TROP ? imp_fwd_node_max(e0, e1, e, t_src, t_w, prev) : imp_fwd_node_any(e0, e1, e, t_src, t_w, prev);
           }
@@ -491,7 +500,8 @@ __device__ __forceinline__ void build_out_lists(
 /* backward                                                            */
 /* ------------------------------------------------------------------ */
 
-template <bool GRAPH_GRAD, bool ARC = false>
+/* E: as in implicit_forward_kernel (only <*, false> is built for 16-bit types); the emission gradient stays float32 */
+template <bool GRAPH_GRAD, bool ARC = false, class E = float>
 __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     const GraphMeta* __restrict__ meta,
     const uint8_t* __restrict__ sg_flags,
@@ -501,7 +511,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     const float* __restrict__ sg_in_w,
     const int32_t* __restrict__ sg_in_arc,
     float* __restrict__ grad_graph,
-    const float* __restrict__ emissions,
+    const E* __restrict__ emissions,
     const float* __restrict__ scores,
     const float* __restrict__ out_scores,
     const float* __restrict__ deltas,
@@ -542,7 +552,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
   if (!is_finite(out) || T < 1) return; // no accepting path (empty lattice): no gradient
   const float delta = deltas ? deltas[blockIdx.x] : 1.0f;
   const float* sc = scores + m.node_base;
-  const float* em = emissions + m.emis_off;
+  const E* em = emissions + m.emis_off;
   float* gem = grad_emis + (long long)blockIdx.x * grad_stride;
   // seeds: nodeGrad[accept] = exp(score - maxA) / exp(out - maxA) (shortest.cpp:49-60)
   float mxa = neg_inf();
@@ -589,23 +599,24 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     if (od > 0) q0 = t_outent[t_outptr[tid]];
     if (od > 1) q1 = t_outent[t_outptr[tid] + 1];
     if (od > 2) q2 = t_outent[t_outptr[tid] + 2];
-    const float* eml = em + (has ? t_lab[tid] : 0);
+    const E* eml = em + (has ? t_lab[tid] : 0);
     const float* scu = sc + (act ? tid : 0);
 
     // iteration i handles level t = T - i and prepares level t - 1, for which it needs frame
     // f = t - 2 = T - 2 - i of the saved scores and of the emissions.  Two register blocks as in
     // the forward sweep: a block of kPf iterations copies nxs/nxe (loaded during the previous
     // block) to ps/pe and issues all loads of the next block.
-    float ps[kPf], pe[kPf], nxs[kPf], nxe[kPf];
+    float ps[kPf], nxs[kPf];
+    ring_t<E> pe[kPf], nxe[kPf]; // (16-bit elements as their bits, as in the forward sweep)
 #pragma unroll
     for (int j = 0; j < kPf; j++) {
       const int f = T - 2 - j;
       nxs[j] = (act && f >= 0) ? __ldg(scu + (long long)f * pitch) : neg_inf();
-      nxe[j] = (has && f >= 0) ? __ldg(eml + (long long)f * C) : 0.0f;
+      nxe[j] = (has && f >= 0) ? ldg_ring(eml + (long long)f * C) : ring_t<E>(0);
     }
     // first frame of the next refill; only dereferenced while >= row 0
     const float* spf = scu + (long long)(T - 2 - kPf) * pitch;
-    const float* epf = eml + (long long)(T - 2 - kPf) * C;
+    const E* epf = eml + (long long)(T - 2 - kPf) * C;
     // prologue: the arc factors of level T need row T-1 in shared memory
     float s_own = act ? __ldg(scu + (long long)T * pitch) : neg_inf(); // S_T[u]
     float s_nxt = act ? __ldg(scu + (long long)(T - 1) * pitch) : neg_inf(); // S_{T-1}[u]
@@ -618,7 +629,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     __syncthreads();
     float E0, E1, E2;
     {
-      const float e = has ? __ldg(eml + (long long)(T - 1) * C) : 0.0f;
+      const float e = has ? ldg_elem(eml + (long long)(T - 1) * C) : 0.0f;
       const float se = (s_own == -CUDART_INF_F) ? CUDART_INF_F : s_own;
       E0 = fexp(Sb[i0] + (w0 + e) - se);
       E1 = fexp(Sb[i1] + (w1 + e) - se);
@@ -644,7 +655,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
       ga2 += c2;                                                                      \
     }                                                                                 \
     const float s_f = ps[j]; /* S_{t-2}[u] */                                         \
-    const float e_f = has ? pe[j] : 0.0f; /* e[t-2][label] */                         \
+    const float e_f = has ? ring_f32<E>(pe[j]) : 0.0f; /* e[t-2][label] */            \
     Sw[tid] = s_f;                                                                    \
     bar_named<1>(nact);                                                                  \
     g = (Cw[q0] + Cw[q1]) + Cw[q2]; /* node gradient of level t-1: the serial chain */ \
@@ -720,7 +731,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
     float* Sown = Sa; // row t
     float* Sprev = Sb; // row t-1
     for (int t = T; t >= 1; t--) {
-      const float* er = em + (long long)(t - 1) * C;
+      const E* er = em + (long long)(t - 1) * C;
       float* gr = gem + (long long)(t - 1) * C;
       for (int i = tid; i < N1; i += kImpThreads) Sprev[i] = sc[(long long)(t - 1) * pitch + i];
       if (ARC) stage_erow(er, E_s, C);
@@ -746,7 +757,7 @@ __global__ void __launch_bounds__(kImpThreads) implicit_backward_kernel(
           if (e1 == e0) continue;
           const float gi = NG[i], sn = Sown[i];
           const bool ex = sn > -CUDART_INF_F;
-          const float e = __ldg(er + t_lab[i]);
+          const float e = ldg_elem(er + t_lab[i]);
           float acc = 0.0f;
 #pragma unroll 1
           for (int a = e0; a < e1; a++) {
@@ -1358,6 +1369,14 @@ int wide_lanes(int max_in, int max_out, int maxN, int C, bool backward, bool arc
 
 } // namespace
 
+/* GTNB_OK when a lattice of element type dtype may take the mode (G: wide_lanes; arc-label; tropical), else
+ * GTNB_ERR_LOGIC: 16-bit emissions have instantiations of the one-node / several-nodes-per-thread log-semiring sweeps
+ * of label-uniform graphs only (the trellis criteria's numerators), and no other kernel may read them as float32 */
+int implicit_elem_mode(int dtype, int G, bool arc, bool tropical) {
+  if (dtype == GTNB_F32) return GTNB_OK;
+  return (dtype == GTNB_BF16 || dtype == GTNB_F16) && G == 0 && !arc && !tropical ? GTNB_OK : GTNB_ERR_LOGIC;
+}
+
 #ifndef GTNB_HOST_EMU
 
 /* arc_C > 0 (gtnb_graph_loss, labels in [0, arc_C)): graphs that are not label-uniform are accepted
@@ -1387,14 +1406,15 @@ bool implicit_supported(const gtnb_lattice* lat) {
   return lay.total <= 200 * 1024;
 }
 
-#define GTNB_FWD_ARGS                                                                             \
+// E: the element type the kernel reads lat->emissions as
+#define GTNB_FWD_ARGS(E)                                                                          \
   lat->meta + b0, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w, \
-      lat->emissions, lat->scores, lat->out_scores + b0, status_dev + b0, lat->C, lay
-#define GTNB_BWD_ARGS                                                                             \
+      reinterpret_cast<const E*>(lat->emissions), lat->scores, lat->out_scores + b0, status_dev + b0, lat->C, lay
+#define GTNB_BWD_ARGS(E)                                                                          \
   lat->meta + b0, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w, \
-      lat->sg_in_arc, grad_graph, lat->emissions, lat->scores, lat->out_scores + b0,             \
-      deltas_dev ? deltas_dev + b0 : nullptr, grad_emis + (long long)b0 * grad_stride,           \
-      (long long)grad_stride, lat->C, lay
+      lat->sg_in_arc, grad_graph, reinterpret_cast<const E*>(lat->emissions), lat->scores,       \
+      lat->out_scores + b0, deltas_dev ? deltas_dev + b0 : nullptr,                               \
+      grad_emis + (long long)b0 * grad_stride, (long long)grad_stride, lat->C, lay
 
 namespace {
 
@@ -1405,16 +1425,31 @@ int implicit_forward_mode(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev,
   const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, false, G > 0, lat->C, ARC);
   const char* name = ARC ? (TROP ? "implicit_forward_arc_max" : "implicit_forward_arc")
                          : (TROP ? "implicit_forward_max" : "implicit_forward");
-#define GTNB_LAUNCH_FWD(K)                                                                \
-  do {                                                                                    \
-    if (lay.total > 48 * 1024) {                                                          \
-      int rc = ensure_max_smem(ctx, (const void*)K);                                      \
-      if (rc) return rc;                                                                  \
-    }                                                                                     \
-    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_FWD_ARGS)); \
+  if (implicit_elem_mode(lat->dtype, G, ARC, TROP))
+    return fail(ctx, GTNB_ERR_LOGIC, "launch_implicit_forward: no instantiation for 16-bit emissions in this mode");
+#define GTNB_LAUNCH_FWD_E(K, E)                                                                  \
+  do {                                                                                           \
+    if (lay.total > 48 * 1024) {                                                                 \
+      int rc = ensure_max_smem(ctx, (const void*)K);                                             \
+      if (rc) return rc;                                                                         \
+    }                                                                                            \
+    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_FWD_ARGS(E)));    \
   } while (0)
+#define GTNB_LAUNCH_FWD(K) GTNB_LAUNCH_FWD_E(K, float)
   switch (G) {
-    case 0: GTNB_LAUNCH_FWD((implicit_forward_kernel<ARC, TROP>)); break;
+    case 0:
+      if constexpr (!ARC && !TROP) {
+        if (lat->dtype == GTNB_BF16) {
+          GTNB_LAUNCH_FWD_E((implicit_forward_kernel<false, false, bf16_t>), bf16_t);
+          break;
+        }
+        if (lat->dtype == GTNB_F16) {
+          GTNB_LAUNCH_FWD_E((implicit_forward_kernel<false, false, f16_t>), f16_t);
+          break;
+        }
+      }
+      GTNB_LAUNCH_FWD((implicit_forward_kernel<ARC, TROP>));
+      break;
     case 1: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<1, ARC, TROP>)); break;
     case 2: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<2, ARC, TROP>)); break;
     case 4: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<4, ARC, TROP>)); break;
@@ -1423,6 +1458,7 @@ int implicit_forward_mode(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev,
     default: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<32, ARC, TROP>)); break;
   }
 #undef GTNB_LAUNCH_FWD
+#undef GTNB_LAUNCH_FWD_E
   return GTNB_OK;
 }
 
@@ -1433,13 +1469,31 @@ int implicit_backward_mode(
   const int G = wide_lanes(lat->max_in_deg, lat->max_out_deg, lat->max_lvl_nodes, lat->C, true, ARC);
   const ImpLayout lay = make_imp_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, true, G > 0, lat->C, ARC);
   const char* name = ARC ? "implicit_backward_arc" : "implicit_backward";
-#define GTNB_LAUNCH_BWD(K)                                                                \
-  do {                                                                                    \
-    if (lay.total > 48 * 1024) {                                                          \
-      int rc = ensure_max_smem(ctx, (const void*)K);                                      \
-      if (rc) return rc;                                                                  \
-    }                                                                                     \
-    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_BWD_ARGS)); \
+  if (implicit_elem_mode(lat->dtype, G, ARC, false))
+    return fail(ctx, GTNB_ERR_LOGIC, "launch_implicit_backward: no instantiation for 16-bit emissions in this mode");
+#define GTNB_LAUNCH_BWD_E(K, E)                                                                  \
+  do {                                                                                           \
+    if (lay.total > 48 * 1024) {                                                                 \
+      int rc = ensure_max_smem(ctx, (const void*)K);                                             \
+      if (rc) return rc;                                                                         \
+    }                                                                                            \
+    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_BWD_ARGS(E)));    \
+  } while (0)
+#define GTNB_LAUNCH_BWD(K) GTNB_LAUNCH_BWD_E(K, float)
+/* the one-node / several-nodes-per-thread kernel for lat->dtype */
+#define GTNB_LAUNCH_BWD_0(GRAPH_GRAD_)                                                           \
+  do {                                                                                           \
+    if constexpr (!ARC) {                                                                        \
+      if (lat->dtype == GTNB_BF16) {                                                             \
+        GTNB_LAUNCH_BWD_E((implicit_backward_kernel<GRAPH_GRAD_, false, bf16_t>), bf16_t);       \
+        break;                                                                                   \
+      }                                                                                          \
+      if (lat->dtype == GTNB_F16) {                                                              \
+        GTNB_LAUNCH_BWD_E((implicit_backward_kernel<GRAPH_GRAD_, false, f16_t>), f16_t);         \
+        break;                                                                                   \
+      }                                                                                          \
+    }                                                                                            \
+    GTNB_LAUNCH_BWD((implicit_backward_kernel<GRAPH_GRAD_, ARC>));                               \
   } while (0)
 #define GTNB_LAUNCH_BWD_G(GG)                                               \
   do {                                                                      \
@@ -1451,9 +1505,9 @@ int implicit_backward_mode(
   switch (G) {
     case 0:
       if (grad_graph)
-        GTNB_LAUNCH_BWD((implicit_backward_kernel<true, ARC>));
+        GTNB_LAUNCH_BWD_0(true);
       else
-        GTNB_LAUNCH_BWD((implicit_backward_kernel<false, ARC>));
+        GTNB_LAUNCH_BWD_0(false);
       break;
     case 1: GTNB_LAUNCH_BWD_G(1); break;
     case 2: GTNB_LAUNCH_BWD_G(2); break;
@@ -1462,8 +1516,10 @@ int implicit_backward_mode(
     case 16: GTNB_LAUNCH_BWD_G(16); break;
     default: GTNB_LAUNCH_BWD_G(32); break;
   }
+#undef GTNB_LAUNCH_BWD_0
 #undef GTNB_LAUNCH_BWD_G
 #undef GTNB_LAUNCH_BWD
+#undef GTNB_LAUNCH_BWD_E
   return GTNB_OK;
 }
 
@@ -1497,6 +1553,8 @@ bool implicit_trace_supported(const gtnb_lattice* lat) {
 int launch_implicit_trace(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int32_t* paths, int32_t* arcs,
                           float* scores_out, int T_out) {
   if (lat->B <= 0) return GTNB_OK;
+  if (lat->dtype != GTNB_F32)
+    return fail(ctx, GTNB_ERR_LOGIC, "launch_implicit_trace: no instantiation for 16-bit emissions");
   const TraceLayout lay = trace_layout(lat);
   if (lay.total > kMaxDynamicSmem) return fail(ctx, GTNB_ERR_UNSUPPORTED, "implicit_trace: graphs too large");
   if (lay.total > 48 * 1024) {

@@ -31,6 +31,12 @@
  * alpha_1 = e[0] + s, and the rows are kept relative to per-frame offsets accumulated in double (see the forward
  * kernel).  Its numerator, compose(fal_b, transitions), is a U+1-node chain that asg_num_build_kernel writes into the
  * same small-graph tables for k_implicit.cu's sweeps; it needs no fold.
+ *
+ * Both trellis kernels take the element type E of the emissions as a template parameter (float, or bf16_t / f16_t for
+ * gtnb_ngram_ctc_loss_typed / gtnb_asg_loss_typed): each element is widened to float32 exactly (prefetched as its
+ * bits and widened where the frame uses it), the is_finite checks see the widened value, and everything after the
+ * load is the float32 kernel's own.  The emission gradient stays float32; E = float compiles to the float32 kernels
+ * as they were.
  */
 #include <algorithm>
 
@@ -88,9 +94,9 @@ __device__ __forceinline__ double* asg_offsets(float* alpha, int B, int T, int C
  * accumulated in double (asg_offsets; c_1 = 0): the stored rows stay within a frame's spread of scores, so the
  * backward kernel's posteriors exp(alpha + beta - Z) do not cancel fp32 scores that grow with t.
  */
-template <int K, bool START = false>
+template <int K, bool START = false, class E = float>
 __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
-    int T, int C, int lanes, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    int T, int C, int lanes, const int32_t* __restrict__ lens, const E* __restrict__ emis, long long stride,
     const float* __restrict__ W, float* __restrict__ alpha, float* __restrict__ den, int32_t* __restrict__ status) {
   GTNB_STATIC_SMEM_2D(float, A, 2, kNgramMaxC);
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -98,7 +104,7 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   const int i = tid / lanes, q = tid % lanes;
   const bool row = i < C;
   const bool lead = row && q == 0;
-  const float* em = emis + (long long)b * stride;
+  const E* em = emis + (long long)b * stride;
   const float* Wm = START ? W + C : W;
   float* al = alpha + (long long)b * (T + 1) * C;
   double* cs = START ? asg_offsets(alpha, gridDim.x, T, C, b) : nullptr;
@@ -120,10 +126,12 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
   for (int j = tid; j < kNgramMaxC; j += blockDim.x) A[0][j] = A[1][j] = 0.0f; // alpha_0 = 0; padding stays 0
   for (int j = tid; j < C; j += blockDim.x) al[j] = 0.0f;
   __syncthreads();
-  float e_nx = (lead && Tb > 0) ? __ldg(em + i) : 0.0f;
+  // the next frame's emission, one frame ahead; a 16-bit one stays in its bits until the frame uses it, so the
+  // load is not waited for before the frame's barrier
+  ring_t<E> e_nx = (lead && Tb > 0) ? ldg_ring(em + i) : ring_t<E>(0);
   if (START && Tb > 0) { // alpha_1 = e[0] + s
-    const float e = e_nx;
-    if (lead && Tb > 1) e_nx = __ldg(em + C + i);
+    const float e = ring_f32<E>(e_nx);
+    if (lead && Tb > 1) e_nx = ldg_ring(em + C + i);
     bad |= !is_finite(e);
     if (lead) {
       const float v = e + s_i;
@@ -134,8 +142,8 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
     __syncthreads();
   }
   for (int t = START ? 2 : 1; t <= Tb; t++) {
-    const float e = e_nx;
-    if (lead && t < Tb) e_nx = __ldg(em + (long long)t * C + i);
+    const float e = ring_f32<E>(e_nx);
+    if (lead && t < Tb) e_nx = ldg_ring(em + (long long)t * C + i);
     bad |= !is_finite(e);
     const float* P = A[(t - 1) & 1];
     float x[K];
@@ -191,9 +199,9 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_forward_kernel(
  * kernel, beta_t = row_t + d_t with d_{t-1} = d_t + G[0] in double (d_T = 0), and a posterior's exponent is
  * row + row' + (float)(c + d - Z).
  */
-template <int K, bool START = false>
+template <int K, bool START = false, class E = float>
 __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
-    int T, int C, int lanes, const int32_t* __restrict__ lens, const float* __restrict__ emis, long long stride,
+    int T, int C, int lanes, const int32_t* __restrict__ lens, const E* __restrict__ emis, long long stride,
     const float* __restrict__ W, const float* __restrict__ alpha, const float* __restrict__ den,
     float* __restrict__ grad, long long grad_stride, float* __restrict__ wgrad) {
   GTNB_STATIC_SMEM_2D(float, Bt, 2, kNgramMaxC); // beta_t, beta_{t-1}
@@ -205,7 +213,7 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
   const int j = tid / lanes, q = tid % lanes;
   const bool col = j < C;
   const bool lead = col && q == 0;
-  const float* em = emis + (long long)b * stride;
+  const E* em = emis + (long long)b * stride;
   const float* al = alpha + (long long)b * (T + 1) * C;
   float* gr = grad + (long long)b * grad_stride;
   const float* Wm = START ? W + C : W;
@@ -226,16 +234,32 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
   // one frame of prefetch: alpha_t and e[t-1] of the rows this thread turns into G, alpha_{t-1} of its column
   const bool rowt = tid < C;
   float a_nx = rowt ? al[(long long)Tb * C + tid] : 0.0f;
-  float e_nx = rowt ? __ldg(em + (long long)(Tb - 1) * C + tid) : 0.0f;
+  // the emission prefetch as in the forward kernel, but for ASG's start mode at K = 32: there the extra live register
+  // of the 16 bits would spill 4 bytes more than the float32 kernel, so the element is widened where it is loaded
+  constexpr bool kBits = !(START && K == 32);
+  using Pf = std::conditional_t<kBits, ring_t<E>, float>;
+  auto load_e = [&](long long k) -> Pf {
+    if constexpr (kBits)
+      return ldg_ring(em + k);
+    else
+      return ldg_elem(em + k);
+  };
+  auto use_e = [](Pf v) -> float {
+    if constexpr (kBits)
+      return ring_f32<E>(v);
+    else
+      return v;
+  };
+  Pf e_nx = rowt ? load_e((long long)(Tb - 1) * C + tid) : Pf(0);
   float aj_nx = col ? al[(long long)(Tb - 1) * C + j] : 0.0f;
   __syncthreads();
   for (int t = Tb; t >= 1; t--) {
-    const float a_t = a_nx, e_t = e_nx, aj = aj_nx;
+    const float a_t = a_nx, e_t = use_e(e_nx), aj = aj_nx;
     const double c_prev = c_nx; // START: c_{t-1}
     if (t > 1) {
       if (rowt) {
         a_nx = al[(long long)(t - 1) * C + tid];
-        e_nx = __ldg(em + (long long)(t - 2) * C + tid);
+        e_nx = load_e((long long)(t - 2) * C + tid);
       }
       if (col) aj_nx = al[(long long)(t - 2) * C + j];
       if (START && t > 2) c_nx = cs[t - 2];
@@ -514,64 +538,84 @@ int launch_ngram_num_build(
 
 namespace {
 
-template <bool START>
-int den_forward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int32_t* lens_dev, const float* emis,
+template <bool START, class E>
+int den_forward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int32_t* lens_dev, const E* emis,
                 long long stride, const float* W, float* alpha, float* den, int32_t* status) {
   if (B == 0) return GTNB_OK;
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
   if (K == 16)
-    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<16, START><<<B, threads, 0, ctx->stream>>>(
+    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<16, START, E><<<B, threads, 0, ctx->stream>>>(
         T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
   else
-    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<32, START><<<B, threads, 0, ctx->stream>>>(
+    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<32, START, E><<<B, threads, 0, ctx->stream>>>(
         T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
   return GTNB_OK;
 }
 
-template <bool START>
-int den_backward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int32_t* lens_dev, const float* emis,
+template <bool START, class E>
+int den_backward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int32_t* lens_dev, const E* emis,
                  long long stride, const float* W, const float* alpha, const float* den, float* grad,
                  long long grad_stride, float* wgrad) {
   if (B == 0) return GTNB_OK;
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
   if (K == 16)
-    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<16, START><<<B, threads, 0, ctx->stream>>>(
+    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<16, START, E><<<B, threads, 0, ctx->stream>>>(
         T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
   else
-    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<32, START><<<B, threads, 0, ctx->stream>>>(
+    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<32, START, E><<<B, threads, 0, ctx->stream>>>(
         T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
   return GTNB_OK;
+}
+
+/* f(typed emissions) for the element type dtype names (GTNB_F32 / GTNB_BF16 / GTNB_F16) */
+template <class F>
+int with_elem(gtnb_ctx* ctx, int dtype, const void* emis, F&& f) {
+  switch (dtype) {
+    case GTNB_F32: return f(static_cast<const float*>(emis));
+    case GTNB_BF16: return f(static_cast<const bf16_t*>(emis));
+    case GTNB_F16: return f(static_cast<const f16_t*>(emis));
+    default: return fail(ctx, GTNB_ERR_LOGIC, "k_ngram.cu: unknown element type");
+  }
 }
 
 } // namespace
 
 int launch_ngram_den_forward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* W, float* alpha, float* den, int32_t* status) {
-  return den_forward<false>(ctx, "ngram_den_forward", B, T, C, lens_dev, emis, stride, W, alpha, den, status);
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
+    const float* W, float* alpha, float* den, int32_t* status, int dtype) {
+  return with_elem(ctx, dtype, emis, [&](auto e) {
+    return den_forward<false>(ctx, "ngram_den_forward", B, T, C, lens_dev, e, stride, W, alpha, den, status);
+  });
 }
 
 int launch_ngram_den_backward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad) {
-  return den_backward<false>(ctx, "ngram_den_backward", B, T, C, lens_dev, emis, stride, W, alpha, den, grad,
-                             grad_stride, wgrad);
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
+    const float* W, const float* alpha, const float* den, float* grad, long long grad_stride, float* wgrad,
+    int dtype) {
+  return with_elem(ctx, dtype, emis, [&](auto e) {
+    return den_backward<false>(ctx, "ngram_den_backward", B, T, C, lens_dev, e, stride, W, alpha, den, grad,
+                               grad_stride, wgrad);
+  });
 }
 
 int launch_asg_den_forward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
-    const float* trans_w, float* alpha, float* den, int32_t* status) {
-  return den_forward<true>(ctx, "asg_den_forward", B, T, C, lens_dev, emis, stride, trans_w, alpha, den, status);
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
+    const float* trans_w, float* alpha, float* den, int32_t* status, int dtype) {
+  return with_elem(ctx, dtype, emis, [&](auto e) {
+    return den_forward<true>(ctx, "asg_den_forward", B, T, C, lens_dev, e, stride, trans_w, alpha, den, status);
+  });
 }
 
 int launch_asg_den_backward(
-    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const float* emis, long long stride,
+    gtnb_ctx* ctx, int B, int T, int C, const int32_t* lens_dev, const void* emis, long long stride,
     const float* trans_w, const float* alpha, const float* den, float* grad, long long grad_stride,
-    float* trans_grad) {
-  return den_backward<true>(ctx, "asg_den_backward", B, T, C, lens_dev, emis, stride, trans_w, alpha, den, grad,
-                            grad_stride, trans_grad);
+    float* trans_grad, int dtype) {
+  return with_elem(ctx, dtype, emis, [&](auto e) {
+    return den_backward<true>(ctx, "asg_den_backward", B, T, C, lens_dev, e, stride, trans_w, alpha, den, grad,
+                              grad_stride, trans_grad);
+  });
 }
 
 int launch_asg_num_build(

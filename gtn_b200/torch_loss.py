@@ -55,21 +55,27 @@ def _allreduce_transitions(ctx, tg, allreduce):
 
 
 def _transition_backward(ctx, grad_output):
-    """(emission gradient, transition gradient) of asg_loss / ngram_ctc_loss times the upstream gradient"""
+    """(emission gradient, transition gradient) of asg_loss / ngram_ctc_loss times the upstream gradient; the emission
+    gradient keeps its dtype (float32, or the 16-bit dtype of the emissions)"""
     grad, tg = ctx.saved_tensors
     if ctx.reduction == "mean":
         # the mean over the GLOBAL batch when the transition gradient was summed over the ranks
         scale = grad_output / ctx.B
         return grad * scale, tg * (scale / ctx.world)
     # reduction "none": the incoming gradient is per utterance; the transition gradient was already summed
-    # over the batch inside the kernel, which is only the chain rule's answer for a uniform grad_output
-    assert bool((grad_output == grad_output.flatten()[0]).all()), \
-        "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
-    return grad * grad_output.view(-1, 1, 1), tg * grad_output.flatten()[0]
+    # over the batch inside the kernel, which is only the chain rule's answer for a uniform grad_output (the
+    # emission gradient is right for any grad_output, so transitions that need no gradient take any)
+    if ctx.needs_input_grad[1]:
+        assert bool((grad_output == grad_output.flatten()[0]).all()), \
+            "reduction='none' supports a uniform upstream gradient (sum / mean of the losses)"
+    # (a 16-bit grad times the float32 [B] upstream gradient promotes to float32: back to the emissions' dtype)
+    return (grad * grad_output.view(-1, 1, 1)).to(grad.dtype), tg * grad_output.flatten()[0]
 
 
-# the element types of ctc_loss's emissions, as gtnb_ctc_loss_ex names them
+# the element types of the emissions of ctc_loss, asg_loss, ngram_ctc_loss and the dense Viterbi decoders, as the
+# C ABI names them (gtnb_ctc_loss_ex, gtnb_*_typed)
 _CTC_DTYPES = {torch.float32: capi.F32, torch.bfloat16: capi.BF16, torch.float16: capi.F16}
+_EMISSION_DTYPES = _CTC_DTYPES
 
 
 class CTCLossFunction(torch.autograd.Function):
@@ -136,26 +142,47 @@ class ASGLossFunction(torch.autograd.Function):
     minibatch -- and by all ranks: with torch.distributed initialised, the transition gradient of the local shard
     is all-reduced (sum) over NCCL, the multi-GPU form of Graph::addGrad under grad_lock (graph.cpp:96-100).
 
-    emissions: float32 CUDA tensor [B, T, C]; transitions: float32 tensor [C + C*C] (start weights, then the
-    C x C matrix, row = destination label) on any device; targets: list of 1-D int sequences.
+    emissions: float32, bfloat16 or float16 CUDA tensor [B, T, C]; transitions: float32 tensor [C + C*C] (start
+    weights, then the C x C matrix, row = destination label) on any device; targets: list of 1-D int sequences.
+    The losses are float32 whatever the emissions' dtype.
 
     input_lengths: None (T frames each), a list or an int tensor (any device).  When given, e_b is the first
     input_lengths[b] frames (the gradient of the padding frames is 0) and the call goes through gtnb_asg_loss_ex
     on device pointers: transitions must then be a float32 CUDA tensor on the emissions' device, and the
     transition gradient stays on the device.
+
+    Half-precision emissions (bf16 / fp16 logits of a model under torch.autocast) go in as they are, through
+    gtnb_asg_loss_typed: the losses and the transition gradient are those of the float32 call on emissions.float(),
+    bit for bit, and the emission gradient, kept for backward in the emissions' dtype, is that call's float32
+    gradient rounded to the dtype.  Without input_lengths that call takes T_b = T, with the transitions copied to the
+    emissions' device as float32 and their gradient returned on transitions.device: asg_loss(e, ...) then equals
+    asg_loss(e.float(), ..., input_lengths=[T] * B).
     """
 
     @staticmethod
     def forward(ctx, emissions, transitions, targets, reduction="mean", allreduce=True, input_lengths=None):
-        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        assert emissions.is_cuda and emissions.dim() == 3
+        assert emissions.dtype in _EMISSION_DTYPES, "asg_loss: emissions must be float32, bfloat16 or float16"
         e = emissions.contiguous()
         B, T, Cn = e.shape
+        half = e.dtype != torch.float32
         assert transitions.numel() == Cn + Cn * Cn
         stream = torch.cuda.current_stream(e.device).cuda_stream
         g = _ctx_for(e.device, stream)
         cat, lens = capi._cat_targets(targets)
         losses = np.zeros(B, np.float32)
-        if input_lengths is not None:
+        if half:
+            assert transitions.dtype == torch.float32, "asg_loss: transitions must be float32"
+            il = _lengths(input_lengths, B)
+            w = transitions.detach().to(e.device).contiguous()
+            grad = torch.empty_like(e)  # every row is written by the call
+            tg = torch.empty(Cn + Cn * Cn, dtype=torch.float32, device=e.device)
+            g._check(capi.lib().gtnb_asg_loss_typed(
+                g.h, B, T, Cn, e.data_ptr(), _EMISSION_DTYPES[e.dtype], None if il is None else il.ctypes.data_as(capi._i32p),
+                w.data_ptr(), cat.ctypes.data_as(capi._i32p), lens.ctypes.data_as(capi._i32p),
+                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), tg.data_ptr()))
+            tg = tg.view_as(transitions)
+        elif input_lengths is not None:
             assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
             il = _lengths(input_lengths, B)
             w = transitions.detach().contiguous()
@@ -200,15 +227,22 @@ class NgramCTCLossFunction(torch.autograd.Function):
     label, column = source label), shared by the minibatch and, with torch.distributed initialised, by all ranks
     (the transition gradient is all-reduced over NCCL, as asg_loss does).
 
-    emissions: float32 CUDA tensor [B, T, C]; transitions: float32 CUDA tensor of C*C elements ([C, C] or flat) on
-    the same device; targets: list of 1-D int sequences; input_lengths: None, a list or an int tensor (any
-    device).  Everything runs on the current stream of the emissions' device, device pointers in and out: only
-    the B losses (and input_lengths, when given on the GPU) are copied to the host.
+    emissions: float32, bfloat16 or float16 CUDA tensor [B, T, C]; transitions: float32 CUDA tensor of C*C elements
+    ([C, C] or flat) on the same device; targets: list of 1-D int sequences; input_lengths: None, a list or an int
+    tensor (any device).  Everything runs on the current stream of the emissions' device, device pointers in and
+    out: only the B losses (and input_lengths, when given on the GPU) are copied to the host.  The losses are
+    float32 whatever the emissions' dtype.
+
+    Half-precision emissions (bf16 / fp16 logits of a model under torch.autocast) go in as they are, through
+    gtnb_ngram_ctc_loss_typed: the losses and the transition gradient are those of the float32 call on
+    emissions.float(), bit for bit, and the emission gradient, kept for backward in the emissions' dtype, is that
+    call's float32 gradient rounded to the dtype.
     """
 
     @staticmethod
     def forward(ctx, emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True):
-        assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+        assert emissions.is_cuda and emissions.dim() == 3
+        assert emissions.dtype in _EMISSION_DTYPES, "ngram_ctc_loss: emissions must be float32, bfloat16 or float16"
         e = emissions.contiguous()
         B, T, Cn = e.shape
         assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
@@ -221,10 +255,17 @@ class NgramCTCLossFunction(torch.autograd.Function):
         losses = np.zeros(B, np.float32)
         grad = torch.empty_like(e)  # every row is written by the call
         tg = torch.empty(Cn * Cn, dtype=torch.float32, device=e.device)
-        g._check(capi.lib().gtnb_ngram_ctc_loss(
-            g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), w.data_ptr(), 1,
-            cat.ctypes.data_as(capi._i32p), lens.ctypes.data_as(capi._i32p), int(blank),
-            losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, tg.data_ptr(), 1))
+        il_p = None if il is None else il.ctypes.data_as(capi._i32p)
+        if e.dtype == torch.float32:
+            g._check(capi.lib().gtnb_ngram_ctc_loss(
+                g.h, B, T, Cn, e.data_ptr(), 1, il_p, w.data_ptr(), 1,
+                cat.ctypes.data_as(capi._i32p), lens.ctypes.data_as(capi._i32p), int(blank),
+                losses.ctypes.data_as(capi._f32p), grad.data_ptr(), 1, tg.data_ptr(), 1))
+        else:
+            g._check(capi.lib().gtnb_ngram_ctc_loss_typed(
+                g.h, B, T, Cn, e.data_ptr(), _EMISSION_DTYPES[e.dtype], il_p, w.data_ptr(), cat.ctypes.data_as(capi._i32p),
+                lens.ctypes.data_as(capi._i32p), int(blank), losses.ctypes.data_as(capi._f32p), grad.data_ptr(),
+                tg.data_ptr()))
         tg = tg.view_as(transitions)
         _allreduce_transitions(ctx, tg, allreduce)
         out = torch.from_numpy(losses).to(e.device)
@@ -245,7 +286,8 @@ def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0,
 
 @torch.no_grad()
 def _viterbi_dense(emissions, transitions, input_lengths, kind):
-    assert emissions.is_cuda and emissions.dtype == torch.float32 and emissions.dim() == 3
+    assert emissions.is_cuda and emissions.dim() == 3
+    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
     e = emissions.contiguous()
     B, T, Cn = e.shape
     assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
@@ -260,9 +302,14 @@ def _viterbi_dense(emissions, transitions, input_lengths, kind):
     # is the legacy default stream (the context then has a stream of its own): order the two both ways
     ctx_stream = torch.cuda.ExternalStream(capi.lib().gtnb_ctx_stream(g.h), device=e.device)
     ctx_stream.wait_stream(current)
-    g._check(capi.lib().gtnb_viterbi_dense_ex(
-        g.h, B, T, Cn, e.data_ptr(), 1, None if il is None else il.ctypes.data_as(capi._i32p), kind, w.data_ptr(), 1,
-        paths.data_ptr(), scores.data_ptr(), 1))
+    il_p = None if il is None else il.ctypes.data_as(capi._i32p)
+    if e.dtype == torch.float32:
+        g._check(capi.lib().gtnb_viterbi_dense_ex(
+            g.h, B, T, Cn, e.data_ptr(), 1, il_p, kind, w.data_ptr(), 1, paths.data_ptr(), scores.data_ptr(), 1))
+    else:  # 16-bit emissions, read in place by the kernel
+        g._check(capi.lib().gtnb_viterbi_dense_typed(
+            g.h, B, T, Cn, e.data_ptr(), _EMISSION_DTYPES[e.dtype], il_p, kind, w.data_ptr(), paths.data_ptr(),
+            scores.data_ptr()))
     current.wait_stream(ctx_stream)
     return paths, scores
 
@@ -271,9 +318,10 @@ def asg_viterbi(emissions, transitions, input_lengths=None):
     """Best path of compose(E_b, transitions) for every utterance, with the transitions asg_loss trains
     (examples/asg.cpp's decoding, test/criterion_test.cpp:328-344), through gtnb_viterbi_dense_ex.
 
-    emissions: float32 CUDA tensor [B, T, C]; transitions: float32 CUDA tensor of C + C*C elements (start weights,
-    then the C x C matrix, row = destination label) on the same device; input_lengths: None, a list or an int tensor
-    (any device).  Returns (paths [B, T] int32, the label of every frame, -1 beyond T_b; scores [B], viterbiScore,
+    emissions: float32, bfloat16 or float16 CUDA tensor [B, T, C] (16-bit emissions go through
+    gtnb_viterbi_dense_typed: the paths and scores of the float32 call on emissions.float(), ties included);
+    transitions: float32 CUDA tensor of C + C*C elements (start weights, then the C x C matrix, row = destination
+    label) on the same device; input_lengths: None, a list or an int tensor (any device).  Returns (paths [B, T] int32, the label of every frame, -1 beyond T_b; scores [B], viterbiScore,
     -inf for T_b = 0), both CUDA tensors written on the current stream; only input_lengths visits the host.
     """
     return _viterbi_dense(emissions, transitions, input_lengths, capi.DENSE_ASG)

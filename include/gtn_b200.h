@@ -353,7 +353,7 @@ int gtnb_ctc_loss(
     float* grads,
     int grads_on_device);
 
-#define GTNB_F32 0 /* float32 elements */
+#define GTNB_F32 0 /* float32 elements (the dtype of the *_ex / *_typed entry points) */
 #define GTNB_BF16 1 /* bfloat16 elements */
 #define GTNB_F16 2 /* IEEE half-precision elements */
 
@@ -473,6 +473,51 @@ int gtnb_ngram_ctc_loss(
     int trans_grad_on_device);
 
 /*
+ * gtnb_ngram_ctc_loss and gtnb_asg_loss_ex on device buffers of a chosen element type: emissions_dev and grads_dev
+ * (nullable) are [B][T][C] of dtype (GTNB_F32, GTNB_BF16 or GTNB_F16), all buffers live on the device, and
+ * trans_w_dev, trans_grad_dev (nullable) and losses_host stay float32.  Targets, lengths, blank, infeasible targets,
+ * T_b = 0, non-finite values, the zeroed rows t >= T_b and every argument check follow the float32 call.
+ * The result is that call's on the emissions widened to float32 (exact): the same losses and transition gradient,
+ * bit for bit, and its float32 emission gradient rounded to dtype (to nearest, ties to even).  The arithmetic is
+ * float32 throughout.  A batch that the float32 call sends to the dense trellis (k_ngram.cu) and the device-built
+ * numerators (k_implicit.cu) -- C <= 128, the "implicit" flag on, numerator graphs inside the implicit layout, every
+ * weight and used emission finite -- is read in place by those kernels, whose gradient is rounded into grads_dev
+ * once.  Any other batch (ASG with C > 128, the flag off, the exact retry after a non-finite value) is widened into
+ * float32 scratch once, run as the float32 call runs it, and its gradient rounded into grads_dev.  GTNB_F32 is the
+ * float32 call with every buffer on the device; an unknown dtype is GTNB_ERR_INVALID_ARGUMENT.
+ */
+int gtnb_ngram_ctc_loss_typed(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev,
+    int dtype,
+    const int32_t* input_lens, /* host, nullable */
+    const float* trans_w_dev,
+    const int32_t* targets,
+    const int32_t* target_lens,
+    int blank,
+    float* losses_host,
+    void* grads_dev, /* nullable */
+    float* trans_grad_dev); /* nullable */
+
+int gtnb_asg_loss_typed(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev,
+    int dtype,
+    const int32_t* input_lens, /* host, nullable */
+    const float* trans_w_dev,
+    const int32_t* targets,
+    const int32_t* target_lens,
+    float* losses_host,
+    void* grads_dev, /* nullable */
+    float* trans_grad_dev); /* nullable */
+
+/*
  * Loss over one user-supplied target graph per utterance (the criterion of the reference's pytorch_loss.py and of
  * its word-decomposition examples):
  *   loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b))
@@ -568,6 +613,27 @@ int gtnb_viterbi_dense_ex(
     int32_t* paths, /* nullable */
     float* scores, /* nullable */
     int outputs_on_device);
+
+/*
+ * gtnb_viterbi_dense_ex on device buffers with emissions of a chosen element type: emissions_dev [B][T][C] of dtype
+ * (GTNB_F32, GTNB_BF16 or GTNB_F16); trans_w_dev, paths_dev (nullable) and scores_dev (nullable) on the device, the
+ * call returning once the work is enqueued.  The factored kernel (k_dense.cu) reads the 16-bit emissions in place and
+ * widens each on load, so paths and scores are == gtnb_viterbi_dense_ex's on the emissions widened to float32, ties
+ * included, for every batch.  GTNB_F32 is gtnb_viterbi_dense_ex with every buffer on the device; an unknown dtype is
+ * GTNB_ERR_INVALID_ARGUMENT.
+ */
+int gtnb_viterbi_dense_typed(
+    gtnb_ctx* ctx,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev,
+    int dtype,
+    const int32_t* input_lens, /* host, nullable */
+    int kind,
+    const float* trans_w_dev,
+    int32_t* paths_dev, /* nullable */
+    float* scores_dev); /* nullable */
 
 /*
  * Loss over one user-supplied target graph per utterance with a learned dense transition graph G (the word
