@@ -100,6 +100,11 @@ SYMBOLS = [
       C.c_int]),
     ("gtnb_ctc_loss_ex", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _i32p, _i32p, C.c_int, _f32p, _vp]),
+    ("gtnb_ctc_loss_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp,
+      C.c_size_t]),
+    ("gtnb_ctc_loss_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     ("gtnb_ngram_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int, _vp, C.c_int]),

@@ -11,6 +11,7 @@
 #include <cstring>
 #include <deque>
 #include <limits>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -608,6 +609,167 @@ extern "C" int gtnb_ctc_loss_ex(
     return ctc_loss_run(scope, B, T, C, emissions_dev, 1, input_lens, targets, target_lens, blank, losses_host,
                         grads_dev, 1, implicit, needs_exact, dtype);
   });
+}
+
+namespace {
+
+/*
+ * The context's arena pointed at a caller's block for one gtnb_ctc_loss_async call (base NULL: sizing only, nothing
+ * is launched).  dev_alloc fails once the block is full instead of allocating; the context's own arena is back when
+ * the scope ends.
+ */
+class BorrowedArena {
+ public:
+  BorrowedArena(gtnb_ctx* ctx, void* base, size_t bytes) : ctx_(ctx), arena_(ctx->arena), cap_(ctx->arena_cap) {
+    ctx->arena = static_cast<unsigned char*>(base);
+    ctx->arena_cap = bytes;
+    ctx->arena_borrowed = true;
+    arena_begin(ctx);
+  }
+  ~BorrowedArena() {
+    ctx_->arena_on = false;
+    ctx_->arena_borrowed = false;
+    ctx_->arena = arena_;
+    ctx_->arena_cap = cap_;
+  }
+  BorrowedArena(const BorrowedArena&) = delete;
+  BorrowedArena& operator=(const BorrowedArena&) = delete;
+  size_t need() const { return ctx_->arena_need; }
+
+ private:
+  gtnb_ctx* ctx_;
+  unsigned char* arena_;
+  size_t cap_;
+};
+
+struct CtcAsyncArgs {
+  int B, T, C, S, dtype;
+  const void* emissions;
+  const int32_t *input_lens, *targets, *target_lens;
+  int blank;
+  float* losses;
+  int32_t* status;
+  void* grads;
+};
+
+/*
+ * gtnb_ctc_loss_async inside a BorrowedArena: the scratch of the call taken from the arena and, when launch, the
+ * call enqueued.  The route is ctc_loss_run's for a batch at the bounds (every utterance U = S, T_b = T, S - 1 skip
+ * arcs), decided from the bounds, the dtype, the buffers' alignment and the context's flags; the prepare kernel
+ * then writes every utterance's own descriptor over the bound-uniform slabs.  Sizing passes NULL buffers: a 16-bit
+ * batch is then sized for the widened route, which needs more scratch than reading the buffers in place.
+ */
+int ctc_async_run(gtnb_ctx* ctx, const CtcAsyncArgs& a, bool launch) {
+  const int B = a.B, T = a.T, C = a.C, S = a.S;
+  const bool half = a.dtype != GTNB_F32;
+  const long long per = (long long)T * C;
+  if (!ctx->use_implicit)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: the \"implicit\" flag is off (materialised route)");
+  if (a.blank < 0 || a.blank >= C) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: blank outside [0, C)");
+  const int L = 2 * S + 1;
+  const std::vector<SgDims> dims(B, SgDims{L, L + (L - 1) + std::max(S - 1, 0), L >= 2 ? 2 : 1, 1, 1, 3, 3});
+  if (!implicit_dims_supported(dims.data(), B))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: bounds outside the implicit sweeps");
+  const std::vector<int32_t> Tv(B, T);
+  std::vector<long long> sgn, sga;
+  gtnb_lattice* lat_raw = nullptr;
+  GTNB_TRY(composed_alloc(ctx, B, dims.data(), B, 0, Tv.data(), C, static_cast<const float*>(a.emissions), per, sgn,
+                          sga, &lat_raw, true));
+  const std::unique_ptr<gtnb_lattice> lat(lat_raw); // (its device buffers lie in the arena: nothing to free)
+  int32_t *small = nullptr, *valid = nullptr, *kstatus = nullptr;
+  float* deltas = nullptr;
+  GTNB_TRY(dev_alloc(ctx, &small, 3ll * B));
+  GTNB_TRY(dev_alloc(ctx, &valid, B));
+  GTNB_TRY(dev_alloc(ctx, &kstatus, B));
+  GTNB_TRY(dev_alloc(ctx, &deltas, B));
+  // 16-bit buffers in place when k_bidir.cu takes them, else widened into float32 scratch (ctc_loss_run's rule)
+  const bool native = half && a.emissions && ctx->use_bidir &&
+                      bidir_supported(lat.get(), a.emissions, per, a.grads, per, a.dtype);
+  const float* e = static_cast<const float*>(a.emissions);
+  float* g = static_cast<float*>(a.grads);
+  if (half && !native) {
+    float* wide = nullptr;
+    GTNB_TRY(dev_alloc(ctx, &wide, per * B));
+    lat->emissions = e = wide;
+    if (a.grads) GTNB_TRY(dev_alloc(ctx, &g, per * B));
+  }
+  const bool bidir = ctx->use_bidir && (native || bidir_supported(lat.get(), e, per, g, per));
+  const bool direct = bidir && ctx->bidir_mode != 0 && bidir_takes_targets(lat.get(), a.blank);
+  // [partial sums of forwardScore(e) | lattice scores] and the block offsets of k_bidir.cu, or the normaliser's
+  // scores and per-frame rows of the sweeps; sizing takes both, since the alignment of the buffers decides
+  float *z = nullptr, *s = nullptr, *boff = nullptr, *rows = nullptr;
+  const int zp = bidir ? 2 * bidir_zparts() : 1;
+  if (bidir || !launch) {
+    GTNB_TRY(dev_alloc(ctx, &z, 2ll * bidir_zparts() * B + B));
+    s = z + (long long)zp * B;
+    GTNB_TRY(dev_alloc(ctx, &boff, 8ll * B * bidir_blocks(T)));
+  }
+  if (!bidir || !launch) {
+    GTNB_TRY(dev_alloc(ctx, &z, B));
+    GTNB_TRY(dev_alloc(ctx, &rows, (long long)B * std::max(T, 1)));
+    s = lat->out_scores;
+  }
+  if (!launch) return GTNB_OK;
+
+  // the gradient the kernels write: the caller's (float32, or 16-bit in place) or the float32 scratch of the widened
+  // route, which launch_narrow rounds into the caller's at the end
+  void* gk = native ? a.grads : static_cast<void*>(g);
+  const long long row_words = native ? per / 2 : per;
+  if (gk && a.input_lens) GTNB_CUDA(ctx, cudaMemsetAsync(gk, 0, 4ull * row_words * B, ctx->stream));
+  if (half && !native) GTNB_TRY(launch_widen(ctx, a.emissions, a.dtype, const_cast<float*>(e), per * B));
+  GTNB_TRY(launch_ctc_async_prepare(ctx, B, S, T, C, lat->meta_h[0], lat->meta_h[B > 1 ? 1 : 0], a.input_lens,
+                                    a.targets, a.target_lens, lat->meta, small, deltas, valid, kstatus));
+  if (!direct) GTNB_TRY(launch_ctc_build(ctx, lat.get(), a.targets, small, small + B, a.blank));
+  if (bidir) {
+    GTNB_TRY(launch_bidir_ctc(ctx, lat.get(), kstatus, z, boff, gk, per, 0, -1, s, a.blank, a.targets, small, nullptr,
+                              native ? a.dtype : GTNB_F32));
+  } else {
+    GTNB_TRY(launch_linear_forward(ctx, B, small + 2ll * B, T, C, e, per, 0, z, g, per, nullptr, 1.0f,
+                                   a.input_lens ? 0 : 1, rows));
+    GTNB_TRY(launch_implicit_forward(ctx, lat.get(), kstatus));
+    if (g) GTNB_TRY(launch_implicit_backward(ctx, lat.get(), deltas, g, per));
+  }
+  GTNB_TRY(launch_ctc_async_finalize(ctx, B, zp, z, s, kstatus, valid, a.losses, a.status, gk, row_words));
+  if (half && !native && a.grads) GTNB_TRY(launch_narrow(ctx, g, a.grads, a.dtype, per * B));
+  return GTNB_OK;
+}
+
+bool ctc_async_dtype(int dtype) { return dtype == GTNB_F32 || dtype == GTNB_BF16 || dtype == GTNB_F16; }
+
+} // namespace
+
+extern "C" int gtnb_ctc_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, int with_grad,
+                                             size_t* bytes) {
+  if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !bytes)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctc_loss_async_workspace: bad arguments");
+  if (!ctc_async_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async_workspace: unknown dtype");
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  // (the sizing reads the grads pointer for its presence only)
+  alignas(16) static float stand_in[4];
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  const CtcAsyncArgs a{B, T, C, S, dtype, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
+                       with_grad ? stand_in : nullptr};
+  GTNB_TRY(ctc_async_run(ctx, a, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+extern "C" int gtnb_ctc_loss_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, int S, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, const int32_t* targets_dev, const int32_t* target_lens_dev, int blank,
+    float* losses_dev, int32_t* status_dev, void* grads_dev, void* workspace_dev, size_t workspace_bytes) {
+  if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !emissions_dev || (S > 0 && !targets_dev) || !target_lens_dev ||
+      !losses_dev || (B > 0 && !workspace_dev) || ((uintptr_t)workspace_dev & 255))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctc_loss_async: bad arguments");
+  if (!ctc_async_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: unknown dtype");
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  const CtcAsyncArgs a{B, T, C, S, dtype, emissions_dev, input_lens_dev, targets_dev, target_lens_dev, blank,
+                       losses_dev, status_dev, grads_dev};
+  return ctc_async_run(ctx, a, true);
 }
 
 namespace {

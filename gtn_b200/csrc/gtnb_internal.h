@@ -74,6 +74,8 @@ struct gtnb_ctx {
   unsigned char* arena = nullptr;
   size_t arena_cap = 0, arena_off = 0, arena_need = 0;
   bool arena_on = false;
+  // the arena is a caller's workspace (gtnb_ctc_loss_async): dev_alloc fails instead of allocating once it is full
+  bool arena_borrowed = false;
   bool profiling = false;
   std::vector<ProfEntry> prof;
   std::vector<cudaEvent_t> ev_pool;
@@ -175,6 +177,17 @@ int readback_reserve(gtnb_ctx* ctx, size_t bytes);
 int launch_ctc_build(
     gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,
     const int32_t* tgt_len_dev, int blank);
+/* gtnb_ctc_loss_async's device-side set-up and epilogue (k_ctc.cu): m0 / m1 are the host descriptors of utterances 0
+ * and 1 (or 0 again) of the bound-uniform layout; small [3B] = [offsets | lens | T]; valid / kstatus [B] */
+int launch_ctc_async_prepare(
+    gtnb_ctx* ctx, int B, int S, int T, int C, const GraphMeta& m0, const GraphMeta& m1, const int32_t* input_lens,
+    const int32_t* targets, const int32_t* target_lens, GraphMeta* meta, int32_t* small, float* deltas,
+    int32_t* valid, int32_t* kstatus);
+/* losses / status [B] from the sweeps' partial sums z (zp per utterance), scores s and flags; grad (nullable):
+ * row_words 32-bit words per utterance, zeroed for a flagged one */
+int launch_ctc_async_finalize(
+    gtnb_ctx* ctx, int B, int zp, const float* z, const float* s, const int32_t* kstatus, const int32_t* valid,
+    float* losses, int32_t* status, void* grad, long long row_words);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
@@ -248,6 +261,8 @@ int dev_alloc(gtnb_ctx* ctx, T** p, long long n) {
       ctx->arena_off += sz;
       return GTNB_OK;
     }
+    if (ctx->arena_borrowed)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "workspace too small for these bounds (gtnb_ctc_loss_async_workspace)");
   }
   GTNB_CUDA(ctx, cudaMallocAsync((void**)p, bytes, ctx->stream));
   return GTNB_OK;

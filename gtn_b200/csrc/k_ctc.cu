@@ -116,9 +116,115 @@ __global__ void __launch_bounds__(256) ctc_build_kernel(
   }
 }
 
+/*
+ * gtnb_ctc_loss_async, before the sweeps: the descriptors and the small arrays of the batch, built on the device from
+ * the caller's padded targets.  One warp per utterance.  The slabs were laid out on the host at the bounds (U = S,
+ * T_b = T for every utterance), so they sit at a constant stride: every base of utterance b is m0's plus b times the
+ * step to m1 (m1 = m0 when B = 1).  The per-utterance fields are what composed_alloc and parse_targets give for the
+ * utterance's own target: T = T_b, L = T_b + 1, sg_N = 2U + 1, sg_A = 3U + 1 + skips, n_accept, tgt_off = b * S.
+ * small = [offsets | lens | T] (Targets::meta, with row b of the padded targets at b * S); deltas = -1 (subtract's
+ * gradFunc, read by the implicit backward).  An utterance with U outside [0, S], T_b outside [0, T] or a label
+ * outside [0, C) gets valid = 0 and is swept as U = 0, T_b = 0, so that no kernel indexes with its lengths or labels;
+ * the finalize kernel reports it.  kstatus, the sweeps' non-finite flags, starts at 0.
+ */
+__global__ void __launch_bounds__(256) ctc_async_prepare_kernel(
+    int B, int S, int T, int C, const GraphMeta m0, const GraphMeta m1,
+    const int32_t* __restrict__ input_lens, // nullable: T each
+    const int32_t* __restrict__ targets, // [B][S]
+    const int32_t* __restrict__ target_lens,
+    GraphMeta* __restrict__ meta, int32_t* __restrict__ small, float* __restrict__ deltas,
+    int32_t* __restrict__ valid, int32_t* __restrict__ kstatus) {
+  const int b = blockIdx.x * 8 + (int)(threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (b >= B) return;
+  int U = target_lens[b];
+  int Tb = input_lens ? input_lens[b] : T;
+  int ok = U >= 0 && U <= S && Tb >= 0 && Tb <= T;
+  int skips = 0;
+  if (ok) {
+    const int32_t* y = targets + (long long)b * S;
+    for (int u0 = 0; u0 < U; u0 += 32) { // (U is the warp's own: every lane runs the same trips)
+      const int u = u0 + lane;
+      const int32_t v = u < U ? y[u] : 0;
+      ok &= __ballot_sync(0xffffffffu, u < U && (unsigned)v >= (unsigned)C) == 0u;
+      skips += __popc(__ballot_sync(0xffffffffu, u > 0 && u < U && v != y[u - 1]));
+    }
+  }
+  if (lane != 0) return;
+  if (!ok) {
+    U = 0;
+    Tb = 0;
+    skips = 0;
+  }
+  const int L = 2 * U + 1;
+  GraphMeta m = m0;
+  m.node_base += b * (m1.node_base - m0.node_base);
+  m.arc_base += b * (m1.arc_base - m0.arc_base);
+  m.lvl_base += b * (m1.lvl_base - m0.lvl_base);
+  m.acc_base += b * (m1.acc_base - m0.acc_base);
+  m.sg_node_base += b * (m1.sg_node_base - m0.sg_node_base);
+  m.sg_arc_base += b * (m1.sg_arc_base - m0.sg_arc_base);
+  m.emis_off += b * (m1.emis_off - m0.emis_off);
+  m.grad_graph_off += b * (m1.grad_graph_off - m0.grad_graph_off);
+  m.L = Tb + 1;
+  m.n_accept = L >= 2 ? 2 : 1;
+  m.T = Tb;
+  m.sg_N = L;
+  m.sg_A = L + (L - 1) + skips;
+  m.tgt_off = b * S;
+  meta[b] = m;
+  small[b] = b * S;
+  small[B + b] = U;
+  small[2 * B + b] = Tb;
+  deltas[b] = -1.0f;
+  valid[b] = ok;
+  kstatus[b] = 0;
+}
+
+/*
+ * gtnb_ctc_loss_async, after the sweeps: losses[b] = sum_k z[zp * b + k] - s[b], added in the order of the host loop
+ * of ctc_loss_run, so the float32 loss is the synchronous call's.  status[b]: 2 for an utterance the prepare kernel
+ * refused, 1 where a sweep met a non-finite value (kstatus), else 0.  A flagged utterance gets a NaN loss and, when
+ * grad is set, a zero gradient (row_words 32-bit words per utterance).  One CTA per utterance.
+ */
+__global__ void __launch_bounds__(256) ctc_async_finalize_kernel(
+    int zp, const float* __restrict__ z, const float* __restrict__ s, const int32_t* __restrict__ kstatus,
+    const int32_t* __restrict__ valid, float* __restrict__ losses, int32_t* __restrict__ status,
+    uint32_t* __restrict__ grad, long long row_words) {
+  const int b = blockIdx.x;
+  const int st = !valid[b] ? 2 : kstatus[b] != 0 ? 1 : 0;
+  if (threadIdx.x == 0) {
+    float zb = 0.0f;
+    for (int k = 0; k < zp; k++) zb += z[(long long)zp * b + k];
+    losses[b] = st ? CUDART_NAN_F : zb - s[b];
+    if (status) status[b] = st;
+  }
+  if (st && grad)
+    for (long long i = threadIdx.x; i < row_words; i += blockDim.x) grad[b * row_words + i] = 0u;
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
+
+int launch_ctc_async_prepare(
+    gtnb_ctx* ctx, int B, int S, int T, int C, const GraphMeta& m0, const GraphMeta& m1, const int32_t* input_lens,
+    const int32_t* targets, const int32_t* target_lens, GraphMeta* meta, int32_t* small, float* deltas,
+    int32_t* valid, int32_t* kstatus) {
+  if (B <= 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "ctc_async_prepare", ctc_async_prepare_kernel<<<(B + 7) / 8, 256, 0, ctx->stream>>>(
+      B, S, T, C, m0, m1, input_lens, targets, target_lens, meta, small, deltas, valid, kstatus));
+  return GTNB_OK;
+}
+
+int launch_ctc_async_finalize(
+    gtnb_ctx* ctx, int B, int zp, const float* z, const float* s, const int32_t* kstatus, const int32_t* valid,
+    float* losses, int32_t* status, void* grad, long long row_words) {
+  if (B <= 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "ctc_async_finalize", ctc_async_finalize_kernel<<<B, 256, 0, ctx->stream>>>(
+      zp, z, s, kstatus, valid, losses, status, static_cast<uint32_t*>(grad), row_words));
+  return GTNB_OK;
+}
 
 int launch_ctc_build(
     gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, const int32_t* tgt_off_dev,

@@ -132,7 +132,85 @@ class CTCLossFunction(torch.autograd.Function):
         return (grad * grad_output.view(-1, 1, 1)).to(grad.dtype), None, None, None, None
 
 
-def ctc_loss(emissions, targets, blank=0, reduction="mean", input_lengths=None):
+_async_ctx_cache = {}
+
+
+def _async_ctx(device):
+    """One context per device for gtnb_ctc_loss_async, which is handed its stream on every call. It is created by the
+    first call outside stream capture: creating a context is not something a capture may record."""
+    g = _async_ctx_cache.get(device.index)
+    if g is None:
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("ctc_loss: call it once with tensor targets before capturing a CUDA graph (warm-up), "
+                               "so that its context exists")
+        g = _async_ctx_cache[device.index] = capi.Ctx(device.index)
+    return g
+
+
+class CTCLossAsyncFunction(torch.autograd.Function):
+    """ctc_loss on tensor targets: gtnb_ctc_loss_async on the current stream, with no host synchronisation in forward
+    or backward, so that the step can be captured in a CUDA graph.
+
+    targets: [B, S] integer tensor on the emissions' device, row b holding target_lengths[b] labels; target_lengths
+    and input_lengths (or None): [B] integer tensors on that device.  The losses are float32 device tensors, those of
+    the list-target call bit for bit.  An utterance the device call flags gets a NaN loss and a zero gradient: a
+    non-finite emission (the list-target call repeats such a batch exactly on the host), or an invalid length or
+    label (the list-target call raises for the whole batch).  Bounds outside the asynchronous routes run the
+    synchronous call on the targets copied to the host -- a documented synchronisation -- and raise under capture.
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, targets, blank, reduction, input_lengths, target_lengths):
+        e = emissions.contiguous()
+        B, T, Cn = e.shape
+        S = targets.shape[1]
+        tg = targets.to(torch.int32).contiguous()
+        tl = target_lengths.to(torch.int32).contiguous()
+        il = None if input_lengths is None else input_lengths.to(torch.int32).contiguous()
+        dtype = _CTC_DTYPES[e.dtype]
+        g = _async_ctx(e.device)
+        nbytes = C.c_size_t()
+        rc = capi.lib().gtnb_ctc_loss_async_workspace(g.h, B, T, Cn, S, dtype, 1, C.byref(nbytes))
+        if rc == capi.ERR_UNSUPPORTED:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("ctc_loss: these bounds are outside the asynchronous routes (%s) and cannot be "
+                                   "captured" % capi.lib().gtnb_last_error(g.h).decode())
+            # the synchronous call on host targets: this synchronises
+            rows = tg.cpu().tolist()
+            lens = tl.cpu().tolist()
+            out = CTCLossFunction.forward(ctx, e, [r[:n] for r, n in zip(rows, lens)], blank, "none", input_lengths)
+            ctx.reduction = reduction
+            return out.mean() if reduction == "mean" else out
+        g._check(rc)
+        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+        losses = torch.empty(B, dtype=torch.float32, device=e.device)
+        grad = torch.empty_like(e)
+        g._check(capi.lib().gtnb_ctc_loss_async(
+            g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, S, e.data_ptr(), dtype,
+            None if il is None else il.data_ptr(), tg.data_ptr(), tl.data_ptr(), int(blank), losses.data_ptr(), None,
+            grad.data_ptr(), ws.data_ptr(), nbytes.value))
+        ctx.save_for_backward(grad)
+        ctx.reduction = reduction
+        ctx.B = B
+        return losses.mean() if reduction == "mean" else losses
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return CTCLossFunction.backward(ctx, grad_output)[:1] + (None,) * 5
+
+
+def ctc_loss(emissions, targets, blank=0, reduction="mean", input_lengths=None, target_lengths=None):
+    """CTC loss (CTCLossFunction).  With targets a 2-D integer CUDA tensor on the emissions' device and target_lengths
+    given, the call runs on the device without a host synchronisation (CTCLossAsyncFunction)."""
+    if torch.is_tensor(targets) and targets.is_cuda and targets.dim() == 2:
+        assert not targets.is_floating_point() and targets.device == emissions.device
+        assert torch.is_tensor(target_lengths) and target_lengths.device == emissions.device, \
+            "ctc_loss: tensor targets need target_lengths on the emissions' device"
+        assert input_lengths is None or (torch.is_tensor(input_lengths) and input_lengths.device == emissions.device), \
+            "ctc_loss: with tensor targets, input_lengths must be None or a tensor on the emissions' device"
+        assert emissions.is_cuda and emissions.dim() == 3 and emissions.dtype in _CTC_DTYPES
+        assert targets.shape[0] == emissions.shape[0] and target_lengths.shape == (emissions.shape[0],)
+        return CTCLossAsyncFunction.apply(emissions, targets, blank, reduction, input_lengths, target_lengths)
     return CTCLossFunction.apply(emissions, targets, blank, reduction, input_lengths)
 
 

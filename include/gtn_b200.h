@@ -383,6 +383,57 @@ int gtnb_ctc_loss_ex(
     void* grads_dev); /* nullable */
 
 /*
+ * gtnb_ctc_loss_ex with every per-utterance input and output in device memory, for a training step that must not wait
+ * on the host (and may be captured into a CUDA graph).  The call enqueues its work on cuda_stream (NULL: the CUDA
+ * default stream, not the context's) and returns: no host synchronisation, no read of device data on the host, no allocation and no
+ * staging through host memory.  It issues kernel launches and, with input_lens, one memset of the gradient, all of
+ * which stream capture accepts; one context per device serves every stream.  Its scratch memory is workspace_dev
+ * (256-byte aligned, at least gtnb_ctc_loss_async_workspace's bytes for the same bounds and dtype; smaller is
+ * GTNB_ERR_INVALID_ARGUMENT).
+ *
+ * targets_dev is [B][S] int32, row b holding target_lens_dev[b] labels; input_lens_dev is [B] (NULL: T each).
+ * The call is sized from the bounds, never from the labels: every utterance as if U = S, T_b = T, with S - 1 skip
+ * arcs.  The routes follow gtnb_ctc_loss_ex's: the one-launch kernel (k_bidir.cu) when the bounds and buffers take it
+ * (16-bit buffers read in place when C % 8 == 0 and both are 16-byte aligned, else widened into the workspace), else
+ * the two implicit sweeps.  Bounds outside both, the "implicit" flag at 0, blank outside [0, C) and an unknown dtype
+ * are GTNB_ERR_UNSUPPORTED: use the synchronous call.
+ *
+ * losses_dev [B] float32 and status_dev [B] (nullable) are written on the device:
+ *   0  the loss is gtnb_ctc_loss_ex's on the same data, bit for bit;
+ *   1  a sweep met a non-finite value.  The synchronous call then repeats the batch on the exact materialised route,
+ *      which needs the host; this call cannot, and writes a NaN loss and a zero gradient for the utterance;
+ *   2  invalid input: target_lens_dev[b] outside [0, S], input_lens_dev[b] outside [0, T] or a label outside [0, C)
+ *      (the synchronous call's GTNB_ERR_INVALID_ARGUMENT, per utterance here): a NaN loss and a zero gradient, and
+ *      the utterance is swept as empty, so that no kernel indexes with its lengths or labels.
+ * Other utterances are unaffected by a flagged one.  grads_dev (nullable) is [B][T][C] of dtype; rows
+ * t >= input_lens_dev[b] are zero.
+ */
+int gtnb_ctc_loss_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    int S,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const int32_t* targets_dev, /* [B][S] */
+    const int32_t* target_lens_dev, /* [B] */
+    int blank,
+    float* losses_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* grads_dev, /* [B][T][C] of dtype, or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/*
+ * *bytes: the workspace gtnb_ctc_loss_async needs for these bounds, dtype and with_grad (any alignment of the
+ * caller's buffers; host work only).  GTNB_ERR_UNSUPPORTED when the bounds are outside the asynchronous routes.
+ */
+int gtnb_ctc_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, int with_grad, size_t* bytes);
+
+/*
  * ASG criterion for a whole minibatch (test/criterion_test.cpp:244-305, examples/asg.cpp:59-81,
  * BASELINE.json configs[2]):
  *   loss_b = forwardScore(compose(e_b, transitions))
