@@ -614,9 +614,9 @@ extern "C" int gtnb_ctc_loss_ex(
 namespace {
 
 /*
- * The context's arena pointed at a caller's block for one gtnb_ctc_loss_async call (base NULL: sizing only, nothing
- * is launched).  dev_alloc fails once the block is full instead of allocating; the context's own arena is back when
- * the scope ends.
+ * The context's arena pointed at a caller's block for one asynchronous call (gtnb_ctc_loss_async,
+ * gtnb_ngram_ctc_loss_async, gtnb_asg_loss_async; base NULL: sizing only, nothing is launched).  dev_alloc fails once
+ * the block is full instead of allocating; the context's own arena is back when the scope ends.
  */
 class BorrowedArena {
  public:
@@ -1608,6 +1608,218 @@ extern "C" int gtnb_asg_loss_typed(
   return asg_loss_ex_call(ctx, TransitionArgs{B, T, C, static_cast<const float*>(emissions_dev), 1, input_lens,
                                               trans_w_dev, 1, targets, target_lens, -1, losses_host,
                                               static_cast<float*>(grads_dev), 1, trans_grad_dev, 1, dtype});
+}
+
+namespace {
+
+struct TrellisAsyncArgs {
+  int B, T, C, S, dtype;
+  const void* emissions;
+  const int32_t* input_lens;
+  const float* trans_w;
+  const int32_t *targets, *target_lens;
+  int blank; // (n-gram only)
+  float* losses;
+  int32_t* status;
+  void* grads;
+  float* trans_grad;
+};
+
+/*
+ * gtnb_ngram_ctc_loss_async / gtnb_asg_loss_async (asg) inside a BorrowedArena: the scratch of the call taken from the
+ * arena and, when launch, the call enqueued.  The route is trellis_loss_fast's for a batch at the bounds (every
+ * utterance U = S, T_b = T, and for n-gram S - 1 skip arcs): the numerator graphs built on the device from the padded
+ * targets and swept by k_implicit.cu on the side stream, the dense trellis of k_ngram.cu on the call's stream.  Where
+ * it differs: the prepare kernel writes the descriptors and [offsets | lens | T] the host would have staged; the gate
+ * kernel, once both forward sweeps are done, keeps a flagged utterance out of the denominator's backward; the
+ * numerator's arc gradients are scattered utterance by utterance, flagged ones left out; the losses and status are
+ * formed on the device.  Sizing passes NULL buffers (want: trans_grad set) and takes the largest scratch.
+ */
+int trellis_async_run(gtnb_ctx* ctx, bool asg, const TrellisAsyncArgs& a, bool launch) {
+  const char* fn = asg ? "gtnb_asg_loss_async" : "gtnb_ngram_ctc_loss_async";
+  const int B = a.B, T = a.T, C = a.C, S = a.S;
+  const bool half = a.dtype != GTNB_F32;
+  const long long per = (long long)T * C;
+  if (C > kNgramMaxLabels)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": C = " + std::to_string(C) +
+                                               " labels; the trellis kernels hold the transitions on chip for C <= " +
+                                               std::to_string(kNgramMaxLabels));
+  if (!ctx->use_implicit)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": the \"implicit\" flag is off (materialised route)");
+  if (!asg && (a.blank < 0 || a.blank >= C))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": blank outside [0, C)");
+  const int L = 2 * S + 1;
+  const SgDims bound = asg ? SgDims{S + 1, 2 * S, S > 0 ? 1 : 0, 1, 1, 2, 2}
+                           : SgDims{L + 1, L + (L - 1) + std::max(S - 1, 0) + std::min(L, 2), L >= 2 ? 2 : 1, 1, 1, 3, 3};
+  const std::vector<SgDims> dims(B, bound);
+  if (!implicit_dims_supported(dims.data(), B))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": bounds outside the implicit sweeps");
+  const long long n_trans = (asg ? C : 0) + (long long)C * C;
+  const long long n_sigma = asg ? 0 : C;
+  const long long tot_A = (long long)B * bound.A;
+  const bool want = a.grads || a.trans_grad;
+  const std::vector<int32_t> Tv(B, T);
+  std::vector<long long> sgn, sga;
+  gtnb_lattice* lat_raw = nullptr;
+  GTNB_TRY(composed_alloc(ctx, B, dims.data(), B, 0, Tv.data(), C, static_cast<const float*>(a.emissions), per, sgn,
+                          sga, &lat_raw, true));
+  const std::unique_ptr<gtnb_lattice> lat(lat_raw); // (its device buffers lie in the arena: nothing to free)
+  if (half) lat->dtype = a.dtype; // 16-bit emissions read in place by both sweeps, as the _typed calls do
+  int32_t *small = nullptr, *valid = nullptr, *kstatus = nullptr, *T_bwd = nullptr, *map = nullptr;
+  float *deltas = nullptr, *sigma = nullptr, *alpha = nullptr, *den = nullptr, *ggrad = nullptr, *tg = nullptr;
+  float* g = half ? nullptr : static_cast<float*>(a.grads);
+  GTNB_TRY(dev_alloc(ctx, &small, 3ll * B));
+  GTNB_TRY(dev_alloc(ctx, &valid, B));
+  GTNB_TRY(dev_alloc(ctx, &kstatus, 2ll * B));
+  GTNB_TRY(dev_alloc(ctx, &T_bwd, B));
+  GTNB_TRY(dev_alloc(ctx, &deltas, B));
+  GTNB_TRY(dev_alloc(ctx, &map, tot_A));
+  if (n_sigma) GTNB_TRY(dev_alloc(ctx, &sigma, n_sigma));
+  GTNB_TRY(dev_alloc(ctx, &alpha, asg ? asg_alpha_floats(B, T, C) : (long long)B * (T + 1) * C));
+  GTNB_TRY(dev_alloc(ctx, &den, B));
+  if (want) {
+    GTNB_TRY(dev_alloc(ctx, &ggrad, tot_A));
+    // [d/dtrans | d/dsigma]: the caller's buffer when it has the room (ASG, no sigma slots), else scratch that is
+    // copied out at the end (sizing takes the scratch: it cannot tell whether trans_grad will be given)
+    if (n_sigma || !a.trans_grad || !launch)
+      GTNB_TRY(dev_alloc(ctx, &tg, n_trans + n_sigma));
+    else
+      tg = a.trans_grad;
+    // float32 emission gradient: the caller's, else (16-bit, or transitions only) scratch
+    if (!g) GTNB_TRY(dev_alloc(ctx, &g, per * B));
+  }
+  if (!launch) return GTNB_OK;
+
+  // the side stream and its events exist once a call has run outside capture; a capture must not create them
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  GTNB_CUDA(ctx, cudaStreamIsCapturing(ctx->stream, &cap));
+  if (cap != cudaStreamCaptureStatusNone && (!ctx->copy_stream || ctx->side_events.empty()))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT,
+                std::string(fn) + ": call it once outside stream capture first (it creates its side stream then)");
+  GTNB_TRY(ensure_side_streams(ctx, 0, 1));
+  const float* e = static_cast<const float*>(a.emissions); // (a.dtype's elements: the kernels read them as such)
+  const int32_t* T_fwd = small + 2ll * B;
+  if (want) {
+    GTNB_CUDA(ctx, cudaMemsetAsync(g, 0, sizeof(float) * per * B, ctx->stream));
+    GTNB_CUDA(ctx, cudaMemsetAsync(tg, 0, sizeof(float) * (n_trans + n_sigma), ctx->stream));
+    GTNB_CUDA(ctx, cudaMemsetAsync(ggrad, 0, sizeof(float) * tot_A, ctx->stream));
+  }
+  GTNB_TRY(launch_trellis_async_prepare(ctx, asg, B, S, T, C, lat->meta_h[0], lat->meta_h[B > 1 ? 1 : 0],
+                                        a.input_lens, a.targets, a.target_lens, lat->meta, small, deltas, valid,
+                                        kstatus));
+  if (asg) {
+    GTNB_TRY(launch_asg_num_build(ctx, lat.get(), a.targets, small, small + B, a.trans_w, map));
+  } else {
+    GTNB_TRY(launch_ngram_sigma(ctx, C, a.trans_w, sigma));
+    GTNB_TRY(launch_ngram_num_build(ctx, lat.get(), a.targets, small, small + B, a.blank, a.trans_w, sigma, map));
+  }
+  // the numerator (a few in-arcs per node) on the side stream beside the denominator (C^2 per frame)
+  cudaEvent_t num_forward_done = ctx->side_events[0];
+  GTNB_TRY(fork_to(ctx, ctx->copy_stream));
+  {
+    OnStream side(ctx, ctx->copy_stream);
+    GTNB_TRY(launch_implicit_forward(ctx, lat.get(), kstatus + B));
+    GTNB_CUDA(ctx, cudaEventRecord(num_forward_done, ctx->copy_stream));
+    if (want) GTNB_TRY(launch_implicit_backward(ctx, lat.get(), deltas, g, per, 0, -1, ggrad));
+  }
+  if (asg)
+    GTNB_TRY(launch_asg_den_forward(ctx, B, T, C, T_fwd, e, per, a.trans_w, alpha, den, kstatus, a.dtype));
+  else
+    GTNB_TRY(launch_ngram_den_forward(ctx, B, T, C, T_fwd, e, per, a.trans_w, alpha, den, kstatus, a.dtype));
+  GTNB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, num_forward_done, 0));
+  GTNB_TRY(launch_trellis_async_gate(ctx, B, T_fwd, valid, kstatus, T_bwd, den));
+  if (want) {
+    if (asg)
+      GTNB_TRY(launch_asg_den_backward(ctx, B, T, C, T_bwd, e, per, a.trans_w, alpha, den, g, per, tg, a.dtype));
+    else
+      GTNB_TRY(launch_ngram_den_backward(ctx, B, T, C, T_bwd, e, per, a.trans_w, alpha, den, g, per, tg, a.dtype));
+  }
+  GTNB_TRY(join_from(ctx, ctx->copy_stream));
+  if (want) {
+    GTNB_TRY(launch_trellis_async_scatter(ctx, B, lat->meta, kstatus, map, ggrad, tg));
+    if (n_sigma) GTNB_TRY(launch_ngram_fold(ctx, C, a.trans_w, sigma, tg));
+  }
+  // losses = den - num in float32 as read_losses forms them; a flagged utterance's emission-gradient row zeroed
+  GTNB_TRY(launch_ctc_async_finalize(ctx, B, 1, den, lat->out_scores, kstatus, valid, a.losses, a.status,
+                                     a.grads ? g : nullptr, per));
+  if (half && a.grads) GTNB_TRY(launch_narrow(ctx, g, a.grads, a.dtype, per * B));
+  if (a.trans_grad && tg != a.trans_grad) // (n-gram: ngram_fold_kernel reads the sigma slots right after W's)
+    GTNB_CUDA(ctx, cudaMemcpyAsync(a.trans_grad, tg, sizeof(float) * n_trans, cudaMemcpyDeviceToDevice,
+                                   ctx->stream));
+  return GTNB_OK;
+}
+
+int trellis_async_workspace(gtnb_ctx* ctx, bool asg, int B, int T, int C, int S, int dtype, int with_grad,
+                            size_t* bytes) {
+  const char* fn = asg ? "gtnb_asg_loss_async_workspace" : "gtnb_ngram_ctc_loss_async_workspace";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !bytes)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": unknown dtype");
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  // (the sizing reads the trans_grad pointer for its presence only; grads NULL sizes the float32 scratch gradient)
+  alignas(16) static float stand_in[4];
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  const TrellisAsyncArgs a{B, T, C, S, dtype, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
+                           nullptr, with_grad ? stand_in : nullptr};
+  GTNB_TRY(trellis_async_run(ctx, asg, a, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+int trellis_async_call(gtnb_ctx* ctx, bool asg, void* cuda_stream, const TrellisAsyncArgs& a, void* workspace_dev,
+                       size_t workspace_bytes) {
+  const char* fn = asg ? "gtnb_asg_loss_async" : "gtnb_ngram_ctc_loss_async";
+  if (!ctx || a.B < 0 || a.T < 0 || a.C <= 0 || a.S < 0 || !a.emissions || !a.trans_w ||
+      (a.S > 0 && !a.targets) || !a.target_lens || !a.losses || (a.B > 0 && !workspace_dev) ||
+      ((uintptr_t)workspace_dev & 255))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  if (!known_dtype(a.dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": unknown dtype");
+  if (a.B == 0) {
+    if (a.trans_grad) {
+      const long long n_trans = (asg ? a.C : 0) + (long long)a.C * a.C;
+      GTNB_CUDA(ctx, cudaMemsetAsync(a.trans_grad, 0, sizeof(float) * n_trans, static_cast<cudaStream_t>(cuda_stream)));
+    }
+    return GTNB_OK;
+  }
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  return trellis_async_run(ctx, asg, a, true);
+}
+
+} // namespace
+
+extern "C" int gtnb_ngram_ctc_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype,
+                                                   int with_grad, size_t* bytes) {
+  return trellis_async_workspace(ctx, false, B, T, C, S, dtype, with_grad, bytes);
+}
+
+extern "C" int gtnb_ngram_ctc_loss_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, int S, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, const float* trans_w_dev, const int32_t* targets_dev,
+    const int32_t* target_lens_dev, int blank, float* losses_dev, int32_t* status_dev, void* grads_dev,
+    float* trans_grad_dev, void* workspace_dev, size_t workspace_bytes) {
+  return trellis_async_call(ctx, false, cuda_stream,
+                            TrellisAsyncArgs{B, T, C, S, dtype, emissions_dev, input_lens_dev, trans_w_dev, targets_dev,
+                                             target_lens_dev, blank, losses_dev, status_dev, grads_dev, trans_grad_dev},
+                            workspace_dev, workspace_bytes);
+}
+
+extern "C" int gtnb_asg_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, int with_grad,
+                                             size_t* bytes) {
+  return trellis_async_workspace(ctx, true, B, T, C, S, dtype, with_grad, bytes);
+}
+
+extern "C" int gtnb_asg_loss_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, int S, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, const float* trans_w_dev, const int32_t* targets_dev,
+    const int32_t* target_lens_dev, float* losses_dev, int32_t* status_dev, void* grads_dev, float* trans_grad_dev,
+    void* workspace_dev, size_t workspace_bytes) {
+  return trellis_async_call(ctx, true, cuda_stream,
+                            TrellisAsyncArgs{B, T, C, S, dtype, emissions_dev, input_lens_dev, trans_w_dev, targets_dev,
+                                             target_lens_dev, 0, losses_dev, status_dev, grads_dev, trans_grad_dev},
+                            workspace_dev, workspace_bytes);
 }
 
 /*

@@ -74,7 +74,7 @@ struct gtnb_ctx {
   unsigned char* arena = nullptr;
   size_t arena_cap = 0, arena_off = 0, arena_need = 0;
   bool arena_on = false;
-  // the arena is a caller's workspace (gtnb_ctc_loss_async): dev_alloc fails instead of allocating once it is full
+  // the arena is a caller's workspace (the *_async calls): dev_alloc fails instead of allocating once it is full
   bool arena_borrowed = false;
   bool profiling = false;
   std::vector<ProfEntry> prof;
@@ -188,6 +188,19 @@ int launch_ctc_async_prepare(
 int launch_ctc_async_finalize(
     gtnb_ctx* ctx, int B, int zp, const float* z, const float* s, const int32_t* kstatus, const int32_t* valid,
     float* losses, int32_t* status, void* grad, long long row_words);
+/* the same set-up for gtnb_ngram_ctc_loss_async / gtnb_asg_loss_async (asg): their numerators' descriptors, kstatus
+ * [2B] (denominator, numerator) zeroed */
+int launch_trellis_async_prepare(
+    gtnb_ctx* ctx, bool asg, int B, int S, int T, int C, const GraphMeta& m0, const GraphMeta& m1,
+    const int32_t* input_lens, const int32_t* targets, const int32_t* target_lens, GraphMeta* meta, int32_t* small,
+    float* deltas, int32_t* valid, int32_t* kstatus);
+/* after both forward sweeps: kstatus[b] |= kstatus[B + b] | !valid[b]; T_bwd[b] = flagged ? 0 : T_fwd[b];
+ * den[b] = NaN where T_fwd[b] = 0 */
+int launch_trellis_async_gate(gtnb_ctx* ctx, int B, const int32_t* T_fwd, const int32_t* valid, int32_t* kstatus,
+                              int32_t* T_bwd, float* den);
+/* dst[map[o + a]] += src[o + a], a < meta[b].sg_A, o = meta[b].grad_graph_off, for every b with kstatus[b] == 0 */
+int launch_trellis_async_scatter(gtnb_ctx* ctx, int B, const GraphMeta* meta, const int32_t* kstatus,
+                                 const int32_t* map, const float* src, float* dst);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
@@ -262,7 +275,8 @@ int dev_alloc(gtnb_ctx* ctx, T** p, long long n) {
       return GTNB_OK;
     }
     if (ctx->arena_borrowed)
-      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "workspace too small for these bounds (gtnb_ctc_loss_async_workspace)");
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT,
+                  "workspace too small for these bounds (the call's *_async_workspace gives the size)");
   }
   GTNB_CUDA(ctx, cudaMallocAsync((void**)p, bytes, ctx->stream));
   return GTNB_OK;

@@ -116,6 +116,10 @@ __global__ void __launch_bounds__(256) ctc_build_kernel(
   }
 }
 
+/* the numerator graph an asynchronous call's prepare kernel describes (gtnb_ctc_loss_async, gtnb_ngram_ctc_loss_async,
+ * gtnb_asg_loss_async) */
+enum class AsyncGraph { Ctc, Ngram, Asg };
+
 /*
  * gtnb_ctc_loss_async, before the sweeps: the descriptors and the small arrays of the batch, built on the device from
  * the caller's padded targets.  One warp per utterance.  The slabs were laid out on the host at the bounds (U = S,
@@ -126,7 +130,12 @@ __global__ void __launch_bounds__(256) ctc_build_kernel(
  * gradFunc, read by the implicit backward).  An utterance with U outside [0, S], T_b outside [0, T] or a label
  * outside [0, C) gets valid = 0 and is swept as U = 0, T_b = 0, so that no kernel indexes with its lengths or labels;
  * the finalize kernel reports it.  kstatus, the sweeps' non-finite flags, starts at 0.
+ * G = Ngram / Asg (gtnb_ngram_ctc_loss_async, gtnb_asg_loss_async): the same, for the numerators the build kernels of
+ * k_ngram.cu write (the dims of ngram_ctc_loss_call / asg_loss_ex_call): n-gram sg_N = 2U + 2, sg_A = L + (L - 1) +
+ * skips + min(L, 2); ASG sg_N = U + 1, sg_A = 2U, n_accept = (U > 0).  kstatus is [2B] there (denominator, numerator),
+ * both halves set to 0.
  */
+template <AsyncGraph G = AsyncGraph::Ctc>
 __global__ void __launch_bounds__(256) ctc_async_prepare_kernel(
     int B, int S, int T, int C, const GraphMeta m0, const GraphMeta m1,
     const int32_t* __restrict__ input_lens, // nullable: T each
@@ -167,10 +176,20 @@ __global__ void __launch_bounds__(256) ctc_async_prepare_kernel(
   m.emis_off += b * (m1.emis_off - m0.emis_off);
   m.grad_graph_off += b * (m1.grad_graph_off - m0.grad_graph_off);
   m.L = Tb + 1;
-  m.n_accept = L >= 2 ? 2 : 1;
   m.T = Tb;
-  m.sg_N = L;
-  m.sg_A = L + (L - 1) + skips;
+  if constexpr (G == AsyncGraph::Ctc) {
+    m.n_accept = L >= 2 ? 2 : 1;
+    m.sg_N = L;
+    m.sg_A = L + (L - 1) + skips;
+  } else if constexpr (G == AsyncGraph::Ngram) {
+    m.n_accept = L >= 2 ? 2 : 1;
+    m.sg_N = L + 1;
+    m.sg_A = L + (L - 1) + skips + (L < 2 ? L : 2);
+  } else {
+    m.n_accept = U > 0 ? 1 : 0;
+    m.sg_N = U + 1;
+    m.sg_A = 2 * U;
+  }
   m.tgt_off = b * S;
   meta[b] = m;
   small[b] = b * S;
@@ -179,6 +198,7 @@ __global__ void __launch_bounds__(256) ctc_async_prepare_kernel(
   deltas[b] = -1.0f;
   valid[b] = ok;
   kstatus[b] = 0;
+  if constexpr (G != AsyncGraph::Ctc) kstatus[B + b] = 0;
 }
 
 /*
@@ -203,6 +223,41 @@ __global__ void __launch_bounds__(256) ctc_async_finalize_kernel(
     for (long long i = threadIdx.x; i < row_words; i += blockDim.x) grad[b * row_words + i] = 0u;
 }
 
+/*
+ * gtnb_ngram_ctc_loss_async / gtnb_asg_loss_async, after both forward sweeps (the numerator's on the side stream waited
+ * for): kstatus[b] |= kstatus[B + b] | !valid[b], the flag of utterance b from then on, and T_bwd[b] = T_b, or 0 for a
+ * flagged utterance, so that the denominator's backward kernel (which returns for T_b < 1) adds nothing for it to the
+ * shared transition gradient.  An utterance with T_b = 0 gets den[b] = NaN: its loss is NaN, as the synchronous call
+ * gives it (run_criterion), where the trellis would score the empty linear graph log C.  One thread per utterance.
+ */
+__global__ void __launch_bounds__(256) trellis_async_gate_kernel(
+    int B, const int32_t* __restrict__ T_fwd, const int32_t* __restrict__ valid, int32_t* __restrict__ kstatus,
+    int32_t* __restrict__ T_bwd, float* __restrict__ den) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int flagged = (kstatus[b] | kstatus[B + b]) != 0 || !valid[b];
+  const int Tb = T_fwd[b];
+  kstatus[b] = flagged;
+  T_bwd[b] = flagged ? 0 : Tb;
+  if (Tb == 0) den[b] = CUDART_NAN_F;
+}
+
+/*
+ * The numerator's arc gradients into the transition gradient, utterance by utterance: dst[map[o + a]] += src[o + a]
+ * for a < meta[b].sg_A, o = meta[b].grad_graph_off, for every utterance whose kstatus (the gate's) is 0.  Only the
+ * arcs the build kernel wrote are read: the slabs are laid out at the bounds, and the tail of a slab past the
+ * utterance's own arcs holds whatever the workspace held.  One CTA per utterance.
+ */
+__global__ void __launch_bounds__(256) trellis_async_scatter_kernel(
+    const GraphMeta* __restrict__ meta, const int32_t* __restrict__ kstatus, const int32_t* __restrict__ map,
+    const float* __restrict__ src, float* __restrict__ dst) {
+  const int b = blockIdx.x;
+  if (kstatus[b]) return;
+  const long long o = meta[b].grad_graph_off;
+  const int n = meta[b].sg_A;
+  for (int a = threadIdx.x; a < n; a += blockDim.x) atomicAdd(dst + map[o + a], src[o + a]);
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
@@ -214,6 +269,38 @@ int launch_ctc_async_prepare(
   if (B <= 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "ctc_async_prepare", ctc_async_prepare_kernel<<<(B + 7) / 8, 256, 0, ctx->stream>>>(
       B, S, T, C, m0, m1, input_lens, targets, target_lens, meta, small, deltas, valid, kstatus));
+  return GTNB_OK;
+}
+
+int launch_trellis_async_prepare(
+    gtnb_ctx* ctx, bool asg, int B, int S, int T, int C, const GraphMeta& m0, const GraphMeta& m1,
+    const int32_t* input_lens, const int32_t* targets, const int32_t* target_lens, GraphMeta* meta, int32_t* small,
+    float* deltas, int32_t* valid, int32_t* kstatus) {
+  if (B <= 0) return GTNB_OK;
+  if (asg)
+    GTNB_LAUNCH(ctx, "trellis_async_prepare", ctc_async_prepare_kernel<AsyncGraph::Asg><<<(B + 7) / 8, 256, 0,
+                ctx->stream>>>(B, S, T, C, m0, m1, input_lens, targets, target_lens, meta, small, deltas, valid,
+                               kstatus));
+  else
+    GTNB_LAUNCH(ctx, "trellis_async_prepare", ctc_async_prepare_kernel<AsyncGraph::Ngram><<<(B + 7) / 8, 256, 0,
+                ctx->stream>>>(B, S, T, C, m0, m1, input_lens, targets, target_lens, meta, small, deltas, valid,
+                               kstatus));
+  return GTNB_OK;
+}
+
+int launch_trellis_async_gate(gtnb_ctx* ctx, int B, const int32_t* T_fwd, const int32_t* valid, int32_t* kstatus,
+                              int32_t* T_bwd, float* den) {
+  if (B <= 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "trellis_async_gate", trellis_async_gate_kernel<<<(B + 255) / 256, 256, 0, ctx->stream>>>(
+      B, T_fwd, valid, kstatus, T_bwd, den));
+  return GTNB_OK;
+}
+
+int launch_trellis_async_scatter(gtnb_ctx* ctx, int B, const GraphMeta* meta, const int32_t* kstatus,
+                                 const int32_t* map, const float* src, float* dst) {
+  if (B <= 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "trellis_async_scatter", trellis_async_scatter_kernel<<<B, 256, 0, ctx->stream>>>(
+      meta, kstatus, map, src, dst));
   return GTNB_OK;
 }
 

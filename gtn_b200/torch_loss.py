@@ -135,14 +135,15 @@ class CTCLossFunction(torch.autograd.Function):
 _async_ctx_cache = {}
 
 
-def _async_ctx(device):
-    """One context per device for gtnb_ctc_loss_async, which is handed its stream on every call. It is created by the
-    first call outside stream capture: creating a context is not something a capture may record."""
+def _async_ctx(device, name="ctc_loss"):
+    """One context per device for the asynchronous calls (gtnb_ctc_loss_async, gtnb_ngram_ctc_loss_async,
+    gtnb_asg_loss_async), which are handed their stream on every call. It is created by the first call outside stream
+    capture: creating a context is not something a capture may record."""
     g = _async_ctx_cache.get(device.index)
     if g is None:
         if torch.cuda.is_current_stream_capturing():
-            raise RuntimeError("ctc_loss: call it once with tensor targets before capturing a CUDA graph (warm-up), "
-                               "so that its context exists")
+            raise RuntimeError("%s: call it once with tensor targets before capturing a CUDA graph (warm-up), "
+                               "so that its context exists" % name)
         g = _async_ctx_cache[device.index] = capi.Ctx(device.index)
     return g
 
@@ -294,7 +295,114 @@ class ASGLossFunction(torch.autograd.Function):
         return grad, tg.to(ctx.tdev), None, None, None, None
 
 
-def asg_loss(emissions, transitions, targets, reduction="mean", allreduce=True, input_lengths=None):
+def _tensor_targets(name, emissions, targets, input_lengths, target_lengths):
+    """True when targets is a 2-D integer CUDA tensor, the asynchronous route's input (its arguments checked)"""
+    if not (torch.is_tensor(targets) and targets.is_cuda and targets.dim() == 2):
+        return False
+    assert not targets.is_floating_point() and targets.device == emissions.device
+    assert torch.is_tensor(target_lengths) and target_lengths.device == emissions.device, \
+        "%s: tensor targets need target_lengths on the emissions' device" % name
+    assert input_lengths is None or (torch.is_tensor(input_lengths) and input_lengths.device == emissions.device), \
+        "%s: with tensor targets, input_lengths must be None or a tensor on the emissions' device" % name
+    assert emissions.is_cuda and emissions.dim() == 3 and emissions.dtype in _EMISSION_DTYPES
+    assert targets.shape[0] == emissions.shape[0] and target_lengths.shape == (emissions.shape[0],)
+    return True
+
+
+class TrellisLossAsyncFunction(torch.autograd.Function):
+    """asg_loss and ngram_ctc_loss on tensor targets: gtnb_asg_loss_async / gtnb_ngram_ctc_loss_async on the current
+    stream, with no host synchronisation in forward or backward, so that a step that trains the transitions can be
+    captured in a CUDA graph.
+
+    targets: [B, S] integer tensor on the emissions' device, row b holding target_lengths[b] labels; target_lengths
+    and input_lengths (or None): [B] integer tensors on that device; transitions: float32 CUDA tensor on that device.
+    The losses are float32 device tensors, those of the list-target call bit for bit.  An utterance the device call
+    flags gets a NaN loss, a zero emission gradient and no share of the transition gradient: a non-finite emission or
+    transition weight (the list-target call repeats such a batch exactly on the host), or an invalid length or label
+    (the list-target call raises for the whole batch).  Bounds outside the asynchronous route run the synchronous call
+    on the targets copied to the host -- a documented synchronisation -- and raise under capture.
+
+    reduction="none": the transition gradient is summed over the batch inside the kernels, the chain rule's answer
+    only for a uniform upstream gradient.  The list-target call asserts that on the host; here, where nothing may
+    synchronise, a non-uniform upstream gradient gives a NaN transition gradient instead.
+    """
+
+    @staticmethod
+    def forward(ctx, emissions, transitions, targets, asg, blank, reduction, allreduce, input_lengths, target_lengths):
+        name = "asg_loss" if asg else "ngram_ctc_loss"
+        e = emissions.contiguous()
+        B, T, Cn = e.shape
+        S = targets.shape[1]
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == (Cn + Cn * Cn if asg else Cn * Cn)
+        w = transitions.detach().contiguous()
+        tgt = targets.to(torch.int32).contiguous()
+        tl = target_lengths.to(torch.int32).contiguous()
+        il = None if input_lengths is None else input_lengths.to(torch.int32).contiguous()
+        dtype = _EMISSION_DTYPES[e.dtype]
+        g = _async_ctx(e.device, name)
+        lib = capi.lib()
+        nbytes = C.c_size_t()
+        call = lib.gtnb_asg_loss_async if asg else lib.gtnb_ngram_ctc_loss_async
+        sizing = lib.gtnb_asg_loss_async_workspace if asg else lib.gtnb_ngram_ctc_loss_async_workspace
+        rc = sizing(g.h, B, T, Cn, S, dtype, 1, C.byref(nbytes))
+        if rc == capi.ERR_UNSUPPORTED:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("%s: these bounds are outside the asynchronous route (%s) and cannot be captured"
+                                   % (name, lib.gtnb_last_error(g.h).decode()))
+            # the synchronous call on host targets: this synchronises
+            rows = tgt.cpu().tolist()
+            lens = tl.cpu().tolist()
+            lists = [r[:n] for r, n in zip(rows, lens)]
+            if asg:
+                out = ASGLossFunction.forward(ctx, e, transitions, lists, "none", allreduce, input_lengths)
+            else:
+                out = NgramCTCLossFunction.forward(ctx, e, transitions, lists, input_lengths, blank, "none", allreduce)
+            ctx.reduction = reduction
+            return out.mean() if reduction == "mean" else out
+        g._check(rc)
+        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+        losses = torch.empty(B, dtype=torch.float32, device=e.device)
+        grad = torch.empty_like(e)
+        tg = torch.empty(transitions.numel(), dtype=torch.float32, device=e.device)
+        stream = torch.cuda.current_stream(e.device).cuda_stream
+        il_p = None if il is None else il.data_ptr()
+        if asg:
+            rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, w.data_ptr(), tgt.data_ptr(), tl.data_ptr(),
+                      losses.data_ptr(), None, grad.data_ptr(), tg.data_ptr(), ws.data_ptr(), nbytes.value)
+        else:
+            rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, w.data_ptr(), tgt.data_ptr(), tl.data_ptr(),
+                      int(blank), losses.data_ptr(), None, grad.data_ptr(), tg.data_ptr(), ws.data_ptr(), nbytes.value)
+        g._check(rc)
+        tg = tg.view_as(transitions)
+        _allreduce_transitions(ctx, tg, allreduce)
+        ctx.save_for_backward(grad, tg)
+        ctx.reduction = reduction
+        ctx.B = B
+        return losses.mean() if reduction == "mean" else losses
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        grad, tg = ctx.saved_tensors
+        if ctx.reduction == "mean":
+            scale = grad_output / ctx.B
+            egrad, tgrad = grad * scale, tg * (scale / ctx.world)
+        else:
+            # (a 16-bit grad times the float32 [B] upstream gradient promotes to float32: back to the emissions' dtype)
+            egrad = (grad * grad_output.view(-1, 1, 1)).to(grad.dtype)
+            g0 = grad_output.flatten()[0]
+            uniform = (grad_output == g0).all()  # a 0-dim device bool: chosen on the device, no synchronisation
+            tgrad = torch.where(uniform, tg * g0, torch.full_like(tg, float("nan")))
+        return egrad, tgrad, None, None, None, None, None, None, None
+
+
+def asg_loss(emissions, transitions, targets, reduction="mean", allreduce=True, input_lengths=None,
+             target_lengths=None):
+    """ASG loss (ASGLossFunction).  With targets a 2-D integer CUDA tensor on the emissions' device and target_lengths
+    given, the call runs on the device without a host synchronisation (TrellisLossAsyncFunction)."""
+    if _tensor_targets("asg_loss", emissions, targets, input_lengths, target_lengths):
+        return TrellisLossAsyncFunction.apply(emissions, transitions, targets, True, 0, reduction, allreduce,
+                                              input_lengths, target_lengths)
     return ASGLossFunction.apply(emissions, transitions, targets, reduction, allreduce, input_lengths)
 
 
@@ -358,7 +466,13 @@ class NgramCTCLossFunction(torch.autograd.Function):
         return grad, tg, None, None, None, None, None
 
 
-def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True):
+def ngram_ctc_loss(emissions, transitions, targets, input_lengths=None, blank=0, reduction="mean", allreduce=True,
+                   target_lengths=None):
+    """n-gram CTC loss (NgramCTCLossFunction).  With targets a 2-D integer CUDA tensor on the emissions' device and
+    target_lengths given, the call runs on the device without a host synchronisation (TrellisLossAsyncFunction)."""
+    if _tensor_targets("ngram_ctc_loss", emissions, targets, input_lengths, target_lengths):
+        return TrellisLossAsyncFunction.apply(emissions, transitions, targets, False, blank, reduction, allreduce,
+                                              input_lengths, target_lengths)
     return NgramCTCLossFunction.apply(emissions, transitions, targets, input_lengths, blank, reduction, allreduce)
 
 

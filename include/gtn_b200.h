@@ -569,6 +569,88 @@ int gtnb_asg_loss_typed(
     float* trans_grad_dev); /* nullable */
 
 /*
+ * gtnb_ngram_ctc_loss_typed and gtnb_asg_loss_typed with every per-utterance input and output in device memory, for a
+ * training step with learned transitions that must not wait on the host (and may be captured into a CUDA graph).
+ * The contract is gtnb_ctc_loss_async's: the call enqueues its work on cuda_stream (NULL: the CUDA default stream) and
+ * returns, without a host synchronisation, a read of device data on the host, an allocation or a staging copy.  It
+ * issues kernel launches, memsets and event records / waits between cuda_stream and the context's side stream, and
+ * for n-gram CTC one device-to-device copy of the transition gradient out of the workspace.  The side stream and its event are created by the first call
+ * made outside stream capture; a call under capture before that is GTNB_ERR_INVALID_ARGUMENT.  Scratch memory is
+ * workspace_dev (256-byte aligned, at least the matching *_async_workspace's bytes for the same bounds and dtype;
+ * smaller is GTNB_ERR_INVALID_ARGUMENT).
+ *
+ * targets_dev is [B][S] int32, row b holding target_lens_dev[b] labels; input_lens_dev is [B] (NULL: T each).  The
+ * call is sized from the bounds, never from the labels: every utterance as if U = S and T_b = T (n-gram CTC: with
+ * S - 1 skip arcs).  The route is the synchronous calls' device route: the numerator graphs built on the device and
+ * swept by the implicit kernels beside the dense trellis of the denominator; emissions of dtype (GTNB_F32, GTNB_BF16,
+ * GTNB_F16) read in place.  C > 128, the "implicit" flag at 0, bounds outside the implicit sweeps, blank outside
+ * [0, C) (n-gram) and an unknown dtype are GTNB_ERR_UNSUPPORTED: use the synchronous call.
+ *
+ * trans_w_dev: float32 on the device, n-gram W [C*C] (row = destination label), ASG [C + C*C] (start weights, then
+ * the matrix).  losses_dev [B] float32 and status_dev [B] (nullable) are written on the device:
+ *   0  the loss is the synchronous call's on the same data, bit for bit (NaN for T_b = 0, as there);
+ *   1  the denominator's or the numerator's sweep met a non-finite value (the synchronous call repeats the batch on
+ *      the exact materialised route, which needs the host): a NaN loss and a zero emission-gradient row;
+ *   2  invalid input: target_lens_dev[b] outside [0, S], input_lens_dev[b] outside [0, T] or a label outside
+ *      [0, C): a NaN loss and a zero row, and the utterance is swept as empty.
+ * A flagged utterance (1 or 2) adds nothing to trans_grad_dev, which sums over the batch: the other utterances'
+ * gradient is what the synchronous call gives on the batch without it.  A non-finite transition weight flags every
+ * utterance, T_b = 0 and 1 included (the denominator checks all of trans_w_dev whatever T_b), and trans_grad_dev is
+ * then all zeros.
+ * grads_dev (nullable): [B][T][C] of dtype, rows t >= input_lens_dev[b] zero.  trans_grad_dev (nullable): float32, the
+ * size of trans_w_dev.  The gradients add with atomics, so they vary from run to run as the synchronous call's do.
+ */
+int gtnb_ngram_ctc_loss_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    int S,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const float* trans_w_dev, /* [C*C] */
+    const int32_t* targets_dev, /* [B][S] */
+    const int32_t* target_lens_dev, /* [B] */
+    int blank,
+    float* losses_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* grads_dev, /* [B][T][C] of dtype, or NULL */
+    float* trans_grad_dev, /* [C*C] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/* gtnb_ngram_ctc_loss_async without a blank, on ASG's transitions */
+int gtnb_asg_loss_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    int S,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const float* trans_w_dev, /* [C + C*C] */
+    const int32_t* targets_dev, /* [B][S] */
+    const int32_t* target_lens_dev, /* [B] */
+    float* losses_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* grads_dev, /* [B][T][C] of dtype, or NULL */
+    float* trans_grad_dev, /* [C + C*C] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/*
+ * *bytes: the workspace gtnb_ngram_ctc_loss_async / gtnb_asg_loss_async need for these bounds and dtype (with_grad:
+ * either gradient will be asked for; host work only).  GTNB_ERR_UNSUPPORTED when the call would be.
+ */
+int gtnb_ngram_ctc_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, int with_grad,
+                                        size_t* bytes);
+int gtnb_asg_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, int with_grad, size_t* bytes);
+
+/*
  * Loss over one user-supplied target graph per utterance (the criterion of the reference's pytorch_loss.py and of
  * its word-decomposition examples):
  *   loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b))
