@@ -115,6 +115,21 @@ SYMBOLS = [
       C.c_size_t]),
     ("gtnb_asg_loss_async_workspace", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_ctc_align_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp,
+      C.c_size_t]),
+    ("gtnb_ngram_ctc_align_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, C.c_int, _vp, _vp, _vp, _vp,
+      _vp, C.c_size_t]),
+    ("gtnb_asg_align_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+      C.c_size_t]),
+    ("gtnb_ctc_align_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_ngram_ctc_align_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_asg_align_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     ("gtnb_ngram_ctc_loss", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, _vp, C.c_int, _i32p, _i32p, C.c_int, _f32p, _vp,
       C.c_int, _vp, C.c_int]),

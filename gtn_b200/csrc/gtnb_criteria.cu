@@ -1823,6 +1823,187 @@ extern "C" int gtnb_asg_loss_async(
 }
 
 /*
+ * Forced alignment without a host synchronisation: viterbiPath / viterbiScore of each loss's own numerator, from
+ * padded device targets, under gtnb_*_loss_async's contract.  The lattices are those of the synchronous aligners:
+ *   CTC         intersect(ctcGraph(y_b), E_b)                 (gtnb_graph_viterbi on CTC graphs)
+ *   n-gram CTC  intersect(intersect(ctc_b, G), E_b)           (gtnb_graph_transitions_viterbi, BIGRAM)
+ *   ASG         compose(compose(fal_b, transitions), E_b)     (gtnb_graph_transitions_viterbi, ASG)
+ * One route for the three, on the call's stream: the prepare kernel's descriptors, the numerator built by the loss's
+ * build kernel (n-gram: its folded start arcs weigh tau_l = max_j W[l][j], the tropical sigma), the tropical forward of
+ * k_implicit.cu, its trace, and align_async_finalize_kernel, which maps the status and each traced arc to its target
+ * position.  16-bit emissions are widened once into the workspace: the tropical kernels are float32 only.
+ */
+namespace {
+
+struct AlignAsyncArgs {
+  int B, T, C, S, dtype;
+  const void* emissions;
+  const int32_t* input_lens;
+  const float* trans_w; // n-gram W [C*C], ASG [C + C*C]; NULL for CTC
+  const int32_t *targets, *target_lens;
+  int blank; // (not ASG)
+  int32_t *paths, *tokens;
+  float* scores;
+  int32_t* status;
+};
+
+const char* align_async_name(AlignCriterion kind) {
+  return kind == AlignCriterion::Ctc     ? "gtnb_ctc_align_async"
+         : kind == AlignCriterion::Ngram ? "gtnb_ngram_ctc_align_async"
+                                         : "gtnb_asg_align_async";
+}
+
+/*
+ * The call inside a BorrowedArena: the scratch taken from the arena and, when launch, the work enqueued.  Sized from
+ * the bounds (every utterance U = S, T_b = T, CTC with S - 1 skips), as the losses' asynchronous calls are; sizing
+ * passes NULL buffers and takes the arcs row of the token mapping whether or not tokens will be asked for.
+ */
+int align_async_run(gtnb_ctx* ctx, AlignCriterion kind, const AlignAsyncArgs& a, bool launch) {
+  const std::string fn = align_async_name(kind);
+  const int B = a.B, T = a.T, C = a.C, S = a.S;
+  const bool half = a.dtype != GTNB_F32;
+  const long long per = (long long)T * C;
+  if (!ctx->use_implicit)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": the \"implicit\" flag is off (materialised route)");
+  if (kind != AlignCriterion::Asg && (a.blank < 0 || a.blank >= C))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": blank outside [0, C)");
+  const int L = 2 * S + 1;
+  const int skips = std::max(S - 1, 0);
+  const SgDims bound = kind == AlignCriterion::Ctc ? SgDims{L, L + (L - 1) + skips, L >= 2 ? 2 : 1, 1, 1, 3, 3}
+                       : kind == AlignCriterion::Ngram
+                           ? SgDims{L + 1, L + (L - 1) + skips + std::min(L, 2), L >= 2 ? 2 : 1, 1, 1, 3, 3}
+                           : SgDims{S + 1, 2 * S, S > 0 ? 1 : 0, 1, 1, 2, 2};
+  const std::vector<SgDims> dims(B, bound);
+  if (!implicit_dims_supported(dims.data(), B))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": bounds outside the implicit sweeps (use the graph aligners)");
+  const std::vector<int32_t> Tv(B, T);
+  std::vector<long long> sgn, sga;
+  gtnb_lattice* lat_raw = nullptr;
+  GTNB_TRY(composed_alloc(ctx, B, dims.data(), B, 0, Tv.data(), C, static_cast<const float*>(a.emissions), per, sgn,
+                          sga, &lat_raw, true));
+  const std::unique_ptr<gtnb_lattice> lat(lat_raw); // (its device buffers lie in the arena: nothing to free)
+  if (!implicit_trace_supported(lat.get()))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": bounds outside the trace's shared memory (use the graph aligners)");
+  int32_t *small = nullptr, *valid = nullptr, *kstatus = nullptr, *map = nullptr, *arcs = nullptr;
+  float *deltas = nullptr, *tau = nullptr;
+  GTNB_TRY(dev_alloc(ctx, &small, 3ll * B));
+  GTNB_TRY(dev_alloc(ctx, &valid, B));
+  GTNB_TRY(dev_alloc(ctx, &kstatus, kind == AlignCriterion::Ctc ? B : 2ll * B)); // (the trellis prepare zeroes 2B)
+  GTNB_TRY(dev_alloc(ctx, &deltas, B)); // (written by the prepare kernel, read by no sweep here)
+  if (kind != AlignCriterion::Ctc) GTNB_TRY(dev_alloc(ctx, &map, (long long)B * bound.A));
+  if (kind == AlignCriterion::Ngram) GTNB_TRY(dev_alloc(ctx, &tau, C));
+  if (a.tokens || !launch) GTNB_TRY(dev_alloc(ctx, &arcs, (long long)B * T));
+  float* wide = nullptr;
+  if (half) {
+    GTNB_TRY(dev_alloc(ctx, &wide, per * B));
+    lat->emissions = wide;
+  }
+  if (!launch) return GTNB_OK;
+
+  if (half) GTNB_TRY(launch_widen(ctx, a.emissions, a.dtype, wide, per * B));
+  const GraphMeta& m0 = lat->meta_h[0];
+  const GraphMeta& m1 = lat->meta_h[B > 1 ? 1 : 0];
+  if (kind == AlignCriterion::Ctc) {
+    GTNB_TRY(launch_ctc_async_prepare(ctx, B, S, T, C, m0, m1, a.input_lens, a.targets, a.target_lens, lat->meta,
+                                      small, deltas, valid, kstatus));
+    GTNB_TRY(launch_ctc_build(ctx, lat.get(), a.targets, small, small + B, a.blank));
+  } else {
+    const bool asg = kind == AlignCriterion::Asg;
+    GTNB_TRY(launch_trellis_async_prepare(ctx, asg, B, S, T, C, m0, m1, a.input_lens, a.targets, a.target_lens,
+                                          lat->meta, small, deltas, valid, kstatus));
+    if (asg) {
+      GTNB_TRY(launch_asg_num_build(ctx, lat.get(), a.targets, small, small + B, a.trans_w, map));
+    } else {
+      GTNB_TRY(launch_ngram_tau(ctx, C, a.trans_w, tau));
+      GTNB_TRY(launch_ngram_num_build(ctx, lat.get(), a.targets, small, small + B, a.blank, a.trans_w, tau, map));
+    }
+  }
+  GTNB_TRY(launch_implicit_forward(ctx, lat.get(), kstatus, 0, -1, /*tropical=*/true));
+  GTNB_TRY(launch_implicit_trace(ctx, lat.get(), kstatus, a.paths, arcs, a.scores, T));
+  return launch_align_async_finalize(ctx, kind, B, T, lat->meta, lat->sg_in_ptr, kstatus, valid, arcs, a.paths,
+                                     a.tokens, a.scores, a.status);
+}
+
+int align_async_workspace(gtnb_ctx* ctx, AlignCriterion kind, int B, int T, int C, int S, int dtype, size_t* bytes) {
+  const std::string fn = std::string(align_async_name(kind)) + "_workspace";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !bytes)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  // (blank 0: sizing does not depend on it)
+  const AlignAsyncArgs a{B, T, C, S, dtype, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
+                         nullptr, nullptr, nullptr, nullptr};
+  GTNB_TRY(align_async_run(ctx, kind, a, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+int align_async_call(gtnb_ctx* ctx, AlignCriterion kind, void* cuda_stream, const AlignAsyncArgs& a,
+                     void* workspace_dev, size_t workspace_bytes) {
+  const std::string fn = align_async_name(kind);
+  if (!ctx || a.B < 0 || a.T < 0 || a.C <= 0 || a.S < 0 || !a.emissions ||
+      (kind != AlignCriterion::Ctc && !a.trans_w) || (a.S > 0 && !a.targets) || !a.target_lens || !a.scores ||
+      (a.B > 0 && !workspace_dev) || ((uintptr_t)workspace_dev & 255))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!known_dtype(a.dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
+  if (a.B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  return align_async_run(ctx, kind, a, true);
+}
+
+} // namespace
+
+extern "C" int gtnb_ctc_align_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, size_t* bytes) {
+  return align_async_workspace(ctx, AlignCriterion::Ctc, B, T, C, S, dtype, bytes);
+}
+
+extern "C" int gtnb_ctc_align_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, int S, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, const int32_t* targets_dev, const int32_t* target_lens_dev, int blank,
+    int32_t* paths_dev, int32_t* tokens_dev, float* scores_dev, int32_t* status_dev, void* workspace_dev,
+    size_t workspace_bytes) {
+  return align_async_call(ctx, AlignCriterion::Ctc, cuda_stream,
+                          AlignAsyncArgs{B, T, C, S, dtype, emissions_dev, input_lens_dev, nullptr, targets_dev,
+                                         target_lens_dev, blank, paths_dev, tokens_dev, scores_dev, status_dev},
+                          workspace_dev, workspace_bytes);
+}
+
+extern "C" int gtnb_ngram_ctc_align_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype,
+                                                    size_t* bytes) {
+  return align_async_workspace(ctx, AlignCriterion::Ngram, B, T, C, S, dtype, bytes);
+}
+
+extern "C" int gtnb_ngram_ctc_align_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, int S, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, const float* trans_w_dev, const int32_t* targets_dev,
+    const int32_t* target_lens_dev, int blank, int32_t* paths_dev, int32_t* tokens_dev, float* scores_dev,
+    int32_t* status_dev, void* workspace_dev, size_t workspace_bytes) {
+  return align_async_call(ctx, AlignCriterion::Ngram, cuda_stream,
+                          AlignAsyncArgs{B, T, C, S, dtype, emissions_dev, input_lens_dev, trans_w_dev, targets_dev,
+                                         target_lens_dev, blank, paths_dev, tokens_dev, scores_dev, status_dev},
+                          workspace_dev, workspace_bytes);
+}
+
+extern "C" int gtnb_asg_align_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, size_t* bytes) {
+  return align_async_workspace(ctx, AlignCriterion::Asg, B, T, C, S, dtype, bytes);
+}
+
+extern "C" int gtnb_asg_align_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, int S, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, const float* trans_w_dev, const int32_t* targets_dev,
+    const int32_t* target_lens_dev, int32_t* paths_dev, int32_t* tokens_dev, float* scores_dev, int32_t* status_dev,
+    void* workspace_dev, size_t workspace_bytes) {
+  return align_async_call(ctx, AlignCriterion::Asg, cuda_stream,
+                          AlignAsyncArgs{B, T, C, S, dtype, emissions_dev, input_lens_dev, trans_w_dev, targets_dev,
+                                         target_lens_dev, 0, paths_dev, tokens_dev, scores_dev, status_dev},
+                          workspace_dev, workspace_bytes);
+}
+
+/*
  * Loss over user-supplied target graphs (the criterion of the reference's pytorch_loss.py and of its word
  * decomposition examples):
  *   loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b))

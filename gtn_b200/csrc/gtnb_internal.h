@@ -201,6 +201,15 @@ int launch_trellis_async_gate(gtnb_ctx* ctx, int B, const int32_t* T_fwd, const 
 /* dst[map[o + a]] += src[o + a], a < meta[b].sg_A, o = meta[b].grad_graph_off, for every b with kstatus[b] == 0 */
 int launch_trellis_async_scatter(gtnb_ctx* ctx, int B, const GraphMeta* meta, const int32_t* kstatus,
                                  const int32_t* map, const float* src, float* dst);
+/* the numerator an asynchronous alignment traces (gtnb_ctc_align_async, gtnb_ngram_ctc_align_async,
+ * gtnb_asg_align_async) */
+enum class AlignCriterion { Ctc, Ngram, Asg };
+/* after launch_implicit_trace: status [B] (nullable) 0 / 1 (kstatus bit 1) / 2 (!valid) / 3 (kstatus bit 2, a tie);
+ * a NaN score and -1 rows of paths and tokens for 1 and 2; tokens [B][T_out] (nullable): the target position of each
+ * traced arc (arcs [B][T_out], read only when tokens is set), -1 for a blank or no arc */
+int launch_align_async_finalize(gtnb_ctx* ctx, AlignCriterion kind, int B, int T_out, const GraphMeta* meta,
+                                const int32_t* sg_in_ptr, const int32_t* kstatus, const int32_t* valid,
+                                const int32_t* arcs, int32_t* paths, int32_t* tokens, float* scores, int32_t* status);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);

@@ -258,6 +258,60 @@ __global__ void __launch_bounds__(256) trellis_async_scatter_kernel(
   for (int a = threadIdx.x; a < n; a += blockDim.x) atomicAdd(dst + map[o + a], src[o + a]);
 }
 
+/*
+ * gtnb_ctc_align_async / gtnb_ngram_ctc_align_async / gtnb_asg_align_async, after the tropical forward and the trace
+ * (k_implicit.cu), which wrote the score, the path's labels and its arcs, and raised kstatus bit 1 (a non-finite
+ * value) or bit 2 (kTrTie: a tie on the traced path).  status[b]: 2 for an utterance the prepare kernel refused,
+ * 1 for bit 1, 3 for bit 2, else 0.  Status 1 and 2 give a NaN score and -1 rows.  tokens[b][t]: the target position
+ * of the arc traced at frame t, found from the numbering of the build kernel G names:
+ *   Ctc    arc ids in ctcGraph's creation order, the arcs of node l in [in_ptr[l], in_ptr[l+1]); position (l - 1) / 2
+ *          for odd l, -1 (blank) for even l;
+ *   Ngram  the in-entry index is the arc id, node n is CTC node l = n - 1, then as Ctc;
+ *   Asg    arc a enters node a / 2 + 1: position a / 2.
+ * An arc of -1 (beyond T_b, no accepting path) gives -1.  paths, tokens, status nullable.  One CTA per utterance.
+ */
+template <AsyncGraph G>
+__global__ void __launch_bounds__(256) align_async_finalize_kernel(
+    int T_out, const GraphMeta* __restrict__ meta, const int32_t* __restrict__ sg_in_ptr,
+    const int32_t* __restrict__ kstatus, const int32_t* __restrict__ valid, const int32_t* __restrict__ arcs,
+    int32_t* __restrict__ paths, int32_t* __restrict__ tokens, float* __restrict__ scores,
+    int32_t* __restrict__ status) {
+  const int b = blockIdx.x;
+  const int ks = kstatus[b];
+  const int st = !valid[b] ? 2 : (ks & 1) ? 1 : (ks & 2) ? 3 : 0;
+  const bool flagged = st == 1 || st == 2;
+  if (threadIdx.x == 0) {
+    if (flagged) scores[b] = CUDART_NAN_F;
+    if (status) status[b] = st;
+  }
+  const GraphMeta m = meta[b];
+  const int32_t* ip = sg_in_ptr + m.sg_node_base;
+  const long long row = (long long)b * T_out;
+  for (int t = threadIdx.x; t < T_out; t += blockDim.x) {
+    if (flagged && paths) paths[row + t] = -1;
+    if (!tokens) continue;
+    const int a = flagged ? -1 : arcs[row + t];
+    int u = -1;
+    if (a >= 0) {
+      if constexpr (G == AsyncGraph::Asg) {
+        u = a / 2;
+      } else {
+        int lo = 0, hi = m.sg_N - 1; // the last node n with in_ptr[n] <= a: the one whose in-entries hold a
+        while (lo < hi) {
+          const int mid = (lo + hi + 1) / 2;
+          if (ip[mid] <= a)
+            lo = mid;
+          else
+            hi = mid - 1;
+        }
+        const int l = G == AsyncGraph::Ngram ? lo - 1 : lo;
+        u = (l & 1) ? (l - 1) / 2 : -1;
+      }
+    }
+    tokens[row + t] = u;
+  }
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
@@ -310,6 +364,23 @@ int launch_ctc_async_finalize(
   if (B <= 0) return GTNB_OK;
   GTNB_LAUNCH(ctx, "ctc_async_finalize", ctc_async_finalize_kernel<<<B, 256, 0, ctx->stream>>>(
       zp, z, s, kstatus, valid, losses, status, static_cast<uint32_t*>(grad), row_words));
+  return GTNB_OK;
+}
+
+int launch_align_async_finalize(gtnb_ctx* ctx, AlignCriterion kind, int B, int T_out, const GraphMeta* meta,
+                                const int32_t* sg_in_ptr, const int32_t* kstatus, const int32_t* valid,
+                                const int32_t* arcs, int32_t* paths, int32_t* tokens, float* scores,
+                                int32_t* status) {
+  if (B <= 0) return GTNB_OK;
+#define GTNB_ALIGN_FINALIZE(G_)                                                                                   \
+  GTNB_LAUNCH(ctx, "align_async_finalize", align_async_finalize_kernel<G_><<<B, 256, 0, ctx->stream>>>(           \
+      T_out, meta, sg_in_ptr, kstatus, valid, arcs, paths, tokens, scores, status))
+  switch (kind) {
+    case AlignCriterion::Ctc: GTNB_ALIGN_FINALIZE(AsyncGraph::Ctc); break;
+    case AlignCriterion::Ngram: GTNB_ALIGN_FINALIZE(AsyncGraph::Ngram); break;
+    case AlignCriterion::Asg: GTNB_ALIGN_FINALIZE(AsyncGraph::Asg); break;
+  }
+#undef GTNB_ALIGN_FINALIZE
   return GTNB_OK;
 }
 

@@ -547,6 +547,111 @@ def collapse(paths, blank=None):
     return out[:, :T].contiguous(), lengths
 
 
+@torch.no_grad()
+def _align_async(name, emissions, transitions, targets, target_lengths, input_lengths, blank, kind):
+    """gtnb_{ctc,ngram_ctc,asg}_align_async on the current stream (kind: "ctc", "ngram", "asg")"""
+    assert _tensor_targets(name, emissions, targets, input_lengths, target_lengths), \
+        "%s: targets must be a 2-D integer CUDA tensor on the emissions' device" % name
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    S = targets.shape[1]
+    w = None
+    if kind != "ctc":
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == (Cn + Cn * Cn if kind == "asg" else Cn * Cn)
+        w = transitions.detach().contiguous()
+    tgt = targets.to(torch.int32).contiguous()
+    tl = target_lengths.to(torch.int32).contiguous()
+    il = None if input_lengths is None else input_lengths.to(torch.int32).contiguous()
+    dtype = _EMISSION_DTYPES[e.dtype]
+    g = _async_ctx(e.device, name)
+    lib = capi.lib()
+    call, sizing = {"ctc": (lib.gtnb_ctc_align_async, lib.gtnb_ctc_align_async_workspace),
+                    "ngram": (lib.gtnb_ngram_ctc_align_async, lib.gtnb_ngram_ctc_align_async_workspace),
+                    "asg": (lib.gtnb_asg_align_async, lib.gtnb_asg_align_async_workspace)}[kind]
+    nbytes = C.c_size_t()
+    rc = sizing(g.h, B, T, Cn, S, dtype, C.byref(nbytes))
+    if rc == capi.ERR_UNSUPPORTED:
+        other = "graph_viterbi" if kind == "ctc" else "graph_transitions_viterbi"
+        raise RuntimeError("%s: these bounds are outside the device alignment (%s); align on the host-built graphs "
+                           "with %s instead" % (name, lib.gtnb_last_error(g.h).decode(), other))
+    g._check(rc)
+    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    tokens = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    scores = torch.empty(B, dtype=torch.float32, device=e.device)
+    status = torch.empty(B, dtype=torch.int32, device=e.device)
+    stream = torch.cuda.current_stream(e.device).cuda_stream
+    il_p = None if il is None else il.data_ptr()
+    outs = (paths.data_ptr(), tokens.data_ptr(), scores.data_ptr(), status.data_ptr(), ws.data_ptr(), nbytes.value)
+    if kind == "ctc":
+        rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, tgt.data_ptr(), tl.data_ptr(), int(blank), *outs)
+    elif kind == "ngram":
+        rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, w.data_ptr(), tgt.data_ptr(), tl.data_ptr(),
+                  int(blank), *outs)
+    else:
+        rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, w.data_ptr(), tgt.data_ptr(), tl.data_ptr(),
+                  *outs)
+    g._check(rc)
+    return paths, tokens, scores, status
+
+
+def ctc_align(emissions, targets, target_lengths, input_lengths=None, blank=0):
+    """Forced alignment of CTC: viterbiPath / viterbiScore of intersect(ctcGraph(y_b), E_b), the numerator of ctc_loss,
+    through gtnb_ctc_align_async on the current stream, without a host synchronisation (it may be captured in a CUDA
+    graph).
+
+    emissions: float32, bfloat16 or float16 CUDA tensor [B, T, C] (16-bit: the results of the float32 call on
+    emissions.float()); targets: [B, S] integer tensor on the emissions' device, row b holding target_lengths[b]
+    labels; target_lengths and input_lengths (or None): [B] integer tensors on that device.  Returns device tensors
+    (paths [B, T] int32, the label of every frame; tokens [B, T] int32, the target position each frame is aligned to,
+    -1 for a blank frame; both -1 beyond T_b and where no path accepts; scores [B] float32, -inf for a target with no
+    path; status [B] int32: 0 as gtnb_graph_viterbi, 1 a non-finite value, 2 an invalid length or label, both with a
+    NaN score and -1 rows, 3 a tie on the path, which is then an optimal path that gtnb_graph_viterbi may break
+    differently).  Bounds outside the device route raise a RuntimeError; graph_viterbi on ctc graphs covers them.
+    """
+    return _align_async("ctc_align", emissions, None, targets, target_lengths, input_lengths, blank, "ctc")
+
+
+def ngram_ctc_align(emissions, transitions, targets, target_lengths, input_lengths=None, blank=0):
+    """Forced alignment of n-gram CTC: viterbiPath / viterbiScore of intersect(intersect(ctc_b, G), E_b), the numerator
+    of ngram_ctc_loss, through gtnb_ngram_ctc_align_async.  transitions: float32 CUDA tensor of C*C elements (row =
+    destination label) on the emissions' device.  Arguments and results otherwise as ctc_align's; any C the device
+    sweeps take, beyond ngram_ctc_loss's 128 labels.  Bounds outside the device route raise a RuntimeError;
+    graph_transitions_viterbi (kind "bigram") covers them.
+    """
+    return _align_async("ngram_ctc_align", emissions, transitions, targets, target_lengths, input_lengths, blank,
+                        "ngram")
+
+
+def asg_align(emissions, transitions, targets, target_lengths, input_lengths=None):
+    """Forced alignment of ASG: viterbiPath / viterbiScore of compose(compose(fal_b, transitions), E_b), the numerator
+    of asg_loss, through gtnb_asg_align_async.  transitions: float32 CUDA tensor of C + C*C elements (start weights,
+    then the matrix) on the emissions' device.  Every frame in [0, T_b) of an accepted path gets a target position.
+    Arguments and results otherwise as ctc_align's.  Bounds outside the device route raise a RuntimeError;
+    graph_transitions_viterbi (kind "asg") on force-align chains covers them.
+    """
+    return _align_async("asg_align", emissions, transitions, targets, target_lengths, input_lengths, 0, "asg")
+
+
+@torch.no_grad()
+def align_spans(tokens, S):
+    """The frames each target position occupies: tokens [B, T] (ctc_align's, -1 for none) -> (start, end), each
+    [B, S] int32, the first frame and one past the last frame of position u, -1 where u is absent.  Elementwise and
+    scatter ops on the tokens' device, without a host synchronisation."""
+    tok = tokens.long()
+    B, T = tok.shape
+    present = (tok >= 0) & (tok < S)
+    slot = torch.where(present, tok, S)  # absent frames go to an extra column that is dropped
+    t = torch.arange(T, device=tok.device).expand(B, T)
+    start = torch.full((B, S + 1), T, dtype=torch.long, device=tok.device)
+    start.scatter_reduce_(1, slot, torch.where(present, t, T), "amin")
+    end = torch.full((B, S + 1), -1, dtype=torch.long, device=tok.device)
+    end.scatter_reduce_(1, slot, torch.where(present, t + 1, -1), "amax")
+    absent = end[:, :S] < 0
+    return (torch.where(absent, -1, start[:, :S]).int(), torch.where(absent, -1, end[:, :S]).int())
+
+
 def _graph_view(g):
     """capi view of a gtn_b200.gtn.Graph built on the host, in its own arc-list order"""
     from . import _gtn

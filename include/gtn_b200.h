@@ -651,6 +651,104 @@ int gtnb_ngram_ctc_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int 
 int gtnb_asg_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, int with_grad, size_t* bytes);
 
 /*
+ * Forced alignment without a host synchronisation: viterbiPath / viterbiScore of the numerator of gtnb_ctc_loss_async,
+ * gtnb_ngram_ctc_loss_async or gtnb_asg_loss_async, which tells which frames each target token occupies:
+ *   gtnb_ctc_align_async        intersect(ctcGraph(y_b), E_b)              (gtnb_graph_viterbi on CTC graphs)
+ *   gtnb_ngram_ctc_align_async  intersect(intersect(ctc_b, G), E_b)        (gtnb_graph_transitions_viterbi, BIGRAM)
+ *   gtnb_asg_align_async        compose(compose(fal_b, transitions), E_b)  (gtnb_graph_transitions_viterbi, ASG)
+ * The contract is gtnb_ctc_loss_async's: the call enqueues kernel launches on cuda_stream (NULL: the CUDA default
+ * stream) and returns, without a host synchronisation, a read of device data on the host, an allocation or a staging
+ * copy; it may be captured into a CUDA graph.  Scratch memory is workspace_dev (256-byte aligned, at least the matching
+ * *_align_async_workspace's bytes for the same bounds and dtype; smaller is GTNB_ERR_INVALID_ARGUMENT).  The call is
+ * sized from the bounds (every utterance as if U = S and T_b = T), never from the labels.  Emissions of dtype
+ * GTNB_BF16 / GTNB_F16 are widened to float32 in the workspace: the results are the float32 call's on the widened
+ * emissions.  The "implicit" flag at 0, bounds outside the implicit sweeps or the trace, blank outside [0, C) and an
+ * unknown dtype are GTNB_ERR_UNSUPPORTED: use gtnb_graph_viterbi / gtnb_graph_transitions_viterbi.  There is no
+ * bound on C beyond the sweeps' own (n-gram and ASG alignment do not hold a dense trellis).
+ *
+ * targets_dev [B][S] int32, row b holding target_lens_dev[b] labels; input_lens_dev [B] (NULL: T each); trans_w_dev
+ * float32 on the device, n-gram W [C*C] (row = destination label), ASG [C + C*C].  Outputs, written on the device:
+ *   paths_dev [B][T] (nullable)   the label of every frame of the best path;
+ *   tokens_dev [B][T] (nullable)  the target position u in [0, U_b) each frame is aligned to, -1 for a blank frame
+ *                                 (CTC, n-gram CTC; every ASG frame in [0, T_b) has one);
+ *                                 both -1 beyond T_b and wherever no path accepts;
+ *   scores_dev [B]                viterbiScore: -inf for T_b = 0 or a target with no path;
+ *   status_dev [B] (nullable)     0  paths, tokens and score are the synchronous aligner's, ties included;
+ *                                 1  the sweep met a non-finite value (the synchronous aligner takes its exact route):
+ *                                    a NaN score and -1 rows;
+ *                                 2  invalid input: target_lens_dev[b] outside [0, S], input_lens_dev[b] outside
+ *                                    [0, T] or a label outside [0, C): a NaN score and -1 rows;
+ *                                 3  a tie on the traced path: the score is the synchronous aligner's and the path
+ *                                    an optimal one, which may break the tie differently (exact_ties off).
+ * A flagged utterance never affects the others.
+ */
+int gtnb_ctc_align_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    int S,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const int32_t* targets_dev, /* [B][S] */
+    const int32_t* target_lens_dev, /* [B] */
+    int blank,
+    int32_t* paths_dev, /* [B][T] or NULL */
+    int32_t* tokens_dev, /* [B][T] or NULL */
+    float* scores_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+int gtnb_ngram_ctc_align_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    int S,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const float* trans_w_dev, /* [C*C] */
+    const int32_t* targets_dev, /* [B][S] */
+    const int32_t* target_lens_dev, /* [B] */
+    int blank,
+    int32_t* paths_dev, /* [B][T] or NULL */
+    int32_t* tokens_dev, /* [B][T] or NULL */
+    float* scores_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+int gtnb_asg_align_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    int S,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const float* trans_w_dev, /* [C + C*C] */
+    const int32_t* targets_dev, /* [B][S] */
+    const int32_t* target_lens_dev, /* [B] */
+    int32_t* paths_dev, /* [B][T] or NULL */
+    int32_t* tokens_dev, /* [B][T] or NULL */
+    float* scores_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/* *bytes: the workspace the matching *_align_async call needs for these bounds and dtype (host work only) */
+int gtnb_ctc_align_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, size_t* bytes);
+int gtnb_ngram_ctc_align_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, size_t* bytes);
+int gtnb_asg_align_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int S, int dtype, size_t* bytes);
+
+/*
  * Loss over one user-supplied target graph per utterance (the criterion of the reference's pytorch_loss.py and of
  * its word-decomposition examples):
  *   loss_b = forwardScore(E_b) - forwardScore(intersect(A_b, E_b))
