@@ -172,6 +172,15 @@ SYMBOLS = [
     ("gtnb_backoff_transitions_viterbi", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _i32p, C.POINTER(GraphView), _vp, C.c_int, C.POINTER(GraphView),
       _vp, C.c_int, _vp, _vp, _vp, C.c_int]),
+    ("gtnb_transitions_create", C.c_int, [_vp, C.POINTER(GraphView), C.c_int, C.c_int, C.POINTER(_vp)]),
+    ("gtnb_transitions_destroy", None, [_vp, _vp]),
+    ("gtnb_viterbi_transitions_async_workspace", C.c_int, [_vp, _vp, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_viterbi_transitions_async", C.c_int,
+     [_vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
+    ("gtnb_viterbi_dense_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_viterbi_dense_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
 ]
 
 _lib = None

@@ -2408,26 +2408,38 @@ extern "C" int gtnb_graph_transitions_loss(
  */
 namespace {
 
-/* G's tables and start groups (gtnb_product.h) in one device buffer, filled by stage() */
+/* G's tables and start groups (gtnb_product.h) in one device buffer: pack() them, then alloc() the buffer from a call's
+ * scratch and stage() it, or place() them at a buffer of packed.size() words the caller owns (gtnb_transitions) */
 struct SparseDevTables {
   std::vector<int32_t> packed;
+  std::vector<size_t> at;
+  int S = 0, A = 0;
   int32_t* tab = nullptr;
   SparseDev dev{};
   const int32_t *grp_ptr = nullptr, *grp_arc = nullptr;
 
-  int alloc(CallScope& scope, const SparseTables& t) {
+  void pack(const SparseTables& t) {
+    S = t.S, A = t.A;
     packed.assign(t.flags.begin(), t.flags.end());
-    std::vector<size_t> at;
+    at.clear();
     for (const std::vector<int32_t>* v : {&t.in_ptr, &t.in_src, &t.in_lab, &t.in_arc, &t.out_ptr, &t.out_dst,
                                           &t.out_lab, &t.out_arc, &t.grp_ptr, &t.grp_arc}) {
       at.push_back(packed.size());
       packed.insert(packed.end(), v->begin(), v->end());
     }
-    GTNB_TRY(scope.alloc(&tab, (long long)packed.size()));
-    dev = SparseDev{t.S, t.A, sparse_den_lanes(t.S, t.A), tab, tab + at[0], tab + at[1], tab + at[2], tab + at[3],
+  }
+  void place(int32_t* buf) {
+    tab = buf;
+    dev = SparseDev{S, A, sparse_den_lanes(S, A), tab, tab + at[0], tab + at[1], tab + at[2], tab + at[3],
                     tab + at[4], tab + at[5], tab + at[6], tab + at[7]};
     grp_ptr = tab + at[8];
     grp_arc = tab + at[9];
+  }
+  int alloc(CallScope& scope, const SparseTables& t) {
+    pack(t);
+    int32_t* buf = nullptr;
+    GTNB_TRY(scope.alloc(&buf, (long long)packed.size()));
+    place(buf);
     return GTNB_OK;
   }
   int stage(CallScope& scope) { return stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()); }
@@ -3110,7 +3122,8 @@ extern "C" int gtnb_sparse_transitions_viterbi(
 namespace {
 
 /* acceptors with epsilon arcs (SparseTables with its epsilon tables) in one device buffer for the sparse_eps_*
- * kernels: add() every graph, its arc ids shifted by arc_base and its score rows at `rows`, then alloc(), stage() */
+ * kernels: add() every graph, its arc ids shifted by arc_base and its score rows at `rows`, then alloc(), stage(); or
+ * place() them at buffers the caller owns (packed.size() words and desc.size() descriptors; gtnb_transitions) */
 struct EpsDevTables {
   std::vector<int32_t> packed;
   std::vector<std::vector<size_t>> at; // per graph: where each of its tables starts in packed
@@ -3150,8 +3163,17 @@ struct EpsDevTables {
     max_AE = std::max(max_AE, t.A + t.E);
   }
   int alloc(CallScope& scope) {
-    GTNB_TRY(scope.alloc(&tab, (long long)packed.size()));
-    GTNB_TRY(scope.alloc(&dev, (long long)desc.size()));
+    int32_t* t = nullptr;
+    SparseEpsDev* d = nullptr;
+    GTNB_TRY(scope.alloc(&t, (long long)packed.size()));
+    GTNB_TRY(scope.alloc(&d, (long long)desc.size()));
+    place(t, d);
+    return GTNB_OK;
+  }
+  /* desc's pointers into tab_buf; dev = dev_buf, which then takes desc */
+  void place(int32_t* tab_buf, SparseEpsDev* dev_buf) {
+    tab = tab_buf;
+    dev = dev_buf;
     for (size_t i = 0; i < desc.size(); i++) {
       const int32_t* p[20];
       for (int j = 0; j < 20; j++) p[j] = tab + at[i][j];
@@ -3163,7 +3185,6 @@ struct EpsDevTables {
       d.eps_out_ptr = p[12], d.eps_out_dst = p[13], d.eps_out_arc = p[14];
       d.fwd_ptr = p[15], d.fwd_node = p[16], d.bwd_ptr = p[17], d.bwd_node = p[18], d.lanes = p[19];
     }
-    return GTNB_OK;
   }
   int stage(CallScope& scope) {
     GTNB_TRY(stage_upload(scope.ctx(), tab, packed.data(), sizeof(int32_t) * packed.size()));
@@ -3770,4 +3791,229 @@ extern "C" int gtnb_backoff_transitions_viterbi(
   return backoff_align_run(scope, GraphViterbiArgs{emissions, emissions_on_device, paths, arcs, scores,
                                                    outputs_on_device},
                            gb, *transitions, t, prods, ptabs, fast, trans_w, trans_on_device);
+}
+
+/*
+ * Decoding without a host synchronisation, under gtnb_ctc_loss_async's contract.
+ *   gtnb_viterbi_transitions_async: gtnb_viterbi_sparse / gtnb_viterbi_backoff on a G prepared once
+ *     (gtnb_transitions): its tables, epsilon descriptor and cluster cuts live in device memory the handle owns, so a
+ *     call uploads nothing.  The route is the synchronous decoders' device route: the prepare kernel, the tropical
+ *     sweep and trace of k_sparse.cu (one CTA or a cluster per utterance, with or without epsilon arcs) and the
+ *     finalize kernel, which maps the kernel status where the synchronous decoders read it back and re-run.
+ *   gtnb_viterbi_dense_async: gtnb_viterbi_dense_typed with device lengths: the prepare kernel, k_dense.cu's decode
+ *     and the finalize kernel (the dense kernel raises no status: only invalid lengths are flagged).
+ * Back-pointers are sized from the bounds.
+ */
+struct gtnb_transitions {
+  int device = 0, C = 0, S = 0;
+  long long n_arcs = 0; // G's arcs: the length of trans_w
+  bool eps = false; // G has epsilon arcs: the sparse_eps_* kernels over eps_dev (else the sparse_* kernels over dev)
+  SparseSplit split{}; // sparse_route's / backoff_route's: N = 1 one CTA per utterance, else a cluster's plan
+  void* mem = nullptr; // every device buffer below
+  SparseDev dev{};
+  SparseEpsDev* eps_dev = nullptr;
+  int32_t* cut = nullptr; // sparse_eps_cluster_cuts (eps and split.N > 1), else NULL
+  ~gtnb_transitions() {
+    if (mem) cudaFree(mem);
+  }
+};
+
+
+extern "C" int gtnb_transitions_create(gtnb_ctx* ctx, const gtnb_graph_view* Gv, int C, int backoff,
+                                       gtnb_transitions** out) {
+  const std::string fn = "gtnb_transitions_create";
+  if (out) *out = nullptr;
+  if (!ctx || !Gv || C <= 0 || !out || (backoff != 0 && backoff != 1))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  const std::string sync = backoff ? "gtnb_viterbi_backoff" : "gtnb_viterbi_sparse";
+  SparseTables t;
+  if (backoff) {
+    GTNB_TRY(check_backoff_graph(ctx, fn, *Gv, C, &t));
+  } else {
+    GTNB_TRY(check_transition_graph(ctx, fn, *Gv));
+    sparse_tables(*Gv, C, &t);
+  }
+  if (!ctx->use_implicit)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": the \"implicit\" flag is off (materialised route): decode with " + sync);
+  std::unique_ptr<gtnb_transitions> h(new gtnb_transitions);
+  h->device = ctx->device;
+  h->C = C;
+  h->S = t.S;
+  h->n_arcs = Gv->num_arcs;
+  h->eps = t.E > 0;
+  const bool fits = h->eps ? backoff_route(ctx, t, C, &h->split) : sparse_route(ctx, t, C, &h->split);
+  if (!fits)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                fn + ": the transition graph is outside the device decoders' envelope: decode with " + sync);
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  // one allocation, 256-byte granules: the packed tables, then (epsilon arcs) the descriptor and the cuts
+  std::vector<const void*> src;
+  std::vector<size_t> bytes;
+  std::vector<void*> dst;
+  SparseDevTables st;
+  EpsDevTables et;
+  std::vector<int32_t> cut_h;
+  if (h->eps) {
+    et.add(t, 0, 0);
+    if (h->split.N > 1) sparse_eps_cluster_cuts(t, h->split, &cut_h);
+    bytes = {sizeof(int32_t) * et.packed.size(), sizeof(SparseEpsDev), sizeof(int32_t) * cut_h.size()};
+  } else {
+    st.pack(t);
+    bytes = {sizeof(int32_t) * st.packed.size()};
+  }
+  size_t total = 0;
+  for (size_t n : bytes) total += (n + 255) & ~(size_t)255;
+  GTNB_CUDA(ctx, cudaMalloc(&h->mem, total));
+  for (size_t i = 0, at = 0; i < bytes.size(); at += (bytes[i] + 255) & ~(size_t)255, i++)
+    dst.push_back(static_cast<unsigned char*>(h->mem) + at);
+  if (h->eps) {
+    et.place(static_cast<int32_t*>(dst[0]), static_cast<SparseEpsDev*>(dst[1]));
+    src = {et.packed.data(), et.desc.data(), cut_h.data()};
+    h->eps_dev = et.dev;
+    if (!cut_h.empty()) h->cut = static_cast<int32_t*>(dst[2]);
+  } else {
+    st.place(static_cast<int32_t*>(dst[0]));
+    src = {st.packed.data()};
+    h->dev = st.dev;
+  }
+  for (size_t i = 0; i < bytes.size(); i++)
+    if (bytes[i]) GTNB_CUDA(ctx, cudaMemcpy(dst[i], src[i], bytes[i], cudaMemcpyHostToDevice));
+  GTNB_CUDA(ctx, cudaDeviceSynchronize()); // (set-up: the tables are on the device before any stream reads them)
+  *out = h.release();
+  return GTNB_OK;
+}
+
+extern "C" void gtnb_transitions_destroy(gtnb_ctx* ctx, gtnb_transitions* G) {
+  if (!G) return;
+  if (ctx) cudaSetDevice(G->device);
+  delete G; // (cudaFree waits for the device: no launch still reads the tables)
+}
+
+namespace {
+
+struct DecodeAsyncArgs {
+  int B, T;
+  const void* emissions;
+  int dtype; // (dense only)
+  const int32_t* input_lens;
+  const float* trans_w;
+  int32_t *paths, *arcs;
+  float* scores;
+  int32_t* status;
+};
+
+/* gtnb_viterbi_transitions_async inside a BorrowedArena: the scratch taken from the arena and, when launch, the work
+ * enqueued */
+int transitions_async_run(gtnb_ctx* ctx, const gtnb_transitions* G, const DecodeAsyncArgs& a, bool launch) {
+  const int B = a.B, T = a.T, C = G->C, S = G->S;
+  int32_t *lens = nullptr, *valid = nullptr, *kstatus = nullptr, *head = nullptr;
+  uint16_t* bp = nullptr;
+  GTNB_TRY(dev_alloc(ctx, &lens, B));
+  GTNB_TRY(dev_alloc(ctx, &valid, B));
+  GTNB_TRY(dev_alloc(ctx, &kstatus, B));
+  GTNB_TRY(dev_alloc(ctx, &head, B));
+  // (the synchronous decoders' sizes at T_b = T)
+  GTNB_TRY(dev_alloc(ctx, &bp, G->eps ? (long long)B * (T + 1) * S : std::max((long long)B * T * S, 1ll)));
+  if (!launch) return GTNB_OK;
+  const float* e = static_cast<const float*>(a.emissions);
+  GTNB_TRY(launch_decode_async_prepare(ctx, B, T, a.input_lens, lens, valid, kstatus));
+  if (G->eps)
+    GTNB_TRY(launch_sparse_eps_viterbi(ctx, G->eps_dev, G->split, G->cut, S, B, T, C, lens, e, (long long)T * C,
+                                       a.trans_w, bp, head, a.scores, a.paths, a.arcs, kstatus));
+  else
+    GTNB_TRY(launch_sparse_viterbi(ctx, G->dev, G->split, B, T, C, lens, e, (long long)T * C, a.trans_w, bp, head,
+                                   a.scores, a.paths, a.arcs, kstatus));
+  return launch_decode_async_finalize(ctx, B, T, lens, kstatus, valid, a.paths, a.arcs, a.scores, a.status);
+}
+
+/* gtnb_viterbi_dense_async inside a BorrowedArena; sizing takes the paths row whether or not paths will be given */
+int dense_async_run(gtnb_ctx* ctx, int C, bool bigram, const DecodeAsyncArgs& a, bool launch) {
+  const int B = a.B, T = a.T;
+  if (!viterbi_dense_supported(C))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_viterbi_dense_async: the transitions tile does not fit shared memory "
+                                           "(C <= 224)");
+  int32_t *lens = nullptr, *valid = nullptr, *kstatus = nullptr, *paths = a.paths;
+  uint8_t* bp = nullptr;
+  GTNB_TRY(dev_alloc(ctx, &lens, B));
+  GTNB_TRY(dev_alloc(ctx, &valid, B));
+  GTNB_TRY(dev_alloc(ctx, &kstatus, B));
+  GTNB_TRY(dev_alloc(ctx, &bp, (long long)B * std::max(T, 1) * dense_bp_pitch(C)));
+  if (!paths || !launch) GTNB_TRY(dev_alloc(ctx, &paths, (long long)B * std::max(T, 1)));
+  if (!launch) return GTNB_OK;
+  GTNB_TRY(launch_decode_async_prepare(ctx, B, T, a.input_lens, lens, valid, kstatus));
+  GTNB_TRY(launch_viterbi_dense(ctx, B, T, C, bigram, lens, a.emissions, (long long)T * C, a.trans_w,
+                                -std::numeric_limits<float>::infinity(), bp, paths, a.scores, a.dtype));
+  return launch_decode_async_finalize(ctx, B, T, lens, kstatus, valid, a.paths, nullptr, a.scores, a.status);
+}
+
+} // namespace
+
+extern "C" int gtnb_viterbi_transitions_async_workspace(gtnb_ctx* ctx, const gtnb_transitions* G, int B, int T,
+                                                        size_t* bytes) {
+  const char* fn = "gtnb_viterbi_transitions_async_workspace";
+  if (!ctx || !G || B < 0 || T < 0 || !bytes) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
+  if (G->device != ctx->device)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": the transition graph was made on another device");
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  const DecodeAsyncArgs a{B, T, nullptr, GTNB_F32, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  GTNB_TRY(transitions_async_run(ctx, G, a, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+extern "C" int gtnb_viterbi_transitions_async(
+    gtnb_ctx* ctx, void* cuda_stream, const gtnb_transitions* G, int B, int T, const float* emissions_dev,
+    const int32_t* input_lens_dev, const float* trans_w_dev, int32_t* paths_dev, int32_t* arcs_dev, float* scores_dev,
+    int32_t* status_dev, void* workspace_dev, size_t workspace_bytes) {
+  const std::string fn = "gtnb_viterbi_transitions_async";
+  if (!ctx || !G || B < 0 || T < 0 || (B > 0 && (!emissions_dev || !trans_w_dev || !paths_dev || !scores_dev)) ||
+      (B > 0 && !workspace_dev) || ((uintptr_t)workspace_dev & 255))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (G->device != ctx->device)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the transition graph was made on another device");
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  return transitions_async_run(ctx, G,
+                               DecodeAsyncArgs{B, T, emissions_dev, GTNB_F32, input_lens_dev, trans_w_dev, paths_dev,
+                                               arcs_dev, scores_dev, status_dev},
+                               true);
+}
+
+extern "C" int gtnb_viterbi_dense_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind,
+                                                  size_t* bytes) {
+  const std::string fn = "gtnb_viterbi_dense_async_workspace";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !bytes || (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  const DecodeAsyncArgs a{B, T, nullptr, dtype, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  GTNB_TRY(dense_async_run(ctx, C, kind == GTNB_DENSE_BIGRAM, a, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+extern "C" int gtnb_viterbi_dense_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, int kind, const float* trans_w_dev, int32_t* paths_dev, float* scores_dev,
+    int32_t* status_dev, void* workspace_dev, size_t workspace_bytes) {
+  const std::string fn = "gtnb_viterbi_dense_async";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM) ||
+      (B > 0 && (!emissions_dev || !trans_w_dev || !scores_dev || !workspace_dev)) ||
+      ((uintptr_t)workspace_dev & 255))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  return dense_async_run(ctx, C, kind == GTNB_DENSE_BIGRAM,
+                         DecodeAsyncArgs{B, T, emissions_dev, dtype, input_lens_dev, trans_w_dev, paths_dev, nullptr,
+                                         scores_dev, status_dev},
+                         true);
 }

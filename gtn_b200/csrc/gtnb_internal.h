@@ -210,6 +210,16 @@ enum class AlignCriterion { Ctc, Ngram, Asg };
 int launch_align_async_finalize(gtnb_ctx* ctx, AlignCriterion kind, int B, int T_out, const GraphMeta* meta,
                                 const int32_t* sg_in_ptr, const int32_t* kstatus, const int32_t* valid,
                                 const int32_t* arcs, int32_t* paths, int32_t* tokens, float* scores, int32_t* status);
+/* the asynchronous decoders' set-up (gtnb_viterbi_transitions_async, gtnb_viterbi_dense_async): lens / valid / kstatus
+ * [B], lens[b] = T_b or 0 where input_lens[b] (NULL: T) lies outside [0, T], valid[b] whether it lies inside, kstatus
+ * zeroed */
+int launch_decode_async_prepare(gtnb_ctx* ctx, int B, int T, const int32_t* input_lens, int32_t* lens,
+                                int32_t* valid, int32_t* kstatus);
+/* after the sweep and trace: status [B] (nullable) 0 / 1 (kstatus bit 1) / 2 (!valid) / 3 (kstatus bit 2), kstatus
+ * ignored where lens[b] = 0; a NaN score and -1 rows of paths and arcs ([B][T_out], nullable) for 1 and 2 */
+int launch_decode_async_finalize(gtnb_ctx* ctx, int B, int T_out, const int32_t* lens, const int32_t* kstatus,
+                                 const int32_t* valid, int32_t* paths, int32_t* arcs, float* scores,
+                                 int32_t* status);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
@@ -390,6 +400,8 @@ int ensure_side_streams(gtnb_ctx* ctx, int n_streams, int n_events);
 // kernel (k_dense.cu): factored dense-trellis Viterbi.  bigram: trans_dev is n-gram CTC's [C*C] W (every state
 // starts), else ASG's [C + C*C]; bp holds [B][T_max][dense_bp_pitch(C)] bytes; 1 <= C <= 224
 int dense_bp_pitch(int C);
+// whether launch_viterbi_dense takes C: the transition tile fits shared memory (C <= 224)
+bool viterbi_dense_supported(int C);
 // emis: elements of dtype (GTNB_F32 / GTNB_BF16 / GTNB_F16), read as they are
 int launch_viterbi_dense(
     gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const void* emis, int64_t stride,

@@ -312,6 +312,50 @@ __global__ void __launch_bounds__(256) align_async_finalize_kernel(
   }
 }
 
+/*
+ * gtnb_viterbi_transitions_async / gtnb_viterbi_dense_async, before the sweep: lens[b] = T_b (input_lens[b], or T when
+ * input_lens is NULL), valid[b] = whether T_b lies in [0, T].  An invalid utterance is swept with lens[b] = 0, so no
+ * kernel indexes with its length.  kstatus[b] = 0.  One thread per utterance.
+ */
+__global__ void __launch_bounds__(256) decode_async_prepare_kernel(int B, int T, const int32_t* __restrict__ input_lens,
+                                                                   int32_t* __restrict__ lens,
+                                                                   int32_t* __restrict__ valid,
+                                                                   int32_t* __restrict__ kstatus) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int Tb = input_lens ? input_lens[b] : T;
+  const int ok = Tb >= 0 && Tb <= T;
+  lens[b] = ok ? Tb : 0;
+  valid[b] = ok;
+  kstatus[b] = 0;
+}
+
+/*
+ * The asynchronous decoders, after the sweep and its trace: status[b] = 2 for an utterance the prepare kernel refused,
+ * else, for T_b > 0, 1 for kstatus bit 1 (a non-finite value), 3 for bit 2 (a tie), else 0.  T_b = 0 is 0 whatever
+ * the kernel raised: no frame is decoded, and the synchronous decoders ignore the status there too.  Status 1 and 2
+ * give a NaN score and -1 rows of paths and arcs (both nullable, [B][T_out]).  status nullable.  One CTA per
+ * utterance.
+ */
+__global__ void __launch_bounds__(256) decode_async_finalize_kernel(
+    int T_out, const int32_t* __restrict__ lens, const int32_t* __restrict__ kstatus,
+    const int32_t* __restrict__ valid, int32_t* __restrict__ paths, int32_t* __restrict__ arcs,
+    float* __restrict__ scores, int32_t* __restrict__ status) {
+  const int b = blockIdx.x;
+  const int ks = lens[b] > 0 ? kstatus[b] : 0;
+  const int st = !valid[b] ? 2 : (ks & 1) ? 1 : (ks & 2) ? 3 : 0;
+  if (threadIdx.x == 0) {
+    if (st == 1 || st == 2) scores[b] = CUDART_NAN_F;
+    if (status) status[b] = st;
+  }
+  if (st != 1 && st != 2) return;
+  const long long row = (long long)b * T_out;
+  for (int t = threadIdx.x; t < T_out; t += blockDim.x) {
+    if (paths) paths[row + t] = -1;
+    if (arcs) arcs[row + t] = -1;
+  }
+}
+
 } // namespace
 
 #ifndef GTNB_HOST_EMU
@@ -381,6 +425,23 @@ int launch_align_async_finalize(gtnb_ctx* ctx, AlignCriterion kind, int B, int T
     case AlignCriterion::Asg: GTNB_ALIGN_FINALIZE(AsyncGraph::Asg); break;
   }
 #undef GTNB_ALIGN_FINALIZE
+  return GTNB_OK;
+}
+
+int launch_decode_async_prepare(gtnb_ctx* ctx, int B, int T, const int32_t* input_lens, int32_t* lens,
+                                int32_t* valid, int32_t* kstatus) {
+  if (B <= 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "decode_async_prepare", decode_async_prepare_kernel<<<(B + 255) / 256, 256, 0, ctx->stream>>>(
+      B, T, input_lens, lens, valid, kstatus));
+  return GTNB_OK;
+}
+
+int launch_decode_async_finalize(gtnb_ctx* ctx, int B, int T_out, const int32_t* lens, const int32_t* kstatus,
+                                 const int32_t* valid, int32_t* paths, int32_t* arcs, float* scores,
+                                 int32_t* status) {
+  if (B <= 0) return GTNB_OK;
+  GTNB_LAUNCH(ctx, "decode_async_finalize", decode_async_finalize_kernel<<<B, 256, 0, ctx->stream>>>(
+      T_out, lens, kstatus, valid, paths, arcs, scores, status));
   return GTNB_OK;
 }
 

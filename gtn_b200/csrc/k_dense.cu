@@ -230,13 +230,24 @@ __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
 
 namespace {
 
+/* lanes per state: G = 256 / C rounded down to a power of two, at most 32 */
+int dense_lanes(int C) {
+  int G = 1;
+  while (G < 32 && C * (G * 2) <= kDenseThreads) G *= 2;
+  return G;
+}
+
+/* the transition tile and the two score rows */
+size_t dense_smem_bytes(int C) {
+  return sizeof(float) * ((size_t)C * (C + 32 / dense_lanes(C)) + 2 * (size_t)C);
+}
+
 template <class E>
 int viterbi_dense_typed(
     gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const E* emis, int64_t stride,
     const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores) {
-  int G = 1;
-  while (G < 32 && C * (G * 2) <= kDenseThreads) G *= 2;
-  const size_t smem = sizeof(float) * ((size_t)C * (C + 32 / G) + 2 * (size_t)C);
+  const int G = dense_lanes(C);
+  const size_t smem = dense_smem_bytes(C);
   if (smem > (size_t)kMaxDynamicSmem)
     return fail(ctx, GTNB_ERR_UNSUPPORTED,
                 "gtnb_viterbi_dense: the transitions tile does not fit shared memory (C <= 224)");
@@ -269,6 +280,10 @@ int viterbi_dense_typed(
 }
 
 } // namespace
+
+bool viterbi_dense_supported(int C) {
+  return C >= 1 && C <= 256 && dense_smem_bytes(C) <= (size_t)kMaxDynamicSmem;
+}
 
 int launch_viterbi_dense(
     gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const void* emis, int64_t stride,

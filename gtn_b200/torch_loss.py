@@ -652,6 +652,139 @@ def align_spans(tokens, S):
     return (torch.where(absent, -1, start[:, :S]).int(), torch.where(absent, -1, end[:, :S]).int())
 
 
+class TransitionGraph:
+    """A transition graph prepared once for transitions_decode: the tables of G (a gtn_b200.gtn.Graph, the structure of
+    sparse_viterbi's or, with backoff=True, backoff_viterbi's transitions_graph) packed and uploaded to `device` (the
+    current CUDA device by default) through gtnb_transitions_create, with the route for num_labels labels.
+    large_transitions: a G beyond one CTA takes the thread-block-cluster kernels, as in sparse_viterbi.  G's weights are
+    not kept: the learned transitions are passed to every transitions_decode call.
+
+    Creating one allocates and synchronises, so it raises while a stream is capturing: build it before capture.  A
+    captured CUDA graph that decodes with it reads its tables, and must not be replayed once it is gone: keep it alive
+    as long as the captured graph.  A G outside the device decoders' envelope raises a RuntimeError that names the
+    synchronous decoder to use instead."""
+
+    def __init__(self, graph, num_labels, device=None, backoff=False, large_transitions=False):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("TransitionGraph: create it before capturing a CUDA graph (it allocates and "
+                               "synchronises)")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.num_labels = int(num_labels)
+        self.backoff = bool(backoff)
+        view, keep = _graph_view(graph)
+        self.num_arcs = view.num_arcs
+        self._g = _async_ctx(self.device, "TransitionGraph")
+        h = C.c_void_p()
+        rc = _clustered(self._g, large_transitions, lambda: capi.lib().gtnb_transitions_create(
+            self._g.h, C.byref(view), self.num_labels, int(self.backoff), C.byref(h)))
+        del keep
+        if rc == capi.ERR_UNSUPPORTED:
+            raise RuntimeError("TransitionGraph: %s" % capi.lib().gtnb_last_error(self._g.h).decode())
+        self._g._check(rc)
+        self.h = h
+
+    def __del__(self):
+        h = getattr(self, "h", None)
+        if h is not None and h.value:
+            capi.lib().gtnb_transitions_destroy(self._g.h, h)
+            self.h = None
+
+
+def _decode_lengths(e, input_lengths):
+    """input_lengths as int32 on the emissions' device, without a copy between devices (None stays None)"""
+    if input_lengths is None:
+        return None
+    assert torch.is_tensor(input_lengths) and input_lengths.device == e.device and \
+        not input_lengths.is_floating_point(), "input_lengths must be None or an integer tensor on the emissions' device"
+    assert input_lengths.shape == (e.shape[0],)
+    return input_lengths.to(torch.int32).contiguous()
+
+
+@torch.no_grad()
+def transitions_decode(emissions, transitions, graph, input_lengths=None):
+    """Best path of intersect(E_b, G) for every utterance, G a prepared TransitionGraph, through
+    gtnb_viterbi_transitions_async on the current stream, without a host synchronisation (it may be captured in a
+    CUDA graph; the workspace comes from torch's allocator).
+
+    emissions: float32 CUDA tensor [B, T, C], C = graph.num_labels, on graph's device; transitions: float32 tensor of
+    graph.num_arcs elements on that device (G's arc numbering); input_lengths: None or a [B] integer tensor on that
+    device.  Returns device tensors (paths [B, T] int32, the label of every frame; scores [B] float32, viterbiScore;
+    arcs [B, T] int32, the emitting G arc of every frame; status [B] int32).  Status 0: sparse_viterbi's (or
+    backoff_viterbi's) result, bit for bit; 1: a NaN or +inf weight or used emission, 2: a length outside [0, T], both
+    with a NaN score and -1 rows; 3: a tie, the score exact and the path an optimal one (the synchronous decoder's
+    with the "exact_ties" flag off).  Rows are -1 beyond T_b and where no path accepts (score -inf).
+    collapse(paths, blank) turns the paths into transcripts.
+    """
+    assert isinstance(graph, TransitionGraph)
+    assert emissions.is_cuda and emissions.dim() == 3 and emissions.dtype == torch.float32, \
+        "emissions must be a float32 CUDA tensor [B, T, C]"
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    assert e.device == graph.device and Cn == graph.num_labels
+    assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+    assert transitions.numel() == graph.num_arcs
+    w = transitions.detach().contiguous() if transitions.numel() else torch.zeros(1, device=e.device)
+    il = _decode_lengths(e, input_lengths)
+    g = graph._g
+    lib = capi.lib()
+    nbytes = C.c_size_t()
+    g._check(lib.gtnb_viterbi_transitions_async_workspace(g.h, graph.h, B, T, C.byref(nbytes)))
+    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    arcs = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    scores = torch.empty(B, dtype=torch.float32, device=e.device)
+    status = torch.empty(B, dtype=torch.int32, device=e.device)
+    g._check(lib.gtnb_viterbi_transitions_async(
+        g.h, torch.cuda.current_stream(e.device).cuda_stream, graph.h, B, T, e.data_ptr(),
+        None if il is None else il.data_ptr(), w.data_ptr(), paths.data_ptr(), arcs.data_ptr(), scores.data_ptr(),
+        status.data_ptr(), ws.data_ptr(), nbytes.value))
+    return paths, scores, arcs, status
+
+
+@torch.no_grad()
+def _dense_decode(name, emissions, transitions, input_lengths, kind):
+    """gtnb_viterbi_dense_async on the current stream"""
+    assert emissions.is_cuda and emissions.dim() == 3
+    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+    assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+    w = transitions.detach().contiguous()
+    il = _decode_lengths(e, input_lengths)
+    dtype = _EMISSION_DTYPES[e.dtype]
+    g = _async_ctx(e.device, name)
+    lib = capi.lib()
+    nbytes = C.c_size_t()
+    g._check(lib.gtnb_viterbi_dense_async_workspace(g.h, B, T, Cn, dtype, kind, C.byref(nbytes)))
+    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    paths = torch.empty((B, T), dtype=torch.int32, device=e.device)
+    scores = torch.empty(B, dtype=torch.float32, device=e.device)
+    status = torch.empty(B, dtype=torch.int32, device=e.device)
+    g._check(lib.gtnb_viterbi_dense_async(
+        g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, e.data_ptr(), dtype,
+        None if il is None else il.data_ptr(), kind, w.data_ptr(), paths.data_ptr(), scores.data_ptr(),
+        status.data_ptr(), ws.data_ptr(), nbytes.value))
+    return paths, scores, status
+
+
+def asg_decode(emissions, transitions, input_lengths=None):
+    """asg_viterbi without a host synchronisation: gtnb_viterbi_dense_async on the current stream (it may be captured
+    in a CUDA graph).  emissions and transitions as in asg_viterbi; input_lengths: None or a [B] integer tensor on the
+    emissions' device.  Returns device tensors (paths [B, T] int32, scores [B] float32, status [B] int32): status 0 is
+    asg_viterbi's result, ties and NaN handling included; status 2 a length outside [0, T], with a NaN score and -1
+    rows."""
+    return _dense_decode("asg_decode", emissions, transitions, input_lengths, capi.DENSE_ASG)
+
+
+def ngram_ctc_decode(emissions, transitions, input_lengths=None):
+    """ngram_ctc_viterbi without a host synchronisation, as asg_decode is asg_viterbi's: (paths, scores, status) on
+    the current stream; collapse(paths, blank) gives the transcripts."""
+    return _dense_decode("ngram_ctc_decode", emissions, transitions, input_lengths, capi.DENSE_BIGRAM)
+
+
 def _graph_view(g):
     """capi view of a gtn_b200.gtn.Graph built on the host, in its own arc-list order"""
     from . import _gtn

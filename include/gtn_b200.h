@@ -1227,6 +1227,94 @@ int gtnb_backoff_transitions_viterbi(
     float* scores, /* [B] nullable: viterbiScore */
     int outputs_on_device);
 
+/*
+ * A transition graph prepared once for decoding without a host synchronisation (gtnb_viterbi_transitions_async): G's
+ * tables packed and uploaded into device memory the handle owns, with the route chosen for them.
+ * gtnb_transitions_create checks G as the synchronous decoder it stands for does: backoff 0 as gtnb_viterbi_sparse
+ * (epsilon arcs refused), backoff 1 as gtnb_viterbi_backoff (epsilon arcs allowed, a cycle of them refused; an
+ * epsilon-free G then takes gtnb_viterbi_sparse's tables).  The route is picked from ctx's flags at creation, as the
+ * synchronous decoders pick it per call: "sparse_cluster" (1, or a forced 2 / 4 / 8) lets a G beyond one CTA take a
+ * thread-block cluster.  A G outside every device route, or the "implicit" flag at 0, is GTNB_ERR_UNSUPPORTED: decode
+ * with gtnb_viterbi_sparse / gtnb_viterbi_backoff instead.  The handle records its device, C, G's arc count (the
+ * length of trans_w) and node count; it holds no weights, which stay a per-call argument since they are learned.
+ * create allocates, uploads and synchronises: it is a set-up call and may not be captured into a CUDA graph.  A
+ * captured graph that decodes with a handle must not be replayed after gtnb_transitions_destroy (which frees the
+ * tables; ctx must be a context of the handle's device).
+ */
+typedef struct gtnb_transitions gtnb_transitions;
+int gtnb_transitions_create(gtnb_ctx* ctx, const gtnb_graph_view* G, int C, int backoff, gtnb_transitions** out);
+void gtnb_transitions_destroy(gtnb_ctx* ctx, gtnb_transitions* G);
+
+/*
+ * Viterbi decoding with a prepared transition graph, without a host synchronisation: viterbiPath / viterbiScore of
+ * intersect(E_b, G), the decode of gtnb_viterbi_sparse (G made with backoff 0) or gtnb_viterbi_backoff (backoff 1).
+ * The contract is gtnb_ctc_loss_async's: the call enqueues kernel launches on cuda_stream (NULL: the CUDA default
+ * stream) and returns, without a host synchronisation, a read of device data on the host, an allocation or a staging
+ * copy; it may be captured into a CUDA graph.  Scratch memory is workspace_dev (256-byte aligned, at least
+ * gtnb_viterbi_transitions_async_workspace's bytes for the same handle and bounds; smaller is
+ * GTNB_ERR_INVALID_ARGUMENT).  It holds 16-bit back-pointers sized from the bounds: 2 * B * T * S bytes, or
+ * 2 * B * (T + 1) * S with epsilon arcs.  A handle made on another device is GTNB_ERR_INVALID_ARGUMENT.  Emissions
+ * are float32 only, as the synchronous decoders take them (dtype is not a parameter).
+ *
+ * emissions_dev [B][T][C] float32; input_lens_dev [B] (NULL: T each); trans_w_dev [G arcs] float32.  Outputs, written
+ * on the device:
+ *   paths_dev [B][T]            the label of every frame of the best path;
+ *   arcs_dev [B][T] (nullable)  the emitting G arc taken at every frame (an epsilon arc uses no frame);
+ *                               both -1 beyond T_b and wherever no path accepts;
+ *   scores_dev [B]              viterbiScore: -inf for T_b = 0 or no accepting path;
+ *   status_dev [B] (nullable)   0  the synchronous decoder's result on the same data, bit for bit (exact_ties on);
+ *                               1  a NaN or +inf weight or used emission (the synchronous decoder re-runs such an
+ *                                  utterance on its exact route): a NaN score and -1 rows;
+ *                               2  input_lens_dev[b] outside [0, T]: a NaN score and -1 rows;
+ *                               3  a tie on the path or between best accept states: the score is the synchronous
+ *                                  decoder's and the path an optimal one, the synchronous decoder's with exact_ties
+ *                                  off.
+ * A flagged utterance never affects the others.  A -inf weight only forbids its arc.
+ */
+int gtnb_viterbi_transitions_async_workspace(gtnb_ctx* ctx, const gtnb_transitions* G, int B, int T, size_t* bytes);
+int gtnb_viterbi_transitions_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    const gtnb_transitions* G,
+    int B,
+    int T,
+    const float* emissions_dev, /* [B][T][C] */
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    const float* trans_w_dev, /* [G arcs] */
+    int32_t* paths_dev, /* [B][T] */
+    int32_t* arcs_dev, /* [B][T] or NULL */
+    float* scores_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/*
+ * gtnb_viterbi_dense_typed without a host synchronisation, under gtnb_viterbi_transitions_async's contract: the
+ * factored dense-trellis decode of kind GTNB_DENSE_ASG / GTNB_DENSE_BIGRAM with device lengths.  Emissions of dtype
+ * GTNB_F32, GTNB_BF16 or GTNB_F16 are read in place.  paths_dev [B][T] (nullable: the paths then go to the workspace),
+ * scores_dev [B] (-inf for T_b = 0).  status_dev [B] (nullable): 0 the synchronous call's result, ties broken as the
+ * reference breaks them and NaN read as -inf, as there; 2 input_lens_dev[b] outside [0, T], with a NaN score and -1
+ * rows.  The kernel's bounds (C <= 224 for the transition tile) and an unknown dtype are GTNB_ERR_UNSUPPORTED, as in
+ * the other asynchronous calls; an unknown kind is GTNB_ERR_INVALID_ARGUMENT.
+ */
+int gtnb_viterbi_dense_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, size_t* bytes);
+int gtnb_viterbi_dense_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    int kind, /* GTNB_DENSE_ASG | GTNB_DENSE_BIGRAM */
+    const float* trans_w_dev, /* ASG [C + C*C], BIGRAM [C*C] */
+    int32_t* paths_dev, /* [B][T] or NULL */
+    float* scores_dev, /* [B] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif
