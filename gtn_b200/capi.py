@@ -181,6 +181,11 @@ SYMBOLS = [
      [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     ("gtnb_viterbi_dense_async", C.c_int,
      [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
+    ("gtnb_edit_distance_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_edit_distance_async", C.c_int,
+     [_vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+      C.c_size_t]),
 ]
 
 _lib = None

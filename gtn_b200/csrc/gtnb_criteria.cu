@@ -4017,3 +4017,61 @@ extern "C" int gtnb_viterbi_dense_async(
                                          scores_dev, status_dev},
                          true);
 }
+
+namespace {
+
+/* gtnb_edit_distance_async inside a BorrowedArena: the move words of the alignment (when asked for) taken from the
+ * arena and, when launch, the one kernel enqueued */
+int edit_async_run(gtnb_ctx* ctx, int B, const int32_t* hyp, int N, const int32_t* hyp_lens, const int32_t* ref,
+                   int M, const int32_t* ref_lens, int word_sep, int32_t* distance, int32_t* ops, int32_t* units,
+                   int32_t* status, int32_t* hyp_align, int32_t* ref_align, bool with_alignment, bool launch) {
+  uint32_t* moves = nullptr;
+  if (with_alignment) GTNB_TRY(dev_alloc(ctx, &moves, edit_distance_move_words(B, N, M, word_sep)));
+  if (!launch) return GTNB_OK;
+  return launch_edit_distance(ctx, B, hyp, N, hyp_lens, ref, M, ref_lens, word_sep, distance, ops, units, status,
+                              hyp_align, ref_align, moves);
+}
+
+/* k_edit.cu holds at most 4096 rows (8 warps of 32 lanes of 16 rows) and both sequences in shared memory */
+int edit_async_bounds(gtnb_ctx* ctx, const std::string& fn, int N, int M) {
+  if (N > 4096 || M > 4096)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": N and M are limited to 4096 units on the device");
+  return GTNB_OK;
+}
+
+} // namespace
+
+extern "C" int gtnb_edit_distance_async_workspace(gtnb_ctx* ctx, int B, int N, int M, int word_sep,
+                                                  int with_alignment, size_t* bytes) {
+  const std::string fn = "gtnb_edit_distance_async_workspace";
+  if (!ctx || B < 0 || N < 0 || M < 0 || !bytes) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  GTNB_TRY(edit_async_bounds(ctx, fn, N, M));
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  GTNB_TRY(edit_async_run(ctx, B, nullptr, N, nullptr, nullptr, M, nullptr, word_sep, nullptr, nullptr, nullptr,
+                          nullptr, nullptr, nullptr, with_alignment != 0, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+extern "C" int gtnb_edit_distance_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, const int32_t* hyp_dev, int N, const int32_t* hyp_lengths_dev,
+    const int32_t* ref_dev, int M, const int32_t* ref_lengths_dev, int word_sep, int32_t* distance_dev,
+    int32_t* ops_dev, int32_t* units_dev, int32_t* status_dev, int32_t* hyp_align_dev, int32_t* ref_align_dev,
+    void* workspace_dev, size_t workspace_bytes) {
+  const std::string fn = "gtnb_edit_distance_async";
+  if (!ctx || B < 0 || N < 0 || M < 0 ||
+      (B > 0 && (!hyp_lengths_dev || !ref_lengths_dev || (N > 0 && !hyp_dev) || (M > 0 && !ref_dev) ||
+                 !distance_dev || !ops_dev || !units_dev || !status_dev)) ||
+      ((uintptr_t)workspace_dev & 255))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  GTNB_TRY(edit_async_bounds(ctx, fn, N, M));
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_dev ? workspace_bytes : 0);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  return edit_async_run(ctx, B, hyp_dev, N, hyp_lengths_dev, ref_dev, M, ref_lengths_dev, word_sep, distance_dev,
+                        ops_dev, units_dev, status_dev, hyp_align_dev, ref_align_dev,
+                        hyp_align_dev || ref_align_dev, true);
+}

@@ -220,6 +220,13 @@ int launch_decode_async_prepare(gtnb_ctx* ctx, int B, int T, const int32_t* inpu
 int launch_decode_async_finalize(gtnb_ctx* ctx, int B, int T_out, const int32_t* lens, const int32_t* kstatus,
                                  const int32_t* valid, int32_t* paths, int32_t* arcs, float* scores,
                                  int32_t* status);
+/* gtnb_edit_distance_async (k_edit.cu): the 32-bit move words its alignment needs for B pairs at these bounds, and
+ * the one launch (moves NULL: no alignment; hyp_align / ref_align each nullable) */
+long long edit_distance_move_words(int B, int N, int M, int word_sep);
+int launch_edit_distance(gtnb_ctx* ctx, int B, const int32_t* hyp, int N, const int32_t* hyp_lens,
+                         const int32_t* ref, int M, const int32_t* ref_lens, int word_sep, int32_t* distance,
+                         int32_t* ops, int32_t* units, int32_t* status, int32_t* hyp_align, int32_t* ref_align,
+                         uint32_t* moves);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);

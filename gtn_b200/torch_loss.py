@@ -6,6 +6,7 @@ Here the [B, T, C] CUDA tensor goes straight into the C ABI (`gtnb_ctc_loss`, de
 device gradients out) on the tensor's own CUDA stream; only the B losses visit the host.
 """
 import ctypes as C
+from typing import NamedTuple, Optional
 
 import numpy as np
 import torch
@@ -783,6 +784,78 @@ def ngram_ctc_decode(emissions, transitions, input_lengths=None):
     """ngram_ctc_viterbi without a host synchronisation, as asg_decode is asg_viterbi's: (paths, scores, status) on
     the current stream; collapse(paths, blank) gives the transcripts."""
     return _dense_decode("ngram_ctc_decode", emissions, transitions, input_lengths, capi.DENSE_BIGRAM)
+
+
+class EditDistance(NamedTuple):
+    """edit_distance's results, device tensors of [B] int32 (alignments [B, N] / [B, M] int32, or None)"""
+    distance: torch.Tensor
+    substitutions: torch.Tensor
+    insertions: torch.Tensor
+    deletions: torch.Tensor
+    hyp_units: torch.Tensor
+    ref_units: torch.Tensor
+    status: torch.Tensor
+    hyp_align: Optional[torch.Tensor] = None
+    ref_align: Optional[torch.Tensor] = None
+
+
+def _edit_operand(name, x, dim, device):
+    assert torch.is_tensor(x) and x.is_cuda and x.dim() == dim and not x.is_floating_point() and \
+        not x.is_complex(), "%s must be an integer CUDA tensor of %d dimension(s)" % (name, dim)
+    assert device is None or x.device == device, "%s must be on the hypotheses' device" % name
+    return x.to(torch.int32).contiguous()
+
+
+@torch.no_grad()
+def edit_distance(hyp, hyp_lengths, ref, ref_lengths, word_sep=None, alignment=False):
+    """Levenshtein distance between every hypothesis hyp[b, :hyp_lengths[b]] and reference ref[b, :ref_lengths[b]],
+    through gtnb_edit_distance_async on the current stream, without a host synchronisation (it may be captured in a
+    CUDA graph; the workspace comes from torch's allocator).  collapse(paths, blank)'s output is taken as hyp,
+    hyp_lengths unchanged.
+
+    hyp [B, N] and ref [B, M]: integer CUDA tensors on one device; the lengths: [B] integer tensors on that device.
+    word_sep None: a unit is a token; an int: a unit is a word, a maximal run of tokens other than word_sep (no empty
+    words), two words being equal when their token spans are.  The distance is -viterbiScore(compose(x, compose(edits,
+    y))) of the reference's edit-distance example over the units, with unit costs.
+
+    Each cell of the recurrence picks one predecessor, preferring the diagonal (a match or a substitution), then a
+    deletion (a reference unit missing from the hypothesis), then an insertion (an extra hypothesis unit); the counts
+    and the alignment follow that chain of predecessors, an optimal path that need not be the reference's viterbiPath.
+
+    Returns an EditDistance of device tensors: distance, substitutions, insertions, deletions (summing to the
+    distance), hyp_units, ref_units and status, all [B] int32, and with alignment=True hyp_align [B, N] (the reference
+    unit each hypothesis unit is aligned to, -1 for an insertion) and ref_align [B, M] (the hypothesis unit, -1 for a
+    deletion), both -1 beyond the unit counts and counted in units (words in word mode).  Status 0 is a result;
+    status 2 a length outside [0, N] or [0, M], with -1 in every output of that pair.  An error rate (WER, or CER at
+    token level) is distance[ok].sum() / ref_units[ok].sum() with ok = status == 0.
+
+    N or M above 4096 raises RuntimeError.
+    """
+    h = _edit_operand("hyp", hyp, 2, None)
+    dev = hyp.device
+    r = _edit_operand("ref", ref, 2, dev)
+    hl = _edit_operand("hyp_lengths", hyp_lengths, 1, dev)
+    rl = _edit_operand("ref_lengths", ref_lengths, 1, dev)
+    B, N = h.shape
+    M = r.shape[1]
+    assert r.shape[0] == B and hl.shape == (B,) and rl.shape == (B,), "one hypothesis, reference and length per pair"
+    sep = -1 if word_sep is None else int(word_sep)
+    assert sep >= -1, "word_sep must be None or a non-negative token"
+    g = _async_ctx(dev, "edit_distance")
+    lib = capi.lib()
+    nbytes = C.c_size_t()
+    g._check(lib.gtnb_edit_distance_async_workspace(g.h, B, N, M, sep, int(bool(alignment)), C.byref(nbytes)))
+    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev) if nbytes.value else None
+    dist, status = (torch.empty(B, dtype=torch.int32, device=dev) for _ in range(2))
+    ops, units = torch.empty((B, 3), dtype=torch.int32, device=dev), torch.empty((B, 2), dtype=torch.int32, device=dev)
+    ha = torch.empty((B, N), dtype=torch.int32, device=dev) if alignment else None
+    ra = torch.empty((B, M), dtype=torch.int32, device=dev) if alignment else None
+    g._check(lib.gtnb_edit_distance_async(
+        g.h, torch.cuda.current_stream(dev).cuda_stream, B, h.data_ptr(), N, hl.data_ptr(), r.data_ptr(), M,
+        rl.data_ptr(), sep, dist.data_ptr(), ops.data_ptr(), units.data_ptr(), status.data_ptr(),
+        None if ha is None else ha.data_ptr(), None if ra is None else ra.data_ptr(),
+        None if ws is None else ws.data_ptr(), nbytes.value))
+    return EditDistance(dist, ops[:, 0], ops[:, 1], ops[:, 2], units[:, 0], units[:, 1], status, ha, ra)
 
 
 def _graph_view(g):

@@ -1315,6 +1315,55 @@ int gtnb_viterbi_dense_async(
     void* workspace_dev,
     size_t workspace_bytes);
 
+/*
+ * Batched Levenshtein distance between padded hypotheses and references, under gtnb_ctc_loss_async's contract: the
+ * call enqueues kernel launches on cuda_stream (NULL: the CUDA default stream) and nothing else -- no memset, no copy,
+ * no host wait -- so it may be captured into a CUDA graph.
+ * Pair b compares hyp_dev[b][0 .. hyp_lengths_dev[b]) ([B][N]) against ref_dev[b][0 .. ref_lengths_dev[b]) ([B][M]).
+ * word_sep < 0: a unit is a token.  word_sep >= 0: a unit is a word, a maximal run of tokens other than word_sep
+ * (leading, trailing and repeated separators make no empty word); two words are equal when their token spans are.
+ * The distance is the unit-cost edit distance, -viterbiScore(compose(x, compose(edits, y))) of the reference's
+ * examples/edit_distance.cpp over the units.  With i hypothesis units and j reference units,
+ *   D[i][j] = min(D[i-1][j-1] + (h_i != r_j), D[i-1][j] + 1 (an insertion), D[i][j-1] + 1 (a deletion)),
+ * and every cell picks one predecessor, preferring the diagonal, then a deletion, then an insertion.  The counts and
+ * the alignment are those of the chain of chosen predecessors from the last cell: an optimal path of the reference's
+ * lattice, not necessarily the one its viterbiPath returns.
+ * Outputs: distance_dev [B]; ops_dev [B][3] substitutions, insertions, deletions (summing to the distance);
+ * units_dev [B][2] hypothesis and reference units (the reference count is the error rate's denominator); status_dev
+ * [B] 0, or 2 for a length outside [0, N] or [0, M], which gets -1 in every scalar and -1 rows (other pairs are
+ * unaffected).  hyp_align_dev [B][N] (nullable): per hypothesis unit the index of the reference unit it is aligned
+ * to, -1 for an insertion; ref_align_dev [B][M] (nullable): per reference unit the hypothesis unit, -1 for a deletion;
+ * both -1 beyond the unit counts.  Indices count units: words in word mode.
+ * N, M <= 4096 (GTNB_ERR_UNSUPPORTED above).  Scratch memory is workspace_dev (256-byte aligned, at least
+ * gtnb_edit_distance_async_workspace's bytes for the same bounds; smaller is GTNB_ERR_INVALID_ARGUMENT).  Without an
+ * alignment pointer it is 0 bytes and workspace_dev may be NULL.  With one it holds the 2-bit move of every grid
+ * cell: with rows = min(n, m) and cols = max(n, m), where n = N and m = M in token mode and n = (N + 1) / 2 and
+ * m = (M + 1) / 2 in word mode, K the least of 1, 2, 4, 8, 16 with 32 K >= rows (else 16) and W = ceil(rows / 32K),
+ *   bytes = 256-byte roundup(4 * (B * W * (cols + 31) * 32 + 16)),
+ * which is B * 2 bits * 512 W * (cols + 31): about 2 bits per cell per pair at the bounds.  B = 0 is a no-op.
+ */
+int gtnb_edit_distance_async_workspace(gtnb_ctx* ctx, int B, int N, int M, int word_sep, int with_alignment,
+                                       size_t* bytes);
+int gtnb_edit_distance_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    const int32_t* hyp_dev, /* [B][N] */
+    int N,
+    const int32_t* hyp_lengths_dev, /* [B] */
+    const int32_t* ref_dev, /* [B][M] */
+    int M,
+    const int32_t* ref_lengths_dev, /* [B] */
+    int word_sep,
+    int32_t* distance_dev, /* [B] */
+    int32_t* ops_dev, /* [B][3]: substitutions, insertions, deletions */
+    int32_t* units_dev, /* [B][2]: hypothesis, reference */
+    int32_t* status_dev, /* [B] */
+    int32_t* hyp_align_dev, /* [B][N] or NULL */
+    int32_t* ref_align_dev, /* [B][M] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif
