@@ -20,6 +20,7 @@ ERR_UNSUPPORTED = 5
 EPSILON = -1
 DENSE_ASG = 0  # gtnb_viterbi_dense_ex graph kinds
 DENSE_BIGRAM = 1
+DENSE_CTC = 2  # gtnb_beam_decode_async: CTC without transitions
 F32 = 0  # element types of gtnb_ctc_loss_ex and the *_typed entry points
 BF16 = 1
 F16 = 2
@@ -183,6 +184,11 @@ SYMBOLS = [
      [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
     ("gtnb_edit_distance_async_workspace", C.c_int,
      [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_beam_decode_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_beam_decode_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp,
+      _vp, _vp, _vp, C.c_size_t]),
     ("gtnb_edit_distance_async", C.c_int,
      [_vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
       C.c_size_t]),

@@ -4075,3 +4075,85 @@ extern "C" int gtnb_edit_distance_async(
                         ops_dev, units_dev, status_dev, hyp_align_dev, ref_align_dev,
                         hyp_align_dev || ref_align_dev, true);
 }
+
+namespace {
+
+struct BeamAsyncArgs {
+  int B, T, C, dtype;
+  const void* emissions;
+  const int32_t* input_lens;
+  int kind;
+  const float* trans_w;
+  int blank, beam, nbest;
+  int32_t *tokens, *lengths;
+  float* scores;
+  int32_t* status;
+};
+
+/* the bounds k_beam.cu covers, and the kind-specific arguments */
+int beam_async_check(gtnb_ctx* ctx, const std::string& fn, const BeamAsyncArgs& a) {
+  if (a.kind != GTNB_DENSE_CTC && a.kind != GTNB_DENSE_BIGRAM && a.kind != GTNB_DENSE_ASG)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": unknown kind");
+  if (!known_dtype(a.dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
+  if (!beam_decode_supported(a.C, a.beam, a.nbest))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": needs 1 <= beam <= 64, 1 <= nbest <= beam and C <= 256");
+  if (a.kind != GTNB_DENSE_ASG && (a.blank < 0 || a.blank >= a.C))
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": blank outside [0, C)");
+  return GTNB_OK;
+}
+
+/* gtnb_beam_decode_async inside a BorrowedArena: the back-pointers and (with transitions) the transposed weights, the
+ * start weights and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued */
+int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch) {
+  uint16_t* bp = nullptr;
+  float *wt = nullptr, *wfirst = nullptr;
+  int32_t* wbad = nullptr;
+  GTNB_TRY(dev_alloc(ctx, &bp, (long long)a.B * std::max(a.T, 1) * a.beam));
+  if (a.kind != GTNB_DENSE_CTC) {
+    GTNB_TRY(dev_alloc(ctx, &wt, (long long)a.C * a.C));
+    GTNB_TRY(dev_alloc(ctx, &wfirst, a.C));
+    GTNB_TRY(dev_alloc(ctx, &wbad, a.C));
+  }
+  if (!launch) return GTNB_OK;
+  if (a.kind != GTNB_DENSE_CTC) GTNB_TRY(launch_beam_weights(ctx, a.C, a.kind, a.trans_w, wt, wfirst, wbad));
+  return launch_beam_decode(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
+                            a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
+                            a.tokens, a.lengths, a.scores, a.status);
+}
+
+} // namespace
+
+extern "C" int gtnb_beam_decode_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, int beam,
+                                                int nbest, size_t* bytes) {
+  const std::string fn = "gtnb_beam_decode_async_workspace";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !bytes) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  const BeamAsyncArgs a{B, T, C, dtype, nullptr, nullptr, kind, nullptr, 0, beam, nbest,
+                        nullptr, nullptr, nullptr, nullptr};
+  GTNB_TRY(beam_async_check(ctx, fn, a));
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  GTNB_TRY(beam_async_run(ctx, a, false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+extern "C" int gtnb_beam_decode_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, int kind, const float* trans_w_dev, int blank, int beam, int nbest,
+    int32_t* tokens_dev, int32_t* lengths_dev, float* scores_dev, int32_t* status_dev, void* workspace_dev,
+    size_t workspace_bytes) {
+  const std::string fn = "gtnb_beam_decode_async";
+  if (!ctx || B < 0 || T < 0 || C <= 0 ||
+      (B > 0 && ((T > 0 && !emissions_dev) || !tokens_dev || !lengths_dev || !scores_dev || !workspace_dev)) ||
+      ((uintptr_t)workspace_dev & 255) || (kind == GTNB_DENSE_CTC) != (trans_w_dev == nullptr))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  const BeamAsyncArgs a{B, T, C, dtype, emissions_dev, input_lens_dev, kind, trans_w_dev, blank, beam, nbest,
+                        tokens_dev, lengths_dev, scores_dev, status_dev};
+  GTNB_TRY(beam_async_check(ctx, fn, a));
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
+  return beam_async_run(ctx, a, true);
+}

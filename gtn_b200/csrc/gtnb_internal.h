@@ -228,6 +228,15 @@ int launch_edit_distance(gtnb_ctx* ctx, int B, const int32_t* hyp, int N, const 
                          int32_t* ops, int32_t* units, int32_t* status, int32_t* hyp_align, int32_t* ref_align,
                          uint32_t* moves);
 
+/* gtnb_beam_decode_async (k_beam.cu): the bounds it covers, the transposed transitions / start weights / row flags of
+ * a call, and the search (wt, wfirst, wbad unused for GTNB_DENSE_CTC) */
+bool beam_decode_supported(int C, int beam, int nbest);
+int launch_beam_weights(gtnb_ctx* ctx, int C, int kind, const float* trans_w, float* wt, float* wfirst, int32_t* wbad);
+int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
+                       const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
+                       int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
+                       int32_t* status);
+
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_sub(gtnb_ctx* ctx, const float* a, const float* b, float* out, int n);

@@ -786,6 +786,80 @@ def ngram_ctc_decode(emissions, transitions, input_lengths=None):
     return _dense_decode("ngram_ctc_decode", emissions, transitions, input_lengths, capi.DENSE_BIGRAM)
 
 
+class BeamDecode(NamedTuple):
+    """The beam decoders' results, device tensors: tokens [B, N, T] int32 (each transcript followed by -1), lengths
+    [B, N] int32, scores [B, N] float32 and status [B] int32"""
+    tokens: torch.Tensor
+    lengths: torch.Tensor
+    scores: torch.Tensor
+    status: torch.Tensor
+
+
+@torch.no_grad()
+def _beam_decode(name, emissions, transitions, input_lengths, kind, beam, nbest, blank):
+    """gtnb_beam_decode_async on the current stream"""
+    assert emissions.is_cuda and emissions.dim() == 3
+    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    w = None
+    if kind != capi.DENSE_CTC:
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+        w = transitions.detach().contiguous()
+    il = _decode_lengths(e, input_lengths)
+    dtype = _EMISSION_DTYPES[e.dtype]
+    g = _async_ctx(e.device, name)
+    lib = capi.lib()
+    nbytes = C.c_size_t()
+    g._check(lib.gtnb_beam_decode_async_workspace(g.h, B, T, Cn, dtype, kind, int(beam), int(nbest),
+                                                  C.byref(nbytes)))
+    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    tokens = torch.empty((B, nbest, T), dtype=torch.int32, device=e.device)
+    lengths = torch.empty((B, nbest), dtype=torch.int32, device=e.device)
+    scores = torch.empty((B, nbest), dtype=torch.float32, device=e.device)
+    status = torch.empty(B, dtype=torch.int32, device=e.device)
+    g._check(lib.gtnb_beam_decode_async(
+        g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, e.data_ptr(), dtype,
+        None if il is None else il.data_ptr(), kind, None if w is None else w.data_ptr(), int(blank), int(beam),
+        int(nbest), tokens.data_ptr(), lengths.data_ptr(), scores.data_ptr(), status.data_ptr(), ws.data_ptr(),
+        nbytes.value))
+    return BeamDecode(tokens, lengths, scores, status)
+
+
+def ctc_beam_decode(emissions, beam=16, nbest=1, input_lengths=None, blank=0):
+    """Prefix beam search over transcripts scored by ctc_loss's numerator, forwardScore(intersect(ctcGraph(y), E_b)),
+    through gtnb_beam_decode_async on the current stream, without a host synchronisation (it may be captured in a
+    CUDA graph; the workspace comes from torch's allocator).
+
+    emissions: [B, T, C] float32, bfloat16 or float16 CUDA tensor (read in place); input_lengths: None or a [B]
+    integer tensor on its device.  beam K in [1, 64] beams, nbest N in [1, K] hypotheses, C <= 256; beyond, a
+    RuntimeError.  Returns a BeamDecode of device tensors: tokens [B, N, T] (each transcript followed by -1), lengths
+    [B, N], scores [B, N] (the numerator over the alignments that survived the beam, a lower bound of ctc_loss's
+    numerator; -inf and length -1 for unused hypotheses) and status [B]: 0 a result, 1 a NaN or +inf emission, 2 a
+    length outside [0, T] (both with NaN scores and -1 rows), 3 a tie decided the beam or the N-best order (the
+    results stand, chosen by the tie rule of include/gtn_b200.h).  tokens[:, 0] and lengths[:, 0] go straight into
+    edit_distance.
+    """
+    return _beam_decode("ctc_beam_decode", emissions, None, input_lengths, capi.DENSE_CTC, beam, nbest, blank)
+
+
+def ngram_ctc_beam_decode(emissions, transitions, beam=16, nbest=1, input_lengths=None, blank=0):
+    """ctc_beam_decode scored by ngram_ctc_loss's numerator, forwardScore(intersect(intersect(ctc_y, G), E_b)), with
+    the learned bigram transitions [C*C] of ngram_ctc_loss (float32, on the emissions' device).  A NaN or +inf weight
+    flags every utterance with T_b >= 1 (status 1)."""
+    return _beam_decode("ngram_ctc_beam_decode", emissions, transitions, input_lengths, capi.DENSE_BIGRAM, beam,
+                        nbest, blank)
+
+
+def asg_beam_decode(emissions, transitions, beam=16, nbest=1, input_lengths=None):
+    """ctc_beam_decode scored by asg_loss's numerator, forwardScore(compose(compose(A_y, G), E_b)), with asg_loss's
+    transitions [C + C*C] (float32, on the emissions' device).  ASG has no blank: a frame stays on the last token or
+    appends any token, the last one included (a repeated token).  Staying and repeating score a frame alike, so such
+    ties are frequent and flagged with status 3."""
+    return _beam_decode("asg_beam_decode", emissions, transitions, input_lengths, capi.DENSE_ASG, beam, nbest, 0)
+
+
 class EditDistance(NamedTuple):
     """edit_distance's results, device tensors of [B] int32 (alignments [B, N] / [B, M] int32, or None)"""
     distance: torch.Tensor

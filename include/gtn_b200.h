@@ -810,6 +810,7 @@ int gtnb_viterbi_dense(
 /* graph kinds of gtnb_viterbi_dense_ex */
 #define GTNB_DENSE_ASG 0 /* trans_w [C + C*C]: start weights, then W; gtnb_asg_loss_ex's layout */
 #define GTNB_DENSE_BIGRAM 1 /* trans_w [C*C]: W alone, every state starts; gtnb_ngram_ctc_loss's layout */
+#define GTNB_DENSE_CTC 2 /* no transitions (trans_w NULL): gtnb_ctc_loss's criterion; gtnb_beam_decode_async only */
 
 /*
  * Batched Viterbi decoding with the learned transitions of gtnb_asg_loss_ex (kind GTNB_DENSE_ASG) or
@@ -1361,6 +1362,92 @@ int gtnb_edit_distance_async(
     int32_t* status_dev, /* [B] */
     int32_t* hyp_align_dev, /* [B][N] or NULL */
     int32_t* ref_align_dev, /* [B][M] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/*
+ * Batched prefix beam search over transcripts, scored by the training criterion, under gtnb_ctc_loss_async's contract:
+ * the call enqueues kernel launches on cuda_stream (NULL: the CUDA default stream) and nothing else -- no memset, no
+ * copy, no allocation, no host wait -- so it may be captured into a CUDA graph.
+ *
+ * Kinds and scores.  For utterance b with T_b = input_lens_dev[b] (NULL: T) frames of emissions_dev [B][T][C], the
+ * score of a transcript y (tokens in [0, C), no blanks) is the log-semiring numerator of the matching loss, the value
+ * its loss_b is denominator_b - numerator_b of:
+ *   GTNB_DENSE_CTC     forwardScore(intersect(ctcGraph(y), E_b)) of gtnb_ctc_loss (trans_w_dev NULL).  A beam
+ *                      carries p_blank and p_label, the two numerator states after the last frame; repeating the
+ *                      last token needs a blank in between; the empty prefix starts with weight 0.
+ *   GTNB_DENSE_BIGRAM  forwardScore(intersect(intersect(ctc_y, G), E_b)) of gtnb_ngram_ctc_loss, trans_w_dev [C*C] in
+ *                      its layout.  G's state is the previous frame's label, so every move weighs W[dst][src] with src
+ *                      blank or the last token, and the two states track G exactly.  Frame 0 enters label i from G's
+ *                      C start states with sigma_i = logsumexp_j W[i][j].
+ *   GTNB_DENSE_ASG     forwardScore(compose(compose(A_y, G), E_b)) of gtnb_asg_loss_ex, trans_w_dev [C + C*C] in its
+ *                      layout.  One state per prefix, whose last frame's label is the last token: a frame stays
+ *                      (W[last][last]) or appends any token c, c == last included, which makes a repeated token as
+ *                      A_y does (W[c][last]); frame 0 appends c with the start weight of c.  blank is unused.
+ * Every kind's accepting states weigh 0, so a transcript's end weight is 0.
+ *
+ * Search.  Frame-synchronous prefix beam search with K = beam beams.  At every frame the candidates are each beam
+ * kept (blank / repeat / stay) and each beam extended by each non-blank token (every token for ASG).  An extension
+ * whose transcript is already a live beam is merged into it (log-add), never kept twice: two live beams never hold
+ * the same transcript.  All C tokens are considered: no per-frame token pruning, no LM weight, no insertion bonus.
+ * Candidates are ranked by score descending; among equal scores kept beams come before extensions, then the lower
+ * previous slot wins, then the lower token.  A candidate of score -inf is not kept.  The N = nbest hypotheses are the
+ * top N live beams after frame T_b - 1, in the same order.  Scores are lower bounds: a returned score sums only the
+ * alignments that survived the beam, so score <= numerator(y), with equality when no prefix was ever pruned.
+ *
+ * Outputs, written on the device:
+ *   tokens_dev [B][N][T]   each hypothesis's transcript, followed by -1;
+ *   lengths_dev [B][N]     its length;
+ *   scores_dev [B][N]      its score (float32);
+ *   status_dev [B]         (nullable) 0 a result;
+ *                          1 a NaN or +inf in an emission of a row t < T_b, or (T_b >= 1, kinds with transitions)
+ *                            anywhere in trans_w_dev: NaN scores, -1 lengths and rows.  A -inf value only forbids its
+ *                            move;
+ *                          2 input_lens_dev[b] outside [0, T]: NaN scores, -1 lengths and rows;
+ *                          3 a tie decided the beam (equal scores at the K-th / (K+1)-th boundary of a frame) or the
+ *                            N-best order (equal scores between consecutive hypotheses, or the N-th and (N+1)-th
+ *                            beam): the results stand, chosen by the tie rule.
+ * Unused hypotheses (fewer live transcripts than N) get score -inf, length -1 and -1 rows.  T_b = 0 gives one
+ * hypothesis, the empty transcript with score 0 (the empty sum over no frames).  For CTC that is the numerator of
+ * the empty target in gtnb_ctc_loss, whose loss there is 0.  gtnb_ngram_ctc_loss and gtnb_asg_loss_ex give NaN at
+ * T_b = 0 instead (their linearGraph(0, C) accepts nothing): the decoder does not follow them.  A flagged utterance
+ * never affects the others.  Results do not vary from run to run.
+ *
+ * Bounds: 1 <= beam <= 64, 1 <= nbest <= beam, 1 <= C <= 256 for every kind; emissions of dtype GTNB_F32, GTNB_BF16
+ * or GTNB_F16 are read in place and widened on load.  Beyond them, or an unknown dtype: GTNB_ERR_UNSUPPORTED.  A NULL
+ * pointer where B > 0 needs one, trans_w_dev given for GTNB_DENSE_CTC or missing for the other kinds, an unknown kind
+ * or negative sizes: GTNB_ERR_INVALID_ARGUMENT.  blank outside [0, C) for CTC or BIGRAM: GTNB_ERR_UNSUPPORTED, as
+ * gtnb_ctc_align_async treats it.  B = 0 is a no-op.
+ *
+ * Scratch memory is workspace_dev (256-byte aligned, at least gtnb_beam_decode_async_workspace's bytes for the same
+ * bounds; smaller is GTNB_ERR_INVALID_ARGUMENT).  With r(x) = x rounded up to a multiple of 256,
+ *   bytes = r(2 * (B * max(T, 1) * beam + 16))                                  (16-bit back-pointers)
+ *         + (kind != GTNB_DENSE_CTC ? r(4 * (C*C + 16)) + 2 * r(4 * (C + 16)) : 0)   (transposed W, sigma, flags).
+ *
+ * Out of scope: beam search with a gtnb_transitions graph (sparse or backoff G: a prefix's state there is a
+ * distribution over G's nodes, not two numbers), LM shallow fusion, lexicons and word-level search, and per-frame
+ * token pruning.
+ */
+int gtnb_beam_decode_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, int beam, int nbest,
+                                     size_t* bytes);
+int gtnb_beam_decode_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    int kind, /* GTNB_DENSE_CTC | GTNB_DENSE_BIGRAM | GTNB_DENSE_ASG */
+    const float* trans_w_dev, /* NULL, BIGRAM [C*C], ASG [C + C*C] */
+    int blank,
+    int beam,
+    int nbest,
+    int32_t* tokens_dev, /* [B][nbest][T] */
+    int32_t* lengths_dev, /* [B][nbest] */
+    float* scores_dev, /* [B][nbest] */
+    int32_t* status_dev, /* [B] or NULL */
     void* workspace_dev,
     size_t workspace_bytes);
 
