@@ -306,6 +306,16 @@ struct HostGraph {
 };
 
 /*
+ * The numerator graph of CTC for U labels: 2U+1 nodes; arcs = self loops + step arcs + skip arcs
+ * (benchmarks/ctc.cpp:40-58), skip arcs exist where consecutive labels differ (`skips` of them).  all_valid: every
+ * label and the blank lie in [0, C).
+ */
+SgDims ctc_num_dims(int U, int skips, int all_valid) {
+  const int L = 2 * U + 1;
+  return SgDims{L, L + (L - 1) + skips, L >= 2 ? 2 : 1, all_valid, /*uniform=*/1, /*max_in=*/3, /*max_out=*/3};
+}
+
+/*
  * One attempt.  allow_implicit: sweep the frames without building the lattice (k_implicit.cu)
  * when the target graphs qualify; *needs_exact is set when that sweep met a non-finite weight,
  * in which case the outputs are not to be used and the caller repeats the call materialised.
@@ -327,16 +337,12 @@ int ctc_loss_run(
   PhaseClock pc;
   const long long per = (long long)T * C;
 
-  // host: only sizes.  Graph b has 2U+1 nodes; arcs = self loops + step arcs + skip arcs
-  // (benchmarks/ctc.cpp:40-58), skip arcs exist where consecutive labels differ.
+  // host: only sizes
   Targets t;
   GTNB_TRY(parse_targets(ctx, "gtnb_ctc_loss", B, T, C, input_lens, targets, target_lens, &t));
   std::vector<SgDims> dims(B);
-  for (int b = 0; b < B; b++) {
-    const int L = 2 * target_lens[b] + 1;
-    const int all_valid = blank >= 0 && blank < C && t.in_range[b];
-    dims[b] = SgDims{L, L + (L - 1) + t.skips[b], L >= 2 ? 2 : 1, all_valid, /*uniform=*/1, /*max_in=*/3, /*max_out=*/3};
-  }
+  for (int b = 0; b < B; b++)
+    dims[b] = ctc_num_dims(target_lens[b], t.skips[b], blank >= 0 && blank < C && t.in_range[b]);
   const long long tot_t = t.tot_t;
   const int maxT = t.maxT;
   pc.mark("sizes");
@@ -614,9 +620,9 @@ extern "C" int gtnb_ctc_loss_ex(
 namespace {
 
 /*
- * The context's arena pointed at a caller's block for one asynchronous call (gtnb_ctc_loss_async,
- * gtnb_ngram_ctc_loss_async, gtnb_asg_loss_async; base NULL: sizing only, nothing is launched).  dev_alloc fails once
- * the block is full instead of allocating; the context's own arena is back when the scope ends.
+ * The context's arena pointed at a caller's block for one asynchronous call (base NULL: sizing only, nothing is
+ * launched).  dev_alloc fails once the block is full instead of allocating; the context's own arena is back when the
+ * scope ends.
  */
 class BorrowedArena {
  public:
@@ -642,6 +648,40 @@ class BorrowedArena {
   size_t cap_;
 };
 
+/*
+ * Every asynchronous call is one run(bool launch) after its argument checks: the call's scratch taken from the arena
+ * and, when launch, its work enqueued.  async_workspace sizes it: the bytes run(false) takes from an unbounded arena,
+ * 0 for an empty batch.
+ */
+template <class Run>
+int async_workspace(gtnb_ctx* ctx, int B, size_t* bytes, Run&& run) {
+  *bytes = 0;
+  if (B == 0) return GTNB_OK;
+  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  GTNB_TRY(run(false));
+  *bytes = arena.need();
+  return GTNB_OK;
+}
+
+/*
+ * async_enqueue runs it on the caller's stream (NULL is the default stream, like any stream handle) with its scratch
+ * in the caller's workspace.  A non-NULL workspace must be 256-byte aligned; a NULL one has 0 bytes, so the first
+ * scratch a call takes from it fails with "workspace too small".
+ */
+template <class Run>
+int async_enqueue(gtnb_ctx* ctx, const std::string& fn, int B, void* cuda_stream, void* workspace, size_t bytes,
+                  Run&& run) {
+  if ((uintptr_t)workspace & 255) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": workspace not 256-byte aligned");
+  if (B == 0) return GTNB_OK;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  BorrowedArena arena(ctx, workspace, workspace ? bytes : 0);
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream));
+  return run(true);
+}
+
+/* an output buffer to a sizing run, which tests it for presence only */
+alignas(16) float stand_in[4];
+
 struct CtcAsyncArgs {
   int B, T, C, S, dtype;
   const void* emissions;
@@ -653,9 +693,8 @@ struct CtcAsyncArgs {
 };
 
 /*
- * gtnb_ctc_loss_async inside a BorrowedArena: the scratch of the call taken from the arena and, when launch, the
- * call enqueued.  The route is ctc_loss_run's for a batch at the bounds (every utterance U = S, T_b = T, S - 1 skip
- * arcs), decided from the bounds, the dtype, the buffers' alignment and the context's flags; the prepare kernel
+ * gtnb_ctc_loss_async's run.  The route is ctc_loss_run's for a batch at the bounds (every utterance U = S, T_b = T,
+ * S - 1 skip arcs), decided from the bounds, the dtype, the buffers' alignment and the context's flags; the prepare kernel
  * then writes every utterance's own descriptor over the bound-uniform slabs.  Sizing passes NULL buffers: a 16-bit
  * batch is then sized for the widened route, which needs more scratch than reading the buffers in place.
  */
@@ -666,8 +705,7 @@ int ctc_async_run(gtnb_ctx* ctx, const CtcAsyncArgs& a, bool launch) {
   if (!ctx->use_implicit)
     return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: the \"implicit\" flag is off (materialised route)");
   if (a.blank < 0 || a.blank >= C) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: blank outside [0, C)");
-  const int L = 2 * S + 1;
-  const std::vector<SgDims> dims(B, SgDims{L, L + (L - 1) + std::max(S - 1, 0), L >= 2 ? 2 : 1, 1, 1, 3, 3});
+  const std::vector<SgDims> dims(B, ctc_num_dims(S, std::max(S - 1, 0), /*all_valid=*/1));
   if (!implicit_dims_supported(dims.data(), B))
     return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: bounds outside the implicit sweeps");
   const std::vector<int32_t> Tv(B, T);
@@ -743,16 +781,9 @@ extern "C" int gtnb_ctc_loss_async_workspace(gtnb_ctx* ctx, int B, int T, int C,
   if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !bytes)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctc_loss_async_workspace: bad arguments");
   if (!ctc_async_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async_workspace: unknown dtype");
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  // (the sizing reads the grads pointer for its presence only)
-  alignas(16) static float stand_in[4];
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
   const CtcAsyncArgs a{B, T, C, S, dtype, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
                        with_grad ? stand_in : nullptr};
-  GTNB_TRY(ctc_async_run(ctx, a, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return ctc_async_run(ctx, a, launch); });
 }
 
 extern "C" int gtnb_ctc_loss_async(
@@ -760,16 +791,13 @@ extern "C" int gtnb_ctc_loss_async(
     const int32_t* input_lens_dev, const int32_t* targets_dev, const int32_t* target_lens_dev, int blank,
     float* losses_dev, int32_t* status_dev, void* grads_dev, void* workspace_dev, size_t workspace_bytes) {
   if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !emissions_dev || (S > 0 && !targets_dev) || !target_lens_dev ||
-      !losses_dev || (B > 0 && !workspace_dev) || ((uintptr_t)workspace_dev & 255))
+      !losses_dev)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ctc_loss_async: bad arguments");
   if (!ctc_async_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, "gtnb_ctc_loss_async: unknown dtype");
-  if (B == 0) return GTNB_OK;
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
   const CtcAsyncArgs a{B, T, C, S, dtype, emissions_dev, input_lens_dev, targets_dev, target_lens_dev, blank,
                        losses_dev, status_dev, grads_dev};
-  return ctc_async_run(ctx, a, true);
+  return async_enqueue(ctx, "gtnb_ctc_loss_async", B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return ctc_async_run(ctx, a, launch); });
 }
 
 namespace {
@@ -1470,6 +1498,15 @@ int asg_loss_generic(CallScope& scope, const TransitionArgs& a, const Targets& t
  */
 namespace {
 
+/* the folded numerator graph of n-gram CTC: the start node S + CTC's graph; arcs = CTC's + the two S arcs (one if
+ * U = 0) */
+SgDims ngram_num_dims(int U, int skips) {
+  SgDims d = ctc_num_dims(U, skips, /*all_valid=*/1);
+  d.A += std::min(d.N, 2);
+  d.N += 1;
+  return d;
+}
+
 /* gtnb_ngram_ctc_loss and gtnb_ngram_ctc_loss_typed: a.dtype's emissions on the native route, or widened */
 int ngram_ctc_loss_call(gtnb_ctx* ctx, const TransitionArgs& a) {
   const int B = a.B, T = a.T, C = a.C;
@@ -1486,10 +1523,7 @@ int ngram_ctc_loss_call(gtnb_ctx* ctx, const TransitionArgs& a) {
   std::vector<SgDims> dims(B);
   for (int b = 0; b < B; b++) {
     if (!t.in_range[b]) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_ngram_ctc_loss: label outside [0, C)");
-    // folded numerator graph: S + 2U+1 CTC nodes; arcs = self loops + steps + skips + the two S arcs (one if U = 0)
-    const int L = 2 * a.target_lens[b] + 1;
-    dims[b] = SgDims{L + 1, L + (L - 1) + t.skips[b] + std::min(L, 2), L >= 2 ? 2 : 1, /*all_valid=*/1,
-                     /*uniform=*/1, /*max_in=*/3, /*max_out=*/3};
+    dims[b] = ngram_num_dims(a.target_lens[b], t.skips[b]);
   }
   TrellisCriterion ngram{(long long)C * C, (long long)B * (T + 1) * C, /*fold=*/true, launch_ngram_den_forward,
                                launch_ngram_den_backward};
@@ -1551,6 +1585,11 @@ int asg_num_build(gtnb_ctx* ctx, gtnb_lattice* lat, const int32_t* targets_dev, 
  */
 namespace {
 
+/* the numerator graph of ASG, compose(fal_b, transitions): U+1 nodes, 2U arcs (none when U = 0), node U accepts */
+SgDims asg_num_dims(int U) {
+  return SgDims{U + 1, 2 * U, U > 0 ? 1 : 0, /*all_valid=*/1, /*uniform=*/1, /*max_in=*/2, /*max_out=*/2};
+}
+
 /* gtnb_asg_loss_ex and gtnb_asg_loss_typed: a.dtype's emissions on the native route, or widened */
 int asg_loss_ex_call(gtnb_ctx* ctx, const TransitionArgs& a) {
   const int B = a.B, T = a.T, C = a.C;
@@ -1562,9 +1601,7 @@ int asg_loss_ex_call(gtnb_ctx* ctx, const TransitionArgs& a) {
   std::vector<SgDims> dims(B);
   for (int b = 0; b < B; b++) {
     if (!t.in_range[b]) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_asg_loss_ex: label outside [0, C)");
-    // compose(fal_b, transitions): U+1 nodes, 2U arcs (none when U = 0), node U accepts
-    const int U = a.target_lens[b];
-    dims[b] = SgDims{U + 1, 2 * U, U > 0 ? 1 : 0, /*all_valid=*/1, /*uniform=*/1, /*max_in=*/2, /*max_out=*/2};
+    dims[b] = asg_num_dims(a.target_lens[b]);
   }
   TrellisCriterion asg{nTrans, asg_alpha_floats(B, T, C), /*fold=*/false, launch_asg_den_forward,
                              launch_asg_den_backward};
@@ -1626,14 +1663,13 @@ struct TrellisAsyncArgs {
 };
 
 /*
- * gtnb_ngram_ctc_loss_async / gtnb_asg_loss_async (asg) inside a BorrowedArena: the scratch of the call taken from the
- * arena and, when launch, the call enqueued.  The route is trellis_loss_fast's for a batch at the bounds (every
- * utterance U = S, T_b = T, and for n-gram S - 1 skip arcs): the numerator graphs built on the device from the padded
- * targets and swept by k_implicit.cu on the side stream, the dense trellis of k_ngram.cu on the call's stream.  Where
- * it differs: the prepare kernel writes the descriptors and [offsets | lens | T] the host would have staged; the gate
- * kernel, once both forward sweeps are done, keeps a flagged utterance out of the denominator's backward; the
- * numerator's arc gradients are scattered utterance by utterance, flagged ones left out; the losses and status are
- * formed on the device.  Sizing passes NULL buffers (want: trans_grad set) and takes the largest scratch.
+ * The run of gtnb_ngram_ctc_loss_async / gtnb_asg_loss_async (asg).  The route is trellis_loss_fast's for a batch at
+ * the bounds (every utterance U = S, T_b = T, and for n-gram S - 1 skip arcs): the numerator graphs built on the
+ * device from the padded targets and swept by k_implicit.cu on the side stream, the dense trellis of k_ngram.cu on the
+ * call's stream.  Where it differs: the prepare kernel writes the descriptors and [offsets | lens | T] the host would
+ * have staged; the gate kernel, once both forward sweeps are done, keeps a flagged utterance out of the denominator's
+ * backward; the numerator's arc gradients are scattered utterance by utterance, flagged ones left out; the losses and
+ * status are formed on the device.  Sizing passes NULL buffers (want: trans_grad set) and takes the largest scratch.
  */
 int trellis_async_run(gtnb_ctx* ctx, bool asg, const TrellisAsyncArgs& a, bool launch) {
   const char* fn = asg ? "gtnb_asg_loss_async" : "gtnb_ngram_ctc_loss_async";
@@ -1648,9 +1684,7 @@ int trellis_async_run(gtnb_ctx* ctx, bool asg, const TrellisAsyncArgs& a, bool l
     return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": the \"implicit\" flag is off (materialised route)");
   if (!asg && (a.blank < 0 || a.blank >= C))
     return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": blank outside [0, C)");
-  const int L = 2 * S + 1;
-  const SgDims bound = asg ? SgDims{S + 1, 2 * S, S > 0 ? 1 : 0, 1, 1, 2, 2}
-                           : SgDims{L + 1, L + (L - 1) + std::max(S - 1, 0) + std::min(L, 2), L >= 2 ? 2 : 1, 1, 1, 3, 3};
+  const SgDims bound = asg ? asg_num_dims(S) : ngram_num_dims(S, std::max(S - 1, 0));
   const std::vector<SgDims> dims(B, bound);
   if (!implicit_dims_supported(dims.data(), B))
     return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": bounds outside the implicit sweeps");
@@ -1755,37 +1789,25 @@ int trellis_async_workspace(gtnb_ctx* ctx, bool asg, int B, int T, int C, int S,
   if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !bytes)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
   if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": unknown dtype");
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  // (the sizing reads the trans_grad pointer for its presence only; grads NULL sizes the float32 scratch gradient)
-  alignas(16) static float stand_in[4];
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
+  // (grads NULL sizes the float32 scratch gradient)
   const TrellisAsyncArgs a{B, T, C, S, dtype, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr,
                            nullptr, with_grad ? stand_in : nullptr};
-  GTNB_TRY(trellis_async_run(ctx, asg, a, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return trellis_async_run(ctx, asg, a, launch); });
 }
 
 int trellis_async_call(gtnb_ctx* ctx, bool asg, void* cuda_stream, const TrellisAsyncArgs& a, void* workspace_dev,
                        size_t workspace_bytes) {
   const char* fn = asg ? "gtnb_asg_loss_async" : "gtnb_ngram_ctc_loss_async";
   if (!ctx || a.B < 0 || a.T < 0 || a.C <= 0 || a.S < 0 || !a.emissions || !a.trans_w ||
-      (a.S > 0 && !a.targets) || !a.target_lens || !a.losses || (a.B > 0 && !workspace_dev) ||
-      ((uintptr_t)workspace_dev & 255))
+      (a.S > 0 && !a.targets) || !a.target_lens || !a.losses)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
   if (!known_dtype(a.dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, std::string(fn) + ": unknown dtype");
-  if (a.B == 0) {
-    if (a.trans_grad) {
-      const long long n_trans = (asg ? a.C : 0) + (long long)a.C * a.C;
-      GTNB_CUDA(ctx, cudaMemsetAsync(a.trans_grad, 0, sizeof(float) * n_trans, static_cast<cudaStream_t>(cuda_stream)));
-    }
-    return GTNB_OK;
+  if (a.B == 0 && a.trans_grad) {
+    const long long n_trans = (asg ? a.C : 0) + (long long)a.C * a.C;
+    GTNB_CUDA(ctx, cudaMemsetAsync(a.trans_grad, 0, sizeof(float) * n_trans, static_cast<cudaStream_t>(cuda_stream)));
   }
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
-  return trellis_async_run(ctx, asg, a, true);
+  return async_enqueue(ctx, fn, a.B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return trellis_async_run(ctx, asg, a, launch); });
 }
 
 } // namespace
@@ -1854,9 +1876,9 @@ const char* align_async_name(AlignCriterion kind) {
 }
 
 /*
- * The call inside a BorrowedArena: the scratch taken from the arena and, when launch, the work enqueued.  Sized from
- * the bounds (every utterance U = S, T_b = T, CTC with S - 1 skips), as the losses' asynchronous calls are; sizing
- * passes NULL buffers and takes the arcs row of the token mapping whether or not tokens will be asked for.
+ * The run of the three.  Sized from the bounds (every utterance U = S, T_b = T, CTC with S - 1 skips), as the losses'
+ * asynchronous calls are; sizing passes NULL buffers and takes the arcs row of the token mapping whether or not tokens
+ * will be asked for.
  */
 int align_async_run(gtnb_ctx* ctx, AlignCriterion kind, const AlignAsyncArgs& a, bool launch) {
   const std::string fn = align_async_name(kind);
@@ -1867,12 +1889,10 @@ int align_async_run(gtnb_ctx* ctx, AlignCriterion kind, const AlignAsyncArgs& a,
     return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": the \"implicit\" flag is off (materialised route)");
   if (kind != AlignCriterion::Asg && (a.blank < 0 || a.blank >= C))
     return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": blank outside [0, C)");
-  const int L = 2 * S + 1;
   const int skips = std::max(S - 1, 0);
-  const SgDims bound = kind == AlignCriterion::Ctc ? SgDims{L, L + (L - 1) + skips, L >= 2 ? 2 : 1, 1, 1, 3, 3}
-                       : kind == AlignCriterion::Ngram
-                           ? SgDims{L + 1, L + (L - 1) + skips + std::min(L, 2), L >= 2 ? 2 : 1, 1, 1, 3, 3}
-                           : SgDims{S + 1, 2 * S, S > 0 ? 1 : 0, 1, 1, 2, 2};
+  const SgDims bound = kind == AlignCriterion::Ctc     ? ctc_num_dims(S, skips, /*all_valid=*/1)
+                       : kind == AlignCriterion::Ngram ? ngram_num_dims(S, skips)
+                                                       : asg_num_dims(S);
   const std::vector<SgDims> dims(B, bound);
   if (!implicit_dims_supported(dims.data(), B))
     return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": bounds outside the implicit sweeps (use the graph aligners)");
@@ -1929,30 +1949,21 @@ int align_async_workspace(gtnb_ctx* ctx, AlignCriterion kind, int B, int T, int 
   if (!ctx || B < 0 || T < 0 || C <= 0 || S < 0 || !bytes)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
   // (blank 0: sizing does not depend on it)
   const AlignAsyncArgs a{B, T, C, S, dtype, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
                          nullptr, nullptr, nullptr, nullptr};
-  GTNB_TRY(align_async_run(ctx, kind, a, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return align_async_run(ctx, kind, a, launch); });
 }
 
 int align_async_call(gtnb_ctx* ctx, AlignCriterion kind, void* cuda_stream, const AlignAsyncArgs& a,
                      void* workspace_dev, size_t workspace_bytes) {
   const std::string fn = align_async_name(kind);
   if (!ctx || a.B < 0 || a.T < 0 || a.C <= 0 || a.S < 0 || !a.emissions ||
-      (kind != AlignCriterion::Ctc && !a.trans_w) || (a.S > 0 && !a.targets) || !a.target_lens || !a.scores ||
-      (a.B > 0 && !workspace_dev) || ((uintptr_t)workspace_dev & 255))
+      (kind != AlignCriterion::Ctc && !a.trans_w) || (a.S > 0 && !a.targets) || !a.target_lens || !a.scores)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   if (!known_dtype(a.dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
-  if (a.B == 0) return GTNB_OK;
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
-  return align_async_run(ctx, kind, a, true);
+  return async_enqueue(ctx, fn, a.B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return align_async_run(ctx, kind, a, launch); });
 }
 
 } // namespace
@@ -3902,8 +3913,7 @@ struct DecodeAsyncArgs {
   int32_t* status;
 };
 
-/* gtnb_viterbi_transitions_async inside a BorrowedArena: the scratch taken from the arena and, when launch, the work
- * enqueued */
+/* gtnb_viterbi_transitions_async's run */
 int transitions_async_run(gtnb_ctx* ctx, const gtnb_transitions* G, const DecodeAsyncArgs& a, bool launch) {
   const int B = a.B, T = a.T, C = G->C, S = G->S;
   int32_t *lens = nullptr, *valid = nullptr, *kstatus = nullptr, *head = nullptr;
@@ -3926,7 +3936,7 @@ int transitions_async_run(gtnb_ctx* ctx, const gtnb_transitions* G, const Decode
   return launch_decode_async_finalize(ctx, B, T, lens, kstatus, valid, a.paths, a.arcs, a.scores, a.status);
 }
 
-/* gtnb_viterbi_dense_async inside a BorrowedArena; sizing takes the paths row whether or not paths will be given */
+/* gtnb_viterbi_dense_async's run; sizing takes the paths row whether or not paths will be given */
 int dense_async_run(gtnb_ctx* ctx, int C, bool bigram, const DecodeAsyncArgs& a, bool launch) {
   const int B = a.B, T = a.T;
   if (!viterbi_dense_supported(C))
@@ -3954,13 +3964,8 @@ extern "C" int gtnb_viterbi_transitions_async_workspace(gtnb_ctx* ctx, const gtn
   if (!ctx || !G || B < 0 || T < 0 || !bytes) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": bad arguments");
   if (G->device != ctx->device)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, std::string(fn) + ": the transition graph was made on another device");
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
   const DecodeAsyncArgs a{B, T, nullptr, GTNB_F32, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  GTNB_TRY(transitions_async_run(ctx, G, a, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return transitions_async_run(ctx, G, a, launch); });
 }
 
 extern "C" int gtnb_viterbi_transitions_async(
@@ -3968,19 +3973,14 @@ extern "C" int gtnb_viterbi_transitions_async(
     const int32_t* input_lens_dev, const float* trans_w_dev, int32_t* paths_dev, int32_t* arcs_dev, float* scores_dev,
     int32_t* status_dev, void* workspace_dev, size_t workspace_bytes) {
   const std::string fn = "gtnb_viterbi_transitions_async";
-  if (!ctx || !G || B < 0 || T < 0 || (B > 0 && (!emissions_dev || !trans_w_dev || !paths_dev || !scores_dev)) ||
-      (B > 0 && !workspace_dev) || ((uintptr_t)workspace_dev & 255))
+  if (!ctx || !G || B < 0 || T < 0 || (B > 0 && (!emissions_dev || !trans_w_dev || !paths_dev || !scores_dev)))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   if (G->device != ctx->device)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the transition graph was made on another device");
-  if (B == 0) return GTNB_OK;
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
-  return transitions_async_run(ctx, G,
-                               DecodeAsyncArgs{B, T, emissions_dev, GTNB_F32, input_lens_dev, trans_w_dev, paths_dev,
-                                               arcs_dev, scores_dev, status_dev},
-                               true);
+  const DecodeAsyncArgs a{B, T, emissions_dev, GTNB_F32, input_lens_dev, trans_w_dev, paths_dev, arcs_dev, scores_dev,
+                          status_dev};
+  return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return transitions_async_run(ctx, G, a, launch); });
 }
 
 extern "C" int gtnb_viterbi_dense_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind,
@@ -3989,13 +3989,9 @@ extern "C" int gtnb_viterbi_dense_async_workspace(gtnb_ctx* ctx, int B, int T, i
   if (!ctx || B < 0 || T < 0 || C <= 0 || !bytes || (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
   const DecodeAsyncArgs a{B, T, nullptr, dtype, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  GTNB_TRY(dense_async_run(ctx, C, kind == GTNB_DENSE_BIGRAM, a, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes,
+                         [&](bool launch) { return dense_async_run(ctx, C, kind == GTNB_DENSE_BIGRAM, a, launch); });
 }
 
 extern "C" int gtnb_viterbi_dense_async(
@@ -4004,24 +4000,19 @@ extern "C" int gtnb_viterbi_dense_async(
     int32_t* status_dev, void* workspace_dev, size_t workspace_bytes) {
   const std::string fn = "gtnb_viterbi_dense_async";
   if (!ctx || B < 0 || T < 0 || C <= 0 || (kind != GTNB_DENSE_ASG && kind != GTNB_DENSE_BIGRAM) ||
-      (B > 0 && (!emissions_dev || !trans_w_dev || !scores_dev || !workspace_dev)) ||
-      ((uintptr_t)workspace_dev & 255))
+      (B > 0 && (!emissions_dev || !trans_w_dev || !scores_dev)))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
-  if (B == 0) return GTNB_OK;
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
-  return dense_async_run(ctx, C, kind == GTNB_DENSE_BIGRAM,
-                         DecodeAsyncArgs{B, T, emissions_dev, dtype, input_lens_dev, trans_w_dev, paths_dev, nullptr,
-                                         scores_dev, status_dev},
-                         true);
+  const DecodeAsyncArgs a{B, T, emissions_dev, dtype, input_lens_dev, trans_w_dev, paths_dev, nullptr, scores_dev,
+                          status_dev};
+  return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return dense_async_run(ctx, C, kind == GTNB_DENSE_BIGRAM, a, launch); });
 }
 
 namespace {
 
-/* gtnb_edit_distance_async inside a BorrowedArena: the move words of the alignment (when asked for) taken from the
- * arena and, when launch, the one kernel enqueued */
+/* gtnb_edit_distance_async's run: the move words of the alignment (when asked for) taken from the arena and, when
+ * launch, the one kernel enqueued */
 int edit_async_run(gtnb_ctx* ctx, int B, const int32_t* hyp, int N, const int32_t* hyp_lens, const int32_t* ref,
                    int M, const int32_t* ref_lens, int word_sep, int32_t* distance, int32_t* ops, int32_t* units,
                    int32_t* status, int32_t* hyp_align, int32_t* ref_align, bool with_alignment, bool launch) {
@@ -4046,13 +4037,10 @@ extern "C" int gtnb_edit_distance_async_workspace(gtnb_ctx* ctx, int B, int N, i
   const std::string fn = "gtnb_edit_distance_async_workspace";
   if (!ctx || B < 0 || N < 0 || M < 0 || !bytes) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   GTNB_TRY(edit_async_bounds(ctx, fn, N, M));
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
-  GTNB_TRY(edit_async_run(ctx, B, nullptr, N, nullptr, nullptr, M, nullptr, word_sep, nullptr, nullptr, nullptr,
-                          nullptr, nullptr, nullptr, with_alignment != 0, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes, [&](bool launch) {
+    return edit_async_run(ctx, B, nullptr, N, nullptr, nullptr, M, nullptr, word_sep, nullptr, nullptr, nullptr,
+                          nullptr, nullptr, nullptr, with_alignment != 0, launch);
+  });
 }
 
 extern "C" int gtnb_edit_distance_async(
@@ -4063,17 +4051,14 @@ extern "C" int gtnb_edit_distance_async(
   const std::string fn = "gtnb_edit_distance_async";
   if (!ctx || B < 0 || N < 0 || M < 0 ||
       (B > 0 && (!hyp_lengths_dev || !ref_lengths_dev || (N > 0 && !hyp_dev) || (M > 0 && !ref_dev) ||
-                 !distance_dev || !ops_dev || !units_dev || !status_dev)) ||
-      ((uintptr_t)workspace_dev & 255))
+                 !distance_dev || !ops_dev || !units_dev || !status_dev)))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   GTNB_TRY(edit_async_bounds(ctx, fn, N, M));
-  if (B == 0) return GTNB_OK;
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_dev ? workspace_bytes : 0);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
-  return edit_async_run(ctx, B, hyp_dev, N, hyp_lengths_dev, ref_dev, M, ref_lengths_dev, word_sep, distance_dev,
-                        ops_dev, units_dev, status_dev, hyp_align_dev, ref_align_dev,
-                        hyp_align_dev || ref_align_dev, true);
+  return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes, [&](bool launch) {
+    return edit_async_run(ctx, B, hyp_dev, N, hyp_lengths_dev, ref_dev, M, ref_lengths_dev, word_sep, distance_dev,
+                          ops_dev, units_dev, status_dev, hyp_align_dev, ref_align_dev,
+                          hyp_align_dev || ref_align_dev, launch);
+  });
 }
 
 namespace {
@@ -4102,8 +4087,8 @@ int beam_async_check(gtnb_ctx* ctx, const std::string& fn, const BeamAsyncArgs& 
   return GTNB_OK;
 }
 
-/* gtnb_beam_decode_async inside a BorrowedArena: the back-pointers and (with transitions) the transposed weights, the
- * start weights and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued */
+/* gtnb_beam_decode_async's run: the back-pointers and (with transitions) the transposed weights, the start weights
+ * and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued */
 int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch) {
   uint16_t* bp = nullptr;
   float *wt = nullptr, *wfirst = nullptr;
@@ -4130,12 +4115,7 @@ extern "C" int gtnb_beam_decode_async_workspace(gtnb_ctx* ctx, int B, int T, int
   const BeamAsyncArgs a{B, T, C, dtype, nullptr, nullptr, kind, nullptr, 0, beam, nbest,
                         nullptr, nullptr, nullptr, nullptr};
   GTNB_TRY(beam_async_check(ctx, fn, a));
-  *bytes = 0;
-  if (B == 0) return GTNB_OK;
-  BorrowedArena arena(ctx, nullptr, std::numeric_limits<size_t>::max());
-  GTNB_TRY(beam_async_run(ctx, a, false));
-  *bytes = arena.need();
-  return GTNB_OK;
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return beam_async_run(ctx, a, launch); });
 }
 
 extern "C" int gtnb_beam_decode_async(
@@ -4145,15 +4125,12 @@ extern "C" int gtnb_beam_decode_async(
     size_t workspace_bytes) {
   const std::string fn = "gtnb_beam_decode_async";
   if (!ctx || B < 0 || T < 0 || C <= 0 ||
-      (B > 0 && ((T > 0 && !emissions_dev) || !tokens_dev || !lengths_dev || !scores_dev || !workspace_dev)) ||
-      ((uintptr_t)workspace_dev & 255) || (kind == GTNB_DENSE_CTC) != (trans_w_dev == nullptr))
+      (B > 0 && ((T > 0 && !emissions_dev) || !tokens_dev || !lengths_dev || !scores_dev)) ||
+      (kind == GTNB_DENSE_CTC) != (trans_w_dev == nullptr))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
   const BeamAsyncArgs a{B, T, C, dtype, emissions_dev, input_lens_dev, kind, trans_w_dev, blank, beam, nbest,
                         tokens_dev, lengths_dev, scores_dev, status_dev};
   GTNB_TRY(beam_async_check(ctx, fn, a));
-  if (B == 0) return GTNB_OK;
-  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  BorrowedArena arena(ctx, workspace_dev, workspace_bytes);
-  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream)); // (NULL is the default stream, like any stream handle)
-  return beam_async_run(ctx, a, true);
+  return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return beam_async_run(ctx, a, launch); });
 }

@@ -149,6 +149,31 @@ def _async_ctx(device, name="ctc_loss"):
     return g
 
 
+def _workspace(g, device, sizing, *args):
+    """The workspace of an asynchronous call: sizing (the call's *_async_workspace) asked for the bytes these
+    arguments need, taken from torch's allocator on device (under capture, from the graph's pool) -> (uint8 tensor,
+    bytes).  A call that needs none gets an empty tensor, whose data_ptr() is NULL.  A nonzero code raises."""
+    nbytes = C.c_size_t()
+    g._check(sizing(g.h, *args, C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=device), nbytes.value
+
+
+def _host_targets(ctx, err, name, routes, reduction, targets, target_lengths, forward):
+    """A loss on tensor targets whose sizing query raised err: for GTNB_ERR_UNSUPPORTED (bounds outside the
+    asynchronous routes) the list-target call forward(lists) with reduction "none" on the targets copied to the host
+    -- a documented synchronisation -- and a RuntimeError under capture; any other error raised as it is."""
+    if err.code != capi.ERR_UNSUPPORTED:
+        raise err
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("%s: these bounds are outside the asynchronous %s (%s) and cannot be captured"
+                           % (name, routes, err)) from None
+    rows = targets.cpu().tolist()
+    lens = target_lengths.cpu().tolist()
+    out = forward([r[:n] for r, n in zip(rows, lens)])
+    ctx.reduction = reduction
+    return out.mean() if reduction == "mean" else out
+
+
 class CTCLossAsyncFunction(torch.autograd.Function):
     """ctc_loss on tensor targets: gtnb_ctc_loss_async on the current stream, with no host synchronisation in forward
     or backward, so that the step can be captured in a CUDA graph.
@@ -171,26 +196,17 @@ class CTCLossAsyncFunction(torch.autograd.Function):
         il = None if input_lengths is None else input_lengths.to(torch.int32).contiguous()
         dtype = _CTC_DTYPES[e.dtype]
         g = _async_ctx(e.device)
-        nbytes = C.c_size_t()
-        rc = capi.lib().gtnb_ctc_loss_async_workspace(g.h, B, T, Cn, S, dtype, 1, C.byref(nbytes))
-        if rc == capi.ERR_UNSUPPORTED:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("ctc_loss: these bounds are outside the asynchronous routes (%s) and cannot be "
-                                   "captured" % capi.lib().gtnb_last_error(g.h).decode())
-            # the synchronous call on host targets: this synchronises
-            rows = tg.cpu().tolist()
-            lens = tl.cpu().tolist()
-            out = CTCLossFunction.forward(ctx, e, [r[:n] for r, n in zip(rows, lens)], blank, "none", input_lengths)
-            ctx.reduction = reduction
-            return out.mean() if reduction == "mean" else out
-        g._check(rc)
-        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+        try:
+            ws, nbytes = _workspace(g, e.device, capi.lib().gtnb_ctc_loss_async_workspace, B, T, Cn, S, dtype, 1)
+        except capi.GtnbError as err:
+            return _host_targets(ctx, err, "ctc_loss", "routes", reduction, tg, tl,
+                                 lambda lists: CTCLossFunction.forward(ctx, e, lists, blank, "none", input_lengths))
         losses = torch.empty(B, dtype=torch.float32, device=e.device)
         grad = torch.empty_like(e)
         g._check(capi.lib().gtnb_ctc_loss_async(
             g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, S, e.data_ptr(), dtype,
             None if il is None else il.data_ptr(), tg.data_ptr(), tl.data_ptr(), int(blank), losses.data_ptr(), None,
-            grad.data_ptr(), ws.data_ptr(), nbytes.value))
+            grad.data_ptr(), ws.data_ptr(), nbytes))
         ctx.save_for_backward(grad)
         ctx.reduction = reduction
         ctx.B = B
@@ -343,26 +359,14 @@ class TrellisLossAsyncFunction(torch.autograd.Function):
         dtype = _EMISSION_DTYPES[e.dtype]
         g = _async_ctx(e.device, name)
         lib = capi.lib()
-        nbytes = C.c_size_t()
         call = lib.gtnb_asg_loss_async if asg else lib.gtnb_ngram_ctc_loss_async
         sizing = lib.gtnb_asg_loss_async_workspace if asg else lib.gtnb_ngram_ctc_loss_async_workspace
-        rc = sizing(g.h, B, T, Cn, S, dtype, 1, C.byref(nbytes))
-        if rc == capi.ERR_UNSUPPORTED:
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("%s: these bounds are outside the asynchronous route (%s) and cannot be captured"
-                                   % (name, lib.gtnb_last_error(g.h).decode()))
-            # the synchronous call on host targets: this synchronises
-            rows = tgt.cpu().tolist()
-            lens = tl.cpu().tolist()
-            lists = [r[:n] for r, n in zip(rows, lens)]
-            if asg:
-                out = ASGLossFunction.forward(ctx, e, transitions, lists, "none", allreduce, input_lengths)
-            else:
-                out = NgramCTCLossFunction.forward(ctx, e, transitions, lists, input_lengths, blank, "none", allreduce)
-            ctx.reduction = reduction
-            return out.mean() if reduction == "mean" else out
-        g._check(rc)
-        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+        try:
+            ws, nbytes = _workspace(g, e.device, sizing, B, T, Cn, S, dtype, 1)
+        except capi.GtnbError as err:
+            return _host_targets(ctx, err, name, "route", reduction, tgt, tl, lambda lists: (
+                ASGLossFunction.forward(ctx, e, transitions, lists, "none", allreduce, input_lengths) if asg else
+                NgramCTCLossFunction.forward(ctx, e, transitions, lists, input_lengths, blank, "none", allreduce)))
         losses = torch.empty(B, dtype=torch.float32, device=e.device)
         grad = torch.empty_like(e)
         tg = torch.empty(transitions.numel(), dtype=torch.float32, device=e.device)
@@ -370,10 +374,10 @@ class TrellisLossAsyncFunction(torch.autograd.Function):
         il_p = None if il is None else il.data_ptr()
         if asg:
             rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, w.data_ptr(), tgt.data_ptr(), tl.data_ptr(),
-                      losses.data_ptr(), None, grad.data_ptr(), tg.data_ptr(), ws.data_ptr(), nbytes.value)
+                      losses.data_ptr(), None, grad.data_ptr(), tg.data_ptr(), ws.data_ptr(), nbytes)
         else:
             rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, w.data_ptr(), tgt.data_ptr(), tl.data_ptr(),
-                      int(blank), losses.data_ptr(), None, grad.data_ptr(), tg.data_ptr(), ws.data_ptr(), nbytes.value)
+                      int(blank), losses.data_ptr(), None, grad.data_ptr(), tg.data_ptr(), ws.data_ptr(), nbytes)
         g._check(rc)
         tg = tg.view_as(transitions)
         _allreduce_transitions(ctx, tg, allreduce)
@@ -570,21 +574,21 @@ def _align_async(name, emissions, transitions, targets, target_lengths, input_le
     call, sizing = {"ctc": (lib.gtnb_ctc_align_async, lib.gtnb_ctc_align_async_workspace),
                     "ngram": (lib.gtnb_ngram_ctc_align_async, lib.gtnb_ngram_ctc_align_async_workspace),
                     "asg": (lib.gtnb_asg_align_async, lib.gtnb_asg_align_async_workspace)}[kind]
-    nbytes = C.c_size_t()
-    rc = sizing(g.h, B, T, Cn, S, dtype, C.byref(nbytes))
-    if rc == capi.ERR_UNSUPPORTED:
+    try:
+        ws, nbytes = _workspace(g, e.device, sizing, B, T, Cn, S, dtype)
+    except capi.GtnbError as err:
+        if err.code != capi.ERR_UNSUPPORTED:
+            raise
         other = "graph_viterbi" if kind == "ctc" else "graph_transitions_viterbi"
         raise RuntimeError("%s: these bounds are outside the device alignment (%s); align on the host-built graphs "
-                           "with %s instead" % (name, lib.gtnb_last_error(g.h).decode(), other))
-    g._check(rc)
-    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+                           "with %s instead" % (name, err, other)) from None
     paths = torch.empty((B, T), dtype=torch.int32, device=e.device)
     tokens = torch.empty((B, T), dtype=torch.int32, device=e.device)
     scores = torch.empty(B, dtype=torch.float32, device=e.device)
     status = torch.empty(B, dtype=torch.int32, device=e.device)
     stream = torch.cuda.current_stream(e.device).cuda_stream
     il_p = None if il is None else il.data_ptr()
-    outs = (paths.data_ptr(), tokens.data_ptr(), scores.data_ptr(), status.data_ptr(), ws.data_ptr(), nbytes.value)
+    outs = (paths.data_ptr(), tokens.data_ptr(), scores.data_ptr(), status.data_ptr(), ws.data_ptr(), nbytes)
     if kind == "ctc":
         rc = call(g.h, stream, B, T, Cn, S, e.data_ptr(), dtype, il_p, tgt.data_ptr(), tl.data_ptr(), int(blank), *outs)
     elif kind == "ngram":
@@ -730,9 +734,7 @@ def transitions_decode(emissions, transitions, graph, input_lengths=None):
     il = _decode_lengths(e, input_lengths)
     g = graph._g
     lib = capi.lib()
-    nbytes = C.c_size_t()
-    g._check(lib.gtnb_viterbi_transitions_async_workspace(g.h, graph.h, B, T, C.byref(nbytes)))
-    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    ws, nbytes = _workspace(g, e.device, lib.gtnb_viterbi_transitions_async_workspace, graph.h, B, T)
     paths = torch.empty((B, T), dtype=torch.int32, device=e.device)
     arcs = torch.empty((B, T), dtype=torch.int32, device=e.device)
     scores = torch.empty(B, dtype=torch.float32, device=e.device)
@@ -740,7 +742,7 @@ def transitions_decode(emissions, transitions, graph, input_lengths=None):
     g._check(lib.gtnb_viterbi_transitions_async(
         g.h, torch.cuda.current_stream(e.device).cuda_stream, graph.h, B, T, e.data_ptr(),
         None if il is None else il.data_ptr(), w.data_ptr(), paths.data_ptr(), arcs.data_ptr(), scores.data_ptr(),
-        status.data_ptr(), ws.data_ptr(), nbytes.value))
+        status.data_ptr(), ws.data_ptr(), nbytes))
     return paths, scores, arcs, status
 
 
@@ -758,16 +760,14 @@ def _dense_decode(name, emissions, transitions, input_lengths, kind):
     dtype = _EMISSION_DTYPES[e.dtype]
     g = _async_ctx(e.device, name)
     lib = capi.lib()
-    nbytes = C.c_size_t()
-    g._check(lib.gtnb_viterbi_dense_async_workspace(g.h, B, T, Cn, dtype, kind, C.byref(nbytes)))
-    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    ws, nbytes = _workspace(g, e.device, lib.gtnb_viterbi_dense_async_workspace, B, T, Cn, dtype, kind)
     paths = torch.empty((B, T), dtype=torch.int32, device=e.device)
     scores = torch.empty(B, dtype=torch.float32, device=e.device)
     status = torch.empty(B, dtype=torch.int32, device=e.device)
     g._check(lib.gtnb_viterbi_dense_async(
         g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, e.data_ptr(), dtype,
         None if il is None else il.data_ptr(), kind, w.data_ptr(), paths.data_ptr(), scores.data_ptr(),
-        status.data_ptr(), ws.data_ptr(), nbytes.value))
+        status.data_ptr(), ws.data_ptr(), nbytes))
     return paths, scores, status
 
 
@@ -811,10 +811,8 @@ def _beam_decode(name, emissions, transitions, input_lengths, kind, beam, nbest,
     dtype = _EMISSION_DTYPES[e.dtype]
     g = _async_ctx(e.device, name)
     lib = capi.lib()
-    nbytes = C.c_size_t()
-    g._check(lib.gtnb_beam_decode_async_workspace(g.h, B, T, Cn, dtype, kind, int(beam), int(nbest),
-                                                  C.byref(nbytes)))
-    ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=e.device)
+    ws, nbytes = _workspace(g, e.device, lib.gtnb_beam_decode_async_workspace, B, T, Cn, dtype, kind, int(beam),
+                            int(nbest))
     tokens = torch.empty((B, nbest, T), dtype=torch.int32, device=e.device)
     lengths = torch.empty((B, nbest), dtype=torch.int32, device=e.device)
     scores = torch.empty((B, nbest), dtype=torch.float32, device=e.device)
@@ -822,8 +820,7 @@ def _beam_decode(name, emissions, transitions, input_lengths, kind, beam, nbest,
     g._check(lib.gtnb_beam_decode_async(
         g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, e.data_ptr(), dtype,
         None if il is None else il.data_ptr(), kind, None if w is None else w.data_ptr(), int(blank), int(beam),
-        int(nbest), tokens.data_ptr(), lengths.data_ptr(), scores.data_ptr(), status.data_ptr(), ws.data_ptr(),
-        nbytes.value))
+        int(nbest), tokens.data_ptr(), lengths.data_ptr(), scores.data_ptr(), status.data_ptr(), ws.data_ptr(), nbytes))
     return BeamDecode(tokens, lengths, scores, status)
 
 
@@ -917,9 +914,7 @@ def edit_distance(hyp, hyp_lengths, ref, ref_lengths, word_sep=None, alignment=F
     assert sep >= -1, "word_sep must be None or a non-negative token"
     g = _async_ctx(dev, "edit_distance")
     lib = capi.lib()
-    nbytes = C.c_size_t()
-    g._check(lib.gtnb_edit_distance_async_workspace(g.h, B, N, M, sep, int(bool(alignment)), C.byref(nbytes)))
-    ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev) if nbytes.value else None
+    ws, nbytes = _workspace(g, dev, lib.gtnb_edit_distance_async_workspace, B, N, M, sep, int(bool(alignment)))
     dist, status = (torch.empty(B, dtype=torch.int32, device=dev) for _ in range(2))
     ops, units = torch.empty((B, 3), dtype=torch.int32, device=dev), torch.empty((B, 2), dtype=torch.int32, device=dev)
     ha = torch.empty((B, N), dtype=torch.int32, device=dev) if alignment else None
@@ -928,7 +923,7 @@ def edit_distance(hyp, hyp_lengths, ref, ref_lengths, word_sep=None, alignment=F
         g.h, torch.cuda.current_stream(dev).cuda_stream, B, h.data_ptr(), N, hl.data_ptr(), r.data_ptr(), M,
         rl.data_ptr(), sep, dist.data_ptr(), ops.data_ptr(), units.data_ptr(), status.data_ptr(),
         None if ha is None else ha.data_ptr(), None if ra is None else ra.data_ptr(),
-        None if ws is None else ws.data_ptr(), nbytes.value))
+        ws.data_ptr(), nbytes))
     return EditDistance(dist, ops[:, 0], ops[:, 1], ops[:, 2], units[:, 0], units[:, 1], status, ha, ra)
 
 
