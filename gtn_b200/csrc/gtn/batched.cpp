@@ -14,6 +14,7 @@
  *                                      gtnb_compose_linear builds the B lattices
  *   forwardScore / viterbiScore (list) the B entries of such a lattice, each once: ONE gtnb_forward;
  *                                      or B linear graphs (the CTC normaliser): ONE gtnb_linear_forward
+ *   viterbiPath (list)                 the B entries of such a lattice, each once: ONE gtnb_viterbi_path
  *   backward (list)                    the entries' gradFuncs only RECORD their seeds (detail::BatchState);
  *                                      the first read of a resulting gradient runs gtnb_backward +
  *                                      gtnb_compose_grad (or the normaliser's gradient pass) once for the
@@ -125,8 +126,19 @@ void readBack(const std::shared_ptr<Context>& c, int slot, const void* owner, co
   }
 }
 
+/* the B entries' arc gradients, as the lattice holds them now, into bs.arcGrads; na: the entries' arc counts
+ * (h->sizes(), read before the caller took bs.m and c->lock) */
+void copyArcGrads(const std::shared_ptr<LatticeHandle>& h, const std::vector<int32_t>& na, BatchState& bs) {
+  auto& c = h->owner;
+  bs.arcGrads.resize((size_t)h->B);
+  for (int b = 0; b < h->B; b++) {
+    bs.arcGrads[b].resize((size_t)na[b]);
+    if (na[b]) check(c, gtnb_lattice_arc_grads(c->ctx, h->lat, b, bs.arcGrads[b].data()));
+  }
+}
+
 /* run the pending backward of a batched lattice once: shortestDistanceGrad for the recorded seeds
- * (shortest.cpp:33-82), host-provided arc gradients on top, then compose's gradFunc (compose.cpp:496-518)
+ * (shortest.cpp:33-82), host-provided arc gradients added on top, then compose's gradFunc (compose.cpp:496-518)
  * for all entries into bs.dLinear / bs.dGraph */
 void flushLattice(const std::shared_ptr<LatticeHandle>& h) {
   BatchState& bs = *h->batch;
@@ -138,17 +150,26 @@ void flushLattice(const std::shared_ptr<LatticeHandle>& h) {
   for (size_t b = 0; b < B; b++) graphTotal = std::max(graphTotal, bs.graphOff[b + 1]);
   bs.dLinear = std::make_shared<DeviceBuffer>(c, std::max<size_t>(B * bs.stride, 1));
   bs.dGraph = std::make_shared<DeviceBuffer>(c, std::max<size_t>(graphTotal, 1));
+  bool hostDeltas = false;
+  for (size_t b = 0; b < B; b++) hostDeltas = hostDeltas || !bs.hostDeltas[b].empty();
+  const auto& na = h->sizes().second;
   std::lock_guard<std::mutex> l(c->lock);
   if (bs.mode >= 0) {
     if (h->scoreMode != bs.mode) { // the lattice was re-scored in the other semiring since: restore
-      std::vector<float> s(B);
-      check(c, gtnb_forward(c->ctx, h->lat, bs.mode, s.data(), nullptr));
+      check(c, gtnb_forward(c->ctx, h->lat, bs.mode, nullptr, nullptr));
       h->scoreMode = bs.mode;
     }
     check(c, gtnb_backward(c->ctx, h->lat, bs.mode, bs.sdDelta.data()));
+    // the entries' own gradients are the seeds' alone: keep them before the host deltas are added in
+    if (hostDeltas) copyArcGrads(h, na, bs);
   }
-  for (size_t b = 0; b < B; b++)
-    if (!bs.hostDeltas[b].empty()) check(c, gtnb_lattice_set_arc_grads(c->ctx, h->lat, (int)b, bs.hostDeltas[b].data()));
+  for (size_t b = 0; b < B; b++) {
+    if (bs.hostDeltas[b].empty()) continue;
+    std::vector<float>& d = bs.hostDeltas[b];
+    if (bs.mode >= 0)
+      for (size_t i = 0; i < d.size() && i < bs.arcGrads[b].size(); i++) d[i] += bs.arcGrads[b][i];
+    check(c, gtnb_lattice_set_arc_grads(c->ctx, h->lat, (int)b, d.data()));
+  }
   check(c, gtnb_memset(c->ctx, bs.dLinear->ptr, 0, sizeof(float) * std::max<size_t>(B * bs.stride, 1)));
   check(c, gtnb_memset(c->ctx, bs.dGraph->ptr, 0, sizeof(float) * std::max<size_t>(graphTotal, 1)));
   check(c, gtnb_compose_grad(c->ctx, h->lat, bs.dGraph->ptr, bs.dLinear->ptr, (int64_t)bs.stride));
@@ -282,9 +303,9 @@ std::vector<Graph> composeBatch(const std::vector<Graph>& a, const std::vector<G
         if (bs.flushed)
           throw std::logic_error("[gtn::compose] the batched backward of this lattice has already run "
                                  "(backward the whole list before reading gradients, or retain and recompose)");
-        // arc gradients still parked on the device (they come from the batched shortest-distance
-        // backward): nothing to do now.  Otherwise they were produced on the host: keep a copy.
-        if (!deltas.hasLazyWeights()) bs.hostDeltas[bi].assign(deltas.weights(), deltas.weights() + deltas.numArcs());
+        // arc gradients still parked on the device come from the batched shortest-distance backward and are
+        // there when it runs; keep a copy of those produced on the host
+        deltas.hostContributions(bs.hostDeltas[bi]);
       }
       auto c = handle->owner;
       Graph& gGraph = inputs[linearFirst ? 1 : 0];
@@ -371,22 +392,29 @@ void flushLinear(const std::shared_ptr<LinearBatch>& lb) {
   lb->flushed = true;
 }
 
+/* the batched lattice whose B entries gs are, each exactly once (in any order); null otherwise */
+std::shared_ptr<LatticeHandle> entriesOfOneBatch(const std::vector<Graph>& gs) {
+  const size_t B = gs.size();
+  auto h = B >= 2 ? gs[0].scoringLattice() : nullptr;
+  if (!h || !h->batch || (size_t)h->B != B) return nullptr;
+  std::vector<char> seen(B, 0);
+  for (size_t i = 0; i < B; i++) {
+    const int bi = gs[i].latticeIndex();
+    if (gs[i].scoringLattice() != h || bi < 0 || bi >= (int)B || seen[bi]) return nullptr;
+    seen[bi] = 1;
+  }
+  return h;
+}
+
 std::vector<Graph> scoreBatch(const std::vector<Graph>& gs, bool tropical) {
   const size_t B = gs.size();
   Graph (*single)(const Graph&) = tropical ? static_cast<Graph (*)(const Graph&)>(viterbiScore)
                                            : static_cast<Graph (*)(const Graph&)>(forwardScore);
   if (B < 2) return parallelMap(single, gs);
   // (1) the B entries of one batched lattice, each exactly once
-  auto h = gs[0].scoringLattice();
-  if (h && h->batch && (size_t)h->B == B) {
-    std::vector<char> seen(B, 0);
-    bool ok = true;
-    for (size_t i = 0; ok && i < B; i++) {
-      ok = gs[i].scoringLattice() == h && gs[i].latticeIndex() >= 0 && gs[i].latticeIndex() < (int)B &&
-           !seen[gs[i].latticeIndex()];
-      if (ok) seen[gs[i].latticeIndex()] = 1;
-    }
-    if (ok) {
+  {
+    auto h = entriesOfOneBatch(gs);
+    if (h) {
       auto& c = h->owner;
       std::vector<float> scores(B);
       {
@@ -415,6 +443,14 @@ std::vector<Graph> scoreBatch(const std::vector<Graph>& gs, bool tropical) {
           // the lattice entry's own gradient: its arc gradients, still on the device
           inputs[0].addLazyGrad(numArcs, [h, bi, numArcs](std::vector<float>& v) {
             flushLattice(h);
+            {
+              BatchState& bs = *h->batch;
+              std::lock_guard<std::mutex> lk(bs.m);
+              if (!bs.arcGrads.empty()) {
+                v = bs.arcGrads[bi];
+                return;
+              }
+            }
             auto& c = h->owner;
             v.resize(numArcs);
             if (numArcs == 0) return;
@@ -498,6 +534,21 @@ bool tapeHasBatch(const Graph& g, int depth = 0) {
 
 } // namespace
 
+namespace detail {
+
+void keepBatchArcGrads(const std::shared_ptr<LatticeHandle>& h) {
+  BatchState& bs = *h->batch;
+  std::lock_guard<std::mutex> lk(bs.m);
+  // not flushed: the flush re-runs the batch's own backward before any of its lazy gradients reads; no seed: no
+  // lazy gradient reads the entries' arc gradients
+  if (!bs.flushed || bs.mode < 0 || !bs.arcGrads.empty()) return;
+  const auto& na = h->sizes().second;
+  std::lock_guard<std::mutex> l(h->owner->lock);
+  copyArcGrads(h, na, bs);
+}
+
+} // namespace detail
+
 std::vector<Graph> compose(const std::vector<Graph>& a, const std::vector<Graph>& b) {
   return composeBatch(a, b, false);
 }
@@ -509,6 +560,16 @@ std::vector<Graph> forwardScore(const std::vector<Graph>& gs) {
 }
 std::vector<Graph> viterbiScore(const std::vector<Graph>& gs) {
   return scoreBatch(gs, true);
+}
+std::vector<Graph> viterbiPath(const std::vector<Graph>& gs) {
+  // the B entries of one batched lattice, each once: ONE gtnb_viterbi_path, split into B paths
+  auto h = entriesOfOneBatch(gs);
+  if (!h) return parallelMap(static_cast<Graph (*)(const Graph&)>(viterbiPath), gs);
+  auto p = detail::latticePaths(h);
+  std::vector<Graph> out;
+  out.reserve(gs.size());
+  for (auto& g : gs) out.push_back(detail::pathGraph(g, p, g.latticeIndex()));
+  return out;
 }
 
 void backward(const std::vector<Graph>& gs, bool retainGraph) {

@@ -76,7 +76,25 @@ struct BatchState {
   std::shared_ptr<DeviceBuffer> dLinear, dGraph; // gradients w.r.t. the emissions [B][stride] / the graphs' arcs
   size_t stride{0};
   std::vector<size_t> graphOff; // entry b's slab in dGraph
+  // the entries' own arc gradients from the recorded seeds, kept on the host once the lattice's arc gradients no
+  // longer hold them (host deltas added on top, or a later single-entry backward); empty while they do
+  std::vector<std::vector<float>> arcGrads;
 };
+
+/* A single-entry op is about to launch a backward on the batched lattice h: if the batch's own backward has
+ * already run, keep the entries' arc gradients its lazy gradients still read (gtn/batched.cpp).  Forces nothing. */
+void keepBatchArcGrads(const std::shared_ptr<LatticeHandle>& h);
+
+/* The best paths of every entry of a lattice, one gtnb_viterbi_path: entry b's arcs start at b * stride.  maxNodes:
+ * the node count of the largest entry, or 0 to read it from the lattice. */
+struct LatticePaths {
+  int stride{0};
+  std::vector<int32_t> arcs, il, ol, len;
+  std::vector<float> w;
+};
+LatticePaths latticePaths(const std::shared_ptr<LatticeHandle>& h, int maxNodes = 0);
+/* viterbiPath's result for g from row b of p (shortest.cpp:250-270) */
+Graph pathGraph(const Graph& g, const LatticePaths& p, int b);
 
 /* Host arrays backing a gtnb_graph_view of a Graph (valid while alive). */
 struct ViewStorage {

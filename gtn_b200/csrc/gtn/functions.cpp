@@ -622,7 +622,9 @@ Graph shortestDistanceLinear(const Graph& g, bool tropical) {
   return result;
 }
 
-/* shortest distance over one graph on the device */
+/* shortest distance over one graph on the device.  An entry of a batched lattice (a list intersect) is scored by a
+ * launch over the whole batch: the forward and the backward run on all B entries, the backward with a one-hot
+ * seed, and this entry's row is taken */
 Graph shortestDistanceDevice(const Graph& g, bool tropical) {
   if (g.isLinear() && g.linearLabels() > 0 && !g.isDeviceResident()) return shortestDistanceLinear(g, tropical);
   std::shared_ptr<LatticeHandle> handle;
@@ -645,38 +647,48 @@ Graph shortestDistanceDevice(const Graph& g, bool tropical) {
     handle->B = 1;
   }
   auto& c = handle->owner;
-  float score = 0.0f;
+  const int B = std::max(handle->B, 1);
+  const int bi = latticeEntry ? g.latticeIndex() : 0;
+  const bool batchEntry = B > 1;
+  std::vector<float> scores(B);
   {
     std::lock_guard<std::mutex> l(c->lock);
-    check(c, gtnb_forward(c->ctx, handle->lat, tropical ? 1 : 0, &score, nullptr));
+    check(c, gtnb_forward(c->ctx, handle->lat, tropical ? 1 : 0, scores.data(), nullptr));
     handle->scoreMode = tropical ? 1 : 0;
   }
   const size_t numArcs = g.numArcs();
-  auto gradFunc = [handle, tropical, latticeEntry, numArcs](std::vector<Graph>& inputs, Graph& deltas) {
+  auto gradFunc = [handle, tropical, latticeEntry, batchEntry, B, bi, numArcs](std::vector<Graph>& inputs,
+                                                                                Graph& deltas) {
     auto& c = handle->owner;
-    const float delta = deltas.item();
-    // a gradient still parked on the device would be overwritten by this launch
-    if (inputs[0].isGradAvailable() && inputs[0].grad().hasLazyWeights()) inputs[0].grad().weights();
+    std::vector<float> delta(B, 0.0f);
+    delta[bi] = deltas.item();
+    if (batchEntry && handle->batch) {
+      keepBatchArcGrads(handle);
+    } else if (latticeEntry && inputs[0].isGradAvailable() && inputs[0].grad().hasPendingWeights()) {
+      // a gradient of this lattice still parked on the device would be overwritten by this launch (no batch
+      // behind it: resolving it reads the lattice and nothing else)
+      inputs[0].grad().weights();
+    }
     {
       std::lock_guard<std::mutex> l(c->lock);
       // the lattice may have been re-used by another score op since: restore the node scores
       if (handle->scoreMode != (tropical ? 1 : 0)) {
-        float s;
-        check(c, gtnb_forward(c->ctx, handle->lat, tropical ? 1 : 0, &s, nullptr));
+        check(c, gtnb_forward(c->ctx, handle->lat, tropical ? 1 : 0, nullptr, nullptr));
         handle->scoreMode = tropical ? 1 : 0;
       }
-      check(c, gtnb_backward(c->ctx, handle->lat, tropical ? 1 : 0, &delta));
+      check(c, gtnb_backward(c->ctx, handle->lat, tropical ? 1 : 0, delta.data()));
     }
-    auto fetch = [handle, numArcs](std::vector<float>& v) {
+    auto fetch = [handle, bi, numArcs](std::vector<float>& v) {
       auto& c = handle->owner;
       v.resize(numArcs);
       if (numArcs == 0) return;
       std::lock_guard<std::mutex> l(c->lock);
-      check(c, gtnb_lattice_arc_grads(c->ctx, handle->lat, 0, v.data()));
+      check(c, gtnb_lattice_arc_grads(c->ctx, handle->lat, bi, v.data()));
     };
-    if (latticeEntry) {
+    if (latticeEntry && !batchEntry) {
       inputs[0].addLazyGrad(numArcs, fetch);
     } else {
+      // the next launch on a shared lattice overwrites every entry's arc gradients: read this one now
       std::vector<float> v;
       fetch(v);
       inputs[0].addGrad(std::move(v));
@@ -685,7 +697,7 @@ Graph shortestDistanceDevice(const Graph& g, bool tropical) {
   Graph result(gradFunc, {g});
   result.addNode(true);
   result.addNode(false, true);
-  result.addArc(0, 1, 0, 0, score);
+  result.addArc(0, 1, 0, 0, scores[bi]);
   return result;
 }
 
@@ -708,11 +720,65 @@ Graph viterbiScore(const Graph& g) {
   return detail::shortestDistanceDevice(g, true);
 }
 
+namespace detail {
+
+LatticePaths latticePaths(const std::shared_ptr<LatticeHandle>& h, int maxNodes) {
+  auto& c = h->owner;
+  const int B = std::max(h->B, 1);
+  if (maxNodes <= 0) // a path visits each node at most once: the largest entry bounds every row
+    for (int b = 0; b < B; b++) maxNodes = std::max(maxNodes, (int)h->sizes().first[b]);
+  maxNodes = std::max(maxNodes, 1);
+  LatticePaths p;
+  p.stride = maxNodes;
+  const size_t n = (size_t)B * maxNodes;
+  p.arcs.resize(n);
+  p.il.resize(n);
+  p.ol.resize(n);
+  p.w.resize(n);
+  p.len.assign(B, 0);
+  std::lock_guard<std::mutex> l(c->lock);
+  check(c, gtnb_viterbi_path(c->ctx, h->lat, maxNodes, p.arcs.data(), p.il.data(), p.ol.data(), p.w.data(),
+                             p.len.data(), nullptr));
+  h->scoreMode = -1; // node scores now hold the path recursion
+  return p;
+}
+
+Graph pathGraph(const Graph& g, const LatticePaths& p, int b) {
+  const size_t row = (size_t)b * p.stride;
+  const int len = p.len[b];
+  Graph out(nullptr, {g});
+  if (len >= 0) {
+    out.addNode(true, len == 0);
+  }
+  for (int i = 0; i < len; i++) {
+    out.addNode(false, i == len - 1);
+    out.addArc(i, i + 1, p.il[row + i], p.ol[row + i], p.w[row + i]);
+  }
+  // shortest.cpp:262-270: the reference keeps the path arcs end -> start and indexes them
+  // with the output graph's (start -> end) arc ids; reproduced as is.
+  std::vector<int> rev(p.arcs.begin() + row, p.arcs.begin() + row + std::max(len, 0));
+  std::reverse(rev.begin(), rev.end());
+  auto gradFunc = [rev = std::move(rev)](std::vector<Graph>& inputs, Graph& deltas) {
+    std::vector<float> grad(inputs[0].numArcs(), 0.0f);
+    for (size_t a = 0; a < deltas.numArcs(); ++a) {
+      grad[rev[a]] += deltas.weight(a);
+    }
+    inputs[0].addGrad(std::move(grad));
+  };
+  out.setGradFunc(std::move(gradFunc));
+  return out;
+}
+
+} // namespace detail
+
+/* an entry of a batched lattice is decoded by a launch over the whole batch; its row is taken */
 Graph viterbiPath(const Graph& g) {
   using namespace detail;
   std::shared_ptr<LatticeHandle> handle;
+  int bi = 0;
   if (g.scoringLattice() && g.scoringLattice()->composed) {
     handle = g.scoringLattice();
+    bi = g.latticeIndex();
   } else {
     auto c = threadContext();
     ViewStorage vs;
@@ -727,37 +793,8 @@ Graph viterbiPath(const Graph& g) {
     handle->lat = lat;
     handle->B = 1;
   }
-  auto& c = handle->owner;
-  const int maxLen = (int)std::max<size_t>(g.numNodes(), 1);
-  std::vector<int32_t> arcs(maxLen), il(maxLen), ol(maxLen);
-  std::vector<float> w(maxLen);
-  int32_t len = 0;
-  {
-    std::lock_guard<std::mutex> l(c->lock);
-    check(c, gtnb_viterbi_path(c->ctx, handle->lat, maxLen, arcs.data(), il.data(), ol.data(), w.data(), &len, nullptr));
-    handle->scoreMode = -1; // node scores now hold the path recursion
-  }
-  Graph out(nullptr, {g});
-  if (len >= 0) {
-    out.addNode(true, len == 0);
-  }
-  for (int i = 0; i < len; i++) {
-    out.addNode(false, i == len - 1);
-    out.addArc(i, i + 1, il[i], ol[i], w[i]);
-  }
-  // shortest.cpp:262-270: the reference keeps the path arcs end -> start and indexes them
-  // with the output graph's (start -> end) arc ids; reproduced as is.
-  std::vector<int> rev(arcs.begin(), arcs.begin() + std::max(len, 0));
-  std::reverse(rev.begin(), rev.end());
-  auto gradFunc = [rev = std::move(rev)](std::vector<Graph>& inputs, Graph& deltas) {
-    std::vector<float> grad(inputs[0].numArcs(), 0.0f);
-    for (size_t a = 0; a < deltas.numArcs(); ++a) {
-      grad[rev[a]] += deltas.weight(a);
-    }
-    inputs[0].addGrad(std::move(grad));
-  };
-  out.setGradFunc(std::move(gradFunc));
-  return out;
+  // (a lattice of its own: g's node count is the row length, no read-back of the sizes)
+  return pathGraph(g, latticePaths(handle, handle->B > 1 ? 0 : (int)g.numNodes()), bi);
 }
 
 } // namespace gtn

@@ -56,13 +56,15 @@ Graph viterbiPath(const Graph& g);
 
 /**
  * List forms (bindings/python/gtn/_functions.cpp:69-135): one packed launch for the whole list where the graphs
- * allow it -- every pair a (graph, gtn::linearGraph) composition, every score over the entries of such a batch
- * or over emission chains -- else parallelMap of the single-graph function.  See gtn/batched.cpp.
+ * allow it -- every pair a (graph, gtn::linearGraph) composition, every score or path over the entries of such a
+ * batch, every score over emission chains -- else parallelMap of the single-graph function.  See gtn/batched.cpp.
  */
 std::vector<Graph> compose(const std::vector<Graph>& graphs1, const std::vector<Graph>& graphs2);
 std::vector<Graph> intersect(const std::vector<Graph>& graphs1, const std::vector<Graph>& graphs2);
 std::vector<Graph> forwardScore(const std::vector<Graph>& graphs);
 std::vector<Graph> viterbiScore(const std::vector<Graph>& graphs);
+/** The entries of one batched lattice, each once: one decoding launch for the list; else parallelMap. */
+std::vector<Graph> viterbiPath(const std::vector<Graph>& graphs);
 
 namespace detail {
 /** Host graph construction for the general case (epsilons, arbitrary operands). */

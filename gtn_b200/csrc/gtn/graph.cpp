@@ -373,6 +373,10 @@ std::vector<float>& Graph::hostWeights() const {
     // in place, one scratch vector per thread otherwise)
     thread_local std::vector<float> part;
     for (auto& a : sw.lazyAdds) {
+      if (!a.fetch) {
+        for (size_t i = 0; i < sw.host.size() && i < a.host.size(); i++) sw.host[i] += a.host[i];
+        continue;
+      }
       if (a.acc && a.acc(sw.host.data(), sw.host.size())) continue;
       part.clear();
       a.fetch(part);
@@ -528,6 +532,13 @@ void Graph::addGrad(std::vector<float>&& other) {
     }
     std::lock_guard<std::mutex> lock(sharedGraph_->grad_lock);
     if (isGradAvailable()) {
+      auto& sw = *sharedGrad_->grad->sharedWeights_;
+      if (sw.lazyFetch || !sw.lazyAdds.empty()) {
+        // resolving a pending gradient here could run a batch's deferred backward before every seed is in
+        std::lock_guard<std::mutex> l(sw.lock);
+        sw.lazyAdds.push_back({nullptr, nullptr, std::move(other)});
+        return;
+      }
       auto& gw = sharedGrad_->grad->hostWeights();
       for (size_t i = 0; i < other.size(); i++) gw[i] += other[i];
     } else {
@@ -540,31 +551,44 @@ void Graph::addGrad(std::vector<float>&& other) {
 }
 
 void Graph::addLazyGrad(
-    size_t n, std::function<void(std::vector<float>&)> fetch, std::function<bool(float*, size_t)> acc) {
+    size_t /* numArcs */, std::function<void(std::vector<float>&)> fetch, std::function<bool(float*, size_t)> acc) {
   if (!calcGrad()) return;
-  {
-    std::lock_guard<std::mutex> lock(sharedGraph_->grad_lock);
-    if (!isGradAvailable()) {
-      sharedGrad_->grad = std::make_unique<Graph>(false);
-      sharedGrad_->grad->sharedGraph_ = sharedGraph_;
-      sharedGrad_->grad->sharedWeights_->lazyFetch = std::move(fetch);
-      return;
-    }
+  std::lock_guard<std::mutex> lock(sharedGraph_->grad_lock);
+  if (!isGradAvailable()) {
+    sharedGrad_->grad = std::make_unique<Graph>(false);
+    sharedGrad_->grad->sharedGraph_ = sharedGraph_;
+    sharedGrad_->grad->sharedWeights_->lazyFetch = std::move(fetch);
+    return;
   }
-  {
-    // a gradient that itself still lives on the device: queue this contribution behind it instead of
-    // forcing both to the host now (the batched list ops park one per op and entry until somebody reads)
-    std::lock_guard<std::mutex> lock(sharedGraph_->grad_lock);
-    auto& gw = *sharedGrad_->grad->sharedWeights_;
-    if (gw.lazyFetch || !gw.lazyAdds.empty()) {
-      std::lock_guard<std::mutex> l(gw.lock);
-      gw.lazyAdds.push_back({std::move(fetch), std::move(acc)});
-      return;
-    }
+  // queue this contribution behind the gradient already present, on the host or not: fetching it now could
+  // run its batch's deferred backward in the middle of backward(), before every seed is recorded (the batched
+  // list ops park one per op and entry until somebody reads)
+  auto& gw = *sharedGrad_->grad->sharedWeights_;
+  std::lock_guard<std::mutex> l(gw.lock);
+  gw.lazyAdds.push_back({std::move(fetch), std::move(acc), {}});
+}
+
+bool Graph::hostContributions(std::vector<float>& out) const {
+  if (!sharedWeights_) return false;
+  auto& sw = *sharedWeights_;
+  if (!hasPendingWeights()) {
+    out = hostWeights();
+    return true;
   }
-  std::vector<float> now(n);
-  fetch(now);
-  addGrad(std::move(now));
+  std::lock_guard<std::mutex> l(sw.lock);
+  bool any = !sw.lazyFetch; // then the host vector holds the first contribution
+  for (auto& a : sw.lazyAdds) any = any || !a.fetch;
+  if (!any) return false;
+  const size_t n = numArcs();
+  if (sw.lazyFetch)
+    out.assign(n, 0.0f);
+  else
+    out = sw.host;
+  out.resize(n, 0.0f);
+  for (auto& a : sw.lazyAdds)
+    if (!a.fetch)
+      for (size_t i = 0; i < n && i < a.host.size(); i++) out[i] += a.host[i];
+  return true;
 }
 
 void Graph::addGrad(const std::vector<float>& other) {

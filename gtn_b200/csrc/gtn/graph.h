@@ -226,18 +226,28 @@ class Graph {
   void cacheDeviceWeights(std::shared_ptr<detail::DeviceBuffer> buf) const;
   /**
    * Install a gradient whose values still live on the device: `fetch` fills the host
-   * vector the first time anybody reads it.  Falls back to an eager fetch + addGrad
-   * when a gradient is already present.  (Used by the shortest-distance gradFunc.)
+   * vector the first time anybody reads it.  When a gradient is already present the
+   * contribution is queued behind it and added when the gradient is read: fetching it
+   * now could run a batch's deferred backward in the middle of backward().
+   * acc (optional): adds the contribution straight into dst (no temporary); returns false if it cannot, then
+   * fetch + add is used.
    */
-  /** acc (optional): adds the contribution straight into dst (no temporary); returns false if it cannot, then
-   * fetch + add is used. */
   void addLazyGrad(
       size_t numArcs, std::function<void(std::vector<float>&)> fetch,
       std::function<bool(float* dst, size_t n)> acc = nullptr);
-  /** True while this graph's weights are still device-only (see addLazyGrad). */
+  /** True while these weights are exactly one contribution that is still on the device (see addLazyGrad). */
   bool hasLazyWeights() const {
-    return sharedWeights_ && sharedWeights_->lazyFetch != nullptr;
+    return sharedWeights_ && sharedWeights_->lazyFetch != nullptr && sharedWeights_->lazyAdds.empty();
   }
+  /** True while any contribution to these weights has not been added up on the host yet. */
+  bool hasPendingWeights() const {
+    return sharedWeights_ && (sharedWeights_->lazyFetch != nullptr || !sharedWeights_->lazyAdds.empty());
+  }
+  /**
+   * The sum of the contributions to these weights that were made on the host, resolving nothing that is still on
+   * the device.  Returns false, leaving `out` alone, when there are none.
+   */
+  bool hostContributions(std::vector<float>& out) const;
   /** The slice of a batch-wide device buffer that holds these weights, if a batched list op gathered them. */
   std::shared_ptr<detail::DeviceBuffer> batchSlice(size_t* offset) const;
   void cacheBatchSlice(std::shared_ptr<detail::DeviceBuffer> buf, size_t offset) const;
@@ -269,11 +279,12 @@ class Graph {
     std::shared_ptr<detail::DeviceBuffer> device; // set by setWeights(device pointer)
     bool hostStale{false}; // device holds the truth, host not yet filled
     std::function<void(std::vector<float>&)> lazyFetch; // see addLazyGrad, fromLattice
-    // further device-side contributions that arrived while the first one was still pending: added to the
-    // host vector when somebody reads it (the batched list ops install one per op and entry)
+    // further contributions that arrived while a gradient was already present: added to the host vector when
+    // somebody reads it (the batched list ops install one per op and entry)
     struct LazyAdd {
-      std::function<void(std::vector<float>&)> fetch;
+      std::function<void(std::vector<float>&)> fetch; // empty for a host contribution
       std::function<bool(float*, size_t)> acc; // may be empty
+      std::vector<float> host; // the values of a host contribution (addGrad)
     };
     std::vector<LazyAdd> lazyAdds;
     // a slice of a batch-wide device buffer that holds exactly these weights (gathered by a batched list

@@ -175,8 +175,14 @@ PYBIND11_MODULE(_gtn, m) {
         return viterbiScore(gs);
       },
       "graphs"_a);
-  m.def("viterbi_path", unary(viterbiPath), "g"_a);
-  m.def("viterbi_path", unaryList(viterbiPath), "graphs"_a);
+  m.def("viterbi_path", unary(static_cast<Graph (*)(const Graph&)>(&viterbiPath)), "g"_a);
+  m.def(
+      "viterbi_path",
+      [](const std::vector<Graph>& gs) {
+        py::gil_scoped_release release;
+        return viterbiPath(gs); // one decoding launch for the entries of one batched lattice (gtn/batched.cpp)
+      },
+      "graphs"_a);
   m.def("project_input", unary(projectInput), "g"_a);
   m.def("project_output", unary(projectOutput), "g"_a);
   m.def(

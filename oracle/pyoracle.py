@@ -433,6 +433,16 @@ class RefGraph:
     def grad(self):
         return RefGraph(libref().ref_graph_grad(self.h))
 
+    def is_grad_available(self):
+        try:
+            self.grad()
+        except RefError:
+            return False
+        return True
+
+    def zero_grad(self):
+        _rc(libref().ref_graph_zero_grad(self.h))
+
     def weights(self):
         return self.arrays()["w"]
 
