@@ -189,6 +189,13 @@ SYMBOLS = [
     ("gtnb_beam_decode_async", C.c_int,
      [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp, _vp,
       _vp, _vp, _vp, C.c_size_t]),
+    ("gtnb_lm_create", C.c_int, [_vp, C.POINTER(GraphView), C.c_int, C.POINTER(_vp)]),
+    ("gtnb_lm_destroy", None, [_vp, _vp]),
+    ("gtnb_beam_decode_lm_async_workspace", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    ("gtnb_beam_decode_lm_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp,
+      C.c_float, C.c_float, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
     ("gtnb_edit_distance_async", C.c_int,
      [_vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
       C.c_size_t]),

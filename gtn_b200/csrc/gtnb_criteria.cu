@@ -6,6 +6,7 @@
  */
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -4061,6 +4062,20 @@ extern "C" int gtnb_edit_distance_async(
   });
 }
 
+/*
+ * The LM of gtnb_beam_decode_lm_async, prepared once: the graph's resolved table, weight [S][C + 1] float32 and
+ * destination [S][C + 1] int32 in one device allocation.  Column C holds the end weights.
+ */
+struct gtnb_lm {
+  int device = 0, C = 0, S = 0, start = 0;
+  void* mem = nullptr;
+  float* w = nullptr;
+  int32_t* d = nullptr;
+  ~gtnb_lm() {
+    if (mem) cudaFree(mem);
+  }
+};
+
 namespace {
 
 struct BeamAsyncArgs {
@@ -4087,9 +4102,18 @@ int beam_async_check(gtnb_ctx* ctx, const std::string& fn, const BeamAsyncArgs& 
   return GTNB_OK;
 }
 
+/* gtnb_beam_decode_lm_async's own arguments beyond gtnb_beam_decode_async's */
+struct BeamLmArgs {
+  const gtnb_lm* lm;
+  float lm_weight, token_bonus;
+  int token_beam;
+  float *am_scores, *lm_scores;
+};
+
 /* gtnb_beam_decode_async's run: the back-pointers and (with transitions) the transposed weights, the start weights
- * and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued */
-int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch) {
+ * and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued; with m, the
+ * fused search of gtnb_beam_decode_lm_async (the same scratch) */
+int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const BeamLmArgs* m = nullptr) {
   uint16_t* bp = nullptr;
   float *wt = nullptr, *wfirst = nullptr;
   int32_t* wbad = nullptr;
@@ -4101,6 +4125,13 @@ int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch) {
   }
   if (!launch) return GTNB_OK;
   if (a.kind != GTNB_DENSE_CTC) GTNB_TRY(launch_beam_weights(ctx, a.C, a.kind, a.trans_w, wt, wfirst, wbad));
+  if (m) {
+    const BeamLmLaunch f{m->token_beam, m->lm ? m->lm->w : nullptr, m->lm ? m->lm->d : nullptr,
+                         m->lm ? m->lm->start : 0, m->lm_weight, m->token_bonus, m->am_scores, m->lm_scores};
+    return launch_beam_decode_lm(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
+                                 a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
+                                 a.tokens, a.lengths, a.scores, a.status, f);
+  }
   return launch_beam_decode(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
                             a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
                             a.tokens, a.lengths, a.scores, a.status);
@@ -4133,4 +4164,164 @@ extern "C" int gtnb_beam_decode_async(
   GTNB_TRY(beam_async_check(ctx, fn, a));
   return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
                        [&](bool launch) { return beam_async_run(ctx, a, launch); });
+}
+
+namespace {
+
+constexpr long long kLmMaxEntries = 1ll << 25;
+
+/*
+ * The checks of gtnb_lm_create and the resolution: w(s, c) is s's arc labelled c, else s's epsilon (backoff) arc's
+ * weight plus the resolution of c from its destination, else -inf.  Nodes are resolved in order of backoff depth, so
+ * a backoff destination's row is complete before the rows that back off to it.  Without any arc labelled C, every
+ * end weight (column C) is 0.
+ */
+int lm_resolve(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, int C, int* start,
+               std::vector<float>* w, std::vector<int32_t>* d) {
+  if (validate_view(ctx, G)) return GTNB_ERR_INVALID_ARGUMENT;
+  const int S = G.num_nodes;
+  if (S < 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has no nodes");
+  if ((long long)S * (C + 1) > kLmMaxEntries)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": S * (C + 1) > 2^25 table entries");
+  *start = -1;
+  for (int s = 0; s < S; s++)
+    if (G.node_flags[s] & 1) {
+      if (*start >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has more than one start node");
+      *start = s;
+    }
+  if (*start < 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has no start node");
+  const long long n = (long long)S * (C + 1);
+  const float ninf = -std::numeric_limits<float>::infinity();
+  std::vector<int32_t> arc(n, -1), eps(S, -1);
+  bool has_end = false;
+  for (int a = 0; a < G.num_arcs; a++) {
+    const int s = G.arc_src[a], l = G.arc_ilabel[a];
+    const float x = G.weights ? G.weights[a] : 0.0f;
+    if (l != G.arc_olabel[a]) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM is not an acceptor");
+    if (x != x || x == std::numeric_limits<float>::infinity())
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has a NaN or +inf weight");
+    if (l == GTNB_EPSILON) {
+      if (eps[s] >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a node has two epsilon arcs");
+      eps[s] = a;
+      continue;
+    }
+    if (l < 0 || l > C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": an LM label outside [0, C]");
+    int32_t& slot = arc[(long long)s * (C + 1) + l];
+    if (slot >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a node has two arcs with one label");
+    slot = a;
+    has_end |= l == C;
+  }
+  // backoff depth: the number of epsilon arcs to a node without one (more than S means a cycle)
+  std::vector<int> depth(S, -1);
+  for (int s = 0; s < S; s++) {
+    int v = s, k = 0;
+    while (depth[v] < 0 && eps[v] >= 0 && k <= S) {
+      v = G.arc_dst[eps[v]];
+      k++;
+    }
+    if (k > S) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has a cycle of epsilon arcs");
+    int base = depth[v] < 0 ? 0 : depth[v];
+    for (int u = s; u != v; u = G.arc_dst[eps[u]]) depth[u] = base + k--;
+    if (depth[v] < 0) depth[v] = 0;
+  }
+  std::vector<int> order(S);
+  for (int s = 0; s < S; s++) order[s] = s;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return depth[a] < depth[b]; });
+  w->assign(n, ninf);
+  d->assign(n, 0);
+  for (int s : order) {
+    const long long row = (long long)s * (C + 1);
+    const int e = eps[s];
+    const long long brow = e >= 0 ? (long long)G.arc_dst[e] * (C + 1) : -1;
+    const float be = e >= 0 ? (G.weights ? G.weights[e] : 0.0f) : 0.0f;
+    for (int c = 0; c <= C; c++) {
+      const int a = arc[row + c];
+      if (a >= 0) {
+        (*w)[row + c] = G.weights ? G.weights[a] : 0.0f;
+        (*d)[row + c] = G.arc_dst[a];
+      } else if (e >= 0) {
+        (*w)[row + c] = be + (*w)[brow + c];
+        (*d)[row + c] = (*d)[brow + c];
+      }
+    }
+    if (!has_end) (*w)[row + C] = 0.0f;
+  }
+  return GTNB_OK;
+}
+
+} // namespace
+
+extern "C" int gtnb_lm_create(gtnb_ctx* ctx, const gtnb_graph_view* lm, int C, gtnb_lm** out) {
+  const std::string fn = "gtnb_lm_create";
+  if (out) *out = nullptr;
+  if (!ctx || !lm || C <= 0 || !out) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (C > 256) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": C > 256");
+  std::unique_ptr<gtnb_lm> h(new gtnb_lm);
+  std::vector<float> w;
+  std::vector<int32_t> d;
+  GTNB_TRY(lm_resolve(ctx, fn, *lm, C, &h->start, &w, &d));
+  h->device = ctx->device;
+  h->C = C;
+  h->S = lm->num_nodes;
+  const size_t wb = (sizeof(float) * w.size() + 255) & ~(size_t)255;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  GTNB_CUDA(ctx, cudaMalloc(&h->mem, wb + sizeof(int32_t) * d.size()));
+  h->w = static_cast<float*>(h->mem);
+  h->d = reinterpret_cast<int32_t*>(static_cast<unsigned char*>(h->mem) + wb);
+  GTNB_CUDA(ctx, cudaMemcpy(h->w, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice));
+  GTNB_CUDA(ctx, cudaMemcpy(h->d, d.data(), sizeof(int32_t) * d.size(), cudaMemcpyHostToDevice));
+  GTNB_CUDA(ctx, cudaDeviceSynchronize()); // (set-up: the table is on the device before any stream reads it)
+  *out = h.release();
+  return GTNB_OK;
+}
+
+extern "C" void gtnb_lm_destroy(gtnb_ctx* ctx, gtnb_lm* lm) {
+  if (!lm) return;
+  if (ctx) cudaSetDevice(lm->device);
+  delete lm; // (cudaFree waits for the device: no launch still reads the table)
+}
+
+namespace {
+
+int beam_lm_check(gtnb_ctx* ctx, const std::string& fn, const BeamAsyncArgs& a, int token_beam) {
+  GTNB_TRY(beam_async_check(ctx, fn, a));
+  if (token_beam < 1 || token_beam > a.C) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": token_beam outside [1, C]");
+  return GTNB_OK;
+}
+
+} // namespace
+
+extern "C" int gtnb_beam_decode_lm_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, int beam,
+                                                   int nbest, int token_beam, size_t* bytes) {
+  const std::string fn = "gtnb_beam_decode_lm_async_workspace";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !bytes) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  const BeamAsyncArgs a{B, T, C, dtype, nullptr, nullptr, kind, nullptr, 0, beam, nbest,
+                        nullptr, nullptr, nullptr, nullptr};
+  GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
+  const BeamLmArgs m{nullptr, 0.0f, 0.0f, token_beam, nullptr, nullptr};
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return beam_async_run(ctx, a, launch, &m); });
+}
+
+extern "C" int gtnb_beam_decode_lm_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, int kind, const float* trans_w_dev, int blank, int beam, int nbest,
+    const gtnb_lm* lm, float lm_weight, float token_bonus, int token_beam, int32_t* tokens_dev, int32_t* lengths_dev,
+    float* scores_dev, float* am_scores_dev, float* lm_scores_dev, int32_t* status_dev, void* workspace_dev,
+    size_t workspace_bytes) {
+  const std::string fn = "gtnb_beam_decode_lm_async";
+  if (!ctx || B < 0 || T < 0 || C <= 0 ||
+      (B > 0 && ((T > 0 && !emissions_dev) || !tokens_dev || !lengths_dev || !scores_dev)) ||
+      (kind == GTNB_DENSE_CTC) != (trans_w_dev == nullptr))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!(lm_weight >= 0.0f && std::isfinite(lm_weight)) || !std::isfinite(token_bonus))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": lm_weight must be finite and >= 0, token_bonus finite");
+  if (lm && lm->device != ctx->device)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM was made on another device");
+  if (lm && lm->C != C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM was made for another C");
+  const BeamAsyncArgs a{B, T, C, dtype, emissions_dev, input_lens_dev, kind, trans_w_dev, blank, beam, nbest,
+                        tokens_dev, lengths_dev, scores_dev, status_dev};
+  GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
+  const BeamLmArgs m{lm, lm_weight, token_bonus, token_beam, am_scores_dev, lm_scores_dev};
+  return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return beam_async_run(ctx, a, launch, &m); });
 }

@@ -236,6 +236,20 @@ int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions
                        const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
                        int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
                        int32_t* status);
+/* gtnb_beam_decode_lm_async's search: launch_beam_decode's with the LM's resolved table (lmw NULL: no LM),
+ * its weights, token_beam P and the acoustic / LM scores of the hypotheses (each nullable) */
+struct BeamLmLaunch {
+  int P;
+  const float* lmw; // [S][C + 1]
+  const int32_t* lmd; // [S][C + 1]
+  int start;
+  float lm_weight, token_bonus;
+  float *am_scores, *lm_scores;
+};
+int launch_beam_decode_lm(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
+                          const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
+                          int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
+                          int32_t* status, const BeamLmLaunch& lm);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);

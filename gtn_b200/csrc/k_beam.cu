@@ -25,6 +25,14 @@
  *   and frame, coalesced over the tokens), made once per call by beam_weights_kernel with the n-gram start weights
  *   sigma_i = logsumexp_j W[i][j] and a per-row NaN / +inf flag.  The emission row of frame t + 1 is loaded while
  *   frame t is searched.
+ * - Fusion and pruning (gtnb_beam_decode_lm_async).  beam_decode_kernel's policy F: BeamLm, or BeamNoLm for
+ *   gtnb_beam_decode_async, which compiles to the code without them.  Each slot also carries its LM
+ *   node and lmacc (the unweighted sum of its resolved LM weights), double-buffered; candidates are ranked by the
+ *   fused key am + (lm_weight * lmacc + token_bonus * len).  With token_beam P < C the P best tokens of each frame
+ *   are selected first (a rank count per token; ties to the lower token), and extension (s, p) takes candidate
+ *   L + s*P + p, token ptok[p].  The LM row of a beam is read through the L2 like WT's; destination nodes, and the
+ *   acoustic score of an extension (recomputed), only for the winners and the merges.  After the last frame each beam
+ *   adds its end weight and the live ones are ranked again by the final fused score.
  */
 #include <cstdint>
 
@@ -50,6 +58,39 @@ inline long long beam_smem_bytes(int K, int C) {
   return 32ll * K + 4ll * (16 + 256 + 4ll * C + 18ll * K + K + (long long)K * C);
 }
 
+/* beam_lm_smem_bytes: beam_smem_bytes plus the LM node and lmacc per slot ([2][K] each), the frame's tokens and
+ * token -> position map ([C] each) and 8 words of per-warp counts */
+inline long long beam_lm_smem_bytes(int K, int C) {
+  return beam_smem_bytes(K, C) + 4ll * (4ll * K + 2ll * C + 8);
+}
+
+/* the policy of beam_decode_kernel: BeamNoLm for gtnb_beam_decode_async, BeamLm for gtnb_beam_decode_lm_async */
+struct BeamNoLm {
+  static constexpr bool on = false;
+  static constexpr int P = 0; // (unused: every token)
+};
+struct BeamLm {
+  static constexpr bool on = true;
+  int P; // token_beam: tokens per frame, P = C: all of them
+  const float* lmw; // [S][C + 1] resolved LM weights (column C: end weights); NULL: no LM, every weight 0
+  const int32_t* lmd; // [S][C + 1] destination nodes
+  int start; // the LM's start node
+  float lw, tb; // lm_weight, token_bonus
+  float *am, *lm; // [B][N] nullable: acoustic and LM scores of the hypotheses
+};
+
+/* the fused ranking key, in this float32 order (no contraction): am + (lw * lmacc + tb * len) */
+__device__ __forceinline__ float beam_mul_rn(float a, float b) {
+#ifdef GTNB_HOST_EMU
+  return a * b;
+#else
+  return __fmul_rn(a, b);
+#endif
+}
+__device__ __forceinline__ float beam_fuse(const BeamLm& f, float am, float lmacc, int len) {
+  return __fadd_rn(am, __fadd_rn(beam_mul_rn(f.lw, lmacc), beam_mul_rn(f.tb, (float)len)));
+}
+
 /* control block words */
 enum { kBcL = 0, kBcNwin, kBcPre, kBcShift, kBcNeed, kBcTie, kBcDone, kBcBad, kBcTieAny };
 
@@ -67,6 +108,22 @@ __device__ __forceinline__ float beam_lse2(float a, float b) {
   const float mx = fmaxf(a, b), mn = fminf(a, b);
   if (mx == neg_inf()) return mx;
   return mx + flog1p(fexp(mn - mx));
+}
+
+/* the acoustic score of extending a beam (p_blank pb, p_label pl, their logsumexp tot, last token l) by token c */
+__device__ __forceinline__ float beam_ext_am(int kind, int blank, int C, const float* er, const float* wp,
+                                             const float* __restrict__ wt, float pb, float pl, float tot, int l, int c) {
+  float v = neg_inf();
+  if (kind == GTNB_DENSE_ASG || c != blank) {
+    if (kind == GTNB_DENSE_CTC) {
+      v = (c == l ? pb : tot) + er[c];
+    } else {
+      const float from_pl = l >= 0 && (kind == GTNB_DENSE_ASG || c != l) ? pl + __ldg(wt + (long long)l * C + c)
+                                                                           : neg_inf();
+      v = beam_lse2(pb + wp[c], from_pl) + er[c];
+    }
+  }
+  return v;
 }
 
 /* one token back along the back-pointers from (t, s): the token, with (t, s) moved to before it */
@@ -147,18 +204,77 @@ __device__ void beam_flag(int b, int T, int N, int code, int32_t* tokens, int32_
   if (tid == 0 && status) status[b] = code;
 }
 
+/* BeamLm: the am and lm scores of a flagged utterance (status 1 or 2), NaN like its scores */
+__device__ void beam_flag_lm(int b, int N, const BeamLm& f) {
+  for (int n = threadIdx.x; n < N; n += kBeamThreads) {
+    if (f.am) f.am[(long long)b * N + n] = CUDART_NAN_F;
+    if (f.lm) f.lm[(long long)b * N + n] = CUDART_NAN_F;
+  }
+}
+
+/*
+ * BeamLm, after frame T_b - 1: every live slot adds its end weight (a beam whose end weight is -inf is dropped) and
+ * the N-best are the top live beams by the final fused score, ties to the lower slot (the search's own order).
+ * fin / lmf ([K]) hold each slot's final fused score and LM score, rank ([K]) rank -> slot.
+ */
+__device__ void beam_finish_lm(int b, int T, int Tb, int C, int K, int N, const uint16_t* bpu, int cur, int* ctl,
+                               const float* stot, const int* slen, const int* snode, const float* slm, float* fin,
+                               float* lmf, int* rank, int32_t* tokens, int32_t* lengths, float* scores,
+                               int32_t* status, const BeamLm& f) {
+  const int tid = threadIdx.x;
+  const int L = ctl[kBcL];
+  if (tid < L) {
+    const int m = cur * K + tid;
+    const float we = f.lmw ? __ldg(f.lmw + (long long)snode[m] * (C + 1) + C) : 0.0f;
+    const float lm = slm[m] + we;
+    fin[tid] = we == neg_inf() ? neg_inf() : beam_fuse(f, stot[m], lm, slen[m]);
+    lmf[tid] = lm;
+  }
+  __syncthreads();
+  int live = 0;
+  for (int i = 0; i < L; i++) live += fin[i] > neg_inf();
+  if (tid < L && fin[tid] > neg_inf()) {
+    int r = 0;
+    for (int i = 0; i < L; i++) r += fin[i] > fin[tid] || (fin[i] == fin[tid] && i < tid);
+    rank[r] = tid;
+  }
+  __syncthreads();
+  int32_t* out = tokens + (long long)b * N * T;
+  for (int n = tid; n < N; n += kBeamThreads) {
+    const int m = n < live ? rank[n] : -1;
+    const int len = m >= 0 ? slen[cur * K + m] : -1;
+    const long long o = (long long)b * N + n;
+    scores[o] = m >= 0 ? fin[m] : neg_inf();
+    if (f.am) f.am[o] = m >= 0 ? stot[cur * K + m] : neg_inf();
+    if (f.lm) f.lm[o] = m >= 0 ? lmf[m] : neg_inf();
+    lengths[o] = len;
+    int tt = Tb - 1, s = m;
+    for (int p = len - 1; p >= 0; p--) out[(long long)n * T + p] = beam_back(bpu, K, tt, s);
+  }
+  for (long long p = tid; p < (long long)N * T; p += kBeamThreads) {
+    const int n = (int)(p / T);
+    if (p - (long long)n * T >= (n < live ? slen[cur * K + rank[n]] : 0)) out[p] = -1;
+  }
+  if (tid == 0) {
+    bool tied = ctl[kBcTieAny] != 0;
+    for (int n = 0; n + 1 < live && n < N; n++) tied |= fin[rank[n]] == fin[rank[n + 1]];
+    if (status) status[b] = tied ? 3 : 0;
+  }
+}
+
 /*
  * One CTA of kBeamThreads per utterance b.  emissions [B][T][C] of E; input_lens [B] (nullable: T); kind
  * GTNB_DENSE_CTC / _BIGRAM / _ASG; wt [C][C] (transposed W), wfirst [C] (BIGRAM sigma, ASG start weights) and wbad
  * [C] from beam_weights_kernel (unused for CTC); blank (CTC, BIGRAM); K beams, N hypotheses.  bp: [B][T][K] back-
- * pointers (scratch).  Out: tokens [B][N][T], lengths [B][N], scores [B][N], status [B] (nullable).
+ * pointers (scratch).  Out: tokens [B][N][T], lengths [B][N], scores [B][N], status [B] (nullable).  F: BeamNoLm, or
+ * BeamLm with the LM, its weights, token_beam and the am / lm outputs.
  */
-template <class E, class Hash>
+template <class E, class Hash, class F = BeamNoLm>
 __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     const E* __restrict__ emissions, int T, int C, const int32_t* __restrict__ input_lens, int kind,
     const float* __restrict__ wt, const float* __restrict__ wfirst, const int32_t* __restrict__ wbad, int blank, int K,
     int N, uint16_t* bp, int32_t* __restrict__ tokens, int32_t* __restrict__ lengths, float* __restrict__ scores,
-    int32_t* __restrict__ status) {
+    int32_t* __restrict__ status, const F fz = F()) {
   GTNB_DYNAMIC_SMEM(uint64_t, hsm);
   uint64_t* hh = hsm; // [2][K] hash of the transcript
   uint64_t* hq = hsm + 2 * K; // [2][K] hash of the transcript minus its last token
@@ -179,12 +295,20 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
   int* src = kslot + K; // [K] new slot -> candidate
   int* widx = src + K; // [K] winners: candidate
   uint32_t* wkey = reinterpret_cast<uint32_t*>(widx + K); // [K] winners: key
-  uint32_t* keys = wkey + K; // [K + K*C]: kept beams r at r, extension (s, c) at L + s*C + c
+  uint32_t* keys = wkey + K; // [K + K*P]: kept beams r at r, extension (s, p) at L + s*P + p
+  // (BeamLm only)
+  int* snode = reinterpret_cast<int*>(keys + K + K * C); // [2][K] LM node
+  float* slm = reinterpret_cast<float*>(snode + 2 * K); // [2][K] lmacc
+  int* ptok = reinterpret_cast<int*>(slm + 2 * K); // [P] the frame's tokens, ascending
+  int* ppos = ptok + C; // [C] token -> its position in ptok, or -1
+  int* wcnt = ppos + C; // [8] selected tokens per warp
+  const int P = F::on ? fz.P : C;
 
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int Tb = input_lens ? input_lens[b] : T;
   if (!(Tb >= 0 && Tb <= T)) {
     beam_flag(b, T, N, 2, tokens, lengths, scores, status);
+    if constexpr (F::on) beam_flag_lm(b, N, fz);
     return;
   }
   const E* em = emissions + (long long)b * T * C;
@@ -200,6 +324,16 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     slast[0] = -1;
     spar[0] = -1;
     hh[0] = hq[0] = 0;
+    if constexpr (F::on) {
+      snode[0] = fz.lmw ? fz.start : 0;
+      slm[0] = 0.0f;
+    }
+  }
+  if constexpr (F::on) {
+    if (tid < C) { // (every frame's selection when P < C)
+      ptok[tid] = tid;
+      ppos[tid] = tid;
+    }
   }
   __syncthreads();
   if (tid < C) {
@@ -223,6 +357,38 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     const float* wp = t == 0 ? w0 : wb;
     const float *pb0 = spb + cur * K, *pl0 = spl + cur * K, *tot0 = stot + cur * K;
     const int *len0 = slen + cur * K, *last0 = slast + cur * K, *par0 = spar + cur * K;
+    const int* node0 = snode + cur * K;
+    const float* lm0 = slm + cur * K;
+
+    if constexpr (F::on) {
+      // token pruning: the P best tokens of the frame (blank excluded for CTC and BIGRAM), ties to the lower token;
+      // a tie at the boundary between finite emissions flags the utterance
+      if (P < C) {
+        bool sel = false;
+        if (tid < C && (kind == GTNB_DENSE_ASG || tid != blank)) {
+          const float v = er[tid];
+          int gt = 0, eq = 0;
+          for (int j = 0; j < C; j++) {
+            const float x = er[j];
+            const bool ok = kind == GTNB_DENSE_ASG || j != blank;
+            gt += ok && x > v;
+            eq += ok && x == v && j < tid;
+          }
+          sel = gt + eq < P;
+          if (gt + eq == P && eq > 0 && v > neg_inf()) ctl[kBcTieAny] = 1;
+        }
+        const unsigned bal = __ballot_sync(0xffffffffu, sel);
+        if (lane == 0) wcnt[warp] = __popc(bal);
+        __syncthreads();
+        if (tid < C) {
+          int pos = __popc(bal & ((1u << lane) - 1u));
+          for (int w = 0; w < warp; w++) pos += wcnt[w];
+          ppos[tid] = sel ? pos : -1;
+          if (sel) ptok[pos] = tid;
+        }
+        __syncthreads();
+      }
+    }
 
     // candidates: kept beams, then every extension
     if (tid < L) {
@@ -240,46 +406,65 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       }
       kpb[tid] = nb;
       kpl[tid] = nl;
-      keys[tid] = beam_key(beam_lse2(nb, nl));
+      float v = beam_lse2(nb, nl);
+      if constexpr (F::on) v = beam_fuse(fz, v, lm0[tid], len0[tid]);
+      keys[tid] = beam_key(v);
       kslot[tid] = -1;
     }
     if (tid == 0) ctl[kBcNwin] = ctl[kBcDone] = 0;
-    const int next = L * C;
+    const int next = L * P;
     {
-      int s = tid / C, c = tid - s * C;
+      int s = tid / P, p = tid - s * P;
       for (int q = tid; q < next; q += kBeamThreads) {
+        const int c = F::on ? ptok[p] : p;
         float v = neg_inf();
-        if (kind == GTNB_DENSE_ASG || c != blank) {
-          const float pb = pb0[s], pl = pl0[s];
-          const int l = last0[s];
-          if (kind == GTNB_DENSE_CTC) {
-            v = (c == l ? pb : tot0[s]) + er[c];
-          } else {
-            const float from_pl = l >= 0 && (kind == GTNB_DENSE_ASG || c != l) ? pl + __ldg(wt + (long long)l * C + c)
-                                                                                 : neg_inf();
-            v = beam_lse2(pb + wp[c], from_pl) + er[c];
+        if constexpr (!F::on) {
+          if (kind == GTNB_DENSE_ASG || c != blank) {
+            const float pb = pb0[s], pl = pl0[s];
+            const int l = last0[s];
+            if (kind == GTNB_DENSE_CTC) {
+              v = (c == l ? pb : tot0[s]) + er[c];
+            } else {
+              const float from_pl = l >= 0 && (kind == GTNB_DENSE_ASG || c != l) ? pl + __ldg(wt + (long long)l * C + c)
+                                                                                   : neg_inf();
+              v = beam_lse2(pb + wp[c], from_pl) + er[c];
+            }
+          }
+        } else {
+          v = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
+          if (v > neg_inf() && fz.lmw) {
+            const float w = __ldg(fz.lmw + (long long)node0[s] * (C + 1) + c); // (one row per beam, via the L2)
+            v = w == neg_inf() ? w : beam_fuse(fz, v, lm0[s] + w, len0[s] + 1);
+          } else if (v > neg_inf()) {
+            v = beam_fuse(fz, v, lm0[s], len0[s] + 1);
           }
         }
         keys[L + q] = beam_key(v);
-        c += kBeamThreads;
-        while (c >= C) {
-          c -= C;
+        p += kBeamThreads;
+        while (p >= P) {
+          p -= P;
           s++;
         }
       }
     }
     __syncthreads();
 
-    // merge: extension (par[r], last[r]) is r's transcript
-    if (tid < L && par0[tid] >= 0) {
-      const int q = L + par0[tid] * C + last0[tid];
-      const float v = beam_key_float(keys[q]);
+    // merge: extension (par[r], last[r]) is r's transcript (absent when last[r] was pruned at this frame)
+    if (tid < L && par0[tid] >= 0 && (!F::on || ppos[last0[tid]] >= 0)) {
+      const int q = L + par0[tid] * P + (F::on ? ppos[last0[tid]] : last0[tid]);
+      float v = beam_key_float(keys[q]);
+      if constexpr (F::on) { // (the key holds the fused score: the acoustic one again)
+        const int s = par0[tid];
+        v = keys[q] ? beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], last0[tid])
+                    : neg_inf();
+      }
       keys[q] = 0u;
       kpl[tid] = beam_lse2(kpl[tid], v);
-      keys[tid] = beam_key(beam_lse2(kpb[tid], kpl[tid]));
+      v = beam_lse2(kpb[tid], kpl[tid]);
+      if constexpr (F::on) v = beam_fuse(fz, v, lm0[tid], len0[tid]);
+      keys[tid] = beam_key(v);
     }
     __syncthreads();
-
     // radix select of the K-th key among the nonzero keys
     const int ncand = L + next;
     uint32_t pre = 0u;
@@ -401,6 +586,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
         n += ki > k || (ki == k && widx[i] < j);
       }
       uint32_t code;
+      float am = 0.0f; // (BeamLm: the acoustic score; the key holds the fused one)
       if (j < L) {
         spb[nx * K + n] = kpb[j];
         spl[nx * K + n] = kpl[j];
@@ -408,19 +594,31 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
         slast[nx * K + n] = last0[j];
         hh[nx * K + n] = hh[cur * K + j];
         hq[nx * K + n] = hq[cur * K + j];
+        if constexpr (F::on) {
+          am = beam_lse2(kpb[j], kpl[j]);
+          snode[nx * K + n] = node0[j];
+          slm[nx * K + n] = lm0[j];
+        }
         kslot[j] = n;
         code = (uint32_t)j << 9;
       } else {
-        const int s = (j - L) / C, c = j - L - s * C;
+        const int s = (j - L) / P, p = j - L - s * P;
+        const int c = F::on ? ptok[p] : p;
+        if constexpr (F::on) {
+          am = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
+          const long long at = (long long)node0[s] * (C + 1) + c;
+          snode[nx * K + n] = fz.lmw ? __ldg(fz.lmd + at) : 0;
+          slm[nx * K + n] = fz.lmw ? lm0[s] + __ldg(fz.lmw + at) : lm0[s];
+        }
         spb[nx * K + n] = neg_inf();
-        spl[nx * K + n] = beam_key_float(k);
+        spl[nx * K + n] = F::on ? am : beam_key_float(k);
         slen[nx * K + n] = len0[s] + 1;
         slast[nx * K + n] = c;
         hh[nx * K + n] = Hash::combine(hh[cur * K + s], c);
         hq[nx * K + n] = hh[cur * K + s];
         code = ((uint32_t)s << 9) | 256u | (uint32_t)c;
       }
-      stot[nx * K + n] = beam_key_float(k);
+      stot[nx * K + n] = F::on ? am : beam_key_float(k);
       src[n] = j;
       bpu[(long long)t * K + n] = (uint16_t)code;
     }
@@ -431,7 +629,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       const int j = src[tid];
       int par = -1;
       if (j >= L) {
-        par = kslot[(j - L) / C];
+        par = kslot[(j - L) / P];
       } else if (par0[j] >= 0) {
         par = kslot[par0[j]];
       } else if (len0[j] >= 2) {
@@ -454,6 +652,12 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
 
   if (ctl[kBcBad]) {
     beam_flag(b, T, N, 1, tokens, lengths, scores, status);
+    if constexpr (F::on) beam_flag_lm(b, N, fz);
+    return;
+  }
+  if constexpr (F::on) {
+    beam_finish_lm(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, snode, slm, kpb, kpl, src, tokens, lengths, scores,
+                   status, fz);
     return;
   }
   const int L = ctl[kBcL];
@@ -498,11 +702,11 @@ int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions
 #define GTNB_BEAM_LAUNCH(E_)                                                                                  \
   {                                                                                                           \
     if (smem > 48 * 1024) {                                                                                   \
-      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash>);                   \
+      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash, BeamNoLm>);                   \
       if (rc__) return rc__;                                                                                  \
     }                                                                                                         \
     GTNB_LAUNCH(ctx, "beam_decode",                                                                           \
-                beam_decode_kernel<E_, BeamHash><<<B, kBeamThreads, smem, ctx->stream>>>(                     \
+                beam_decode_kernel<E_, BeamHash, BeamNoLm><<<B, kBeamThreads, smem, ctx->stream>>>(                     \
                     static_cast<const E_*>(emissions), T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, \
                     tokens, lengths, scores, status));                                                        \
   }
@@ -513,6 +717,34 @@ int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions
   else
     GTNB_BEAM_LAUNCH(float)
 #undef GTNB_BEAM_LAUNCH
+  return GTNB_OK;
+}
+
+int launch_beam_decode_lm(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
+                          const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
+                          int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
+                          int32_t* status, const BeamLmLaunch& lm) {
+  if (B <= 0) return GTNB_OK;
+  const long long smem = beam_lm_smem_bytes(K, C);
+  const BeamLm f{lm.P, lm.lmw, lm.lmd, lm.start, lm.lm_weight, lm.token_bonus, lm.am_scores, lm.lm_scores};
+#define GTNB_BEAM_LM_LAUNCH(E_)                                                                               \
+  {                                                                                                           \
+    if (smem > 48 * 1024) {                                                                                   \
+      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash, BeamLm>);           \
+      if (rc__) return rc__;                                                                                  \
+    }                                                                                                         \
+    GTNB_LAUNCH(ctx, "beam_decode_lm",                                                                        \
+                beam_decode_kernel<E_, BeamHash, BeamLm><<<B, kBeamThreads, smem, ctx->stream>>>(             \
+                    static_cast<const E_*>(emissions), T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, \
+                    tokens, lengths, scores, status, f));                                                     \
+  }
+  if (dtype == GTNB_BF16)
+    GTNB_BEAM_LM_LAUNCH(bf16_t)
+  else if (dtype == GTNB_F16)
+    GTNB_BEAM_LM_LAUNCH(f16_t)
+  else
+    GTNB_BEAM_LM_LAUNCH(float)
+#undef GTNB_BEAM_LM_LAUNCH
   return GTNB_OK;
 }
 

@@ -857,6 +857,123 @@ def asg_beam_decode(emissions, transitions, beam=16, nbest=1, input_lengths=None
     return _beam_decode("asg_beam_decode", emissions, transitions, input_lengths, capi.DENSE_ASG, beam, nbest, 0)
 
 
+class LanguageModel:
+    """A token n-gram LM prepared once for the fused beam decoders (ctc_lm_beam_decode, ngram_ctc_lm_beam_decode,
+    asg_lm_beam_decode): graph, a gtn_b200.gtn.Graph acceptor over the tokens [0, num_labels) with label num_labels
+    for end of sentence and epsilon arcs as backoff (failure) arcs, resolved on the host into a dense table and
+    uploaded to `device` (the current CUDA device by default) through gtnb_lm_create.  Its weights are baked in.  The
+    graph's conditions (one start node, at most one arc per node and label, at most one epsilon arc per node and no
+    cycle of them, no NaN or +inf weight) are in include/gtn_b200.h; a graph that breaks one raises a RuntimeError.
+
+    Creating one allocates and synchronises, so it raises while a stream is capturing: build it before capture, and
+    keep it alive as long as a captured CUDA graph that decodes with it."""
+
+    def __init__(self, graph, num_labels, device=None):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("LanguageModel: create it before capturing a CUDA graph (it allocates and "
+                               "synchronises)")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.num_labels = int(num_labels)
+        view, keep = _graph_view(graph)
+        self._g = _async_ctx(self.device, "LanguageModel")
+        h = C.c_void_p()
+        rc = capi.lib().gtnb_lm_create(self._g.h, C.byref(view), self.num_labels, C.byref(h))
+        del keep
+        if rc != 0:
+            raise RuntimeError("LanguageModel: %s" % capi.lib().gtnb_last_error(self._g.h).decode())
+        self.h = h
+
+    def __del__(self):
+        h = getattr(self, "h", None)
+        if h is not None and h.value:
+            capi.lib().gtnb_lm_destroy(self._g.h, h)
+            self.h = None
+
+
+class LMBeamDecode(NamedTuple):
+    """The fused beam decoders' results, device tensors: tokens [B, N, T] int32 (each transcript followed by -1),
+    lengths [B, N] int32, scores [B, N] float32 (am + lm_weight * lm + token_bonus * length), am_scores [B, N] float32
+    (the acoustic lower bound), lm_scores [B, N] float32 (the LM's score of the transcript, end weight included) and
+    status [B] int32"""
+    tokens: torch.Tensor
+    lengths: torch.Tensor
+    scores: torch.Tensor
+    am_scores: torch.Tensor
+    lm_scores: torch.Tensor
+    status: torch.Tensor
+
+
+@torch.no_grad()
+def _lm_beam_decode(name, emissions, transitions, lm, lm_weight, token_bonus, beam, nbest, token_beam, input_lengths,
+                    kind, blank):
+    """gtnb_beam_decode_lm_async on the current stream"""
+    assert emissions.is_cuda and emissions.dim() == 3
+    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    w = None
+    if kind != capi.DENSE_CTC:
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+        w = transitions.detach().contiguous()
+    assert lm is None or isinstance(lm, LanguageModel)
+    il = _decode_lengths(e, input_lengths)
+    dtype = _EMISSION_DTYPES[e.dtype]
+    P = Cn if token_beam is None else int(token_beam)
+    g = _async_ctx(e.device, name)
+    lib = capi.lib()
+    ws, nbytes = _workspace(g, e.device, lib.gtnb_beam_decode_lm_async_workspace, B, T, Cn, dtype, kind, int(beam),
+                            int(nbest), P)
+    tokens = torch.empty((B, nbest, T), dtype=torch.int32, device=e.device)
+    lengths = torch.empty((B, nbest), dtype=torch.int32, device=e.device)
+    scores = torch.empty((B, nbest), dtype=torch.float32, device=e.device)
+    am = torch.empty((B, nbest), dtype=torch.float32, device=e.device)
+    lms = torch.empty((B, nbest), dtype=torch.float32, device=e.device)
+    status = torch.empty(B, dtype=torch.int32, device=e.device)
+    g._check(lib.gtnb_beam_decode_lm_async(
+        g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, e.data_ptr(), dtype,
+        None if il is None else il.data_ptr(), kind, None if w is None else w.data_ptr(), int(blank), int(beam),
+        int(nbest), None if lm is None else lm.h, float(lm_weight), float(token_bonus), P, tokens.data_ptr(),
+        lengths.data_ptr(), scores.data_ptr(), am.data_ptr(), lms.data_ptr(), status.data_ptr(), ws.data_ptr(),
+        nbytes))
+    return LMBeamDecode(tokens, lengths, scores, am, lms, status)
+
+
+def ctc_lm_beam_decode(emissions, lm=None, lm_weight=1.0, token_bonus=0.0, beam=16, nbest=1, token_beam=None,
+                       input_lengths=None, blank=0):
+    """ctc_beam_decode with LM shallow fusion, an insertion bonus and per-frame token pruning, through
+    gtnb_beam_decode_lm_async on the current stream, without a host synchronisation (it may be captured in a CUDA
+    graph).  Beams are ranked by am + (lm_weight * lmacc + token_bonus * length), lmacc the LanguageModel's resolved
+    weights along the prefix; after the last frame each beam adds its end weight and the N-best are ranked by
+    scores = am + lm_weight * lm + token_bonus * length.
+
+    lm: a LanguageModel for C = emissions.shape[2] on the emissions' device, or None (no LM).  lm_weight >= 0 and
+    token_bonus finite.  token_beam P in [1, C] (None: C, no pruning): each frame extends beams by its P most likely
+    tokens only, blank excluded.  Returns an LMBeamDecode of device tensors; status as ctc_beam_decode's, where 3 also
+    covers equal emissions at the P-th token boundary and equal final scores.  With lm None, token_bonus 0 and
+    token_beam None, tokens, lengths, scores and status are those of ctc_beam_decode.
+    """
+    return _lm_beam_decode("ctc_lm_beam_decode", emissions, None, lm, lm_weight, token_bonus, beam, nbest, token_beam,
+                           input_lengths, capi.DENSE_CTC, blank)
+
+
+def ngram_ctc_lm_beam_decode(emissions, transitions, lm=None, lm_weight=1.0, token_bonus=0.0, beam=16, nbest=1,
+                             token_beam=None, input_lengths=None, blank=0):
+    """ctc_lm_beam_decode scored by ngram_ctc_loss's numerator, as ngram_ctc_beam_decode is ctc_beam_decode's"""
+    return _lm_beam_decode("ngram_ctc_lm_beam_decode", emissions, transitions, lm, lm_weight, token_bonus, beam, nbest,
+                           token_beam, input_lengths, capi.DENSE_BIGRAM, blank)
+
+
+def asg_lm_beam_decode(emissions, transitions, lm=None, lm_weight=1.0, token_bonus=0.0, beam=16, nbest=1,
+                       token_beam=None, input_lengths=None):
+    """ctc_lm_beam_decode scored by asg_loss's numerator, as asg_beam_decode is ctc_beam_decode's (every token may be
+    selected by token_beam: ASG has no blank)"""
+    return _lm_beam_decode("asg_lm_beam_decode", emissions, transitions, lm, lm_weight, token_bonus, beam, nbest,
+                           token_beam, input_lengths, capi.DENSE_ASG, 0)
+
+
 class EditDistance(NamedTuple):
     """edit_distance's results, device tensors of [B] int32 (alignments [B, N] / [B, M] int32, or None)"""
     distance: torch.Tensor

@@ -1425,8 +1425,8 @@ int gtnb_edit_distance_async(
  *         + (kind != GTNB_DENSE_CTC ? r(4 * (C*C + 16)) + 2 * r(4 * (C + 16)) : 0)   (transposed W, sigma, flags).
  *
  * Out of scope: beam search with a gtnb_transitions graph (sparse or backoff G: a prefix's state there is a
- * distribution over G's nodes, not two numbers), LM shallow fusion, lexicons and word-level search, and per-frame
- * token pruning.
+ * distribution over G's nodes, not two numbers), and lexicons and word-level search.  LM shallow fusion, an
+ * insertion bonus and per-frame token pruning are gtnb_beam_decode_lm_async's.
  */
 int gtnb_beam_decode_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, int beam, int nbest,
                                      size_t* bytes);
@@ -1447,6 +1447,91 @@ int gtnb_beam_decode_async(
     int32_t* tokens_dev, /* [B][nbest][T] */
     int32_t* lengths_dev, /* [B][nbest] */
     float* scores_dev, /* [B][nbest] */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/*
+ * A token n-gram LM prepared once for gtnb_beam_decode_lm_async.  lm is a gtn graph over the tokens that must be
+ *   - an acceptor (ilabel == olabel), labelled in [0, C] or GTNB_EPSILON; label C is end of sentence;
+ *   - with exactly one start node (node flags other than start are ignored);
+ *   - with at most one arc per (node, label) and at most one epsilon arc per node, and no cycle of epsilon arcs;
+ *   - free of NaN and +inf weights (a -inf weight is allowed and forbids its arc).
+ * Anything else is GTNB_ERR_INVALID_ARGUMENT.  Epsilon arcs are backoff (failure) arcs, as in ARPA: one is taken only
+ * when the node has no arc for the token, unlike the log-semiring sum over epsilon paths of
+ * gtnb_backoff_transitions_loss.  From node s, token c resolves to
+ *   - the arc of s labelled c, if s has one;
+ *   - otherwise the weight of s's epsilon arc plus the resolution of c from that arc's destination;
+ *   - -inf if neither exists.
+ * LM(y) is the sum of the resolved weights along y from the start node, plus the end weight of the node reached: the
+ * resolved weight of label C, or 0 for every node when the graph has no arc labelled C at all.  For an epsilon-free
+ * LM, LM(y) is forwardScore(compose(linear(y [+ C]), lm)).
+ * The handle holds the resolved table on the device, weight [S][C + 1] float32 and destination [S][C + 1] int32, built
+ * on the host in order of backoff depth and uploaded once.  Unlike gtnb_transitions it bakes the weights in:
+ * resolution sums backoff weights into the table, and a fusion LM is not trained.  Bounds: S * (C + 1) <= 2^25
+ * entries (256 MB) and C <= 256, else GTNB_ERR_UNSUPPORTED.  create allocates, uploads and synchronises: it is a
+ * set-up call and may not be captured.  A captured graph that decodes with the LM must not be replayed after
+ * gtnb_lm_destroy (ctx must be a context of the handle's device).
+ */
+typedef struct gtnb_lm gtnb_lm;
+int gtnb_lm_create(gtnb_ctx* ctx, const gtnb_graph_view* lm, int C, gtnb_lm** out);
+void gtnb_lm_destroy(gtnb_ctx* ctx, gtnb_lm* lm);
+
+/*
+ * gtnb_beam_decode_async with LM shallow fusion, an insertion bonus and per-frame token pruning, under its contract:
+ * the same parameters, kinds (CTC, BIGRAM, ASG), dtypes, tie rule, status codes, bounds and workspace formula
+ * (gtnb_beam_decode_lm_async_workspace returns gtnb_beam_decode_async_workspace's bytes); it only launches kernels
+ * and may be captured.  The LM acts on the transcript only, so it is independent of the kind.
+ *
+ * Each beam also carries its LM node and lmacc, the unweighted sum (float32) of its resolved LM weights.
+ *   - Ranking key: logsumexp(p_blank, p_label) + (lm_weight * lmacc + token_bonus * len), in that float32 order.  An
+ *     extension by c from node s adds the resolved w(s, c) to lmacc; a -inf weight forbids the move for any
+ *     lm_weight.  A merged extension has the same transcript, hence the same node and lmacc: only the acoustic states
+ *     log-add.
+ *   - After frame T_b - 1 each live beam adds its end weight; a beam whose end weight is -inf is dropped.  The N-best
+ *     are the top N live beams by the final fused score, ties to the earlier beam (the tie rule's order); status 3
+ *     also covers equal final scores between consecutive hypotheses.
+ *   - token_beam = P in [1, C]: at each frame extensions use only the P tokens of highest emission (blank excluded
+ *     for CTC and BIGRAM); kept moves (blank, repeat, stay) are never pruned.  Equal emissions at the P-th boundary go
+ *     to the lower token and, when finite, flag status 3.  P = C means no pruning.  When r's last token was pruned at
+ *     a frame, the extension (par[r], last[r]) is simply absent.  Scores stay lower bounds.
+ *   - lm NULL: every resolved weight and end weight is 0.
+ * Outputs: scores_dev [B][N] am + lm_weight * lm + token_bonus * len (float32, the order above);
+ * am_scores_dev [B][N] (nullable) the acoustic lower bound, as gtnb_beam_decode_async returns it; lm_scores_dev
+ * [B][N] (nullable) LM(y).  Each is -inf for unused hypotheses and NaN for status 1 and 2.  T_b = 0 gives the empty
+ * transcript with am 0 and lm the start node's end weight, or no hypothesis when that is -inf.
+ * Errors: lm_weight negative or not finite, token_bonus not finite, or an LM made on another device or for another C:
+ * GTNB_ERR_INVALID_ARGUMENT.  token_beam outside [1, C]: GTNB_ERR_UNSUPPORTED, like the other bounds.
+ * With lm NULL, token_bonus 0 and token_beam = C, tokens, lengths, scores and status are == gtnb_beam_decode_async's.
+ *
+ * Out of scope: lexicons and word-level search, LMs beyond the dense table, and C > 256 (which pruning makes
+ * possible later: the candidates are K * P, not K * C).
+ */
+int gtnb_beam_decode_lm_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, int beam, int nbest,
+                                        int token_beam, size_t* bytes);
+int gtnb_beam_decode_lm_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    int kind, /* GTNB_DENSE_CTC | GTNB_DENSE_BIGRAM | GTNB_DENSE_ASG */
+    const float* trans_w_dev, /* NULL, BIGRAM [C*C], ASG [C + C*C] */
+    int blank,
+    int beam,
+    int nbest,
+    const gtnb_lm* lm, /* or NULL */
+    float lm_weight,
+    float token_bonus,
+    int token_beam,
+    int32_t* tokens_dev, /* [B][nbest][T] */
+    int32_t* lengths_dev, /* [B][nbest] */
+    float* scores_dev, /* [B][nbest] */
+    float* am_scores_dev, /* [B][nbest] or NULL */
+    float* lm_scores_dev, /* [B][nbest] or NULL */
     int32_t* status_dev, /* [B] or NULL */
     void* workspace_dev,
     size_t workspace_bytes);
