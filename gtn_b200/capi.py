@@ -196,6 +196,12 @@ SYMBOLS = [
     ("gtnb_beam_decode_lm_async", C.c_int,
      [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp,
       C.c_float, C.c_float, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
+    ("gtnb_lexicon_create", C.c_int,
+     [_vp, C.c_int, _vp, C.c_int, C.c_int, _vp, _vp, _vp, C.POINTER(GraphView), C.POINTER(_vp)]),
+    ("gtnb_lexicon_destroy", None, [_vp, _vp]),
+    ("gtnb_beam_decode_lexicon_async", C.c_int,
+     [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp,
+      C.c_float, C.c_float, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
     ("gtnb_edit_distance_async", C.c_int,
      [_vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
       C.c_size_t]),

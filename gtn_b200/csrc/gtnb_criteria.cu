@@ -14,6 +14,7 @@
 #include <limits>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "gtnb_internal.h"
@@ -4112,8 +4113,10 @@ struct BeamLmArgs {
 
 /* gtnb_beam_decode_async's run: the back-pointers and (with transitions) the transposed weights, the start weights
  * and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued; with m, the
- * fused search of gtnb_beam_decode_lm_async (the same scratch) */
-int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const BeamLmArgs* m = nullptr) {
+ * fused search of gtnb_beam_decode_lm_async, with x the lexicon search of gtnb_beam_decode_lexicon_async (the same
+ * scratch) */
+int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const BeamLmArgs* m = nullptr,
+                   const BeamLexLaunch* x = nullptr) {
   uint16_t* bp = nullptr;
   float *wt = nullptr, *wfirst = nullptr;
   int32_t* wbad = nullptr;
@@ -4125,6 +4128,10 @@ int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const Bea
   }
   if (!launch) return GTNB_OK;
   if (a.kind != GTNB_DENSE_CTC) GTNB_TRY(launch_beam_weights(ctx, a.C, a.kind, a.trans_w, wt, wfirst, wbad));
+  if (x)
+    return launch_beam_decode_lex(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
+                                  a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
+                                  a.tokens, a.lengths, a.scores, a.status, *x);
   if (m) {
     const BeamLmLaunch f{m->token_beam, m->lm ? m->lm->w : nullptr, m->lm ? m->lm->d : nullptr,
                          m->lm ? m->lm->start : 0, m->lm_weight, m->token_bonus, m->am_scores, m->lm_scores};
@@ -4171,29 +4178,36 @@ namespace {
 constexpr long long kLmMaxEntries = 1ll << 25;
 
 /*
- * The checks of gtnb_lm_create and the resolution: w(s, c) is s's arc labelled c, else s's epsilon (backoff) arc's
- * weight plus the resolution of c from its destination, else -inf.  Nodes are resolved in order of backoff depth, so
- * a backoff destination's row is complete before the rows that back off to it.  Without any arc labelled C, every
- * end weight (column C) is 0.
+ * The graph checks of a backoff LM over the labels [0, L] (gtnb_lm_create: L = C; gtnb_lexicon_create's word LM:
+ * L = V), label L being end of sentence: one start node, an acceptor, no NaN or +inf weight, labels in [0, L] or
+ * epsilon, at most one arc per (node, label) and one epsilon arc per node, no cycle of epsilon arcs.  A graph of more
+ * than max_nodes nodes is GTNB_ERR_UNSUPPORTED (too_big).  Out: the start node, each node's epsilon (backoff) arc or -1
+ * and backoff depth (the number of epsilon arcs to a node without one), the emitting arcs sorted by (source, label),
+ * and whether any arc is labelled L.
  */
-int lm_resolve(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, int C, int* start,
-               std::vector<float>* w, std::vector<int32_t>* d) {
+struct LmGraph {
+  int start = -1;
+  std::vector<int32_t> eps, arcs;
+  std::vector<int> depth;
+  bool has_end = false;
+};
+
+int lm_check(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, int L, long long max_nodes,
+             const char* too_big, LmGraph* g) {
   if (validate_view(ctx, G)) return GTNB_ERR_INVALID_ARGUMENT;
   const int S = G.num_nodes;
   if (S < 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has no nodes");
-  if ((long long)S * (C + 1) > kLmMaxEntries)
-    return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": S * (C + 1) > 2^25 table entries");
-  *start = -1;
+  if (S > max_nodes) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + too_big);
+  g->start = -1;
   for (int s = 0; s < S; s++)
     if (G.node_flags[s] & 1) {
-      if (*start >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has more than one start node");
-      *start = s;
+      if (g->start >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has more than one start node");
+      g->start = s;
     }
-  if (*start < 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has no start node");
-  const long long n = (long long)S * (C + 1);
-  const float ninf = -std::numeric_limits<float>::infinity();
-  std::vector<int32_t> arc(n, -1), eps(S, -1);
-  bool has_end = false;
+  if (g->start < 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has no start node");
+  g->eps.assign(S, -1);
+  g->arcs.clear();
+  g->has_end = false;
   for (int a = 0; a < G.num_arcs; a++) {
     const int s = G.arc_src[a], l = G.arc_ilabel[a];
     const float x = G.weights ? G.weights[a] : 0.0f;
@@ -4201,18 +4215,27 @@ int lm_resolve(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, i
     if (x != x || x == std::numeric_limits<float>::infinity())
       return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM has a NaN or +inf weight");
     if (l == GTNB_EPSILON) {
-      if (eps[s] >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a node has two epsilon arcs");
-      eps[s] = a;
+      if (g->eps[s] >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a node has two epsilon arcs");
+      g->eps[s] = a;
       continue;
     }
-    if (l < 0 || l > C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": an LM label outside [0, C]");
-    int32_t& slot = arc[(long long)s * (C + 1) + l];
-    if (slot >= 0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a node has two arcs with one label");
-    slot = a;
-    has_end |= l == C;
+    if (l < 0 || l > L)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": an LM label outside [0, " + std::to_string(L) + "]");
+    g->arcs.push_back(a);
+    g->has_end |= l == L;
   }
-  // backoff depth: the number of epsilon arcs to a node without one (more than S means a cycle)
-  std::vector<int> depth(S, -1);
+  std::stable_sort(g->arcs.begin(), g->arcs.end(), [&](int32_t a, int32_t b) {
+    return G.arc_src[a] != G.arc_src[b] ? G.arc_src[a] < G.arc_src[b] : G.arc_ilabel[a] < G.arc_ilabel[b];
+  });
+  for (size_t i = 1; i < g->arcs.size(); i++) {
+    const int a = g->arcs[i - 1], b = g->arcs[i];
+    if (G.arc_src[a] == G.arc_src[b] && G.arc_ilabel[a] == G.arc_ilabel[b])
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a node has two arcs with one label");
+  }
+  // backoff depth (more than S epsilon arcs in a row means a cycle)
+  std::vector<int>& depth = g->depth;
+  const std::vector<int32_t>& eps = g->eps;
+  depth.assign(S, -1);
   for (int s = 0; s < S; s++) {
     int v = s, k = 0;
     while (depth[v] < 0 && eps[v] >= 0 && k <= S) {
@@ -4224,14 +4247,39 @@ int lm_resolve(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, i
     for (int u = s; u != v; u = G.arc_dst[eps[u]]) depth[u] = base + k--;
     if (depth[v] < 0) depth[v] = 0;
   }
-  std::vector<int> order(S);
-  for (int s = 0; s < S; s++) order[s] = s;
-  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return depth[a] < depth[b]; });
+  return GTNB_OK;
+}
+
+/* the nodes of a checked LM in order of backoff depth: a backoff destination comes before the nodes that back off
+ * to it */
+std::vector<int> lm_depth_order(const LmGraph& g) {
+  std::vector<int> order(g.depth.size());
+  for (size_t s = 0; s < order.size(); s++) order[s] = (int)s;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return g.depth[a] < g.depth[b]; });
+  return order;
+}
+
+/*
+ * gtnb_lm_create's resolution: w(s, c) is s's arc labelled c, else s's epsilon (backoff) arc's weight plus the
+ * resolution of c from its destination, else -inf.  Nodes are resolved in order of backoff depth, so a backoff
+ * destination's row is complete before the rows that back off to it.  Without any arc labelled C, every end weight
+ * (column C) is 0.
+ */
+int lm_resolve(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, int C, int* start,
+               std::vector<float>* w, std::vector<int32_t>* d) {
+  LmGraph g;
+  GTNB_TRY(lm_check(ctx, fn, G, C, kLmMaxEntries / (C + 1), ": S * (C + 1) > 2^25 table entries", &g));
+  *start = g.start;
+  const int S = G.num_nodes;
+  const long long n = (long long)S * (C + 1);
+  const float ninf = -std::numeric_limits<float>::infinity();
+  std::vector<int32_t> arc(n, -1);
+  for (int a : g.arcs) arc[(long long)G.arc_src[a] * (C + 1) + G.arc_ilabel[a]] = a;
   w->assign(n, ninf);
   d->assign(n, 0);
-  for (int s : order) {
+  for (int s : lm_depth_order(g)) {
     const long long row = (long long)s * (C + 1);
-    const int e = eps[s];
+    const int e = g.eps[s];
     const long long brow = e >= 0 ? (long long)G.arc_dst[e] * (C + 1) : -1;
     const float be = e >= 0 ? (G.weights ? G.weights[e] : 0.0f) : 0.0f;
     for (int c = 0; c <= C; c++) {
@@ -4244,7 +4292,7 @@ int lm_resolve(gtnb_ctx* ctx, const std::string& fn, const gtnb_graph_view& G, i
         (*d)[row + c] = (*d)[brow + c];
       }
     }
-    if (!has_end) (*w)[row + C] = 0.0f;
+    if (!g.has_end) (*w)[row + C] = 0.0f;
   }
   return GTNB_OK;
 }
@@ -4324,4 +4372,283 @@ extern "C" int gtnb_beam_decode_lm_async(
   const BeamLmArgs m{lm, lm_weight, token_bonus, token_beam, am_scores_dev, lm_scores_dev};
   return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
                        [&](bool launch) { return beam_async_run(ctx, a, launch, &m); });
+}
+
+/*
+ * The lexicon of gtnb_beam_decode_lexicon_async, prepared once, in one device allocation:
+ *   the token classes [C]; the trie, numbered breadth first so that each node's children are consecutive in token
+ *   order (the root is 0, its children 1, 2, ...): child masks [nodes][MW], first child, word id and smear [nodes];
+ *   the word LM: an open-addressing hash of its emitting arcs [H][2] (key node << 32 | word, all ones in an empty
+ *   slot; value destination << 32 | weight bits; H a power of two >= 2 * arcs, linear probing from the key times
+ *   hmul's top hbits bits), and each node's backoff weight, backoff destination and resolved end weight [S].
+ */
+struct gtnb_lexicon {
+  int device = 0, C = 0, V = 0, nodes = 0, S = 0, start = 0, hbits = 0, max_depth = 0;
+  unsigned long long hmul = 0;
+  std::vector<int32_t> cls;
+  std::vector<uint8_t> spelled; // [C] the token appears in a spelling
+  void* mem = nullptr;
+  int32_t *d_cls = nullptr, *d_first = nullptr, *d_word = nullptr, *d_bod = nullptr;
+  unsigned long long* d_hash = nullptr;
+  uint32_t* d_mask = nullptr;
+  float *d_smear = nullptr, *d_bow = nullptr, *d_endw = nullptr;
+  ~gtnb_lexicon() {
+    if (mem) cudaFree(mem);
+  }
+};
+
+namespace {
+
+constexpr int kLexMaxV = 1 << 20;
+constexpr int kLexMaxNodes = 1 << 24;
+constexpr long long kLexMaxLmArcs = 1ll << 26;
+constexpr unsigned long long kLexHashMul = 0x9e3779b97f4a7c15ull;
+
+/* the word LM's emitting arcs in the order lm_check sorted them, with a row start per node */
+struct WordLm {
+  const gtnb_graph_view* G = nullptr;
+  LmGraph g;
+  std::vector<long long> row; // [S + 1] into g.arcs
+  float weight(int a) const { return G->weights ? G->weights[a] : 0.0f; }
+  /* the arc of s labelled x, or -1 */
+  int arc(int s, int x) const {
+    long long lo = row[s], hi = row[s + 1];
+    while (lo < hi) {
+      const long long mid = (lo + hi) / 2;
+      const int l = G->arc_ilabel[g.arcs[mid]];
+      if (l == x) return g.arcs[mid];
+      if (l < x)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    return -1;
+  }
+  /* w(s, x) in float32, backoff weights added innermost first (gtnb_lm_create's order) */
+  float resolve(int s, int x) const {
+    std::vector<int> chain;
+    int v = s, a;
+    while ((a = arc(v, x)) < 0) {
+      const int e = g.eps[v];
+      if (e < 0) return -std::numeric_limits<float>::infinity();
+      chain.push_back(e);
+      v = G->arc_dst[e];
+    }
+    float w = weight(a);
+    for (size_t i = chain.size(); i-- > 0;) w = weight(chain[i]) + w;
+    return w;
+  }
+};
+
+} // namespace
+
+extern "C" int gtnb_lexicon_create(gtnb_ctx* ctx, int C, const int32_t* token_class, int V, int num_spellings,
+                                   const int32_t* spelling_offsets, const int32_t* spelling_tokens,
+                                   const int32_t* spelling_words, const gtnb_graph_view* word_lm,
+                                   gtnb_lexicon** out) {
+  const std::string fn = "gtnb_lexicon_create";
+  if (out) *out = nullptr;
+  if (!ctx || C <= 0 || V <= 0 || num_spellings < 0 || !token_class || !out ||
+      (num_spellings > 0 && (!spelling_offsets || !spelling_tokens || !spelling_words)))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (C > 256) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": C > 256");
+  if (V > kLexMaxV) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": V > 2^20 words");
+  std::unique_ptr<gtnb_lexicon> h(new gtnb_lexicon);
+  h->C = C;
+  h->V = V;
+  h->cls.assign(token_class, token_class + C);
+  h->spelled.assign(C, 0);
+  for (int c = 0; c < C; c++)
+    if (token_class[c] < 0 || token_class[c] > 2)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a token class outside {0, 1, 2}");
+  // the trie, first with children in insertion order
+  std::vector<std::vector<std::pair<int, int>>> kids(1);
+  std::vector<int32_t> wid(1, -1);
+  if (num_spellings > 0 && spelling_offsets[0] != 0)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": spelling_offsets[0] != 0");
+  for (int i = 0; i < num_spellings; i++) {
+    const int o0 = spelling_offsets[i], o1 = spelling_offsets[i + 1], w = spelling_words[i];
+    if (o1 <= o0) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": an empty spelling");
+    if (w < 0 || w >= V) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a word id outside [0, V)");
+    int n = 0;
+    for (int p = o0; p < o1; p++) {
+      const int c = spelling_tokens[p];
+      if (c < 0 || c >= C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a spelling token outside [0, C)");
+      if (token_class[c] == 1) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a separator in a spelling");
+      if (token_class[c] == 2 && p > o0)
+        return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": a word-start token after a spelling's first position");
+      h->spelled[c] = 1;
+      int next = -1;
+      for (const auto& k : kids[n])
+        if (k.first == c) next = k.second;
+      if (next < 0) {
+        if ((int)kids.size() >= kLexMaxNodes)
+          return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": the trie has more than 2^24 nodes");
+        next = (int)kids.size();
+        kids[n].push_back({c, next});
+        kids.emplace_back();
+        wid.push_back(-1);
+      }
+      n = next;
+    }
+    if (wid[n] >= 0 && wid[n] != w)
+      return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": two words share a spelling");
+    wid[n] = w;
+  }
+  // the word LM
+  WordLm lm;
+  if (word_lm) {
+    if ((long long)word_lm->num_arcs > kLexMaxLmArcs)
+      return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": the word LM has more than 2^26 arcs");
+    lm.G = word_lm;
+    GTNB_TRY(lm_check(ctx, fn, *word_lm, V, kLexMaxLmArcs, ": the word LM has more than 2^26 nodes", &lm.g));
+    const int S = word_lm->num_nodes;
+    lm.row.assign(S + 1, 0);
+    for (int a : lm.g.arcs) lm.row[word_lm->arc_src[a] + 1]++;
+    for (int s = 0; s < S; s++) lm.row[s + 1] += lm.row[s];
+    h->S = S;
+    h->start = lm.g.start;
+    for (int d : lm.g.depth) h->max_depth = std::max(h->max_depth, d);
+  }
+  // breadth-first numbering, each node's children in token order
+  const int nodes = (int)kids.size(), MW = (C + 31) / 32;
+  std::vector<int> bfs(1, 0), id(nodes, 0);
+  for (size_t q = 0; q < bfs.size(); q++) {
+    auto& k = kids[bfs[q]];
+    std::sort(k.begin(), k.end());
+    for (const auto& x : k) {
+      id[x.second] = (int)bfs.size();
+      bfs.push_back(x.second);
+    }
+  }
+  std::vector<uint32_t> mask((size_t)nodes * MW, 0u);
+  std::vector<int32_t> first(nodes, 0), word(nodes, -1);
+  std::vector<float> smear(nodes, -std::numeric_limits<float>::infinity());
+  for (int q = 0; q < nodes; q++) {
+    const int n = bfs[q];
+    word[q] = wid[n];
+    first[q] = kids[n].empty() ? 0 : id[kids[n][0].second];
+    for (const auto& x : kids[n]) mask[(size_t)q * MW + (x.first >> 5)] |= 1u << (x.first & 31);
+  }
+  // smear: the largest finite w(start, word) at or below each node (0 when none is, at the root, without an LM)
+  if (word_lm) {
+    for (int q = nodes - 1; q > 0; q--) {
+      float best = word[q] >= 0 ? lm.resolve(lm.g.start, word[q]) : -std::numeric_limits<float>::infinity();
+      const int n = bfs[q];
+      for (size_t i = 0; i < kids[n].size(); i++) best = std::max(best, smear[first[q] + i]);
+      smear[q] = best;
+    }
+  }
+  for (int q = 0; q < nodes; q++)
+    if (q == 0 || !(smear[q] > -std::numeric_limits<float>::infinity())) smear[q] = 0.0f;
+  // the word LM's arc hash, backoff arrays and end weights
+  std::vector<unsigned long long> hash;
+  std::vector<int32_t> bod;
+  std::vector<float> bow, endw;
+  if (word_lm) {
+    const int S = h->S;
+    long long n_emit = 0;
+    for (int a : lm.g.arcs) n_emit += word_lm->arc_ilabel[a] < V;
+    int hb = 1;
+    while ((1ll << hb) < 2 * n_emit) hb++;
+    h->hbits = hb;
+    h->hmul = kLexHashMul;
+    const long long H = 1ll << hb;
+    hash.assign(2 * H, 0ull);
+    for (long long i = 0; i < H; i++) hash[2 * i] = ~0ull;
+    for (int a : lm.g.arcs) {
+      const int x = word_lm->arc_ilabel[a];
+      if (x >= V) continue;
+      const unsigned long long key = ((unsigned long long)(unsigned)word_lm->arc_src[a] << 32) | (unsigned)x;
+      long long i = (long long)((key * h->hmul) >> (64 - hb));
+      while (hash[2 * i] != ~0ull) i = (i + 1) & (H - 1);
+      const float wt = lm.weight(a);
+      uint32_t bits;
+      std::memcpy(&bits, &wt, 4);
+      hash[2 * i] = key;
+      hash[2 * i + 1] = ((unsigned long long)(unsigned)word_lm->arc_dst[a] << 32) | bits;
+    }
+    bod.assign(S, -1);
+    bow.assign(S, 0.0f);
+    endw.assign(S, -std::numeric_limits<float>::infinity());
+    for (int s = 0; s < S; s++)
+      if (lm.g.eps[s] >= 0) {
+        bod[s] = word_lm->arc_dst[lm.g.eps[s]];
+        bow[s] = lm.weight(lm.g.eps[s]);
+      }
+    for (int s : lm_depth_order(lm.g)) {
+      const int a = lm.arc(s, V);
+      if (!lm.g.has_end)
+        endw[s] = 0.0f;
+      else if (a >= 0)
+        endw[s] = lm.weight(a);
+      else if (bod[s] >= 0)
+        endw[s] = bow[s] + endw[bod[s]];
+    }
+  }
+  // one device allocation: each array at a 256-byte boundary
+  auto r256 = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t b_cls = r256(4ull * C), b_mask = r256(4ull * nodes * MW), b_node = r256(4ull * nodes),
+               b_hash = r256(8ull * hash.size()), b_s = r256(4ull * bod.size());
+  const size_t total = b_cls + b_mask + 3 * b_node + b_hash + 3 * b_s;
+  h->device = ctx->device;
+  h->nodes = nodes;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  GTNB_CUDA(ctx, cudaMalloc(&h->mem, total));
+  unsigned char* m = static_cast<unsigned char*>(h->mem);
+  auto put = [&](auto** dst, const void* src, size_t bytes, size_t span) -> int {
+    *dst = reinterpret_cast<std::remove_pointer_t<decltype(dst)>>(m);
+    m += span;
+    if (bytes) GTNB_CUDA(ctx, cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
+    return GTNB_OK;
+  };
+  GTNB_TRY(put(&h->d_cls, h->cls.data(), 4ull * C, b_cls));
+  GTNB_TRY(put(&h->d_mask, mask.data(), 4ull * mask.size(), b_mask));
+  GTNB_TRY(put(&h->d_first, first.data(), 4ull * nodes, b_node));
+  GTNB_TRY(put(&h->d_word, word.data(), 4ull * nodes, b_node));
+  GTNB_TRY(put(&h->d_smear, smear.data(), 4ull * nodes, b_node));
+  if (word_lm) {
+    GTNB_TRY(put(&h->d_hash, hash.data(), 8ull * hash.size(), b_hash));
+    GTNB_TRY(put(&h->d_bow, bow.data(), 4ull * bow.size(), b_s));
+    GTNB_TRY(put(&h->d_bod, bod.data(), 4ull * bod.size(), b_s));
+    GTNB_TRY(put(&h->d_endw, endw.data(), 4ull * endw.size(), b_s));
+  }
+  GTNB_CUDA(ctx, cudaDeviceSynchronize()); // (set-up: the lexicon is on the device before any stream reads it)
+  *out = h.release();
+  return GTNB_OK;
+}
+
+extern "C" void gtnb_lexicon_destroy(gtnb_ctx* ctx, gtnb_lexicon* lex) {
+  if (!lex) return;
+  if (ctx) cudaSetDevice(lex->device);
+  delete lex; // (cudaFree waits for the device: no launch still reads the lexicon)
+}
+
+extern "C" int gtnb_beam_decode_lexicon_async(
+    gtnb_ctx* ctx, void* cuda_stream, int B, int T, int C, const void* emissions_dev, int dtype,
+    const int32_t* input_lens_dev, int kind, const float* trans_w_dev, int blank, int beam, int nbest,
+    const gtnb_lexicon* lexicon, float lm_weight, float word_bonus, int token_beam, int32_t* tokens_dev,
+    int32_t* lengths_dev, float* scores_dev, float* am_scores_dev, float* lm_scores_dev, int32_t* words_dev,
+    int32_t* word_counts_dev, int32_t* status_dev, void* workspace_dev, size_t workspace_bytes) {
+  const std::string fn = "gtnb_beam_decode_lexicon_async";
+  if (!ctx || B < 0 || T < 0 || C <= 0 || !lexicon ||
+      (B > 0 && ((T > 0 && !emissions_dev) || !tokens_dev || !lengths_dev || !scores_dev)) ||
+      (kind == GTNB_DENSE_CTC) != (trans_w_dev == nullptr))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!(lm_weight >= 0.0f && std::isfinite(lm_weight)) || !std::isfinite(word_bonus))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": lm_weight must be finite and >= 0, word_bonus finite");
+  if (lexicon->device != ctx->device)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the lexicon was made on another device");
+  if (lexicon->C != C) return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the lexicon was made for another C");
+  const BeamAsyncArgs a{B, T, C, dtype, emissions_dev, input_lens_dev, kind, trans_w_dev, blank, beam, nbest,
+                        tokens_dev, lengths_dev, scores_dev, status_dev};
+  GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
+  if (kind != GTNB_DENSE_ASG && (lexicon->spelled[blank] || lexicon->cls[blank] == 1))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the lexicon spells with the blank or makes it a separator");
+  const BeamLexLaunch x{token_beam, lexicon->start, lm_weight, word_bonus, am_scores_dev, lm_scores_dev,
+                        lexicon->d_cls, lexicon->d_mask, lexicon->d_first, lexicon->d_word, lexicon->d_smear,
+                        lexicon->d_hash, lexicon->hmul, lexicon->hbits, lexicon->d_bow, lexicon->d_bod,
+                        lexicon->d_endw, words_dev, word_counts_dev};
+  return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
+                       [&](bool launch) { return beam_async_run(ctx, a, launch, nullptr, &x); });
 }

@@ -33,6 +33,11 @@
  *   L + s*P + p, token ptok[p].  The LM row of a beam is read through the L2 like WT's; destination nodes, and the
  *   acoustic score of an extension (recomputed), only for the winners and the merges.  After the last frame each beam
  *   adds its end weight and the live ones are ranked again by the final fused score.
+ * - Lexicon and word LM (gtnb_beam_decode_lexicon_async).  Policy BeamLex: each slot also carries its trie node, word
+ *   count, child mask, first child, smear and, at a word end, the completion's word-LM weight and destination, looked
+ *   up once by the thread that writes the slot; admission is a bit test in shared memory and the key is
+ *   am + (lm_weight * (lmacc + smear) + word_bonus * words).  After the last frame a beam completes its pending word
+ *   (dropped inside one), adds its end weight, and the word ids are read off the traced tokens by walking the trie.
  */
 #include <cstdint>
 
@@ -64,19 +69,48 @@ inline long long beam_lm_smem_bytes(int K, int C) {
   return beam_smem_bytes(K, C) + 4ll * (4ll * K + 2ll * C + 8);
 }
 
-/* the policy of beam_decode_kernel: BeamNoLm for gtnb_beam_decode_async, BeamLm for gtnb_beam_decode_lm_async */
+/* beam_lex_smem_bytes: beam_lm_smem_bytes plus the lexicon state per slot (trie node, word count, word id, completion
+ * weight and LM destination, first child, smear: [2][K] each; the child mask [2][K][MW]), the root's mask [MW], the
+ * smear of the root's children [C] and the token classes [C]; MW = ceil(C / 32) */
+inline long long beam_lex_smem_bytes(int K, int C) {
+  const long long MW = (C + 31) / 32;
+  return beam_lm_smem_bytes(K, C) + 4ll * (14ll * K + 2ll * K * MW + MW + 2ll * C);
+}
+
+/* the policy of beam_decode_kernel: BeamNoLm for gtnb_beam_decode_async, BeamLm for gtnb_beam_decode_lm_async,
+ * BeamLex for gtnb_beam_decode_lexicon_async */
 struct BeamNoLm {
   static constexpr bool on = false;
+  static constexpr bool lex = false;
   static constexpr int P = 0; // (unused: every token)
 };
 struct BeamLm {
   static constexpr bool on = true;
+  static constexpr bool lex = false;
   int P; // token_beam: tokens per frame, P = C: all of them
   const float* lmw; // [S][C + 1] resolved LM weights (column C: end weights); NULL: no LM, every weight 0
   const int32_t* lmd; // [S][C + 1] destination nodes
   int start; // the LM's start node
   float lw, tb; // lm_weight, token_bonus
   float *am, *lm; // [B][N] nullable: acoustic and LM scores of the hypotheses
+};
+/* BeamLex: BeamLm's P, start (the word LM's start node), lw, tb (word_bonus), am and lm; lmw and lmd are NULL */
+struct BeamLex : BeamLm {
+  static constexpr bool lex = true;
+  const int32_t* cls; // [C] token classes: 0 in-word, 1 separator, 2 word-start
+  int MW; // ceil(C / 32)
+  const uint32_t* mask; // [nodes][MW] trie child masks (bit c: a child labelled c)
+  const int32_t* first; // [nodes] index of the first child (children numbered in token order)
+  const int32_t* word; // [nodes] word id spelled at the node, or -1
+  const float* smear; // [nodes] lookahead of the node
+  const unsigned long long* hash; // [H][2] word LM emitting arcs: key node << 32 | word (all ones: empty), value
+                                  // destination << 32 | weight bits
+  unsigned long long hmul; // multiplier of the arc hash (0: every key probes from slot 0)
+  int hbits; // log2 H
+  const float* bow; // [S] backoff weight of each LM node
+  const int32_t* bod; // [S] backoff destination, or -1
+  const float* endw; // [S] resolved end weights
+  int32_t *words, *counts; // [B][N][T] / [B][N] nullable: word ids and word counts of the hypotheses
 };
 
 /* the fused ranking key, in this float32 order (no contraction): am + (lw * lmacc + tb * len) */
@@ -89,6 +123,67 @@ __device__ __forceinline__ float beam_mul_rn(float a, float b) {
 }
 __device__ __forceinline__ float beam_fuse(const BeamLm& f, float am, float lmacc, int len) {
   return __fadd_rn(am, __fadd_rn(beam_mul_rn(f.lw, lmacc), beam_mul_rn(f.tb, (float)len)));
+}
+
+/* BeamLex's ranking key, in this float32 order (no contraction): am + (lw * (lmacc + smear) + tb * words) */
+__device__ __forceinline__ float beam_lex_fuse(const BeamLm& f, float am, float lmacc, float sm, int words) {
+  return __fadd_rn(am, __fadd_rn(beam_mul_rn(f.lw, __fadd_rn(lmacc, sm)), beam_mul_rn(f.tb, (float)words)));
+}
+
+/* the rank of child c among the children in mask m (the children below it) */
+__device__ __forceinline__ int lex_rank(const uint32_t* m, int c) {
+  int r = __popc(m[c >> 5] & ((1u << (c & 31)) - 1u));
+  for (int w = 0; w < (c >> 5); w++) r += __popc(m[w]);
+  return r;
+}
+__device__ __forceinline__ bool lex_has(const uint32_t* m, int c) { return (m[c >> 5] >> (c & 31)) & 1u; }
+
+/* the trie move of a slot at node n (word id wd or -1, first child fc, child mask m) by token c of class k; rm and
+ * rfc: the root's mask and first child.  -> the node reached, or -1 when forbidden; done: the move completes n's
+ * word first */
+__device__ __forceinline__ int lex_move(int k, int c, int n, int wd, int fc, const uint32_t* m, const uint32_t* rm,
+                                        int rfc, bool& done) {
+  done = false;
+  if (k == 0) return lex_has(m, c) ? fc + lex_rank(m, c) : -1;
+  if (n != 0 && wd < 0) return -1;
+  done = n != 0;
+  if (k == 1) return 0;
+  return lex_has(rm, c) ? rfc + lex_rank(rm, c) : -1;
+}
+
+/* w(s, x) of the word LM: the arc of s labelled x, else s's backoff weight plus w(backoff destination, x), added
+ * innermost first as gtnb_lm_create's table adds them; -inf (dst -1) when neither exists */
+__device__ float lex_resolve(const BeamLex& f, int s, int x, int& dst) {
+  dst = -1;
+  if (!f.hash) {
+    dst = 0;
+    return 0.0f;
+  }
+  const unsigned H = 1u << f.hbits;
+  int v = s, hops = 0;
+  float w = 0.0f;
+  for (;;) {
+    const unsigned long long key = ((unsigned long long)(unsigned)v << 32) | (unsigned)x;
+    unsigned i = (unsigned)((key * f.hmul) >> (64 - f.hbits));
+    unsigned long long k;
+    while ((k = __ldg(f.hash + 2 * i)) != key && k != ~0ull) i = (i + 1) & (H - 1);
+    if (k == key) {
+      const unsigned long long e = __ldg(f.hash + 2 * i + 1);
+      w = __int_as_float((int)(unsigned)e);
+      dst = (int)(e >> 32);
+      break;
+    }
+    const int nb = __ldg(f.bod + v);
+    if (nb < 0) return neg_inf();
+    v = nb;
+    hops++;
+  }
+  for (int h = hops - 1; h >= 0; h--) {
+    int u = s;
+    for (int j = 0; j < h; j++) u = __ldg(f.bod + u);
+    w = __fadd_rn(__ldg(f.bow + u), w);
+  }
+  return w;
 }
 
 /* control block words */
@@ -262,6 +357,96 @@ __device__ void beam_finish_lm(int b, int T, int Tb, int C, int K, int N, const 
   }
 }
 
+/* BeamLex: beam_flag_lm, and -1 word rows and counts */
+__device__ void beam_flag_lex(int b, int T, int N, const BeamLex& f) {
+  beam_flag_lm(b, N, f);
+  for (long long p = threadIdx.x; p < (long long)N * T; p += kBeamThreads)
+    if (f.words) f.words[(long long)b * N * T + p] = -1;
+  for (int n = threadIdx.x; n < N; n += kBeamThreads)
+    if (f.counts) f.counts[(long long)b * N + n] = -1;
+}
+
+/*
+ * BeamLex, after frame T_b - 1: every live slot at a word end completes its word, a slot inside a word is dropped;
+ * each adds its end weight (dropped at -inf) and the N-best are the top live beams by am + (lw * lm + tb * words),
+ * ties to the lower slot.  Each hypothesis's words are read off its traced tokens by walking the trie.  fin / lmf /
+ * nwd ([K]) hold each slot's final fused score, LM score and word count, rank ([K]) rank -> slot.
+ */
+__device__ void beam_finish_lex(int b, int T, int Tb, int K, int N, const uint16_t* bpu, int cur, int* ctl,
+                                const float* stot, const int* slen, const int* snode, const float* slm,
+                                const int* strie, const int* swn, const int* swd, const float* scw, const int* scd,
+                                const int* tcls, float* fin, float* lmf, int* nwd, int* rank, int32_t* tokens,
+                                int32_t* lengths, float* scores, int32_t* status, const BeamLex& f) {
+  const int tid = threadIdx.x;
+  const int L = ctl[kBcL];
+  if (tid < L) {
+    const int m = cur * K + tid;
+    float lm = slm[m];
+    int node = snode[m], nw = swn[m];
+    bool ok = true;
+    if (strie[m] != 0) {
+      ok = swd[m] >= 0 && scw[m] > neg_inf();
+      lm = __fadd_rn(lm, scw[m]);
+      node = scd[m];
+      nw++;
+    }
+    const float we = ok ? (f.endw ? __ldg(f.endw + node) : 0.0f) : neg_inf();
+    lm = __fadd_rn(lm, we);
+    fin[tid] = we == neg_inf() ? neg_inf() : beam_fuse(f, stot[m], lm, nw);
+    lmf[tid] = lm;
+    nwd[tid] = nw;
+  }
+  __syncthreads();
+  int live = 0;
+  for (int i = 0; i < L; i++) live += fin[i] > neg_inf();
+  if (tid < L && fin[tid] > neg_inf()) {
+    int r = 0;
+    for (int i = 0; i < L; i++) r += fin[i] > fin[tid] || (fin[i] == fin[tid] && i < tid);
+    rank[r] = tid;
+  }
+  __syncthreads();
+  int32_t* out = tokens + (long long)b * N * T;
+  int32_t* wout = f.words ? f.words + (long long)b * N * T : nullptr;
+  for (int n = tid; n < N; n += kBeamThreads) {
+    const int m = n < live ? rank[n] : -1;
+    const int len = m >= 0 ? slen[cur * K + m] : -1;
+    const long long o = (long long)b * N + n;
+    scores[o] = m >= 0 ? fin[m] : neg_inf();
+    if (f.am) f.am[o] = m >= 0 ? stot[cur * K + m] : neg_inf();
+    if (f.lm) f.lm[o] = m >= 0 ? lmf[m] : neg_inf();
+    if (f.counts) f.counts[o] = m >= 0 ? nwd[m] : -1;
+    lengths[o] = len;
+    int tt = Tb - 1, s = m;
+    for (int p = len - 1; p >= 0; p--) out[(long long)n * T + p] = beam_back(bpu, K, tt, s);
+    if (wout && len > 0) { // (the transcript was admitted: every move exists)
+      int node = 0, k = 0;
+      for (int p = 0; p < len; p++) {
+        const int c = out[(long long)n * T + p], cl = tcls[c];
+        if (cl != 0 && node != 0) wout[(long long)n * T + k++] = __ldg(f.word + node);
+        if (cl == 1) {
+          node = 0;
+        } else {
+          const int from = cl == 0 ? node : 0;
+          node = __ldg(f.first + from) + lex_rank(f.mask + (long long)from * f.MW, c);
+        }
+      }
+      if (node != 0) wout[(long long)n * T + k++] = __ldg(f.word + node);
+    }
+  }
+  __syncthreads();
+  for (long long p = tid; p < (long long)N * T; p += kBeamThreads) {
+    const int n = (int)(p / T);
+    const int r = n < live ? rank[n] : -1;
+    if (p - (long long)n * T >= (r >= 0 ? slen[cur * K + r] : 0)) out[p] = -1;
+    if (wout && p - (long long)n * T >= (r >= 0 ? nwd[r] : 0)) wout[p] = -1;
+  }
+  if (tid == 0) {
+    bool tied = ctl[kBcTieAny] != 0;
+    for (int n = 0; n + 1 < live && n < N; n++) tied |= fin[rank[n]] == fin[rank[n + 1]];
+    if (status) status[b] = tied ? 3 : 0;
+  }
+}
+
 /*
  * One CTA of kBeamThreads per utterance b.  emissions [B][T][C] of E; input_lens [B] (nullable: T); kind
  * GTNB_DENSE_CTC / _BIGRAM / _ASG; wt [C][C] (transposed W), wfirst [C] (BIGRAM sigma, ASG start weights) and wbad
@@ -302,13 +487,29 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
   int* ptok = reinterpret_cast<int*>(slm + 2 * K); // [P] the frame's tokens, ascending
   int* ppos = ptok + C; // [C] token -> its position in ptok, or -1
   int* wcnt = ppos + C; // [8] selected tokens per warp
+  // (BeamLex only)
+  const int MW = (C + 31) / 32;
+  int* strie = wcnt + 8; // [2][K] trie node (the root is 0, its children 1, 2, ... in token order)
+  int* swn = strie + 2 * K; // [2][K] word count
+  int* swd = swn + 2 * K; // [2][K] word id of the trie node, or -1
+  float* scw = reinterpret_cast<float*>(swd + 2 * K); // [2][K] completion weight w(LM node, word id), word ends
+  int* scd = reinterpret_cast<int*>(scw + 2 * K); // [2][K] ... and its LM destination
+  int* sfc = scd + 2 * K; // [2][K] first child
+  float* ssm = reinterpret_cast<float*>(sfc + 2 * K); // [2][K] smear
+  uint32_t* smask = reinterpret_cast<uint32_t*>(ssm + 2 * K); // [2][K][MW] child mask
+  uint32_t* rmask = smask + 2 * K * MW; // [MW] the root's child mask
+  float* rsm = reinterpret_cast<float*>(rmask + MW); // [C] smear of the root's child labelled c
+  int* tcls = reinterpret_cast<int*>(rsm + C); // [C] token classes
   const int P = F::on ? fz.P : C;
 
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int Tb = input_lens ? input_lens[b] : T;
   if (!(Tb >= 0 && Tb <= T)) {
     beam_flag(b, T, N, 2, tokens, lengths, scores, status);
-    if constexpr (F::on) beam_flag_lm(b, N, fz);
+    if constexpr (F::lex)
+      beam_flag_lex(b, T, N, fz);
+    else if constexpr (F::on)
+      beam_flag_lm(b, N, fz);
     return;
   }
   const E* em = emissions + (long long)b * T * C;
@@ -335,6 +536,20 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       ppos[tid] = tid;
     }
   }
+  if constexpr (F::lex) {
+    if (tid == 0) {
+      snode[0] = fz.start;
+      strie[0] = swn[0] = scd[0] = 0;
+      swd[0] = -1;
+      scw[0] = ssm[0] = 0.0f;
+      sfc[0] = __ldg(fz.first);
+    }
+    if (tid < MW) smask[tid] = rmask[tid] = __ldg(fz.mask + tid);
+    if (tid < C) {
+      tcls[tid] = __ldg(fz.cls + tid);
+      rsm[tid] = lex_has(fz.mask, tid) ? __ldg(fz.smear + 1 + lex_rank(fz.mask, tid)) : 0.0f;
+    }
+  }
   __syncthreads();
   if (tid < C) {
     w0[tid] = kind == GTNB_DENSE_CTC ? 0.0f : wfirst[tid];
@@ -359,6 +574,10 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     const int *len0 = slen + cur * K, *last0 = slast + cur * K, *par0 = spar + cur * K;
     const int* node0 = snode + cur * K;
     const float* lm0 = slm + cur * K;
+    const int *trie0 = strie + cur * K, *wn0 = swn + cur * K, *wd0 = swd + cur * K, *cd0 = scd + cur * K;
+    const int* fc0 = sfc + cur * K;
+    const float *cw0 = scw + cur * K, *sm0 = ssm + cur * K;
+    const uint32_t* mask0 = smask + cur * K * MW;
 
     if constexpr (F::on) {
       // token pruning: the P best tokens of the frame (blank excluded for CTC and BIGRAM), ties to the lower token;
@@ -407,7 +626,10 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       kpb[tid] = nb;
       kpl[tid] = nl;
       float v = beam_lse2(nb, nl);
-      if constexpr (F::on) v = beam_fuse(fz, v, lm0[tid], len0[tid]);
+      if constexpr (F::lex)
+        v = beam_lex_fuse(fz, v, lm0[tid], sm0[tid], wn0[tid]);
+      else if constexpr (F::on)
+        v = beam_fuse(fz, v, lm0[tid], len0[tid]);
       keys[tid] = beam_key(v);
       kslot[tid] = -1;
     }
@@ -428,6 +650,19 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
               const float from_pl = l >= 0 && (kind == GTNB_DENSE_ASG || c != l) ? pl + __ldg(wt + (long long)l * C + c)
                                                                                    : neg_inf();
               v = beam_lse2(pb + wp[c], from_pl) + er[c];
+            }
+          }
+        } else if constexpr (F::lex) {
+          v = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
+          if (v > neg_inf()) { // (admission is a bit test; an in-word child's smear is one row per beam, via the L2)
+            bool done;
+            const int k = tcls[c];
+            const int ch = lex_move(k, c, trie0[s], wd0[s], fc0[s], mask0 + s * MW, rmask, 1, done);
+            if (ch < 0 || (done && !(cw0[s] > neg_inf()))) {
+              v = neg_inf();
+            } else {
+              const float sm = k == 0 ? __ldg(fz.smear + ch) : k == 2 ? rsm[c] : 0.0f;
+              v = beam_lex_fuse(fz, v, done ? __fadd_rn(lm0[s], cw0[s]) : lm0[s], sm, wn0[s] + (int)done);
             }
           }
         } else {
@@ -461,7 +696,10 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       keys[q] = 0u;
       kpl[tid] = beam_lse2(kpl[tid], v);
       v = beam_lse2(kpb[tid], kpl[tid]);
-      if constexpr (F::on) v = beam_fuse(fz, v, lm0[tid], len0[tid]);
+      if constexpr (F::lex)
+        v = beam_lex_fuse(fz, v, lm0[tid], sm0[tid], wn0[tid]);
+      else if constexpr (F::on)
+        v = beam_fuse(fz, v, lm0[tid], len0[tid]);
       keys[tid] = beam_key(v);
     }
     __syncthreads();
@@ -599,12 +837,43 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
           snode[nx * K + n] = node0[j];
           slm[nx * K + n] = lm0[j];
         }
+        if constexpr (F::lex) {
+          const int o = nx * K + n;
+          strie[o] = trie0[j];
+          swn[o] = wn0[j];
+          swd[o] = wd0[j];
+          scw[o] = cw0[j];
+          scd[o] = cd0[j];
+          sfc[o] = fc0[j];
+          ssm[o] = sm0[j];
+          for (int w = 0; w < MW; w++) smask[o * MW + w] = mask0[j * MW + w];
+        }
         kslot[j] = n;
         code = (uint32_t)j << 9;
       } else {
         const int s = (j - L) / P, p = j - L - s * P;
         const int c = F::on ? ptok[p] : p;
-        if constexpr (F::on) {
+        if constexpr (F::lex) {
+          // the new slot's trie node and LM state; on a word end, the completion's weight and destination are looked
+          // up here, once, so that no LM lookup sits on the per-candidate path
+          am = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
+          bool done;
+          const int ch = lex_move(tcls[c], c, trie0[s], wd0[s], fc0[s], mask0 + s * MW, rmask, 1, done);
+          const int o = nx * K + n;
+          const int ln = done ? cd0[s] : node0[s];
+          snode[o] = ln;
+          slm[o] = done ? __fadd_rn(lm0[s], cw0[s]) : lm0[s];
+          swn[o] = wn0[s] + (int)done;
+          strie[o] = ch;
+          const int wd = __ldg(fz.word + ch);
+          swd[o] = wd;
+          sfc[o] = __ldg(fz.first + ch);
+          ssm[o] = __ldg(fz.smear + ch);
+          for (int w = 0; w < MW; w++) smask[o * MW + w] = __ldg(fz.mask + (long long)ch * MW + w);
+          int d = 0;
+          scw[o] = wd >= 0 ? lex_resolve(fz, ln, wd, d) : 0.0f;
+          scd[o] = d;
+        } else if constexpr (F::on) {
           am = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
           const long long at = (long long)node0[s] * (C + 1) + c;
           snode[nx * K + n] = fz.lmw ? __ldg(fz.lmd + at) : 0;
@@ -652,10 +921,17 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
 
   if (ctl[kBcBad]) {
     beam_flag(b, T, N, 1, tokens, lengths, scores, status);
-    if constexpr (F::on) beam_flag_lm(b, N, fz);
+    if constexpr (F::lex)
+      beam_flag_lex(b, T, N, fz);
+    else if constexpr (F::on)
+      beam_flag_lm(b, N, fz);
     return;
   }
-  if constexpr (F::on) {
+  if constexpr (F::lex) {
+    beam_finish_lex(b, T, Tb, K, N, bpu, cur, ctl, stot, slen, snode, slm, strie, swn, swd, scw, scd, tcls, kpb, kpl,
+                    widx, src, tokens, lengths, scores, status, fz);
+    return;
+  } else if constexpr (F::on) {
     beam_finish_lm(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, snode, slm, kpb, kpl, src, tokens, lengths, scores,
                    status, fz);
     return;
@@ -745,6 +1021,50 @@ int launch_beam_decode_lm(gtnb_ctx* ctx, int B, int T, int C, const void* emissi
   else
     GTNB_BEAM_LM_LAUNCH(float)
 #undef GTNB_BEAM_LM_LAUNCH
+  return GTNB_OK;
+}
+
+int launch_beam_decode_lex(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
+                           const int32_t* input_lens, int kind, const float* wt, const float* wfirst,
+                           const int32_t* wbad, int blank, int K, int N, uint16_t* bp, int32_t* tokens,
+                           int32_t* lengths, float* scores, int32_t* status, const BeamLexLaunch& x) {
+  if (B <= 0) return GTNB_OK;
+  const long long smem = beam_lex_smem_bytes(K, C);
+  BeamLex f;
+  static_cast<BeamLm&>(f) = BeamLm{x.P, nullptr, nullptr, x.start, x.lm_weight, x.word_bonus, x.am_scores,
+                                   x.lm_scores};
+  f.cls = x.cls;
+  f.MW = (C + 31) / 32;
+  f.mask = x.mask;
+  f.first = x.first;
+  f.word = x.word;
+  f.smear = x.smear;
+  f.hash = x.hash;
+  f.hmul = x.hmul;
+  f.hbits = x.hbits;
+  f.bow = x.bow;
+  f.bod = x.bod;
+  f.endw = x.endw;
+  f.words = x.words;
+  f.counts = x.counts;
+#define GTNB_BEAM_LEX_LAUNCH(E_)                                                                              \
+  {                                                                                                           \
+    if (smem > 48 * 1024) {                                                                                   \
+      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash, BeamLex>);          \
+      if (rc__) return rc__;                                                                                  \
+    }                                                                                                         \
+    GTNB_LAUNCH(ctx, "beam_decode_lexicon",                                                                   \
+                beam_decode_kernel<E_, BeamHash, BeamLex><<<B, kBeamThreads, smem, ctx->stream>>>(            \
+                    static_cast<const E_*>(emissions), T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, \
+                    tokens, lengths, scores, status, f));                                                     \
+  }
+  if (dtype == GTNB_BF16)
+    GTNB_BEAM_LEX_LAUNCH(bf16_t)
+  else if (dtype == GTNB_F16)
+    GTNB_BEAM_LEX_LAUNCH(f16_t)
+  else
+    GTNB_BEAM_LEX_LAUNCH(float)
+#undef GTNB_BEAM_LEX_LAUNCH
   return GTNB_OK;
 }
 

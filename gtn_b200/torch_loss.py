@@ -974,6 +974,217 @@ def asg_lm_beam_decode(emissions, transitions, lm=None, lm_weight=1.0, token_bon
                            token_beam, input_lengths, capi.DENSE_ASG, 0)
 
 
+class Lexicon:
+    """A lexicon with an optional word n-gram LM, prepared once for the lexicon beam decoders
+    (ctc_lexicon_beam_decode, ngram_ctc_lexicon_beam_decode, asg_lexicon_beam_decode) through gtnb_lexicon_create.
+
+    spellings: (tokens, word id) pairs, each a non-empty token sequence in [0, num_labels) spelling a word in
+    [0, num_words); a word may have several spellings, two words may not share one.  separator: a token that ends a word
+    and is in no spelling (wav2letter's "|"), or None.  word_start: tokens that end the current word and begin a new
+    spelling, allowed only at a spelling's position 0 (SentencePiece pieces with a leading space).  Every other token is
+    an in-word token.  lm: the word LM, a gtn_b200.gtn.Graph or a (graph dict, weights) pair as arpa_graph returns,
+    an acceptor over [0, num_words] with label num_words for end of sentence and epsilon arcs as backoff arcs (the
+    conditions of include/gtn_b200.h), or None (every weight 0).  A lexicon or LM that breaks a condition raises a
+    RuntimeError.
+
+    Creating one allocates and synchronises, so it raises while a stream is capturing: build it before capture, and
+    keep it alive as long as a captured CUDA graph that decodes with it."""
+
+    def __init__(self, spellings, num_labels, num_words, separator=None, word_start=(), lm=None, device=None):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("Lexicon: create it before capturing a CUDA graph (it allocates and synchronises)")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.num_labels, self.num_words = int(num_labels), int(num_words)
+        cls = np.zeros(self.num_labels, np.int32)
+        for c in word_start:
+            cls[int(c)] = 2
+        if separator is not None:
+            cls[int(separator)] = 1
+        toks, words, offs = [], [], [0]
+        for y, w in spellings:
+            toks.extend(int(c) for c in y)
+            offs.append(len(toks))
+            words.append(int(w))
+        toks = np.asarray(toks, np.int32)
+        offs = np.asarray(offs, np.int32)
+        words = np.asarray(words, np.int32)
+        view, keep = None, None
+        if lm is not None:
+            if isinstance(lm, tuple):
+                G, w = lm
+                view, keep = capi.make_view(G["flags"], G["src"], G["dst"], G["ilabel"], G.get("olabel", G["ilabel"]),
+                                            np.asarray(w, np.float32))
+            else:
+                view, keep = _graph_view(lm)
+        self._g = _async_ctx(self.device, "Lexicon")
+        h = C.c_void_p()
+        rc = capi.lib().gtnb_lexicon_create(self._g.h, self.num_labels, cls.ctypes.data, self.num_words, len(words),
+                                            offs.ctypes.data, toks.ctypes.data if len(toks) else None,
+                                            words.ctypes.data if len(words) else None,
+                                            None if view is None else C.byref(view), C.byref(h))
+        del keep
+        if rc != 0:
+            raise RuntimeError("Lexicon: %s" % capi.lib().gtnb_last_error(self._g.h).decode())
+        self.h = h
+
+    def __del__(self):
+        h = getattr(self, "h", None)
+        if h is not None and h.value:
+            capi.lib().gtnb_lexicon_destroy(self._g.h, h)
+            self.h = None
+
+
+class LexiconBeamDecode(NamedTuple):
+    """The lexicon beam decoders' results, device tensors: tokens [B, N, T] int32 (each transcript followed by -1),
+    lengths [B, N] int32, words [B, N, T] int32 (each hypothesis's word ids followed by -1), word_counts [B, N] int32,
+    scores [B, N] float32 (am + lm_weight * lm + word_bonus * word_count), am_scores [B, N] float32 (the acoustic lower
+    bound), lm_scores [B, N] float32 (the word LM's score of the words, end weight included) and status [B] int32.
+    words[:, 0] and word_counts[:, 0] go straight into edit_distance for a word error rate on the device."""
+    tokens: torch.Tensor
+    lengths: torch.Tensor
+    words: torch.Tensor
+    word_counts: torch.Tensor
+    scores: torch.Tensor
+    am_scores: torch.Tensor
+    lm_scores: torch.Tensor
+    status: torch.Tensor
+
+
+@torch.no_grad()
+def _lexicon_beam_decode(name, emissions, transitions, lexicon, lm_weight, word_bonus, beam, nbest, token_beam,
+                         input_lengths, kind, blank):
+    """gtnb_beam_decode_lexicon_async on the current stream"""
+    assert emissions.is_cuda and emissions.dim() == 3
+    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
+    e = emissions.contiguous()
+    B, T, Cn = e.shape
+    w = None
+    if kind != capi.DENSE_CTC:
+        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
+        assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+        w = transitions.detach().contiguous()
+    assert isinstance(lexicon, Lexicon)
+    il = _decode_lengths(e, input_lengths)
+    dtype = _EMISSION_DTYPES[e.dtype]
+    P = Cn if token_beam is None else int(token_beam)
+    g = _async_ctx(e.device, name)
+    lib = capi.lib()
+    ws, nbytes = _workspace(g, e.device, lib.gtnb_beam_decode_lm_async_workspace, B, T, Cn, dtype, kind, int(beam),
+                            int(nbest), P)
+    i32, f32 = dict(dtype=torch.int32, device=e.device), dict(dtype=torch.float32, device=e.device)
+    out = LexiconBeamDecode(torch.empty((B, nbest, T), **i32), torch.empty((B, nbest), **i32),
+                            torch.empty((B, nbest, T), **i32), torch.empty((B, nbest), **i32),
+                            torch.empty((B, nbest), **f32), torch.empty((B, nbest), **f32),
+                            torch.empty((B, nbest), **f32), torch.empty(B, **i32))
+    g._check(lib.gtnb_beam_decode_lexicon_async(
+        g.h, torch.cuda.current_stream(e.device).cuda_stream, B, T, Cn, e.data_ptr(), dtype,
+        None if il is None else il.data_ptr(), kind, None if w is None else w.data_ptr(), int(blank), int(beam),
+        int(nbest), lexicon.h, float(lm_weight), float(word_bonus), P, out.tokens.data_ptr(), out.lengths.data_ptr(),
+        out.scores.data_ptr(), out.am_scores.data_ptr(), out.lm_scores.data_ptr(), out.words.data_ptr(),
+        out.word_counts.data_ptr(), out.status.data_ptr(), ws.data_ptr(), nbytes))
+    return out
+
+
+def ctc_lexicon_beam_decode(emissions, lexicon, lm_weight=1.0, word_bonus=0.0, beam=16, nbest=1, token_beam=None,
+                            input_lengths=None, blank=0):
+    """ctc_lm_beam_decode constrained by a Lexicon and fused with its word LM, through gtnb_beam_decode_lexicon_async
+    on the current stream, without a host synchronisation (it may be captured in a CUDA graph).  Transcripts are
+    sequences of spelled words (with separators or word-start tokens between them, as the lexicon's token classes
+    say); beams are ranked by am + (lm_weight * (lmacc + smear) + word_bonus * words), lmacc the word LM's weights of
+    the completed words and smear the best unigram weight of a word the pending prefix can still become.  After the
+    last frame a beam completes its pending word (a beam inside a word is dropped), adds the end weight, and the
+    N-best are ranked by scores = am + lm_weight * lm + word_bonus * words.
+
+    lexicon: a Lexicon for C = emissions.shape[2] on the emissions' device; it may not spell with the blank or make it
+    the separator.  lm_weight >= 0 and word_bonus finite; token_beam P in [1, C] (None: C).  Returns a
+    LexiconBeamDecode of device tensors; status as ctc_lm_beam_decode's.  Hypotheses are distinct token transcripts,
+    so two of them may spell the same words."""
+    return _lexicon_beam_decode("ctc_lexicon_beam_decode", emissions, None, lexicon, lm_weight, word_bonus, beam, nbest,
+                                token_beam, input_lengths, capi.DENSE_CTC, blank)
+
+
+def ngram_ctc_lexicon_beam_decode(emissions, transitions, lexicon, lm_weight=1.0, word_bonus=0.0, beam=16, nbest=1,
+                                  token_beam=None, input_lengths=None, blank=0):
+    """ctc_lexicon_beam_decode scored by ngram_ctc_loss's numerator, as ngram_ctc_beam_decode is ctc_beam_decode's"""
+    return _lexicon_beam_decode("ngram_ctc_lexicon_beam_decode", emissions, transitions, lexicon, lm_weight,
+                                word_bonus, beam, nbest, token_beam, input_lengths, capi.DENSE_BIGRAM, blank)
+
+
+def asg_lexicon_beam_decode(emissions, transitions, lexicon, lm_weight=1.0, word_bonus=0.0, beam=16, nbest=1,
+                            token_beam=None, input_lengths=None):
+    """ctc_lexicon_beam_decode scored by asg_loss's numerator, as asg_beam_decode is ctc_beam_decode's"""
+    return _lexicon_beam_decode("asg_lexicon_beam_decode", emissions, transitions, lexicon, lm_weight, word_bonus,
+                                beam, nbest, token_beam, input_lengths, capi.DENSE_ASG, 0)
+
+
+def arpa_graph(path_or_lines, words):
+    """An ARPA n-gram LM as the backoff graph Lexicon takes -> (graph dict of int32 / uint8 numpy arrays flags, src,
+    dst, ilabel, olabel; float32 weights).
+
+    words: the vocabulary, a list (word id = position) or a dict word -> id; V = its size.  Nodes are the histories:
+    every n-gram of order < the LM's order that the file lists (with "<s>" as a history only), and the empty history.
+    The start node is the history "<s>" (the empty history when the file has no "<s>" unigram).  An n-gram
+    (h, x) with probability p becomes an arc from node h labelled x (V for "</s>") weighted ln p, to the longest
+    suffix of h + x that is a node; an n-gram's backoff weight b becomes an epsilon arc from its node to the node of
+    its history minus the oldest word, weighted ln b (ln 1 when the file lists none).  log10 values are converted to natural logs.  n-grams naming a
+    word outside the vocabulary (other than "<s>" and "</s>") are dropped, and "<s>" is never a label."""
+    if isinstance(path_or_lines, str):
+        with open(path_or_lines, encoding="utf-8") as f:
+            lines = f.read().splitlines()
+    else:
+        lines = list(path_or_lines)
+    vocab = dict(words) if isinstance(words, dict) else {w: i for i, w in enumerate(words)}
+    V = len(vocab)
+    ln10 = float(np.log(10.0))
+    grams = {}  # tuple of words -> (log10 p, log10 backoff or None)
+    order = 0
+    for line in lines:
+        line = line.strip()
+        if not line or line.startswith("\\") or line.startswith("ngram "):
+            if line.startswith("\\") and line.endswith("-grams:"):
+                order = int(line[1:line.index("-")])
+            continue
+        if order == 0:
+            continue
+        parts = line.split()
+        if len(parts) < 1 + order:
+            continue
+        ng = tuple(parts[1:1 + order])
+        if any(w not in vocab and w not in ("<s>", "</s>") for w in ng):
+            continue
+        bo = float(parts[1 + order]) if len(parts) > 1 + order else None
+        grams[ng] = (float(parts[0]), bo)
+    max_order = max((len(g) for g in grams), default=1)
+    hist = {(): 0}
+    for g in sorted(grams, key=len):
+        if len(g) < max_order and g[-1] != "</s>" and g not in hist:
+            hist[g] = len(hist)
+    S = len(hist)
+    src, dst, lab, w = [], [], [], []
+
+    def node_of(h):
+        while h not in hist:
+            h = h[1:]
+        return hist[h]
+    for g, (lp, bo) in grams.items():
+        if g[-1] != "<s>":
+            h = g[:-1]
+            if h in hist:
+                x = V if g[-1] == "</s>" else vocab[g[-1]]
+                src.append(hist[h]), lab.append(x), w.append(lp * ln10), dst.append(node_of(g))
+    for g, s in hist.items():  # (a history without a listed backoff weight backs off with weight 1)
+        if g:
+            bo = grams.get(g, (0.0, None))[1]
+            src.append(s), lab.append(-1), w.append((bo or 0.0) * ln10), dst.append(node_of(g[1:]))
+    flags = np.full(S, 2, np.uint8)
+    flags[hist.get(("<s>",), 0)] |= 1
+    lab = np.asarray(lab, np.int32)
+    return (dict(flags=flags, src=np.asarray(src, np.int32), dst=np.asarray(dst, np.int32), ilabel=lab,
+                 olabel=lab.copy()), np.asarray(w, np.float32))
+
+
 class EditDistance(NamedTuple):
     """edit_distance's results, device tensors of [B] int32 (alignments [B, N] / [B, M] int32, or None)"""
     distance: torch.Tensor

@@ -1504,8 +1504,8 @@ void gtnb_lm_destroy(gtnb_ctx* ctx, gtnb_lm* lm);
  * GTNB_ERR_INVALID_ARGUMENT.  token_beam outside [1, C]: GTNB_ERR_UNSUPPORTED, like the other bounds.
  * With lm NULL, token_bonus 0 and token_beam = C, tokens, lengths, scores and status are == gtnb_beam_decode_async's.
  *
- * Out of scope: lexicons and word-level search, LMs beyond the dense table, and C > 256 (which pruning makes
- * possible later: the candidates are K * P, not K * C).
+ * Out of scope: C > 256 (which pruning makes possible later: the candidates are K * P, not K * C).  Lexicons,
+ * word-level search and word LMs beyond the dense table are gtnb_beam_decode_lexicon_async's.
  */
 int gtnb_beam_decode_lm_async_workspace(gtnb_ctx* ctx, int B, int T, int C, int dtype, int kind, int beam, int nbest,
                                         int token_beam, size_t* bytes);
@@ -1532,6 +1532,104 @@ int gtnb_beam_decode_lm_async(
     float* scores_dev, /* [B][nbest] */
     float* am_scores_dev, /* [B][nbest] or NULL */
     float* lm_scores_dev, /* [B][nbest] or NULL */
+    int32_t* status_dev, /* [B] or NULL */
+    void* workspace_dev,
+    size_t workspace_bytes);
+
+/*
+ * A lexicon with an optional word n-gram LM, prepared once for gtnb_beam_decode_lexicon_async.
+ *   - token_class[c], c in [0, C): 0 an in-word token; 1 a separator (such as wav2letter's "|"), which ends the current
+ *     word and belongs to no spelling; 2 a word-start token (such as a SentencePiece piece with a leading space), which
+ *     ends the current word and begins a new spelling.
+ *   - num_spellings spellings: spelling i is spelling_tokens[spelling_offsets[i] .. spelling_offsets[i + 1]), a
+ *     non-empty token sequence, and spells word spelling_words[i] in [0, V).  A word may have several spellings; two
+ *     words may not share one (no homophones).  A separator may not appear in a spelling, a word-start token only at
+ *     its position 0.
+ *   - word_lm (nullable): gtnb_lm_create's graph contract over the labels [0, V], label V being end of sentence: an
+ *     acceptor with one start node, at most one arc per (node, label), at most one epsilon (backoff) arc per node, no
+ *     cycle of epsilon arcs, no NaN or +inf weight.  w(s, x) is the arc of s labelled x if there is one, else s's
+ *     backoff weight plus w(backoff destination, x), added innermost first as gtnb_lm_create's table adds them, else
+ *     -inf.  A node's end weight is w(s, V), or 0 for every node when the graph has no arc labelled V.  NULL: every
+ *     weight is 0.
+ *   - Lookahead: smear(n) is the largest finite w(start, word) over the words spelled at or below trie node n; 0 when
+ *     none is finite, at the root, and without a word LM (flashlight's max-unigram smearing).  It only steers the
+ *     search: returned scores never include it.
+ * Breaking any of these rules, a token outside [0, C) or an empty spelling is GTNB_ERR_INVALID_ARGUMENT.
+ * Bounds: C <= 256, V <= 2^20 words, a trie of at most 2^24 nodes (the root and one per distinct spelling prefix), a
+ * word LM of at most 2^26 arcs and 2^26 nodes; beyond them GTNB_ERR_UNSUPPORTED.
+ * Device bytes, each term rounded up to 256: 4C (classes) + 4 * nodes * ceil(C / 32) (child masks) + 3 * 4 * nodes
+ * (first child, word id, smear) and, with a word LM of S nodes and A arcs of labels below V, 16H (an open-addressing
+ * hash of those arcs, H the least power of two >= max(2, 2A)) + 3 * 4S (backoff weight and destination, end weight).
+ * create allocates, uploads and synchronises: it is a set-up call and may not be captured.  A captured graph that
+ * decodes with the lexicon must not be replayed after gtnb_lexicon_destroy (ctx must be a context of its device).
+ */
+typedef struct gtnb_lexicon gtnb_lexicon;
+int gtnb_lexicon_create(gtnb_ctx* ctx, int C, const int32_t* token_class /* [C] */, int V, int num_spellings,
+                        const int32_t* spelling_offsets /* [num_spellings + 1] */, const int32_t* spelling_tokens,
+                        const int32_t* spelling_words /* [num_spellings] */,
+                        const gtnb_graph_view* word_lm /* or NULL */, gtnb_lexicon** out);
+void gtnb_lexicon_destroy(gtnb_ctx* ctx, gtnb_lexicon* lexicon);
+
+/*
+ * Lexicon-constrained prefix beam search with a word LM: gtnb_beam_decode_lm_async under its contract (parameters,
+ * kinds CTC, BIGRAM and ASG, dtypes, tie rule, status codes, token_beam P, bounds, workspace: size it with
+ * gtnb_beam_decode_lm_async_workspace), with lexicon in place of the LM and word_bonus in place of token_bonus.  It
+ * only launches kernels and may be captured.
+ *
+ * Each beam also carries a trie node (the root: no pending word), a word-LM node, lmacc (the float32 sum of its
+ * completed words' w) and its word count, all functions of the transcript, so a merged extension stays exact.
+ *   - Extending a beam at trie node n by token c: an in-word c moves to n's child labelled c, and is forbidden
+ *     without one.  A separator changes nothing at the root; at a word end it completes the word and returns to the
+ *     root; anywhere else it is forbidden.  A word-start c, at the root or at a word end (completing that word first),
+ *     moves to the root's child labelled c; it is forbidden without that child or when n is neither.  Completing word
+ *     x adds w(LM node, x) to lmacc, moves the LM node and adds 1 to the word count; a -inf weight forbids the move.
+ *     Kept moves (blank, repeat, stay) change none of this.
+ *   - Ranking key: am + (lm_weight * (lmacc + smear(n)) + word_bonus * words), each operation rounded to float32 in
+ *     that order.
+ *   - After frame T_b - 1 each beam at a word end completes its word; a beam still inside a word is dropped.  Each
+ *     survivor adds its LM node's end weight (dropped at -inf) and the N-best are ranked by
+ *     am + (lm_weight * lm + word_bonus * words), ties to the earlier beam.  T_b = 0 gives the empty transcript, with
+ *     no words and lm the start node's end weight (no hypothesis when that is -inf).
+ * Outputs: as gtnb_beam_decode_lm_async (scores, am_scores, lm_scores: lm = the word LM's score of the words,
+ * end weight included), plus words_dev [B][N][T] (nullable): each hypothesis's word ids followed by -1, read off its
+ * tokens by walking the trie; word_counts_dev [B][N] (nullable), -1 for unused hypotheses and status 1 and 2.
+ * Hypotheses are distinct token transcripts: two of them may spell the same words (with and without a leading
+ * separator, say).
+ * Errors: lm_weight negative or not finite, word_bonus not finite, lexicon NULL or made on another device or for
+ * another C, or (CTC, BIGRAM) a lexicon that spells with the blank or makes it a separator:
+ * GTNB_ERR_INVALID_ARGUMENT.  token_beam outside [1, C]: GTNB_ERR_UNSUPPORTED.
+ * Identity: with the identity lexicon (every non-blank token, every token for ASG, a word-start token spelling itself
+ * as the word of the same id), no word LM, word_bonus 0 and token_beam = C, tokens, lengths, scores and status are
+ * == gtnb_beam_decode_async's.
+ *
+ * Out of scope: unknown words, a separator score, homophones, lookahead beyond max-unigram smearing, a token LM with
+ * the lexicon, C > 256, and merging hypotheses by state instead of by transcript.
+ */
+int gtnb_beam_decode_lexicon_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    int B,
+    int T,
+    int C,
+    const void* emissions_dev, /* [B][T][C] of dtype */
+    int dtype,
+    const int32_t* input_lens_dev, /* [B] or NULL */
+    int kind, /* GTNB_DENSE_CTC | GTNB_DENSE_BIGRAM | GTNB_DENSE_ASG */
+    const float* trans_w_dev, /* NULL, BIGRAM [C*C], ASG [C + C*C] */
+    int blank,
+    int beam,
+    int nbest,
+    const gtnb_lexicon* lexicon,
+    float lm_weight,
+    float word_bonus,
+    int token_beam,
+    int32_t* tokens_dev, /* [B][nbest][T] */
+    int32_t* lengths_dev, /* [B][nbest] */
+    float* scores_dev, /* [B][nbest] */
+    float* am_scores_dev, /* [B][nbest] or NULL */
+    float* lm_scores_dev, /* [B][nbest] or NULL */
+    int32_t* words_dev, /* [B][nbest][T] or NULL */
+    int32_t* word_counts_dev, /* [B][nbest] or NULL */
     int32_t* status_dev, /* [B] or NULL */
     void* workspace_dev,
     size_t workspace_bytes);
