@@ -84,7 +84,7 @@ SYMBOLS = [
     ("gtnb_forward", C.c_int, [_vp, _vp, C.c_int, _f32p, _i32p]),
     ("gtnb_backward", C.c_int, [_vp, _vp, C.c_int, _f32p]),
     ("gtnb_lattice_arc_grads", C.c_int, [_vp, _vp, C.c_int, _f32p]),
-    ("gtnb_lattice_arc_grads_dev", _vp, [_vp]),
+    ("gtnb_lattice_arc_grads_dev", _vp, [_vp, _vp]),
     ("gtnb_lattice_set_arc_grads", C.c_int, [_vp, _vp, C.c_int, _f32p]),
     ("gtnb_compose_grad", C.c_int, [_vp, _vp, _vp, _vp, C.c_int64]),
     ("gtnb_viterbi_path", C.c_int, [_vp, _vp, C.c_int, _i32p, _i32p, _i32p, _f32p, _i32p, _i32p]),
@@ -823,6 +823,14 @@ class Lattice:
         out = np.zeros(max(num_arcs, 1), np.float32)
         self.ctx._check(lib().gtnb_lattice_arc_grads(self.ctx.h, self.h, b, _p(out, _f32p)))
         return out[:num_arcs]
+
+    def set_arc_grads(self, b, grads):
+        g = np.ascontiguousarray(grads, np.float32)
+        self.ctx._check(lib().gtnb_lattice_set_arc_grads(self.ctx.h, self.h, b, _p(g, _f32p)))
+
+    def arc_grads_dev(self):
+        """device address of every entry's arc gradients, in download order (0: error or no backward yet)"""
+        return lib().gtnb_lattice_arc_grads_dev(self.ctx.h, self.h) or 0
 
     def compose_grad(self, grad_graph_dev=None, grad_emissions_dev=None, grad_stride=0):
         self.ctx._check(lib().gtnb_compose_grad(

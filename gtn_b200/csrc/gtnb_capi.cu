@@ -961,6 +961,18 @@ int gtnb_lattice_sizes(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* num_nodes, int
   return GTNB_OK;
 }
 
+/* exact_ties: a composed lattice's rows are put in the reference's relaxation order (k_order.cu) before the first
+ * call that hands out arc ids or per-arc values -- download, arc gradients in or out, a Viterbi path -- so that every
+ * such call sees one numbering whatever ran before it.  forward and backward work in either order (the sort
+ * carries arc_grad), so a lattice whose arcs never cross the ABI is never sorted.  Runs at most once. */
+static int settle_order(gtnb_ctx* ctx, gtnb_lattice* lat) {
+  if (!lat->order_pending) return GTNB_OK;
+  int rc = launch_relax_order(ctx, lat);
+  if (rc) return rc;
+  lat->order_pending = false;
+  return GTNB_OK;
+}
+
 int gtnb_lattice_download(
     gtnb_ctx* ctx, gtnb_lattice* lat, int b, uint8_t* node_flags, int32_t* arc_src,
     int32_t* arc_dst, int32_t* arc_ilabel, int32_t* arc_olabel, float* weights,
@@ -969,11 +981,7 @@ int gtnb_lattice_download(
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_lattice_download: bad arguments");
   int rc = fetch_sizes(ctx, lat);
   if (rc) return rc;
-  if (lat->order_pending && !lat->order_locked) { // hand the arcs out in the reference's order
-    if ((rc = launch_relax_order(ctx, lat))) return rc;
-    lat->order_pending = false;
-  }
-  lat->order_locked = true;
+  if ((rc = settle_order(ctx, lat))) return rc;
   const GraphMeta& m = lat->meta_h[b];
   std::vector<uint32_t> rp(m.N + 1);
   std::vector<int32_t> src(std::max(m.A, 1)), gg(std::max(m.A, 1), -1), gl(std::max(m.A, 1), -1);
@@ -1078,7 +1086,6 @@ int gtnb_backward(gtnb_ctx* ctx, gtnb_lattice* lat, int tropical, const float* d
   if (!lat->forward_done || lat->forward_mode != (tropical ? MODE_TROPICAL : MODE_LOG))
     return fail(ctx, GTNB_ERR_LOGIC, "gtnb_backward: no matching gtnb_forward on this lattice");
   GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
-  lat->order_locked = true; // arc gradients are indexed by the current arc order
   float* deltas_dev = nullptr;
   int rc;
   if (deltas_host) {
@@ -1091,16 +1098,23 @@ int gtnb_backward(gtnb_ctx* ctx, gtnb_lattice* lat, int tropical, const float* d
   return rc;
 }
 
-const float* gtnb_lattice_arc_grads_dev(const gtnb_lattice* lat) {
-  return lat ? lat->arc_grad : nullptr;
+const float* gtnb_lattice_arc_grads_dev(gtnb_ctx* ctx, gtnb_lattice* lat) {
+  if (!ctx || !lat) {
+    fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_lattice_arc_grads_dev: NULL");
+    return nullptr;
+  }
+  if (cudaSetDevice(ctx->device) != cudaSuccess || settle_order(ctx, lat)) return nullptr;
+  return lat->arc_grad;
 }
 
 int gtnb_lattice_arc_grads(gtnb_ctx* ctx, gtnb_lattice* lat, int b, float* out_host) {
   if (!ctx || !lat || b < 0 || b >= lat->B || !out_host)
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, "gtnb_lattice_arc_grads: bad arguments");
   if (!lat->arc_grad) return fail(ctx, GTNB_ERR_LOGIC, "gtnb_lattice_arc_grads: no backward yet");
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
   int rc = fetch_sizes(ctx, lat);
   if (rc) return rc;
+  if ((rc = settle_order(ctx, lat))) return rc;
   const GraphMeta& m = lat->meta_h[b];
   if (lat->composed) {
     GTNB_CUDA(ctx, cudaMemcpyAsync(out_host, lat->arc_grad + m.arc_base, sizeof(float) * m.A,
@@ -1127,7 +1141,7 @@ int gtnb_lattice_set_arc_grads(gtnb_ctx* ctx, gtnb_lattice* lat, int b, const fl
   int rc = fetch_sizes(ctx, lat);
   if (rc) return rc;
   if (!lat->arc_grad && (rc = dev_alloc(ctx, &lat->arc_grad, lat->tot_A))) return rc;
-  lat->order_locked = true;
+  if ((rc = settle_order(ctx, lat))) return rc;
   const GraphMeta& m = lat->meta_h[b];
   GTNB_CUDA(ctx, cudaMemcpyAsync(lat->arc_grad + m.arc_base, grads_host, sizeof(float) * m.A,
                                  cudaMemcpyHostToDevice, ctx->stream));
@@ -1144,10 +1158,7 @@ int gtnb_viterbi_path(
   int bad = first_bad_status(ctx, lat, status_host);
   int rc;
   if (!lat->back_ptr && (rc = dev_alloc(ctx, &lat->back_ptr, lat->tot_N))) return rc;
-  if (lat->order_pending && !lat->order_locked) {
-    if ((rc = launch_relax_order(ctx, lat))) return rc;
-    lat->order_pending = false;
-  }
+  if ((rc = settle_order(ctx, lat))) return rc;
   if ((rc = launch_forward(ctx, lat, MODE_PATH))) return rc;
   lat->forward_done = false; // scores now hold the path recursion, not shortestDistance
   int B = lat->B;

@@ -94,8 +94,7 @@ struct gtnb_lattice {
   bool forward_done = false;
   bool sizes_known = false;
   int score_pitch = 0; // implicit lattices: floats per saved-score row when every row has the same (0: the graph's node count rounded up to 4)
-  bool order_pending = false; // exact_ties: rows still in compose order; sorted by the first viterbi_path
-  bool order_locked = false; // arc ids already handed out (download / backward): the rows stay as they are
+  bool order_pending = false; // exact_ties: rows still in compose order; sorted before arc ids or per-arc values first cross the ABI
   int forward_mode = -1;
   int C = 0;
   int max_lvl_nodes = 0, max_lvl_arcs = 0; // upper bounds over the batch

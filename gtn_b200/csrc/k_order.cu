@@ -2,7 +2,12 @@
  * k_order.cu -- the reference's tie-breaking order on a device-composed lattice (on by default;
  * gtnb_ctx_set_flag("exact_ties", 0) before gtnb_compose_linear skips it).  GPU-validated in round 2
  * (tests/test_gpu_parity.py::test_viterbi_exact_ties_vs_oracle,
- * tests/test_gpu_config_parity.py::test_forced_alignment_config4_vs_reference).
+ * tests/test_gpu_config_parity.py::test_forced_alignment_config4_vs_reference).  The sort is deferred until a
+ * lattice's arc ids or per-arc values first cross the ABI (gtnb_capi.cu, settle_order) and carries arc_grad with the
+ * arcs, so the answers do not depend on the order of calls: tests/test_gpu_lattice_call_order.py (every measured
+ * call after every call history, against the reference) and
+ * tests/test_compose_emulation.py::test_exact_ties_sort_carries_arc_grads (gradients follow their arcs through
+ * lattice_sort_rows_kernel).
  *
  * detail::shortestPath (shortest.cpp:190-245) keeps, for every node, the FIRST-RELAXED predecessor
  * among those that reach the maximum, and the first strictly greatest accept node in g.accept()
@@ -183,34 +188,40 @@ __global__ void __launch_bounds__(kOrderThreads) lattice_relax_order_kernel(
 }
 
 /* sort the arcs of every lattice row by relaxation rank (rows are a handful of arcs: insertion sort,
- * one thread per lattice node); the provenance moves with the arc */
+ * one thread per lattice node); the provenance and, when a backward pass has run, the arc gradient move
+ * with the arc */
 __global__ void __launch_bounds__(256) lattice_sort_rows_kernel(
     const GraphMeta* __restrict__ meta,
     const uint32_t* __restrict__ row_ptr,
     int32_t* __restrict__ relax_rank,
     int2* __restrict__ arcs,
-    int2* __restrict__ gi) {
+    int2* __restrict__ gi,
+    float* __restrict__ arc_grad = nullptr) { // nullable: no backward pass has run yet
   const int b = blockIdx.y;
   const GraphMeta m = meta[b];
   const uint32_t* rp = row_ptr + m.node_base;
   int32_t* rr = relax_rank + m.arc_base;
   int2* ar = arcs + m.arc_base;
   int2* gp = gi + m.arc_base;
+  float* ag = arc_grad ? arc_grad + m.arc_base : nullptr;
   for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < m.N; n += gridDim.x * blockDim.x) {
     const int r0 = (int)(rp[n] & kRowMask), r1 = (int)(rp[n + 1] & kRowMask);
     for (int a = r0 + 1; a < r1; a++) {
       const int key = rr[a];
       const int2 av = ar[a], gv = gp[a];
+      const float dv = ag ? ag[a] : 0.0f;
       int p = a - 1;
       while (p >= r0 && rr[p] > key) {
         rr[p + 1] = rr[p];
         ar[p + 1] = ar[p];
         gp[p + 1] = gp[p];
+        if (ag) ag[p + 1] = ag[p];
         p--;
       }
       rr[p + 1] = key;
       ar[p + 1] = av;
       gp[p + 1] = gv;
+      if (ag) ag[p + 1] = dv;
     }
   }
 }
@@ -219,8 +230,9 @@ __global__ void __launch_bounds__(256) lattice_sort_rows_kernel(
 
 #ifndef GTNB_HOST_EMU
 
-/* put a freshly composed lattice in the reference's relaxation order (rows) and accept order; needs the
- * tables the "exact_ties" flag makes gtnb_compose_linear upload */
+/* put a composed lattice in the reference's relaxation order (rows) and accept order, carrying the arc
+ * gradients of a backward pass that ran before it; needs the tables the "exact_ties" flag makes
+ * gtnb_compose_linear upload */
 int launch_relax_order(gtnb_ctx* ctx, gtnb_lattice* lat) {
   if (lat->B == 0) return GTNB_OK;
   if (!lat->sg_out_pos || !lat->sg_start_rank || !lat->alive || !lat->gi)
@@ -246,7 +258,8 @@ int launch_relax_order(gtnb_ctx* ctx, gtnb_lattice* lat) {
   for (int b = 0; b < lat->B; b++) capN = std::max(capN, lat->meta_h[b].cap_N);
   dim3 grid(std::min((capN + 255) / 256, 4096), lat->B);
   GTNB_LAUNCH(ctx, "sort_rows",
-              lattice_sort_rows_kernel<<<grid, 256, 0, ctx->stream>>>(lat->meta, lat->row_ptr, rank, lat->arcs, lat->gi));
+              lattice_sort_rows_kernel<<<grid, 256, 0, ctx->stream>>>(lat->meta, lat->row_ptr, rank, lat->arcs, lat->gi,
+                                                                       lat->arc_grad));
   dev_free(ctx, rank);
   return GTNB_OK;
 }

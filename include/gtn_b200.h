@@ -271,8 +271,9 @@ int gtnb_lattice_arc_grads(gtnb_ctx* ctx, gtnb_lattice* lat, int b, float* out_h
  * when the deltas were produced or accumulated on the host (autograd.h:37).
  */
 int gtnb_lattice_set_arc_grads(gtnb_ctx* ctx, gtnb_lattice* lat, int b, const float* grads_host);
-/* device pointer to all arc gradients (device arc order) -- advanced use */
-const float* gtnb_lattice_arc_grads_dev(const gtnb_lattice* lat);
+/* device pointer to all arc gradients (device arc order, the order gtnb_lattice_download
+ * returns) -- advanced use.  NULL on error (gtnb_last_error) or before any backward. */
+const float* gtnb_lattice_arc_grads_dev(gtnb_ctx* ctx, gtnb_lattice* lat);
 
 /*
  * compose gradFunc (compose.cpp:496-518) for a lattice made by

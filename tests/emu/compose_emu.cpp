@@ -148,6 +148,46 @@ int build_lattice(
   return 0;
 }
 
+/* launch_relax_order on a lattice build_lattice made: lattice_relax_order_kernel, then lattice_sort_rows_kernel,
+ * which moves arc_grad (nullable) with the arcs */
+void relax_order(Lat& L, int B, const int32_t* n_nodes, const int32_t* in_ptr, const int32_t* out_pos,
+                 const int32_t* start_rank, int max_out, float* arc_grad) {
+  using namespace gtnb;
+  // the two extra tables, in the slab layout build_lattice gave the others
+  std::vector<int32_t> sg_out_pos(L.sg_src.size(), 0), sg_start_rank(L.sg_ptr.size(), -1);
+  long long nb = 0, pb = 0, ab = 0;
+  int maxN = 0;
+  for (int b = 0; b < B; b++) {
+    const int N = n_nodes[b], A = in_ptr[pb + N];
+    for (int a = 0; a < A; a++) sg_out_pos[L.meta[b].sg_arc_base + a] = out_pos[ab + a];
+    for (int n = 0; n < N; n++) sg_start_rank[L.meta[b].sg_node_base + n] = start_rank[nb + n];
+    maxN = std::max(maxN, N);
+    nb += N;
+    pb += N + 1;
+    ab += A;
+  }
+  std::vector<int32_t> relax((size_t)L.ta + 16, 0);
+  // launch_relax_order's shared-memory size: positions / keys + the key bitmaps and their prefix popcounts
+  emu::launch(B, kOrderThreads, sizeof(int) * (4 * std::max(maxN, 1) + 4 * ((std::max(maxN, 1) * (max_out + 1) + 31) / 32)), [&] {
+    lattice_relax_order_kernel(L.meta.data(), L.sg_flags.data(), L.sg_ptr.data(), L.sg_src.data(), L.sg_lab.data(),
+                               sg_out_pos.data(), sg_start_rank.data(), L.alive.data(), L.W, L.maxT, max_out + 1,
+                               L.lnp.data(), L.rp.data(), relax.data(), L.acc_stage.data());
+  });
+  {
+    int capN = 1;
+    for (int b = 0; b < B; b++) capN = std::max(capN, L.meta[b].cap_N);
+    const int ggx = std::min((capN + 255) / 256, 4096);
+    for (int by = 0; by < B; by++)
+      for (int bx = 0; bx < ggx; bx++)
+        emu::launch(1, 256, 0, [&] {
+          blockIdx.x = bx;
+          blockIdx.y = by;
+          gridDim.x = ggx;
+          lattice_sort_rows_kernel(L.meta.data(), L.rp.data(), relax.data(), L.arcs.data(), L.gi.data(), arc_grad);
+        });
+  }
+}
+
 } // namespace
 
 extern "C" {
@@ -307,39 +347,7 @@ int emu_viterbi_exact(
   Lat L;
   if (int rc = build_lattice(L, B, T, C, emissions, lens, n_nodes, flags, in_ptr, in_src, in_label, in_arc, in_w, n_acc, acc))
     return rc;
-  // the two extra tables, in the slab layout build_lattice gave the others
-  std::vector<int32_t> sg_out_pos(L.sg_src.size(), 0), sg_start_rank(L.sg_ptr.size(), -1);
-  long long nb = 0, pb = 0, ab = 0;
-  int maxN = 0;
-  for (int b = 0; b < B; b++) {
-    const int N = n_nodes[b], A = in_ptr[pb + N];
-    for (int a = 0; a < A; a++) sg_out_pos[L.meta[b].sg_arc_base + a] = out_pos[ab + a];
-    for (int n = 0; n < N; n++) sg_start_rank[L.meta[b].sg_node_base + n] = start_rank[nb + n];
-    maxN = std::max(maxN, N);
-    nb += N;
-    pb += N + 1;
-    ab += A;
-  }
-  std::vector<int32_t> relax((size_t)L.ta + 16, 0);
-  // launch_relax_order's shared-memory size: positions / keys + the key bitmaps and their prefix popcounts
-  emu::launch(B, kOrderThreads, sizeof(int) * (4 * std::max(maxN, 1) + 4 * ((std::max(maxN, 1) * (max_out + 1) + 31) / 32)), [&] {
-    lattice_relax_order_kernel(L.meta.data(), L.sg_flags.data(), L.sg_ptr.data(), L.sg_src.data(), L.sg_lab.data(),
-                               sg_out_pos.data(), sg_start_rank.data(), L.alive.data(), L.W, L.maxT, max_out + 1,
-                               L.lnp.data(), L.rp.data(), relax.data(), L.acc_stage.data());
-  });
-  {
-    int capN = 1;
-    for (int b = 0; b < B; b++) capN = std::max(capN, L.meta[b].cap_N);
-    const int ggx = std::min((capN + 255) / 256, 4096);
-    for (int by = 0; by < B; by++)
-      for (int bx = 0; bx < ggx; bx++)
-        emu::launch(1, 256, 0, [&] {
-          blockIdx.x = bx;
-          blockIdx.y = by;
-          gridDim.x = ggx;
-          lattice_sort_rows_kernel(L.meta.data(), L.rp.data(), relax.data(), L.arcs.data(), L.gi.data());
-        });
-  }
+  relax_order(L, B, n_nodes, in_ptr, out_pos, start_rank, max_out, nullptr);
   std::vector<float> scores((size_t)L.tn + 16, 0.0f);
   std::vector<int32_t> back_ptr((size_t)L.tn + 16, -1), best(B, -1);
   if (staged) {
@@ -380,6 +388,49 @@ int emu_viterbi_exact(
       vit_labels[(size_t)b * T + t] = on ? pl[(size_t)b * T + t] % C : -1;
       vit_graph_arcs[(size_t)b * T + t] = on ? pg[(size_t)b * T + t] : -1;
     }
+  if (emu::g_launch_failed.exchange(false)) return emu::kEmuNoThreads; // the host refused the threads
+  return 0;
+}
+
+/*
+ * The exact-ties row sort on a lattice whose arc gradients a backward pass wrote before it (gtnb_backward may run
+ * before the sort): compose -> arc_grad = grad_in -> lattice_relax_order_kernel -> lattice_sort_rows_kernel.
+ * Tables as in emu_viterbi_exact.  grad_in, grad_out, gi_in and gi_out hold the arcs graph after graph, n_arcs[b]
+ * (out) of them each: grad_in in compose order, grad_out the sorted arc_grad, gi_in / gi_out every arc's provenance
+ * {graph arc, emissions arc} before / after the sort.
+ */
+int emu_sort_rows_with_grads(
+    int B, int T, int C, const float* emissions, const int32_t* lens, const int32_t* n_nodes, const uint8_t* flags,
+    const int32_t* in_ptr, const int32_t* in_src, const int32_t* in_label, const int32_t* in_arc, const float* in_w,
+    const int32_t* out_pos, const int32_t* start_rank, int max_out, const int32_t* n_acc, const int32_t* acc,
+    const float* grad_in, float* grad_out, int32_t* gi_in, int32_t* gi_out, int32_t* n_arcs) {
+  using namespace gtnb;
+  Lat L;
+  if (int rc = build_lattice(L, B, T, C, emissions, lens, n_nodes, flags, in_ptr, in_src, in_label, in_arc, in_w, n_acc, acc))
+    return rc;
+  std::vector<float> arc_grad(L.arcs.size(), 0.0f);
+  long long off = 0;
+  for (int b = 0; b < B; b++) {
+    n_arcs[b] = L.meta[b].A;
+    for (int a = 0; a < L.meta[b].A; a++) {
+      const long long k = off + a, d = L.meta[b].arc_base + a;
+      arc_grad[d] = grad_in[k];
+      gi_in[2 * k] = L.gi[d].x;
+      gi_in[2 * k + 1] = L.gi[d].y;
+    }
+    off += L.meta[b].A;
+  }
+  relax_order(L, B, n_nodes, in_ptr, out_pos, start_rank, max_out, arc_grad.data());
+  off = 0;
+  for (int b = 0; b < B; b++) {
+    for (int a = 0; a < L.meta[b].A; a++) {
+      const long long k = off + a, d = L.meta[b].arc_base + a;
+      grad_out[k] = arc_grad[d];
+      gi_out[2 * k] = L.gi[d].x;
+      gi_out[2 * k + 1] = L.gi[d].y;
+    }
+    off += L.meta[b].A;
+  }
   if (emu::g_launch_failed.exchange(false)) return emu::kEmuNoThreads; // the host refused the threads
   return 0;
 }

@@ -392,6 +392,85 @@ def test_exact_ties_option_on_general_graph_operands(emu, seed):
         assert vs[b] == want_score
 
 
+def run_sort_with_grads(lib, e, lens, tabs, grad_in):
+    """The exact-ties row sort on a lattice whose arc_grad holds grad_in (compose order, graph after graph) ->
+    (arc counts, grad_out, provenance before, provenance after), the last three in that layout"""
+    B, T, Cn = e.shape
+    e = np.ascontiguousarray(e, np.float32)
+    lens = np.ascontiguousarray(lens, np.int32)
+    grad_in = np.ascontiguousarray(grad_in, np.float32)
+    nn = np.array([len(t["flags"]) for t in tabs], np.int32)
+    n_acc = np.array([len(t["acc"]) for t in tabs], np.int32)
+    n_arcs = np.zeros(B, np.int32)
+    grad_out = np.full(len(grad_in), np.nan, np.float32)
+    gi_in, gi_out = np.zeros((len(grad_in), 2), np.int32), np.zeros((len(grad_in), 2), np.int32)
+    P = lambda a, t: a.ctypes.data_as(t)
+    flags, ptr = cat([t["flags"] for t in tabs], np.uint8), cat([t["ptr"] for t in tabs], np.int32)
+    src, lab = cat([t["src"] for t in tabs], np.int32), cat([t["lab"] for t in tabs], np.int32)
+    arc, w, acc = cat([t["arc"] for t in tabs], np.int32), cat([t["w"] for t in tabs], np.float32), cat([t["acc"] for t in tabs], np.int32)
+    opos, sr = cat([t["out_pos"] for t in tabs], np.int32), cat([t["start_rank"] for t in tabs], np.int32)
+    lib.emu_sort_rows_with_grads.argtypes = [C.c_int, C.c_int, C.c_int, f32p, i32p, i32p, u8p, i32p, i32p, i32p, i32p,
+                                             f32p, i32p, i32p, C.c_int, i32p, i32p, f32p, f32p, i32p, i32p, i32p]
+    rc = lib.emu_sort_rows_with_grads(B, T, Cn, P(e, f32p), P(lens, i32p), P(nn, i32p), P(flags, u8p), P(ptr, i32p),
+                                      P(src, i32p), P(lab, i32p), P(arc, i32p), P(w, f32p), P(opos, i32p), P(sr, i32p),
+                                      max(t["max_out"] for t in tabs), P(n_acc, i32p), P(acc, i32p), P(grad_in, f32p),
+                                      P(grad_out, f32p), P(gi_in, i32p), P(gi_out, i32p), P(n_arcs, i32p))
+    emu_build.check(rc)
+    A = int(n_arcs.sum())
+    return n_arcs, grad_out[:A], gi_in[:A], gi_out[:A]
+
+
+def sort_operands(kind, seed):
+    """tie-heavy emissions and the exact-ties tables of CTC graphs (blank first / last, a repeated label) or of
+    general graph operands, sorted or not"""
+    rng = np.random.default_rng(6000 + seed)
+    if kind == "general":
+        Cn, T = 4, int(rng.integers(2, 8))
+        ogs = []
+        for i in range(3):
+            n = int(rng.integers(2, 8))
+            flags = np.zeros(n, np.uint8)
+            flags[rng.integers(0, n, max(1, n // 3))] |= 1
+            flags[rng.integers(0, n, max(1, n // 2))] |= 2
+            na = int(rng.integers(n, 3 * n + 1))
+            src, dst, lab = rng.integers(0, n, na), rng.integers(0, n, na), rng.integers(0, Cn, na)
+            og = po.Graph.from_arrays(flags, src, dst, lab, lab, rng.integers(-1, 2, na).astype(np.float32))
+            if i % 2:
+                og.arc_sort(False)
+            ogs.append(og)
+        lens = [T, T - 1, 1]
+    else:
+        Cn, T, U = 5, 16, 3
+        blank = Cn - 1 if kind == "ctc_blank_last" else 0
+        labels = [l for l in range(Cn) if l != blank]
+        targets = [rng.choice(labels, U).astype(np.int32) for _ in range(3)]
+        targets[1][1] = targets[1][0]
+        ogs = [po.Graph.ctc(t, blank, True) for t in targets]
+        lens = [T, T - 5, 2 * U + 1]
+    e = rng.integers(-1, 2, (len(ogs), T, Cn)).astype(np.float32)
+    return rng, e, np.array(lens, np.int32), [tables_with_out_pos(g, Cn) for g in ogs]
+
+
+@pytest.mark.parametrize("kind,seed", [("ctc_blank_first", 0), ("ctc_blank_last", 1), ("general", 2), ("general", 3),
+                                       ("general", 4), ("general", 5)])
+def test_exact_ties_sort_carries_arc_grads(emu, kind, seed):
+    """gtnb_backward may run before the exact-ties sort: lattice_sort_rows_kernel then moves arc_grad with the arcs.
+    Looked up by entry and provenance (which names an arc of a composed lattice), every arc's gradient is the one it
+    had before the sort.  On the CTC lattices the sort does move arcs, so a gradient left in place is caught."""
+    rng, e, lens, tabs = sort_operands(kind, seed)
+    cap = max(sum(int(lens[b]) * len(tabs[b]["src"]) for b in range(len(tabs))), 1)  # >= every lattice's arc count
+    grad_in = rng.integers(-50, 51, cap).astype(np.float32) / 8
+    n_arcs, grad_out, gi_in, gi_out = run_sort_with_grads(emu, e, lens, tabs, grad_in)
+    entry = np.repeat(np.arange(len(tabs)), n_arcs).tolist()
+    before = [(b, *g) for b, g in zip(entry, gi_in.tolist())]
+    after = [(b, *g) for b, g in zip(entry, gi_out.tolist())]
+    assert len(set(before)) == len(before) and sorted(after) == sorted(before)
+    was = dict(zip(before, grad_in[:len(before)].tolist()))
+    assert [was[k] for k in after] == grad_out.tolist()
+    if kind != "general":
+        assert before != after
+
+
 def run_staged(lib, e, lens, tabs, deltas, fused, viterbi=False):
     B, T, Cn = e.shape
     e = np.ascontiguousarray(e, np.float32)

@@ -56,10 +56,12 @@ def ctc_arrays(target, blank=0):
 class Batch:
     """The same B (CTC graph, emissions) pairs in gtn_b200.gtn (ctcs, ems) and in the reference (rctcs, rems)."""
 
-    def __init__(self, gtn, seed=7):
+    def __init__(self, gtn, seed=7, integer=False):
+        """integer: emissions in {-1, 0, 1}, so that most lattice nodes tie"""
         rng = np.random.default_rng(seed)
         self.gtn = gtn
-        self.es = [rng.uniform(-5, 5, (T, C)).astype(np.float32) for T in TS]
+        self.es = [(rng.integers(-1, 2, (T, C)) if integer else rng.uniform(-5, 5, (T, C))).astype(np.float32)
+                   for T in TS]
         self.targets = [rng.integers(1, C, U).astype(np.int32).tolist() for U in US]
         self.arrays = [ctc_arrays(t) for t in self.targets]
         self.ctcs, self.ems, self.rctcs, self.rems = [], [], [], []
