@@ -4103,20 +4103,11 @@ int beam_async_check(gtnb_ctx* ctx, const std::string& fn, const BeamAsyncArgs& 
   return GTNB_OK;
 }
 
-/* gtnb_beam_decode_lm_async's own arguments beyond gtnb_beam_decode_async's */
-struct BeamLmArgs {
-  const gtnb_lm* lm;
-  float lm_weight, token_bonus;
-  int token_beam;
-  float *am_scores, *lm_scores;
-};
-
 /* gtnb_beam_decode_async's run: the back-pointers and (with transitions) the transposed weights, the start weights
- * and the row flags taken from the arena and, when launch, the weights kernel and the search enqueued; with m, the
- * fused search of gtnb_beam_decode_lm_async, with x the lexicon search of gtnb_beam_decode_lexicon_async (the same
- * scratch) */
-int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const BeamLmArgs* m = nullptr,
-                   const BeamLexLaunch* x = nullptr) {
+ * and the row flags taken from the arena and, when launch, the weights kernel and the search under policy f enqueued
+ * (the same scratch for every policy) */
+template <class F>
+int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const F& f) {
   uint16_t* bp = nullptr;
   float *wt = nullptr, *wfirst = nullptr;
   int32_t* wbad = nullptr;
@@ -4128,20 +4119,9 @@ int beam_async_run(gtnb_ctx* ctx, const BeamAsyncArgs& a, bool launch, const Bea
   }
   if (!launch) return GTNB_OK;
   if (a.kind != GTNB_DENSE_CTC) GTNB_TRY(launch_beam_weights(ctx, a.C, a.kind, a.trans_w, wt, wfirst, wbad));
-  if (x)
-    return launch_beam_decode_lex(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
-                                  a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
-                                  a.tokens, a.lengths, a.scores, a.status, *x);
-  if (m) {
-    const BeamLmLaunch f{m->token_beam, m->lm ? m->lm->w : nullptr, m->lm ? m->lm->d : nullptr,
-                         m->lm ? m->lm->start : 0, m->lm_weight, m->token_bonus, m->am_scores, m->lm_scores};
-    return launch_beam_decode_lm(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
-                                 a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
-                                 a.tokens, a.lengths, a.scores, a.status, f);
-  }
   return launch_beam_decode(ctx, a.B, a.T, a.C, a.emissions, a.dtype, a.input_lens, a.kind, wt,
                             a.kind == GTNB_DENSE_ASG ? a.trans_w : wfirst, wbad, a.blank, a.beam, a.nbest, bp,
-                            a.tokens, a.lengths, a.scores, a.status);
+                            a.tokens, a.lengths, a.scores, a.status, f);
 }
 
 } // namespace
@@ -4153,7 +4133,7 @@ extern "C" int gtnb_beam_decode_async_workspace(gtnb_ctx* ctx, int B, int T, int
   const BeamAsyncArgs a{B, T, C, dtype, nullptr, nullptr, kind, nullptr, 0, beam, nbest,
                         nullptr, nullptr, nullptr, nullptr};
   GTNB_TRY(beam_async_check(ctx, fn, a));
-  return async_workspace(ctx, B, bytes, [&](bool launch) { return beam_async_run(ctx, a, launch); });
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return beam_async_run(ctx, a, launch, BeamNoLm()); });
 }
 
 extern "C" int gtnb_beam_decode_async(
@@ -4170,7 +4150,7 @@ extern "C" int gtnb_beam_decode_async(
                         tokens_dev, lengths_dev, scores_dev, status_dev};
   GTNB_TRY(beam_async_check(ctx, fn, a));
   return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
-                       [&](bool launch) { return beam_async_run(ctx, a, launch); });
+                       [&](bool launch) { return beam_async_run(ctx, a, launch, BeamNoLm()); });
 }
 
 namespace {
@@ -4346,8 +4326,8 @@ extern "C" int gtnb_beam_decode_lm_async_workspace(gtnb_ctx* ctx, int B, int T, 
   const BeamAsyncArgs a{B, T, C, dtype, nullptr, nullptr, kind, nullptr, 0, beam, nbest,
                         nullptr, nullptr, nullptr, nullptr};
   GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
-  const BeamLmArgs m{nullptr, 0.0f, 0.0f, token_beam, nullptr, nullptr};
-  return async_workspace(ctx, B, bytes, [&](bool launch) { return beam_async_run(ctx, a, launch, &m); });
+  const BeamLm f{token_beam, nullptr, nullptr, 0, 0.0f, 0.0f, nullptr, nullptr};
+  return async_workspace(ctx, B, bytes, [&](bool launch) { return beam_async_run(ctx, a, launch, f); });
 }
 
 extern "C" int gtnb_beam_decode_lm_async(
@@ -4369,9 +4349,10 @@ extern "C" int gtnb_beam_decode_lm_async(
   const BeamAsyncArgs a{B, T, C, dtype, emissions_dev, input_lens_dev, kind, trans_w_dev, blank, beam, nbest,
                         tokens_dev, lengths_dev, scores_dev, status_dev};
   GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
-  const BeamLmArgs m{lm, lm_weight, token_bonus, token_beam, am_scores_dev, lm_scores_dev};
+  const BeamLm f{token_beam, lm ? lm->w : nullptr, lm ? lm->d : nullptr, lm ? lm->start : 0,
+                 lm_weight, token_bonus, am_scores_dev, lm_scores_dev};
   return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
-                       [&](bool launch) { return beam_async_run(ctx, a, launch, &m); });
+                       [&](bool launch) { return beam_async_run(ctx, a, launch, f); });
 }
 
 /*
@@ -4645,10 +4626,21 @@ extern "C" int gtnb_beam_decode_lexicon_async(
   GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
   if (kind != GTNB_DENSE_ASG && (lexicon->spelled[blank] || lexicon->cls[blank] == 1))
     return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the lexicon spells with the blank or makes it a separator");
-  const BeamLexLaunch x{token_beam, lexicon->start, lm_weight, word_bonus, am_scores_dev, lm_scores_dev,
-                        lexicon->d_cls, lexicon->d_mask, lexicon->d_first, lexicon->d_word, lexicon->d_smear,
-                        lexicon->d_hash, lexicon->hmul, lexicon->hbits, lexicon->d_bow, lexicon->d_bod,
-                        lexicon->d_endw, words_dev, word_counts_dev};
+  const BeamLex f{{token_beam, nullptr, nullptr, lexicon->start, lm_weight, word_bonus, am_scores_dev, lm_scores_dev},
+                 lexicon->d_cls,
+                 (C + 31) / 32,
+                 lexicon->d_mask,
+                 lexicon->d_first,
+                 lexicon->d_word,
+                 lexicon->d_smear,
+                 lexicon->d_hash,
+                 lexicon->hmul,
+                 lexicon->hbits,
+                 lexicon->d_bow,
+                 lexicon->d_bod,
+                 lexicon->d_endw,
+                 words_dev,
+                 word_counts_dev};
   return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
-                       [&](bool launch) { return beam_async_run(ctx, a, launch, nullptr, &x); });
+                       [&](bool launch) { return beam_async_run(ctx, a, launch, f); });
 }

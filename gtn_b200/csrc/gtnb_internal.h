@@ -228,50 +228,15 @@ int launch_edit_distance(gtnb_ctx* ctx, int B, const int32_t* hyp, int N, const 
                          uint32_t* moves);
 
 /* gtnb_beam_decode_async (k_beam.cu): the bounds it covers, the transposed transitions / start weights / row flags of
- * a call, and the search (wt, wfirst, wbad unused for GTNB_DENSE_CTC) */
+ * a call, and the search under policy F (gtnb_meta.h: BeamNoLm, BeamLm or BeamLex; wt, wfirst, wbad unused for
+ * GTNB_DENSE_CTC) */
 bool beam_decode_supported(int C, int beam, int nbest);
 int launch_beam_weights(gtnb_ctx* ctx, int C, int kind, const float* trans_w, float* wt, float* wfirst, int32_t* wbad);
+template <class F>
 int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
                        const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
                        int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
-                       int32_t* status);
-/* gtnb_beam_decode_lm_async's search: launch_beam_decode's with the LM's resolved table (lmw NULL: no LM),
- * its weights, token_beam P and the acoustic / LM scores of the hypotheses (each nullable) */
-struct BeamLmLaunch {
-  int P;
-  const float* lmw; // [S][C + 1]
-  const int32_t* lmd; // [S][C + 1]
-  int start;
-  float lm_weight, token_bonus;
-  float *am_scores, *lm_scores;
-};
-int launch_beam_decode_lm(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
-                          const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
-                          int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
-                          int32_t* status, const BeamLmLaunch& lm);
-/* gtnb_beam_decode_lexicon_async's search: launch_beam_decode_lm's with the lexicon's device arrays in place of the
- * token LM (hash NULL: no word LM, every weight 0) and the word outputs (each nullable) */
-struct BeamLexLaunch {
-  int P;
-  int start; // the word LM's start node
-  float lm_weight, word_bonus;
-  float *am_scores, *lm_scores;
-  const int32_t* cls; // [C]
-  const uint32_t* mask; // [nodes][ceil(C / 32)]
-  const int32_t *first, *word; // [nodes]
-  const float* smear; // [nodes]
-  const unsigned long long* hash; // [H][2]: key node << 32 | word (all ones: empty), value destination << 32 | weight bits
-  unsigned long long hmul;
-  int hbits;
-  const float* bow; // [S]
-  const int32_t* bod; // [S]
-  const float* endw; // [S]
-  int32_t *words, *counts; // [B][N][T], [B][N]
-};
-int launch_beam_decode_lex(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
-                           const int32_t* input_lens, int kind, const float* wt, const float* wfirst,
-                           const int32_t* wbad, int blank, int K, int N, uint16_t* bp, int32_t* tokens,
-                           int32_t* lengths, float* scores, int32_t* status, const BeamLexLaunch& lex);
+                       int32_t* status, const F& f);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);

@@ -144,4 +144,44 @@ struct GraphMeta {
   int pad_;
 };
 
+/*
+ * The policies of k_beam.cu's beam search, as the entry points fill them (their device code is in k_beam.cu):
+ * BeamNoLm for gtnb_beam_decode_async, BeamLm for gtnb_beam_decode_lm_async, BeamLex for
+ * gtnb_beam_decode_lexicon_async.  on: the policy prunes tokens and ranks by a fused score.  The outputs a policy
+ * lacks are static NULLs, so that code writing every output compiles the missing ones away.
+ */
+struct BeamNoLm {
+  static constexpr bool on = false;
+  static constexpr int P = 0; // (unused: every token)
+  static constexpr float *am = nullptr, *lm = nullptr;
+  static constexpr int32_t *words = nullptr, *counts = nullptr;
+};
+struct BeamLm {
+  static constexpr bool on = true;
+  int P; // token_beam: tokens per frame, P = C: all of them
+  const float* lmw; // [S][C + 1] resolved LM weights (column C: end weights); NULL: no LM, every weight 0
+  const int32_t* lmd; // [S][C + 1] destination nodes
+  int start; // the LM's start node
+  float lw, tb; // lm_weight, token_bonus
+  float *am, *lm; // [B][N] nullable: acoustic and LM scores of the hypotheses
+  static constexpr int32_t *words = nullptr, *counts = nullptr;
+};
+/* BeamLex: BeamLm's P, start (the word LM's start node), lw, tb (word_bonus), am and lm; lmw and lmd are NULL */
+struct BeamLex : BeamLm {
+  const int32_t* cls; // [C] token classes: 0 in-word, 1 separator, 2 word-start
+  int MW; // ceil(C / 32)
+  const uint32_t* mask; // [nodes][MW] trie child masks (bit c: a child labelled c)
+  const int32_t* first; // [nodes] index of the first child (children numbered in token order)
+  const int32_t* word; // [nodes] word id spelled at the node, or -1
+  const float* smear; // [nodes] lookahead of the node
+  const unsigned long long* hash; // [H][2] word LM emitting arcs: key node << 32 | word (all ones: empty), value
+                                  // destination << 32 | weight bits; NULL: no word LM, every weight 0
+  unsigned long long hmul; // multiplier of the arc hash (0: every key probes from slot 0)
+  int hbits; // log2 H
+  const float* bow; // [S] backoff weight of each LM node
+  const int32_t* bod; // [S] backoff destination, or -1
+  const float* endw; // [S] resolved end weights
+  int32_t *words, *counts; // [B][N][T] / [B][N] nullable: word ids and word counts of the hypotheses
+};
+
 } // namespace gtnb

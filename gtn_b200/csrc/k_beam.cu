@@ -25,8 +25,11 @@
  *   and frame, coalesced over the tokens), made once per call by beam_weights_kernel with the n-gram start weights
  *   sigma_i = logsumexp_j W[i][j] and a per-row NaN / +inf flag.  The emission row of frame t + 1 is loaded while
  *   frame t is searched.
- * - Fusion and pruning (gtnb_beam_decode_lm_async).  beam_decode_kernel's policy F: BeamLm, or BeamNoLm for
- *   gtnb_beam_decode_async, which compiles to the code without them.  Each slot also carries its LM
+ * - Policies.  beam_decode_kernel's policy F (gtnb_meta.h) is BeamNoLm for gtnb_beam_decode_async, BeamLm or BeamLex;
+ *   BeamSlots<F> holds its per-slot state and the operations the frame loop and the epilogue call (BeamNoLm's are
+ *   empty, its key the acoustic score), BeamSmem<F> carves the shared memory for the kernel and sizes it for the
+ *   host, and beam_finish ranks every policy's final scores the same way.
+ * - Fusion and pruning (gtnb_beam_decode_lm_async).  Policy BeamLm: each slot also carries its LM
  *   node and lmacc (the unweighted sum of its resolved LM weights), double-buffered; candidates are ranked by the
  *   fused key am + (lm_weight * lmacc + token_bonus * len).  With token_beam P < C the P best tokens of each frame
  *   are selected first (a rank count per token; ties to the lower token), and extension (s, p) takes candidate
@@ -55,62 +58,6 @@ struct BeamHash {
     h ^= (uint64_t)(uint32_t)tok + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
     return h * 0xff51afd7ed558ccdull;
   }
-};
-
-/* dynamic shared memory of one CTA: two hash arrays [2][K] of 8 bytes, then 4-byte words (control block, histogram,
- * two emission rows, the two start-weight rows, the double-buffered state, the candidates' scratch and keys) */
-inline long long beam_smem_bytes(int K, int C) {
-  return 32ll * K + 4ll * (16 + 256 + 4ll * C + 18ll * K + K + (long long)K * C);
-}
-
-/* beam_lm_smem_bytes: beam_smem_bytes plus the LM node and lmacc per slot ([2][K] each), the frame's tokens and
- * token -> position map ([C] each) and 8 words of per-warp counts */
-inline long long beam_lm_smem_bytes(int K, int C) {
-  return beam_smem_bytes(K, C) + 4ll * (4ll * K + 2ll * C + 8);
-}
-
-/* beam_lex_smem_bytes: beam_lm_smem_bytes plus the lexicon state per slot (trie node, word count, word id, completion
- * weight and LM destination, first child, smear: [2][K] each; the child mask [2][K][MW]), the root's mask [MW], the
- * smear of the root's children [C] and the token classes [C]; MW = ceil(C / 32) */
-inline long long beam_lex_smem_bytes(int K, int C) {
-  const long long MW = (C + 31) / 32;
-  return beam_lm_smem_bytes(K, C) + 4ll * (14ll * K + 2ll * K * MW + MW + 2ll * C);
-}
-
-/* the policy of beam_decode_kernel: BeamNoLm for gtnb_beam_decode_async, BeamLm for gtnb_beam_decode_lm_async,
- * BeamLex for gtnb_beam_decode_lexicon_async */
-struct BeamNoLm {
-  static constexpr bool on = false;
-  static constexpr bool lex = false;
-  static constexpr int P = 0; // (unused: every token)
-};
-struct BeamLm {
-  static constexpr bool on = true;
-  static constexpr bool lex = false;
-  int P; // token_beam: tokens per frame, P = C: all of them
-  const float* lmw; // [S][C + 1] resolved LM weights (column C: end weights); NULL: no LM, every weight 0
-  const int32_t* lmd; // [S][C + 1] destination nodes
-  int start; // the LM's start node
-  float lw, tb; // lm_weight, token_bonus
-  float *am, *lm; // [B][N] nullable: acoustic and LM scores of the hypotheses
-};
-/* BeamLex: BeamLm's P, start (the word LM's start node), lw, tb (word_bonus), am and lm; lmw and lmd are NULL */
-struct BeamLex : BeamLm {
-  static constexpr bool lex = true;
-  const int32_t* cls; // [C] token classes: 0 in-word, 1 separator, 2 word-start
-  int MW; // ceil(C / 32)
-  const uint32_t* mask; // [nodes][MW] trie child masks (bit c: a child labelled c)
-  const int32_t* first; // [nodes] index of the first child (children numbered in token order)
-  const int32_t* word; // [nodes] word id spelled at the node, or -1
-  const float* smear; // [nodes] lookahead of the node
-  const unsigned long long* hash; // [H][2] word LM emitting arcs: key node << 32 | word (all ones: empty), value
-                                  // destination << 32 | weight bits
-  unsigned long long hmul; // multiplier of the arc hash (0: every key probes from slot 0)
-  int hbits; // log2 H
-  const float* bow; // [S] backoff weight of each LM node
-  const int32_t* bod; // [S] backoff destination, or -1
-  const float* endw; // [S] resolved end weights
-  int32_t *words, *counts; // [B][N][T] / [B][N] nullable: word ids and word counts of the hypotheses
 };
 
 /* the fused ranking key, in this float32 order (no contraction): am + (lw * lmacc + tb * len) */
@@ -221,6 +168,15 @@ __device__ __forceinline__ float beam_ext_am(int kind, int blank, int C, const f
   return v;
 }
 
+/* the same for beam s of the state arrays, read only past the blank test (BeamNoLm's form: the fused policies read
+ * the slot anyway, and each form is the one that keeps its kernel's registers down) */
+__device__ __forceinline__ float beam_ext_am(int kind, int blank, int C, const float* er, const float* wp,
+                                             const float* __restrict__ wt, const float* pb, const float* pl,
+                                             const float* tot, const int* last, int s, int c) {
+  if (kind != GTNB_DENSE_ASG && c == blank) return neg_inf();
+  return beam_ext_am(kind, blank, C, er, wp, wt, pb[s], pl[s], tot[s], last[s], c);
+}
+
 /* one token back along the back-pointers from (t, s): the token, with (t, s) moved to before it */
 __device__ __forceinline__ int beam_back(const uint16_t* bpu, int K, int& t, int& s) {
   for (;;) {
@@ -287,159 +243,359 @@ __global__ void __launch_bounds__(kBeamThreads) beam_weights_kernel(int C, int k
   }
 }
 
-/* status 1 or 2: NaN scores, -1 lengths and rows */
-__device__ void beam_flag(int b, int T, int N, int code, int32_t* tokens, int32_t* lengths, float* scores,
-                          int32_t* status) {
-  const int tid = threadIdx.x;
-  for (long long p = tid; p < (long long)N * T; p += kBeamThreads) tokens[(long long)b * N * T + p] = -1;
-  for (int n = tid; n < N; n += kBeamThreads) {
-    scores[(long long)b * N + n] = CUDART_NAN_F;
-    lengths[(long long)b * N + n] = -1;
+/* carves a CTA's dynamic shared memory front to back; on the host a NULL base only counts the bytes (int: at most
+ * kMaxDynamicSmem) */
+struct BeamCarve {
+  char* base;
+  int bytes = 0;
+  template <class T>
+  __host__ __device__ T* take(int n) {
+#ifdef __CUDA_ARCH__
+    T* p = reinterpret_cast<T*>(base + bytes);
+#else
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+#endif
+    bytes += (int)sizeof(T) * n;
+    return p;
   }
-  if (tid == 0 && status) status[b] = code;
-}
-
-/* BeamLm: the am and lm scores of a flagged utterance (status 1 or 2), NaN like its scores */
-__device__ void beam_flag_lm(int b, int N, const BeamLm& f) {
-  for (int n = threadIdx.x; n < N; n += kBeamThreads) {
-    if (f.am) f.am[(long long)b * N + n] = CUDART_NAN_F;
-    if (f.lm) f.lm[(long long)b * N + n] = CUDART_NAN_F;
-  }
-}
+};
 
 /*
- * BeamLm, after frame T_b - 1: every live slot adds its end weight (a beam whose end weight is -inf is dropped) and
- * the N-best are the top live beams by the final fused score, ties to the lower slot (the search's own order).
- * fin / lmf ([K]) hold each slot's final fused score and LM score, rank ([K]) rank -> slot.
+ * A policy's per-slot state in shared memory ([2][K] arrays, indexed by buffer * K + slot) and the operations
+ * beam_decode_kernel calls: init (the root slot, and tables the frames read), key (of a kept or merged candidate whose
+ * acoustic score is am), ext_key (of extension (m, c) whose acoustic score is am, -inf when the policy forbids it),
+ * keep (slot o carries slot m), extend (slot o is extension (m, c)), final (the final score of slot m, after the last
+ * frame), hyp (a hypothesis's own outputs, m -1 for none) and words (the lexicon's word read-off).
  */
-__device__ void beam_finish_lm(int b, int T, int Tb, int C, int K, int N, const uint16_t* bpu, int cur, int* ctl,
-                               const float* stot, const int* slen, const int* snode, const float* slm, float* fin,
-                               float* lmf, int* rank, int32_t* tokens, int32_t* lengths, float* scores,
-                               int32_t* status, const BeamLm& f) {
-  const int tid = threadIdx.x;
-  const int L = ctl[kBcL];
-  if (tid < L) {
-    const int m = cur * K + tid;
-    const float we = f.lmw ? __ldg(f.lmw + (long long)snode[m] * (C + 1) + C) : 0.0f;
-    const float lm = slm[m] + we;
-    fin[tid] = we == neg_inf() ? neg_inf() : beam_fuse(f, stot[m], lm, slen[m]);
-    lmf[tid] = lm;
-  }
-  __syncthreads();
-  int live = 0;
-  for (int i = 0; i < L; i++) live += fin[i] > neg_inf();
-  if (tid < L && fin[tid] > neg_inf()) {
-    int r = 0;
-    for (int i = 0; i < L; i++) r += fin[i] > fin[tid] || (fin[i] == fin[tid] && i < tid);
-    rank[r] = tid;
-  }
-  __syncthreads();
-  int32_t* out = tokens + (long long)b * N * T;
-  for (int n = tid; n < N; n += kBeamThreads) {
-    const int m = n < live ? rank[n] : -1;
-    const int len = m >= 0 ? slen[cur * K + m] : -1;
-    const long long o = (long long)b * N + n;
-    scores[o] = m >= 0 ? fin[m] : neg_inf();
-    if (f.am) f.am[o] = m >= 0 ? stot[cur * K + m] : neg_inf();
-    if (f.lm) f.lm[o] = m >= 0 ? lmf[m] : neg_inf();
-    lengths[o] = len;
-    int tt = Tb - 1, s = m;
-    for (int p = len - 1; p >= 0; p--) out[(long long)n * T + p] = beam_back(bpu, K, tt, s);
-  }
-  for (long long p = tid; p < (long long)N * T; p += kBeamThreads) {
-    const int n = (int)(p / T);
-    if (p - (long long)n * T >= (n < live ? slen[cur * K + rank[n]] : 0)) out[p] = -1;
-  }
-  if (tid == 0) {
-    bool tied = ctl[kBcTieAny] != 0;
-    for (int n = 0; n + 1 < live && n < N; n++) tied |= fin[rank[n]] == fin[rank[n + 1]];
-    if (status) status[b] = tied ? 3 : 0;
-  }
-}
+template <class F>
+struct BeamSlots;
 
-/* BeamLex: beam_flag_lm, and -1 word rows and counts */
-__device__ void beam_flag_lex(int b, int T, int N, const BeamLex& f) {
-  beam_flag_lm(b, N, f);
-  for (long long p = threadIdx.x; p < (long long)N * T; p += kBeamThreads)
-    if (f.words) f.words[(long long)b * N * T + p] = -1;
-  for (int n = threadIdx.x; n < N; n += kBeamThreads)
-    if (f.counts) f.counts[(long long)b * N + n] = -1;
-}
+/* BeamNoLm: no state; the key is the acoustic score */
+template <>
+struct BeamSlots<BeamNoLm> {
+  __host__ __device__ void carve(BeamCarve&, int, int) {}
+  __device__ void init(const BeamNoLm&, int, int) const {}
+  __device__ float key(const BeamNoLm&, float am, int, int) const { return am; }
+  __device__ float ext_key(const BeamNoLm&, float am, int, int, int, int) const { return am; }
+  __device__ void keep(int, int) const {}
+  __device__ void extend(const BeamNoLm&, int, int, int, int) const {}
+  __device__ float final(const BeamNoLm&, int, float am, int, int) const { return am; }
+  __device__ void hyp(const BeamNoLm&, long long, int, float) const {}
+  __device__ void words(const BeamNoLm&, int, int, int, int, const int*, const int*, int, const int32_t*) const {}
+};
 
-/*
- * BeamLex, after frame T_b - 1: every live slot at a word end completes its word, a slot inside a word is dropped;
- * each adds its end weight (dropped at -inf) and the N-best are the top live beams by am + (lw * lm + tb * words),
- * ties to the lower slot.  Each hypothesis's words are read off its traced tokens by walking the trie.  fin / lmf /
- * nwd ([K]) hold each slot's final fused score, LM score and word count, rank ([K]) rank -> slot.
- */
-__device__ void beam_finish_lex(int b, int T, int Tb, int K, int N, const uint16_t* bpu, int cur, int* ctl,
-                                const float* stot, const int* slen, const int* snode, const float* slm,
-                                const int* strie, const int* swn, const int* swd, const float* scw, const int* scd,
-                                const int* tcls, float* fin, float* lmf, int* nwd, int* rank, int32_t* tokens,
-                                int32_t* lengths, float* scores, int32_t* status, const BeamLex& f) {
-  const int tid = threadIdx.x;
-  const int L = ctl[kBcL];
-  if (tid < L) {
-    const int m = cur * K + tid;
-    float lm = slm[m];
-    int node = snode[m], nw = swn[m];
+/* BeamLm: the LM node and lmacc (the unweighted sum of the slot's resolved LM weights); the key is
+ * am + (lw * lmacc + tb * len) */
+template <>
+struct BeamSlots<BeamLm> {
+  int* node;
+  float* lm;
+  __host__ __device__ void carve(BeamCarve& m, int K, int) {
+    node = m.take<int>(2 * K);
+    lm = m.take<float>(2 * K);
+  }
+  __device__ void init(const BeamLm& f, int tid, int) const {
+    if (tid == 0) {
+      node[0] = f.lmw ? f.start : 0;
+      lm[0] = 0.0f;
+    }
+  }
+  __device__ float key(const BeamLm& f, float am, int m, int len) const { return beam_fuse(f, am, lm[m], len); }
+  __device__ float ext_key(const BeamLm& f, float v, int m, int c, int len, int C) const {
+    if (v > neg_inf() && f.lmw) {
+      const float w = __ldg(f.lmw + (long long)node[m] * (C + 1) + c); // (one row per beam, via the L2)
+      v = w == neg_inf() ? w : beam_fuse(f, v, lm[m] + w, len + 1);
+    } else if (v > neg_inf()) {
+      v = beam_fuse(f, v, lm[m], len + 1);
+    }
+    return v;
+  }
+  __device__ void keep(int o, int m) const {
+    node[o] = node[m];
+    lm[o] = lm[m];
+  }
+  __device__ void extend(const BeamLm& f, int o, int m, int c, int C) const {
+    const long long at = (long long)node[m] * (C + 1) + c;
+    node[o] = f.lmw ? __ldg(f.lmd + at) : 0;
+    lm[o] = f.lmw ? lm[m] + __ldg(f.lmw + at) : lm[m];
+  }
+  /* adds the end weight to lmacc (a beam whose end weight is -inf is dropped) */
+  __device__ float final(const BeamLm& f, int m, float am, int len, int C) const {
+    const float we = f.lmw ? __ldg(f.lmw + (long long)node[m] * (C + 1) + C) : 0.0f;
+    lm[m] = lm[m] + we;
+    return we == neg_inf() ? neg_inf() : beam_fuse(f, am, lm[m], len);
+  }
+  __device__ void hyp(const BeamLm& f, long long o, int m, float am) const {
+    if (f.am) f.am[o] = am;
+    if (f.lm) f.lm[o] = m >= 0 ? lm[m] : neg_inf();
+  }
+  __device__ void words(const BeamLm&, int, int, int, int, const int*, const int*, int, const int32_t*) const {}
+};
+
+/* BeamLex: the word LM's node and lmacc, and the trie node, word count, word id of the trie node (or -1), at a word
+ * end the completion's weight w(LM node, word id) and LM destination, first child, smear and child mask [2][K][MW]
+ * of each slot; the root's child mask [MW], the smear of the root's child labelled c [C] and the token classes [C].
+ * The key is am + (lw * (lmacc + smear) + tb * words) */
+template <>
+struct BeamSlots<BeamLex> {
+  int* node;
+  float* lm;
+  int *trie, *wn, *wd; // (the root is trie node 0, its children 1, 2, ... in token order)
+  float* cw;
+  int *cd, *fc;
+  float* sm;
+  uint32_t *mask, *rmask;
+  float* rsm;
+  int* cls;
+  int MW;
+  __host__ __device__ void carve(BeamCarve& m, int K, int C) {
+    MW = (C + 31) / 32;
+    node = m.take<int>(2 * K);
+    lm = m.take<float>(2 * K);
+    trie = m.take<int>(2 * K);
+    wn = m.take<int>(2 * K);
+    wd = m.take<int>(2 * K);
+    cw = m.take<float>(2 * K);
+    cd = m.take<int>(2 * K);
+    fc = m.take<int>(2 * K);
+    sm = m.take<float>(2 * K);
+    mask = m.take<uint32_t>(2 * K * MW);
+    rmask = m.take<uint32_t>(MW);
+    rsm = m.take<float>(C);
+    cls = m.take<int>(C);
+  }
+  __device__ void init(const BeamLex& f, int tid, int C) const {
+    if (tid == 0) {
+      node[0] = f.start;
+      lm[0] = 0.0f;
+      trie[0] = wn[0] = cd[0] = 0;
+      wd[0] = -1;
+      cw[0] = sm[0] = 0.0f;
+      fc[0] = __ldg(f.first);
+    }
+    if (tid < MW) mask[tid] = rmask[tid] = __ldg(f.mask + tid);
+    if (tid < C) {
+      cls[tid] = __ldg(f.cls + tid);
+      rsm[tid] = lex_has(f.mask, tid) ? __ldg(f.smear + 1 + lex_rank(f.mask, tid)) : 0.0f;
+    }
+  }
+  __device__ float key(const BeamLex& f, float am, int m, int) const {
+    return beam_lex_fuse(f, am, lm[m], sm[m], wn[m]);
+  }
+  /* admission is a bit test; an in-word child's smear is one row per beam, via the L2 */
+  __device__ float ext_key(const BeamLex& f, float v, int m, int c, int, int) const {
+    if (v > neg_inf()) {
+      bool done;
+      const int k = cls[c];
+      const int ch = lex_move(k, c, trie[m], wd[m], fc[m], mask + m * MW, rmask, 1, done);
+      if (ch < 0 || (done && !(cw[m] > neg_inf()))) {
+        v = neg_inf();
+      } else {
+        const float s = k == 0 ? __ldg(f.smear + ch) : k == 2 ? rsm[c] : 0.0f;
+        v = beam_lex_fuse(f, v, done ? __fadd_rn(lm[m], cw[m]) : lm[m], s, wn[m] + (int)done);
+      }
+    }
+    return v;
+  }
+  __device__ void keep(int o, int m) const {
+    node[o] = node[m];
+    lm[o] = lm[m];
+    trie[o] = trie[m];
+    wn[o] = wn[m];
+    wd[o] = wd[m];
+    cw[o] = cw[m];
+    cd[o] = cd[m];
+    fc[o] = fc[m];
+    sm[o] = sm[m];
+    for (int w = 0; w < MW; w++) mask[o * MW + w] = mask[m * MW + w];
+  }
+  /* the new slot's trie node and LM state; on a word end, the completion's weight and destination are looked up
+   * here, once, so that no LM lookup sits on the per-candidate path */
+  __device__ void extend(const BeamLex& f, int o, int m, int c, int) const {
+    bool done;
+    const int ch = lex_move(cls[c], c, trie[m], wd[m], fc[m], mask + m * MW, rmask, 1, done);
+    const int ln = done ? cd[m] : node[m];
+    node[o] = ln;
+    lm[o] = done ? __fadd_rn(lm[m], cw[m]) : lm[m];
+    wn[o] = wn[m] + (int)done;
+    trie[o] = ch;
+    const int w = __ldg(f.word + ch);
+    wd[o] = w;
+    fc[o] = __ldg(f.first + ch);
+    sm[o] = __ldg(f.smear + ch);
+    for (int i = 0; i < MW; i++) mask[o * MW + i] = __ldg(f.mask + (long long)ch * MW + i);
+    int d = 0;
+    cw[o] = w >= 0 ? lex_resolve(f, ln, w, d) : 0.0f;
+    cd[o] = d;
+  }
+  /* completes the pending word at a word end (a slot inside a word is dropped), then adds the end weight (dropped at
+   * -inf) */
+  __device__ float final(const BeamLex& f, int m, float am, int, int) const {
+    float l = lm[m];
+    int n = node[m], nw = wn[m];
     bool ok = true;
-    if (strie[m] != 0) {
-      ok = swd[m] >= 0 && scw[m] > neg_inf();
-      lm = __fadd_rn(lm, scw[m]);
-      node = scd[m];
+    if (trie[m] != 0) {
+      ok = wd[m] >= 0 && cw[m] > neg_inf();
+      l = __fadd_rn(l, cw[m]);
+      n = cd[m];
       nw++;
     }
-    const float we = ok ? (f.endw ? __ldg(f.endw + node) : 0.0f) : neg_inf();
-    lm = __fadd_rn(lm, we);
-    fin[tid] = we == neg_inf() ? neg_inf() : beam_fuse(f, stot[m], lm, nw);
-    lmf[tid] = lm;
-    nwd[tid] = nw;
+    const float we = ok ? (f.endw ? __ldg(f.endw + n) : 0.0f) : neg_inf();
+    l = __fadd_rn(l, we);
+    lm[m] = l;
+    wn[m] = nw;
+    return we == neg_inf() ? neg_inf() : beam_fuse(f, am, l, nw);
   }
-  __syncthreads();
-  int live = 0;
-  for (int i = 0; i < L; i++) live += fin[i] > neg_inf();
-  if (tid < L && fin[tid] > neg_inf()) {
-    int r = 0;
-    for (int i = 0; i < L; i++) r += fin[i] > fin[tid] || (fin[i] == fin[tid] && i < tid);
-    rank[r] = tid;
+  __device__ void hyp(const BeamLex& f, long long o, int m, float am) const {
+    if (f.am) f.am[o] = am;
+    if (f.lm) f.lm[o] = m >= 0 ? lm[m] : neg_inf();
+    if (f.counts) f.counts[o] = m >= 0 ? wn[m] : -1;
   }
-  __syncthreads();
-  int32_t* out = tokens + (long long)b * N * T;
-  int32_t* wout = f.words ? f.words + (long long)b * N * T : nullptr;
-  for (int n = tid; n < N; n += kBeamThreads) {
-    const int m = n < live ? rank[n] : -1;
-    const int len = m >= 0 ? slen[cur * K + m] : -1;
-    const long long o = (long long)b * N + n;
-    scores[o] = m >= 0 ? fin[m] : neg_inf();
-    if (f.am) f.am[o] = m >= 0 ? stot[cur * K + m] : neg_inf();
-    if (f.lm) f.lm[o] = m >= 0 ? lmf[m] : neg_inf();
-    if (f.counts) f.counts[o] = m >= 0 ? nwd[m] : -1;
-    lengths[o] = len;
-    int tt = Tb - 1, s = m;
-    for (int p = len - 1; p >= 0; p--) out[(long long)n * T + p] = beam_back(bpu, K, tt, s);
-    if (wout && len > 0) { // (the transcript was admitted: every move exists)
+  /* each hypothesis's word ids, read off its traced tokens (out, of this thread's hypotheses) by walking the trie,
+   * then -1; slot m0 + rank[n] holds hypothesis n < live, len its token count */
+  __device__ void words(const BeamLex& f, int b, int T, int N, int live, const int* rank, const int* len, int m0,
+                        const int32_t* out) const {
+    if (!f.words) return;
+    int32_t* wout = f.words + (long long)b * N * T;
+    for (int n = threadIdx.x; n < live && n < N; n += kBeamThreads) {
+      const int m = m0 + rank[n]; // (the transcript was admitted: every move exists)
       int node = 0, k = 0;
-      for (int p = 0; p < len; p++) {
-        const int c = out[(long long)n * T + p], cl = tcls[c];
+      for (int p = 0; p < len[m]; p++) {
+        const int c = out[(long long)n * T + p], cl = cls[c];
         if (cl != 0 && node != 0) wout[(long long)n * T + k++] = __ldg(f.word + node);
         if (cl == 1) {
           node = 0;
         } else {
           const int from = cl == 0 ? node : 0;
-          node = __ldg(f.first + from) + lex_rank(f.mask + (long long)from * f.MW, c);
+          node = __ldg(f.first + from) + lex_rank(f.mask + (long long)from * MW, c);
         }
       }
       if (node != 0) wout[(long long)n * T + k++] = __ldg(f.word + node);
     }
+    for (long long p = threadIdx.x; p < (long long)N * T; p += kBeamThreads) {
+      const int n = (int)(p / T);
+      if (p - (long long)n * T >= (n < live ? wn[m0 + rank[n]] : 0)) wout[p] = -1;
+    }
+  }
+};
+
+/*
+ * The dynamic shared memory of one CTA, one carve for the kernel and for the host's size: two hash arrays [2][K] of
+ * 8 bytes, then 4-byte words (control block, histogram, two emission rows, the two start-weight rows, the double-
+ * buffered state, the candidates' scratch and keys); with token pruning (F::on) the frame's tokens and token ->
+ * position map and per-warp counts; then the policy's BeamSlots.
+ */
+template <class F>
+struct BeamSmem {
+  uint64_t *hh, *hq; // [2][K] hash of the transcript, and of the transcript minus its last token
+  int *ctl, *hist; // [16] control block, [256] histogram
+  float* erow; // [2][C]
+  float *w0, *wb; // [C] weight of a token entered from p_blank at frame 0 (BIGRAM sigma, ASG start), at frames >= 1
+                  // (BIGRAM W[c][blank])
+  float *spb, *spl, *stot; // [2][K] p_blank, p_label, logsumexp(p_blank, p_label)
+  int *slen, *slast, *spar; // [2][K] length, last token (-1: the empty transcript), the slot holding the transcript
+                            // minus its last token (or -1)
+  float *kpb, *kpl; // [K] kept candidates' states
+  int *kslot, *src, *widx; // [K] old slot -> its kept beam's new slot (or -1); new slot -> candidate; winners:
+                           // candidate
+  uint32_t *wkey, *keys; // [K] winners: key; [K + K*P]: kept beams r at r, extension (s, p) at L + s*P + p
+  int *ptok, *ppos, *wcnt; // (F::on) [P] the frame's tokens, ascending; [C] token -> position in ptok, or -1; [8]
+                           // selected tokens per warp
+  BeamSlots<F> x;
+  int bytes;
+  __host__ __device__ BeamSmem(char* base, int K, int C) {
+    BeamCarve m{base};
+    hh = m.take<uint64_t>(2 * K);
+    hq = m.take<uint64_t>(2 * K);
+    ctl = m.take<int>(16);
+    hist = m.take<int>(256);
+    erow = m.take<float>(2 * C);
+    w0 = m.take<float>(C);
+    wb = m.take<float>(C);
+    spb = m.take<float>(2 * K);
+    spl = m.take<float>(2 * K);
+    stot = m.take<float>(2 * K);
+    slen = m.take<int>(2 * K);
+    slast = m.take<int>(2 * K);
+    spar = m.take<int>(2 * K);
+    kpb = m.take<float>(K);
+    kpl = m.take<float>(K);
+    kslot = m.take<int>(K);
+    src = m.take<int>(K);
+    widx = m.take<int>(K);
+    wkey = m.take<uint32_t>(K);
+    keys = m.take<uint32_t>(K + K * C);
+    ptok = ppos = wcnt = nullptr;
+    if (F::on) {
+      ptok = m.take<int>(C);
+      ppos = m.take<int>(C);
+      wcnt = m.take<int>(8);
+    }
+    x.carve(m, K, C);
+    bytes = m.bytes;
+  }
+};
+
+/* status 1 or 2: NaN scores, -1 lengths and rows in every output of the policy */
+template <class F>
+__device__ void beam_flag(int b, int T, int N, int code, int32_t* tokens, int32_t* lengths, float* scores,
+                          int32_t* status, const F& f) {
+  const int tid = threadIdx.x;
+  for (long long p = tid; p < (long long)N * T; p += kBeamThreads) {
+    tokens[(long long)b * N * T + p] = -1;
+    if (f.words) f.words[(long long)b * N * T + p] = -1;
+  }
+  for (int n = tid; n < N; n += kBeamThreads) {
+    const long long o = (long long)b * N + n;
+    scores[o] = CUDART_NAN_F;
+    lengths[o] = -1;
+    if (f.am) f.am[o] = CUDART_NAN_F;
+    if (f.lm) f.lm[o] = CUDART_NAN_F;
+    if (f.counts) f.counts[o] = -1;
+  }
+  if (tid == 0 && status) status[b] = code;
+}
+
+/*
+ * After frame T_b - 1: each live slot's final score from the policy (dropped at -inf), and the N-best are the top
+ * live beams by it, ties to the lower slot (the search's own order).  fin ([K]) holds each slot's final score, rank
+ * ([K]) rank -> slot.  For BeamNoLm this is the slots' own order, exactly: they are ranked by (key, candidate order)
+ * and the key is order-preserving on stot, so ranking by stot with ties to the lower slot is the identity, no slot is
+ * dropped, and the tie check compares what the search compared.
+ */
+template <class F>
+__device__ void beam_finish(int b, int T, int Tb, int C, int K, int N, const uint16_t* bpu, int cur, const int* ctl,
+                            const float* stot, const int* slen, const BeamSlots<F>& x, float* fin, int* rank,
+                            int32_t* tokens, int32_t* lengths, float* scores, int32_t* status, const F& f) {
+  const int tid = threadIdx.x;
+  const int L = ctl[kBcL];
+  const int m0 = cur * K;
+  if (tid < L) fin[tid] = x.final(f, m0 + tid, stot[m0 + tid], slen[m0 + tid], C);
+  __syncthreads();
+  int live = 0;
+  for (int i = 0; i < L; i++) live += fin[i] > neg_inf();
+  if (tid < L && fin[tid] > neg_inf()) {
+    int r = 0;
+    for (int i = 0; i < L; i++) r += fin[i] > fin[tid] || (fin[i] == fin[tid] && i < tid);
+    rank[r] = tid;
   }
   __syncthreads();
+  int32_t* out = tokens + (long long)b * N * T;
+  for (int n = tid; n < N; n += kBeamThreads) {
+    const int r = n < live ? rank[n] : -1;
+    const int len = r >= 0 ? slen[m0 + r] : -1;
+    const long long o = (long long)b * N + n;
+    scores[o] = r >= 0 ? fin[r] : neg_inf();
+    x.hyp(f, o, r >= 0 ? m0 + r : -1, r >= 0 ? stot[m0 + r] : neg_inf());
+    lengths[o] = len;
+    int tt = Tb - 1, s = r;
+    for (int p = len - 1; p >= 0; p--) out[(long long)n * T + p] = beam_back(bpu, K, tt, s);
+  }
   for (long long p = tid; p < (long long)N * T; p += kBeamThreads) {
     const int n = (int)(p / T);
-    const int r = n < live ? rank[n] : -1;
-    if (p - (long long)n * T >= (r >= 0 ? slen[cur * K + r] : 0)) out[p] = -1;
-    if (wout && p - (long long)n * T >= (r >= 0 ? nwd[r] : 0)) wout[p] = -1;
+    if (p - (long long)n * T >= (n < live ? slen[m0 + rank[n]] : 0)) out[p] = -1;
   }
+  x.words(f, b, T, N, live, rank, slen, m0, out);
   if (tid == 0) {
     bool tied = ctl[kBcTieAny] != 0;
     for (int n = 0; n + 1 < live && n < N; n++) tied |= fin[rank[n]] == fin[rank[n + 1]];
@@ -451,8 +607,8 @@ __device__ void beam_finish_lex(int b, int T, int Tb, int K, int N, const uint16
  * One CTA of kBeamThreads per utterance b.  emissions [B][T][C] of E; input_lens [B] (nullable: T); kind
  * GTNB_DENSE_CTC / _BIGRAM / _ASG; wt [C][C] (transposed W), wfirst [C] (BIGRAM sigma, ASG start weights) and wbad
  * [C] from beam_weights_kernel (unused for CTC); blank (CTC, BIGRAM); K beams, N hypotheses.  bp: [B][T][K] back-
- * pointers (scratch).  Out: tokens [B][N][T], lengths [B][N], scores [B][N], status [B] (nullable).  F: BeamNoLm, or
- * BeamLm with the LM, its weights, token_beam and the am / lm outputs.
+ * pointers (scratch).  Out: tokens [B][N][T], lengths [B][N], scores [B][N], status [B] (nullable), and the policy's
+ * own outputs.  F: the policy (BeamNoLm, BeamLm, BeamLex).
  */
 template <class E, class Hash, class F = BeamNoLm>
 __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
@@ -461,55 +617,22 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     int N, uint16_t* bp, int32_t* __restrict__ tokens, int32_t* __restrict__ lengths, float* __restrict__ scores,
     int32_t* __restrict__ status, const F fz = F()) {
   GTNB_DYNAMIC_SMEM(uint64_t, hsm);
-  uint64_t* hh = hsm; // [2][K] hash of the transcript
-  uint64_t* hq = hsm + 2 * K; // [2][K] hash of the transcript minus its last token
-  int* ctl = reinterpret_cast<int*>(hsm + 4 * K);
-  int* hist = ctl + 16;
-  float* erow = reinterpret_cast<float*>(hist + 256); // [2][C]
-  float* w0 = erow + 2 * C; // weight of a token entered from p_blank at frame 0 (BIGRAM sigma, ASG start)
-  float* wb = w0 + C; // ... at frames >= 1 (BIGRAM W[c][blank])
-  float* spb = wb + C; // [2][K] p_blank
-  float* spl = spb + 2 * K; // [2][K] p_label
-  float* stot = spl + 2 * K; // [2][K] logsumexp(p_blank, p_label)
-  int* slen = reinterpret_cast<int*>(stot + 2 * K); // [2][K]
-  int* slast = slen + 2 * K; // [2][K] last token, -1 for the empty transcript
-  int* spar = slast + 2 * K; // [2][K] the slot holding the transcript minus its last token, or -1
-  float* kpb = reinterpret_cast<float*>(spar + 2 * K); // [K] kept candidates' states
-  float* kpl = kpb + K;
-  int* kslot = reinterpret_cast<int*>(kpl + K); // [K] old slot -> its kept beam's new slot, or -1
-  int* src = kslot + K; // [K] new slot -> candidate
-  int* widx = src + K; // [K] winners: candidate
-  uint32_t* wkey = reinterpret_cast<uint32_t*>(widx + K); // [K] winners: key
-  uint32_t* keys = wkey + K; // [K + K*P]: kept beams r at r, extension (s, p) at L + s*P + p
-  // (BeamLm only)
-  int* snode = reinterpret_cast<int*>(keys + K + K * C); // [2][K] LM node
-  float* slm = reinterpret_cast<float*>(snode + 2 * K); // [2][K] lmacc
-  int* ptok = reinterpret_cast<int*>(slm + 2 * K); // [P] the frame's tokens, ascending
-  int* ppos = ptok + C; // [C] token -> its position in ptok, or -1
-  int* wcnt = ppos + C; // [8] selected tokens per warp
-  // (BeamLex only)
-  const int MW = (C + 31) / 32;
-  int* strie = wcnt + 8; // [2][K] trie node (the root is 0, its children 1, 2, ... in token order)
-  int* swn = strie + 2 * K; // [2][K] word count
-  int* swd = swn + 2 * K; // [2][K] word id of the trie node, or -1
-  float* scw = reinterpret_cast<float*>(swd + 2 * K); // [2][K] completion weight w(LM node, word id), word ends
-  int* scd = reinterpret_cast<int*>(scw + 2 * K); // [2][K] ... and its LM destination
-  int* sfc = scd + 2 * K; // [2][K] first child
-  float* ssm = reinterpret_cast<float*>(sfc + 2 * K); // [2][K] smear
-  uint32_t* smask = reinterpret_cast<uint32_t*>(ssm + 2 * K); // [2][K][MW] child mask
-  uint32_t* rmask = smask + 2 * K * MW; // [MW] the root's child mask
-  float* rsm = reinterpret_cast<float*>(rmask + MW); // [C] smear of the root's child labelled c
-  int* tcls = reinterpret_cast<int*>(rsm + C); // [C] token classes
+  const BeamSmem<F> sm(reinterpret_cast<char*>(hsm), K, C);
+  uint64_t *hh = sm.hh, *hq = sm.hq;
+  int *ctl = sm.ctl, *hist = sm.hist;
+  float *erow = sm.erow, *w0 = sm.w0, *wb = sm.wb, *spb = sm.spb, *spl = sm.spl, *stot = sm.stot;
+  int *slen = sm.slen, *slast = sm.slast, *spar = sm.spar;
+  float *kpb = sm.kpb, *kpl = sm.kpl;
+  int *kslot = sm.kslot, *src = sm.src, *widx = sm.widx;
+  uint32_t *wkey = sm.wkey, *keys = sm.keys;
+  int *ptok = sm.ptok, *ppos = sm.ppos, *wcnt = sm.wcnt;
+  const BeamSlots<F>& xs = sm.x;
   const int P = F::on ? fz.P : C;
 
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int Tb = input_lens ? input_lens[b] : T;
   if (!(Tb >= 0 && Tb <= T)) {
-    beam_flag(b, T, N, 2, tokens, lengths, scores, status);
-    if constexpr (F::lex)
-      beam_flag_lex(b, T, N, fz);
-    else if constexpr (F::on)
-      beam_flag_lm(b, N, fz);
+    beam_flag(b, T, N, 2, tokens, lengths, scores, status, fz);
     return;
   }
   const E* em = emissions + (long long)b * T * C;
@@ -525,10 +648,6 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     slast[0] = -1;
     spar[0] = -1;
     hh[0] = hq[0] = 0;
-    if constexpr (F::on) {
-      snode[0] = fz.lmw ? fz.start : 0;
-      slm[0] = 0.0f;
-    }
   }
   if constexpr (F::on) {
     if (tid < C) { // (every frame's selection when P < C)
@@ -536,20 +655,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       ppos[tid] = tid;
     }
   }
-  if constexpr (F::lex) {
-    if (tid == 0) {
-      snode[0] = fz.start;
-      strie[0] = swn[0] = scd[0] = 0;
-      swd[0] = -1;
-      scw[0] = ssm[0] = 0.0f;
-      sfc[0] = __ldg(fz.first);
-    }
-    if (tid < MW) smask[tid] = rmask[tid] = __ldg(fz.mask + tid);
-    if (tid < C) {
-      tcls[tid] = __ldg(fz.cls + tid);
-      rsm[tid] = lex_has(fz.mask, tid) ? __ldg(fz.smear + 1 + lex_rank(fz.mask, tid)) : 0.0f;
-    }
-  }
+  xs.init(fz, tid, C);
   __syncthreads();
   if (tid < C) {
     w0[tid] = kind == GTNB_DENSE_CTC ? 0.0f : wfirst[tid];
@@ -572,12 +678,6 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     const float* wp = t == 0 ? w0 : wb;
     const float *pb0 = spb + cur * K, *pl0 = spl + cur * K, *tot0 = stot + cur * K;
     const int *len0 = slen + cur * K, *last0 = slast + cur * K, *par0 = spar + cur * K;
-    const int* node0 = snode + cur * K;
-    const float* lm0 = slm + cur * K;
-    const int *trie0 = strie + cur * K, *wn0 = swn + cur * K, *wd0 = swd + cur * K, *cd0 = scd + cur * K;
-    const int* fc0 = sfc + cur * K;
-    const float *cw0 = scw + cur * K, *sm0 = ssm + cur * K;
-    const uint32_t* mask0 = smask + cur * K * MW;
 
     if constexpr (F::on) {
       // token pruning: the P best tokens of the frame (blank excluded for CTC and BIGRAM), ties to the lower token;
@@ -625,12 +725,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       }
       kpb[tid] = nb;
       kpl[tid] = nl;
-      float v = beam_lse2(nb, nl);
-      if constexpr (F::lex)
-        v = beam_lex_fuse(fz, v, lm0[tid], sm0[tid], wn0[tid]);
-      else if constexpr (F::on)
-        v = beam_fuse(fz, v, lm0[tid], len0[tid]);
-      keys[tid] = beam_key(v);
+      keys[tid] = beam_key(xs.key(fz, beam_lse2(nb, nl), cur * K + tid, len0[tid]));
       kslot[tid] = -1;
     }
     if (tid == 0) ctl[kBcNwin] = ctl[kBcDone] = 0;
@@ -639,42 +734,9 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       int s = tid / P, p = tid - s * P;
       for (int q = tid; q < next; q += kBeamThreads) {
         const int c = F::on ? ptok[p] : p;
-        float v = neg_inf();
-        if constexpr (!F::on) {
-          if (kind == GTNB_DENSE_ASG || c != blank) {
-            const float pb = pb0[s], pl = pl0[s];
-            const int l = last0[s];
-            if (kind == GTNB_DENSE_CTC) {
-              v = (c == l ? pb : tot0[s]) + er[c];
-            } else {
-              const float from_pl = l >= 0 && (kind == GTNB_DENSE_ASG || c != l) ? pl + __ldg(wt + (long long)l * C + c)
-                                                                                   : neg_inf();
-              v = beam_lse2(pb + wp[c], from_pl) + er[c];
-            }
-          }
-        } else if constexpr (F::lex) {
-          v = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
-          if (v > neg_inf()) { // (admission is a bit test; an in-word child's smear is one row per beam, via the L2)
-            bool done;
-            const int k = tcls[c];
-            const int ch = lex_move(k, c, trie0[s], wd0[s], fc0[s], mask0 + s * MW, rmask, 1, done);
-            if (ch < 0 || (done && !(cw0[s] > neg_inf()))) {
-              v = neg_inf();
-            } else {
-              const float sm = k == 0 ? __ldg(fz.smear + ch) : k == 2 ? rsm[c] : 0.0f;
-              v = beam_lex_fuse(fz, v, done ? __fadd_rn(lm0[s], cw0[s]) : lm0[s], sm, wn0[s] + (int)done);
-            }
-          }
-        } else {
-          v = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
-          if (v > neg_inf() && fz.lmw) {
-            const float w = __ldg(fz.lmw + (long long)node0[s] * (C + 1) + c); // (one row per beam, via the L2)
-            v = w == neg_inf() ? w : beam_fuse(fz, v, lm0[s] + w, len0[s] + 1);
-          } else if (v > neg_inf()) {
-            v = beam_fuse(fz, v, lm0[s], len0[s] + 1);
-          }
-        }
-        keys[L + q] = beam_key(v);
+        const float am = F::on ? beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c)
+                               : beam_ext_am(kind, blank, C, er, wp, wt, pb0, pl0, tot0, last0, s, c);
+        keys[L + q] = beam_key(xs.ext_key(fz, am, cur * K + s, c, len0[s], C));
         p += kBeamThreads;
         while (p >= P) {
           p -= P;
@@ -687,20 +749,14 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     // merge: extension (par[r], last[r]) is r's transcript (absent when last[r] was pruned at this frame)
     if (tid < L && par0[tid] >= 0 && (!F::on || ppos[last0[tid]] >= 0)) {
       const int q = L + par0[tid] * P + (F::on ? ppos[last0[tid]] : last0[tid]);
-      float v = beam_key_float(keys[q]);
-      if constexpr (F::on) { // (the key holds the fused score: the acoustic one again)
-        const int s = par0[tid];
-        v = keys[q] ? beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], last0[tid])
-                    : neg_inf();
-      }
+      const int s = par0[tid];
+      // (BeamNoLm: the key is the acoustic score; otherwise it holds the fused one: the acoustic one again)
+      const float v = !F::on ? beam_key_float(keys[q])
+                      : keys[q] ? beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], last0[tid])
+                                : neg_inf();
       keys[q] = 0u;
       kpl[tid] = beam_lse2(kpl[tid], v);
-      v = beam_lse2(kpb[tid], kpl[tid]);
-      if constexpr (F::lex)
-        v = beam_lex_fuse(fz, v, lm0[tid], sm0[tid], wn0[tid]);
-      else if constexpr (F::on)
-        v = beam_fuse(fz, v, lm0[tid], len0[tid]);
-      keys[tid] = beam_key(v);
+      keys[tid] = beam_key(xs.key(fz, beam_lse2(kpb[tid], kpl[tid]), cur * K + tid, len0[tid]));
     }
     __syncthreads();
     // radix select of the K-th key among the nonzero keys
@@ -824,7 +880,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
         n += ki > k || (ki == k && widx[i] < j);
       }
       uint32_t code;
-      float am = 0.0f; // (BeamLm: the acoustic score; the key holds the fused one)
+      float am; // (BeamNoLm: the key; otherwise it holds the fused score: the acoustic one again)
       if (j < L) {
         spb[nx * K + n] = kpb[j];
         spl[nx * K + n] = kpl[j];
@@ -832,62 +888,25 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
         slast[nx * K + n] = last0[j];
         hh[nx * K + n] = hh[cur * K + j];
         hq[nx * K + n] = hq[cur * K + j];
-        if constexpr (F::on) {
-          am = beam_lse2(kpb[j], kpl[j]);
-          snode[nx * K + n] = node0[j];
-          slm[nx * K + n] = lm0[j];
-        }
-        if constexpr (F::lex) {
-          const int o = nx * K + n;
-          strie[o] = trie0[j];
-          swn[o] = wn0[j];
-          swd[o] = wd0[j];
-          scw[o] = cw0[j];
-          scd[o] = cd0[j];
-          sfc[o] = fc0[j];
-          ssm[o] = sm0[j];
-          for (int w = 0; w < MW; w++) smask[o * MW + w] = mask0[j * MW + w];
-        }
+        am = F::on ? beam_lse2(kpb[j], kpl[j]) : beam_key_float(k);
+        xs.keep(nx * K + n, cur * K + j);
         kslot[j] = n;
         code = (uint32_t)j << 9;
       } else {
         const int s = (j - L) / P, p = j - L - s * P;
         const int c = F::on ? ptok[p] : p;
-        if constexpr (F::lex) {
-          // the new slot's trie node and LM state; on a word end, the completion's weight and destination are looked
-          // up here, once, so that no LM lookup sits on the per-candidate path
-          am = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
-          bool done;
-          const int ch = lex_move(tcls[c], c, trie0[s], wd0[s], fc0[s], mask0 + s * MW, rmask, 1, done);
-          const int o = nx * K + n;
-          const int ln = done ? cd0[s] : node0[s];
-          snode[o] = ln;
-          slm[o] = done ? __fadd_rn(lm0[s], cw0[s]) : lm0[s];
-          swn[o] = wn0[s] + (int)done;
-          strie[o] = ch;
-          const int wd = __ldg(fz.word + ch);
-          swd[o] = wd;
-          sfc[o] = __ldg(fz.first + ch);
-          ssm[o] = __ldg(fz.smear + ch);
-          for (int w = 0; w < MW; w++) smask[o * MW + w] = __ldg(fz.mask + (long long)ch * MW + w);
-          int d = 0;
-          scw[o] = wd >= 0 ? lex_resolve(fz, ln, wd, d) : 0.0f;
-          scd[o] = d;
-        } else if constexpr (F::on) {
-          am = beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c);
-          const long long at = (long long)node0[s] * (C + 1) + c;
-          snode[nx * K + n] = fz.lmw ? __ldg(fz.lmd + at) : 0;
-          slm[nx * K + n] = fz.lmw ? lm0[s] + __ldg(fz.lmw + at) : lm0[s];
-        }
+        am = F::on ? beam_ext_am(kind, blank, C, er, wp, wt, pb0[s], pl0[s], tot0[s], last0[s], c)
+                   : beam_key_float(k);
+        xs.extend(fz, nx * K + n, cur * K + s, c, C);
         spb[nx * K + n] = neg_inf();
-        spl[nx * K + n] = F::on ? am : beam_key_float(k);
+        spl[nx * K + n] = am;
         slen[nx * K + n] = len0[s] + 1;
         slast[nx * K + n] = c;
         hh[nx * K + n] = Hash::combine(hh[cur * K + s], c);
         hq[nx * K + n] = hh[cur * K + s];
         code = ((uint32_t)s << 9) | 256u | (uint32_t)c;
       }
-      stot[nx * K + n] = F::on ? am : beam_key_float(k);
+      stot[nx * K + n] = am;
       src[n] = j;
       bpu[(long long)t * K + n] = (uint16_t)code;
     }
@@ -920,41 +939,20 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
   }
 
   if (ctl[kBcBad]) {
-    beam_flag(b, T, N, 1, tokens, lengths, scores, status);
-    if constexpr (F::lex)
-      beam_flag_lex(b, T, N, fz);
-    else if constexpr (F::on)
-      beam_flag_lm(b, N, fz);
+    beam_flag(b, T, N, 1, tokens, lengths, scores, status, fz);
     return;
   }
-  if constexpr (F::lex) {
-    beam_finish_lex(b, T, Tb, K, N, bpu, cur, ctl, stot, slen, snode, slm, strie, swn, swd, scw, scd, tcls, kpb, kpl,
-                    widx, src, tokens, lengths, scores, status, fz);
-    return;
-  } else if constexpr (F::on) {
-    beam_finish_lm(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, snode, slm, kpb, kpl, src, tokens, lengths, scores,
-                   status, fz);
-    return;
-  }
-  const int L = ctl[kBcL];
-  int32_t* out = tokens + (long long)b * N * T;
-  for (int n = tid; n < N; n += kBeamThreads) {
-    const int len = n < L ? slen[cur * K + n] : -1;
-    scores[(long long)b * N + n] = n < L ? stot[cur * K + n] : neg_inf();
-    lengths[(long long)b * N + n] = len;
-    int tt = Tb - 1, s = n;
-    for (int p = len - 1; p >= 0; p--) out[(long long)n * T + p] = beam_back(bpu, K, tt, s);
-  }
-  for (long long p = tid; p < (long long)N * T; p += kBeamThreads) {
-    const int n = (int)(p / T);
-    if (p - (long long)n * T >= (n < L ? slen[cur * K + n] : 0)) out[p] = -1;
-  }
-  if (tid == 0) {
-    bool tied = ctl[kBcTieAny] != 0;
-    for (int n = 0; n + 1 < L && n < N; n++) tied |= stot[cur * K + n] == stot[cur * K + n + 1];
-    if (status) status[b] = tied ? 3 : 0;
-  }
+  beam_finish(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, xs, kpb, src, tokens, lengths, scores, status, fz);
 }
+
+/* the dynamic shared memory of beam_decode_kernel<E, Hash, F> at K beams and C tokens; the by-policy names are the
+ * same carve, for callers that size one policy's launch (the per-policy emulation drivers) */
+template <class F = BeamNoLm>
+long long beam_smem_bytes(int K, int C) {
+  return BeamSmem<F>(nullptr, K, C).bytes;
+}
+inline long long beam_lm_smem_bytes(int K, int C) { return beam_smem_bytes<BeamLm>(K, C); }
+inline long long beam_lex_smem_bytes(int K, int C) { return beam_smem_bytes<BeamLex>(K, C); }
 
 #ifndef GTNB_HOST_EMU
 
@@ -969,104 +967,36 @@ int launch_beam_weights(gtnb_ctx* ctx, int C, int kind, const float* trans_w, fl
   return GTNB_OK;
 }
 
+template <class F>
 int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
                        const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
                        int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
-                       int32_t* status) {
+                       int32_t* status, const F& f) {
   if (B <= 0) return GTNB_OK;
-  const long long smem = beam_smem_bytes(K, C);
-#define GTNB_BEAM_LAUNCH(E_)                                                                                  \
-  {                                                                                                           \
-    if (smem > 48 * 1024) {                                                                                   \
-      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash, BeamNoLm>);                   \
-      if (rc__) return rc__;                                                                                  \
-    }                                                                                                         \
-    GTNB_LAUNCH(ctx, "beam_decode",                                                                           \
-                beam_decode_kernel<E_, BeamHash, BeamNoLm><<<B, kBeamThreads, smem, ctx->stream>>>(                     \
-                    static_cast<const E_*>(emissions), T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, \
-                    tokens, lengths, scores, status));                                                        \
-  }
-  if (dtype == GTNB_BF16)
-    GTNB_BEAM_LAUNCH(bf16_t)
-  else if (dtype == GTNB_F16)
-    GTNB_BEAM_LAUNCH(f16_t)
-  else
-    GTNB_BEAM_LAUNCH(float)
-#undef GTNB_BEAM_LAUNCH
-  return GTNB_OK;
+  const long long smem = beam_smem_bytes<F>(K, C);
+  // (the names the per-kernel profile reports)
+  const char* name = std::is_same_v<F, BeamLex> ? "beam_decode_lexicon" : F::on ? "beam_decode_lm" : "beam_decode";
+  const auto run = [&](const auto* e) {
+    using E = std::remove_const_t<std::remove_pointer_t<decltype(e)>>;
+    if (smem > 48 * 1024)
+      if (const int rc = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E, BeamHash, F>)) return rc;
+    GTNB_LAUNCH(ctx, name,
+                beam_decode_kernel<E, BeamHash, F><<<B, kBeamThreads, smem, ctx->stream>>>(
+                    e, T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, tokens, lengths, scores, status, f));
+    return (int)GTNB_OK;
+  };
+  if (dtype == GTNB_BF16) return run(static_cast<const bf16_t*>(emissions));
+  if (dtype == GTNB_F16) return run(static_cast<const f16_t*>(emissions));
+  return run(static_cast<const float*>(emissions));
 }
-
-int launch_beam_decode_lm(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
-                          const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
-                          int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
-                          int32_t* status, const BeamLmLaunch& lm) {
-  if (B <= 0) return GTNB_OK;
-  const long long smem = beam_lm_smem_bytes(K, C);
-  const BeamLm f{lm.P, lm.lmw, lm.lmd, lm.start, lm.lm_weight, lm.token_bonus, lm.am_scores, lm.lm_scores};
-#define GTNB_BEAM_LM_LAUNCH(E_)                                                                               \
-  {                                                                                                           \
-    if (smem > 48 * 1024) {                                                                                   \
-      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash, BeamLm>);           \
-      if (rc__) return rc__;                                                                                  \
-    }                                                                                                         \
-    GTNB_LAUNCH(ctx, "beam_decode_lm",                                                                        \
-                beam_decode_kernel<E_, BeamHash, BeamLm><<<B, kBeamThreads, smem, ctx->stream>>>(             \
-                    static_cast<const E_*>(emissions), T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, \
-                    tokens, lengths, scores, status, f));                                                     \
-  }
-  if (dtype == GTNB_BF16)
-    GTNB_BEAM_LM_LAUNCH(bf16_t)
-  else if (dtype == GTNB_F16)
-    GTNB_BEAM_LM_LAUNCH(f16_t)
-  else
-    GTNB_BEAM_LM_LAUNCH(float)
-#undef GTNB_BEAM_LM_LAUNCH
-  return GTNB_OK;
-}
-
-int launch_beam_decode_lex(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype,
-                           const int32_t* input_lens, int kind, const float* wt, const float* wfirst,
-                           const int32_t* wbad, int blank, int K, int N, uint16_t* bp, int32_t* tokens,
-                           int32_t* lengths, float* scores, int32_t* status, const BeamLexLaunch& x) {
-  if (B <= 0) return GTNB_OK;
-  const long long smem = beam_lex_smem_bytes(K, C);
-  BeamLex f;
-  static_cast<BeamLm&>(f) = BeamLm{x.P, nullptr, nullptr, x.start, x.lm_weight, x.word_bonus, x.am_scores,
-                                   x.lm_scores};
-  f.cls = x.cls;
-  f.MW = (C + 31) / 32;
-  f.mask = x.mask;
-  f.first = x.first;
-  f.word = x.word;
-  f.smear = x.smear;
-  f.hash = x.hash;
-  f.hmul = x.hmul;
-  f.hbits = x.hbits;
-  f.bow = x.bow;
-  f.bod = x.bod;
-  f.endw = x.endw;
-  f.words = x.words;
-  f.counts = x.counts;
-#define GTNB_BEAM_LEX_LAUNCH(E_)                                                                              \
-  {                                                                                                           \
-    if (smem > 48 * 1024) {                                                                                   \
-      const int rc__ = ensure_max_smem(ctx, (const void*)beam_decode_kernel<E_, BeamHash, BeamLex>);          \
-      if (rc__) return rc__;                                                                                  \
-    }                                                                                                         \
-    GTNB_LAUNCH(ctx, "beam_decode_lexicon",                                                                   \
-                beam_decode_kernel<E_, BeamHash, BeamLex><<<B, kBeamThreads, smem, ctx->stream>>>(            \
-                    static_cast<const E_*>(emissions), T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, \
-                    tokens, lengths, scores, status, f));                                                     \
-  }
-  if (dtype == GTNB_BF16)
-    GTNB_BEAM_LEX_LAUNCH(bf16_t)
-  else if (dtype == GTNB_F16)
-    GTNB_BEAM_LEX_LAUNCH(f16_t)
-  else
-    GTNB_BEAM_LEX_LAUNCH(float)
-#undef GTNB_BEAM_LEX_LAUNCH
-  return GTNB_OK;
-}
+#define GTNB_BEAM_POLICY(F_)                                                                                     \
+  template int launch_beam_decode<F_>(gtnb_ctx*, int, int, int, const void*, int, const int32_t*, int,          \
+                                      const float*, const float*, const int32_t*, int, int, int, uint16_t*,       \
+                                      int32_t*, int32_t*, float*, int32_t*, const F_&);
+GTNB_BEAM_POLICY(BeamNoLm)
+GTNB_BEAM_POLICY(BeamLm)
+GTNB_BEAM_POLICY(BeamLex)
+#undef GTNB_BEAM_POLICY
 
 #endif // GTNB_HOST_EMU
 

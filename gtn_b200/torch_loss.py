@@ -795,20 +795,26 @@ class BeamDecode(NamedTuple):
     status: torch.Tensor
 
 
-@torch.no_grad()
-def _beam_decode(name, emissions, transitions, input_lengths, kind, beam, nbest, blank):
-    """gtnb_beam_decode_async on the current stream"""
+def _beam_inputs(emissions, transitions, input_lengths, kind):
+    """The beam decoders' common inputs, checked: (emissions contiguous, transitions contiguous or None for CTC,
+    input lengths as _decode_lengths gives them, the dtype code)"""
     assert emissions.is_cuda and emissions.dim() == 3
     assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
     e = emissions.contiguous()
-    B, T, Cn = e.shape
+    Cn = e.shape[2]
     w = None
     if kind != capi.DENSE_CTC:
         assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
         assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
         w = transitions.detach().contiguous()
-    il = _decode_lengths(e, input_lengths)
-    dtype = _EMISSION_DTYPES[e.dtype]
+    return e, w, _decode_lengths(e, input_lengths), _EMISSION_DTYPES[e.dtype]
+
+
+@torch.no_grad()
+def _beam_decode(name, emissions, transitions, input_lengths, kind, beam, nbest, blank):
+    """gtnb_beam_decode_async on the current stream"""
+    e, w, il, dtype = _beam_inputs(emissions, transitions, input_lengths, kind)
+    B, T, Cn = e.shape
     g = _async_ctx(e.device, name)
     lib = capi.lib()
     ws, nbytes = _workspace(g, e.device, lib.gtnb_beam_decode_async_workspace, B, T, Cn, dtype, kind, int(beam),
@@ -909,18 +915,9 @@ class LMBeamDecode(NamedTuple):
 def _lm_beam_decode(name, emissions, transitions, lm, lm_weight, token_bonus, beam, nbest, token_beam, input_lengths,
                     kind, blank):
     """gtnb_beam_decode_lm_async on the current stream"""
-    assert emissions.is_cuda and emissions.dim() == 3
-    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
-    e = emissions.contiguous()
+    e, w, il, dtype = _beam_inputs(emissions, transitions, input_lengths, kind)
     B, T, Cn = e.shape
-    w = None
-    if kind != capi.DENSE_CTC:
-        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
-        assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
-        w = transitions.detach().contiguous()
     assert lm is None or isinstance(lm, LanguageModel)
-    il = _decode_lengths(e, input_lengths)
-    dtype = _EMISSION_DTYPES[e.dtype]
     P = Cn if token_beam is None else int(token_beam)
     g = _async_ctx(e.device, name)
     lib = capi.lib()
@@ -1056,18 +1053,9 @@ class LexiconBeamDecode(NamedTuple):
 def _lexicon_beam_decode(name, emissions, transitions, lexicon, lm_weight, word_bonus, beam, nbest, token_beam,
                          input_lengths, kind, blank):
     """gtnb_beam_decode_lexicon_async on the current stream"""
-    assert emissions.is_cuda and emissions.dim() == 3
-    assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
-    e = emissions.contiguous()
+    e, w, il, dtype = _beam_inputs(emissions, transitions, input_lengths, kind)
     B, T, Cn = e.shape
-    w = None
-    if kind != capi.DENSE_CTC:
-        assert transitions.is_cuda and transitions.device == e.device and transitions.dtype == torch.float32
-        assert transitions.numel() == (Cn * Cn if kind == capi.DENSE_BIGRAM else Cn + Cn * Cn)
-        w = transitions.detach().contiguous()
     assert isinstance(lexicon, Lexicon)
-    il = _decode_lengths(e, input_lengths)
-    dtype = _EMISSION_DTYPES[e.dtype]
     P = Cn if token_beam is None else int(token_beam)
     g = _async_ctx(e.device, name)
     lib = capi.lib()

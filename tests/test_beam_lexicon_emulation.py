@@ -29,7 +29,7 @@ HMUL = 0x9E3779B97F4A7C15
 
 @pytest.fixture(scope="module")
 def emu():
-    lib = C_.CDLL(emu_build.build("beam_lexicon", ["k_beam.cu"]))
+    lib = C_.CDLL(emu_build.build("beam", ["k_beam.cu"]))
     lib.emu_beam_lexicon.argtypes = ([C_.c_int] * 3 + [vp, C_.c_int, vp, C_.c_int, vp] + [C_.c_int] * 3 + [vp] * 6 +
                                      [C_.c_ulonglong, C_.c_int, vp, vp, vp, C_.c_int, C_.c_float, C_.c_float,
                                       C_.c_int, C_.c_int] + [vp] * 8)

@@ -25,7 +25,7 @@ F32, BF16, F16 = 0, 1, 2
 
 @pytest.fixture(scope="module")
 def emu():
-    lib = C_.CDLL(emu_build.build("beam_lm", ["k_beam.cu"]))
+    lib = C_.CDLL(emu_build.build("beam", ["k_beam.cu"]))
     lib.emu_beam_lm.argtypes = [C_.c_int, C_.c_int, C_.c_int, vp, C_.c_int, vp, C_.c_int, vp, C_.c_int, C_.c_int,
                                 C_.c_int, vp, vp, C_.c_int, C_.c_float, C_.c_float, C_.c_int, C_.c_int, vp, vp, vp, vp,
                                 vp, vp]
