@@ -293,7 +293,6 @@ inline void prof_end(gtnb_ctx* ctx) {
 /* Opt a kernel in to the full dynamic shared-memory window, once per (device, kernel).  The
  * attribute is process-wide: setting it per launch to that launch's size races between the
  * per-thread contexts of the gtn:: layer (one thread lowers it under another's launch). */
-constexpr int kMaxDynamicSmem = 227 * 1024;
 int ensure_max_smem(gtnb_ctx* ctx, const void* kernel);
 
 template <typename T>

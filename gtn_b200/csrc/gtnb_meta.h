@@ -13,6 +13,7 @@ constexpr uint32_t kRowMask = 0x3FFFFFFFu; // low 30 bits of a row_ptr entry
 constexpr uint32_t kStartBit = 0x40000000u; // node is a start node
 constexpr uint32_t kAcceptBit = 0x80000000u; // node is an accept node
 constexpr int kAlign = 4; // elements; keeps every per-graph slab 16-byte aligned
+constexpr int kMaxDynamicSmem = 227 * 1024; // a CTA's opt-in dynamic shared memory on sm_90 (ensure_max_smem)
 
 /*
  * G's tables as k_sparse.cu's denominator sweeps read them (gtnb_product.h's SparseTables on the device): S nodes,

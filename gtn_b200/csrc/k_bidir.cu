@@ -1519,6 +1519,41 @@ __global__ void __launch_bounds__(32 * ((MODE == 1 ? kMaxPairWarps : kMaxNodeWar
 
 } // namespace bidir
 
+/* launch_bidir_ctc's kernel and geometry */
+struct BidirPlan {
+  void (*kernel)(const bidir::Params);
+  bool fx; // compile-time strides over saved-score rows of the fixed pitch
+  bool pair; // the PAIR kernels (two nodes per thread), which read the CTC graphs from the targets themselves
+  int nwn; // node warps
+  bidir::Layout lay;
+  unsigned block; // threads per CTA
+};
+
+/*
+ * For C labels, levels of at most max_nodes nodes, saved-score rows of the fixed pitch (fixed_pitch: gtnb_compose_linear,
+ * implicit lattices) or of each graph's node count rounded up to 4, and emissions and gradient of type E.  pair_ok: the
+ * graphs are ctc_build_kernel's (gtnb_ctc_loss) with the targets at hand, and gtnb_ctx_set_flag("bidir_mode", 0) does
+ * not ask for one node per thread.
+ */
+template <class E>
+BidirPlan bidir_plan(int C, int max_nodes, bool fixed_pitch, bool pair_ok) {
+  BidirPlan p;
+  // FX: the benchmark's shapes (C == 64 or 128)
+  p.fx = (C == 64 || C == 128) && fixed_pitch;
+  p.pair = p.fx && pair_ok && max_nodes <= 2 * 32 * bidir::kMaxPairWarps - 1;
+  // NQ: float4 chunks of an emission row per helper lane
+  if (p.pair)
+    p.kernel = C == 64 ? bidir::bidir_ctc_kernel<1, true, 1, E> : bidir::bidir_ctc_kernel<2, true, 1, E>;
+  else if (p.fx)
+    p.kernel = C == 64 ? bidir::bidir_ctc_kernel<1, true, 0, E> : bidir::bidir_ctc_kernel<2, true, 0, E>;
+  else
+    p.kernel = C <= 64 ? bidir::bidir_ctc_kernel<1, false, 0, E> : bidir::bidir_ctc_kernel<2, false, 0, E>;
+  p.nwn = std::max(1, ((p.pair ? (max_nodes + 1) / 2 : max_nodes) + 31) / 32);
+  p.lay = bidir::make_layout(C, p.fx ? bidir::kFixedPitch : ((max_nodes + 3) & ~3), (int)sizeof(E));
+  p.block = 32 * (p.nwn + 1 + bidir::kHelpers);
+  return p;
+}
+
 #ifndef GTNB_HOST_EMU
 
 static_assert(bidir::kFixedPitch == kImplicitFixedPitch, "gtnb_compose_linear allocates the rows");
@@ -1543,8 +1578,9 @@ bool bidir_supported(const gtnb_lattice* lat, const void* emissions, int64_t str
 /* true when launch_bidir_ctc would run its PAIR kernels, which read the CTC target graphs from the targets
  * themselves: the caller (gtnb_ctc_loss) then skips ctc_build_kernel altogether */
 bool bidir_takes_targets(const gtnb_lattice* lat, int ctc_blank) {
-  const bool fx = (lat->C == 64 || lat->C == 128) && lat->score_pitch == bidir::kFixedPitch;
-  return fx && ctc_blank >= 0 && ctc_blank < lat->C && lat->max_lvl_nodes <= 2 * 32 * bidir::kMaxPairWarps - 1;
+  return bidir_plan<float>(lat->C, lat->max_lvl_nodes, lat->score_pitch == bidir::kFixedPitch,
+                           ctc_blank >= 0 && ctc_blank < lat->C)
+      .pair;
 }
 
 /* blocks of 8 frames per utterance: boff_dev holds B * 2 * bidir_blocks(max T) * 4 floats */
@@ -1556,18 +1592,6 @@ int bidir_blocks(int max_T) {
 int bidir_zparts() {
   return bidir::kHelpers;
 }
-namespace {
-/* the instantiation launch_bidir_ctc runs for element type E */
-template <class E>
-void (*bidir_kernel_for(int mode, bool fx, int C))(const bidir::Params) {
-  if (mode == 1) return C == 64 ? bidir::bidir_ctc_kernel<1, true, 1, E> : bidir::bidir_ctc_kernel<2, true, 1, E>;
-  if (fx && C == 64) return bidir::bidir_ctc_kernel<1, true, 0, E>;
-  if (fx) return bidir::bidir_ctc_kernel<2, true, 0, E>;
-  if (C <= 64) return bidir::bidir_ctc_kernel<1, false, 0, E>;
-  return bidir::bidir_ctc_kernel<2, false, 0, E>;
-}
-} // namespace
-
 int launch_bidir_ctc(
     gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, float* zparts_dev, float* boff_dev, void* grad_emis,
     int64_t grad_stride, int b0, int nb, float* out_scores_dev, int ctc_blank, const int32_t* targets_dev,
@@ -1592,31 +1616,23 @@ int launch_bidir_ctc(
   P.grad = grad_emis ? static_cast<char*>(grad_emis) + (long long)b0 * grad_stride * esize : nullptr;
   P.grad_stride = grad_stride;
   P.C = lat->C;
-  P.nwn = std::max(1, (lat->max_lvl_nodes + 31) / 32);
-  // FX: the benchmark's shapes (C == 64 or 128) on a lattice whose saved-score rows were allocated with the
-  // fixed pitch (gtnb_compose_linear, implicit lattices): compile-time strides in the node warps
-  const bool fx = (lat->C == 64 || lat->C == 128) && lat->score_pitch == bidir::kFixedPitch;
-  const int max_pitch = fx ? bidir::kFixedPitch : ((lat->max_lvl_nodes + 3) & ~3);
-  P.lay = bidir::make_layout(lat->C, max_pitch, esize);
-  // NQ: float4 chunks of an emission row per helper lane
-  // the graphs are ctc_build_kernel's (gtnb_ctc_loss): the PAIR kernels (two nodes per thread) unless
-  // gtnb_ctx_set_flag("bidir_mode", 0) asks for one node per thread
   (void)tgt_off_dev; // (the offsets travel in the descriptors: GraphMeta::tgt_off)
-  const bool ctc_ok = bidir_takes_targets(lat, ctc_blank) && targets_dev;
   P.targets = targets_dev;
-  const int mode = !ctc_ok || ctx->bidir_mode == 0 ? 0 : 1;
-  void (*kern)(const bidir::Params) = dtype == GTNB_BF16  ? bidir_kernel_for<bf16_t>(mode, fx, lat->C)
-                                      : dtype == GTNB_F16 ? bidir_kernel_for<f16_t>(mode, fx, lat->C)
-                                                          : bidir_kernel_for<float>(mode, fx, lat->C);
-  if (mode == 1) P.nwn = std::max(1, ((lat->max_lvl_nodes + 1) / 2 + 31) / 32);
   P.ctc_blank = ctc_blank;
+  const bool fixed = lat->score_pitch == bidir::kFixedPitch;
+  const bool pair_ok = targets_dev && ctc_blank >= 0 && ctc_blank < lat->C && ctx->bidir_mode != 0;
+  const BidirPlan p = dtype == GTNB_BF16  ? bidir_plan<bf16_t>(lat->C, lat->max_lvl_nodes, fixed, pair_ok)
+                      : dtype == GTNB_F16 ? bidir_plan<f16_t>(lat->C, lat->max_lvl_nodes, fixed, pair_ok)
+                                          : bidir_plan<float>(lat->C, lat->max_lvl_nodes, fixed, pair_ok);
+  P.nwn = p.nwn;
+  P.lay = p.lay;
   if (P.lay.total > 48 * 1024) {
-    int rc = ensure_max_smem(ctx, (const void*)kern);
+    int rc = ensure_max_smem(ctx, (const void*)p.kernel);
     if (rc) return rc;
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(2 * nb, 1, 1);
-  cfg.blockDim = dim3(32 * (P.nwn + 1 + bidir::kHelpers), 1, 1);
+  cfg.blockDim = dim3(p.block, 1, 1);
   cfg.dynamicSmemBytes = P.lay.total;
   cfg.stream = ctx->stream;
   cudaLaunchAttribute attr[1];
@@ -1626,7 +1642,7 @@ int launch_bidir_ctc(
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  GTNB_LAUNCH(ctx, "bidir_ctc", GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, kern, P)));
+  GTNB_LAUNCH(ctx, "bidir_ctc", GTNB_CUDA(ctx, cudaLaunchKernelEx(&cfg, p.kernel, P)));
   return GTNB_OK;
 }
 

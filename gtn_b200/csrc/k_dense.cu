@@ -224,12 +224,6 @@ __global__ void __launch_bounds__(kDenseThreads) viterbi_dense_kernel(
   }
 }
 
-} // namespace
-
-#ifndef GTNB_HOST_EMU
-
-namespace {
-
 /* lanes per state: G = 256 / C rounded down to a power of two, at most 32 */
 int dense_lanes(int C) {
   int G = 1;
@@ -243,40 +237,20 @@ size_t dense_smem_bytes(int C) {
 }
 
 template <class E>
-int viterbi_dense_typed(
-    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const E* emis, int64_t stride,
-    const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores) {
-  const int G = dense_lanes(C);
-  const size_t smem = dense_smem_bytes(C);
-  if (smem > (size_t)kMaxDynamicSmem)
-    return fail(ctx, GTNB_ERR_UNSUPPORTED,
-                "gtnb_viterbi_dense: the transitions tile does not fit shared memory (C <= 224)");
-#define LAUNCH_DENSE(G_, K_)                                                                        \
-  do {                                                                                              \
-    int rc__ = ensure_max_smem(ctx, (const void*)viterbi_dense_kernel<G_, K_, E>);                  \
-    if (rc__) return rc__;                                                                          \
-    GTNB_LAUNCH(ctx, K_ ? "viterbi_dense_bigram" : "viterbi_dense",                                 \
-                viterbi_dense_kernel<G_, K_, E><<<B, kDenseThreads, smem, ctx->stream>>>(           \
-                    T_max, C, T_dev, emis, (long long)stride, trans_dev, bp, paths, scores, empty_score)); \
-  } while (0)
-#define LAUNCH_KIND(G_)            \
-  do {                             \
-    if (bigram)                    \
-      LAUNCH_DENSE(G_, true);      \
-    else                           \
-      LAUNCH_DENSE(G_, false);     \
-  } while (0)
+using DenseKernel = void (*)(int, int, const int32_t*, const E*, long long, const float*, uint8_t*, int32_t*, float*,
+                             float);
+
+/* the instantiation for G lanes per state (dense_lanes) and the graph kind */
+template <class E>
+DenseKernel<E> viterbi_dense_kernel_for(int G, bool bigram) {
   switch (G) {
-    case 1: LAUNCH_KIND(1); break;
-    case 2: LAUNCH_KIND(2); break;
-    case 4: LAUNCH_KIND(4); break;
-    case 8: LAUNCH_KIND(8); break;
-    case 16: LAUNCH_KIND(16); break;
-    default: LAUNCH_KIND(32); break;
+    case 1: return bigram ? viterbi_dense_kernel<1, true, E> : viterbi_dense_kernel<1, false, E>;
+    case 2: return bigram ? viterbi_dense_kernel<2, true, E> : viterbi_dense_kernel<2, false, E>;
+    case 4: return bigram ? viterbi_dense_kernel<4, true, E> : viterbi_dense_kernel<4, false, E>;
+    case 8: return bigram ? viterbi_dense_kernel<8, true, E> : viterbi_dense_kernel<8, false, E>;
+    case 16: return bigram ? viterbi_dense_kernel<16, true, E> : viterbi_dense_kernel<16, false, E>;
+    default: return bigram ? viterbi_dense_kernel<32, true, E> : viterbi_dense_kernel<32, false, E>;
   }
-#undef LAUNCH_KIND
-#undef LAUNCH_DENSE
-  return GTNB_OK;
 }
 
 } // namespace
@@ -284,6 +258,29 @@ int viterbi_dense_typed(
 bool viterbi_dense_supported(int C) {
   return C >= 1 && C <= 256 && dense_smem_bytes(C) <= (size_t)kMaxDynamicSmem;
 }
+
+#ifndef GTNB_HOST_EMU
+
+namespace {
+
+template <class E>
+int viterbi_dense_typed(
+    gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const E* emis, int64_t stride,
+    const float* trans_dev, float empty_score, uint8_t* bp, int32_t* paths, float* scores) {
+  const size_t smem = dense_smem_bytes(C);
+  if (smem > (size_t)kMaxDynamicSmem)
+    return fail(ctx, GTNB_ERR_UNSUPPORTED,
+                "gtnb_viterbi_dense: the transitions tile does not fit shared memory (C <= 224)");
+  const DenseKernel<E> kernel = viterbi_dense_kernel_for<E>(dense_lanes(C), bigram);
+  int rc = ensure_max_smem(ctx, (const void*)kernel);
+  if (rc) return rc;
+  GTNB_LAUNCH(ctx, bigram ? "viterbi_dense_bigram" : "viterbi_dense",
+              kernel<<<B, kDenseThreads, smem, ctx->stream>>>(T_max, C, T_dev, emis, (long long)stride, trans_dev, bp,
+                                                              paths, scores, empty_score));
+  return GTNB_OK;
+}
+
+} // namespace
 
 int launch_viterbi_dense(
     gtnb_ctx* ctx, int B, int T_max, int C, bool bigram, const int32_t* T_dev, const void* emis, int64_t stride,

@@ -1377,6 +1377,63 @@ int implicit_elem_mode(int dtype, int G, bool arc, bool tropical) {
   return (dtype == GTNB_BF16 || dtype == GTNB_F16) && G == 0 && !arc && !tropical ? GTNB_OK : GTNB_ERR_LOGIC;
 }
 
+/* the staged block of the traceback: kTrMaxFrames frames, halved until the CTA fits two per SM */
+TraceLayout trace_layout(int max_lvl_nodes, int max_lvl_arcs, int C) {
+  TraceLayout lay = make_trace_layout(max_lvl_nodes, max_lvl_arcs, C, kTrMaxFrames);
+  while (lay.K > 1 && lay.total > kTrSmemTarget) lay = make_trace_layout(max_lvl_nodes, max_lvl_arcs, C, lay.K / 2);
+  return lay;
+}
+
+template <class E>
+using ImpForwardKernel = void (*)(const GraphMeta*, const uint8_t*, const int32_t*, const int32_t*, const int32_t*,
+                                  const float*, const E*, float*, float*, int32_t*, int, const ImpLayout);
+template <class E>
+using ImpBackwardKernel = void (*)(const GraphMeta*, const uint8_t*, const int32_t*, const int32_t*, const int32_t*,
+                                   const float*, const int32_t*, float*, const E*, const float*, const float*,
+                                   const float*, float*, long long, int, const ImpLayout);
+
+/* the forward sweep's instantiation for G lanes per node (wide_lanes; 0: the one-node / several-nodes-per-thread
+ * kernel) over emissions of type E; nullptr where E has none (implicit_elem_mode) */
+template <bool ARC, bool TROP, class E = float>
+ImpForwardKernel<E> implicit_forward_kernel_for(int G) {
+  if constexpr (!std::is_same_v<E, float>) {
+    if constexpr (ARC || TROP) return nullptr;
+    else return G == 0 ? implicit_forward_kernel<false, false, E> : nullptr;
+  } else {
+    switch (G) {
+      case 0: return implicit_forward_kernel<ARC, TROP>;
+      case 1: return implicit_forward_wide_kernel<1, ARC, TROP>;
+      case 2: return implicit_forward_wide_kernel<2, ARC, TROP>;
+      case 4: return implicit_forward_wide_kernel<4, ARC, TROP>;
+      case 8: return implicit_forward_wide_kernel<8, ARC, TROP>;
+      case 16: return implicit_forward_wide_kernel<16, ARC, TROP>;
+      default: return implicit_forward_wide_kernel<32, ARC, TROP>;
+    }
+  }
+}
+
+/* the backward sweep's, likewise; grad_graph: it also accumulates the graph operands' arc gradients */
+template <bool ARC, class E = float>
+ImpBackwardKernel<E> implicit_backward_kernel_for(int G, bool grad_graph) {
+  if constexpr (!std::is_same_v<E, float>) {
+    if constexpr (ARC) return nullptr;
+    else if (G != 0) return nullptr;
+    else return grad_graph ? implicit_backward_kernel<true, false, E> : implicit_backward_kernel<false, false, E>;
+  } else {
+    switch (G) {
+      case 0: return grad_graph ? implicit_backward_kernel<true, ARC> : implicit_backward_kernel<false, ARC>;
+      case 1: return grad_graph ? implicit_backward_wide_kernel<1, true, ARC> : implicit_backward_wide_kernel<1, false, ARC>;
+      case 2: return grad_graph ? implicit_backward_wide_kernel<2, true, ARC> : implicit_backward_wide_kernel<2, false, ARC>;
+      case 4: return grad_graph ? implicit_backward_wide_kernel<4, true, ARC> : implicit_backward_wide_kernel<4, false, ARC>;
+      case 8: return grad_graph ? implicit_backward_wide_kernel<8, true, ARC> : implicit_backward_wide_kernel<8, false, ARC>;
+      case 16:
+        return grad_graph ? implicit_backward_wide_kernel<16, true, ARC> : implicit_backward_wide_kernel<16, false, ARC>;
+      default:
+        return grad_graph ? implicit_backward_wide_kernel<32, true, ARC> : implicit_backward_wide_kernel<32, false, ARC>;
+    }
+  }
+}
+
 #ifndef GTNB_HOST_EMU
 
 /* arc_C > 0 (gtnb_graph_loss, labels in [0, arc_C)): graphs that are not label-uniform are accepted
@@ -1406,17 +1463,15 @@ bool implicit_supported(const gtnb_lattice* lat) {
   return lay.total <= 200 * 1024;
 }
 
-// E: the element type the kernel reads lat->emissions as
-#define GTNB_FWD_ARGS(E)                                                                          \
-  lat->meta + b0, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w, \
-      reinterpret_cast<const E*>(lat->emissions), lat->scores, lat->out_scores + b0, status_dev + b0, lat->C, lay
-#define GTNB_BWD_ARGS(E)                                                                          \
-  lat->meta + b0, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w, \
-      lat->sg_in_arc, grad_graph, reinterpret_cast<const E*>(lat->emissions), lat->scores,       \
-      lat->out_scores + b0, deltas_dev ? deltas_dev + b0 : nullptr,                               \
-      grad_emis + (long long)b0 * grad_stride, (long long)grad_stride, lat->C, lay
-
 namespace {
+
+/* f((const E*)nullptr) for the element type dtype names (GTNB_F32 / GTNB_BF16 / GTNB_F16) */
+template <class F>
+int with_elem(int dtype, F&& f) {
+  if (dtype == GTNB_BF16) return f((const bf16_t*)nullptr);
+  if (dtype == GTNB_F16) return f((const f16_t*)nullptr);
+  return f((const float*)nullptr);
+}
 
 /* the launch of one mode; the arc-label instantiations carry their own names in the profile log */
 template <bool ARC, bool TROP>
@@ -1427,39 +1482,18 @@ int implicit_forward_mode(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev,
                          : (TROP ? "implicit_forward_max" : "implicit_forward");
   if (implicit_elem_mode(lat->dtype, G, ARC, TROP))
     return fail(ctx, GTNB_ERR_LOGIC, "launch_implicit_forward: no instantiation for 16-bit emissions in this mode");
-#define GTNB_LAUNCH_FWD_E(K, E)                                                                  \
-  do {                                                                                           \
-    if (lay.total > 48 * 1024) {                                                                 \
-      int rc = ensure_max_smem(ctx, (const void*)K);                                             \
-      if (rc) return rc;                                                                         \
-    }                                                                                            \
-    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_FWD_ARGS(E)));    \
-  } while (0)
-#define GTNB_LAUNCH_FWD(K) GTNB_LAUNCH_FWD_E(K, float)
-  switch (G) {
-    case 0:
-      if constexpr (!ARC && !TROP) {
-        if (lat->dtype == GTNB_BF16) {
-          GTNB_LAUNCH_FWD_E((implicit_forward_kernel<false, false, bf16_t>), bf16_t);
-          break;
-        }
-        if (lat->dtype == GTNB_F16) {
-          GTNB_LAUNCH_FWD_E((implicit_forward_kernel<false, false, f16_t>), f16_t);
-          break;
-        }
-      }
-      GTNB_LAUNCH_FWD((implicit_forward_kernel<ARC, TROP>));
-      break;
-    case 1: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<1, ARC, TROP>)); break;
-    case 2: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<2, ARC, TROP>)); break;
-    case 4: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<4, ARC, TROP>)); break;
-    case 8: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<8, ARC, TROP>)); break;
-    case 16: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<16, ARC, TROP>)); break;
-    default: GTNB_LAUNCH_FWD((implicit_forward_wide_kernel<32, ARC, TROP>)); break;
-  }
-#undef GTNB_LAUNCH_FWD
-#undef GTNB_LAUNCH_FWD_E
-  return GTNB_OK;
+  return with_elem(lat->dtype, [&](auto e) {
+    using E = std::remove_const_t<std::remove_pointer_t<decltype(e)>>;
+    const ImpForwardKernel<E> kernel = implicit_forward_kernel_for<ARC, TROP, E>(G);
+    if (lay.total > 48 * 1024) {
+      int rc = ensure_max_smem(ctx, (const void*)kernel);
+      if (rc) return rc;
+    }
+    GTNB_LAUNCH(ctx, name, kernel<<<nb, kImpThreads, lay.total, ctx->stream>>>(
+        lat->meta + b0, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w,
+        reinterpret_cast<const E*>(lat->emissions), lat->scores, lat->out_scores + b0, status_dev + b0, lat->C, lay));
+    return GTNB_OK;
+  });
 }
 
 template <bool ARC>
@@ -1471,56 +1505,20 @@ int implicit_backward_mode(
   const char* name = ARC ? "implicit_backward_arc" : "implicit_backward";
   if (implicit_elem_mode(lat->dtype, G, ARC, false))
     return fail(ctx, GTNB_ERR_LOGIC, "launch_implicit_backward: no instantiation for 16-bit emissions in this mode");
-#define GTNB_LAUNCH_BWD_E(K, E)                                                                  \
-  do {                                                                                           \
-    if (lay.total > 48 * 1024) {                                                                 \
-      int rc = ensure_max_smem(ctx, (const void*)K);                                             \
-      if (rc) return rc;                                                                         \
-    }                                                                                            \
-    GTNB_LAUNCH(ctx, name, K<<<nb, kImpThreads, lay.total, ctx->stream>>>(GTNB_BWD_ARGS(E)));    \
-  } while (0)
-#define GTNB_LAUNCH_BWD(K) GTNB_LAUNCH_BWD_E(K, float)
-/* the one-node / several-nodes-per-thread kernel for lat->dtype */
-#define GTNB_LAUNCH_BWD_0(GRAPH_GRAD_)                                                           \
-  do {                                                                                           \
-    if constexpr (!ARC) {                                                                        \
-      if (lat->dtype == GTNB_BF16) {                                                             \
-        GTNB_LAUNCH_BWD_E((implicit_backward_kernel<GRAPH_GRAD_, false, bf16_t>), bf16_t);       \
-        break;                                                                                   \
-      }                                                                                          \
-      if (lat->dtype == GTNB_F16) {                                                              \
-        GTNB_LAUNCH_BWD_E((implicit_backward_kernel<GRAPH_GRAD_, false, f16_t>), f16_t);         \
-        break;                                                                                   \
-      }                                                                                          \
-    }                                                                                            \
-    GTNB_LAUNCH_BWD((implicit_backward_kernel<GRAPH_GRAD_, ARC>));                               \
-  } while (0)
-#define GTNB_LAUNCH_BWD_G(GG)                                               \
-  do {                                                                      \
-    if (grad_graph)                                                         \
-      GTNB_LAUNCH_BWD((implicit_backward_wide_kernel<GG, true, ARC>));      \
-    else                                                                    \
-      GTNB_LAUNCH_BWD((implicit_backward_wide_kernel<GG, false, ARC>));     \
-  } while (0)
-  switch (G) {
-    case 0:
-      if (grad_graph)
-        GTNB_LAUNCH_BWD_0(true);
-      else
-        GTNB_LAUNCH_BWD_0(false);
-      break;
-    case 1: GTNB_LAUNCH_BWD_G(1); break;
-    case 2: GTNB_LAUNCH_BWD_G(2); break;
-    case 4: GTNB_LAUNCH_BWD_G(4); break;
-    case 8: GTNB_LAUNCH_BWD_G(8); break;
-    case 16: GTNB_LAUNCH_BWD_G(16); break;
-    default: GTNB_LAUNCH_BWD_G(32); break;
-  }
-#undef GTNB_LAUNCH_BWD_0
-#undef GTNB_LAUNCH_BWD_G
-#undef GTNB_LAUNCH_BWD
-#undef GTNB_LAUNCH_BWD_E
-  return GTNB_OK;
+  return with_elem(lat->dtype, [&](auto e) {
+    using E = std::remove_const_t<std::remove_pointer_t<decltype(e)>>;
+    const ImpBackwardKernel<E> kernel = implicit_backward_kernel_for<ARC, E>(G, grad_graph != nullptr);
+    if (lay.total > 48 * 1024) {
+      int rc = ensure_max_smem(ctx, (const void*)kernel);
+      if (rc) return rc;
+    }
+    GTNB_LAUNCH(ctx, name, kernel<<<nb, kImpThreads, lay.total, ctx->stream>>>(
+        lat->meta + b0, lat->sg_flags, lat->sg_in_ptr, lat->sg_in_src, lat->sg_in_label, lat->sg_in_w,
+        lat->sg_in_arc, grad_graph, reinterpret_cast<const E*>(lat->emissions), lat->scores, lat->out_scores + b0,
+        deltas_dev ? deltas_dev + b0 : nullptr, grad_emis + (long long)b0 * grad_stride, (long long)grad_stride,
+        lat->C, lay));
+    return GTNB_OK;
+  });
 }
 
 } // namespace
@@ -1536,18 +1534,8 @@ int launch_implicit_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_de
                          : implicit_forward_mode<false, false>(ctx, lat, status_dev, b0, nb);
 }
 
-namespace {
-/* the staged block of the traceback: kTrMaxFrames frames, halved until the CTA fits two per SM */
-TraceLayout trace_layout(const gtnb_lattice* lat) {
-  TraceLayout lay = make_trace_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, lat->C, kTrMaxFrames);
-  while (lay.K > 1 && lay.total > kTrSmemTarget)
-    lay = make_trace_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, lat->C, lay.K / 2);
-  return lay;
-}
-} // namespace
-
 bool implicit_trace_supported(const gtnb_lattice* lat) {
-  return trace_layout(lat).total <= kMaxDynamicSmem;
+  return trace_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, lat->C).total <= kMaxDynamicSmem;
 }
 
 int launch_implicit_trace(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev, int32_t* paths, int32_t* arcs,
@@ -1555,7 +1543,7 @@ int launch_implicit_trace(gtnb_ctx* ctx, gtnb_lattice* lat, int32_t* status_dev,
   if (lat->B <= 0) return GTNB_OK;
   if (lat->dtype != GTNB_F32)
     return fail(ctx, GTNB_ERR_LOGIC, "launch_implicit_trace: no instantiation for 16-bit emissions");
-  const TraceLayout lay = trace_layout(lat);
+  const TraceLayout lay = trace_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, lat->C);
   if (lay.total > kMaxDynamicSmem) return fail(ctx, GTNB_ERR_UNSUPPORTED, "implicit_trace: graphs too large");
   if (lay.total > 48 * 1024) {
     int rc = ensure_max_smem(ctx, (const void*)implicit_trace_kernel);

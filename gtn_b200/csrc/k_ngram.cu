@@ -307,6 +307,16 @@ __global__ void __launch_bounds__(kNgramMaxThreads) ngram_den_backward_kernel(
   }
 }
 
+/* the trellis kernels' instantiations for K entries of W per thread (ngram_den_shape) */
+template <bool START, class E>
+auto ngram_den_forward_kernel_for(int K) {
+  return K == 16 ? ngram_den_forward_kernel<16, START, E> : ngram_den_forward_kernel<32, START, E>;
+}
+template <bool START, class E>
+auto ngram_den_backward_kernel_for(int K) {
+  return K == 16 ? ngram_den_backward_kernel<16, START, E> : ngram_den_backward_kernel<32, START, E>;
+}
+
 /* sigma_i = logsumexp_j W[i][j], one warp per row */
 __global__ void __launch_bounds__(256) ngram_sigma_kernel(int C, const float* __restrict__ W, float* __restrict__ sigma) {
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
@@ -544,12 +554,8 @@ int den_forward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int3
   if (B == 0) return GTNB_OK;
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
-  if (K == 16)
-    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<16, START, E><<<B, threads, 0, ctx->stream>>>(
-        T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
-  else
-    GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel<32, START, E><<<B, threads, 0, ctx->stream>>>(
-        T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
+  GTNB_LAUNCH(ctx, name, ngram_den_forward_kernel_for<START, E>(K)<<<B, threads, 0, ctx->stream>>>(
+      T, C, lanes, lens_dev, emis, stride, W, alpha, den, status));
   return GTNB_OK;
 }
 
@@ -560,12 +566,8 @@ int den_backward(gtnb_ctx* ctx, const char* name, int B, int T, int C, const int
   if (B == 0) return GTNB_OK;
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
-  if (K == 16)
-    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<16, START, E><<<B, threads, 0, ctx->stream>>>(
-        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
-  else
-    GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel<32, START, E><<<B, threads, 0, ctx->stream>>>(
-        T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
+  GTNB_LAUNCH(ctx, name, ngram_den_backward_kernel_for<START, E>(K)<<<B, threads, 0, ctx->stream>>>(
+      T, C, lanes, lens_dev, emis, stride, W, alpha, den, grad, grad_stride, wgrad));
   return GTNB_OK;
 }
 

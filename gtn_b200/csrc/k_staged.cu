@@ -1004,26 +1004,22 @@ __global__ void __launch_bounds__(32 * consumer_warps(1) + 32) sd_backward_fused
   }
 }
 
-#ifdef GTNB_HOST_EMU
-} // namespace
-#else
-
 struct StagedPlan {
   bool ok;
   int G, max_L;
   Layout fwd, bwd;
 };
 
-StagedPlan plan(const gtnb_lattice* lat) {
+/* the B graphs' descriptors; max_lvl_nodes / max_lvl_arcs: bounds on a level's nodes and arcs over the batch */
+StagedPlan plan(const GraphMeta* meta, int B, int max_lvl_nodes, int max_lvl_arcs) {
   StagedPlan p;
   p.ok = false;
-  if (!lat->composed || !lat->level_local) return p;
   int max_L = 0;
   long long sumA = 0, sumN = 0;
-  for (int b = 0; b < lat->B; b++) {
-    max_L = std::max(max_L, lat->meta_h[b].L);
-    sumA += lat->meta_h[b].sg_A;
-    sumN += lat->meta_h[b].sg_N;
+  for (int b = 0; b < B; b++) {
+    max_L = std::max(max_L, meta[b].L);
+    sumA += meta[b].sg_A;
+    sumN += meta[b].sg_N;
   }
   if (max_L + 1 > kMaxLevelsInSmem) return p;
   p.max_L = max_L;
@@ -1031,8 +1027,8 @@ StagedPlan plan(const gtnb_lattice* lat) {
   p.G = deg <= 4.0 ? 1 : (deg <= 16.0 ? 4 : (deg <= 48.0 ? 16 : 32));
   const int budget = 200 * 1024;
   for (int ls = 3; ls >= 1; ls--) {
-    Layout f = make_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, max_L, ls, 2, false);
-    Layout bw = make_layout(lat->max_lvl_nodes, lat->max_lvl_arcs, max_L, ls, 4, true);
+    Layout f = make_layout(max_lvl_nodes, max_lvl_arcs, max_L, ls, 2, false);
+    Layout bw = make_layout(max_lvl_nodes, max_lvl_arcs, max_L, ls, 4, true);
     // keep two CTAs per SM resident when the graph is small enough
     const int cap = (bw.total <= 100 * 1024 || ls == 1) ? budget : 100 * 1024;
     if (bw.total <= cap && f.total <= cap) {
@@ -1045,74 +1041,76 @@ StagedPlan plan(const gtnb_lattice* lat) {
   return p;
 }
 
+/* sd_backward_fused's layout: the backward's, then the graph operands' tables; false when it exceeds the budget */
+bool fused_layout(Layout& lay, int max_lvl_nodes, int max_lvl_arcs) {
+  lay.tab_nodes = max_lvl_nodes;
+  lay.tab_arcs = max_lvl_arcs;
+  lay.off_tab = (lay.total + 15) / 16 * 16;
+  lay.total = lay.off_tab + 4 * (3 * lay.tab_nodes + 2 + 3 * lay.tab_arcs) + 16;
+  return lay.total <= 200 * 1024;
+}
+
+using StagedForward = void (*)(const GraphMeta*, const int32_t*, const int32_t*, const uint32_t*, const int2*,
+                               const int32_t*, float*, int32_t*, float*, int32_t*, const Layout);
+using StagedBackward = void (*)(const GraphMeta*, const int32_t*, const int32_t*, const uint32_t*, const int2*,
+                                const int32_t*, const float*, const float*, const int32_t*, const float*, float*,
+                                const Layout);
+
+/* the instantiations for mode (MODE_*) and G lanes per node (StagedPlan::G) */
+template <int MODE>
+StagedForward sd_forward_staged_for(int G) {
+  return G == 1 ? sd_forward_staged<MODE, 1>
+                : G == 4 ? sd_forward_staged<MODE, 4> : G == 16 ? sd_forward_staged<MODE, 16> : sd_forward_staged<MODE, 32>;
+}
+StagedForward sd_forward_staged_kernel_for(int mode, int G) {
+  return mode == MODE_LOG ? sd_forward_staged_for<MODE_LOG>(G)
+                          : mode == MODE_TROPICAL ? sd_forward_staged_for<MODE_TROPICAL>(G) : sd_forward_staged_for<MODE_PATH>(G);
+}
+template <bool TROPICAL>
+StagedBackward sd_backward_staged_for(int G) {
+  return G == 1 ? sd_backward_staged<TROPICAL, 1>
+                : G == 4 ? sd_backward_staged<TROPICAL, 4>
+                         : G == 16 ? sd_backward_staged<TROPICAL, 16> : sd_backward_staged<TROPICAL, 32>;
+}
+StagedBackward sd_backward_staged_kernel_for(bool tropical, int G) {
+  return tropical ? sd_backward_staged_for<true>(G) : sd_backward_staged_for<false>(G);
+}
+
+#ifndef GTNB_HOST_EMU
+
+StagedPlan plan(const gtnb_lattice* lat) {
+  if (!lat->composed || !lat->level_local) return StagedPlan{};
+  return plan(lat->meta_h.data(), lat->B, lat->max_lvl_nodes, lat->max_lvl_arcs);
+}
+
 template <typename K>
 int set_smem(gtnb_ctx* ctx, K kernel, int bytes) {
   if (bytes > kMaxDynamicSmem) return GTNB_ERR_UNSUPPORTED;
   return ensure_max_smem(ctx, (const void*)kernel);
 }
 
+#endif // GTNB_HOST_EMU
+
 } // namespace
+
+#ifndef GTNB_HOST_EMU
 
 bool staged_supported(const gtnb_lattice* lat) {
   return plan(lat).ok;
 }
 
-#define FWD_ARGS                                                                      \
-  lat->meta, lat->lvl_node_ptr, lat->lvl_arc_ptr, lat->row_ptr, lat->arcs,            \
-      lat->acc_nodes, lat->scores, lat->back_ptr, lat->out_scores, lat->best_accept, p.fwd
-
-#define LAUNCH_FWD(MODE_, G_)                                                                  \
-  do {                                                                                         \
-    int rc__ = set_smem(ctx, sd_forward_staged<MODE_, G_>, p.fwd.total);                       \
-    if (rc__) return rc__;                                                                     \
-    GTNB_LAUNCH(ctx, "sd_forward",                                                             \
-                sd_forward_staged<MODE_, G_><<<lat->B, 32 * consumer_warps(G_) + 32, p.fwd.total, ctx->stream>>>(FWD_ARGS)); \
-  } while (0)
-
-#define DISPATCH_G_FWD(MODE_)                \
-  do {                                       \
-    switch (p.G) {                           \
-      case 1: LAUNCH_FWD(MODE_, 1); break;   \
-      case 4: LAUNCH_FWD(MODE_, 4); break;   \
-      case 16: LAUNCH_FWD(MODE_, 16); break; \
-      default: LAUNCH_FWD(MODE_, 32); break; \
-    }                                        \
-  } while (0)
-
 int launch_forward_staged(gtnb_ctx* ctx, gtnb_lattice* lat, int mode) {
   const StagedPlan p = plan(lat);
   if (!p.ok) return GTNB_ERR_UNSUPPORTED;
-  if (mode == MODE_LOG)
-    DISPATCH_G_FWD(MODE_LOG);
-  else if (mode == MODE_TROPICAL)
-    DISPATCH_G_FWD(MODE_TROPICAL);
-  else
-    DISPATCH_G_FWD(MODE_PATH);
+  const StagedForward kernel = sd_forward_staged_kernel_for(mode, p.G);
+  int rc = set_smem(ctx, kernel, p.fwd.total);
+  if (rc) return rc;
+  GTNB_LAUNCH(ctx, "sd_forward",
+              kernel<<<lat->B, 32 * consumer_warps(p.G) + 32, p.fwd.total, ctx->stream>>>(
+                  lat->meta, lat->lvl_node_ptr, lat->lvl_arc_ptr, lat->row_ptr, lat->arcs, lat->acc_nodes,
+                  lat->scores, lat->back_ptr, lat->out_scores, lat->best_accept, p.fwd));
   return GTNB_OK;
 }
-
-#define BWD_ARGS                                                                      \
-  lat->meta, lat->lvl_node_ptr, lat->lvl_arc_ptr, lat->row_ptr, lat->arcs,            \
-      lat->acc_nodes, lat->scores, lat->out_scores, lat->best_accept, deltas_dev,     \
-      lat->arc_grad, p.bwd
-
-#define LAUNCH_BWD(TROP_, G_)                                                                  \
-  do {                                                                                         \
-    int rc__ = set_smem(ctx, sd_backward_staged<TROP_, G_>, p.bwd.total);                      \
-    if (rc__) return rc__;                                                                     \
-    GTNB_LAUNCH(ctx, "sd_backward",                                                            \
-                sd_backward_staged<TROP_, G_><<<lat->B, 32 * consumer_warps(G_) + 32, p.bwd.total, ctx->stream>>>(BWD_ARGS)); \
-  } while (0)
-
-#define DISPATCH_G_BWD(TROP_)                \
-  do {                                       \
-    switch (p.G) {                           \
-      case 1: LAUNCH_BWD(TROP_, 1); break;   \
-      case 4: LAUNCH_BWD(TROP_, 4); break;   \
-      case 16: LAUNCH_BWD(TROP_, 16); break; \
-      default: LAUNCH_BWD(TROP_, 32); break; \
-    }                                        \
-  } while (0)
 
 /* shortestDistanceGrad + compose gradFunc in one kernel (log semiring, emission gradients
  * only).  GTNB_ERR_UNSUPPORTED when the lattice does not qualify: the caller then runs
@@ -1124,11 +1122,7 @@ int launch_backward_fused(
   for (int b = 0; b < lat->B; b++)
     if (!lat->meta_h[b].sg_uniform) return GTNB_ERR_UNSUPPORTED;
   Layout lay = p.bwd;
-  lay.tab_nodes = lat->max_lvl_nodes;
-  lay.tab_arcs = lat->max_lvl_arcs;
-  lay.off_tab = (lay.total + 15) / 16 * 16;
-  lay.total = lay.off_tab + 4 * (3 * lay.tab_nodes + 2 + 3 * lay.tab_arcs) + 16;
-  if (lay.total > 200 * 1024) return GTNB_ERR_UNSUPPORTED;
+  if (!fused_layout(lay, lat->max_lvl_nodes, lat->max_lvl_arcs)) return GTNB_ERR_UNSUPPORTED;
   int rc = set_smem(ctx, sd_backward_fused, lay.total);
   if (rc) return rc;
   GTNB_LAUNCH(ctx, "sd_backward_fused",
@@ -1142,10 +1136,13 @@ int launch_backward_fused(
 int launch_backward_staged(gtnb_ctx* ctx, gtnb_lattice* lat, int tropical, const float* deltas_dev) {
   const StagedPlan p = plan(lat);
   if (!p.ok) return GTNB_ERR_UNSUPPORTED;
-  if (tropical)
-    DISPATCH_G_BWD(true);
-  else
-    DISPATCH_G_BWD(false);
+  const StagedBackward kernel = sd_backward_staged_kernel_for(tropical != 0, p.G);
+  int rc = set_smem(ctx, kernel, p.bwd.total);
+  if (rc) return rc;
+  GTNB_LAUNCH(ctx, "sd_backward",
+              kernel<<<lat->B, 32 * consumer_warps(p.G) + 32, p.bwd.total, ctx->stream>>>(
+                  lat->meta, lat->lvl_node_ptr, lat->lvl_arc_ptr, lat->row_ptr, lat->arcs, lat->acc_nodes,
+                  lat->scores, lat->out_scores, lat->best_accept, deltas_dev, lat->arc_grad, p.bwd));
   return GTNB_OK;
 }
 

@@ -3,8 +3,9 @@
  * gtnb_ctc_align_async / gtnb_ngram_ctc_align_async / gtnb_asg_align_async on the CPU through tests/emu/simt_emu.h:
  * k_ctc.cu's prepare kernel, the numerator build kernels (k_ctc.cu's ctc_build_kernel; k_ngram.cu's ngram_tau_kernel
  * then ngram_num_build_kernel, or asg_num_build_kernel), k_implicit.cu's tropical forward and implicit_trace_kernel,
- * and k_ctc.cu's align_async_finalize_kernel.  Only the launch geometry and the bound-sized slabs are restated here;
- * the bound-uniform descriptors of utterances 0 and 1 come from the caller.
+ * and k_ctc.cu's align_async_finalize_kernel.  Only the launch geometry (apart from the traceback's staged block,
+ * trace_layout's) and the bound-sized slabs are restated here; the bound-uniform descriptors of utterances 0 and 1 come
+ * from the caller.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_ctc.cu"
@@ -76,8 +77,7 @@ int emu_align_async(int kind, int B, int T, int C, int S, int N, int A, const Gr
     implicit_forward_kernel<false, true>(meta.data(), flags.data(), in_ptr.data(), in_src.data(), in_label.data(),
                                          in_w.data(), emissions, sc.data(), out.data(), kstatus.data(), C, lf);
   });
-  TraceLayout lt = make_trace_layout(N, A, C, kTrMaxFrames);
-  while (lt.K > 1 && lt.total > kTrSmemTarget) lt = make_trace_layout(N, A, C, lt.K / 2);
+  const TraceLayout lt = trace_layout(N, A, C);
   int32_t* arc_out = tokens ? arcs.data() : nullptr;
   emu::launch(B, kImpThreads, lt.total, [&] {
     implicit_trace_kernel(meta.data(), flags.data(), in_ptr.data(), in_src.data(), in_label.data(), in_w.data(),

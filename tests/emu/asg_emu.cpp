@@ -1,9 +1,9 @@
 /*
  * tests/emu/asg_emu.cpp -- TEST INFRASTRUCTURE: the device side of gtnb_asg_loss_ex as trellis_loss_fast runs it,
  * from the SOURCE of gtn_b200/csrc/k_ngram.cu (ASG's numerator graphs, the dense trellis in its start mode) and
- * k_implicit.cu (the numerator's sweeps), on the CPU through tests/emu/simt_emu.h.  Only the launch geometry, the
- * table slabs and the scatter of the numerator's arc gradients (launch_scatter_add: dst[map[a]] += src[a]) are
- * restated here.
+ * k_implicit.cu (the numerator's sweeps), on the CPU through tests/emu/simt_emu.h.  The trellis launches take their
+ * instantiations and geometry from k_ngram.cu; only the table slabs, the numerator sweeps' narrow kernels and layouts
+ * and the scatter of the numerator's arc gradients (launch_scatter_add: dst[map[a]] += src[a]) are restated here.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_implicit.cu"
@@ -79,22 +79,14 @@ int emu_asg(int B, int T, int C, const float* emissions, const int32_t* input_le
   });
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
-#define RUN(KK)                                                                                                 \
-  do {                                                                                                          \
-    emu::launch(B, threads, 0, [&] {                                                                            \
-      ngram_den_forward_kernel<KK, true>(T, C, lanes, Tb.data(), emissions, (long long)T * C, trans_w,         \
-                                         alpha.data(), den.data(), status);                                     \
-    });                                                                                                         \
-    emu::launch(B, threads, 0, [&] {                                                                            \
-      ngram_den_backward_kernel<KK, true>(T, C, lanes, Tb.data(), emissions, (long long)T * C, trans_w,        \
-                                          alpha.data(), den.data(), grad, (long long)T * C, tg.data());         \
-    });                                                                                                         \
-  } while (0)
-  if (K == 16)
-    RUN(16);
-  else
-    RUN(32);
-#undef RUN
+  emu::launch(B, threads, 0, [&] {
+    ngram_den_forward_kernel_for<true, float>(K)(T, C, lanes, Tb.data(), emissions, (long long)T * C, trans_w,
+                                                 alpha.data(), den.data(), status);
+  });
+  emu::launch(B, threads, 0, [&] {
+    ngram_den_backward_kernel_for<true, float>(K)(T, C, lanes, Tb.data(), emissions, (long long)T * C, trans_w,
+                                                  alpha.data(), den.data(), grad, (long long)T * C, tg.data());
+  });
   for (long long a = 0; a < gg; a++) tg[map[a]] += ggrad[a];
   for (int b = 0; b < B; b++) losses[b] = den[b] - num[b];
   for (long long k = 0; k < nTrans; k++) trans_grad[k] = tg[k];

@@ -2,8 +2,8 @@
  * tests/emu/bidir_half_emu.cpp -- TEST INFRASTRUCTURE: tests/emu/bidir_emu.cpp's run of the SOURCE of
  * gtn_b200/csrc/k_bidir.cu on the CPU (tests/emu/simt_emu.h, fed by k_ctc.cu's ctc_build_kernel exactly as
  * gtnb_ctc_loss feeds it), for any element type of the emissions and the gradient: float, bf16_t or fp16 --
- * gtnb_ctc_loss_ex's native route.  Also exports gtnb_ptx.h's emulated 16-bit conversions.  Only the launch
- * geometry and the device tables are restated here.
+ * gtnb_ctc_loss_ex's native route.  Also exports gtnb_ptx.h's emulated 16-bit conversions.  The kernel and its
+ * geometry are bidir_plan's, as for launch_bidir_ctc; only the device tables are restated here.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_ctc.cu"
@@ -25,7 +25,9 @@ int run_bidir_ctc(
   std::vector<int32_t> tgt_off(B);
   long long nodes = 0, arcs = 0, scores_len = 0, acc = 0, toff = 0;
   int maxN = 0;
-  const bool fx = C == 64 || C == 128; // launch_bidir_ctc's rule: fixed row pitch for the FX kernels
+  for (int b = 0; b < B; b++) maxN = std::max(maxN, 2 * target_lens[b] + 1);
+  // saved-score rows of the fixed pitch where the graphs fit it, as gtnb_compose_linear allocates them
+  const BidirPlan p = bidir_plan<E>(C, maxN, maxN <= bidir::kFixedPitch, bidir_mode != 0);
   for (int b = 0; b < B; b++) {
     const int L = 2 * target_lens[b] + 1;
     GraphMeta& m = meta[b];
@@ -42,8 +44,7 @@ int run_bidir_ctc(
     nodes += L + 1;
     arcs += 3 * L;
     acc += 2;
-    scores_len += (long long)(T + 1) * (fx ? bidir::kFixedPitch : ((L + 3) & ~3));
-    maxN = std::max(maxN, L);
+    scores_len += (long long)(T + 1) * (p.fx ? bidir::kFixedPitch : ((L + 3) & ~3));
   }
   std::vector<uint8_t> flags(nodes, 0);
   std::vector<int32_t> in_ptr(nodes, 0), in_src(arcs, 0), in_label(arcs, 0), in_arc(arcs, 0), il(arcs, 0),
@@ -79,26 +80,12 @@ int run_bidir_ctc(
   P.grad = grad;
   P.grad_stride = (long long)T * C;
   P.C = C;
-  // launch_bidir_ctc's rule: the PAIR kernels (two nodes per thread) for gtnb_ctc_loss's own graphs
-  const bool pair = fx && bidir_mode != 0 && maxN <= 2 * 32 * bidir::kMaxPairWarps - 1;
   P.ctc_blank = blank;
   P.targets = targets;
   for (int b = 0; b < B; b++) meta[b].tgt_off = tgt_off[b];
-  P.nwn = pair ? std::max(1, ((maxN + 1) / 2 + 31) / 32) : std::max(1, (maxN + 31) / 32);
-  P.lay = bidir::make_layout(C, fx ? bidir::kFixedPitch : ((maxN + 3) & ~3), (int)sizeof(E));
-  const unsigned block = 32 * (P.nwn + 1 + bidir::kHelpers);
-  emu::launch_clusters(2 * B, 2, block, P.lay.total, [&] {
-    if (pair)
-      C == 64 ? bidir::bidir_ctc_kernel<1, true, 1, E>(P) : bidir::bidir_ctc_kernel<2, true, 1, E>(P);
-    else if (fx && C == 64)
-      bidir::bidir_ctc_kernel<1, true, 0, E>(P);
-    else if (fx)
-      bidir::bidir_ctc_kernel<2, true, 0, E>(P);
-    else if (C <= 64)
-      bidir::bidir_ctc_kernel<1, false, 0, E>(P);
-    else
-      bidir::bidir_ctc_kernel<2, false, 0, E>(P);
-  });
+  P.nwn = p.nwn;
+  P.lay = p.lay;
+  emu::launch_clusters(2 * B, 2, p.block, P.lay.total, [&] { p.kernel(P); });
   if (emu::g_launch_failed.exchange(false)) return emu::kEmuNoThreads;
   for (int b = 0; b < B; b++) {
     znorm[b] = 0.0f;

@@ -3,7 +3,8 @@
  * (frame-synchronous device composition: alive sets, counts, scans, CSR emission, and compose's
  * gradFunc) and of k_shortest.cu's generic shortest-distance kernels on the CPU through
  * tests/emu/simt_emu.h.  The slab layout of gtnb_capi.cu's composed_alloc and the launch geometry
- * of launch_compose / launch_forward / launch_backward are restated here.
+ * of launch_compose / launch_forward / launch_backward are restated here; the staged kernels' plan, fused layout and
+ * instantiations are k_staged.cu's own.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_compose.cu"
@@ -441,7 +442,7 @@ int emu_sort_rows_with_grads(
  * (fused == 0) or sd_backward_fused (fused != 0).  cp.async.bulk / mbarrier are emulated (simt_emu.h).
  * Tables as in emu_compose; out_scores[B]; grad_emis [B][T][C] zero on entry; viterbi != 0 additionally
  * runs the MODE_PATH sweep + traceback (labels into vit_labels [B][T], scores into vit_scores).
- * Returns 0, or 3 when the staged plan does not apply (mean degree > 4 or too large).
+ * Returns 0, or 3 when k_staged.cu's plan is not G = 1 (mean degree > 4), does not fit, or refuses the fused layout.
  */
 int emu_materialised_staged(
     int B, int T, int C, const float* emissions, const int32_t* lens, const int32_t* n_nodes, const uint8_t* flags,
@@ -452,40 +453,25 @@ int emu_materialised_staged(
   Lat L;
   if (int rc = build_lattice(L, B, T, C, emissions, lens, n_nodes, flags, in_ptr, in_src, in_label, in_arc, in_w, n_acc, acc))
     return rc;
-  // plan() of k_staged.cu, restated: stages, layouts, lanes per node
-  int max_L = 0, maxN = 0, maxA = 0;
-  long long sumA = 0, sumN = 0;
+  int maxN = 0, maxA = 0;
   for (int b = 0; b < B; b++) {
-    max_L = std::max(max_L, L.meta[b].L);
-    sumA += L.meta[b].sg_A;
-    sumN += L.meta[b].sg_N;
     maxN = std::max(maxN, L.meta[b].sg_N);
     maxA = std::max(maxA, L.meta[b].sg_A);
   }
-  const double deg = sumN ? (double)sumA / (double)sumN : 0.0;
-  if (deg > 4.0 || max_L + 1 > kMaxLevelsInSmem) return 3;
-  Layout lf{}, lb{};
-  bool ok = false;
-  for (int ls = 3; ls >= 1 && !ok; ls--) {
-    lf = make_layout(maxN, maxA, max_L, ls, 2, false);
-    lb = make_layout(maxN, maxA, max_L, ls, 4, true);
-    const int cap = (lb.total <= 100 * 1024 || ls == 1) ? 200 * 1024 : 100 * 1024;
-    ok = lb.total <= cap && lf.total <= cap;
-  }
-  if (!ok) return 3;
+  const StagedPlan p = plan(L.meta.data(), B, maxN, maxA);
+  if (!p.ok || p.G != 1) return 3;
+  const Layout &lf = p.fwd, &lb = p.bwd;
+  Layout lay = lb; // sd_backward_fused's
+  if (fused && !fused_layout(lay, maxN, maxA)) return 3;
   constexpr int kT = 32 * consumer_warps(1) + 32;
   std::vector<float> scores((size_t)L.tn + 16, 0.0f), arc_grad((size_t)L.ta + 16, 0.0f);
   std::vector<int32_t> back_ptr((size_t)L.tn + 16, -1), best(B, -1);
   emu::launch(B, kT, lf.total, [&] {
-    sd_forward_staged<MODE_LOG, 1>(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(), L.arcs.data(),
-                                   L.acc_stage.data(), scores.data(), back_ptr.data(), out_scores, best.data(), lf);
+    sd_forward_staged_kernel_for(MODE_LOG, p.G)(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(),
+                                                L.arcs.data(), L.acc_stage.data(), scores.data(), back_ptr.data(),
+                                                out_scores, best.data(), lf);
   });
   if (fused) {
-    Layout lay = lb;
-    lay.tab_nodes = maxN;
-    lay.tab_arcs = maxA;
-    lay.off_tab = (lay.total + 15) / 16 * 16;
-    lay.total = lay.off_tab + 4 * (3 * lay.tab_nodes + 2 + 3 * lay.tab_arcs) + 16;
     emu::launch(B, kT, lay.total, [&] {
       sd_backward_fused(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(), L.arcs.data(), L.gi.data(),
                         L.acc_stage.data(), scores.data(), out_scores, deltas, L.sg_ptr.data(), L.sg_src.data(),
@@ -493,9 +479,9 @@ int emu_materialised_staged(
     });
   } else {
     emu::launch(B, kT, lb.total, [&] {
-      sd_backward_staged<false, 1>(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(), L.arcs.data(),
-                                   L.acc_stage.data(), scores.data(), out_scores, best.data(), deltas,
-                                   arc_grad.data(), lb);
+      sd_backward_staged_kernel_for(false, p.G)(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(),
+                                                L.arcs.data(), L.acc_stage.data(), scores.data(), out_scores,
+                                                best.data(), deltas, arc_grad.data(), lb);
     });
     int capN = 1;
     for (int b = 0; b < B; b++) capN = std::max(capN, L.meta[b].cap_N);
@@ -512,8 +498,9 @@ int emu_materialised_staged(
   }
   if (viterbi) {
     emu::launch(B, kT, lf.total, [&] {
-      sd_forward_staged<MODE_PATH, 1>(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(), L.arcs.data(),
-                                      L.acc_stage.data(), scores.data(), back_ptr.data(), vit_scores, best.data(), lf);
+      sd_forward_staged_kernel_for(MODE_PATH, p.G)(L.meta.data(), L.lnp.data(), L.lap.data(), L.rp.data(),
+                                                   L.arcs.data(), L.acc_stage.data(), scores.data(), back_ptr.data(),
+                                                   vit_scores, best.data(), lf);
     });
     std::vector<int32_t> path((size_t)B * std::max(T, 1), -1), plen(B, 0), pg((size_t)B * std::max(T, 1), -1),
         pl((size_t)B * std::max(T, 1), -1);

@@ -2,8 +2,8 @@
  * tests/emu/ctc_async_emu.cpp -- TEST INFRASTRUCTURE: runs the SOURCE of gtn_b200/csrc/k_ctc.cu's
  * gtnb_ctc_loss_async kernels (ctc_async_prepare_kernel, ctc_async_finalize_kernel) on the CPU through
  * tests/emu/simt_emu.h, alone and around k_bidir.cu's kernel on the padded, bound-uniform layout the asynchronous
- * call gives it.  Only the launch geometry and the buffers are restated here; the descriptors of utterances 0 and 1
- * (m0, m1) come from the caller.
+ * call gives it.  The bidirectional kernel and its geometry are bidir_plan's; only the 1-D grids and the buffers are
+ * restated here, and the descriptors of utterances 0 and 1 (m0, m1) come from the caller.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_ctc.cu"
@@ -71,10 +71,9 @@ int emu_ctc_async_bidir(int B, int T, int C, int S, const GraphMeta* m01, long l
   std::vector<int32_t> in_ptr((size_t)B * sgn, 0), in_src((size_t)B * sga, 0), in_label((size_t)B * sga, 0),
       in_arc((size_t)B * sga, 0), il((size_t)B * sga, 0), ol((size_t)B * sga, 0), acc_nodes(4 * (size_t)B, 0);
   std::vector<float> in_w((size_t)B * sga, 0.0f);
-  // launch_bidir_ctc's rules: fixed row pitch for C = 64, 128 on the fixed-pitch layout; PAIR kernels below 224 nodes
-  const bool fx = (C == 64 || C == 128) && maxN <= bidir::kFixedPitch;
-  const bool pair = fx && bidir_mode != 0 && maxN <= 2 * 32 * bidir::kMaxPairWarps - 1;
-  if (!pair)
+  // the padded layout's saved-score rows have the fixed pitch where the graphs fit it
+  const BidirPlan p = bidir_plan<float>(C, maxN, maxN <= bidir::kFixedPitch, bidir_mode != 0);
+  if (!p.pair)
     emu::launch(B, 256, 0, [&] {
       ctc_build_kernel(meta.data(), targets, small.data(), small.data() + B, blank, C, flags.data(), in_ptr.data(),
                        in_src.data(), in_label.data(), in_arc.data(), in_w.data(), il.data(), ol.data(),
@@ -104,21 +103,9 @@ int emu_ctc_async_bidir(int B, int T, int C, int S, const GraphMeta* m01, long l
   P.C = C;
   P.ctc_blank = blank;
   P.targets = targets;
-  P.nwn = pair ? std::max(1, ((maxN + 1) / 2 + 31) / 32) : std::max(1, (maxN + 31) / 32);
-  P.lay = bidir::make_layout(C, fx ? bidir::kFixedPitch : ((maxN + 3) & ~3));
-  const unsigned block = 32 * (P.nwn + 1 + bidir::kHelpers);
-  emu::launch_clusters(2 * B, 2, block, P.lay.total, [&] {
-    if (pair)
-      C == 64 ? bidir::bidir_ctc_kernel<1, true, 1>(P) : bidir::bidir_ctc_kernel<2, true, 1>(P);
-    else if (fx && C == 64)
-      bidir::bidir_ctc_kernel<1, true, 0>(P);
-    else if (fx)
-      bidir::bidir_ctc_kernel<2, true, 0>(P);
-    else if (C <= 64)
-      bidir::bidir_ctc_kernel<1, false, 0>(P);
-    else
-      bidir::bidir_ctc_kernel<2, false, 0>(P);
-  });
+  P.nwn = p.nwn;
+  P.lay = p.lay;
+  emu::launch_clusters(2 * B, 2, p.block, P.lay.total, [&] { p.kernel(P); });
   finalize(B, zp, zs.data(), zs.data() + (size_t)zp * B, kstatus.data(), valid.data(), losses, status, grad,
            (long long)T * C);
   return emu::g_launch_failed.exchange(false) ? emu::kEmuNoThreads : 0;

@@ -14,24 +14,12 @@ extern "C" {
 int emu_viterbi_dense(int B, int T, int C, const float* emissions, const int32_t* lens, const float* trans,
                       int32_t* paths, float* scores) {
   using namespace gtnb;
-  if (C < 1 || C > 256 || (C % 4) != 0) return 1;
-  int G = 1;
-  while (G < 32 && C * (G * 2) <= kDenseThreads) G *= 2;
-  const size_t smem = sizeof(float) * ((size_t)C * (C + 32 / G) + 2 * (size_t)C);
-  std::vector<uint8_t> bp((size_t)B * std::max(T, 1) * C, 0);
-#define RUN(G_)                                                                                            \
-  emu::launch(B, kDenseThreads, smem, [&] {                                                                \
-    viterbi_dense_kernel<G_>(T, C, lens, emissions, (long long)T * C, trans, bp.data(), paths, scores);    \
-  })
-  switch (G) {
-    case 1: RUN(1); break;
-    case 2: RUN(2); break;
-    case 4: RUN(4); break;
-    case 8: RUN(8); break;
-    case 16: RUN(16); break;
-    default: RUN(32); break;
-  }
-#undef RUN
+  if (!viterbi_dense_supported(C) || (C % 4) != 0) return 1;
+  std::vector<uint8_t> bp((size_t)B * std::max(T, 1) * dense_bp_pitch(C), 0);
+  const auto kernel = viterbi_dense_kernel_for<float>(dense_lanes(C), false);
+  emu::launch(B, kDenseThreads, dense_smem_bytes(C), [&] {
+    kernel(T, C, lens, emissions, (long long)T * C, trans, bp.data(), paths, scores, 0.0f);
+  });
   if (emu::g_launch_failed.exchange(false)) return emu::kEmuNoThreads; // the host refused the threads
   return 0;
 }

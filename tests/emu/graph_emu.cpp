@@ -1,7 +1,8 @@
 /*
  * tests/emu/graph_emu.cpp -- TEST INFRASTRUCTURE: runs the SOURCE of gtn_b200/csrc/k_implicit.cu's arc-label
  * instantiations (gtnb_graph_loss on graphs whose nodes have in-arcs of different labels) on the CPU through
- * tests/emu/simt_emu.h.  Only the launch geometry and the device tables are restated here.
+ * tests/emu/simt_emu.h.  The kernels and layouts are picked as launch_implicit_forward / _backward pick them; only the
+ * device tables are restated here.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_implicit.cu"
@@ -71,35 +72,15 @@ int emu_graph_arc(
   const int Gb = force_narrow ? 0 : wide_lanes(max_in, max_out, maxN, C, true, true);
   const ImpLayout lf = make_imp_layout(maxN, maxA, false, Gf > 0, C, true);
   const ImpLayout lb = make_imp_layout(maxN, maxA, true, Gb > 0, C, true);
-#define FWD_ARGS \
-  meta.data(), flags.data(), ptr.data(), src.data(), lab.data(), w.data(), emissions, scores.data(), out_scores, status, C, lf
-#define BWD_ARGS                                                                                                \
-  meta.data(), flags.data(), ptr.data(), src.data(), lab.data(), w.data(), arc.data(), grad_graph, emissions, \
-      scores.data(), out_scores, deltas, grad, (long long)T * C, C, lb
-#define RUN_FWD(K) emu::launch(B, kImpThreads, lf.total, [&] { K(FWD_ARGS); })
-#define RUN_BWD(K) emu::launch(B, kImpThreads, lb.total, [&] { K(BWD_ARGS); })
-  switch (Gf) {
-    case 0: RUN_FWD(implicit_forward_kernel<true>); break;
-    case 1: RUN_FWD((implicit_forward_wide_kernel<1, true>)); break;
-    case 2: RUN_FWD((implicit_forward_wide_kernel<2, true>)); break;
-    case 4: RUN_FWD((implicit_forward_wide_kernel<4, true>)); break;
-    case 8: RUN_FWD((implicit_forward_wide_kernel<8, true>)); break;
-    case 16: RUN_FWD((implicit_forward_wide_kernel<16, true>)); break;
-    default: RUN_FWD((implicit_forward_wide_kernel<32, true>)); break;
-  }
-  switch (Gb) {
-    case 0: RUN_BWD((implicit_backward_kernel<true, true>)); break;
-    case 1: RUN_BWD((implicit_backward_wide_kernel<1, true, true>)); break;
-    case 2: RUN_BWD((implicit_backward_wide_kernel<2, true, true>)); break;
-    case 4: RUN_BWD((implicit_backward_wide_kernel<4, true, true>)); break;
-    case 8: RUN_BWD((implicit_backward_wide_kernel<8, true, true>)); break;
-    case 16: RUN_BWD((implicit_backward_wide_kernel<16, true, true>)); break;
-    default: RUN_BWD((implicit_backward_wide_kernel<32, true, true>)); break;
-  }
-#undef RUN_FWD
-#undef RUN_BWD
-#undef FWD_ARGS
-#undef BWD_ARGS
+  emu::launch(B, kImpThreads, lf.total, [&] {
+    implicit_forward_kernel_for<true, false>(Gf)(meta.data(), flags.data(), ptr.data(), src.data(), lab.data(),
+                                                 w.data(), emissions, scores.data(), out_scores, status, C, lf);
+  });
+  emu::launch(B, kImpThreads, lb.total, [&] {
+    implicit_backward_kernel_for<true>(Gb, true)(meta.data(), flags.data(), ptr.data(), src.data(), lab.data(),
+                                                 w.data(), arc.data(), grad_graph, emissions, scores.data(),
+                                                 out_scores, deltas, grad, (long long)T * C, C, lb);
+  });
   if (emu::g_launch_failed.exchange(false)) return -emu::kEmuNoThreads;
   return Gb;
 }

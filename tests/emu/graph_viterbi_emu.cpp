@@ -1,7 +1,8 @@
 /*
  * tests/emu/graph_viterbi_emu.cpp -- TEST INFRASTRUCTURE: runs the SOURCE of gtn_b200/csrc/k_implicit.cu's tropical
  * forward instantiations and its traceback kernel (gtnb_graph_viterbi's device route) on the CPU through
- * tests/emu/simt_emu.h.  Only the launch geometry and the device tables are restated here.
+ * tests/emu/simt_emu.h.  The kernels and layouts are picked as launch_implicit_forward / _trace pick them (unless the
+ * caller overrides the lanes or the traceback's block); only the device tables are restated here.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_implicit.cu"
@@ -68,28 +69,12 @@ int emu_graph_viterbi(
   for (int b = 0; b < B; b++) status[b] = 0;
   const int G = lanes >= 0 ? lanes : wide_lanes(max_in, max_out, maxN, C, false, arc != 0);
   const ImpLayout lf = make_imp_layout(maxN, maxA, false, G > 0, C, arc != 0);
-#define FWD_ARGS \
-  meta.data(), flags.data(), ptr.data(), src.data(), lab.data(), w.data(), emissions, scores.data(), out.data(), status, C, lf
-#define RUN_FWD(K) emu::launch(B, kImpThreads, lf.total, [&] { K(FWD_ARGS); })
-#define RUN_MODE(A)                                                       \
-  switch (G) {                                                            \
-    case 0: RUN_FWD((implicit_forward_kernel<A, true>)); break;           \
-    case 1: RUN_FWD((implicit_forward_wide_kernel<1, A, true>)); break;   \
-    case 2: RUN_FWD((implicit_forward_wide_kernel<2, A, true>)); break;   \
-    case 4: RUN_FWD((implicit_forward_wide_kernel<4, A, true>)); break;   \
-    case 8: RUN_FWD((implicit_forward_wide_kernel<8, A, true>)); break;   \
-    case 16: RUN_FWD((implicit_forward_wide_kernel<16, A, true>)); break; \
-    default: RUN_FWD((implicit_forward_wide_kernel<32, A, true>)); break; \
-  }
-  if (arc)
-    RUN_MODE(true)
-  else
-    RUN_MODE(false)
-#undef RUN_MODE
-#undef RUN_FWD
-#undef FWD_ARGS
-  TraceLayout lt = make_trace_layout(maxN, maxA, C, frames > 0 ? frames : kTrMaxFrames);
-  while (frames <= 0 && lt.K > 1 && lt.total > kTrSmemTarget) lt = make_trace_layout(maxN, maxA, C, lt.K / 2);
+  const auto forward = arc ? implicit_forward_kernel_for<true, true>(G) : implicit_forward_kernel_for<false, true>(G);
+  emu::launch(B, kImpThreads, lf.total, [&] {
+    forward(meta.data(), flags.data(), ptr.data(), src.data(), lab.data(), w.data(), emissions, scores.data(),
+            out.data(), status, C, lf);
+  });
+  const TraceLayout lt = frames > 0 ? make_trace_layout(maxN, maxA, C, frames) : trace_layout(maxN, maxA, C);
   emu::launch(B, kImpThreads, lt.total, [&] {
     implicit_trace_kernel(meta.data(), flags.data(), ptr.data(), src.data(), lab.data(), w.data(), ids.data(),
                           emissions, scores.data(), status, paths, arcs, scores_out, T, C, lt);

@@ -1,7 +1,8 @@
 /*
  * tests/emu/implicit_emu.cpp -- TEST INFRASTRUCTURE: runs the SOURCE of gtn_b200/csrc/k_implicit.cu
  * (the criterion's implicit-lattice sweeps: the hot kernels of bench.py) on the CPU through
- * tests/emu/simt_emu.h.  Only the launch geometry and the device tables are restated here.
+ * tests/emu/simt_emu.h.  emu_implicit_general picks its kernels and layouts as launch_implicit_forward / _backward
+ * do; emu_implicit and emu_implicit_ctc run the narrow kernels directly.  The device tables are restated here.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_ctc.cu"
@@ -131,36 +132,17 @@ int emu_implicit_general(
   const int Gf = wide_lanes(max_in, max_out, t.maxN, C, false), Gb = wide_lanes(max_in, max_out, t.maxN, C, true);
   const ImpLayout lf = make_imp_layout(t.maxN, t.maxA, false, Gf > 0, C);
   const ImpLayout lb = make_imp_layout(t.maxN, t.maxA, true, Gb > 0, C);
-#define FWD_ARGS                                                                                            \
-  t.meta.data(), t.flags.data(), t.in_ptr.data(), t.in_src.data(), t.in_label.data(), t.in_w.data(), emissions, \
-      scores.data(), out_scores, status, C, lf
-#define BWD_ARGS                                                                                            \
-  t.meta.data(), t.flags.data(), t.in_ptr.data(), t.in_src.data(), t.in_label.data(), t.in_w.data(),        \
-      t.in_arc.data(), grad_graph, emissions, scores.data(), out_scores, deltas, grad, (long long)T * C, C, lb
-#define RUN_FWD(K) emu::launch(B, kImpThreads, lf.total, [&] { K(FWD_ARGS); })
-#define RUN_BWD(K) emu::launch(B, kImpThreads, lb.total, [&] { K(BWD_ARGS); })
-  switch (Gf) {
-    case 0: RUN_FWD(implicit_forward_kernel); break;
-    case 1: RUN_FWD(implicit_forward_wide_kernel<1>); break;
-    case 2: RUN_FWD(implicit_forward_wide_kernel<2>); break;
-    case 4: RUN_FWD(implicit_forward_wide_kernel<4>); break;
-    case 8: RUN_FWD(implicit_forward_wide_kernel<8>); break;
-    case 16: RUN_FWD(implicit_forward_wide_kernel<16>); break;
-    default: RUN_FWD(implicit_forward_wide_kernel<32>); break;
-  }
-  switch (Gb) {
-    case 0: RUN_BWD(implicit_backward_kernel<true>); break;
-    case 1: RUN_BWD((implicit_backward_wide_kernel<1, true>)); break;
-    case 2: RUN_BWD((implicit_backward_wide_kernel<2, true>)); break;
-    case 4: RUN_BWD((implicit_backward_wide_kernel<4, true>)); break;
-    case 8: RUN_BWD((implicit_backward_wide_kernel<8, true>)); break;
-    case 16: RUN_BWD((implicit_backward_wide_kernel<16, true>)); break;
-    default: RUN_BWD((implicit_backward_wide_kernel<32, true>)); break;
-  }
-#undef RUN_FWD
-#undef RUN_BWD
-#undef FWD_ARGS
-#undef BWD_ARGS
+  emu::launch(B, kImpThreads, lf.total, [&] {
+    implicit_forward_kernel_for<false, false>(Gf)(t.meta.data(), t.flags.data(), t.in_ptr.data(), t.in_src.data(),
+                                                  t.in_label.data(), t.in_w.data(), emissions, scores.data(),
+                                                  out_scores, status, C, lf);
+  });
+  emu::launch(B, kImpThreads, lb.total, [&] {
+    implicit_backward_kernel_for<false>(Gb, true)(t.meta.data(), t.flags.data(), t.in_ptr.data(), t.in_src.data(),
+                                                  t.in_label.data(), t.in_w.data(), t.in_arc.data(), grad_graph,
+                                                  emissions, scores.data(), out_scores, deltas, grad,
+                                                  (long long)T * C, C, lb);
+  });
   if (emu::g_launch_failed.exchange(false)) return -emu::kEmuNoThreads;
   return Gb;
 }

@@ -2,7 +2,8 @@
  * tests/emu/ngram_emu.cpp -- TEST INFRASTRUCTURE: the device side of gtnb_ngram_ctc_loss as
  * trellis_loss_fast runs it, from the SOURCE of gtn_b200/csrc/k_ngram.cu (sigma, the folded numerator
  * graphs, the dense-trellis forward / backward, the sigma fold) and k_implicit.cu (the numerator's sweeps), on
- * the CPU through tests/emu/simt_emu.h.  Only the launch geometry, the table slabs and the scatter of the
+ * the CPU through tests/emu/simt_emu.h.  The trellis launches take their instantiations and geometry from k_ngram.cu;
+ * only the table slabs, the numerator sweeps' narrow kernels and layouts, the 1-D grids and the scatter of the
  * numerator's arc gradients (launch_scatter_add: dst[map[a]] += src[a]) are restated here.
  */
 #define GTNB_HOST_EMU 1
@@ -82,22 +83,14 @@ int emu_ngram_ctc(int B, int T, int C, const float* emissions, const int32_t* in
   });
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
-#define RUN(KK)                                                                                                 \
-  do {                                                                                                          \
-    emu::launch(B, threads, 0, [&] {                                                                            \
-      ngram_den_forward_kernel<KK>(T, C, lanes, Tb.data(), emissions, (long long)T * C, W, alpha.data(),       \
-                                   den.data(), status);                                                         \
-    });                                                                                                         \
-    emu::launch(B, threads, 0, [&] {                                                                            \
-      ngram_den_backward_kernel<KK>(T, C, lanes, Tb.data(), emissions, (long long)T * C, W, alpha.data(),      \
-                                    den.data(), grad, (long long)T * C, tg.data());                             \
-    });                                                                                                         \
-  } while (0)
-  if (K == 16)
-    RUN(16);
-  else
-    RUN(32);
-#undef RUN
+  emu::launch(B, threads, 0, [&] {
+    ngram_den_forward_kernel_for<false, float>(K)(T, C, lanes, Tb.data(), emissions, (long long)T * C, W,
+                                                  alpha.data(), den.data(), status);
+  });
+  emu::launch(B, threads, 0, [&] {
+    ngram_den_backward_kernel_for<false, float>(K)(T, C, lanes, Tb.data(), emissions, (long long)T * C, W,
+                                                   alpha.data(), den.data(), grad, (long long)T * C, tg.data());
+  });
   for (long long a = 0; a < gg; a++) tg[map[a]] += ggrad[a];
   emu::launch((C * C + 255) / 256, 256, 0, [&] { ngram_fold_kernel(C, W, sigma.data(), tg.data()); });
   for (int b = 0; b < B; b++) losses[b] = den[b] - num[b];

@@ -4,8 +4,9 @@
  * the dense trellis), k_implicit.cu (the numerator's sweeps) and k_dense.cu (the factored Viterbi) on the CPU through
  * tests/emu/simt_emu.h, for any element type of the emissions: float, bf16_t or f16_t.  As on the device, the
  * gradients stay float32 (the caller rounds them once).  ngram_emu.cpp / asg_emu.cpp / dense_emu.cpp run the float32
- * kernels the same way; only the launch geometry and the table slabs are restated here.  Also exports k_implicit.cu's
- * host check of which modes a 16-bit lattice may take.
+ * kernels the same way.  The trellis and Viterbi launches take their instantiations and geometry from the kernel files;
+ * only the table slabs, the numerator sweeps' narrow kernels (wide_lanes' pick for in-degrees of at most three) and
+ * their layouts are restated here.  Also exports k_implicit.cu's host check of which modes a 16-bit lattice may take.
  */
 #define GTNB_HOST_EMU 1
 #include "../../gtn_b200/csrc/k_dense.cu"
@@ -97,26 +98,15 @@ int run_trellis(int asg, int B, int T, int C, const E* emissions, const int32_t*
   });
   int K, lanes, threads;
   ngram_den_shape(C, &K, &lanes, &threads);
-#define RUN(KK, START)                                                                                          \
-  do {                                                                                                          \
-    emu::launch(B, threads, 0, [&] {                                                                            \
-      ngram_den_forward_kernel<KK, START, E>(T, C, lanes, Tb.data(), emissions, (long long)T * C, W,            \
-                                             alpha.data(), den, status);                                        \
-    });                                                                                                         \
-    emu::launch(B, threads, 0, [&] {                                                                            \
-      ngram_den_backward_kernel<KK, START, E>(T, C, lanes, Tb.data(), emissions, (long long)T * C, W,           \
-                                              alpha.data(), den, grad, (long long)T * C, tg.data());            \
-    });                                                                                                         \
-  } while (0)
-  if (K == 16 && asg)
-    RUN(16, true);
-  else if (K == 16)
-    RUN(16, false);
-  else if (asg)
-    RUN(32, true);
-  else
-    RUN(32, false);
-#undef RUN
+  const auto forward = asg ? ngram_den_forward_kernel_for<true, E>(K) : ngram_den_forward_kernel_for<false, E>(K);
+  const auto backward = asg ? ngram_den_backward_kernel_for<true, E>(K) : ngram_den_backward_kernel_for<false, E>(K);
+  emu::launch(B, threads, 0, [&] {
+    forward(T, C, lanes, Tb.data(), emissions, (long long)T * C, W, alpha.data(), den, status);
+  });
+  emu::launch(B, threads, 0, [&] {
+    backward(T, C, lanes, Tb.data(), emissions, (long long)T * C, W, alpha.data(), den, grad, (long long)T * C,
+             tg.data());
+  });
   for (long long a = 0; a < gg; a++) tg[map[a]] += ggrad[a];
   for (long long k = 0; k < nTrans; k++) trans_grad[k] = tg[k];
   for (long long a = 0; a < gg; a++) arc_grad[a] = ggrad[a];
@@ -125,35 +115,18 @@ int run_trellis(int asg, int B, int T, int C, const E* emissions, const int32_t*
   return 0;
 }
 
-/* launch_viterbi_dense's geometry for any C <= 224 */
+/* launch_viterbi_dense for emissions of element type E */
 template <class E>
 int run_dense(int B, int T, int C, const E* emissions, const int32_t* lens, int bigram, const float* trans,
               int32_t* paths, float* scores) {
   using namespace gtnb;
-  if (C < 1 || C > 224) return 1;
-  int G = 1;
-  while (G < 32 && C * (G * 2) <= kDenseThreads) G *= 2;
-  const size_t smem = sizeof(float) * ((size_t)C * (C + 32 / G) + 2 * (size_t)C);
+  if (!viterbi_dense_supported(C)) return 1;
   std::vector<uint8_t> bp((size_t)B * std::max(T, 1) * dense_bp_pitch(C), 0);
-  const float empty = -std::numeric_limits<float>::infinity();
-#define RUN(G_)                                                                                                 \
-  emu::launch(B, kDenseThreads, smem, [&] {                                                                     \
-    if (bigram)                                                                                                 \
-      viterbi_dense_kernel<G_, true, E>(T, C, lens, emissions, (long long)T * C, trans, bp.data(), paths, scores, \
-                                        empty);                                                                 \
-    else                                                                                                        \
-      viterbi_dense_kernel<G_, false, E>(T, C, lens, emissions, (long long)T * C, trans, bp.data(), paths,      \
-                                         scores, empty);                                                        \
-  })
-  switch (G) {
-    case 1: RUN(1); break;
-    case 2: RUN(2); break;
-    case 4: RUN(4); break;
-    case 8: RUN(8); break;
-    case 16: RUN(16); break;
-    default: RUN(32); break;
-  }
-#undef RUN
+  const auto kernel = viterbi_dense_kernel_for<E>(dense_lanes(C), bigram != 0);
+  emu::launch(B, kDenseThreads, dense_smem_bytes(C), [&] {
+    kernel(T, C, lens, emissions, (long long)T * C, trans, bp.data(), paths, scores,
+           -std::numeric_limits<float>::infinity());
+  });
   if (emu::g_launch_failed.exchange(false)) return emu::kEmuNoThreads;
   return 0;
 }
