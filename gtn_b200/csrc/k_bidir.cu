@@ -87,7 +87,7 @@ namespace bidir {
 
 constexpr int kMaxNodes = 256; // table capacity
 constexpr int kMaxNodeWarps = 7; // graph nodes per utterance: at most 224, one per thread (4 CTAs of 12 warps per SM at 40 registers)
-constexpr int kMaxPairWarps = 4; // PAIR kernels: two nodes per thread, (U + 1) <= 112 pairs
+constexpr int kMaxPairWarps = 4; // PAIR kernels: two nodes per thread, at most kHalfPitch (112) pairs
 constexpr int kRowF = 264; // floats per chain row in shared memory
 constexpr int kDummy = 256; // slot of every chain row that holds kNeg (absent arcs point here)
 constexpr int kBlk = 8; // frames per block (one TMA copy, one helper pass, one renormalisation)
@@ -107,8 +107,10 @@ constexpr int kIntMin = -2147483647 - 1;
 // overflow area of a posterior row all have this many floats, whatever the utterance's node count -- which makes
 // every per-level address of the node warps base + compile-time constant (no pointer arithmetic on the chain)
 constexpr int kFixedPitch = 32 * kMaxNodeWarps;
-// PAIR kernels: floats per saved LABEL row (one per pair, <= 112 pairs); see pair_role for the block layout
+// PAIR kernels: floats per saved LABEL row, one per pair, which bounds the pairs (bidir_plan); see pair_role for the
+// block layout
 constexpr int kHalfPitch = kFixedPitch / 2;
+static_assert(kHalfPitch <= 32 * kMaxPairWarps, "the PAIR kernels' node warps hold every pair");
 
 struct Layout {
   int off_ring, off_e, off_o, off_g, off_od, off_seg, off_perm, off_nlab, off_hlist, off_red, off_redi,
@@ -1540,7 +1542,8 @@ BidirPlan bidir_plan(int C, int max_nodes, bool fixed_pitch, bool pair_ok) {
   BidirPlan p;
   // FX: the benchmark's shapes (C == 64 or 128)
   p.fx = (C == 64 || C == 128) && fixed_pitch;
-  p.pair = p.fx && pair_ok && max_nodes <= 2 * 32 * bidir::kMaxPairWarps - 1;
+  // one saved label row per pair: (max_nodes + 1) / 2 <= kHalfPitch, i.e. U <= 111 for a CTC graph of 2U + 1 nodes
+  p.pair = p.fx && pair_ok && (max_nodes + 1) / 2 <= bidir::kHalfPitch;
   // NQ: float4 chunks of an emission row per helper lane
   if (p.pair)
     p.kernel = C == 64 ? bidir::bidir_ctc_kernel<1, true, 1, E> : bidir::bidir_ctc_kernel<2, true, 1, E>;
@@ -1554,6 +1557,14 @@ BidirPlan bidir_plan(int C, int max_nodes, bool fixed_pitch, bool pair_ok) {
   return p;
 }
 
+/* bidir_supported's shape rules: C labels, levels of at most max_nodes nodes, the graphs' largest in- and
+ * out-degree, esize bytes per emission element (4: float32, 2: bf16 / fp16) */
+inline bool bidir_shape_supported(int C, int max_nodes, int max_in_deg, int max_out_deg, int esize) {
+  if (C % 4 != 0 || C > 128 || C < 4) return false;
+  if (esize != 4 && C % 8 != 0) return false;
+  return max_nodes <= 32 * bidir::kMaxNodeWarps && max_in_deg <= 3 && max_out_deg <= 3;
+}
+
 #ifndef GTNB_HOST_EMU
 
 static_assert(bidir::kFixedPitch == kImplicitFixedPitch, "gtnb_compose_linear allocates the rows");
@@ -1563,9 +1574,9 @@ static_assert(bidir::kFixedPitch == kImplicitFixedPitch, "gtnb_compose_linear al
  * access of the helper warps then stays a multiple of 16 / 8 bytes */
 bool bidir_supported(const gtnb_lattice* lat, const void* emissions, int64_t stride, const void* grad, int64_t grad_stride,
                      int dtype) {
-  if (!lat->composed || lat->C % 4 != 0 || lat->C > 128 || lat->C < 4) return false;
-  if (dtype != GTNB_F32 && lat->C % 8 != 0) return false;
-  if (lat->max_lvl_nodes > 32 * bidir::kMaxNodeWarps || lat->max_in_deg > 3 || lat->max_out_deg > 3) return false;
+  if (!lat->composed) return false;
+  if (!bidir_shape_supported(lat->C, lat->max_lvl_nodes, lat->max_in_deg, lat->max_out_deg, dtype == GTNB_F32 ? 4 : 2))
+    return false;
   if (((uintptr_t)emissions & 15) || (stride & 3)) return false;
   if (grad && (((uintptr_t)grad & 15) || (grad_stride & 3))) return false;
   for (int b = 0; b < lat->B; b++)

@@ -331,6 +331,8 @@ static bool use_staged(const gtnb_ctx* ctx, const gtnb_lattice* lat) {
   return ctx->use_staged && staged_supported(lat);
 }
 
+/* the generic kernels log under their own names ("sd_forward_generic", "sd_backward_generic"), so a launch profile
+ * tells them from the staged kernels ("sd_forward", "sd_backward") */
 int launch_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int mode) {
   if (lat->B == 0) return GTNB_OK;
   if (use_staged(ctx, lat)) return launch_forward_staged(ctx, lat, mode);
@@ -340,11 +342,11 @@ int launch_forward(gtnb_ctx* ctx, gtnb_lattice* lat, int mode) {
       (mode == MODE_PATH ? lat->relax_rank : nullptr), lat->acc_nodes, lat->scores,    \
       lat->back_ptr, lat->out_scores, lat->best_accept
   if (mode == MODE_LOG)
-    GTNB_LAUNCH(ctx, "sd_forward", sd_forward_generic<MODE_LOG><<<grid, block, 0, ctx->stream>>>(ARGS));
+    GTNB_LAUNCH(ctx, "sd_forward_generic", sd_forward_generic<MODE_LOG><<<grid, block, 0, ctx->stream>>>(ARGS));
   else if (mode == MODE_TROPICAL)
-    GTNB_LAUNCH(ctx, "sd_forward", sd_forward_generic<MODE_TROPICAL><<<grid, block, 0, ctx->stream>>>(ARGS));
+    GTNB_LAUNCH(ctx, "sd_forward_generic", sd_forward_generic<MODE_TROPICAL><<<grid, block, 0, ctx->stream>>>(ARGS));
   else
-    GTNB_LAUNCH(ctx, "sd_forward", sd_forward_generic<MODE_PATH><<<grid, block, 0, ctx->stream>>>(ARGS));
+    GTNB_LAUNCH(ctx, "sd_forward_generic", sd_forward_generic<MODE_PATH><<<grid, block, 0, ctx->stream>>>(ARGS));
 #undef ARGS
   return GTNB_OK;
 }
@@ -362,9 +364,9 @@ int launch_backward(gtnb_ctx* ctx, gtnb_lattice* lat, int tropical, const float*
       lat->acc_nodes, lat->scores, lat->out_scores, lat->best_accept, deltas_dev, \
       lat->node_grad, lat->arc_grad
   if (tropical)
-    GTNB_LAUNCH(ctx, "sd_backward", sd_backward_generic<true><<<grid, block, 0, ctx->stream>>>(ARGS));
+    GTNB_LAUNCH(ctx, "sd_backward_generic", sd_backward_generic<true><<<grid, block, 0, ctx->stream>>>(ARGS));
   else
-    GTNB_LAUNCH(ctx, "sd_backward", sd_backward_generic<false><<<grid, block, 0, ctx->stream>>>(ARGS));
+    GTNB_LAUNCH(ctx, "sd_backward_generic", sd_backward_generic<false><<<grid, block, 0, ctx->stream>>>(ARGS));
 #undef ARGS
   return GTNB_OK;
 }

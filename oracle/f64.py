@@ -134,3 +134,82 @@ def asg_f64(emissions, trans_w, target):
                 if U > 1:
                     np.add.at(tgn, C + tg[1:] * C + tg[:-1], s_step[1:])
     return loss, grad, tgd - tgn
+
+
+def lattice_f64(flags, src, dst, w, tropical=False):
+    """forwardScore of a lattice (a DAG) in float64, and its gradient with respect to every arc weight, which is the
+    arc's posterior: exp(alpha[src] + w + beta[dst] - Z) in the log semiring; in the tropical semiring 1 on the arcs
+    of the best path (first maximum in topological order), 0 elsewhere.  flags: bit 0 start, bit 1 accept.  Nodes are
+    taken in a topological order computed here, so the lattice's own node numbering does not matter.
+    Returns (score, arc gradient [A], best path as arc ids or None, smallest margin of a decision on that path)."""
+    flags = np.asarray(flags)
+    src = np.asarray(src, np.int64)
+    dst = np.asarray(dst, np.int64)
+    w = np.asarray(w, np.float64)
+    N, A = len(flags), len(src)
+    indeg = np.bincount(dst, minlength=N)
+    order, stack = [], [n for n in range(N) if indeg[n] == 0]
+    ins = [[] for _ in range(N)]
+    outs = [[] for _ in range(N)]
+    for a in range(A):
+        ins[dst[a]].append(a)
+        outs[src[a]].append(a)
+    while stack:
+        n = stack.pop()
+        order.append(n)
+        for a in outs[n]:
+            indeg[dst[a]] -= 1
+            if indeg[dst[a]] == 0:
+                stack.append(dst[a])
+    assert len(order) == N, "not a DAG"
+    NEG = -np.inf
+    alpha = np.full(N, NEG)
+    best_in = np.full(N, -1)
+    margin_in = np.full(N, np.inf)
+    for n in order:
+        cand = [alpha[src[a]] + w[a] for a in ins[n]]
+        if flags[n] & 1:
+            cand.append(0.0)
+        if not cand:
+            continue
+        c = np.asarray(cand)
+        if tropical:
+            k = int(np.argmax(c))
+            alpha[n] = c[k]
+            if k < len(ins[n]):
+                best_in[n] = ins[n][k]
+            rest = np.delete(c, k)
+            margin_in[n] = c[k] - rest.max() if len(rest) and np.isfinite(c[k]) else np.inf
+        else:
+            alpha[n] = _lse(c)
+    acc = [n for n in range(N) if flags[n] & 2]
+    if not acc:
+        return -np.inf, np.zeros(A), None, np.inf
+    fin = alpha[acc]
+    Z = float(np.max(fin)) if tropical else _lse(fin)
+    grad = np.zeros(A)
+    if not np.isfinite(Z):
+        return Z, grad, None, np.inf
+    if tropical:
+        k = int(np.argmax(fin))
+        rest = np.delete(fin, k)
+        margin = fin[k] - rest.max() if len(rest) else np.inf
+        path, n = [], acc[k]
+        while best_in[n] >= 0:
+            margin = min(margin, margin_in[n])
+            path.append(int(best_in[n]))
+            n = src[best_in[n]]
+        margin = min(margin, margin_in[n])
+        path.reverse()
+        grad[path] = 1.0
+        return Z, grad, path, margin
+    beta = np.full(N, NEG)
+    for n in reversed(order):
+        cand = [w[a] + beta[dst[a]] for a in outs[n]]
+        if flags[n] & 2:
+            cand.append(0.0)
+        if cand:
+            beta[n] = _lse(np.asarray(cand))
+    with np.errstate(invalid="ignore"):
+        grad = np.nan_to_num(np.exp(alpha[src] + w + beta[dst] - Z), nan=0.0)
+    return Z, grad, None, np.inf
