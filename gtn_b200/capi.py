@@ -21,6 +21,8 @@ EPSILON = -1
 DENSE_ASG = 0  # gtnb_viterbi_dense_ex graph kinds
 DENSE_BIGRAM = 1
 DENSE_CTC = 2  # gtnb_beam_decode_async: CTC without transitions
+BEAM_RESET = 1  # gtnb_beam_decode_chunk_async's per-row control bits
+BEAM_END = 2
 F32 = 0  # element types of gtnb_ctc_loss_ex and the *_typed entry points
 BF16 = 1
 F16 = 2
@@ -202,6 +204,12 @@ SYMBOLS = [
     ("gtnb_beam_decode_lexicon_async", C.c_int,
      [_vp, _vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, _vp,
       C.c_float, C.c_float, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t]),
+    ("gtnb_beam_state_create", C.c_int,
+     [_vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, C.c_float,
+      C.c_float, C.POINTER(_vp)]),
+    ("gtnb_beam_state_destroy", None, [_vp, _vp]),
+    ("gtnb_beam_decode_chunk_async", C.c_int,
+     [_vp, _vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     ("gtnb_edit_distance_async", C.c_int,
      [_vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
       C.c_size_t]),

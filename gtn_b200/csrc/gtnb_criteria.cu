@@ -4644,3 +4644,139 @@ extern "C" int gtnb_beam_decode_lexicon_async(
   return async_enqueue(ctx, fn, B, cuda_stream, workspace_dev, workspace_bytes,
                        [&](bool launch) { return beam_async_run(ctx, a, launch, f); });
 }
+
+/*
+ * The streaming decoder of gtnb_beam_decode_chunk_async, in one device allocation: back-pointers [B][T_max][K] by
+ * absolute frame, the rows' state blocks [B][words] (k_beam.cu's beam_state_words, all zero: every row fresh) and, for
+ * BIGRAM and ASG, the transposed weights [C][C], start weights [C] and row flags [C].  The policy's arguments are kept
+ * with their outputs NULL; each call fills those in.
+ */
+struct gtnb_beam_state {
+  int device = 0, B = 0, T = 0, C = 0, kind = 0, blank = 0, K = 0, N = 0;
+  bool lexicon = false;
+  BeamLm lm{};
+  BeamLex lex{};
+  long long words = 0;
+  void* mem = nullptr;
+  uint16_t* bp = nullptr;
+  uint32_t* state = nullptr;
+  float *wt = nullptr, *wfirst = nullptr;
+  int32_t* wbad = nullptr;
+  ~gtnb_beam_state() {
+    if (mem) cudaFree(mem);
+  }
+};
+
+extern "C" int gtnb_beam_state_create(gtnb_ctx* ctx, int B, int T_max, int C, int kind, const float* trans_w_dev,
+                                      int blank, int beam, int nbest, int token_beam, const gtnb_lm* lm,
+                                      const gtnb_lexicon* lexicon, float lm_weight, float bonus,
+                                      gtnb_beam_state** out) {
+  const std::string fn = "gtnb_beam_state_create";
+  if (out) *out = nullptr;
+  if (!ctx || B < 1 || T_max < 1 || C <= 0 || !out || (lm && lexicon) ||
+      (kind == GTNB_DENSE_CTC) != (trans_w_dev == nullptr))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (!(lm_weight >= 0.0f && std::isfinite(lm_weight)) || !std::isfinite(bonus))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": lm_weight must be finite and >= 0, bonus finite");
+  if ((lm && lm->device != ctx->device) || (lexicon && lexicon->device != ctx->device))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM or lexicon was made on another device");
+  if ((lm && lm->C != C) || (lexicon && lexicon->C != C))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the LM or lexicon was made for another C");
+  const BeamAsyncArgs a{B, T_max, C, GTNB_F32, nullptr, nullptr, kind, trans_w_dev, blank, beam, nbest,
+                        nullptr, nullptr, nullptr, nullptr};
+  GTNB_TRY(beam_lm_check(ctx, fn, a, token_beam));
+  if (lexicon && kind != GTNB_DENSE_ASG && (lexicon->spelled[blank] || lexicon->cls[blank] == 1))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the lexicon spells with the blank or makes it a separator");
+  std::unique_ptr<gtnb_beam_state> h(new gtnb_beam_state);
+  h->device = ctx->device;
+  h->B = B;
+  h->T = T_max;
+  h->C = C;
+  h->kind = kind;
+  h->blank = blank;
+  h->K = beam;
+  h->N = nbest;
+  h->lexicon = lexicon != nullptr;
+  h->words = beam_state_row_words(h->lexicon, beam, C);
+  if (lexicon)
+    h->lex = BeamLex{{token_beam, nullptr, nullptr, lexicon->start, lm_weight, bonus, nullptr, nullptr},
+                     lexicon->d_cls,
+                     (C + 31) / 32,
+                     lexicon->d_mask,
+                     lexicon->d_first,
+                     lexicon->d_word,
+                     lexicon->d_smear,
+                     lexicon->d_hash,
+                     lexicon->hmul,
+                     lexicon->hbits,
+                     lexicon->d_bow,
+                     lexicon->d_bod,
+                     lexicon->d_endw,
+                     nullptr,
+                     nullptr};
+  else
+    h->lm = BeamLm{token_beam, lm ? lm->w : nullptr, lm ? lm->d : nullptr, lm ? lm->start : 0,
+                   lm_weight, bonus, nullptr, nullptr};
+  // the byte count of include/gtn_b200.h
+  auto r256 = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t b_bp = r256(2ull * B * T_max * beam), b_st = r256(4ull * B * h->words);
+  const size_t b_wt = kind != GTNB_DENSE_CTC ? r256(4ull * C * C) : 0, b_c = kind != GTNB_DENSE_CTC ? r256(4ull * C) : 0;
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  GTNB_CUDA(ctx, cudaMalloc(&h->mem, b_bp + b_st + b_wt + 2 * b_c));
+  unsigned char* m = static_cast<unsigned char*>(h->mem);
+  h->bp = reinterpret_cast<uint16_t*>(m);
+  h->state = reinterpret_cast<uint32_t*>(m + b_bp);
+  GTNB_CUDA(ctx, cudaMemset(h->state, 0, b_st));
+  if (kind != GTNB_DENSE_CTC) {
+    h->wt = reinterpret_cast<float*>(m + b_bp + b_st);
+    h->wfirst = reinterpret_cast<float*>(m + b_bp + b_st + b_wt);
+    h->wbad = reinterpret_cast<int32_t*>(m + b_bp + b_st + b_wt + b_c);
+    OnStream on(ctx, nullptr);
+    GTNB_TRY(launch_beam_weights(ctx, C, kind, trans_w_dev, h->wt, h->wfirst, h->wbad));
+    if (kind == GTNB_DENSE_ASG) // (the one-shot call reads ASG's start weights from trans_w_dev itself)
+      GTNB_CUDA(ctx, cudaMemcpy(h->wfirst, trans_w_dev, 4ull * C, cudaMemcpyDeviceToDevice));
+  }
+  GTNB_CUDA(ctx, cudaDeviceSynchronize()); // (set-up: the state is on the device before any stream reads it)
+  *out = h.release();
+  return GTNB_OK;
+}
+
+extern "C" void gtnb_beam_state_destroy(gtnb_ctx* ctx, gtnb_beam_state* s) {
+  if (!s) return;
+  if (ctx) cudaSetDevice(s->device);
+  delete s; // (cudaFree waits for the device: no launch still reads the state)
+}
+
+extern "C" int gtnb_beam_decode_chunk_async(gtnb_ctx* ctx, void* cuda_stream, gtnb_beam_state* s, int Tc,
+                                            const void* emissions_dev, int dtype, const int32_t* chunk_lens_dev,
+                                            const int32_t* control_dev, int32_t* tokens_dev, int32_t* lengths_dev,
+                                            float* scores_dev, float* am_scores_dev, float* lm_scores_dev,
+                                            int32_t* words_dev, int32_t* word_counts_dev, int32_t* status_dev,
+                                            int32_t* best_tokens_dev, int32_t* best_lengths_dev,
+                                            float* best_scores_dev) {
+  const std::string fn = "gtnb_beam_decode_chunk_async";
+  const bool best = best_tokens_dev != nullptr;
+  if (!ctx || !s || Tc < 0 || (Tc > 0 && !emissions_dev) || !tokens_dev || !lengths_dev || !scores_dev ||
+      (!s->lexicon && (words_dev || word_counts_dev)) || best != (best_lengths_dev != nullptr) ||
+      best != (best_scores_dev != nullptr))
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": bad arguments");
+  if (s->device != ctx->device)
+    return fail(ctx, GTNB_ERR_INVALID_ARGUMENT, fn + ": the state was made on another device");
+  if (!known_dtype(dtype)) return fail(ctx, GTNB_ERR_UNSUPPORTED, fn + ": unknown dtype");
+  GTNB_CUDA(ctx, cudaSetDevice(ctx->device));
+  OnStream on(ctx, static_cast<cudaStream_t>(cuda_stream));
+  const BeamChunk r{Tc, s->state, s->words, chunk_lens_dev, control_dev, best_tokens_dev, best_lengths_dev,
+                    best_scores_dev};
+  const float* wfirst = s->wfirst;
+  const auto run = [&](auto f) {
+    f.am = am_scores_dev;
+    f.lm = lm_scores_dev;
+    return launch_beam_chunk(ctx, s->B, s->T, s->C, emissions_dev, dtype, s->kind, s->wt, wfirst, s->wbad, s->blank,
+                             s->K, s->N, s->bp, tokens_dev, lengths_dev, scores_dev, status_dev, f, r);
+  };
+  if (!s->lexicon) return run(s->lm);
+  BeamLex f = s->lex;
+  f.words = words_dev;
+  f.counts = word_counts_dev;
+  return run(f);
+}

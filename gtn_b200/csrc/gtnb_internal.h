@@ -237,6 +237,14 @@ int launch_beam_decode(gtnb_ctx* ctx, int B, int T, int C, const void* emissions
                        const int32_t* input_lens, int kind, const float* wt, const float* wfirst, const int32_t* wbad,
                        int blank, int K, int N, uint16_t* bp, int32_t* tokens, int32_t* lengths, float* scores,
                        int32_t* status, const F& f);
+/* the streaming decoder (gtnb_beam_decode_chunk_async): a row's state block in 32-bit words under the BeamLm or the
+ * BeamLex policy, and one chunk of the search under policy F (BeamLm, BeamLex); T is T_max */
+long long beam_state_row_words(bool lexicon, int K, int C);
+template <class F>
+int launch_beam_chunk(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype, int kind,
+                      const float* wt, const float* wfirst, const int32_t* wbad, int blank, int K, int N, uint16_t* bp,
+                      int32_t* tokens, int32_t* lengths, float* scores, int32_t* status, const F& f,
+                      const BeamChunk& r);
 
 int launch_scatter_add(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);
 int launch_gather(gtnb_ctx* ctx, float* dst, const int32_t* idx, const float* src, long long n);

@@ -185,4 +185,21 @@ struct BeamLex : BeamLm {
   int32_t *words, *counts; // [B][N][T] / [B][N] nullable: word ids and word counts of the hypotheses
 };
 
+/*
+ * One chunk call of the streaming beam decoder (gtnb_beam_decode_chunk_async), for k_beam.cu's beam_chunk_kernel:
+ * each row resumes its saved search, runs its frames of the chunk and saves it again (k_beam.cu's beam_state_words
+ * gives a row's block).
+ */
+struct BeamChunk {
+  static constexpr bool on = true;
+  int Tc; // frames per row of the chunk's emissions [B][Tc][C]
+  uint32_t* state; // [B][words] the rows' state blocks
+  long long words;
+  const int32_t* lens; // [B] frames of each row, nullable: Tc
+  const int32_t* control; // [B] GTNB_BEAM_RESET | GTNB_BEAM_END, nullable: 0
+  int32_t* best_tokens; // [B][T_max] nullable (with the two below): each row's best beam after its frames
+  int32_t* best_lengths; // [B]
+  float* best_scores; // [B]
+};
+
 } // namespace gtnb

@@ -41,6 +41,10 @@
  *   up once by the thread that writes the slot; admission is a bit test in shared memory and the key is
  *   am + (lm_weight * (lmacc + smear) + word_bonus * words).  After the last frame a beam completes its pending word
  *   (dropped inside one), adds its end weight, and the word ids are read off the traced tokens by walking the trie.
+ * - Streaming (gtnb_beam_decode_chunk_async).  beam_chunk_kernel runs the same body, beam_search, under BeamChunk:
+ *   a row's live slots and control words are restored from its state block in global memory (or, at its first frame,
+ *   the one-shot init runs), its chunk's frames run at their absolute frame numbers, and the state is saved again;
+ *   on END the one-shot epilogue runs at the frames consumed.  The arrays saved are the ones BeamSmem<F>::each lists.
  */
 #include <cstdint>
 
@@ -260,9 +264,16 @@ struct BeamCarve {
   }
 };
 
+/* a state array as 32-bit words, for the streaming decoder's save and restore */
+template <class T>
+__host__ __device__ uint32_t* beam_words(T* p) {
+  return reinterpret_cast<uint32_t*>(p);
+}
+
 /*
  * A policy's per-slot state in shared memory ([2][K] arrays, indexed by buffer * K + slot) and the operations
- * beam_decode_kernel calls: init (the root slot, and tables the frames read), key (of a kept or merged candidate whose
+ * beam_decode_kernel calls: each (visits every per-slot array as (32-bit words, words per slot): what a streaming
+ * decoder saves between chunks), init (the root slot when root, and the tables the frames read), key (of a kept or merged candidate whose
  * acoustic score is am), ext_key (of extension (m, c) whose acoustic score is am, -inf when the policy forbids it),
  * keep (slot o carries slot m), extend (slot o is extension (m, c)), final (the final score of slot m, after the last
  * frame), hyp (a hypothesis's own outputs, m -1 for none) and words (the lexicon's word read-off).
@@ -274,7 +285,9 @@ struct BeamSlots;
 template <>
 struct BeamSlots<BeamNoLm> {
   __host__ __device__ void carve(BeamCarve&, int, int) {}
-  __device__ void init(const BeamNoLm&, int, int) const {}
+  template <class Op>
+  __host__ __device__ void each(Op&&) const {}
+  __device__ void init(const BeamNoLm&, int, int, bool) const {}
   __device__ float key(const BeamNoLm&, float am, int, int) const { return am; }
   __device__ float ext_key(const BeamNoLm&, float am, int, int, int, int) const { return am; }
   __device__ void keep(int, int) const {}
@@ -294,8 +307,13 @@ struct BeamSlots<BeamLm> {
     node = m.take<int>(2 * K);
     lm = m.take<float>(2 * K);
   }
-  __device__ void init(const BeamLm& f, int tid, int) const {
-    if (tid == 0) {
+  template <class Op>
+  __host__ __device__ void each(Op&& op) const {
+    op(beam_words(node), 1);
+    op(beam_words(lm), 1);
+  }
+  __device__ void init(const BeamLm& f, int tid, int, bool root) const {
+    if (root && tid == 0) {
       node[0] = f.lmw ? f.start : 0;
       lm[0] = 0.0f;
     }
@@ -364,8 +382,21 @@ struct BeamSlots<BeamLex> {
     rsm = m.take<float>(C);
     cls = m.take<int>(C);
   }
-  __device__ void init(const BeamLex& f, int tid, int C) const {
-    if (tid == 0) {
+  template <class Op>
+  __host__ __device__ void each(Op&& op) const {
+    op(beam_words(node), 1);
+    op(beam_words(lm), 1);
+    op(beam_words(trie), 1);
+    op(beam_words(wn), 1);
+    op(beam_words(wd), 1);
+    op(beam_words(cw), 1);
+    op(beam_words(cd), 1);
+    op(beam_words(fc), 1);
+    op(beam_words(sm), 1);
+    op(mask, MW);
+  }
+  __device__ void init(const BeamLex& f, int tid, int C, bool root) const {
+    if (root && tid == 0) {
       node[0] = f.start;
       lm[0] = 0.0f;
       trie[0] = wn[0] = cd[0] = 0;
@@ -373,7 +404,11 @@ struct BeamSlots<BeamLex> {
       cw[0] = sm[0] = 0.0f;
       fc[0] = __ldg(f.first);
     }
-    if (tid < MW) mask[tid] = rmask[tid] = __ldg(f.mask + tid);
+    if (tid < MW) {
+      const uint32_t v = __ldg(f.mask + tid);
+      rmask[tid] = v;
+      if (root) mask[tid] = v;
+    }
     if (tid < C) {
       cls[tid] = __ldg(f.cls + tid);
       rsm[tid] = lex_has(f.mask, tid) ? __ldg(f.smear + 1 + lex_rank(f.mask, tid)) : 0.0f;
@@ -534,7 +569,33 @@ struct BeamSmem {
     x.carve(m, K, C);
     bytes = m.bytes;
   }
+  /* every per-slot array of the search, the policy's last: a streaming decoder's state between chunks */
+  template <class Op>
+  __host__ __device__ void each(Op&& op) const {
+    op(beam_words(hh), 2);
+    op(beam_words(hq), 2);
+    op(beam_words(spb), 1);
+    op(beam_words(spl), 1);
+    op(beam_words(stot), 1);
+    op(beam_words(slen), 1);
+    op(beam_words(slast), 1);
+    op(beam_words(spar), 1);
+    x.each(op);
+  }
 };
+
+/*
+ * The streaming decoder's state block of a row (32-bit words): a header, then each array BeamSmem<F>::each visits, as
+ * [K][words per slot] (its live slots, the first kBcL, are what a resumed search reads).  Header: frames consumed since
+ * the utterance began, the sticky invalid flag (status 2), and the control words kBcL, kBcTieAny and kBcBad.
+ */
+enum { kStT = 0, kStInv, kStL, kStTie, kStBad, kStHeader = 8 };
+template <class F>
+__host__ __device__ long long beam_state_words(int K, int C) {
+  long long w = kStHeader;
+  BeamSmem<F>(nullptr, K, C).each([&](uint32_t*, int per) { w += (long long)K * per; });
+  return w;
+}
 
 /* status 1 or 2: NaN scores, -1 lengths and rows in every output of the policy */
 template <class F>
@@ -603,19 +664,30 @@ __device__ void beam_finish(int b, int T, int Tb, int C, int K, int N, const uin
   }
 }
 
+/* the one-shot search: every row from frame 0 to its input length, nothing kept */
+struct BeamOnce {
+  static constexpr bool on = false;
+};
+
 /*
- * One CTA of kBeamThreads per utterance b.  emissions [B][T][C] of E; input_lens [B] (nullable: T); kind
- * GTNB_DENSE_CTC / _BIGRAM / _ASG; wt [C][C] (transposed W), wfirst [C] (BIGRAM sigma, ASG start weights) and wbad
- * [C] from beam_weights_kernel (unused for CTC); blank (CTC, BIGRAM); K beams, N hypotheses.  bp: [B][T][K] back-
- * pointers (scratch).  Out: tokens [B][N][T], lengths [B][N], scores [B][N], status [B] (nullable), and the policy's
- * own outputs.  F: the policy (BeamNoLm, BeamLm, BeamLex).
+ * The search of utterance b, one CTA of kBeamThreads (beam_decode_kernel, beam_chunk_kernel).  emissions [B][T][C]
+ * of E; input_lens [B] (nullable: T); kind GTNB_DENSE_CTC / _BIGRAM / _ASG; wt [C][C] (transposed W), wfirst [C]
+ * (BIGRAM sigma, ASG start weights) and wbad [C] from beam_weights_kernel (unused for CTC); blank (CTC, BIGRAM); K
+ * beams, N hypotheses.  bp: [B][T][K] back-pointers (scratch).  Out: tokens [B][N][T], lengths [B][N], scores [B][N],
+ * status [B] (nullable), and the policy's own outputs.  F: the policy (BeamNoLm, BeamLm, BeamLex).
+ * R: BeamOnce, or BeamChunk (gtnb_meta.h): a chunk of a streaming decoder.  Then T is T_max, emissions are [B][Tc][C]
+ * and input_lens is unused: the row's saved state is restored (or, at its first frame, the search starts as the
+ * one-shot one does), its chunk_lens[b] frames run at their absolute frame numbers, and the state is saved again, or
+ * on END the one-shot epilogue runs at the frames consumed and the row restarts.
  */
-template <class E, class Hash, class F = BeamNoLm>
-__global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
-    const E* __restrict__ emissions, int T, int C, const int32_t* __restrict__ input_lens, int kind,
-    const float* __restrict__ wt, const float* __restrict__ wfirst, const int32_t* __restrict__ wbad, int blank, int K,
-    int N, uint16_t* bp, int32_t* __restrict__ tokens, int32_t* __restrict__ lengths, float* __restrict__ scores,
-    int32_t* __restrict__ status, const F fz = F()) {
+template <class E, class Hash, class F, class R>
+__device__ __forceinline__ void beam_search(const E* __restrict__ emissions, int T, int C,
+                                            const int32_t* __restrict__ input_lens, int kind,
+                                            const float* __restrict__ wt, const float* __restrict__ wfirst,
+                                            const int32_t* __restrict__ wbad, int blank, int K, int N, uint16_t* bp,
+                                            int32_t* __restrict__ tokens, int32_t* __restrict__ lengths,
+                                            float* __restrict__ scores, int32_t* __restrict__ status, const F& fz,
+                                            const R& rz) {
   GTNB_DYNAMIC_SMEM(uint64_t, hsm);
   const BeamSmem<F> sm(reinterpret_cast<char*>(hsm), K, C);
   uint64_t *hh = sm.hh, *hq = sm.hq;
@@ -630,16 +702,51 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
   const int P = F::on ? fz.P : C;
 
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int Tb = input_lens ? input_lens[b] : T;
-  if (!(Tb >= 0 && Tb <= T)) {
-    beam_flag(b, T, N, 2, tokens, lengths, scores, status, fz);
-    return;
+  // frames [t0, Tb) run; em: frame t0's row
+  int t0 = 0, Tb;
+  bool fresh = true, end = false, inv = false;
+  uint32_t* st = nullptr;
+  if constexpr (R::on) {
+    st = rz.state + (long long)b * rz.words;
+    const int bits = rz.control ? rz.control[b] : 0;
+    const int n = rz.lens ? rz.lens[b] : rz.Tc;
+    if (n == 0 && bits == 0) return; // (the row is left as it is)
+    const bool reset = (bits & GTNB_BEAM_RESET) != 0;
+    end = (bits & GTNB_BEAM_END) != 0;
+    t0 = reset ? 0 : (int)st[kStT];
+    inv = !reset && st[kStInv] != 0;
+    if (!(n >= 0 && n <= rz.Tc) || n > T - t0) inv = true;
+    Tb = inv ? t0 : t0 + n;
+    fresh = t0 == 0;
+  } else {
+    Tb = input_lens ? input_lens[b] : T;
+    if (!(Tb >= 0 && Tb <= T)) {
+      beam_flag(b, T, N, 2, tokens, lengths, scores, status, fz);
+      return;
+    }
   }
-  const E* em = emissions + (long long)b * T * C;
+  int Te = T; // frames per row of emissions
+  if constexpr (R::on) Te = rz.Tc;
+  const E* em = emissions + (long long)b * Te * C;
   uint16_t* bpu = bp + (long long)b * T * K;
-  if (tid < 16) ctl[tid] = 0;
+  if (tid < 16) {
+    int v = 0;
+    if constexpr (R::on)
+      if (!fresh) v = tid == kBcL ? st[kStL] : tid == kBcTieAny ? st[kStTie] : tid == kBcBad ? st[kStBad] : 0;
+    ctl[tid] = v;
+  }
   for (int i = tid; i < 256; i += kBeamThreads) hist[i] = 0;
-  if (tid == 0) {
+  if constexpr (R::on) {
+    if (!fresh) { // the live slots into buffer 0
+      const int L = (int)st[kStL];
+      long long off = kStHeader;
+      sm.each([&](uint32_t* a, int per) {
+        for (int i = tid; i < L * per; i += kBeamThreads) a[i] = st[off + i];
+        off += (long long)K * per;
+      });
+    }
+  }
+  if (fresh && tid == 0) {
     ctl[kBcL] = 1;
     spb[0] = 0.0f;
     spl[0] = neg_inf();
@@ -655,26 +762,26 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       ppos[tid] = tid;
     }
   }
-  xs.init(fz, tid, C);
+  xs.init(fz, tid, C, fresh);
   __syncthreads();
   if (tid < C) {
     w0[tid] = kind == GTNB_DENSE_CTC ? 0.0f : wfirst[tid];
     wb[tid] = kind == GTNB_DENSE_BIGRAM ? wt[(long long)blank * C + tid] : 0.0f;
-    if (Tb > 0) {
+    if (Tb > t0) {
       const float v = ldg_elem(em + tid);
       erow[tid] = v;
-      if (v != v || v == CUDART_INF_F || (kind != GTNB_DENSE_CTC && wbad[tid])) ctl[kBcBad] = 1;
+      if (v != v || v == CUDART_INF_F || (kind != GTNB_DENSE_CTC && t0 == 0 && wbad[tid])) ctl[kBcBad] = 1;
     }
   }
   __syncthreads();
 
   int cur = 0;
-  for (int t = 0; t < Tb; t++) {
+  for (int t = t0; t < Tb; t++) {
     if (ctl[kBcBad]) break;
     const int L = ctl[kBcL];
-    const float* er = erow + (t & 1) * C;
+    const float* er = erow + ((t - t0) & 1) * C;
     const bool pf = t + 1 < Tb && tid < C;
-    const float ahead = pf ? ldg_elem(em + (long long)(t + 1) * C + tid) : 0.0f;
+    const float ahead = pf ? ldg_elem(em + (long long)(t + 1 - t0) * C + tid) : 0.0f;
     const float* wp = t == 0 ? w0 : wb;
     const float *pb0 = spb + cur * K, *pl0 = spl + cur * K, *tot0 = stot + cur * K;
     const int *len0 = slen + cur * K, *last0 = slast + cur * K, *par0 = spar + cur * K;
@@ -930,7 +1037,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
       spar[nx * K + tid] = par;
     }
     if (pf) {
-      erow[((t + 1) & 1) * C + tid] = ahead;
+      erow[((t + 1 - t0) & 1) * C + tid] = ahead;
       if (ahead != ahead || ahead == CUDART_INF_F) ctl[kBcBad] = 1;
     }
     if (tid == 0) ctl[kBcL] = nw;
@@ -938,11 +1045,73 @@ __global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
     __syncthreads();
   }
 
-  if (ctl[kBcBad]) {
-    beam_flag(b, T, N, 1, tokens, lengths, scores, status, fz);
-    return;
+  if constexpr (R::on) {
+    const int L = ctl[kBcL];
+    const bool bad = ctl[kBcBad] != 0;
+    if (rz.best_tokens) { // slot 0: the best key, in the search's tie order
+      const int m0 = cur * K;
+      const int len = inv || bad || L == 0 ? -1 : slen[m0];
+      int32_t* out = rz.best_tokens + (long long)b * T;
+      if (tid == 0) {
+        rz.best_lengths[b] = len;
+        rz.best_scores[b] = inv || bad ? CUDART_NAN_F : L == 0 ? neg_inf() : xs.key(fz, stot[m0], m0, len);
+        int tt = Tb - 1, s = 0;
+        for (int p = len - 1; p >= 0; p--) out[p] = beam_back(bpu, K, tt, s);
+      }
+      for (int p = tid; p < T; p += kBeamThreads)
+        if (p >= len) out[p] = -1;
+      __syncthreads(); // (the epilogue's final scores change the policy's state)
+    }
+    if (end) {
+      if (inv || bad)
+        beam_flag(b, T, N, inv ? 2 : 1, tokens, lengths, scores, status, fz);
+      else
+        beam_finish(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, xs, kpb, src, tokens, lengths, scores, status,
+                    fz);
+      if (tid == 0) st[kStT] = st[kStInv] = 0;
+      return;
+    }
+    long long off = kStHeader;
+    sm.each([&](uint32_t* a, int per) {
+      for (int i = tid; i < L * per; i += kBeamThreads) st[off + i] = a[(long long)cur * K * per + i];
+      off += (long long)K * per;
+    });
+    if (tid == 0) {
+      st[kStT] = (uint32_t)Tb;
+      st[kStInv] = inv;
+      st[kStL] = (uint32_t)L;
+      st[kStTie] = (uint32_t)ctl[kBcTieAny];
+      st[kStBad] = bad;
+    }
+  } else {
+    if (ctl[kBcBad]) {
+      beam_flag(b, T, N, 1, tokens, lengths, scores, status, fz);
+      return;
+    }
+    beam_finish(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, xs, kpb, src, tokens, lengths, scores, status, fz);
   }
-  beam_finish(b, T, Tb, C, K, N, bpu, cur, ctl, stot, slen, xs, kpb, src, tokens, lengths, scores, status, fz);
+}
+
+/* the one-shot search (gtnb_beam_decode_async, _lm_async, _lexicon_async) */
+template <class E, class Hash, class F = BeamNoLm>
+__global__ void __launch_bounds__(kBeamThreads) beam_decode_kernel(
+    const E* __restrict__ emissions, int T, int C, const int32_t* __restrict__ input_lens, int kind,
+    const float* __restrict__ wt, const float* __restrict__ wfirst, const int32_t* __restrict__ wbad, int blank, int K,
+    int N, uint16_t* bp, int32_t* __restrict__ tokens, int32_t* __restrict__ lengths, float* __restrict__ scores,
+    int32_t* __restrict__ status, const F fz = F()) {
+  beam_search<E, Hash, F>(emissions, T, C, input_lens, kind, wt, wfirst, wbad, blank, K, N, bp, tokens, lengths,
+                          scores, status, fz, BeamOnce());
+}
+
+/* one chunk of the streaming decoder (gtnb_beam_decode_chunk_async): T = T_max, emissions [B][rz.Tc][C] */
+template <class E, class Hash, class F>
+__global__ void __launch_bounds__(kBeamThreads) beam_chunk_kernel(
+    const E* __restrict__ emissions, int T, int C, int kind, const float* __restrict__ wt,
+    const float* __restrict__ wfirst, const int32_t* __restrict__ wbad, int blank, int K, int N, uint16_t* bp,
+    int32_t* __restrict__ tokens, int32_t* __restrict__ lengths, float* __restrict__ scores,
+    int32_t* __restrict__ status, const F fz, const BeamChunk rz) {
+  beam_search<E, Hash, F>(emissions, T, C, nullptr, kind, wt, wfirst, wbad, blank, K, N, bp, tokens, lengths, scores,
+                          status, fz, rz);
 }
 
 /* the dynamic shared memory of beam_decode_kernel<E, Hash, F> at K beams and C tokens; the by-policy names are the
@@ -997,6 +1166,39 @@ GTNB_BEAM_POLICY(BeamNoLm)
 GTNB_BEAM_POLICY(BeamLm)
 GTNB_BEAM_POLICY(BeamLex)
 #undef GTNB_BEAM_POLICY
+
+long long beam_state_row_words(bool lexicon, int K, int C) {
+  return lexicon ? beam_state_words<BeamLex>(K, C) : beam_state_words<BeamLm>(K, C);
+}
+
+template <class F>
+int launch_beam_chunk(gtnb_ctx* ctx, int B, int T, int C, const void* emissions, int dtype, int kind,
+                      const float* wt, const float* wfirst, const int32_t* wbad, int blank, int K, int N, uint16_t* bp,
+                      int32_t* tokens, int32_t* lengths, float* scores, int32_t* status, const F& f,
+                      const BeamChunk& r) {
+  if (B <= 0) return GTNB_OK;
+  const long long smem = beam_smem_bytes<F>(K, C);
+  const char* name = std::is_same_v<F, BeamLex> ? "beam_chunk_lexicon" : "beam_chunk_lm";
+  const auto run = [&](const auto* e) {
+    using E = std::remove_const_t<std::remove_pointer_t<decltype(e)>>;
+    if (smem > 48 * 1024)
+      if (const int rc = ensure_max_smem(ctx, (const void*)beam_chunk_kernel<E, BeamHash, F>)) return rc;
+    GTNB_LAUNCH(ctx, name,
+                beam_chunk_kernel<E, BeamHash, F><<<B, kBeamThreads, smem, ctx->stream>>>(
+                    e, T, C, kind, wt, wfirst, wbad, blank, K, N, bp, tokens, lengths, scores, status, f, r));
+    return (int)GTNB_OK;
+  };
+  if (dtype == GTNB_BF16) return run(static_cast<const bf16_t*>(emissions));
+  if (dtype == GTNB_F16) return run(static_cast<const f16_t*>(emissions));
+  return run(static_cast<const float*>(emissions));
+}
+#define GTNB_BEAM_CHUNK_POLICY(F_)                                                                              \
+  template int launch_beam_chunk<F_>(gtnb_ctx*, int, int, int, const void*, int, int, const float*, const float*, \
+                                     const int32_t*, int, int, int, uint16_t*, int32_t*, int32_t*, float*,        \
+                                     int32_t*, const F_&, const BeamChunk&);
+GTNB_BEAM_CHUNK_POLICY(BeamLm)
+GTNB_BEAM_CHUNK_POLICY(BeamLex)
+#undef GTNB_BEAM_CHUNK_POLICY
 
 #endif // GTNB_HOST_EMU
 

@@ -1603,3 +1603,122 @@ def backoff_transitions_viterbi(emissions, transitions, transitions_graph, graph
         c.g, large_transitions, lambda: capi.lib().gtnb_backoff_transitions_viterbi(
             c.g.h, c.B, c.T, c.C, c.e.data_ptr(), 1, c.il, c.arr, c.w, 1, C.byref(gv[0]), tw.data_ptr(), 1, paths,
             arcs, scores, 1)))
+
+
+class StreamingBeamDecoder:
+    """The beam search of ctc_lm_beam_decode (lexicon None) or ctc_lexicon_beam_decode (with a Lexicon), and their
+    n-gram CTC and ASG forms, fed a chunk of frames at a time, for online recognition: every row's beams stay on the
+    device between steps (gtnb_beam_state_create / gtnb_beam_decode_chunk_async).
+
+    batch rows of at most max_frames frames each, num_labels tokens; kind "ctc", "ngram_ctc" (transitions [C*C]) or
+    "asg" (transitions [C + C*C]), float32 on the device; the transitions are baked in at construction.  lm: a
+    LanguageModel (lexicon None), lexicon: a Lexicon (lm None); bonus is token_bonus without a lexicon and word_bonus
+    with one.  beam, nbest, token_beam (None: C) and blank as in the one-shot decoders, with their bounds.  Each row
+    starts as a fresh utterance.
+
+    step(emissions, chunk_lengths=None, end=None, reset=None): emissions [batch, Tc, C] (float32, bfloat16 or
+    float16); chunk_lengths [batch] integers in [0, Tc] (None: Tc each); end and reset [batch] booleans (None: none).
+    For each row: reset discards its utterance so far; the row consumes its chunk_lengths frames; the best beam after
+    them is returned; with end, self.results gets the row's final N-best and the row restarts empty.  A row with zero
+    frames and neither flag is left untouched.  It runs on the current stream without a host synchronisation, so it
+    may be captured in a CUDA graph and the graph replayed for every chunk (same tensors, new contents).  Returns
+    (tokens [batch, max_frames] int32, each transcript followed by -1; lengths [batch] int32; scores [batch] float32,
+    the ranking key).  A row flagged as below has length -1 and a NaN score.  With best=False the best beam is not
+    traced (it walks the back-pointers, O(frames so far) per row) and step returns None.
+
+    results: an LMBeamDecode (no lexicon) or LexiconBeamDecode with T = max_frames, written only for the rows ended in
+    a step and kept until a later step ends them again.  At end they are == the one-shot decoder's on the frames the
+    row consumed since its last end or reset, whatever the chunking; status 2 also flags a chunk length outside
+    [0, Tc] or a row pushed past max_frames, until end or reset.
+
+    The returned tensors and results are buffers of this decoder, reused by every step: copy what must outlive the next
+    step.  That reuse is what makes a captured step replayable.  Creating one allocates and synchronises, so it raises
+    while a stream is capturing; keep it (and its lm or lexicon) alive as long as a captured graph that steps it."""
+
+    _KINDS = {"ctc": capi.DENSE_CTC, "ngram_ctc": capi.DENSE_BIGRAM, "asg": capi.DENSE_ASG}
+
+    def __init__(self, batch, max_frames, num_labels, kind="ctc", transitions=None, lm=None, lexicon=None,
+                 lm_weight=1.0, bonus=0.0, beam=16, nbest=1, token_beam=None, blank=0, device=None, best=True):
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("StreamingBeamDecoder: create it before capturing a CUDA graph (it allocates and "
+                               "synchronises)")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        assert kind in self._KINDS, "kind must be ctc, ngram_ctc or asg"
+        assert lm is None or isinstance(lm, LanguageModel)
+        assert lexicon is None or isinstance(lexicon, Lexicon)
+        self.batch, self.max_frames, self.num_labels = int(batch), int(max_frames), int(num_labels)
+        self.kind, self.nbest, self.lexicon, self.lm, self.best = kind, int(nbest), lexicon, lm, bool(best)
+        k = self._KINDS[kind]
+        w = None
+        if k != capi.DENSE_CTC:
+            assert transitions is not None and transitions.is_cuda and transitions.dtype == torch.float32
+            assert transitions.device == self.device
+            Cn = self.num_labels
+            assert transitions.numel() == (Cn * Cn if k == capi.DENSE_BIGRAM else Cn + Cn * Cn)
+            w = transitions.detach().contiguous()
+        P = self.num_labels if token_beam is None else int(token_beam)
+        self._g = _async_ctx(self.device, "StreamingBeamDecoder")
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            self._g._check(capi.lib().gtnb_beam_state_create(
+                self._g.h, self.batch, self.max_frames, self.num_labels, k, None if w is None else w.data_ptr(),
+                int(blank), int(beam), self.nbest, P, None if lm is None else lm.h,
+                None if lexicon is None else lexicon.h, float(lm_weight), float(bonus), C.byref(h)))
+        self.h = h
+        B, N, T = self.batch, self.nbest, self.max_frames
+        i32, f32 = dict(dtype=torch.int32, device=self.device), dict(dtype=torch.float32, device=self.device)
+        if lexicon is None:
+            self.results = LMBeamDecode(torch.full((B, N, T), -1, **i32), torch.full((B, N), -1, **i32),
+                                        torch.full((B, N), float("nan"), **f32),
+                                        torch.full((B, N), float("nan"), **f32),
+                                        torch.full((B, N), float("nan"), **f32), torch.zeros(B, **i32))
+        else:
+            self.results = LexiconBeamDecode(torch.full((B, N, T), -1, **i32), torch.full((B, N), -1, **i32),
+                                             torch.full((B, N, T), -1, **i32), torch.full((B, N), -1, **i32),
+                                             torch.full((B, N), float("nan"), **f32),
+                                             torch.full((B, N), float("nan"), **f32),
+                                             torch.full((B, N), float("nan"), **f32), torch.zeros(B, **i32))
+        self.best_tokens = torch.full((B, T), -1, **i32)
+        self.best_lengths = torch.zeros(B, **i32)
+        self.best_scores = torch.zeros(B, **f32)
+
+    @torch.no_grad()
+    def step(self, emissions, chunk_lengths=None, end=None, reset=None):
+        assert emissions.is_cuda and emissions.device == self.device and emissions.dim() == 3
+        assert emissions.dtype in _EMISSION_DTYPES, "emissions must be float32, bfloat16 or float16"
+        if emissions.shape[0] != self.batch or emissions.shape[2] != self.num_labels:
+            raise ValueError("StreamingBeamDecoder.step: emissions must be [%d, Tc, %d], not %s"
+                             % (self.batch, self.num_labels, list(emissions.shape)))
+        e = emissions.contiguous()
+        ln = None
+        if chunk_lengths is not None:
+            assert chunk_lengths.is_cuda and chunk_lengths.device == self.device and chunk_lengths.numel() == self.batch
+            lens = chunk_lengths.to(torch.int32).contiguous()  # (the tensor itself when it is int32 already)
+            ln = lens.data_ptr()
+        ctl = None
+        if reset is not None:
+            ctl = reset.to(torch.int32) * capi.BEAM_RESET
+        if end is not None:
+            x = end.to(torch.int32) * capi.BEAM_END
+            ctl = x if ctl is None else ctl + x
+        if ctl is not None:
+            assert ctl.device == self.device and ctl.numel() == self.batch
+            ctl = ctl.contiguous()
+        r = self.results
+        lex = self.lexicon is not None
+        b = (self.best_tokens.data_ptr(), self.best_lengths.data_ptr(), self.best_scores.data_ptr()) if self.best \
+            else (None, None, None)
+        self._g._check(capi.lib().gtnb_beam_decode_chunk_async(
+            self._g.h, torch.cuda.current_stream(self.device).cuda_stream, self.h, e.shape[1], e.data_ptr(),
+            _EMISSION_DTYPES[e.dtype], ln, None if ctl is None else ctl.data_ptr(), r.tokens.data_ptr(), r.lengths.data_ptr(), r.scores.data_ptr(),
+            r.am_scores.data_ptr(), r.lm_scores.data_ptr(), r.words.data_ptr() if lex else None,
+            r.word_counts.data_ptr() if lex else None, r.status.data_ptr(), *b))
+        return (self.best_tokens, self.best_lengths, self.best_scores) if self.best else None
+
+    def __del__(self):
+        h = getattr(self, "h", None)
+        if h is not None and h.value:
+            capi.lib().gtnb_beam_state_destroy(self._g.h, h)
+            self.h = None

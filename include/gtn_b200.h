@@ -1635,6 +1635,87 @@ int gtnb_beam_decode_lexicon_async(
     void* workspace_dev,
     size_t workspace_bytes);
 
+/*
+ * Streaming beam search: the search of gtnb_beam_decode_lm_async or gtnb_beam_decode_lexicon_async fed a chunk of
+ * frames at a time, with every row's beams kept on the device between calls, for online recognition (a best
+ * transcript after every chunk, the N-best at the end of the utterance, no re-decoding of the prefix).
+ *
+ * gtnb_beam_state_create makes a decoder of B rows of at most T_max frames each, for one configuration:
+ *   - lexicon NULL: gtnb_beam_decode_lm_async's search, lm nullable, bonus = token_bonus;
+ *   - lexicon given: gtnb_beam_decode_lexicon_async's search, lm NULL, bonus = word_bonus.
+ * gtnb_beam_decode_async is the first with lm NULL, bonus 0 and token_beam = C (its identity rule).  Arguments, bounds
+ * and errors are the mirrored call's (1 <= beam <= 64, nbest <= beam, C <= 256, token_beam in [1, C], blank, the
+ * lexicon's blank rule, an LM or lexicon made on ctx's device for this C), with B >= 1 and T_max >= 1.  The state
+ * keeps pointers to lm and lexicon: the caller keeps them alive as long as it.  For BIGRAM and ASG the transposed
+ * weights, start weights and row flags are made from trans_w_dev once, here: the transitions are baked in (a decoder
+ * whose transitions change needs a new state).  Every row starts as a fresh utterance.  create allocates and
+ * synchronises: it is a set-up call and may not be captured.  One device allocation of, each term rounded up to a
+ * multiple of 256 (r(x)),
+ *   bytes = r(2 * B * T_max * beam)                                      (16-bit back-pointers, by absolute frame)
+ *         + r(4 * B * (8 + beam * (10 + p)))                             (one state block per row)
+ *         + (kind != GTNB_DENSE_CTC ? r(4 * C*C) + 2 * r(4 * C) : 0)     (transposed W, start weights, row flags)
+ * with p = 2 without a lexicon (LM node, lmacc) and p = 9 + ceil(C / 32) with one (the trie state and child mask).
+ *
+ * gtnb_beam_decode_chunk_async consumes one chunk under the beam calls' contract: kernel launches on cuda_stream and
+ * nothing else, so it may be captured, and a graph captured once may be replayed for every chunk.  Calls on one state
+ * must be ordered on one stream.  emissions_dev is [B][Tc][C] of dtype.  For each row b:
+ *   1. control_dev[b] (NULL: 0 each) with GTNB_BEAM_RESET: the row's utterance so far is discarded, the row restarts.
+ *   2. The row consumes its first chunk_lens_dev[b] frames (NULL: Tc each) of its slice.
+ *   3. best_tokens_dev [B][T_max], best_lengths_dev [B], best_scores_dev [B] (all three or none) receive the row's
+ *      current best beam: slot 0 after its last frame, the highest ranking key in the tie rule's order.  Its tokens
+ *      followed by -1, its length, and its ranking key (am + lm_weight * lmacc + bonus * len, or the lexicon's key
+ *      with smear).  A flagged row (status 1 or 2 at END) gets length -1, NaN and -1 rows; no live beam, length -1
+ *      and -inf.
+ *   4. With GTNB_BEAM_END, the final outputs are written in the mirrored call's layout with T = T_max: tokens_dev
+ *      [B][nbest][T_max], lengths_dev, scores_dev, am_scores_dev, lm_scores_dev [B][nbest] (nullable),
+ *      words_dev [B][nbest][T_max] and word_counts_dev [B][nbest] (nullable, lexicon only) and status_dev [B]
+ *      (nullable).  The row then restarts empty.
+ *   5. A row without END has none of its final outputs written.  A row with zero frames and no control bits is left
+ *      untouched, its best outputs included.
+ * Equality: the outputs written at END are == bit for bit to the mirrored one-shot call on the frames the row consumed
+ * since its previous END or RESET, n in all, padded to T = T_max with input_lens = n, for every split into chunks
+ * (chunks of 0 and 1 frames included), tie flags (status 3) and the NaN / +inf flag (status 1) included.  Status 2
+ * covers chunk_lens_dev[b] outside [0, Tc] and a row pushed past T_max frames: the flag sticks until END or RESET,
+ * which give NaN scores and -1 rows; no other row is affected.  The best beam is the mirrored call's top hypothesis at
+ * the frames so far wherever the final ranking is the key ranking (no LM end weights, no lexicon).
+ * The best beam is traced through the back-pointers, O(frames so far) dependent loads per row and call: pass NULL
+ * best outputs to skip it.  Tc = 0 is allowed.  Errors: NULL state, emissions (Tc > 0), tokens, lengths or scores,
+ * words_dev or word_counts_dev without a lexicon, part of the best outputs, or a state made on another device:
+ * GTNB_ERR_INVALID_ARGUMENT; an unknown dtype: GTNB_ERR_UNSUPPORTED.
+ *
+ * Out of scope: streams longer than T_max (a back-pointer ring), word ids or timestamps in the best beam, lattices,
+ * changing the transitions, LM or lexicon of a live state, and one state used from two streams at once.
+ */
+#define GTNB_BEAM_RESET 1
+#define GTNB_BEAM_END 2
+typedef struct gtnb_beam_state gtnb_beam_state;
+int gtnb_beam_state_create(gtnb_ctx* ctx, int B, int T_max, int C, int kind,
+                           const float* trans_w_dev, /* NULL, BIGRAM [C*C], ASG [C + C*C] */
+                           int blank, int beam, int nbest, int token_beam, const gtnb_lm* lm /* or NULL */,
+                           const gtnb_lexicon* lexicon /* or NULL */, float lm_weight, float bonus,
+                           gtnb_beam_state** out);
+void gtnb_beam_state_destroy(gtnb_ctx* ctx, gtnb_beam_state* state);
+int gtnb_beam_decode_chunk_async(
+    gtnb_ctx* ctx,
+    void* cuda_stream,
+    gtnb_beam_state* state,
+    int Tc,
+    const void* emissions_dev, /* [B][Tc][C] of dtype */
+    int dtype,
+    const int32_t* chunk_lens_dev, /* [B] in [0, Tc], or NULL */
+    const int32_t* control_dev, /* [B] GTNB_BEAM_RESET | GTNB_BEAM_END, or NULL */
+    int32_t* tokens_dev, /* [B][nbest][T_max] */
+    int32_t* lengths_dev, /* [B][nbest] */
+    float* scores_dev, /* [B][nbest] */
+    float* am_scores_dev, /* [B][nbest] or NULL */
+    float* lm_scores_dev, /* [B][nbest] or NULL */
+    int32_t* words_dev, /* [B][nbest][T_max] or NULL (lexicon) */
+    int32_t* word_counts_dev, /* [B][nbest] or NULL (lexicon) */
+    int32_t* status_dev, /* [B] or NULL */
+    int32_t* best_tokens_dev, /* [B][T_max] or NULL */
+    int32_t* best_lengths_dev, /* [B] or NULL */
+    float* best_scores_dev); /* [B] or NULL */
+
 #ifdef __cplusplus
 }
 #endif
